@@ -1,5 +1,5 @@
 /*
- * sgdml_b200 -- C ABI of the B200-native engine for sGDML's two dense hot paths
+ * sgdml_b200 -- C ABI of the H100-native engine for sGDML's two dense hot paths
  * (SURVEY.md section 8).  Plain pointers and sizes only; no torch / C++ types.
  *
  * Conventions
@@ -124,7 +124,7 @@ int sgdml_b200_predict_train(sgdml_b200_model* model, int64_t m_begin, int64_t m
                              double* E, double* F, void* stream);
 
 /* Large-descriptor models (D > 256: the predictor is four GEMMs around two element-wise kernels): run those GEMMs on
- * the tcgen05 tensor cores through `slices` exact int8 slices per operand (2..7; csrc/ozaki.cu) or in FP64 DMMA (0, the
+ * the int8 tensor cores (wgmma) through `slices` exact int8 slices per operand (2..7; csrc/ozaki.cu) or in FP64 DMMA (0, the
  * default unless SGDML_B200_OZAKI_PREDICT_SLICES is set when the model is created).  Forces against the FP64 form:
  * 8.8e-9 / 6.5e-11 / 5.4e-13 relative for 4 / 5 / 6 slices.  The iterative solver sets 5 for its K.v products
  * (iterative.py:183-204: tolerance 1e-4).  No effect for D <= 256. */
@@ -275,9 +275,9 @@ int sgdml_b200_dgemm_nt(int64_t m, int64_t n, int64_t k, double alpha, const dou
                         int64_t lda, const double* B, int64_t ldb, double beta, double* C,
                         int64_t ldc, void* stream);
 
-/* EXPERIMENTAL (not yet run on hardware, see csrc/ozaki.cu): the same product through the tcgen05 tensor
+/* The same product through the int8 tensor
  * cores -- A and B are cut into n_slices signed 7-bit slices per row-scaled entry and every slice pair is
- * multiplied exactly by tcgen05.mma kind::i8 (int32 accumulators in tensor memory); C += alpha * A * B^T.
+ * multiplied exactly by wgmma s8 (int32 accumulators in registers); C += alpha * A * B^T.
  * n_slices = 7 reproduces the FP64 Cholesky trailing update (analytic.py:94-96) to ~1e-14 relative, 8 would
  * be FP64-equivalent (tools/ozaki_study.py).  tri != 0: m == n, only tiles touching the lower triangle.
  * All pointers must be device pointers; k <= 16384. */
@@ -303,19 +303,19 @@ int sgdml_b200_profile_reset(void);
 int sgdml_b200_profile_get(int family, double* total_ms, int64_t* scopes, int64_t* launches);
 
 /* FP64 tensor-pipe peak of the current device, measured live with a register-resident
- * mma.sync.m8n8k4.f64 loop (TFLOP/s); the roofline denominator for the FP64 kernels
- * (MEASURED_PEAKS.json only carries HBM and bf16 numbers). */
+ * mma.sync.m8n8k4.f64 loop (TFLOP/s); the roofline denominator for the FP64 kernels. */
 int sgdml_b200_fp64_peak_tflops(double* tflops);
 /* Same probe held for `seconds` (<= 30); reports the second half: the sustained figure for
  * kernels timed inside a long step (clocks settle under the power cap). */
 int sgdml_b200_fp64_peak_tflops_sustained(double seconds, double* tflops);
 
 /* Trailing updates of the Cholesky factorisation: -1 = automatic (default), 0 = FP64 DMMA, 2..7 = that many signed 7-bit
- * slices per operand on the tcgen05 tensor cores (kind::i8, exact int32 accumulation in tensor memory, summed in FP64;
- * csrc/ozaki.cu).  Automatic = the environment variable SGDML_B200_OZAKI_SLICES if set, otherwise 7 slices inside
- * sgdml_b200_solve_analytic for n >= 16384 (BASELINE config 2: residual 3.7e-11, training forces equal to the FP64
- * factorisation's to 2e-11 relative) and FP64 everywhere else (sgdml_b200_potrf, the Nystroem factor). */
+ * slices per operand on the int8 tensor cores (wgmma s8, exact int32 accumulation in registers, summed in FP64;
+ * csrc/ozaki.cu).  Automatic = the environment variable SGDML_B200_OZAKI_SLICES if set, otherwise FP64 (on an H100 the
+ * FP64 DMMA trailing updates are faster than 7 int8 slices at BASELINE config 2, and exact). */
 int sgdml_b200_set_solve_slices(int n_slices);
+/* The slice count the next factorisation will use (0 = FP64 DMMA), after resolving the automatic setting. */
+int sgdml_b200_get_solve_slices(void);
 
 /* Test / tuning hook: selects the GEMM kernel used by dgemm_nt and potrf's trailing update.
  * 0 = 128x128 DMMA tiles fed by cp.async, 1 = 128x64 DMMA tiles, 2 = scalar FMA reference kernel,

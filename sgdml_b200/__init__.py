@@ -1,8 +1,8 @@
-"""sgdml_b200 -- B200-native engine for sGDML's two dense hot paths (SURVEY.md section 8):
+"""sgdml_b200 -- H100-native engine for sGDML's two dense hot paths (SURVEY.md section 8):
 (a) Hessian-kernel matrix assembly + FP64 Cholesky solve behind ``GDMLTrain.train(task)``,
 (b) batched energy/force prediction behind ``GDMLPredict(model).predict(R)``.
 
-Host code is Python; all arithmetic runs in hand-written sm_100a CUDA kernels behind the C
+Host code is Python; all arithmetic runs in hand-written sm_90a CUDA kernels behind the C
 ABI declared in ``include/sgdml_b200.h`` (``sgdml_b200/libsgdml_b200.so``).  There is no
 CPU fallback.
 """

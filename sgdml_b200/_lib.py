@@ -92,6 +92,7 @@ SIGNATURES = {
          c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64_p, c_double_p, c_void_p],
     ),
     'sgdml_b200_set_solve_slices': (C.c_int, [C.c_int]),
+    'sgdml_b200_get_solve_slices': (C.c_int, []),
     'sgdml_b200_set_gemm_variant': (C.c_int, [C.c_int]),
     'sgdml_b200_profile_enable': (C.c_int, [C.c_int]),
     'sgdml_b200_profile_reset': (C.c_int, []),

@@ -2,7 +2,7 @@
 // rows a-K / a-KT) -- reference sgdml/train.py:97-232 (_assemble_kernel_mat_wkr),
 // train.py:1260-1535 (_assemble_kernel_mat), torchtools.py:110-392 (GDMLTorchAssemble).
 //
-// B200 design.  The reference materialises the dense Jacobians (D x 3N, six non-zeros per
+// Design.  The reference materialises the dense Jacobians (D x 3N, six non-zeros per
 // row) and runs three S-fold einsums plus a 3N x D x 3N product per block
 // (train.py:209-226).  Here the Jacobian never exists.  With the antisymmetric pair vectors
 //   G_m[a][g] = (r_a - r_g)/|r_a - r_g|^3      (J_m[d(a,g), atom a] = -G_m[a][g])
@@ -319,7 +319,7 @@ __global__ void __launch_bounds__(256, 2) k_assemble(const AsmArgs p) {
 
 // ---------------------------------------------------------------------------------------------
 // k_assemble_v3: the same mathematics, restructured around what the first kernel's profile showed
-// (profiles/r01_ncu_assemble.txt: 24.6 % warps active, 14.4 % FP64 pipe, barrier / short-scoreboard / wait stalls):
+// (few warps active, a mostly idle FP64 pipe, barrier / short-scoreboard / wait stalls):
 //  * permutations are processed in CHUNKS of PG: phase A computes the per-(point, permutation) vectors u, v, Dg of
 //    the whole chunk in one go -- tj * PG * 5N independent row tasks instead of tj * 5N, so all 256 threads have
 //    work -- with the delta table evaluated on the fly (delta_p[Pa][Pg] = x_i[a][g] - x_j[Pa][Pg]; no staged table,
@@ -1603,8 +1603,7 @@ extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_
   int64_t* d_dest = nullptr;
   double* d_slabs = nullptr;
   // the integer tables (and the large-molecule kernel's slabs) live in persistent workspaces: a cudaMalloc / cudaFree
-  // pair per table costs milliseconds once the K buffer and the factorisation workspaces exist (measured: 36 ms of
-  // kernel inside a 74 ms assembly on the second training run of a process)
+  // pair per table costs milliseconds once the K buffer and the factorisation workspaces exist
   auto cleanup = [&]() {};
   auto body = [&]() -> int {
     SG_TRY(ws_get(WS_ASM_DPERM, sizeof(int) * dperm.size(), (void**)&d_dperm));
@@ -1655,8 +1654,8 @@ extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_
       int PG = S;
       while (PG > 1 && asm_v3_smem_bytes(N, S, TJ, PG) > 100 * 1024) PG = (PG + 1) / 2;
       const size_t smem3 = asm_v3_smem_bytes(N, S, TJ, PG);
-      // measured on B200 (tools/asm_variants.py): 35.9 vs 41.3 ms at BASELINE config 2 (S = 6, one chunk); with many
-      // permutations (S = 243, chunks of 8) the chunked kernel is 15 % SLOWER than the per-permutation one, so it is
+      // chosen by timing the variants (tools/asm_variants.py): faster at BASELINE config 2 (S = 6, one chunk); with many
+      // permutations (S = 243, chunks of 8) the chunked kernel is SLOWER than the per-permutation one, so it is
       // only used when all permutations fit one chunk -- unless a test forces it (variant 3)
       const bool use_v3 = smem3 <= 220 * 1024 && TJ * PG <= 256 && (g_asm_kernel == 3 || (g_asm_kernel == 0 && PG == S));
       // v4 kernel: chunks of up to 16 permutations; two CTAs per SM when everything fits in ~110 KB, else one
@@ -1668,8 +1667,8 @@ extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_
         if (asm_v4_smem_bytes(N, S, TJ, q) <= 110 * 1024) PG4 = q;
       }
       const size_t smem4 = asm_v4_smem_bytes(N, S, TJ, PG4);
-      // measured on B200 (tools/asm_variants.py): BASELINE config 2, full matrix: 42.4 (k_assemble) / 37.6 (v3) / 36.7 ms
-      // (v4); Ac-Ala3 shape, S = 243, 3000 random columns of M = 300 points: 616 / 805 / 312 ms -- v4 is the default
+      // chosen by timing the variants (tools/asm_variants.py) at BASELINE config 2 (full matrix) and on the Ac-Ala3 shape
+      // (S = 243, random column subsets): v4 was the fastest on both -- v4 is the default
       const bool use_v4 = N <= 255 && smem4 <= 220 * 1024 && TJ * PG4 <= 256 && (g_asm_kernel == 4 || g_asm_kernel == 0);
       const int tiles_per_cta = 4;
       if (use_v5) {

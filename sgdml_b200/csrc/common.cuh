@@ -1,4 +1,4 @@
-// Shared helpers for the sgdml_b200 CUDA sources (sm_100a only).
+// Shared helpers for the sgdml_b200 CUDA sources (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -41,9 +41,8 @@ bool is_device_ptr(const void* p);
 // RAII staging buffer: presents a device view of a user pointer that may live on the host.
 // in:  copy host->device on construction when the user pointer is a host pointer
 // out: copy device->host in finish() when the user pointer is a host pointer
-// The device buffers come from a small per-thread pool: cudaMalloc + cudaFree cost ~10 ms each in a
-// process that holds tens of GB (measured: 4 pairs per preconditioner application = 86 ms), which
-// dominated calls made once per CG iteration.  On destruction the stream the buffer was used on is
+// The device buffers come from a small per-thread pool: cudaMalloc + cudaFree can cost milliseconds each in a
+// process that holds tens of GB, which would dominate calls made once per CG iteration.  On destruction the stream the buffer was used on is
 // synchronised (what the implicit synchronisation of cudaFree used to guarantee) and the buffer is
 // kept for the next call.
 class Staged {
@@ -81,7 +80,7 @@ int ws_get(int slot, size_t bytes, void** out);
 
 // Device-block cache for the predictor's model arrays and per-batch workspaces: `GDMLTrain.train` creates and destroys a
 // predictor of the same shape every run (integration constant), and on some hosts a cudaMalloc / cudaFree pair next to
-// a 32 GB K buffer costs 5-15 ms (measured: 0.2-0.5 s of a 1.3 s training run on such a box, 3 ms on others).
+// a 32 GB K buffer costs milliseconds.
 // cached_free keeps a block (exact-size reuse, at most 8 GB in total); the CALLER makes sure no kernel still uses it
 // (cudaFree's implicit synchronisation is gone).  sgdml_b200_release_workspaces() empties the cache.
 cudaError_t cached_malloc_bytes(void** p, size_t bytes);

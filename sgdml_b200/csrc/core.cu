@@ -30,7 +30,7 @@ int require_device() {
   if (e != cudaSuccess || n == 0) {
     cudaGetLastError();
     g_last_error =
-        "sgdml_b200: no CUDA device visible -- this engine has no CPU fallback (B200 / sm_100a required)";
+        "sgdml_b200: no CUDA device visible -- this engine has no CPU fallback (H100 / sm_90a required)";
     return SGDML_B200_ERR_NO_DEVICE;
   }
   return 0;
@@ -226,11 +226,11 @@ cudaError_t cached_free(void* p) {
 int num_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-  if (dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];

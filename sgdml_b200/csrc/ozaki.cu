@@ -1,9 +1,10 @@
-// FP64 GEMM on the 5th-generation tensor cores: C += alpha * A * B^T with A and B cut into signed
-// 7-bit slices (int8) and every slice-pair product computed EXACTLY by tcgen05.mma kind::i8 with
-// int32 accumulators in tensor memory (Ozaki-style error-free splitting).  This is the tcgen05 form
-// of the Cholesky trailing update of path (a) (reference: scipy cho_factor = LAPACK dpotrf,
-// sgdml/solvers/analytic.py:94-96): B200 has no f64 tensor-core kind, and the FP64 DMMA pipe tops
-// out at 37 TFLOP/s, while 28 exact int8 GEMMs (7 slices) at 4.5 POP/s are worth ~160 TFLOP/s.
+// FP64 GEMM on the Hopper tensor cores: C += alpha * A * B^T with A and B cut into signed 7-bit slices (int8)
+// and every slice-pair product computed EXACTLY by wgmma (s8 x s8 -> s32, accumulators in registers):
+// Ozaki-style error-free splitting.  This is the int8 form of the Cholesky trailing update of path (a)
+// (reference: scipy cho_factor = LAPACK dpotrf, sgdml/solvers/analytic.py:94-96).  The H100 data sheet gives
+// 67 TFLOP/s of FP64 tensor-core throughput and 1979 TOP/s of dense int8; 28 exact int8 GEMMs (7 slices)
+// bring the latter to ~70 TFLOP/s-equivalent at best, so which path is faster is a measured choice
+// (csrc/solve.cu resolve_slices).
 //
 //   x_ij = 2^(e_i) * sum_{p=1..S} q_ij^(p) 2^(-7p),   |q^(p)| <= 64,   e_i per ROW
 //   (A B^T)_ij = 2^(ea_i + eb_j) * sum_{L=2..S+1} 2^(-7L) * sum_{p+q=L} (A^(p) B^(q)T)_ij
@@ -12,25 +13,19 @@
 // tools/ozaki_study.py (CPU, exact) shows what that buys on the sGDML system: with S = 7 the trained
 // forces agree with the FP64 factorisation to 2e-11 at cond(K) = 2e10; S = 8 is FP64-equivalent.
 //
-// Kernel structure (one CTA per 128 x 64 tile of C, 192 threads, warp-specialised):
+// Kernel structure (persistent, one CTA per SM, 128 x 32 tiles of C, 288 threads, warp-specialised):
 //   layout   the split kernel writes the slices UNIT-MAJOR and PRE-SWIZZLED: a pipeline unit -- slice p of one
 //            64-wide k-block for a tile of 128 rows -- is one contiguous 8 KB block of global memory holding
 //            exactly the bytes of the canonical K-major 64-byte-swizzle shared-memory tile, so a unit is fetched
-//            with two 1-D bulk copies (cp.async.bulk, A 8 KB + B 4 KB) that stream whole DRAM pages.  (The first
-//            version read row-major planes through 3-D tensor maps: 64-byte fragments 1 KB apart, which ran at
-//            14 GB/s per SM -- measured, profiles/r02_ozaki_bringup.md.)
-//   warp 0   producer: a pipeline stage holds one k-block -- the S slices of A (8 KB each), then the S slices of B
-//            (4 KB each) in slice order -- filled by 2 S bulk copies; 2 stages at S = 7 (168 KB), more for fewer slices
-//   warp 1   MMA issuer (whole warp waits on the stage, one elected lane issues): slice pa of A times up to four
-//            CONSECUTIVE slices of B in one M = 128, N <= 256 instruction -- consecutive B slices are consecutive
-//            levels, whose accumulators are consecutive 64-column blocks of tensor memory (see oz_issue_kblock)
-//   warps 2-5 epilogue: the S level accumulators (S x 64 TMEM columns) are read with tcgen05.ld, summed
-//            smallest level first in FP64 registers, scaled by 2^(ea_i + eb_j), transposed through shared
-//            memory and added to C with row-contiguous (coalesced) accesses
-//   raster   CTAs are numbered super-tile by super-tile (8 x 16 tiles = 1024 x 1024 of C, one wave of CTAs), so
-//            the slices a wave reads (2 x 1024 rows) stay L2-resident while they are reused
-//
-// Brought up on hardware in round 2 (tests/test_ozaki.py: exact integer level sums, FP64 parity, potrf).
+//            with one 1-D bulk copy (cp.async.bulk, TMA engine) that streams whole DRAM pages; a 32-row B tile is
+//            a contiguous quarter of a unit.
+//   warps 8-11 producer (one thread): a pipeline stage holds one k-block -- the S slices of A (8 KB each), then the S slices of B
+//            (2 KB each) in slice order -- filled by 2 S bulk copies; 3 stages at S = 7 (210 KB)
+//   warps 0-7  two consumer warpgroups, 64 rows of the tile each: one m64 n32 k32 wgmma per slice pair into the
+//            register accumulator of its level (16 registers each, 16 S in all).  The level accumulators are summed
+//            smallest level first in FP64, scaled by 2^(ea_i + eb_j) and added to C straight from registers.
+//   raster   CTAs walk the tiles super-tile by super-tile (8 x 32 tiles = 1024 x 1024 of C), so the slices
+//            the concurrently running CTAs read (2 x 1024 rows) stay L2-resident while they are reused
 #include <cuda.h>
 
 #include "common.cuh"
@@ -40,21 +35,17 @@ namespace sgdml {
 
 constexpr int OZ_BITS = 7;
 constexpr int OZ_MAX_S = 7;
-constexpr int OZ_BM = 128, OZ_BN = 64;
+constexpr int OZ_BM = 128, OZ_BN = 32;
 constexpr int OZ_KPAD = 128;                               // the contraction length is padded to a multiple of this
-// BK = bytes (= int8 elements) of k per pipeline unit = width of one swizzle row (64-byte swizzle): a unit is
-// 12 KB, the ring holds 18 of them = two and a half k-blocks of all 7 slices, so the loads of the next k-block
-// never wait for the current one to retire.
+// BK = bytes (= int8 elements) of k per pipeline unit = width of one swizzle row (64-byte swizzle)
 constexpr int OZ_BK = 64;
-constexpr int OZ_RING_BYTES = 216 * 1024;
-constexpr int OZ_MAX_RING = 18;
-constexpr int OZ_UMMA_K = 32;                              // k per tcgen05.mma for 8-bit operands
-constexpr int OZ_TMEM_COLS = 512;                          // S * 64 <= 448, allocation must be a power of two
+constexpr int OZ_RING_BYTES = 210 * 1024;
+constexpr int OZ_MAX_RING = 8;
+constexpr int OZ_MMA_K = 32;                               // k per wgmma for 8-bit operands
 constexpr int OZ_A_BYTES = OZ_BM * OZ_BK;                  // 8 KB: one unit of a 128-row tile (global and shared)
-constexpr int OZ_B_BYTES = OZ_BN * OZ_BK;                  // 4 KB
-constexpr int OZ_UNIT_BYTES = OZ_A_BYTES + OZ_B_BYTES;     // 12 KB; both parts 1024-byte aligned
-constexpr int OZ_GSM = 8, OZ_GSN = 16;                     // super-tile: 8 x 16 tiles = 1024 x 1024 elements of C
-__host__ __device__ inline int oz_ring_slots(int S) { return (2 * S + 4 < OZ_MAX_RING) ? 2 * S + 4 : OZ_MAX_RING; }
+constexpr int OZ_B_BYTES = OZ_BN * OZ_BK;                  // 2 KB
+constexpr int OZ_UNIT_BYTES = OZ_A_BYTES + OZ_B_BYTES;     // 10 KB; both parts 1024-byte aligned
+constexpr int OZ_GSM = 8, OZ_GSN = 32;                     // super-tile: 8 x 32 tiles = 1024 x 1024 elements of C
 
 // ---------------------------------------------------------------- splitting kernels
 // Row exponent + S rounds of (scale by 2^7, round to nearest, subtract): x = 2^e sum_p q_p 2^(-7p), |q_p| <= 64.
@@ -101,7 +92,7 @@ __global__ void __launch_bounds__(256) k_ozaki_split(const double* __restrict__ 
 // Unit-major pre-swizzled layout (what the GEMM reads): units [kb][p][row tile of 128] of 8192 bytes each; inside a
 // unit, row r (0..127) is 64 bytes at r*64 and its 16-byte chunk c is stored at chunk c ^ ((r >> 1) & 3) -- the
 // byte image of the canonical K-major SWIZZLE_64B shared-memory tile, so that a unit is fetched by ONE contiguous
-// bulk copy (a 64-row B tile is the upper or lower half of a unit: the swizzle only involves row bits 1-2).
+// bulk copy (a 32-row B tile is a contiguous quarter of a unit: the swizzle only involves row bits 1-2).
 // One warp per row; every lane converts 4 consecutive k (one 32-bit store per slice).
 __global__ void __launch_bounds__(256) k_ozaki_split_sw(const double* __restrict__ X, int64_t rows, int64_t k,
                                                        int64_t ldx, int S, int64_t rows_pad, int64_t kp,
@@ -138,75 +129,43 @@ __global__ void __launch_bounds__(256) k_ozaki_split_sw(const double* __restrict
   }
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM helpers
-// one lane of the (converged) warp; the compiler keeps the elected lane's address arithmetic on the uniform datapath
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "elect.sync _|p, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// arrives (count 1) on an mbarrier once every tcgen05.mma issued so far by this thread has completed
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, int8 x int8 -> int32, single CTA
-__device__ __forceinline__ void tc_mma_i8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Shared-memory matrix descriptor, K-major operand in the canonical 64-byte-swizzle layout
-// (cute::UMMA::SmemDescriptor, cute/arch/mma_sm100_desc.hpp): rows are 64 bytes apart, an 8-row swizzle atom is
-// 512 bytes, the 16-byte chunk index of a row is XORed with bits [1,3) of the row number.
-//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (1 for swizzled K-major) |
-//   [32,46) stride byte offset >> 4 (512 B between 8-row groups) | [46,48) version = 1 (Blackwell) |
-//   [49,52) base offset = 0 (tiles are 1024-byte aligned) | [61,64) layout type = 4 (SWIZZLE_64B)
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t smem_addr) {
+// ---------------------------------------------------------------- wgmma helpers
+// Shared-memory matrix descriptor (sm_90 wgmma), K-major operand in the canonical 64-byte-swizzle layout: rows are
+// 64 bytes apart, an 8-row swizzle atom is 512 bytes, the 16-byte chunk index of a row is XORed with bits [1,3) of
+// the row number.
+//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1) |
+//   [32,46) stride byte offset >> 4 (512 B between 8-row groups) | [49,52) base offset = 0 (atoms 512-byte aligned) |
+//   [62,64) layout type = 2 (SWIZZLE_64B)
+__device__ __forceinline__ uint64_t gmma_desc_kmajor_sw64(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)((8 * OZ_BK) >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)4 << 61;
+  d |= (uint64_t)2 << 62;
   return d;
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): [4,6) D format = 2 (S32) | [7,10) A format = 1
-// (signed 8-bit) | [10,13) B format = 1 | [15] A major = 0 (K) | [16] B major = 0 (K) | [17,23) N >> 3 |
-// [24,29) M >> 4; dense, no saturation, no negation.
-__host__ __device__ constexpr uint32_t umma_idesc_s8(int M, int N) {
-  return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// 32 lanes x 32 consecutive 32-bit columns: thread t of the warp receives row (lane quadrant base + t)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, int (&v)[32]) {
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
+// D (64 x 32, int32, registers) += A (64 x 32) * B (32 x 32)^T, signed 8-bit, both K-major in shared memory
+__device__ __forceinline__ void wgmma_s8_n32(int* d, uint64_t da, uint64_t db) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n"
+      "}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+      : "l"(da), "l"(db), "n"(1));
 }
 
 struct OzArgs {
@@ -225,19 +184,16 @@ struct OzArgs {
   int* dbg_levels;   // bring-up: raw int32 level sums, [S][m][n] (NULL in production)
   int overwrite;     // 1: C = alpha A B^T (the old contents of C are not read)
   int dbg_flags;     // timing experiments (SGDML_B200_OZAKI_DBG): 1 = no global read-modify-write in the epilogue,
-                     // 2 = no tcgen05.mma issued, 4 = epilogue reads only one level
+                     // 2 = no wgmma issued, 4 = epilogue reads only one level
 };
 
 struct OzSmemTail {
   uint64_t full[OZ_MAX_RING];
   uint64_t empty[OZ_MAX_RING];
-  uint64_t acc_full;
-  uint64_t tmem_empty;
-  uint32_t tmem_base;
 };
 
 constexpr size_t OZ_SMEM_BYTES = (size_t)OZ_RING_BYTES + sizeof(OzSmemTail) + 1024;
-constexpr int OZ_STAGE_LD = 33;  // doubles per row of the epilogue transpose tiles (32 + 1: conflict-free both ways)
+static_assert(OZ_SMEM_BYTES <= 232448, "exceeds 227 KB of shared memory");
 
 // CTA number -> tile (tm, tn), super-tile by super-tile; false if the CTA has no tile
 __device__ __forceinline__ bool oz_tile_of_cta(const OzArgs& p, int64_t cta, int64_t& tm, int64_t& tn) {
@@ -265,90 +221,65 @@ __device__ __forceinline__ bool oz_tile_of_cta(const OzArgs& p, int64_t cta, int
   return true;
 }
 
-// S is a template parameter: the pair schedule of a k-block (28 pairs for S = 7) is then a compile-time list and the
-// single MMA-issuing thread runs straight-line code -- one tcgen05.mma per instruction slot, ring slots advanced
-// with adds and compares.  (The first version computed `unit % ring` with 64-bit runtime divisions, ~150 cycles
-// each, ~70 per k-block: the issuing thread, not the tensor pipe, set the pace -- 5.4 us per k-block against the
-// 0.9 us the MMAs need; profiles/r02_ozaki_bringup.md.)
-// The tcgen05.mma sequence of one k-block.  Several level accumulators are updated by ONE instruction: for slice
-// pa of A, the slices pb = q, q+1, ... of B contribute to the CONSECUTIVE levels pa+q, pa+q+1, ..., whose accumulators
-// are consecutive 64-column blocks of tensor memory, and the B tiles of consecutive slices are consecutive in shared
-// memory -- so A_pa x [B_q; B_q+1; B_q+2; B_q+3]^T is a single M = 128, N = 256 product into 256 consecutive columns.
-// That quarters the number of times an A tile is read from shared memory: an N = 64 product reads 6 KB of operands
-// for 32 tensor-core cycles (192 B/cycle, above the 128 B/cycle the shared memory delivers -- measured: 69 cycles
-// per product, r02), an N = 256 one 12 KB for 128 cycles.  All products come from one thread (they overlap in the
-// accumulators they touch), 13 wide instructions x 2 k-halves per k-block for S = 7 instead of 56.
-template <int S>
-__device__ __forceinline__ void oz_issue_kblock(uint32_t tmem, uint64_t desc_hi, uint32_t a0_lo, uint32_t b0_lo,
-                                                bool first_kb, bool no_mma) {
-#pragma unroll
-  for (int pa = 1; pa <= S; ++pa) {
-    constexpr int GMAX = 4;  // consecutive B slices per instruction (N = 64 * g <= 256)
-#pragma unroll
-    for (int q0 = 1; q0 <= S + 1 - pa; q0 += GMAX) {
-      const int g = (S + 1 - pa - q0 + 1) < GMAX ? (S + 1 - pa - q0 + 1) : GMAX;
-      const uint32_t idesc = umma_idesc_s8(OZ_BM, OZ_BN * g);
-      const uint32_t d_addr = tmem + (uint32_t)(pa + q0 - 2) * OZ_BN;
-#pragma unroll
-      for (int ks = 0; ks < OZ_BK / OZ_UMMA_K; ++ks) {
-        // tiles are 8192 B (A) / 4096 B (B) apart: +512 / +256 in the >> 4 address field; K advance: +2
-        const uint64_t da = desc_hi | (uint64_t)((a0_lo + (uint32_t)(pa - 1) * (OZ_A_BYTES >> 4) + 2 * ks) & 0x3FFF);
-        const uint64_t db = desc_hi | (uint64_t)((b0_lo + (uint32_t)(q0 - 1) * (OZ_B_BYTES >> 4) + 2 * ks) & 0x3FFF);
-        const uint32_t acc = (pa == 1 && ks == 0 && first_kb) ? 0u : 1u;  // slice 1 of A opens every accumulator
-        if (!no_mma) tc_mma_i8(d_addr, da, db, idesc, acc);
-      }
-    }
+// The wgmma sequence of one k32 step for one consumer warpgroup: one m64 n32 k32 product per slice pair (pa, q),
+// pa + q <= S + 1, into the accumulator of level pa + q.  S is a template parameter, so the pair schedule (28 pairs
+// for S = 7) is a compile-time list and the accumulator indices are constants: the level accumulators stay in
+// registers.  Every product has the same shape on its own 16 registers; wider products over several consecutive
+// levels (N = 64, 128) would overlap the windows of other slices' products at other alignments, and ptxas then
+// serialises the whole wgmma pipeline (C7511).
+template <int S, int PA, int Q>
+__device__ __forceinline__ void oz_issue_slice(int* acc, uint64_t desc_hi, uint32_t a_lo, uint32_t b_lo) {
+  if constexpr (PA + Q <= S + 1) {
+    // A tiles are 8192 B apart (+512 in the >> 4 address field), B tiles 2048 B (+128)
+    const uint64_t da = desc_hi | (uint64_t)((a_lo + (uint32_t)(PA - 1) * (OZ_A_BYTES >> 4)) & 0x3FFF);
+    const uint64_t db = desc_hi | (uint64_t)((b_lo + (uint32_t)(Q - 1) * (OZ_B_BYTES >> 4)) & 0x3FFF);
+    wgmma_s8_n32(acc + 16 * (PA + Q - 2), da, db);
+    oz_issue_slice<S, PA, Q + 1>(acc, desc_hi, a_lo, b_lo);
+  }
+}
+template <int S, int PA>
+__device__ __forceinline__ void oz_issue_kstep(int* acc, uint64_t desc_hi, uint32_t a_lo, uint32_t b_lo) {
+  if constexpr (PA <= S) {
+    oz_issue_slice<S, PA, 1>(acc, desc_hi, a_lo, b_lo);
+    oz_issue_kstep<S, PA + 1>(acc, desc_hi, a_lo, b_lo);
   }
 }
 
-constexpr int OZ_THREADS = 192;  // warp 0: producer; warp 1: MMA issuer; warps 2-5: epilogue
-constexpr int OZ_STAGING_BYTES = 4 * 32 * OZ_STAGE_LD * 8;  // the epilogue's transpose tiles (one 32 x 32 per warp)
+constexpr int OZ_CONSUMERS = 256;               // warps 0-7: two consumer warpgroups
+constexpr int OZ_THREADS = OZ_CONSUMERS + 128;  // warps 8-11: producer warpgroup (one thread issues the copies)
 
 // PERSISTENT: a CTA walks over the tiles  blockIdx.x, blockIdx.x + gridDim.x, ...  of the super-tile raster (so the
 // CTAs that run at the same time still work on neighbouring tiles).  The producer streams the k-block stages of one
-// tile after the other without a bubble; the issuer starts a tile as soon as the epilogue warps have READ the previous
-// tile's accumulators out of tensor memory (mbarrier `tmem_empty`); the read-modify-write of C -- and tensor-memory
-// allocation, barrier set-up, CTA launch -- overlap the next tile's products.  Measured before (one tile per CTA,
-// 8192^2 x 1024): 32.8 us per tile of which ~6 us set-up / launch and ~2 us the update of C.
+// tile after the other without a bubble; the read-modify-write of C at the end of a tile overlaps the loads of the
+// next tile's first stages.
 template <int S>
 __global__ void __launch_bounds__(OZ_THREADS, 1) k_ozaki_gemm(const OzArgs p, int64_t n_ids) {
   extern __shared__ unsigned char oz_raw[];
   // 1024-byte alignment for the swizzled tiles
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(oz_raw) + 1023) & ~(uintptr_t)1023);
-  // a pipeline stage holds one k-block: the S slices of A (8 KB each), then the S slices of B (4 KB each) in slice order
+  // a pipeline stage holds one k-block: the S slices of A (8 KB each), then the S slices of B (2 KB each) in slice order
   constexpr int STAGE_BYTES = S * OZ_UNIT_BYTES;
-  constexpr int NST_FIT = (OZ_RING_BYTES - OZ_STAGING_BYTES) / STAGE_BYTES;
+  constexpr int NST_FIT = OZ_RING_BYTES / STAGE_BYTES;
   constexpr int NST = NST_FIT < OZ_MAX_RING ? NST_FIT : OZ_MAX_RING;
   static_assert(NST >= 2, "at least two k-blocks in flight");
-  double* staging = reinterpret_cast<double*>(smem + (size_t)NST * STAGE_BYTES);
   OzSmemTail* tail = reinterpret_cast<OzSmemTail*>(smem + (size_t)OZ_RING_BYTES);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
     for (int i = 0; i < NST; ++i) {
       mbar_init(&tail->full[i], 1);
-      mbar_init(&tail->empty[i], 1);
+      mbar_init(&tail->empty[i], OZ_CONSUMERS / 32);  // one arrival per consumer warp
     }
-    mbar_init(&tail->acc_full, 1);
-    mbar_init(&tail->tmem_empty, 4);  // one arrival per epilogue warp
     fence_mbar_init();
   }
-  if (warp == 0) {  // one warp allocates the tensor memory (and frees it at the end)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tail->tmem_base)),
-                 "n"(OZ_TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tail->tmem_base;
   const int KB = (int)(p.kp / OZ_BK);
-  const uint32_t smem_base = smem_u32(smem);
 
-  if (warp == 0) {
+  if (warp >= OZ_CONSUMERS / 32) {
     // ===================================================== producer: 2 S contiguous bulk copies per k-block
-    if (lane == 0) {
+    // the register file goes to the consumers' level accumulators (128 x 40 + 256 x 232 <= 64 K registers)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (tid == OZ_CONSUMERS) {
       const int64_t a_stride = p.rt_a * (int64_t)OZ_A_BYTES, b_stride = p.rt_b * (int64_t)OZ_A_BYTES;  // per (kb, slice)
       int st = 0;
       uint32_t round = 0;
@@ -376,127 +307,83 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) k_ozaki_gemm(const OzArgs p, in
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer (whole warp waits, one elected lane issues)
-    const uint64_t desc_hi = umma_desc_kmajor(0);  // everything but the 14-bit start-address field
-    int st = 0;
-    uint32_t round = 0, tile_it = 0;
-    for (int64_t id = blockIdx.x; id < n_ids; id += gridDim.x) {
-      int64_t tm, tn;
-      if (!oz_tile_of_cta(p, id, tm, tn)) continue;
-      if (tile_it > 0) {  // the previous tile's accumulators have been read out of tensor memory
-        mbar_wait(&tail->tmem_empty, (tile_it - 1) & 1);
-        tc_fence_after();
-      }
-      for (int kb = 0; kb < KB; ++kb) {
-        mbar_wait(&tail->full[st], round & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a0 = smem_base + (uint32_t)st * STAGE_BYTES;
-          oz_issue_kblock<S>(tmem, desc_hi, (a0 >> 4) & 0x3FFF, ((a0 + S * OZ_A_BYTES) >> 4) & 0x3FFF, kb == 0,
-                             (p.dbg_flags & 2) != 0);
-          tc_commit(&tail->empty[st]);                    // the stage is free once these products have completed
-          if (kb == KB - 1) tc_commit(&tail->acc_full);  // every accumulator of this tile is final
-        }
-        __syncwarp();
-        if (++st == NST) {
-          st = 0;
-          ++round;
-        }
-      }
-      ++tile_it;
-    }
-  } else {
-    // ===================================================== epilogue (warps 2..5 = 128 threads)
-    const int quad = warp & 3;               // TMEM lane quadrant this warp may read
-    const int ew = warp - 2;                 // epilogue warp 0..3 (staging tile)
-    double* stage = staging + (size_t)ew * 32 * OZ_STAGE_LD;  // this warp's 32 x 32 transpose tile
-    uint32_t tile_it = 0;
-    for (int64_t id = blockIdx.x; id < n_ids; id += gridDim.x) {
-      int64_t tm, tn;
-      if (!oz_tile_of_cta(p, id, tm, tn)) continue;
-      const int64_t m0 = tm * OZ_BM, n0 = tn * OZ_BN;
-      const int64_t gr = m0 + quad * 32 + lane;  // row of the tile owned by this thread on the TMEM side
-      const double row_scale = (gr < p.m) ? p.alpha * ldexp(1.0, p.ea[gr]) : 0.0;
-      // column scales 2^(eb_j): lane j holds those of columns j and 32 + j, handed round with shuffles
-      const double cs0 = (n0 + lane < p.n) ? ldexp(1.0, p.eb[n0 + lane]) : 0.0;
-      const double cs1 = (n0 + 32 + lane < p.n) ? ldexp(1.0, p.eb[n0 + 32 + lane]) : 0.0;
-      const int rows_here = (int)max((int64_t)0, min((int64_t)32, p.m - (m0 + quad * 32)));
-      // the old values of C (first half): 32 independent row-contiguous loads in flight during the wait
-      double cold[32];
-      {
-        const int64_t gc = n0 + lane;
-        const bool ok = gc < p.n && !(p.dbg_flags & 1) && !p.overwrite;
-        const double* cp = p.C + (m0 + quad * 32) * p.ldc + gc;
-#pragma unroll
-        for (int r = 0; r < 32; ++r) cold[r] = (ok && r < rows_here) ? cp[(int64_t)r * p.ldc] : 0.0;
-      }
-      mbar_wait(&tail->acc_full, tile_it & 1);
-      tc_fence_after();
-      double acc1[32];  // second half, kept in registers until the first half has left the staging tile
-#pragma unroll 1
-      for (int half = 0; half < OZ_BN / 32; ++half) {
-        double acc[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] = 0.0;
-#pragma unroll 1
-        for (int level = (p.dbg_flags & 4) ? 2 : S + 1; level >= 2; --level) {  // smallest contributions first
-          int v[32];
-          tmem_ld_32x32(tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)((level - 2) * OZ_BN + half * 32), v);
-          const double w = __longlong_as_double((long long)(1023 - OZ_BITS * level) << 52);  // 2^(-7 level), exact
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = fma((double)v[j], w, acc[j]);
-          if (p.dbg_levels != nullptr && gr < p.m) {
-            for (int j = 0; j < 32; ++j) {
-              const int64_t gcj = n0 + half * 32 + j;
-              if (gcj < p.n) p.dbg_levels[((int64_t)(level - 2) * p.m + gr) * p.n + gcj] = v[j];
-            }
-          }
-        }
-        const double cs = half == 0 ? cs0 : cs1;
-        if (half == 0) {
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) stage[lane * OZ_STAGE_LD + j] = acc[j] * row_scale * __shfl_sync(0xffffffffu, cs, j);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc1[j] = acc[j] * row_scale * __shfl_sync(0xffffffffu, cs, j);
-        }
-      }
-      // tensor memory has been read: the issuer may start the next tile while C is updated
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tail->tmem_empty);
-      // ---- C update, transposed through shared memory: thread = row on the TMEM side, lane = column on the global
-      //      side, so that every warp-wide access to C covers 256 contiguous bytes of one row
-#pragma unroll 1
-      for (int half = 0; half < OZ_BN / 32; ++half) {
-        const int64_t gc = n0 + half * 32 + lane;
-        const bool col_ok = gc < p.n && !(p.dbg_flags & 1);
-        double* cp = p.C + (m0 + quad * 32) * p.ldc + gc;
-        if (half == 1) {
-          const bool ok = col_ok && !p.overwrite;
-#pragma unroll
-          for (int r = 0; r < 32; ++r) cold[r] = (ok && r < rows_here) ? cp[(int64_t)r * p.ldc] : 0.0;
-          __syncwarp();  // every lane has read the first half out of the staging tile
-#pragma unroll
-          for (int j = 0; j < 32; ++j) stage[lane * OZ_STAGE_LD + j] = acc1[j];
-        }
-        __syncwarp();
-        if (col_ok) {
-#pragma unroll
-          for (int r = 0; r < 32; ++r)
-            if (r < rows_here) cp[(int64_t)r * p.ldc] = cold[r] + stage[r * OZ_STAGE_LD + lane];
-        }
-      }
-      ++tile_it;
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(OZ_TMEM_COLS) : "memory");
+
+  // ===================================================== consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of a tile
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wg = warp >> 2;
+  const uint64_t desc_hi = gmma_desc_kmajor_sw64(0);  // everything but the 14-bit start-address field
+  const uint32_t smem_base = smem_u32(smem);
+  const bool no_mma = (p.dbg_flags & 2) != 0;
+  int st = 0;
+  uint32_t round = 0;
+  for (int64_t id = blockIdx.x; id < n_ids; id += gridDim.x) {
+    int64_t tm, tn;
+    if (!oz_tile_of_cta(p, id, tm, tn)) continue;
+    int acc[16 * S];  // level L = 2 .. S + 1 in acc[16 (L - 2) .. 16 (L - 2) + 15]
+#pragma unroll
+    for (int i = 0; i < 16 * S; ++i) acc[i] = 0;
+    int prev = -1;  // stage of the previous k-block, released once its products have completed
+    for (int kb = 0; kb < KB; ++kb) {
+      mbar_wait(&tail->full[st], round & 1);
+      if (!no_mma) {
+        const uint32_t a0 = smem_base + (uint32_t)st * STAGE_BYTES + (uint32_t)wg * (64 * OZ_BK);
+        const uint32_t b0 = smem_base + (uint32_t)st * STAGE_BYTES + (uint32_t)(S * OZ_A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < OZ_BK / OZ_MMA_K; ++ks)  // K advance inside the 64-byte swizzle row: +32 B = +2
+          oz_issue_kstep<S, 1>(acc, desc_hi, ((a0 >> 4) + 2 * ks) & 0x3FFF, ((b0 >> 4) + 2 * ks) & 0x3FFF);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's products have completed: its stage may be refilled
+      }
+      if (prev >= 0 && lane == 0) mbar_arrive(&tail->empty[prev]);
+      prev = st;
+      if (++st == NST) {
+        st = 0;
+        ++round;
+      }
+    }
+    wgmma_wait<0>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&tail->empty[prev]);
+
+    // ---- epilogue: thread holds rows r0, r0 + 8 and columns n0 + 8 j + 2 (lane % 4) + {0, 1}, j = 0..3
+    //      (acc[16 l + 4 j + {0, 1}] on row r0, acc[16 l + 4 j + {2, 3}] on row r0 + 8)
+    const int64_t m0 = tm * OZ_BM, n0 = tn * OZ_BN;
+    const int64_t r0 = m0 + 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    double v[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) v[i] = 0.0;
+#pragma unroll
+    for (int level = S + 1; level >= 2; --level) {  // smallest contributions first
+      if ((p.dbg_flags & 4) && level > 2) continue;
+      const double w = __longlong_as_double((long long)(1023 - OZ_BITS * level) << 52);  // 2^(-7 level), exact
+#pragma unroll
+      for (int i = 0; i < 16; ++i) v[i] = fma((double)acc[16 * (level - 2) + i], w, v[i]);
+      if (p.dbg_levels != nullptr) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int64_t r = r0 + 8 * ((i >> 1) & 1), c = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+          if (r < p.m && c < p.n) p.dbg_levels[((int64_t)(level - 2) * p.m + r) * p.n + c] = acc[16 * (level - 2) + i];
+        }
+      }
+    }
+    if (p.dbg_flags & 1) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t r = r0 + 8 * h;
+      if (r >= p.m) continue;
+      const double row_scale = p.alpha * ldexp(1.0, p.ea[r]);
+      double* crow = p.C + r * p.ldc;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        if (((i >> 1) & 1) != h) continue;
+        const int64_t c = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        if (c >= p.n) continue;
+        const double upd = v[i] * row_scale * ldexp(1.0, p.eb[c]);
+        crow[c] = p.overwrite ? upd : crow[c] + upd;
+      }
+    }
   }
 }
 
@@ -597,7 +484,7 @@ int ozaki_gemm(const OzOperand& a, const OzOperand& b, int64_t m, int64_t n, dou
 }
 
 // Workspace of the symmetric update used by potrf: allocated once per factorisation (a cudaMalloc /
-// cudaFree pair costs ~20 ms in a process that holds tens of GB -- see csrc/core.cu), reused by every
+// cudaFree pair costs milliseconds in a process that holds tens of GB -- see csrc/core.cu), reused by every
 // outer step, no host synchronisation in between.
 int ozaki_syrk_workspace_bytes(int64_t max_rows, int64_t max_k, int S, size_t* plane_bytes, size_t* exp_bytes) {
   *plane_bytes = oz_plane_bytes(max_rows, max_k, S);

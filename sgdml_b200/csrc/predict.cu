@@ -3,7 +3,7 @@
 // caches), predict.py:551-601 (set_alphas), predict.py:1286-1288 (output scaling),
 // torchtools.py:877-1046 (_forward).
 //
-// B200 design (not a port of either reference engine):
+// Design (not a port of either reference engine):
 //  * Permutations are applied to the QUERY, never to the model: with e = perm_p[d],
 //      delta_p[d] = x[d] - X_m[perm_p[d]]  ==  q_p[e] - X_m[e],  q_p[e] = x[pinv_p[e]],
 //    so query b becomes S "virtual rows" q_{b,p} and the model stays an (M, D) pair of
@@ -12,7 +12,7 @@
 //    (B, M*S, D) temporary on the GPU (torchtools.py:964-966).
 //  * The sum over training points is two GEMM-shaped contractions around an elementwise
 //    Matern-5/2 transform -- the same shape as attention -- and both run on the FP64
-//    tensor pipe (mma.sync m8n8k4.f64, SASS DMMA; tcgen05 has no f64 kind):
+//    tensor pipe (mma.sync m8n8k4.f64, SASS DMMA; wgmma has no f64 type):
 //      GEMM1: S1 = Q Xc^T, S2 = Q JA^T                      (contraction over D)
 //      n^2 = |q|^2 + |Xc_m|^2 - 2 S1,  a = S2 - Xc_m.JA_m,  c1, c2 = Matern factors
 //      GEMM2: G = (sum_m c1) Q - C1 Xc - C2 JA             (contraction over M)
@@ -522,8 +522,8 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
 
 // ============================================================== main kernel, two-group ("ping-pong") form
 // The sweep of k_predict_main alternates tensor-pipe phases (GEMM1, GEMM2) with phases that leave the pipe idle (the
-// split-k reduction + Matern transform, two CTA-wide barriers per tile): measured 77 % DMMA-active at BASELINE config 2
-// (profiles/r01_ncu_predict_aspirin.txt).  Here the 8 warps form TWO groups of 4 (one warp of each group per SM
+// split-k reduction + Matern transform, two CTA-wide barriers per tile), which leaves the DMMA pipe idle for part of
+// every tile.  Here the 8 warps form TWO groups of 4 (one warp of each group per SM
 // sub-partition) that own half of the virtual query rows each and synchronise only among themselves (named
 // barriers).  Group 0 runs  GEMM1(t) | transform(t) | GEMM2(t);  group 1 runs the same loop rotated,
 // GEMM2(t) GEMM1(t+1) | transform(t+1), so the transform / barrier phases of one group fall into the tensor phases of
@@ -1077,7 +1077,7 @@ __global__ void __launch_bounds__(128) k_predict_finish(const double* __restrict
 }
 
 // The same for batches of a few queries (the MD latency path: one geometry per call).  There the one-CTA-per-query form
-// is a chain of S * n_splits dependent L2 round trips per thread (126 at BASELINE config 2, B = 1: ~25 us); here 1024
+// is a chain of S * n_splits dependent L2 round trips per thread (126 at BASELINE config 2, B = 1); here 1024
 // threads split every descriptor entry's terms into `parts` interleaved partial sums (fixed order: bit-reproducible).
 __global__ void __launch_bounds__(1024) k_predict_finish_small(const double* __restrict__ G, const double* __restrict__ Erow,
                                                                const double* __restrict__ gq, const int* __restrict__ perm,
@@ -1228,7 +1228,7 @@ struct sgdml_b200_model {
   double sig = 0, std = 1, c = 0;
   double *X = nullptr;    // (M, D) raw descriptors (training-point queries)
   double *Xc = nullptr, *JA = nullptr, *mm = nullptr, *xja = nullptr, *mu = nullptr;
-  // large descriptors: the four contractions on the tcgen05 tensor cores through int8 slices (csrc/ozaki.cu) when
+  // large descriptors: the four contractions on the int8 tensor cores (wgmma) through int8 slices (csrc/ozaki.cu) when
   // oz_s >= 2; the slices of the model matrices are kept (those of JA / JA^T are refreshed by set_alphas)
   int oz_s = 0;
   OzOperand ozXc, ozJA, ozXcT, ozJAT;
@@ -1354,10 +1354,9 @@ int launch_main(int cfg, const PredictArgs& a, int n_splits, cudaStream_t s) {
   }
   if (g_predict_variant == 5 && cfg == 0) return launch_main_t<Cfg40o16>(a, n_splits, s);
   if (g_predict_variant == 0) {
-    // default: the measured-fastest kernel per size (tools/predict_variants.py, 65536 queries, M = 1000, S = 6, ms per
-    // call round-1 kernel -> one-barrier kernel): DP = 72: 9.09 -> 8.89, 112: 13.98 -> 12.73, 160: 20.07 -> 18.12,
-    // 224 (BASELINE config 2): 25.81 -> 24.01; DP = 40 (config 1) stays on the round-1 kernel (1.31 vs 1.51 ms: the
-    // doubled C1 / C2 buffers cost it its second CTA per SM)
+    // default: the fastest kernel per size when the variants were timed (tools/predict_variants.py, 65536 queries,
+    // M = 1000, S = 6): the one-barrier kernel for DP >= 72; DP = 40 (config 1) stays on the round-1 kernel (the
+    // doubled C1 / C2 buffers cost the one-barrier form its second CTA per SM).  Not re-timed on H100.
     switch (cfg) {
       case 1: return launch_main_t<Cfg72o>(a, n_splits, s);
       case 2: return launch_main_t<Cfg112o>(a, n_splits, s);
@@ -1417,7 +1416,7 @@ void free_ws(sgdml_b200_model* m) {
 int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
   sgdml_b200_model::WS& w = m->ws[slot];
   if (!m->large) {  // room for the per-split output planes of small batches (<= ~300 CTAs x BQ rows)
-    const int64_t min_geo = (int64_t)(2 * 148 + 8) * m->BQ / m->S + 1;
+    const int64_t min_geo = (int64_t)(2 * num_sms() + 8) * m->BQ / m->S + 1;
     n_geo = std::max<int64_t>(n_geo, std::min<int64_t>(min_geo, chunk_geos(m)));
   }
   if (n_geo <= w.geo) return 0;
@@ -1515,7 +1514,7 @@ int run_queries(sgdml_b200_model* m, int slot, const double* xq, const double* g
     g.mode = 0;
     g.tri = 0;
     g.abort_flag = nullptr;
-    // The four contractions on the tcgen05 tensor cores through exact int8 slice products (csrc/ozaki.cu): the
+    // The four contractions on the int8 tensor cores (wgmma) through exact int8 slice products (csrc/ozaki.cu): the
     // slices of the model matrices are kept with the model, those of Q, C1, C2 are cut per batch; everything is
     // stream-ordered (this path runs once per CG iteration inside sgdml_b200_pcg).  Slice count: m->oz_s
     // (tools/ozaki_study.py predict: forces 8.8e-9 / 6.5e-11 / 5.4e-13 vs FP64 for 4 / 5 / 6 slices).
@@ -1781,8 +1780,8 @@ int sgdml_b200_model_create(sgdml_b200_model** out, int64_t n_atoms, int64_t n_t
 
 namespace {
 
-// SGDML_B200_GRAPH=0 switches the CUDA-graph replay of small host-buffer batches off (measured on B200, B = 1,
-// NumPy in/out: 54 vs 65 us per call at BASELINE config 1, 92 vs 105 us at config 2)
+// SGDML_B200_GRAPH=0 switches the CUDA-graph replay of small host-buffer batches off (the replay saves launch
+// overhead on the B = 1 NumPy in/out path of MD stepping)
 bool g_graph_enabled() {
   const char* e = getenv("SGDML_B200_GRAPH");
   return e != nullptr ? (e[0] == '1') : true;

@@ -2,7 +2,7 @@
 // triangular solves replacing scipy.linalg.cho_factor / cho_solve (LAPACK dpotrf/dpotrs) in
 // sgdml/solvers/analytic.py:94-99 and iterative.py:447-449.
 //
-// B200 design.  K stays in HBM from assembly to the solve (the reference round-trips every
+// Design.  K stays in HBM from assembly to the solve (the reference round-trips every
 // block-column through the host, torchtools.py:233).  Blocked right-looking Cholesky on the
 // lower triangle of the row-major matrix, panel width NB = 128:
 //   1. k_potf2_tile   one CTA factorises the 128 x 128 diagonal block in shared memory;
@@ -10,7 +10,7 @@
 //                     (no explicit inverse: diagonal blocks of sGDML kernels have condition
 //                     numbers ~1e11, lam = 1e-10) and also emit -X into a workspace;
 //   3. k_gemm_nt      trailing update C += (-X) X^T on the FP64 tensor pipe (mma.sync
-//                     m8n8k4.f64 -> SASS DMMA; tcgen05 has no f64 kind), lower tiles only,
+//                     m8n8k4.f64 -> SASS DMMA; wgmma has no f64 type), lower tiles only,
 //                     4-stage cp.async pipeline, fragment-major shared-memory tiles.
 // FP64 throughout: TF32/BF16 factorisations cannot deliver 1e-6 forces at cond ~4e11.
 #include <cuda.h>  // CUtensorMap types only: cuTensorMapEncodeTiled is resolved at run time (no libcuda link)
@@ -56,7 +56,7 @@ __global__ void __launch_bounds__(256) k_gemm_nt(const GemmArgs p) {
   int64_t ti, tj;
   if (p.tri) {
     // L2-friendly rasterisation of the lower triangle: super-tiles of GS x GS row tiles are
-    // enumerated in triangular order, tiles inside a super-tile row-major, so that the ~148
+    // enumerated in triangular order, tiles inside a super-tile row-major, so that the ~132
     // co-resident CTAs share a small set of A and B operand panels.
     constexpr int r = G::BM / G::BN;
     constexpr int GS = 8;
@@ -853,15 +853,15 @@ constexpr int NBO_MAX = 1024;
 // Dependencies: inner(ob+1) needs a(ob); a(ob+1) and b(ob+1) need b(ob) (same tiles, += updates);
 // b(ob) reads the -X workspace of block ob, so the workspace is double buffered.
 // Slice count of the lazy trailing updates (csrc/ozaki.cu): -1 = automatic, 0 = FP64 DMMA, 2..7 = int8 slices on the
-// tcgen05 tensor cores.  Automatic: SGDML_B200_OZAKI_SLICES if set; otherwise 7 slices for the analytic solver's
-// factorisation when n >= 16384 (where the trailing updates are > 90 % of the time), FP64 for every other caller
-// (the Nystroem factor's inner matrix tolerates no more than 1e-14 of regularisation, iterative.py:305-307).
+// wgmma tensor cores.  Automatic: SGDML_B200_OZAKI_SLICES if set, otherwise FP64.  Measured on an H100 SXM at a 400 W
+// power limit (BASELINE config 2, n = 63 000): solve 3.46 s with FP64 DMMA trailing updates, 3.65 s with 7 int8 slices
+// (at a 700 W limit: 2.84 s against 2.88 s) -- the FP64 path is both faster and exact there.
 static int g_solve_slices = -1;
-static int resolve_slices(int64_t n, bool analytic_solver) {
+static int resolve_slices() {
   if (g_solve_slices >= 0) return g_solve_slices;
   const char* oz = getenv("SGDML_B200_OZAKI_SLICES");
   if (oz != nullptr) return std::max(0, std::min(7, atoi(oz)));
-  return (analytic_solver && n >= 16384) ? 7 : 0;
+  return 0;
 }
 
 int potrf_device(double* A, int64_t n, int64_t lda, int* info_host, cudaStream_t s, bool analytic_solver) {
@@ -871,13 +871,13 @@ int potrf_device(double* A, int64_t n, int64_t lda, int* info_host, cudaStream_t
   cudaEvent_t evI[2] = {nullptr, nullptr}, evB[2] = {nullptr, nullptr};
   // outer block: wide for large matrices (fewer passes over C), narrower when n is small
   const int NBO = (n >= 16384) ? NBO_MAX : ((n >= 4096) ? 512 : 256);
-  // Measured on B200 (n = 32768): 0.423 s with look-ahead vs 0.413 s without -- the 1-CTA-per-SM GEMM leaves
-  // no room for the panel kernels to co-run, so the split only costs GEMM efficiency.  Kept behind an
+  // Measured slower with look-ahead than without -- the 1-CTA-per-SM GEMM leaves no room for the panel kernels to
+  // co-run, so the split only costs GEMM efficiency.  Kept behind an
   // environment switch (SGDML_B200_LOOKAHEAD=1) until the trailing GEMM is made persistent on a subset of SMs.
   const char* la = getenv("SGDML_B200_LOOKAHEAD");
   const bool lookahead = (la && la[0] == '1') && (n > 2 * (int64_t)NBO) && !profiling_enabled();
-  const int oz_slices = resolve_slices(n, analytic_solver);
-  int8_t* oz_planes = nullptr;  // slice planes of the current outer panel (tcgen05 path)
+  const int oz_slices = resolve_slices();
+  int8_t* oz_planes = nullptr;  // slice planes of the current outer panel (int8 path)
   int* oz_exps = nullptr;
   auto cleanup = [&]() {  // (the device buffers are persistent workspaces: csrc/core.cu ws_get)
     if (s2) cudaStreamDestroy(s2);
@@ -964,8 +964,7 @@ int potrf_device(double* A, int64_t n, int64_t lda, int* info_host, cudaStream_t
       g.abort_flag = d_info;
       if (!lookahead) {
         if (oz_slices > 0) {
-          // EXPERIMENTAL (csrc/ozaki.cu, not validated on hardware yet): the trailing update on the tcgen05
-          // tensor cores, C -= X X^T through exact int8 slice products
+          // the trailing update on the int8 tensor cores (csrc/ozaki.cu), C -= X X^T through exact int8 slice products
           const double* X = A + K1 * lda + K0;
           SG_TRY(ozaki_syrk_device(rem, K1 - K0, -1.0, X, lda, A + K1 * lda + K1, lda, oz_slices, oz_planes, oz_exps, s));
           continue;
@@ -1275,6 +1274,8 @@ int sgdml_b200_set_solve_slices(int n_slices) {
   g_solve_slices = n_slices;
   return 0;
 }
+
+int sgdml_b200_get_solve_slices(void) { return resolve_slices(); }
 
 int sgdml_b200_set_gemm_variant(int v) {
   g_gemm_variant = v;

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's ``sgdml.utils.desc.Desc`` for the hot path.
 
 Same method names / argument meaning as utils/desc.py:242-539, but every numeric method
-runs on the B200 through the C ABI (no NumPy fallback).  ``Desc.perm`` /
+runs on the GPU through the C ABI (no NumPy fallback).  ``Desc.perm`` /
 ``tril_perms_lin`` are the integer host routines of the library (bit-exact).
 """
 

@@ -12,7 +12,7 @@ the reference's own class, unchanged.
 
 def install_into_reference(ref_pkg=None):
     """Rebinds ``sgdml.cli.GDMLTrain`` / ``sgdml.cli.GDMLPredict`` (and the names the training module itself uses for
-    its predictor, train.py:1136) to the B200 engine.  `ref_pkg`: the imported reference package (default: import
+    its predictor, train.py:1136) to the engine.  `ref_pkg`: the imported reference package (default: import
     ``sgdml``).  Returns (train_class, predict_class)."""
     import importlib
 

@@ -1,4 +1,4 @@
-"""ASE calculator on the B200 engine -- the reference's ``sgdml.intf.ase_calc.SGDMLCalculator``
+"""ASE calculator on the H100 engine -- the reference's ``sgdml.intf.ase_calc.SGDMLCalculator``
 (intf/ase_calc.py:36-110): same constructor arguments, unit handling and ``results`` layout, float64 end to end
 (the reference's torch path downcasts positions to float32, predict.py:1197-1201).
 

@@ -1,5 +1,5 @@
 """``GDMLPredict`` -- the reference's public prediction API (sgdml/predict.py:248-1294)
-backed by the B200 engine.
+backed by the H100 engine.
 
 Drop-in for ``sgdml.predict.GDMLPredict`` on the hot path: same constructor signature,
 ``predict(R, return_E)``, ``set_R_desc``, ``set_R_d_desc``, ``set_alphas``,
@@ -104,7 +104,7 @@ class GDMLPredict(object):
             self._handle = None
 
     def set_contraction_slices(self, slices):
-        """Extension (large descriptors, D > 256): run the predictor's four GEMMs on the tcgen05 tensor cores through
+        """Extension (large descriptors, D > 256): run the predictor's four GEMMs on the int8 tensor cores (wgmma) through
         `slices` exact int8 slices per operand (4..7) instead of FP64 DMMA (0).  See include/sgdml_b200.h."""
         _lib.check(
             _lib.lib().sgdml_b200_model_set_contraction_slices(self._handle, int(slices), _lib.current_stream()),

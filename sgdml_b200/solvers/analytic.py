@@ -1,4 +1,4 @@
-"""``Analytic`` -- closed-form solver (reference sgdml/solvers/analytic.py:37-159) on the B200.
+"""``Analytic`` -- closed-form solver (reference sgdml/solvers/analytic.py:37-159) on the H100.
 
 Assembly writes -K straight into HBM (scale = -1, analytic.py:65), lam is added to the
 diagonal, and the FP64 Cholesky factorisation + two triangular solves run on the device
@@ -76,10 +76,11 @@ class Analytic(object):
                 'solve_analytic',
             )
         except np.linalg.LinAlgError:
-            # The factorisation overwrote K: assemble it again.  First retry with all-FP64 trailing updates (the
-            # default for large n runs them through int8 slices on the tcgen05 tensor cores, whose 2e-14 error
-            # could push a borderline matrix over the edge); only then the reference's fallback, a solver that
-            # makes fewer assumptions (host LU, analytic.py:101-114).
+            # The factorisation overwrote K: assemble it again.  If the trailing updates ran on int8 slices (selected
+            # with SGDML_B200_OZAKI_SLICES / sgdml_b200_set_solve_slices), whose 2e-14 error could push a borderline
+            # matrix over the edge, first retry with all-FP64 ones; then the reference's fallback, a solver that
+            # makes fewer assumptions (host LU, analytic.py:101-114).  A failed FP64 factorisation is deterministic
+            # and is not repeated.
             import scipy.linalg
 
             def reassemble():
@@ -91,22 +92,26 @@ class Analytic(object):
             del K
             K = reassemble()
             L = _lib.lib()
-            L.sgdml_b200_set_solve_slices(0)
-            try:
-                _lib.check(
-                    L.sgdml_b200_solve_analytic(K.data_ptr(), n, K.shape[1], float(lam), _lib.ptr(y), _lib.ptr(alphas), _lib.current_stream()),
-                    'solve_analytic',
-                )
-                self.log.warning('Cholesky factorisation with int8-sliced trailing updates failed; the FP64 factorisation succeeded.')
-            except np.linalg.LinAlgError:
+            solved = False
+            if L.sgdml_b200_get_solve_slices() > 0:
+                L.sgdml_b200_set_solve_slices(0)
+                try:
+                    _lib.check(
+                        L.sgdml_b200_solve_analytic(K.data_ptr(), n, K.shape[1], float(lam), _lib.ptr(y), _lib.ptr(alphas), _lib.current_stream()),
+                        'solve_analytic',
+                    )
+                    solved = True
+                    self.log.warning('Cholesky factorisation with int8-sliced trailing updates failed; the FP64 factorisation succeeded.')
+                except np.linalg.LinAlgError:
+                    del K
+                    K = reassemble()
+                finally:
+                    L.sgdml_b200_set_solve_slices(-1)
+            if not solved:
                 self.log.warning('Cholesky factorisation failed (matrix not positive definite); falling back to LU.')
-                del K
-                K = reassemble()
                 Kh = K[:, :n].cpu().numpy()
                 Kh[np.diag_indices_from(Kh)] += lam
                 alphas = -scipy.linalg.solve(Kh, y, overwrite_a=True, check_finite=False)
-            finally:
-                L.sgdml_b200_set_solve_slices(-1)
         ev[2].record()
         torch.cuda.synchronize()
         self.timings = {

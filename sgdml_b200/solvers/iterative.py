@@ -1,5 +1,5 @@
 """``Iterative`` -- Nystroem-preconditioned CG (reference sgdml/solvers/iterative.py:60-866) on
-the B200 engine.
+the H100 engine.
 
 Same algorithm and knobs as the reference: leverage-score sampling of inducing columns
 (iterative.py:353-411), the Nystroem factor B = L_inv_K_mn (iterative.py:208-351), the
@@ -34,7 +34,7 @@ NOT_DONE = 0
 
 def _dot(a, b):
     """Inner product of two CG vectors without the BLAS thread pool: on the 128-thread host waking the
-    pool up between two GPU calls cost ~10-20 ms per call (more than the K.v product itself)."""
+    pool up between two GPU calls can cost more than the K.v product itself."""
     return float(np.einsum('i,i->', a, b))
 
 
@@ -268,8 +268,9 @@ class Iterative(object):
         v_F = np.zeros(n)
         model = self.gdml_train.create_model(task, 'cg', R_desc, R_d_desc, tril_perms_lin, 1.0, v_F)
         self.gdml_predict = GDMLPredict(model, max_memory=self._max_memory, max_processes=self._max_processes)
-        # K.v on the tcgen05 tensor cores for large descriptors (5 exact int8 slices: forces within 6.5e-11 of the FP64
-        # contractions, CG tolerance 1e-4); SGDML_B200_OZAKI_PREDICT_SLICES (0 = FP64) overrides
+        # K.v on the int8 tensor cores (wgmma) for large descriptors (5 exact int8 slices: forces within 6.5e-11 of the FP64
+        # contractions, CG tolerance 1e-4; 1.43x the FP64 contractions' throughput at BASELINE config 3 on an H100 at 400 W);
+        # SGDML_B200_OZAKI_PREDICT_SLICES (0 = FP64) overrides
         import os
 
         if 'SGDML_B200_OZAKI_PREDICT_SLICES' not in os.environ:

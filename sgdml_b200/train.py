@@ -1,4 +1,4 @@
-"""``GDMLTrain`` -- the reference's training API (sgdml/train.py:305-1258) on the B200 engine.
+"""``GDMLTrain`` -- the reference's training API (sgdml/train.py:305-1258) on the H100 engine.
 
 Hot path only: ``train(task)``, ``create_model``, ``_recov_int_const`` and
 ``_assemble_kernel_mat`` keep the reference's names, arguments and model/.npz layout
@@ -249,8 +249,8 @@ class GDMLTrain(object):
         E_ref = np.squeeze(task['E_train'])
 
         # slope of the least-squares line E_ref ~ e_fact * E_pred + b and the correlation coefficient, in closed form
-        # (the reference calls np.linalg.lstsq / np.corrcoef, train.py:1150-1170; on a 128-thread host the LAPACK
-        # thread pool of that 1000 x 2 problem was measured at up to 0.6 s of a 1.3 s training run)
+        # (the reference calls np.linalg.lstsq / np.corrcoef, train.py:1150-1170; on a many-core host waking the LAPACK
+        # thread pool for that 1000 x 2 problem can cost more than the rest of the training run)
         dp = E_pred - (E_pred.sum() / E_pred.size)
         dr = E_ref - (E_ref.sum() / E_ref.size)
         spp, srr, spr = float((dp * dp).sum()), float((dr * dr).sum()), float((dp * dr).sum())

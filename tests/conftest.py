@@ -18,7 +18,7 @@ GOLDEN_CASES = sorted(
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on an H100 with -m gpu)')
 
 
 def load_golden(name):

@@ -11,6 +11,7 @@ GPU box):
     PYTHONPATH=baseline/_ref:. python tests/golden/make_golden.py c60
     PYTHONPATH=baseline/_ref:. python tests/golden/make_golden.py n100
     PYTHONPATH=baseline/_ref:. python tests/golden/make_golden.py pbc_ecstr
+    PYTHONPATH=baseline/_ref:. python tests/golden/make_golden.py dropin
 
 Each fixture holds the inputs (geometries, labels, perms, sig, lam, query geometries) and
 the reference outputs of every hot-path stage: tril_perms_lin (Desc.perm / train.py:897-904),
@@ -316,8 +317,60 @@ def main_n100():
     print('big_n100_m2_s12: K_cols', K_cols.shape, 'size %.0f KB' % (os.path.getsize(out) / 1024))
 
 
+def main_dropin():
+    """What the drop-in behind the reference's CLI is compared against (tests/test_dropin_cli.py): the parameter lists of the
+    reference's GDMLTrain / GDMLPredict entry points, and a task made by the reference's own create_task (permutations
+    discovered by the reference) with the model its GDMLTrain.train makes of it (keys, shapes, dtypes, c, std) and that
+    model's predictions by the reference's GDMLPredict."""
+    import inspect
+    import json
+
+    out_dir = os.path.join(HERE, 'dropin')
+    os.makedirs(out_dir, exist_ok=True)
+    N, n_train, n_valid, sig = 9, 40, 20, 20
+    R = synth.geometries(N, n_train + n_valid + 18, 0)
+    E, F = synth.toy_pes(R)
+    ds = {'type': 'd', 'code_version': 'synthetic', 'name': 'synthetic_9', 'theory': 'toy_inverse_distance',
+          'z': np.arange(1, N + 1) % 9 + 1, 'R': R, 'E': E, 'F': F, 'r_unit': 'Ang', 'e_unit': 'kcal/mol'}
+    from sgdml.utils import io
+
+    ds['md5'] = io.dataset_md5(ds)
+    ds = {k: np.asarray(v) for k, v in ds.items()}  # as the CLI hands it over: loaded from the .npz
+    np.random.seed(0)
+    gdml_train = GDMLTrain(max_processes=1, use_torch=False)
+    task = gdml_train.create_task(ds, n_train, ds, n_valid, sig)
+    model = gdml_train.train(task)
+    Rq = R[-8:].reshape(8, -1)
+    E_q, F_q = GDMLPredict(model, max_processes=1, use_torch=False).predict(Rq)
+    np.savez_compressed(os.path.join(out_dir, 'reference_task.npz'), R_query=Rq, **task)
+
+    def params(f):
+        return list(inspect.signature(f).parameters)
+
+    keys = sorted(model.keys())
+    ref = {
+        'reference_version': sgdml.__version__,
+        'signatures': {
+            'GDMLTrain.__init__': params(GDMLTrain.__init__), 'GDMLTrain.train': params(GDMLTrain.train),
+            'GDMLPredict.__init__': params(GDMLPredict.__init__), 'GDMLPredict.predict': params(GDMLPredict.predict),
+        },
+        'model_keys': keys,
+        'model_shapes': {k: list(np.asarray(model[k]).shape) for k in keys},
+        'model_dtypes': {k: str(np.asarray(model[k]).dtype) for k in keys},
+        'c': float(model['c']),
+        'std': float(model['std']),
+        'E_query': E_q.tolist(),
+        'F_query': F_q.tolist(),
+    }
+    with open(os.path.join(out_dir, 'reference_model.json'), 'w') as f:
+        json.dump(ref, f, indent=1)
+    print('dropin: task keys', sorted(task.keys()))
+
+
 if __name__ == '__main__':
-    if len(sys.argv) > 1 and sys.argv[1] == 'n100':
+    if len(sys.argv) > 1 and sys.argv[1] == 'dropin':
+        main_dropin()
+    elif len(sys.argv) > 1 and sys.argv[1] == 'n100':
         main_n100()
     elif len(sys.argv) > 1 and sys.argv[1] == 'c60':
         main_c60()

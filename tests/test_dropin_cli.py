@@ -1,74 +1,97 @@
-"""(f)1 -- the engine as a drop-in behind the reference's own CLI (north_star; INTEGRATION.md section 4).
-The reference package is the unmodified copy under baseline/_ref (it travels to the GPU box; /root/reference does
-not).  The CLI functions call os._exit on errors, so every flow runs in a subprocess (tools/reference_cli_dropin.py)."""
+"""The engine as a drop-in behind the reference's own CLI (INTEGRATION.md section 4), checked against what the unmodified
+reference recorded in tests/golden/dropin/ (make_golden.py dropin): the parameter lists of its GDMLTrain / GDMLPredict
+entry points, and a task made by its create_task with the model its GDMLTrain.train makes of it.  The rebinding of
+`install_into_reference` is checked on a stub package shaped like the reference (a `cli` and a `train` module)."""
 
-import inspect
 import json
 import os
-import subprocess
 import sys
+import types
 
 import numpy as np
 import pytest
 
-from conftest import ROOT, rel_err
+from conftest import GOLDEN_DIR, rel_err
 
-REF_DIR = os.path.join(ROOT, 'baseline', '_ref')
-needs_ref = pytest.mark.skipif(not os.path.isfile(os.path.join(REF_DIR, 'sgdml', 'cli.py')), reason='baseline/_ref not installed')
-
-
-def _run_tool(engine, workdir):
-    env = dict(os.environ)
-    env['OMP_NUM_THREADS'] = '4'
-    res = subprocess.run(
-        [sys.executable, os.path.join(ROOT, 'tools', 'reference_cli_dropin.py'), '--engine', engine, '--workdir', str(workdir)],
-        env=env, capture_output=True, text=True, timeout=600,
-    )
-    for ln in res.stdout.splitlines():
-        if ln.startswith('DROPIN_JSON '):
-            return json.loads(ln[len('DROPIN_JSON '):])
-    raise AssertionError('no result from the CLI flow (rc %d):\n%s\n%s' % (res.returncode, res.stdout[-2000:], res.stderr[-2000:]))
+DROPIN_DIR = os.path.join(GOLDEN_DIR, 'dropin')
 
 
-@needs_ref
-def test_install_rebinds_reference_cli_and_signatures_match():
-    """CPU: the two names the reference CLI instantiates are rebound; constructor / train / predict signatures of
-    the engine classes equal the reference's (train.py:306, 836-841; predict.py:249-258, 1146)."""
-    code = (
-        'import sys, json, inspect\n'
-        'sys.path.insert(0, %r); sys.path.insert(0, %r)\n'
-        'import sgdml, sgdml.cli, sgdml.train, sgdml.predict\n'
-        'RefT, RefP = sgdml.train.GDMLTrain, sgdml.predict.GDMLPredict\n'
-        'from sgdml_b200.integration import install_into_reference\n'
-        'T, P = install_into_reference(sgdml)\n'
-        'sig = lambda f: list(inspect.signature(f).parameters)\n'
-        'out = dict(bound=sgdml.cli.GDMLTrain is T and sgdml.cli.GDMLPredict is P,\n'
-        '           init_t=[sig(T.__init__), sig(RefT.__init__)], train=[sig(T.train), sig(RefT.train)],\n'
-        '           init_p=[sig(P.__init__), sig(RefP.__init__)], predict=[sig(P.predict)[:3], sig(RefP.predict)[:3]],\n'
-        '           borrowed=T.create_task is RefT.create_task and T.draw_strat_sample is RefT.draw_strat_sample)\n'
-        'print(json.dumps(out))\n'
-    ) % (ROOT, REF_DIR)
-    res = subprocess.run([sys.executable, '-c', code], capture_output=True, text=True, timeout=300)
-    assert res.returncode == 0, res.stderr[-2000:]
-    out = json.loads(res.stdout.strip().splitlines()[-1])
-    assert out['bound'] and out['borrowed']
-    for k in ('init_t', 'train', 'init_p', 'predict'):
-        assert out[k][0] == out[k][1], (k, out[k])
+def _reference():
+    with open(os.path.join(DROPIN_DIR, 'reference_model.json')) as f:
+        return json.load(f)
 
 
-@needs_ref
+def _params(f):
+    import inspect
+
+    return list(inspect.signature(f).parameters)
+
+
+def _stub_reference(monkeypatch):
+    """A package `refstub` with the two modules install_into_reference touches: `cli` (module-level GDMLTrain /
+    GDMLPredict names) and `train` (a GDMLTrain owning the host-side task functions the engine borrows)."""
+
+    class RefTrain(object):
+        def create_task(self, *a, **k):
+            return 'task'
+
+        def create_task_from_model(self, *a, **k):
+            return 'task from model'
+
+        def draw_strat_sample(self, *a, **k):
+            return 'sample'
+
+    pkg = types.ModuleType('refstub')
+    cli = types.ModuleType('refstub.cli')
+    train = types.ModuleType('refstub.train')
+    cli.GDMLTrain, cli.GDMLPredict = RefTrain, object
+    train.GDMLTrain = RefTrain
+    pkg.cli, pkg.train = cli, train
+    for name, mod in (('refstub', pkg), ('refstub.cli', cli), ('refstub.train', train)):
+        monkeypatch.setitem(sys.modules, name, mod)
+    return pkg, RefTrain
+
+
+def test_install_rebinds_reference_cli_and_signatures_match(monkeypatch):
+    """CPU: the two names the reference CLI instantiates are rebound, the task functions are borrowed from the
+    reference's class unchanged, and the constructor / train / predict parameter lists of the engine classes equal the
+    reference's (train.py:306, 836-841; predict.py:249-258, 1146)."""
+    import sgdml_b200
+    from sgdml_b200.integration import install_into_reference
+
+    pkg, RefTrain = _stub_reference(monkeypatch)
+    T, P = install_into_reference(pkg)
+    assert pkg.cli.GDMLTrain is T and pkg.cli.GDMLPredict is P
+    assert issubclass(T, sgdml_b200.GDMLTrain) and P is sgdml_b200.GDMLPredict
+    for name in ('create_task', 'create_task_from_model', 'draw_strat_sample'):
+        assert getattr(T, name) is getattr(RefTrain, name)
+
+    sig = _reference()['signatures']
+    assert _params(T.__init__) == sig['GDMLTrain.__init__']
+    assert _params(T.train) == sig['GDMLTrain.train']
+    assert _params(P.__init__) == sig['GDMLPredict.__init__']
+    assert _params(P.predict)[:3] == sig['GDMLPredict.predict'][:3]
+
+
 @pytest.mark.gpu
-def test_reference_cli_train_and_test_through_engine(tmp_path):
-    """`sgdml create` -> `sgdml train` -> `sgdml test` (the reference's own functions) with the engine installed:
-    the .npz it writes has the reference's keys / shapes / dtypes, loads in the UNMODIFIED reference GDMLPredict,
-    and predicts what the reference-trained model predicts (1e-6 rel, north_star)."""
-    eng = _run_tool('b200', tmp_path / 'b200')
-    ref = _run_tool('reference', tmp_path / 'ref')
-    assert eng['model_file'] == ref['model_file']
-    assert eng['keys'] == ref['keys'] and eng['shapes'] == ref['shapes'] and eng['dtypes'] == ref['dtypes']
-    assert eng['solver_name'] == ref['solver_name'] == 'analytic' and eng['n_test'] == ref['n_test']
-    assert rel_err(eng['E_ref_predict'], ref['E_ref_predict']) < 1e-6
-    assert rel_err(eng['F_ref_predict_first'], ref['F_ref_predict_first']) < 1e-6
-    assert abs(eng['c'] - ref['c']) < 1e-6 * abs(ref['c']) and abs(eng['std'] - ref['std']) < 1e-12 * ref['std']
-    # test errors recorded in the model file by cli.test (cli.py:1502-1570) agree to solver accuracy
-    assert abs(eng['f_err']['rmse'] - ref['f_err']['rmse']) < 1e-6 + 0.05 * ref['f_err']['rmse']
+def test_train_reference_task_matches_reference_model():
+    """GDMLTrain.train on a task made by the reference's own create_task: the model dict has the reference model's
+    keys, shapes and dtypes, its c and std, and predicts what the reference-trained model predicts (1e-6 rel)."""
+    import sgdml_b200
+
+    ref = _reference()
+    with np.load(os.path.join(DROPIN_DIR, 'reference_task.npz'), allow_pickle=False) as f:
+        task = {k: f[k] for k in f.files}
+    Rq = task.pop('R_query')
+    model = sgdml_b200.GDMLTrain().train(task)
+    assert sorted(model.keys()) == ref['model_keys']
+    for k in ('R_desc', 'R_d_desc_alpha', 'alphas_F', 'perms', 'tril_perms_lin'):
+        assert list(np.asarray(model[k]).shape) == ref['model_shapes'][k], k
+    for k in ('R_desc', 'R_d_desc_alpha', 'alphas_F', 'perms', 'tril_perms_lin', 'sig', 'c', 'std', 'solver_name'):
+        assert str(np.asarray(model[k]).dtype) == ref['model_dtypes'][k], k
+    assert str(model['solver_name']) == 'analytic'
+    assert abs(float(model['c']) - ref['c']) < 1e-6 * abs(ref['c'])
+    assert abs(float(model['std']) - ref['std']) < 1e-12 * ref['std']
+    E, F = sgdml_b200.GDMLPredict(model).predict(Rq)
+    assert rel_err(E, ref['E_query']) < 1e-6
+    assert rel_err(F, ref['F_query']) < 1e-6

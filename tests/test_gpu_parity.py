@@ -499,7 +499,7 @@ def test_potrf_potrs(eng, variant, n):
 def test_potrf_potrs_large_outer_block(eng, oz_slices, monkeypatch):
     """n >= 16384 takes the NBO = 1024 outer blocking and the triangular super-tile order of the trailing GEMM --
     the configuration BASELINE config 2 (n = 63000) runs -- against scipy's LAPACK dpotrf / dpotrs
-    (analytic.py:94-99).  oz_slices = 7: the same factorisation with the tcgen05 int8 trailing updates."""
+    (analytic.py:94-99).  oz_slices = 7: the same factorisation with the int8 (wgmma) trailing updates."""
     import scipy.linalg
     import torch
     from sgdml_b200 import _lib

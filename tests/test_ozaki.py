@@ -1,4 +1,4 @@
-"""Bring-up harness for the tcgen05 FP64-via-INT8 GEMM (csrc/ozaki.cu): against NumPy FP64 and against an
+"""Bring-up harness for the wgmma FP64-via-INT8 GEMM (csrc/ozaki.cu): against NumPy FP64 and against an
 exact NumPy model of the slicing.  GPU only."""
 
 import numpy as np
@@ -153,7 +153,7 @@ def test_ozaki_gemm_slice_count(S):
 
 
 def test_potrf_with_int8_trailing_updates(monkeypatch):
-    """Cholesky with the trailing updates on the tcgen05 int8 path (SGDML_B200_OZAKI_SLICES=7) against the
+    """Cholesky with the trailing updates on the int8 path (SGDML_B200_OZAKI_SLICES=7) against the
     FP64 DMMA factorisation of the same matrix."""
     import torch
 
@@ -177,7 +177,7 @@ def test_potrf_with_int8_trailing_updates(monkeypatch):
 
 
 def test_large_descriptor_predictor_on_int8_path(monkeypatch):
-    """GEMM-composed predictor (D > 256) with its four contractions on the tcgen05 int8 path, 4 and 5
+    """GEMM-composed predictor (D > 256) with its four contractions on the int8 path, 4 and 5
     slices: forces against the oracle (tools/ozaki_study.py predict: 8.8e-9 / 6.5e-11)."""
     import sgdml_b200
     from oracle import predict as opredict

@@ -1,4 +1,4 @@
-"""CPU checks of the numerical claims behind the planned tcgen05 (FP64-via-INT8) trailing updates
+"""CPU checks of the numerical claims behind the int8 (FP64-via-INT8) trailing updates
 (DESIGN.md section 7, tools/ozaki_study.py): exact integer emulation, no GPU."""
 
 import importlib.util

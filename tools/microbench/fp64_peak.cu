@@ -1,8 +1,7 @@
-// FP64 pipe microbenchmarks for B200 (sm_100a). Decides DFMA-vs-DMMA for the
-// sgdml_b200 kernels and provides the FP64 roofline denominator (MEASURED_PEAKS.json
-// only carries HBM and bf16 numbers).
+// FP64 pipe microbenchmarks for H100 (sm_90a). Decides DFMA-vs-DMMA for the
+// sgdml_b200 kernels and provides the FP64 roofline denominator.
 //
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o fp64_peak fp64_peak.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o fp64_peak fp64_peak.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""Throughput of the tcgen05 int8-slice GEMM (csrc/ozaki.cu) next to the DMMA GEMM, same shapes.
+"""Throughput of the wgmma int8-slice GEMM (csrc/ozaki.cu) next to the DMMA GEMM, same shapes.
 FP64-equivalent TFLOP/s = 2 m n k / time; the int8 path's time includes slicing both operands."""
 import ctypes
 import os

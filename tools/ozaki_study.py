@@ -1,11 +1,11 @@
 """CPU feasibility study (NumPy, exact integer arithmetic) for running the Cholesky trailing updates
-of the analytic solve as FP64-via-INT8 GEMMs on the tcgen05 tensor cores (Ozaki-style error-free
+of the analytic solve as FP64-via-INT8 GEMMs on the int8 tensor cores (Ozaki-style error-free
 splitting): how many 7-bit slices does the sGDML system need so that the trained model still meets
 the 1e-6 force tolerance?
 
 For C -= W W^T every row of W is scaled by a power of two and cut into `s` signed 7-bit slices
-(int8); every slice-pair product W_p W_q^T is an exact int32 GEMM (what `tcgen05.mma kind::i8` with a
-TMEM int32 accumulator computes), and the pairs with p + q <= s + 1 are summed in FP64.  The panel
+(int8); every slice-pair product W_p W_q^T is an exact int32 GEMM (what `wgmma` s8 with a
+int32 register accumulator computes), and the pairs with p + q <= s + 1 are summed in FP64.  The panel
 work (potf2, TRSM) stays in FP64.  Nothing here is product code.
 
     python tools/ozaki_study.py [--n-atoms 21] [--n-train 40] [--nb 128]

@@ -5,7 +5,7 @@ kernels that produced alphas, and compares it with the labels y (analytic.py:65-
 system).  Also reports the force error on a sample of training points.
 
     python tools/solve_check.py --workload aspirin --n-train 300        # n = 18900 (NBO = 1024 path)
-    SGDML_B200_OZAKI_SLICES=7 python tools/solve_check.py ...          # tcgen05 int8 trailing updates
+    SGDML_B200_OZAKI_SLICES=7 python tools/solve_check.py ...          # int8 (wgmma) trailing updates
 """
 
 import argparse

@@ -190,9 +190,11 @@ int sgdml_b200_set_assemble_variant(int variant);
 
 /* scipy.linalg.cho_factor (LAPACK dpotrf) as used by analytic.py:94-96 and
  * iterative.py:447-449.  A (n, n) symmetric, row stride lda; only the LOWER triangle
- * (row-major) is read and overwritten with L (A = L L^T).  Returns info > 0 if the
- * leading minor of order info is not positive definite (analytic.py:101 catches the
- * resulting LinAlgError). */
+ * (row-major) is read, and on return it holds L (A = L L^T).  Strictly upper entries near
+ * the diagonal (inside the diagonal blocks the trailing updates store whole) may be
+ * overwritten with intermediate values; nothing reads them.  Padding columns (lda > n) are
+ * neither read nor written.  Returns info > 0 if the leading minor of order info is not
+ * positive definite (analytic.py:101 catches the resulting LinAlgError). */
 int sgdml_b200_potrf(double* A, int64_t n, int64_t lda, void* stream);
 
 /* scipy.linalg.cho_solve (dpotrs), analytic.py:97-99: solves L L^T X = B in place.
@@ -216,11 +218,13 @@ int sgdml_b200_gather_rows_neg(const double* X, int64_t ldx, int64_t m, const in
                                double* out, int64_t ldo, void* stream);
 /* A[i][i] += value (the jitter escalation of _cho_factor_stable, iterative.py:414-471). */
 int sgdml_b200_add_diag(double* A, int64_t n, int64_t lda, double value, void* stream);
-/* X <- X L^-T for lower-triangular L (m x m): scipy.linalg.solve_triangular(L, X.T, trans='T').T,
- * iterative.py:278-287 and 337-347. */
+/* X <- X L^-T for lower-triangular L (m x m): scipy.linalg.solve_triangular(L, X.T, lower=True).T, which is
+ * iterative.py:278-287 and 337-347 with the upper factor U = L^T of cho_factor.  Only the lower triangle of L
+ * is read. */
 int sgdml_b200_trsm_right_lt(const double* L, int64_t m, int64_t ldl, double* X, int64_t n_rows,
                              int64_t ldx, void* stream);
-/* C = X^T X + lam I, lower triangle (iterative.py:293-295). */
+/* C = X^T X + lam I, lower triangle (iterative.py:293-295).  Strictly upper entries of C inside the
+ * 128 x 128 diagonal tiles may be written too (with the same products); padding columns (ldc > m) are not. */
 int sgdml_b200_gram_tn(const double* X, int64_t n_rows, int64_t m, int64_t ldx, double lam, double* C,
                        int64_t ldc, void* stream);
 /* out[r] = |X[r, :]|^2 -- the leverage scores (iterative.py:107-109). */

@@ -466,6 +466,50 @@ def test_dgemm_nt(eng, variant, m, n, k):
     assert rel_err(C, ref) < 1e-13
 
 
+@pytest.mark.parametrize('layout', ['lda_padded', 'offset', 'beta0_nan'])
+@pytest.mark.parametrize('variant', [0, 1, 2, 3])
+@pytest.mark.parametrize('m,n,k', [(128, 128, 128), (300, 200, 64), (257, 129, 130), (64, 1000, 16), (33, 17, 7)])
+def test_dgemm_nt_device_layouts(eng, variant, m, n, k, layout):
+    """test_dgemm_nt on device operands.  layout: padded row strides with NaN in every padding column (read by
+    no kernel, C's not written); A one double off 16-byte alignment (the scalar fallback kernel); beta = 0 with
+    NaN in C (C must not be read)."""
+    import torch
+    from sgdml_b200 import _lib
+
+    L = _lib.lib()
+    rng = np.random.default_rng(m + n + k)
+    A = rng.standard_normal((m, k))
+    B = rng.standard_normal((n, k))
+    C = rng.standard_normal((m, n))
+    alpha, beta = 0.75, (0.0 if layout == 'beta0_nan' else -1.25)
+    ref = alpha * A @ B.T + beta * C
+    pad = 2 if layout == 'lda_padded' else 0
+    lda, ldb, ldc = k + pad, k + 2 * pad, n + pad
+    nan = float('nan')
+    off = 1 if layout == 'offset' else 0
+    Ad = torch.full((m * lda + 1,), nan, dtype=torch.float64, device='cuda')
+    Ad[off : off + m * lda].view(m, lda)[:, :k] = torch.from_numpy(A).cuda()
+    Bd = torch.full((n, ldb), nan, dtype=torch.float64, device='cuda')
+    Bd[:, :k] = torch.from_numpy(B).cuda()
+    Cd = torch.full((m, ldc), nan, dtype=torch.float64, device='cuda')
+    if layout != 'beta0_nan':
+        Cd[:, :n] = torch.from_numpy(C).cuda()
+    L.sgdml_b200_set_gemm_variant(variant)
+    try:
+        _lib.check(
+            L.sgdml_b200_dgemm_nt(
+                m, n, k, alpha, Ad.data_ptr() + 8 * off, lda, Bd.data_ptr(), ldb, beta, Cd.data_ptr(), ldc, _lib.current_stream()
+            ),
+            'dgemm',
+        )
+        torch.cuda.synchronize()
+    finally:
+        L.sgdml_b200_set_gemm_variant(3)
+    Ch = Cd.cpu().numpy()
+    assert np.isnan(Ch[:, n:]).all()  # padding columns of C not written
+    assert rel_err(Ch[:, :n], ref) < 1e-13
+
+
 @pytest.mark.parametrize('variant', [0, 1, 3])
 @pytest.mark.parametrize('n', [64, 128, 200, 513, 1400])
 def test_potrf_potrs(eng, variant, n):
@@ -495,17 +539,15 @@ def test_potrf_potrs(eng, variant, n):
     assert rel_err(x1, x[:, 0]) < 1e-12
 
 
-@pytest.mark.parametrize('oz_slices', [0, 7])
-def test_potrf_potrs_large_outer_block(eng, oz_slices, monkeypatch):
-    """n >= 16384 takes the NBO = 1024 outer blocking and the triangular super-tile order of the trailing GEMM --
-    the configuration BASELINE config 2 (n = 63000) runs -- against scipy's LAPACK dpotrf / dpotrs
-    (analytic.py:94-99).  oz_slices = 7: the same factorisation with the int8 (wgmma) trailing updates."""
+def _potrf_potrs_vs_lapack(n, lda, oz_slices, monkeypatch):
+    """potrf + potrs on a device buffer of row stride lda whose strictly upper triangle and padding columns hold
+    NaN, against scipy's LAPACK dpotrf / dpotrs (analytic.py:94-99): neither canary may reach L or x, and the
+    padding columns must not be written."""
     import scipy.linalg
     import torch
     from sgdml_b200 import _lib
 
     L = _lib.lib()
-    n = 16500  # not a multiple of any block size
     rng = np.random.default_rng(7)
     X = rng.standard_normal((n, 64))
     d = rng.uniform(0.5, 2.0, size=n)
@@ -516,17 +558,36 @@ def test_potrf_potrs_large_outer_block(eng, oz_slices, monkeypatch):
     x_ref = scipy.linalg.cho_solve((c, low), b, check_finite=False)
     if oz_slices:
         monkeypatch.setenv('SGDML_B200_OZAKI_SLICES', str(oz_slices))
-    Ad = torch.from_numpy(A).cuda()
-    _lib.check(L.sgdml_b200_potrf(Ad.data_ptr(), n, n, _lib.current_stream()), 'potrf')
+    Ad = torch.full((n, lda), float('nan'), dtype=torch.float64, device='cuda')
+    Ad[:, :n] = torch.from_numpy(A).cuda().tril_() + Ad.new_full((n, n), float('nan')).triu_(1)
+    _lib.check(L.sgdml_b200_potrf(Ad.data_ptr(), n, lda, _lib.current_stream()), 'potrf')
     xd = torch.from_numpy(b.copy()).cuda()
-    _lib.check(L.sgdml_b200_potrs(Ad.data_ptr(), n, n, xd.data_ptr(), 2, 2, _lib.current_stream()), 'potrs')
+    _lib.check(L.sgdml_b200_potrs(Ad.data_ptr(), n, lda, xd.data_ptr(), 2, 2, _lib.current_stream()), 'potrs')
     torch.cuda.synchronize()
-    Lg = np.tril(Ad.cpu().numpy())
+    if lda > n:
+        assert bool(torch.isnan(Ad[:, n:]).all())
+    Lg = np.tril(Ad[:, :n].cpu().numpy())
     tol = 1e-11 if not oz_slices else 1e-9
     assert rel_err(Lg, np.tril(c)) < tol
     x = xd.cpu().numpy()
     assert rel_err(x, x_ref) < tol * 10
     assert rel_err(A @ x, b) < tol * 10
+
+
+@pytest.mark.parametrize('oz_slices', [0, 7])
+def test_potrf_potrs_large_outer_block(eng, oz_slices, monkeypatch):
+    """n >= 16384 takes the NBO = 1024 outer blocking and the triangular super-tile order of the trailing GEMM --
+    the configuration BASELINE config 2 (n = 63000) runs -- against scipy's LAPACK dpotrf / dpotrs
+    (analytic.py:94-99).  oz_slices = 7: the same factorisation with the int8 (wgmma) trailing updates.
+    n = 16500 is not a multiple of any block size."""
+    _potrf_potrs_vs_lapack(16500, 16500, oz_slices, monkeypatch)
+
+
+@pytest.mark.parametrize('oz_slices', [0, 7])
+def test_potrf_potrs_large_outer_block_padded_stride(eng, oz_slices, monkeypatch):
+    """The NBO = 1024 path with the padded stride lda = n + 1 of the analytic solver, ending in a one-column
+    block: n = 16385 = 16 * 1024 + 1."""
+    _potrf_potrs_vs_lapack(16385, 16386, oz_slices, monkeypatch)
 
 
 def test_train_analytic_large_outer_block_residual(eng):
@@ -608,12 +669,10 @@ def test_train_end_to_end_golden(eng, golden):
     assert rel_err(E, golden['E_query']) < 1e-6
 
 
-def test_train_ethanol_config_vs_oracle(eng):
-    """BASELINE config 1 (9 atoms, 200 training points, 6 perms): engine-trained model vs
-    oracle-trained model, predictions on 100 query geometries within 1e-6."""
+def _train_vs_oracle(eng, task):
+    """Engine-trained model vs oracle-trained model, predictions on 100 query geometries within 1e-6."""
     from sgdml_b200 import synth
 
-    task = synth.make_config_task('ethanol')
     model = eng.GDMLTrain().train(task)
     ref = otrain.train(task)
     Rq = synth.geometries(9, 100, 1).reshape(100, -1)
@@ -621,6 +680,22 @@ def test_train_ethanol_config_vs_oracle(eng):
     E, F = eng.GDMLPredict(model).predict(Rq)
     assert rel_err(F, F_ref) < 1e-6
     assert rel_err(E, E_ref) < 1e-6
+
+
+def test_train_ethanol_config_vs_oracle(eng):
+    """BASELINE config 1 (9 atoms, 200 training points, 6 perms): engine-trained model vs
+    oracle-trained model, predictions on 100 query geometries within 1e-6."""
+    from sgdml_b200 import synth
+
+    _train_vs_oracle(eng, synth.make_config_task('ethanol'))
+
+
+def test_train_ethanol_odd_size_padded_stride(eng):
+    """The ethanol configuration at 201 training points: n = 5427 is odd, so the analytic solver assembles and
+    factorises K with the padded row stride n + 1 from start to finish."""
+    from sgdml_b200 import synth
+
+    _train_vs_oracle(eng, synth.make_config_task('ethanol', n_train=201))
 
 
 def test_model_npz_roundtrip(eng, golden, tmp_path):

@@ -139,6 +139,54 @@ def test_engine_qr_fallback(monkeypatch):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize('force_qr', [False, True])
+@pytest.mark.parametrize('m', [351, 1107])
+def test_engine_nystroem_factor_multi_block(m, force_qr, monkeypatch):
+    """The engine's Nystroem factor at m > 128 inducing columns (odd m = 351: three 128-column blocks of TRSM,
+    padded square stride m + 1; m = 1107: nine blocks, a Gram matrix spanning two super-tile rows), on a synthetic
+    N = 9, M = 150 task: leverage scores and P.v against the oracle's factor on the same columns, through the
+    inner Cholesky and through the CholeskyQR3 branch (force_qr).  Both factorisations work on K_mm of
+    condition ~1e11, so the two factors agree to conditioning, not to rounding.  Measured on an H100 80GB HBM3
+    (400 W), relative to the largest entry: leverage scores 3.1e-9 (m = 351) and 3.3e-8 (m = 1107), P.v 7.0e-9
+    and 1.2e-7, the same with and without force_qr; the bounds are ~10x the larger figure."""
+    import sgdml_b200
+    from sgdml_b200 import synth
+    from sgdml_b200.desc import Desc
+    from sgdml_b200.solvers.iterative import Iterative
+
+    N, M, sig = 9, 150, 20
+    perms = synth.rotor_swap_group(N, 1, 1)
+    task = synth.make_task(N, M, perms, sig)
+    lam = float(task['lam'])
+    R = task['R_train'].reshape(M, -1)
+    cols = np.sort(np.random.default_rng(m).choice(3 * N * M, m, replace=False))
+    v = np.random.default_rng(1).standard_normal(3 * N * M)
+    x, gd = odesc.from_R(R)
+    lin = odesc.tril_perms_lin(perms)
+    B = oiter.nystroem_factor(x, gd, lin, sig, lam, cols, force_qr=force_qr)
+    lev_ref, Pv_ref = np.einsum('ij,ij->j', B, B), oiter.precon(B, lam)(v)
+
+    d = Desc(N)
+    xe, gde = d.from_R(R)
+    it = Iterative(sgdml_b200.GDMLTrain(max_memory=1.0), d, 1.0, None, False)
+    if force_qr:
+        real, calls = it._cho_factor_stable, []
+
+        def fake(A, pre_reg=False, eps_mag_max=1):
+            if eps_mag_max == -14:  # the inner factorisation of iterative.py:305 reports failure
+                calls.append(1)
+                return False
+            return real(A, pre_reg=pre_reg, eps_mag_max=eps_mag_max)
+
+        monkeypatch.setattr(it, '_cho_factor_stable', fake)
+    P, lev = it._init_precon_operator(task, xe, gde, lin, cols)
+    assert not force_qr or calls
+    e_lev, e_pv = rel_err(lev, lev_ref), rel_err(P(v), Pv_ref)
+    assert e_lev < 4e-7
+    assert e_pv < 1.5e-6
+
+
+@pytest.mark.gpu
 def test_engine_cg_train_matches_reference():
     """GDMLTrain.train with a memory cap that forces the iterative solver, same inducing columns as the
     reference run: converges to the same tolerance in a similar number of iterations and predicts

@@ -177,6 +177,20 @@ int sgdml_b200_assemble_ecstr(const double* R_desc, const double* R_d_desc, cons
                               int64_t n_atoms, int64_t n_train, int64_t n_perms, double sig, double scale, double* K,
                               int64_t ldk, void* stream);
 
+/* Row block of the energy-constrained matrix at a column subset (the Nystroem set-up of iterative.py:232-247 with
+ * use_E_cstr; train.py:1376-1407): with K_full the (3NM + M)-square matrix of sgdml_b200_assemble(+_ecstr) in the
+ * layout [forces (3NM); energies (M)], and col_idxs a sorted, duplicate-free int64 list in [0, 3NM + M),
+ *   K[(i - m_begin)*3N + r, c]              = scale * K_full[i*3N + r, col_idxs[c]]   (force rows)
+ *   K[(m_end - m_begin)*3N + (i - m_begin), c] = scale * K_full[3NM + i, col_idxs[c]] (energy rows)
+ * for i in [m_begin, m_end): (m_end - m_begin)(3N + 1) rows of row stride ldk >= n_cols.  K must be a DEVICE
+ * pointer.  The force columns (the prefix of the list) of the force rows are exactly what sgdml_b200_assemble_rows
+ * writes; every other entry costs one pass over the (row point, column point) pair.  Padding columns (ldk > n_cols)
+ * are neither read nor written.  Same limits as sgdml_b200_assemble_ecstr (N <= 128, M <= 65535). */
+int sgdml_b200_assemble_ecstr_rows(const double* R_desc, const double* R_d_desc, const int64_t* tril_perms_lin,
+                                   int64_t n_atoms, int64_t n_train, int64_t n_perms, double sig,
+                                   const int64_t* col_idxs, int64_t n_cols, double scale, int64_t m_begin,
+                                   int64_t m_end, double* K, int64_t ldk, void* stream);
+
 /* Tuning / test hook: 0 = kernel chosen by molecule size (default), 1 = always the large-molecule
  * kernel (tables in global memory), which molecules above ~50 atoms need; 2 / 3 / 4 = small-molecule kernel with
  * per-permutation phases (k_assemble) / with permutation chunks and resident row tables (k_assemble_v3) / chunks of
@@ -260,7 +274,9 @@ int sgdml_b200_nystroem_expand(const double* X, int64_t n_rows, int64_t m, int64
  * the rows X_loc ((m_end - m_begin)*3N x m_ind, row stride ldx) of the factor; `exchange` is called, in stream
  * order, with DEVICE buffers inside `workspace`:
  *   op 0: sum `count` doubles at `buf` over the ranks in place   (X^T v, m_ind doubles)
- *   op 1: all-gather: `buf` is the full vector (count = n), the rows this rank owns are in place
+ *   op 1: all-gather: `buf` is the full force vector (count = 3N * n_train), the rows this rank owns are in place
+ *   op 2: all-gather of the energy tail (sgdml_b200_pcg_ecstr only): `buf` is the M-entry tail (count = n_train),
+ *         entries [m_begin, m_end) are this rank's and in place
  * and must enqueue the collective on `stream` (torch.distributed / NCCL on the Python host).  exchange == NULL:
  * single rank, m_begin = 0, m_end = n_train.  m_ind = 0: no preconditioner (z = r). */
 typedef int (*sgdml_b200_exchange_fn)(void* ctx, int op, double* buf, int64_t count);
@@ -271,6 +287,20 @@ int sgdml_b200_pcg(sgdml_b200_model* model, int64_t m_begin, int64_t m_end, cons
                    int64_t max_iters, int64_t check_every, double* workspace, int64_t workspace_doubles,
                    sgdml_b200_exchange_fn exchange, void* exchange_ctx, sgdml_b200_pcg_progress_fn progress,
                    void* progress_ctx, int64_t* iters_out, double* resid_out, void* stream);
+
+/* The same solve with energy constraints in the kernel (use_E_cstr): n = 3N * n_train + n_train, vectors in the
+ * layout [forces; energies], K v = [F; -E] of the predictor with alphas_F = v[:3NM], alphas_E = v[3NM:] (raw sums,
+ * iterative.py:183-204).  X_loc holds this rank's force rows, then its energy rows: (m_end - m_begin)(3N + 1) rows
+ * (sgdml_b200_assemble_ecstr_rows' layout).  Every K.v and P.v ends with op 1 on the force part and op 2 on the
+ * energy tail.  `workspace` holds at least sgdml_b200_pcg_ecstr_workspace_doubles(n, n_rows_loc, m_ind,
+ * check_every) doubles, n_rows_loc = (m_end - m_begin)(3N + 1): the common layout plus two n_rows_loc-vectors that
+ * stage this rank's two segments in X_loc's row order. */
+int64_t sgdml_b200_pcg_ecstr_workspace_doubles(int64_t n, int64_t n_rows_loc, int64_t m_ind, int64_t check_every);
+int sgdml_b200_pcg_ecstr(sgdml_b200_model* model, int64_t m_begin, int64_t m_end, const double* X_loc, int64_t m_ind,
+                         int64_t ldx, double lam, const double* y, double* x, int x_is_zero, double tol_abs,
+                         int64_t max_iters, int64_t check_every, double* workspace, int64_t workspace_doubles,
+                         sgdml_b200_exchange_fn exchange, void* exchange_ctx, sgdml_b200_pcg_progress_fn progress,
+                         void* progress_ctx, int64_t* iters_out, double* resid_out, void* stream);
 
 /* C = alpha * A * B^T + beta * C on the FP64 tensor pipe (the building block of potrf's
  * trailing update; exported for tests and benchmarks).  A (m, k) lda, B (n, k) ldb,

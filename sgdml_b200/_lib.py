@@ -51,6 +51,11 @@ SIGNATURES = {
     ),
     'sgdml_b200_assemble_ecstr': (
         C.c_int, [c_void_p, c_void_p, c_void_p, i64, i64, i64, C.c_double, C.c_double, c_void_p, i64, c_void_p]),
+    'sgdml_b200_assemble_ecstr_rows': (
+        C.c_int,
+        [c_void_p, c_void_p, c_void_p, i64, i64, i64, C.c_double, c_void_p, i64, C.c_double, i64, i64, c_void_p, i64,
+         c_void_p],
+    ),
     'sgdml_b200_set_assemble_variant': (C.c_int, [C.c_int]),
     'sgdml_b200_potrf': (C.c_int, [c_void_p, i64, i64, c_void_p]),
     'sgdml_b200_potrs': (C.c_int, [c_void_p, i64, i64, c_void_p, i64, i64, c_void_p]),
@@ -87,6 +92,12 @@ SIGNATURES = {
     'sgdml_b200_model_dims': (C.c_int, [c_void_p, c_int64_p, c_int64_p, c_int64_p]),
     'sgdml_b200_pcg_workspace_doubles': (C.c_int64, [i64, i64, i64, i64]),
     'sgdml_b200_pcg': (
+        C.c_int,
+        [c_void_p, i64, i64, c_void_p, i64, i64, C.c_double, c_void_p, c_void_p, C.c_int, C.c_double, i64, i64,
+         c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64_p, c_double_p, c_void_p],
+    ),
+    'sgdml_b200_pcg_ecstr_workspace_doubles': (C.c_int64, [i64, i64, i64, i64]),
+    'sgdml_b200_pcg_ecstr': (
         C.c_int,
         [c_void_p, i64, i64, c_void_p, i64, i64, C.c_double, c_void_p, c_void_p, C.c_int, C.c_double, i64, i64,
          c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64_p, c_double_p, c_void_p],

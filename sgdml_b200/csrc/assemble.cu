@@ -1320,18 +1320,16 @@ __global__ void __launch_bounds__(256, 2)
 //   K[n + j, n + i] = -sum_p (1 + (n_p/sig)(1 + n_p/(3 sig))) exp(-n_p/sig)           (train.py:296-300)
 // No tables: the pair quantities are read straight from the compressed arrays (L1/L2 resident); the work is
 // O(S N^2) per pair against O(S N^2 * 33) for the force-force block.
-__global__ void __launch_bounds__(128) k_assemble_ecstr(const double* __restrict__ R_desc, const double* __restrict__ R_d_desc,
-                                                       const int* __restrict__ aperm_inv, int N, int D, int M, int S,
-                                                       double sig, double scale, double* __restrict__ K, int64_t ldk) {
-  __shared__ double red[4];
-  __shared__ double s_cp, s_kee;
-  const int i = blockIdx.y, j = blockIdx.x;
-  const int b = threadIdx.x;  // atom of point j (blockDim.x = N rounded up to a warp multiple)
-  const double* xi = R_desc + (int64_t)i * D;
-  const double* xj = R_desc + (int64_t)j * D;
-  const double* gj = R_d_desc + (int64_t)j * D * 3;
-  const int64_t n = (int64_t)M * 3 * N;
-  double r0 = 0.0, r1 = 0.0, r2 = 0.0, kee = 0.0;
+// The per-pair part, shared by k_assemble_ecstr and k_assemble_ecstr_rows: for the pair (i, j) returns r[b] of
+// atom b = threadIdx.x of point j in (r0, r1, r2) and, in thread 0, the sum over permutations of the K_ee terms in
+// kee (the matrix entry is -scale * kee).  Block-wide:
+// every thread of the CTA calls it; red holds one double per warp (blockDim.x <= 128).
+__device__ __forceinline__ void ecstr_pair(const double* __restrict__ xi, const double* __restrict__ xj,
+                                           const double* __restrict__ gj, const int* __restrict__ aperm_inv, int N,
+                                           int S, double sig, double* red, double& s_cp, double& s_kee, double& r0,
+                                           double& r1, double& r2, double& kee) {
+  const int b = threadIdx.x;
+  r0 = 0.0, r1 = 0.0, r2 = 0.0, kee = 0.0;
   for (int pp = 0; pp < S; ++pp) {
     const int* Pi = aperm_inv + pp * N;
     double v0 = 0.0, v1 = 0.0, v2 = 0.0, s2 = 0.0;
@@ -1372,6 +1370,21 @@ __global__ void __launch_bounds__(128) k_assemble_ecstr(const double* __restrict
     if (threadIdx.x == 0) kee += s_kee;
     __syncthreads();  // red / s_cp are rewritten by the next permutation
   }
+}
+
+__global__ void __launch_bounds__(128) k_assemble_ecstr(const double* __restrict__ R_desc, const double* __restrict__ R_d_desc,
+                                                       const int* __restrict__ aperm_inv, int N, int D, int M, int S,
+                                                       double sig, double scale, double* __restrict__ K, int64_t ldk) {
+  __shared__ double red[4];
+  __shared__ double s_cp, s_kee;
+  const int i = blockIdx.y, j = blockIdx.x;
+  const int b = threadIdx.x;  // atom of point j (blockDim.x = N rounded up to a warp multiple)
+  const double* xi = R_desc + (int64_t)i * D;
+  const double* xj = R_desc + (int64_t)j * D;
+  const double* gj = R_d_desc + (int64_t)j * D * 3;
+  const int64_t n = (int64_t)M * 3 * N;
+  double r0, r1, r2, kee;
+  ecstr_pair(xi, xj, gj, aperm_inv, N, S, sig, red, s_cp, s_kee, r0, r1, r2, kee);
   if (b < N) {
     const int64_t col = (int64_t)j * 3 * N + 3 * b;
     double* rowE = K + (n + i) * ldk + col;
@@ -1383,6 +1396,46 @@ __global__ void __launch_bounds__(128) k_assemble_ecstr(const double* __restrict
     K[(col + 2) * ldk + n + i] = scale * r2;
   }
   if (threadIdx.x == 0) K[(n + j) * ldk + n + i] = -scale * kee;
+}
+
+// Energy parts of a row block of K_nm (sgdml_b200_assemble_ecstr_rows): row point a = m_begin + blockIdx.y, column
+// item blockIdx.x.  An item is either one energy column 3NM + q at output column dst >= 0 -- the pair (q, a) gives
+// the force rows of a (r) and the energy row of a (K_ee) in that column -- or the selected force columns of point q
+// (dst = -1 - t, fdest[t*3N + k] = output column of component k or -1) -- the pair (a, q) gives the energy row of a
+// in them.  Force rows come first in K (n_rowpts * 3N of them), then one energy row per row point.
+__global__ void __launch_bounds__(128) k_assemble_ecstr_rows(const double* __restrict__ R_desc,
+                                                            const double* __restrict__ R_d_desc,
+                                                            const int* __restrict__ aperm_inv, int N, int D, int S,
+                                                            double sig, double scale, const int* __restrict__ item_pt,
+                                                            const int64_t* __restrict__ item_dst,
+                                                            const int64_t* __restrict__ fdest, int m_begin,
+                                                            int64_t n_frows, double* __restrict__ K, int64_t ldk) {
+  __shared__ double red[4];
+  __shared__ double s_cp, s_kee;
+  const int a = m_begin + (int)blockIdx.y, q = item_pt[blockIdx.x];
+  const int64_t dst = item_dst[blockIdx.x];
+  const bool ecol = dst >= 0;
+  const int i = ecol ? q : a, j = ecol ? a : q;
+  const int b = threadIdx.x;
+  double r0, r1, r2, kee;
+  ecstr_pair(R_desc + (int64_t)i * D, R_desc + (int64_t)j * D, R_d_desc + (int64_t)j * D * 3, aperm_inv, N, S, sig, red,
+             s_cp, s_kee, r0, r1, r2, kee);
+  const int N3 = 3 * N;
+  double* rowE = K + (n_frows + blockIdx.y) * ldk;
+  if (ecol) {
+    if (b < N) {
+      double* Kf = K + ((int64_t)blockIdx.y * N3 + 3 * b) * ldk + dst;
+      Kf[0] = scale * r0;
+      Kf[ldk] = scale * r1;
+      Kf[2 * ldk] = scale * r2;
+    }
+    if (threadIdx.x == 0) rowE[dst] = -scale * kee;
+  } else if (b < N) {
+    const int64_t* d3 = fdest + (-1 - dst) * N3 + 3 * b;
+    if (d3[0] >= 0) rowE[d3[0]] = scale * r0;
+    if (d3[1] >= 0) rowE[d3[1]] = scale * r1;
+    if (d3[2] >= 0) rowE[d3[2]] = scale * r2;
+  }
 }
 
 static size_t asm_large_slab_doubles(int N, int S) {
@@ -1736,6 +1789,29 @@ extern "C" int sgdml_b200_assemble(const double* R_desc, const double* R_d_desc,
                                   scale, 0, n_train, K, ldk, stream);
 }
 
+// Inverse atom permutations (S x N) of tril_perms_lin, the tables of the energy-constraint kernels.
+static int ecstr_apinv(const int64_t* tril_perms_lin, int N, int S, std::vector<int>& apinv) {
+  const int D = N * (N - 1) / 2;
+  std::vector<int64_t> lin((size_t)S * D);
+  if (is_device_ptr(tril_perms_lin))
+    SG_CUDA(cudaMemcpy(lin.data(), tril_perms_lin, sizeof(int64_t) * lin.size(), cudaMemcpyDeviceToHost));
+  else
+    std::copy(tril_perms_lin, tril_perms_lin + lin.size(), lin.begin());
+  std::vector<int> dperm((size_t)D), aperm((size_t)N);
+  apinv.assign((size_t)S * N, 0);
+  for (int pp = 0; pp < S; ++pp) {
+    for (int d = 0; d < D; ++d) {
+      const int64_t e = lin[(size_t)d * S + pp] - (int64_t)pp * D;
+      SG_ARG(e >= 0 && e < D);
+      dperm[(size_t)d] = (int)e;
+    }
+    if (!atom_perm_from_desc_perm(dperm.data(), N, aperm.data()))
+      return fail_arg("tril_perms_lin is not induced by atom permutations (utils/desc.py:509-539)");
+    for (int a = 0; a < N; ++a) apinv[(size_t)pp * N + aperm[(size_t)a]] = a;
+  }
+  return 0;
+}
+
 // GDMLTrain._assemble_kernel_mat(use_E_cstr=True), train.py:234-300: fills the M energy rows and columns (and the
 // M x M energy-energy block) of the (3NM + M)-square matrix whose force-force part sgdml_b200_assemble writes.
 extern "C" int sgdml_b200_assemble_ecstr(const double* R_desc, const double* R_d_desc, const int64_t* tril_perms_lin,
@@ -1749,22 +1825,8 @@ extern "C" int sgdml_b200_assemble_ecstr(const double* R_desc, const double* R_d
   const int64_t nt = (int64_t)M * 3 * N + M;
   SG_ARG(ldk >= nt && is_device_ptr(K));
   cudaStream_t s = (cudaStream_t)stream;
-  std::vector<int64_t> lin((size_t)S * D);
-  if (is_device_ptr(tril_perms_lin))
-    SG_CUDA(cudaMemcpy(lin.data(), tril_perms_lin, sizeof(int64_t) * lin.size(), cudaMemcpyDeviceToHost));
-  else
-    std::copy(tril_perms_lin, tril_perms_lin + lin.size(), lin.begin());
-  std::vector<int> dperm((size_t)D), aperm((size_t)N), apinv((size_t)S * N);
-  for (int pp = 0; pp < S; ++pp) {
-    for (int d = 0; d < D; ++d) {
-      const int64_t e = lin[(size_t)d * S + pp] - (int64_t)pp * D;
-      SG_ARG(e >= 0 && e < D);
-      dperm[(size_t)d] = (int)e;
-    }
-    if (!atom_perm_from_desc_perm(dperm.data(), N, aperm.data()))
-      return fail_arg("tril_perms_lin is not induced by atom permutations (utils/desc.py:509-539)");
-    for (int a = 0; a < N; ++a) apinv[(size_t)pp * N + aperm[(size_t)a]] = a;
-  }
+  std::vector<int> apinv;
+  SG_TRY(ecstr_apinv(tril_perms_lin, N, S, apinv));
   Staged sX, sG;
   SG_TRY(sX.init(R_desc, sizeof(double) * (size_t)M * D, true, s));
   SG_TRY(sG.init(R_d_desc, sizeof(double) * (size_t)M * D * 3, true, s));
@@ -1782,5 +1844,90 @@ extern "C" int sgdml_b200_assemble_ecstr(const double* R_desc, const double* R_d
   };
   int rc = body();
   cudaFree(d_apinv);
+  return rc;
+}
+
+// Row block of the energy-constrained K_nm (the Nystroem set-up of iterative.py:232-247 with use_E_cstr): the force
+// prefix of the column list goes through sgdml_b200_assemble_rows, every other entry through k_assemble_ecstr_rows,
+// which computes each (row point, column point) pair the list touches once.
+extern "C" int sgdml_b200_assemble_ecstr_rows(const double* R_desc, const double* R_d_desc,
+                                              const int64_t* tril_perms_lin, int64_t n_atoms, int64_t n_train,
+                                              int64_t n_perms, double sig, const int64_t* col_idxs, int64_t n_cols,
+                                              double scale, int64_t m_begin, int64_t m_end, double* K, int64_t ldk,
+                                              void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(R_desc != nullptr && R_d_desc != nullptr && tril_perms_lin != nullptr && col_idxs != nullptr && K != nullptr);
+  SG_ARG(n_atoms >= 2 && n_atoms <= 128 && n_train >= 1 && n_train <= 65535 && n_perms >= 1 && sig > 0);
+  SG_ARG(m_begin >= 0 && m_begin < m_end && m_end <= n_train);
+  const int N = (int)n_atoms, M = (int)n_train, S = (int)n_perms;
+  const int D = N * (N - 1) / 2, N3 = 3 * N;
+  const int64_t n = (int64_t)M * N3, nt = n + M;
+  SG_ARG(n_cols >= 1 && n_cols <= nt && ldk >= n_cols && is_device_ptr(K));
+  cudaStream_t s = (cudaStream_t)stream;
+  std::vector<int64_t> cols((size_t)n_cols);
+  if (is_device_ptr(col_idxs))
+    SG_CUDA(cudaMemcpy(cols.data(), col_idxs, sizeof(int64_t) * cols.size(), cudaMemcpyDeviceToHost));
+  else
+    std::copy(col_idxs, col_idxs + n_cols, cols.begin());
+  int64_t n_fcols = 0;
+  for (int64_t c = 0; c < n_cols; ++c) {
+    SG_ARG(cols[(size_t)c] >= 0 && cols[(size_t)c] < nt);
+    if (c > 0 && cols[(size_t)c] <= cols[(size_t)c - 1])
+      return fail_arg("col_idxs must be sorted ascending without duplicates (train.py:1341-1345)");
+    if (cols[(size_t)c] < n) ++n_fcols;
+  }
+  std::vector<int> apinv;
+  SG_TRY(ecstr_apinv(tril_perms_lin, N, S, apinv));
+  // force rows x force columns: exactly the row block sgdml_b200_assemble_rows writes
+  if (n_fcols > 0)
+    SG_TRY(sgdml_b200_assemble_rows(R_desc, R_d_desc, tril_perms_lin, n_atoms, n_train, n_perms, sig, col_idxs,
+                                    n_fcols, scale, m_begin, m_end, K, ldk, stream));
+  // column items: one per force-column point (with its destination map), one per energy column
+  std::vector<int> item_pt;
+  std::vector<int64_t> item_dst, fdest;
+  for (int64_t c = 0; c < n_fcols; ++c) {
+    const int q = (int)(cols[(size_t)c] / N3), k = (int)(cols[(size_t)c] % N3);
+    if (item_pt.empty() || item_pt.back() != q) {
+      item_dst.push_back(-1 - (int64_t)item_pt.size());
+      item_pt.push_back(q);
+      fdest.insert(fdest.end(), (size_t)N3, (int64_t)-1);
+    }
+    fdest[(item_pt.size() - 1) * N3 + k] = c;
+  }
+  for (int64_t c = n_fcols; c < n_cols; ++c) {
+    item_pt.push_back((int)(cols[(size_t)c] - n));
+    item_dst.push_back(c);
+  }
+  const int64_t n_items = (int64_t)item_pt.size();
+  const int n_rowpts = (int)(m_end - m_begin);
+  Staged sX, sG;
+  SG_TRY(sX.init(R_desc, sizeof(double) * (size_t)M * D, true, s));
+  SG_TRY(sG.init(R_d_desc, sizeof(double) * (size_t)M * D * 3, true, s));
+  int *d_apinv = nullptr, *d_pt = nullptr;
+  int64_t *d_dst = nullptr, *d_fdest = nullptr;
+  auto body = [&]() -> int {
+    SG_CUDA(cudaMalloc(&d_apinv, sizeof(int) * apinv.size()));
+    SG_CUDA(cudaMalloc(&d_pt, sizeof(int) * (size_t)n_items));
+    SG_CUDA(cudaMalloc(&d_dst, sizeof(int64_t) * (size_t)n_items));
+    SG_CUDA(cudaMalloc(&d_fdest, sizeof(int64_t) * std::max<size_t>(fdest.size(), 1)));
+    SG_CUDA(cudaMemcpyAsync(d_apinv, apinv.data(), sizeof(int) * apinv.size(), cudaMemcpyHostToDevice, s));
+    SG_CUDA(cudaMemcpyAsync(d_pt, item_pt.data(), sizeof(int) * (size_t)n_items, cudaMemcpyHostToDevice, s));
+    SG_CUDA(cudaMemcpyAsync(d_dst, item_dst.data(), sizeof(int64_t) * (size_t)n_items, cudaMemcpyHostToDevice, s));
+    if (!fdest.empty())
+      SG_CUDA(cudaMemcpyAsync(d_fdest, fdest.data(), sizeof(int64_t) * fdest.size(), cudaMemcpyHostToDevice, s));
+    ProfScope ps(KID_ASSEMBLE, s);
+    k_assemble_ecstr_rows<<<dim3((unsigned)n_items, (unsigned)n_rowpts), (N + 31) / 32 * 32, 0, s>>>(
+        (const double*)sX.dev(), (const double*)sG.dev(), d_apinv, N, D, S, sig, scale, d_pt, d_dst, d_fdest,
+        (int)m_begin, (int64_t)n_rowpts * N3, K, ldk);
+    SG_CUDA(cudaGetLastError());
+    count_launch(KID_ASSEMBLE);
+    SG_CUDA(cudaStreamSynchronize(s));  // the tables are freed below
+    return 0;
+  };
+  int rc = body();
+  cudaFree(d_apinv);
+  cudaFree(d_pt);
+  cudaFree(d_dst);
+  cudaFree(d_fdest);
   return rc;
 }

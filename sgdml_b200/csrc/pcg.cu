@@ -122,6 +122,12 @@ __global__ void __launch_bounds__(PCG_NT) k_pcg_update(int64_t n, const double* 
   if (threadIdx.x == 0) partial[blockIdx.x] = s;
 }
 
+// v = -v  (the energy rows of K.v with energy constraints: the operator returns [F; -E], iterative.py:196-198)
+__global__ void __launch_bounds__(PCG_NT) k_pcg_neg(int64_t n, double* __restrict__ v) {
+  const int64_t i = (int64_t)blockIdx.x * PCG_NT + threadIdx.x;
+  if (i < n) v[i] = -v[i];
+}
+
 // p = z + beta p
 __global__ void __launch_bounds__(PCG_NT) k_pcg_p(int64_t n, const double* __restrict__ sc, const double* __restrict__ z,
                                                  double* __restrict__ p) {
@@ -171,37 +177,44 @@ using namespace sgdml;
 namespace {
 
 struct PcgWs {
-  double *x, *r, *p, *z, *kv, *t, *part_xt, *partial, *sc, *hist;
+  double *x, *r, *p, *z, *kv, *t, *part_xt, *partial, *sc, *hist, *vloc, *zloc;
 };
 
 int pcg_grid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(PCG_MAX_CTAS, (n + PCG_ELEMS_PER_CTA - 1) / PCG_ELEMS_PER_CTA)); }
 
-}  // namespace
-
-extern "C" {
-
-int64_t sgdml_b200_pcg_workspace_doubles(int64_t n, int64_t n_rows_loc, int64_t m_ind, int64_t check_every) {
+int64_t pcg_ws_doubles(int64_t n, int64_t n_rows_loc, int64_t m_ind, int64_t check_every) {
   if (n < 1 || n_rows_loc < 0 || m_ind < 0 || check_every < 1) return -1;
   return 5 * n + m_ind + m_ind * xtv_chunks(std::max<int64_t>(n_rows_loc, 1)) + PCG_MAX_CTAS + SC_COUNT + check_every + 8;
 }
 
-int sgdml_b200_pcg(sgdml_b200_model* model, int64_t m_begin, int64_t m_end, const double* X_loc, int64_t m_ind,
-                   int64_t ldx, double lam, const double* y, double* x, int x_is_zero, double tol_abs,
-                   int64_t max_iters, int64_t check_every, double* workspace, int64_t workspace_doubles,
-                   sgdml_b200_exchange_fn exchange, void* exchange_ctx, sgdml_b200_pcg_progress_fn progress,
-                   void* progress_ctx, int64_t* iters_out, double* resid_out, void* stream) {
+// The energy-constrained solve stages this rank's two segments of a vector (force rows, energy rows) contiguously,
+// in the row order of X_loc: two more n_rows_loc-vectors after the common layout.
+int64_t pcg_ecstr_ws_doubles(int64_t n, int64_t n_rows_loc, int64_t m_ind, int64_t check_every) {
+  const int64_t base = pcg_ws_doubles(n, n_rows_loc, m_ind, check_every);
+  return base < 0 ? -1 : base + 2 * n_rows_loc;
+}
+
+// sgdml_b200_pcg (ecstr = false) and sgdml_b200_pcg_ecstr (ecstr = true): one implementation; with ecstr = false
+// every launch and every exchange is the force-only solve's.
+int pcg_impl(bool ecstr, sgdml_b200_model* model, int64_t m_begin, int64_t m_end, const double* X_loc, int64_t m_ind,
+             int64_t ldx, double lam, const double* y, double* x, int x_is_zero, double tol_abs, int64_t max_iters,
+             int64_t check_every, double* workspace, int64_t workspace_doubles, sgdml_b200_exchange_fn exchange,
+             void* exchange_ctx, sgdml_b200_pcg_progress_fn progress, void* progress_ctx, int64_t* iters_out,
+             double* resid_out, void* stream) {
   SG_TRY(require_device());
   SG_ARG(model != nullptr && y != nullptr && x != nullptr && workspace != nullptr && iters_out != nullptr &&
          resid_out != nullptr);
   SG_ARG(lam > 0.0 && tol_abs >= 0.0 && max_iters >= 0 && check_every >= 1);
   int64_t n_atoms = 0, n_train = 0;
   SG_TRY(sgdml_b200_model_dims(model, &n_atoms, &n_train, nullptr));
-  const int64_t dimi = 3 * n_atoms, n = dimi * n_train;
+  const int64_t dimi = 3 * n_atoms, n_f = dimi * n_train, n = n_f + (ecstr ? n_train : 0);
   SG_ARG(m_begin >= 0 && m_begin <= m_end && m_end <= n_train);
   SG_ARG(exchange != nullptr || (m_begin == 0 && m_end == n_train));  // one rank evaluates everything
-  const int64_t n_rows_loc = (m_end - m_begin) * dimi;
+  const int64_t n_pts_loc = m_end - m_begin, n_frows_loc = n_pts_loc * dimi;
+  const int64_t n_rows_loc = n_frows_loc + (ecstr ? n_pts_loc : 0);
   SG_ARG(m_ind >= 0 && (m_ind == 0 || (X_loc != nullptr && ldx >= m_ind && is_device_ptr(X_loc))));
-  SG_ARG(is_device_ptr(workspace) && workspace_doubles >= sgdml_b200_pcg_workspace_doubles(n, n_rows_loc, m_ind, check_every));
+  SG_ARG(is_device_ptr(workspace) &&
+         workspace_doubles >= (ecstr ? pcg_ecstr_ws_doubles : pcg_ws_doubles)(n, n_rows_loc, m_ind, check_every));
   cudaStream_t s = (cudaStream_t)stream;
 
   PcgWs w;
@@ -216,17 +229,41 @@ int sgdml_b200_pcg(sgdml_b200_model* model, int64_t m_begin, int64_t m_end, cons
     w.part_xt = q, q += m_ind * xtv_chunks(std::max<int64_t>(n_rows_loc, 1));
     w.partial = q, q += PCG_MAX_CTAS;
     w.sc = q, q += SC_COUNT;
-    w.hist = q;
+    w.hist = q, q += check_every;
+    w.vloc = ecstr ? q : nullptr, q += ecstr ? n_rows_loc : 0;
+    w.zloc = ecstr ? q : nullptr;
   }
   const int G = pcg_grid(n);
   const int64_t off_loc = m_begin * dimi;
 
-  // K v for the replicated vector v (device) into w.kv: rows of this rank, then the all-gather
+  // K v for the replicated vector v (device) into w.kv: rows of this rank, then the all-gather.  With energy
+  // constraints v = [v_F; v_E] and K v = [F; -E] of the predictor with alphas_F = v_F, alphas_E = v_E.
   auto k_vec = [&](const double* v) -> int {
     SG_TRY(sgdml_b200_model_set_alphas(model, v, stream));
-    if (m_end > m_begin)
-      SG_TRY(sgdml_b200_predict_train(model, m_begin, m_end, 0, nullptr, w.kv + off_loc, stream));
-    if (exchange != nullptr && exchange(exchange_ctx, 1, w.kv, n) != 0) return fail_arg("exchange (all-gather of K.v) failed");
+    if (ecstr) SG_TRY(sgdml_b200_model_set_alphas_E(model, v + n_f, stream));
+    if (m_end > m_begin) {
+      double* e_loc = ecstr ? w.kv + n_f + m_begin : nullptr;
+      SG_TRY(sgdml_b200_predict_train(model, m_begin, m_end, 0, e_loc, w.kv + off_loc, stream));
+      if (ecstr) {
+        k_pcg_neg<<<ceil_div(n_pts_loc, PCG_NT), PCG_NT, 0, s>>>(n_pts_loc, e_loc);
+        SG_CUDA(cudaGetLastError());
+        count_launch(KID_MISC);
+      }
+    }
+    if (exchange != nullptr && exchange(exchange_ctx, 1, w.kv, n_f) != 0) return fail_arg("exchange (all-gather of K.v) failed");
+    if (ecstr && exchange != nullptr && exchange(exchange_ctx, 2, w.kv + n_f, n_train) != 0)
+      return fail_arg("exchange (all-gather of the energy rows of K.v) failed");
+    return 0;
+  };
+  // this rank's rows of a replicated vector in the row order of X_loc (force rows, then energy rows) and back
+  auto gather_loc = [&](const double* v, double* loc) -> int {
+    SG_CUDA(cudaMemcpyAsync(loc, v + off_loc, sizeof(double) * n_frows_loc, cudaMemcpyDeviceToDevice, s));
+    SG_CUDA(cudaMemcpyAsync(loc + n_frows_loc, v + n_f + m_begin, sizeof(double) * n_pts_loc, cudaMemcpyDeviceToDevice, s));
+    return 0;
+  };
+  auto scatter_loc = [&](const double* loc, double* v) -> int {
+    SG_CUDA(cudaMemcpyAsync(v + off_loc, loc, sizeof(double) * n_frows_loc, cudaMemcpyDeviceToDevice, s));
+    SG_CUDA(cudaMemcpyAsync(v + n_f + m_begin, loc + n_frows_loc, sizeof(double) * n_pts_loc, cudaMemcpyDeviceToDevice, s));
     return 0;
   };
   // z = P r
@@ -235,14 +272,20 @@ int sgdml_b200_pcg(sgdml_b200_model* model, int64_t m_begin, int64_t m_end, cons
       SG_CUDA(cudaMemcpyAsync(w.z, w.r, sizeof(double) * n, cudaMemcpyDeviceToDevice, s));
       return 0;
     }
+    const double* r_loc = ecstr ? w.vloc : w.r + off_loc;
+    double* z_loc = ecstr ? w.zloc : w.z + off_loc;
+    if (ecstr && n_rows_loc > 0) SG_TRY(gather_loc(w.r, w.vloc));
     if (n_rows_loc > 0) {
-      SG_TRY(xt_v_device(X_loc, n_rows_loc, m_ind, ldx, w.r + off_loc, w.t, w.part_xt, s));
+      SG_TRY(xt_v_device(X_loc, n_rows_loc, m_ind, ldx, r_loc, w.t, w.part_xt, s));
     } else {
       SG_CUDA(cudaMemsetAsync(w.t, 0, sizeof(double) * m_ind, s));
     }
     if (exchange != nullptr && exchange(exchange_ctx, 0, w.t, m_ind) != 0) return fail_arg("exchange (all-reduce of X^T v) failed");
-    if (n_rows_loc > 0) SG_TRY(x_t_minus_v_device(X_loc, n_rows_loc, m_ind, ldx, lam, w.t, w.r + off_loc, w.z + off_loc, s));
-    if (exchange != nullptr && exchange(exchange_ctx, 1, w.z, n) != 0) return fail_arg("exchange (all-gather of P.v) failed");
+    if (n_rows_loc > 0) SG_TRY(x_t_minus_v_device(X_loc, n_rows_loc, m_ind, ldx, lam, w.t, r_loc, z_loc, s));
+    if (ecstr && n_rows_loc > 0) SG_TRY(scatter_loc(w.zloc, w.z));
+    if (exchange != nullptr && exchange(exchange_ctx, 1, w.z, n_f) != 0) return fail_arg("exchange (all-gather of P.v) failed");
+    if (ecstr && exchange != nullptr && exchange(exchange_ctx, 2, w.z + n_f, n_train) != 0)
+      return fail_arg("exchange (all-gather of the energy rows of P.v) failed");
     return 0;
   };
   auto scalar = [&](int mode, int arg) -> int {
@@ -332,6 +375,38 @@ int sgdml_b200_pcg(sgdml_b200_model* model, int64_t m_begin, int64_t m_end, cons
   *iters_out = iters;
   *resid_out = resid;
   return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t sgdml_b200_pcg_workspace_doubles(int64_t n, int64_t n_rows_loc, int64_t m_ind, int64_t check_every) {
+  return pcg_ws_doubles(n, n_rows_loc, m_ind, check_every);
+}
+
+int64_t sgdml_b200_pcg_ecstr_workspace_doubles(int64_t n, int64_t n_rows_loc, int64_t m_ind, int64_t check_every) {
+  return pcg_ecstr_ws_doubles(n, n_rows_loc, m_ind, check_every);
+}
+
+int sgdml_b200_pcg(sgdml_b200_model* model, int64_t m_begin, int64_t m_end, const double* X_loc, int64_t m_ind,
+                   int64_t ldx, double lam, const double* y, double* x, int x_is_zero, double tol_abs,
+                   int64_t max_iters, int64_t check_every, double* workspace, int64_t workspace_doubles,
+                   sgdml_b200_exchange_fn exchange, void* exchange_ctx, sgdml_b200_pcg_progress_fn progress,
+                   void* progress_ctx, int64_t* iters_out, double* resid_out, void* stream) {
+  return pcg_impl(false, model, m_begin, m_end, X_loc, m_ind, ldx, lam, y, x, x_is_zero, tol_abs, max_iters,
+                  check_every, workspace, workspace_doubles, exchange, exchange_ctx, progress, progress_ctx, iters_out,
+                  resid_out, stream);
+}
+
+int sgdml_b200_pcg_ecstr(sgdml_b200_model* model, int64_t m_begin, int64_t m_end, const double* X_loc, int64_t m_ind,
+                         int64_t ldx, double lam, const double* y, double* x, int x_is_zero, double tol_abs,
+                         int64_t max_iters, int64_t check_every, double* workspace, int64_t workspace_doubles,
+                         sgdml_b200_exchange_fn exchange, void* exchange_ctx, sgdml_b200_pcg_progress_fn progress,
+                         void* progress_ctx, int64_t* iters_out, double* resid_out, void* stream) {
+  return pcg_impl(true, model, m_begin, m_end, X_loc, m_ind, ldx, lam, y, x, x_is_zero, tol_abs, max_iters,
+                  check_every, workspace, workspace_doubles, exchange, exchange_ctx, progress, progress_ctx, iters_out,
+                  resid_out, stream);
 }
 
 }  // extern "C"

@@ -93,7 +93,9 @@ def exchange_on_workspace(ws, off, count, op, n_train, dim_i, group=None):
     solver's device workspace (a flat float64 tensor), [off, off + count) the buffer of this exchange.
       op 0: sum over the ranks in place (X^T v of the row-sharded Nystroem factor, m doubles);
       op 1: all-gather of a replicated n-vector whose rows [lo*dim_i, hi*dim_i) this rank has just written
-            (K.v rows, P.v rows): in place when the shards are equal, through a padded staging tensor otherwise.
+            (K.v rows, P.v rows): in place when the shards are equal, through a padded staging tensor otherwise;
+      op 2: the same for the M-entry energy tail of an energy-constrained solve (sgdml_b200_pcg_ecstr): entries
+            [lo, hi) are this rank's.
     Collectives are enqueued in stream order on the backend's stream; nothing is copied to the host."""
     import torch
 
@@ -105,8 +107,10 @@ def exchange_on_workspace(ws, off, count, op, n_train, dim_i, group=None):
     if op == 0:
         dist.all_reduce(view, op=dist.ReduceOp.SUM, group=group)
         return
-    if op != 1:
+    if op not in (1, 2):
         raise ValueError('unknown exchange op %r' % (op,))
+    if op == 2:
+        dim_i = 1  # one energy entry per training point
     assert count == n_train * dim_i
     lo, hi = shard_bounds(n_train, world, rank)
     if n_train % world == 0:
@@ -187,16 +191,32 @@ def all_reduce_sum_(t, group=None):
     return t
 
 
-def nystroem_factor_steps(ops, rank, world, n_train, dim_i, cols, lam):
+def _own_rows(cols, lo, hi, n_train, dim_i, use_E_cstr):
+    """Positions in `cols` of the inducing columns whose rows live on the rank with training points [lo, hi), and
+    their rows in that rank's block.  With energy constraints the block is the force rows of [lo, hi), then their
+    energy rows, and energy column c >= 3NM belongs to point c - 3NM."""
+    n_f = n_train * dim_i
+    own = np.nonzero((cols >= lo * dim_i) & (cols < hi * dim_i))[0]
+    local = cols[own] - lo * dim_i
+    if use_E_cstr:
+        own_e = np.nonzero((cols >= n_f + lo) & (cols < n_f + hi))[0]
+        own = np.concatenate([own, own_e])
+        local = np.concatenate([local, (hi - lo) * dim_i + (cols[own_e] - n_f - lo)])
+    return own, local
+
+
+def nystroem_factor_steps(ops, rank, world, n_train, dim_i, cols, lam, use_E_cstr=False):
     """Row-sharded iterative.py:208-351.  Returns (X_loc, lo, hi): the rows [lo*dim_i, hi*dim_i) of
-    the factor B^T = K_nm L^-T L_inner^-T (first len(cols) columns of X_loc)."""
+    the factor B^T = K_nm L^-T L_inner^-T (first len(cols) columns of X_loc).  use_E_cstr: the system is
+    (3NM + M)-square, `cols` index its columns, and X_loc holds the force rows of [lo, hi), then their energy
+    rows (ops.assemble_rows returns that block)."""
     lo, hi = shard_bounds(n_train, world, rank)
     cols = np.ascontiguousarray(cols, dtype=np.int64)
     m = len(cols)
     X = ops.assemble_rows(lo, hi, cols)  # local rows of K_nm (iterative.py:237-247)
-    own = np.nonzero((cols >= lo * dim_i) & (cols < hi * dim_i))[0]
+    own, local = _own_rows(cols, lo, hi, n_train, dim_i, use_E_cstr)
     A = ops.new_square(m)
-    ops.put_neg_rows(A, own, X, cols[own] - lo * dim_i, m)  # rows of K_mm = -K_nm[cols] owned here (iterative.py:253)
+    ops.put_neg_rows(A, own, X, local, m)  # rows of K_mm = -K_nm[cols] owned here (iterative.py:253)
     yield 'sum', A
     if not ops.cho_factor_stable(A, pre_reg=True):  # iterative.py:267
         raise np.linalg.LinAlgError('Failed to factorize K_mm despite strong regularization')
@@ -212,7 +232,7 @@ def nystroem_factor_steps(ops, rank, world, n_train, dim_i, cols, lam):
         # so X R^-1 is the top block of the thin Q factor; it is formed here by shifted CholeskyQR3
         # (three Gram + Cholesky + triangular-solve passes, the first one shifted), which is
         # backward stable for condition numbers up to ~1/eps and needs only the (m x m) all-reduce.
-        n_rows = n_train * dim_i
+        n_rows = n_train * dim_i + (n_train if use_E_cstr else 0)
         Y = ops.scaled_identity(m, np.sqrt(lam))  # the bottom block, replicated on every rank
         for it in range(3):
             ops.gram(X, m, A)
@@ -228,21 +248,37 @@ def nystroem_factor_steps(ops, rank, world, n_train, dim_i, cols, lam):
     return X, lo, hi
 
 
-def lev_scores_steps(ops, X, m, dim_i):
-    """Leverage scores (iterative.py:107-109) of a row-sharded factor, gathered on every rank."""
-    full = yield 'gather', ops.row_sqnorms(X, m).reshape(-1, dim_i)
-    return full.ravel()
+def lev_scores_steps(ops, X, m, dim_i, use_E_cstr=False):
+    """Leverage scores (iterative.py:107-109) of a row-sharded factor, gathered on every rank.  use_E_cstr: the
+    force part and the energy part of the local rows are gathered separately, into [forces; energies]."""
+    sq = ops.row_sqnorms(X, m)
+    if not use_E_cstr:
+        full = yield 'gather', sq.reshape(-1, dim_i)
+        return full.ravel()
+    n_f_loc = sq.size // (dim_i + 1) * dim_i
+    full_f = yield 'gather', sq[:n_f_loc].reshape(-1, dim_i)
+    full_e = yield 'gather', sq[n_f_loc:].reshape(-1, 1)
+    return np.concatenate([np.asarray(full_f).ravel(), np.asarray(full_e).ravel()])
 
 
-def precon_apply_steps(ops, X, m, lam, v, lo, hi, dim_i):
+def precon_apply_steps(ops, X, m, lam, v, lo, hi, dim_i, use_E_cstr=False):
     """P v = (B^T (B v) - v)/lam (iterative.py:136-138) with B^T row-sharded: one m-vector
-    all-reduce and one all-gather of the n-vector per application."""
+    all-reduce and one all-gather of the n-vector per application (two with use_E_cstr: the force part and the
+    energy tail of v = [forces; energies])."""
     v_loc = np.ascontiguousarray(v[lo * dim_i : hi * dim_i], dtype=np.float64)
+    if use_E_cstr:
+        n_f = len(v) // (dim_i + 1) * dim_i
+        v_loc = np.concatenate([v_loc, np.asarray(v[n_f + lo : n_f + hi], dtype=np.float64)])
     t = ops.project(X, m, v_loc)
     yield 'sum', t
     out_loc = ops.expand(X, m, lam, t, v_loc)
-    full = yield 'gather', out_loc.reshape(-1, dim_i)
-    return full.ravel()
+    if not use_E_cstr:
+        full = yield 'gather', out_loc.reshape(-1, dim_i)
+        return full.ravel()
+    n_f_loc = (hi - lo) * dim_i
+    full_f = yield 'gather', out_loc[:n_f_loc].reshape(-1, dim_i)
+    full_e = yield 'gather', out_loc[n_f_loc:].reshape(-1, 1)
+    return np.concatenate([np.asarray(full_f).ravel(), np.asarray(full_e).ravel()])
 
 
 def run_steps(gen, n_train, group=None):

@@ -264,16 +264,17 @@ class GDMLPredict(object):
                 if (not buf.is_cuda) and r_dev is not None and r_dev.type == 'cuda':
                     raise ValueError('out buffer %s is a host tensor but R is a CUDA tensor' % name)
 
-    def kmatvec_train(self, m_begin=0, m_end=None, out=None):
+    def kmatvec_train(self, m_begin=0, m_end=None, out=None, E_out=None):
         """Raw (std = 1, c = 0) force sums on training points [m_begin, m_end): the K.v operator
-        of the iterative solver (iterative.py:183-204) for alphas = v set via set_alphas."""
+        of the iterative solver (iterative.py:183-204) for alphas = v set via set_alphas.  E_out: optional
+        (m_end - m_begin,) array that receives the raw energy sums too."""
         if m_end is None:
             m_end = self.n_train
         n = m_end - m_begin
         F = out if out is not None else np.empty((n, 3 * self.n_atoms))
         _lib.check(
             _lib.lib().sgdml_b200_predict_train(
-                self._handle, m_begin, m_end, 0, None, _lib.ptr(F), _lib.current_stream()
+                self._handle, m_begin, m_end, 0, _lib.ptr(E_out), _lib.ptr(F), _lib.current_stream()
             ),
             'predict_train',
         )

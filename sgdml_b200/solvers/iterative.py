@@ -46,11 +46,15 @@ class _EngineNystroemOps(object):
     """Compute side of the row-sharded Nystroem factor (dist.nystroem_factor_steps and friends) on
     the CUDA engine: every method is one C-ABI call on this rank's rows; matrices are CUDA tensors."""
 
-    def __init__(self, solver, R_desc, R_d_desc, tril_perms_lin, sig):
+    def __init__(self, solver, R_desc, R_d_desc, tril_perms_lin, sig, use_E_cstr=False):
         self.solver = solver
         self.args = (R_desc, R_d_desc, tril_perms_lin, sig)
+        self.use_E_cstr = use_E_cstr
 
     def assemble_rows(self, lo, hi, cols):
+        if self.use_E_cstr:  # force rows of [lo, hi), then their energy rows (sgdml_b200_assemble_ecstr_rows)
+            X, _ = self.solver.gdml_train._assemble_kernel_mat_ecstr_rows_device(*self.args, cols, rows=(lo, hi))
+            return X
         X, _ = self.solver.gdml_train._assemble_kernel_mat_device(*self.args, col_idxs=cols, rows=(lo, hi))
         return X
 
@@ -196,13 +200,13 @@ class Iterative(object):
         dist.nystroem_factor_steps (the same steps, no exchange)."""
         from .. import dist as sdist
 
-        if use_E_cstr:
-            raise NotImplementedError('use_E_cstr is supported with the analytic solver only (the reference marks its iterative path unfinished, iterative.py:602)')
         n_train, dim_d = R_d_desc.shape[:2]
         dim_i = 3 * int((1 + np.sqrt(8 * dim_d + 1)) / 2)
         cols = np.ascontiguousarray(col_idxs, dtype=np.int64)
-        ops = _EngineNystroemOps(self, R_desc, R_d_desc, tril_perms_lin, sig)
-        X, _, _ = sdist.run_steps_virtual([sdist.nystroem_factor_steps(ops, 0, 1, n_train, dim_i, cols, lam)])[0]
+        ops = _EngineNystroemOps(self, R_desc, R_d_desc, tril_perms_lin, sig, use_E_cstr=use_E_cstr)
+        X, _, _ = sdist.run_steps_virtual(
+            [sdist.nystroem_factor_steps(ops, 0, 1, n_train, dim_i, cols, lam, use_E_cstr=use_E_cstr)]
+        )[0]
         return X, len(cols)
 
     def _shard_precon(self, n_train):
@@ -222,14 +226,15 @@ class Iterative(object):
         n_train = R_desc.shape[0]
         dim_i = 3 * task['R_train'].shape[1]
         m = len(inducing_pts_idxs)
-        ops = _EngineNystroemOps(self, R_desc, R_d_desc, tril_perms_lin, task['sig'])
+        ecstr = bool(task['use_E_cstr'])
+        ops = _EngineNystroemOps(self, R_desc, R_d_desc, tril_perms_lin, task['sig'], use_E_cstr=ecstr)
         X, lo, hi = sdist.run_steps(
-            sdist.nystroem_factor_steps(ops, rank, world, n_train, dim_i, inducing_pts_idxs, lam), n_train
+            sdist.nystroem_factor_steps(ops, rank, world, n_train, dim_i, inducing_pts_idxs, lam, use_E_cstr=ecstr), n_train
         )
-        lev_scores = sdist.run_steps(sdist.lev_scores_steps(ops, X, m, dim_i), n_train)
+        lev_scores = sdist.run_steps(sdist.lev_scores_steps(ops, X, m, dim_i, use_E_cstr=ecstr), n_train)
 
         def _P_vec(v):
-            return sdist.run_steps(sdist.precon_apply_steps(ops, X, m, lam, v, lo, hi, dim_i), n_train)
+            return sdist.run_steps(sdist.precon_apply_steps(ops, X, m, lam, v, lo, hi, dim_i, use_E_cstr=ecstr), n_train)
 
         _P_vec.keepalive = X
         _P_vec.factor = (X, m, lo, hi)  # the device PCG applies the factor itself (sgdml_b200_pcg)
@@ -262,11 +267,15 @@ class Iterative(object):
         return _P_vec, lev_scores
 
     def _init_kernel_operator(self, task, R_desc, R_d_desc, tril_perms_lin, lam, n, callback=None):
-        """iterative.py:144-206: K v = predict_train(alphas = v, std = 1) - lam v."""
+        """iterative.py:144-206: K v = predict_train(alphas = v, std = 1) - lam v.  With energy constraints
+        v = [v_F; v_E] and K v = [F; -E] of the predictor with alphas_F = v_F, alphas_E = v_E."""
         from ..predict import GDMLPredict
 
-        v_F = np.zeros(n)
-        model = self.gdml_train.create_model(task, 'cg', R_desc, R_d_desc, tril_perms_lin, 1.0, v_F)
+        n_train = R_desc.shape[0]
+        ecstr = bool(task['use_E_cstr'])
+        v_F = np.zeros(n - n_train) if ecstr else np.zeros(n)
+        v_E = np.zeros(n_train) if ecstr else None
+        model = self.gdml_train.create_model(task, 'cg', R_desc, R_d_desc, tril_perms_lin, 1.0, v_F, alphas_E=v_E)
         self.gdml_predict = GDMLPredict(model, max_memory=self._max_memory, max_processes=self._max_processes)
         # K.v on the int8 tensor cores (wgmma) for large descriptors (5 exact int8 slices: forces within 6.5e-11 of the FP64
         # contractions, CG tolerance 1e-4; 1.43x the FP64 contractions' throughput at BASELINE config 3 on an H100 at 400 W);
@@ -281,10 +290,24 @@ class Iterative(object):
         from .. import dist as sdist
 
         rank, world = self._world()
-        n_train = R_desc.shape[0]
 
         def _K_vec(v):
             v = np.ascontiguousarray(v, dtype=np.float64)
+            if ecstr:
+                n_f = v.size - n_train
+                self.gdml_predict.set_alphas(v[:n_f], alphas_E=v[n_f:])
+
+                def rows(lo, hi):  # [F | E] of training points [lo, hi), raw sums
+                    FE = np.empty((hi - lo, 3 * self.gdml_predict.n_atoms + 1))
+                    E = np.empty(hi - lo)
+                    FE[:, :-1] = self.gdml_predict.kmatvec_train(lo, hi, E_out=E)
+                    FE[:, -1] = E
+                    return FE
+
+                FE = sdist.kmatvec_sharded(rows, n_train) if world > 1 else rows(0, n_train)
+                pred = np.concatenate([FE[:, :-1].ravel(), -FE[:, -1]])  # iterative.py:196-198
+                pred -= lam * v
+                return pred
             self.gdml_predict.set_alphas(v)
             if world > 1:
                 # SURVEY 8e: output rows (training points) sharded over the ranks, alphas replicated, one
@@ -302,19 +325,19 @@ class Iterative(object):
         n_train, dim_d = R_d_desc.shape[:2]
         dim_i = 3 * int((1 + np.sqrt(8 * dim_d + 1)) / 2)
         dim_m = dim_i * min(n_inducing_pts, 10)
-        lev_approx_idxs = np.sort(np.random.choice(n_train * dim_i, dim_m, replace=False))
+        # columns of the (3NM + M)-square system with energy constraints (iterative.py:372-379)
+        lev_approx_idxs = np.sort(np.random.choice(n_train * dim_i + (n_train if use_E_cstr else 0), dim_m, replace=False))
         if self._shard_precon(n_train):
             from .. import dist as sdist
 
-            if use_E_cstr:
-                raise NotImplementedError('use_E_cstr is supported with the analytic solver only (the reference marks its iterative path unfinished, iterative.py:602)')
             rank, world = self._world()
             lev_approx_idxs = self._bcast_idxs(lev_approx_idxs)  # one draw (rank 0's) for the shared factor
-            ops = _EngineNystroemOps(self, R_desc, R_d_desc, tril_perms_lin, sig)
+            ops = _EngineNystroemOps(self, R_desc, R_d_desc, tril_perms_lin, sig, use_E_cstr=use_E_cstr)
             X, lo, hi = sdist.run_steps(
-                sdist.nystroem_factor_steps(ops, rank, world, n_train, dim_i, lev_approx_idxs, lam), n_train
+                sdist.nystroem_factor_steps(ops, rank, world, n_train, dim_i, lev_approx_idxs, lam, use_E_cstr=use_E_cstr),
+                n_train,
             )
-            return sdist.run_steps(sdist.lev_scores_steps(ops, X, len(lev_approx_idxs), dim_i), n_train)
+            return sdist.run_steps(sdist.lev_scores_steps(ops, X, len(lev_approx_idxs), dim_i, use_E_cstr=use_E_cstr), n_train)
         X, m = self._nystroem_cholesky_factor(R_desc, R_d_desc, tril_perms_lin, sig, lam, use_E_cstr, lev_approx_idxs)
         lev = np.empty(X.shape[0])
         _lib.check(
@@ -336,6 +359,8 @@ class Iterative(object):
         sig, lam = task['sig'], float(task['lam'])
 
         alphas0_F = task['alphas0_F'] if 'alphas0_F' in task else None
+        alphas0_E = task['alphas0_E'] if 'alphas0_E' in task else None
+        ecstr = bool(task['use_E_cstr'])
         num_iters0 = int(task['solver_iters']) if 'solver_iters' in task else 0
 
         max_memory_bytes = self._max_memory * 1024**3
@@ -361,7 +386,12 @@ class Iterative(object):
 
         y = np.ascontiguousarray(y, dtype=np.float64)
         norm_y = _norm(y)
-        x0 = None if alphas0_F is None else -np.asarray(alphas0_F, dtype=np.float64).copy()
+        x0 = None
+        if alphas0_F is not None:  # iterative.py:608-613: x0 = -[alphas0_F; alphas0_E]
+            x0 = -np.asarray(alphas0_F, dtype=np.float64).ravel()
+            if ecstr:
+                a0_E = np.zeros(n_train) if alphas0_E is None else np.asarray(alphas0_E, dtype=np.float64).ravel()
+                x0 = np.concatenate([x0, -a0_E])
         maxiter = 3 * n_atoms * n_train * 10  # iterative.py:746-749
 
         state = {
@@ -411,7 +441,7 @@ class Iterative(object):
         x = x0
         while True:  # restart loop (iterative.py:737-801)
             state['restart'] = False
-            x, resid = self._pcg_device(P_vec.factor, lam, y, x, tol * norm_y, maxiter, dim_i, on_progress, state)
+            x, resid = self._pcg_device(P_vec.factor, lam, y, x, tol * norm_y, maxiter, dim_i, on_progress, state, ecstr=ecstr)
             if not state['restart']:
                 is_conv = resid <= tol * norm_y
                 break
@@ -438,11 +468,13 @@ class Iterative(object):
             )
         return alphas, tol, num_iters, resid, train_rmse, inducing_pts_idxs, is_conv
 
-    def _pcg_device(self, factor, lam, y, x0, tol_abs, maxiter, dim_i, on_progress, state, check_every=25):
+    def _pcg_device(self, factor, lam, y, x0, tol_abs, maxiter, dim_i, on_progress, state, check_every=25, ecstr=False):
         """One run of the device-resident PCG (`sgdml_b200_pcg`, csrc/pcg.cu): every CG vector stays in HBM, the
         host gets the residual history every <= check_every iterations.  With several ranks the K.v rows and the
         Nystroem factor rows are those of this rank's training points and the three exchanges per iteration run
-        as torch.distributed collectives on views of the device workspace (dist.exchange_on_workspace)."""
+        as torch.distributed collectives on views of the device workspace (dist.exchange_on_workspace).
+        ecstr: the (3NM + M)-square energy-constrained system (`sgdml_b200_pcg_ecstr`), vectors [forces; energies];
+        the energy tails of K.v and P.v are exchanged separately (op 2)."""
         import ctypes
 
         import torch
@@ -453,11 +485,12 @@ class Iterative(object):
         X, m, lo, hi = factor
         rank, world = self._world()
         n_train = self.gdml_predict.n_train
-        n = n_train * dim_i
+        n = n_train * dim_i + (n_train if ecstr else 0)
         if world == 1:
             lo, hi = 0, n_train
-        n_rows_loc = (hi - lo) * dim_i
-        ws_doubles = int(L.sgdml_b200_pcg_workspace_doubles(n, n_rows_loc, m, check_every))
+        n_rows_loc = (hi - lo) * (dim_i + 1 if ecstr else dim_i)
+        ws_fn = L.sgdml_b200_pcg_ecstr_workspace_doubles if ecstr else L.sgdml_b200_pcg_workspace_doubles
+        ws_doubles = int(ws_fn(n, n_rows_loc, m, check_every))
         ws = torch.empty(ws_doubles, dtype=torch.float64, device='cuda')
         state['x_dev'] = ws[:n]  # the solution vector is the first slot of the workspace (csrc/pcg.cu)
         if state['resid'] is None:
@@ -491,8 +524,9 @@ class Iterative(object):
         prog = _lib.PROGRESS_FN(_progress)
         x = np.zeros(n) if x0 is None else np.ascontiguousarray(x0, dtype=np.float64)
         iters, resid = ctypes.c_int64(0), ctypes.c_double(0.0)
+        pcg = L.sgdml_b200_pcg_ecstr if ecstr else L.sgdml_b200_pcg
         _lib.check(
-            L.sgdml_b200_pcg(
+            pcg(
                 self.gdml_predict._handle, lo, hi, X.data_ptr() if m > 0 else None, m, X.shape[1] if m > 0 else 0,
                 float(lam), _lib.ptr(y), _lib.ptr(x), 1 if x0 is None else 0, float(tol_abs), int(maxiter),
                 int(check_every), ws.data_ptr(), ws_doubles, exch, None, prog, None,
@@ -522,7 +556,12 @@ class Iterative(object):
         return t.cpu().numpy()
 
     def _checkpoint_model(self, task, R_desc, R_d_desc, tril_perms_lin, y_std, xk, tol, num_iters, resid, norm_y, idxs):
-        model = self.gdml_train.create_model(task, 'cg', R_desc, R_d_desc, tril_perms_lin, y_std, -xk)
+        """iterative.py:685-724: the current iterate as a model (alphas_F and, with energy constraints, alphas_E)."""
+        alphas_F, alphas_E = -xk, None
+        if task['use_E_cstr']:
+            n_train = R_desc.shape[0]
+            alphas_F, alphas_E = -xk[:-n_train], -xk[-n_train:]
+        model = self.gdml_train.create_model(task, 'cg', R_desc, R_d_desc, tril_perms_lin, y_std, alphas_F, alphas_E=alphas_E)
         model.update(
             {
                 'solver_tol': tol,
@@ -534,7 +573,7 @@ class Iterative(object):
         )
         model['c'] = 0
         if 'E_train' in task:
-            self.gdml_predict.set_alphas(-xk)
+            self.gdml_predict.set_alphas(alphas_F, alphas_E=alphas_E)
             E_pred = self.gdml_predict.predict()[0]  # std = 1, c = 0 model
             model['c'] = np.mean(np.squeeze(task['E_train']) - E_pred * y_std)
         return model

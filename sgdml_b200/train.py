@@ -182,11 +182,9 @@ class GDMLTrain(object):
             from . import dist as sdist
 
             max_bytes = sdist.all_reduce_min_scalar(max_bytes)
+        # with energy constraints the iterative solver works on the (3NM + M)-square system [forces; energies], as the
+        # reference's does (iterative.py:183-204, 372-379, 685-698)
         use_analytic_solver = est_bytes_analytic < max_bytes
-        if use_E_cstr and not use_analytic_solver:
-            # the reference's own iterative path is unfinished for energy constraints (iterative.py:602 "TODO: ... this
-            # will not work with E_cstr"); the engine supports them with the analytic solver
-            raise NotImplementedError('use_E_cstr needs the analytic solver (the kernel matrix must fit the device memory)')
 
         solver_keys = {}
         if use_analytic_solver:
@@ -346,6 +344,32 @@ class GDMLTrain(object):
         )
         return K
 
+    def _assemble_kernel_mat_ecstr_rows_device(self, R_desc, R_d_desc, tril_perms_lin, sig, col_idxs, rows=None, scale=1.0):
+        """Columns col_idxs (sorted unique, in [0, 3NM + M)) of the energy-constrained kernel matrix as a CUDA tensor
+        (n_rows, ldk), first len(col_idxs) columns meaningful.  Rows: the force rows of training points
+        rows=(m_begin, m_end) (default: all), then their energy rows -- (m_end - m_begin)(3N + 1) rows."""
+        torch = _torch()
+        views = getattr(self, '_dev_views', {})
+        R_desc = views.get(id(R_desc), None) if id(R_desc) in views else np.ascontiguousarray(R_desc, dtype=np.float64)
+        R_d_desc = views.get(id(R_d_desc), None) if id(R_d_desc) in views else np.ascontiguousarray(R_d_desc, dtype=np.float64)
+        tril_perms_lin = np.ascontiguousarray(tril_perms_lin, dtype=np.int64)
+        n_train, dim_d = R_d_desc.shape[:2]
+        n_atoms = int((1 + np.sqrt(8 * dim_d + 1)) / 2)
+        n_perms = len(tril_perms_lin) // dim_d
+        cols = np.ascontiguousarray(col_idxs, dtype=np.int64)
+        n_cols = len(cols)
+        ldk = (n_cols + 1) // 2 * 2  # even row stride, as _assemble_kernel_mat_device
+        m_begin, m_end = (0, n_train) if rows is None else (int(rows[0]), int(rows[1]))
+        K = torch.empty(((m_end - m_begin) * (3 * n_atoms + 1), ldk), dtype=torch.float64, device='cuda')
+        _lib.check(
+            _lib.lib().sgdml_b200_assemble_ecstr_rows(
+                _lib.ptr(R_desc), _lib.ptr(R_d_desc), _lib.ptr(tril_perms_lin), n_atoms, n_train, n_perms, float(sig),
+                _lib.ptr(cols), n_cols, float(scale), m_begin, m_end, K.data_ptr(), ldk, _lib.current_stream(),
+            ),
+            'assemble_ecstr_rows',
+        )
+        return K, n_cols
+
     def _assemble_kernel_mat(
         self,
         R_desc,
@@ -363,13 +387,23 @@ class GDMLTrain(object):
         n_train, dim_d = R_d_desc.shape[:2]
         dim_i = 3 * int((1 + np.sqrt(8 * dim_d + 1)) / 2)
         K_n_rows = n_train * dim_i
-        if use_E_cstr:  # train.py:1333-1335: M extra rows and columns; full matrix only (what the analytic solver needs)
-            if not (isinstance(col_idxs, slice) and col_idxs == np.s_[:]):
-                raise NotImplementedError('column subsets of the energy-constrained kernel matrix are not supported')
-            Kd = self._assemble_kernel_mat_ecstr_device(R_desc, R_d_desc, tril_perms_lin, sig, scale=1.0)
+        if use_E_cstr:  # train.py:1333-1335: M extra rows and columns
             n_tot = K_n_rows + n_train
-            K = np.empty((n_tot + alloc_extra_rows, n_tot))
-            K[:n_tot, :] = Kd[:, :n_tot].cpu().numpy()
+            if isinstance(col_idxs, slice) and col_idxs == np.s_[:]:
+                Kd = self._assemble_kernel_mat_ecstr_device(R_desc, R_d_desc, tril_perms_lin, sig, scale=1.0)
+                K = np.empty((n_tot + alloc_extra_rows, n_tot))
+                K[:n_tot, :] = Kd[:, :n_tot].cpu().numpy()
+                return K
+            # column subset (the Nystroem set-up, iterative.py:232-247): the engine's rows are already in the
+            # reference's order [forces; energies]
+            cols = np.arange(n_tot)[col_idxs] if isinstance(col_idxs, slice) else np.asarray(col_idxs, dtype=np.int64)
+            assert len(cols) == len(set(cols.tolist()))  # train.py:1337
+            assert np.array_equal(cols, np.sort(cols))  # train.py:1341-1345
+            if len(cols) > n_tot or (len(cols) and (cols[0] < 0 or cols[-1] >= n_tot)):
+                raise ValueError('Columns indexed beyond range.')  # train.py:1349-1350
+            Kd, n_cols = self._assemble_kernel_mat_ecstr_rows_device(R_desc, R_d_desc, tril_perms_lin, sig, cols)
+            K = np.empty((n_tot + alloc_extra_rows, n_cols))
+            K[:n_tot, :] = Kd[:, :n_cols].cpu().numpy()
             return K
         if isinstance(col_idxs, slice):
             cols = np.arange(K_n_rows)[col_idxs]

@@ -19,6 +19,7 @@ ap.add_argument('--max-memory', type=float, default=8.0, help='GB; below the ana
 ap.add_argument('--n-query', type=int, default=64)
 ap.add_argument('--profile', action='store_true', help='per-kernel-family device times (adds synchronisation)')
 ap.add_argument('--trace', type=int, default=0, help='print the CG residual every this many iterations')
+ap.add_argument('--E-cstr', action='store_true', help='energy constraints in the kernel: the (3NM + M)-square system')
 a = ap.parse_args()
 
 world = int(os.environ.get('WORLD_SIZE', '1'))
@@ -34,6 +35,7 @@ import sgdml_b200  # noqa: E402
 from sgdml_b200 import synth  # noqa: E402
 
 task = synth.make_config_task(a.workload, n_train=a.n_train)
+task['use_E_cstr'] = a.E_cstr
 N = task['R_train'].shape[1]
 np.random.seed(0)
 trainer = sgdml_b200.GDMLTrain(max_memory=a.max_memory)
@@ -74,7 +76,8 @@ if rank == 0:
         'n_atoms': N,
         'n_train': a.n_train,
         'n_perms': int(len(task['perms'])),
-        'n': 3 * N * a.n_train,
+        'use_E_cstr': bool(a.E_cstr),
+        'n': 3 * N * a.n_train + (a.n_train if a.E_cstr else 0),
         'solver': str(model['solver_name']),
         'train_s': dt,
         'timings': {k: float(v) for k, v in trainer.timings.items()},
@@ -85,6 +88,8 @@ if rank == 0:
             iters=int(model['solver_iters']),
             n_inducing_cols=int(len(model['inducing_pts_idxs'])),
             resid_rel=float(model['solver_resid'] / model['norm_y_train']),
+            setup_s=float(trainer.timings.get('precon_s', float('nan'))),  # leverage scores + preconditioner
+            cg_s_per_iter=float(trainer.timings['cg_s'] / max(1, trainer.timings['iters'])),
         )
     print(json.dumps(out))
 if world > 1:

@@ -130,14 +130,6 @@ int sgdml_b200_predict_train(sgdml_b200_model* model, int64_t m_begin, int64_t m
  * (iterative.py:183-204: tolerance 1e-4).  No effect for D <= 256. */
 int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* model, int slices, void* stream);
 
-/* Test / tuning hook: main kernel of the fused predictor (D <= 256).  0 = default (the measured-fastest kernel per
- * descriptor size); 1 = two warp groups running the sweep half a tile apart (72 < D; measured slower); 2 = no split
- * over k in the first contraction: Matern transform on the accumulator fragments, two CTA-wide barriers per tile
- * instead of three (72 < D <= 224); 3 = 2 with C1 / C2 double-buffered and ONE barrier per tile (D <= 224); 4 = the
- * round-1 kernels for every size; 5 = the one-barrier form on 16-point tiles for D <= 40 (two CTAs per SM).  A variant
- * without a kernel for a size runs the default kernel of that size. */
-int sgdml_b200_set_predict_variant(int variant);
-
 /* Shape of a model: n_atoms, n_train, n_perms (any pointer may be NULL). */
 int sgdml_b200_model_dims(const sgdml_b200_model* model, int64_t* n_atoms, int64_t* n_train, int64_t* n_perms);
 
@@ -192,10 +184,10 @@ int sgdml_b200_assemble_ecstr_rows(const double* R_desc, const double* R_d_desc,
                                    int64_t m_end, double* K, int64_t ldk, void* stream);
 
 /* Tuning / test hook: 0 = kernel chosen by molecule size (default), 1 = always the large-molecule
- * kernel (tables in global memory), which molecules above ~50 atoms need; 2 / 3 / 4 = small-molecule kernel with
- * per-permutation phases (k_assemble) / with permutation chunks and resident row tables (k_assemble_v3) / chunks of
- * up to 16 permutations with byte permutation tables and per-kind phases over the kept column atoms (k_assemble_v4);
- * 1000 + r = at most r row
+ * kernel (tables in global memory), which molecules above ~50 atoms need; 2 / 4 / 5 = small-molecule kernel with
+ * per-permutation phases (k_assemble) / chunks of up to 16 permutations with byte permutation tables and per-kind
+ * phases over the kept column atoms (k_assemble_v4) / the same on the compressed pair arrays (k_assemble_v5), where
+ * the shared-memory budget allows it; any other value is rejected; 1000 + r = at most r row
  * points per launch of the small-molecule kernel (default 65535, the grid limit; tests lower it to
  * cover the multi-launch path that row ranges above 65535 training points take). */
 int sgdml_b200_set_assemble_variant(int variant);
@@ -352,8 +344,10 @@ int sgdml_b200_set_solve_slices(int n_slices);
 int sgdml_b200_get_solve_slices(void);
 
 /* Test / tuning hook: selects the GEMM kernel used by dgemm_nt and potrf's trailing update.
- * 0 = 128x128 DMMA tiles fed by cp.async, 1 = 128x64 DMMA tiles, 2 = scalar FMA reference kernel,
- * 3 = 128x128 DMMA tiles fed by TMA tensor maps (cp.async.bulk.tensor + mbarrier ring; default). */
+ * 0 = 128x128 DMMA tiles fed by cp.async, 2 = scalar FMA reference kernel, 3 = 128x128 DMMA tiles fed by TMA tensor
+ * maps (cp.async.bulk.tensor + mbarrier ring; default).  Any other value is rejected.  Whatever the setting, operands
+ * the tiled kernels cannot load (odd k or strides, or not 16-byte aligned) run the scalar kernel, and 3 runs the
+ * cp.async tiles when the driver offers no tensor-map encoder. */
 int sgdml_b200_set_gemm_variant(int variant);
 
 #ifdef __cplusplus

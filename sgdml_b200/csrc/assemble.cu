@@ -318,264 +318,21 @@ __global__ void __launch_bounds__(256, 2) k_assemble(const AsmArgs p) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// k_assemble_v3: the same mathematics, restructured around what the first kernel's profile showed
-// (few warps active, a mostly idle FP64 pipe, barrier / short-scoreboard / wait stalls):
-//  * permutations are processed in CHUNKS of PG: phase A computes the per-(point, permutation) vectors u, v, Dg of
-//    the whole chunk in one go -- tj * PG * 5N independent row tasks instead of tj * 5N, so all 256 threads have
-//    work -- with the delta table evaluated on the fly (delta_p[Pa][Pg] = x_i[a][g] - x_j[Pa][Pg]; no staged table,
-//    no barrier between "delta" and "vectors"); |delta_p|^2 falls out of the v rows;
-//  * three CTA barriers per chunk (after the vectors, after the Matern factors, before the vectors are overwritten)
-//    instead of two per permutation;
-//  * a CTA walks over `tiles_per_cta` column tiles with the row point's tables (G_i, X_i, permutations) resident.
-// Phase B (the 3x3 sub-block accumulation in registers) is unchanged.
-__global__ void __launch_bounds__(256, 2) k_assemble_v3(const AsmArgs p, int PG, int tiles_per_cta) {
-  extern __shared__ __align__(16) double sm[];
-  const int N = p.N, S = p.S, TJ = p.TJ;
-  const int N3 = 3 * N, NN = N * N, NN3 = NN * 3;
-  const int tid = threadIdx.x, nt = blockDim.x;
-  const int warp = tid >> 5, lane = tid & 31, nw = nt >> 5;
-  const int i = p.i0 + blockIdx.y;
-
-  double* Gi = sm;                      // NN3
-  double* Xi = Gi + NN3;                // NN
-  double* Gj = Xi + NN;                 // TJ*NN3
-  double* Xj = Gj + TJ * NN3;           // TJ*NN
-  double* uS = Xj + TJ * NN;            // TJ*PG*N3
-  double* vS = uS + TJ * PG * N3;       // TJ*PG*N3
-  double* DgS = vS + TJ * PG * N3;      // TJ*PG*3*N3
-  double* n2p = DgS + TJ * PG * 3 * N3; // TJ*PG*N   per-row sums of squared deltas (each pair twice)
-  double* cc = n2p + TJ * PG * N;       // TJ*PG*2
-  int* sP = reinterpret_cast<int*>(cc + TJ * PG * 2);  // S*N
-  int* sPi = sP + S * N;                                    // S*N
-  int* need = sPi + S * N;                                  // TJ*N: column atom b of point t has a kept column
-  int* klist = need + TJ * N;                               // TJ*N: the kept column atoms of point t, compact
-  int* nk = klist + TJ * N;                                 // TJ: how many
-
-  load_pair_tables(p.R_d_desc + (int64_t)i * p.D * 3, p.R_desc + (int64_t)i * p.D, N, Gi, Xi, warp, lane, nw);
-  for (int idx = tid; idx < S * N; idx += nt) {
-    sP[idx] = p.aperm[idx];
-    sPi[idx] = p.apinv[idx];
-  }
-  const double sig = p.sig;
-  const double sig2 = sig * sig;
-  const double inv_div = 1.0 / (3.0 * sig2 * sig2);  // 1/mat52_base_div (train.py:179)
-  const int per = 5 * N;  // row tasks per (point, permutation): N (u) + N (v) + 3N (Dg rows a,c)
-
-  const int tile_begin = blockIdx.x * tiles_per_cta;
-  const int tile_end = min(tile_begin + tiles_per_cta, ceil_div_dev(p.nJ, TJ));
-  for (int tile = tile_begin; tile < tile_end; ++tile) {
-    const int jt0 = tile * TJ;
-    const int tj = min(TJ, p.nJ - jt0);
-    if (p.sym && jt0 + tj - 1 < i) continue;  // (sym: jpts is the identity) every column point of the tile is < i
-    __syncthreads();  // the previous tile's phase B has finished with Gj / the vectors
-    for (int t = 0; t < tj; ++t) {
-      const int j = p.jpts[jt0 + t];
-      load_pair_tables(p.R_d_desc + (int64_t)j * p.D * 3, p.R_desc + (int64_t)j * p.D, N, Gj + t * NN3, Xj + t * NN, warp,
-                       lane, nw);
-    }
-    for (int idx = tid; idx < tj * N; idx += nt) {  // column atoms with at least one kept column (column subsets)
-      const int64_t* dst = p.dest + (int64_t)(jt0 + idx / N) * N3 + 3 * (idx % N);
-      need[idx] = (dst[0] >= 0 || dst[1] >= 0 || dst[2] >= 0) ? 1 : 0;
-    }
-    if (tid < tj) {  // compact list of the kept column atoms of every column point
-      int c = 0;
-      for (int b = 0; b < N; ++b) {
-        const int64_t* dst = p.dest + (int64_t)(jt0 + tid) * N3 + 3 * b;
-        if (dst[0] >= 0 || dst[1] >= 0 || dst[2] >= 0) klist[tid * N + c++] = b;
-      }
-      nk[tid] = c;
-    }
-    __syncthreads();
-    // this thread's output items: (t, a, b) = column point, row atom, kept column atom
-    int it_t[ASM_NI], it_a[ASM_NI], it_b[ASM_NI];
-    double acc[ASM_NI][9];
-#pragma unroll
-    for (int q = 0; q < ASM_NI; ++q) {
-      const int it = (int)blockIdx.z * ASM_NI * nt + tid + q * nt;  // grid.z splits the sub-blocks of large molecules
-      bool ok = it < tj * N * p.NK;
-      const int t = ok ? fastdiv(it, p.mNNK) : 0;
-      if (p.sym && jt0 + t < i) ok = false;  // mirrored from block (j, i) instead
-      const int ak = ok ? it - t * N * p.NK : 0;
-      it_a[q] = fastdiv(ak, p.mNK);
-      const int k = ak - it_a[q] * p.NK;
-      if (k >= nk[t]) ok = false;
-      it_b[q] = ok ? klist[t * N + k] : 0;
-      it_t[q] = ok ? t : -1;
-#pragma unroll
-      for (int e = 0; e < 9; ++e) acc[q][e] = 0.0;
-    }
-
-    for (int p0 = 0; p0 < S; p0 += PG) {
-      const int pg = min(PG, S - p0);
-      // ---- phase A: u, v (+ row sums of delta^2), Dg for every (column point, permutation) of the chunk
-      for (int idx = tid; idx < tj * pg * per; idx += nt) {
-        const int tp = fastdiv(idx, p.mPer);
-        const int r = idx - tp * per;
-        const int t = tp / pg, pl = tp - t * pg;
-        const int* P = sP + (p0 + pl) * N;
-        const int* Pi = sPi + (p0 + pl) * N;
-        const double* Gjt = Gj + t * NN3;
-        const double* Xjt = Xj + t * NN;
-        const int slot = t * PG + pl;
-        if (r < N) {  // u[a] = -sum_g G_i[a][g] delta[Pa][Pg],  delta[Pa][Pg] = x_i[a][g] - x_j[Pa][Pg]
-          const int a = r;
-          const double* gi = Gi + a * N3;
-          const double* xi = Xi + a * N;
-          const double* xj = Xjt + P[a] * N;
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double d = xi[g] - xj[P[g]];
-            s0 = fma(gi[g * 3 + 0], d, s0);
-            s1 = fma(gi[g * 3 + 1], d, s1);
-            s2 = fma(gi[g * 3 + 2], d, s2);
-          }
-          double* u = uS + slot * N3 + 3 * a;
-          u[0] = -s0;
-          u[1] = -s1;
-          u[2] = -s2;
-        } else if (r < 2 * N) {  // v[b] = -sum_g G_j[b][g] delta[b][g],  delta[b][g] = x_i[P^-1 b][P^-1 g] - x_j[b][g]
-          const int b = r - N;
-          const double* gj = Gjt + b * N3;
-          const double* xj = Xjt + b * N;
-          const double* xi = Xi + Pi[b] * N;
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0, q2 = 0.0;
-          if (need[t * N + b]) {
-            for (int g = 0; g < N; ++g) {
-              const double d = xi[Pi[g]] - xj[g];
-              q2 = fma(d, d, q2);
-              s0 = fma(gj[g * 3 + 0], d, s0);
-              s1 = fma(gj[g * 3 + 1], d, s1);
-              s2 = fma(gj[g * 3 + 2], d, s2);
-            }
-          } else {  // v[b] is never read: only this row's share of |delta|^2 (same summation order)
-            for (int g = 0; g < N; ++g) {
-              const double d = xi[Pi[g]] - xj[g];
-              q2 = fma(d, d, q2);
-            }
-          }
-          double* v = vS + slot * N3 + 3 * b;
-          v[0] = -s0;
-          v[1] = -s1;
-          v[2] = -s2;
-          n2p[slot * N + b] = q2;
-        } else {  // Dg[a][c][0..2] = sum_g G_i[a][g][c] G_j[Pa][Pg][0..2]
-          const int ac = r - 2 * N;
-          const int a = (int)__umulhi((unsigned)ac, 0x55555556u), c = ac - 3 * a;
-          if (!need[t * N + P[a]]) continue;  // only read for the sub-block (a, b = P a)
-          const double* gi = Gi + a * N3 + c;
-          const double* gj = Gjt + P[a] * N3;
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double x = gi[g * 3];
-            const double* y = gj + P[g] * 3;
-            s0 = fma(x, y[0], s0);
-            s1 = fma(x, y[1], s1);
-            s2 = fma(x, y[2], s2);
-          }
-          double* dg = DgS + slot * 3 * N3 + ac * 3;
-          dg[0] = s0;
-          dg[1] = s1;
-          dg[2] = s2;
-        }
-      }
-      __syncthreads();
-      // ---- Matern factors of the chunk (fixed-order sum of the row partials: bit-reproducible K)
-      if (tid < tj * pg) {
-        const int t = tid / pg, pl = tid - t * pg;
-        const int slot = t * PG + pl;
-        double n2 = 0.0;
-        for (int b = 0; b < N; ++b) n2 += n2p[slot * N + b];
-        const double nrm = sqrt(5.0) * sqrt(0.5 * n2);  // every pair twice; train.py:201
-        const double base = exp(-nrm / sig) * inv_div * 5.0;          // train.py:202
-        cc[slot * 2 + 0] = base * 5.0;                                 // c1 (train.py:211)
-        cc[slot * 2 + 1] = (sig2 + sig * nrm) * base;                  // c2 (train.py:219)
-      }
-      __syncthreads();
-      // ---- phase B: acc[a][b] += c1 u[a] (x) v[b] - c2 T[a][b] for the permutations of the chunk
-      for (int pl = 0; pl < pg; ++pl) {
-        const int* P = sP + (p0 + pl) * N;
-        const int* Pi = sPi + (p0 + pl) * N;
-#pragma unroll
-        for (int q = 0; q < ASM_NI; ++q) {
-          const int t = it_t[q];
-          if (t < 0) continue;
-          const int slot = t * PG + pl;
-          const int a = it_a[q], b = it_b[q];
-          const double c1 = cc[slot * 2 + 0], c2 = cc[slot * 2 + 1];
-          const double* ua = uS + slot * N3 + 3 * a;
-          const double* vb = vS + slot * N3 + 3 * b;
-          const int pa = P[a];
-          if (b != pa) {
-            const double* gi = Gi + (a * N + Pi[b]) * 3;
-            const double* gj = Gj + t * NN3 + (pa * N + b) * 3;
-            double t0[3], t1[3];  // T[a][b] = -gi (x) gj  ->  -c2 T = +c2 gi (x) gj
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              t0[c] = c2 * gi[c];
-              t1[c] = gj[c];
-            }
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              const double cu = c1 * ua[c];
-#pragma unroll
-              for (int c2i = 0; c2i < 3; ++c2i)
-                acc[q][c * 3 + c2i] = fma(t0[c], t1[c2i], fma(cu, vb[c2i], acc[q][c * 3 + c2i]));
-            }
-          } else {
-            const double* dg = DgS + slot * 3 * N3 + 9 * a;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              const double cu = c1 * ua[c];
-#pragma unroll
-              for (int c2i = 0; c2i < 3; ++c2i)
-                acc[q][c * 3 + c2i] = fma(-c2, dg[c * 3 + c2i], fma(cu, vb[c2i], acc[q][c * 3 + c2i]));
-            }
-          }
-        }
-      }
-      if (p0 + PG < S) __syncthreads();  // the next chunk overwrites the vectors
-    }
-
-    // ---- single store of the finished 3x3 sub-blocks (+ the mirrored block in symmetric mode)
-#pragma unroll
-    for (int q = 0; q < ASM_NI; ++q) {
-      const int t = it_t[q];
-      if (t < 0) continue;
-      const int a = it_a[q], b = it_b[q];
-      const int64_t* dst = p.dest + (int64_t)(jt0 + t) * N3 + 3 * b;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        double* Krow = p.K + ((int64_t)(i - p.i0) * N3 + 3 * a + c) * p.ldk;
-#pragma unroll
-        for (int c2i = 0; c2i < 3; ++c2i) {
-          const int64_t col = dst[c2i];
-          if (col >= 0) Krow[col] = p.scale * acc[q][c * 3 + c2i];
-        }
-      }
-      if (p.sym && jt0 + t > i) {  // (sym implies i0 == 0)
-        const int j = jt0 + t;
-#pragma unroll
-        for (int c2i = 0; c2i < 3; ++c2i) {
-          double* Krow = p.K + ((int64_t)j * N3 + 3 * b + c2i) * p.ldk + (int64_t)i * N3 + 3 * a;
-#pragma unroll
-          for (int c = 0; c < 3; ++c) Krow[c] = p.scale * acc[q][c * 3 + c2i];
-        }
-      }
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// k_assemble_v4: the chunked kernel for MANY permutations and column subsets (BASELINE config 3: N = 42, S = 243, the
-// Nystroem set-up keeps ~9 of a point's 126 columns).  Against k_assemble_v3:
+// k_assemble_v4: the default small-molecule kernel, built for many permutations and column subsets as well (BASELINE
+// config 3: N = 42, S = 243, the Nystroem set-up keeps ~9 of a point's 126 columns).  Against k_assemble, what the
+// first kernel's profile showed (few warps active, a mostly idle FP64 pipe, barrier / short-scoreboard / wait stalls):
+//  * permutations are processed in CHUNKS of PG: phase A computes the per-(point, permutation) vectors u, v, Dg of the
+//    whole chunk in one go, with the delta table evaluated on the fly (delta_p[Pa][Pg] = x_i[a][g] - x_j[Pa][Pg]; no
+//    staged table); three CTA barriers per chunk instead of two per permutation;
+//  * phase A is enumerated TYPE-major over the chunk -- all u rows, then the v rows, then the Dg rows -- so a warp runs
+//    one kind of row task, and v / Dg rows exist only for column atoms with a kept column (compact list); |delta|^2
+//    comes out of the u rows, which are always needed;
 //  * the atom-permutation tables are bytes (20 KB instead of 82 KB at S = 243, N = 42), which leaves room for chunks of
 //    up to 16 permutations next to the four pair tables of a 42-atom block;
 //  * the pair tables have ODD row strides (3N | 1, N | 1 doubles): threads of a warp work on different table rows, and
-//    with N = 42 the even strides of v3 put every fourth row on the same banks;
-//  * phase A is enumerated TYPE-major over the chunk -- all u rows, then the v rows, then the Dg rows -- so a warp runs
-//    one kind of row task (v3 interleaves the three kinds per permutation: divergent warps), and v / Dg rows exist only
-//    for column atoms with a kept column (compact list); |delta|^2 comes out of the u rows, which are always needed.
-// Phase B (3x3 sub-blocks in registers) is that of v3.
+//    with N = 42 even strides put every fourth row on the same banks;
+//  * a CTA walks over `tiles_per_cta` column tiles with the row point's tables resident.
+// Phase B (the 3x3 sub-block accumulation in registers) is that of k_assemble.
 __device__ void load_pair_tables_strided(const double* __restrict__ g, const double* __restrict__ x, int N, int gs, int xs,
                                          double* __restrict__ G, double* __restrict__ X, int warp, int lane, int nw) {
   for (int a = warp; a < N; a += nw)
@@ -1443,12 +1200,6 @@ static size_t asm_large_slab_doubles(int N, int S) {
   return 2 * (NN * 3 + NN) + (size_t)S * (2 * N3 + 3 * N3 + 2) + NN;
 }
 
-static size_t asm_v3_smem_bytes(int N, int S, int TJ, int PG) {
-  const size_t N3 = 3 * (size_t)N, NN = (size_t)N * N;
-  const size_t dbl = NN * 3 + NN + (size_t)TJ * (NN * 3 + NN) + (size_t)TJ * PG * (2 * N3 + 3 * N3 + N + 2);
-  return dbl * 8 + 2 * (size_t)S * N * 4 + 2 * (size_t)TJ * N * 4 + (size_t)TJ * 4 + 16;
-}
-
 static size_t asm_v4_smem_bytes(int N, int S, int TJ, int PG) {
   const size_t N3 = 3 * (size_t)N, GS = N3 | 1, XS = (size_t)N | 1;
   const size_t dbl = (size_t)N * (GS + XS) * (1 + TJ) + (size_t)TJ * PG * (2 * N3 + 3 * N3 + N + 2);
@@ -1517,7 +1268,7 @@ static bool atom_perm_from_desc_perm(const int* dperm, int N, int* P) {
 }
 
 static int g_asm_variant = 0;  // 0: by size; 1: always the large-molecule kernel (tests)
-static int g_asm_kernel = 0;  // small-molecule kernel: 0 = by size (default), 2 = k_assemble (per-permutation phases), 3 = k_assemble_v3 (chunked), 4 = k_assemble_v4 (chunked, byte permutation tables, type-major phase A)
+static int g_asm_kernel = 0;  // small-molecule kernel: 0 = by size (default), 2 = k_assemble (per-permutation phases), 4 = k_assemble_v4 (chunked), 5 = k_assemble_v5 (chunked, compressed pair arrays)
 static int g_asm_max_rowpts = 65535;  // row points per launch of k_assemble (grid.y limit; lowered by tests)
 
 extern "C" int sgdml_b200_set_assemble_variant(int variant) {
@@ -1527,7 +1278,7 @@ extern "C" int sgdml_b200_set_assemble_variant(int variant) {
     g_asm_max_rowpts = variant - 1000;
     return 0;
   }
-  if (variant >= 2 && variant <= 5) {  // which small-molecule kernel
+  if (variant == 2 || variant == 4 || variant == 5) {  // which small-molecule kernel
     g_asm_kernel = variant;
     return 0;
   }
@@ -1702,15 +1453,6 @@ extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_
       // each with its own first row point and K row offset
       const int max_rows_per_launch = g_asm_max_rowpts;
       if (n_rowpts > max_rows_per_launch) a.sym = 0;  // the mirrored store addresses absolute row points
-      // v3 kernel: permutation chunk PG = as many permutations as keep the shared memory within ~100 KB (two CTAs per
-      // SM) -- all of them for small groups; a CTA walks over 4 column tiles with the row tables resident
-      int PG = S;
-      while (PG > 1 && asm_v3_smem_bytes(N, S, TJ, PG) > 100 * 1024) PG = (PG + 1) / 2;
-      const size_t smem3 = asm_v3_smem_bytes(N, S, TJ, PG);
-      // chosen by timing the variants (tools/asm_variants.py): faster at BASELINE config 2 (S = 6, one chunk); with many
-      // permutations (S = 243, chunks of 8) the chunked kernel is SLOWER than the per-permutation one, so it is
-      // only used when all permutations fit one chunk -- unless a test forces it (variant 3)
-      const bool use_v3 = smem3 <= 220 * 1024 && TJ * PG <= 256 && (g_asm_kernel == 3 || (g_asm_kernel == 0 && PG == S));
       // v4 kernel: chunks of up to 16 permutations; two CTAs per SM when everything fits in ~110 KB, else one
       int PG4 = std::min(S, 16);
       while (PG4 > 1 && (asm_v4_smem_bytes(N, S, TJ, PG4) > 220 * 1024 || TJ * PG4 > 256)) --PG4;
@@ -1728,9 +1470,7 @@ extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_
         SG_CUDA(cudaFuncSetAttribute(k_assemble_v5, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem5));
       } else if (use_v4) {
         SG_CUDA(cudaFuncSetAttribute(k_assemble_v4, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4));
-      } else if (use_v3)
-        SG_CUDA(cudaFuncSetAttribute(k_assemble_v3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
-      else
+      } else
         SG_CUDA(cudaFuncSetAttribute(k_assemble, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       ProfScope ps(KID_ASSEMBLE, s);
       for (int r0 = 0; r0 < n_rowpts; r0 += max_rows_per_launch) {
@@ -1744,9 +1484,6 @@ extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_
         } else if (use_v4) {
           dim3 grid((unsigned)ceil_div(ceil_div(nJ, TJ), tiles_per_cta), (unsigned)nr, (unsigned)n_chunks);
           k_assemble_v4<<<grid, 256, smem4, s>>>(ac, PG4, tiles_per_cta);
-        } else if (use_v3) {
-          dim3 grid((unsigned)ceil_div(ceil_div(nJ, TJ), tiles_per_cta), (unsigned)nr, (unsigned)n_chunks);
-          k_assemble_v3<<<grid, 256, smem3, s>>>(ac, PG, tiles_per_cta);
         } else {
           dim3 grid((unsigned)ceil_div(nJ, TJ), (unsigned)nr, (unsigned)n_chunks);
           k_assemble<<<grid, 256, smem, s>>>(ac);

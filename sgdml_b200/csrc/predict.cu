@@ -98,8 +98,6 @@ struct PredictArgs {
   int64_t n_rows;       // B*S virtual rows
   int64_t n_rows_pad;   // rows rounded up to BQ (stride between the per-split output planes)
   int tiles_per_split;  // blockIdx.y handles training tiles [y*tps, (y+1)*tps): small batches split the sweep over M
-  int bm;               // training points per tile that tiles_per_split is counted in (the model's BM; a kernel with a
-                        // smaller tile converts)
   // outputs
   double* G;            // (n_rows, DP)
   double* Erow;         // (n_rows)
@@ -520,332 +518,6 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
   if (tid < C::BQ && r0 + tid < p.n_rows) p.Erow[(int64_t)blockIdx.y * p.n_rows_pad + r0 + tid] = E_s[tid];
 }
 
-// ============================================================== main kernel, two-group ("ping-pong") form
-// The sweep of k_predict_main alternates tensor-pipe phases (GEMM1, GEMM2) with phases that leave the pipe idle (the
-// split-k reduction + Matern transform, two CTA-wide barriers per tile), which leaves the DMMA pipe idle for part of
-// every tile.  Here the 8 warps form TWO groups of 4 (one warp of each group per SM
-// sub-partition) that own half of the virtual query rows each and synchronise only among themselves (named
-// barriers).  Group 0 runs  GEMM1(t) | transform(t) | GEMM2(t);  group 1 runs the same loop rotated,
-// GEMM2(t) GEMM1(t+1) | transform(t+1), so the transform / barrier phases of one group fall into the tensor phases of
-// the other and the pipe always has a warp with DMMA work.  The X / JA stage of a tile is handed back by whichever
-// warp finishes with it last (a shared-memory counter): that warp issues the bulk copies of tile t + 2 -- no
-// dedicated producer, nobody waits.  Used for the configurations with split-k GEMM1 (D > 72).
-template <class C>
-struct PPCfg {
-  static constexpr int NG = 2;                // groups
-  static constexpr int GT = C::NT / NG;       // threads per group (128)
-  static constexpr int BQG = C::BQ / NG;      // virtual query rows per group
-  static constexpr int W1Q = C::W1Q / NG, W1M = C::W1M, W1K = C::W1K;  // GEMM1 warp grid inside a group
-  static constexpr int W2Q = C::W2Q / NG, W2D = C::W2D;                // GEMM2 warp grid inside a group
-  static_assert(C::W1K > 1 && C::W2S == 1 && C::W1Q % NG == 0 && C::W2Q % NG == 0, "split-k configurations only");
-  static_assert(W1Q * W1M * W1K == 4 && W2Q * W2D == 4, "4 warps per group");
-  static constexpr int TR1 = BQG / (8 * W1Q), TC1 = C::BM / (8 * W1M), KS1 = C::DP / 4 / W1K;
-  static constexpr int TR2 = BQG / (8 * W2Q), TD2 = C::DP / (8 * W2D);
-  static constexpr int EPT = BQG * C::BM / GT;
-  static_assert(TR1 * 8 * W1Q == BQG && TR2 * 8 * W2Q == BQG && (BQG * C::BM) % GT == 0, "group tiling");
-  // shared memory (doubles): Q | X[2] | JA[2] | mm[2] | xja[2] | ae[2] | P [NG][W1K][2][BQG*CS] | Cc [NG][2][BQG*CS] | qq | csum | E | bars | cnt
-  static constexpr int OFF_Q = 0;
-  static constexpr int OFF_X = OFF_Q + C::BQ * C::DS;
-  static constexpr int OFF_JA = OFF_X + 2 * C::BM * C::DS;
-  static constexpr int OFF_MM = OFF_JA + 2 * C::BM * C::DS;
-  static constexpr int OFF_XJA = OFF_MM + 2 * C::BM;
-  static constexpr int OFF_AE = OFF_XJA + 2 * C::BM;
-  static constexpr int OFF_P = OFF_AE + 2 * C::BM;
-  static constexpr int P_GROUP = W1K * 2 * BQG * C::CS;
-  static constexpr int OFF_C = OFF_P + NG * P_GROUP;
-  static constexpr int C_GROUP = 2 * BQG * C::CS;
-  static constexpr int OFF_QQ = OFF_C + NG * C_GROUP;
-  static constexpr int OFF_CSUM = OFF_QQ + C::BQ;
-  static constexpr int OFF_E = OFF_CSUM + C::BQ;
-  static constexpr int OFF_BAR = OFF_E + C::BQ;  // 3 x uint64 + 2 x int
-  static constexpr int SMEM_DOUBLES = OFF_BAR + 6;
-  static constexpr size_t SMEM_BYTES = (size_t)SMEM_DOUBLES * 8;
-  static_assert(SMEM_BYTES <= 232448, "exceeds 227 KB of shared memory");
-};
-
-__device__ __forceinline__ void group_barrier(int group) {
-  asm volatile("bar.sync %0, 128;" ::"r"(1 + group) : "memory");
-}
-
-template <class C>
-__global__ void __launch_bounds__(256, 1) k_predict_main_pp(const PredictArgs p) {
-  using G = PPCfg<C>;
-  extern __shared__ __align__(128) double smem[];
-  double* Qs = smem + G::OFF_Q;
-  double* Xs = smem + G::OFF_X;
-  double* JAs = smem + G::OFF_JA;
-  double* mms = smem + G::OFF_MM;
-  double* xjas = smem + G::OFF_XJA;
-  double* aes = smem + G::OFF_AE;
-  double* qq = smem + G::OFF_QQ;
-  double* csum_s = smem + G::OFF_CSUM;
-  double* E_s = smem + G::OFF_E;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + G::OFF_BAR);
-  int* cnt = reinterpret_cast<int*>(smem + G::OFF_BAR + 3);  // [2] stage hand-back counters
-
-  const int tid = threadIdx.x;
-  const int warp = tid >> 5, lane = tid & 31;
-  const int group = warp >> 2, wg = warp & 3, gtid = tid & (G::GT - 1);
-  const int lr = lane >> 2, lc = lane & 3;
-  const int64_t r0 = (int64_t)blockIdx.x * C::BQ;
-  const int t_begin = (int)blockIdx.y * p.tiles_per_split;
-  const int n_tiles = min(p.Mpad / C::BM, t_begin + p.tiles_per_split);
-  constexpr uint32_t STAGE_BYTES = (uint32_t)((2 * C::BM * C::DS + 3 * C::BM) * 8);
-  double* Ps = smem + G::OFF_P + group * G::P_GROUP;   // this group's split-k partials
-  double* C1s = smem + G::OFF_C + group * G::C_GROUP;  // this group's transformed coefficients
-  double* C2s = C1s + G::BQG * C::CS;
-  const int grow0 = group * G::BQG;                    // first row of this group inside the CTA's Q tile
-
-  if (tid == 0) {
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    mbar_init(&bars[2], 1);
-    cnt[0] = cnt[1] = 0;
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  auto issue_tile = [&](int t) {
-    const int s = (t - t_begin) & 1;
-    const int64_t m0 = (int64_t)t * C::BM;
-    mbar_arrive_expect_tx(&bars[s], STAGE_BYTES);
-    bulk_g2s(Xs + s * C::BM * C::DS, p.Xc + m0 * C::DS, C::BM * C::DS * 8, &bars[s]);
-    bulk_g2s(JAs + s * C::BM * C::DS, p.JA + m0 * C::DS, C::BM * C::DS * 8, &bars[s]);
-    bulk_g2s(mms + s * C::BM, p.mm + m0, C::BM * 8, &bars[s]);
-    bulk_g2s(xjas + s * C::BM, p.xja + m0, C::BM * 8, &bars[s]);
-    bulk_g2s(aes + s * C::BM, p.ae + m0, C::BM * 8, &bars[s]);
-  };
-  if (tid == 0) {
-    mbar_arrive_expect_tx(&bars[2], (uint32_t)((C::BQ * C::DS + C::BQ) * 8));
-    bulk_g2s(Qs, p.Qg + r0 * C::DS, C::BQ * C::DS * 8, &bars[2]);
-    bulk_g2s(qq, p.qqg + r0, C::BQ * 8, &bars[2]);
-    issue_tile(t_begin);
-    if (t_begin + 1 < n_tiles) issue_tile(t_begin + 1);
-  }
-  if (tid < C::BQ) {
-    csum_s[tid] = 0.0;
-    E_s[tid] = 0.0;
-  }
-  __syncthreads();
-  mbar_wait(&bars[2], 0);
-
-  // warp coordinates inside the group
-  const int w1k = wg % G::W1K;
-  const int w1m = (wg / G::W1K) % G::W1M;
-  const int w1q = wg / (G::W1K * G::W1M);
-  const int row1 = w1q * (G::TR1 * 8);
-  const int col1 = w1m * (G::TC1 * 8);
-  const int k1 = w1k * G::KS1 * 4;
-  const int w2d = wg % G::W2D;
-  const int w2q = wg / G::W2D;
-  const int row2 = w2q * (G::TR2 * 8);
-  const int dcol2 = w2d * (G::TD2 * 8);
-
-  double accG[G::TR2][G::TD2][2];
-#pragma unroll
-  for (int i = 0; i < G::TR2; ++i)
-#pragma unroll
-    for (int j = 0; j < G::TD2; ++j) accG[i][j][0] = accG[i][j][1] = 0.0;
-  double csum_part[G::EPT], E_part[G::EPT];
-#pragma unroll
-  for (int j = 0; j < G::EPT; ++j) csum_part[j] = E_part[j] = 0.0;
-
-  MaternK mk;
-  mk.sig = p.sig;
-  mk.sig_inv = 1.0 / p.sig;
-  mk.k_base = 5.0 / (3.0 * p.sig * p.sig * p.sig);
-  mk.k_c1 = mk.k_base * 5.0 / p.sig;
-
-  auto wait_full = [&](int t) { mbar_wait(&bars[(t - t_begin) & 1], (uint32_t)(((t - t_begin) >> 1) & 1)); };
-
-  // ---------------- GEMM1 of tile t: this warp's k-range of S1 = Q Xc^T, S2 = Q JA^T -> partials in Ps
-  auto gemm1 = [&](int t) {
-    const int s = (t - t_begin) & 1;
-    const double* Xt = Xs + s * C::BM * C::DS;
-    const double* JAt = JAs + s * C::BM * C::DS;
-    const int mvalid = min(C::BM, p.M - t * C::BM);
-    double a1[G::TR1][G::TC1][2], a2[G::TR1][G::TC1][2];
-#pragma unroll
-    for (int i = 0; i < G::TR1; ++i)
-#pragma unroll
-      for (int j = 0; j < G::TC1; ++j) a1[i][j][0] = a1[i][j][1] = a2[i][j][0] = a2[i][j][1] = 0.0;
-    const double* qa = Qs + (grow0 + row1 + lr) * C::DS + k1 + lc;
-    const double* xb = Xt + (col1 + lr) * C::DS + k1 + lc;
-    const double* jb = JAt + (col1 + lr) * C::DS + k1 + lc;
-#pragma unroll 2
-    for (int ks = 0; ks < G::KS1; ++ks) {
-      double fa[G::TR1], fx[G::TC1], fj[G::TC1];
-#pragma unroll
-      for (int i = 0; i < G::TR1; ++i) fa[i] = qa[i * 8 * C::DS + ks * 4];
-#pragma unroll
-      for (int j = 0; j < G::TC1; ++j) {
-        fx[j] = xb[j * 8 * C::DS + ks * 4];
-        fj[j] = jb[j * 8 * C::DS + ks * 4];
-      }
-#pragma unroll
-      for (int j = 0; j < G::TC1; ++j) {
-        if (col1 + j * 8 < mvalid) {  // warp-uniform
-#pragma unroll
-          for (int i = 0; i < G::TR1; ++i) {
-            dmma884(a1[i][j][0], a1[i][j][1], fa[i], fx[j]);
-            dmma884(a2[i][j][0], a2[i][j][1], fa[i], fj[j]);
-          }
-        }
-      }
-    }
-    double* P1 = Ps + (w1k * 2 + 0) * G::BQG * C::CS;
-    double* P2 = Ps + (w1k * 2 + 1) * G::BQG * C::CS;
-#pragma unroll
-    for (int i = 0; i < G::TR1; ++i)
-#pragma unroll
-      for (int j = 0; j < G::TC1; ++j) {
-        const int off = (row1 + i * 8 + lr) * C::CS + col1 + j * 8 + 2 * lc;
-        *reinterpret_cast<double2*>(P1 + off) = make_double2(a1[i][j][0], a1[i][j][1]);
-        *reinterpret_cast<double2*>(P2 + off) = make_double2(a2[i][j][0], a2[i][j][1]);
-      }
-  };
-
-  // ---------------- split-k sum + Matern transform of tile t: Ps -> C1s, C2s
-  auto transform = [&](int t) {
-    const int s = (t - t_begin) & 1;
-    const double* mmt = mms + s * C::BM;
-    const double* xjat = xjas + s * C::BM;
-    const double* aet = aes + s * C::BM;
-#pragma unroll
-    for (int j = 0; j < G::EPT; ++j) {
-      const int e = gtid + j * G::GT;
-      const int r = e / C::BM, mc = e % C::BM;
-      const int off = r * C::CS + mc;
-      double s1 = Ps[off], s2 = Ps[G::BQG * C::CS + off];
-#pragma unroll
-      for (int wk = 1; wk < G::W1K; ++wk) {
-        s1 += Ps[(wk * 2 + 0) * G::BQG * C::CS + off];
-        s2 += Ps[(wk * 2 + 1) * G::BQG * C::CS + off];
-      }
-      const double a = s2 - xjat[mc];
-      double c1, c2;
-      if (p.use_ae) {
-        E_part[j] += matern52_ecstr(fma(-10.0, s1, 5.0 * (qq[grow0 + r] + mmt[mc])), a, aet[mc], mk, c1, c2);
-      } else {
-        matern52(fma(-10.0, s1, 5.0 * (qq[grow0 + r] + mmt[mc])), a, mk, c1, c2);
-        E_part[j] = fma(a, c2, E_part[j]);
-      }
-      if (mc >= p.M - t * C::BM) c1 = c2 = 0.0;  // zero-padded training points of the last tile (C is read unmasked)
-      csum_part[j] += c1;
-      C1s[off] = c1;
-      C2s[off] = c2;
-    }
-  };
-
-  // ---------------- GEMM2 of tile t: accG += C1 Xc + C2 JA, then hand the stage back
-  auto gemm2 = [&](int t) {
-    const int s = (t - t_begin) & 1;
-    const double* Xt = Xs + s * C::BM * C::DS;
-    const double* JAt = JAs + s * C::BM * C::DS;
-    const int mvalid = min(C::BM, p.M - t * C::BM);
-    const double* c1a = C1s + (row2 + lr) * C::CS + lc;
-    const double* c2a = C2s + (row2 + lr) * C::CS + lc;
-    const double* xb = Xt + lc * C::DS + dcol2 + lr;
-    const double* jb = JAt + lc * C::DS + dcol2 + lr;
-    const int ks_end = (mvalid + 3) >> 2;
-#pragma unroll 2
-    for (int ks = 0; ks < ks_end; ++ks) {
-      double f1[G::TR2], f2[G::TR2], fx[G::TD2], fj[G::TD2];
-#pragma unroll
-      for (int i = 0; i < G::TR2; ++i) {
-        f1[i] = c1a[i * 8 * C::CS + ks * 4];
-        f2[i] = c2a[i * 8 * C::CS + ks * 4];
-      }
-#pragma unroll
-      for (int j = 0; j < G::TD2; ++j) {
-        fx[j] = xb[ks * 4 * C::DS + j * 8];
-        fj[j] = jb[ks * 4 * C::DS + j * 8];
-      }
-#pragma unroll
-      for (int i = 0; i < G::TR2; ++i)
-#pragma unroll
-        for (int j = 0; j < G::TD2; ++j) {
-          dmma884(accG[i][j][0], accG[i][j][1], f1[i], fx[j]);
-          dmma884(accG[i][j][0], accG[i][j][1], f2[i], fj[j]);
-        }
-    }
-    // the last of the 8 warps to finish with this stage refills it with tile t + 2
-    __syncwarp();
-    if (lane == 0) {
-      const int old = atomicAdd(&cnt[s], 1);
-      if (old == 7) {
-        atomicExch(&cnt[s], 0);
-        if (t + 2 < n_tiles) issue_tile(t + 2);
-      }
-    }
-  };
-
-  if (group == 0) {
-    for (int t = t_begin; t < n_tiles; ++t) {
-      wait_full(t);
-      gemm1(t);
-      group_barrier(group);
-      transform(t);
-      group_barrier(group);
-      gemm2(t);
-    }
-  } else {
-    if (t_begin < n_tiles) {
-      wait_full(t_begin);
-      gemm1(t_begin);
-      group_barrier(group);
-      transform(t_begin);
-      group_barrier(group);
-    }
-    for (int t = t_begin; t < n_tiles; ++t) {
-      gemm2(t);
-      if (t + 1 < n_tiles) {
-        wait_full(t + 1);
-        gemm1(t + 1);
-        group_barrier(group);
-        transform(t + 1);
-        group_barrier(group);
-      }
-    }
-  }
-
-  // ---- row sums csum[r] = sum_m c1, E[r] = sum_m a c2 (fixed order: shuffles inside the BM-lane segments)
-#pragma unroll
-  for (int j = 0; j < G::EPT; ++j) {
-    double cs = csum_part[j], es = E_part[j];
-#pragma unroll
-    for (int o = C::BM / 2; o > 0; o >>= 1) {
-      cs += __shfl_xor_sync(0xffffffffu, cs, o);
-      es += __shfl_xor_sync(0xffffffffu, es, o);
-    }
-    const int e = gtid + j * G::GT;
-    if (e % C::BM == 0) {
-      csum_s[grow0 + e / C::BM] = cs;
-      E_s[grow0 + e / C::BM] = es;
-    }
-  }
-  group_barrier(group);
-
-  // ---- G = (sum_m c1) Q - (C1 Xc + C2 JA)
-#pragma unroll
-  for (int i = 0; i < G::TR2; ++i) {
-    const int r = grow0 + row2 + i * 8 + lr;
-    const int64_t row = r0 + r;
-    if (row < p.n_rows) {
-      const double cs = csum_s[r];
-#pragma unroll
-      for (int j = 0; j < G::TD2; ++j) {
-        const int col = dcol2 + j * 8 + 2 * lc;
-        const double g0 = cs * Qs[r * C::DS + col] - accG[i][j][0];
-        const double g1 = cs * Qs[r * C::DS + col + 1] - accG[i][j][1];
-        *reinterpret_cast<double2*>(p.G + ((int64_t)blockIdx.y * p.n_rows_pad + row) * C::DP + col) = make_double2(g0, g1);
-      }
-    }
-  }
-  if (gtid < G::BQG && r0 + grow0 + gtid < p.n_rows)
-    p.Erow[(int64_t)blockIdx.y * p.n_rows_pad + r0 + grow0 + gtid] = E_s[grow0 + gtid];
-}
-
 // ============================================================== query rows
 // One warp per virtual row (b, p): Qg[row][e] = x_b[pinv_p[e]] - mu[e] (zero beyond D and beyond the
 // last real row, so that every main-kernel tile is one contiguous bulk copy) and qq[row] = |Qg[row]|^2.
@@ -1263,50 +935,26 @@ struct sgdml_b200_model {
 
 namespace {
 
-// tile configurations: <DP, BQ, BM, W1Q, W1M, W1K, W2Q, W2D>
-// D <= 40: two co-resident CTAs per SM so that one CTA's transform / barriers / prologue overlap
-// the other's DMMA phases (the sweep over M is only a handful of tiles at ethanol size)
+// tile configurations: <DP, BQ, BM, W1Q, W1M, W1K, W2Q, W2D, MINB, W2S, OB>, the fastest per size when the
+// alternatives were timed (65536 queries, M = 1000, S = 6; not re-timed on H100)
+// D <= 40: two co-resident CTAs per SM so that one CTA's transform / barriers / prologue overlap the other's DMMA
+// phases (the sweep over M is only a handful of tiles at ethanol size); the doubled C1 / C2 buffers of the
+// one-barrier form would cost it the second CTA
+// 40 < D <= 224: no split over k -- every warp owns whole S1 / S2 fragments, the Matern transform runs on the
+// accumulator registers, and one CTA-wide barrier per tile (OB)
+// 224 < D <= 256: split-k GEMM1
 using Cfg40 = PCfg<40, 64, 32, 4, 2, 1, 4, 1, 2, 2>;
-using Cfg72 = PCfg<72, 64, 32, 4, 2, 1, 8, 1>;
-using Cfg112 = PCfg<112, 64, 16, 4, 1, 2, 4, 2>;
-using Cfg160 = PCfg<160, 32, 16, 2, 1, 4, 2, 4>;
-using Cfg224 = PCfg<224, 32, 16, 2, 1, 4, 2, 4>;
-using Cfg256 = PCfg<256, 32, 8, 2, 1, 4, 2, 4>;
-// variant 2: the same tiles without the split over k -- every warp owns whole S1 / S2 fragments, the Matern transform
-// runs on the accumulator registers and one of the three barriers per tile (and the partial-sum round trip through
-// shared memory) goes away; the price is three operand loads per two DMMAs in GEMM1
-using Cfg112f = PCfg<112, 64, 16, 4, 2, 1, 4, 2>;
-using Cfg160f = PCfg<160, 32, 16, 4, 2, 1, 2, 4>;
-using Cfg224f = PCfg<224, 32, 16, 4, 2, 1, 2, 4>;
-// variant 3: variant 2 with one barrier per tile (OB), for every descriptor size up to 224
-using Cfg40o = PCfg<40, 64, 32, 4, 2, 1, 4, 1, 2, 2, 1>;
 using Cfg72o = PCfg<72, 64, 32, 4, 2, 1, 8, 1, 1, 1, 1>;
 using Cfg112o = PCfg<112, 64, 16, 4, 2, 1, 4, 2, 1, 1, 1>;
 using Cfg160o = PCfg<160, 32, 16, 4, 2, 1, 2, 4, 1, 1, 1>;
 using Cfg224o = PCfg<224, 32, 16, 4, 2, 1, 2, 4, 1, 1, 1>;
-// variant 5 (DP = 40 only): the one-barrier form on 16-point tiles, which keeps two CTAs per SM (88 KB)
-using Cfg40o16 = PCfg<40, 64, 16, 4, 2, 1, 4, 1, 2, 2, 1>;
+using Cfg256 = PCfg<256, 32, 8, 2, 1, 4, 2, 4>;
 
 struct CfgInfo {
   int DP, BQ, BM;
 };
 const CfgInfo kCfgs[] = {{40, 64, 32}, {72, 64, 32}, {112, 64, 16}, {160, 32, 16}, {224, 32, 16}, {256, 32, 8}};
 const int kNumCfgs = 6;
-
-template <class C>
-int launch_main_pp_t(const PredictArgs& a, int n_splits, cudaStream_t s) {
-  static bool configured[64] = {false};
-  int dev = 0;
-  SG_CUDA(cudaGetDevice(&dev));
-  if (dev >= 0 && dev < 64 && !configured[dev]) {
-    SG_CUDA(cudaFuncSetAttribute(k_predict_main_pp<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PPCfg<C>::SMEM_BYTES));
-    configured[dev] = true;
-  }
-  const int64_t grid = (a.n_rows + C::BQ - 1) / C::BQ;
-  k_predict_main_pp<C><<<dim3((unsigned)grid, (unsigned)n_splits), C::NT, PPCfg<C>::SMEM_BYTES, s>>>(a);
-  SG_CUDA(cudaGetLastError());
-  return 0;
-}
 
 template <class C>
 int launch_main_t(const PredictArgs& a, int n_splits, cudaStream_t s) {
@@ -1318,58 +966,19 @@ int launch_main_t(const PredictArgs& a, int n_splits, cudaStream_t s) {
     configured[dev] = true;
   }
   const int64_t grid = (a.n_rows + C::BQ - 1) / C::BQ;
-  PredictArgs b = a;
-  if (a.bm > C::BM) b.tiles_per_split = a.tiles_per_split * (a.bm / C::BM);  // (a.bm is a multiple of C::BM)
-  k_predict_main<C><<<dim3((unsigned)grid, (unsigned)n_splits), C::NT, C::SMEM_BYTES, s>>>(b);
+  k_predict_main<C><<<dim3((unsigned)grid, (unsigned)n_splits), C::NT, C::SMEM_BYTES, s>>>(a);
   SG_CUDA(cudaGetLastError());
   return 0;
 }
 
-int g_predict_variant = 0;  // see sgdml_b200_set_predict_variant (include/sgdml_b200.h)
-
+// cfg indexes kCfgs; each case's tiles must match its entry there
 int launch_main(int cfg, const PredictArgs& a, int n_splits, cudaStream_t s) {
-  if (g_predict_variant == 1) {
-    switch (cfg) {
-      case 2: return launch_main_pp_t<Cfg112>(a, n_splits, s);
-      case 3: return launch_main_pp_t<Cfg160>(a, n_splits, s);
-      case 4: return launch_main_pp_t<Cfg224>(a, n_splits, s);
-      case 5: return launch_main_pp_t<Cfg256>(a, n_splits, s);
-    }
-  }
-  if (g_predict_variant == 2) {
-    switch (cfg) {
-      case 2: return launch_main_t<Cfg112f>(a, n_splits, s);
-      case 3: return launch_main_t<Cfg160f>(a, n_splits, s);
-      case 4: return launch_main_t<Cfg224f>(a, n_splits, s);
-    }
-  }
-  if (g_predict_variant == 3) {
-    switch (cfg) {
-      case 0: return launch_main_t<Cfg40o>(a, n_splits, s);
-      case 1: return launch_main_t<Cfg72o>(a, n_splits, s);
-      case 2: return launch_main_t<Cfg112o>(a, n_splits, s);
-      case 3: return launch_main_t<Cfg160o>(a, n_splits, s);
-      case 4: return launch_main_t<Cfg224o>(a, n_splits, s);
-    }
-  }
-  if (g_predict_variant == 5 && cfg == 0) return launch_main_t<Cfg40o16>(a, n_splits, s);
-  if (g_predict_variant == 0) {
-    // default: the fastest kernel per size when the variants were timed (tools/predict_variants.py, 65536 queries,
-    // M = 1000, S = 6): the one-barrier kernel for DP >= 72; DP = 40 (config 1) stays on the round-1 kernel (the
-    // doubled C1 / C2 buffers cost the one-barrier form its second CTA per SM).  Not re-timed on H100.
-    switch (cfg) {
-      case 1: return launch_main_t<Cfg72o>(a, n_splits, s);
-      case 2: return launch_main_t<Cfg112o>(a, n_splits, s);
-      case 3: return launch_main_t<Cfg160o>(a, n_splits, s);
-      case 4: return launch_main_t<Cfg224o>(a, n_splits, s);
-    }
-  }
-  switch (cfg) {  // (variant 4: the round-1 kernels for every size)
+  switch (cfg) {
     case 0: return launch_main_t<Cfg40>(a, n_splits, s);
-    case 1: return launch_main_t<Cfg72>(a, n_splits, s);
-    case 2: return launch_main_t<Cfg112>(a, n_splits, s);
-    case 3: return launch_main_t<Cfg160>(a, n_splits, s);
-    case 4: return launch_main_t<Cfg224>(a, n_splits, s);
+    case 1: return launch_main_t<Cfg72o>(a, n_splits, s);
+    case 2: return launch_main_t<Cfg112o>(a, n_splits, s);
+    case 3: return launch_main_t<Cfg160o>(a, n_splits, s);
+    case 4: return launch_main_t<Cfg224o>(a, n_splits, s);
     case 5: return launch_main_t<Cfg256>(a, n_splits, s);
   }
   return fail_arg("no predictor tile configuration for this descriptor size");
@@ -1583,7 +1192,6 @@ int run_queries(sgdml_b200_model* m, int slot, const double* xq, const double* g
     a.qqg = w.qq;
     a.n_rows = n_rows;
     a.n_rows_pad = n_rows_pad;
-    a.bm = m->BM;
     a.G = w.G;
     a.Erow = w.Erow;
     // small batches: split the sweep over the training points across CTAs so that the grid fills the
@@ -2090,12 +1698,6 @@ int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* m, int slices, voi
     free_oz(m->ozXcT);
     free_oz(m->ozJAT);
   }
-  return 0;
-}
-
-int sgdml_b200_set_predict_variant(int variant) {
-  SG_ARG(variant >= 0 && variant <= 5);
-  g_predict_variant = variant;
   return 0;
 }
 

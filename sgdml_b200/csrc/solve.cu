@@ -467,9 +467,8 @@ static int launch_gemm_tma(const GemmArgs& a, cudaStream_t s) {
 }
 
 using GBig = GCfg<128, 128, 2, 4, 32, 3>;   // 196 KB smem, 1 CTA/SM
-using GTall = GCfg<128, 64, 4, 2, 16, 4>;   // 98 KB smem, 2 CTAs/SM
 
-static int g_gemm_variant = 3;  // 0: 128x128 cp.async, 1: 128x64 cp.async (2 CTAs/SM), 2: scalar, 3: 128x128 TMA (default)
+static int g_gemm_variant = 3;  // 0: 128x128 cp.async, 2: scalar, 3: 128x128 TMA (default)
 
 template <class G>
 static int launch_gemm_t(const GemmArgs& a, cudaStream_t s) {
@@ -511,7 +510,6 @@ int launch_gemm(const GemmArgs& a, cudaStream_t s) {
     count_launch(KID_GEMM);
     return 0;
   }
-  if (g_gemm_variant == 1) return launch_gemm_t<GTall>(a, s);
   if (g_gemm_variant == 3 && tmap_encoder() != nullptr) return launch_gemm_tma(a, s);  // else: cp.async tiles
   return launch_gemm_t<GBig>(a, s);
 }
@@ -846,12 +844,6 @@ __global__ void __launch_bounds__(256) k_dmma_peak(double* out, int iters, doubl
 // more math.
 constexpr int NBO_MAX = 1024;
 
-// Look-ahead: the lazy update of outer block `ob` is split into (a) the next outer block's columns,
-// issued on the caller's stream, and (b) everything to the right of them, issued on a lower-priority
-// side stream.  The latency-bound panel work of block ob+1 (potf2 tiles, substitution strips, small
-// GEMMs) then runs concurrently with (b) instead of leaving the GPU to one CTA at a time.
-// Dependencies: inner(ob+1) needs a(ob); a(ob+1) and b(ob+1) need b(ob) (same tiles, += updates);
-// b(ob) reads the -X workspace of block ob, so the workspace is double buffered.
 // Slice count of the lazy trailing updates (csrc/ozaki.cu): -1 = automatic, 0 = FP64 DMMA, 2..7 = int8 slices on the
 // wgmma tensor cores.  Automatic: SGDML_B200_OZAKI_SLICES if set, otherwise FP64.  Measured on an H100 SXM at a 400 W
 // power limit (BASELINE config 2, n = 63 000): solve 3.46 s with FP64 DMMA trailing updates, 3.65 s with 7 int8 slices
@@ -866,153 +858,90 @@ static int resolve_slices() {
 
 int potrf_device(double* A, int64_t n, int64_t lda, int* info_host, cudaStream_t s, bool analytic_solver) {
   int* d_info = nullptr;
-  double* W[2] = {nullptr, nullptr};
-  cudaStream_t s2 = nullptr;
-  cudaEvent_t evI[2] = {nullptr, nullptr}, evB[2] = {nullptr, nullptr};
+  double* W = nullptr;  // -X of the current outer block (the device buffers are persistent workspaces: csrc/core.cu ws_get)
   // outer block: wide for large matrices (fewer passes over C), narrower when n is small
   const int NBO = (n >= 16384) ? NBO_MAX : ((n >= 4096) ? 512 : 256);
-  // Measured slower with look-ahead than without -- the 1-CTA-per-SM GEMM leaves no room for the panel kernels to
-  // co-run, so the split only costs GEMM efficiency.  Kept behind an
-  // environment switch (SGDML_B200_LOOKAHEAD=1) until the trailing GEMM is made persistent on a subset of SMs.
-  const char* la = getenv("SGDML_B200_LOOKAHEAD");
-  const bool lookahead = (la && la[0] == '1') && (n > 2 * (int64_t)NBO) && !profiling_enabled();
   const int oz_slices = resolve_slices();
   int8_t* oz_planes = nullptr;  // slice planes of the current outer panel (int8 path)
   int* oz_exps = nullptr;
-  auto cleanup = [&]() {  // (the device buffers are persistent workspaces: csrc/core.cu ws_get)
-    if (s2) cudaStreamDestroy(s2);
-    for (int i = 0; i < 2; ++i) {
-      if (evI[i]) cudaEventDestroy(evI[i]);
-      if (evB[i]) cudaEventDestroy(evB[i]);
-    }
-  };
-  auto body = [&]() -> int {
-    SG_TRY(ws_get(WS_POTRF_INFO, sizeof(int), (void**)&d_info));
-    SG_TRY(ws_get(WS_POTRF_W0, sizeof(double) * (size_t)n * NBO, (void**)&W[0]));
-    if (oz_slices > 0 && !lookahead) {
-      size_t pb = 0, eb = 0;
-      SG_TRY(ozaki_syrk_workspace_bytes(n, NBO, oz_slices, &pb, &eb));
-      SG_TRY(ws_get(WS_OZ_PLANES, pb, (void**)&oz_planes));
-      SG_TRY(ws_get(WS_OZ_EXPS, eb, (void**)&oz_exps));
-    }
-    if (lookahead) {
-      SG_TRY(ws_get(WS_POTRF_W1, sizeof(double) * (size_t)n * NBO, (void**)&W[1]));
-      int lo = 0, hi = 0;
-      SG_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));  // lo = least priority
-      SG_CUDA(cudaStreamCreateWithPriority(&s2, cudaStreamNonBlocking, lo));
-      for (int i = 0; i < 2; ++i) {
-        SG_CUDA(cudaEventCreateWithFlags(&evI[i], cudaEventDisableTiming));
-        SG_CUDA(cudaEventCreateWithFlags(&evB[i], cudaEventDisableTiming));
+  SG_TRY(ws_get(WS_POTRF_INFO, sizeof(int), (void**)&d_info));
+  SG_TRY(ws_get(WS_POTRF_W, sizeof(double) * (size_t)n * NBO, (void**)&W));
+  if (oz_slices > 0) {
+    size_t pb = 0, eb = 0;
+    SG_TRY(ozaki_syrk_workspace_bytes(n, NBO, oz_slices, &pb, &eb));
+    SG_TRY(ws_get(WS_OZ_PLANES, pb, (void**)&oz_planes));
+    SG_TRY(ws_get(WS_OZ_EXPS, eb, (void**)&oz_exps));
+  }
+  SG_CUDA(cudaMemsetAsync(d_info, 0, sizeof(int), s));
+  const size_t trsm_smem = sizeof(double) * (NB + RS) * (NB + 4);
+  SG_CUDA(cudaFuncSetAttribute(k_trsm_strip, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_smem));
+  for (int64_t K0 = 0; K0 < n; K0 += NBO) {
+    const int64_t K1 = std::min<int64_t>(K0 + NBO, n);  // end of the outer block
+    for (int64_t k0 = K0; k0 < K1; k0 += NB) {
+      const int kb = (int)std::min<int64_t>(NB, n - k0);
+      {
+        ProfScope ps(KID_POTF2, s);
+        k_potf2_tile<<<1, 1024, 0, s>>>(A + k0 * lda + k0, lda, kb, k0, d_info);
+        SG_CUDA(cudaGetLastError());
+        count_launch(KID_POTF2);
       }
-    }
-    SG_CUDA(cudaMemsetAsync(d_info, 0, sizeof(int), s));
-    const size_t trsm_smem = sizeof(double) * (NB + RS) * (NB + 4);
-    SG_CUDA(cudaFuncSetAttribute(k_trsm_strip, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_smem));
-    int ob = 0;
-    int last_b = -1;
-    for (int64_t K0 = 0; K0 < n; K0 += NBO, ++ob) {
-      double* Wc = W[lookahead ? (ob & 1) : 0];
-      const int64_t K1 = std::min<int64_t>(K0 + NBO, n);  // end of the outer block
-      for (int64_t k0 = K0; k0 < K1; k0 += NB) {
-        const int kb = (int)std::min<int64_t>(NB, n - k0);
-        {
-          ProfScope ps(KID_POTF2, s);
-          k_potf2_tile<<<1, 1024, 0, s>>>(A + k0 * lda + k0, lda, kb, k0, d_info);
-          SG_CUDA(cudaGetLastError());
-          count_launch(KID_POTF2);
-        }
-        const int64_t rem = n - k0 - kb;
-        if (rem <= 0) break;
-        {
-          ProfScope ps(KID_TRSM, s);
-          k_trsm_strip<<<(unsigned)((rem + RS - 1) / RS), 256, trsm_smem, s>>>(
-              A + k0 * lda + k0, lda, kb, A + (k0 + kb) * lda + k0, lda, rem, Wc + (k0 + kb) * NBO + (k0 - K0), NBO,
-              d_info);
-          SG_CUDA(cudaGetLastError());
-          count_launch(KID_TRSM);
-        }
-        const int64_t cols_in = K1 - (k0 + kb);  // columns of the outer block still to be factorised
-        if (cols_in > 0) {
-          GemmArgs g;
-          g.m = rem;
-          g.n = cols_in;
-          g.k = kb;
-          g.A = Wc + (k0 + kb) * NBO + (k0 - K0);  // -X
-          g.lda = NBO;
-          g.B = A + (k0 + kb) * lda + k0;  // X rows of the outer block
-          g.ldb = lda;
-          g.C = A + (k0 + kb) * lda + (k0 + kb);
-          g.ldc = lda;
-          g.alpha = 1.0;
-          g.beta = 1.0;
-          g.mode = 1;
-          g.tri = 0;
-          g.abort_flag = d_info;
-          SG_TRY(launch_gemm(g, s));
-        }
-      }
-      const int64_t rem = n - K1;
+      const int64_t rem = n - k0 - kb;
       if (rem <= 0) break;
-      GemmArgs g;
-      g.k = K1 - K0;
-      g.lda = NBO;
-      g.ldb = lda;
-      g.ldc = lda;
-      g.alpha = 1.0;
-      g.beta = 1.0;
-      g.mode = 1;
-      g.abort_flag = d_info;
-      if (!lookahead) {
-        if (oz_slices > 0) {
-          // the trailing update on the int8 tensor cores (csrc/ozaki.cu), C -= X X^T through exact int8 slice products
-          const double* X = A + K1 * lda + K0;
-          SG_TRY(ozaki_syrk_device(rem, K1 - K0, -1.0, X, lda, A + K1 * lda + K1, lda, oz_slices, oz_planes, oz_exps, s));
-          continue;
-        }
-        g.m = rem;
-        g.n = rem;
-        g.A = Wc + K1 * NBO;  // -X, all panels of the outer block
-        g.B = A + K1 * lda + K0;
-        g.C = A + K1 * lda + K1;
-        g.tri = 1;
-        SG_TRY(launch_gemm(g, s));
-        continue;
+      {
+        ProfScope ps(KID_TRSM, s);
+        k_trsm_strip<<<(unsigned)((rem + RS - 1) / RS), 256, trsm_smem, s>>>(
+            A + k0 * lda + k0, lda, kb, A + (k0 + kb) * lda + k0, lda, rem, W + (k0 + kb) * NBO + (k0 - K0), NBO, d_info);
+        SG_CUDA(cudaGetLastError());
+        count_launch(KID_TRSM);
       }
-      const int64_t K2 = std::min<int64_t>(K1 + NBO, n);
-      SG_CUDA(cudaEventRecord(evI[ob & 1], s));  // panels of this block are final
-      if (last_b >= 0) SG_CUDA(cudaStreamWaitEvent(s, evB[last_b & 1], 0));
-      // (a) columns of the next outer block, all rows below
-      g.m = rem;
-      g.n = K2 - K1;
-      g.A = Wc + K1 * NBO;
-      g.B = A + K1 * lda + K0;
-      g.C = A + K1 * lda + K1;
-      g.tri = 0;
-      SG_TRY(launch_gemm(g, s));
-      // (b) the rest of the trailing matrix, lower triangle, on the side stream
-      const int64_t rem2 = n - K2;
-      if (rem2 > 0) {
-        SG_CUDA(cudaStreamWaitEvent(s2, evI[ob & 1], 0));
-        g.m = rem2;
-        g.n = rem2;
-        g.A = Wc + K2 * NBO;
-        g.B = A + K2 * lda + K0;
-        g.C = A + K2 * lda + K2;
-        g.tri = 1;
-        SG_TRY(launch_gemm(g, s2));
-        SG_CUDA(cudaEventRecord(evB[ob & 1], s2));
-        last_b = ob;
+      const int64_t cols_in = K1 - (k0 + kb);  // columns of the outer block still to be factorised
+      if (cols_in > 0) {
+        GemmArgs g;
+        g.m = rem;
+        g.n = cols_in;
+        g.k = kb;
+        g.A = W + (k0 + kb) * NBO + (k0 - K0);  // -X
+        g.lda = NBO;
+        g.B = A + (k0 + kb) * lda + k0;  // X rows of the outer block
+        g.ldb = lda;
+        g.C = A + (k0 + kb) * lda + (k0 + kb);
+        g.ldc = lda;
+        g.alpha = 1.0;
+        g.beta = 1.0;
+        g.mode = 1;
+        g.tri = 0;
+        g.abort_flag = d_info;
+        SG_TRY(launch_gemm(g, s));
       }
     }
-    if (lookahead && last_b >= 0) SG_CUDA(cudaStreamWaitEvent(s, evB[last_b & 1], 0));
-    SG_CUDA(cudaMemcpyAsync(info_host, d_info, sizeof(int), cudaMemcpyDeviceToHost, s));
-    SG_CUDA(cudaStreamSynchronize(s));
-    if (s2) SG_CUDA(cudaStreamSynchronize(s2));
-    return 0;
-  };
-  int rc = body();
-  cleanup();
-  return rc;
+    const int64_t rem = n - K1;
+    if (rem <= 0) break;
+    if (oz_slices > 0) {
+      // the trailing update on the int8 tensor cores (csrc/ozaki.cu), C -= X X^T through exact int8 slice products
+      const double* X = A + K1 * lda + K0;
+      SG_TRY(ozaki_syrk_device(rem, K1 - K0, -1.0, X, lda, A + K1 * lda + K1, lda, oz_slices, oz_planes, oz_exps, s));
+      continue;
+    }
+    GemmArgs g;
+    g.m = rem;
+    g.n = rem;
+    g.k = K1 - K0;
+    g.A = W + K1 * NBO;  // -X, all panels of the outer block
+    g.lda = NBO;
+    g.B = A + K1 * lda + K0;
+    g.ldb = lda;
+    g.C = A + K1 * lda + K1;
+    g.ldc = lda;
+    g.alpha = 1.0;
+    g.beta = 1.0;
+    g.mode = 1;
+    g.tri = 1;
+    g.abort_flag = d_info;
+    SG_TRY(launch_gemm(g, s));
+  }
+  SG_CUDA(cudaMemcpyAsync(info_host, d_info, sizeof(int), cudaMemcpyDeviceToHost, s));
+  SG_CUDA(cudaStreamSynchronize(s));
+  return 0;
 }
 
 int potrs_device(const double* L, int64_t n, int64_t lda, double* B, int64_t nrhs, int64_t ldb, cudaStream_t s) {
@@ -1268,7 +1197,6 @@ int sgdml_b200_fp64_peak_tflops_sustained(double seconds, double* tflops) {
   return 0;
 }
 
-// test / tuning hook: 0 = 128x128 tiles, 1 = 128x64 tiles, 2 = naive kernel
 int sgdml_b200_set_solve_slices(int n_slices) {
   SG_ARG(n_slices == -1 || n_slices == 0 || (n_slices >= 2 && n_slices <= 7));
   g_solve_slices = n_slices;
@@ -1278,6 +1206,7 @@ int sgdml_b200_set_solve_slices(int n_slices) {
 int sgdml_b200_get_solve_slices(void) { return resolve_slices(); }
 
 int sgdml_b200_set_gemm_variant(int v) {
+  SG_ARG(v == 0 || v == 2 || v == 3);
   g_gemm_variant = v;
   return 0;
 }

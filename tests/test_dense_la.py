@@ -256,20 +256,6 @@ def test_potrf(lib, n, pad, slices, monkeypatch):
         assert _bits_equal(h[:, :n][low], out[:, :n][low])
 
 
-def test_potrf_lookahead(lib, monkeypatch):
-    """SGDML_B200_LOOKAHEAD=1 (DESIGN section 6): the lazy update split over two streams, n = 5000 (NBO = 512,
-    ten outer blocks), padded lda."""
-    monkeypatch.setenv('SGDML_B200_LOOKAHEAD', '1')
-    monkeypatch.setenv('SGDML_B200_OZAKI_SLICES', '0')
-    n = 5000
-    A, Ac, _ = _potrf_inputs(n, n + 2)
-    Ad = _dev(Ac)
-    _check(lib.sgdml_b200_potrf(Ad.data_ptr(), n, n + 2, _stream()), 'potrf')
-    out = _host(Ad)
-    lc.check_padding_unchanged(Ac, out, n, 'A')
-    lc.check_cholesky(A, out[:, :n], forward_tol=1e-12)
-
-
 def test_potrf_sgdml_system(lib):
     """The matrix the analytic solver factorises, -K + lam I of a golden task (condition ~1e11), assembled by the
     engine into a padded buffer (odd n + 1 row stride): backward error against LAPACK's on the same matrix."""

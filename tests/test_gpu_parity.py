@@ -128,6 +128,9 @@ def test_predict_vs_oracle_shapes(eng, N, M, rot, swap, sig):
     E, F = p.predict(Rq)
     assert rel_err(F, F_ref) < 1e-10
     assert rel_err(E, E_ref) < 1e-10
+    E1, F1 = p.predict(Rq[:1])  # one geometry: the sweep over the training points split across CTAs
+    assert rel_err(F1, F_ref[:1]) < 1e-10
+    assert rel_err(E1, E_ref[:1]) < 1e-10
 
 
 def test_predict_torch_device_tensors(eng):
@@ -270,7 +273,7 @@ def test_assemble_large_kernel_matches_small(eng, golden):
     t = eng.GDMLTrain()
     args = (golden['R_desc'], golden['R_d_desc'], golden['tril_perms_lin'], int(golden['sig']), Desc(N))
     cols = np.unique(np.random.default_rng(1).integers(0, n, size=31))
-    K_default_cols = t._assemble_kernel_mat(*args, col_idxs=cols)  # default small-molecule kernel (k_assemble_v3 here)
+    K_default_cols = t._assemble_kernel_mat(*args, col_idxs=cols)  # default small-molecule kernel (k_assemble_v4 here)
     _lib.lib().sgdml_b200_set_assemble_variant(2)  # the per-permutation kernel whose summation order the large one keeps
     try:
         K_small_full = t._assemble_kernel_mat(*args)
@@ -447,6 +450,15 @@ def test_n100_reference_fixture(eng):
 
 
 # --------------------------------------------------------------------------- dense solve
+_ERR_ARG = -1000  # SGDML_B200_ERR_ARG (include/sgdml_b200.h)
+
+
+def _set_gemm_variant(L, variant):
+    """GEMM kernel hook: 0 cp.async tiles, 2 scalar kernel, 3 TMA tiles (default).  Variant 1 selected 128x64 tiles,
+    which are removed: the hook rejects it and keeps the kernel selected before, so such a case runs the default."""
+    assert L.sgdml_b200_set_gemm_variant(variant) == (_ERR_ARG if variant == 1 else 0)
+
+
 @pytest.mark.parametrize('variant', [0, 1, 2, 3])
 @pytest.mark.parametrize('m,n,k', [(128, 128, 128), (300, 200, 64), (257, 129, 130), (64, 1000, 16), (33, 17, 7)])
 def test_dgemm_nt(eng, variant, m, n, k):
@@ -458,7 +470,7 @@ def test_dgemm_nt(eng, variant, m, n, k):
     B = rng.standard_normal((n, k))
     C = rng.standard_normal((m, n))
     ref = 0.75 * A @ B.T - 1.25 * C
-    L.sgdml_b200_set_gemm_variant(variant)
+    _set_gemm_variant(L, variant)
     try:
         _lib.check(L.sgdml_b200_dgemm_nt(m, n, k, 0.75, _lib.ptr(A), k, _lib.ptr(B), k, -1.25, _lib.ptr(C), n, None), 'dgemm')
     finally:
@@ -494,7 +506,7 @@ def test_dgemm_nt_device_layouts(eng, variant, m, n, k, layout):
     Cd = torch.full((m, ldc), nan, dtype=torch.float64, device='cuda')
     if layout != 'beta0_nan':
         Cd[:, :n] = torch.from_numpy(C).cuda()
-    L.sgdml_b200_set_gemm_variant(variant)
+    _set_gemm_variant(L, variant)
     try:
         _lib.check(
             L.sgdml_b200_dgemm_nt(
@@ -522,7 +534,7 @@ def test_potrf_potrs(eng, variant, n):
     A = X @ X.T + 1e-3 * np.eye(n)
     b = rng.standard_normal((n, 3))
     Af = A.copy()
-    L.sgdml_b200_set_gemm_variant(variant)
+    _set_gemm_variant(L, variant)
     try:
         _lib.check(L.sgdml_b200_potrf(_lib.ptr(Af), n, n, None), 'potrf')
     finally:
@@ -856,12 +868,14 @@ def test_ase_calculator_core_units(eng, golden):
     assert abs(_KCAL_PER_MOL_IN_EV - 0.0433641) < 1e-6
 
 
-# --------------------------------------------------------------------------- assembly kernels v3 / v4 (chunked permutations)
-@pytest.mark.parametrize('variant', [3, 4, 5])
+# --------------------------------------------------------------------------- small-molecule assembly kernels
+@pytest.mark.parametrize('variant', [2, 3, 4, 5])
 def test_assemble_v3_kernel(eng, golden, variant):
-    """k_assemble_v3 (permutation chunks, delta on the fly, resident row tables) and k_assemble_v4 (byte permutation
-    tables, odd table strides, type-major phase A over kept column atoms) against the reference's K: full matrix
-    (symmetric mode), a column subset, row ranges, and the multi-launch row path."""
+    """k_assemble_v4 (permutation chunks, delta on the fly, resident row tables, byte permutation tables, odd table
+    strides, type-major phase A over kept column atoms), k_assemble_v5 (the same on the compressed pair arrays) and
+    k_assemble (per-permutation phases, the kernel they are compared with elsewhere) against the reference's K: full
+    matrix (symmetric mode), a column subset, row ranges, and the multi-launch row path.  Variant 3 selected
+    k_assemble_v3, which is removed: the hook rejects it and keeps the default routing."""
     from sgdml_b200 import _lib
 
     N, M = int(golden['n_atoms']), golden['R_desc'].shape[0]
@@ -870,7 +884,7 @@ def test_assemble_v3_kernel(eng, golden, variant):
     args = (golden['R_desc'], golden['R_d_desc'], golden['tril_perms_lin'], int(golden['sig']))
     cols = np.unique(np.random.default_rng(11).integers(0, n, size=37))
     L = _lib.lib()
-    L.sgdml_b200_set_assemble_variant(variant)
+    assert L.sgdml_b200_set_assemble_variant(variant) == (_ERR_ARG if variant == 3 else 0)
     try:
         K, _ = t._assemble_kernel_mat_device(*args)
         assert rel_err(K[:, :n].cpu().numpy(), golden['K']) < 1e-12
@@ -889,7 +903,7 @@ def test_assemble_v3_kernel(eng, golden, variant):
 
 def test_assemble_v3_many_permutations(eng):
     """A permutation group too large for one chunk (S = 81, 12 atoms... PG < S) and a mid-sized molecule whose sub-blocks
-    are split over grid.z (N = 36): v3 and v4 against the per-permutation kernel, full matrix and a column subset."""
+    are split over grid.z (N = 36): v4 and v5 against the per-permutation kernel, full matrix and a column subset."""
     from sgdml_b200 import _lib, synth
     from sgdml_b200.desc import Desc, tril_perms_lin
 
@@ -902,7 +916,7 @@ def test_assemble_v3_many_permutations(eng):
         lin = tril_perms_lin(perms)
         out, sub = {}, {}
         cols = np.unique(np.random.default_rng(N).integers(0, 3 * N * M, size=3 * M))
-        for v in (2, 3, 4, 5):
+        for v in (2, 4, 5):
             L.sgdml_b200_set_assemble_variant(v)
             try:
                 K, nc = t._assemble_kernel_mat_device(x, g, lin, 25)
@@ -911,7 +925,7 @@ def test_assemble_v3_many_permutations(eng):
                 sub[v] = Kc[:, :ncc].cpu().numpy()
             finally:
                 L.sgdml_b200_set_assemble_variant(0)
-        for v in (3, 4, 5):
+        for v in (4, 5):
             assert rel_err(out[v], out[2]) < 1e-12
             assert rel_err(out[v], out[v].T) < 1e-12  # the mirrored blocks
             assert rel_err(sub[v], out[2][:, cols]) < 1e-12 and rel_err(sub[2], out[2][:, cols]) < 1e-12
@@ -948,34 +962,6 @@ def test_small_batch_graph_replay(eng, golden, monkeypatch, zero_copy):
     p.set_alphas(2.0 * golden['alphas_F'])
     E2, F2 = p.predict(golden['R_query'][:1])
     assert rel_err(F2, 2.0 * golden['F_query'][:1]) < 1e-10
-
-
-@pytest.mark.parametrize('variant', [1, 2, 3, 4, 5])
-@pytest.mark.parametrize(
-    'N,M,rot,swap,sig', [(9, 70, 1, 1, 20), (12, 45, 2, 0, 20), (15, 40, 2, 0, 30), (18, 21, 1, 1, 40), (21, 50, 1, 1, 20), (23, 19, 0, 1, 20)]
-)
-def test_predict_main_kernel_variants(eng, N, M, rot, swap, sig, variant):
-    """The alternative main kernels (sgdml_b200_set_predict_variant) give the same predictions as the default one on
-    every tile configuration (DP = 40, 72, 112, 160, 224, 256; a variant without a kernel for a size runs the default):
-    1 = two warp groups half a tile apart ("ping-pong"; measured slower), 2 = no split over k in GEMM1 (transform on
-    the accumulator fragments, two barriers per tile), 3 = 2 with double-buffered C1 / C2 and one barrier per tile,
-    4 = the round-1 kernels, 5 = one barrier on 16-point tiles (DP = 40 only)."""
-    from sgdml_b200 import _lib, synth
-
-    perms = synth.rotor_swap_group(N, rot, swap)
-    model, _, _ = _oracle_model(N, M, perms, sig)
-    Rq = synth.geometries(N, 70, 1).reshape(70, -1)
-    p = eng.GDMLPredict(model)
-    _lib.lib().sgdml_b200_set_predict_variant(0)
-    E0, F0 = p.predict(Rq)
-    _lib.lib().sgdml_b200_set_predict_variant(variant)
-    try:
-        E1, F1 = p.predict(Rq)
-        E1s, F1s = p.predict(Rq[:1])  # small batch: the sweep over the training points split across CTAs
-    finally:
-        _lib.lib().sgdml_b200_set_predict_variant(0)
-    assert rel_err(F1, F0) < 1e-12 and rel_err(E1, E0) < 1e-12
-    assert rel_err(F1s, F0[:1]) < 1e-12
 
 
 # --------------------------------------------------------------------------- device-block cache of the predictor

@@ -8,7 +8,7 @@ from sgdml_b200 import synth, _lib
 from sgdml_b200.desc import Desc, tril_perms_lin
 L = _lib.lib()
 t = sgdml_b200.GDMLTrain()
-def run(name, N, M, perms, sig, cols, variants=(2, 3, 4, 5, 2, 3, 4, 5)):
+def run(name, N, M, perms, sig, cols, variants=(2, 4, 5, 1, 2, 4, 5, 1)):
     R = synth.geometries(N, M, 0).reshape(M, -1)
     x, g = Desc(N).from_R(R)
     lin = tril_perms_lin(perms)

@@ -9,4 +9,4 @@ A0 = torch.randn(n, n, dtype=torch.float64, device='cuda'); A0 = A0 @ A0.T; A0 +
 for rep in range(3):
     A = A0.clone(); torch.cuda.synchronize()
     t0 = time.perf_counter(); rc = L.sgdml_b200_potrf(A.data_ptr(), n, n, None); torch.cuda.synchronize(); dt = time.perf_counter() - t0
-    print('potrf n=%d lookahead=%s rc=%d  %.4f s  %.2f TFLOP/s' % (n, os.environ.get('SGDML_B200_NO_LOOKAHEAD', '0') != '1', rc, dt, n ** 3 / 3 / dt * 1e-12), flush=True)
+    print('potrf n=%d rc=%d  %.4f s  %.2f TFLOP/s' % (n, rc, dt, n ** 3 / 3 / dt * 1e-12), flush=True)

@@ -9,7 +9,7 @@ from sgdml_b200 import _lib, synth
 
 ap = argparse.ArgumentParser()
 ap.add_argument('workload'); ap.add_argument('n_train', type=int)
-ap.add_argument('--profile', action='store_true'); ap.add_argument('--variant', type=int, default=3)
+ap.add_argument('--profile', action='store_true'); ap.add_argument('--variant', type=int, default=3, choices=(0, 2, 3))
 ap.add_argument('--reps', type=int, default=1)
 a = ap.parse_args()
 L = _lib.lib()

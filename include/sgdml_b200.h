@@ -130,6 +130,13 @@ int sgdml_b200_predict_train(sgdml_b200_model* model, int64_t m_begin, int64_t m
  * (iterative.py:183-204: tolerance 1e-4).  No effect for D <= 256. */
 int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* model, int slices, void* stream);
 
+/* Test hook: at most max_geos queries (or training points) per chunk of sgdml_b200_predict and
+ * sgdml_b200_predict_train, for every model; 0 = no cap (the default: chunks bounded by workspace size only).  Negative
+ * values are rejected.  The cap also bounds the minimum per-batch workspace, which limits how far small batches split
+ * the sweep over the training points.  Workspaces never shrink: it applies fully to models created after the call.
+ * Tests lower it to cover the multi-chunk, pipelined and tail-chunk paths at small batch sizes. */
+int sgdml_b200_set_predict_chunk(int64_t max_geos);
+
 /* Shape of a model: n_atoms, n_train, n_perms (any pointer may be NULL). */
 int sgdml_b200_model_dims(const sgdml_b200_model* model, int64_t* n_atoms, int64_t* n_train, int64_t* n_perms);
 

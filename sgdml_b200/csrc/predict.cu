@@ -1084,6 +1084,8 @@ int ensure_pipe(sgdml_b200_model* m) {
   return 0;
 }
 
+int64_t g_chunk_cap = 0;  // sgdml_b200_set_predict_chunk (test hook): upper bound on chunk_geos, 0 = none
+
 // queries per chunk: bounds the G workspace (rows * DP * 8 bytes) to ~256 MB
 int64_t chunk_geos(const sgdml_b200_model* m) {
   int64_t rows = (int64_t)(256ll << 20) / ((int64_t)m->DP * 8);
@@ -1091,6 +1093,7 @@ int64_t chunk_geos(const sgdml_b200_model* m) {
   int64_t g = rows / m->S;
   if (g < 1) g = 1;
   if (g > 65536) g = 65536;
+  if (g_chunk_cap > 0 && g > g_chunk_cap) g = g_chunk_cap;
   return g;
 }
 
@@ -1698,6 +1701,12 @@ int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* m, int slices, voi
     free_oz(m->ozXcT);
     free_oz(m->ozJAT);
   }
+  return 0;
+}
+
+int sgdml_b200_set_predict_chunk(int64_t max_geos) {
+  SG_ARG(max_geos >= 0);
+  g_chunk_cap = max_geos;
   return 0;
 }
 

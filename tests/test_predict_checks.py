@@ -1,0 +1,220 @@
+"""The acceptance checks of tests/predict_checks.py on CPU: the chunk plan against hand-computed plans, and the
+componentwise force / energy bound against the oracle -- it passes an independent FP64 evaluation and fails each
+injected defect of the kind a multi-chunk prediction could have.  No GPU needed."""
+
+import numpy as np
+import pytest
+
+import predict_checks as pc
+from oracle import desc as odesc
+from oracle import predict as opredict
+
+
+# ------------------------------------------------------------------------------------------------ chunk plans
+def _plan(n_atoms, n_train, S, B, host_io, **kw):
+    ly = pc.layout(n_atoms, n_train)
+    return pc.chunk_plan(ly.D, ly.DP, ly.Mpad, S, ly.large, B, host_io, **kw)
+
+
+def test_layout():
+    assert pc.layout(9, 200) == pc.Layout(36, 40, 64, 32, 224, False)
+    assert pc.layout(21, 1000) == pc.Layout(210, 224, 32, 16, 1008, False)
+    assert pc.layout(23, 19) == pc.Layout(253, 256, 32, 8, 24, False)
+    assert pc.layout(24, 29) == pc.Layout(276, 280, 8, 8, 32, True)
+    assert pc.layout(42, 2000) == pc.Layout(861, 864, 8, 8, 2000, True)
+    assert pc.layout(60, 3000) == pc.Layout(1770, 1776, 8, 8, 3000, True)
+
+
+def test_chunk_plan_aspirin():
+    # 2^28 / (224 * 8) / 6 = 24 966 queries per chunk
+    assert pc.chunk_geos(224, 1008, 6, False) == 24966
+    dev = _plan(21, 1000, 6, 65536, False)
+    assert dev.chunks == [(0, 24966), (24966, 49932), (49932, 65536)]
+    assert dev.slots == [0, 0, 0] and not dev.pipelined and not dev.graph and dev.main_launches == 3
+    host = _plan(21, 1000, 6, 65536, True)
+    assert host.chunks == [(0, 16384), (16384, 32768), (32768, 49152), (49152, 65536)]
+    assert host.slots == [0, 1, 0, 1] and host.pipelined and host.main_launches == 4
+    assert pc.edge_rows(dev) == [0, 24965, 24966, 49931, 49932, 65535]
+
+
+def test_chunk_plan_ethanol():
+    assert pc.chunk_geos(40, 224, 6, False) == 65536  # the 65 536 cap applies
+    assert _plan(9, 200, 6, 65536, False).chunks == [(0, 65536)]
+    assert _plan(9, 200, 6, 65536, True).chunks == [(i * 16384, (i + 1) * 16384) for i in range(4)]
+    tail = _plan(9, 200, 6, 3 * 65536 + 3, False)
+    assert tail.chunks == [(0, 65536), (65536, 131072), (131072, 196608), (196608, 196611)]
+    assert tail.main_launches == 4
+    h4096 = _plan(9, 200, 6, 4096, True)
+    assert h4096.chunks == [(0, 1024), (1024, 2048), (2048, 3072), (3072, 4096)] and h4096.slots == [0, 1, 0, 1]
+    h4095 = _plan(9, 200, 6, 4095, True)  # one chunk on the caller's stream
+    assert h4095.chunks == [(0, 4095)] and not h4095.pipelined and h4095.main_launches == 1
+    h4097 = _plan(9, 200, 6, 4097, True)  # max(1024, ceil(4097 / 4)) = 1025
+    assert h4097.chunks == [(0, 1025), (1025, 2050), (2050, 3075), (3075, 4097)]
+    g16 = _plan(9, 200, 6, 16, True)
+    assert g16.graph and g16.chunks == [(0, 16)] and g16.main_launches == 0
+    g17 = _plan(9, 200, 6, 17, True)
+    assert not g17.graph and g17.chunks == [(0, 17)] and g17.main_launches == 1
+    assert not _plan(9, 200, 6, 16, False).graph  # device buffers never take the graph path
+    assert _plan(9, 200, 6, 0, True).chunks == []
+
+
+def test_chunk_plan_large_descriptors():
+    # ac-ala3-nhme: min(2^31 / (864 * 8), 2^31 / (2000 * 8)) / 243 = 552
+    assert pc.chunk_geos(864, 2000, 243, True) == 552
+    p = _plan(42, 2000, 243, 4096, False)
+    assert len(p.chunks) == 8 and p.chunks[-1] == (3864, 4096) and p.main_launches == 16
+    # c60, I_h: 89 478 / 120 = 745; K.v over 3000 training points is 4 chunks of 745 and a tail of 20
+    assert pc.chunk_geos(1776, 3000, 120, True) == 745
+    t = _plan(60, 3000, 120, 3000, True, train=True)
+    assert t.chunks == [(0, 745), (745, 1490), (1490, 2235), (2235, 2980), (2980, 3000)]
+    assert not t.pipelined and not t.graph and t.main_launches == 10
+
+
+def test_chunk_cap_hook_arguments():
+    """sgdml_b200_set_predict_chunk is host code: it runs without a GPU.  Negative caps are rejected."""
+    from sgdml_b200 import _lib
+
+    L = _lib.lib()
+    try:
+        assert L.sgdml_b200_set_predict_chunk(-1) == -1000
+        assert 'max_geos >= 0' in _lib.last_error()
+        assert L.sgdml_b200_set_predict_chunk(7) == 0
+    finally:
+        assert L.sgdml_b200_set_predict_chunk(0) == 0
+
+
+def test_chunk_plan_cap():
+    p = _plan(9, 200, 6, 4097, True, cap=7)  # hundreds of alternating chunks
+    assert len(p.chunks) == 586 and p.chunks[-1] == (4095, 4097)
+    assert p.slots[:4] == [0, 1, 0, 1] and p.slots[-1] == 1 and p.main_launches == 586
+    assert _plan(9, 200, 6, 23, False, cap=7).chunks == [(0, 7), (7, 14), (14, 21), (21, 23)]
+    assert _plan(24, 29, 6, 23, False, cap=5).main_launches == 10
+    assert _plan(21, 40, 6, 1, False, cap=1).chunks == [(0, 1)]
+    assert _plan(9, 200, 6, 7, True, cap=2).graph  # the graph path runs the batch whole, whatever the cap
+
+
+# ------------------------------------------------------------------------------------------------ the bound
+N, M, SIG, B = 9, 50, 20, 40  # M = 50: the last 32-point training tile is partially padded (18 real points)
+CAP = 16
+
+
+def _model(M_=M, reverse=False):
+    from sgdml_b200 import synth
+
+    perms = synth.rotor_swap_group(N, 1, 1)
+    R = synth.geometries(N, M, 0).reshape(M, -1)
+    alphas = np.random.default_rng(99).standard_normal((M, 3 * N))
+    x, g = odesc.from_R(R)
+    ja = odesc.d_desc_dot_vec(g, alphas)
+    x, ja = x[:M_], ja[:M_]
+    if reverse:
+        x, ja = x[::-1], ja[::-1]
+    return {
+        'type': 'm',
+        'z': np.ones(N, dtype=np.int64),
+        'R_desc': np.ascontiguousarray(x.T),
+        'R_d_desc_alpha': np.ascontiguousarray(ja),
+        'c': 0.37,
+        'std': 1.7,
+        'sig': SIG,
+        'perms': perms,
+        'tril_perms_lin': odesc.tril_perms_lin(perms),
+    }
+
+
+@pytest.fixture(scope='module')
+def case():
+    from sgdml_b200 import synth
+
+    model = _model()
+    op = opredict.Predictor(model)
+    R = synth.geometries(N, B, 1).reshape(B, -1)
+    E, F = op.predict(R)
+    scale = pc.predict_abs_scale(model, R, oracle=op)
+    k = pc.n_terms(M, op.n_perms, N * (N - 1) // 2)
+    plan = _plan(N, M, op.n_perms, B, False, cap=CAP)
+    assert plan.chunks == [(0, 16), (16, 32), (32, 40)]
+    return dict(model=model, op=op, R=R, E=E, F=F, scale=scale, k=k, plan=plan)
+
+
+def test_tau_at_aspirin_shape():
+    assert pc.tau(pc.n_terms(1000, 6, 210)) < 1e-11
+
+
+def test_scale_dominates_the_result(case):
+    sE, sF = case['scale']
+    assert np.all(sF >= np.abs(case['F']) * (1 - 1e-12)) and np.all(sE > 0)
+    assert np.all(sE >= np.abs(case['E'] - 0.37) * (1 - 1e-12))
+
+
+def test_independent_fp64_evaluation_passes(case):
+    """The training points in reverse order: every sum runs in another order, so the rounding differs."""
+    E2, F2 = opredict.Predictor(_model(reverse=True)).predict(case['R'])
+    assert not np.array_equal(F2, case['F'])
+    rF, rE = pc.check_predict(E2, F2, case['E'], case['F'], case['scale'], case['k'])
+    assert rF < pc.tau(case['k']) / 10 and rE < pc.tau(case['k']) / 10
+    pc.check_predict(None, F2, None, case['F'], case['scale'], case['k'])  # return_E=False
+
+
+def _fails(case, E, F, match=None):
+    with pytest.raises(AssertionError, match=match):
+        pc.check_predict(E, F, case['E'], case['F'], case['scale'], case['k'])
+
+
+def test_chunk_shifted_by_one_geometry_fails(case):
+    lo, hi = case['plan'].chunks[1]
+    E, F = case['E'].copy(), case['F'].copy()
+    F[lo:hi] = case['F'][lo + 1 : hi + 1]
+    E[lo:hi] = case['E'][lo + 1 : hi + 1]
+    _fails(case, E, F, 'force entries')
+
+
+def test_stale_chunk_fails(case):
+    """One chunk holds the previous call's outputs (another batch of the same size)."""
+    from sgdml_b200 import synth
+
+    E_prev, F_prev = case['op'].predict(synth.geometries(N, B, 2).reshape(B, -1))
+    lo, hi = case['plan'].chunks[2]
+    E, F = case['E'].copy(), case['F'].copy()
+    F[lo:hi], E[lo:hi] = F_prev[lo:hi], E_prev[lo:hi]
+    _fails(case, E, F)
+
+
+def test_dropped_term_fails(case):
+    """One (training point, permutation) term missing from one geometry's sums."""
+    op = case['op']
+    S = op.n_perms
+    k_drop = (M - 1) * S + S - 1  # last training point, last permutation
+    sub = opredict.Predictor(case['model'])
+    sub.R_desc_perms = np.delete(op.R_desc_perms, k_drop, axis=0)
+    sub.R_d_desc_alpha_perms = np.delete(op.R_d_desc_alpha_perms, k_drop, axis=0)
+    i = 21
+    E_i, F_i = sub.predict(case['R'][i : i + 1])
+    E, F = case['E'].copy(), case['F'].copy()
+    E[i], F[i] = E_i[0], F_i[0]
+    _fails(case, E, F, 'force entries')
+    _fails(case, E, case['F'], 'energies')  # the energy alone gives it away too
+
+
+def test_dropped_padded_tile_fails(case):
+    """The last, partially padded 32-point training tile (points 32..49) missing from every sum."""
+    ly = pc.layout(N, M)
+    assert ly.BM == 32 and ly.Mpad == 64 and M % ly.BM != 0
+    E, F = opredict.Predictor(_model(M_=M - M % ly.BM)).predict(case['R'])
+    _fails(case, E, F, 'force entries')
+
+
+def test_one_entry_perturbed_fails(case):
+    sF = case['scale'][1]
+    F = case['F'].copy()
+    F[29, 17] += 1e-10 * sF[29, 17]
+    _fails(case, case['E'], F, r'first at \(29, 17\)')
+
+
+def test_nan_fails(case):
+    F = case['F'].copy()
+    F[39, 0] = np.nan
+    _fails(case, case['E'], F)
+    E = case['E'].copy()
+    E[3] = np.nan
+    _fails(case, E, case['F'])

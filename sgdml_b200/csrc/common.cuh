@@ -125,6 +125,26 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
                : "d"(a), "d"(b));
 }
 
+// Hopper FP64 MMA shapes (sm_90; SASS DMMA.16x8x16 / DMMA.16x8x8, each one instruction at twice the FMA rate of
+// m8n8k4 on H100).  With g = l/4, t = l%4, lane l holds (PTX ISA, mma.m16n8k{8,16} .f64):
+//   a[i] = A[g + 8*(i&1)][t + 4*(i>>1)],  b[i] = B[t + 4*i][g],
+//   c0,c1 = C[g][2t + {0,1}],  c2,c3 = C[g + 8][2t + {0,1}].
+// D(16x8) += A(16x16, row) * B(16x8, col)
+__device__ __forceinline__ void dmma16816(double* c, const double* a, const double* b) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+      "{%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]),
+        "d"(b[1]), "d"(b[2]), "d"(b[3]));
+}
+// D(16x8) += A(16x8, row) * B(8x8, col); a[0..3], b[0..1] as above
+__device__ __forceinline__ void dmma1688(double* c, const double* a, const double* b) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+               : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+               : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }

@@ -12,16 +12,20 @@
 //    (B, M*S, D) temporary on the GPU (torchtools.py:964-966).
 //  * The sum over training points is two GEMM-shaped contractions around an elementwise
 //    Matern-5/2 transform -- the same shape as attention -- and both run on the FP64
-//    tensor pipe (mma.sync m8n8k4.f64, SASS DMMA; wgmma has no f64 type):
+//    tensor pipe in Hopper's m16n8k16 shape (m16n8k8 for 8-wide k-steps; SASS DMMA.16x8x16,
+//    twice the FMA rate of the Ampere m8n8k4 shape on H100; wgmma has no f64 type):
 //      GEMM1: S1 = Q Xc^T, S2 = Q JA^T                      (contraction over D)
 //      n^2 = |q|^2 + |Xc_m|^2 - 2 S1,  a = S2 - Xc_m.JA_m,  c1, c2 = Matern factors
 //      GEMM2: G = (sum_m c1) Q - C1 Xc - C2 JA             (contraction over M)
+//    A GEMM1 warp owns 16 query rows x 8 training points of BOTH S1 and S2, so every Q
+//    fragment it loads from shared memory feeds at least two MMAs.
 //    G (BQ x DP) lives in registers for the whole sweep over M; Xc/JA tiles arrive through
 //    a double-buffered cp.async.bulk (TMA engine) + mbarrier pipeline from L2.
 //  * A small finishing kernel folds the S virtual rows back (F_desc[d] = sum_p
 //    G_p[perm_p[d]]), applies J_x^T (predict.py:240-243) and the std / c scaling.
 #include <algorithm>
 #include <cmath>
+#include <type_traits>
 
 #include "common.cuh"
 #include "desc.cuh"
@@ -38,7 +42,12 @@ struct PCfg {
   // pipe sees DMMA work from one warp while another runs the Matern transform; the bulk copies of tile t + 1 are issued
   // right after the barrier of tile t (its stage was last read by GEMM2 of tile t - 1)
   static constexpr int OB = OB_;
-  static_assert(OB_ == 0 || W1K_ == 1, "one-barrier form needs the transform on the accumulator fragments");
+  // XK (one-barrier form with W1K == 2): the two warps of a pair split GEMM1 over k, then swap row halves of their
+  // partial S1 / S2 fragments through a small exchange area (ordered by a 64-thread named barrier), so that each warp
+  // finishes 8 of the 16 rows and the transform stays on registers
+  static constexpr bool XK = OB_ && W1K_ == 2;
+  static_assert(OB_ == 0 || W1K_ <= 2, "one-barrier form needs the transform on the accumulator fragments");
+  static constexpr bool FUSED = W1K_ == 1 || XK;  // Matern transform on the GEMM1 accumulators
   static constexpr int W2S = W2S_;      // 2: GEMM2 split by operand (warps 0-3: C1*Xc, warps 4-7: C2*JA)
   static constexpr int MINB = MINB_;    // CTAs per SM the kernel is compiled for
   static constexpr int DP = DP_;        // padded descriptor size (multiple of 8)
@@ -49,19 +58,27 @@ struct PCfg {
   static constexpr int W1Q = W1Q_, W1M = W1M_, W1K = W1K_;  // GEMM1 warp grid (rows, cols, split-k)
   static constexpr int W2Q = W2Q_, W2D = W2D_;              // GEMM2 warp grid (rows, cols)
   static constexpr int NT = 256;
-  static constexpr int TR1 = BQ / (8 * W1Q);
-  static constexpr int TC1 = BM / (8 * W1M);
-  static constexpr int KS1 = DP / 4 / W1K;  // k-steps per warp in GEMM1
-  static constexpr int TR2 = BQ / (8 * W2Q);
+  // all contractions run on m16n8k16 (m16n8k8 for a trailing 8-wide k-step): fragments are 16 rows x 8 columns
+  static constexpr int TR1 = BQ / (16 * W1Q);  // 16-row fragments per warp in GEMM1
+  static constexpr int TC1 = BM / (8 * W1M);   // 8-point fragments per warp in GEMM1 (each one of S1 and of S2)
+  static constexpr int KR1 = DP / W1K;         // GEMM1 k-range per warp
+  // GEMM1 k-step: m16n8k8 under the 128-register cap of two CTAs per SM (half the fragment registers), else m16n8k16
+  static constexpr int KW1 = MINB_ > 1 ? 8 : 16;
+  static constexpr int KN1 = KR1 / KW1, K8 = (KR1 % KW1) / 8;  // KW1-wide k-steps, then at most one k8 step
+  static constexpr int TR2 = BQ / (16 * W2Q);
   static constexpr int TD2 = DP / (8 * W2D);
+  static constexpr int KW2 = BM_ >= 16 ? 16 : 8;  // GEMM2 k-step (contraction over the BM points)
   static constexpr int EPT = BQ * BM / NT;  // epilogue-1 elements per thread
-  // a warp that owns a single 8 x 8 fragment of S1 / S2 runs two interleaved accumulation chains over k (summed in
-  // registers before the transform): four independent DMMAs in flight per warp instead of two
-  static constexpr int KI = (W1K_ == 1 && TR1 * TC1 == 1 && KS1 % 2 == 0) ? 2 : 1;
+  // a warp that owns one S1 / S2 fragment pair runs two interleaved accumulation chains over k (summed in registers
+  // before the transform): four independent DMMAs in flight per warp instead of two
+  static constexpr int KI = (TR1 * TC1 == 1 && KN1 + K8 >= 2) ? 2 : 1;
+  static constexpr int PK = XK ? 1 : W1K;   // partial S1 / S2 sets in shared memory
   static_assert(W1Q * W1M * W1K == 8 && W2Q * W2D * W2S == 8 && (W2S == 1 || W2S == 2), "8 warps");
-  static_assert(W2S == 1 || W1K * 2 * BQ_ * (BM_ + 4) >= BQ_ * DP_, "combine scratch must fit in the S/C region");
-  static_assert(BQ % (8 * W1Q) == 0 && BM % (8 * W1M) == 0 && (DP / 4) % W1K == 0, "GEMM1 tiling");
-  static_assert(BQ % (8 * W2Q) == 0 && DP % (8 * W2D) == 0, "GEMM2 tiling");
+  static_assert(W2S == 1 || (OB_ ? 2 : 1) * PK * 2 * BQ_ * (BM_ + 4) >= BQ_ * DP_,
+                "combine scratch must fit in the S/C region");
+  static_assert(BQ % (16 * W1Q) == 0 && BM % (8 * W1M) == 0 && DP % (8 * W1K) == 0, "GEMM1 tiling");
+  static_assert(!XK || TR1 * TC1 == 1, "the exchange swaps one fragment pair per warp");
+  static_assert(BQ % (16 * W2Q) == 0 && DP % (8 * W2D) == 0 && BM % KW2 == 0, "GEMM2 tiling");
   static_assert(BM == 8 || BM == 16 || BM == 32, "row reduction uses shuffles inside one warp");
   static_assert((BQ * BM) % NT == 0, "epilogue mapping");
   // shared memory carve-up (in doubles)
@@ -71,11 +88,12 @@ struct PCfg {
   static constexpr int OFF_MM = OFF_JA + 2 * BM * DS;     // [2][BM]
   static constexpr int OFF_XJA = OFF_MM + 2 * BM;         // [2][BM]
   static constexpr int OFF_AE = OFF_XJA + 2 * BM;         // [2][BM] energy-constraint coefficients (zeros when unused)
-  static constexpr int OFF_P = OFF_AE + 2 * BM;           // [W1K][2][BQ*CS]; set 0 becomes C1/C2
-  static constexpr int OFF_QQ = OFF_P + (OB_ ? 2 : 1) * W1K * 2 * BQ * CS;
+  static constexpr int OFF_P = OFF_AE + 2 * BM;           // [PK][2][BQ*CS]; set 0 becomes C1/C2
+  static constexpr int OFF_QQ = OFF_P + (OB_ ? 2 : 1) * PK * 2 * BQ * CS;
   static constexpr int OFF_CSUM = OFF_QQ + BQ;
   static constexpr int OFF_E = OFF_CSUM + BQ;
-  static constexpr int OFF_BAR = OFF_E + BQ;              // 3 x uint64
+  static constexpr int OFF_XCH = OFF_E + BQ;              // XK: [4 pairs][2 senders][S1, S2][32 lanes] double2
+  static constexpr int OFF_BAR = OFF_XCH + (XK ? 4 * 2 * 2 * 32 * 2 : 0);  // 3 x uint64
   static constexpr int SMEM_DOUBLES = OFF_BAR + 4;
   static constexpr size_t SMEM_BYTES = (size_t)SMEM_DOUBLES * 8;
   static_assert(SMEM_BYTES <= 232448, "exceeds 227 KB of shared memory");
@@ -159,6 +177,37 @@ __device__ __forceinline__ double matern52_ecstr(double x5, double a, double ae,
   return fma(a, c2, ae * kee);
 }
 
+// ============================================================== MMA fragments (layouts in common.cuh)
+// A fragment (16 x KW) of a row-major tile with leading dimension ld; p points at its element (g, t)
+template <int KW>
+__device__ __forceinline__ void frag_a(double* f, const double* p, int ld) {
+#pragma unroll
+  for (int i = 0; i < KW / 2; ++i) f[i] = p[(i & 1) * 8 * ld + (i >> 1) * 4];
+}
+// B fragment (KW x 8) whose column n is row n of the tile in shared memory (Xc / JA rows in GEMM1); p at (k t, n g)
+template <int KW>
+__device__ __forceinline__ void frag_b_rows(double* f, const double* p) {
+#pragma unroll
+  for (int i = 0; i < KW / 4; ++i) f[i] = p[i * 4];
+}
+// B fragment (KW x 8) stored k-major with leading dimension ld (Xc / JA tiles in GEMM2); p at (k t, n g)
+template <int KW>
+__device__ __forceinline__ void frag_b_cols(double* f, const double* p, int ld) {
+#pragma unroll
+  for (int i = 0; i < KW / 4; ++i) f[i] = p[i * 4 * ld];
+}
+template <int KW>
+__device__ __forceinline__ void mma_f64(double* c, const double* a, const double* b) {
+  if constexpr (KW == 16)
+    dmma16816(c, a, b);
+  else
+    dmma1688(c, a, b);
+}
+
+__device__ __forceinline__ void bar_sync_named(int id, int n_threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n_threads) : "memory");
+}
+
 // ============================================================== main kernel
 template <class C>
 __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs p) {
@@ -220,25 +269,26 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
   const int w1k = warp % C::W1K;
   const int w1m = (warp / C::W1K) % C::W1M;
   const int w1q = warp / (C::W1K * C::W1M);
-  const int row1 = w1q * (C::TR1 * 8);
+  const int row1 = w1q * (C::TR1 * 16);
   const int col1 = w1m * (C::TC1 * 8);
-  const int k1 = w1k * C::KS1 * 4;
+  const int k1 = w1k * C::KR1;
   // GEMM2 warp coordinates
   constexpr int W2G = C::W2Q * C::W2D;  // warps per operand group
   const int w2s = warp / W2G;           // 0: Xc (and JA when W2S == 1), 1: JA
   const int w2d = (warp % W2G) % C::W2D;
   const int w2q = (warp % W2G) / C::W2D;
-  const int row2 = w2q * (C::TR2 * 8);
+  const int row2 = w2q * (C::TR2 * 16);
   const int dcol2 = w2d * (C::TD2 * 8);
 
-  double accG[C::TR2][C::TD2][2];
+  double accG[C::TR2][C::TD2][4];
 #pragma unroll
   for (int i = 0; i < C::TR2; ++i)
 #pragma unroll
-    for (int j = 0; j < C::TD2; ++j) accG[i][j][0] = accG[i][j][1] = 0.0;
+    for (int j = 0; j < C::TD2; ++j) accG[i][j][0] = accG[i][j][1] = accG[i][j][2] = accG[i][j][3] = 0.0;
 
-  // running row sums: split-k path -> per epilogue element; fused path -> per fragment row
-  constexpr int NPART = (C::W1K > 1) ? C::EPT : C::TR1;
+  // running row sums: split-k path -> per epilogue element; fused path -> per fragment row (g and g + 8 of each
+  // 16-row fragment; XK: the one half this warp transforms)
+  constexpr int NPART = !C::FUSED ? C::EPT : C::XK ? 1 : 2 * C::TR1;
   double csum_part[NPART], E_part[NPART];
 #pragma unroll
   for (int j = 0; j < NPART; ++j) csum_part[j] = E_part[j] = 0.0;
@@ -264,102 +314,117 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
     const double* xjat = xjas + s * C::BM;
     const double* aet = aes + s * C::BM;
     mbar_wait(&bars[s], (uint32_t)(((t - t_begin) >> 1) & 1));
-    // real training points in this tile: the zero-padded tail of the last tile is skipped
-    // (whole 8-point fragment columns in GEMM1, whole 4-point k-steps in GEMM2)
+    // real training points in this tile.  GEMM1 skips the 8-point fragments of the zero-padded tail: their S1 / S2
+    // are exactly zero, as are the model rows, so the transform below turns them into c1 = 0 and a finite c2 that
+    // GEMM2 multiplies by zero rows.  GEMM2's k16 steps read every C1 / C2 column, and every one is written each tile.
     const int mvalid = min(C::BM, p.M - t * C::BM);
 
     // ---------------- GEMM1: S1 = Q Xc^T, S2 = Q JA^T (over this warp's k-range)
     {
-      double a1[C::TR1][C::TC1][2], a2[C::TR1][C::TC1][2];
+      double a1[C::KI][C::TR1][C::TC1][4], a2[C::KI][C::TR1][C::TC1][4];
 #pragma unroll
-      for (int i = 0; i < C::TR1; ++i)
+      for (int c = 0; c < C::KI; ++c)
 #pragma unroll
-        for (int j = 0; j < C::TC1; ++j) a1[i][j][0] = a1[i][j][1] = a2[i][j][0] = a2[i][j][1] = 0.0;
+        for (int i = 0; i < C::TR1; ++i)
+#pragma unroll
+          for (int j = 0; j < C::TC1; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) a1[c][i][j][e] = a2[c][i][j][e] = 0.0;
       const double* qa = Qs + (row1 + lr) * C::DS + k1 + lc;
       const double* xb = Xt + (col1 + lr) * C::DS + k1 + lc;
       const double* jb = JAt + (col1 + lr) * C::DS + k1 + lc;
-      if constexpr (C::KI == 2) {
-        // one fragment per warp: even and odd k-steps accumulate into separate registers
-        double b1[2] = {0.0, 0.0}, b2[2] = {0.0, 0.0};
-        if (col1 < mvalid) {  // warp-uniform
-#pragma unroll 2
-          for (int ks = 0; ks < C::KS1; ks += 2) {
-            const double fa0 = qa[ks * 4], fa1 = qa[ks * 4 + 4];
-            const double fx0 = xb[ks * 4], fx1 = xb[ks * 4 + 4];
-            const double fj0 = jb[ks * 4], fj1 = jb[ks * 4 + 4];
-            dmma884(a1[0][0][0], a1[0][0][1], fa0, fx0);
-            dmma884(a2[0][0][0], a2[0][0][1], fa0, fj0);
-            dmma884(b1[0], b1[1], fa1, fx1);
-            dmma884(b2[0], b2[1], fa1, fj1);
-          }
-        }
-        a1[0][0][0] += b1[0];
-        a1[0][0][1] += b1[1];
-        a2[0][0][0] += b2[0];
-        a2[0][0][1] += b2[1];
-      } else {
-#pragma unroll 2
-        for (int ks = 0; ks < C::KS1; ++ks) {
-          double fa[C::TR1], fx[C::TC1], fj[C::TC1];
+      // one k-step of width KW at k0, into accumulation chain c: each Q fragment feeds 2 * TC1 MMAs
+      auto kstep = [&](auto kw, int k0, int c) {
+        constexpr int KW = decltype(kw)::value;
+        double fa[C::TR1][KW / 2], fx[C::TC1][KW / 4], fj[C::TC1][KW / 4];
 #pragma unroll
-          for (int i = 0; i < C::TR1; ++i) fa[i] = qa[i * 8 * C::DS + ks * 4];
-#pragma unroll
-          for (int j = 0; j < C::TC1; ++j) {
-            fx[j] = xb[j * 8 * C::DS + ks * 4];
-            fj[j] = jb[j * 8 * C::DS + ks * 4];
-          }
-#pragma unroll
-          for (int j = 0; j < C::TC1; ++j) {
-            if (col1 + j * 8 < mvalid) {  // warp-uniform
-#pragma unroll
-              for (int i = 0; i < C::TR1; ++i) {
-                dmma884(a1[i][j][0], a1[i][j][1], fa[i], fx[j]);
-                dmma884(a2[i][j][0], a2[i][j][1], fa[i], fj[j]);
-              }
-            }
-          }
-        }
-      }
-      if constexpr (C::W1K == 1) {
-        // fused: Matern transform straight on the accumulator fragments (predict.py:199-217)
+        for (int i = 0; i < C::TR1; ++i) frag_a<KW>(fa[i], qa + i * 16 * C::DS + k0, C::DS);
 #pragma unroll
         for (int j = 0; j < C::TC1; ++j) {
-          const int mc = col1 + j * 8 + 2 * lc;
-          if (col1 + j * 8 < mvalid) {  // warp-uniform: fragment columns of real training points
-            const double m5a = 5.0 * mmt[mc], m5b = 5.0 * mmt[mc + 1];
-            const double xa = xjat[mc], xb2 = xjat[mc + 1];
+          frag_b_rows<KW>(fx[j], xb + j * 8 * C::DS + k0);
+          frag_b_rows<KW>(fj[j], jb + j * 8 * C::DS + k0);
+        }
+#pragma unroll
+        for (int j = 0; j < C::TC1; ++j) {
+          if (j == 0 || col1 + j * 8 < mvalid) {  // warp-uniform
 #pragma unroll
             for (int i = 0; i < C::TR1; ++i) {
-              const int r = row1 + i * 8 + lr;
-              const double q5 = 5.0 * qq[r];
-              double c1a_, c2a_, c1b_, c2b_;
-              const double aa = a2[i][j][0] - xa, ab = a2[i][j][1] - xb2;
-              if (p.use_ae) {  // warp-uniform: models with energy constraints in the kernel
-                E_part[i] += matern52_ecstr(fma(-10.0, a1[i][j][0], q5 + m5a), aa, aet[mc], mk, c1a_, c2a_);
-                E_part[i] += matern52_ecstr(fma(-10.0, a1[i][j][1], q5 + m5b), ab, aet[mc + 1], mk, c1b_, c2b_);
-              } else {
-                matern52(fma(-10.0, a1[i][j][0], q5 + m5a), aa, mk, c1a_, c2a_);
-                matern52(fma(-10.0, a1[i][j][1], q5 + m5b), ab, mk, c1b_, c2b_);
-                E_part[i] = fma(aa, c2a_, fma(ab, c2b_, E_part[i]));
-              }
-              csum_part[i] += c1a_ + c1b_;
-              const int off = r * C::CS + mc;
-              *reinterpret_cast<double2*>(C1s + off) = make_double2(c1a_, c1b_);
-              *reinterpret_cast<double2*>(C2s + off) = make_double2(c2a_, c2b_);
+              mma_f64<KW>(a1[c][i][j], fa[i], fx[j]);
+              mma_f64<KW>(a2[c][i][j], fa[i], fj[j]);
             }
           }
         }
+      };
+      if (col1 < mvalid) {  // warp-uniform
+#pragma unroll
+        for (int ks = 0; ks < C::KN1; ++ks) kstep(std::integral_constant<int, C::KW1>(), ks * C::KW1, ks % C::KI);
+        if constexpr (C::K8 == 1) kstep(std::integral_constant<int, 8>(), C::KN1 * C::KW1, C::KN1 % C::KI);
+      }
+      if constexpr (C::KI == 2) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          a1[0][0][0][e] += a1[1][0][0][e];
+          a2[0][0][0][e] += a2[1][0][0][e];
+        }
+      }
+
+      // Matern transform of the elements (r, mc), (r, mc + 1) (predict.py:199-217) into C1 / C2; part: row-sum slot
+      auto xform = [&](int r, int mc, double s1a, double s1b, double s2a, double s2b, int part) {
+        const double q5 = 5.0 * qq[r];
+        const double aa = s2a - xjat[mc], ab = s2b - xjat[mc + 1];
+        const double x5a = fma(-10.0, s1a, q5 + 5.0 * mmt[mc]), x5b = fma(-10.0, s1b, q5 + 5.0 * mmt[mc + 1]);
+        double c1a_, c2a_, c1b_, c2b_;
+        if (p.use_ae) {  // warp-uniform: models with energy constraints in the kernel
+          E_part[part] += matern52_ecstr(x5a, aa, aet[mc], mk, c1a_, c2a_);
+          E_part[part] += matern52_ecstr(x5b, ab, aet[mc + 1], mk, c1b_, c2b_);
+        } else {
+          matern52(x5a, aa, mk, c1a_, c2a_);
+          matern52(x5b, ab, mk, c1b_, c2b_);
+          E_part[part] = fma(aa, c2a_, fma(ab, c2b_, E_part[part]));
+        }
+        csum_part[part] += c1a_ + c1b_;
+        const int off = r * C::CS + mc;
+        *reinterpret_cast<double2*>(C1s + off) = make_double2(c1a_, c1b_);
+        *reinterpret_cast<double2*>(C2s + off) = make_double2(c2a_, c2b_);
+      };
+      if constexpr (C::W1K == 1) {
+        // fused: the transform straight on the accumulator fragments
+#pragma unroll
+        for (int j = 0; j < C::TC1; ++j)
+#pragma unroll
+          for (int i = 0; i < C::TR1; ++i)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              xform(row1 + i * 16 + h * 8 + lr, col1 + j * 8 + 2 * lc, a1[0][i][j][2 * h], a1[0][i][j][2 * h + 1],
+                    a2[0][i][j][2 * h], a2[0][i][j][2 * h + 1], 2 * i + h);
+      } else if constexpr (C::XK) {
+        // warp w1k = 0 finishes rows g (c0, c1), w1k = 1 rows g + 8 (c2, c3); each hands its partner the other half.
+        // One exchange area suffices: the partner reads it before the CTA-wide barrier of this tile, and it is next
+        // written after that barrier.
+        const double* f1 = a1[0][0][0];
+        const double* f2 = a2[0][0][0];
+        double* xs = smem + C::OFF_XCH + (warp >> 1) * 256;
+        double2* out = reinterpret_cast<double2*>(xs + w1k * 128);
+        const double2* in = reinterpret_cast<const double2*>(xs + (w1k ^ 1) * 128);
+        out[lane] = w1k ? make_double2(f1[0], f1[1]) : make_double2(f1[2], f1[3]);
+        out[32 + lane] = w1k ? make_double2(f2[0], f2[1]) : make_double2(f2[2], f2[3]);
+        bar_sync_named(1 + (warp >> 1), 64);
+        const double2 o1 = in[lane], o2 = in[32 + lane];
+        xform(row1 + 8 * w1k + lr, col1 + 2 * lc, (w1k ? f1[2] : f1[0]) + o1.x, (w1k ? f1[3] : f1[1]) + o1.y,
+              (w1k ? f2[2] : f2[0]) + o2.x, (w1k ? f2[3] : f2[1]) + o2.y, 0);
       } else {
         double* P1 = Ps + (w1k * 2 + 0) * C::BQ * C::CS;
         double* P2 = Ps + (w1k * 2 + 1) * C::BQ * C::CS;
 #pragma unroll
         for (int i = 0; i < C::TR1; ++i)
 #pragma unroll
-          for (int j = 0; j < C::TC1; ++j) {
-            const int off = (row1 + i * 8 + lr) * C::CS + col1 + j * 8 + 2 * lc;
-            *reinterpret_cast<double2*>(P1 + off) = make_double2(a1[i][j][0], a1[i][j][1]);
-            *reinterpret_cast<double2*>(P2 + off) = make_double2(a2[i][j][0], a2[i][j][1]);
-          }
+          for (int j = 0; j < C::TC1; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int off = (row1 + i * 16 + h * 8 + lr) * C::CS + col1 + j * 8 + 2 * lc;
+              *reinterpret_cast<double2*>(P1 + off) = make_double2(a1[0][i][j][2 * h], a1[0][i][j][2 * h + 1]);
+              *reinterpret_cast<double2*>(P2 + off) = make_double2(a2[0][i][j][2 * h], a2[0][i][j][2 * h + 1]);
+            }
       }
     }
     __syncthreads();
@@ -367,7 +432,7 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
       if (tid == 0 && t + 1 < n_tiles) issue_tile(t + 1);
     }
 
-    if constexpr (C::W1K > 1) {
+    if constexpr (!C::FUSED) {
       // ---------------- split-k: sum the partials, Matern transform in place
 #pragma unroll
       for (int j = 0; j < C::EPT; ++j) {
@@ -397,47 +462,47 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
 
     // ---------------- GEMM2: accG += C1 Xc + C2 JA (contraction over the BM points)
     {
+      constexpr int KW = C::KW2;
       const double* c1a = C1s + (row2 + lr) * C::CS + lc;
       const double* c2a = C2s + (row2 + lr) * C::CS + lc;
       const double* xb = Xt + lc * C::DS + dcol2 + lr;
       const double* jb = JAt + lc * C::DS + dcol2 + lr;
-      const int ks_end = (mvalid + 3) >> 2;
       if constexpr (C::W2S == 1) {
-#pragma unroll 2
-        for (int ks = 0; ks < ks_end; ++ks) {
-          double f1[C::TR2], f2[C::TR2], fx[C::TD2], fj[C::TD2];
+#pragma unroll
+        for (int k0 = 0; k0 < C::BM; k0 += KW) {
+          double f1[C::TR2][KW / 2], f2[C::TR2][KW / 2];
 #pragma unroll
           for (int i = 0; i < C::TR2; ++i) {
-            f1[i] = c1a[i * 8 * C::CS + ks * 4];
-            f2[i] = c2a[i * 8 * C::CS + ks * 4];
+            frag_a<KW>(f1[i], c1a + i * 16 * C::CS + k0, C::CS);
+            frag_a<KW>(f2[i], c2a + i * 16 * C::CS + k0, C::CS);
           }
 #pragma unroll
           for (int j = 0; j < C::TD2; ++j) {
-            fx[j] = xb[ks * 4 * C::DS + j * 8];
-            fj[j] = jb[ks * 4 * C::DS + j * 8];
-          }
+            double fx[KW / 4], fj[KW / 4];
+            frag_b_cols<KW>(fx, xb + k0 * C::DS + j * 8, C::DS);
+            frag_b_cols<KW>(fj, jb + k0 * C::DS + j * 8, C::DS);
 #pragma unroll
-          for (int i = 0; i < C::TR2; ++i)
-#pragma unroll
-            for (int j = 0; j < C::TD2; ++j) {
-              dmma884(accG[i][j][0], accG[i][j][1], f1[i], fx[j]);
-              dmma884(accG[i][j][0], accG[i][j][1], f2[i], fj[j]);
+            for (int i = 0; i < C::TR2; ++i) {
+              mma_f64<KW>(accG[i][j], f1[i], fx);
+              mma_f64<KW>(accG[i][j], f2[i], fj);
             }
+          }
         }
       } else {
         const double* ca = w2s ? c2a : c1a;
         const double* ob = w2s ? jb : xb;
-#pragma unroll 2
-        for (int ks = 0; ks < ks_end; ++ks) {
-          double f[C::TR2], fo[C::TD2];
 #pragma unroll
-          for (int i = 0; i < C::TR2; ++i) f[i] = ca[i * 8 * C::CS + ks * 4];
+        for (int k0 = 0; k0 < C::BM; k0 += KW) {
+          double f[C::TR2][KW / 2];
 #pragma unroll
-          for (int j = 0; j < C::TD2; ++j) fo[j] = ob[ks * 4 * C::DS + j * 8];
+          for (int i = 0; i < C::TR2; ++i) frag_a<KW>(f[i], ca + i * 16 * C::CS + k0, C::CS);
 #pragma unroll
-          for (int i = 0; i < C::TR2; ++i)
+          for (int j = 0; j < C::TD2; ++j) {
+            double fo[KW / 4];
+            frag_b_cols<KW>(fo, ob + k0 * C::DS + j * 8, C::DS);
 #pragma unroll
-            for (int j = 0; j < C::TD2; ++j) dmma884(accG[i][j][0], accG[i][j][1], f[i], fo[j]);
+            for (int i = 0; i < C::TR2; ++i) mma_f64<KW>(accG[i][j], f[i], fo);
+          }
         }
       }
     }
@@ -448,7 +513,7 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
   }
 
   // ---- row sums csum[r] = sum_m c1, E[r] = sum_m a c2
-  if constexpr (C::W1K > 1) {
+  if constexpr (!C::FUSED) {
 #pragma unroll
     for (int j = 0; j < C::EPT; ++j) {
       double cs = csum_part[j], es = E_part[j];
@@ -465,15 +530,16 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
     }
   } else {
 #pragma unroll
-    for (int i = 0; i < C::TR1; ++i) {
+    for (int i = 0; i < NPART; ++i) {
       double cs = csum_part[i], es = E_part[i];
       cs += __shfl_xor_sync(0xffffffffu, cs, 1);
       es += __shfl_xor_sync(0xffffffffu, es, 1);
       cs += __shfl_xor_sync(0xffffffffu, cs, 2);
       es += __shfl_xor_sync(0xffffffffu, es, 2);
+      const int r = C::XK ? row1 + 8 * w1k + lr : row1 + (i >> 1) * 16 + (i & 1) * 8 + lr;
       if (lc == 0) {  // W1M warps share a row: csum_s / E_s were zeroed before the sweep
-        atomicAdd(&csum_s[row1 + i * 8 + lr], cs);
-        atomicAdd(&E_s[row1 + i * 8 + lr], es);
+        atomicAdd(&csum_s[r], cs);
+        atomicAdd(&E_s[r], es);
       }
     }
   }
@@ -485,8 +551,10 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
       for (int i = 0; i < C::TR2; ++i)
 #pragma unroll
         for (int j = 0; j < C::TD2; ++j)
-          *reinterpret_cast<double2*>(Ps + (row2 + i * 8 + lr) * C::DP + dcol2 + j * 8 + 2 * lc) =
-              make_double2(accG[i][j][0], accG[i][j][1]);
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            *reinterpret_cast<double2*>(Ps + (row2 + i * 16 + h * 8 + lr) * C::DP + dcol2 + j * 8 + 2 * lc) =
+                make_double2(accG[i][j][2 * h], accG[i][j][2 * h + 1]);
     }
   }
   __syncthreads();
@@ -494,16 +562,17 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
   // ---- G = (sum_m c1) Q - (C1 Xc + C2 JA)
   if (C::W2S == 1 || w2s == 0) {
 #pragma unroll
-    for (int i = 0; i < C::TR2; ++i) {
-      const int r = row2 + i * 8 + lr;
+    for (int ih = 0; ih < 2 * C::TR2; ++ih) {
+      const int i = ih >> 1, h = ih & 1;
+      const int r = row2 + i * 16 + h * 8 + lr;
       const int64_t row = r0 + r;
       if (row < p.n_rows) {
         const double cs = csum_s[r];
 #pragma unroll
         for (int j = 0; j < C::TD2; ++j) {
           const int col = dcol2 + j * 8 + 2 * lc;
-          double g0 = cs * Qs[r * C::DS + col] - accG[i][j][0];
-          double g1 = cs * Qs[r * C::DS + col + 1] - accG[i][j][1];
+          double g0 = cs * Qs[r * C::DS + col] - accG[i][j][2 * h];
+          double g1 = cs * Qs[r * C::DS + col + 1] - accG[i][j][2 * h + 1];
           if constexpr (C::W2S == 2) {
             const double2 o = *reinterpret_cast<const double2*>(Ps + r * C::DP + col);
             g0 -= o.x;
@@ -936,18 +1005,22 @@ struct sgdml_b200_model {
 namespace {
 
 // tile configurations: <DP, BQ, BM, W1Q, W1M, W1K, W2Q, W2D, MINB, W2S, OB>, the fastest per size when the
-// alternatives were timed (65536 queries, M = 1000, S = 6; not re-timed on H100)
+// alternatives were timed (65536 queries, M = 1000, S = 6; not re-timed on H100).  Fragments are 16 rows x 8 columns.
 // D <= 40: two co-resident CTAs per SM so that one CTA's transform / barriers / prologue overlap the other's DMMA
 // phases (the sweep over M is only a handful of tiles at ethanol size); the doubled C1 / C2 buffers of the
-// one-barrier form would cost it the second CTA
-// 40 < D <= 224: no split over k -- every warp owns whole S1 / S2 fragments, the Matern transform runs on the
-// accumulator registers, and one CTA-wide barrier per tile (OB)
-// 224 < D <= 256: split-k GEMM1
+// one-barrier form would cost it the second CTA.  GEMM1 runs k8 steps there: the fragments of a k16 step do not fit
+// next to the accumulators under two CTAs' 128-register cap.
+// 40 < D <= 112: no split over k -- every warp owns whole S1 / S2 fragment pairs (two at BQ 64 / BM 32, one at BM 16),
+// the Matern transform runs on the accumulator registers, and one CTA-wide barrier per tile (OB).  D <= 72 splits GEMM2
+// by operand: 72 columns do not divide into two groups of whole n8 fragments.
+// 112 < D <= 224: BQ 32 x BM 16 holds only four fragment pairs, so two warps split each over k and swap row halves
+// (XK); the transform stays on registers, still one CTA-wide barrier per tile
+// 224 < D <= 256: split-k GEMM1 through shared memory, transform in shared memory
 using Cfg40 = PCfg<40, 64, 32, 4, 2, 1, 4, 1, 2, 2>;
-using Cfg72o = PCfg<72, 64, 32, 4, 2, 1, 8, 1, 1, 1, 1>;
+using Cfg72o = PCfg<72, 64, 32, 4, 2, 1, 4, 1, 1, 2, 1>;
 using Cfg112o = PCfg<112, 64, 16, 4, 2, 1, 4, 2, 1, 1, 1>;
-using Cfg160o = PCfg<160, 32, 16, 4, 2, 1, 2, 4, 1, 1, 1>;
-using Cfg224o = PCfg<224, 32, 16, 4, 2, 1, 2, 4, 1, 1, 1>;
+using Cfg160o = PCfg<160, 32, 16, 2, 2, 2, 2, 4, 1, 1, 1>;
+using Cfg224o = PCfg<224, 32, 16, 2, 2, 2, 2, 4, 1, 1, 1>;
 using Cfg256 = PCfg<256, 32, 8, 2, 1, 4, 2, 4>;
 
 struct CfgInfo {

@@ -1667,9 +1667,13 @@ int sgdml_b200_predict(sgdml_b200_model* m, const double* R, int64_t n_geo, doub
 
 int sgdml_b200_model_set_lattice(sgdml_b200_model* m, const double* lattice, const double* lattice_inv) {
   SG_ARG(m != nullptr);
+  // parse into a local first: a rejected call leaves the model's cell as it was
+  Lattice l;
+  SG_TRY(lattice_from_host(lattice, lattice_inv, &l));
   SG_CUDA(cudaDeviceSynchronize());  // no stream argument: kernels in flight copied the old cell by value, but keep calls ordered
   ++m->generation;  // captured graphs carry the cell as a kernel argument
-  return lattice_from_host(lattice, lattice_inv, &m->lat);
+  m->lat = l;
+  return 0;
 }
 
 int sgdml_b200_model_set_alphas_E(sgdml_b200_model* m, const double* alphas_E, void* stream) {

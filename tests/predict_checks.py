@@ -82,6 +82,60 @@ def n_terms(M, S, D):
     return M * S + D
 
 
+# ------------------------------------------------------------------------------------------------ periodic cells
+def _pair_frac(R, lattice_inv):
+    """Pair differences d = r_a - r_b (B, D, 3) in tril order and their fractional coordinates lat_inv @ d."""
+    R = np.asarray(R, dtype=np.float64)
+    r = R.reshape(R.shape[0], -1, 3)
+    a, b = np.tril_indices(r.shape[1], -1)
+    d = r[:, a, :] - r[:, b, :]
+    return d, np.einsum('ij,...j->...i', np.asarray(lattice_inv, dtype=np.float64), d)
+
+
+def skewed_cell(n_atoms):
+    """A triclinic cell (lattice vectors as the COLUMNS, as model['lattice']) whose edges, 1.5 ceil(N^(1/3)) + 0.1 A,
+    are just longer than the 1.5 A grid of synth.base_geometry spans: pairs three grid steps apart wrap to images
+    1.6 A away, and the skew mixes the axes in lat_inv @ d."""
+    e = 1.5 * np.ceil(n_atoms ** (1.0 / 3.0) - 1e-9) + 0.1
+    A = np.array([[1.0, 0.18, -0.12], [0.0, 0.98, 0.21], [0.0, 0.0, 0.97]])
+    return e * A / np.linalg.norm(A, axis=0)
+
+
+def pbc_margin(R, lattice, lattice_inv):
+    """Per geometry of R (B, 3N): the smallest distance of any pair's fractional difference lat_inv @ d (any of its
+    three components) from a half-integer.  Near such a tie the engine (whose cell code contracts to FMAs) and the
+    oracle (np.einsum) may round to different images, whose Jacobian rows differ in sign: random periodic queries are
+    kept at a margin from ties, and exact ties are tested on their own."""
+    assert np.asarray(lattice).shape == (3, 3)
+    _, c = _pair_frac(R, lattice_inv)
+    return np.min(np.abs(c - np.floor(c) - 0.5), axis=(1, 2))
+
+
+DESC_C = 64
+
+
+def desc_pbc_bound(R, lattice, lattice_inv):
+    """Componentwise bounds (bx (B, D), bg (B, D)) on |x - x_ref| and on each component of |g - g_ref| for the
+    descriptor x = 1/|d'| and Jacobian factor g = d'/|d'|^3 of periodic geometries, d' = d - L round(L^-1 d), away
+    from rounding ties (both sides pick the same integer k):
+      bx = DESC_C u |w|_2 / |d'|^2,   bg = DESC_C u |w|_2 / |d'|^3,   w = |d| + |L| |k|.
+    Derivation (per side, u = 2^-53, gamma_n ~ n u): d = r_a - r_b rounds once (u |d|), L k rounds within gamma_3
+    |L||k| (k exact), and the subtraction once more, so |dd'| <= gamma_5 w componentwise -- relative to w, not to |d'|:
+    the cancellation in d - L k is what the bound must cover, and |w| / |d'| >= 1 measures it.  Then |d'| moves by at
+    most 5u |w| + 2u |d'| (sum of squares and sqrt), x by 9u |w| / |d'|^2 (with the division), and g_c =
+    d'_c / |d'|^3 by (|dd'_c| + 3 |d'_c| d|d'| / |d'|) / |d'|^3 + 6u |g_c| <= 26u |w| / |d'|^3.  Two sides: 18u and 52u;
+    DESC_C = 64 leaves margin for the FMA-contracted forms."""
+    assert np.asarray(lattice).shape == (3, 3)
+    L = np.asarray(lattice, dtype=np.float64)
+    d, c = _pair_frac(R, lattice_inv)
+    k = np.around(c)
+    dp = d - np.einsum('ij,...j->...i', L, k)
+    w = np.abs(d) + np.einsum('ij,...j->...i', np.abs(L), np.abs(k))
+    wn = np.sqrt(np.sum(w * w, axis=-1))
+    dist = np.sqrt(np.sum(dp * dp, axis=-1))
+    return DESC_C * U * wn / dist ** 2, DESC_C * U * wn / dist ** 3
+
+
 # ------------------------------------------------------------------------------------------------ magnitude
 def _abs_jt(r_d_desc, w):
     """|J|^T w for w >= 0: every pair d = (a, b) adds |g_d| w_d to both atoms (vec_dot_d_desc with all signs +)."""
@@ -107,7 +161,8 @@ def predict_abs_scale(model, R=None, oracle=None, R_desc=None, R_d_desc=None):
         and a_k as q.JA_k - x_k.JA_k, so its rounding scales with |q| + |x|, not with their difference;
       * the error of the expanded squared distance (see check_predict) through the Matern factors, with
         rho_k = |q_k|^2 + |x_k|^2:  dc1_k = base_k (5/sig) 2 sqrt5 |JA_k|_2 rho_k / sig,  dc2_k = base_k 5 rho_k / sig,
-        added to |c1_k| and |c2_k|.
+        added to |c1_k| and |c2_k|; with alphas_E also the energy-energy factor's,
+        |alphas_E_k| (5/3) (1 + n_k/sig) e_k rho_k / sig^2, added to E.
     model: the model dict; oracle: an oracle.predict.Predictor of it (built if None).  R (B, 3N) queries, or R=None
     with R_desc (B, D) / R_d_desc (B, D, 3) given (the training-point evaluation)."""
     from oracle import desc as odesc
@@ -151,6 +206,7 @@ def predict_abs_scale(model, R=None, oracle=None, R_desc=None, R_d_desc=None):
         if ae is not None:
             c1 = c1 + ae * c2
             E += ae.dot((1 + (norm / sig) * (1 + norm / (3 * sig))) * e)
+            E += ae.dot((5.0 / 3.0) * (1 + norm / sig) * e * rho / sig ** 2)
         Fd = c1.dot(A) + c2.dot(JAa)
         sE[i] = E
         sF[i] = _abs_jt(R_d_desc[i], Fd)
@@ -187,6 +243,9 @@ def check_predict(E, F, E_ref, F_ref, scale, k, what='predict'):
         first order through e' = -e/sig: by a k_c1 e dn / sig with |a| <= (n/sqrt5)|JA|_2, i.e. at most
         k_c1 e |JA|_2 dx5 / (2 sqrt5 sig) -- the dc1 term times gamma_{D+2} (2 sqrt5 absorbs 10 / (2 sqrt5) = sqrt5).
         As n -> 0 (a query on a training point) a itself is rounding noise and the same bound holds with dn <= sqrt(dx5).
+        With alphas_E, K_ee = (1 + (n/sig)(1 + n/(3 sig))) e^{-n/sig} is flat at n = 0 too: dK_ee/dn =
+        -(n/(3 sig^2))(1 + n/sig) e^{-n/sig}, so with dn <= dx5/(2n) and dx5 <= 10 gamma_{D+2} rho it moves by at most
+        gamma_{D+2} (5/3)(1 + n/sig) e rho / sig^2 -- the K_ee term of predict_abs_scale times gamma_{D+2}.
       * GEMM2 and the row sums: G = (sum_m c1) q - sum_m (c1 x + c2 JA), 2M + 1 terms per virtual row: gamma_{2M+1}.
         The finishing kernel adds the S permutations times the split count (<= 2 sqrt(2 Mpad/BM) + 1), J^T adds
         N - 1 terms per force component, std one rounding: together gamma_{S(sp+1) + N + 1}.

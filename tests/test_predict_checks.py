@@ -1,6 +1,7 @@
 """The acceptance checks of tests/predict_checks.py on CPU: the chunk plan against hand-computed plans, and the
-componentwise force / energy bound against the oracle -- it passes an independent FP64 evaluation and fails each
-injected defect of the kind a multi-chunk prediction could have.  No GPU needed."""
+componentwise force / energy bound against the oracle -- on a plain, an energy-constrained and a periodic model it
+passes an independent FP64 evaluation and fails each injected defect of the kind a multi-chunk prediction could have,
+plus defects specific to energy constraints and to cells.  No GPU needed."""
 
 import numpy as np
 import pytest
@@ -96,20 +97,24 @@ def test_chunk_plan_cap():
 # ------------------------------------------------------------------------------------------------ the bound
 N, M, SIG, B = 9, 50, 20, 40  # M = 50: the last 32-point training tile is partially padded (18 real points)
 CAP = 16
+KINDS = ('plain', 'ecstr', 'pbc')  # energy constraints in the kernel; a periodic model in the skewed cell
+AE_SCALE = 0.05
 
 
-def _model(M_=M, reverse=False):
+def _model(M_=M, reverse=False, kind='plain'):
     from sgdml_b200 import synth
 
     perms = synth.rotor_swap_group(N, 1, 1)
     R = synth.geometries(N, M, 0).reshape(M, -1)
     alphas = np.random.default_rng(99).standard_normal((M, 3 * N))
-    x, g = odesc.from_R(R)
+    lat = pc.skewed_cell(N) if kind == 'pbc' else None
+    x, g = odesc.from_R(R, None if lat is None else (lat, np.linalg.inv(lat)))
     ja = odesc.d_desc_dot_vec(g, alphas)
-    x, ja = x[:M_], ja[:M_]
+    ae = AE_SCALE * np.random.default_rng(98).standard_normal(M)
+    x, ja, ae = x[:M_], ja[:M_], ae[:M_]
     if reverse:
-        x, ja = x[::-1], ja[::-1]
-    return {
+        x, ja, ae = x[::-1], ja[::-1], ae[::-1]
+    model = {
         'type': 'm',
         'z': np.ones(N, dtype=np.int64),
         'R_desc': np.ascontiguousarray(x.T),
@@ -120,40 +125,96 @@ def _model(M_=M, reverse=False):
         'perms': perms,
         'tril_perms_lin': odesc.tril_perms_lin(perms),
     }
+    if kind == 'ecstr':
+        model['alphas_E'] = np.ascontiguousarray(ae)
+    if lat is not None:
+        model['lattice'] = lat
+    return model
+
+
+_CASES = {}
+
+
+def _case(kind):
+    from sgdml_b200 import synth
+
+    if kind not in _CASES:
+        model = _model(kind=kind)
+        op = opredict.Predictor(model)
+        R = synth.geometries(N, B, 1).reshape(B, -1)
+        if kind == 'pbc':
+            assert np.min(pc.pbc_margin(R, *op.lat_and_inv)) >= 1e-6
+        E, F = op.predict(R)
+        scale = pc.predict_abs_scale(model, R, oracle=op)
+        k = pc.n_terms(M, op.n_perms, N * (N - 1) // 2)
+        plan = _plan(N, M, op.n_perms, B, False, cap=CAP)
+        assert plan.chunks == [(0, 16), (16, 32), (32, 40)]
+        _CASES[kind] = dict(kind=kind, model=model, op=op, R=R, E=E, F=F, scale=scale, k=k, plan=plan)
+    return _CASES[kind]
 
 
 @pytest.fixture(scope='module')
-def case():
-    from sgdml_b200 import synth
+def cases():
+    """The plain, energy-constrained and periodic cases: every generic check below runs on all three."""
+    return [_case(kind) for kind in KINDS]
 
-    model = _model()
-    op = opredict.Predictor(model)
-    R = synth.geometries(N, B, 1).reshape(B, -1)
-    E, F = op.predict(R)
-    scale = pc.predict_abs_scale(model, R, oracle=op)
-    k = pc.n_terms(M, op.n_perms, N * (N - 1) // 2)
-    plan = _plan(N, M, op.n_perms, B, False, cap=CAP)
-    assert plan.chunks == [(0, 16), (16, 32), (32, 40)]
-    return dict(model=model, op=op, R=R, E=E, F=F, scale=scale, k=k, plan=plan)
+
+@pytest.fixture(scope='module')
+def ecstr_case():
+    return _case('ecstr')
+
+
+@pytest.fixture(scope='module')
+def pbc_case():
+    return _case('pbc')
 
 
 def test_tau_at_aspirin_shape():
     assert pc.tau(pc.n_terms(1000, 6, 210)) < 1e-11
 
 
-def test_scale_dominates_the_result(case):
-    sE, sF = case['scale']
-    assert np.all(sF >= np.abs(case['F']) * (1 - 1e-12)) and np.all(sE > 0)
-    assert np.all(sE >= np.abs(case['E'] - 0.37) * (1 - 1e-12))
+def test_scale_dominates_the_result(cases):
+    for case in cases:
+        sE, sF = case['scale']
+        assert np.all(sF >= np.abs(case['F']) * (1 - 1e-12)) and np.all(sE > 0)
+        assert np.all(sE >= np.abs(case['E'] - 0.37) * (1 - 1e-12))
 
 
-def test_independent_fp64_evaluation_passes(case):
-    """The training points in reverse order: every sum runs in another order, so the rounding differs."""
-    E2, F2 = opredict.Predictor(_model(reverse=True)).predict(case['R'])
-    assert not np.array_equal(F2, case['F'])
-    rF, rE = pc.check_predict(E2, F2, case['E'], case['F'], case['scale'], case['k'])
-    assert rF < pc.tau(case['k']) / 10 and rE < pc.tau(case['k']) / 10
-    pc.check_predict(None, F2, None, case['F'], case['scale'], case['k'])  # return_E=False
+def _longdouble_desc(R, lat):
+    """Periodic descriptors evaluated in np.longdouble and rounded once to FP64 (the same images: no query is near a
+    tie)."""
+    ld = np.longdouble
+    r = np.asarray(R, dtype=ld).reshape(R.shape[0], -1, 3)
+    a, b = np.tril_indices(r.shape[1], -1)
+    d = r[:, a, :] - r[:, b, :]
+    L, Li = np.asarray(lat, dtype=ld), np.asarray(np.linalg.inv(lat), dtype=ld)
+    k = np.round(np.einsum('ij,...j->...i', Li, d))
+    d = d - np.einsum('ij,...j->...i', L, k)
+    dist = np.sqrt(np.sum(d * d, axis=-1))
+    return (1 / dist).astype(np.float64), (d / (dist ** 3)[..., None]).astype(np.float64)
+
+
+def _predict_desc(model, x, g):
+    """The oracle's prediction from given query descriptors (its R=None path)."""
+    op = opredict.Predictor(model)
+    op.set_R_desc(x)
+    op.set_R_d_desc(g)
+    return op.predict()
+
+
+def test_independent_fp64_evaluation_passes(cases):
+    """The training points in reverse order: every sum runs in another order, so the rounding differs.  The periodic
+    case takes its query descriptors from an np.longdouble evaluation."""
+    for case in cases:
+        rev = _model(reverse=True, kind=case['kind'])
+        if case['kind'] == 'pbc':
+            E2, F2 = _predict_desc(rev, *_longdouble_desc(case['R'], rev['lattice']))
+        else:
+            E2, F2 = opredict.Predictor(rev).predict(case['R'])
+        assert not np.array_equal(F2, case['F'])
+        rF, rE = pc.check_predict(E2, F2, case['E'], case['F'], case['scale'], case['k'])
+        assert rF < pc.tau(case['k']) / 10 and rE < pc.tau(case['k']) / 10
+        pc.check_predict(None, F2, None, case['F'], case['scale'], case['k'])  # return_E=False
 
 
 def _fails(case, E, F, match=None):
@@ -161,60 +222,165 @@ def _fails(case, E, F, match=None):
         pc.check_predict(E, F, case['E'], case['F'], case['scale'], case['k'])
 
 
-def test_chunk_shifted_by_one_geometry_fails(case):
-    lo, hi = case['plan'].chunks[1]
-    E, F = case['E'].copy(), case['F'].copy()
-    F[lo:hi] = case['F'][lo + 1 : hi + 1]
-    E[lo:hi] = case['E'][lo + 1 : hi + 1]
-    _fails(case, E, F, 'force entries')
+def test_chunk_shifted_by_one_geometry_fails(cases):
+    for case in cases:
+        lo, hi = case['plan'].chunks[1]
+        E, F = case['E'].copy(), case['F'].copy()
+        F[lo:hi] = case['F'][lo + 1 : hi + 1]
+        E[lo:hi] = case['E'][lo + 1 : hi + 1]
+        _fails(case, E, F, 'force entries')
 
 
-def test_stale_chunk_fails(case):
+def test_stale_chunk_fails(cases):
     """One chunk holds the previous call's outputs (another batch of the same size)."""
     from sgdml_b200 import synth
 
-    E_prev, F_prev = case['op'].predict(synth.geometries(N, B, 2).reshape(B, -1))
-    lo, hi = case['plan'].chunks[2]
-    E, F = case['E'].copy(), case['F'].copy()
-    F[lo:hi], E[lo:hi] = F_prev[lo:hi], E_prev[lo:hi]
-    _fails(case, E, F)
+    for case in cases:
+        E_prev, F_prev = case['op'].predict(synth.geometries(N, B, 2).reshape(B, -1))
+        lo, hi = case['plan'].chunks[2]
+        E, F = case['E'].copy(), case['F'].copy()
+        F[lo:hi], E[lo:hi] = F_prev[lo:hi], E_prev[lo:hi]
+        _fails(case, E, F)
 
 
-def test_dropped_term_fails(case):
+def test_dropped_term_fails(cases):
     """One (training point, permutation) term missing from one geometry's sums."""
-    op = case['op']
-    S = op.n_perms
-    k_drop = (M - 1) * S + S - 1  # last training point, last permutation
-    sub = opredict.Predictor(case['model'])
-    sub.R_desc_perms = np.delete(op.R_desc_perms, k_drop, axis=0)
-    sub.R_d_desc_alpha_perms = np.delete(op.R_d_desc_alpha_perms, k_drop, axis=0)
-    i = 21
-    E_i, F_i = sub.predict(case['R'][i : i + 1])
-    E, F = case['E'].copy(), case['F'].copy()
-    E[i], F[i] = E_i[0], F_i[0]
-    _fails(case, E, F, 'force entries')
-    _fails(case, E, case['F'], 'energies')  # the energy alone gives it away too
+    for case in cases:
+        op = case['op']
+        S = op.n_perms
+        k_drop = (M - 1) * S + S - 1  # last training point, last permutation
+        sub = opredict.Predictor(case['model'])
+        sub.R_desc_perms = np.delete(op.R_desc_perms, k_drop, axis=0)
+        sub.R_d_desc_alpha_perms = np.delete(op.R_d_desc_alpha_perms, k_drop, axis=0)
+        if op.alphas_E_lin is not None:
+            sub.alphas_E_lin = np.delete(op.alphas_E_lin, k_drop)
+        i = 21
+        E_i, F_i = sub.predict(case['R'][i : i + 1])
+        E, F = case['E'].copy(), case['F'].copy()
+        E[i], F[i] = E_i[0], F_i[0]
+        _fails(case, E, F, 'force entries')
+        _fails(case, E, case['F'], 'energies')  # the energy alone gives it away too
 
 
-def test_dropped_padded_tile_fails(case):
+def test_dropped_padded_tile_fails(cases):
     """The last, partially padded 32-point training tile (points 32..49) missing from every sum."""
-    ly = pc.layout(N, M)
-    assert ly.BM == 32 and ly.Mpad == 64 and M % ly.BM != 0
-    E, F = opredict.Predictor(_model(M_=M - M % ly.BM)).predict(case['R'])
-    _fails(case, E, F, 'force entries')
+    for case in cases:
+        ly = pc.layout(N, M)
+        assert ly.BM == 32 and ly.Mpad == 64 and M % ly.BM != 0
+        E, F = opredict.Predictor(_model(M_=M - M % ly.BM, kind=case['kind'])).predict(case['R'])
+        _fails(case, E, F, 'force entries')
 
 
-def test_one_entry_perturbed_fails(case):
-    sF = case['scale'][1]
-    F = case['F'].copy()
-    F[29, 17] += 1e-10 * sF[29, 17]
-    _fails(case, case['E'], F, r'first at \(29, 17\)')
+def test_one_entry_perturbed_fails(cases):
+    for case in cases:
+        sF = case['scale'][1]
+        F = case['F'].copy()
+        F[29, 17] += 1e-10 * sF[29, 17]
+        _fails(case, case['E'], F, r'first at \(29, 17\)')
 
 
-def test_nan_fails(case):
-    F = case['F'].copy()
-    F[39, 0] = np.nan
-    _fails(case, case['E'], F)
-    E = case['E'].copy()
-    E[3] = np.nan
-    _fails(case, E, case['F'])
+def test_nan_fails(cases):
+    for case in cases:
+        F = case['F'].copy()
+        F[39, 0] = np.nan
+        _fails(case, case['E'], F)
+        E = case['E'].copy()
+        E[3] = np.nan
+        _fails(case, E, case['F'])
+
+
+# ------------------------------------------------------------------------------------------------ energy constraints
+def _norms(op, R_desc):
+    """n = sqrt5 |q - x_k| (B, M S) for query descriptors R_desc (B, D)."""
+    diff = np.asarray(R_desc)[:, None, :] - op.R_desc_perms[None]
+    return np.sqrt(5.0) * np.sqrt(np.sum(diff * diff, axis=-1))
+
+
+def test_alphas_E_dropped_for_one_point_fails(ecstr_case):
+    model = dict(ecstr_case['model'])
+    model['alphas_E'] = model['alphas_E'].copy()
+    model['alphas_E'][17] = 0.0
+    E, F = opredict.Predictor(model).predict(ecstr_case['R'])
+    _fails(ecstr_case, E, F, 'force entries')
+    _fails(ecstr_case, E, ecstr_case['F'], 'energies')
+
+
+def test_alphas_E_on_one_permutation_only_fails(ecstr_case):
+    """alphas_E of one training point applied to its first permutation instead of all S."""
+    sub = opredict.Predictor(ecstr_case['model'])
+    S = sub.n_perms
+    sub.alphas_E_lin = sub.alphas_E_lin.copy()
+    sub.alphas_E_lin[17 * S + 1 : 18 * S] = 0.0
+    E, F = sub.predict(ecstr_case['R'])
+    _fails(ecstr_case, E, F, 'force entries')
+    _fails(ecstr_case, E, ecstr_case['F'], 'energies')
+
+
+def test_kee_without_cubic_term_fails(ecstr_case):
+    """K_ee = (1 + n/sig) e^{-n/sig}: the n/(3 sig) term dropped (the energy alone carries K_ee)."""
+    op = ecstr_case['op']
+    x, _ = odesc.from_R(ecstr_case['R'])
+    n = _norms(op, x)
+    dE = -op.std * (op.alphas_E_lin[None] * (n * n / (3 * SIG ** 2)) * np.exp(-n / SIG)).sum(axis=1)
+    assert np.all(np.abs(dE) > 0)
+    _fails(ecstr_case, ecstr_case['E'] + dE, ecstr_case['F'], 'energies')
+
+
+def test_kv_energy_rows_with_the_wrong_sign_fail(ecstr_case):
+    """K.v on the training points (std = 1, c = 0, R=None) as the iterative solver takes it: energies negated."""
+    from sgdml_b200 import synth
+
+    model = dict(ecstr_case['model'], std=1.0, c=0.0)
+    x, g = odesc.from_R(synth.geometries(N, M, 0).reshape(M, -1))
+    op = opredict.Predictor(model)
+    op.set_R_desc(x)
+    op.set_R_d_desc(g)
+    E, F = op.predict()
+    scale = pc.predict_abs_scale(model, oracle=op, R_desc=x, R_d_desc=g)
+    k = ecstr_case['k']
+    pc.check_predict(E, F, E, F, scale, k)
+    with pytest.raises(AssertionError, match='energies'):
+        pc.check_predict(-E, F, E, F, scale, k)
+
+
+# ------------------------------------------------------------------------------------------------ periodic models
+def test_pbc_case_wraps(pbc_case):
+    lat, lat_inv = pbc_case['op'].lat_and_inv
+    _, c = pc._pair_frac(pbc_case['R'], lat_inv)
+    assert np.mean(np.any(np.around(c) != 0, axis=-1)) >= 0.2
+    x, _ = odesc.from_R(pbc_case['R'], (lat, lat_inv))
+    assert np.max(x) <= 1.0  # every image at least 1 A away
+
+
+def test_lattice_transposed_fails(pbc_case):
+    model = dict(pbc_case['model'], lattice=pbc_case['model']['lattice'].T.copy())
+    E, F = opredict.Predictor(model).predict(pbc_case['R'])
+    _fails(pbc_case, E, F, 'force entries')
+
+
+def test_one_pair_image_moved_fails(pbc_case):
+    """Geometry 21, pair 30: its difference vector moved by the first lattice vector."""
+    lat, lat_inv = pbc_case['op'].lat_and_inv
+    i, d0 = 21, 30
+    R = pbc_case['R'][i : i + 1]
+    d, c = pc._pair_frac(R, lat_inv)
+    d = d - np.einsum('ij,...j->...i', lat, np.around(c))
+    d[0, d0] += lat[:, 0]
+    dist = np.sqrt(np.sum(d * d, axis=-1))
+    E_i, F_i = _predict_desc(pbc_case['model'], 1 / dist, d / (dist ** 3)[..., None])
+    E, F = pbc_case['E'].copy(), pbc_case['F'].copy()
+    E[i], F[i] = E_i[0], F_i[0]
+    _fails(pbc_case, E, F, 'force entries')
+
+
+def test_desc_pbc_bound(pbc_case):
+    """The descriptor bound passes the np.longdouble evaluation with margin and fails a one-ulp-scale shift of the
+    cell."""
+    lat, lat_inv = pbc_case['op'].lat_and_inv
+    R = pbc_case['R']
+    x, g = odesc.from_R(R, (lat, lat_inv))
+    xl, gl = _longdouble_desc(R, lat)
+    bx, bg = pc.desc_pbc_bound(R, lat, lat_inv)
+    assert np.all(np.abs(x - xl) <= bx / 10) and np.all(np.abs(g - gl) <= bg[..., None] / 10)
+    x2, g2 = odesc.from_R(R, (lat * (1 + 1e-12), lat_inv))
+    assert not np.all(np.abs(g2 - g) <= bg[..., None])

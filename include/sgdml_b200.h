@@ -184,7 +184,7 @@ int sgdml_b200_assemble_ecstr(const double* R_desc, const double* R_d_desc, cons
  * for i in [m_begin, m_end): (m_end - m_begin)(3N + 1) rows of row stride ldk >= n_cols.  K must be a DEVICE
  * pointer.  The force columns (the prefix of the list) of the force rows are exactly what sgdml_b200_assemble_rows
  * writes; every other entry costs one pass over the (row point, column point) pair.  Padding columns (ldk > n_cols)
- * are neither read nor written.  Same limits as sgdml_b200_assemble_ecstr (N <= 128, M <= 65535). */
+ * are neither read nor written.  Same limits as sgdml_b200_assemble_ecstr (N <= 1023, M <= 65535). */
 int sgdml_b200_assemble_ecstr_rows(const double* R_desc, const double* R_d_desc, const int64_t* tril_perms_lin,
                                    int64_t n_atoms, int64_t n_train, int64_t n_perms, double sig,
                                    const int64_t* col_idxs, int64_t n_cols, double scale, int64_t m_begin,
@@ -326,7 +326,8 @@ int sgdml_b200_ozaki_debug(int64_t m, int64_t n, int64_t k, const double* A, int
 /* ---------------------------------------------------------------- launch accounting / profiling
  * Kernel families: 0 predictor main kernel, 1 predictor auxiliary kernels, 2 K assembly,
  * 3 DMMA GEMM (Cholesky trailing update), 4 potf2 diagonal tiles, 5 panel TRSM strips,
- * 6 triangular solves, 7 descriptor kernels, 8 misc.
+ * 6 triangular solves, 7 descriptor kernels, 8 misc, 9 the predictor's finishing kernels for
+ * descriptors longer than 25,600 entries (N >= 227 atoms; shorter ones finish under family 1).
  * `launches` counts kernel launches per family since the last reset (always on).  With
  * profiling enabled, the library brackets each family's launches with CUDA events on the
  * launching stream and accumulates the device time (this synchronises; benchmarks enable it

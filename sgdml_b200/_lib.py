@@ -206,7 +206,8 @@ def require_gpu():
         raise EngineError('sgdml_b200: no CUDA device visible; this engine has no CPU fallback')
 
 
-KERNEL_FAMILIES = ['predict_main', 'predict_aux', 'assemble', 'gemm', 'potf2', 'trsm', 'trsv', 'desc', 'misc']
+KERNEL_FAMILIES = ['predict_main', 'predict_aux', 'assemble', 'gemm', 'potf2', 'trsm', 'trsv', 'desc', 'misc',
+                   'predict_finish']
 
 
 def profile_snapshot():

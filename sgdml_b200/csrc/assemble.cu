@@ -1080,7 +1080,8 @@ __global__ void __launch_bounds__(256, 2)
 // The per-pair part, shared by k_assemble_ecstr and k_assemble_ecstr_rows: for the pair (i, j) returns r[b] of
 // atom b = threadIdx.x of point j in (r0, r1, r2) and, in thread 0, the sum over permutations of the K_ee terms in
 // kee (the matrix entry is -scale * kee).  Block-wide:
-// every thread of the CTA calls it; red holds one double per warp (blockDim.x <= 128).
+// every thread of the CTA calls it; red holds one double per warp (blockDim.x = N rounded up to a warp multiple, so
+// up to 32 warps at the assembly's bound of N <= 1023; the order of every sum depends only on N).
 __device__ __forceinline__ void ecstr_pair(const double* __restrict__ xi, const double* __restrict__ xj,
                                            const double* __restrict__ gj, const int* __restrict__ aperm_inv, int N,
                                            int S, double sig, double* red, double& s_cp, double& s_kee, double& r0,
@@ -1129,10 +1130,10 @@ __device__ __forceinline__ void ecstr_pair(const double* __restrict__ xi, const 
   }
 }
 
-__global__ void __launch_bounds__(128) k_assemble_ecstr(const double* __restrict__ R_desc, const double* __restrict__ R_d_desc,
-                                                       const int* __restrict__ aperm_inv, int N, int D, int M, int S,
-                                                       double sig, double scale, double* __restrict__ K, int64_t ldk) {
-  __shared__ double red[4];
+__global__ void __launch_bounds__(1024) k_assemble_ecstr(const double* __restrict__ R_desc, const double* __restrict__ R_d_desc,
+                                                        const int* __restrict__ aperm_inv, int N, int D, int M, int S,
+                                                        double sig, double scale, double* __restrict__ K, int64_t ldk) {
+  __shared__ double red[32];
   __shared__ double s_cp, s_kee;
   const int i = blockIdx.y, j = blockIdx.x;
   const int b = threadIdx.x;  // atom of point j (blockDim.x = N rounded up to a warp multiple)
@@ -1160,14 +1161,14 @@ __global__ void __launch_bounds__(128) k_assemble_ecstr(const double* __restrict
 // the force rows of a (r) and the energy row of a (K_ee) in that column -- or the selected force columns of point q
 // (dst = -1 - t, fdest[t*3N + k] = output column of component k or -1) -- the pair (a, q) gives the energy row of a
 // in them.  Force rows come first in K (n_rowpts * 3N of them), then one energy row per row point.
-__global__ void __launch_bounds__(128) k_assemble_ecstr_rows(const double* __restrict__ R_desc,
-                                                            const double* __restrict__ R_d_desc,
-                                                            const int* __restrict__ aperm_inv, int N, int D, int S,
-                                                            double sig, double scale, const int* __restrict__ item_pt,
-                                                            const int64_t* __restrict__ item_dst,
-                                                            const int64_t* __restrict__ fdest, int m_begin,
-                                                            int64_t n_frows, double* __restrict__ K, int64_t ldk) {
-  __shared__ double red[4];
+__global__ void __launch_bounds__(1024) k_assemble_ecstr_rows(const double* __restrict__ R_desc,
+                                                             const double* __restrict__ R_d_desc,
+                                                             const int* __restrict__ aperm_inv, int N, int D, int S,
+                                                             double sig, double scale, const int* __restrict__ item_pt,
+                                                             const int64_t* __restrict__ item_dst,
+                                                             const int64_t* __restrict__ fdest, int m_begin,
+                                                             int64_t n_frows, double* __restrict__ K, int64_t ldk) {
+  __shared__ double red[32];
   __shared__ double s_cp, s_kee;
   const int a = m_begin + (int)blockIdx.y, q = item_pt[blockIdx.x];
   const int64_t dst = item_dst[blockIdx.x];
@@ -1194,6 +1195,9 @@ __global__ void __launch_bounds__(128) k_assemble_ecstr_rows(const double* __res
     if (d3[2] >= 0) rowE[d3[2]] = scale * r2;
   }
 }
+
+// bound on the slabs of k_assemble_large, one per persistent CTA (sgdml_b200_assemble_rows)
+constexpr size_t ASM_SLAB_BYTES_MAX = (size_t)2 << 30;
 
 static size_t asm_large_slab_doubles(int N, int S) {
   const size_t N3 = 3 * (size_t)N, NN = (size_t)N * N;
@@ -1496,10 +1500,13 @@ extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_
       SG_CUDA(cudaGetDevice(&dev));
       SG_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
       const int64_t n_work = (int64_t)n_rowpts * nJ;
-      const int n_cta = (int)std::min<int64_t>(n_work, 2 * (int64_t)n_sm);  // persistent, 2 per SM
       const size_t dl_bytes = sizeof(double) * (size_t)N * N;
       const int dl_in_smem = dl_bytes <= 100 * 1024 ? 1 : 0;  // two CTAs per SM keep their delta tables on chip
       const size_t slab = (asm_large_slab_doubles(N, S) + 1) / 2 * 2;
+      // persistent, 2 per SM; fewer once the slabs (kept in a workspace until sgdml_b200_release_workspaces) would pass
+      // ASM_SLAB_BYTES_MAX: on 132 SMs from N ~ 335 at S = 3 (214 CTAs of 10 MB at N = 370); C60 takes 0.3 GB
+      const int64_t slab_ctas = std::max<int64_t>(1, (int64_t)(ASM_SLAB_BYTES_MAX / (sizeof(double) * slab)));
+      const int n_cta = (int)std::min<int64_t>(std::min<int64_t>(n_work, 2 * (int64_t)n_sm), slab_ctas);
       SG_TRY(ws_get(WS_ASM_SLABS, sizeof(double) * slab * (size_t)n_cta, (void**)&d_slabs));
       if (dl_in_smem)
         SG_CUDA(cudaFuncSetAttribute(k_assemble_large, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dl_bytes));
@@ -1556,7 +1563,7 @@ extern "C" int sgdml_b200_assemble_ecstr(const double* R_desc, const double* R_d
                                          double* K, int64_t ldk, void* stream) {
   SG_TRY(require_device());
   SG_ARG(R_desc != nullptr && R_d_desc != nullptr && tril_perms_lin != nullptr && K != nullptr);
-  SG_ARG(n_atoms >= 2 && n_atoms <= 128 && n_train >= 1 && n_train <= 65535 && n_perms >= 1 && sig > 0);
+  SG_ARG(n_atoms >= 2 && n_atoms <= 1023 && n_train >= 1 && n_train <= 65535 && n_perms >= 1 && sig > 0);
   const int N = (int)n_atoms, M = (int)n_train, S = (int)n_perms;
   const int D = N * (N - 1) / 2;
   const int64_t nt = (int64_t)M * 3 * N + M;
@@ -1594,7 +1601,7 @@ extern "C" int sgdml_b200_assemble_ecstr_rows(const double* R_desc, const double
                                               void* stream) {
   SG_TRY(require_device());
   SG_ARG(R_desc != nullptr && R_d_desc != nullptr && tril_perms_lin != nullptr && col_idxs != nullptr && K != nullptr);
-  SG_ARG(n_atoms >= 2 && n_atoms <= 128 && n_train >= 1 && n_train <= 65535 && n_perms >= 1 && sig > 0);
+  SG_ARG(n_atoms >= 2 && n_atoms <= 1023 && n_train >= 1 && n_train <= 65535 && n_perms >= 1 && sig > 0);
   SG_ARG(m_begin >= 0 && m_begin < m_end && m_end <= n_train);
   const int N = (int)n_atoms, M = (int)n_train, S = (int)n_perms;
   const int D = N * (N - 1) / 2, N3 = 3 * N;

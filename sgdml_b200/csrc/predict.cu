@@ -881,6 +881,122 @@ __global__ void __launch_bounds__(1024) k_predict_finish_small(const double* __r
   }
 }
 
+// ============================================================== finishing path for long descriptors
+// From D > 25,600 (N >= 227 atoms) the F_desc of one query no longer fits the shared memory of k_predict_finish; it goes
+// to a device workspace Fd (n_geo x D) between two kernels:
+//   k_fdesc_gather:  Fd[b][d] = sum_p sum_split G[b*S+p][perm_p[d]]   (the summation order of k_predict_finish)
+//   k_fdesc_project: F = J_x^T Fd * std, E = sum Erow * std + c
+// Both are HBM-bound (S*DP*8 bytes of G, 3*D*8 of gq and 2*D*8 of Fd per query) and use no atomics: fixed order, so the
+// results are bit-identical run to run and between graph replay and plain launches.
+//
+// k_fdesc_gather: one thread per descriptor entry, grid x = entry tiles of one query, y = queries.  The blocks in flight
+// cover the S rows of a few queries (S*DP*8 bytes each, 1.6 MB at N = 370, S = 3), so the permuted reads (scattered only
+// where an atom permutation breaks up runs of consecutive pairs; the identity is read in order) hit L2 and HBM delivers
+// every sector of G once.
+__global__ void __launch_bounds__(256) k_fdesc_gather(const double* __restrict__ G, const int* __restrict__ perm, int D,
+                                                      int DP, int S, int n_splits, int64_t plane_rows, int64_t n_geo,
+                                                      double* __restrict__ Fd) {
+  const int d = blockIdx.x * blockDim.x + threadIdx.x;
+  if (d >= D) return;
+  const int64_t stride = plane_rows * DP;
+  for (int64_t b = blockIdx.y; b < n_geo; b += gridDim.y) {
+    double acc0 = 0.0, acc1 = 0.0, acc2 = 0.0, acc3 = 0.0;
+    for (int pp = 0; pp < S; ++pp) {
+      const double* gp = G + (b * S + pp) * DP + perm[pp * D + d];
+      int sp = 0;
+      for (; sp + 4 <= n_splits; sp += 4) {
+        acc0 += gp[(int64_t)sp * stride];
+        acc1 += gp[(int64_t)(sp + 1) * stride];
+        acc2 += gp[(int64_t)(sp + 2) * stride];
+        acc3 += gp[(int64_t)(sp + 3) * stride];
+      }
+      for (; sp < n_splits; ++sp) acc0 += gp[(int64_t)sp * stride];
+    }
+    Fd[b * D + d] = (acc0 + acc1) + (acc2 + acc3);
+  }
+}
+
+// k_fdesc_project: one CTA (8 warps) per group of 32 atoms k0..k0+31 of one query; lane l owns atom k0 + l.
+//   F[k] = sum_{o > k} g(o,k) Fd(o,k) - sum_{o < k} g(k,o) Fd(k,o)     (the signs of k_predict_finish)
+// Column part (o > k): for each o the 32 entries (o, k0..k0+31) are consecutive, so a warp reads 32 Fd values and
+// 96 gq values in one piece; the o are dealt round-robin to the warps.  Row part (o < k): entries (k, 0..k-1) are
+// consecutive; one warp per atom, lanes over o.  Each entry is read by two CTAs of the same query, which run side by
+// side (grid x = atom groups), so the second read comes from L2.
+constexpr int FDP_WARPS = 8;
+__global__ void __launch_bounds__(FDP_WARPS * 32) k_fdesc_project(const double* __restrict__ Fd, const double* __restrict__ gq,
+                                                                  const double* __restrict__ Erow, int n_atoms, int D,
+                                                                  int S, double std, double c, int n_splits,
+                                                                  int64_t plane_rows, int64_t n_geo,
+                                                                  double* __restrict__ E, double* __restrict__ F) {
+  __shared__ double col[FDP_WARPS][32][3];
+  __shared__ double row[32][3];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int k0 = blockIdx.x * 32;
+  const int k = k0 + lane;
+  const int dimi = 3 * n_atoms;
+  for (int64_t b = blockIdx.y; b < n_geo; b += gridDim.y) {
+    const double* f = Fd + b * D;
+    const double* g = gq + b * (int64_t)D * 3;
+    double c0 = 0.0, c1 = 0.0, c2 = 0.0;
+    for (int o = k0 + 1 + warp; o < n_atoms; o += FDP_WARPS) {
+      if (k < o) {
+        const int d = pair_index(o, k);
+        const double fv = f[d];
+        c0 += g[d * 3 + 0] * fv;
+        c1 += g[d * 3 + 1] * fv;
+        c2 += g[d * 3 + 2] * fv;
+      }
+    }
+    col[warp][lane][0] = c0;
+    col[warp][lane][1] = c1;
+    col[warp][lane][2] = c2;
+    for (int kl = warp; kl < 32; kl += FDP_WARPS) {
+      const int ka = k0 + kl;
+      double r0 = 0.0, r1 = 0.0, r2 = 0.0;
+      if (ka < n_atoms) {
+        const int base = pair_index(ka, 0);
+        for (int o = lane; o < ka; o += 32) {
+          const double fv = f[base + o];
+          r0 += g[(base + o) * 3 + 0] * fv;
+          r1 += g[(base + o) * 3 + 1] * fv;
+          r2 += g[(base + o) * 3 + 2] * fv;
+        }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        r0 += __shfl_xor_sync(0xffffffffu, r0, o);
+        r1 += __shfl_xor_sync(0xffffffffu, r1, o);
+        r2 += __shfl_xor_sync(0xffffffffu, r2, o);
+      }
+      if (lane == 0) {
+        row[kl][0] = r0;
+        row[kl][1] = r1;
+        row[kl][2] = r2;
+      }
+    }
+    __syncthreads();
+    if (threadIdx.x < 96) {
+      const int kl = threadIdx.x / 3, cc = threadIdx.x - 3 * kl;
+      if (k0 + kl < n_atoms) {
+        double s = 0.0;
+        for (int w = 0; w < FDP_WARPS; ++w) s += col[w][kl][cc];
+        F[b * dimi + 3 * (k0 + kl) + cc] = (s - row[kl][cc]) * std;
+      }
+    }
+    if (E != nullptr && blockIdx.x == 0 && warp == FDP_WARPS - 1) {
+      double s = 0.0;
+      for (int t = lane; t < n_splits * S; t += 32) {
+        const int sp = t / S, pp = t - sp * S;
+        s += Erow[(int64_t)sp * plane_rows + b * S + pp];
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      if (lane == 0) E[b] = s * std + c;
+    }
+    __syncthreads();  // col / row are rewritten for the next query
+  }
+}
+
 // ============================================================== model maintenance kernels
 __global__ void k_col_mean(const double* __restrict__ X, int M, int D, double* __restrict__ mu, int DP) {
   // one block per column
@@ -983,6 +1099,7 @@ struct sgdml_b200_model {
     int64_t geo = 0;
     double *xq = nullptr, *gq = nullptr, *G = nullptr, *Erow = nullptr, *R = nullptr, *E = nullptr, *F = nullptr,
            *Qg = nullptr, *qq = nullptr, *S1 = nullptr, *S2 = nullptr, *csum = nullptr;
+    double* Fd = nullptr;       // (geo, D) F_desc of long descriptors (fdesc_in_ws)
     OzOperand ozQ, ozC1, ozC2;  // slices of the per-batch operands (int8 path of large descriptors)
   } ws[2];
   cudaStream_t pipe_stream[2] = {nullptr, nullptr};
@@ -1091,9 +1208,14 @@ void free_ws(sgdml_b200_model* m) {
     cached_free(w.S1);
     cached_free(w.S2);
     cached_free(w.csum);
+    cached_free(w.Fd);
     w = sgdml_b200_model::WS();
   }
 }
+
+// F_desc of one query beyond the shared memory of k_predict_finish (D > 25,600, N >= 227 atoms): the finishing path
+// k_fdesc_gather / k_fdesc_project with the workspace w.Fd
+bool fdesc_in_ws(const sgdml_b200_model* m) { return sizeof(double) * (size_t)m->D > 200 * 1024; }
 
 int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
   sgdml_b200_model::WS& w = m->ws[slot];
@@ -1119,6 +1241,7 @@ int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
   cached_free(w.S1);
   cached_free(w.S2);
   cached_free(w.csum);
+  cached_free(w.Fd);
   w = sgdml_b200_model::WS();
   SG_CUDA(cached_malloc(&w.xq, sizeof(double) * n_geo * m->D));
   SG_CUDA(cached_malloc(&w.gq, sizeof(double) * n_geo * m->D * 3));
@@ -1131,6 +1254,8 @@ int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
   SG_CUDA(cached_malloc(&w.R, sizeof(double) * n_geo * 3 * m->N));
   SG_CUDA(cached_malloc(&w.E, sizeof(double) * n_geo));
   SG_CUDA(cached_malloc(&w.F, sizeof(double) * n_geo * 3 * m->N));
+  // n_geo * D * 8 bytes: at most 1/S of G, which chunk_geos bounds
+  if (fdesc_in_ws(m)) SG_CUDA(cached_malloc(&w.Fd, sizeof(double) * n_geo * m->D));
   {
     const int64_t rows_pad = (n_geo * m->S + m->BQ - 1) / m->BQ * m->BQ;
     SG_CUDA(cached_malloc(&w.Qg, sizeof(double) * rows_pad * m->DS));
@@ -1288,17 +1413,24 @@ int run_queries(sgdml_b200_model* m, int slot, const double* xq, const double* g
     SG_TRY(launch_main(m->cfg, a, n_splits, s));
     count_launch(KID_PREDICT_MAIN);
   }
+  if (fdesc_in_ws(m)) {
+    ProfScope ps(KID_PREDICT_FINISH, s);
+    const unsigned gy = (unsigned)std::min<int64_t>(n_geo, 65535);
+    k_fdesc_gather<<<dim3((unsigned)ceil_div(m->D, 256), gy), 256, 0, s>>>(w.G, m->perm, m->D, m->DP, m->S, n_splits,
+                                                                         n_rows_pad, n_geo, w.Fd);
+    SG_CUDA(cudaGetLastError());
+    k_fdesc_project<<<dim3((unsigned)ceil_div(m->N, 32), gy), FDP_WARPS * 32, 0, s>>>(
+        w.Fd, gq, w.Erow, m->N, m->D, m->S, std, c, n_splits, n_rows_pad, n_geo, E_dev, F_dev);
+    SG_CUDA(cudaGetLastError());
+    count_launch(KID_PREDICT_FINISH, 2);
+    return 0;
+  }
   {
     ProfScope ps(KID_PREDICT_AUX, s);
     const int QPB = std::max(1, 128 / m->D);  // small molecules: several queries per CTA
     const size_t fd_bytes = sizeof(double) * (size_t)m->D * QPB;
-    if (fd_bytes > 48 * 1024) {  // molecules above 111 atoms: opt in to more than the default dynamic shared memory
-      if (fd_bytes > 200 * 1024) {
-        set_last_error("sgdml_b200_predict: descriptor too long for the finishing kernel (n_atoms <= ~225 supported)");
-        return SGDML_B200_ERR_UNSUPPORTED;
-      }
+    if (fd_bytes > 48 * 1024)  // molecules above 111 atoms: opt in to more than the default dynamic shared memory
       SG_CUDA(cudaFuncSetAttribute(k_predict_finish, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fd_bytes));
-    }
     const int parts = std::max(1, std::min(8, 1024 / m->D));
     const size_t fds_bytes = sizeof(double) * (size_t)m->D * (parts + 1);
     if (n_geo <= GRAPH_MAX_GEO && n_splits > 1 && parts > 1 && fds_bytes <= 48 * 1024) {

@@ -18,6 +18,7 @@
 // One CTA owns row point i and a tile of TJ column points; the per-(j,p) vectors are staged in
 // shared memory; each thread then owns 3x3 atom-pair sub-blocks and writes them once.
 #include <algorithm>
+#include <numeric>
 
 #include "common.cuh"
 #include "desc.cuh"
@@ -1196,8 +1197,9 @@ __global__ void __launch_bounds__(1024) k_assemble_ecstr_rows(const double* __re
   }
 }
 
-// bound on the slabs of k_assemble_large, one per persistent CTA (sgdml_b200_assemble_rows)
+// bound on the slabs of k_assemble_large, one per persistent CTA (asm_plan)
 constexpr size_t ASM_SLAB_BYTES_MAX = (size_t)2 << 30;
+constexpr int ASM_TILES_PER_CTA = 4;  // column tiles walked by one CTA of k_assemble_v4 / k_assemble_v5
 
 static size_t asm_large_slab_doubles(int N, int S) {
   const size_t N3 = 3 * (size_t)N, NN = (size_t)N * N;
@@ -1216,11 +1218,113 @@ static size_t asm_v5_smem_bytes(int N, int S, int TJ, int PG) {
   return dbl * 8 + ((size_t)TJ * N + TJ) * 4 + 2 * (size_t)S * N + 16;
 }
 
-static size_t asm_smem_bytes(int N, int D, int S, int TJ) {
-  (void)D;
+static size_t asm_smem_bytes(int N, int S, int TJ) {
   const size_t N3 = 3 * (size_t)N, NN = (size_t)N * N;
   size_t dbl = NN * 3 + NN + (size_t)TJ * (NN * 3 + NN + NN + 2 * N3 + 3 * N3) + (size_t)S * TJ * 2 + (size_t)TJ * 8;
   return dbl * 8 + 2 * (size_t)S * N * 4 + 2 * (size_t)TJ * N * 4 + (size_t)TJ * 4 + 16;
+}
+
+// Test and tuning hooks of the force-force assembly (sgdml_b200_set_assemble_variant).
+struct AsmHooks {
+  bool force_large = false;  // variant 1: k_assemble_large for every size
+  int kernel = 0;            // 0: by size; 2, 4, 5: k_assemble, k_assemble_v4, k_assemble_v5 where it fits
+  int max_rowpts = 65535;    // row points per launch of the grid.y kernels: the grid.y limit (1000 + r lowers it)
+};
+
+enum AsmKernel { ASM_K = 0, ASM_V4 = 1, ASM_V5 = 2, ASM_LARGE = 3 };
+
+struct AsmPlan {
+  AsmKernel kernel = ASM_LARGE;
+  int TJ = 1;               // column points per tile
+  int PG = 0;               // permutations per chunk (v4, v5)
+  int n_chunks = 1;         // grid.z: the sub-blocks of one column point split over CTAs
+  int grid_x = 0;           // column tiles (k_assemble), groups of ASM_TILES_PER_CTA tiles (v4, v5), CTAs (large)
+  size_t smem = 0;          // dynamic shared memory per CTA
+  int sym = 0;              // compute the upper block triangle only and mirror it
+  int rows_per_launch = 0;  // grid.y; k_assemble_large takes every row point in one launch
+  size_t slab = 0;          // k_assemble_large: doubles per CTA slab
+  int dl_in_smem = 0;       // k_assemble_large: the delta table sits in shared memory
+};
+
+// How one force-force assembly call runs (N atoms, S permutations, nJ column points with at most NK kept column atoms
+// each, n_rowpts row points; `square`: every row point and no column list; n_sm SMs).  Shared memory per CTA: 110 KB
+// keeps two CTAs on an SM, 220 KB one.
+//
+//   k_assemble_large  hooks.force_large; else when k_assemble's tables exceed 220 KB at TJ = 1 and v5 does not run
+//   k_assemble_v5     hooks.kernel 5, or 0 where k_assemble_large would run; N <= 255, 220 KB at PG >= 4 or PG = S
+//   k_assemble_v4     hooks.kernel 0 or 4; N <= 255, 220 KB
+//   k_assemble        otherwise (hooks.kernel 2; 4 or 5 where theirs do not fit)
+//
+// TJ is 1 for k_assemble_large and v5 (grid.z splits v5's N NK sub-blocks, 1024 per CTA); v4 and k_assemble take the
+// largest TJ <= 8 with TJ N^2 <= 1024 sub-blocks and k_assemble's tables within 110 KB, else TJ = 1 with the same
+// grid.z split; TJ <= nJ.  PG (v4, v5): the most permutations per chunk, up to 16, that fit.  The grid.y kernels
+// mirror blocks (sym) only when every row point is in one launch.
+static AsmPlan asm_plan(int N, int S, int NK, int nJ, int n_rowpts, bool square, const AsmHooks& hooks, int n_sm) {
+  constexpr size_t KB = 1024;
+  AsmPlan p;
+  p.rows_per_launch = hooks.max_rowpts;
+  p.sym = square && n_rowpts <= hooks.max_rowpts;  // the mirrored store addresses absolute row points
+  const int z_chunks = ceil_div((int64_t)N * NK, ASM_NI * 256);
+  if (!hooks.force_large) {
+    int TJ = 0;
+    for (int t = 8; t >= 1; --t)
+      if ((int64_t)t * N * N <= (int64_t)ASM_NI * 256 && asm_smem_bytes(N, S, t) <= 110 * KB) {
+        TJ = t;
+        break;
+      }
+    const bool small_fits = TJ > 0 || asm_smem_bytes(N, S, 1) <= 220 * KB;
+    int PG5 = std::min(S, 16);
+    while (PG5 > 1 && asm_v5_smem_bytes(N, S, 1, PG5) > 220 * KB) --PG5;
+    const bool fits5 = N <= 255 && asm_v5_smem_bytes(N, S, 1, PG5) <= 220 * KB && (PG5 >= 4 || PG5 == S);
+    if (fits5 && (hooks.kernel == 5 || (hooks.kernel == 0 && !small_fits))) {
+      p.kernel = ASM_V5;
+      p.PG = PG5;
+      p.n_chunks = z_chunks;
+      p.smem = asm_v5_smem_bytes(N, S, 1, PG5);
+      p.grid_x = ceil_div(nJ, ASM_TILES_PER_CTA);
+      return p;
+    }
+    if (small_fits) {
+      if (TJ == 0) {  // one column point per CTA, its sub-blocks split over grid.z
+        TJ = 1;
+        p.n_chunks = z_chunks;
+      }
+      p.TJ = TJ = std::min(TJ, nJ);
+      int PG4 = std::min(S, 16);
+      while (PG4 > 1 && (asm_v4_smem_bytes(N, S, TJ, PG4) > 220 * KB || TJ * PG4 > 256)) --PG4;
+      if (PG4 == S && asm_v4_smem_bytes(N, S, TJ, PG4) > 110 * KB) {  // chunks of >= 8 for two CTAs per SM
+        int q = PG4;
+        while (q > 8 && asm_v4_smem_bytes(N, S, TJ, q) > 110 * KB) --q;
+        if (asm_v4_smem_bytes(N, S, TJ, q) <= 110 * KB) PG4 = q;
+      }
+      const size_t smem4 = asm_v4_smem_bytes(N, S, TJ, PG4);
+      // chosen by timing the variants (tools/asm_variants.py) at BASELINE config 2 (full matrix) and on the Ac-Ala3
+      // shape (S = 243, random column subsets): v4 was the fastest on both
+      if (N <= 255 && smem4 <= 220 * KB && TJ * PG4 <= 256 && (hooks.kernel == 0 || hooks.kernel == 4)) {
+        p.kernel = ASM_V4;
+        p.PG = PG4;
+        p.smem = smem4;
+        p.grid_x = ceil_div(ceil_div(nJ, TJ), ASM_TILES_PER_CTA);
+      } else {
+        p.kernel = ASM_K;
+        p.smem = asm_smem_bytes(N, S, TJ);
+        p.grid_x = ceil_div(nJ, TJ);
+      }
+      return p;
+    }
+  }
+  p.kernel = ASM_LARGE;
+  p.sym = 0;
+  p.rows_per_launch = n_rowpts;
+  const size_t dl_bytes = sizeof(double) * (size_t)N * N;
+  p.dl_in_smem = dl_bytes <= 100 * KB ? 1 : 0;  // two CTAs per SM keep their delta tables on chip
+  p.smem = p.dl_in_smem ? dl_bytes : 0;
+  p.slab = (asm_large_slab_doubles(N, S) + 1) / 2 * 2;
+  // persistent, 2 per SM; fewer once the slabs (kept in a workspace until sgdml_b200_release_workspaces) would pass
+  // ASM_SLAB_BYTES_MAX: on 132 SMs from N ~ 335 at S = 3 (214 CTAs of 10 MB at N = 370); C60 takes 0.3 GB
+  const int64_t slab_ctas = std::max<int64_t>(1, (int64_t)(ASM_SLAB_BYTES_MAX / (sizeof(double) * p.slab)));
+  p.grid_x = (int)std::min<int64_t>(std::min<int64_t>((int64_t)n_rowpts * nJ, 2 * (int64_t)n_sm), slab_ctas);
+  return p;
 }
 
 }  // namespace sgdml
@@ -1230,25 +1334,18 @@ using namespace sgdml;
 // Recovers the atom permutation P that induces a descriptor permutation (dperm[d(a,b)] =
 // d(P a, P b)); returns false if dperm is not induced by any atom permutation.
 static bool atom_perm_from_desc_perm(const int* dperm, int N, int* P) {
-  const int D = N * (N - 1) / 2;
+  auto d_of = [](int x, int y) { return x > y ? pair_index(x, y) : pair_index(y, x); };
   if (N == 2) {
     P[0] = 0;
     P[1] = 1;
     return dperm[0] == 0;
   }
   for (int a = 0; a < N; ++a) {
-    // two pairs containing a
-    int o1 = (a == 0) ? 1 : 0, o2 = -1;
-    for (int o = 0; o < N; ++o)
-      if (o != a && o != o1) {
-        o2 = o;
-        break;
-      }
-    auto d_of = [](int x, int y) { return x > y ? x * (x - 1) / 2 + y : y * (y - 1) / 2 + x; };
-    int e1 = dperm[d_of(a, o1)], e2 = dperm[d_of(a, o2)];
+    // P a is the atom that the images of two pairs containing a have in common
+    const int o1 = a == 0 ? 1 : 0, o2 = a < 2 ? 2 : 1;
     int a1, b1, a2, b2;
-    pair_from_d(e1, a1, b1);
-    pair_from_d(e2, a2, b2);
+    pair_from_d(dperm[d_of(a, o1)], a1, b1);
+    pair_from_d(dperm[d_of(a, o2)], a2, b2);
     int common = -1;
     if (a1 == a2 || a1 == b2) common = a1;
     if (b1 == a2 || b1 == b2) common = (common == -1) ? b1 : -2;
@@ -1262,33 +1359,96 @@ static bool atom_perm_from_desc_perm(const int* dperm, int N, int* P) {
     seen[(size_t)P[a]] = 1;
   }
   for (int a = 1; a < N; ++a)
-    for (int b = 0; b < a; ++b) {
-      int pa = P[a], pb = P[b];
-      int e = pa > pb ? pa * (pa - 1) / 2 + pb : pb * (pb - 1) / 2 + pa;
-      if (dperm[a * (a - 1) / 2 + b] != e) return false;
-    }
-  (void)D;
+    for (int b = 0; b < a; ++b)
+      if (dperm[pair_index(a, b)] != d_of(P[a], P[b])) return false;
   return true;
 }
 
-static int g_asm_variant = 0;  // 0: by size; 1: always the large-molecule kernel (tests)
-static int g_asm_kernel = 0;  // small-molecule kernel: 0 = by size (default), 2 = k_assemble (per-permutation phases), 4 = k_assemble_v4 (chunked), 5 = k_assemble_v5 (chunked, compressed pair arrays)
-static int g_asm_max_rowpts = 65535;  // row points per launch of k_assemble (grid.y limit; lowered by tests)
+// The permutation tables of tril_perms_lin (D x S, entry d S + p = p D + perm_p[d]): descriptor permutations dperm
+// (S x D), the atom permutations aperm (S x N) that induce them and their inverses apinv (S x N).
+struct PermTables {
+  std::vector<int> dperm, aperm, apinv;
+};
+
+static int perm_tables(const int64_t* tril_perms_lin, int N, int S, PermTables& t) {
+  const int D = N * (N - 1) / 2;
+  std::vector<int64_t> lin;
+  SG_TRY(read_int64s(tril_perms_lin, (size_t)S * D, lin));
+  t.dperm.resize((size_t)S * D);
+  t.aperm.resize((size_t)S * N);
+  t.apinv.resize((size_t)S * N);
+  for (int pp = 0; pp < S; ++pp) {
+    for (int d = 0; d < D; ++d) {
+      const int64_t e = lin[(size_t)d * S + pp] - (int64_t)pp * D;
+      SG_ARG(e >= 0 && e < D);
+      t.dperm[(size_t)pp * D + d] = (int)e;
+    }
+    if (!atom_perm_from_desc_perm(&t.dperm[(size_t)pp * D], N, &t.aperm[(size_t)pp * N]))
+      return fail_arg("tril_perms_lin is not induced by atom permutations (utils/desc.py:509-539)");
+    for (int a = 0; a < N; ++a) t.apinv[(size_t)pp * N + t.aperm[(size_t)pp * N + a]] = a;
+  }
+  return 0;
+}
+
+// Reads a column list and checks that it is sorted ascending without duplicates and lies in [0, limit).
+static int read_cols(const int64_t* col_idxs, int64_t n_cols, int64_t limit, std::vector<int64_t>& cols) {
+  SG_TRY(read_int64s(col_idxs, (size_t)n_cols, cols));
+  for (size_t c = 0; c < cols.size(); ++c) {
+    SG_ARG(cols[c] >= 0 && cols[c] < limit);
+    if (c > 0 && cols[c] <= cols[c - 1])
+      return fail_arg("col_idxs must be sorted ascending without duplicates (train.py:1341-1345)");
+  }
+  return 0;
+}
+
+// Block-columns of the force columns cols[0, n_fcols) (train.py:1357-1407): appends the column points they touch to
+// pts and, per column point, the output column of each of its 3N components or -1 to dest.  Returns NK, the most
+// column atoms with a kept column in one column point.
+static int block_columns(const std::vector<int64_t>& cols, int64_t n_fcols, int N3, std::vector<int>& pts,
+                         std::vector<int64_t>& dest) {
+  int NK = 0, nk = 0, atom = -1;  // nk: kept column atoms of the current column point so far, atom: the last one
+  for (int64_t c = 0; c < n_fcols; ++c) {
+    const int j = (int)(cols[(size_t)c] / N3), k = (int)(cols[(size_t)c] % N3);
+    if (pts.empty() || pts.back() != j) {
+      pts.push_back(j);
+      dest.insert(dest.end(), (size_t)N3, (int64_t)-1);
+      nk = 0;
+      atom = -1;
+    }
+    if (k / 3 != atom) {
+      atom = k / 3;
+      NK = std::max(NK, ++nk);
+    }
+    dest[(pts.size() - 1) * N3 + k] = c;
+  }
+  return NK;
+}
+
+// Copies a host table into a persistent workspace slot: a cudaMalloc / cudaFree pair per table costs milliseconds once
+// the K buffer and the factorisation workspaces exist.  Every caller synchronises its stream before returning, so the
+// next call's upload cannot overwrite a table a kernel still reads.
+template <class T>
+static int ws_upload(int slot, const std::vector<T>& v, cudaStream_t s, const T** out) {
+  SG_TRY(ws_get(slot, sizeof(T) * v.size(), (void**)out));
+  SG_CUDA(cudaMemcpyAsync((void*)*out, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+static AsmHooks g_asm_hooks;
 
 extern "C" int sgdml_b200_set_assemble_variant(int variant) {
-  // 0 / 1: kernel choice; 1000 + r (test hook): at most r row points per launch of the small-molecule kernel
+  // 0: the defaults; 1: k_assemble_large for every size; 2 / 4 / 5: that small-molecule kernel where it fits;
+  // 1000 + r (test hook): at most r row points per launch of the small-molecule kernels
   if (variant >= 1000) {
     SG_ARG(variant - 1000 >= 1 && variant - 1000 <= 65535);
-    g_asm_max_rowpts = variant - 1000;
-    return 0;
+    g_asm_hooks.max_rowpts = variant - 1000;
+  } else if (variant == 2 || variant == 4 || variant == 5) {
+    g_asm_hooks.kernel = variant;
+  } else {
+    SG_ARG(variant == 0 || variant == 1);
+    g_asm_hooks.force_large = variant == 1;
+    if (variant == 0) g_asm_hooks.kernel = 0;
   }
-  if (variant == 2 || variant == 4 || variant == 5) {  // which small-molecule kernel
-    g_asm_kernel = variant;
-    return 0;
-  }
-  SG_ARG(variant == 0 || variant == 1);
-  g_asm_variant = variant;
-  if (variant == 0) g_asm_kernel = 0;  // back to the defaults
   return 0;
 }
 
@@ -1309,220 +1469,96 @@ extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_
   SG_ARG(n_cols >= 1 && n_cols <= n && ldk >= n_cols);
   cudaStream_t s = (cudaStream_t)stream;
 
-  // ---- integer tables (host)
-  std::vector<int64_t> lin((size_t)S * D);
-  if (is_device_ptr(tril_perms_lin))
-    SG_CUDA(cudaMemcpy(lin.data(), tril_perms_lin, sizeof(int64_t) * lin.size(), cudaMemcpyDeviceToHost));
-  else
-    std::copy(tril_perms_lin, tril_perms_lin + lin.size(), lin.begin());
-  std::vector<int> dperm((size_t)S * D), aperm((size_t)S * N), apinv((size_t)S * N);
-  for (int pp = 0; pp < S; ++pp) {
-    for (int d = 0; d < D; ++d) {
-      const int64_t e = lin[(size_t)d * S + pp] - (int64_t)pp * D;
-      SG_ARG(e >= 0 && e < D);
-      dperm[(size_t)pp * D + d] = (int)e;
-    }
-    if (!atom_perm_from_desc_perm(&dperm[(size_t)pp * D], N, &aperm[(size_t)pp * N]))
-      return fail_arg("tril_perms_lin is not induced by atom permutations (utils/desc.py:509-539)");
-    for (int a = 0; a < N; ++a) apinv[(size_t)pp * N + aperm[(size_t)pp * N + a]] = a;
-  }
-  // block-columns and destination map (train.py:1357-1407)
+  // ---- parse: integer tables (host)
+  PermTables perms;
+  SG_TRY(perm_tables(tril_perms_lin, N, S, perms));
   std::vector<int> jpts;
   std::vector<int64_t> dest;
-  if (col_idxs == nullptr) {
+  // the sub-blocks of a block are dealt out over N * NK (row atom, kept column atom) pairs -- N * N for the full
+  // matrix, far fewer for the column subsets of the Nystroem set-up
+  int NK = N;
+  if (col_idxs == nullptr) {  // every column point, every column at its own index
     jpts.resize((size_t)M);
-    dest.resize((size_t)M * N3);
-    for (int j = 0; j < M; ++j) {
-      jpts[(size_t)j] = j;
-      for (int k = 0; k < N3; ++k) dest[(size_t)j * N3 + k] = (int64_t)j * N3 + k;
-    }
+    dest.resize((size_t)n);
+    std::iota(jpts.begin(), jpts.end(), 0);
+    std::iota(dest.begin(), dest.end(), (int64_t)0);
   } else {
-    std::vector<int64_t> cols((size_t)n_cols);
-    if (is_device_ptr(col_idxs))
-      SG_CUDA(cudaMemcpy(cols.data(), col_idxs, sizeof(int64_t) * cols.size(), cudaMemcpyDeviceToHost));
-    else
-      std::copy(col_idxs, col_idxs + n_cols, cols.begin());
-    for (int64_t c = 0; c < n_cols; ++c) {
-      SG_ARG(cols[(size_t)c] >= 0 && cols[(size_t)c] < n);
-      if (c > 0 && cols[(size_t)c] <= cols[(size_t)c - 1])
-        return fail_arg("col_idxs must be sorted ascending without duplicates (train.py:1341-1345)");
-      const int j = (int)(cols[(size_t)c] / N3), k = (int)(cols[(size_t)c] % N3);
-      if (jpts.empty() || jpts.back() != j) {
-        jpts.push_back(j);
-        dest.insert(dest.end(), (size_t)N3, (int64_t)-1);
-      }
-      dest[(jpts.size() - 1) * N3 + k] = c;
-    }
+    std::vector<int64_t> cols;
+    SG_TRY(read_cols(col_idxs, n_cols, n, cols));
+    NK = block_columns(cols, n_cols, N3, jpts, dest);
   }
   const int nJ = (int)jpts.size();
-  // kept column atoms per column point, at most: the sub-blocks of a block are dealt out over N * NK (row atom, kept
-  // column atom) pairs -- N * N for the full matrix, far fewer for the column subsets of the Nystroem set-up
-  int NK = 1;
-  for (int jt = 0; jt < nJ; ++jt) {
-    int c = 0;
-    for (int b = 0; b < N; ++b) {
-      const int64_t* d3 = &dest[(size_t)jt * N3 + 3 * b];
-      if (d3[0] >= 0 || d3[1] >= 0 || d3[2] >= 0) ++c;
-    }
-    NK = std::max(NK, c);
-  }
-
-  // ---- tile size: at most ASM_NI 3x3 sub-blocks per thread, and shared memory small enough for
-  //      two co-resident CTAs per SM
-  int TJ = 0, n_chunks = 1;
-  bool large = g_asm_variant == 1;
-  for (int t = 8; t >= 1 && !large; --t)
-    if ((int64_t)t * N * N <= (int64_t)ASM_NI * 256 && asm_smem_bytes(N, D, S, t) <= 110 * 1024) {
-      TJ = t;
-      break;
-    }
-  if (TJ == 0 && !large) {
-    // mid-sized molecule: one column point per CTA, its N*N sub-blocks split over grid.z (the
-    // per-permutation vectors are then recomputed by every chunk)
-    TJ = 1;
-    n_chunks = (int)(((int64_t)N * NK + ASM_NI * 256 - 1) / (ASM_NI * 256));
-    if (asm_smem_bytes(N, D, S, 1) > 220 * 1024) large = true;  // tables beyond shared memory: k_assemble_large
-  }
-  // v5 kernel (compressed pair arrays on chip): for molecules whose expanded tables do not fit shared memory, up to
-  // ~64 atoms; one column point per CTA, chunks of up to 16 permutations
-  int PG5 = std::min(S, 16);
-  while (PG5 > 1 && asm_v5_smem_bytes(N, S, 1, PG5) > 220 * 1024) --PG5;
-  const size_t smem5 = asm_v5_smem_bytes(N, S, 1, PG5);
-  const bool fits5 = N <= 255 && smem5 <= 220 * 1024 && (PG5 >= 4 || PG5 == S);
-  const bool use_v5 = g_asm_variant != 1 && fits5 && (g_asm_kernel == 5 || (g_asm_kernel == 0 && large));
-  if (use_v5) {
-    large = false;
-    TJ = 1;
-    n_chunks = (int)(((int64_t)N * NK + ASM_NI * 256 - 1) / (ASM_NI * 256));
-  }
-  if (large) TJ = 1;
-  TJ = std::min(TJ, nJ);
-  const size_t smem = asm_smem_bytes(N, D, S, TJ);
   SG_ARG((int64_t)N * N < (1 << 20) && N < 4096);  // fastdiv range
 
+  // ---- plan
+  const AsmPlan plan = asm_plan(N, S, NK, nJ, n_rowpts, col_idxs == nullptr && n_rowpts == M, g_asm_hooks, num_sms());
+
+  // ---- upload
   Staged sX, sG, sK;
   SG_TRY(sX.init(R_desc, sizeof(double) * (size_t)M * D, true, s));
   SG_TRY(sG.init(R_d_desc, sizeof(double) * (size_t)M * D * 3, true, s));
   const bool K_host = !is_device_ptr(K);
   SG_TRY(sK.init(K, sizeof(double) * (size_t)n_rows * ldk, false, s));
   if (K_host && ldk != n_cols) SG_CUDA(cudaMemsetAsync(sK.dev(), 0, sizeof(double) * (size_t)n_rows * ldk, s));
-
-  int *d_dperm = nullptr, *d_aperm = nullptr, *d_apinv = nullptr, *d_jpts = nullptr;
-  int64_t* d_dest = nullptr;
+  AsmArgs a;
+  SG_TRY(ws_upload(WS_ASM_DPERM, perms.dperm, s, &a.dperm));
+  SG_TRY(ws_upload(WS_ASM_APERM, perms.aperm, s, &a.aperm));
+  SG_TRY(ws_upload(WS_ASM_APINV, perms.apinv, s, &a.apinv));
+  SG_TRY(ws_upload(WS_ASM_JPTS, jpts, s, &a.jpts));
+  SG_TRY(ws_upload(WS_ASM_DEST, dest, s, &a.dest));
   double* d_slabs = nullptr;
-  // the integer tables (and the large-molecule kernel's slabs) live in persistent workspaces: a cudaMalloc / cudaFree
-  // pair per table costs milliseconds once the K buffer and the factorisation workspaces exist
-  auto cleanup = [&]() {};
-  auto body = [&]() -> int {
-    SG_TRY(ws_get(WS_ASM_DPERM, sizeof(int) * dperm.size(), (void**)&d_dperm));
-    SG_TRY(ws_get(WS_ASM_APERM, sizeof(int) * aperm.size(), (void**)&d_aperm));
-    SG_TRY(ws_get(WS_ASM_APINV, sizeof(int) * apinv.size(), (void**)&d_apinv));
-    SG_TRY(ws_get(WS_ASM_JPTS, sizeof(int) * jpts.size(), (void**)&d_jpts));
-    SG_TRY(ws_get(WS_ASM_DEST, sizeof(int64_t) * dest.size(), (void**)&d_dest));
-    SG_CUDA(cudaMemcpyAsync(d_dperm, dperm.data(), sizeof(int) * dperm.size(), cudaMemcpyHostToDevice, s));
-    SG_CUDA(cudaMemcpyAsync(d_aperm, aperm.data(), sizeof(int) * aperm.size(), cudaMemcpyHostToDevice, s));
-    SG_CUDA(cudaMemcpyAsync(d_apinv, apinv.data(), sizeof(int) * apinv.size(), cudaMemcpyHostToDevice, s));
-    SG_CUDA(cudaMemcpyAsync(d_jpts, jpts.data(), sizeof(int) * jpts.size(), cudaMemcpyHostToDevice, s));
-    SG_CUDA(cudaMemcpyAsync(d_dest, dest.data(), sizeof(int64_t) * dest.size(), cudaMemcpyHostToDevice, s));
-    AsmArgs a;
-    a.R_desc = (const double*)sX.dev();
-    a.R_d_desc = (const double*)sG.dev();
-    a.dperm = d_dperm;
-    a.aperm = d_aperm;
-    a.apinv = d_apinv;
-    a.jpts = d_jpts;
-    a.dest = d_dest;
-    a.N = N;
-    a.D = D;
-    a.M = M;
-    a.S = S;
-    a.nJ = nJ;
-    a.TJ = TJ;
-    a.i0 = (int)m_begin;
-    // symmetric mode (upper block triangle computed, lower mirrored) needs every row point in this call
-    a.sym = (col_idxs == nullptr && n_rowpts == M && !large) ? 1 : 0;
-    a.mN = (unsigned)((0x100000000ull + N - 1) / N);
-    a.mNN = (unsigned)((0x100000000ull + (uint64_t)N * N - 1) / ((uint64_t)N * N));
-    a.mPer = (unsigned)((0x100000000ull + 5 * N - 1) / (5 * N));
-    a.NK = NK;
-    a.mNK = (unsigned)((0x100000000ull + NK - 1) / NK);
-    a.mNNK = (unsigned)((0x100000000ull + (uint64_t)N * NK - 1) / ((uint64_t)N * NK));
-    a.sig = sig;
-    a.scale = scale;
-    a.K = (double*)sK.dev();
-    a.ldk = ldk;
-    if (!large) {
-      // rows on grid.y, column tiles on grid.x; grid.y is limited to 65535, so longer row ranges (the
-      // iterative solver assembles K_nm over ALL training points of a rank) run as several launches,
-      // each with its own first row point and K row offset
-      const int max_rows_per_launch = g_asm_max_rowpts;
-      if (n_rowpts > max_rows_per_launch) a.sym = 0;  // the mirrored store addresses absolute row points
-      // v4 kernel: chunks of up to 16 permutations; two CTAs per SM when everything fits in ~110 KB, else one
-      int PG4 = std::min(S, 16);
-      while (PG4 > 1 && (asm_v4_smem_bytes(N, S, TJ, PG4) > 220 * 1024 || TJ * PG4 > 256)) --PG4;
-      if (PG4 == S && asm_v4_smem_bytes(N, S, TJ, PG4) > 110 * 1024) {
-        int q = PG4;
-        while (q > 8 && asm_v4_smem_bytes(N, S, TJ, q) > 110 * 1024) --q;
-        if (asm_v4_smem_bytes(N, S, TJ, q) <= 110 * 1024) PG4 = q;
+  if (plan.kernel == ASM_LARGE)
+    SG_TRY(ws_get(WS_ASM_SLABS, sizeof(double) * plan.slab * (size_t)plan.grid_x, (void**)&d_slabs));
+  a.R_desc = (const double*)sX.dev();
+  a.R_d_desc = (const double*)sG.dev();
+  a.N = N;
+  a.D = D;
+  a.M = M;
+  a.S = S;
+  a.nJ = nJ;
+  a.TJ = plan.TJ;
+  a.sym = plan.sym;
+  a.mN = (unsigned)((0x100000000ull + N - 1) / N);
+  a.mNN = (unsigned)((0x100000000ull + (uint64_t)N * N - 1) / ((uint64_t)N * N));
+  a.mPer = (unsigned)((0x100000000ull + 5 * N - 1) / (5 * N));
+  a.NK = NK;
+  a.mNK = (unsigned)((0x100000000ull + NK - 1) / NK);
+  a.mNNK = (unsigned)((0x100000000ull + (uint64_t)N * NK - 1) / ((uint64_t)N * NK));
+  a.sig = sig;
+  a.scale = scale;
+  a.K = (double*)sK.dev();
+  a.ldk = ldk;
+
+  // ---- launch: rows on grid.y, which is limited to 65535, so longer row ranges (the iterative solver assembles K_nm
+  //      over ALL training points of a rank) run as several launches, each with its own first row point and K row offset
+  const void* const kernel_fn[] = {(const void*)k_assemble, (const void*)k_assemble_v4, (const void*)k_assemble_v5,
+                                   (const void*)k_assemble_large};  // indexed by AsmKernel
+  if (plan.smem > 0)
+    SG_CUDA(cudaFuncSetAttribute(kernel_fn[plan.kernel], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
+  {
+    ProfScope ps(KID_ASSEMBLE, s);
+    for (int r0 = 0; r0 < n_rowpts; r0 += plan.rows_per_launch) {
+      const int nr = std::min(plan.rows_per_launch, n_rowpts - r0);
+      AsmArgs ac = a;
+      ac.i0 = (int)m_begin + r0;
+      ac.K = a.K + (int64_t)r0 * N3 * ldk;
+      const dim3 grid((unsigned)plan.grid_x, (unsigned)nr, (unsigned)plan.n_chunks);
+      switch (plan.kernel) {
+        case ASM_K: k_assemble<<<grid, 256, plan.smem, s>>>(ac); break;
+        case ASM_V4: k_assemble_v4<<<grid, 256, plan.smem, s>>>(ac, plan.PG, ASM_TILES_PER_CTA); break;
+        case ASM_V5: k_assemble_v5<<<grid, 256, plan.smem, s>>>(ac, plan.PG, ASM_TILES_PER_CTA); break;
+        case ASM_LARGE:
+          k_assemble_large<<<plan.grid_x, 256, plan.smem, s>>>(ac, d_slabs, (int64_t)plan.slab, (int64_t)nr * nJ,
+                                                                plan.dl_in_smem);
+          break;
       }
-      const size_t smem4 = asm_v4_smem_bytes(N, S, TJ, PG4);
-      // chosen by timing the variants (tools/asm_variants.py) at BASELINE config 2 (full matrix) and on the Ac-Ala3 shape
-      // (S = 243, random column subsets): v4 was the fastest on both -- v4 is the default
-      const bool use_v4 = N <= 255 && smem4 <= 220 * 1024 && TJ * PG4 <= 256 && (g_asm_kernel == 4 || g_asm_kernel == 0);
-      const int tiles_per_cta = 4;
-      if (use_v5) {
-        SG_CUDA(cudaFuncSetAttribute(k_assemble_v5, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem5));
-      } else if (use_v4) {
-        SG_CUDA(cudaFuncSetAttribute(k_assemble_v4, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4));
-      } else
-        SG_CUDA(cudaFuncSetAttribute(k_assemble, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      ProfScope ps(KID_ASSEMBLE, s);
-      for (int r0 = 0; r0 < n_rowpts; r0 += max_rows_per_launch) {
-        const int nr = std::min(max_rows_per_launch, n_rowpts - r0);
-        AsmArgs ac = a;
-        ac.i0 = (int)m_begin + r0;
-        ac.K = a.K + (int64_t)r0 * N3 * ldk;
-        if (use_v5) {
-          dim3 grid((unsigned)ceil_div(nJ, tiles_per_cta), (unsigned)nr, (unsigned)n_chunks);
-          k_assemble_v5<<<grid, 256, smem5, s>>>(ac, PG5, tiles_per_cta);
-        } else if (use_v4) {
-          dim3 grid((unsigned)ceil_div(ceil_div(nJ, TJ), tiles_per_cta), (unsigned)nr, (unsigned)n_chunks);
-          k_assemble_v4<<<grid, 256, smem4, s>>>(ac, PG4, tiles_per_cta);
-        } else {
-          dim3 grid((unsigned)ceil_div(nJ, TJ), (unsigned)nr, (unsigned)n_chunks);
-          k_assemble<<<grid, 256, smem, s>>>(ac);
-        }
-        SG_CUDA(cudaGetLastError());
-        count_launch(KID_ASSEMBLE);
-      }
-    } else {
-      int dev = 0, n_sm = 0;
-      SG_CUDA(cudaGetDevice(&dev));
-      SG_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-      const int64_t n_work = (int64_t)n_rowpts * nJ;
-      const size_t dl_bytes = sizeof(double) * (size_t)N * N;
-      const int dl_in_smem = dl_bytes <= 100 * 1024 ? 1 : 0;  // two CTAs per SM keep their delta tables on chip
-      const size_t slab = (asm_large_slab_doubles(N, S) + 1) / 2 * 2;
-      // persistent, 2 per SM; fewer once the slabs (kept in a workspace until sgdml_b200_release_workspaces) would pass
-      // ASM_SLAB_BYTES_MAX: on 132 SMs from N ~ 335 at S = 3 (214 CTAs of 10 MB at N = 370); C60 takes 0.3 GB
-      const int64_t slab_ctas = std::max<int64_t>(1, (int64_t)(ASM_SLAB_BYTES_MAX / (sizeof(double) * slab)));
-      const int n_cta = (int)std::min<int64_t>(std::min<int64_t>(n_work, 2 * (int64_t)n_sm), slab_ctas);
-      SG_TRY(ws_get(WS_ASM_SLABS, sizeof(double) * slab * (size_t)n_cta, (void**)&d_slabs));
-      if (dl_in_smem)
-        SG_CUDA(cudaFuncSetAttribute(k_assemble_large, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dl_bytes));
-      ProfScope ps(KID_ASSEMBLE, s);
-      k_assemble_large<<<n_cta, 256, dl_in_smem ? dl_bytes : 0, s>>>(a, d_slabs, (int64_t)slab, n_work, dl_in_smem);
       SG_CUDA(cudaGetLastError());
       count_launch(KID_ASSEMBLE);
     }
-    SG_TRY(sK.finish(s));
-    // the integer tables are read by the kernel: wait before freeing them
-    SG_CUDA(cudaStreamSynchronize(s));
-    return 0;
-  };
-  int rc = body();
-  cleanup();
-  return rc;
+  }
+  SG_TRY(sK.finish(s));
+  SG_CUDA(cudaStreamSynchronize(s));  // the kernels read the table workspaces, which the next call overwrites
+  return 0;
 }
 
 extern "C" int sgdml_b200_assemble(const double* R_desc, const double* R_d_desc, const int64_t* tril_perms_lin,
@@ -1531,29 +1567,6 @@ extern "C" int sgdml_b200_assemble(const double* R_desc, const double* R_d_desc,
                                    void* stream) {
   return sgdml_b200_assemble_rows(R_desc, R_d_desc, tril_perms_lin, n_atoms, n_train, n_perms, sig, col_idxs, n_cols,
                                   scale, 0, n_train, K, ldk, stream);
-}
-
-// Inverse atom permutations (S x N) of tril_perms_lin, the tables of the energy-constraint kernels.
-static int ecstr_apinv(const int64_t* tril_perms_lin, int N, int S, std::vector<int>& apinv) {
-  const int D = N * (N - 1) / 2;
-  std::vector<int64_t> lin((size_t)S * D);
-  if (is_device_ptr(tril_perms_lin))
-    SG_CUDA(cudaMemcpy(lin.data(), tril_perms_lin, sizeof(int64_t) * lin.size(), cudaMemcpyDeviceToHost));
-  else
-    std::copy(tril_perms_lin, tril_perms_lin + lin.size(), lin.begin());
-  std::vector<int> dperm((size_t)D), aperm((size_t)N);
-  apinv.assign((size_t)S * N, 0);
-  for (int pp = 0; pp < S; ++pp) {
-    for (int d = 0; d < D; ++d) {
-      const int64_t e = lin[(size_t)d * S + pp] - (int64_t)pp * D;
-      SG_ARG(e >= 0 && e < D);
-      dperm[(size_t)d] = (int)e;
-    }
-    if (!atom_perm_from_desc_perm(dperm.data(), N, aperm.data()))
-      return fail_arg("tril_perms_lin is not induced by atom permutations (utils/desc.py:509-539)");
-    for (int a = 0; a < N; ++a) apinv[(size_t)pp * N + aperm[(size_t)a]] = a;
-  }
-  return 0;
 }
 
 // GDMLTrain._assemble_kernel_mat(use_E_cstr=True), train.py:234-300: fills the M energy rows and columns (and the
@@ -1569,26 +1582,20 @@ extern "C" int sgdml_b200_assemble_ecstr(const double* R_desc, const double* R_d
   const int64_t nt = (int64_t)M * 3 * N + M;
   SG_ARG(ldk >= nt && is_device_ptr(K));
   cudaStream_t s = (cudaStream_t)stream;
-  std::vector<int> apinv;
-  SG_TRY(ecstr_apinv(tril_perms_lin, N, S, apinv));
+  PermTables perms;
+  SG_TRY(perm_tables(tril_perms_lin, N, S, perms));
   Staged sX, sG;
   SG_TRY(sX.init(R_desc, sizeof(double) * (size_t)M * D, true, s));
   SG_TRY(sG.init(R_d_desc, sizeof(double) * (size_t)M * D * 3, true, s));
-  int* d_apinv = nullptr;
-  SG_CUDA(cudaMalloc(&d_apinv, sizeof(int) * apinv.size()));
-  auto body = [&]() -> int {
-    SG_CUDA(cudaMemcpyAsync(d_apinv, apinv.data(), sizeof(int) * apinv.size(), cudaMemcpyHostToDevice, s));
-    ProfScope ps(KID_ASSEMBLE, s);
-    k_assemble_ecstr<<<dim3((unsigned)M, (unsigned)M), (N + 31) / 32 * 32, 0, s>>>(
-        (const double*)sX.dev(), (const double*)sG.dev(), d_apinv, N, D, M, S, sig, scale, K, ldk);
-    SG_CUDA(cudaGetLastError());
-    count_launch(KID_ASSEMBLE);
-    SG_CUDA(cudaStreamSynchronize(s));
-    return 0;
-  };
-  int rc = body();
-  cudaFree(d_apinv);
-  return rc;
+  const int* d_apinv;
+  SG_TRY(ws_upload(WS_ASM_APINV, perms.apinv, s, &d_apinv));
+  ProfScope ps(KID_ASSEMBLE, s);
+  k_assemble_ecstr<<<dim3((unsigned)M, (unsigned)M), (N + 31) / 32 * 32, 0, s>>>(
+      (const double*)sX.dev(), (const double*)sG.dev(), d_apinv, N, D, M, S, sig, scale, K, ldk);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_ASSEMBLE);
+  SG_CUDA(cudaStreamSynchronize(s));
+  return 0;
 }
 
 // Row block of the energy-constrained K_nm (the Nystroem set-up of iterative.py:232-247 with use_E_cstr): the force
@@ -1608,70 +1615,43 @@ extern "C" int sgdml_b200_assemble_ecstr_rows(const double* R_desc, const double
   const int64_t n = (int64_t)M * N3, nt = n + M;
   SG_ARG(n_cols >= 1 && n_cols <= nt && ldk >= n_cols && is_device_ptr(K));
   cudaStream_t s = (cudaStream_t)stream;
-  std::vector<int64_t> cols((size_t)n_cols);
-  if (is_device_ptr(col_idxs))
-    SG_CUDA(cudaMemcpy(cols.data(), col_idxs, sizeof(int64_t) * cols.size(), cudaMemcpyDeviceToHost));
-  else
-    std::copy(col_idxs, col_idxs + n_cols, cols.begin());
-  int64_t n_fcols = 0;
-  for (int64_t c = 0; c < n_cols; ++c) {
-    SG_ARG(cols[(size_t)c] >= 0 && cols[(size_t)c] < nt);
-    if (c > 0 && cols[(size_t)c] <= cols[(size_t)c - 1])
-      return fail_arg("col_idxs must be sorted ascending without duplicates (train.py:1341-1345)");
-    if (cols[(size_t)c] < n) ++n_fcols;
-  }
-  std::vector<int> apinv;
-  SG_TRY(ecstr_apinv(tril_perms_lin, N, S, apinv));
-  // force rows x force columns: exactly the row block sgdml_b200_assemble_rows writes
+  std::vector<int64_t> cols;
+  SG_TRY(read_cols(col_idxs, n_cols, nt, cols));
+  const int64_t n_fcols = std::lower_bound(cols.begin(), cols.end(), n) - cols.begin();
+  PermTables perms;
+  SG_TRY(perm_tables(tril_perms_lin, N, S, perms));
+  // force rows x force columns: exactly the row block sgdml_b200_assemble_rows writes; it synchronises before
+  // returning, so the table workspaces below are free again
   if (n_fcols > 0)
     SG_TRY(sgdml_b200_assemble_rows(R_desc, R_d_desc, tril_perms_lin, n_atoms, n_train, n_perms, sig, col_idxs,
                                     n_fcols, scale, m_begin, m_end, K, ldk, stream));
-  // column items: one per force-column point (with its destination map), one per energy column
+  // column items: one per force-column point (dst = -1 - t with the destination map fdest of point t), one per energy
+  // column; the kernel reads item_dst and fdest from one table, fdest after the n_items entries of item_dst
   std::vector<int> item_pt;
   std::vector<int64_t> item_dst, fdest;
-  for (int64_t c = 0; c < n_fcols; ++c) {
-    const int q = (int)(cols[(size_t)c] / N3), k = (int)(cols[(size_t)c] % N3);
-    if (item_pt.empty() || item_pt.back() != q) {
-      item_dst.push_back(-1 - (int64_t)item_pt.size());
-      item_pt.push_back(q);
-      fdest.insert(fdest.end(), (size_t)N3, (int64_t)-1);
-    }
-    fdest[(item_pt.size() - 1) * N3 + k] = c;
-  }
+  block_columns(cols, n_fcols, N3, item_pt, fdest);
+  for (size_t t = 0; t < item_pt.size(); ++t) item_dst.push_back(-1 - (int64_t)t);
   for (int64_t c = n_fcols; c < n_cols; ++c) {
     item_pt.push_back((int)(cols[(size_t)c] - n));
     item_dst.push_back(c);
   }
   const int64_t n_items = (int64_t)item_pt.size();
+  item_dst.insert(item_dst.end(), fdest.begin(), fdest.end());
   const int n_rowpts = (int)(m_end - m_begin);
   Staged sX, sG;
   SG_TRY(sX.init(R_desc, sizeof(double) * (size_t)M * D, true, s));
   SG_TRY(sG.init(R_d_desc, sizeof(double) * (size_t)M * D * 3, true, s));
-  int *d_apinv = nullptr, *d_pt = nullptr;
-  int64_t *d_dst = nullptr, *d_fdest = nullptr;
-  auto body = [&]() -> int {
-    SG_CUDA(cudaMalloc(&d_apinv, sizeof(int) * apinv.size()));
-    SG_CUDA(cudaMalloc(&d_pt, sizeof(int) * (size_t)n_items));
-    SG_CUDA(cudaMalloc(&d_dst, sizeof(int64_t) * (size_t)n_items));
-    SG_CUDA(cudaMalloc(&d_fdest, sizeof(int64_t) * std::max<size_t>(fdest.size(), 1)));
-    SG_CUDA(cudaMemcpyAsync(d_apinv, apinv.data(), sizeof(int) * apinv.size(), cudaMemcpyHostToDevice, s));
-    SG_CUDA(cudaMemcpyAsync(d_pt, item_pt.data(), sizeof(int) * (size_t)n_items, cudaMemcpyHostToDevice, s));
-    SG_CUDA(cudaMemcpyAsync(d_dst, item_dst.data(), sizeof(int64_t) * (size_t)n_items, cudaMemcpyHostToDevice, s));
-    if (!fdest.empty())
-      SG_CUDA(cudaMemcpyAsync(d_fdest, fdest.data(), sizeof(int64_t) * fdest.size(), cudaMemcpyHostToDevice, s));
-    ProfScope ps(KID_ASSEMBLE, s);
-    k_assemble_ecstr_rows<<<dim3((unsigned)n_items, (unsigned)n_rowpts), (N + 31) / 32 * 32, 0, s>>>(
-        (const double*)sX.dev(), (const double*)sG.dev(), d_apinv, N, D, S, sig, scale, d_pt, d_dst, d_fdest,
-        (int)m_begin, (int64_t)n_rowpts * N3, K, ldk);
-    SG_CUDA(cudaGetLastError());
-    count_launch(KID_ASSEMBLE);
-    SG_CUDA(cudaStreamSynchronize(s));  // the tables are freed below
-    return 0;
-  };
-  int rc = body();
-  cudaFree(d_apinv);
-  cudaFree(d_pt);
-  cudaFree(d_dst);
-  cudaFree(d_fdest);
-  return rc;
+  const int *d_apinv, *d_pt;
+  const int64_t* d_dst;
+  SG_TRY(ws_upload(WS_ASM_APINV, perms.apinv, s, &d_apinv));
+  SG_TRY(ws_upload(WS_ASM_JPTS, item_pt, s, &d_pt));
+  SG_TRY(ws_upload(WS_ASM_DEST, item_dst, s, &d_dst));
+  ProfScope ps(KID_ASSEMBLE, s);
+  k_assemble_ecstr_rows<<<dim3((unsigned)n_items, (unsigned)n_rowpts), (N + 31) / 32 * 32, 0, s>>>(
+      (const double*)sX.dev(), (const double*)sG.dev(), d_apinv, N, D, S, sig, scale, d_pt, d_dst, d_dst + n_items,
+      (int)m_begin, (int64_t)n_rowpts * N3, K, ldk);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_ASSEMBLE);
+  SG_CUDA(cudaStreamSynchronize(s));
+  return 0;
 }

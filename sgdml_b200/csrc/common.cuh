@@ -37,6 +37,8 @@ int require_device();
 
 // ------------------------------------------------------------------ host/device staging
 bool is_device_ptr(const void* p);
+// Copies n int64 index values (permutation tables, column lists) from a host or device pointer into out.
+int read_int64s(const int64_t* src, size_t n, std::vector<int64_t>& out);
 
 // RAII staging buffer: presents a device view of a user pointer that may live on the host.
 // in:  copy host->device on construction when the user pointer is a host pointer

@@ -1,6 +1,7 @@
 // Error plumbing, host/device staging and misc entry points of the sgdml_b200 C ABI.
 #include "common.cuh"
 
+#include <algorithm>
 #include <map>
 #include <mutex>
 
@@ -45,6 +46,15 @@ bool is_device_ptr(const void* p) {
     return false;
   }
   return attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged;
+}
+
+int read_int64s(const int64_t* src, size_t n, std::vector<int64_t>& out) {
+  out.resize(n);
+  if (is_device_ptr(src))
+    SG_CUDA(cudaMemcpy(out.data(), src, sizeof(int64_t) * n, cudaMemcpyDeviceToHost));
+  else
+    std::copy(src, src + n, out.begin());
+  return 0;
 }
 
 // ---- staging-buffer pool (see the comment on class Staged)

@@ -1492,6 +1492,19 @@ int sgdml_b200_model_create(sgdml_b200_model** out, int64_t n_atoms, int64_t n_t
   SG_ARG(out != nullptr && R_desc != nullptr && R_d_desc_alpha != nullptr && tril_perms_lin != nullptr);
   SG_ARG(n_atoms >= 2 && n_train >= 1 && n_perms >= 1 && sig > 0);
   const int64_t D = n_atoms * (n_atoms - 1) / 2;
+  // integer tables on the host (bit-exact), then to the device
+  std::vector<int64_t> lin;
+  SG_TRY(read_int64s(tril_perms_lin, (size_t)(n_perms * D), lin));
+  std::vector<int> perm((size_t)(n_perms * D)), pinv((size_t)(n_perms * D), -1);
+  for (int64_t pp = 0; pp < n_perms; ++pp)
+    for (int64_t d = 0; d < D; ++d) {
+      const int64_t e = lin[(size_t)(d * n_perms + pp)] - pp * D;  // train.py:903-904
+      if (e < 0 || e >= D || pinv[(size_t)(pp * D + e)] != -1)
+        return fail_arg("tril_perms_lin must encode S permutations of 0..D-1");
+      perm[(size_t)(pp * D + d)] = (int)e;
+      pinv[(size_t)(pp * D + e)] = (int)d;
+    }
+
   int cfg = -1;
   for (int i = 0; i < kNumCfgs; ++i)
     if (D <= kCfgs[i].DP) {
@@ -1521,29 +1534,6 @@ int sgdml_b200_model_create(sgdml_b200_model** out, int64_t n_atoms, int64_t n_t
   m->std = std;
   m->c = c;
   cudaGetDevice(&m->device);
-
-  // integer tables on the host (bit-exact), then to the device
-  std::vector<int64_t> lin((size_t)(n_perms * D));
-  if (is_device_ptr(tril_perms_lin)) {
-    cudaError_t e = cudaMemcpy(lin.data(), tril_perms_lin, sizeof(int64_t) * lin.size(), cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) {
-      delete m;
-      return fail_cuda(e, "copy tril_perms_lin", __FILE__, __LINE__);
-    }
-  } else {
-    std::copy(tril_perms_lin, tril_perms_lin + lin.size(), lin.begin());
-  }
-  std::vector<int> perm((size_t)(n_perms * D)), pinv((size_t)(n_perms * D), -1);
-  for (int64_t pp = 0; pp < n_perms; ++pp)
-    for (int64_t d = 0; d < D; ++d) {
-      const int64_t e = lin[(size_t)(d * n_perms + pp)] - pp * D;  // train.py:903-904
-      if (e < 0 || e >= D || pinv[(size_t)(pp * D + e)] != -1) {
-        delete m;
-        return fail_arg("tril_perms_lin must encode S permutations of 0..D-1");
-      }
-      perm[(size_t)(pp * D + d)] = (int)e;
-      pinv[(size_t)(pp * D + e)] = (int)d;
-    }
 
   int rc = 0;
   auto body = [&]() -> int {

@@ -199,6 +199,16 @@ int sgdml_b200_assemble_ecstr_rows(const double* R_desc, const double* R_d_desc,
  * cover the multi-launch path that row ranges above 65535 training points take). */
 int sgdml_b200_set_assemble_variant(int variant);
 
+/* How sgdml_b200_assemble_rows would run a force-force call under the current sgdml_b200_set_assemble_variant hooks,
+ * on a device with n_sm SMs: n_atoms atoms, n_perms permutations, n_colpts column points with at most nk kept column
+ * atoms each (nk = n_atoms without a column list), n_rowpts row points; square = 1 for the full matrix (no column list,
+ * every row point: nk = n_atoms, n_colpts = n_rowpts).  Writes 10 values to out:
+ *   {kernel (0 k_assemble, 1 k_assemble_v4, 2 k_assemble_v5, 3 k_assemble_large), TJ, PG, n_chunks (grid.z), grid_x,
+ *    dynamic shared memory bytes, sym, rows_per_launch, slab (doubles per CTA, large only), dl_in_smem}.
+ * Host only: needs no device. */
+int sgdml_b200_assemble_plan(int64_t n_atoms, int64_t n_perms, int64_t nk, int64_t n_colpts, int64_t n_rowpts,
+                             int square, int n_sm, int64_t* out);
+
 /* ---------------------------------------------------------------- dense solve (path a) */
 
 /* scipy.linalg.cho_factor (LAPACK dpotrf) as used by analytic.py:94-96 and

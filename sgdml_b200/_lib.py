@@ -57,6 +57,7 @@ SIGNATURES = {
          c_void_p],
     ),
     'sgdml_b200_set_assemble_variant': (C.c_int, [C.c_int]),
+    'sgdml_b200_assemble_plan': (C.c_int, [i64, i64, i64, i64, i64, C.c_int, C.c_int, c_int64_p]),
     'sgdml_b200_potrf': (C.c_int, [c_void_p, i64, i64, c_void_p]),
     'sgdml_b200_potrs': (C.c_int, [c_void_p, i64, i64, c_void_p, i64, i64, c_void_p]),
     'sgdml_b200_solve_analytic': (C.c_int, [c_void_p, i64, i64, C.c_double, c_void_p, c_void_p, c_void_p]),

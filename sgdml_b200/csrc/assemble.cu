@@ -1452,6 +1452,21 @@ extern "C" int sgdml_b200_set_assemble_variant(int variant) {
   return 0;
 }
 
+extern "C" int sgdml_b200_assemble_plan(int64_t n_atoms, int64_t n_perms, int64_t nk, int64_t n_colpts,
+                                        int64_t n_rowpts, int square, int n_sm, int64_t* out) {
+  // host only: the plan sgdml_b200_assemble_rows would launch under the current hooks, for n_sm SMs
+  SG_ARG(out != nullptr);
+  SG_ARG(n_atoms >= 2 && n_atoms * n_atoms < (1 << 20) && n_perms >= 1 && n_perms <= INT32_MAX / n_atoms);
+  SG_ARG(nk >= 1 && nk <= n_atoms && n_colpts >= 1 && n_colpts <= INT32_MAX && n_rowpts >= 1 && n_rowpts <= INT32_MAX);
+  SG_ARG((square == 0 || square == 1) && (!square || (nk == n_atoms && n_colpts == n_rowpts)) && n_sm >= 1);
+  const AsmPlan p = asm_plan((int)n_atoms, (int)n_perms, (int)nk, (int)n_colpts, (int)n_rowpts, square != 0,
+                             g_asm_hooks, n_sm);
+  const int64_t v[] = {p.kernel, p.TJ,  p.PG,  p.n_chunks, p.grid_x, (int64_t)p.smem, p.sym, p.rows_per_launch,
+                       (int64_t)p.slab, p.dl_in_smem};
+  std::copy(v, v + 10, out);
+  return 0;
+}
+
 extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_desc, const int64_t* tril_perms_lin,
                                         int64_t n_atoms, int64_t n_train, int64_t n_perms, double sig,
                                         const int64_t* col_idxs, int64_t n_cols, double scale, int64_t m_begin,

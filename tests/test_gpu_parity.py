@@ -298,8 +298,9 @@ def test_assemble_large_kernel_matches_small(eng, golden):
 @pytest.mark.parametrize('N,M,rot,swap,sig', [(60, 3, 1, 1, 50), (100, 2, 2, 0, 50), (53, 2, 0, 1, 30), (64, 2, 2, 1, 40)])
 def test_assemble_large_molecules_vs_oracle(eng, N, M, rot, swap, sig, variant):
     """BASELINE configs 4-5 sizes (60 and 100 atoms): expanded pair tables beyond shared memory.  variant 0: the default
-    routing (up to ~64 atoms k_assemble_v5, compressed pair arrays on chip; above that k_assemble_large), variant 1: the
-    large-molecule kernel (tables in global memory) for every size."""
+    routing (k_assemble_v5, compressed pair arrays on chip, up to N = 70...82 depending on S -- 76 at S = 6, 82 at
+    S = 1; above that k_assemble_large, whose delta table stays in shared memory up to N = 113, so at N = 100 too),
+    variant 1: the large-molecule kernel (other tables in global memory) for every size."""
     from sgdml_b200 import _lib, synth
     from sgdml_b200.desc import Desc
 

@@ -96,6 +96,25 @@ int sgdml_b200_model_destroy(sgdml_b200_model* model);
 int sgdml_b200_predict(sgdml_b200_model* model, const double* R, int64_t n_geo, double* E,
                        double* F, void* stream);
 
+/* Extension (the reference has no such output): sgdml_b200_predict plus the virial W of each geometry, in a cell given
+ * per call.  Take the rows r_i of a geometry and a cell L whose lattice vectors are its COLUMNS (model['lattice']), and
+ * strain both homogeneously, r_i -> (I + eps) r_i, L -> (I + eps) L.  Then
+ *   W = -dE/d(eps) at eps = 0   (symmetric 3 x 3, in the model's energy unit)
+ *     = sum_d (dE/dx_d) delta_d delta_d^T / |delta_d|^3,
+ * x_d = 1/|delta_d| the descriptor and delta_d = r_a - r_b - L rint(L^-1 (r_a - r_b)) the minimum-image vector of pair d
+ * (the rint term is locally constant), with the image the descriptor of the same call picked.  For a free molecule W
+ * equals the classical virial sum_i r_i F_i^T; in a periodic cell it does not once pairs wrap.  The stress an ASE
+ * calculator reports is -W / V.  Energy-constraint terms (sgdml_b200_model_set_alphas_E) are included.
+ *   R (B, 3N) -> E (B,) [may be NULL], F (B, 3N), W (B, 9) row-major; each output host or device as in
+ *   sgdml_b200_predict, whose E and F (bit for bit) this call returns for the same cell.
+ *   lattice, lattice_inv: 9 HOST doubles each, row-major, lattice vectors as columns (the sgdml_b200_model_set_lattice
+ *   convention), used for this call only; both NULL: the model's current cell, which may be none.  A singular or
+ *   non-finite cell, one NULL of the two, or device pointers are rejected, and a rejected call changes nothing.
+ * Small host batches replay a captured CUDA graph into which the cell is read at run time, so a call with a new cell
+ * neither captures again nor synchronises the device. */
+int sgdml_b200_predict_virial(sgdml_b200_model* model, const double* R, int64_t n_geo, const double* lattice,
+                              const double* lattice_inv, double* E, double* F, double* W, void* stream);
+
 /* Periodic model (predict.py:332-334: lat_and_inv from model['lattice']): query descriptors of
  * sgdml_b200_predict are built with the minimum-image convention.  Both NULL: back to a free molecule. */
 int sgdml_b200_model_set_lattice(sgdml_b200_model* model, const double* lattice, const double* lattice_inv);

@@ -10,8 +10,9 @@ namespace sgdml {
 // reference: utils/desc.py:80-110 (_pdist), 139-163, 166-205, 288-365
 // lat.on != 0: minimum-image convention (utils/desc.py:44-77): d -= lat @ rint(lat_inv @ d), lattice vectors as the
 // COLUMNS of lat; np.around and rint both round half to even
-__global__ void k_desc_from_R(const double* __restrict__ R, int64_t n_geo, int n_atoms, int dim_d,
-                              double* __restrict__ R_desc, double* __restrict__ R_d_desc, const Lattice lat) {
+__device__ __forceinline__ void desc_from_R_body(const double* __restrict__ R, int64_t n_geo, int n_atoms, int dim_d,
+                                                 double* __restrict__ R_desc, double* __restrict__ R_d_desc,
+                                                 const Lattice& lat) {
   int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   int64_t total = n_geo * dim_d;
   if (idx >= total) return;
@@ -40,6 +41,19 @@ __global__ void k_desc_from_R(const double* __restrict__ R, int64_t n_geo, int n
     R_d_desc[idx * 3 + 1] = dy * inv3;
     R_d_desc[idx * 3 + 2] = dz * inv3;
   }
+}
+__global__ void k_desc_from_R(const double* __restrict__ R, int64_t n_geo, int n_atoms, int dim_d,
+                              double* __restrict__ R_desc, double* __restrict__ R_d_desc, const Lattice lat) {
+  desc_from_R_body(R, n_geo, n_atoms, dim_d, R_desc, R_d_desc, lat);
+}
+// the same with the cell in device memory (a captured graph copies each call's cell there, next to R)
+__global__ void k_desc_from_R_lp(const double* __restrict__ R, int64_t n_geo, int n_atoms, int dim_d,
+                                 double* __restrict__ R_desc, double* __restrict__ R_d_desc,
+                                 const Lattice* __restrict__ latp) {
+  __shared__ Lattice lat;
+  if (threadIdx.x == 0) lat = *latp;
+  __syncthreads();
+  desc_from_R_body(R, n_geo, n_atoms, dim_d, R_desc, R_d_desc, lat);
 }
 
 // ---------------------------------------------------------------- a-D3: (J v)_d = g_d . (v_b - v_a)
@@ -99,6 +113,18 @@ int launch_desc_from_R(const double* R, int64_t n_geo, int n_atoms, double* R_de
   if (lat != nullptr) l = *lat;
   ProfScope ps(KID_DESC, s);
   k_desc_from_R<<<ceil_div(total, 256), 256, 0, s>>>(R, n_geo, n_atoms, D, R_desc, R_d_desc, l);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_DESC);
+  return 0;
+}
+
+int launch_desc_from_R_lp(const double* R, int64_t n_geo, int n_atoms, double* R_desc, double* R_d_desc,
+                          cudaStream_t s, const Lattice* lat_dev) {
+  if (n_geo == 0) return 0;
+  const int D = n_atoms * (n_atoms - 1) / 2;
+  int64_t total = n_geo * D;
+  ProfScope ps(KID_DESC, s);
+  k_desc_from_R_lp<<<ceil_div(total, 256), 256, 0, s>>>(R, n_geo, n_atoms, D, R_desc, R_d_desc, lat_dev);
   SG_CUDA(cudaGetLastError());
   count_launch(KID_DESC);
   return 0;

@@ -620,11 +620,11 @@ __global__ void __launch_bounds__(256) k_query_rows(const double* __restrict__ x
 // Small host-buffer batches (the CUDA-graph path): descriptor, its derivative factors and the S query rows of one
 // geometry in ONE launch, one CTA per geometry.  R may live in pinned host memory (read once into shared memory through
 // the unified address space); the arithmetic is that of k_desc_from_R (csrc/desc.cu) followed by k_query_rows.
-__global__ void __launch_bounds__(256) k_desc_query_rows(const double* __restrict__ R, int n_atoms,
-                                                         const int* __restrict__ pinv, const double* __restrict__ mu,
-                                                         int D, int DS, int S, int64_t n_rows, int64_t n_rows_pad,
-                                                         double* __restrict__ gq, double* __restrict__ Qg,
-                                                         double* __restrict__ qqg, const Lattice lat) {
+__device__ __forceinline__ void desc_query_rows_body(const double* __restrict__ R, int n_atoms,
+                                                     const int* __restrict__ pinv, const double* __restrict__ mu,
+                                                     int D, int DS, int S, int64_t n_rows, int64_t n_rows_pad,
+                                                     double* __restrict__ gq, double* __restrict__ Qg,
+                                                     double* __restrict__ qqg, const Lattice& lat) {
   extern __shared__ double dq_sm[];  // r: 3N, x: D
   double* r = dq_sm;
   double* x = dq_sm + 3 * n_atoms;
@@ -675,6 +675,25 @@ __global__ void __launch_bounds__(256) k_desc_query_rows(const double* __restric
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     if (lane == 0) qqg[row] = s;
   }
+}
+__global__ void __launch_bounds__(256) k_desc_query_rows(const double* __restrict__ R, int n_atoms,
+                                                         const int* __restrict__ pinv, const double* __restrict__ mu,
+                                                         int D, int DS, int S, int64_t n_rows, int64_t n_rows_pad,
+                                                         double* __restrict__ gq, double* __restrict__ Qg,
+                                                         double* __restrict__ qqg, const Lattice lat) {
+  desc_query_rows_body(R, n_atoms, pinv, mu, D, DS, S, n_rows, n_rows_pad, gq, Qg, qqg, lat);
+}
+// The same with the cell read from memory (the pinned staging slot of sgdml_b200_predict_virial's graphs, next to R):
+// a replayed graph picks up the call's cell as it picks up its geometries.
+__global__ void __launch_bounds__(256) k_desc_query_rows_lp(const double* __restrict__ R, int n_atoms,
+                                                            const int* __restrict__ pinv, const double* __restrict__ mu,
+                                                            int D, int DS, int S, int64_t n_rows, int64_t n_rows_pad,
+                                                            double* __restrict__ gq, double* __restrict__ Qg,
+                                                            double* __restrict__ qqg, const Lattice* __restrict__ latp) {
+  __shared__ Lattice lat;
+  if (threadIdx.x == 0) lat = *latp;
+  __syncthreads();
+  desc_query_rows_body(R, n_atoms, pinv, mu, D, DS, S, n_rows, n_rows_pad, gq, Qg, qqg, lat);
 }
 
 // ============================================================== large descriptors (D > 256)
@@ -747,16 +766,54 @@ __global__ void k_transpose_pad(const double* __restrict__ src, int64_t rows, in
   }
 }
 
+// ============================================================== virial
+// W = -dE/d(eps) under the homogeneous strain r -> (I + eps) r, L -> (I + eps) L.  E depends on the geometry only through
+// x_d = 1/|delta_d|, delta_d the minimum-image pair vector, and dE/dx_d = -std F_desc[d] (F = std J_x^T F_desc is
+// -dE/dR), so
+//   W = -std sum_d F_desc[d] g_d delta_d^T,   g_d = delta_d / |delta_d|^3.
+// The pair vector is rebuilt from g_d rather than from x_d: |g_d| = |delta_d|^-2, so delta_d = g_d |g_d|^-3/2.  gq is
+// what every finishing kernel already reads for the forces (the zero-copy graph path does not store x at all), g_d
+// carries the image of the call's descriptor (no second rint), and the rebuild costs two square roots and a division per
+// pair and no memory traffic beyond one more read of g_d.  g_d delta_d^T = g_d g_d^T / |g_d|^3/2 is symmetric: six sums
+// per query, mirrored into the 3 x 3 output.  Every reduction below has a fixed order (shuffle trees and in-order sums
+// over warps or CTAs, no atomics).
+__device__ __forceinline__ void virial_term(const double* __restrict__ g, double f, double* w) {
+  const double gx = g[0], gy = g[1], gz = g[2];
+  const double gn = sqrt(gx * gx + gy * gy + gz * gz);
+  const double s = f / (gn * sqrt(gn));
+  const double sx = s * gx, sy = s * gy;
+  w[0] += sx * gx;
+  w[1] += sy * gy;
+  w[2] += s * gz * gz;
+  w[3] += sx * gy;
+  w[4] += sx * gz;
+  w[5] += sy * gz;
+}
+__device__ __forceinline__ void warp_sum6(double* w) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+    for (int i = 0; i < 6; ++i) w[i] += __shfl_xor_sync(0xffffffffu, w[i], o);
+}
+// entry e (0..8, row-major) of W from the six sums: xx, yy, zz, xy, xz, yz
+__device__ __forceinline__ int virial_slot(int e) {
+  const int i = e / 3, j = e - 3 * (e / 3);
+  return i == j ? i : i + j + 2;
+}
+
 // ============================================================== finishing kernel
 // F_desc[d] = sum_p G[b*S+p][perm_p[d]];  F = J_x^T F_desc (predict.py:240-243);
 // E = sum_p Erow;  outputs scaled by std, E += c (predict.py:1286-1288).
 // One CTA per QPB queries (QPB = 128 / D for small molecules, else 1): threads over (query, descriptor entry), then
-// over (query, force component).
-__global__ void __launch_bounds__(128) k_predict_finish(const double* __restrict__ G, const double* __restrict__ Erow,
-                                                        const double* __restrict__ gq, const int* __restrict__ perm,
-                                                        int n_atoms, int D, int DP, int S, double std, double c,
-                                                        int n_splits, int64_t plane_rows, int64_t n_geo, int QPB,
-                                                        double* __restrict__ E, double* __restrict__ F) {
+// over (query, force component).  WITH_W: also the virial W (n_geo x 9), from the F_desc in shared memory -- one warp
+// per query for QPB > 1, all four warps for QPB = 1 (summed in warp order).
+template <bool WITH_W>
+__device__ __forceinline__ void predict_finish_body(const double* __restrict__ G, const double* __restrict__ Erow,
+                                                    const double* __restrict__ gq, const int* __restrict__ perm,
+                                                    int n_atoms, int D, int DP, int S, double std, double c,
+                                                    int n_splits, int64_t plane_rows, int64_t n_geo, int QPB,
+                                                    double* __restrict__ E, double* __restrict__ F,
+                                                    double* __restrict__ W) {
   extern __shared__ double fd[];  // QPB * D
   const int64_t b0 = (int64_t)blockIdx.x * QPB;
   const int nq = (int)min((int64_t)QPB, n_geo - b0);
@@ -815,16 +872,60 @@ __global__ void __launch_bounds__(128) k_predict_finish(const double* __restrict
       if (lane == 0) E[b] = s * std + c;
     }
   }
+  if constexpr (WITH_W) {
+    __shared__ double wpart[4][6];  // QPB = 1: the four warps' sums
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (QPB > 1) {
+      for (int ql = warp; ql < nq; ql += 4) {
+        const double* g = gq + (b0 + ql) * (int64_t)D * 3;
+        double w[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        for (int d = lane; d < D; d += 32) virial_term(g + 3 * d, fd[ql * D + d], w);
+        warp_sum6(w);
+        if (lane < 9) W[(b0 + ql) * 9 + lane] = -std * w[virial_slot(lane)];
+      }
+    } else {
+      const double* g = gq + b0 * (int64_t)D * 3;
+      double w[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+      for (int d = threadIdx.x; d < D; d += 128) virial_term(g + 3 * d, fd[d], w);
+      warp_sum6(w);
+      if (lane < 6) wpart[warp][lane] = w[lane];
+      __syncthreads();
+      if (threadIdx.x < 9) {
+        const int k = virial_slot(threadIdx.x);
+        W[b0 * 9 + threadIdx.x] = -std * (((wpart[0][k] + wpart[1][k]) + wpart[2][k]) + wpart[3][k]);
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(128) k_predict_finish(const double* __restrict__ G, const double* __restrict__ Erow,
+                                                        const double* __restrict__ gq, const int* __restrict__ perm,
+                                                        int n_atoms, int D, int DP, int S, double std, double c,
+                                                        int n_splits, int64_t plane_rows, int64_t n_geo, int QPB,
+                                                        double* __restrict__ E, double* __restrict__ F) {
+  predict_finish_body<false>(G, Erow, gq, perm, n_atoms, D, DP, S, std, c, n_splits, plane_rows, n_geo, QPB, E, F,
+                             nullptr);
+}
+__global__ void __launch_bounds__(128) k_predict_finish_w(const double* __restrict__ G, const double* __restrict__ Erow,
+                                                          const double* __restrict__ gq, const int* __restrict__ perm,
+                                                          int n_atoms, int D, int DP, int S, double std, double c,
+                                                          int n_splits, int64_t plane_rows, int64_t n_geo, int QPB,
+                                                          double* __restrict__ E, double* __restrict__ F,
+                                                          double* __restrict__ W) {
+  predict_finish_body<true>(G, Erow, gq, perm, n_atoms, D, DP, S, std, c, n_splits, plane_rows, n_geo, QPB, E, F, W);
 }
 
 // The same for batches of a few queries (the MD latency path: one geometry per call).  There the one-CTA-per-query form
 // is a chain of S * n_splits dependent L2 round trips per thread (126 at BASELINE config 2, B = 1); here 1024
 // threads split every descriptor entry's terms into `parts` interleaved partial sums (fixed order: bit-reproducible).
-__global__ void __launch_bounds__(1024) k_predict_finish_small(const double* __restrict__ G, const double* __restrict__ Erow,
-                                                               const double* __restrict__ gq, const int* __restrict__ perm,
-                                                               int n_atoms, int D, int DP, int S, double std, double c,
-                                                               int n_splits, int64_t plane_rows, int parts,
-                                                               double* __restrict__ E, double* __restrict__ F) {
+// WITH_W: the virial of the query, 32 warps' sums added in warp order.
+template <bool WITH_W>
+__device__ __forceinline__ void predict_finish_small_body(const double* __restrict__ G, const double* __restrict__ Erow,
+                                                          const double* __restrict__ gq, const int* __restrict__ perm,
+                                                          int n_atoms, int D, int DP, int S, double std, double c,
+                                                          int n_splits, int64_t plane_rows, int parts,
+                                                          double* __restrict__ E, double* __restrict__ F,
+                                                          double* __restrict__ W) {
   extern __shared__ double fds[];  // parts * D partial sums, then D totals
   double* fd = fds + parts * D;
   const int64_t b = blockIdx.x;
@@ -879,6 +980,39 @@ __global__ void __launch_bounds__(1024) k_predict_finish_small(const double* __r
     for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
     if (lane == 0) E[b] = sum * std + c;
   }
+  if constexpr (WITH_W) {
+    __shared__ double wpart[32][6];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double w[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int d = threadIdx.x; d < D; d += blockDim.x) virial_term(g + 3 * d, fd[d], w);
+    warp_sum6(w);
+    if (lane < 6) wpart[warp][lane] = w[lane];
+    __syncthreads();
+    if (threadIdx.x < 9) {
+      const int k = virial_slot(threadIdx.x);
+      double s = 0.0;
+      for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += wpart[i][k];
+      W[b * 9 + threadIdx.x] = -std * s;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(1024) k_predict_finish_small(const double* __restrict__ G, const double* __restrict__ Erow,
+                                                               const double* __restrict__ gq, const int* __restrict__ perm,
+                                                               int n_atoms, int D, int DP, int S, double std, double c,
+                                                               int n_splits, int64_t plane_rows, int parts,
+                                                               double* __restrict__ E, double* __restrict__ F) {
+  predict_finish_small_body<false>(G, Erow, gq, perm, n_atoms, D, DP, S, std, c, n_splits, plane_rows, parts, E, F,
+                                   nullptr);
+}
+__global__ void __launch_bounds__(1024) k_predict_finish_small_w(const double* __restrict__ G,
+                                                                 const double* __restrict__ Erow,
+                                                                 const double* __restrict__ gq,
+                                                                 const int* __restrict__ perm, int n_atoms, int D,
+                                                                 int DP, int S, double std, double c, int n_splits,
+                                                                 int64_t plane_rows, int parts, double* __restrict__ E,
+                                                                 double* __restrict__ F, double* __restrict__ W) {
+  predict_finish_small_body<true>(G, Erow, gq, perm, n_atoms, D, DP, S, std, c, n_splits, plane_rows, parts, E, F, W);
 }
 
 // ============================================================== finishing path for long descriptors
@@ -893,26 +1027,59 @@ __global__ void __launch_bounds__(1024) k_predict_finish_small(const double* __r
 // cover the S rows of a few queries (S*DP*8 bytes each, 1.6 MB at N = 370, S = 3), so the permuted reads (scattered only
 // where an atom permutation breaks up runs of consecutive pairs; the identity is read in order) hit L2 and HBM delivers
 // every sector of G once.
+__device__ __forceinline__ double fdesc_entry(const double* __restrict__ G, const int* __restrict__ perm, int D, int DP,
+                                              int S, int n_splits, int64_t stride, int64_t b, int d) {
+  double acc0 = 0.0, acc1 = 0.0, acc2 = 0.0, acc3 = 0.0;
+  for (int pp = 0; pp < S; ++pp) {
+    const double* gp = G + (b * S + pp) * DP + perm[pp * D + d];
+    int sp = 0;
+    for (; sp + 4 <= n_splits; sp += 4) {
+      acc0 += gp[(int64_t)sp * stride];
+      acc1 += gp[(int64_t)(sp + 1) * stride];
+      acc2 += gp[(int64_t)(sp + 2) * stride];
+      acc3 += gp[(int64_t)(sp + 3) * stride];
+    }
+    for (; sp < n_splits; ++sp) acc0 += gp[(int64_t)sp * stride];
+  }
+  return (acc0 + acc1) + (acc2 + acc3);
+}
+
 __global__ void __launch_bounds__(256) k_fdesc_gather(const double* __restrict__ G, const int* __restrict__ perm, int D,
                                                       int DP, int S, int n_splits, int64_t plane_rows, int64_t n_geo,
                                                       double* __restrict__ Fd) {
   const int d = blockIdx.x * blockDim.x + threadIdx.x;
   if (d >= D) return;
   const int64_t stride = plane_rows * DP;
+  for (int64_t b = blockIdx.y; b < n_geo; b += gridDim.y) Fd[b * D + d] = fdesc_entry(G, perm, D, DP, S, n_splits, stride, b, d);
+}
+
+// With the virial: the gather touches every pair exactly once, so each CTA also sums the virial terms of its 256
+// entries (shuffle tree, then its eight warps in order) into Wp[b][blockIdx.x][6]; k_fdesc_project_w adds those
+// ceil(D/256) partials in CTA order.
+__global__ void __launch_bounds__(256) k_fdesc_gather_w(const double* __restrict__ G, const int* __restrict__ perm,
+                                                        const double* __restrict__ gq, int D, int DP, int S,
+                                                        int n_splits, int64_t plane_rows, int64_t n_geo,
+                                                        double* __restrict__ Fd, double* __restrict__ Wp) {
+  __shared__ double wpart[8][6];
+  const int d = blockIdx.x * blockDim.x + threadIdx.x;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t stride = plane_rows * DP;
   for (int64_t b = blockIdx.y; b < n_geo; b += gridDim.y) {
-    double acc0 = 0.0, acc1 = 0.0, acc2 = 0.0, acc3 = 0.0;
-    for (int pp = 0; pp < S; ++pp) {
-      const double* gp = G + (b * S + pp) * DP + perm[pp * D + d];
-      int sp = 0;
-      for (; sp + 4 <= n_splits; sp += 4) {
-        acc0 += gp[(int64_t)sp * stride];
-        acc1 += gp[(int64_t)(sp + 1) * stride];
-        acc2 += gp[(int64_t)(sp + 2) * stride];
-        acc3 += gp[(int64_t)(sp + 3) * stride];
-      }
-      for (; sp < n_splits; ++sp) acc0 += gp[(int64_t)sp * stride];
+    double w[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    if (d < D) {
+      const double f = fdesc_entry(G, perm, D, DP, S, n_splits, stride, b, d);
+      Fd[b * D + d] = f;
+      virial_term(gq + (b * D + d) * 3, f, w);
     }
-    Fd[b * D + d] = (acc0 + acc1) + (acc2 + acc3);
+    warp_sum6(w);
+    if (lane < 6) wpart[warp][lane] = w[lane];
+    __syncthreads();
+    if (threadIdx.x < 6) {
+      double s = 0.0;
+      for (int i = 0; i < 8; ++i) s += wpart[i][threadIdx.x];
+      Wp[(b * gridDim.x + blockIdx.x) * 6 + threadIdx.x] = s;
+    }
+    __syncthreads();  // wpart is rewritten for the next query
   }
 }
 
@@ -923,11 +1090,10 @@ __global__ void __launch_bounds__(256) k_fdesc_gather(const double* __restrict__
 // consecutive; one warp per atom, lanes over o.  Each entry is read by two CTAs of the same query, which run side by
 // side (grid x = atom groups), so the second read comes from L2.
 constexpr int FDP_WARPS = 8;
-__global__ void __launch_bounds__(FDP_WARPS * 32) k_fdesc_project(const double* __restrict__ Fd, const double* __restrict__ gq,
-                                                                  const double* __restrict__ Erow, int n_atoms, int D,
-                                                                  int S, double std, double c, int n_splits,
-                                                                  int64_t plane_rows, int64_t n_geo,
-                                                                  double* __restrict__ E, double* __restrict__ F) {
+__device__ __forceinline__ void fdesc_project_body(const double* __restrict__ Fd, const double* __restrict__ gq,
+                                                     const double* __restrict__ Erow, int n_atoms, int D, int S,
+                                                     double std, double c, int n_splits, int64_t plane_rows,
+                                                     int64_t n_geo, double* __restrict__ E, double* __restrict__ F) {
   __shared__ double col[FDP_WARPS][32][3];
   __shared__ double row[32][3];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -994,6 +1160,32 @@ __global__ void __launch_bounds__(FDP_WARPS * 32) k_fdesc_project(const double* 
       if (lane == 0) E[b] = s * std + c;
     }
     __syncthreads();  // col / row are rewritten for the next query
+  }
+}
+__global__ void __launch_bounds__(FDP_WARPS * 32) k_fdesc_project(const double* __restrict__ Fd, const double* __restrict__ gq,
+                                                                  const double* __restrict__ Erow, int n_atoms, int D,
+                                                                  int S, double std, double c, int n_splits,
+                                                                  int64_t plane_rows, int64_t n_geo,
+                                                                  double* __restrict__ E, double* __restrict__ F) {
+  fdesc_project_body(Fd, gq, Erow, n_atoms, D, S, std, c, n_splits, plane_rows, n_geo, E, F);
+}
+
+// k_fdesc_project, then the virial of each query from the n_parts per-CTA partials of k_fdesc_gather_w (CTA order)
+__global__ void __launch_bounds__(FDP_WARPS * 32) k_fdesc_project_w(const double* __restrict__ Fd,
+                                                                    const double* __restrict__ gq,
+                                                                    const double* __restrict__ Erow, int n_atoms,
+                                                                    int D, int S, double std, double c, int n_splits,
+                                                                    int64_t plane_rows, int64_t n_geo,
+                                                                    double* __restrict__ E, double* __restrict__ F,
+                                                                    const double* __restrict__ Wp, int n_parts,
+                                                                    double* __restrict__ W) {
+  fdesc_project_body(Fd, gq, Erow, n_atoms, D, S, std, c, n_splits, plane_rows, n_geo, E, F);
+  if (blockIdx.x != 0 || threadIdx.x >= 9) return;
+  const int k = virial_slot(threadIdx.x);
+  for (int64_t b = blockIdx.y; b < n_geo; b += gridDim.y) {
+    double s = 0.0;
+    for (int i = 0; i < n_parts; ++i) s += Wp[(b * n_parts + i) * 6 + k];
+    W[b * 9 + threadIdx.x] = -std * s;
   }
 }
 
@@ -1100,6 +1292,8 @@ struct sgdml_b200_model {
     double *xq = nullptr, *gq = nullptr, *G = nullptr, *Erow = nullptr, *R = nullptr, *E = nullptr, *F = nullptr,
            *Qg = nullptr, *qq = nullptr, *S1 = nullptr, *S2 = nullptr, *csum = nullptr;
     double* Fd = nullptr;       // (geo, D) F_desc of long descriptors (fdesc_in_ws)
+    double* W = nullptr;        // (geo, 9) virial staging for host outputs
+    double* Wp = nullptr;       // (geo, ceil(D / 256), 6) per-CTA virial partials of k_fdesc_gather_w (fdesc_in_ws)
     OzOperand ozQ, ozC1, ozC2;  // slices of the per-batch operands (int8 path of large descriptors)
   } ws[2];
   cudaStream_t pipe_stream[2] = {nullptr, nullptr};
@@ -1108,10 +1302,13 @@ struct sgdml_b200_model {
   struct GraphSlot {
     int64_t n_geo = 0;
     int with_E = 0;
+    int with_W = 0;  // sgdml_b200_predict_virial: the cell is read from hLat at run time, not baked in
     int n_kernels = 0;
     uint64_t generation = 0;
     cudaGraphExec_t exec = nullptr;
-    double *hR = nullptr, *hF = nullptr, *hE = nullptr;  // pinned staging
+    double *hR = nullptr, *hF = nullptr, *hE = nullptr, *hW = nullptr;  // pinned staging
+    Lattice* hLat = nullptr;  // pinned: the call's cell (with_W)
+    Lattice* dLat = nullptr;  // device copy of hLat (with_W, copy-node form)
   } graphs[4];
   int graph_next = 0;
   uint64_t generation = 1;  // bumped whenever something a captured graph has baked in changes (workspace, cell, alphas_E)
@@ -1209,6 +1406,8 @@ void free_ws(sgdml_b200_model* m) {
     cached_free(w.S2);
     cached_free(w.csum);
     cached_free(w.Fd);
+    cached_free(w.W);
+    cached_free(w.Wp);
     w = sgdml_b200_model::WS();
   }
 }
@@ -1242,8 +1441,12 @@ int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
   cached_free(w.S2);
   cached_free(w.csum);
   cached_free(w.Fd);
+  cached_free(w.W);
+  cached_free(w.Wp);
   w = sgdml_b200_model::WS();
   SG_CUDA(cached_malloc(&w.xq, sizeof(double) * n_geo * m->D));
+  SG_CUDA(cached_malloc(&w.W, sizeof(double) * n_geo * 9));
+  if (fdesc_in_ws(m)) SG_CUDA(cached_malloc(&w.Wp, sizeof(double) * n_geo * ceil_div(m->D, 256) * 6));
   SG_CUDA(cached_malloc(&w.gq, sizeof(double) * n_geo * m->D * 3));
   {
     // padded to whole row tiles: the per-split output planes of small batches are laid out with that stride
@@ -1298,8 +1501,9 @@ int64_t chunk_geos(const sgdml_b200_model* m) {
 // Runs the predictor on n_geo queries whose descriptors (xq, gq) are on the device.
 constexpr int64_t GRAPH_MAX_GEO = 16;  // batches up to this size with host buffers replay a captured graph
 // xq == nullptr: the query rows (w.Qg, w.qq) are already in place (k_desc_query_rows)
+// W_dev != nullptr: the finishing kernels' virial variants also write W (n_geo x 9); E and F are unchanged by it
 int run_queries(sgdml_b200_model* m, int slot, const double* xq, const double* gq, int64_t n_geo, double std,
-                double c, double* E_dev, double* F_dev, cudaStream_t s) {
+                double c, double* E_dev, double* F_dev, cudaStream_t s, double* W_dev = nullptr) {
   sgdml_b200_model::WS& w = m->ws[slot];
   const int64_t n_rows = n_geo * m->S;
   const int64_t n_rows_pad = (n_rows + m->BQ - 1) / m->BQ * m->BQ;
@@ -1416,11 +1620,20 @@ int run_queries(sgdml_b200_model* m, int slot, const double* xq, const double* g
   if (fdesc_in_ws(m)) {
     ProfScope ps(KID_PREDICT_FINISH, s);
     const unsigned gy = (unsigned)std::min<int64_t>(n_geo, 65535);
-    k_fdesc_gather<<<dim3((unsigned)ceil_div(m->D, 256), gy), 256, 0, s>>>(w.G, m->perm, m->D, m->DP, m->S, n_splits,
-                                                                         n_rows_pad, n_geo, w.Fd);
-    SG_CUDA(cudaGetLastError());
-    k_fdesc_project<<<dim3((unsigned)ceil_div(m->N, 32), gy), FDP_WARPS * 32, 0, s>>>(
-        w.Fd, gq, w.Erow, m->N, m->D, m->S, std, c, n_splits, n_rows_pad, n_geo, E_dev, F_dev);
+    const int n_parts = ceil_div(m->D, 256);
+    if (W_dev != nullptr) {
+      k_fdesc_gather_w<<<dim3((unsigned)n_parts, gy), 256, 0, s>>>(w.G, m->perm, gq, m->D, m->DP, m->S, n_splits,
+                                                                   n_rows_pad, n_geo, w.Fd, w.Wp);
+      SG_CUDA(cudaGetLastError());
+      k_fdesc_project_w<<<dim3((unsigned)ceil_div(m->N, 32), gy), FDP_WARPS * 32, 0, s>>>(
+          w.Fd, gq, w.Erow, m->N, m->D, m->S, std, c, n_splits, n_rows_pad, n_geo, E_dev, F_dev, w.Wp, n_parts, W_dev);
+    } else {
+      k_fdesc_gather<<<dim3((unsigned)n_parts, gy), 256, 0, s>>>(w.G, m->perm, m->D, m->DP, m->S, n_splits,
+                                                                 n_rows_pad, n_geo, w.Fd);
+      SG_CUDA(cudaGetLastError());
+      k_fdesc_project<<<dim3((unsigned)ceil_div(m->N, 32), gy), FDP_WARPS * 32, 0, s>>>(
+          w.Fd, gq, w.Erow, m->N, m->D, m->S, std, c, n_splits, n_rows_pad, n_geo, E_dev, F_dev);
+    }
     SG_CUDA(cudaGetLastError());
     count_launch(KID_PREDICT_FINISH, 2);
     return 0;
@@ -1429,14 +1642,29 @@ int run_queries(sgdml_b200_model* m, int slot, const double* xq, const double* g
     ProfScope ps(KID_PREDICT_AUX, s);
     const int QPB = std::max(1, 128 / m->D);  // small molecules: several queries per CTA
     const size_t fd_bytes = sizeof(double) * (size_t)m->D * QPB;
-    if (fd_bytes > 48 * 1024)  // molecules above 111 atoms: opt in to more than the default dynamic shared memory
+    if (fd_bytes > 48 * 1024 && W_dev == nullptr)  // molecules above 111 atoms: opt in to more than the default dynamic shared memory
       SG_CUDA(cudaFuncSetAttribute(k_predict_finish, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fd_bytes));
     const int parts = std::max(1, std::min(8, 1024 / m->D));
     const size_t fds_bytes = sizeof(double) * (size_t)m->D * (parts + 1);
+    // the virial variants add up to 1.5 KB of static shared memory, which counts against the 48 KB default: they opt
+    // in a little earlier, so that they take exactly the plain kernels' routes
+    if (W_dev != nullptr && fd_bytes > 46 * 1024)
+      SG_CUDA(cudaFuncSetAttribute(k_predict_finish_w, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fd_bytes));
+    if (W_dev != nullptr && fds_bytes > 46 * 1024 && fds_bytes <= 48 * 1024)
+      SG_CUDA(cudaFuncSetAttribute(k_predict_finish_small_w, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fds_bytes));
     if (n_geo <= GRAPH_MAX_GEO && n_splits > 1 && parts > 1 && fds_bytes <= 48 * 1024) {
       // a few queries, the sweep over the training points split across CTAs: the latency form
-      k_predict_finish_small<<<(unsigned)n_geo, 1024, fds_bytes, s>>>(w.G, w.Erow, gq, m->perm, m->N, m->D, m->DP, m->S, std, c,
-                                                                     n_splits, n_rows_pad, parts, E_dev, F_dev);
+      if (W_dev != nullptr)
+        k_predict_finish_small_w<<<(unsigned)n_geo, 1024, fds_bytes, s>>>(w.G, w.Erow, gq, m->perm, m->N, m->D, m->DP,
+                                                                         m->S, std, c, n_splits, n_rows_pad, parts,
+                                                                         E_dev, F_dev, W_dev);
+      else
+        k_predict_finish_small<<<(unsigned)n_geo, 1024, fds_bytes, s>>>(w.G, w.Erow, gq, m->perm, m->N, m->D, m->DP, m->S, std, c,
+                                                                       n_splits, n_rows_pad, parts, E_dev, F_dev);
+    } else if (W_dev != nullptr) {
+      k_predict_finish_w<<<(unsigned)((n_geo + QPB - 1) / QPB), 128, fd_bytes, s>>>(
+          w.G, w.Erow, gq, m->perm, m->N, m->D, m->DP, m->S, std, c, n_splits, n_rows_pad, n_geo, QPB, E_dev, F_dev,
+          W_dev);
     } else {
       k_predict_finish<<<(unsigned)((n_geo + QPB - 1) / QPB), 128, fd_bytes, s>>>(w.G, w.Erow, gq, m->perm, m->N, m->D,
                                                                                  m->DP, m->S, std, c, n_splits,
@@ -1602,15 +1830,24 @@ void free_graph_slot(sgdml_b200_model::GraphSlot& g) {
   cudaFreeHost(g.hR);
   cudaFreeHost(g.hF);
   cudaFreeHost(g.hE);
+  cudaFreeHost(g.hW);
+  cudaFreeHost(g.hLat);
+  cached_free(g.dLat);
   g = sgdml_b200_model::GraphSlot();
 }
 
 // Small host-buffer batch (molecular dynamics: one geometry per call, ase_calc.py:98-110): pinned staging buffers and
 // the whole launch sequence (H2D copy, descriptor kernel, query rows, main kernel, finishing kernel, D2H copies)
 // replayed from a CUDA graph -- one launch call instead of seven.
-int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, double* E, double* F, cudaStream_t s) {
+// W != nullptr (sgdml_b200_predict_virial): the slot also stages W, and the cell `lat` of the call travels with the
+// geometries -- staged in pinned memory and read there by the descriptor kernel (zero copy) or copied to the device by
+// the graph's first nodes (copy-node form) -- so a call with a new cell replays the graph: no capture, no device
+// synchronisation.
+int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lattice& lat, double* E, double* F,
+                  double* W, cudaStream_t s) {
   const int dimi = 3 * m->N;
   const int with_E = E != nullptr ? 1 : 0;
+  const int with_W = W != nullptr ? 1 : 0;
   SG_TRY(ensure_ws(m, 0, n_geo));
   if (m->graph_stream == nullptr) {
     SG_CUDA(cudaStreamCreateWithFlags(&m->graph_stream, cudaStreamNonBlocking));
@@ -1620,7 +1857,9 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, double* E
   sgdml_b200_model::WS& w = m->ws[0];
   sgdml_b200_model::GraphSlot* g = nullptr;
   for (auto& c : m->graphs)
-    if (c.exec != nullptr && c.n_geo == n_geo && c.with_E == with_E && c.generation == m->generation) g = &c;
+    if (c.exec != nullptr && c.n_geo == n_geo && c.with_E == with_E && c.with_W == with_W &&
+        c.generation == m->generation)
+      g = &c;
   // Three kernel nodes and no copy nodes: the first kernel reads the geometries straight from the pinned staging
   // buffer (unified addressing) and builds descriptors + query rows, the finishing kernel stores E and F straight
   // into pinned host memory.  SGDML_B200_GRAPH_ZEROCOPY=0: the earlier form (H2D copy, descriptor kernel, query-row
@@ -1631,20 +1870,34 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, double* E
     if (zero_copy) {
       const int64_t n_rows = n_geo * m->S;
       const int64_t n_rows_pad = (n_rows + m->BQ - 1) / m->BQ * m->BQ;
-      if (dq_bytes > 48 * 1024)
-        SG_CUDA(cudaFuncSetAttribute(k_desc_query_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_bytes));
-      k_desc_query_rows<<<(unsigned)n_geo, 256, dq_bytes, gs>>>(q->hR, m->N, m->pinv, m->mu, m->D, m->DS, m->S, n_rows,
-                                                               n_rows_pad, w.gq, w.Qg, w.qq, m->lat);
+      if (with_W) {
+        // (the Lattice in static shared memory counts against the 48 KB default)
+        if (dq_bytes > 46 * 1024)
+          SG_CUDA(cudaFuncSetAttribute(k_desc_query_rows_lp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_bytes));
+        k_desc_query_rows_lp<<<(unsigned)n_geo, 256, dq_bytes, gs>>>(q->hR, m->N, m->pinv, m->mu, m->D, m->DS, m->S,
+                                                                    n_rows, n_rows_pad, w.gq, w.Qg, w.qq, q->hLat);
+      } else {
+        if (dq_bytes > 48 * 1024)
+          SG_CUDA(cudaFuncSetAttribute(k_desc_query_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_bytes));
+        k_desc_query_rows<<<(unsigned)n_geo, 256, dq_bytes, gs>>>(q->hR, m->N, m->pinv, m->mu, m->D, m->DS, m->S, n_rows,
+                                                                 n_rows_pad, w.gq, w.Qg, w.qq, m->lat);
+      }
       SG_CUDA(cudaGetLastError());
       count_launch(KID_PREDICT_AUX);
-      SG_TRY(run_queries(m, 0, nullptr, w.gq, n_geo, m->std, m->c, with_E ? q->hE : nullptr, q->hF, gs));
+      SG_TRY(run_queries(m, 0, nullptr, w.gq, n_geo, m->std, m->c, with_E ? q->hE : nullptr, q->hF, gs, q->hW));
       return 0;
     }
     SG_CUDA(cudaMemcpyAsync(w.R, q->hR, sizeof(double) * n_geo * dimi, cudaMemcpyHostToDevice, gs));
-    SG_TRY(launch_desc_from_R(w.R, n_geo, m->N, w.xq, w.gq, gs, &m->lat));
-    SG_TRY(run_queries(m, 0, w.xq, w.gq, n_geo, m->std, m->c, with_E ? w.E : nullptr, w.F, gs));
+    if (with_W) {
+      SG_CUDA(cudaMemcpyAsync(q->dLat, q->hLat, sizeof(Lattice), cudaMemcpyHostToDevice, gs));
+      SG_TRY(launch_desc_from_R_lp(w.R, n_geo, m->N, w.xq, w.gq, gs, q->dLat));
+    } else {
+      SG_TRY(launch_desc_from_R(w.R, n_geo, m->N, w.xq, w.gq, gs, &m->lat));
+    }
+    SG_TRY(run_queries(m, 0, w.xq, w.gq, n_geo, m->std, m->c, with_E ? w.E : nullptr, w.F, gs, with_W ? w.W : nullptr));
     SG_CUDA(cudaMemcpyAsync(q->hF, w.F, sizeof(double) * n_geo * dimi, cudaMemcpyDeviceToHost, gs));
     if (with_E) SG_CUDA(cudaMemcpyAsync(q->hE, w.E, sizeof(double) * n_geo, cudaMemcpyDeviceToHost, gs));
+    if (with_W) SG_CUDA(cudaMemcpyAsync(q->hW, w.W, sizeof(double) * n_geo * 9, cudaMemcpyDeviceToHost, gs));
     return 0;
   };
   if (g == nullptr) {
@@ -1658,6 +1911,12 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, double* E
     SG_CUDA(cudaMallocHost(&g->hR, sizeof(double) * n_geo * dimi));
     SG_CUDA(cudaMallocHost(&g->hF, sizeof(double) * n_geo * dimi));
     SG_CUDA(cudaMallocHost(&g->hE, sizeof(double) * n_geo));
+    if (with_W) {
+      SG_CUDA(cudaMallocHost(&g->hW, sizeof(double) * n_geo * 9));
+      SG_CUDA(cudaMallocHost(&g->hLat, sizeof(Lattice)));
+      SG_CUDA(cached_malloc(&g->dLat, sizeof(Lattice)));
+      *g->hLat = lat;
+    }
     std::copy(R, R + n_geo * dimi, g->hR);
     // first call: run the sequence un-captured (sets the kernels' shared-memory attributes) ...
     SG_TRY(enqueue(g));
@@ -1689,16 +1948,86 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, double* E
     g->n_kernels = (int)(after - before);
     g->n_geo = n_geo;
     g->with_E = with_E;
+    g->with_W = with_W;
     g->generation = m->generation;
   } else {
     // replay on the CALLER's stream: ordered after whatever it has queued, no event round trip
     std::copy(R, R + n_geo * dimi, g->hR);
+    if (with_W) *g->hLat = lat;  // the previous replay has finished (synchronised below): the slot is free
     SG_CUDA(cudaGraphLaunch(g->exec, s));
     count_launch(KID_PREDICT_AUX, g->n_kernels);  // the kernels of a replay are launches too
     SG_CUDA(cudaStreamSynchronize(s));
   }
   std::copy(g->hF, g->hF + n_geo * dimi, F);
   if (with_E) std::copy(g->hE, g->hE + n_geo, E);
+  if (with_W) std::copy(g->hW, g->hW + n_geo * 9, W);
+  return 0;
+}
+
+// sgdml_b200_predict and sgdml_b200_predict_virial: `lat` is the cell of this call's descriptors; W == nullptr: no
+// virial (the plain finishing kernels)
+int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lattice& lat, double* E, double* F,
+                 double* W, cudaStream_t s) {
+  const bool R_dev = is_device_ptr(R), F_dev = is_device_ptr(F), E_dev = (E != nullptr) && is_device_ptr(E);
+  const bool W_dev = (W != nullptr) && is_device_ptr(W);
+  const bool host_io = !R_dev || !F_dev || (E != nullptr && !E_dev) || (W != nullptr && !W_dev);
+  const int dimi = 3 * m->N;
+  if (!R_dev && !F_dev && (E == nullptr || !E_dev) && (W == nullptr || !W_dev) && n_geo <= GRAPH_MAX_GEO &&
+      !profiling_enabled() && g_graph_enabled())
+    return predict_graph(m, R, n_geo, lat, E, F, W, s);
+  int64_t chunk = std::min<int64_t>(chunk_geos(m), n_geo);
+  // Host buffers: split the batch into >= 4 chunks and run them on two side streams so that the
+  // H2D copy of chunk k+1 and the D2H copy of chunk k-1 overlap the kernels of chunk k.
+  const bool pipelined = host_io && n_geo >= 4096 && !profiling_enabled();
+  if (pipelined) chunk = std::min<int64_t>(chunk, std::max<int64_t>(1024, (n_geo + 3) / 4));
+  SG_TRY(ensure_ws(m, 0, chunk));
+  if (pipelined) {
+    SG_TRY(ensure_ws(m, 1, chunk));
+    SG_TRY(ensure_pipe(m));
+    SG_CUDA(cudaEventRecord(m->pipe_event[2], s));
+    SG_CUDA(cudaStreamWaitEvent(m->pipe_stream[0], m->pipe_event[2], 0));
+    SG_CUDA(cudaStreamWaitEvent(m->pipe_stream[1], m->pipe_event[2], 0));
+  }
+  int c_idx = 0;
+  for (int64_t g0 = 0; g0 < n_geo; g0 += chunk, ++c_idx) {
+    const int slot = pipelined ? (c_idx & 1) : 0;
+    cudaStream_t st = pipelined ? m->pipe_stream[slot] : s;
+    sgdml_b200_model::WS& w = m->ws[slot];
+    const int64_t ng = std::min<int64_t>(chunk, n_geo - g0);
+    const double* Rd = R + g0 * dimi;
+    if (!R_dev) {
+      SG_CUDA(cudaMemcpyAsync(w.R, Rd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, st));
+      Rd = w.R;
+    }
+    SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, st, &lat));
+    double* Fd = F_dev ? F + g0 * dimi : w.F;
+    double* Ed = (E == nullptr) ? nullptr : (E_dev ? E + g0 : w.E);
+    double* Wd = (W == nullptr) ? nullptr : (W_dev ? W + g0 * 9 : w.W);
+    SG_TRY(run_queries(m, slot, w.xq, w.gq, ng, m->std, m->c, Ed, Fd, st, Wd));
+    if (!F_dev) SG_CUDA(cudaMemcpyAsync(F + g0 * dimi, Fd, sizeof(double) * ng * dimi, cudaMemcpyDeviceToHost, st));
+    if (E != nullptr && !E_dev) SG_CUDA(cudaMemcpyAsync(E + g0, Ed, sizeof(double) * ng, cudaMemcpyDeviceToHost, st));
+    if (W != nullptr && !W_dev) SG_CUDA(cudaMemcpyAsync(W + g0 * 9, Wd, sizeof(double) * ng * 9, cudaMemcpyDeviceToHost, st));
+  }
+  if (pipelined) {
+    for (int i = 0; i < 2; ++i) {
+      SG_CUDA(cudaEventRecord(m->pipe_event[i], m->pipe_stream[i]));
+      SG_CUDA(cudaStreamWaitEvent(s, m->pipe_event[i], 0));
+    }
+  }
+  if (host_io) SG_CUDA(cudaStreamSynchronize(s));
+  return 0;
+}
+
+// A cell given to sgdml_b200_predict_virial: host arrays (lattice_from_host), finite, and not singular
+int lattice_for_call(const double* lattice, const double* lattice_inv, Lattice* l) {
+  SG_TRY(lattice_from_host(lattice, lattice_inv, l));
+  if (!l->on) return 0;
+  for (int i = 0; i < 9; ++i)
+    if (!std::isfinite(l->vec[i]) || !std::isfinite(l->inv[i])) return fail_arg("the cell must be finite");
+  const double* a = l->vec;
+  const double det = a[0] * (a[4] * a[8] - a[5] * a[7]) - a[1] * (a[3] * a[8] - a[5] * a[6]) +
+                     a[2] * (a[3] * a[7] - a[4] * a[6]);
+  if (!(det != 0.0)) return fail_arg("the cell is singular");
   return 0;
 }
 
@@ -1739,52 +2068,19 @@ int sgdml_b200_predict(sgdml_b200_model* m, const double* R, int64_t n_geo, doub
   SG_TRY(require_device());
   SG_ARG(m != nullptr && R != nullptr && F != nullptr && n_geo >= 0);
   if (n_geo == 0) return 0;
-  cudaStream_t s = (cudaStream_t)stream;
-  const bool R_dev = is_device_ptr(R), F_dev = is_device_ptr(F), E_dev = (E != nullptr) && is_device_ptr(E);
-  const bool host_io = !R_dev || !F_dev || (E != nullptr && !E_dev);
-  const int dimi = 3 * m->N;
-  if (!R_dev && !F_dev && (E == nullptr || !E_dev) && n_geo <= GRAPH_MAX_GEO && !profiling_enabled() &&
-      g_graph_enabled())
-    return predict_graph(m, R, n_geo, E, F, s);
-  int64_t chunk = std::min<int64_t>(chunk_geos(m), n_geo);
-  // Host buffers: split the batch into >= 4 chunks and run them on two side streams so that the
-  // H2D copy of chunk k+1 and the D2H copy of chunk k-1 overlap the kernels of chunk k.
-  const bool pipelined = host_io && n_geo >= 4096 && !profiling_enabled();
-  if (pipelined) chunk = std::min<int64_t>(chunk, std::max<int64_t>(1024, (n_geo + 3) / 4));
-  SG_TRY(ensure_ws(m, 0, chunk));
-  if (pipelined) {
-    SG_TRY(ensure_ws(m, 1, chunk));
-    SG_TRY(ensure_pipe(m));
-    SG_CUDA(cudaEventRecord(m->pipe_event[2], s));
-    SG_CUDA(cudaStreamWaitEvent(m->pipe_stream[0], m->pipe_event[2], 0));
-    SG_CUDA(cudaStreamWaitEvent(m->pipe_stream[1], m->pipe_event[2], 0));
-  }
-  int c_idx = 0;
-  for (int64_t g0 = 0; g0 < n_geo; g0 += chunk, ++c_idx) {
-    const int slot = pipelined ? (c_idx & 1) : 0;
-    cudaStream_t st = pipelined ? m->pipe_stream[slot] : s;
-    sgdml_b200_model::WS& w = m->ws[slot];
-    const int64_t ng = std::min<int64_t>(chunk, n_geo - g0);
-    const double* Rd = R + g0 * dimi;
-    if (!R_dev) {
-      SG_CUDA(cudaMemcpyAsync(w.R, Rd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, st));
-      Rd = w.R;
-    }
-    SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, st, &m->lat));
-    double* Fd = F_dev ? F + g0 * dimi : w.F;
-    double* Ed = (E == nullptr) ? nullptr : (E_dev ? E + g0 : w.E);
-    SG_TRY(run_queries(m, slot, w.xq, w.gq, ng, m->std, m->c, Ed, Fd, st));
-    if (!F_dev) SG_CUDA(cudaMemcpyAsync(F + g0 * dimi, Fd, sizeof(double) * ng * dimi, cudaMemcpyDeviceToHost, st));
-    if (E != nullptr && !E_dev) SG_CUDA(cudaMemcpyAsync(E + g0, Ed, sizeof(double) * ng, cudaMemcpyDeviceToHost, st));
-  }
-  if (pipelined) {
-    for (int i = 0; i < 2; ++i) {
-      SG_CUDA(cudaEventRecord(m->pipe_event[i], m->pipe_stream[i]));
-      SG_CUDA(cudaStreamWaitEvent(s, m->pipe_event[i], 0));
-    }
-  }
-  if (host_io) SG_CUDA(cudaStreamSynchronize(s));
-  return 0;
+  return predict_impl(m, R, n_geo, m->lat, E, F, nullptr, (cudaStream_t)stream);
+}
+
+int sgdml_b200_predict_virial(sgdml_b200_model* m, const double* R, int64_t n_geo, const double* lattice,
+                              const double* lattice_inv, double* E, double* F, double* W, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(m != nullptr && R != nullptr && F != nullptr && W != nullptr && n_geo >= 0);
+  // parsed into a local: the model's own cell is never touched, and a rejected cell changes nothing
+  Lattice l;
+  SG_TRY(lattice_for_call(lattice, lattice_inv, &l));
+  if (lattice == nullptr) l = m->lat;
+  if (n_geo == 0) return 0;
+  return predict_impl(m, R, n_geo, l, E, F, W, (cudaStream_t)stream);
 }
 
 int sgdml_b200_model_set_lattice(sgdml_b200_model* m, const double* lattice, const double* lattice_inv) {

@@ -240,29 +240,100 @@ class GDMLPredict(object):
         )
         return (E, F) if return_E else (F,)
 
+    def predict_virial(self, R, lattice=None, return_E=True, out=None):
+        """Extension (the reference has no such output): `predict` plus the virial W of every geometry, optionally in a
+        cell given for this call.  R (B, 3N) [or (3N,)] -> (E (B,), F (B, 3N), W (B, 3, 3)) or (F, W).
+
+        With the rows r_i of a geometry and the cell L (lattice vectors as COLUMNS, model units, as model['lattice'])
+        strained homogeneously, r_i -> (I + eps) r_i and L -> (I + eps) L:
+            W = -dE/d(eps) at eps = 0 = sum_d (dE/dx_d) delta_d delta_d^T / |delta_d|^3,
+        symmetric and in the model's energy unit, with x_d = 1/|delta_d| and delta_d = r_a - r_b - L rint(L^-1 (r_a - r_b))
+        the minimum-image vector of pair d.  For a free molecule W equals sum_i r_i F_i^T; the stress of a periodic
+        system is -W / V.  E and F are bit-identical to `predict` in the same cell.
+
+        lattice: (3, 3) cell for this call (its inverse from np.linalg.inv); None: the model's own cell, or none for a
+        free-molecule model.  The model keeps its cell either way.  `out=(E, F, W)`: preallocated outputs as for
+        `predict`, W of shape (B, 3, 3).  NumPy / torch conventions as `predict`: CUDA tensors in place, pinned in ->
+        pinned out."""
+        L = _lib.lib()
+        dim_i = 3 * self.n_atoms
+        lat = lat_inv = None
+        if lattice is not None:
+            lat = np.ascontiguousarray(np.asarray(lattice, dtype=np.float64))
+            if lat.shape != (3, 3):
+                raise ValueError('lattice must be a 3 x 3 matrix (lattice vectors as columns)')
+            lat_inv = np.ascontiguousarray(np.linalg.inv(lat))
+        if isinstance(R, np.ndarray) or not hasattr(R, 'data_ptr'):
+            R = np.ascontiguousarray(R, dtype=np.float64)
+            if R.ndim == 1:
+                R = R[None, :]
+            if R.size % dim_i != 0 or (R.ndim == 2 and R.shape[1] != dim_i):
+                raise ValueError('R must have 3*n_atoms columns')
+            R = R.reshape(-1, dim_i)
+            n = R.shape[0]
+            if out is not None:
+                E, F, W = out
+            else:
+                F = np.empty((n, dim_i))
+                E = np.empty(n) if return_E else None
+                W = np.empty((n, 3, 3))
+        else:
+            import torch
+
+            if R.dtype != torch.float64:
+                raise ValueError('torch inputs must be float64')
+            R = R.contiguous().reshape(-1, dim_i) if R.dim() != 1 else R.contiguous().reshape(1, dim_i)
+            n = R.shape[0]
+            if out is not None:
+                E, F, W = out
+            else:
+                pin = (not R.is_cuda) and R.is_pinned()
+                F = torch.empty((n, dim_i), dtype=torch.float64, device=R.device, pin_memory=pin)
+                E = torch.empty((n,), dtype=torch.float64, device=R.device, pin_memory=pin) if return_E else None
+                W = torch.empty((n, 3, 3), dtype=torch.float64, device=R.device, pin_memory=pin)
+        if not return_E:
+            E = None
+        if out is not None:
+            if W is None:
+                raise ValueError('out must hold a W buffer')
+            self._check_out(R, E, F, n, dim_i)
+            self._check_buf(R, W, (n, 3, 3), 'W')
+        _lib.check(
+            L.sgdml_b200_predict_virial(
+                self._handle, _lib.ptr(R), n, _lib.ptr(lat), _lib.ptr(lat_inv), _lib.ptr(E), _lib.ptr(F), _lib.ptr(W),
+                _lib.current_stream(),
+            ),
+            'predict_virial',
+        )
+        return (E, F, W) if return_E else (F, W)
+
     @staticmethod
     def _check_out(R, E, F, n, dim_i):
         """Output buffers go to the engine as raw double*: wrong dtype / layout / device would corrupt memory."""
         for buf, shape, name in ((F, (n, dim_i), 'F'), (E, (n,), 'E')):
-            if buf is None:
-                continue
-            if tuple(buf.shape) != shape:
-                raise ValueError('out buffer %s has the wrong shape %s (expected %s)' % (name, tuple(buf.shape), shape))
-            if isinstance(buf, np.ndarray):
-                if buf.dtype != np.float64 or not buf.flags['C_CONTIGUOUS'] or not buf.flags['WRITEABLE']:
-                    raise ValueError('out buffer %s must be a writeable C-contiguous float64 array' % name)
-                if not isinstance(R, np.ndarray) and R.is_cuda:
-                    raise ValueError('out buffer %s is a host array but R is a CUDA tensor' % name)
-            else:
-                import torch
+            GDMLPredict._check_buf(R, buf, shape, name)
 
-                if buf.dtype != torch.float64 or not buf.is_contiguous():
-                    raise ValueError('out buffer %s must be a contiguous float64 tensor' % name)
-                r_dev = None if isinstance(R, np.ndarray) else R.device
-                if buf.is_cuda and (r_dev is None or buf.device != r_dev):
-                    raise ValueError('out buffer %s lives on %s but R does not' % (name, buf.device))
-                if (not buf.is_cuda) and r_dev is not None and r_dev.type == 'cuda':
-                    raise ValueError('out buffer %s is a host tensor but R is a CUDA tensor' % name)
+    @staticmethod
+    def _check_buf(R, buf, shape, name):
+        if buf is None:
+            return
+        if tuple(buf.shape) != shape:
+            raise ValueError('out buffer %s has the wrong shape %s (expected %s)' % (name, tuple(buf.shape), shape))
+        if isinstance(buf, np.ndarray):
+            if buf.dtype != np.float64 or not buf.flags['C_CONTIGUOUS'] or not buf.flags['WRITEABLE']:
+                raise ValueError('out buffer %s must be a writeable C-contiguous float64 array' % name)
+            if not isinstance(R, np.ndarray) and R.is_cuda:
+                raise ValueError('out buffer %s is a host array but R is a CUDA tensor' % name)
+        else:
+            import torch
+
+            if buf.dtype != torch.float64 or not buf.is_contiguous():
+                raise ValueError('out buffer %s must be a contiguous float64 tensor' % name)
+            r_dev = None if isinstance(R, np.ndarray) else R.device
+            if buf.is_cuda and (r_dev is None or buf.device != r_dev):
+                raise ValueError('out buffer %s lives on %s but R does not' % (name, buf.device))
+            if (not buf.is_cuda) and r_dev is not None and r_dev.type == 'cuda':
+                raise ValueError('out buffer %s is a host tensor but R is a CUDA tensor' % name)
 
     def kmatvec_train(self, m_begin=0, m_end=None, out=None, E_out=None):
         """Raw (std = 1, c = 0) force sums on training points [m_begin, m_end): the K.v operator

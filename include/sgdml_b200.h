@@ -115,6 +115,17 @@ int sgdml_b200_predict(sgdml_b200_model* model, const double* R, int64_t n_geo, 
 int sgdml_b200_predict_virial(sgdml_b200_model* model, const double* R, int64_t n_geo, const double* lattice,
                               const double* lattice_inv, double* E, double* F, double* W, void* stream);
 
+/* Extension: sgdml_b200_predict_virial with one cell per geometry (variable-cell trajectories, NPT replicas).
+ *   lattices, lattice_invs: (B, 9) HOST doubles each, row-major per geometry, lattice vectors as columns, as for
+ *   sgdml_b200_predict_virial; geometry g is evaluated in cell g.  Device pointers are rejected.  R, E [may be NULL], F
+ *   and W: host or device as in sgdml_b200_predict.
+ * Every cell is checked (finite, not singular) before any work is queued; a rejected call writes nothing and changes
+ * nothing.  With every cell equal to L, E, F and W are bit-identical to sgdml_b200_predict_virial in L.  Small host
+ * batches replay a captured CUDA graph that reads the cells from its pinned staging at run time, so new cells neither
+ * capture again nor synchronise the device. */
+int sgdml_b200_predict_virial_cells(sgdml_b200_model* model, const double* R, int64_t n_geo, const double* lattices,
+                                    const double* lattice_invs, double* E, double* F, double* W, void* stream);
+
 /* Periodic model (predict.py:332-334: lat_and_inv from model['lattice']): query descriptors of
  * sgdml_b200_predict are built with the minimum-image convention.  Both NULL: back to a free molecule. */
 int sgdml_b200_model_set_lattice(sgdml_b200_model* model, const double* lattice, const double* lattice_inv);
@@ -141,6 +152,12 @@ int sgdml_b200_model_set_alphas(sgdml_b200_model* model, const double* alphas_F,
  * raw sums (std = 1, c = 0), i.e. F = (K v)[m_begin*3N : m_end*3N] for alphas = v. */
 int sgdml_b200_predict_train(sgdml_b200_model* model, int64_t m_begin, int64_t m_end, int scaled,
                              double* E, double* F, void* stream);
+
+/* Extension: sgdml_b200_predict_train plus the virial W (B, 9) of each training point (see sgdml_b200_predict_virial),
+ * with the same `scaled` semantics; E and F are bit-identical to sgdml_b200_predict_train.  W comes from the cached
+ * training Jacobians (sgdml_b200_model_set_R_d_desc), so it is in the cell those were built in. */
+int sgdml_b200_predict_train_virial(sgdml_b200_model* model, int64_t m_begin, int64_t m_end, int scaled,
+                                    double* E, double* F, double* W, void* stream);
 
 /* Large-descriptor models (D > 256: the predictor is four GEMMs around two element-wise kernels): run those GEMMs on
  * the int8 tensor cores (wgmma) through `slices` exact int8 slices per operand (2..7; csrc/ozaki.cu) or in FP64 DMMA (0, the

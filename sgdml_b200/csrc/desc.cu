@@ -55,6 +55,16 @@ __global__ void k_desc_from_R_lp(const double* __restrict__ R, int64_t n_geo, in
   __syncthreads();
   desc_from_R_body(R, n_geo, n_atoms, dim_d, R_desc, R_d_desc, lat);
 }
+// the same with one cell per geometry in device memory (sgdml_b200_predict_virial_cells): lats[g] is the cell of
+// geometry g.  With small D one block spans several geometries, so every thread reads its own geometry's cell (152 B,
+// shared through L1 by the D threads of that geometry)
+__global__ void k_desc_from_R_cells(const double* __restrict__ R, int64_t n_geo, int n_atoms, int dim_d,
+                                    double* __restrict__ R_desc, double* __restrict__ R_d_desc,
+                                    const Lattice* __restrict__ lats) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_geo * dim_d) return;
+  desc_from_R_body(R, n_geo, n_atoms, dim_d, R_desc, R_d_desc, lats[idx / dim_d]);
+}
 
 // ---------------------------------------------------------------- a-D3: (J v)_d = g_d . (v_b - v_a)
 // reference: utils/desc.py:368-385
@@ -125,6 +135,18 @@ int launch_desc_from_R_lp(const double* R, int64_t n_geo, int n_atoms, double* R
   int64_t total = n_geo * D;
   ProfScope ps(KID_DESC, s);
   k_desc_from_R_lp<<<ceil_div(total, 256), 256, 0, s>>>(R, n_geo, n_atoms, D, R_desc, R_d_desc, lat_dev);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_DESC);
+  return 0;
+}
+
+int launch_desc_from_R_cells(const double* R, int64_t n_geo, int n_atoms, double* R_desc, double* R_d_desc,
+                             cudaStream_t s, const Lattice* lats_dev) {
+  if (n_geo == 0) return 0;
+  const int D = n_atoms * (n_atoms - 1) / 2;
+  int64_t total = n_geo * D;
+  ProfScope ps(KID_DESC, s);
+  k_desc_from_R_cells<<<ceil_div(total, 256), 256, 0, s>>>(R, n_geo, n_atoms, D, R_desc, R_d_desc, lats_dev);
   SG_CUDA(cudaGetLastError());
   count_launch(KID_DESC);
   return 0;

@@ -33,6 +33,9 @@ int launch_desc_from_R(const double* R, int64_t n_geo, int n_atoms, double* R_de
 // the same with the cell read by the kernel from DEVICE memory at lat_dev (a captured graph's per-call cell)
 int launch_desc_from_R_lp(const double* R, int64_t n_geo, int n_atoms, double* R_desc, double* R_d_desc,
                           cudaStream_t s, const Lattice* lat_dev);
+// one cell per geometry: lats_dev (n_geo) in DEVICE memory, cell g for geometry g
+int launch_desc_from_R_cells(const double* R, int64_t n_geo, int n_atoms, double* R_desc, double* R_d_desc,
+                             cudaStream_t s, const Lattice* lats_dev);
 int launch_d_desc_dot_vec(const double* R_d_desc, const double* vecs, int64_t n_geo, int n_atoms, double* out,
                           int64_t out_stride, cudaStream_t s);
 int launch_vec_dot_d_desc(const double* R_d_desc, const double* vecs, int64_t n_geo, int n_atoms,

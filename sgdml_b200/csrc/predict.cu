@@ -695,6 +695,17 @@ __global__ void __launch_bounds__(256) k_desc_query_rows_lp(const double* __rest
   __syncthreads();
   desc_query_rows_body(R, n_atoms, pinv, mu, D, DS, S, n_rows, n_rows_pad, gq, Qg, qqg, lat);
 }
+// One cell per geometry (sgdml_b200_predict_virial_cells): CTA b reads cell b of the array staged next to R
+__global__ void __launch_bounds__(256) k_desc_query_rows_cells(const double* __restrict__ R, int n_atoms,
+                                                               const int* __restrict__ pinv, const double* __restrict__ mu,
+                                                               int D, int DS, int S, int64_t n_rows, int64_t n_rows_pad,
+                                                               double* __restrict__ gq, double* __restrict__ Qg,
+                                                               double* __restrict__ qqg, const Lattice* __restrict__ lats) {
+  __shared__ Lattice lat;
+  if (threadIdx.x == 0) lat = lats[blockIdx.x];
+  __syncthreads();
+  desc_query_rows_body(R, n_atoms, pinv, mu, D, DS, S, n_rows, n_rows_pad, gq, Qg, qqg, lat);
+}
 
 // ============================================================== large descriptors (D > 256)
 // The accumulator tile G (BQ x DP) of the fused kernel no longer fits the register file, so the
@@ -1294,6 +1305,7 @@ struct sgdml_b200_model {
     double* Fd = nullptr;       // (geo, D) F_desc of long descriptors (fdesc_in_ws)
     double* W = nullptr;        // (geo, 9) virial staging for host outputs
     double* Wp = nullptr;       // (geo, ceil(D / 256), 6) per-CTA virial partials of k_fdesc_gather_w (fdesc_in_ws)
+    Lattice* lat = nullptr;     // (geo) one cell per geometry (sgdml_b200_predict_virial_cells)
     OzOperand ozQ, ozC1, ozC2;  // slices of the per-batch operands (int8 path of large descriptors)
   } ws[2];
   cudaStream_t pipe_stream[2] = {nullptr, nullptr};
@@ -1303,11 +1315,12 @@ struct sgdml_b200_model {
     int64_t n_geo = 0;
     int with_E = 0;
     int with_W = 0;  // sgdml_b200_predict_virial: the cell is read from hLat at run time, not baked in
+    int cells = 0;   // sgdml_b200_predict_virial_cells: hLat / dLat hold one cell per geometry
     int n_kernels = 0;
     uint64_t generation = 0;
     cudaGraphExec_t exec = nullptr;
     double *hR = nullptr, *hF = nullptr, *hE = nullptr, *hW = nullptr;  // pinned staging
-    Lattice* hLat = nullptr;  // pinned: the call's cell (with_W)
+    Lattice* hLat = nullptr;  // pinned: the call's cell, or n_geo cells (with_W)
     Lattice* dLat = nullptr;  // device copy of hLat (with_W, copy-node form)
   } graphs[4];
   int graph_next = 0;
@@ -1408,6 +1421,7 @@ void free_ws(sgdml_b200_model* m) {
     cached_free(w.Fd);
     cached_free(w.W);
     cached_free(w.Wp);
+    cached_free(w.lat);
     w = sgdml_b200_model::WS();
   }
 }
@@ -1443,9 +1457,11 @@ int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
   cached_free(w.Fd);
   cached_free(w.W);
   cached_free(w.Wp);
+  cached_free(w.lat);
   w = sgdml_b200_model::WS();
   SG_CUDA(cached_malloc(&w.xq, sizeof(double) * n_geo * m->D));
   SG_CUDA(cached_malloc(&w.W, sizeof(double) * n_geo * 9));
+  SG_CUDA(cached_malloc(&w.lat, sizeof(Lattice) * n_geo));
   if (fdesc_in_ws(m)) SG_CUDA(cached_malloc(&w.Wp, sizeof(double) * n_geo * ceil_div(m->D, 256) * 6));
   SG_CUDA(cached_malloc(&w.gq, sizeof(double) * n_geo * m->D * 3));
   {
@@ -1843,11 +1859,15 @@ void free_graph_slot(sgdml_b200_model::GraphSlot& g) {
 // geometries -- staged in pinned memory and read there by the descriptor kernel (zero copy) or copied to the device by
 // the graph's first nodes (copy-node form) -- so a call with a new cell replays the graph: no capture, no device
 // synchronisation.
+// cells != nullptr (sgdml_b200_predict_virial_cells, with W): n_geo host cells, one per geometry, staged the same way
+// (k_desc_query_rows_cells / k_desc_from_R_cells); such graphs live in slots of their own.
 int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lattice& lat, double* E, double* F,
-                  double* W, cudaStream_t s) {
+                  double* W, cudaStream_t s, const Lattice* cells = nullptr) {
   const int dimi = 3 * m->N;
   const int with_E = E != nullptr ? 1 : 0;
   const int with_W = W != nullptr ? 1 : 0;
+  const int with_cells = cells != nullptr ? 1 : 0;
+  const int64_t n_lat = with_cells ? n_geo : 1;  // cells staged in hLat / dLat
   SG_TRY(ensure_ws(m, 0, n_geo));
   if (m->graph_stream == nullptr) {
     SG_CUDA(cudaStreamCreateWithFlags(&m->graph_stream, cudaStreamNonBlocking));
@@ -1857,7 +1877,7 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
   sgdml_b200_model::WS& w = m->ws[0];
   sgdml_b200_model::GraphSlot* g = nullptr;
   for (auto& c : m->graphs)
-    if (c.exec != nullptr && c.n_geo == n_geo && c.with_E == with_E && c.with_W == with_W &&
+    if (c.exec != nullptr && c.n_geo == n_geo && c.with_E == with_E && c.with_W == with_W && c.cells == with_cells &&
         c.generation == m->generation)
       g = &c;
   // Three kernel nodes and no copy nodes: the first kernel reads the geometries straight from the pinned staging
@@ -1870,7 +1890,12 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
     if (zero_copy) {
       const int64_t n_rows = n_geo * m->S;
       const int64_t n_rows_pad = (n_rows + m->BQ - 1) / m->BQ * m->BQ;
-      if (with_W) {
+      if (with_cells) {
+        if (dq_bytes > 46 * 1024)
+          SG_CUDA(cudaFuncSetAttribute(k_desc_query_rows_cells, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_bytes));
+        k_desc_query_rows_cells<<<(unsigned)n_geo, 256, dq_bytes, gs>>>(q->hR, m->N, m->pinv, m->mu, m->D, m->DS, m->S,
+                                                                       n_rows, n_rows_pad, w.gq, w.Qg, w.qq, q->hLat);
+      } else if (with_W) {
         // (the Lattice in static shared memory counts against the 48 KB default)
         if (dq_bytes > 46 * 1024)
           SG_CUDA(cudaFuncSetAttribute(k_desc_query_rows_lp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_bytes));
@@ -1888,7 +1913,10 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
       return 0;
     }
     SG_CUDA(cudaMemcpyAsync(w.R, q->hR, sizeof(double) * n_geo * dimi, cudaMemcpyHostToDevice, gs));
-    if (with_W) {
+    if (with_cells) {
+      SG_CUDA(cudaMemcpyAsync(q->dLat, q->hLat, sizeof(Lattice) * n_lat, cudaMemcpyHostToDevice, gs));
+      SG_TRY(launch_desc_from_R_cells(w.R, n_geo, m->N, w.xq, w.gq, gs, q->dLat));
+    } else if (with_W) {
       SG_CUDA(cudaMemcpyAsync(q->dLat, q->hLat, sizeof(Lattice), cudaMemcpyHostToDevice, gs));
       SG_TRY(launch_desc_from_R_lp(w.R, n_geo, m->N, w.xq, w.gq, gs, q->dLat));
     } else {
@@ -1913,9 +1941,12 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
     SG_CUDA(cudaMallocHost(&g->hE, sizeof(double) * n_geo));
     if (with_W) {
       SG_CUDA(cudaMallocHost(&g->hW, sizeof(double) * n_geo * 9));
-      SG_CUDA(cudaMallocHost(&g->hLat, sizeof(Lattice)));
-      SG_CUDA(cached_malloc(&g->dLat, sizeof(Lattice)));
-      *g->hLat = lat;
+      SG_CUDA(cudaMallocHost(&g->hLat, sizeof(Lattice) * n_lat));
+      SG_CUDA(cached_malloc(&g->dLat, sizeof(Lattice) * n_lat));
+      if (with_cells)
+        std::copy(cells, cells + n_geo, g->hLat);
+      else
+        *g->hLat = lat;
     }
     std::copy(R, R + n_geo * dimi, g->hR);
     // first call: run the sequence un-captured (sets the kernels' shared-memory attributes) ...
@@ -1949,11 +1980,16 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
     g->n_geo = n_geo;
     g->with_E = with_E;
     g->with_W = with_W;
+    g->cells = with_cells;
     g->generation = m->generation;
   } else {
     // replay on the CALLER's stream: ordered after whatever it has queued, no event round trip
     std::copy(R, R + n_geo * dimi, g->hR);
-    if (with_W) *g->hLat = lat;  // the previous replay has finished (synchronised below): the slot is free
+    // the previous replay has finished (synchronised below): the slot is free
+    if (with_cells)
+      std::copy(cells, cells + n_geo, g->hLat);
+    else if (with_W)
+      *g->hLat = lat;
     SG_CUDA(cudaGraphLaunch(g->exec, s));
     count_launch(KID_PREDICT_AUX, g->n_kernels);  // the kernels of a replay are launches too
     SG_CUDA(cudaStreamSynchronize(s));
@@ -1965,16 +2001,17 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
 }
 
 // sgdml_b200_predict and sgdml_b200_predict_virial: `lat` is the cell of this call's descriptors; W == nullptr: no
-// virial (the plain finishing kernels)
+// virial (the plain finishing kernels).  cells != nullptr (sgdml_b200_predict_virial_cells): n_geo HOST cells, one per
+// geometry, in place of `lat`; each chunk's cells go to the device on the chunk's stream next to its geometries
 int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lattice& lat, double* E, double* F,
-                 double* W, cudaStream_t s) {
+                 double* W, cudaStream_t s, const Lattice* cells = nullptr) {
   const bool R_dev = is_device_ptr(R), F_dev = is_device_ptr(F), E_dev = (E != nullptr) && is_device_ptr(E);
   const bool W_dev = (W != nullptr) && is_device_ptr(W);
   const bool host_io = !R_dev || !F_dev || (E != nullptr && !E_dev) || (W != nullptr && !W_dev);
   const int dimi = 3 * m->N;
   if (!R_dev && !F_dev && (E == nullptr || !E_dev) && (W == nullptr || !W_dev) && n_geo <= GRAPH_MAX_GEO &&
       !profiling_enabled() && g_graph_enabled())
-    return predict_graph(m, R, n_geo, lat, E, F, W, s);
+    return predict_graph(m, R, n_geo, lat, E, F, W, s, cells);
   int64_t chunk = std::min<int64_t>(chunk_geos(m), n_geo);
   // Host buffers: split the batch into >= 4 chunks and run them on two side streams so that the
   // H2D copy of chunk k+1 and the D2H copy of chunk k-1 overlap the kernels of chunk k.
@@ -1999,7 +2036,12 @@ int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Latt
       SG_CUDA(cudaMemcpyAsync(w.R, Rd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, st));
       Rd = w.R;
     }
-    SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, st, &lat));
+    if (cells != nullptr) {
+      SG_CUDA(cudaMemcpyAsync(w.lat, cells + g0, sizeof(Lattice) * ng, cudaMemcpyHostToDevice, st));
+      SG_TRY(launch_desc_from_R_cells(Rd, ng, m->N, w.xq, w.gq, st, w.lat));
+    } else {
+      SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, st, &lat));
+    }
     double* Fd = F_dev ? F + g0 * dimi : w.F;
     double* Ed = (E == nullptr) ? nullptr : (E_dev ? E + g0 : w.E);
     double* Wd = (W == nullptr) ? nullptr : (W_dev ? W + g0 * 9 : w.W);
@@ -2019,15 +2061,50 @@ int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Latt
 }
 
 // A cell given to sgdml_b200_predict_virial: host arrays (lattice_from_host), finite, and not singular
-int lattice_for_call(const double* lattice, const double* lattice_inv, Lattice* l) {
-  SG_TRY(lattice_from_host(lattice, lattice_inv, l));
-  if (!l->on) return 0;
+int check_cell(const Lattice& l) {
   for (int i = 0; i < 9; ++i)
-    if (!std::isfinite(l->vec[i]) || !std::isfinite(l->inv[i])) return fail_arg("the cell must be finite");
-  const double* a = l->vec;
+    if (!std::isfinite(l.vec[i]) || !std::isfinite(l.inv[i])) return fail_arg("the cell must be finite");
+  const double* a = l.vec;
   const double det = a[0] * (a[4] * a[8] - a[5] * a[7]) - a[1] * (a[3] * a[8] - a[5] * a[6]) +
                      a[2] * (a[3] * a[7] - a[4] * a[6]);
   if (!(det != 0.0)) return fail_arg("the cell is singular");
+  return 0;
+}
+int lattice_for_call(const double* lattice, const double* lattice_inv, Lattice* l) {
+  SG_TRY(lattice_from_host(lattice, lattice_inv, l));
+  if (!l->on) return 0;
+  return check_cell(*l);
+}
+
+// sgdml_b200_predict_train and sgdml_b200_predict_train_virial (W != nullptr)
+int predict_train_impl(sgdml_b200_model* m, int64_t m_begin, int64_t m_end, int scaled, double* E, double* F,
+                       double* W, cudaStream_t s) {
+  if (m->R_d_desc == nullptr) {
+    set_last_error("sgdml_b200_predict_train: call sgdml_b200_model_set_R_d_desc first (predict.py:1223-1229)");
+    return SGDML_B200_ERR_ARG;
+  }
+  const int64_t n_geo = m_end - m_begin;
+  if (n_geo == 0) return 0;
+  const int64_t chunk = std::min<int64_t>(chunk_geos(m), n_geo);
+  SG_TRY(ensure_ws(m, 0, chunk));
+  sgdml_b200_model::WS& w = m->ws[0];
+  const bool F_dev = is_device_ptr(F), E_dev = (E != nullptr) && is_device_ptr(E);
+  const bool W_dev = (W != nullptr) && is_device_ptr(W);
+  const int dimi = 3 * m->N;
+  const double std = scaled ? m->std : 1.0, c = scaled ? m->c : 0.0;
+  for (int64_t g0 = 0; g0 < n_geo; g0 += chunk) {
+    const int64_t ng = std::min<int64_t>(chunk, n_geo - g0);
+    const double* xq = m->X + (m_begin + g0) * m->D;
+    const double* gq = m->R_d_desc + (m_begin + g0) * m->D * 3;
+    double* Fd = F_dev ? F + g0 * dimi : w.F;
+    double* Ed = (E == nullptr) ? nullptr : (E_dev ? E + g0 : w.E);
+    double* Wd = (W == nullptr) ? nullptr : (W_dev ? W + g0 * 9 : w.W);
+    SG_TRY(run_queries(m, 0, xq, gq, ng, std, c, Ed, Fd, s, Wd));
+    if (!F_dev) SG_CUDA(cudaMemcpyAsync(F + g0 * dimi, Fd, sizeof(double) * ng * dimi, cudaMemcpyDeviceToHost, s));
+    if (E != nullptr && !E_dev) SG_CUDA(cudaMemcpyAsync(E + g0, Ed, sizeof(double) * ng, cudaMemcpyDeviceToHost, s));
+    if (W != nullptr && !W_dev) SG_CUDA(cudaMemcpyAsync(W + g0 * 9, Wd, sizeof(double) * ng * 9, cudaMemcpyDeviceToHost, s));
+  }
+  if (!F_dev || (E != nullptr && !E_dev) || (W != nullptr && !W_dev)) SG_CUDA(cudaStreamSynchronize(s));
   return 0;
 }
 
@@ -2081,6 +2158,25 @@ int sgdml_b200_predict_virial(sgdml_b200_model* m, const double* R, int64_t n_ge
   if (lattice == nullptr) l = m->lat;
   if (n_geo == 0) return 0;
   return predict_impl(m, R, n_geo, l, E, F, W, (cudaStream_t)stream);
+}
+
+int sgdml_b200_predict_virial_cells(sgdml_b200_model* m, const double* R, int64_t n_geo, const double* lattices,
+                                    const double* lattice_invs, double* E, double* F, double* W, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(m != nullptr && R != nullptr && F != nullptr && W != nullptr && n_geo >= 0);
+  SG_ARG(lattices != nullptr && lattice_invs != nullptr);
+  SG_ARG(!is_device_ptr(lattices) && !is_device_ptr(lattice_invs));
+  // every cell is parsed and checked before anything is queued: a rejected call changes nothing
+  std::vector<Lattice> cells((size_t)n_geo);
+  for (int64_t g = 0; g < n_geo; ++g) {
+    Lattice& l = cells[(size_t)g];
+    l.on = 1;
+    std::copy(lattices + 9 * g, lattices + 9 * g + 9, l.vec);
+    std::copy(lattice_invs + 9 * g, lattice_invs + 9 * g + 9, l.inv);
+    SG_TRY(check_cell(l));
+  }
+  if (n_geo == 0) return 0;
+  return predict_impl(m, R, n_geo, cells[0], E, F, W, (cudaStream_t)stream, cells.data());
 }
 
 int sgdml_b200_model_set_lattice(sgdml_b200_model* m, const double* lattice, const double* lattice_inv) {
@@ -2152,31 +2248,15 @@ int sgdml_b200_predict_train(sgdml_b200_model* m, int64_t m_begin, int64_t m_end
   SG_TRY(require_device());
   SG_ARG(m != nullptr && F != nullptr);
   SG_ARG(m_begin >= 0 && m_end <= m->M && m_begin <= m_end);
-  if (m->R_d_desc == nullptr) {
-    set_last_error("sgdml_b200_predict_train: call sgdml_b200_model_set_R_d_desc first (predict.py:1223-1229)");
-    return SGDML_B200_ERR_ARG;
-  }
-  const int64_t n_geo = m_end - m_begin;
-  if (n_geo == 0) return 0;
-  cudaStream_t s = (cudaStream_t)stream;
-  const int64_t chunk = std::min<int64_t>(chunk_geos(m), n_geo);
-  SG_TRY(ensure_ws(m, 0, chunk));
-  sgdml_b200_model::WS& w = m->ws[0];
-  const bool F_dev = is_device_ptr(F), E_dev = (E != nullptr) && is_device_ptr(E);
-  const int dimi = 3 * m->N;
-  const double std = scaled ? m->std : 1.0, c = scaled ? m->c : 0.0;
-  for (int64_t g0 = 0; g0 < n_geo; g0 += chunk) {
-    const int64_t ng = std::min<int64_t>(chunk, n_geo - g0);
-    const double* xq = m->X + (m_begin + g0) * m->D;
-    const double* gq = m->R_d_desc + (m_begin + g0) * m->D * 3;
-    double* Fd = F_dev ? F + g0 * dimi : w.F;
-    double* Ed = (E == nullptr) ? nullptr : (E_dev ? E + g0 : w.E);
-    SG_TRY(run_queries(m, 0, xq, gq, ng, std, c, Ed, Fd, s));
-    if (!F_dev) SG_CUDA(cudaMemcpyAsync(F + g0 * dimi, Fd, sizeof(double) * ng * dimi, cudaMemcpyDeviceToHost, s));
-    if (E != nullptr && !E_dev) SG_CUDA(cudaMemcpyAsync(E + g0, Ed, sizeof(double) * ng, cudaMemcpyDeviceToHost, s));
-  }
-  if (!F_dev || (E != nullptr && !E_dev)) SG_CUDA(cudaStreamSynchronize(s));
-  return 0;
+  return predict_train_impl(m, m_begin, m_end, scaled, E, F, nullptr, (cudaStream_t)stream);
+}
+
+int sgdml_b200_predict_train_virial(sgdml_b200_model* m, int64_t m_begin, int64_t m_end, int scaled, double* E,
+                                    double* F, double* W, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(m != nullptr && F != nullptr && W != nullptr);
+  SG_ARG(m_begin >= 0 && m_end <= m->M && m_begin <= m_end);
+  return predict_train_impl(m, m_begin, m_end, scaled, E, F, W, (cudaStream_t)stream);
 }
 
 int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* m, int slices, void* stream) {

@@ -80,8 +80,10 @@ def all_gather_rows(local, n_total, group=None):
     else:
         buf = torch.zeros((max_rows,) + tail, dtype=torch.float64, device=dev)
         buf[: loc_t.shape[0]] = loc_t
-        out = torch.empty((world, max_rows) + tail, dtype=torch.float64, device=dev)
+        # gathered along the first dimension of a flat (world * max_rows) tensor: gloo takes no stacked output
+        out = torch.empty((world * max_rows,) + tail, dtype=torch.float64, device=dev)
         dist.all_gather_into_tensor(out, buf, group=group)
+        out = out.view((world, max_rows) + tail)
         full = torch.cat([out[r, : shard_bounds(n_total, world, r)[1] - shard_bounds(n_total, world, r)[0]] for r in range(world)], dim=0)
     if is_tensor:
         return full.to(local.device)
@@ -138,6 +140,30 @@ def predict_sharded(predict_fn, R, gather=True, group=None):
     if not gather:
         return lo, hi, E, F
     return all_gather_rows(E, n, group), all_gather_rows(F, n, group)
+
+
+def predict_virial_sharded(predict_virial_fn, R, lattice=None, gather=True, group=None):
+    """predict_virial_fn(R_shard, lattice_shard) -> (E, F, W) (GDMLPredict.predict_virial).  Splits the query batch
+    across ranks like `predict_sharded`; a (B, 3, 3) `lattice` (one cell per geometry) is split with it, a (3, 3) one or
+    None goes to every rank as it is.  With gather=True every rank receives the full (E, F, W), otherwise each rank
+    keeps (lo, hi, E_local, F_local, W_local)."""
+    rank, world = world_info(group)
+    R = np.asarray(R, dtype=np.float64)
+    n = R.shape[0]
+    lo, hi = shard_bounds(n, world, rank)
+    lat = None
+    if lattice is not None:
+        if hasattr(lattice, 'data_ptr'):
+            lattice = lattice.detach().cpu().numpy()
+        lat = np.asarray(lattice, dtype=np.float64)
+        if lat.ndim == 3:
+            if lat.shape[0] != n:
+                raise ValueError('lattice holds %d cells for %d geometries' % (lat.shape[0], n))
+            lat = lat[lo:hi]
+    E, F, W = predict_virial_fn(R[lo:hi], lat)
+    if not gather:
+        return lo, hi, E, F, W
+    return all_gather_rows(E, n, group), all_gather_rows(F, n, group), all_gather_rows(W, n, group)
 
 
 def kmatvec_sharded(rows_fn, n_train, group=None):
@@ -342,6 +368,8 @@ def model_shard(model, lo, hi):
     sub['R_desc'] = np.ascontiguousarray(np.asarray(model['R_desc'])[:, lo:hi])  # stored (D, M), train.py:807
     sub['R_d_desc_alpha'] = np.ascontiguousarray(np.asarray(model['R_d_desc_alpha'])[lo:hi])
     sub['alphas_F'] = np.asarray(model['alphas_F']).reshape(n_train, -1)[lo:hi].ravel()
+    if 'alphas_E' in model:  # energy-constrained models: one coefficient per training point
+        sub['alphas_E'] = np.asarray(model['alphas_E']).ravel()[lo:hi]
     if 'idxs_train' in model:
         sub['idxs_train'] = np.asarray(model['idxs_train'])[lo:hi]
     sub['std'] = 1.0
@@ -355,8 +383,8 @@ class TrainPointShardedPredictor(object):
     rank evaluates the WHOLE query batch against its shard, then ONE all-reduce of B*(3N+1) doubles
     (the back-projection J^T is linear, so the partial forces are summed after it).
 
-    predictor_cls(model) must offer .predict(R) -> (E, F): sgdml_b200.GDMLPredict on the GPU box,
-    the oracle predictor in the CPU tests."""
+    predictor_cls(model) must offer .predict(R) -> (E, F), and .predict_virial(R, lattice=...) -> (E, F, W) for
+    `predict_virial`: sgdml_b200.GDMLPredict on the GPU box, the oracle predictor in the CPU tests."""
 
     def __init__(self, model, predictor_cls, group=None):
         self.group = group
@@ -406,3 +434,46 @@ class TrainPointShardedPredictor(object):
         E_v *= self.std
         E_v += self.c
         return E_v, F_v
+
+    def predict_virial(self, R, lattice=None, return_E=True):
+        """`predict` plus the virial: R and lattice as GDMLPredict.predict_virial ((3, 3), one cell per geometry
+        (B, 3, 3), or None for the model's own) -> (E, F, W) or (F, W).  W is linear in F_desc, hence in the sum over
+        training points, so each rank's raw shard virial (std = 1, c = 0) rides in the same ONE all-reduce as E and F:
+        a buffer [F | E | W] of B*(3N+10) doubles.  std and c are applied afterwards.  CUDA tensors stay on the device
+        (NCCL)."""
+        import torch
+
+        on_device = hasattr(R, 'data_ptr') and R.is_cuda
+        if on_device:
+            R = R.reshape(-1, self.dim_i)
+            B = R.shape[0]
+            buf = torch.zeros(B * (self.dim_i + 10), dtype=torch.float64, device=R.device)
+        else:
+            R = np.asarray(R, dtype=np.float64).reshape(-1, self.dim_i)
+            B = R.shape[0]
+            buf = torch.zeros(B * (self.dim_i + 10), dtype=torch.float64)
+        F_v = buf[: B * self.dim_i].view(B, self.dim_i)
+        E_v = buf[B * self.dim_i : B * (self.dim_i + 1)]
+        W_v = buf[B * (self.dim_i + 1) :].view(B, 3, 3)
+        if self.part is not None:
+            if on_device:
+                self.part.predict_virial(R, lattice=lattice, out=(E_v, F_v, W_v))
+            else:
+                E, F, W = self.part.predict_virial(R, lattice=lattice)
+                E_v.copy_(torch.from_numpy(np.asarray(E, dtype=np.float64)))
+                F_v.copy_(torch.from_numpy(np.asarray(F, dtype=np.float64).reshape(B, -1)))
+                W_v.copy_(torch.from_numpy(np.asarray(W, dtype=np.float64).reshape(B, 3, 3)))
+        if world_info(self.group)[1] > 1:
+            if on_device:
+                all_reduce_sum_(buf, self.group)
+            else:
+                t = buf.to(_device_for_backend(self.group))
+                all_reduce_sum_(t, self.group)
+                buf.copy_(t.cpu())
+        F_v *= self.std
+        W_v *= self.std
+        E_v *= self.std
+        E_v += self.c
+        if not on_device:
+            F_v, E_v, W_v = F_v.numpy(), E_v.numpy(), W_v.numpy()
+        return (E_v, F_v, W_v) if return_E else (F_v, W_v)

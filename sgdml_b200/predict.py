@@ -17,6 +17,20 @@ from . import _lib
 from .desc import Desc
 
 
+def cells_and_inverses(lattice):
+    """(lat, lat_inv) as C-contiguous float64 host arrays for `GDMLPredict.predict_virial`, or (None, None).
+    lattice: (3, 3), or (B, 3, 3) with one cell per geometry; a torch tensor is copied to the host.  np.linalg.inv of
+    the stack inverts each cell exactly as it inverts that cell alone."""
+    if lattice is None:
+        return None, None
+    if hasattr(lattice, 'data_ptr'):
+        lattice = lattice.detach().cpu().numpy()
+    lat = np.ascontiguousarray(np.asarray(lattice, dtype=np.float64))
+    if lat.shape != (3, 3) and not (lat.ndim == 3 and lat.shape[1:] == (3, 3)):
+        raise ValueError('lattice must be a 3 x 3 matrix or a (B, 3, 3) stack (lattice vectors as columns)')
+    return lat, np.ascontiguousarray(np.linalg.inv(lat))
+
+
 class GDMLPredict(object):
     def __init__(
         self,
@@ -240,9 +254,10 @@ class GDMLPredict(object):
         )
         return (E, F) if return_E else (F,)
 
-    def predict_virial(self, R, lattice=None, return_E=True, out=None):
+    def predict_virial(self, R=None, lattice=None, return_E=True, out=None):
         """Extension (the reference has no such output): `predict` plus the virial W of every geometry, optionally in a
-        cell given for this call.  R (B, 3N) [or (3N,)] -> (E (B,), F (B, 3N), W (B, 3, 3)) or (F, W).
+        cell given for this call, or in one cell per geometry.  R (B, 3N) [or (3N,)] -> (E (B,), F (B, 3N), W (B, 3, 3))
+        or (F, W).
 
         With the rows r_i of a geometry and the cell L (lattice vectors as COLUMNS, model units, as model['lattice'])
         strained homogeneously, r_i -> (I + eps) r_i and L -> (I + eps) L:
@@ -251,18 +266,36 @@ class GDMLPredict(object):
         the minimum-image vector of pair d.  For a free molecule W equals sum_i r_i F_i^T; the stress of a periodic
         system is -W / V.  E and F are bit-identical to `predict` in the same cell.
 
-        lattice: (3, 3) cell for this call (its inverse from np.linalg.inv); None: the model's own cell, or none for a
+        lattice: (3, 3) cell for this call, or (B, 3, 3) with one cell per geometry (a NumPy array or a torch tensor,
+        which is copied to the host; inverses from np.linalg.inv); None: the model's own cell, or none for a
         free-molecule model.  The model keeps its cell either way.  `out=(E, F, W)`: preallocated outputs as for
         `predict`, W of shape (B, 3, 3).  NumPy / torch conventions as `predict`: CUDA tensors in place, pinned in ->
-        pinned out."""
+        pinned out.
+
+        R=None: the training points from the cached descriptors (set_R_d_desc), as `predict(R=None)`, in the cell those
+        descriptors were built in (a `lattice` is refused); E and F are bit-identical to `predict(R=None)`."""
         L = _lib.lib()
         dim_i = 3 * self.n_atoms
-        lat = lat_inv = None
-        if lattice is not None:
-            lat = np.ascontiguousarray(np.asarray(lattice, dtype=np.float64))
-            if lat.shape != (3, 3):
-                raise ValueError('lattice must be a 3 x 3 matrix (lattice vectors as columns)')
-            lat_inv = np.ascontiguousarray(np.linalg.inv(lat))
+        if R is None:
+            if lattice is not None:
+                raise ValueError('the training points are evaluated in the cell of their cached descriptors: no lattice')
+            if self.R_d_desc is None:
+                raise RuntimeError(
+                    'A reference to the training geometry descriptors needs to be set (using '
+                    "'set_R_d_desc()') for this function to work without arguments."
+                )
+            n = self.n_train
+            F = np.empty((n, dim_i))
+            E = np.empty(n) if return_E else None
+            W = np.empty((n, 3, 3))
+            _lib.check(
+                L.sgdml_b200_predict_train_virial(
+                    self._handle, 0, n, 1, _lib.ptr(E), _lib.ptr(F), _lib.ptr(W), _lib.current_stream()
+                ),
+                'predict_train_virial',
+            )
+            return (E, F, W) if return_E else (F, W)
+        lat, lat_inv = cells_and_inverses(lattice)
         if isinstance(R, np.ndarray) or not hasattr(R, 'data_ptr'):
             R = np.ascontiguousarray(R, dtype=np.float64)
             if R.ndim == 1:
@@ -298,12 +331,16 @@ class GDMLPredict(object):
                 raise ValueError('out must hold a W buffer')
             self._check_out(R, E, F, n, dim_i)
             self._check_buf(R, W, (n, 3, 3), 'W')
+        if lat is not None and lat.ndim == 3:
+            if lat.shape[0] != n:
+                raise ValueError('lattice holds %d cells for %d geometries' % (lat.shape[0], n))
+            fn, name = L.sgdml_b200_predict_virial_cells, 'predict_virial_cells'
+        else:
+            fn, name = L.sgdml_b200_predict_virial, 'predict_virial'
         _lib.check(
-            L.sgdml_b200_predict_virial(
-                self._handle, _lib.ptr(R), n, _lib.ptr(lat), _lib.ptr(lat_inv), _lib.ptr(E), _lib.ptr(F), _lib.ptr(W),
-                _lib.current_stream(),
-            ),
-            'predict_virial',
+            fn(self._handle, _lib.ptr(R), n, _lib.ptr(lat), _lib.ptr(lat_inv), _lib.ptr(E), _lib.ptr(F), _lib.ptr(W),
+               _lib.current_stream()),
+            name,
         )
         return (E, F, W) if return_E else (F, W)
 

@@ -245,6 +245,35 @@ int sgdml_b200_set_assemble_variant(int variant);
 int sgdml_b200_assemble_plan(int64_t n_atoms, int64_t n_perms, int64_t nk, int64_t n_colpts, int64_t n_rowpts,
                              int square, int n_sm, int64_t* out);
 
+/* ---------------------------------------------------------------- permutation discovery
+ * utils/perm.py:53-87 (_bipartite_match_wkr): the pairwise matching of training geometries that perm.find_perms starts
+ * from, for all pairs or a list of pairs in one launch.  For the pair (i, j), i < j:
+ *   cost = -absv_i absv_j^T;  cost[a][b] += max|cost| where z[a] != z[b]                      (perm.py:70-71, 97-98)
+ *   perm = the minimum-cost assignment of rows to columns (shortest augmenting paths, FP64; rows inserted in index
+ *          order, ties to the lowest column index), perm[a] = column of row a                 (perm.py:73)
+ *   score_before = |adj_i - adj_j|_F,  score = |adj_i[perm][:, perm] - adj_j|_F              (perm.py:75-79)
+ *   match_cost = min(score, score_before);  has_perm = score < score_before and not numpy.isclose(score_before, score)
+ *                (|a - b| <= 1e-8 + 1e-5 |b|): the pairs whose permutation perm.py:84-85 keeps.
+ *   adj   (M, N, N) symmetric pair-distance matrices            absv  (M, N, N) |eigenvectors| of adj, one per column,
+ *   z     (N,) atomic numbers                                           columns by descending eigenvalue (perm.py:185-186)
+ *   pairs (n_pairs, 2) int64 with 0 <= i < j < M, in any order and with repeats allowed, or NULL = every i < j in
+ *         row-major order (n_pairs is then ignored and taken as M(M-1)/2)
+ *   match_cost  with a pair list (n_pairs,); for all pairs (M, M) of which entry [i][j], i < j, is written and no other
+ *   perms       (n_pairs, N) int32 or NULL;   has_perm (n_pairs,) bytes or NULL: one row per pair, in the list's order
+ * adj, absv, match_cost, perms and has_perm may be host or device pointers; z and pairs are read on the host.  2 <= N
+ * <= 1023, 1 <= M <= 65535.  Argument errors are reported before the device is touched.  The call returns after the
+ * kernel has finished, whatever the pointers.  Results are bit-identical between calls and between the two forms; the
+ * kernel ends after a number of steps bounded by the sizes alone for any input, NaN included.
+ * Up to 112 atoms the cost matrix of a pair lives in shared memory, above in a per-CTA slab of a persistent global
+ * workspace (freed by sgdml_b200_release_workspaces).  Launches count under family 8. */
+int sgdml_b200_bipartite_match(const double* adj, const double* absv, const int64_t* z, int64_t n_geo, int64_t n_atoms,
+                               const int64_t* pairs, int64_t n_pairs, double* match_cost, int32_t* perms,
+                               uint8_t* has_perm, void* stream);
+/* How sgdml_b200_bipartite_match runs at n_atoms atoms (host only: needs no device).  Writes 5 values to out:
+ *   {cost matrix (0 shared memory, 1 global slab), threads per CTA, dynamic shared memory bytes, slab doubles per CTA,
+ *    persistent CTAs per SM}. */
+int sgdml_b200_bipartite_match_plan(int64_t n_atoms, int64_t* out);
+
 /* ---------------------------------------------------------------- dense solve (path a) */
 
 /* scipy.linalg.cho_factor (LAPACK dpotrf) as used by analytic.py:94-96 and
@@ -372,7 +401,8 @@ int sgdml_b200_ozaki_debug(int64_t m, int64_t n, int64_t k, const double* A, int
 /* ---------------------------------------------------------------- launch accounting / profiling
  * Kernel families: 0 predictor main kernel, 1 predictor auxiliary kernels, 2 K assembly,
  * 3 DMMA GEMM (Cholesky trailing update), 4 potf2 diagonal tiles, 5 panel TRSM strips,
- * 6 triangular solves, 7 descriptor kernels, 8 misc, 9 the predictor's finishing kernels for
+ * 6 triangular solves, 7 descriptor kernels, 8 misc (the permutation search's matching kernel among them), 9 the
+ * predictor's finishing kernels for
  * descriptors longer than 25,600 entries (N >= 227 atoms; shorter ones finish under family 1).
  * `launches` counts kernel launches per family since the last reset (always on).  With
  * profiling enabled, the library brackets each family's launches with CUDA events on the

@@ -9,5 +9,6 @@ CPU fallback.
 
 __version__ = '0.1.0'
 
+from .perm import find_perms  # noqa: F401
 from .predict import GDMLPredict  # noqa: F401
 from .train import GDMLTrain  # noqa: F401

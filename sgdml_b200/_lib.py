@@ -108,6 +108,9 @@ SIGNATURES = {
         [c_void_p, i64, i64, c_void_p, i64, i64, C.c_double, c_void_p, c_void_p, C.c_int, C.c_double, i64, i64,
          c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64_p, c_double_p, c_void_p],
     ),
+    'sgdml_b200_bipartite_match': (
+        C.c_int, [c_void_p, c_void_p, c_void_p, i64, i64, c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_bipartite_match_plan': (C.c_int, [i64, c_int64_p]),
     'sgdml_b200_set_solve_slices': (C.c_int, [C.c_int]),
     'sgdml_b200_get_solve_slices': (C.c_int, []),
     'sgdml_b200_set_gemm_variant': (C.c_int, [C.c_int]),

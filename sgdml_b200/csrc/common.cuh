@@ -76,7 +76,8 @@ class Staged {
 // sgdml_b200_release_workspaces().  The caller must have finished with the buffer (stream synchronised) before the
 // next ws_get of the same slot -- true for every user: they all synchronise before returning.
 enum WsSlot { WS_POTRF_W = 0, WS_OZ_PLANES = 1, WS_OZ_EXPS = 2, WS_POTRF_INFO = 3, WS_SOLVE_TMP = 4, WS_ASM_DPERM = 5,
-              WS_ASM_APERM = 6, WS_ASM_APINV = 7, WS_ASM_JPTS = 8, WS_ASM_DEST = 9, WS_ASM_SLABS = 10, WS_SLOT_COUNT = 11 };
+              WS_ASM_APERM = 6, WS_ASM_APINV = 7, WS_ASM_JPTS = 8, WS_ASM_DEST = 9, WS_ASM_SLABS = 10, WS_PERM_SLAB = 11,
+              WS_SLOT_COUNT = 12 };
 int ws_get(int slot, size_t bytes, void** out);
 
 // Device-block cache for the predictor's model arrays and per-batch workspaces: `GDMLTrain.train` creates and destroys a

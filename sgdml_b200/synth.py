@@ -234,3 +234,41 @@ def random_model(n_atoms, n_train, perms, sig, seed=0, alpha_scale=1.0, r0=None)
         'tril_perms_lin': tril_perms_lin(perms),
         'use_E': True,
     }
+
+
+def orbit_species(perms, palette=(1, 6, 7, 8)):
+    """Atomic numbers that are constant on the orbits of a permutation group (perms (S, N)), as a molecule's symmetry
+    requires: every orbit with more than one atom gets one species, the atoms the group leaves alone cycle through the
+    palette."""
+    perms = np.asarray(perms, dtype=np.int64)
+    n_atoms = perms.shape[1]
+    orbit = np.min(perms, axis=0)  # the lowest atom each atom is mapped to: one label per orbit
+    z = np.empty(n_atoms, dtype=np.int64)
+    for a in range(n_atoms):
+        moved = np.count_nonzero(orbit == orbit[a]) > 1
+        z[a] = palette[(orbit[a] + (1 if moved else 0)) % len(palette)]
+    return z
+
+
+def planted_symmetry_geometries(n_atoms, n_geos, perms, seed, spread=0.005, r0=None):
+    """Geometries that are related by the permutations of a given group (`rotor_swap_group`, `close_group`), which
+    `geometries` never produces: R_k = r0[g_k] + spread * N(0, 1) with g_k drawn uniformly (seeded) from `perms`.
+    Geometry k is the base geometry with its atoms relabelled by g_k -- what a trajectory of a molecule with rotating
+    methyl groups looks like to a permutation search -- so geometries i and j are related by g_i^-1 g_j (atom a of j sits
+    where atom g_i^-1[g_j[a]] of i sits), a search finds that element or its inverse, and the closure of what it finds
+    is the group.  The base geometry needs no symmetry of its own.  The spread is small on purpose: the spectral
+    matching of perm.py loses pairs once the noise mixes close-lying eigenvectors (0.02 already does at 9 atoms).  Returns (R (n_geos, N, 3), z (N,) constant on the group's orbits, g (n_geos,) the index of
+    each geometry's group element).
+
+    How many geometries: a spanning tree over the geometries carries a generating set once every one of the S elements
+    has been drawn (the products of the matches along the tree's paths then reach every element); a draw of n_geos
+    misses some element with probability at most S (1 - 1/S)^n_geos, about S exp(-n_geos / S): 7 % at n_geos = 4 S for
+    S = 6, below 1 % from 6 S.  Fewer elements usually still generate the group, but nothing guarantees it."""
+    perms = np.asarray(perms, dtype=np.int64)
+    if r0 is None:
+        r0 = base_geometry(n_atoms)
+    rng = np.random.default_rng(seed)
+    g = rng.integers(0, perms.shape[0], size=n_geos)
+    noise = rng.standard_normal((n_geos, n_atoms, 3))
+    R = r0[perms[g]] + spread * noise
+    return R, orbit_species(perms), g

@@ -8,15 +8,10 @@ namespace sgdml {
 
 // ---------------------------------------------------------------- a-D1: from_R
 // reference: utils/desc.py:80-110 (_pdist), 139-163, 166-205, 288-365
-// lat.on != 0: minimum-image convention (utils/desc.py:44-77): d -= lat @ rint(lat_inv @ d), lattice vectors as the
-// COLUMNS of lat; np.around and rint both round half to even
-__device__ __forceinline__ void desc_from_R_body(const double* __restrict__ R, int64_t n_geo, int n_atoms, int dim_d,
-                                                 double* __restrict__ R_desc, double* __restrict__ R_d_desc,
-                                                 const Lattice& lat) {
-  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  int64_t total = n_geo * dim_d;
-  if (idx >= total) return;
-  int64_t g = idx / dim_d;
+// lat.on != 0: minimum-image convention (minimum_image, desc.cuh).  Thread idx = g * dim_d + d.
+__device__ __forceinline__ void desc_from_R_body(int64_t idx, int64_t g, const double* __restrict__ R, int n_atoms,
+                                                 int dim_d, double* __restrict__ R_desc,
+                                                 double* __restrict__ R_d_desc, const Lattice& lat) {
   int d = (int)(idx - g * dim_d);
   int a, b;
   pair_from_d(d, a, b);
@@ -24,15 +19,8 @@ __device__ __forceinline__ void desc_from_R_body(const double* __restrict__ R, i
   double dx = r[3 * a + 0] - r[3 * b + 0];
   double dy = r[3 * a + 1] - r[3 * b + 1];
   double dz = r[3 * a + 2] - r[3 * b + 2];
-  if (lat.on) {
-    const double c0 = rint(lat.inv[0] * dx + lat.inv[1] * dy + lat.inv[2] * dz);
-    const double c1 = rint(lat.inv[3] * dx + lat.inv[4] * dy + lat.inv[5] * dz);
-    const double c2 = rint(lat.inv[6] * dx + lat.inv[7] * dy + lat.inv[8] * dz);
-    dx -= lat.vec[0] * c0 + lat.vec[1] * c1 + lat.vec[2] * c2;
-    dy -= lat.vec[3] * c0 + lat.vec[4] * c1 + lat.vec[5] * c2;
-    dz -= lat.vec[6] * c0 + lat.vec[7] * c1 + lat.vec[8] * c2;
-  }
-  double dist = sqrt(dx * dx + dy * dy + dz * dz);
+  minimum_image(lat, dx, dy, dz);
+  double dist = sqrt(dot3(dx, dy, dz, dx, dy, dz));
   double inv = 1.0 / dist;
   double inv3 = 1.0 / (dist * dist * dist);
   if (R_desc) R_desc[idx] = inv;
@@ -42,28 +30,19 @@ __device__ __forceinline__ void desc_from_R_body(const double* __restrict__ R, i
     R_d_desc[idx * 3 + 2] = dz * inv3;
   }
 }
+// lats == nullptr: every geometry in the cell `lat`, a kernel argument, so the bulk path reads no cell from memory.
+// Otherwise geometry g takes lats[g]; with small D one block spans several geometries, so every thread reads its own
+// geometry's cell (152 B, shared through L1 by the D threads of that geometry).
 __global__ void k_desc_from_R(const double* __restrict__ R, int64_t n_geo, int n_atoms, int dim_d,
-                              double* __restrict__ R_desc, double* __restrict__ R_d_desc, const Lattice lat) {
-  desc_from_R_body(R, n_geo, n_atoms, dim_d, R_desc, R_d_desc, lat);
-}
-// the same with the cell in device memory (a captured graph copies each call's cell there, next to R)
-__global__ void k_desc_from_R_lp(const double* __restrict__ R, int64_t n_geo, int n_atoms, int dim_d,
-                                 double* __restrict__ R_desc, double* __restrict__ R_d_desc,
-                                 const Lattice* __restrict__ latp) {
-  __shared__ Lattice lat;
-  if (threadIdx.x == 0) lat = *latp;
-  __syncthreads();
-  desc_from_R_body(R, n_geo, n_atoms, dim_d, R_desc, R_d_desc, lat);
-}
-// the same with one cell per geometry in device memory (sgdml_b200_predict_virial_cells): lats[g] is the cell of
-// geometry g.  With small D one block spans several geometries, so every thread reads its own geometry's cell (152 B,
-// shared through L1 by the D threads of that geometry)
-__global__ void k_desc_from_R_cells(const double* __restrict__ R, int64_t n_geo, int n_atoms, int dim_d,
-                                    double* __restrict__ R_desc, double* __restrict__ R_d_desc,
-                                    const Lattice* __restrict__ lats) {
+                              double* __restrict__ R_desc, double* __restrict__ R_d_desc, const Lattice lat,
+                              const Lattice* __restrict__ lats) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n_geo * dim_d) return;
-  desc_from_R_body(R, n_geo, n_atoms, dim_d, R_desc, R_d_desc, lats[idx / dim_d]);
+  const int64_t g = idx / dim_d;
+  if (lats != nullptr)
+    desc_from_R_body(idx, g, R, n_atoms, dim_d, R_desc, R_d_desc, lats[g]);
+  else
+    desc_from_R_body(idx, g, R, n_atoms, dim_d, R_desc, R_d_desc, lat);
 }
 
 // ---------------------------------------------------------------- a-D3: (J v)_d = g_d . (v_b - v_a)
@@ -114,39 +93,12 @@ __global__ void k_vec_dot_d_desc(const double* __restrict__ R_d_desc, const doub
 }
 
 int launch_desc_from_R(const double* R, int64_t n_geo, int n_atoms, double* R_desc, double* R_d_desc,
-                       cudaStream_t s, const Lattice* lat) {
-  if (n_geo == 0) return 0;
-  const int D = n_atoms * (n_atoms - 1) / 2;
-  int64_t total = n_geo * D;
-  Lattice l;
-  l.on = 0;
-  if (lat != nullptr) l = *lat;
-  ProfScope ps(KID_DESC, s);
-  k_desc_from_R<<<ceil_div(total, 256), 256, 0, s>>>(R, n_geo, n_atoms, D, R_desc, R_d_desc, l);
-  SG_CUDA(cudaGetLastError());
-  count_launch(KID_DESC);
-  return 0;
-}
-
-int launch_desc_from_R_lp(const double* R, int64_t n_geo, int n_atoms, double* R_desc, double* R_d_desc,
-                          cudaStream_t s, const Lattice* lat_dev) {
+                       cudaStream_t s, const Lattice& lat, const Lattice* lats_dev) {
   if (n_geo == 0) return 0;
   const int D = n_atoms * (n_atoms - 1) / 2;
   int64_t total = n_geo * D;
   ProfScope ps(KID_DESC, s);
-  k_desc_from_R_lp<<<ceil_div(total, 256), 256, 0, s>>>(R, n_geo, n_atoms, D, R_desc, R_d_desc, lat_dev);
-  SG_CUDA(cudaGetLastError());
-  count_launch(KID_DESC);
-  return 0;
-}
-
-int launch_desc_from_R_cells(const double* R, int64_t n_geo, int n_atoms, double* R_desc, double* R_d_desc,
-                             cudaStream_t s, const Lattice* lats_dev) {
-  if (n_geo == 0) return 0;
-  const int D = n_atoms * (n_atoms - 1) / 2;
-  int64_t total = n_geo * D;
-  ProfScope ps(KID_DESC, s);
-  k_desc_from_R_cells<<<ceil_div(total, 256), 256, 0, s>>>(R, n_geo, n_atoms, D, R_desc, R_d_desc, lats_dev);
+  k_desc_from_R<<<ceil_div(total, 256), 256, 0, s>>>(R, n_geo, n_atoms, D, R_desc, R_d_desc, lat, lats_dev);
   SG_CUDA(cudaGetLastError());
   count_launch(KID_DESC);
   return 0;
@@ -232,7 +184,8 @@ int sgdml_b200_desc_from_R_pbc(const double* R, int64_t n_geo, int64_t n_atoms, 
   SG_TRY(sR.init(R, sizeof(double) * n_geo * 3 * n_atoms, true, s));
   SG_TRY(sX.init(R_desc, sizeof(double) * n_geo * D, false, s));
   SG_TRY(sG.init(R_d_desc, sizeof(double) * n_geo * D * 3, false, s));
-  SG_TRY(launch_desc_from_R((const double*)sR.dev(), n_geo, (int)n_atoms, (double*)sX.dev(), (double*)sG.dev(), s, &l));
+  SG_TRY(launch_desc_from_R((const double*)sR.dev(), n_geo, (int)n_atoms, (double*)sX.dev(), (double*)sG.dev(), s, l,
+                            nullptr));
   SG_TRY(sX.finish(s));
   SG_TRY(sG.finish(s));
   if (sR.staged() || sX.staged() || sG.staged()) SG_CUDA(cudaStreamSynchronize(s));
@@ -250,7 +203,8 @@ int sgdml_b200_desc_from_R(const double* R, int64_t n_geo, int64_t n_atoms, doub
   SG_TRY(sR.init(R, sizeof(double) * n_geo * 3 * n_atoms, true, s));
   SG_TRY(sX.init(R_desc, sizeof(double) * n_geo * D, false, s));
   SG_TRY(sG.init(R_d_desc, sizeof(double) * n_geo * D * 3, false, s));
-  SG_TRY(launch_desc_from_R((const double*)sR.dev(), n_geo, (int)n_atoms, (double*)sX.dev(), (double*)sG.dev(), s));
+  SG_TRY(launch_desc_from_R((const double*)sR.dev(), n_geo, (int)n_atoms, (double*)sX.dev(), (double*)sG.dev(), s,
+                            Lattice{}, nullptr));
   SG_TRY(sX.finish(s));
   SG_TRY(sG.finish(s));
   if (sR.staged() || sX.staged() || sG.staged()) SG_CUDA(cudaStreamSynchronize(s));

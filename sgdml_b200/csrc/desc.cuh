@@ -27,15 +27,30 @@ struct Lattice {
 };
 int lattice_from_host(const double* lattice, const double* lattice_inv, Lattice* l);
 
+// a x + b y + c z as fma(c, z, fma(a, x, b y)), with the roundings spelled out: which product the compiler fuses
+// otherwise depends on the code around the expression, and the descriptor kernels must round alike
+__device__ __forceinline__ double dot3(double a, double b, double c, double x, double y, double z) {
+  return __fma_rn(c, z, __fma_rn(a, x, __dmul_rn(b, y)));
+}
+
+// minimum-image convention (utils/desc.py:44-77): d -= lat @ rint(lat_inv @ d), lattice vectors as the COLUMNS of
+// lat; np.around and rint both round half to even.  Every descriptor kernel wraps through here, so all of them pick
+// the same images, also at exact rounding ties.
+__device__ __forceinline__ void minimum_image(const Lattice& lat, double& dx, double& dy, double& dz) {
+  if (!lat.on) return;
+  const double c0 = rint(dot3(lat.inv[0], lat.inv[1], lat.inv[2], dx, dy, dz));
+  const double c1 = rint(dot3(lat.inv[3], lat.inv[4], lat.inv[5], dx, dy, dz));
+  const double c2 = rint(dot3(lat.inv[6], lat.inv[7], lat.inv[8], dx, dy, dz));
+  dx -= dot3(lat.vec[0], lat.vec[1], lat.vec[2], c0, c1, c2);
+  dy -= dot3(lat.vec[3], lat.vec[4], lat.vec[5], c0, c1, c2);
+  dz -= dot3(lat.vec[6], lat.vec[7], lat.vec[8], c0, c1, c2);
+}
+
 // host-side launchers defined in desc.cu (device pointers only), reused by predict.cu
+// lats_dev == nullptr: every geometry in the cell `lat` (passed by value); otherwise geometry g in lats_dev[g], n_geo
+// cells in DEVICE memory
 int launch_desc_from_R(const double* R, int64_t n_geo, int n_atoms, double* R_desc, double* R_d_desc,
-                       cudaStream_t s, const Lattice* lat = nullptr);
-// the same with the cell read by the kernel from DEVICE memory at lat_dev (a captured graph's per-call cell)
-int launch_desc_from_R_lp(const double* R, int64_t n_geo, int n_atoms, double* R_desc, double* R_d_desc,
-                          cudaStream_t s, const Lattice* lat_dev);
-// one cell per geometry: lats_dev (n_geo) in DEVICE memory, cell g for geometry g
-int launch_desc_from_R_cells(const double* R, int64_t n_geo, int n_atoms, double* R_desc, double* R_d_desc,
-                             cudaStream_t s, const Lattice* lats_dev);
+                       cudaStream_t s, const Lattice& lat, const Lattice* lats_dev);
 int launch_d_desc_dot_vec(const double* R_d_desc, const double* vecs, int64_t n_geo, int n_atoms, double* out,
                           int64_t out_stride, cudaStream_t s);
 int launch_vec_dot_d_desc(const double* R_d_desc, const double* vecs, int64_t n_geo, int n_atoms,

@@ -620,15 +620,21 @@ __global__ void __launch_bounds__(256) k_query_rows(const double* __restrict__ x
 // Small host-buffer batches (the CUDA-graph path): descriptor, its derivative factors and the S query rows of one
 // geometry in ONE launch, one CTA per geometry.  R may live in pinned host memory (read once into shared memory through
 // the unified address space); the arithmetic is that of k_desc_from_R (csrc/desc.cu) followed by k_query_rows.
-__device__ __forceinline__ void desc_query_rows_body(const double* __restrict__ R, int n_atoms,
-                                                     const int* __restrict__ pinv, const double* __restrict__ mu,
-                                                     int D, int DS, int S, int64_t n_rows, int64_t n_rows_pad,
-                                                     double* __restrict__ gq, double* __restrict__ Qg,
-                                                     double* __restrict__ qqg, const Lattice& lat) {
+// CTA b takes the cell lats[b], staged next to R (a free molecule's cells have on = 0), so a replayed graph picks up
+// each call's cells as it picks up its geometries: no cell is baked into a graph.
+__global__ void __launch_bounds__(256) k_desc_query_rows(const double* __restrict__ R, int n_atoms,
+                                                         const int* __restrict__ pinv, const double* __restrict__ mu,
+                                                         int D, int DS, int S, int64_t n_rows, int64_t n_rows_pad,
+                                                         double* __restrict__ gq, double* __restrict__ Qg,
+                                                         double* __restrict__ qqg, const Lattice* __restrict__ lats) {
   extern __shared__ double dq_sm[];  // r: 3N, x: D
+  __shared__ Lattice lat;
   double* r = dq_sm;
   double* x = dq_sm + 3 * n_atoms;
   const int64_t b = blockIdx.x;
+  // the cell and the geometry are read in one phase: one round trip to (pinned) memory, not two.  The last thread
+  // takes the cell; it has no coordinate to load unless 3N > 255.
+  if (threadIdx.x == blockDim.x - 1) lat = lats[b];
   for (int i = threadIdx.x; i < 3 * n_atoms; i += blockDim.x) r[i] = R[b * 3 * n_atoms + i];
   __syncthreads();
   for (int d = threadIdx.x; d < D; d += blockDim.x) {
@@ -637,15 +643,8 @@ __device__ __forceinline__ void desc_query_rows_body(const double* __restrict__ 
     double dx = r[3 * a + 0] - r[3 * c + 0];
     double dy = r[3 * a + 1] - r[3 * c + 1];
     double dz = r[3 * a + 2] - r[3 * c + 2];
-    if (lat.on) {
-      const double c0 = rint(lat.inv[0] * dx + lat.inv[1] * dy + lat.inv[2] * dz);
-      const double c1 = rint(lat.inv[3] * dx + lat.inv[4] * dy + lat.inv[5] * dz);
-      const double c2 = rint(lat.inv[6] * dx + lat.inv[7] * dy + lat.inv[8] * dz);
-      dx -= lat.vec[0] * c0 + lat.vec[1] * c1 + lat.vec[2] * c2;
-      dy -= lat.vec[3] * c0 + lat.vec[4] * c1 + lat.vec[5] * c2;
-      dz -= lat.vec[6] * c0 + lat.vec[7] * c1 + lat.vec[8] * c2;
-    }
-    const double dist = sqrt(dx * dx + dy * dy + dz * dz);
+    minimum_image(lat, dx, dy, dz);
+    const double dist = sqrt(dot3(dx, dy, dz, dx, dy, dz));
     const double inv3 = 1.0 / (dist * dist * dist);
     x[d] = 1.0 / dist;
     double* g = gq + (b * D + d) * 3;
@@ -675,36 +674,6 @@ __device__ __forceinline__ void desc_query_rows_body(const double* __restrict__ 
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     if (lane == 0) qqg[row] = s;
   }
-}
-__global__ void __launch_bounds__(256) k_desc_query_rows(const double* __restrict__ R, int n_atoms,
-                                                         const int* __restrict__ pinv, const double* __restrict__ mu,
-                                                         int D, int DS, int S, int64_t n_rows, int64_t n_rows_pad,
-                                                         double* __restrict__ gq, double* __restrict__ Qg,
-                                                         double* __restrict__ qqg, const Lattice lat) {
-  desc_query_rows_body(R, n_atoms, pinv, mu, D, DS, S, n_rows, n_rows_pad, gq, Qg, qqg, lat);
-}
-// The same with the cell read from memory (the pinned staging slot of sgdml_b200_predict_virial's graphs, next to R):
-// a replayed graph picks up the call's cell as it picks up its geometries.
-__global__ void __launch_bounds__(256) k_desc_query_rows_lp(const double* __restrict__ R, int n_atoms,
-                                                            const int* __restrict__ pinv, const double* __restrict__ mu,
-                                                            int D, int DS, int S, int64_t n_rows, int64_t n_rows_pad,
-                                                            double* __restrict__ gq, double* __restrict__ Qg,
-                                                            double* __restrict__ qqg, const Lattice* __restrict__ latp) {
-  __shared__ Lattice lat;
-  if (threadIdx.x == 0) lat = *latp;
-  __syncthreads();
-  desc_query_rows_body(R, n_atoms, pinv, mu, D, DS, S, n_rows, n_rows_pad, gq, Qg, qqg, lat);
-}
-// One cell per geometry (sgdml_b200_predict_virial_cells): CTA b reads cell b of the array staged next to R
-__global__ void __launch_bounds__(256) k_desc_query_rows_cells(const double* __restrict__ R, int n_atoms,
-                                                               const int* __restrict__ pinv, const double* __restrict__ mu,
-                                                               int D, int DS, int S, int64_t n_rows, int64_t n_rows_pad,
-                                                               double* __restrict__ gq, double* __restrict__ Qg,
-                                                               double* __restrict__ qqg, const Lattice* __restrict__ lats) {
-  __shared__ Lattice lat;
-  if (threadIdx.x == 0) lat = lats[blockIdx.x];
-  __syncthreads();
-  desc_query_rows_body(R, n_atoms, pinv, mu, D, DS, S, n_rows, n_rows_pad, gq, Qg, qqg, lat);
 }
 
 // ============================================================== large descriptors (D > 256)
@@ -1305,7 +1274,7 @@ struct sgdml_b200_model {
     double* Fd = nullptr;       // (geo, D) F_desc of long descriptors (fdesc_in_ws)
     double* W = nullptr;        // (geo, 9) virial staging for host outputs
     double* Wp = nullptr;       // (geo, ceil(D / 256), 6) per-CTA virial partials of k_fdesc_gather_w (fdesc_in_ws)
-    Lattice* lat = nullptr;     // (geo) one cell per geometry (sgdml_b200_predict_virial_cells)
+    Lattice* lat = nullptr;     // (geo) the chunk's cells of a call with one cell per geometry
     OzOperand ozQ, ozC1, ozC2;  // slices of the per-batch operands (int8 path of large descriptors)
   } ws[2];
   cudaStream_t pipe_stream[2] = {nullptr, nullptr};
@@ -1314,17 +1283,16 @@ struct sgdml_b200_model {
   struct GraphSlot {
     int64_t n_geo = 0;
     int with_E = 0;
-    int with_W = 0;  // sgdml_b200_predict_virial: the cell is read from hLat at run time, not baked in
-    int cells = 0;   // sgdml_b200_predict_virial_cells: hLat / dLat hold one cell per geometry
+    int with_W = 0;  // the graph also writes W
     int n_kernels = 0;
     uint64_t generation = 0;
     cudaGraphExec_t exec = nullptr;
     double *hR = nullptr, *hF = nullptr, *hE = nullptr, *hW = nullptr;  // pinned staging
-    Lattice* hLat = nullptr;  // pinned: the call's cell, or n_geo cells (with_W)
-    Lattice* dLat = nullptr;  // device copy of hLat (with_W, copy-node form)
+    Lattice* hLat = nullptr;  // pinned: one cell per geometry, read at run time
+    Lattice* dLat = nullptr;  // device copy of hLat (copy-node form)
   } graphs[4];
   int graph_next = 0;
-  uint64_t generation = 1;  // bumped whenever something a captured graph has baked in changes (workspace, cell, alphas_E)
+  uint64_t generation = 1;  // bumped whenever something a captured graph has baked in changes (workspace, alphas_E)
   cudaStream_t graph_stream = nullptr;
   cudaEvent_t graph_event = nullptr;
 };
@@ -1400,45 +1368,9 @@ int alloc_oz(OzOperand& o, int64_t rows, int64_t k, int S) {
   return 0;
 }
 
-void free_ws(sgdml_b200_model* m) {
-  cudaDeviceSynchronize();  // the blocks go back to the cache (no implicit synchronisation as in cudaFree)
-  for (auto& w : m->ws) {
-    free_oz(w.ozQ);
-    free_oz(w.ozC1);
-    free_oz(w.ozC2);
-    cached_free(w.xq);
-    cached_free(w.gq);
-    cached_free(w.G);
-    cached_free(w.Erow);
-    cached_free(w.R);
-    cached_free(w.E);
-    cached_free(w.F);
-    cached_free(w.Qg);
-    cached_free(w.qq);
-    cached_free(w.S1);
-    cached_free(w.S2);
-    cached_free(w.csum);
-    cached_free(w.Fd);
-    cached_free(w.W);
-    cached_free(w.Wp);
-    cached_free(w.lat);
-    w = sgdml_b200_model::WS();
-  }
-}
-
-// F_desc of one query beyond the shared memory of k_predict_finish (D > 25,600, N >= 227 atoms): the finishing path
-// k_fdesc_gather / k_fdesc_project with the workspace w.Fd
-bool fdesc_in_ws(const sgdml_b200_model* m) { return sizeof(double) * (size_t)m->D > 200 * 1024; }
-
-int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
-  sgdml_b200_model::WS& w = m->ws[slot];
-  if (!m->large) {  // room for the per-split output planes of small batches (<= ~300 CTAs x BQ rows)
-    const int64_t min_geo = (int64_t)(2 * num_sms() + 8) * m->BQ / m->S + 1;
-    n_geo = std::max<int64_t>(n_geo, std::min<int64_t>(min_geo, chunk_geos(m)));
-  }
-  if (n_geo <= w.geo) return 0;
-  ++m->generation;  // captured graphs hold the old workspace pointers
-  if (w.geo > 0) SG_CUDA(cudaDeviceSynchronize());  // earlier batches may still run on the old workspace
+// the caller makes sure that no kernel still uses the slot (its blocks go back to the cache: no implicit
+// synchronisation as in cudaFree)
+void free_ws_slot(sgdml_b200_model::WS& w) {
   free_oz(w.ozQ);
   free_oz(w.ozC1);
   free_oz(w.ozC2);
@@ -1459,6 +1391,27 @@ int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
   cached_free(w.Wp);
   cached_free(w.lat);
   w = sgdml_b200_model::WS();
+}
+
+void free_ws(sgdml_b200_model* m) {
+  cudaDeviceSynchronize();
+  for (auto& w : m->ws) free_ws_slot(w);
+}
+
+// F_desc of one query beyond the shared memory of k_predict_finish (D > 25,600, N >= 227 atoms): the finishing path
+// k_fdesc_gather / k_fdesc_project with the workspace w.Fd
+bool fdesc_in_ws(const sgdml_b200_model* m) { return sizeof(double) * (size_t)m->D > 200 * 1024; }
+
+int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
+  sgdml_b200_model::WS& w = m->ws[slot];
+  if (!m->large) {  // room for the per-split output planes of small batches (<= ~300 CTAs x BQ rows)
+    const int64_t min_geo = (int64_t)(2 * num_sms() + 8) * m->BQ / m->S + 1;
+    n_geo = std::max<int64_t>(n_geo, std::min<int64_t>(min_geo, chunk_geos(m)));
+  }
+  if (n_geo <= w.geo) return 0;
+  ++m->generation;  // captured graphs hold the old workspace pointers
+  if (w.geo > 0) SG_CUDA(cudaDeviceSynchronize());  // earlier batches may still run on the old workspace
+  free_ws_slot(w);
   SG_CUDA(cached_malloc(&w.xq, sizeof(double) * n_geo * m->D));
   SG_CUDA(cached_malloc(&w.W, sizeof(double) * n_geo * 9));
   SG_CUDA(cached_malloc(&w.lat, sizeof(Lattice) * n_geo));
@@ -1854,20 +1807,16 @@ void free_graph_slot(sgdml_b200_model::GraphSlot& g) {
 
 // Small host-buffer batch (molecular dynamics: one geometry per call, ase_calc.py:98-110): pinned staging buffers and
 // the whole launch sequence (H2D copy, descriptor kernel, query rows, main kernel, finishing kernel, D2H copies)
-// replayed from a CUDA graph -- one launch call instead of seven.
-// W != nullptr (sgdml_b200_predict_virial): the slot also stages W, and the cell `lat` of the call travels with the
-// geometries -- staged in pinned memory and read there by the descriptor kernel (zero copy) or copied to the device by
-// the graph's first nodes (copy-node form) -- so a call with a new cell replays the graph: no capture, no device
+// replayed from a CUDA graph -- one launch call instead of seven.  W != nullptr: the slot also stages W.
+// The cells of the call travel with its geometries: every call stages one cell per geometry in pinned memory, read
+// there by the descriptor kernel (zero copy) or copied to the device by the graph's first nodes (copy-node form).  No
+// cell is baked into a graph, so a call with new cells, or after set_lattice, replays it: no capture, no device
 // synchronisation.
-// cells != nullptr (sgdml_b200_predict_virial_cells, with W): n_geo host cells, one per geometry, staged the same way
-// (k_desc_query_rows_cells / k_desc_from_R_cells); such graphs live in slots of their own.
-int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lattice& lat, double* E, double* F,
-                  double* W, cudaStream_t s, const Lattice* cells = nullptr) {
+int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lattice* cells, int64_t n_cells,
+                  double* E, double* F, double* W, cudaStream_t s) {
   const int dimi = 3 * m->N;
   const int with_E = E != nullptr ? 1 : 0;
   const int with_W = W != nullptr ? 1 : 0;
-  const int with_cells = cells != nullptr ? 1 : 0;
-  const int64_t n_lat = with_cells ? n_geo : 1;  // cells staged in hLat / dLat
   SG_TRY(ensure_ws(m, 0, n_geo));
   if (m->graph_stream == nullptr) {
     SG_CUDA(cudaStreamCreateWithFlags(&m->graph_stream, cudaStreamNonBlocking));
@@ -1877,12 +1826,12 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
   sgdml_b200_model::WS& w = m->ws[0];
   sgdml_b200_model::GraphSlot* g = nullptr;
   for (auto& c : m->graphs)
-    if (c.exec != nullptr && c.n_geo == n_geo && c.with_E == with_E && c.with_W == with_W && c.cells == with_cells &&
+    if (c.exec != nullptr && c.n_geo == n_geo && c.with_E == with_E && c.with_W == with_W &&
         c.generation == m->generation)
       g = &c;
   // Three kernel nodes and no copy nodes: the first kernel reads the geometries straight from the pinned staging
   // buffer (unified addressing) and builds descriptors + query rows, the finishing kernel stores E and F straight
-  // into pinned host memory.  SGDML_B200_GRAPH_ZEROCOPY=0: the earlier form (H2D copy, descriptor kernel, query-row
+  // into pinned host memory.  SGDML_B200_GRAPH_ZEROCOPY=0: the earlier form (H2D copies, descriptor kernel, query-row
   // kernel, ..., two D2H copies).
   const size_t dq_bytes = sizeof(double) * (size_t)(dimi + m->D);
   const bool zero_copy = g_graph_zero_copy() && dq_bytes <= 200 * 1024;
@@ -1890,43 +1839,31 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
     if (zero_copy) {
       const int64_t n_rows = n_geo * m->S;
       const int64_t n_rows_pad = (n_rows + m->BQ - 1) / m->BQ * m->BQ;
-      if (with_cells) {
-        if (dq_bytes > 46 * 1024)
-          SG_CUDA(cudaFuncSetAttribute(k_desc_query_rows_cells, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_bytes));
-        k_desc_query_rows_cells<<<(unsigned)n_geo, 256, dq_bytes, gs>>>(q->hR, m->N, m->pinv, m->mu, m->D, m->DS, m->S,
-                                                                       n_rows, n_rows_pad, w.gq, w.Qg, w.qq, q->hLat);
-      } else if (with_W) {
-        // (the Lattice in static shared memory counts against the 48 KB default)
-        if (dq_bytes > 46 * 1024)
-          SG_CUDA(cudaFuncSetAttribute(k_desc_query_rows_lp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_bytes));
-        k_desc_query_rows_lp<<<(unsigned)n_geo, 256, dq_bytes, gs>>>(q->hR, m->N, m->pinv, m->mu, m->D, m->DS, m->S,
-                                                                    n_rows, n_rows_pad, w.gq, w.Qg, w.qq, q->hLat);
-      } else {
-        if (dq_bytes > 48 * 1024)
-          SG_CUDA(cudaFuncSetAttribute(k_desc_query_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_bytes));
-        k_desc_query_rows<<<(unsigned)n_geo, 256, dq_bytes, gs>>>(q->hR, m->N, m->pinv, m->mu, m->D, m->DS, m->S, n_rows,
-                                                                 n_rows_pad, w.gq, w.Qg, w.qq, m->lat);
-      }
+      // the kernel's static shared memory (its Lattice) counts against the 48 KB allowed without opt-in
+      cudaFuncAttributes fa;
+      SG_CUDA(cudaFuncGetAttributes(&fa, k_desc_query_rows));
+      if (dq_bytes + fa.sharedSizeBytes > 48 * 1024)
+        SG_CUDA(cudaFuncSetAttribute(k_desc_query_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_bytes));
+      k_desc_query_rows<<<(unsigned)n_geo, 256, dq_bytes, gs>>>(q->hR, m->N, m->pinv, m->mu, m->D, m->DS, m->S, n_rows,
+                                                               n_rows_pad, w.gq, w.Qg, w.qq, q->hLat);
       SG_CUDA(cudaGetLastError());
       count_launch(KID_PREDICT_AUX);
       SG_TRY(run_queries(m, 0, nullptr, w.gq, n_geo, m->std, m->c, with_E ? q->hE : nullptr, q->hF, gs, q->hW));
       return 0;
     }
     SG_CUDA(cudaMemcpyAsync(w.R, q->hR, sizeof(double) * n_geo * dimi, cudaMemcpyHostToDevice, gs));
-    if (with_cells) {
-      SG_CUDA(cudaMemcpyAsync(q->dLat, q->hLat, sizeof(Lattice) * n_lat, cudaMemcpyHostToDevice, gs));
-      SG_TRY(launch_desc_from_R_cells(w.R, n_geo, m->N, w.xq, w.gq, gs, q->dLat));
-    } else if (with_W) {
-      SG_CUDA(cudaMemcpyAsync(q->dLat, q->hLat, sizeof(Lattice), cudaMemcpyHostToDevice, gs));
-      SG_TRY(launch_desc_from_R_lp(w.R, n_geo, m->N, w.xq, w.gq, gs, q->dLat));
-    } else {
-      SG_TRY(launch_desc_from_R(w.R, n_geo, m->N, w.xq, w.gq, gs, &m->lat));
-    }
+    SG_CUDA(cudaMemcpyAsync(q->dLat, q->hLat, sizeof(Lattice) * n_geo, cudaMemcpyHostToDevice, gs));
+    SG_TRY(launch_desc_from_R(w.R, n_geo, m->N, w.xq, w.gq, gs, Lattice{}, q->dLat));
     SG_TRY(run_queries(m, 0, w.xq, w.gq, n_geo, m->std, m->c, with_E ? w.E : nullptr, w.F, gs, with_W ? w.W : nullptr));
     SG_CUDA(cudaMemcpyAsync(q->hF, w.F, sizeof(double) * n_geo * dimi, cudaMemcpyDeviceToHost, gs));
     if (with_E) SG_CUDA(cudaMemcpyAsync(q->hE, w.E, sizeof(double) * n_geo, cudaMemcpyDeviceToHost, gs));
     if (with_W) SG_CUDA(cudaMemcpyAsync(q->hW, w.W, sizeof(double) * n_geo * 9, cudaMemcpyDeviceToHost, gs));
     return 0;
+  };
+  // the call's geometries and one cell per geometry into the slot (a replay has finished before its call returns)
+  auto stage = [&](sgdml_b200_model::GraphSlot* q) {
+    std::copy(R, R + n_geo * dimi, q->hR);
+    for (int64_t i = 0; i < n_geo; ++i) q->hLat[i] = cells[n_cells == 1 ? 0 : i];
   };
   if (g == nullptr) {
     // capture happens on a private stream (the caller's may be the legacy stream, which cannot be captured); work
@@ -1939,16 +1876,10 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
     SG_CUDA(cudaMallocHost(&g->hR, sizeof(double) * n_geo * dimi));
     SG_CUDA(cudaMallocHost(&g->hF, sizeof(double) * n_geo * dimi));
     SG_CUDA(cudaMallocHost(&g->hE, sizeof(double) * n_geo));
-    if (with_W) {
-      SG_CUDA(cudaMallocHost(&g->hW, sizeof(double) * n_geo * 9));
-      SG_CUDA(cudaMallocHost(&g->hLat, sizeof(Lattice) * n_lat));
-      SG_CUDA(cached_malloc(&g->dLat, sizeof(Lattice) * n_lat));
-      if (with_cells)
-        std::copy(cells, cells + n_geo, g->hLat);
-      else
-        *g->hLat = lat;
-    }
-    std::copy(R, R + n_geo * dimi, g->hR);
+    if (with_W) SG_CUDA(cudaMallocHost(&g->hW, sizeof(double) * n_geo * 9));
+    SG_CUDA(cudaMallocHost(&g->hLat, sizeof(Lattice) * n_geo));
+    if (!zero_copy) SG_CUDA(cached_malloc(&g->dLat, sizeof(Lattice) * n_geo));
+    stage(g);
     // first call: run the sequence un-captured (sets the kernels' shared-memory attributes) ...
     SG_TRY(enqueue(g));
     SG_CUDA(cudaStreamSynchronize(gs));
@@ -1980,16 +1911,10 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
     g->n_geo = n_geo;
     g->with_E = with_E;
     g->with_W = with_W;
-    g->cells = with_cells;
     g->generation = m->generation;
   } else {
     // replay on the CALLER's stream: ordered after whatever it has queued, no event round trip
-    std::copy(R, R + n_geo * dimi, g->hR);
-    // the previous replay has finished (synchronised below): the slot is free
-    if (with_cells)
-      std::copy(cells, cells + n_geo, g->hLat);
-    else if (with_W)
-      *g->hLat = lat;
+    stage(g);
     SG_CUDA(cudaGraphLaunch(g->exec, s));
     count_launch(KID_PREDICT_AUX, g->n_kernels);  // the kernels of a replay are launches too
     SG_CUDA(cudaStreamSynchronize(s));
@@ -2000,18 +1925,19 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
   return 0;
 }
 
-// sgdml_b200_predict and sgdml_b200_predict_virial: `lat` is the cell of this call's descriptors; W == nullptr: no
-// virial (the plain finishing kernels).  cells != nullptr (sgdml_b200_predict_virial_cells): n_geo HOST cells, one per
-// geometry, in place of `lat`; each chunk's cells go to the device on the chunk's stream next to its geometries
-int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lattice& lat, double* E, double* F,
-                 double* W, cudaStream_t s, const Lattice* cells = nullptr) {
+// Every prediction of new geometries.  cells: n_cells HOST cells, 1 (every geometry in cells[0]) or n_geo (geometry g
+// in cells[g]); a free molecule's cell has on = 0.  W == nullptr: no virial (the plain finishing kernels).  On the
+// chunked path one cell goes to the descriptor kernel by value, and one cell per geometry goes to the device on the
+// chunk's stream next to its geometries.
+int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lattice* cells, int64_t n_cells,
+                 double* E, double* F, double* W, cudaStream_t s) {
   const bool R_dev = is_device_ptr(R), F_dev = is_device_ptr(F), E_dev = (E != nullptr) && is_device_ptr(E);
   const bool W_dev = (W != nullptr) && is_device_ptr(W);
   const bool host_io = !R_dev || !F_dev || (E != nullptr && !E_dev) || (W != nullptr && !W_dev);
   const int dimi = 3 * m->N;
   if (!R_dev && !F_dev && (E == nullptr || !E_dev) && (W == nullptr || !W_dev) && n_geo <= GRAPH_MAX_GEO &&
       !profiling_enabled() && g_graph_enabled())
-    return predict_graph(m, R, n_geo, lat, E, F, W, s, cells);
+    return predict_graph(m, R, n_geo, cells, n_cells, E, F, W, s);
   int64_t chunk = std::min<int64_t>(chunk_geos(m), n_geo);
   // Host buffers: split the batch into >= 4 chunks and run them on two side streams so that the
   // H2D copy of chunk k+1 and the D2H copy of chunk k-1 overlap the kernels of chunk k.
@@ -2036,12 +1962,12 @@ int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Latt
       SG_CUDA(cudaMemcpyAsync(w.R, Rd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, st));
       Rd = w.R;
     }
-    if (cells != nullptr) {
+    const Lattice* lats = nullptr;
+    if (n_cells != 1) {
       SG_CUDA(cudaMemcpyAsync(w.lat, cells + g0, sizeof(Lattice) * ng, cudaMemcpyHostToDevice, st));
-      SG_TRY(launch_desc_from_R_cells(Rd, ng, m->N, w.xq, w.gq, st, w.lat));
-    } else {
-      SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, st, &lat));
+      lats = w.lat;
     }
+    SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, st, cells[0], lats));
     double* Fd = F_dev ? F + g0 * dimi : w.F;
     double* Ed = (E == nullptr) ? nullptr : (E_dev ? E + g0 : w.E);
     double* Wd = (W == nullptr) ? nullptr : (W_dev ? W + g0 * 9 : w.W);
@@ -2145,7 +2071,7 @@ int sgdml_b200_predict(sgdml_b200_model* m, const double* R, int64_t n_geo, doub
   SG_TRY(require_device());
   SG_ARG(m != nullptr && R != nullptr && F != nullptr && n_geo >= 0);
   if (n_geo == 0) return 0;
-  return predict_impl(m, R, n_geo, m->lat, E, F, nullptr, (cudaStream_t)stream);
+  return predict_impl(m, R, n_geo, &m->lat, 1, E, F, nullptr, (cudaStream_t)stream);
 }
 
 int sgdml_b200_predict_virial(sgdml_b200_model* m, const double* R, int64_t n_geo, const double* lattice,
@@ -2157,7 +2083,7 @@ int sgdml_b200_predict_virial(sgdml_b200_model* m, const double* R, int64_t n_ge
   SG_TRY(lattice_for_call(lattice, lattice_inv, &l));
   if (lattice == nullptr) l = m->lat;
   if (n_geo == 0) return 0;
-  return predict_impl(m, R, n_geo, l, E, F, W, (cudaStream_t)stream);
+  return predict_impl(m, R, n_geo, &l, 1, E, F, W, (cudaStream_t)stream);
 }
 
 int sgdml_b200_predict_virial_cells(sgdml_b200_model* m, const double* R, int64_t n_geo, const double* lattices,
@@ -2176,7 +2102,7 @@ int sgdml_b200_predict_virial_cells(sgdml_b200_model* m, const double* R, int64_
     SG_TRY(check_cell(l));
   }
   if (n_geo == 0) return 0;
-  return predict_impl(m, R, n_geo, cells[0], E, F, W, (cudaStream_t)stream, cells.data());
+  return predict_impl(m, R, n_geo, cells.data(), n_geo, E, F, W, (cudaStream_t)stream);
 }
 
 int sgdml_b200_model_set_lattice(sgdml_b200_model* m, const double* lattice, const double* lattice_inv) {
@@ -2185,8 +2111,7 @@ int sgdml_b200_model_set_lattice(sgdml_b200_model* m, const double* lattice, con
   Lattice l;
   SG_TRY(lattice_from_host(lattice, lattice_inv, &l));
   SG_CUDA(cudaDeviceSynchronize());  // no stream argument: kernels in flight copied the old cell by value, but keep calls ordered
-  ++m->generation;  // captured graphs carry the cell as a kernel argument
-  m->lat = l;
+  m->lat = l;  // (captured graphs stay valid: each call stages its cells)
   return 0;
 }
 

@@ -201,58 +201,7 @@ class GDMLPredict(object):
         (e.g. pinned host tensors), filled in place and returned.
         NumPy in -> NumPy out; torch tensor in (CUDA, or pinned/pageable host) -> torch tensors out on the
         same device (CUDA tensors are used in place, no copies)."""
-        L = _lib.lib()
-        dim_i = 3 * self.n_atoms
-        if R is None:
-            if self.R_d_desc is None:
-                raise RuntimeError(
-                    'A reference to the training geometry descriptors needs to be set (using '
-                    "'set_R_d_desc()') for this function to work without arguments."
-                )
-            n = self.n_train
-            F = np.empty((n, dim_i))
-            E = np.empty(n) if return_E else None
-            _lib.check(
-                L.sgdml_b200_predict_train(self._handle, 0, n, 1, _lib.ptr(E), _lib.ptr(F), _lib.current_stream()),
-                'predict_train',
-            )
-            return (E, F) if return_E else (F,)
-
-        if isinstance(R, np.ndarray) or not hasattr(R, 'data_ptr'):
-            R = np.ascontiguousarray(R, dtype=np.float64)
-            if R.ndim == 1:
-                R = R[None, :]  # predict.py:1183-1184
-            if R.size % dim_i != 0 or (R.ndim == 2 and R.shape[1] != dim_i):
-                raise ValueError('R must have 3*n_atoms columns')
-            R = R.reshape(-1, dim_i)
-            n = R.shape[0]
-            if out is not None:
-                E, F = out
-            else:
-                F = np.empty((n, dim_i))
-                E = np.empty(n) if return_E else None
-        else:
-            import torch
-
-            if R.dtype != torch.float64:
-                raise ValueError('torch inputs must be float64')
-            R = R.contiguous().reshape(-1, dim_i) if R.dim() != 1 else R.contiguous().reshape(1, dim_i)
-            n = R.shape[0]
-            if out is not None:
-                E, F = out
-            else:
-                pin = (not R.is_cuda) and R.is_pinned()  # pinned host tensor in -> pinned host tensors out
-                F = torch.empty((n, dim_i), dtype=torch.float64, device=R.device, pin_memory=pin)
-                E = torch.empty((n,), dtype=torch.float64, device=R.device, pin_memory=pin) if return_E else None
-        if not return_E:
-            E = None  # the engine skips the energy output entirely
-        if out is not None:  # (buffers allocated above are right by construction)
-            self._check_out(R, E, F, n, dim_i)
-        _lib.check(
-            L.sgdml_b200_predict(self._handle, _lib.ptr(R), n, _lib.ptr(E), _lib.ptr(F), _lib.current_stream()),
-            'predict',
-        )
-        return (E, F) if return_E else (F,)
+        return self._predict(R, return_E, out, with_W=False)
 
     def predict_virial(self, R=None, lattice=None, return_E=True, out=None):
         """Extension (the reference has no such output): `predict` plus the virial W of every geometry, optionally in a
@@ -274,11 +223,16 @@ class GDMLPredict(object):
 
         R=None: the training points from the cached descriptors (set_R_d_desc), as `predict(R=None)`, in the cell those
         descriptors were built in (a `lattice` is refused); E and F are bit-identical to `predict(R=None)`."""
+        if R is None and lattice is not None:
+            raise ValueError('the training points are evaluated in the cell of their cached descriptors: no lattice')
+        return self._predict(R, return_E, out, with_W=True, lattice=lattice)
+
+    def _predict(self, R, return_E, out, with_W, lattice=None):
+        """`predict`, and `predict_virial` when with_W: R in either form, outputs allocated like R or taken from `out`
+        and checked, then one engine call."""
         L = _lib.lib()
         dim_i = 3 * self.n_atoms
         if R is None:
-            if lattice is not None:
-                raise ValueError('the training points are evaluated in the cell of their cached descriptors: no lattice')
             if self.R_d_desc is None:
                 raise RuntimeError(
                     'A reference to the training geometry descriptors needs to be set (using '
@@ -287,50 +241,57 @@ class GDMLPredict(object):
             n = self.n_train
             F = np.empty((n, dim_i))
             E = np.empty(n) if return_E else None
-            W = np.empty((n, 3, 3))
-            _lib.check(
-                L.sgdml_b200_predict_train_virial(
+            W = np.empty((n, 3, 3)) if with_W else None
+            if with_W:
+                rc = L.sgdml_b200_predict_train_virial(
                     self._handle, 0, n, 1, _lib.ptr(E), _lib.ptr(F), _lib.ptr(W), _lib.current_stream()
-                ),
-                'predict_train_virial',
-            )
-            return (E, F, W) if return_E else (F, W)
+                )
+            else:
+                rc = L.sgdml_b200_predict_train(self._handle, 0, n, 1, _lib.ptr(E), _lib.ptr(F), _lib.current_stream())
+            _lib.check(rc, 'predict_train_virial' if with_W else 'predict_train')
+            return self._results(E, F, W, return_E, with_W)
+
         lat, lat_inv = cells_and_inverses(lattice)
         if isinstance(R, np.ndarray) or not hasattr(R, 'data_ptr'):
             R = np.ascontiguousarray(R, dtype=np.float64)
             if R.ndim == 1:
-                R = R[None, :]
+                R = R[None, :]  # predict.py:1183-1184
             if R.size % dim_i != 0 or (R.ndim == 2 and R.shape[1] != dim_i):
                 raise ValueError('R must have 3*n_atoms columns')
             R = R.reshape(-1, dim_i)
-            n = R.shape[0]
-            if out is not None:
-                E, F, W = out
-            else:
-                F = np.empty((n, dim_i))
-                E = np.empty(n) if return_E else None
-                W = np.empty((n, 3, 3))
+            empty = np.empty
         else:
             import torch
 
             if R.dtype != torch.float64:
                 raise ValueError('torch inputs must be float64')
             R = R.contiguous().reshape(-1, dim_i) if R.dim() != 1 else R.contiguous().reshape(1, dim_i)
-            n = R.shape[0]
-            if out is not None:
-                E, F, W = out
-            else:
-                pin = (not R.is_cuda) and R.is_pinned()
-                F = torch.empty((n, dim_i), dtype=torch.float64, device=R.device, pin_memory=pin)
-                E = torch.empty((n,), dtype=torch.float64, device=R.device, pin_memory=pin) if return_E else None
-                W = torch.empty((n, 3, 3), dtype=torch.float64, device=R.device, pin_memory=pin)
+            pin = (not R.is_cuda) and R.is_pinned()  # pinned host tensor in -> pinned host tensors out
+
+            def empty(shape):
+                return torch.empty(shape, dtype=torch.float64, device=R.device, pin_memory=pin)
+
+        n = R.shape[0]
+        if out is None:
+            F = empty((n, dim_i))
+            E = empty((n,)) if return_E else None
+            W = empty((n, 3, 3)) if with_W else None
+        elif with_W:
+            E, F, W = out
+        else:
+            (E, F), W = out, None
         if not return_E:
-            E = None
-        if out is not None:
-            if W is None:
+            E = None  # the engine skips the energy output entirely
+        if out is not None:  # (buffers allocated above are right by construction)
+            if with_W and W is None:
                 raise ValueError('out must hold a W buffer')
-            self._check_out(R, E, F, n, dim_i)
-            self._check_buf(R, W, (n, 3, 3), 'W')
+            self._check_out(R, E, F, W, n, dim_i)
+        if not with_W:
+            _lib.check(
+                L.sgdml_b200_predict(self._handle, _lib.ptr(R), n, _lib.ptr(E), _lib.ptr(F), _lib.current_stream()),
+                'predict',
+            )
+            return self._results(E, F, W, return_E, with_W)
         if lat is not None and lat.ndim == 3:
             if lat.shape[0] != n:
                 raise ValueError('lattice holds %d cells for %d geometries' % (lat.shape[0], n))
@@ -342,35 +303,36 @@ class GDMLPredict(object):
                _lib.current_stream()),
             name,
         )
-        return (E, F, W) if return_E else (F, W)
+        return self._results(E, F, W, return_E, with_W)
 
     @staticmethod
-    def _check_out(R, E, F, n, dim_i):
+    def _results(E, F, W, return_E, with_W):
+        res = (F, W) if with_W else (F,)
+        return (E,) + res if return_E else res
+
+    @staticmethod
+    def _check_out(R, E, F, W, n, dim_i):
         """Output buffers go to the engine as raw double*: wrong dtype / layout / device would corrupt memory."""
-        for buf, shape, name in ((F, (n, dim_i), 'F'), (E, (n,), 'E')):
-            GDMLPredict._check_buf(R, buf, shape, name)
+        for buf, shape, name in ((F, (n, dim_i), 'F'), (E, (n,), 'E'), (W, (n, 3, 3), 'W')):
+            if buf is None:
+                continue
+            if tuple(buf.shape) != shape:
+                raise ValueError('out buffer %s has the wrong shape %s (expected %s)' % (name, tuple(buf.shape), shape))
+            if isinstance(buf, np.ndarray):
+                if buf.dtype != np.float64 or not buf.flags['C_CONTIGUOUS'] or not buf.flags['WRITEABLE']:
+                    raise ValueError('out buffer %s must be a writeable C-contiguous float64 array' % name)
+                if not isinstance(R, np.ndarray) and R.is_cuda:
+                    raise ValueError('out buffer %s is a host array but R is a CUDA tensor' % name)
+            else:
+                import torch
 
-    @staticmethod
-    def _check_buf(R, buf, shape, name):
-        if buf is None:
-            return
-        if tuple(buf.shape) != shape:
-            raise ValueError('out buffer %s has the wrong shape %s (expected %s)' % (name, tuple(buf.shape), shape))
-        if isinstance(buf, np.ndarray):
-            if buf.dtype != np.float64 or not buf.flags['C_CONTIGUOUS'] or not buf.flags['WRITEABLE']:
-                raise ValueError('out buffer %s must be a writeable C-contiguous float64 array' % name)
-            if not isinstance(R, np.ndarray) and R.is_cuda:
-                raise ValueError('out buffer %s is a host array but R is a CUDA tensor' % name)
-        else:
-            import torch
-
-            if buf.dtype != torch.float64 or not buf.is_contiguous():
-                raise ValueError('out buffer %s must be a contiguous float64 tensor' % name)
-            r_dev = None if isinstance(R, np.ndarray) else R.device
-            if buf.is_cuda and (r_dev is None or buf.device != r_dev):
-                raise ValueError('out buffer %s lives on %s but R does not' % (name, buf.device))
-            if (not buf.is_cuda) and r_dev is not None and r_dev.type == 'cuda':
-                raise ValueError('out buffer %s is a host tensor but R is a CUDA tensor' % name)
+                if buf.dtype != torch.float64 or not buf.is_contiguous():
+                    raise ValueError('out buffer %s must be a contiguous float64 tensor' % name)
+                r_dev = None if isinstance(R, np.ndarray) else R.device
+                if buf.is_cuda and (r_dev is None or buf.device != r_dev):
+                    raise ValueError('out buffer %s lives on %s but R does not' % (name, buf.device))
+                if (not buf.is_cuda) and r_dev is not None and r_dev.type == 'cuda':
+                    raise ValueError('out buffer %s is a host tensor but R is a CUDA tensor' % name)
 
     def kmatvec_train(self, m_begin=0, m_end=None, out=None, E_out=None):
         """Raw (std = 1, c = 0) force sums on training points [m_begin, m_end): the K.v operator

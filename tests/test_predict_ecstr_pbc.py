@@ -5,8 +5,9 @@ fused register transform of D <= 112, the split-k row-half exchange of the BQ 32
 shared-memory split-k transform of 224 < D <= 256 and the GEMM-composed path of D > 256.  Periodic models build
 their query descriptors with the minimum-image convention in two kernels, k_desc_from_R (chunked path, device
 tensors, copy-node graph) and k_desc_query_rows (zero-copy graph), which must pick the same images -- also at exact
-rounding ties -- and round alike.  Captured graphs carry the cell and use_ae as kernel arguments, so set_lattice and
-set_alphas_E must invalidate them, and a rejected set_lattice must leave the model as it was.
+rounding ties -- and round alike.  Captured graphs carry use_ae as a kernel argument, so set_alphas_E must invalidate
+them; they read the cell staged by each call, so after set_lattice a replay must see the new cell; and a rejected
+set_lattice must leave the model as it was.
 
 Every model is built with the oracle's descriptor code.  Output buffers passed with out= are filled with NaN first,
 and two calls on one handle see different inputs.  Each check prints max |err| / scale against tau (10x margin)."""
@@ -405,7 +406,8 @@ def test_graph_invalidation_and_rejected_calls(eng, monkeypatch):
     """A class 3 handle (D = 153, split-k row-half exchange) created without alphas_E, with a graph captured at B = 3,
     then: alphas_E set, alphas_E switched off, alphas_E from a CUDA tensor through the C ABI, a new cell, no cell, and
     two rejected set_lattice calls on a periodic handle.  Each step toggles what the graph captured before it carries
-    as a kernel argument (use_ae, the cell), so a graph that is not captured again gives the old state's results.
+    as a kernel argument (use_ae) or stages per call (the cell), so a graph that is not captured again, or that reads a
+    stale cell, gives the old state's results.
     After each step the graph, the chunked path and K.v match the oracle of the handle's new state."""
     from sgdml_b200 import _lib
 

@@ -267,6 +267,36 @@ def test_cell_changes_replay_without_capture(eng):
     assert _main_launches() == n0, 'a new cell recaptured the graph'
 
 
+def test_set_lattice_replays_the_graph(eng):
+    """No cell is baked into a graph: B = 3 graphs of `predict_virial` and `predict` captured on a periodic handle
+    replay after set_lattice with a new cell, and after set_lattice(NULL, NULL), and match the oracle in the handle's
+    cell of the moment (E and F of `predict` bit for bit)."""
+    from sgdml_b200 import _lib
+
+    N, M = SHAPES['d36']
+    lat = pc.skewed_cell(N)
+    model = vc.make_model(N, M, seed=85, lattice=lat)
+    op = opredict.Predictor(model)
+    p = eng.GDMLPredict(model)
+    R = vc.queries(N, 3, 86, lat)
+    p.predict_virial(R)  # captures
+    p.predict(R)  # captures
+    n0 = _main_launches()
+    lat2 = np.ascontiguousarray(np.diag([1.07, 0.96, 1.03]) @ lat)
+    for cell, seed in ((lat2, 87), (None, 88)):
+        if cell is None:
+            rc = _lib.lib().sgdml_b200_model_set_lattice(p._handle, None, None)
+        else:
+            rc = _lib.lib().sgdml_b200_model_set_lattice(p._handle, _lib.ptr(cell),
+                                                         _lib.ptr(np.ascontiguousarray(np.linalg.inv(cell))))
+        assert rc == 0
+        R = vc.queries(N, 3, seed, cell)
+        E, F, W = p.predict_virial(R)
+        _check('set_lattice(%s)' % ('NULL' if cell is None else 'cell'), model, vc.with_cell(op, cell), R, E, F, W)
+        _same_as_predict(p, R, E, F, 'set_lattice')
+        assert _main_launches() == n0, 'set_lattice recaptured the graph'
+
+
 def test_int8_slice_route_classical_identity(eng):
     """The int8-slice contractions of D > 256 (5 slices): W equals sum_i r_i F_i^T of the same call."""
     N, M = SHAPES['d276']

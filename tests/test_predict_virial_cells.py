@@ -110,7 +110,7 @@ def _routes(eng, monkeypatch, model, op, base, Rq, tag, seed, pipelined_B=4100):
                 n0 = _main_launches()
                 E, F, W = pg.predict_virial(R, lattice=cells, out=_nan(B, dim_i))  # replays with new cells
                 assert _main_launches() == n0, 'graph not replayed'
-                # all-equal cells against the single-cell graph (a slot of its own), both replayed
+                # all-equal cells against the single-cell call, both replaying the same graph
                 for _ in range(2):
                     a, b = pg.predict_virial(R, lattice=stack(B)), pg.predict_virial(R, lattice=base)
                 assert _same(a, b), '%s B=%d zero copy %s: equal cells differ from the single-cell call' % (tag, B, zc)

@@ -6,7 +6,7 @@ changes on every call.
   2. N = 370, M = 500 (S = 6) at B = 256 (the long-descriptor finishing pair), the same way.
   3. B = 1 NumPy in / out (the MD path, CUDA-graph replay) in the aspirin model put in a skewed cell: host time per call
      of predict_virial with a fixed cell, of predict_virial with a new cell on every call, and of set_lattice + predict
-     with a new cell on every call (which recaptures the graph).
+     with a new cell on every call (which synchronises the device, and replays the graph).
 
 Prints the results as JSON, with the card's name and power limit; `--out FILE` also writes them to FILE."""
 

@@ -383,6 +383,19 @@ int sgdml_b200_dgemm_nt(int64_t m, int64_t n, int64_t k, double alpha, const dou
                         int64_t lda, const double* B, int64_t ldb, double beta, double* C,
                         int64_t ldc, void* stream);
 
+/* Test hook: the internal GEMM launch exactly as potrf, trsm_right_lt, gram_tn and the large-descriptor predictor issue
+ * it, which sgdml_b200_dgemm_nt (mode 0, tri 0, no flag) cannot reach.
+ *   mode 0: C = alpha A B^T + beta C (C is not read when beta == 0);  mode 1: C += A B^T, alpha and beta ignored.
+ *   tri 1 (needs m == n): only the lower triangle is computed.  The tile kernels write whole 128 x 128 tiles that touch
+ *         it, entries above the diagonal inside the diagonal tiles included, and no tile strictly above the diagonal;
+ *         the scalar kernel writes no entry with col > row.
+ *   abort_flag: NULL, or a device int; when it is non-zero at kernel start the call leaves C unchanged.
+ * All pointers must be DEVICE pointers: nothing is staged, and the call returns without synchronising.  The kernel is
+ * the one sgdml_b200_set_gemm_variant selects. */
+int sgdml_b200_gemm_nt_args(int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,
+                            const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int mode, int tri,
+                            const int* abort_flag, void* stream);
+
 /* The same product through the int8 tensor
  * cores -- A and B are cut into n_slices signed 7-bit slices per row-scaled entry and every slice pair is
  * multiplied exactly by wgmma s8 (int32 accumulators in registers); C += alpha * A * B^T.

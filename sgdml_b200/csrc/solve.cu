@@ -1132,6 +1132,32 @@ int sgdml_b200_dgemm_nt(int64_t m, int64_t n, int64_t k, double alpha, const dou
   return 0;
 }
 
+int sgdml_b200_gemm_nt_args(int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,
+                            const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int mode, int tri,
+                            const int* abort_flag, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(A != nullptr && B != nullptr && C != nullptr && m >= 1 && n >= 1 && k >= 1);
+  SG_ARG(lda >= k && ldb >= k && ldc >= n);
+  SG_ARG((mode == 0 || mode == 1) && (tri == 0 || tri == 1) && (tri == 0 || m == n));
+  SG_ARG(is_device_ptr(A) && is_device_ptr(B) && is_device_ptr(C) && (abort_flag == nullptr || is_device_ptr(abort_flag)));
+  GemmArgs g;
+  g.m = m;
+  g.n = n;
+  g.k = k;
+  g.A = A;
+  g.lda = lda;
+  g.B = B;
+  g.ldb = ldb;
+  g.C = C;
+  g.ldc = ldc;
+  g.alpha = alpha;
+  g.beta = beta;
+  g.mode = mode;
+  g.tri = tri;
+  g.abort_flag = abort_flag;
+  return launch_gemm(g, (cudaStream_t)stream);
+}
+
 int sgdml_b200_fp64_peak_tflops(double* tflops) {
   SG_TRY(require_device());
   SG_ARG(tflops != nullptr);

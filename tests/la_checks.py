@@ -1,6 +1,6 @@
 """Acceptance checks for the dense linear-algebra building blocks (csrc/solve.cu, csrc/nystroem.cu).
 
-Plain functions on NumPy arrays, shared by the GPU tests (tests/test_dense_la.py) and by a CPU test that shows
+Plain functions on NumPy arrays, shared by the GPU tests (tests/test_dense_la.py, tests/test_gemm_classes.py) and by a CPU test that shows
 every check can fail (tests/test_la_checks.py).  Each check raises AssertionError with a short diagnosis.
 
 Bounds are componentwise wherever standard error analysis gives one, with u = 2^-53 and
@@ -76,6 +76,48 @@ def check_gram(X, C_hat, lam):
     low = np.tril_indices(m)
     check_finite(C_hat[low], 'gram lower triangle')
     _within(np.abs(C_hat - ref)[low], bound[low], 'gram_tn')
+
+
+GEMM_TILE = 128  # tile edge of the DMMA GEMM kernels (csrc/solve.cu); failures are reported by tile
+
+
+def tiles_of(bad, limit=6):
+    """'(ti, tj), ...' of the GEMM tiles that hold a True entry of the boolean matrix `bad`."""
+    idx = np.argwhere(bad)
+    tiles = sorted(set(map(tuple, (idx // GEMM_TILE).tolist())))
+    return ', '.join('(%d, %d)' % t for t in tiles[:limit]) + (' and %d more' % (len(tiles) - limit) if len(tiles) > limit else '')
+
+
+def check_gemm_nt(A, B, C0, C_hat, alpha=1.0, beta=1.0, tri=False, what='gemm_nt'):
+    """C = alpha A B^T + beta C0 with A (m x k), B (n x k), componentwise:
+    |C^ - C| <= 2 gamma_{k+2} (|alpha| |A| |B|^T + |beta| |C0|).
+    The k products and k - 1 additions of an entry, in any order, carry gamma_k; scaling by alpha, scaling C0 by beta
+    and adding the two give gamma_{k+2}.  The accumulating form C0 + A B^T (accumulators that start from C0: k
+    additions, no scaling) is alpha = beta = 1 and lies inside the same bound.  C0 may be None when beta == 0.
+    tri: only entries with col <= row are part of the result."""
+    A = np.asarray(A, dtype=np.float64)
+    B = np.asarray(B, dtype=np.float64)
+    m, k = A.shape
+    n = B.shape[0]
+    C_hat = np.asarray(C_hat, dtype=np.float64)[:m, :n]
+    ref = alpha * (A @ B.T)
+    bound = abs(alpha) * (np.abs(A) @ np.abs(B).T)
+    if beta != 0.0:
+        C0 = np.asarray(C0, dtype=np.float64)[:m, :n]
+        ref += beta * C0
+        bound += abs(beta) * np.abs(C0)
+    bound *= 2 * gamma(k + 2)
+    with np.errstate(invalid='ignore'):
+        err = np.abs(C_hat - ref)
+        bad = ~(err <= bound)  # NaN fails
+    if tri:
+        bad &= np.tri(m, n, dtype=bool)
+    if bad.any():
+        r, c = np.argwhere(bad)[0]
+        raise AssertionError(
+            '%s: %d entries outside the bound, in tiles %s; first at (%d, %d): %r, expected %r, error %.3e > bound %.3e'
+            % (what, int(bad.sum()), tiles_of(bad), r, c, float(C_hat[r, c]), float(ref[r, c]), float(err[r, c]), float(bound[r, c]))
+        )
 
 
 def check_row_sqnorms(X, out):

@@ -1,6 +1,8 @@
 """The acceptance checks of tests/la_checks.py on CPU: each passes a correct NumPy result and fails one with a
 single injected defect of the kind a kernel could have.  No GPU needed."""
 
+import re
+
 import numpy as np
 import pytest
 import scipy.linalg
@@ -138,3 +140,93 @@ def test_cholesky_check():
     used_upper[200:, 150] = np.nan  # what reading the NaN canaries of the upper triangle leaves behind
     with pytest.raises(AssertionError, match='non-finite'):
         lc.check_cholesky(A, used_upper)
+
+
+# ------------------------------------------------------------------------------------------------ GEMM
+def _gemm_case(seed=9, m=257, n=257, k=66):
+    """Standard-normal operands with rows scaled by 2^e, e in [-20, 20]; C0 at the scale of the product.  Row 9 of A
+    and row 5 of B carry 2^-20 and row 0 of each 2^20, so entry (9, 5) is 2^-80 of the largest."""
+    rng = np.random.default_rng(seed)
+    ea, eb = rng.integers(-20, 21, size=m), rng.integers(-20, 21, size=n)
+    ea[[0, 9]] = [20, -20]
+    eb[[0, 5]] = [20, -20]
+    A = np.ldexp(rng.standard_normal((m, k)), ea[:, None])
+    B = np.ldexp(rng.standard_normal((n, k)), eb[:, None])
+    C0 = np.ldexp(rng.standard_normal((m, n)) * np.sqrt(k), ea[:, None] + eb[None, :])
+    return A, B, C0
+
+
+def test_gemm_check_accepts_an_independent_evaluation():
+    """Extended precision, the k sum taken backwards, rounded once: inside the bound in both forms, with the upper
+    triangle NaN under tri, and with NaN in C0 when beta == 0."""
+    A, B, C0 = _gemm_case()
+    P = A[:, ::-1].astype(np.longdouble) @ B[:, ::-1].T.astype(np.longdouble)
+    lc.check_gemm_nt(A, B, C0, (P + C0).astype(np.float64))
+    lc.check_gemm_nt(A, B, C0, (0.75 * P - 1.25 * C0).astype(np.float64), alpha=0.75, beta=-1.25)
+    lc.check_gemm_nt(A, B, None, P.astype(np.float64), beta=0.0)
+    upper_nan = (P + C0).astype(np.float64)
+    upper_nan[np.triu_indices(A.shape[0], 1)] = np.nan
+    lc.check_gemm_nt(A, B, C0, upper_nan, tri=True)
+    with pytest.raises(AssertionError, match='gemm_nt'):
+        lc.check_gemm_nt(A, B, C0, upper_nan)
+
+
+def _gemm_defects():
+    A, B, C0 = _gemm_case()
+    good = A @ B.T + C0
+    out = {}
+    d = good.copy()
+    d[128:256, :128] = A[128:256, :-4] @ B[:128, :-4].T + C0[128:256, :128]
+    out['last k-step dropped in tile (1, 0)'] = (d, '(1, 0)')
+    d = good.copy()
+    d[136:144, 8:16] = good[136:144, 8:16].T
+    out['fragment transposed'] = (d, '(1, 0)')
+    d = good.copy()
+    d[16:24, 128:136] = C0[16:24, 128:136]
+    out['stale fragment'] = (d, '(0, 1)')
+    d = good.copy()
+    d[:, -1] = C0[:, -1]
+    out['last column of an odd n not stored'] = (d, '(0, 2)')
+    d = good.copy()
+    d[128:256, 128:256] += A[128:256] @ B[128:256].T
+    out['tile accumulated twice'] = (d, '(1, 1)')
+    out['beta = 0 applied to the accumulating form'] = (A @ B.T, '(0, 0)')
+    d = good.copy()
+    d[9, 5] = -d[9, 5]
+    out['wrong sign in a small row'] = (d, '(0, 0); first at (9, 5)')
+    return A, B, C0, good, out
+
+
+_GEMM_DEFECTS = ['last k-step dropped in tile (1, 0)', 'fragment transposed', 'stale fragment',
+                 'last column of an odd n not stored', 'tile accumulated twice',
+                 'beta = 0 applied to the accumulating form', 'wrong sign in a small row']
+
+
+@pytest.mark.parametrize('defect', _GEMM_DEFECTS)
+def test_gemm_check_rejects(defect):
+    """One defect of the kind a tiled kernel could have, in the accumulating form C0 + A B^T: the check fails and
+    names the tile."""
+    A, B, C0, good, defects = _gemm_defects()
+    assert sorted(defects) == sorted(_GEMM_DEFECTS)
+    lc.check_gemm_nt(A, B, C0, good)
+    bad, where = defects[defect]
+    with pytest.raises(AssertionError, match='gemm_nt: .* in tiles ' + re.escape(where)):
+        lc.check_gemm_nt(A, B, C0, bad)
+    if defect != 'wrong sign in a small row':
+        return
+    with pytest.raises(AssertionError):  # (9, 5) is below the diagonal
+        lc.check_gemm_nt(A, B, C0, bad, tri=True)
+    nan = good.copy()
+    nan[200, 3] = np.nan
+    with pytest.raises(AssertionError, match=r'tiles \(1, 0\)'):
+        lc.check_gemm_nt(A, B, C0, nan, tri=True)
+
+
+def test_gemm_max_norm_check_misses_what_the_componentwise_bound_sees():
+    """max|err| / max|ref| < 1e-13, the assertion of the older GEMM tests, accepts a wrong sign in an entry that is
+    2^-80 of the largest; the componentwise bound does not."""
+    A, B, C0, good, defects = _gemm_defects()
+    bad, _ = defects['wrong sign in a small row']
+    assert np.max(np.abs(bad - good)) / np.max(np.abs(good)) < 1e-13
+    with pytest.raises(AssertionError):
+        lc.check_gemm_nt(A, B, C0, bad)

@@ -126,6 +126,17 @@ int sgdml_b200_predict_virial(sgdml_b200_model* model, const double* R, int64_t 
 int sgdml_b200_predict_virial_cells(sgdml_b200_model* model, const double* R, int64_t n_geo, const double* lattices,
                                     const double* lattice_invs, double* E, double* F, double* W, void* stream);
 
+/* Extension: directional derivative of the forces, HV = (dF/dR) V = -H V, per geometry.
+ * R, V (B, 3N) -> HV (B, 3N); host or device as in sgdml_b200_predict; the model's cell; FP64 always.
+ * This is the vector-Jacobian product of F (H is symmetric) that lets autograd differentiate through the forces
+ * (sgdml_b200/torchtools.py); it costs about one more prediction.  It runs the four contractions as FP64 GEMMs on query
+ * rows stacked with their tangent rows, for every descriptor size and whatever sgdml_b200_model_set_contraction_slices
+ * chose.  The first call on a model with D <= 256 keeps transposed copies of its training matrices, which
+ * sgdml_b200_model_set_alphas refreshes from then on.  Its workspace is separate from sgdml_b200_predict's, whose results
+ * and captured graphs it does not change.  A rejected call writes nothing. */
+int sgdml_b200_predict_hvp(sgdml_b200_model* model, const double* R, const double* V, int64_t n_geo,
+                           double* HV, void* stream);
+
 /* Periodic model (predict.py:332-334: lat_and_inv from model['lattice']): query descriptors of
  * sgdml_b200_predict are built with the minimum-image convention.  Both NULL: back to a free molecule. */
 int sgdml_b200_model_set_lattice(sgdml_b200_model* model, const double* lattice, const double* lattice_inv);
@@ -166,8 +177,8 @@ int sgdml_b200_predict_train_virial(sgdml_b200_model* model, int64_t m_begin, in
  * (iterative.py:183-204: tolerance 1e-4).  No effect for D <= 256. */
 int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* model, int slices, void* stream);
 
-/* Test hook: at most max_geos queries (or training points) per chunk of sgdml_b200_predict and
- * sgdml_b200_predict_train, for every model; 0 = no cap (the default: chunks bounded by workspace size only).  Negative
+/* Test hook: at most max_geos queries (or training points) per chunk of sgdml_b200_predict,
+ * sgdml_b200_predict_train and sgdml_b200_predict_hvp, for every model; 0 = no cap (the default: chunks bounded by workspace size only).  Negative
  * values are rejected.  The cap also bounds the minimum per-batch workspace, which limits how far small batches split
  * the sweep over the training points.  Workspaces never shrink: it applies fully to models created after the call.
  * Tests lower it to cover the multi-chunk, pipelined and tail-chunk paths at small batch sizes. */

@@ -40,6 +40,7 @@ SIGNATURES = {
         C.c_int, [c_void_p, c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_predict_virial_cells': (
         C.c_int, [c_void_p, c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_predict_hvp': (C.c_int, [c_void_p, c_void_p, c_void_p, i64, c_void_p, c_void_p]),
     'sgdml_b200_model_set_R_d_desc': (C.c_int, [c_void_p, c_void_p]),
     'sgdml_b200_model_set_alphas': (C.c_int, [c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_predict_train': (C.c_int, [c_void_p, i64, i64, C.c_int, c_void_p, c_void_p, c_void_p]),

@@ -1243,6 +1243,146 @@ __global__ void k_unpad_rows(const double* __restrict__ src, int M, int D, int D
   dst[idx] = src[(int64_t)m * DS + d];
 }
 
+// ============================================================== Hessian-vector product (sgdml_b200_predict_hvp)
+// HV = (dF/dR) V = -H V per geometry: the derivative of the GEMM-composed prediction along V.  The descriptor moves along
+// t = J V (k_d_desc_dot_vec); each virtual row q gets a companion tangent row T (t permuted like q, not centred), stacked
+// below the query rows, so that every GEMM of the large-descriptor path runs once on 2 x rows.  With S3 = T Xc^T,
+// S4 = T JA^T, delta = q - Xc_m, n = sqrt5 |delta|, e = exp(-n/sig), a = delta . JA_m:
+//   ds = delta . T = q.t - S3,  da = S4,
+//   dc2 = -5 k_base e ds / sig                       (n cancels: no singularity)
+//   dc1 = k_c1 e (da - 5 a ds / (n sig))  [+ ae dc2]
+//   dG  = (sum dc1) q + (sum c1) T - sum dc1 Xc_m - sum dc2 JA_m
+// then F_desc and dF_desc are folded over the permutations (k_fdesc_gather) and HV = std (J^T dF_desc + (dJ)^T F_desc).
+//
+// The floor under n in a ds / n: at a training geometry delta = 0 exactly for one permutation, but the GEMM form gives
+// x5 = 5 (qq + mm - 2 S1) as a difference of O(qq + mm) dot products, so x5 is rounding noise of either sign (a and ds
+// likewise, ~eps |q| |JA| and ~eps |q| |t|), and 1 / n would be up to 1e150 where the true term tends to 0:
+// |a ds / n| <= |JA_m| |t| |delta| / sqrt5.  Below x5 = HVP_X5_FLOOR (qq + mm), well above the rounding level
+// 10 gamma (qq + mm) of x5, n carries no information; flooring it there replaces a term whose true size is at most
+// |JA_m| |t| n_floor / 5 by a smaller one: a change of ~n_floor / sig relative to the da term (4e-7 |q| / sig), only
+// within n_floor of a training point, where the forward's own n is uncertain by as much.  Above the floor the term is
+// evaluated as is.  The forward c1, c2 need no floor: they multiply, never divide by n.
+constexpr double HVP_X5_FLOOR = 5.0 * 64.0 * 2.220446049250313e-16;
+
+// One warp per virtual row r < n_rows: S1 -> C1, S2 -> C2 in rows r, S3 -> dC1, S4 -> dC2 in rows n_rows + r (in place);
+// csum[r] = sum_m c1, csum[n_rows + r] = sum_m dc1.  Qg holds the query rows, then the tangent rows.
+__global__ void __launch_bounds__(256) k_transform_tangent_rows(double* __restrict__ SX, double* __restrict__ SJ,
+                                                                int64_t ldS, const double* __restrict__ Qg, int DS,
+                                                                const double* __restrict__ qq,
+                                                                const double* __restrict__ mm,
+                                                                const double* __restrict__ xja,
+                                                                const double* __restrict__ ae, int M, int Mpad,
+                                                                int64_t n_rows, MaternK mk, double* __restrict__ csum) {
+  const int lane = threadIdx.x & 31;
+  const int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (r >= n_rows) return;
+  const double* q = Qg + r * DS;
+  const double* t = Qg + (n_rows + r) * DS;
+  double qt = 0.0;
+  for (int e = lane; e < DS; e += 32) qt = fma(q[e], t[e], qt);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) qt += __shfl_xor_sync(0xffffffffu, qt, o);
+  double* s1 = SX + r * ldS;
+  double* s2 = SJ + r * ldS;
+  double* s3 = SX + (n_rows + r) * ldS;
+  double* s4 = SJ + (n_rows + r) * ldS;
+  const double qqr = qq[r];
+  const double q5 = 5.0 * qqr;
+  const double k_dc2 = -5.0 * mk.k_base * mk.sig_inv;
+  const double k_ads = 5.0 * mk.sig_inv;
+  double cs = 0.0, dcs = 0.0;
+  for (int m = lane; m < Mpad; m += 32) {
+    double c1 = 0.0, c2 = 0.0, dc1 = 0.0, dc2 = 0.0;
+    if (m < M) {
+      const double a = s2[m] - xja[m];
+      const double x5 = fma(-10.0, s1[m], q5 + 5.0 * mm[m]);
+      const double x = fmax(x5, 1e-300);
+      const double nrm = x * rsqrt(x);
+      const double e = exp_neg(nrm * mk.sig_inv);
+      c2 = (e * mk.k_base) * (nrm + mk.sig);
+      c1 = a * (e * mk.k_c1);
+      const double ds = qt - s3[m];
+      const double inv_nf = rsqrt(fmax(x5, fmax(HVP_X5_FLOOR * (qqr + mm[m]), 1e-300)));
+      dc2 = k_dc2 * e * ds;
+      dc1 = (e * mk.k_c1) * (s4[m] - k_ads * a * ds * inv_nf);
+      if (ae != nullptr) {
+        c1 = fma(ae[m], c2, c1);
+        dc1 = fma(ae[m], dc2, dc1);
+      }
+      cs += c1;
+      dcs += dc1;
+    }
+    s1[m] = c1;
+    s2[m] = c2;
+    s3[m] = dc1;
+    s4[m] = dc2;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    cs += __shfl_xor_sync(0xffffffffu, cs, o);
+    dcs += __shfl_xor_sync(0xffffffffu, dcs, o);
+  }
+  if (lane == 0) {
+    csum[r] = cs;
+    csum[n_rows + r] = dcs;
+  }
+}
+
+// acc (2 n_rows x DP) = [C1; dC1] XcT^T + [C2; dC2] JAT^T  ->  G = (sum c1) q - acc, dG = (sum dc1) q + (sum c1) T - acc
+__global__ void k_combine_tangent_rows(const double* __restrict__ Qg, int64_t ldq, const double* __restrict__ csum,
+                                       double* __restrict__ G, int DP, int64_t n_rows) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_rows * DP) return;
+  const int64_t r = idx / DP;
+  const int d = (int)(idx - r * DP);
+  const double q = Qg[r * ldq + d], t = Qg[(n_rows + r) * ldq + d];
+  const double cs = csum[r];
+  G[idx] = cs * q - G[idx];
+  double* dG = G + n_rows * DP;
+  dG[idx] = fma(csum[n_rows + r], q, cs * t) - dG[idx];
+}
+
+// One thread per (geometry, atom k):  HV[k] = std sum_d s_kd (g_d dF_desc[d] + dg_d F_desc[d]), s_kd = +1 for atom b
+// and -1 for atom a of pair d = (a, b), a > b (the signs of k_vec_dot_d_desc), where
+//   dg_d = d(delta / |delta|^3) = dd / |delta|^3 - 3 delta (delta . dd) / |delta|^5,   dd = v_a - v_b,
+// with the minimum-image pair vector delta rebuilt from g_d as the virial kernels do (|g| = |delta|^-2):
+//   dg_d = |g|^3/2 dd - 3 (g . dd) g / |g|^1/2.
+__global__ void __launch_bounds__(256) k_hvp_project(const double* __restrict__ Fd, const double* __restrict__ dFd,
+                                                     const double* __restrict__ gq, const double* __restrict__ V,
+                                                     int n_atoms, int D, double std, int64_t n_geo,
+                                                     double* __restrict__ HV) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_geo * n_atoms) return;
+  const int64_t b = idx / n_atoms;
+  const int k = (int)(idx - b * n_atoms);
+  const double* v = V + b * 3 * n_atoms;
+  const double* f = Fd + b * D;
+  const double* df = dFd + b * D;
+  const double* g = gq + b * (int64_t)D * 3;
+  double h0 = 0.0, h1 = 0.0, h2 = 0.0;
+  for (int o = 0; o < n_atoms; ++o) {
+    if (o == k) continue;
+    const int pa = max(o, k), pb = min(o, k);
+    const int d = pair_index(pa, pb);
+    const double gx = g[d * 3 + 0], gy = g[d * 3 + 1], gz = g[d * 3 + 2];
+    const double ddx = v[3 * pa + 0] - v[3 * pb + 0];
+    const double ddy = v[3 * pa + 1] - v[3 * pb + 1];
+    const double ddz = v[3 * pa + 2] - v[3 * pb + 2];
+    const double gn = sqrt(gx * gx + gy * gy + gz * gz);
+    const double sgn = sqrt(gn);
+    const double fv = f[d], dfv = df[d];
+    const double cd = gn * sgn * fv;                              // |g|^3/2 F_desc
+    const double cg = dfv - 3.0 * (gx * ddx + gy * ddy + gz * ddz) * fv / sgn;  // dF_desc - 3 (g . dd) F_desc / |g|^1/2
+    const double s = (k == pb) ? 1.0 : -1.0;
+    h0 += s * fma(cg, gx, cd * ddx);
+    h1 += s * fma(cg, gy, cd * ddy);
+    h2 += s * fma(cg, gz, cd * ddz);
+  }
+  HV[idx * 3 + 0] = h0 * std;
+  HV[idx * 3 + 1] = h1 * std;
+  HV[idx * 3 + 2] = h2 * std;
+}
+
 }  // namespace sgdml
 
 using namespace sgdml;
@@ -1277,6 +1417,14 @@ struct sgdml_b200_model {
     Lattice* lat = nullptr;     // (geo) the chunk's cells of a call with one cell per geometry
     OzOperand ozQ, ozC1, ozC2;  // slices of the per-batch operands (int8 path of large descriptors)
   } ws[2];
+  // sgdml_b200_predict_hvp: a workspace of its own, grown on first use (predict's slots, graphs and generation are never
+  // touched).  Query and tangent rows are stacked: Qg, qq, SX (S1; S3), SJ (S2; S4), G (G; dG), csum hold 2 x rows.
+  struct HvpWS {
+    int64_t geo = 0;
+    double *R = nullptr, *V = nullptr, *HV = nullptr, *xq = nullptr, *gq = nullptr, *t = nullptr, *Qg = nullptr,
+           *qq = nullptr, *SX = nullptr, *SJ = nullptr, *G = nullptr, *csum = nullptr, *Fd = nullptr, *dFd = nullptr,
+           *mu0 = nullptr;  // mu0: DS zeros, the "mean" of the tangent rows
+  } hvp;
   cudaStream_t pipe_stream[2] = {nullptr, nullptr};
   cudaEvent_t pipe_event[3] = {nullptr, nullptr, nullptr};
   // MD latency path: the launch sequence of a small host-buffer batch, captured once per batch size into a CUDA graph
@@ -2034,6 +2182,158 @@ int predict_train_impl(sgdml_b200_model* m, int64_t m_begin, int64_t m_end, int 
   return 0;
 }
 
+// ---------------------------------------------------------------- Hessian-vector products
+void free_hvp_ws(sgdml_b200_model::HvpWS& w) {
+  for (double* p : {w.R, w.V, w.HV, w.xq, w.gq, w.t, w.Qg, w.qq, w.SX, w.SJ, w.G, w.csum, w.Fd, w.dFd, w.mu0})
+    cached_free(p);
+  w = sgdml_b200_model::HvpWS();
+}
+
+// geometries per HVP chunk: S1-S4 (4 x Mpad) and G, dG (2 x DP) per virtual row within ~2 GB
+int64_t hvp_chunk_geos(const sgdml_b200_model* m) {
+  const int64_t row_bytes = 8 * (4 * (int64_t)m->Mpad + 2 * (int64_t)m->DP);
+  int64_t g = (int64_t)(2048ll << 20) / (row_bytes * m->S);
+  g = std::max<int64_t>(1, std::min<int64_t>(g, 65536));
+  if (g_chunk_cap > 0 && g > g_chunk_cap) g = g_chunk_cap;
+  return g;
+}
+
+// The transposed model matrices of the second contraction: kept by large-descriptor models anyway, made on the first HVP
+// of a fused-kernel model (and from then on refreshed by set_alphas); then the workspace for n_geo geometries.
+int ensure_hvp_ws(sgdml_b200_model* m, int64_t n_geo, cudaStream_t s) {
+  if (m->XcT == nullptr) {
+    SG_CUDA(cached_malloc(&m->XcT, sizeof(double) * (size_t)m->DP * m->Mpad));
+    SG_CUDA(cached_malloc(&m->JAT, sizeof(double) * (size_t)m->DP * m->Mpad));
+    SG_TRY(refresh_transposes(m, true, s));
+  }
+  sgdml_b200_model::HvpWS& w = m->hvp;
+  if (n_geo <= w.geo) return 0;
+  if (w.geo > 0) SG_CUDA(cudaDeviceSynchronize());  // earlier calls may still run on the old workspace
+  free_hvp_ws(w);
+  const int64_t rows2 = 2 * n_geo * m->S;
+  const int64_t dimi = 3 * (int64_t)m->N;
+  SG_CUDA(cached_malloc(&w.R, sizeof(double) * n_geo * dimi));
+  SG_CUDA(cached_malloc(&w.V, sizeof(double) * n_geo * dimi));
+  SG_CUDA(cached_malloc(&w.HV, sizeof(double) * n_geo * dimi));
+  SG_CUDA(cached_malloc(&w.xq, sizeof(double) * n_geo * m->D));
+  SG_CUDA(cached_malloc(&w.gq, sizeof(double) * n_geo * m->D * 3));
+  SG_CUDA(cached_malloc(&w.t, sizeof(double) * n_geo * m->D));
+  SG_CUDA(cached_malloc(&w.Qg, sizeof(double) * rows2 * m->DS));
+  SG_CUDA(cached_malloc(&w.qq, sizeof(double) * rows2));
+  SG_CUDA(cached_malloc(&w.SX, sizeof(double) * rows2 * m->Mpad));
+  SG_CUDA(cached_malloc(&w.SJ, sizeof(double) * rows2 * m->Mpad));
+  SG_CUDA(cached_malloc(&w.G, sizeof(double) * rows2 * m->DP));
+  SG_CUDA(cached_malloc(&w.csum, sizeof(double) * rows2));
+  SG_CUDA(cached_malloc(&w.Fd, sizeof(double) * n_geo * m->D));
+  SG_CUDA(cached_malloc(&w.dFd, sizeof(double) * n_geo * m->D));
+  SG_CUDA(cached_malloc(&w.mu0, sizeof(double) * m->DS));
+  SG_CUDA(cudaMemsetAsync(w.mu0, 0, sizeof(double) * m->DS, s));
+  w.geo = n_geo;
+  return 0;
+}
+
+// sgdml_b200_predict_hvp: always the GEMM-composed form in FP64 (the int8-slice setting of large descriptors does not
+// apply), in the model's cell, chunk by chunk on the caller's stream
+int hvp_impl(sgdml_b200_model* m, const double* R, const double* V, int64_t n_geo, double* HV, cudaStream_t s) {
+  const bool R_dev = is_device_ptr(R), V_dev = is_device_ptr(V), HV_dev = is_device_ptr(HV);
+  const int dimi = 3 * m->N;
+  const int64_t chunk = std::min<int64_t>(hvp_chunk_geos(m), n_geo);
+  SG_TRY(ensure_hvp_ws(m, chunk, s));
+  sgdml_b200_model::HvpWS& w = m->hvp;
+  MaternK mk;
+  mk.sig = m->sig;
+  mk.sig_inv = 1.0 / m->sig;
+  mk.k_base = 5.0 / (3.0 * m->sig * m->sig * m->sig);
+  mk.k_c1 = mk.k_base * 5.0 / m->sig;
+  for (int64_t g0 = 0; g0 < n_geo; g0 += chunk) {
+    const int64_t ng = std::min<int64_t>(chunk, n_geo - g0);
+    const int64_t rows = ng * m->S;
+    const double* Rd = R + g0 * dimi;
+    const double* Vd = V + g0 * dimi;
+    if (!R_dev) {
+      SG_CUDA(cudaMemcpyAsync(w.R, Rd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, s));
+      Rd = w.R;
+    }
+    if (!V_dev) {
+      SG_CUDA(cudaMemcpyAsync(w.V, Vd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, s));
+      Vd = w.V;
+    }
+    double* HVd = HV_dev ? HV + g0 * dimi : w.HV;
+    SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, s, m->lat, nullptr));
+    SG_TRY(launch_d_desc_dot_vec(w.gq, Vd, ng, m->N, w.t, m->D, s));
+    {
+      ProfScope ps(KID_PREDICT_AUX, s);
+      k_query_rows<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(w.xq, m->pinv, m->mu, m->D, m->DS, m->S, rows, rows,
+                                                                w.Qg, w.qq);
+      SG_CUDA(cudaGetLastError());
+      k_query_rows<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(w.t, m->pinv, w.mu0, m->D, m->DS, m->S, rows, rows,
+                                                                w.Qg + rows * m->DS, w.qq + rows);
+      SG_CUDA(cudaGetLastError());
+      count_launch(KID_PREDICT_AUX, 2);
+    }
+    {
+      ProfScope ps(KID_PREDICT_MAIN, s);
+      GemmArgs g;
+      g.alpha = 1.0;
+      g.beta = 0.0;
+      g.mode = 0;
+      g.tri = 0;
+      g.abort_flag = nullptr;
+      // [S1; S3] = [Q; T] Xc^T, [S2; S4] = [Q; T] JA^T   (2 rows x Mpad, contraction over the padded descriptor)
+      g.m = 2 * rows;
+      g.n = m->Mpad;
+      g.k = m->DS;
+      g.A = w.Qg;
+      g.lda = m->DS;
+      g.ldb = m->DS;
+      g.ldc = m->Mpad;
+      g.B = m->Xc;
+      g.C = w.SX;
+      SG_TRY(launch_gemm(g, s));
+      g.B = m->JA;
+      g.C = w.SJ;
+      SG_TRY(launch_gemm(g, s));
+      k_transform_tangent_rows<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(
+          w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, m->use_ae ? m->ae : nullptr, m->M, m->Mpad, rows, mk,
+          w.csum);
+      SG_CUDA(cudaGetLastError());
+      // acc = [C1; dC1] XcT^T + [C2; dC2] JAT^T   (2 rows x DP, contraction over the training points)
+      g.n = m->DP;
+      g.k = m->Mpad;
+      g.lda = m->Mpad;
+      g.ldb = m->Mpad;
+      g.ldc = m->DP;
+      g.A = w.SX;
+      g.B = m->XcT;
+      g.C = w.G;
+      SG_TRY(launch_gemm(g, s));
+      g.mode = 1;
+      g.A = w.SJ;
+      g.B = m->JAT;
+      SG_TRY(launch_gemm(g, s));
+      k_combine_tangent_rows<<<(unsigned)((rows * m->DP + 255) / 256), 256, 0, s>>>(w.Qg, m->DS, w.csum, w.G, m->DP,
+                                                                                     rows);
+      SG_CUDA(cudaGetLastError());
+      count_launch(KID_PREDICT_MAIN, 2);
+    }
+    {
+      ProfScope ps(KID_PREDICT_FINISH, s);
+      const dim3 grid((unsigned)ceil_div(m->D, 256), (unsigned)std::min<int64_t>(ng, 65535));
+      k_fdesc_gather<<<grid, 256, 0, s>>>(w.G, m->perm, m->D, m->DP, m->S, 1, rows, ng, w.Fd);
+      SG_CUDA(cudaGetLastError());
+      k_fdesc_gather<<<grid, 256, 0, s>>>(w.G + rows * m->DP, m->perm, m->D, m->DP, m->S, 1, rows, ng, w.dFd);
+      SG_CUDA(cudaGetLastError());
+      k_hvp_project<<<(unsigned)ceil_div(ng * m->N, 256), 256, 0, s>>>(w.Fd, w.dFd, w.gq, Vd, m->N, m->D, m->std, ng,
+                                                                       HVd);
+      SG_CUDA(cudaGetLastError());
+      count_launch(KID_PREDICT_FINISH, 3);
+    }
+    if (!HV_dev) SG_CUDA(cudaMemcpyAsync(HV + g0 * dimi, HVd, sizeof(double) * ng * dimi, cudaMemcpyDeviceToHost, s));
+  }
+  if (!R_dev || !V_dev || !HV_dev) SG_CUDA(cudaStreamSynchronize(s));
+  return 0;
+}
+
 }  // namespace
 
 int sgdml_b200_model_destroy(sgdml_b200_model* m) {
@@ -2059,6 +2359,7 @@ int sgdml_b200_model_destroy(sgdml_b200_model* m) {
   free_oz(m->ozXcT);
   free_oz(m->ozJAT);
   free_ws(m);
+  free_hvp_ws(m->hvp);
   for (int i = 0; i < 2; ++i)
     if (m->pipe_stream[i]) cudaStreamDestroy(m->pipe_stream[i]);
   for (int i = 0; i < 3; ++i)
@@ -2103,6 +2404,14 @@ int sgdml_b200_predict_virial_cells(sgdml_b200_model* m, const double* R, int64_
   }
   if (n_geo == 0) return 0;
   return predict_impl(m, R, n_geo, cells.data(), n_geo, E, F, W, (cudaStream_t)stream);
+}
+
+int sgdml_b200_predict_hvp(sgdml_b200_model* m, const double* R, const double* V, int64_t n_geo, double* HV,
+                           void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(m != nullptr && R != nullptr && V != nullptr && HV != nullptr && n_geo >= 0);
+  if (n_geo == 0) return 0;
+  return hvp_impl(m, R, V, n_geo, HV, (cudaStream_t)stream);
 }
 
 int sgdml_b200_model_set_lattice(sgdml_b200_model* m, const double* lattice, const double* lattice_inv) {
@@ -2160,10 +2469,9 @@ int sgdml_b200_model_set_alphas(sgdml_b200_model* m, const double* alphas_F, voi
   SG_CUDA(cudaGetLastError());
   count_launch(KID_PREDICT_AUX);
   SG_TRY(refresh_row_dots(m, false, s));
-  if (m->large) {
-    SG_TRY(refresh_transposes(m, false, s));
-    SG_TRY(refresh_oz_model(m, false, s));
-  }
+  // JA^T: always kept by large-descriptor models, and by fused-kernel models once they have served an HVP
+  if (m->JAT != nullptr) SG_TRY(refresh_transposes(m, false, s));
+  if (m->large) SG_TRY(refresh_oz_model(m, false, s));
   if (sA.staged()) SG_CUDA(cudaStreamSynchronize(s));
   return 0;
 }

@@ -305,6 +305,43 @@ class GDMLPredict(object):
         )
         return self._results(E, F, W, return_E, with_W)
 
+    def predict_hvp(self, R, V, out=None):
+        """Extension: the directional derivative of the forces along V, HV = (dF/dR) V = -H V with H the energy Hessian,
+        for every geometry.  R, V (B, 3N) [or (3N,)] -> HV (B, 3N), in the model's cell, always in FP64.
+
+        This is the product autograd needs to differentiate through F (`torchtools.GDMLTorchPredict`); it costs about
+        one more prediction.  V must match R in shape, dtype and device.  `out`: a preallocated HV buffer checked as
+        `predict`'s F.  NumPy / torch conventions as `predict`: CUDA tensors in place, pinned in -> pinned out."""
+        if type(V) is not type(R) or tuple(V.shape) != tuple(R.shape) or V.dtype != R.dtype:
+            raise ValueError('V must match R in type, shape and dtype')
+        if not isinstance(R, np.ndarray) and V.device != R.device:
+            raise ValueError('V lives on %s but R on %s' % (V.device, R.device))
+        dim_i = 3 * self.n_atoms
+        size = R.size if isinstance(R, np.ndarray) else R.numel()
+        if size % dim_i != 0 or (R.ndim == 2 and R.shape[1] != dim_i):
+            raise ValueError('R must have 3*n_atoms columns')
+        if isinstance(R, np.ndarray):
+            R = np.ascontiguousarray(R, dtype=np.float64).reshape(-1, dim_i)
+            V = np.ascontiguousarray(V, dtype=np.float64).reshape(-1, dim_i)
+            HV = np.empty_like(R) if out is None else out
+        else:
+            import torch
+
+            if R.dtype != torch.float64:
+                raise ValueError('torch inputs must be float64')
+            R = R.contiguous().reshape(-1, dim_i)
+            V = V.contiguous().reshape(-1, dim_i)
+            pin = (not R.is_cuda) and R.is_pinned()
+            HV = torch.empty(R.shape, dtype=torch.float64, device=R.device, pin_memory=pin) if out is None else out
+        n = R.shape[0]
+        if out is not None:
+            self._check_out(R, None, HV, None, n, dim_i)
+        _lib.check(
+            _lib.lib().sgdml_b200_predict_hvp(self._handle, _lib.ptr(R), _lib.ptr(V), n, _lib.ptr(HV), _lib.current_stream()),
+            'predict_hvp',
+        )
+        return HV
+
     @staticmethod
     def _results(E, F, W, return_E, with_W):
         res = (F, W) if with_W else (F,)

@@ -137,6 +137,49 @@ int sgdml_b200_predict_virial_cells(sgdml_b200_model* model, const double* R, in
 int sgdml_b200_predict_hvp(sgdml_b200_model* model, const double* R, const double* V, int64_t n_geo,
                            double* HV, void* stream);
 
+/* ---------------------------------------------------------------- molecular dynamics on the device
+ * Extension: BAOAB Langevin (velocity Verlet at gamma = 0) trajectories of n_rep replicas of one model, many steps per
+ * call.  Positions, velocities and forces stay in device memory between steps and between calls; one step is the
+ * integrator kernel followed by sgdml_b200_predict's descriptor and predictor kernels on the device-resident positions,
+ * captured once into a CUDA graph and replayed n_steps times on `stream` without host synchronisation
+ * (SGDML_B200_GRAPH=0: plain launches, bit-identical).
+ * Units: the model's throughout.  Positions in its length unit L, forces and E_pot as sgdml_b200_predict returns them
+ * (std and c applied), a time unit T of the caller's choice; inv_mass[a] turns the force on atom a into an acceleration
+ * in L / T^2, and kT is in the model's energy unit.
+ * One step from (r, v, F(r)), with h = dt / 2, c1 = exp(-gamma dt), s_i the inv_mass of the atom of coordinate i and
+ * sigma_i = sqrt((1 - c1^2) kT s_i), all computed once per run on the host in double precision:
+ *   B  v = v + h (F s)    A  r = r + h v    O  v = c1 v + sigma xi    A  r = r + h v    F, E_pot at r    B  v = v + h (F s)
+ * The B and A updates are rounded exactly as written (no fused multiply-add).  gamma == 0 skips O (no draws).
+ * xi: Philox4x32-10 with key (seed mod 2^32, seed >> 32) and counter (j, replica, step mod 2^32, step >> 32) for the
+ * coordinates 2j and 2j + 1, step being the handle's step index of the step taken; the output words u0..u3 give
+ * U_a = ((u0 2^32 + u1) >> 11 + 0.5) 2^-53, U_b likewise from u2, u3, and xi_2j = sqrt(-2 ln U_a) cos(2 pi U_b),
+ * xi_2j+1 = sqrt(-2 ln U_a) sin(2 pi U_b).  A trajectory continued over several runs draws the noise of one long run.
+ * E_kin = 1/2 sum_i v_i^2 / s_i per replica, summed in a fixed order (runs are reproducible bit for bit).
+ * The model must outlive the handle.  The handle keeps its own predictor workspace: sgdml_b200_predict* calls and MD
+ * runs never invalidate each other's buffers or graphs.  The F and E_pot that set_state stored are NOT refreshed when
+ * the model changes (set_alphas, set_alphas_E, set_lattice, ...): call sgdml_b200_md_set_state again after such a
+ * change.  Later runs do evaluate the changed model.  Batches above the predictor's chunk size (fixed when the handle is
+ * created) run their chunks inside each step.  Launches count under family 8 (integrator) and 1 (graph replays).
+ * Arrays are host or device pointers as elsewhere in this header; calls with host outputs synchronise `stream`.
+ * Argument errors are reported before anything is queued, and a rejected call changes nothing. */
+typedef struct sgdml_b200_md sgdml_b200_md;
+/* inv_mass (N,) HOST doubles, each finite and > 0; n_rep >= 1. */
+int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* model, int64_t n_rep, const double* inv_mass);
+int sgdml_b200_md_destroy(sgdml_b200_md* md);
+/* R, V (n_rep, 3N); V may be NULL (= 0).  Sets every replica's step index to `step` and evaluates F and E_pot at R.
+ * V is the full-step velocity that belongs to R. */
+int sgdml_b200_md_set_state(sgdml_b200_md* md, const double* R, const double* V, uint64_t step, void* stream);
+/* R, V, F (n_rep, 3N), E_pot (n_rep), step (1,): the state after the last run; any output may be NULL. */
+int sgdml_b200_md_get_state(sgdml_b200_md* md, double* R, double* V, double* F, double* E_pot, uint64_t* step,
+                            void* stream);
+/* n_steps >= 0 steps of size dt (finite, > 0) with friction gamma >= 0 (1 / T) at temperature kT >= 0; kT > 0 with
+ * gamma == 0 is rejected.  stride = 0: no frames; otherwise n_steps must be a multiple of stride, and frame k is the
+ * state after step (k + 1) stride of this run: R_frames, V_frames (n_frames, n_rep, 3N), E_pot_frames, E_kin_frames
+ * (n_frames, n_rep), n_frames = n_steps / stride; each may be NULL.  Needs a state (sgdml_b200_md_set_state). */
+int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, uint64_t seed,
+                      int64_t stride, double* R_frames, double* V_frames, double* E_pot_frames,
+                      double* E_kin_frames, void* stream);
+
 /* Periodic model (predict.py:332-334: lat_and_inv from model['lattice']): query descriptors of
  * sgdml_b200_predict are built with the minimum-image convention.  Both NULL: back to a free molecule. */
 int sgdml_b200_model_set_lattice(sgdml_b200_model* model, const double* lattice, const double* lattice_inv);

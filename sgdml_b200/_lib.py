@@ -41,6 +41,15 @@ SIGNATURES = {
     'sgdml_b200_predict_virial_cells': (
         C.c_int, [c_void_p, c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_predict_hvp': (C.c_int, [c_void_p, c_void_p, c_void_p, i64, c_void_p, c_void_p]),
+    'sgdml_b200_md_create': (C.c_int, [C.POINTER(c_void_p), c_void_p, i64, c_void_p]),
+    'sgdml_b200_md_destroy': (C.c_int, [c_void_p]),
+    'sgdml_b200_md_set_state': (C.c_int, [c_void_p, c_void_p, c_void_p, C.c_uint64, c_void_p]),
+    'sgdml_b200_md_get_state': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_md_run': (
+        C.c_int,
+        [c_void_p, i64, C.c_double, C.c_double, C.c_double, C.c_uint64, i64, c_void_p, c_void_p, c_void_p, c_void_p,
+         c_void_p],
+    ),
     'sgdml_b200_model_set_R_d_desc': (C.c_int, [c_void_p, c_void_p]),
     'sgdml_b200_model_set_alphas': (C.c_int, [c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_predict_train': (C.c_int, [c_void_p, i64, i64, C.c_int, c_void_p, c_void_p, c_void_p]),

@@ -29,6 +29,7 @@
 
 #include "common.cuh"
 #include "desc.cuh"
+#include "md.cuh"
 #include "solve.cuh"
 
 namespace sgdml {
@@ -1550,14 +1551,13 @@ void free_ws(sgdml_b200_model* m) {
 // k_fdesc_gather / k_fdesc_project with the workspace w.Fd
 bool fdesc_in_ws(const sgdml_b200_model* m) { return sizeof(double) * (size_t)m->D > 200 * 1024; }
 
-int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
-  sgdml_b200_model::WS& w = m->ws[slot];
+// grows w to n_geo queries; returns 1 when it reallocated (pointers changed), 0 when it was large enough
+int grow_ws(sgdml_b200_model* m, sgdml_b200_model::WS& w, int64_t n_geo) {
   if (!m->large) {  // room for the per-split output planes of small batches (<= ~300 CTAs x BQ rows)
     const int64_t min_geo = (int64_t)(2 * num_sms() + 8) * m->BQ / m->S + 1;
     n_geo = std::max<int64_t>(n_geo, std::min<int64_t>(min_geo, chunk_geos(m)));
   }
   if (n_geo <= w.geo) return 0;
-  ++m->generation;  // captured graphs hold the old workspace pointers
   if (w.geo > 0) SG_CUDA(cudaDeviceSynchronize());  // earlier batches may still run on the old workspace
   free_ws_slot(w);
   SG_CUDA(cached_malloc(&w.xq, sizeof(double) * n_geo * m->D));
@@ -1592,7 +1592,13 @@ int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
     }
   }
   w.geo = n_geo;
-  return 0;
+  return 1;
+}
+
+int ensure_ws(sgdml_b200_model* m, int slot, int64_t n_geo) {
+  const int rc = grow_ws(m, m->ws[slot], n_geo);
+  if (rc != 0) ++m->generation;  // captured graphs hold the old (or freed) workspace pointers
+  return rc < 0 ? rc : 0;
 }
 
 int ensure_pipe(sgdml_b200_model* m) {
@@ -1619,9 +1625,9 @@ int64_t chunk_geos(const sgdml_b200_model* m) {
 constexpr int64_t GRAPH_MAX_GEO = 16;  // batches up to this size with host buffers replay a captured graph
 // xq == nullptr: the query rows (w.Qg, w.qq) are already in place (k_desc_query_rows)
 // W_dev != nullptr: the finishing kernels' virial variants also write W (n_geo x 9); E and F are unchanged by it
-int run_queries(sgdml_b200_model* m, int slot, const double* xq, const double* gq, int64_t n_geo, double std,
-                double c, double* E_dev, double* F_dev, cudaStream_t s, double* W_dev = nullptr) {
-  sgdml_b200_model::WS& w = m->ws[slot];
+// w: one of the model's workspace slots, or the workspace of an MD handle
+int run_queries(sgdml_b200_model* m, sgdml_b200_model::WS& w, const double* xq, const double* gq, int64_t n_geo,
+                double std, double c, double* E_dev, double* F_dev, cudaStream_t s, double* W_dev = nullptr) {
   const int64_t n_rows = n_geo * m->S;
   const int64_t n_rows_pad = (n_rows + m->BQ - 1) / m->BQ * m->BQ;
   int n_splits = 1;
@@ -1996,13 +2002,13 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
                                                                n_rows_pad, w.gq, w.Qg, w.qq, q->hLat);
       SG_CUDA(cudaGetLastError());
       count_launch(KID_PREDICT_AUX);
-      SG_TRY(run_queries(m, 0, nullptr, w.gq, n_geo, m->std, m->c, with_E ? q->hE : nullptr, q->hF, gs, q->hW));
+      SG_TRY(run_queries(m, w, nullptr, w.gq, n_geo, m->std, m->c, with_E ? q->hE : nullptr, q->hF, gs, q->hW));
       return 0;
     }
     SG_CUDA(cudaMemcpyAsync(w.R, q->hR, sizeof(double) * n_geo * dimi, cudaMemcpyHostToDevice, gs));
     SG_CUDA(cudaMemcpyAsync(q->dLat, q->hLat, sizeof(Lattice) * n_geo, cudaMemcpyHostToDevice, gs));
     SG_TRY(launch_desc_from_R(w.R, n_geo, m->N, w.xq, w.gq, gs, Lattice{}, q->dLat));
-    SG_TRY(run_queries(m, 0, w.xq, w.gq, n_geo, m->std, m->c, with_E ? w.E : nullptr, w.F, gs, with_W ? w.W : nullptr));
+    SG_TRY(run_queries(m, w, w.xq, w.gq, n_geo, m->std, m->c, with_E ? w.E : nullptr, w.F, gs, with_W ? w.W : nullptr));
     SG_CUDA(cudaMemcpyAsync(q->hF, w.F, sizeof(double) * n_geo * dimi, cudaMemcpyDeviceToHost, gs));
     if (with_E) SG_CUDA(cudaMemcpyAsync(q->hE, w.E, sizeof(double) * n_geo, cudaMemcpyDeviceToHost, gs));
     if (with_W) SG_CUDA(cudaMemcpyAsync(q->hW, w.W, sizeof(double) * n_geo * 9, cudaMemcpyDeviceToHost, gs));
@@ -2119,7 +2125,7 @@ int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Latt
     double* Fd = F_dev ? F + g0 * dimi : w.F;
     double* Ed = (E == nullptr) ? nullptr : (E_dev ? E + g0 : w.E);
     double* Wd = (W == nullptr) ? nullptr : (W_dev ? W + g0 * 9 : w.W);
-    SG_TRY(run_queries(m, slot, w.xq, w.gq, ng, m->std, m->c, Ed, Fd, st, Wd));
+    SG_TRY(run_queries(m, w, w.xq, w.gq, ng, m->std, m->c, Ed, Fd, st, Wd));
     if (!F_dev) SG_CUDA(cudaMemcpyAsync(F + g0 * dimi, Fd, sizeof(double) * ng * dimi, cudaMemcpyDeviceToHost, st));
     if (E != nullptr && !E_dev) SG_CUDA(cudaMemcpyAsync(E + g0, Ed, sizeof(double) * ng, cudaMemcpyDeviceToHost, st));
     if (W != nullptr && !W_dev) SG_CUDA(cudaMemcpyAsync(W + g0 * 9, Wd, sizeof(double) * ng * 9, cudaMemcpyDeviceToHost, st));
@@ -2173,7 +2179,7 @@ int predict_train_impl(sgdml_b200_model* m, int64_t m_begin, int64_t m_end, int 
     double* Fd = F_dev ? F + g0 * dimi : w.F;
     double* Ed = (E == nullptr) ? nullptr : (E_dev ? E + g0 : w.E);
     double* Wd = (W == nullptr) ? nullptr : (W_dev ? W + g0 * 9 : w.W);
-    SG_TRY(run_queries(m, 0, xq, gq, ng, std, c, Ed, Fd, s, Wd));
+    SG_TRY(run_queries(m, w, xq, gq, ng, std, c, Ed, Fd, s, Wd));
     if (!F_dev) SG_CUDA(cudaMemcpyAsync(F + g0 * dimi, Fd, sizeof(double) * ng * dimi, cudaMemcpyDeviceToHost, s));
     if (E != nullptr && !E_dev) SG_CUDA(cudaMemcpyAsync(E + g0, Ed, sizeof(double) * ng, cudaMemcpyDeviceToHost, s));
     if (W != nullptr && !W_dev) SG_CUDA(cudaMemcpyAsync(W + g0 * 9, Wd, sizeof(double) * ng * 9, cudaMemcpyDeviceToHost, s));
@@ -2538,6 +2544,325 @@ int sgdml_b200_model_get_R_d_desc_alpha(sgdml_b200_model* m, double* out) {
   SG_TRY(sO.finish(0));
   SG_CUDA(cudaStreamSynchronize(0));
   return 0;
+}
+
+}  // extern "C"
+
+// ============================================================== molecular dynamics (sgdml_b200_md_*)
+// The state of n_rep replicas stays in device memory between steps and between runs.  One step is the integrator
+// kernel (csrc/md.cu), then the descriptors of the new positions in the model's cell and the predictor on them, chunk by
+// chunk, writing F and E_pot back into the state.  That sequence is captured once into a CUDA graph and replayed
+// n_steps times on the caller's stream; everything a run changes (dt, gamma, kT, seed, frame buffers) lives in device
+// memory, and the step counter is advanced by the integrator, so the graph bakes in no run.
+struct sgdml_b200_md {
+  sgdml_b200_model* m = nullptr;
+  int64_t n_rep = 0, chunk = 0;
+  int dimi = 0;
+  sgdml_b200_model::WS ws;  // the handle's own predictor workspace: predict calls never touch it, MD never theirs
+  int ws_oz = 0;            // the int8 slice count its buffers were sized for
+  double *R = nullptr, *V = nullptr, *F = nullptr, *E = nullptr;  // state: (n_rep, 3N) x 3, (n_rep)
+  double *Fs = nullptr, *Es = nullptr;  // outputs of the force evaluation that precedes a capture
+  uint64_t* step = nullptr;             // (n_rep) step counters, all equal
+  uint64_t step_host = 0;               // their value once the queued runs have finished
+  bool has_state = false;
+  double *s = nullptr, *sigma = nullptr;  // (3N) inverse mass and noise scale per coordinate
+  std::vector<double> s_host;             // s on the host
+  MdParams* dP = nullptr;
+  MdParams* hP = nullptr;     // pinned staging of dP and sigma, reused once the previous run's upload is done
+  double* hSigma = nullptr;
+  cudaEvent_t uploaded = nullptr;
+  cudaStream_t gs = nullptr;  // capture stream
+  cudaEvent_t ge = nullptr;
+  cudaGraphExec_t exec = nullptr;
+  uint64_t generation = 0;    // the model's generation at capture
+  Lattice lat = {0, {0}, {0}};  // the model's cell at capture (passed to the descriptor kernel by value)
+  int n_kernels = 0;
+};
+
+namespace {
+
+void md_free(sgdml_b200_md* md) {
+  cudaDeviceSynchronize();  // blocks go back to the cache: nothing may still use them
+  if (md->exec) cudaGraphExecDestroy(md->exec);
+  if (md->gs) cudaStreamDestroy(md->gs);
+  if (md->ge) cudaEventDestroy(md->ge);
+  if (md->uploaded) cudaEventDestroy(md->uploaded);
+  free_ws_slot(md->ws);
+  for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s, md->sigma}) cached_free(p);
+  cached_free(md->step);
+  cached_free(md->dP);
+  cudaFreeHost(md->hP);
+  cudaFreeHost(md->hSigma);
+  delete md;
+}
+
+// the workspace for the current model settings; a reallocation drops the captured step
+int md_ready(sgdml_b200_md* md) {
+  sgdml_b200_model* m = md->m;
+  if (md->ws_oz != m->oz_s) {  // slice buffers sized for another contraction setting
+    SG_CUDA(cudaDeviceSynchronize());
+    free_ws_slot(md->ws);
+    md->ws_oz = m->oz_s;
+  }
+  const int rc = grow_ws(m, md->ws, md->chunk);
+  if (rc != 0 && md->exec != nullptr) {
+    cudaGraphExecDestroy(md->exec);
+    md->exec = nullptr;
+  }
+  return rc < 0 ? rc : 0;
+}
+
+// F(R), E(R) of every replica, chunk by chunk, exactly as sgdml_b200_predict evaluates device-resident geometries
+int md_forces(sgdml_b200_md* md, double* F, double* E, cudaStream_t s) {
+  sgdml_b200_model* m = md->m;
+  sgdml_b200_model::WS& w = md->ws;
+  for (int64_t g0 = 0; g0 < md->n_rep; g0 += md->chunk) {
+    const int64_t ng = std::min<int64_t>(md->chunk, md->n_rep - g0);
+    SG_TRY(launch_desc_from_R(md->R + g0 * md->dimi, ng, m->N, w.xq, w.gq, s, m->lat, nullptr));
+    SG_TRY(run_queries(m, w, w.xq, w.gq, ng, m->std, m->c, E + g0, F + g0 * md->dimi, s));
+  }
+  return 0;
+}
+
+int md_step(sgdml_b200_md* md, cudaStream_t s) {
+  SG_TRY(launch_md_step(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step, md->n_rep, md->dimi, 1, s));
+  return md_forces(md, md->F, md->E, s);
+}
+
+bool same_cell(const Lattice& a, const Lattice& b) {
+  if (a.on != b.on) return false;
+  return !a.on || (std::equal(a.vec, a.vec + 9, b.vec) && std::equal(a.inv, a.inv + 9, b.inv));
+}
+
+// the step graph, captured again whenever something it bakes in has changed: the workspace (md_ready), the model's
+// generation (use_ae, contraction slices) or the model's cell
+int md_graph(sgdml_b200_md* md, cudaStream_t s) {
+  sgdml_b200_model* m = md->m;
+  if (md->exec != nullptr && md->generation == m->generation && same_cell(md->lat, m->lat)) return 0;
+  if (md->exec != nullptr) {
+    cudaGraphExecDestroy(md->exec);
+    md->exec = nullptr;
+  }
+  if (md->gs == nullptr) {
+    SG_CUDA(cudaStreamCreateWithFlags(&md->gs, cudaStreamNonBlocking));
+    SG_CUDA(cudaEventCreateWithFlags(&md->ge, cudaEventDisableTiming));
+  }
+  // captured on a private stream (the caller's may be the legacy stream); after the caller's queued work
+  SG_CUDA(cudaEventRecord(md->ge, s));
+  SG_CUDA(cudaStreamWaitEvent(md->gs, md->ge, 0));
+  // the force evaluation once un-captured, into scratch outputs: sets the kernels' shared-memory attributes
+  SG_TRY(md_forces(md, md->Fs, md->Es, md->gs));
+  SG_CUDA(cudaStreamSynchronize(md->gs));
+  int64_t before = 0, after = 0;
+  for (int k = 0; k < KID_COUNT; ++k) {
+    int64_t ln = 0;
+    sgdml_b200_profile_get(k, nullptr, nullptr, &ln);
+    before += ln;
+  }
+  cudaGraph_t graph = nullptr;
+  SG_CUDA(cudaStreamBeginCapture(md->gs, cudaStreamCaptureModeThreadLocal));
+  const int rc = md_step(md, md->gs);
+  cudaError_t e = cudaStreamEndCapture(md->gs, &graph);
+  if (rc != 0) {
+    if (graph) cudaGraphDestroy(graph);
+    return rc;
+  }
+  SG_CUDA(e);
+  e = cudaGraphInstantiate(&md->exec, graph, 0);
+  cudaGraphDestroy(graph);
+  SG_CUDA(e);
+  for (int k = 0; k < KID_COUNT; ++k) {
+    int64_t ln = 0;
+    sgdml_b200_profile_get(k, nullptr, nullptr, &ln);
+    after += ln;
+  }
+  md->n_kernels = (int)(after - before);
+  md->generation = m->generation;
+  md->lat = m->lat;
+  return 0;
+}
+
+// a frame output: the caller's device buffer, or device staging for a host buffer (copied back at the end)
+struct FrameOut {
+  double* user = nullptr;
+  double* dev = nullptr;
+  size_t bytes = 0;
+  bool staged = false;
+  int init(double* p, size_t b) {
+    user = p;
+    bytes = b;
+    if (p == nullptr) return 0;
+    if (is_device_ptr(p)) {
+      dev = p;
+      return 0;
+    }
+    staged = true;
+    SG_CUDA(cached_malloc(&dev, b));
+    return 0;
+  }
+  ~FrameOut() {
+    if (staged) cached_free(dev);
+  }
+};
+
+int md_run_impl(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, uint64_t seed, int64_t stride,
+                double* R_f, double* V_f, double* Ep_f, double* Ek_f, cudaStream_t s) {
+  const int64_t n_frames = stride > 0 ? n_steps / stride : 0;
+  const size_t fr = sizeof(double) * (size_t)(n_frames * md->n_rep);
+  FrameOut out[4];
+  if (n_frames > 0) {
+    SG_TRY(out[0].init(R_f, fr * md->dimi));
+    SG_TRY(out[1].init(V_f, fr * md->dimi));
+    SG_TRY(out[2].init(Ep_f, fr));
+    SG_TRY(out[3].init(Ek_f, fr));
+  }
+  SG_TRY(md_ready(md));
+  // the run's constants, once on the host in double precision
+  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous run has read the staging
+  MdParams& p = *md->hP;
+  p.h = 0.5 * dt;
+  p.c1 = std::exp(-gamma * dt);
+  p.key[0] = (uint32_t)seed;
+  p.key[1] = (uint32_t)(seed >> 32);
+  p.use_O = gamma > 0.0 ? 1 : 0;
+  p.stride = n_frames > 0 ? (int)stride : 0;
+  p.run_start = md->step_host;
+  p.R_f = out[0].dev;
+  p.V_f = out[1].dev;
+  p.Ep_f = out[2].dev;
+  p.Ek_f = out[3].dev;
+  for (int i = 0; i < md->dimi; ++i) md->hSigma[i] = std::sqrt((1.0 - p.c1 * p.c1) * kT * md->s_host[(size_t)i]);
+  SG_CUDA(cudaMemcpyAsync(md->dP, md->hP, sizeof(MdParams), cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * md->dimi, cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaEventRecord(md->uploaded, s));
+  if (g_graph_enabled() && !profiling_enabled()) {
+    SG_TRY(md_graph(md, s));
+    for (int64_t k = 0; k < n_steps; ++k) {
+      SG_CUDA(cudaGraphLaunch(md->exec, s));
+      count_launch(KID_PREDICT_AUX, md->n_kernels);  // the kernels of a replay are launches too
+    }
+  } else {
+    for (int64_t k = 0; k < n_steps; ++k) SG_TRY(md_step(md, s));
+  }
+  md->step_host += (uint64_t)n_steps;
+  // the second half-kick of the last step (and its frame)
+  SG_TRY(launch_md_step(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step, md->n_rep, md->dimi, 0, s));
+  bool sync = false;
+  for (auto& o : out)
+    if (o.staged) {
+      SG_CUDA(cudaMemcpyAsync(o.user, o.dev, o.bytes, cudaMemcpyDeviceToHost, s));
+      sync = true;
+    }
+  if (sync) SG_CUDA(cudaStreamSynchronize(s));
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, const double* inv_mass) {
+  SG_TRY(require_device());
+  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
+  SG_ARG(n_rep >= 1 && n_rep <= INT32_MAX);
+  SG_ARG(!is_device_ptr(inv_mass));
+  for (int i = 0; i < m->N; ++i)
+    if (!(std::isfinite(inv_mass[i]) && inv_mass[i] > 0.0)) return fail_arg("inv_mass must be finite and > 0");
+  sgdml_b200_md* md = new sgdml_b200_md();
+  md->m = m;
+  md->n_rep = n_rep;
+  md->dimi = 3 * m->N;
+  md->chunk = std::min<int64_t>(chunk_geos(m), n_rep);
+  md->ws_oz = m->oz_s;
+  auto body = [&]() -> int {
+    const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
+    for (double** p : {&md->R, &md->V, &md->F, &md->Fs}) SG_CUDA(cached_malloc(p, st));
+    SG_CUDA(cached_malloc(&md->E, sizeof(double) * n_rep));
+    SG_CUDA(cached_malloc(&md->Es, sizeof(double) * n_rep));
+    SG_CUDA(cached_malloc(&md->step, sizeof(uint64_t) * n_rep));
+    SG_CUDA(cached_malloc(&md->s, sizeof(double) * md->dimi));
+    SG_CUDA(cached_malloc(&md->sigma, sizeof(double) * md->dimi));
+    SG_CUDA(cached_malloc(&md->dP, sizeof(MdParams)));
+    SG_CUDA(cudaMallocHost(&md->hP, sizeof(MdParams)));
+    SG_CUDA(cudaMallocHost(&md->hSigma, sizeof(double) * md->dimi));
+    SG_CUDA(cudaEventCreateWithFlags(&md->uploaded, cudaEventDisableTiming));
+    md->s_host.resize((size_t)md->dimi);
+    for (int i = 0; i < md->dimi; ++i) md->s_host[(size_t)i] = inv_mass[i / 3];
+    SG_CUDA(cudaMemcpy(md->s, md->s_host.data(), sizeof(double) * md->dimi, cudaMemcpyHostToDevice));
+    SG_TRY(md_ready(md));
+    return 0;
+  };
+  const int rc = body();
+  if (rc != 0) {
+    md_free(md);
+    return rc;
+  }
+  *out = md;
+  return 0;
+}
+
+int sgdml_b200_md_destroy(sgdml_b200_md* md) {
+  if (md != nullptr) md_free(md);
+  return 0;
+}
+
+int sgdml_b200_md_set_state(sgdml_b200_md* md, const double* R, const double* V, uint64_t step, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr && R != nullptr);
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
+  SG_TRY(md_ready(md));
+  SG_CUDA(cudaMemcpyAsync(md->R, R, st, cudaMemcpyDefault, s));
+  if (V != nullptr)
+    SG_CUDA(cudaMemcpyAsync(md->V, V, st, cudaMemcpyDefault, s));
+  else
+    SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
+  const std::vector<uint64_t> steps((size_t)md->n_rep, step);
+  SG_CUDA(cudaMemcpyAsync(md->step, steps.data(), sizeof(uint64_t) * md->n_rep, cudaMemcpyHostToDevice, s));
+  SG_TRY(md_forces(md, md->F, md->E, s));
+  SG_CUDA(cudaStreamSynchronize(s));  // (the counters' host vector goes out of scope)
+  md->step_host = step;
+  md->has_state = true;
+  return 0;
+}
+
+int sgdml_b200_md_get_state(sgdml_b200_md* md, double* R, double* V, double* F, double* E_pot, uint64_t* step,
+                            void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr);
+  if (!md->has_state) return fail_arg("sgdml_b200_md_get_state: no state yet (call sgdml_b200_md_set_state)");
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
+  bool host = false;
+  auto get = [&](void* dst, const void* src, size_t bytes) -> int {
+    if (dst == nullptr) return 0;
+    host = host || !is_device_ptr(dst);
+    SG_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, s));
+    return 0;
+  };
+  SG_TRY(get(R, md->R, st));
+  SG_TRY(get(V, md->V, st));
+  SG_TRY(get(F, md->F, st));
+  SG_TRY(get(E_pot, md->E, sizeof(double) * md->n_rep));
+  SG_TRY(get(step, md->step, sizeof(uint64_t)));
+  if (host) SG_CUDA(cudaStreamSynchronize(s));
+  return 0;
+}
+
+int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, uint64_t seed,
+                      int64_t stride, double* R_frames, double* V_frames, double* E_pot_frames, double* E_kin_frames,
+                      void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
+  SG_ARG(std::isfinite(dt) && dt > 0.0);
+  SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
+  SG_ARG(std::isfinite(kT) && kT >= 0.0);
+  if (kT > 0.0 && gamma == 0.0) return fail_arg("kT > 0 needs a friction gamma > 0 (a thermostat without coupling)");
+  if (stride > 0 && n_steps % stride != 0) return fail_arg("n_steps must be a multiple of stride");
+  if (!md->has_state) return fail_arg("sgdml_b200_md_run: no state yet (call sgdml_b200_md_set_state)");
+  if (n_steps == 0) return 0;
+  return md_run_impl(md, n_steps, dt, gamma, kT, seed, stride, R_frames, V_frames, E_pot_frames, E_kin_frames,
+                     (cudaStream_t)stream);
 }
 
 }  // extern "C"

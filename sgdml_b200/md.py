@@ -1,0 +1,160 @@
+"""``GDMLDynamics`` -- molecular dynamics of many replicas on the device (``sgdml_b200_md_*`` in
+include/sgdml_b200.h): velocity-Verlet (NVE) and BAOAB Langevin (NVT) trajectories, many steps per call, with
+positions, velocities and forces kept in GPU memory between steps.
+
+Units follow ASE and ``intf.ase_calc.SGDMLCalculator``: positions in Angstrom, velocities in Angstrom/fs, masses in
+amu, energies in eV, time in fs, temperature in K.  ``E_to_eV`` and ``F_to_eV_Ang`` convert the model's units as in
+the calculator (defaults: kcal/mol and Angstrom).  Internally the engine works in the model's units with the
+femtosecond as its time unit.
+"""
+
+import ctypes
+
+import numpy as np
+
+from . import _lib
+from .intf.ase_calc import _KCAL_PER_MOL_IN_EV
+from .predict import GDMLPredict
+
+# CODATA 2014, the values ASE's units use by default (and that _KCAL_PER_MOL_IN_EV is built from)
+_E_CHARGE = 1.6021766208e-19  # C
+_AMU = 1.660539040e-27  # kg
+_K_B = 1.38064852e-23  # J / K
+FS = 1e-15 * 1e10 * np.sqrt(_E_CHARGE / _AMU)  # ase.units.fs: 1 fs in ASE's time unit Angstrom sqrt(amu / eV)
+KB_EV = _K_B / _E_CHARGE  # ase.units.kB: eV / K
+
+
+class GDMLDynamics(object):
+    """Trajectories of `n_replicas` copies of one model's system.
+
+    model: a model dict or .npz path (as ``SGDMLCalculator``), or a ``GDMLPredict``.  masses: (N,) in amu (e.g.
+    ``atoms.get_masses()``; the model stores atomic numbers, the engine has no element table).
+
+    ``set_state(positions, velocities=None, step=0)`` starts (or restarts) every replica: positions (n_replicas, N, 3)
+    [or (N, 3) for one replica] in Angstrom, velocities in Angstrom/fs (None: at rest), `step` the step index the
+    random stream continues from.  NumPy arrays or float64 CUDA tensors; ``run`` and ``get_state`` return the same
+    kind.  ``run(n_steps, dt_fs, temperature_K=0, friction_per_fs=0, seed=0, stride=0)`` integrates and returns the
+    frames after every `stride`-th step: {'positions', 'velocities': (n_frames, n_replicas, N, 3), 'potential_energy',
+    'kinetic_energy': (n_frames, n_replicas)} in Angstrom, Angstrom/fs and eV (stride 0: an empty dict).  Zero friction
+    is velocity Verlet; a temperature needs friction.
+
+    The model's F and E stored by ``set_state`` are not refreshed if the model changes afterwards: call ``set_state``
+    again then."""
+
+    def __init__(self, model, masses, n_replicas=1, E_to_eV=_KCAL_PER_MOL_IN_EV, F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        _lib.require_gpu()
+        self.gdml_predict = model if isinstance(model, GDMLPredict) else GDMLPredict(
+            model if isinstance(model, dict) else np.load(model, allow_pickle=True))
+        self.n_atoms = self.gdml_predict.n_atoms
+        self.n_replicas = int(n_replicas)
+        self.E_to_eV = float(E_to_eV)
+        self.F_to_eV_Ang = float(F_to_eV_Ang)
+        self.Ang_to_R = self.F_to_eV_Ang / self.E_to_eV  # Angstrom -> model length unit (ase_calc.py:93-94)
+        masses = np.ascontiguousarray(np.asarray(masses, dtype=np.float64).ravel())
+        if masses.shape != (self.n_atoms,):
+            raise ValueError('masses must hold one value (amu) per atom: %d' % self.n_atoms)
+        # a = F inv_mass in model length per fs^2, F in the model's force unit
+        self.inv_mass = self.F_to_eV_Ang * self.Ang_to_R * FS**2 / masses
+        self._torch_device = None
+        handle = ctypes.c_void_p()
+        _lib.check(
+            _lib.lib().sgdml_b200_md_create(ctypes.byref(handle), self.gdml_predict._handle, self.n_replicas,
+                                            _lib.ptr(self.inv_mass)),
+            'md_create',
+        )
+        self._handle = handle
+
+    def __del__(self):
+        h = getattr(self, '_handle', None)
+        if h is not None and h.value:
+            try:
+                _lib.lib().sgdml_b200_md_destroy(h)
+            except Exception:
+                pass
+            self._handle = None
+
+    # ------------------------------------------------------------------ arrays
+    def _flat(self, x, name):
+        dimi = 3 * self.n_atoms
+        if hasattr(x, 'data_ptr'):
+            import torch
+
+            if x.dtype != torch.float64 or not x.is_cuda:
+                raise ValueError('%s: torch inputs must be float64 CUDA tensors' % name)
+            n = x.numel()
+        else:
+            x = np.ascontiguousarray(x, dtype=np.float64)
+            n = x.size
+        if n != self.n_replicas * dimi:
+            raise ValueError('%s must hold n_replicas x 3N = %d x %d values' % (name, self.n_replicas, dimi))
+        return x.reshape(self.n_replicas, dimi).contiguous() if hasattr(x, 'data_ptr') else x.reshape(self.n_replicas, dimi)
+
+    def _empty(self, shape):
+        if self._torch_device is None:
+            return np.empty(shape)
+        import torch
+
+        return torch.empty(shape, dtype=torch.float64, device=self._torch_device)
+
+    # ------------------------------------------------------------------ model units (L, model energy, fs)
+    def _set_state_raw(self, R, V=None, step=0):
+        R = self._flat(R, 'positions')
+        V = None if V is None else self._flat(V, 'velocities')
+        if V is not None and hasattr(V, 'data_ptr') != hasattr(R, 'data_ptr'):
+            raise ValueError('positions and velocities must be of the same kind')
+        _lib.check(
+            _lib.lib().sgdml_b200_md_set_state(self._handle, _lib.ptr(R), _lib.ptr(V), int(step), _lib.current_stream()),
+            'md_set_state',
+        )
+        self._torch_device = R.device if hasattr(R, 'data_ptr') else None
+
+    def _get_state_raw(self):
+        shape = (self.n_replicas, 3 * self.n_atoms)
+        R, V, F, E = self._empty(shape), self._empty(shape), self._empty(shape), self._empty((self.n_replicas,))
+        step = np.zeros(1, dtype=np.uint64)
+        _lib.check(
+            _lib.lib().sgdml_b200_md_get_state(self._handle, _lib.ptr(R), _lib.ptr(V), _lib.ptr(F), _lib.ptr(E),
+                                               _lib.ptr(step), _lib.current_stream()),
+            'md_get_state',
+        )
+        return {'R': R, 'V': V, 'F': F, 'E_pot': E, 'step': int(step[0])}
+
+    def _run_raw(self, n_steps, dt, gamma=0.0, kT=0.0, seed=0, stride=0, frames=('R', 'V', 'E_pot', 'E_kin')):
+        n_steps, stride = int(n_steps), int(stride)
+        n_frames = n_steps // stride if stride > 0 and n_steps % stride == 0 else 0
+        shape = {'R': (n_frames, self.n_replicas, 3 * self.n_atoms), 'V': (n_frames, self.n_replicas, 3 * self.n_atoms),
+                 'E_pot': (n_frames, self.n_replicas), 'E_kin': (n_frames, self.n_replicas)}
+        out = {k: self._empty(shape[k]) for k in frames} if n_frames > 0 else {}
+        _lib.check(
+            _lib.lib().sgdml_b200_md_run(self._handle, n_steps, float(dt), float(gamma), float(kT), int(seed), stride,
+                                         *(_lib.ptr(out.get(k)) for k in ('R', 'V', 'E_pot', 'E_kin')),
+                                         _lib.current_stream()),
+            'md_run',
+        )
+        return out
+
+    # ------------------------------------------------------------------ ASE units
+    def set_state(self, positions, velocities=None, step=0):
+        R = self._flat(positions, 'positions') * self.Ang_to_R
+        V = None if velocities is None else self._flat(velocities, 'velocities') * self.Ang_to_R
+        self._set_state_raw(R, V, step)
+
+    def get_state(self):
+        """{'positions', 'velocities', 'forces' (n_replicas, N, 3), 'potential_energy' (n_replicas,), 'step'}: Angstrom,
+        Angstrom/fs, eV/Angstrom, eV."""
+        s = self._get_state_raw()
+        N = self.n_atoms
+        return {'positions': (s['R'] / self.Ang_to_R).reshape(-1, N, 3),
+                'velocities': (s['V'] / self.Ang_to_R).reshape(-1, N, 3),
+                'forces': (s['F'] * self.F_to_eV_Ang).reshape(-1, N, 3),
+                'potential_energy': s['E_pot'] * self.E_to_eV, 'step': s['step']}
+
+    def run(self, n_steps, dt_fs, temperature_K=0.0, friction_per_fs=0.0, seed=0, stride=0):
+        kT = KB_EV * float(temperature_K) / self.E_to_eV
+        f = self._run_raw(n_steps, dt_fs, friction_per_fs, kT, seed, stride)
+        if not f:
+            return {}
+        N, nf = self.n_atoms, f['R'].shape[0]
+        return {'positions': (f['R'] / self.Ang_to_R).reshape(nf, -1, N, 3),
+                'velocities': (f['V'] / self.Ang_to_R).reshape(nf, -1, N, 3),
+                'potential_energy': f['E_pot'] * self.E_to_eV, 'kinetic_energy': f['E_kin'] * self.E_to_eV}

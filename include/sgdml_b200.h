@@ -180,6 +180,48 @@ int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamm
                       int64_t stride, double* R_frames, double* V_frames, double* E_pot_frames,
                       double* E_kin_frames, void* stream);
 
+/* ---------------------------------------------------------------- path-integral molecular dynamics on the device
+ * Extension: ring polymers of P beads (1 <= P <= 64), thermostatted mode by mode with PILE-L (Ceriotti, Parrinello,
+ * Markland & Manolopoulos, J. Chem. Phys. 133, 124104 (2010)) in the BAOAB order of Liu, Li & Liu (J. Chem. Phys. 145,
+ * 024103 (2016)).  A handle from sgdml_b200_pimd_create holds n_poly polymers; replica r = p P + j is bead j of polymer
+ * p, and every state array has the layout of sgdml_b200_md_*: (n_poly P, 3N).  sgdml_b200_md_destroy, _set_state and
+ * _get_state work on it unchanged; sgdml_b200_md_run on a handle with P > 1 is an argument error, and a handle from
+ * sgdml_b200_md_create runs sgdml_b200_pimd_run as P = 1.  Units, streams, the step graph (one k_pimd_step launch,
+ * then the forces of every bead as ordinary replicas, chunk by chunk), SGDML_B200_GRAPH=0, the step counters, the
+ * workspace and the launch families are those of sgdml_b200_md_run above.
+ * Per run, on the host in double precision: h = dt / 2, kT_P = P kT, omega_P = kT_P / hbar,
+ * omega_k = 2 omega_P sin(k pi / P); per mode cos(omega_k h), sin(omega_k h) / omega_k and -omega_k sin(omega_k h)
+ * (1, h and 0 for k = 0); frictions gamma_0 = gamma, gamma_k = 2 lambda omega_k (k >= 1); c1_k = exp(-gamma_k dt) and
+ * sigma_{k,i} = sqrt((1 - c1_k c1_k) kT_P s_i).  Normal modes through the real orthonormal C (P x P): C_j0 = sqrt(1/P);
+ * C_jk = sqrt(2/P) cos(2 pi j k / P) for 1 <= k < P/2; C_jk = sqrt(1/P) (-1)^j for k = P/2;
+ * C_jk = sqrt(2/P) sin(2 pi j k / P) for P/2 < k < P.
+ * One step, bead by bead and mode by mode:
+ *   B  v += h (F s)      q_k = sum_j C_jk x_j, u_k = sum_j C_jk v_j (j in order, no fused multiply-add)
+ *   A  (q_k, u_k) = (cos q_k + (sin / omega) u_k, (-omega sin) q_k + cos u_k)
+ *   O  u_k = c1_k u_k + sigma_{k,i} xi      A again      x_j = sum_k C_jk q_k, v_j likewise
+ *   F, E_pot at the new positions            B  v += h (F s)
+ * Every update rounds as written.  xi is sgdml_b200_md_run's Philox normal with replica index p P + k (k the mode), so
+ * P = 1 gives sgdml_b200_md_run's trajectory bit for bit.  No mode is thermostatted (no draws) when gamma == 0 and
+ * (lambda == 0 or P == 1).  lambda = 1 damps every internal mode critically; lambda = 0.5 with gamma = 0 is
+ * thermostatted RPMD; gamma = lambda = 0 is NVE RPMD.
+ * Frames (stride as in sgdml_b200_md_run): R_frames, V_frames (n_frames, n_poly P, 3N) and E_pot_frames, E_kin_frames
+ * (n_frames, n_poly P) per bead as there; per polymer (n_frames, n_poly), with beads cyclic (x_P = x_0), m_i = 1 / s_i
+ * and xbar the centroid:
+ *   K_prim = 3N P kT / 2 - (1 / P) sum_j sum_i 1/2 m_i omega_P^2 (x_{j,i} - x_{j+1,i})^2
+ *   K_cv   = 3N kT / 2 - (1 / 2P) sum_j (x_j - xbar) . F_j
+ * the per-coordinate sums over beads in order, then over coordinates in sgdml_b200_md_run's E_kin order.  Positions
+ * are never wrapped into a cell, so both estimators hold for periodic models too. */
+/* inv_mass (N,) HOST doubles, each finite and > 0; n_poly >= 1, 1 <= n_beads <= 64, n_poly n_beads <= 2^31 - 1. */
+int sgdml_b200_pimd_create(sgdml_b200_md** out, sgdml_b200_model* model, int64_t n_poly, int64_t n_beads,
+                           const double* inv_mass);
+/* n_steps >= 0 steps of size dt (finite, > 0) at temperature kT >= 0 with hbar > 0 in the model's energy unit times T,
+ * centroid friction gamma >= 0 (1 / T) and PILE-L scale lambda >= 0.  P > 1 needs kT > 0; P = 1 follows
+ * sgdml_b200_md_run's rules (kT > 0 needs gamma > 0).  Each frame output may be NULL.  Needs a state. */
+int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma,
+                        double lambda, uint64_t seed, int64_t stride, double* R_frames, double* V_frames,
+                        double* E_pot_frames, double* E_kin_frames, double* K_prim_frames, double* K_cv_frames,
+                        void* stream);
+
 /* Periodic model (predict.py:332-334: lat_and_inv from model['lattice']): query descriptors of
  * sgdml_b200_predict are built with the minimum-image convention.  Both NULL: back to a free molecule. */
 int sgdml_b200_model_set_lattice(sgdml_b200_model* model, const double* lattice, const double* lattice_inv);

@@ -50,6 +50,12 @@ SIGNATURES = {
         [c_void_p, i64, C.c_double, C.c_double, C.c_double, C.c_uint64, i64, c_void_p, c_void_p, c_void_p, c_void_p,
          c_void_p],
     ),
+    'sgdml_b200_pimd_create': (C.c_int, [C.POINTER(c_void_p), c_void_p, i64, i64, c_void_p]),
+    'sgdml_b200_pimd_run': (
+        C.c_int,
+        [c_void_p, i64, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_uint64, i64, c_void_p,
+         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
     'sgdml_b200_model_set_R_d_desc': (C.c_int, [c_void_p, c_void_p]),
     'sgdml_b200_model_set_alphas': (C.c_int, [c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_predict_train': (C.c_int, [c_void_p, i64, i64, C.c_int, c_void_p, c_void_p, c_void_p]),

@@ -2558,6 +2558,7 @@ struct sgdml_b200_md {
   sgdml_b200_model* m = nullptr;
   int64_t n_rep = 0, chunk = 0;
   int dimi = 0;
+  int nb = 1;  // beads per ring polymer: replica p nb + j is bead j of polymer p (1 for sgdml_b200_md_create)
   sgdml_b200_model::WS ws;  // the handle's own predictor workspace: predict calls never touch it, MD never theirs
   int ws_oz = 0;            // the int8 slice count its buffers were sized for
   double *R = nullptr, *V = nullptr, *F = nullptr, *E = nullptr;  // state: (n_rep, 3N) x 3, (n_rep)
@@ -2565,15 +2566,19 @@ struct sgdml_b200_md {
   uint64_t* step = nullptr;             // (n_rep) step counters, all equal
   uint64_t step_host = 0;               // their value once the queued runs have finished
   bool has_state = false;
-  double *s = nullptr, *sigma = nullptr;  // (3N) inverse mass and noise scale per coordinate
+  double *s = nullptr, *sigma = nullptr;  // (3N) inverse mass, (nb, 3N) noise scale per mode and coordinate
   std::vector<double> s_host;             // s on the host
   MdParams* dP = nullptr;
   MdParams* hP = nullptr;     // pinned staging of dP and sigma, reused once the previous run's upload is done
   double* hSigma = nullptr;
+  PimdParams* dQ = nullptr;  // the ring-polymer run's parameter block
+  PimdParams* hQ = nullptr;
+  double *tab = nullptr, *hTab = nullptr;  // C (nb x nb) and the four mode tables (nb each)
   cudaEvent_t uploaded = nullptr;
   cudaStream_t gs = nullptr;  // capture stream
   cudaEvent_t ge = nullptr;
   cudaGraphExec_t exec = nullptr;
+  bool graph_pimd = false;    // the captured step runs k_pimd_step (sgdml_b200_pimd_run), not k_md_step
   uint64_t generation = 0;    // the model's generation at capture
   Lattice lat = {0, {0}, {0}};  // the model's cell at capture (passed to the descriptor kernel by value)
   int n_kernels = 0;
@@ -2591,7 +2596,11 @@ void md_free(sgdml_b200_md* md) {
   for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s, md->sigma}) cached_free(p);
   cached_free(md->step);
   cached_free(md->dP);
+  cached_free(md->dQ);
+  cached_free(md->tab);
   cudaFreeHost(md->hP);
+  cudaFreeHost(md->hQ);
+  cudaFreeHost(md->hTab);
   cudaFreeHost(md->hSigma);
   delete md;
 }
@@ -2624,8 +2633,17 @@ int md_forces(sgdml_b200_md* md, double* F, double* E, cudaStream_t s) {
   return 0;
 }
 
-int md_step(sgdml_b200_md* md, cudaStream_t s) {
-  SG_TRY(launch_md_step(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step, md->n_rep, md->dimi, 1, s));
+// the integrator of sgdml_b200_md_run or sgdml_b200_pimd_run; advance == 0 completes a run's last step
+int md_integrate(sgdml_b200_md* md, bool pimd, int advance, cudaStream_t s) {
+  if (pimd)
+    return launch_pimd_step(md->dQ, md->tab, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step,
+                            md->n_rep / md->nb, md->dimi, md->nb, advance, s);
+  return launch_md_step(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step, md->n_rep, md->dimi, advance,
+                        s);
+}
+
+int md_step(sgdml_b200_md* md, bool pimd, cudaStream_t s) {
+  SG_TRY(md_integrate(md, pimd, 1, s));
   return md_forces(md, md->F, md->E, s);
 }
 
@@ -2635,10 +2653,11 @@ bool same_cell(const Lattice& a, const Lattice& b) {
 }
 
 // the step graph, captured again whenever something it bakes in has changed: the workspace (md_ready), the model's
-// generation (use_ae, contraction slices) or the model's cell
-int md_graph(sgdml_b200_md* md, cudaStream_t s) {
+// generation (use_ae, contraction slices), the model's cell, or the integrator (classical or ring-polymer run)
+int md_graph(sgdml_b200_md* md, bool pimd, cudaStream_t s) {
   sgdml_b200_model* m = md->m;
-  if (md->exec != nullptr && md->generation == m->generation && same_cell(md->lat, m->lat)) return 0;
+  if (md->exec != nullptr && md->generation == m->generation && same_cell(md->lat, m->lat) && md->graph_pimd == pimd)
+    return 0;
   if (md->exec != nullptr) {
     cudaGraphExecDestroy(md->exec);
     md->exec = nullptr;
@@ -2661,7 +2680,7 @@ int md_graph(sgdml_b200_md* md, cudaStream_t s) {
   }
   cudaGraph_t graph = nullptr;
   SG_CUDA(cudaStreamBeginCapture(md->gs, cudaStreamCaptureModeThreadLocal));
-  const int rc = md_step(md, md->gs);
+  const int rc = md_step(md, pimd, md->gs);
   cudaError_t e = cudaStreamEndCapture(md->gs, &graph);
   if (rc != 0) {
     if (graph) cudaGraphDestroy(graph);
@@ -2679,6 +2698,7 @@ int md_graph(sgdml_b200_md* md, cudaStream_t s) {
   md->n_kernels = (int)(after - before);
   md->generation = m->generation;
   md->lat = m->lat;
+  md->graph_pimd = pimd;
   return 0;
 }
 
@@ -2704,6 +2724,31 @@ struct FrameOut {
     if (staged) cached_free(dev);
   }
 };
+
+// n_steps steps after the run's parameters are queued: graph replays or plain launches, then the completing launch
+// and the copy of host-staged frames
+int md_steps(sgdml_b200_md* md, bool pimd, int64_t n_steps, FrameOut* out, int n_out, cudaStream_t s) {
+  if (g_graph_enabled() && !profiling_enabled()) {
+    SG_TRY(md_graph(md, pimd, s));
+    for (int64_t k = 0; k < n_steps; ++k) {
+      SG_CUDA(cudaGraphLaunch(md->exec, s));
+      count_launch(KID_PREDICT_AUX, md->n_kernels);  // the kernels of a replay are launches too
+    }
+  } else {
+    for (int64_t k = 0; k < n_steps; ++k) SG_TRY(md_step(md, pimd, s));
+  }
+  md->step_host += (uint64_t)n_steps;
+  // the second half-kick of the last step (and its frame)
+  SG_TRY(md_integrate(md, pimd, 0, s));
+  bool sync = false;
+  for (int i = 0; i < n_out; ++i)
+    if (out[i].staged) {
+      SG_CUDA(cudaMemcpyAsync(out[i].user, out[i].dev, out[i].bytes, cudaMemcpyDeviceToHost, s));
+      sync = true;
+    }
+  if (sync) SG_CUDA(cudaStreamSynchronize(s));
+  return 0;
+}
 
 int md_run_impl(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, uint64_t seed, int64_t stride,
                 double* R_f, double* V_f, double* Ep_f, double* Ek_f, cudaStream_t s) {
@@ -2735,42 +2780,96 @@ int md_run_impl(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, dou
   SG_CUDA(cudaMemcpyAsync(md->dP, md->hP, sizeof(MdParams), cudaMemcpyHostToDevice, s));
   SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * md->dimi, cudaMemcpyHostToDevice, s));
   SG_CUDA(cudaEventRecord(md->uploaded, s));
-  if (g_graph_enabled() && !profiling_enabled()) {
-    SG_TRY(md_graph(md, s));
-    for (int64_t k = 0; k < n_steps; ++k) {
-      SG_CUDA(cudaGraphLaunch(md->exec, s));
-      count_launch(KID_PREDICT_AUX, md->n_kernels);  // the kernels of a replay are launches too
-    }
-  } else {
-    for (int64_t k = 0; k < n_steps; ++k) SG_TRY(md_step(md, s));
-  }
-  md->step_host += (uint64_t)n_steps;
-  // the second half-kick of the last step (and its frame)
-  SG_TRY(launch_md_step(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step, md->n_rep, md->dimi, 0, s));
-  bool sync = false;
-  for (auto& o : out)
-    if (o.staged) {
-      SG_CUDA(cudaMemcpyAsync(o.user, o.dev, o.bytes, cudaMemcpyDeviceToHost, s));
-      sync = true;
-    }
-  if (sync) SG_CUDA(cudaStreamSynchronize(s));
-  return 0;
+  return md_steps(md, false, n_steps, out, 4, s);
 }
 
-}  // namespace
+int pimd_run_impl(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma, double lambda,
+                  uint64_t seed, int64_t stride, double* R_f, double* V_f, double* Ep_f, double* Ek_f, double* Kp_f,
+                  double* Kcv_f, cudaStream_t s) {
+  const int nb = md->nb, dimi = md->dimi;
+  const int64_t n_poly = md->n_rep / nb;
+  const int64_t n_frames = stride > 0 ? n_steps / stride : 0;
+  const size_t fr = sizeof(double) * (size_t)(n_frames * md->n_rep);
+  const size_t fp = sizeof(double) * (size_t)(n_frames * n_poly);
+  FrameOut out[6];
+  if (n_frames > 0) {
+    SG_TRY(out[0].init(R_f, fr * dimi));
+    SG_TRY(out[1].init(V_f, fr * dimi));
+    SG_TRY(out[2].init(Ep_f, fr));
+    SG_TRY(out[3].init(Ek_f, fr));
+    SG_TRY(out[4].init(Kp_f, fp));
+    SG_TRY(out[5].init(Kcv_f, fp));
+  }
+  SG_TRY(md_ready(md));
+  // the run's constants, once on the host in double precision (tests/pimd_oracle.py restates them)
+  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous run has read the staging
+  PimdParams& p = *md->hQ;
+  const double h = 0.5 * dt;
+  const double kTP = nb * kT;
+  const double wP = kTP / hbar;
+  p.h = h;
+  p.key[0] = (uint32_t)seed;
+  p.key[1] = (uint32_t)(seed >> 32);
+  p.use_O = gamma > 0.0 || (lambda > 0.0 && nb > 1) ? 1 : 0;
+  p.stride = n_frames > 0 ? (int)stride : 0;
+  p.run_start = md->step_host;
+  p.kprim0 = 0.5 * (double)(dimi * nb) * kT;
+  p.kspring = 0.5 * wP * wP / nb;
+  p.kcv0 = 0.5 * dimi * kT;
+  p.kvir = 0.5 / nb;
+  p.R_f = out[0].dev;
+  p.V_f = out[1].dev;
+  p.Ep_f = out[2].dev;
+  p.Ek_f = out[3].dev;
+  p.Kp_f = out[4].dev;
+  p.Kcv_f = out[5].dev;
+  double* C = md->hTab;
+  double *m_cos = C + nb * nb, *m_sow = m_cos + nb, *m_msin = m_sow + nb, *m_c1 = m_msin + nb;
+  for (int j = 0; j < nb; ++j)
+    for (int k = 0; k < nb; ++k) {
+      double c;
+      if (k == 0)
+        c = std::sqrt(1.0 / nb);
+      else if (2 * k < nb)
+        c = std::sqrt(2.0 / nb) * std::cos(2.0 * M_PI * j * k / nb);
+      else if (2 * k == nb)
+        c = std::sqrt(1.0 / nb) * (j % 2 ? -1.0 : 1.0);
+      else
+        c = std::sqrt(2.0 / nb) * std::sin(2.0 * M_PI * j * k / nb);
+      C[j * nb + k] = c;
+    }
+  for (int k = 0; k < nb; ++k) {
+    double g = gamma;
+    m_cos[k] = 1.0;
+    m_sow[k] = h;
+    m_msin[k] = 0.0;
+    if (k > 0) {
+      const double wk = 2.0 * wP * std::sin(M_PI * k / nb);
+      m_cos[k] = std::cos(wk * h);
+      m_sow[k] = std::sin(wk * h) / wk;
+      m_msin[k] = -wk * std::sin(wk * h);
+      g = 2.0 * lambda * wk;
+    }
+    m_c1[k] = std::exp(-g * dt);
+    for (int i = 0; i < dimi; ++i)
+      md->hSigma[(size_t)k * dimi + i] = std::sqrt((1.0 - m_c1[k] * m_c1[k]) * kTP * md->s_host[(size_t)i]);
+  }
+  SG_CUDA(cudaMemcpyAsync(md->dQ, md->hQ, sizeof(PimdParams), cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaMemcpyAsync(md->tab, md->hTab, sizeof(double) * (nb * nb + 4 * nb), cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * nb * dimi, cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaEventRecord(md->uploaded, s));
+  return md_steps(md, true, n_steps, out, 6, s);
+}
 
-extern "C" {
-
-int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, const double* inv_mass) {
-  SG_TRY(require_device());
-  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
-  SG_ARG(n_rep >= 1 && n_rep <= INT32_MAX);
+// a handle of n_rep = n_poly nb replicas; the caller has checked the counts
+int md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, int nb, const double* inv_mass) {
   SG_ARG(!is_device_ptr(inv_mass));
   for (int i = 0; i < m->N; ++i)
     if (!(std::isfinite(inv_mass[i]) && inv_mass[i] > 0.0)) return fail_arg("inv_mass must be finite and > 0");
   sgdml_b200_md* md = new sgdml_b200_md();
   md->m = m;
   md->n_rep = n_rep;
+  md->nb = nb;
   md->dimi = 3 * m->N;
   md->chunk = std::min<int64_t>(chunk_geos(m), n_rep);
   md->ws_oz = m->oz_s;
@@ -2781,10 +2880,14 @@ int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep
     SG_CUDA(cached_malloc(&md->Es, sizeof(double) * n_rep));
     SG_CUDA(cached_malloc(&md->step, sizeof(uint64_t) * n_rep));
     SG_CUDA(cached_malloc(&md->s, sizeof(double) * md->dimi));
-    SG_CUDA(cached_malloc(&md->sigma, sizeof(double) * md->dimi));
+    SG_CUDA(cached_malloc(&md->sigma, sizeof(double) * nb * md->dimi));
     SG_CUDA(cached_malloc(&md->dP, sizeof(MdParams)));
+    SG_CUDA(cached_malloc(&md->dQ, sizeof(PimdParams)));
+    SG_CUDA(cached_malloc(&md->tab, sizeof(double) * (nb * nb + 4 * nb)));
     SG_CUDA(cudaMallocHost(&md->hP, sizeof(MdParams)));
-    SG_CUDA(cudaMallocHost(&md->hSigma, sizeof(double) * md->dimi));
+    SG_CUDA(cudaMallocHost(&md->hQ, sizeof(PimdParams)));
+    SG_CUDA(cudaMallocHost(&md->hTab, sizeof(double) * (nb * nb + 4 * nb)));
+    SG_CUDA(cudaMallocHost(&md->hSigma, sizeof(double) * nb * md->dimi));
     SG_CUDA(cudaEventCreateWithFlags(&md->uploaded, cudaEventDisableTiming));
     md->s_host.resize((size_t)md->dimi);
     for (int i = 0; i < md->dimi; ++i) md->s_host[(size_t)i] = inv_mass[i / 3];
@@ -2799,6 +2902,26 @@ int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep
   }
   *out = md;
   return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, const double* inv_mass) {
+  SG_TRY(require_device());
+  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
+  SG_ARG(n_rep >= 1 && n_rep <= INT32_MAX);
+  return md_create(out, m, n_rep, 1, inv_mass);
+}
+
+int sgdml_b200_pimd_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_poly, int64_t n_beads,
+                           const double* inv_mass) {
+  SG_TRY(require_device());
+  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
+  SG_ARG(n_beads >= 1 && n_beads <= PIMD_MAX_BEADS);
+  SG_ARG(n_poly >= 1 && n_poly <= INT32_MAX / n_beads);
+  return md_create(out, m, n_poly * n_beads, (int)n_beads, inv_mass);
 }
 
 int sgdml_b200_md_destroy(sgdml_b200_md* md) {
@@ -2854,6 +2977,7 @@ int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamm
                       void* stream) {
   SG_TRY(require_device());
   SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
+  if (md->nb > 1) return fail_arg("sgdml_b200_md_run: a ring-polymer handle (n_beads > 1) runs with sgdml_b200_pimd_run");
   SG_ARG(std::isfinite(dt) && dt > 0.0);
   SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
   SG_ARG(std::isfinite(kT) && kT >= 0.0);
@@ -2863,6 +2987,27 @@ int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamm
   if (n_steps == 0) return 0;
   return md_run_impl(md, n_steps, dt, gamma, kT, seed, stride, R_frames, V_frames, E_pot_frames, E_kin_frames,
                      (cudaStream_t)stream);
+}
+
+int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma,
+                        double lambda, uint64_t seed, int64_t stride, double* R_frames, double* V_frames,
+                        double* E_pot_frames, double* E_kin_frames, double* K_prim_frames, double* K_cv_frames,
+                        void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
+  SG_ARG(std::isfinite(dt) && dt > 0.0);
+  SG_ARG(std::isfinite(kT) && kT >= 0.0);
+  SG_ARG(std::isfinite(hbar) && hbar > 0.0);
+  SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
+  SG_ARG(std::isfinite(lambda) && lambda >= 0.0);
+  if (md->nb > 1 && kT == 0.0) return fail_arg("a ring polymer (n_beads > 1) needs kT > 0");
+  if (md->nb == 1 && kT > 0.0 && gamma == 0.0)
+    return fail_arg("kT > 0 needs a friction gamma > 0 (a thermostat without coupling)");
+  if (stride > 0 && n_steps % stride != 0) return fail_arg("n_steps must be a multiple of stride");
+  if (!md->has_state) return fail_arg("sgdml_b200_pimd_run: no state yet (call sgdml_b200_md_set_state)");
+  if (n_steps == 0) return 0;
+  return pimd_run_impl(md, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, R_frames, V_frames, E_pot_frames,
+                       E_kin_frames, K_prim_frames, K_cv_frames, (cudaStream_t)stream);
 }
 
 }  // extern "C"

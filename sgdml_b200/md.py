@@ -1,6 +1,8 @@
 """``GDMLDynamics`` -- molecular dynamics of many replicas on the device (``sgdml_b200_md_*`` in
 include/sgdml_b200.h): velocity-Verlet (NVE) and BAOAB Langevin (NVT) trajectories, many steps per call, with
-positions, velocities and forces kept in GPU memory between steps.
+positions, velocities and forces kept in GPU memory between steps.  ``GDMLPathIntegralDynamics`` -- path-integral MD
+of ring polymers on the same engine (``sgdml_b200_pimd_*``): PILE-L thermostatted (or NVE) ring-polymer trajectories
+with the primitive and centroid-virial quantum kinetic-energy estimators.
 
 Units follow ASE and ``intf.ase_calc.SGDMLCalculator``: positions in Angstrom, velocities in Angstrom/fs, masses in
 amu, energies in eV, time in fs, temperature in K.  ``E_to_eV`` and ``F_to_eV_Ang`` convert the model's units as in
@@ -22,6 +24,8 @@ _AMU = 1.660539040e-27  # kg
 _K_B = 1.38064852e-23  # J / K
 FS = 1e-15 * 1e10 * np.sqrt(_E_CHARGE / _AMU)  # ase.units.fs: 1 fs in ASE's time unit Angstrom sqrt(amu / eV)
 KB_EV = _K_B / _E_CHARGE  # ase.units.kB: eV / K
+_HBAR = 1.054571800e-34  # J s
+HBAR_EV_FS = _HBAR / _E_CHARGE * 1e15  # eV fs (0.6582119514)
 
 
 class GDMLDynamics(object):
@@ -56,13 +60,16 @@ class GDMLDynamics(object):
         # a = F inv_mass in model length per fs^2, F in the model's force unit
         self.inv_mass = self.F_to_eV_Ang * self.Ang_to_R * FS**2 / masses
         self._torch_device = None
+        self._handle = self._create_handle()
+
+    def _create_handle(self):
         handle = ctypes.c_void_p()
         _lib.check(
             _lib.lib().sgdml_b200_md_create(ctypes.byref(handle), self.gdml_predict._handle, self.n_replicas,
                                             _lib.ptr(self.inv_mass)),
             'md_create',
         )
-        self._handle = handle
+        return handle
 
     def __del__(self):
         h = getattr(self, '_handle', None)
@@ -158,3 +165,97 @@ class GDMLDynamics(object):
         return {'positions': (f['R'] / self.Ang_to_R).reshape(nf, -1, N, 3),
                 'velocities': (f['V'] / self.Ang_to_R).reshape(nf, -1, N, 3),
                 'potential_energy': f['E_pot'] * self.E_to_eV, 'kinetic_energy': f['E_kin'] * self.E_to_eV}
+
+
+class GDMLPathIntegralDynamics(GDMLDynamics):
+    """Path-integral MD of `n_polymers` ring polymers of `n_beads` beads (1 to 64) each, in the units of
+    ``GDMLDynamics``.  Bead j of polymer p is replica p n_beads + j of the engine's handle.
+
+    ``set_state(positions, velocities=None, step=0)``: positions (n_polymers, n_beads, N, 3), or (n_polymers, N, 3) /
+    (N, 3) copied to every bead (and polymer); velocities likewise (None: at rest).
+    ``run(n_steps, dt_fs, temperature_K, centroid_friction_per_fs=0, pile_lambda=1, seed=0, stride=0)`` integrates
+    with the PILE-L thermostat (the centroid mode at the given friction, internal mode k at 2 pile_lambda omega_k:
+    pile_lambda = 1 damps every internal mode critically, 0.5 with zero centroid friction is thermostatted RPMD, zero
+    for both is NVE RPMD) and returns the frames after every `stride`-th step: {'positions', 'velocities':
+    (n_frames, n_polymers, n_beads, N, 3), 'potential_energy': (n_frames, n_polymers, n_beads),
+    'kinetic_energy_primitive', 'kinetic_energy_virial': (n_frames, n_polymers)} in Angstrom, Angstrom/fs and eV (the
+    kinetic energies are the quantum estimators of the whole molecule; stride 0: an empty dict).  A ring polymer
+    needs a temperature > 0; with one bead ``run`` is ``GDMLDynamics.run`` bit for bit."""
+
+    def __init__(self, model, masses, n_beads, n_polymers=1, E_to_eV=_KCAL_PER_MOL_IN_EV,
+                 F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        self.n_beads = int(n_beads)
+        self.n_polymers = int(n_polymers)
+        super().__init__(model, masses, self.n_polymers * self.n_beads, E_to_eV, F_to_eV_Ang)
+
+    def _create_handle(self):
+        handle = ctypes.c_void_p()
+        _lib.check(
+            _lib.lib().sgdml_b200_pimd_create(ctypes.byref(handle), self.gdml_predict._handle, self.n_polymers,
+                                              self.n_beads, _lib.ptr(self.inv_mass)),
+            'pimd_create',
+        )
+        return handle
+
+    def _beads(self, x, name):
+        """(n_polymers, n_beads, N, 3), (n_polymers, N, 3) or (N, 3) -> (n_polymers n_beads, 3N)."""
+        N, n_p, P = self.n_atoms, self.n_polymers, self.n_beads
+        shape = tuple(x.shape)
+        if shape == (n_p, P, N, 3):
+            return x
+        if shape == (n_p, N, 3) or shape == (N, 3):
+            x = x.reshape(-1, 1, N, 3)
+            if hasattr(x, 'data_ptr'):
+                return x.expand(n_p, P, N, 3).contiguous()
+            return np.ascontiguousarray(np.broadcast_to(np.asarray(x, dtype=np.float64), (n_p, P, N, 3)))
+        raise ValueError('%s must be (n_polymers, n_beads, N, 3), (n_polymers, N, 3) or (N, 3) = (%d, %d, %d, 3): %s'
+                         % (name, n_p, P, N, shape))
+
+    # ------------------------------------------------------------------ model units (L, model energy, fs)
+    def _run_raw(self, n_steps, dt, kT, hbar, gamma=0.0, lam=0.0, seed=0, stride=0,
+                 frames=('R', 'V', 'E_pot', 'E_kin', 'K_prim', 'K_cv')):
+        n_steps, stride = int(n_steps), int(stride)
+        n_frames = n_steps // stride if stride > 0 and n_steps % stride == 0 else 0
+        B, dimi = self.n_replicas, 3 * self.n_atoms
+        shape = {'R': (n_frames, B, dimi), 'V': (n_frames, B, dimi), 'E_pot': (n_frames, B), 'E_kin': (n_frames, B),
+                 'K_prim': (n_frames, self.n_polymers), 'K_cv': (n_frames, self.n_polymers)}
+        out = {k: self._empty(shape[k]) for k in frames} if n_frames > 0 else {}
+        _lib.check(
+            _lib.lib().sgdml_b200_pimd_run(self._handle, n_steps, float(dt), float(kT), float(hbar), float(gamma),
+                                           float(lam), int(seed), stride,
+                                           *(_lib.ptr(out.get(k)) for k in ('R', 'V', 'E_pot', 'E_kin', 'K_prim',
+                                                                           'K_cv')),
+                                           _lib.current_stream()),
+            'pimd_run',
+        )
+        return out
+
+    # ------------------------------------------------------------------ ASE units
+    def set_state(self, positions, velocities=None, step=0):
+        positions = self._beads(positions, 'positions')
+        velocities = None if velocities is None else self._beads(velocities, 'velocities')
+        super().set_state(positions, velocities, step)
+
+    def get_state(self):
+        """{'positions', 'velocities', 'forces' (n_polymers, n_beads, N, 3), 'potential_energy' (n_polymers, n_beads),
+        'step'}: Angstrom, Angstrom/fs, eV/Angstrom, eV."""
+        st = super().get_state()
+        shape = (self.n_polymers, self.n_beads)
+        for k in ('positions', 'velocities', 'forces'):
+            st[k] = st[k].reshape(shape + (self.n_atoms, 3))
+        st['potential_energy'] = st['potential_energy'].reshape(shape)
+        return st
+
+    def run(self, n_steps, dt_fs, temperature_K, centroid_friction_per_fs=0.0, pile_lambda=1.0, seed=0, stride=0):
+        kT = KB_EV * float(temperature_K) / self.E_to_eV
+        hbar = HBAR_EV_FS / self.E_to_eV
+        f = self._run_raw(n_steps, dt_fs, kT, hbar, centroid_friction_per_fs, pile_lambda, seed, stride,
+                          frames=('R', 'V', 'E_pot', 'K_prim', 'K_cv'))
+        if not f:
+            return {}
+        N, nf, n_p, P = self.n_atoms, f['R'].shape[0], self.n_polymers, self.n_beads
+        return {'positions': (f['R'] / self.Ang_to_R).reshape(nf, n_p, P, N, 3),
+                'velocities': (f['V'] / self.Ang_to_R).reshape(nf, n_p, P, N, 3),
+                'potential_energy': (f['E_pot'] * self.E_to_eV).reshape(nf, n_p, P),
+                'kinetic_energy_primitive': f['K_prim'] * self.E_to_eV,
+                'kinetic_energy_virial': f['K_cv'] * self.E_to_eV}

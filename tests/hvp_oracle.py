@@ -125,9 +125,15 @@ def central_diff_hvp(f_of_R, R, V, h=1e-5):
     return (f_of_R(R + h * V) - f_of_R(R - h * V)) / (2 * h)
 
 
-def gemm_form_hvp(model, R, V, lat_and_inv='model', guard=True):
+DEFECTS = ('dJ', 'csT', 'ae_dc2', 'pinv_fold')
+
+
+def gemm_form_hvp(model, R, V, lat_and_inv='model', guard=True, defect=None, floor_scale=1.0):
     """The engine's HVP in NumPy, R, V (B, 3N) -> HV (B, 3N).  guard=False drops the floor under n in a ds / n and
-    clamps x5 at 1e-300 as the forward does."""
+    clamps x5 at 1e-300 as the forward does.  defect (for showing that a check fails; one of DEFECTS): 'dJ' drops the
+    (dJ)^T F_desc term of k_hvp_project, 'csT' the (sum c1) T term of dG, 'ae_dc2' leaves ae dc2 out of dc1,
+    'pinv_fold' folds the permutations with pinv instead of perm; floor_scale multiplies the floor."""
+    assert defect is None or defect in DEFECTS, defect
     R = np.asarray(R, dtype=np.float64).reshape(-1, np.asarray(model['z']).shape[0] * 3)
     V = np.asarray(V, dtype=np.float64).reshape(R.shape)
     N = R.shape[1] // 3
@@ -166,23 +172,25 @@ def gemm_form_hvp(model, R, V, lat_and_inv='model', guard=True):
         c2 = k_base * e * (n + sig)
         c1 = k_c1 * e * a
         ds = qt - S3
-        floor = X5_FLOOR * (qq + mm) if guard else 0.0
+        floor = X5_FLOOR * floor_scale * (qq + mm) if guard else 0.0
         nf = np.sqrt(np.maximum(x5, np.maximum(floor, 1e-300)))
         dc2 = -5.0 * k_base * e * ds / sig
         dc1 = k_c1 * e * (S4 - 5.0 * a * ds / (nf * sig))
         if ae is not None:
             c1 = c1 + ae * c2
-            dc1 = dc1 + ae * dc2
+            if defect != 'ae_dc2':
+                dc1 = dc1 + ae * dc2
         cs = c1.sum(1)[:, None]
         G = cs * Q - c1 @ Xc - c2 @ JA
-        dG = dc1.sum(1)[:, None] * Q + cs * T - dc1 @ Xc - dc2 @ JA
-        Fd = sum(G[p][perm[p]] for p in range(S))
-        dFd = sum(dG[p][perm[p]] for p in range(S))
+        dG = dc1.sum(1)[:, None] * Q + (0.0 if defect == 'csT' else cs * T) - dc1 @ Xc - dc2 @ JA
+        fold = pinv if defect == 'pinv_fold' else perm
+        Fd = sum(G[p][fold[p]] for p in range(S))
+        dFd = sum(dG[p][fold[p]] for p in range(S))
         g = gq[i]
         v = V[i].reshape(N, 3)
         dd = v[a_idx] - v[b_idx]
         gn = np.sqrt((g * g).sum(1))[:, None]
         dg = gn**1.5 * dd - 3.0 * (g * dd).sum(1)[:, None] * g / np.sqrt(gn)
-        h = g * dFd[:, None] + dg * Fd[:, None]
+        h = g * dFd[:, None] + (0.0 if defect == 'dJ' else dg * Fd[:, None])
         out[i] = std * (P.T @ h).ravel()
     return out

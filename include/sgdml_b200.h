@@ -496,11 +496,26 @@ int sgdml_b200_gemm_nt_args(int64_t m, int64_t n, int64_t k, double alpha, const
  * cores -- A and B are cut into n_slices signed 7-bit slices per row-scaled entry and every slice pair is
  * multiplied exactly by wgmma s8 (int32 accumulators in registers); C += alpha * A * B^T.
  * n_slices = 7 reproduces the FP64 Cholesky trailing update (analytic.py:94-96) to ~1e-14 relative, 8 would
- * be FP64-equivalent (tools/ozaki_study.py).  tri != 0: m == n, only tiles touching the lower triangle.
- * All pointers must be device pointers; k <= 16384. */
+ * be FP64-equivalent (tools/ozaki_study.py).  n_slices must be 2..7.
+ *   k <= 16384: the int32 level sums (at most 64^2 k n_slices) stay exact.  k = 16385 is an argument error.
+ *   Each row x of A and of B is x = 2^e sum_p q_p 2^(-7 p), e = frexp(max |x|) + 1, q_p = rint of the remainder scaled
+ *         by 2^7, p = 1..n_slices; the pairs with p + q <= n_slices + 1 are summed level by level, smallest level
+ *         first, in FP64, and the update is ldexp(alpha * sum, e_A + e_B) (tests/ozaki_model.py states it bit for bit).
+ *   Non-finite operands: every entry of C whose row of A or row of B holds a NaN or an infinity becomes NaN.
+ *   tri != 0 (needs m == n): the kernel computes 128 x 32 tiles of C and writes every entry of each tile (tm, tn) with
+ *         32 tn <= 128 tm + 127, entries above the diagonal included; every other entry of C keeps its bits.
+ * All pointers must be device pointers. */
 int sgdml_b200_ozaki_gemm_nt(int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,
                              const double* B, int64_t ldb, double* C, int64_t ldc, int n_slices, int tri,
                              void* stream);
+/* Test hook: the int8-slice GEMM launched exactly as its callers launch it, which sgdml_b200_ozaki_gemm_nt cannot reach.
+ * Each operand is split once (once in all when A == B, m == n and lda == ldb, as potrf's symmetric update does), then
+ * one launch: overwrite 0: C += alpha A B^T;  overwrite 1: C = alpha A B^T, the old C is not read (the large-descriptor
+ * predictor's first write of S1, S2 and G).  tri and overwrite must be 0 or 1; otherwise the arguments and their
+ * rejections are those of sgdml_b200_ozaki_gemm_nt.  Device pointers only; the call synchronises the stream. */
+int sgdml_b200_ozaki_gemm_args(int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,
+                               const double* B, int64_t ldb, double* C, int64_t ldc, int n_slices, int tri,
+                               int overwrite, void* stream);
 /* Bring-up aid for the above: also returns the int8 slice planes ([n_slices][rows padded to 128][k padded to
  * 128]), the row exponents and the raw int32 level sums ([n_slices][m][n]); any output may be NULL. */
 int sgdml_b200_ozaki_debug(int64_t m, int64_t n, int64_t k, const double* A, int64_t lda, const double* B,

@@ -95,6 +95,10 @@ SIGNATURES = {
         C.c_int,
         [i64, i64, i64, C.c_double, c_void_p, i64, c_void_p, i64, c_void_p, i64, C.c_int, C.c_int, c_void_p],
     ),
+    'sgdml_b200_ozaki_gemm_args': (
+        C.c_int,
+        [i64, i64, i64, C.c_double, c_void_p, i64, c_void_p, i64, c_void_p, i64, C.c_int, C.c_int, C.c_int, c_void_p],
+    ),
     'sgdml_b200_ozaki_debug': (
         C.c_int,
         [i64, i64, i64, c_void_p, i64, c_void_p, i64, c_void_p, i64, C.c_int, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -28,6 +28,8 @@
 //            the concurrently running CTAs read (2 x 1024 rows) stay L2-resident while they are reused
 #include <cuda.h>
 
+#include <cfloat>
+
 #include "common.cuh"
 #include "solve.cuh"
 
@@ -49,9 +51,19 @@ constexpr int OZ_GSM = 8, OZ_GSN = 32;                     // super-tile: 8 x 32
 
 // ---------------------------------------------------------------- splitting kernels
 // Row exponent + S rounds of (scale by 2^7, round to nearest, subtract): x = 2^e sum_p q_p 2^(-7p), |q_p| <= 64.
+// A row that holds a NaN or an infinity gets the exponent OZ_EXP_NONFINITE and all-zero slices; the epilogue writes NaN
+// to every entry of C in its row (A) or column (B).  fmax skips NaN, so without the mark such a row would be sliced as if
+// the entry were zero (and an infinity would leave the row's other slices out of int8 range).
+constexpr int OZ_EXP_NONFINITE = 1 << 20;
 __device__ __forceinline__ int oz_row_exponent(const double* __restrict__ x, int64_t k, int lane) {
   double amax = 0.0;
-  for (int64_t j = lane; j < k; j += 32) amax = fmax(amax, fabs(x[j]));
+  bool finite = true;
+  for (int64_t j = lane; j < k; j += 32) {
+    const double a = fabs(x[j]);
+    amax = fmax(amax, a);
+    finite = finite && a <= DBL_MAX;  // false for NaN and infinities
+  }
+  if (!__all_sync(0xffffffffu, finite)) return OZ_EXP_NONFINITE;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) amax = fmax(amax, __shfl_xor_sync(0xffffffffu, amax, o));
   int e = 0;
@@ -79,7 +91,7 @@ __global__ void __launch_bounds__(256) k_ozaki_split(const double* __restrict__ 
   const int e = oz_row_exponent(x, k, lane);
   if (lane == 0) exps[r] = e;
   for (int64_t j = lane; j < kp; j += 32) {
-    double v = (j < k) ? ldexp(x[j], -e) : 0.0;
+    double v = (j < k && e != OZ_EXP_NONFINITE) ? ldexp(x[j], -e) : 0.0;
     for (int p = 0; p < S; ++p) {
       v *= (double)(1 << OZ_BITS);
       const double q = rint(v);  // |q| <= 64, remainder in [-1/2, 1/2]
@@ -107,11 +119,16 @@ __global__ void __launch_bounds__(256) k_ozaki_split_sw(const double* __restrict
   const double* x = X + r * ldx;
   if (r < rows) e = oz_row_exponent(x, k, lane);
   if (lane == 0) exps[r] = e;
-  const double sc = ldexp(1.0, -e);  // exact power of two
+  const bool live = r < rows && e != OZ_EXP_NONFINITE;
+  // x 2^-e, rounded once (= ldexp(x, -e)): 2^-e is a double for e >= -1023 (2^-1025 is subnormal but exact); below that,
+  // for rows whose largest entry is under 2^-1025, scale in two exact steps through 2^512
+  const bool tiny = e < -1021;
+  const double pre = tiny ? 0x1p512 : 1.0;
+  const double sc = ldexp(1.0, tiny ? -e - 512 : -e);  // exact power of two
   for (int64_t j0 = (int64_t)lane * 4; j0 < kp; j0 += 128) {
     double v[4];
 #pragma unroll
-    for (int t = 0; t < 4; ++t) v[t] = (r < rows && j0 + t < k) ? x[j0 + t] * sc : 0.0;
+    for (int t = 0; t < 4; ++t) v[t] = (live && j0 + t < k) ? x[j0 + t] * pre * sc : 0.0;
     const int64_t kb = j0 / OZ_BK;
     const int jj = (int)(j0 - kb * OZ_BK);  // byte within the 64-byte row: chunk jj/16, offset jj%16 (multiple of 4)
     const int off = rin * OZ_BK + (((jj >> 4) ^ sw) << 4) + (jj & 15);
@@ -373,14 +390,25 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) k_ozaki_gemm(const OzArgs p, in
     for (int h = 0; h < 2; ++h) {
       const int64_t r = r0 + 8 * h;
       if (r >= p.m) continue;
-      const double row_scale = p.alpha * ldexp(1.0, p.ea[r]);
+      const int ea = p.ea[r];
       double* crow = p.C + r * p.ldc;
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         if (((i >> 1) & 1) != h) continue;
         const int64_t c = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
         if (c >= p.n) continue;
-        const double upd = v[i] * row_scale * ldexp(1.0, p.eb[c]);
+        const int eb = p.eb[c];
+        // one scaling by 2^(ea + eb), = ldexp(alpha v, ea + eb): 2^ea alone is infinite for a row whose largest entry
+        // is >= 2^1023 (ea = 1025).  In the normal range the power of two is built from its bits (one rounding either way).
+        const int es = ea + eb;
+        const double av = p.alpha * v[i];
+        double upd;
+        if (ea == OZ_EXP_NONFINITE || eb == OZ_EXP_NONFINITE)
+          upd = __longlong_as_double(0x7ff8000000000000ll);
+        else if (es >= -1022 && es <= 1023)
+          upd = av * __longlong_as_double((long long)(es + 1023) << 52);
+        else
+          upd = ldexp(av, es);
         crow[c] = p.overwrite ? upd : crow[c] + upd;
       }
     }
@@ -506,7 +534,7 @@ int ozaki_syrk_device(int64_t n, int64_t k, double alpha, const double* X, int64
 // Self-contained form (allocates and frees its slice planes, synchronises the stream): tests and the
 // predictor experiment; the Cholesky uses ozaki_syrk_device.
 int ozaki_gemm_nt_device(int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda, const double* B,
-                         int64_t ldb, double* C, int64_t ldc, int S, int tri, cudaStream_t s) {
+                         int64_t ldb, double* C, int64_t ldc, int S, int tri, int overwrite, cudaStream_t s) {
   SG_ARG(S >= 2 && S <= OZ_MAX_S && m >= 1 && n >= 1 && k >= 1);
   SG_ARG(k <= (1 << 14));  // int32 accumulation stays exact: 64^2 * k * S < 2^31
   const bool same = (A == B && m == n && lda == ldb);
@@ -530,7 +558,7 @@ int ozaki_gemm_nt_device(int64_t m, int64_t n, int64_t k, double alpha, const do
       SG_CUDA(cudaMalloc(&xb, sizeof(int) * (size_t)((n + OZ_BM - 1) / OZ_BM * OZ_BM)));
       SG_TRY(oz_split_into(B, n, k, ldb, S, pb, xb, &ob, s));
     }
-    SG_TRY(oz_launch(oa, ob, m, n, alpha, C, ldc, S, tri, s));
+    SG_TRY(oz_launch(oa, ob, m, n, alpha, C, ldc, S, tri, s, nullptr, overwrite));
     SG_CUDA(cudaStreamSynchronize(s));  // the planes are freed below
     return 0;
   };
@@ -605,5 +633,15 @@ extern "C" int sgdml_b200_ozaki_gemm_nt(int64_t m, int64_t n, int64_t k, double 
   SG_ARG(A != nullptr && B != nullptr && C != nullptr && lda >= k && ldb >= k && ldc >= n);
   SG_ARG(is_device_ptr(A) && is_device_ptr(B) && is_device_ptr(C));
   if (tri) SG_ARG(m == n);
-  return ozaki_gemm_nt_device(m, n, k, alpha, A, lda, B, ldb, C, ldc, n_slices, tri, (cudaStream_t)stream);
+  return ozaki_gemm_nt_device(m, n, k, alpha, A, lda, B, ldb, C, ldc, n_slices, tri, 0, (cudaStream_t)stream);
+}
+
+extern "C" int sgdml_b200_ozaki_gemm_args(int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,
+                                          const double* B, int64_t ldb, double* C, int64_t ldc, int n_slices, int tri,
+                                          int overwrite, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(A != nullptr && B != nullptr && C != nullptr && lda >= k && ldb >= k && ldc >= n);
+  SG_ARG((tri == 0 || tri == 1) && (tri == 0 || m == n) && (overwrite == 0 || overwrite == 1));
+  SG_ARG(is_device_ptr(A) && is_device_ptr(B) && is_device_ptr(C));
+  return ozaki_gemm_nt_device(m, n, k, alpha, A, lda, B, ldb, C, ldc, n_slices, tri, overwrite, (cudaStream_t)stream);
 }

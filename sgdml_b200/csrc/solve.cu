@@ -845,14 +845,18 @@ __global__ void __launch_bounds__(256) k_dmma_peak(double* out, int iters, doubl
 constexpr int NBO_MAX = 1024;
 
 // Slice count of the lazy trailing updates (csrc/ozaki.cu): -1 = automatic, 0 = FP64 DMMA, 2..7 = int8 slices on the
-// wgmma tensor cores.  Automatic: SGDML_B200_OZAKI_SLICES if set, otherwise FP64.  Measured on an H100 SXM at a 400 W
+// wgmma tensor cores.  Automatic: SGDML_B200_OZAKI_SLICES if set (values below 2 mean FP64, as for
+// SGDML_B200_OZAKI_PREDICT_SLICES), otherwise FP64.  Measured on an H100 SXM at a 400 W
 // power limit (BASELINE config 2, n = 63 000): solve 3.46 s with FP64 DMMA trailing updates, 3.65 s with 7 int8 slices
 // (at a 700 W limit: 2.84 s against 2.88 s) -- the FP64 path is both faster and exact there.
 static int g_solve_slices = -1;
 static int resolve_slices() {
   if (g_solve_slices >= 0) return g_solve_slices;
   const char* oz = getenv("SGDML_B200_OZAKI_SLICES");
-  if (oz != nullptr) return std::max(0, std::min(7, atoi(oz)));
+  if (oz != nullptr) {
+    const int v = atoi(oz);
+    return v >= 2 ? std::min(7, v) : 0;
+  }
   return 0;
 }
 

@@ -49,9 +49,10 @@ int ozaki_split(const double* X, int64_t rows, int64_t k, int64_t ldx, int n_sli
 int ozaki_gemm(const OzOperand& a, const OzOperand& b, int64_t m, int64_t n, double alpha, int overwrite, double* C,
                int64_t ldc, int n_slices, cudaStream_t s);
 
-// csrc/ozaki.cu: C += alpha A B^T through n_slices int8 slices per operand on the int8 tensor cores (wgmma)
+// csrc/ozaki.cu: C += alpha A B^T (overwrite: C = alpha A B^T) through n_slices int8 slices per operand on the int8
+// tensor cores (wgmma)
 int ozaki_gemm_nt_device(int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda, const double* B,
-                         int64_t ldb, double* C, int64_t ldc, int n_slices, int tri, cudaStream_t s);
+                         int64_t ldb, double* C, int64_t ldc, int n_slices, int tri, int overwrite, cudaStream_t s);
 int ozaki_syrk_workspace_bytes(int64_t max_rows, int64_t max_k, int n_slices, size_t* plane_bytes, size_t* exp_bytes);
 int ozaki_syrk_device(int64_t n, int64_t k, double alpha, const double* X, int64_t ldx, double* C, int64_t ldc,
                       int n_slices, int8_t* planes, int* exps, cudaStream_t s);

@@ -153,6 +153,14 @@ __device__ __forceinline__ double exp_neg(double t) {
 
 struct MaternK {
   double sig, sig_inv, k_base, k_c1;  // k_c1 = k_base * 5/sig
+  static MaternK from_sig(double sig) {
+    MaternK k;
+    k.sig = sig;
+    k.sig_inv = 1.0 / sig;
+    k.k_base = 5.0 / (3.0 * sig * sig * sig);  // predict.py:195 mat52_base_fact
+    k.k_c1 = k.k_base * 5.0 / sig;              // ... times predict.py:196 diag_scale_fact
+    return k;
+  }
 };
 // x5 = 5 (|q|^2 + |x|^2 - 2 q.x) (may be slightly negative), a = delta . JA  ->  c1, c2
 // (predict.py:204-213):  n = sqrt(x5) = sqrt5 |delta|, base = exp(-n/sig) 5/(3 sig^3),
@@ -589,33 +597,35 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
 }
 
 // ============================================================== query rows
-// One warp per virtual row (b, p): Qg[row][e] = x_b[pinv_p[e]] - mu[e] (zero beyond D and beyond the
-// last real row, so that every main-kernel tile is one contiguous bulk copy) and qq[row] = |Qg[row]|^2.
-__global__ void __launch_bounds__(256) k_query_rows(const double* __restrict__ xq, const int* __restrict__ pinv,
-                                                    const double* __restrict__ mu, int D, int DS, int S,
-                                                    int64_t n_rows, int64_t n_rows_pad, double* __restrict__ Qg,
-                                                    double* __restrict__ qqg) {
+// One warp writes virtual row `row` of the query descriptor x under the permutation pi: Qg[row][e] = x[pi[e]] - mu[e]
+// (zero beyond D, and the whole row for x == nullptr: the padding rows beyond the last real row, so that every
+// main-kernel tile is one contiguous bulk copy) and qq[row] = |Qg[row]|^2.
+__device__ __forceinline__ void query_row(const double* __restrict__ x, const int* __restrict__ pi,
+                                          const double* __restrict__ mu, int D, int DS, int64_t row,
+                                          double* __restrict__ Qg, double* __restrict__ qqg) {
   const int lane = threadIdx.x & 31;
-  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= n_rows_pad) return;
   double s = 0.0;
-  if (row < n_rows) {
-    const int64_t b = row / S;
-    const int pp = (int)(row - b * S);
-    const double* x = xq + b * D;
-    const int* pi = pinv + pp * D;
-    for (int e = lane; e < DS; e += 32) {
-      double v = 0.0;
-      if (e < D) v = x[pi[e]] - mu[e];
-      Qg[row * DS + e] = v;
-      s = fma(v, v, s);
-    }
-  } else {
-    for (int e = lane; e < DS; e += 32) Qg[row * DS + e] = 0.0;
+  for (int e = lane; e < DS; e += 32) {
+    double v = 0.0;
+    if (x != nullptr && e < D) v = x[pi[e]] - mu[e];
+    Qg[row * DS + e] = v;
+    s = fma(v, v, s);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if (lane == 0) qqg[row] = s;
+}
+
+// One warp per virtual row (b, p) of the queries xq
+__global__ void __launch_bounds__(256) k_query_rows(const double* __restrict__ xq, const int* __restrict__ pinv,
+                                                    const double* __restrict__ mu, int D, int DS, int S,
+                                                    int64_t n_rows, int64_t n_rows_pad, double* __restrict__ Qg,
+                                                    double* __restrict__ qqg) {
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= n_rows_pad) return;
+  const int64_t b = row / S;
+  const int pp = (int)(row - b * S);
+  query_row(row < n_rows ? xq + b * D : nullptr, pinv + pp * D, mu, D, DS, row, Qg, qqg);
 }
 
 // Small host-buffer batches (the CUDA-graph path): descriptor, its derivative factors and the S query rows of one
@@ -654,27 +664,11 @@ __global__ void __launch_bounds__(256) k_desc_query_rows(const double* __restric
     g[2] = dz * inv3;
   }
   __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+  const int warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
   // rows b*S .. b*S+S-1; the last CTA also clears the padding rows of the last main-kernel tile
   const int extra = b == (int64_t)gridDim.x - 1 ? (int)(n_rows_pad - n_rows) : 0;
-  for (int pp = warp; pp < S + extra; pp += n_warps) {
-    const int64_t row = b * S + pp;
-    double s = 0.0;
-    if (pp < S) {
-      const int* pi = pinv + pp * D;
-      for (int e = lane; e < DS; e += 32) {
-        double v = 0.0;
-        if (e < D) v = x[pi[e]] - mu[e];
-        Qg[row * DS + e] = v;
-        s = fma(v, v, s);
-      }
-    } else {
-      for (int e = lane; e < DS; e += 32) Qg[row * DS + e] = 0.0;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) qqg[row] = s;
-  }
+  for (int pp = warp; pp < S + extra; pp += n_warps)
+    query_row(pp < S ? x : nullptr, pinv + pp * D, mu, D, DS, b * S + pp, Qg, qqg);
 }
 
 // ============================================================== large descriptors (D > 256)
@@ -782,118 +776,125 @@ __device__ __forceinline__ int virial_slot(int e) {
   return i == j ? i : i + j + 2;
 }
 
-// ============================================================== finishing kernel
-// F_desc[d] = sum_p G[b*S+p][perm_p[d]];  F = J_x^T F_desc (predict.py:240-243);
-// E = sum_p Erow;  outputs scaled by std, E += c (predict.py:1286-1288).
+// ============================================================== finishing kernels
+// The pieces every finishing kernel shares, so that they sum in one order: F_desc, E and W of the plain and virial
+// variants are bit-identical, as are those of the shared-memory and the workspace forms of F_desc.
+
+// F_desc[d] of query b = sum_p sum_split G[b*S+p][perm_p[d]]: fixed order (permutation-major, then split) with four
+// independent accumulators so that the L2 round trips of the gathered loads overlap (n_splits * S terms per entry)
+__device__ __forceinline__ double fdesc_entry(const double* __restrict__ G, const int* __restrict__ perm, int D, int DP,
+                                              int S, int n_splits, int64_t stride, int64_t b, int d) {
+  double acc0 = 0.0, acc1 = 0.0, acc2 = 0.0, acc3 = 0.0;
+  for (int pp = 0; pp < S; ++pp) {
+    const double* gp = G + (b * S + pp) * DP + perm[pp * D + d];
+    int sp = 0;
+    for (; sp + 4 <= n_splits; sp += 4) {
+      acc0 += gp[(int64_t)sp * stride];
+      acc1 += gp[(int64_t)(sp + 1) * stride];
+      acc2 += gp[(int64_t)(sp + 2) * stride];
+      acc3 += gp[(int64_t)(sp + 3) * stride];
+    }
+    for (; sp < n_splits; ++sp) acc0 += gp[(int64_t)sp * stride];
+  }
+  return (acc0 + acc1) + (acc2 + acc3);
+}
+
+// F[k][cc] / std = (J_x^T F_desc)[3k + cc] (predict.py:240-243) from the query's g (D x 3) and F_desc f
+__device__ __forceinline__ double force_entry(const double* __restrict__ g, const double* f, int n_atoms, int k, int cc) {
+  double s = 0.0;
+  for (int o = 0; o < n_atoms; ++o) {
+    if (o == k) continue;
+    if (o > k) {
+      const int d = pair_index(o, k);
+      s += g[d * 3 + cc] * f[d];
+    } else {
+      const int d = pair_index(k, o);
+      s -= g[d * 3 + cc] * f[d];
+    }
+  }
+  return s;
+}
+
+// E[b] = std sum_split sum_p Erow[split][b*S+p] + c (predict.py:1286-1288): one warp, lanes over the terms
+__device__ __forceinline__ void energy_sum(const double* __restrict__ Erow, int S, int n_splits, int64_t plane_rows,
+                                           int64_t b, double std, double c, double* __restrict__ E) {
+  const int lane = threadIdx.x & 31;
+  double s = 0.0;
+  for (int t = lane; t < n_splits * S; t += 32) {
+    const int sp = t / S, pp = t - sp * S;
+    s += Erow[(int64_t)sp * plane_rows + b * S + pp];
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) E[b] = s * std + c;
+}
+
+// The six virial sums w of every thread of the CTA added in a fixed order: a shuffle tree per warp, the warps' sums
+// staged in wpart (one row per warp), then the warps in index order.  W_OUT: out[0..8] = -std W, mirrored through
+// virial_slot; else out[0..5] = the six sums (a per-CTA partial).  The caller synchronises before wpart is reused.
+template <bool W_OUT>
+__device__ __forceinline__ void block_sum6(double* w, double (*wpart)[6], double std, double* __restrict__ out) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  warp_sum6(w);
+  if (lane < 6) wpart[warp][lane] = w[lane];
+  __syncthreads();
+  if (threadIdx.x < (W_OUT ? 9 : 6)) {
+    const int k = W_OUT ? virial_slot(threadIdx.x) : (int)threadIdx.x;
+    double s = 0.0;
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += wpart[i][k];
+    out[threadIdx.x] = W_OUT ? -std * s : s;
+  }
+}
+
+// F_desc[d] = sum_p G[b*S+p][perm_p[d]];  F = J_x^T F_desc;  E = sum_p Erow;  outputs scaled by std, E += c.
 // One CTA per QPB queries (QPB = 128 / D for small molecules, else 1): threads over (query, descriptor entry), then
 // over (query, force component).  WITH_W: also the virial W (n_geo x 9), from the F_desc in shared memory -- one warp
 // per query for QPB > 1, all four warps for QPB = 1 (summed in warp order).
 template <bool WITH_W>
-__device__ __forceinline__ void predict_finish_body(const double* __restrict__ G, const double* __restrict__ Erow,
-                                                    const double* __restrict__ gq, const int* __restrict__ perm,
-                                                    int n_atoms, int D, int DP, int S, double std, double c,
-                                                    int n_splits, int64_t plane_rows, int64_t n_geo, int QPB,
-                                                    double* __restrict__ E, double* __restrict__ F,
-                                                    double* __restrict__ W) {
+__global__ void __launch_bounds__(128) k_predict_finish(const double* __restrict__ G, const double* __restrict__ Erow,
+                                                        const double* __restrict__ gq, const int* __restrict__ perm,
+                                                        int n_atoms, int D, int DP, int S, double std, double c,
+                                                        int n_splits, int64_t plane_rows, int64_t n_geo, int QPB,
+                                                        double* __restrict__ E, double* __restrict__ F,
+                                                        double* __restrict__ W) {
   extern __shared__ double fd[];  // QPB * D
   const int64_t b0 = (int64_t)blockIdx.x * QPB;
   const int nq = (int)min((int64_t)QPB, n_geo - b0);
-  // fixed summation order (permutation-major, then split) with four independent accumulators so
-  // that the L2 round trips of the gathered loads overlap (n_splits * S terms per descriptor entry)
   const int64_t stride = plane_rows * DP;
   for (int e = threadIdx.x; e < nq * D; e += blockDim.x) {
     const int ql = e / D, d = e - ql * D;
-    const int64_t b = b0 + ql;
-    double acc0 = 0.0, acc1 = 0.0, acc2 = 0.0, acc3 = 0.0;
-    for (int pp = 0; pp < S; ++pp) {
-      const double* gp = G + (b * S + pp) * DP + perm[pp * D + d];
-      int sp = 0;
-      for (; sp + 4 <= n_splits; sp += 4) {
-        acc0 += gp[(int64_t)sp * stride];
-        acc1 += gp[(int64_t)(sp + 1) * stride];
-        acc2 += gp[(int64_t)(sp + 2) * stride];
-        acc3 += gp[(int64_t)(sp + 3) * stride];
-      }
-      for (; sp < n_splits; ++sp) acc0 += gp[(int64_t)sp * stride];
-    }
-    fd[e] = (acc0 + acc1) + (acc2 + acc3);
+    fd[e] = fdesc_entry(G, perm, D, DP, S, n_splits, stride, b0 + ql, d);
   }
   __syncthreads();
   const int dimi = 3 * n_atoms;
   for (int e = threadIdx.x; e < nq * dimi; e += blockDim.x) {
     const int ql = e / dimi, idx = e - ql * dimi;
     const int64_t b = b0 + ql;
-    const double* g = gq + b * (int64_t)D * 3;
-    const double* f = fd + ql * D;
     const int k = idx / 3, cc = idx - 3 * k;
-    double s = 0.0;
-    for (int o = 0; o < n_atoms; ++o) {
-      if (o == k) continue;
-      if (o > k) {
-        const int d = pair_index(o, k);
-        s += g[d * 3 + cc] * f[d];
-      } else {
-        const int d = pair_index(k, o);
-        s -= g[d * 3 + cc] * f[d];
-      }
-    }
-    F[b * dimi + idx] = s * std;
+    F[b * dimi + idx] = force_entry(gq + b * (int64_t)D * 3, fd + ql * D, n_atoms, k, cc) * std;
   }
-  if (E != nullptr) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int ql = warp; ql < nq; ql += (int)(blockDim.x >> 5)) {
-      const int64_t b = b0 + ql;
-      double s = 0.0;
-      for (int t = lane; t < n_splits * S; t += 32) {
-        const int sp = t / S, pp = t - sp * S;
-        s += Erow[(int64_t)sp * plane_rows + b * S + pp];
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      if (lane == 0) E[b] = s * std + c;
-    }
-  }
+  if (E != nullptr)
+    for (int ql = threadIdx.x >> 5; ql < nq; ql += (int)(blockDim.x >> 5))
+      energy_sum(Erow, S, n_splits, plane_rows, b0 + ql, std, c, E);
   if constexpr (WITH_W) {
-    __shared__ double wpart[4][6];  // QPB = 1: the four warps' sums
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double w[6];
     if (QPB > 1) {
+      const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
       for (int ql = warp; ql < nq; ql += 4) {
         const double* g = gq + (b0 + ql) * (int64_t)D * 3;
-        double w[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        for (double& x : w) x = 0.0;
         for (int d = lane; d < D; d += 32) virial_term(g + 3 * d, fd[ql * D + d], w);
         warp_sum6(w);
         if (lane < 9) W[(b0 + ql) * 9 + lane] = -std * w[virial_slot(lane)];
       }
     } else {
+      __shared__ double wpart[4][6];
       const double* g = gq + b0 * (int64_t)D * 3;
-      double w[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+      for (double& x : w) x = 0.0;
       for (int d = threadIdx.x; d < D; d += 128) virial_term(g + 3 * d, fd[d], w);
-      warp_sum6(w);
-      if (lane < 6) wpart[warp][lane] = w[lane];
-      __syncthreads();
-      if (threadIdx.x < 9) {
-        const int k = virial_slot(threadIdx.x);
-        W[b0 * 9 + threadIdx.x] = -std * (((wpart[0][k] + wpart[1][k]) + wpart[2][k]) + wpart[3][k]);
-      }
+      block_sum6<true>(w, wpart, std, W + b0 * 9);
     }
   }
-}
-
-__global__ void __launch_bounds__(128) k_predict_finish(const double* __restrict__ G, const double* __restrict__ Erow,
-                                                        const double* __restrict__ gq, const int* __restrict__ perm,
-                                                        int n_atoms, int D, int DP, int S, double std, double c,
-                                                        int n_splits, int64_t plane_rows, int64_t n_geo, int QPB,
-                                                        double* __restrict__ E, double* __restrict__ F) {
-  predict_finish_body<false>(G, Erow, gq, perm, n_atoms, D, DP, S, std, c, n_splits, plane_rows, n_geo, QPB, E, F,
-                             nullptr);
-}
-__global__ void __launch_bounds__(128) k_predict_finish_w(const double* __restrict__ G, const double* __restrict__ Erow,
-                                                          const double* __restrict__ gq, const int* __restrict__ perm,
-                                                          int n_atoms, int D, int DP, int S, double std, double c,
-                                                          int n_splits, int64_t plane_rows, int64_t n_geo, int QPB,
-                                                          double* __restrict__ E, double* __restrict__ F,
-                                                          double* __restrict__ W) {
-  predict_finish_body<true>(G, Erow, gq, perm, n_atoms, D, DP, S, std, c, n_splits, plane_rows, n_geo, QPB, E, F, W);
 }
 
 // The same for batches of a few queries (the MD latency path: one geometry per call).  There the one-CTA-per-query form
@@ -901,12 +902,12 @@ __global__ void __launch_bounds__(128) k_predict_finish_w(const double* __restri
 // threads split every descriptor entry's terms into `parts` interleaved partial sums (fixed order: bit-reproducible).
 // WITH_W: the virial of the query, 32 warps' sums added in warp order.
 template <bool WITH_W>
-__device__ __forceinline__ void predict_finish_small_body(const double* __restrict__ G, const double* __restrict__ Erow,
-                                                          const double* __restrict__ gq, const int* __restrict__ perm,
-                                                          int n_atoms, int D, int DP, int S, double std, double c,
-                                                          int n_splits, int64_t plane_rows, int parts,
-                                                          double* __restrict__ E, double* __restrict__ F,
-                                                          double* __restrict__ W) {
+__global__ void __launch_bounds__(1024) k_predict_finish_small(const double* __restrict__ G, const double* __restrict__ Erow,
+                                                               const double* __restrict__ gq, const int* __restrict__ perm,
+                                                               int n_atoms, int D, int DP, int S, double std, double c,
+                                                               int n_splits, int64_t plane_rows, int parts,
+                                                               double* __restrict__ E, double* __restrict__ F,
+                                                               double* __restrict__ W) {
   extern __shared__ double fds[];  // parts * D partial sums, then D totals
   double* fd = fds + parts * D;
   const int64_t b = blockIdx.x;
@@ -937,69 +938,21 @@ __device__ __forceinline__ void predict_finish_small_body(const double* __restri
   const double* g = gq + b * (int64_t)D * 3;
   for (int idx = threadIdx.x; idx < dimi; idx += blockDim.x) {
     const int k = idx / 3, cc = idx - 3 * k;
-    double sum = 0.0;
-    for (int o = 0; o < n_atoms; ++o) {
-      if (o == k) continue;
-      if (o > k) {
-        const int d = pair_index(o, k);
-        sum += g[d * 3 + cc] * fd[d];
-      } else {
-        const int d = pair_index(k, o);
-        sum -= g[d * 3 + cc] * fd[d];
-      }
-    }
-    F[b * dimi + idx] = sum * std;
+    F[b * dimi + idx] = force_entry(g, fd, n_atoms, k, cc) * std;
   }
-  if (E != nullptr && threadIdx.x >= blockDim.x - 32) {  // last warp
-    const int lane = threadIdx.x & 31;
-    double sum = 0.0;
-    for (int t = lane; t < n_terms; t += 32) {
-      const int sp = t / S, pp = t - sp * S;
-      sum += Erow[(int64_t)sp * plane_rows + b * S + pp];
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    if (lane == 0) E[b] = sum * std + c;
-  }
+  if (E != nullptr && threadIdx.x >= blockDim.x - 32) energy_sum(Erow, S, n_splits, plane_rows, b, std, c, E);  // last warp
   if constexpr (WITH_W) {
     __shared__ double wpart[32][6];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     double w[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
     for (int d = threadIdx.x; d < D; d += blockDim.x) virial_term(g + 3 * d, fd[d], w);
-    warp_sum6(w);
-    if (lane < 6) wpart[warp][lane] = w[lane];
-    __syncthreads();
-    if (threadIdx.x < 9) {
-      const int k = virial_slot(threadIdx.x);
-      double s = 0.0;
-      for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += wpart[i][k];
-      W[b * 9 + threadIdx.x] = -std * s;
-    }
+    block_sum6<true>(w, wpart, std, W + b * 9);
   }
-}
-
-__global__ void __launch_bounds__(1024) k_predict_finish_small(const double* __restrict__ G, const double* __restrict__ Erow,
-                                                               const double* __restrict__ gq, const int* __restrict__ perm,
-                                                               int n_atoms, int D, int DP, int S, double std, double c,
-                                                               int n_splits, int64_t plane_rows, int parts,
-                                                               double* __restrict__ E, double* __restrict__ F) {
-  predict_finish_small_body<false>(G, Erow, gq, perm, n_atoms, D, DP, S, std, c, n_splits, plane_rows, parts, E, F,
-                                   nullptr);
-}
-__global__ void __launch_bounds__(1024) k_predict_finish_small_w(const double* __restrict__ G,
-                                                                 const double* __restrict__ Erow,
-                                                                 const double* __restrict__ gq,
-                                                                 const int* __restrict__ perm, int n_atoms, int D,
-                                                                 int DP, int S, double std, double c, int n_splits,
-                                                                 int64_t plane_rows, int parts, double* __restrict__ E,
-                                                                 double* __restrict__ F, double* __restrict__ W) {
-  predict_finish_small_body<true>(G, Erow, gq, perm, n_atoms, D, DP, S, std, c, n_splits, plane_rows, parts, E, F, W);
 }
 
 // ============================================================== finishing path for long descriptors
 // From D > 25,600 (N >= 227 atoms) the F_desc of one query no longer fits the shared memory of k_predict_finish; it goes
 // to a device workspace Fd (n_geo x D) between two kernels:
-//   k_fdesc_gather:  Fd[b][d] = sum_p sum_split G[b*S+p][perm_p[d]]   (the summation order of k_predict_finish)
+//   k_fdesc_gather:  Fd[b][d] = sum_p sum_split G[b*S+p][perm_p[d]]   (fdesc_entry, as in k_predict_finish)
 //   k_fdesc_project: F = J_x^T Fd * std, E = sum Erow * std + c
 // Both are HBM-bound (S*DP*8 bytes of G, 3*D*8 of gq and 2*D*8 of Fd per query) and use no atomics: fixed order, so the
 // results are bit-identical run to run and between graph replay and plain launches.
@@ -1008,59 +961,28 @@ __global__ void __launch_bounds__(1024) k_predict_finish_small_w(const double* _
 // cover the S rows of a few queries (S*DP*8 bytes each, 1.6 MB at N = 370, S = 3), so the permuted reads (scattered only
 // where an atom permutation breaks up runs of consecutive pairs; the identity is read in order) hit L2 and HBM delivers
 // every sector of G once.
-__device__ __forceinline__ double fdesc_entry(const double* __restrict__ G, const int* __restrict__ perm, int D, int DP,
-                                              int S, int n_splits, int64_t stride, int64_t b, int d) {
-  double acc0 = 0.0, acc1 = 0.0, acc2 = 0.0, acc3 = 0.0;
-  for (int pp = 0; pp < S; ++pp) {
-    const double* gp = G + (b * S + pp) * DP + perm[pp * D + d];
-    int sp = 0;
-    for (; sp + 4 <= n_splits; sp += 4) {
-      acc0 += gp[(int64_t)sp * stride];
-      acc1 += gp[(int64_t)(sp + 1) * stride];
-      acc2 += gp[(int64_t)(sp + 2) * stride];
-      acc3 += gp[(int64_t)(sp + 3) * stride];
-    }
-    for (; sp < n_splits; ++sp) acc0 += gp[(int64_t)sp * stride];
-  }
-  return (acc0 + acc1) + (acc2 + acc3);
-}
-
+// WITH_W: the gather touches every pair exactly once, so each CTA also sums the virial terms of its 256 entries into
+// Wp[b][blockIdx.x][6]; k_fdesc_project<true> adds those ceil(D/256) partials in CTA order.
+template <bool WITH_W>
 __global__ void __launch_bounds__(256) k_fdesc_gather(const double* __restrict__ G, const int* __restrict__ perm, int D,
                                                       int DP, int S, int n_splits, int64_t plane_rows, int64_t n_geo,
-                                                      double* __restrict__ Fd) {
+                                                      double* __restrict__ Fd, const double* __restrict__ gq,
+                                                      double* __restrict__ Wp) {
   const int d = blockIdx.x * blockDim.x + threadIdx.x;
-  if (d >= D) return;
-  const int64_t stride = plane_rows * DP;
-  for (int64_t b = blockIdx.y; b < n_geo; b += gridDim.y) Fd[b * D + d] = fdesc_entry(G, perm, D, DP, S, n_splits, stride, b, d);
-}
-
-// With the virial: the gather touches every pair exactly once, so each CTA also sums the virial terms of its 256
-// entries (shuffle tree, then its eight warps in order) into Wp[b][blockIdx.x][6]; k_fdesc_project_w adds those
-// ceil(D/256) partials in CTA order.
-__global__ void __launch_bounds__(256) k_fdesc_gather_w(const double* __restrict__ G, const int* __restrict__ perm,
-                                                        const double* __restrict__ gq, int D, int DP, int S,
-                                                        int n_splits, int64_t plane_rows, int64_t n_geo,
-                                                        double* __restrict__ Fd, double* __restrict__ Wp) {
-  __shared__ double wpart[8][6];
-  const int d = blockIdx.x * blockDim.x + threadIdx.x;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (!WITH_W && d >= D) return;
   const int64_t stride = plane_rows * DP;
   for (int64_t b = blockIdx.y; b < n_geo; b += gridDim.y) {
     double w[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
     if (d < D) {
       const double f = fdesc_entry(G, perm, D, DP, S, n_splits, stride, b, d);
       Fd[b * D + d] = f;
-      virial_term(gq + (b * D + d) * 3, f, w);
+      if constexpr (WITH_W) virial_term(gq + (b * D + d) * 3, f, w);
     }
-    warp_sum6(w);
-    if (lane < 6) wpart[warp][lane] = w[lane];
-    __syncthreads();
-    if (threadIdx.x < 6) {
-      double s = 0.0;
-      for (int i = 0; i < 8; ++i) s += wpart[i][threadIdx.x];
-      Wp[(b * gridDim.x + blockIdx.x) * 6 + threadIdx.x] = s;
+    if constexpr (WITH_W) {
+      __shared__ double wpart[8][6];
+      block_sum6<false>(w, wpart, 0.0, Wp + (b * gridDim.x + blockIdx.x) * 6);
+      __syncthreads();  // wpart is rewritten for the next query
     }
-    __syncthreads();  // wpart is rewritten for the next query
   }
 }
 
@@ -1070,11 +992,16 @@ __global__ void __launch_bounds__(256) k_fdesc_gather_w(const double* __restrict
 // 96 gq values in one piece; the o are dealt round-robin to the warps.  Row part (o < k): entries (k, 0..k-1) are
 // consecutive; one warp per atom, lanes over o.  Each entry is read by two CTAs of the same query, which run side by
 // side (grid x = atom groups), so the second read comes from L2.
+// WITH_W: then the virial of each query from the n_parts per-CTA partials of k_fdesc_gather<true> (CTA order).
 constexpr int FDP_WARPS = 8;
-__device__ __forceinline__ void fdesc_project_body(const double* __restrict__ Fd, const double* __restrict__ gq,
-                                                     const double* __restrict__ Erow, int n_atoms, int D, int S,
-                                                     double std, double c, int n_splits, int64_t plane_rows,
-                                                     int64_t n_geo, double* __restrict__ E, double* __restrict__ F) {
+template <bool WITH_W>
+__global__ void __launch_bounds__(FDP_WARPS * 32) k_fdesc_project(const double* __restrict__ Fd, const double* __restrict__ gq,
+                                                                  const double* __restrict__ Erow, int n_atoms, int D,
+                                                                  int S, double std, double c, int n_splits,
+                                                                  int64_t plane_rows, int64_t n_geo,
+                                                                  double* __restrict__ E, double* __restrict__ F,
+                                                                  const double* __restrict__ Wp, int n_parts,
+                                                                  double* __restrict__ W) {
   __shared__ double col[FDP_WARPS][32][3];
   __shared__ double row[32][3];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1130,43 +1057,17 @@ __device__ __forceinline__ void fdesc_project_body(const double* __restrict__ Fd
         F[b * dimi + 3 * (k0 + kl) + cc] = (s - row[kl][cc]) * std;
       }
     }
-    if (E != nullptr && blockIdx.x == 0 && warp == FDP_WARPS - 1) {
-      double s = 0.0;
-      for (int t = lane; t < n_splits * S; t += 32) {
-        const int sp = t / S, pp = t - sp * S;
-        s += Erow[(int64_t)sp * plane_rows + b * S + pp];
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      if (lane == 0) E[b] = s * std + c;
-    }
+    if (E != nullptr && blockIdx.x == 0 && warp == FDP_WARPS - 1) energy_sum(Erow, S, n_splits, plane_rows, b, std, c, E);
     __syncthreads();  // col / row are rewritten for the next query
   }
-}
-__global__ void __launch_bounds__(FDP_WARPS * 32) k_fdesc_project(const double* __restrict__ Fd, const double* __restrict__ gq,
-                                                                  const double* __restrict__ Erow, int n_atoms, int D,
-                                                                  int S, double std, double c, int n_splits,
-                                                                  int64_t plane_rows, int64_t n_geo,
-                                                                  double* __restrict__ E, double* __restrict__ F) {
-  fdesc_project_body(Fd, gq, Erow, n_atoms, D, S, std, c, n_splits, plane_rows, n_geo, E, F);
-}
-
-// k_fdesc_project, then the virial of each query from the n_parts per-CTA partials of k_fdesc_gather_w (CTA order)
-__global__ void __launch_bounds__(FDP_WARPS * 32) k_fdesc_project_w(const double* __restrict__ Fd,
-                                                                    const double* __restrict__ gq,
-                                                                    const double* __restrict__ Erow, int n_atoms,
-                                                                    int D, int S, double std, double c, int n_splits,
-                                                                    int64_t plane_rows, int64_t n_geo,
-                                                                    double* __restrict__ E, double* __restrict__ F,
-                                                                    const double* __restrict__ Wp, int n_parts,
-                                                                    double* __restrict__ W) {
-  fdesc_project_body(Fd, gq, Erow, n_atoms, D, S, std, c, n_splits, plane_rows, n_geo, E, F);
-  if (blockIdx.x != 0 || threadIdx.x >= 9) return;
-  const int k = virial_slot(threadIdx.x);
-  for (int64_t b = blockIdx.y; b < n_geo; b += gridDim.y) {
-    double s = 0.0;
-    for (int i = 0; i < n_parts; ++i) s += Wp[(b * n_parts + i) * 6 + k];
-    W[b * 9 + threadIdx.x] = -std * s;
+  if constexpr (WITH_W) {
+    if (blockIdx.x != 0 || threadIdx.x >= 9) return;
+    const int slot = virial_slot(threadIdx.x);
+    for (int64_t b = blockIdx.y; b < n_geo; b += gridDim.y) {
+      double s = 0.0;
+      for (int i = 0; i < n_parts; ++i) s += Wp[(b * n_parts + i) * 6 + slot];
+      W[b * 9 + threadIdx.x] = -std * s;
+    }
   }
 }
 
@@ -1621,6 +1522,100 @@ int64_t chunk_geos(const sgdml_b200_model* m) {
   return g;
 }
 
+// Opts kernel K in to dyn bytes of dynamic shared memory when they and its static shared memory exceed the 48 KB
+// allowed without opt-in.  The static size is looked up once per kernel and device.
+template <auto K>
+int opt_in_smem(size_t dyn) {
+  static size_t static_bytes[64];
+  static bool known[64] = {false};
+  int dev = 0;
+  SG_CUDA(cudaGetDevice(&dev));
+  size_t st;
+  if (dev >= 0 && dev < 64 && known[dev]) {
+    st = static_bytes[dev];
+  } else {
+    cudaFuncAttributes fa;
+    SG_CUDA(cudaFuncGetAttributes(&fa, K));
+    st = fa.sharedSizeBytes;
+    if (dev >= 0 && dev < 64) {
+      static_bytes[dev] = st;
+      known[dev] = true;
+    }
+  }
+  if (dyn + st > 48 * 1024) SG_CUDA(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
+  return 0;
+}
+
+// Captures the work enqueue() queues on gs (not the legacy stream) into *exec; *n_kernels: the kernel launches counted
+// while it was queued, which a replay of the graph counts again
+template <class Enqueue>
+int capture_graph(cudaStream_t gs, Enqueue&& enqueue, cudaGraphExec_t* exec, int* n_kernels) {
+  auto launches = [] {
+    int64_t n = 0;
+    for (int k = 0; k < KID_COUNT; ++k) {
+      int64_t ln = 0;
+      sgdml_b200_profile_get(k, nullptr, nullptr, &ln);
+      n += ln;
+    }
+    return n;
+  };
+  const int64_t before = launches();
+  cudaGraph_t graph = nullptr;
+  SG_CUDA(cudaStreamBeginCapture(gs, cudaStreamCaptureModeThreadLocal));
+  const int rc = enqueue();
+  cudaError_t e = cudaStreamEndCapture(gs, &graph);
+  if (rc != 0) {
+    if (graph) cudaGraphDestroy(graph);
+    return rc;
+  }
+  SG_CUDA(e);
+  e = cudaGraphInstantiate(exec, graph, 0);
+  cudaGraphDestroy(graph);
+  SG_CUDA(e);
+  *n_kernels = (int)(launches() - before);
+  return 0;
+}
+
+// The two FP64 contractions of the GEMM-composed path (D > 256, and every Hessian-vector product) over `rows` rows of A:
+//   S1 = A Xc^T, S2 = A JA^T        (rows x Mpad, contraction over the padded descriptor)
+int contract_desc(const sgdml_b200_model* m, const double* A, int64_t rows, double* S1, double* S2, cudaStream_t s) {
+  GemmArgs g{};
+  g.m = rows;
+  g.n = m->Mpad;
+  g.k = m->DS;
+  g.A = A;
+  g.lda = m->DS;
+  g.B = m->Xc;
+  g.ldb = m->DS;
+  g.C = S1;
+  g.ldc = m->Mpad;
+  g.alpha = 1.0;
+  SG_TRY(launch_gemm(g, s));
+  g.B = m->JA;
+  g.C = S2;
+  return launch_gemm(g, s);
+}
+//   G = C1 XcT^T + C2 JAT^T         (rows x DP, contraction over the training points; the second GEMM accumulates)
+int contract_points(const sgdml_b200_model* m, const double* C1, const double* C2, int64_t rows, double* G,
+                    cudaStream_t s) {
+  GemmArgs g{};
+  g.m = rows;
+  g.n = m->DP;
+  g.k = m->Mpad;
+  g.A = C1;
+  g.lda = m->Mpad;
+  g.B = m->XcT;
+  g.ldb = m->Mpad;
+  g.C = G;
+  g.ldc = m->DP;
+  g.alpha = 1.0;
+  SG_TRY(launch_gemm(g, s));
+  g.mode = 1;
+  g.A = C2;
+  g.B = m->JAT;
+  return launch_gemm(g, s);
+}
+
 // Runs the predictor on n_geo queries whose descriptors (xq, gq) are on the device.
 constexpr int64_t GRAPH_MAX_GEO = 16;  // batches up to this size with host buffers replay a captured graph
 // xq == nullptr: the query rows (w.Qg, w.qq) are already in place (k_desc_query_rows)
@@ -1640,17 +1635,8 @@ int run_queries(sgdml_b200_model* m, sgdml_b200_model::WS& w, const double* xq, 
   }
   if (m->large) {
     ProfScope ps(KID_PREDICT_MAIN, s);
-    MaternK mk;
-    mk.sig = m->sig;
-    mk.sig_inv = 1.0 / m->sig;
-    mk.k_base = 5.0 / (3.0 * m->sig * m->sig * m->sig);
-    mk.k_c1 = mk.k_base * 5.0 / m->sig;
-    GemmArgs g;
-    g.alpha = 1.0;
-    g.beta = 0.0;
-    g.mode = 0;
-    g.tri = 0;
-    g.abort_flag = nullptr;
+    const MaternK mk = MaternK::from_sig(m->sig);
+    const double* ae = m->use_ae ? m->ae : nullptr;
     // The four contractions on the int8 tensor cores (wgmma) through exact int8 slice products (csrc/ozaki.cu): the
     // slices of the model matrices are kept with the model, those of Q, C1, C2 are cut per batch; everything is
     // stream-ordered (this path runs once per CG iteration inside sgdml_b200_pcg).  Slice count: m->oz_s
@@ -1660,7 +1646,7 @@ int run_queries(sgdml_b200_model* m, sgdml_b200_model::WS& w, const double* xq, 
       SG_TRY(ozaki_split(w.Qg, n_rows, m->DS, m->DS, S, w.ozQ.units, w.ozQ.exps, &w.ozQ, s));
       SG_TRY(ozaki_gemm(w.ozQ, m->ozXc, n_rows, m->Mpad, 1.0, 1, w.S1, m->Mpad, S, s));
       SG_TRY(ozaki_gemm(w.ozQ, m->ozJA, n_rows, m->Mpad, 1.0, 1, w.S2, m->Mpad, S, s));
-      k_transform_rows<<<(unsigned)((n_rows + 7) / 8), 256, 0, s>>>(w.S1, w.S2, m->Mpad, w.qq, m->mm, m->xja, m->use_ae ? m->ae : nullptr, m->M,
+      k_transform_rows<<<(unsigned)((n_rows + 7) / 8), 256, 0, s>>>(w.S1, w.S2, m->Mpad, w.qq, m->mm, m->xja, ae, m->M,
                                                                      m->Mpad, n_rows, mk, w.csum, w.Erow);
       SG_CUDA(cudaGetLastError());
       SG_TRY(ozaki_split(w.S1, n_rows, m->Mpad, m->Mpad, S, w.ozC1.units, w.ozC1.exps, &w.ozC1, s));
@@ -1668,37 +1654,11 @@ int run_queries(sgdml_b200_model* m, sgdml_b200_model::WS& w, const double* xq, 
       SG_TRY(ozaki_gemm(w.ozC1, m->ozXcT, n_rows, m->DP, 1.0, 1, w.G, m->DP, S, s));
       SG_TRY(ozaki_gemm(w.ozC2, m->ozJAT, n_rows, m->DP, 1.0, 0, w.G, m->DP, S, s));
     } else {
-    // S1 = Q Xc^T, S2 = Q JA^T   (rows x Mpad, contraction over the padded descriptor)
-    g.m = n_rows;
-    g.n = m->Mpad;
-    g.k = m->DS;
-    g.A = w.Qg;
-    g.lda = m->DS;
-    g.ldb = m->DS;
-    g.ldc = m->Mpad;
-    g.B = m->Xc;
-    g.C = w.S1;
-    SG_TRY(launch_gemm(g, s));
-    g.B = m->JA;
-    g.C = w.S2;
-    SG_TRY(launch_gemm(g, s));
-    k_transform_rows<<<(unsigned)((n_rows + 7) / 8), 256, 0, s>>>(w.S1, w.S2, m->Mpad, w.qq, m->mm, m->xja, m->use_ae ? m->ae : nullptr, m->M,
-                                                                   m->Mpad, n_rows, mk, w.csum, w.Erow);
-    SG_CUDA(cudaGetLastError());
-    // acc = C1 XcT^T + C2 JAT^T   (rows x DP, contraction over the training points)
-    g.n = m->DP;
-    g.k = m->Mpad;
-    g.lda = m->Mpad;
-    g.ldb = m->Mpad;
-    g.ldc = m->DP;
-    g.A = w.S1;
-    g.B = m->XcT;
-    g.C = w.G;
-    SG_TRY(launch_gemm(g, s));
-    g.mode = 1;
-    g.A = w.S2;
-    g.B = m->JAT;
-    SG_TRY(launch_gemm(g, s));
+      SG_TRY(contract_desc(m, w.Qg, n_rows, w.S1, w.S2, s));
+      k_transform_rows<<<(unsigned)((n_rows + 7) / 8), 256, 0, s>>>(w.S1, w.S2, m->Mpad, w.qq, m->mm, m->xja, ae, m->M,
+                                                                     m->Mpad, n_rows, mk, w.csum, w.Erow);
+      SG_CUDA(cudaGetLastError());
+      SG_TRY(contract_points(m, w.S1, w.S2, n_rows, w.G, s));
     }
     k_combine_rows<<<(unsigned)((n_rows * m->DP + 255) / 256), 256, 0, s>>>(w.Qg, m->DS, w.csum, w.G, m->DP, n_rows);
     SG_CUDA(cudaGetLastError());
@@ -1740,63 +1700,50 @@ int run_queries(sgdml_b200_model* m, sgdml_b200_model::WS& w, const double* xq, 
     SG_TRY(launch_main(m->cfg, a, n_splits, s));
     count_launch(KID_PREDICT_MAIN);
   }
-  if (fdesc_in_ws(m)) {
-    ProfScope ps(KID_PREDICT_FINISH, s);
-    const unsigned gy = (unsigned)std::min<int64_t>(n_geo, 65535);
-    const int n_parts = ceil_div(m->D, 256);
-    if (W_dev != nullptr) {
-      k_fdesc_gather_w<<<dim3((unsigned)n_parts, gy), 256, 0, s>>>(w.G, m->perm, gq, m->D, m->DP, m->S, n_splits,
-                                                                   n_rows_pad, n_geo, w.Fd, w.Wp);
+  // the finishing kernels, plain or with the virial (WITH_W is compile-time: the plain kernels carry no virial code)
+  auto finish = [&](auto with_w) -> int {
+    constexpr bool WITH_W = decltype(with_w)::value;
+    if (fdesc_in_ws(m)) {
+      ProfScope ps(KID_PREDICT_FINISH, s);
+      const unsigned gy = (unsigned)std::min<int64_t>(n_geo, 65535);
+      const int n_parts = ceil_div(m->D, 256);
+      k_fdesc_gather<WITH_W><<<dim3((unsigned)n_parts, gy), 256, 0, s>>>(w.G, m->perm, m->D, m->DP, m->S, n_splits,
+                                                                         n_rows_pad, n_geo, w.Fd, gq, w.Wp);
       SG_CUDA(cudaGetLastError());
-      k_fdesc_project_w<<<dim3((unsigned)ceil_div(m->N, 32), gy), FDP_WARPS * 32, 0, s>>>(
+      k_fdesc_project<WITH_W><<<dim3((unsigned)ceil_div(m->N, 32), gy), FDP_WARPS * 32, 0, s>>>(
           w.Fd, gq, w.Erow, m->N, m->D, m->S, std, c, n_splits, n_rows_pad, n_geo, E_dev, F_dev, w.Wp, n_parts, W_dev);
-    } else {
-      k_fdesc_gather<<<dim3((unsigned)n_parts, gy), 256, 0, s>>>(w.G, m->perm, m->D, m->DP, m->S, n_splits,
-                                                                 n_rows_pad, n_geo, w.Fd);
       SG_CUDA(cudaGetLastError());
-      k_fdesc_project<<<dim3((unsigned)ceil_div(m->N, 32), gy), FDP_WARPS * 32, 0, s>>>(
-          w.Fd, gq, w.Erow, m->N, m->D, m->S, std, c, n_splits, n_rows_pad, n_geo, E_dev, F_dev);
+      count_launch(KID_PREDICT_FINISH, 2);
+      return 0;
     }
-    SG_CUDA(cudaGetLastError());
-    count_launch(KID_PREDICT_FINISH, 2);
-    return 0;
-  }
-  {
     ProfScope ps(KID_PREDICT_AUX, s);
     const int QPB = std::max(1, 128 / m->D);  // small molecules: several queries per CTA
     const size_t fd_bytes = sizeof(double) * (size_t)m->D * QPB;
-    if (fd_bytes > 48 * 1024 && W_dev == nullptr)  // molecules above 111 atoms: opt in to more than the default dynamic shared memory
-      SG_CUDA(cudaFuncSetAttribute(k_predict_finish, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fd_bytes));
     const int parts = std::max(1, std::min(8, 1024 / m->D));
     const size_t fds_bytes = sizeof(double) * (size_t)m->D * (parts + 1);
-    // the virial variants add up to 1.5 KB of static shared memory, which counts against the 48 KB default: they opt
-    // in a little earlier, so that they take exactly the plain kernels' routes
-    if (W_dev != nullptr && fd_bytes > 46 * 1024)
-      SG_CUDA(cudaFuncSetAttribute(k_predict_finish_w, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fd_bytes));
-    if (W_dev != nullptr && fds_bytes > 46 * 1024 && fds_bytes <= 48 * 1024)
-      SG_CUDA(cudaFuncSetAttribute(k_predict_finish_small_w, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fds_bytes));
     if (n_geo <= GRAPH_MAX_GEO && n_splits > 1 && parts > 1 && fds_bytes <= 48 * 1024) {
       // a few queries, the sweep over the training points split across CTAs: the latency form
-      if (W_dev != nullptr)
-        k_predict_finish_small_w<<<(unsigned)n_geo, 1024, fds_bytes, s>>>(w.G, w.Erow, gq, m->perm, m->N, m->D, m->DP,
-                                                                         m->S, std, c, n_splits, n_rows_pad, parts,
-                                                                         E_dev, F_dev, W_dev);
-      else
-        k_predict_finish_small<<<(unsigned)n_geo, 1024, fds_bytes, s>>>(w.G, w.Erow, gq, m->perm, m->N, m->D, m->DP, m->S, std, c,
-                                                                       n_splits, n_rows_pad, parts, E_dev, F_dev);
-    } else if (W_dev != nullptr) {
-      k_predict_finish_w<<<(unsigned)((n_geo + QPB - 1) / QPB), 128, fd_bytes, s>>>(
+      SG_TRY(opt_in_smem<k_predict_finish_small<WITH_W>>(fds_bytes));
+      k_predict_finish_small<WITH_W><<<(unsigned)n_geo, 1024, fds_bytes, s>>>(
+          w.G, w.Erow, gq, m->perm, m->N, m->D, m->DP, m->S, std, c, n_splits, n_rows_pad, parts, E_dev, F_dev, W_dev);
+    } else {
+      SG_TRY(opt_in_smem<k_predict_finish<WITH_W>>(fd_bytes));  // molecules above 111 atoms
+      k_predict_finish<WITH_W><<<(unsigned)((n_geo + QPB - 1) / QPB), 128, fd_bytes, s>>>(
           w.G, w.Erow, gq, m->perm, m->N, m->D, m->DP, m->S, std, c, n_splits, n_rows_pad, n_geo, QPB, E_dev, F_dev,
           W_dev);
-    } else {
-      k_predict_finish<<<(unsigned)((n_geo + QPB - 1) / QPB), 128, fd_bytes, s>>>(w.G, w.Erow, gq, m->perm, m->N, m->D,
-                                                                                 m->DP, m->S, std, c, n_splits,
-                                                                                 n_rows_pad, n_geo, QPB, E_dev, F_dev);
     }
     SG_CUDA(cudaGetLastError());
     count_launch(KID_PREDICT_AUX);
-  }
-  return 0;
+    return 0;
+  };
+  return W_dev != nullptr ? finish(std::true_type()) : finish(std::false_type());
+}
+
+// The contraction setting a large-descriptor model takes for a requested slice count: at most 7 slices; FP64 (0) for
+// fewer than 2, or where DS or Mpad exceed the 2^14 the int8-slice path takes
+int contraction_slices(const sgdml_b200_model* m, int slices) {
+  slices = std::min(7, slices);
+  return slices >= 2 && m->DS <= (1 << 14) && m->Mpad <= (1 << 14) ? slices : 0;
 }
 
 int refresh_transposes(sgdml_b200_model* m, bool with_x, cudaStream_t s) {
@@ -1919,8 +1866,7 @@ int sgdml_b200_model_create(sgdml_b200_model** out, int64_t n_atoms, int64_t n_t
       SG_CUDA(cached_malloc(&m->JAT, sizeof(double) * (size_t)m->DP * m->Mpad));
       SG_TRY(refresh_transposes(m, true, s));
       const char* ozp = getenv("SGDML_B200_OZAKI_PREDICT_SLICES");
-      const int oz_s = (ozp != nullptr) ? std::max(0, std::min(7, atoi(ozp))) : 0;
-      if (oz_s >= 2 && m->DS <= (1 << 14) && m->Mpad <= (1 << 14)) m->oz_s = oz_s;
+      if (ozp != nullptr) m->oz_s = contraction_slices(m, atoi(ozp));
       SG_TRY(refresh_oz_model(m, true, s));
     }
     SG_CUDA(cudaStreamSynchronize(s));
@@ -1993,11 +1939,7 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
     if (zero_copy) {
       const int64_t n_rows = n_geo * m->S;
       const int64_t n_rows_pad = (n_rows + m->BQ - 1) / m->BQ * m->BQ;
-      // the kernel's static shared memory (its Lattice) counts against the 48 KB allowed without opt-in
-      cudaFuncAttributes fa;
-      SG_CUDA(cudaFuncGetAttributes(&fa, k_desc_query_rows));
-      if (dq_bytes + fa.sharedSizeBytes > 48 * 1024)
-        SG_CUDA(cudaFuncSetAttribute(k_desc_query_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_bytes));
+      SG_TRY(opt_in_smem<k_desc_query_rows>(dq_bytes));
       k_desc_query_rows<<<(unsigned)n_geo, 256, dq_bytes, gs>>>(q->hR, m->N, m->pinv, m->mu, m->D, m->DS, m->S, n_rows,
                                                                n_rows_pad, w.gq, w.Qg, w.qq, q->hLat);
       SG_CUDA(cudaGetLastError());
@@ -2038,30 +1980,7 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
     SG_TRY(enqueue(g));
     SG_CUDA(cudaStreamSynchronize(gs));
     // ... then capture it
-    long long before = 0, after = 0;
-    for (int k = 0; k < KID_COUNT; ++k) {
-      int64_t ln = 0;
-      sgdml_b200_profile_get(k, nullptr, nullptr, &ln);
-      before += ln;
-    }
-    cudaGraph_t graph = nullptr;
-    SG_CUDA(cudaStreamBeginCapture(gs, cudaStreamCaptureModeThreadLocal));
-    int rc = enqueue(g);
-    cudaError_t e = cudaStreamEndCapture(gs, &graph);
-    if (rc != 0) {
-      if (graph) cudaGraphDestroy(graph);
-      return rc;
-    }
-    SG_CUDA(e);
-    e = cudaGraphInstantiate(&g->exec, graph, 0);
-    cudaGraphDestroy(graph);
-    SG_CUDA(e);
-    for (int k = 0; k < KID_COUNT; ++k) {
-      int64_t ln = 0;
-      sgdml_b200_profile_get(k, nullptr, nullptr, &ln);
-      after += ln;
-    }
-    g->n_kernels = (int)(after - before);
+    SG_TRY(capture_graph(gs, [&] { return enqueue(g); }, &g->exec, &g->n_kernels));
     g->n_geo = n_geo;
     g->with_E = with_E;
     g->with_W = with_W;
@@ -2079,18 +1998,34 @@ int predict_graph(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lat
   return 0;
 }
 
+// An output of k doubles per geometry, written chunk by chunk: into the caller's array where it is device memory, else
+// into a staging buffer of the chunk's workspace and copied back to the caller's host array
+struct ChunkOut {
+  double* p;  // the caller's array, or nullptr (no such output)
+  int64_t k;
+  bool dev;
+  ChunkOut(double* p_, int64_t k_) : p(p_), k(k_), dev(p_ != nullptr && is_device_ptr(p_)) {}
+  bool staged() const { return p != nullptr && !dev; }
+  // where the kernels write the chunk at geometry g0
+  double* at(int64_t g0, double* staging) const { return p == nullptr ? nullptr : dev ? p + g0 * k : staging; }
+  // queues the copy of a staged chunk of ng geometries back to the host
+  int copy_back(int64_t g0, int64_t ng, const double* staging, cudaStream_t s) const {
+    if (staged()) SG_CUDA(cudaMemcpyAsync(p + g0 * k, staging, sizeof(double) * ng * k, cudaMemcpyDeviceToHost, s));
+    return 0;
+  }
+};
+
 // Every prediction of new geometries.  cells: n_cells HOST cells, 1 (every geometry in cells[0]) or n_geo (geometry g
 // in cells[g]); a free molecule's cell has on = 0.  W == nullptr: no virial (the plain finishing kernels).  On the
 // chunked path one cell goes to the descriptor kernel by value, and one cell per geometry goes to the device on the
 // chunk's stream next to its geometries.
 int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Lattice* cells, int64_t n_cells,
                  double* E, double* F, double* W, cudaStream_t s) {
-  const bool R_dev = is_device_ptr(R), F_dev = is_device_ptr(F), E_dev = (E != nullptr) && is_device_ptr(E);
-  const bool W_dev = (W != nullptr) && is_device_ptr(W);
-  const bool host_io = !R_dev || !F_dev || (E != nullptr && !E_dev) || (W != nullptr && !W_dev);
   const int dimi = 3 * m->N;
-  if (!R_dev && !F_dev && (E == nullptr || !E_dev) && (W == nullptr || !W_dev) && n_geo <= GRAPH_MAX_GEO &&
-      !profiling_enabled() && g_graph_enabled())
+  const bool R_dev = is_device_ptr(R);
+  const ChunkOut oF(F, dimi), oE(E, 1), oW(W, 9);
+  const bool host_io = !R_dev || oF.staged() || oE.staged() || oW.staged();
+  if (!R_dev && !oF.dev && !oE.dev && !oW.dev && n_geo <= GRAPH_MAX_GEO && !profiling_enabled() && g_graph_enabled())
     return predict_graph(m, R, n_geo, cells, n_cells, E, F, W, s);
   int64_t chunk = std::min<int64_t>(chunk_geos(m), n_geo);
   // Host buffers: split the batch into >= 4 chunks and run them on two side streams so that the
@@ -2122,13 +2057,10 @@ int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Latt
       lats = w.lat;
     }
     SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, st, cells[0], lats));
-    double* Fd = F_dev ? F + g0 * dimi : w.F;
-    double* Ed = (E == nullptr) ? nullptr : (E_dev ? E + g0 : w.E);
-    double* Wd = (W == nullptr) ? nullptr : (W_dev ? W + g0 * 9 : w.W);
-    SG_TRY(run_queries(m, w, w.xq, w.gq, ng, m->std, m->c, Ed, Fd, st, Wd));
-    if (!F_dev) SG_CUDA(cudaMemcpyAsync(F + g0 * dimi, Fd, sizeof(double) * ng * dimi, cudaMemcpyDeviceToHost, st));
-    if (E != nullptr && !E_dev) SG_CUDA(cudaMemcpyAsync(E + g0, Ed, sizeof(double) * ng, cudaMemcpyDeviceToHost, st));
-    if (W != nullptr && !W_dev) SG_CUDA(cudaMemcpyAsync(W + g0 * 9, Wd, sizeof(double) * ng * 9, cudaMemcpyDeviceToHost, st));
+    SG_TRY(run_queries(m, w, w.xq, w.gq, ng, m->std, m->c, oE.at(g0, w.E), oF.at(g0, w.F), st, oW.at(g0, w.W)));
+    SG_TRY(oF.copy_back(g0, ng, w.F, st));
+    SG_TRY(oE.copy_back(g0, ng, w.E, st));
+    SG_TRY(oW.copy_back(g0, ng, w.W, st));
   }
   if (pipelined) {
     for (int i = 0; i < 2; ++i) {
@@ -2168,23 +2100,18 @@ int predict_train_impl(sgdml_b200_model* m, int64_t m_begin, int64_t m_end, int 
   const int64_t chunk = std::min<int64_t>(chunk_geos(m), n_geo);
   SG_TRY(ensure_ws(m, 0, chunk));
   sgdml_b200_model::WS& w = m->ws[0];
-  const bool F_dev = is_device_ptr(F), E_dev = (E != nullptr) && is_device_ptr(E);
-  const bool W_dev = (W != nullptr) && is_device_ptr(W);
-  const int dimi = 3 * m->N;
+  const ChunkOut oF(F, 3 * m->N), oE(E, 1), oW(W, 9);
   const double std = scaled ? m->std : 1.0, c = scaled ? m->c : 0.0;
   for (int64_t g0 = 0; g0 < n_geo; g0 += chunk) {
     const int64_t ng = std::min<int64_t>(chunk, n_geo - g0);
     const double* xq = m->X + (m_begin + g0) * m->D;
     const double* gq = m->R_d_desc + (m_begin + g0) * m->D * 3;
-    double* Fd = F_dev ? F + g0 * dimi : w.F;
-    double* Ed = (E == nullptr) ? nullptr : (E_dev ? E + g0 : w.E);
-    double* Wd = (W == nullptr) ? nullptr : (W_dev ? W + g0 * 9 : w.W);
-    SG_TRY(run_queries(m, w, xq, gq, ng, std, c, Ed, Fd, s, Wd));
-    if (!F_dev) SG_CUDA(cudaMemcpyAsync(F + g0 * dimi, Fd, sizeof(double) * ng * dimi, cudaMemcpyDeviceToHost, s));
-    if (E != nullptr && !E_dev) SG_CUDA(cudaMemcpyAsync(E + g0, Ed, sizeof(double) * ng, cudaMemcpyDeviceToHost, s));
-    if (W != nullptr && !W_dev) SG_CUDA(cudaMemcpyAsync(W + g0 * 9, Wd, sizeof(double) * ng * 9, cudaMemcpyDeviceToHost, s));
+    SG_TRY(run_queries(m, w, xq, gq, ng, std, c, oE.at(g0, w.E), oF.at(g0, w.F), s, oW.at(g0, w.W)));
+    SG_TRY(oF.copy_back(g0, ng, w.F, s));
+    SG_TRY(oE.copy_back(g0, ng, w.E, s));
+    SG_TRY(oW.copy_back(g0, ng, w.W, s));
   }
-  if (!F_dev || (E != nullptr && !E_dev) || (W != nullptr && !W_dev)) SG_CUDA(cudaStreamSynchronize(s));
+  if (oF.staged() || oE.staged() || oW.staged()) SG_CUDA(cudaStreamSynchronize(s));
   return 0;
 }
 
@@ -2241,16 +2168,13 @@ int ensure_hvp_ws(sgdml_b200_model* m, int64_t n_geo, cudaStream_t s) {
 // sgdml_b200_predict_hvp: always the GEMM-composed form in FP64 (the int8-slice setting of large descriptors does not
 // apply), in the model's cell, chunk by chunk on the caller's stream
 int hvp_impl(sgdml_b200_model* m, const double* R, const double* V, int64_t n_geo, double* HV, cudaStream_t s) {
-  const bool R_dev = is_device_ptr(R), V_dev = is_device_ptr(V), HV_dev = is_device_ptr(HV);
+  const bool R_dev = is_device_ptr(R), V_dev = is_device_ptr(V);
   const int dimi = 3 * m->N;
+  const ChunkOut oHV(HV, dimi);
   const int64_t chunk = std::min<int64_t>(hvp_chunk_geos(m), n_geo);
   SG_TRY(ensure_hvp_ws(m, chunk, s));
   sgdml_b200_model::HvpWS& w = m->hvp;
-  MaternK mk;
-  mk.sig = m->sig;
-  mk.sig_inv = 1.0 / m->sig;
-  mk.k_base = 5.0 / (3.0 * m->sig * m->sig * m->sig);
-  mk.k_c1 = mk.k_base * 5.0 / m->sig;
+  const MaternK mk = MaternK::from_sig(m->sig);
   for (int64_t g0 = 0; g0 < n_geo; g0 += chunk) {
     const int64_t ng = std::min<int64_t>(chunk, n_geo - g0);
     const int64_t rows = ng * m->S;
@@ -2264,7 +2188,6 @@ int hvp_impl(sgdml_b200_model* m, const double* R, const double* V, int64_t n_ge
       SG_CUDA(cudaMemcpyAsync(w.V, Vd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, s));
       Vd = w.V;
     }
-    double* HVd = HV_dev ? HV + g0 * dimi : w.HV;
     SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, s, m->lat, nullptr));
     SG_TRY(launch_d_desc_dot_vec(w.gq, Vd, ng, m->N, w.t, m->D, s));
     {
@@ -2279,44 +2202,13 @@ int hvp_impl(sgdml_b200_model* m, const double* R, const double* V, int64_t n_ge
     }
     {
       ProfScope ps(KID_PREDICT_MAIN, s);
-      GemmArgs g;
-      g.alpha = 1.0;
-      g.beta = 0.0;
-      g.mode = 0;
-      g.tri = 0;
-      g.abort_flag = nullptr;
-      // [S1; S3] = [Q; T] Xc^T, [S2; S4] = [Q; T] JA^T   (2 rows x Mpad, contraction over the padded descriptor)
-      g.m = 2 * rows;
-      g.n = m->Mpad;
-      g.k = m->DS;
-      g.A = w.Qg;
-      g.lda = m->DS;
-      g.ldb = m->DS;
-      g.ldc = m->Mpad;
-      g.B = m->Xc;
-      g.C = w.SX;
-      SG_TRY(launch_gemm(g, s));
-      g.B = m->JA;
-      g.C = w.SJ;
-      SG_TRY(launch_gemm(g, s));
+      // [S1; S3] = [Q; T] Xc^T, [S2; S4] = [Q; T] JA^T, then acc = [C1; dC1] XcT^T + [C2; dC2] JAT^T
+      SG_TRY(contract_desc(m, w.Qg, 2 * rows, w.SX, w.SJ, s));
       k_transform_tangent_rows<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(
           w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, m->use_ae ? m->ae : nullptr, m->M, m->Mpad, rows, mk,
           w.csum);
       SG_CUDA(cudaGetLastError());
-      // acc = [C1; dC1] XcT^T + [C2; dC2] JAT^T   (2 rows x DP, contraction over the training points)
-      g.n = m->DP;
-      g.k = m->Mpad;
-      g.lda = m->Mpad;
-      g.ldb = m->Mpad;
-      g.ldc = m->DP;
-      g.A = w.SX;
-      g.B = m->XcT;
-      g.C = w.G;
-      SG_TRY(launch_gemm(g, s));
-      g.mode = 1;
-      g.A = w.SJ;
-      g.B = m->JAT;
-      SG_TRY(launch_gemm(g, s));
+      SG_TRY(contract_points(m, w.SX, w.SJ, 2 * rows, w.G, s));
       k_combine_tangent_rows<<<(unsigned)((rows * m->DP + 255) / 256), 256, 0, s>>>(w.Qg, m->DS, w.csum, w.G, m->DP,
                                                                                      rows);
       SG_CUDA(cudaGetLastError());
@@ -2325,18 +2217,19 @@ int hvp_impl(sgdml_b200_model* m, const double* R, const double* V, int64_t n_ge
     {
       ProfScope ps(KID_PREDICT_FINISH, s);
       const dim3 grid((unsigned)ceil_div(m->D, 256), (unsigned)std::min<int64_t>(ng, 65535));
-      k_fdesc_gather<<<grid, 256, 0, s>>>(w.G, m->perm, m->D, m->DP, m->S, 1, rows, ng, w.Fd);
+      k_fdesc_gather<false><<<grid, 256, 0, s>>>(w.G, m->perm, m->D, m->DP, m->S, 1, rows, ng, w.Fd, nullptr, nullptr);
       SG_CUDA(cudaGetLastError());
-      k_fdesc_gather<<<grid, 256, 0, s>>>(w.G + rows * m->DP, m->perm, m->D, m->DP, m->S, 1, rows, ng, w.dFd);
+      k_fdesc_gather<false><<<grid, 256, 0, s>>>(w.G + rows * m->DP, m->perm, m->D, m->DP, m->S, 1, rows, ng, w.dFd,
+                                                 nullptr, nullptr);
       SG_CUDA(cudaGetLastError());
       k_hvp_project<<<(unsigned)ceil_div(ng * m->N, 256), 256, 0, s>>>(w.Fd, w.dFd, w.gq, Vd, m->N, m->D, m->std, ng,
-                                                                       HVd);
+                                                                       oHV.at(g0, w.HV));
       SG_CUDA(cudaGetLastError());
       count_launch(KID_PREDICT_FINISH, 3);
     }
-    if (!HV_dev) SG_CUDA(cudaMemcpyAsync(HV + g0 * dimi, HVd, sizeof(double) * ng * dimi, cudaMemcpyDeviceToHost, s));
+    SG_TRY(oHV.copy_back(g0, ng, w.HV, s));
   }
-  if (!R_dev || !V_dev || !HV_dev) SG_CUDA(cudaStreamSynchronize(s));
+  if (!R_dev || !V_dev || oHV.staged()) SG_CUDA(cudaStreamSynchronize(s));
   return 0;
 }
 
@@ -2501,7 +2394,7 @@ int sgdml_b200_predict_train_virial(sgdml_b200_model* m, int64_t m_begin, int64_
 int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* m, int slices, void* stream) {
   SG_ARG(m != nullptr && (slices == 0 || (slices >= 2 && slices <= 7)));
   if (!m->large) return 0;  // D <= 256: the fused FP64 kernel, nothing to choose
-  if (slices >= 2 && !(m->DS <= (1 << 14) && m->Mpad <= (1 << 14))) slices = 0;
+  slices = contraction_slices(m, slices);
   if (slices == m->oz_s) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   free_ws(m);  // (synchronises) the per-batch workspaces carry slice buffers sized for the old setting
@@ -2672,30 +2565,7 @@ int md_graph(sgdml_b200_md* md, bool pimd, cudaStream_t s) {
   // the force evaluation once un-captured, into scratch outputs: sets the kernels' shared-memory attributes
   SG_TRY(md_forces(md, md->Fs, md->Es, md->gs));
   SG_CUDA(cudaStreamSynchronize(md->gs));
-  int64_t before = 0, after = 0;
-  for (int k = 0; k < KID_COUNT; ++k) {
-    int64_t ln = 0;
-    sgdml_b200_profile_get(k, nullptr, nullptr, &ln);
-    before += ln;
-  }
-  cudaGraph_t graph = nullptr;
-  SG_CUDA(cudaStreamBeginCapture(md->gs, cudaStreamCaptureModeThreadLocal));
-  const int rc = md_step(md, pimd, md->gs);
-  cudaError_t e = cudaStreamEndCapture(md->gs, &graph);
-  if (rc != 0) {
-    if (graph) cudaGraphDestroy(graph);
-    return rc;
-  }
-  SG_CUDA(e);
-  e = cudaGraphInstantiate(&md->exec, graph, 0);
-  cudaGraphDestroy(graph);
-  SG_CUDA(e);
-  for (int k = 0; k < KID_COUNT; ++k) {
-    int64_t ln = 0;
-    sgdml_b200_profile_get(k, nullptr, nullptr, &ln);
-    after += ln;
-  }
-  md->n_kernels = (int)(after - before);
+  SG_TRY(capture_graph(md->gs, [&] { return md_step(md, pimd, md->gs); }, &md->exec, &md->n_kernels));
   md->generation = m->generation;
   md->lat = m->lat;
   md->graph_pimd = pimd;

@@ -1,9 +1,9 @@
 """sgdml_b200_predict_virial / GDMLPredict.predict_virial on every finishing route against the oracle virial
 (tests/virial_checks.py) with the componentwise bound check_W, and E / F against `predict` bit for bit.
 
-Routes: k_predict_finish_w with QPB > 1 (D <= 40) and QPB = 1, k_predict_finish_small_w (graph-sized batches whose
-sweep over the training points is split), the GEMM-composed path (D > 256), the long-descriptor pair
-k_fdesc_gather_w / k_fdesc_project_w (N >= 227); batches through the zero-copy graph, the copy-node graph, plain
+Routes: k_predict_finish<true> with QPB > 1 (D <= 40) and QPB = 1, k_predict_finish_small<true> (graph-sized batches
+whose sweep over the training points is split), the GEMM-composed path (D > 256), the long-descriptor pair
+k_fdesc_gather<true> / k_fdesc_project<true> (N >= 227); batches through the zero-copy graph, the copy-node graph, plain
 launches, several chunks and the pipelined host path; NumPy, pinned and CUDA-tensor I/O.  Cells given per call travel
 with the geometries through the graph: a new cell replays the graph, which the launch counter of the main kernel shows
 (a replay counts none).  Output buffers are NaN-filled first."""
@@ -189,7 +189,7 @@ def test_virial_periodic_golden_pbc_n6_m8(eng, monkeypatch):
 
 
 def test_virial_long_descriptors_n240(eng):
-    """N = 240, M = 2 (D = 28 680): k_fdesc_gather_w / k_fdesc_project_w, graph and plain batches and CUDA tensors."""
+    """N = 240, M = 2 (D = 28 680): k_fdesc_gather<true> / k_fdesc_project<true>, graph and plain batches and CUDA tensors."""
     import torch
 
     g = load_golden('big_n240_m2_s3')

@@ -154,7 +154,7 @@ def test_cells_energy_constrained(eng, monkeypatch):
 
 
 def test_cells_long_descriptors_n240(eng, monkeypatch):
-    """N = 240, M = 2 (D = 28 680): the k_fdesc_gather_w / k_fdesc_project_w finishing pair with per-geometry cells."""
+    """N = 240, M = 2 (D = 28 680): the k_fdesc_gather<true> / k_fdesc_project<true> finishing pair with per-geometry cells."""
     g = load_golden('big_n240_m2_s3')
     N = int(g['n_atoms'])
     M = g['R_train'].shape[0]

@@ -222,6 +222,46 @@ int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT
                         double* E_pot_frames, double* E_kin_frames, double* K_prim_frames, double* K_cv_frames,
                         void* stream);
 
+/* ---------------------------------------------------------------- geometry optimisation on the device
+ * Extension: relax every replica of an sgdml_b200_md handle to a local minimum of the model's energy with FIRE or
+ * L-BFGS, many steps per call and no host round trip per step.  The handle needs a state (sgdml_b200_md_set_state);
+ * its inverse masses are not read.  Beads of a ring-polymer handle are relaxed as independent replicas.  One step is
+ * the optimiser kernel (k_fire_step or k_lbfgs_step, one CTA per replica) followed by the forces of every replica,
+ * chunk by chunk, as in sgdml_b200_md_run: the handle's step graph with the optimiser as its integrator, captured again
+ * when the optimiser changes (SGDML_B200_GRAPH=0: plain launches, bit-identical).
+ * Convergence (ASE's criterion): max over atoms of Fx^2 + Fy^2 + Fz^2 < fmax^2, tested on the forces at the current
+ * positions before every step.  A replica that has converged is frozen: its positions never change again in this
+ * call.  fmax = 0 runs max_steps steps.  Replays run in blocks; after each block a kernel counts the unconverged
+ * replicas into mapped pinned memory and the call returns once none is left or max_steps steps have run.  The block
+ * length changes only the cost, never a result.
+ * Every call starts its optimiser afresh (as a new ASE optimiser would).  After it, R holds the final positions with F
+ * and E_pot evaluated there, V is zero (a following sgdml_b200_md_run starts at rest), and the step counter is
+ * unchanged (the Philox stream is untouched).  The stored F and E_pot are those of the last force evaluation, as for
+ * sgdml_b200_md_run: call sgdml_b200_md_set_state again after the model changes.
+ * Outputs, each host, device or NULL: n_steps_out (n_rep) int64, the position updates each replica took;
+ * converged_out (n_rep) int32, 1 if max_a |F_a| < fmax at the final positions; fmax_out (n_rep) double,
+ * max_a |F_a| there.  Calls with host outputs synchronise `stream`; every call waits for its convergence read-backs.
+ * Units are the model's: positions in L, forces as sgdml_b200_predict returns them.  The exact update of each
+ * optimiser, every sum's order and every rounding are stated in csrc/md.cuh; sums run in a fixed order, so results
+ * are reproducible bit for bit.  The optimiser state (for L-BFGS 2 m + 2 vectors of 3N doubles per replica) is made
+ * on the handle at the first relaxation, grown when a call asks for more memory, and freed with the handle.  Launches
+ * count under family 8 (optimiser, test, count) and 1 (graph replays).  Argument errors are reported before anything
+ * is queued, and a rejected call changes nothing. */
+/* FIRE (Bitzek et al., PRL 97, 170201 (2006)) in ASE's mass-free form with its constants (Nmin 5, finc 1.1, fdec 0.5,
+ * alpha_start 0.1, f_alpha 0.99): max_steps >= 0; fmax >= 0 (force unit); maxstep > 0 (L), the cap on |dr| of a
+ * replica's whole step; dt > 0 the initial and dtmax > 0 the largest time step, in sqrt(L^2 / force unit). */
+int sgdml_b200_relax_fire(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, double dt, double dtmax,
+                          int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream);
+/* L-BFGS (two-loop recursion, Nocedal & Wright Alg. 7.4) without line search: memory m in [1, 32] pairs; h0 > 0
+ * (L^2 / energy) the inverse Hessian guess while the history is empty, afterwards s.y / y.y of the newest pair; a pair
+ * with s.y <= 0, an energy rise or a non-descent direction clears the history.  maxstep > 0 (L) caps the step of
+ * every atom (ASE's rule: the whole step is scaled so that its longest atom step is maxstep). */
+int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, int memory, double h0,
+                           int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream);
+/* Test hook: graph replays between convergence read-backs of sgdml_b200_relax_*; 0 = the default (16).  Negative
+ * values are rejected. */
+int sgdml_b200_set_relax_block(int64_t n_steps);
+
 /* Periodic model (predict.py:332-334: lat_and_inv from model['lattice']): query descriptors of
  * sgdml_b200_predict are built with the minimum-image convention.  Both NULL: back to a free molecule. */
 int sgdml_b200_model_set_lattice(sgdml_b200_model* model, const double* lattice, const double* lattice_inv);

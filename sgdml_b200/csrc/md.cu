@@ -317,6 +317,239 @@ __global__ void __launch_bounds__(MD_THREADS) k_pimd_step(const PimdParams* __re
   if (tid < nb) step[rep0 + tid] = n + 1;  // every thread read the counter before the first barrier
 }
 
+// ---------------------------------------------------------------------------------- geometry optimisation
+// The FIRE and L-BFGS steps of sgdml_b200_relax_* (driver: relax_impl in predict.cu); the exact sums and updates are
+// in md.cuh.  Every thread holds the replica's RelaxState and every CTA-wide sum, so branches on them are uniform;
+// thread 0 writes the state back at the end.  Each thread updates only its own coordinates, except where the per-atom
+// maximum reads three of them (a barrier precedes it).
+
+constexpr double FIRE_FINC = 1.1, FIRE_FDEC = 0.5, FIRE_ALPHA0 = 0.1, FIRE_FALPHA = 0.99;
+constexpr int FIRE_NMIN = 5;
+
+// the maximum over the CTA, NaN if any thread holds NaN (max is exact: the order does not matter)
+__device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
+
+__device__ __forceinline__ double block_max(double x, double* red) {
+  red[threadIdx.x] = x;
+  __syncthreads();
+  for (int w = MD_THREADS / 2; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) red[threadIdx.x] = nan_max(red[threadIdx.x], red[threadIdx.x + w]);
+    __syncthreads();
+  }
+  const double r = red[0];
+  __syncthreads();
+  return r;
+}
+
+// max over atoms of |x_a|^2 = (x_a0^2 + x_a1^2) + x_a2^2 of one replica's (3N) vector
+__device__ __forceinline__ double atom_max2(const double* x, int dimi, double* red) {
+  double m = 0.0;
+  for (int a = threadIdx.x; 3 * a < dimi; a += MD_THREADS) {
+    const double* xa = x + 3 * a;
+    m = nan_max(m, __dadd_rn(__dadd_rn(__dmul_rn(xa[0], xa[0]), __dmul_rn(xa[1], xa[1])), __dmul_rn(xa[2], xa[2])));
+  }
+  return block_max(m, red);
+}
+
+// the convergence test on F at the current positions; true: the replica is frozen (now or earlier)
+__device__ __forceinline__ bool relax_test(RelaxState& z, const double* f, int dimi, double fmax2, double* red) {
+  if (z.conv) return true;
+  z.fmax2 = atom_max2(f, dimi, red);
+  z.conv = z.fmax2 < fmax2 ? 1 : 0;
+  return z.conv != 0;
+}
+
+__device__ __forceinline__ void relax_store(RelaxState* st, const RelaxState& z) {
+  __syncthreads();  // every thread has read the state
+  if (threadIdx.x == 0) *st = z;
+}
+
+__global__ void __launch_bounds__(MD_THREADS) k_fire_step(const RelaxParams* __restrict__ P, RelaxState* st,
+                                                         double* __restrict__ R, double* __restrict__ V,
+                                                         const double* __restrict__ F, int dimi, int advance) {
+  __shared__ double red[MD_THREADS];
+  const int64_t rep = blockIdx.x;
+  const RelaxParams p = *P;
+  RelaxState z = st[rep];
+  double* r = R + rep * dimi;
+  double* v = V + rep * dimi;
+  const double* f = F + rep * dimi;
+  if (relax_test(z, f, dimi, p.fmax2, red) || !advance) return relax_store(st + rep, z);
+
+  if (z.n_steps == 0) {  // ASE's first step: no mixing, dt kept
+    z.dt = p.dt0;
+    z.alpha = FIRE_ALPHA0;
+    z.n_pos = 0;
+  } else {
+    double fv = 0.0;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) fv = __dadd_rn(fv, __dmul_rn(f[i], v[i]));
+    fv = block_sum(fv, red);
+    if (fv > 0.0) {
+      double vv = 0.0, ff = 0.0;
+      for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+        vv = __dadd_rn(vv, __dmul_rn(v[i], v[i]));
+        ff = __dadd_rn(ff, __dmul_rn(f[i], f[i]));
+      }
+      vv = block_sum(vv, red);
+      ff = block_sum(ff, red);
+      const double c = __dmul_rn(z.alpha, __ddiv_rn(sqrt(vv), sqrt(ff)));
+      const double om = __dsub_rn(1.0, z.alpha);
+      for (int i = threadIdx.x; i < dimi; i += MD_THREADS) v[i] = __dadd_rn(__dmul_rn(om, v[i]), __dmul_rn(c, f[i]));
+      if (z.n_pos > FIRE_NMIN) {
+        z.dt = fmin(__dmul_rn(z.dt, FIRE_FINC), p.dtmax);
+        z.alpha = __dmul_rn(z.alpha, FIRE_FALPHA);
+      }
+      ++z.n_pos;
+    } else {
+      for (int i = threadIdx.x; i < dimi; i += MD_THREADS) v[i] = 0.0;
+      z.alpha = FIRE_ALPHA0;
+      z.dt = __dmul_rn(z.dt, FIRE_FDEC);
+      z.n_pos = 0;
+    }
+  }
+  double nn = 0.0;
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+    const double vi = __dadd_rn(v[i], __dmul_rn(z.dt, f[i]));
+    v[i] = vi;
+    const double dr = __dmul_rn(z.dt, vi);
+    nn = __dadd_rn(nn, __dmul_rn(dr, dr));
+  }
+  const double nrm = sqrt(block_sum(nn, red));
+  const bool cap = nrm > p.maxstep;
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+    double dr = __dmul_rn(z.dt, v[i]);
+    if (cap) dr = __ddiv_rn(__dmul_rn(p.maxstep, dr), nrm);
+    r[i] = __dadd_rn(r[i], dr);
+  }
+  ++z.n_steps;
+  relax_store(st + rep, z);
+}
+
+__global__ void __launch_bounds__(MD_THREADS) k_lbfgs_step(const RelaxParams* __restrict__ P, RelaxState* st,
+                                                          double* __restrict__ R, double* __restrict__ D,
+                                                          const double* __restrict__ F,
+                                                          const double* __restrict__ E, int dimi, int advance) {
+  __shared__ double red[MD_THREADS];
+  __shared__ double sa[LBFGS_MAX_MEMORY];  // a_k of the first loop, k = 0 the newest pair
+  const int64_t rep = blockIdx.x;
+  const RelaxParams p = *P;
+  RelaxState z = st[rep];
+  double* r = R + rep * dimi;
+  double* d = D + rep * dimi;
+  const double* f = F + rep * dimi;
+  if (relax_test(z, f, dimi, p.fmax2, red) || !advance) return relax_store(st + rep, z);
+
+  const int m = p.memory;
+  double* S = p.S + rep * p.m_cap * dimi;
+  double* Y = p.Y + rep * p.m_cap * dimi;
+  double* rho = p.rho + rep * p.m_cap;
+  double* rp = p.r_prev + rep * dimi;
+  double* gp = p.g_prev + rep * dimi;
+  const double e = E[rep];
+  if (z.n_steps != 0) {
+    // the new pair goes into the slot after the newest; if it is rejected the history is cleared anyway
+    const int slot = (z.head + 1) % m;
+    double* sk = S + (int64_t)slot * dimi;
+    double* yk = Y + (int64_t)slot * dimi;
+    double sy = 0.0, yy = 0.0;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+      const double si = __dsub_rn(r[i], rp[i]), yi = __dsub_rn(-f[i], gp[i]);
+      sk[i] = si;
+      yk[i] = yi;
+      sy = __dadd_rn(sy, __dmul_rn(si, yi));
+      yy = __dadd_rn(yy, __dmul_rn(yi, yi));
+    }
+    sy = block_sum(sy, red);
+    yy = block_sum(yy, red);
+    if (sy > 0.0) {
+      z.head = slot;
+      z.n_hist = min(z.n_hist + 1, m);
+      z.gamma = __ddiv_rn(sy, yy);
+      if (threadIdx.x == 0) rho[slot] = __ddiv_rn(1.0, sy);
+    } else {
+      z.n_hist = 0;
+    }
+    if (e > z.E_prev) z.n_hist = 0;
+    __syncthreads();  // rho[slot] is stored before any thread reads it
+  }
+  // two-loop recursion on d, which holds q, then z, then the direction
+  const int nh = z.n_hist;
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) d[i] = -f[i];
+  for (int k = 0; k < nh; ++k) {
+    const int sl = (z.head - k + m) % m;
+    const double* sk = S + (int64_t)sl * dimi;
+    const double* yk = Y + (int64_t)sl * dimi;
+    double t = 0.0;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) t = __dadd_rn(t, __dmul_rn(sk[i], d[i]));
+    t = block_sum(t, red);  // a statement of its own: rho[sl] is read after its barriers
+    const double a = __dmul_rn(rho[sl], t);
+    if (threadIdx.x == 0) sa[k] = a;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) d[i] = __dsub_rn(d[i], __dmul_rn(a, yk[i]));
+  }
+  const double gam = nh > 0 ? z.gamma : p.h0;
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) d[i] = __dmul_rn(gam, d[i]);
+  for (int k = nh - 1; k >= 0; --k) {
+    const int sl = (z.head - k + m) % m;
+    const double* sk = S + (int64_t)sl * dimi;
+    const double* yk = Y + (int64_t)sl * dimi;
+    double t = 0.0;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) t = __dadd_rn(t, __dmul_rn(yk[i], d[i]));
+    t = block_sum(t, red);
+    const double b = __dmul_rn(rho[sl], t);
+    const double c = __dsub_rn(sa[k], b);
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) d[i] = __dadd_rn(d[i], __dmul_rn(sk[i], c));
+  }
+  double dg = 0.0;
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+    const double di = -d[i];
+    d[i] = di;
+    dg = __dadd_rn(dg, __dmul_rn(di, -f[i]));
+  }
+  dg = block_sum(dg, red);
+  if (!(dg < 0.0)) {  // not a descent direction: steepest descent from a fresh history
+    z.n_hist = 0;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) d[i] = __dmul_rn(p.h0, f[i]);
+  }
+  __syncthreads();  // d is complete: the per-atom maximum reads other threads' coordinates
+  const double L = sqrt(atom_max2(d, dimi, red));
+  const bool cap = L > p.maxstep;
+  const double sc = __ddiv_rn(p.maxstep, L);
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+    double di = d[i];
+    if (cap) di = __dmul_rn(di, sc);
+    const double ri = r[i];
+    rp[i] = ri;
+    gp[i] = -f[i];
+    r[i] = __dadd_rn(ri, di);
+  }
+  z.E_prev = e;
+  ++z.n_steps;
+  relax_store(st + rep, z);
+}
+
+__global__ void __launch_bounds__(MD_THREADS) k_relax_count(const RelaxState* __restrict__ st, int64_t n_rep,
+                                                           int* n_active) {
+  __shared__ int red[MD_THREADS];
+  int c = 0;
+  for (int64_t r = threadIdx.x; r < n_rep; r += MD_THREADS) c += st[r].conv == 0;
+  red[threadIdx.x] = c;
+  __syncthreads();
+  for (int w = MD_THREADS / 2; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *n_active = red[0];
+}
+
+__global__ void k_relax_report(const RelaxState* __restrict__ st, int64_t n_rep, int64_t* n_steps, int* conv,
+                               double* fmax) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rep) return;
+  if (n_steps) n_steps[r] = st[r].n_steps;
+  if (conv) conv[r] = st[r].conv;
+  if (fmax) fmax[r] = sqrt(st[r].fmax2);
+}
+
 }  // namespace
 
 int launch_md_step(const MdParams* P, const double* s, const double* sigma, double* R, double* V, const double* F,
@@ -332,6 +565,37 @@ int launch_pimd_step(const PimdParams* P, const double* tab, const double* s, co
                      cudaStream_t st) {
   if (nb < 1 || nb > PIMD_MAX_BEADS) return fail_arg("launch_pimd_step: n_beads outside [1, PIMD_MAX_BEADS]");
   k_pimd_step<<<(unsigned)n_poly, MD_THREADS, 0, st>>>(P, tab, s, sigma, R, V, F, E, step, dimi, nb, advance);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_MISC);
+  return 0;
+}
+
+int launch_fire_step(const RelaxParams* P, RelaxState* st, double* R, double* V, const double* F, int64_t n_rep,
+                     int dimi, int advance, cudaStream_t s) {
+  k_fire_step<<<(unsigned)n_rep, MD_THREADS, 0, s>>>(P, st, R, V, F, dimi, advance);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_MISC);
+  return 0;
+}
+
+int launch_lbfgs_step(const RelaxParams* P, RelaxState* st, double* R, double* D, const double* F, const double* E,
+                      int64_t n_rep, int dimi, int advance, cudaStream_t s) {
+  k_lbfgs_step<<<(unsigned)n_rep, MD_THREADS, 0, s>>>(P, st, R, D, F, E, dimi, advance);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_MISC);
+  return 0;
+}
+
+int launch_relax_count(const RelaxState* st, int64_t n_rep, int* n_active, cudaStream_t s) {
+  k_relax_count<<<1, MD_THREADS, 0, s>>>(st, n_rep, n_active);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_MISC);
+  return 0;
+}
+
+int launch_relax_report(const RelaxState* st, int64_t n_rep, int64_t* n_steps, int* conv, double* fmax,
+                        cudaStream_t s) {
+  k_relax_report<<<(unsigned)((n_rep + 255) / 256), 256, 0, s>>>(st, n_rep, n_steps, conv, fmax);
   SG_CUDA(cudaGetLastError());
   count_launch(KID_MISC);
   return 0;

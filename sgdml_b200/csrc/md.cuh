@@ -55,4 +55,70 @@ int launch_pimd_step(const PimdParams* P, const double* tab, const double* s, co
                      const double* F, const double* E, uint64_t* step, int64_t n_poly, int dimi, int nb, int advance,
                      cudaStream_t st);
 
+// Geometry optimisation (sgdml_b200_relax_fire, sgdml_b200_relax_lbfgs): one CTA of MD_THREADS per replica.
+//
+// Sums.  Every dot product x.y and squared norm of a replica is block_sum's: thread t adds the products x_i y_i of its
+// coordinates i = t, t + MD_THREADS, ... in increasing i, starting from 0.0 (each product and each addition rounded),
+// then a tree over the MD_THREADS partials adds red[t] + red[t + w] for w = MD_THREADS / 2, ..., 1.  Per-atom maxima
+// (|F_a|^2 for convergence, |d_a|^2 for the L-BFGS step cap) take |x_a|^2 = (x_a0 x_a0 + x_a1 x_a1) + x_a2 x_a2,
+// rounded as written, and a NaN anywhere makes the maximum NaN.  Every update rounds as written: no fused
+// multiply-add, so tests/relax_oracle.py, fed the same forces, reproduces the kernels bit for bit.
+//
+// Convergence: max_a |F_a|^2 < fmax2 at the current positions (ASE's criterion).  Each step kernel tests first; a replica
+// that passes is frozen (its state and positions never change again in this call).  fmax2 = 0 never passes.
+constexpr int LBFGS_MAX_MEMORY = 32;
+
+// Per replica, zeroed at the start of every call: n_steps == 0 is the first step of the call.
+struct RelaxState {
+  double dt, alpha;     // FIRE: time step and mixing (set on the first step)
+  double gamma;         // L-BFGS: s.y / y.y of the newest pair
+  double E_prev;        // L-BFGS: the energy at r_prev
+  double fmax2;         // max_a |F_a|^2 at the last test
+  int64_t n_steps;      // position updates taken in this call
+  int n_pos;            // FIRE: steps with F.v > 0 since the last reset
+  int n_hist, head;     // L-BFGS: pairs in the ring and the slot of the newest
+  int conv;             // 1: converged and frozen
+};
+
+// Everything a call changes, read from device memory: the captured step graph bakes in none of it.
+struct RelaxParams {
+  double fmax2;         // fmax^2 (0: run every step)
+  double maxstep;       // FIRE: |dr| of the whole replica; L-BFGS: |d_a| of every atom
+  double dt0, dtmax;    // FIRE
+  double h0;            // L-BFGS: initial inverse Hessian when the history is empty
+  int memory;           // L-BFGS: m, 1 <= m <= LBFGS_MAX_MEMORY
+  int m_cap;            // L-BFGS: slots per replica in S, Y, rho (>= memory)
+  double *S, *Y;        // L-BFGS: (n_rep, m_cap, 3N) ring of s and y
+  double* rho;          // L-BFGS: (n_rep, m_cap) 1 / s.y
+  double *r_prev, *g_prev;  // L-BFGS: (n_rep, 3N) positions and -F of the previous step
+};
+
+// FIRE (Bitzek et al., PRL 97, 170201 (2006); ASE's mass-free form, Nmin 5, finc 1.1, fdec 0.5, alpha_start 0.1,
+// f_alpha 0.99) with velocities V (n_rep, 3N).  After the test, on every step but the first:
+//   P = F.v;  P > 0:  vv = v.v, ff = F.F, c = alpha (sqrt(vv) / sqrt(ff)), v = (1 - alpha) v + c F,
+//                     if n_pos > 5: dt = min(dt 1.1, dtmax), alpha = alpha 0.99;  n_pos += 1
+//             else:   v = 0, alpha = 0.1, dt = dt 0.5, n_pos = 0
+// then on every step (the first starts from dt = dt0, alpha = 0.1, n_pos = 0 and the V the driver zeroed):
+//   v = v + dt F,  dr = dt v,  |dr| = sqrt(dr.dr),  if |dr| > maxstep: dr = (maxstep dr) / |dr|,  r = r + dr.
+//
+// L-BFGS (Nocedal & Wright, Alg. 7.4) with g = -F, direction scratch D (n_rep, 3N).  On every step but the first:
+//   s = r - r_prev, y = g - g_prev into the slot after the newest;  sy = s.y, yy = y.y;
+//   sy > 0: push (rho = 1 / sy, gamma = sy / yy), the ring holding the newest min(n + 1, m);  else clear the history;
+//   E > E_prev: clear the history.
+// Then q = g; for pairs newest to oldest: a_k = rho_k (s_k.q), q = q - a_k y_k;  z = gamma q (h0 q with no history);
+// for pairs oldest to newest: b = rho_k (y_k.z), z = z + s_k (a_k - b);  d = -z.  If d.g >= 0 (or NaN): clear the
+// history and d = h0 F.  Cap: L = sqrt(max_a |d_a|^2), if L > maxstep: d = d (maxstep / L).  r_prev = r, g_prev = g,
+// E_prev = E, r = r + d.
+//
+// advance == 0 runs only the test (it sets conv and fmax2 for every replica).
+int launch_fire_step(const RelaxParams* P, RelaxState* st, double* R, double* V, const double* F, int64_t n_rep,
+                     int dimi, int advance, cudaStream_t s);
+int launch_lbfgs_step(const RelaxParams* P, RelaxState* st, double* R, double* D, const double* F, const double* E,
+                      int64_t n_rep, int dimi, int advance, cudaStream_t s);
+// the number of replicas not yet converged, written by the device into *n_active (host-mapped pinned memory)
+int launch_relax_count(const RelaxState* st, int64_t n_rep, int* n_active, cudaStream_t s);
+// n_steps (int64), conv (int32) and sqrt(fmax2) per replica, into device arrays; each may be null
+int launch_relax_report(const RelaxState* st, int64_t n_rep, int64_t* n_steps, int* conv, double* fmax,
+                        cudaStream_t s);
+
 }  // namespace sgdml

@@ -2471,10 +2471,20 @@ struct sgdml_b200_md {
   cudaStream_t gs = nullptr;  // capture stream
   cudaEvent_t ge = nullptr;
   cudaGraphExec_t exec = nullptr;
-  bool graph_pimd = false;    // the captured step runs k_pimd_step (sgdml_b200_pimd_run), not k_md_step
+  int graph_kind = -1;        // the MdKind of the captured step
   uint64_t generation = 0;    // the model's generation at capture
   Lattice lat = {0, {0}, {0}};  // the model's cell at capture (passed to the descriptor kernel by value)
   int n_kernels = 0;
+  // geometry optimisation (sgdml_b200_relax_*), allocated by the first relaxation
+  RelaxState* rst = nullptr;  // (n_rep) per-replica optimiser state
+  RelaxParams* dR = nullptr;
+  RelaxParams* hR = nullptr;  // pinned staging of dR
+  int* hActive = nullptr;     // mapped pinned: unconverged replicas, written by k_relax_count
+  int* dActive = nullptr;     // its device address
+  cudaEvent_t counted = nullptr;
+  double *S = nullptr, *Y = nullptr, *rho = nullptr;        // L-BFGS ring, m_cap pairs per replica
+  double *r_prev = nullptr, *g_prev = nullptr;              // (n_rep, 3N)
+  int m_cap = 0;
 };
 
 namespace {
@@ -2485,12 +2495,18 @@ void md_free(sgdml_b200_md* md) {
   if (md->gs) cudaStreamDestroy(md->gs);
   if (md->ge) cudaEventDestroy(md->ge);
   if (md->uploaded) cudaEventDestroy(md->uploaded);
+  if (md->counted) cudaEventDestroy(md->counted);
   free_ws_slot(md->ws);
   for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s, md->sigma}) cached_free(p);
   cached_free(md->step);
   cached_free(md->dP);
   cached_free(md->dQ);
   cached_free(md->tab);
+  for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev}) cached_free(p);
+  cached_free(md->rst);
+  cached_free(md->dR);
+  cudaFreeHost(md->hR);
+  cudaFreeHost(md->hActive);
   cudaFreeHost(md->hP);
   cudaFreeHost(md->hQ);
   cudaFreeHost(md->hTab);
@@ -2526,17 +2542,28 @@ int md_forces(sgdml_b200_md* md, double* F, double* E, cudaStream_t s) {
   return 0;
 }
 
-// the integrator of sgdml_b200_md_run or sgdml_b200_pimd_run; advance == 0 completes a run's last step
-int md_integrate(sgdml_b200_md* md, bool pimd, int advance, cudaStream_t s) {
-  if (pimd)
-    return launch_pimd_step(md->dQ, md->tab, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step,
-                            md->n_rep / md->nb, md->dimi, md->nb, advance, s);
-  return launch_md_step(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step, md->n_rep, md->dimi, advance,
-                        s);
+// what one step of the handle's graph integrates
+enum MdKind { MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3 };
+
+// the integrator of sgdml_b200_md_run, sgdml_b200_pimd_run or sgdml_b200_relax_*; advance == 0 completes a run's last
+// step (MD) or only tests convergence (relaxation).  L-BFGS keeps its direction in V, which relax_impl zeroes after.
+int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
+  switch (kind) {
+    case MD_RING_POLYMER:
+      return launch_pimd_step(md->dQ, md->tab, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step,
+                              md->n_rep / md->nb, md->dimi, md->nb, advance, s);
+    case MD_FIRE:
+      return launch_fire_step(md->dR, md->rst, md->R, md->V, md->F, md->n_rep, md->dimi, advance, s);
+    case MD_LBFGS:
+      return launch_lbfgs_step(md->dR, md->rst, md->R, md->V, md->F, md->E, md->n_rep, md->dimi, advance, s);
+    default:
+      return launch_md_step(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step, md->n_rep, md->dimi,
+                            advance, s);
+  }
 }
 
-int md_step(sgdml_b200_md* md, bool pimd, cudaStream_t s) {
-  SG_TRY(md_integrate(md, pimd, 1, s));
+int md_step(sgdml_b200_md* md, int kind, cudaStream_t s) {
+  SG_TRY(md_integrate(md, kind, 1, s));
   return md_forces(md, md->F, md->E, s);
 }
 
@@ -2546,10 +2573,10 @@ bool same_cell(const Lattice& a, const Lattice& b) {
 }
 
 // the step graph, captured again whenever something it bakes in has changed: the workspace (md_ready), the model's
-// generation (use_ae, contraction slices), the model's cell, or the integrator (classical or ring-polymer run)
-int md_graph(sgdml_b200_md* md, bool pimd, cudaStream_t s) {
+// generation (use_ae, contraction slices), the model's cell, or the integrator (MdKind)
+int md_graph(sgdml_b200_md* md, int kind, cudaStream_t s) {
   sgdml_b200_model* m = md->m;
-  if (md->exec != nullptr && md->generation == m->generation && same_cell(md->lat, m->lat) && md->graph_pimd == pimd)
+  if (md->exec != nullptr && md->generation == m->generation && same_cell(md->lat, m->lat) && md->graph_kind == kind)
     return 0;
   if (md->exec != nullptr) {
     cudaGraphExecDestroy(md->exec);
@@ -2565,10 +2592,10 @@ int md_graph(sgdml_b200_md* md, bool pimd, cudaStream_t s) {
   // the force evaluation once un-captured, into scratch outputs: sets the kernels' shared-memory attributes
   SG_TRY(md_forces(md, md->Fs, md->Es, md->gs));
   SG_CUDA(cudaStreamSynchronize(md->gs));
-  SG_TRY(capture_graph(md->gs, [&] { return md_step(md, pimd, md->gs); }, &md->exec, &md->n_kernels));
+  SG_TRY(capture_graph(md->gs, [&] { return md_step(md, kind, md->gs); }, &md->exec, &md->n_kernels));
   md->generation = m->generation;
   md->lat = m->lat;
-  md->graph_pimd = pimd;
+  md->graph_kind = kind;
   return 0;
 }
 
@@ -2597,19 +2624,25 @@ struct FrameOut {
 
 // n_steps steps after the run's parameters are queued: graph replays or plain launches, then the completing launch
 // and the copy of host-staged frames
-int md_steps(sgdml_b200_md* md, bool pimd, int64_t n_steps, FrameOut* out, int n_out, cudaStream_t s) {
+// n_steps steps of the handle's integrator: graph replays, or plain launches with SGDML_B200_GRAPH=0 or profiling
+int md_replay(sgdml_b200_md* md, int kind, int64_t n_steps, cudaStream_t s) {
   if (g_graph_enabled() && !profiling_enabled()) {
-    SG_TRY(md_graph(md, pimd, s));
+    SG_TRY(md_graph(md, kind, s));
     for (int64_t k = 0; k < n_steps; ++k) {
       SG_CUDA(cudaGraphLaunch(md->exec, s));
       count_launch(KID_PREDICT_AUX, md->n_kernels);  // the kernels of a replay are launches too
     }
   } else {
-    for (int64_t k = 0; k < n_steps; ++k) SG_TRY(md_step(md, pimd, s));
+    for (int64_t k = 0; k < n_steps; ++k) SG_TRY(md_step(md, kind, s));
   }
+  return 0;
+}
+
+int md_steps(sgdml_b200_md* md, int kind, int64_t n_steps, FrameOut* out, int n_out, cudaStream_t s) {
+  SG_TRY(md_replay(md, kind, n_steps, s));
   md->step_host += (uint64_t)n_steps;
   // the second half-kick of the last step (and its frame)
-  SG_TRY(md_integrate(md, pimd, 0, s));
+  SG_TRY(md_integrate(md, kind, 0, s));
   bool sync = false;
   for (int i = 0; i < n_out; ++i)
     if (out[i].staged) {
@@ -2650,7 +2683,7 @@ int md_run_impl(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, dou
   SG_CUDA(cudaMemcpyAsync(md->dP, md->hP, sizeof(MdParams), cudaMemcpyHostToDevice, s));
   SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * md->dimi, cudaMemcpyHostToDevice, s));
   SG_CUDA(cudaEventRecord(md->uploaded, s));
-  return md_steps(md, false, n_steps, out, 4, s);
+  return md_steps(md, MD_CLASSICAL, n_steps, out, 4, s);
 }
 
 int pimd_run_impl(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma, double lambda,
@@ -2728,7 +2761,120 @@ int pimd_run_impl(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, doub
   SG_CUDA(cudaMemcpyAsync(md->tab, md->hTab, sizeof(double) * (nb * nb + 4 * nb), cudaMemcpyHostToDevice, s));
   SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * nb * dimi, cudaMemcpyHostToDevice, s));
   SG_CUDA(cudaEventRecord(md->uploaded, s));
-  return md_steps(md, true, n_steps, out, 6, s);
+  return md_steps(md, MD_RING_POLYMER, n_steps, out, 6, s);
+}
+
+// ------------------------------------------------------------------ geometry optimisation (sgdml_b200_relax_*)
+constexpr int64_t RELAX_BLOCK = 16;  // replays between convergence read-backs
+int64_t g_relax_block = 0;           // sgdml_b200_set_relax_block (test hook): 0 = RELAX_BLOCK
+
+// the optimiser state, made at the first relaxation; the L-BFGS ring grows to `memory` pairs per replica
+int relax_alloc(sgdml_b200_md* md, int memory) {
+  if (md->rst == nullptr) SG_CUDA(cached_malloc(&md->rst, sizeof(RelaxState) * (size_t)md->n_rep));
+  if (md->dR == nullptr) SG_CUDA(cached_malloc(&md->dR, sizeof(RelaxParams)));
+  if (md->hR == nullptr) SG_CUDA(cudaMallocHost(&md->hR, sizeof(RelaxParams)));
+  if (md->hActive == nullptr) {
+    SG_CUDA(cudaHostAlloc(&md->hActive, sizeof(int), cudaHostAllocMapped));
+    SG_CUDA(cudaHostGetDevicePointer((void**)&md->dActive, md->hActive, 0));
+  }
+  if (md->counted == nullptr) SG_CUDA(cudaEventCreateWithFlags(&md->counted, cudaEventDisableTiming));
+  if (memory > md->m_cap) {
+    const size_t vec = sizeof(double) * (size_t)(md->n_rep * md->dimi);
+    SG_CUDA(cudaDeviceSynchronize());  // the old ring goes back to the cache: nothing may still use it
+    for (double** p : {&md->S, &md->Y, &md->rho}) {
+      cached_free(*p);
+      *p = nullptr;
+    }
+    md->m_cap = 0;
+    SG_CUDA(cached_malloc(&md->S, vec * memory));
+    SG_CUDA(cached_malloc(&md->Y, vec * memory));
+    SG_CUDA(cached_malloc(&md->rho, sizeof(double) * (size_t)md->n_rep * memory));
+    if (md->r_prev == nullptr) {
+      SG_CUDA(cached_malloc(&md->r_prev, vec));
+      SG_CUDA(cached_malloc(&md->g_prev, vec));
+    }
+    md->m_cap = memory;
+  }
+  return 0;
+}
+
+// Relaxes every replica from the handle's state: blocks of step-graph replays, each followed by the convergence test
+// and a count of unconverged replicas read back through mapped pinned memory; stops when none is left or after
+// max_steps.  Frozen replicas make the block length a matter of cost only.  V is zero before and after.
+int relax_impl(sgdml_b200_md* md, int kind, int64_t max_steps, const RelaxParams& prm, int64_t* n_steps_out,
+               int* conv_out, double* fmax_out, cudaStream_t s) {
+  const int64_t n_rep = md->n_rep;
+  SG_TRY(md_ready(md));
+  SG_TRY(relax_alloc(md, kind == MD_LBFGS ? prm.memory : 0));
+  // outputs: the caller's device arrays, or one device staging block for the host ones
+  void* user[3] = {n_steps_out, conv_out, fmax_out};
+  const size_t bytes[3] = {sizeof(int64_t) * (size_t)n_rep, sizeof(int) * (size_t)n_rep,
+                           sizeof(double) * (size_t)n_rep};
+  void* dev[3] = {nullptr, nullptr, nullptr};
+  char* stage = nullptr;
+  size_t staged = 0;
+  for (int i = 0; i < 3; ++i)
+    if (user[i] != nullptr && !is_device_ptr(user[i])) staged += (bytes[i] + 255) & ~(size_t)255;
+  if (staged > 0) SG_CUDA(cached_malloc(&stage, staged));
+  auto body = [&]() -> int {
+    size_t off = 0;
+    for (int i = 0; i < 3; ++i) {
+      if (user[i] == nullptr) continue;
+      if (is_device_ptr(user[i])) {
+        dev[i] = user[i];
+      } else {
+        dev[i] = stage + off;
+        off += (bytes[i] + 255) & ~(size_t)255;
+      }
+    }
+    SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the staging
+    RelaxParams& p = *md->hR;
+    p = prm;
+    p.m_cap = md->m_cap;
+    p.S = md->S;
+    p.Y = md->Y;
+    p.rho = md->rho;
+    p.r_prev = md->r_prev;
+    p.g_prev = md->g_prev;
+    SG_CUDA(cudaMemcpyAsync(md->dR, md->hR, sizeof(RelaxParams), cudaMemcpyHostToDevice, s));
+    SG_CUDA(cudaEventRecord(md->uploaded, s));
+    const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
+    SG_CUDA(cudaMemsetAsync(md->rst, 0, sizeof(RelaxState) * (size_t)n_rep, s));
+    SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
+    const int64_t block = g_relax_block > 0 ? g_relax_block : RELAX_BLOCK;
+    for (int64_t done = 0;;) {
+      SG_TRY(md_integrate(md, kind, 0, s));  // the test on the current forces
+      SG_TRY(launch_relax_count(md->rst, n_rep, md->dActive, s));
+      SG_CUDA(cudaEventRecord(md->counted, s));
+      SG_CUDA(cudaEventSynchronize(md->counted));
+      if (*(volatile int*)md->hActive == 0 || done >= max_steps) break;
+      const int64_t n = std::min(block, max_steps - done);
+      SG_TRY(md_replay(md, kind, n, s));
+      done += n;
+    }
+    SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));  // a following MD run starts at rest
+    SG_TRY(launch_relax_report(md->rst, n_rep, (int64_t*)dev[0], (int*)dev[1], (double*)dev[2], s));
+    for (int i = 0; i < 3; ++i)
+      if (dev[i] != nullptr && dev[i] != user[i])
+        SG_CUDA(cudaMemcpyAsync(user[i], dev[i], bytes[i], cudaMemcpyDeviceToHost, s));
+    if (staged > 0) SG_CUDA(cudaStreamSynchronize(s));
+    return 0;
+  };
+  const int rc = body();
+  if (stage != nullptr) {
+    if (rc != 0) cudaStreamSynchronize(s);
+    cached_free(stage);
+  }
+  return rc;
+}
+
+// the checks both optimisers share; a rejected call queues nothing
+int relax_check(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, const char* what) {
+  SG_ARG(md != nullptr && max_steps >= 0);
+  SG_ARG(std::isfinite(fmax) && fmax >= 0.0);
+  SG_ARG(std::isfinite(maxstep) && maxstep > 0.0);
+  if (!md->has_state) return fail_arg(what);
+  return 0;
 }
 
 // a handle of n_rep = n_poly nb replicas; the caller has checked the counts
@@ -2878,6 +3024,42 @@ int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT
   if (n_steps == 0) return 0;
   return pimd_run_impl(md, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, R_frames, V_frames, E_pot_frames,
                        E_kin_frames, K_prim_frames, K_cv_frames, (cudaStream_t)stream);
+}
+
+int sgdml_b200_relax_fire(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, double dt, double dtmax,
+                          int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(relax_check(md, max_steps, fmax, maxstep,
+                     "sgdml_b200_relax_fire: no state yet (call sgdml_b200_md_set_state)"));
+  SG_ARG(std::isfinite(dt) && dt > 0.0);
+  SG_ARG(std::isfinite(dtmax) && dtmax > 0.0);
+  RelaxParams p = {};
+  p.fmax2 = fmax * fmax;
+  p.maxstep = maxstep;
+  p.dt0 = dt;
+  p.dtmax = dtmax;
+  return relax_impl(md, MD_FIRE, max_steps, p, n_steps_out, converged_out, fmax_out, (cudaStream_t)stream);
+}
+
+int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, int memory, double h0,
+                           int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(relax_check(md, max_steps, fmax, maxstep,
+                     "sgdml_b200_relax_lbfgs: no state yet (call sgdml_b200_md_set_state)"));
+  SG_ARG(memory >= 1 && memory <= LBFGS_MAX_MEMORY);
+  SG_ARG(std::isfinite(h0) && h0 > 0.0);
+  RelaxParams p = {};
+  p.fmax2 = fmax * fmax;
+  p.maxstep = maxstep;
+  p.h0 = h0;
+  p.memory = memory;
+  return relax_impl(md, MD_LBFGS, max_steps, p, n_steps_out, converged_out, fmax_out, (cudaStream_t)stream);
+}
+
+int sgdml_b200_set_relax_block(int64_t n_steps) {
+  SG_ARG(n_steps >= 0);
+  g_relax_block = n_steps;
+  return 0;
 }
 
 }  // extern "C"

@@ -4,6 +4,9 @@ positions, velocities and forces kept in GPU memory between steps.  ``GDMLPathIn
 of ring polymers on the same engine (``sgdml_b200_pimd_*``): PILE-L thermostatted (or NVE) ring-polymer trajectories
 with the primitive and centroid-virial quantum kinetic-energy estimators.
 
+``GDMLRelaxation`` -- geometry optimisation of many replicas on the same engine (``sgdml_b200_relax_*``): FIRE and
+L-BFGS, each replica frozen once it has converged.
+
 Units follow ASE and ``intf.ase_calc.SGDMLCalculator``: positions in Angstrom, velocities in Angstrom/fs, masses in
 amu, energies in eV, time in fs, temperature in K.  ``E_to_eV`` and ``F_to_eV_Ang`` convert the model's units as in
 the calculator (defaults: kcal/mol and Angstrom).  Internally the engine works in the model's units with the
@@ -46,6 +49,15 @@ class GDMLDynamics(object):
     again then."""
 
     def __init__(self, model, masses, n_replicas=1, E_to_eV=_KCAL_PER_MOL_IN_EV, F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        self._init_model(model, n_replicas, E_to_eV, F_to_eV_Ang)
+        masses = np.ascontiguousarray(np.asarray(masses, dtype=np.float64).ravel())
+        if masses.shape != (self.n_atoms,):
+            raise ValueError('masses must hold one value (amu) per atom: %d' % self.n_atoms)
+        # a = F inv_mass in model length per fs^2, F in the model's force unit
+        self.inv_mass = self.F_to_eV_Ang * self.Ang_to_R * FS**2 / masses
+        self._handle = self._create_handle()
+
+    def _init_model(self, model, n_replicas, E_to_eV, F_to_eV_Ang):
         _lib.require_gpu()
         self.gdml_predict = model if isinstance(model, GDMLPredict) else GDMLPredict(
             model if isinstance(model, dict) else np.load(model, allow_pickle=True))
@@ -54,13 +66,7 @@ class GDMLDynamics(object):
         self.E_to_eV = float(E_to_eV)
         self.F_to_eV_Ang = float(F_to_eV_Ang)
         self.Ang_to_R = self.F_to_eV_Ang / self.E_to_eV  # Angstrom -> model length unit (ase_calc.py:93-94)
-        masses = np.ascontiguousarray(np.asarray(masses, dtype=np.float64).ravel())
-        if masses.shape != (self.n_atoms,):
-            raise ValueError('masses must hold one value (amu) per atom: %d' % self.n_atoms)
-        # a = F inv_mass in model length per fs^2, F in the model's force unit
-        self.inv_mass = self.F_to_eV_Ang * self.Ang_to_R * FS**2 / masses
         self._torch_device = None
-        self._handle = self._create_handle()
 
     def _create_handle(self):
         handle = ctypes.c_void_p()
@@ -259,3 +265,70 @@ class GDMLPathIntegralDynamics(GDMLDynamics):
                 'potential_energy': (f['E_pot'] * self.E_to_eV).reshape(nf, n_p, P),
                 'kinetic_energy_primitive': f['K_prim'] * self.E_to_eV,
                 'kinetic_energy_virial': f['K_cv'] * self.E_to_eV}
+
+
+class GDMLRelaxation(GDMLDynamics):
+    """Relaxes `n_replicas` geometries of one model to local minima of its energy, on the device, with FIRE or L-BFGS.
+
+    The handle is an MD handle with unit inverse masses, which the optimisers never read; ``set_state`` and
+    ``get_state`` are ``GDMLDynamics``'s, and ``run`` raises (there are no masses to integrate with).  ``relax(positions=None, fmax=0.05, max_steps=1000, optimizer='lbfgs',
+    maxstep=0.2, memory=20, alpha=70.0, dt=0.1, dtmax=1.0)`` relaxes from `positions` ((n_replicas, N, 3) or (N, 3) for
+    one replica, Angstrom; None: the current state) until every replica has max_a |F_a| < fmax (eV/Angstrom, ASE's
+    criterion) or max_steps steps have run, and returns {'positions', 'forces' (n_replicas, N, 3), 'potential_energy',
+    'fmax' (n_replicas,), 'converged' (n_replicas,) bool, 'n_steps' (n_replicas,) int64} in Angstrom, eV/Angstrom and
+    eV.  The arguments and defaults are those of ASE's optimisers: maxstep in Angstrom (FIRE: the whole step, L-BFGS:
+    each atom's); L-BFGS keeps `memory` pairs (1 to 32) and starts from the inverse Hessian 1/alpha (Angstrom^2/eV);
+    FIRE starts at time step dt and grows it up to dtmax (ASE's time unit).  Every call starts afresh, as a new ASE
+    optimiser would; afterwards the velocities are zero and the step index is unchanged.  NumPy arrays or float64 CUDA
+    tensors in, the same kind out."""
+
+    def __init__(self, model, n_replicas=1, E_to_eV=_KCAL_PER_MOL_IN_EV, F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        self._init_model(model, n_replicas, E_to_eV, F_to_eV_Ang)
+        self.inv_mass = np.ones(self.n_atoms)
+        self._handle = self._create_handle()
+
+    def run(self, *args, **kwargs):
+        """Not available: the handle's inverse masses are ones in model units, not the masses ``GDMLDynamics.run``
+        integrates with.  Run MD on relaxed geometries with a ``GDMLDynamics`` of the real masses."""
+        raise TypeError('GDMLRelaxation has no MD run: pass the relaxed positions to GDMLDynamics(model, masses)')
+
+    # ------------------------------------------------------------------ model units
+    def _relax_raw(self, optimizer, max_steps, fmax, maxstep, *args):
+        """FIRE: args = (dt, dtmax); L-BFGS: args = (memory, h0), all in model units.  -> (n_steps, converged, fmax)."""
+        n = self.n_replicas
+        if self._torch_device is None:
+            out = (np.empty(n, dtype=np.int64), np.empty(n, dtype=np.int32), np.empty(n))
+        else:
+            import torch
+
+            out = tuple(torch.empty(n, dtype=t, device=self._torch_device)
+                        for t in (torch.int64, torch.int32, torch.float64))
+        L = _lib.lib()
+        if optimizer == 'fire':
+            rc = L.sgdml_b200_relax_fire(self._handle, int(max_steps), float(fmax), float(maxstep), float(args[0]),
+                                         float(args[1]), *(_lib.ptr(x) for x in out), _lib.current_stream())
+        elif optimizer == 'lbfgs':
+            rc = L.sgdml_b200_relax_lbfgs(self._handle, int(max_steps), float(fmax), float(maxstep), int(args[0]),
+                                          float(args[1]), *(_lib.ptr(x) for x in out), _lib.current_stream())
+        else:
+            raise ValueError("optimizer must be 'lbfgs' or 'fire': %r" % (optimizer,))
+        _lib.check(rc, 'relax_' + optimizer)
+        return out
+
+    # ------------------------------------------------------------------ ASE units
+    def relax(self, positions=None, fmax=0.05, max_steps=1000, optimizer='lbfgs', maxstep=0.2, memory=20, alpha=70.0,
+              dt=0.1, dtmax=1.0):
+        if optimizer not in ('lbfgs', 'fire'):
+            raise ValueError("optimizer must be 'lbfgs' or 'fire': %r" % (optimizer,))
+        if positions is not None:
+            self.set_state(positions)
+        c = self.Ang_to_R * self.F_to_eV_Ang  # dt^2 and the inverse Hessian: Angstrom^2 / eV -> model units
+        if optimizer == 'fire':
+            args = (float(dt) * np.sqrt(c), float(dtmax) * np.sqrt(c))
+        else:
+            args = (memory, c / float(alpha))
+        n_steps, conv, fm = self._relax_raw(optimizer, max_steps, float(fmax) / self.F_to_eV_Ang,
+                                            float(maxstep) * self.Ang_to_R, *args)
+        st = self.get_state()
+        return {'positions': st['positions'], 'forces': st['forces'], 'potential_energy': st['potential_energy'],
+                'fmax': fm * self.F_to_eV_Ang, 'converged': conv != 0, 'n_steps': n_steps}

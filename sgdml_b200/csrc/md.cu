@@ -1,4 +1,8 @@
-// The BAOAB Langevin integrator step of sgdml_b200_md_run (driver: md_run in predict.cu).
+// Molecular dynamics, path-integral MD and geometry optimisation on the device: the integrator and optimiser kernels
+// (contract in md.cuh), then the driver of sgdml_b200_md_*, sgdml_b200_pimd_* and sgdml_b200_relax_*, which evaluates
+// forces through the predictor interface of predict.cuh.
+//
+// The BAOAB Langevin integrator step of sgdml_b200_md_run.
 //
 // A step from (r, v, F(r)) with h = dt/2, c1 = exp(-gamma dt), s_i = inverse mass of the atom of coordinate i and
 // sigma_i = sqrt((1 - c1^2) kT s_i):
@@ -11,10 +15,14 @@
 // step >> 32) for the coordinate pair (2j, 2j + 1), Box-Muller on the two 53-bit uniforms of its four output words.
 // The step index comes from the handle's counter in device memory, so a replayed graph draws fresh noise each step
 // and a run continued over several calls draws exactly the noise of one long run.
+#include <algorithm>
 #include <cmath>
+#include <initializer_list>
+#include <vector>
 
 #include "common.cuh"
 #include "md.cuh"
+#include "predict.cuh"
 
 namespace sgdml {
 
@@ -127,7 +135,7 @@ __device__ __forceinline__ double block_sum(double x, double* red) {
   return r;
 }
 
-// The ring-polymer step (launch_pimd_step in md.cuh).  Each tile holds TI coordinates of all nb beads in shared memory
+// The ring-polymer step (contract in md.cuh).  Each tile holds TI coordinates of all nb beads in shared memory
 // (TI = PIMD_TILE / nb rounded down to even, so a Philox coordinate pair never straddles two tiles); every thread owns
 // at most PIMD_TILE / MD_THREADS = 4 elements of it in each transform, whatever nb.  Sums over beads and modes run in
 // index order from the first product, and every update rounds as written.  At nb = 1 (C = 1, cos = 1, sin/w = h,
@@ -318,8 +326,8 @@ __global__ void __launch_bounds__(MD_THREADS) k_pimd_step(const PimdParams* __re
 }
 
 // ---------------------------------------------------------------------------------- geometry optimisation
-// The FIRE and L-BFGS steps of sgdml_b200_relax_* (driver: relax_impl in predict.cu); the exact sums and updates are
-// in md.cuh.  Every thread holds the replica's RelaxState and every CTA-wide sum, so branches on them are uniform;
+// The FIRE and L-BFGS steps of sgdml_b200_relax_* (driver: relax_impl below); the exact sums and updates are in
+// md.cuh.  Every thread holds the replica's RelaxState and every CTA-wide sum, so branches on them are uniform;
 // thread 0 writes the state back at the end.  Each thread updates only its own coordinates, except where the per-atom
 // maximum reads three of them (a barrier precedes it).
 
@@ -552,53 +560,579 @@ __global__ void k_relax_report(const RelaxState* __restrict__ st, int64_t n_rep,
 
 }  // namespace
 
-int launch_md_step(const MdParams* P, const double* s, const double* sigma, double* R, double* V, const double* F,
-                   const double* E, uint64_t* step, int64_t n_rep, int dimi, int advance, cudaStream_t st) {
-  k_md_step<<<(unsigned)n_rep, MD_THREADS, 0, st>>>(P, s, sigma, R, V, F, E, step, dimi, advance);
-  SG_CUDA(cudaGetLastError());
-  count_launch(KID_MISC);
-  return 0;
-}
-
-int launch_pimd_step(const PimdParams* P, const double* tab, const double* s, const double* sigma, double* R, double* V,
-                     const double* F, const double* E, uint64_t* step, int64_t n_poly, int dimi, int nb, int advance,
-                     cudaStream_t st) {
-  if (nb < 1 || nb > PIMD_MAX_BEADS) return fail_arg("launch_pimd_step: n_beads outside [1, PIMD_MAX_BEADS]");
-  k_pimd_step<<<(unsigned)n_poly, MD_THREADS, 0, st>>>(P, tab, s, sigma, R, V, F, E, step, dimi, nb, advance);
-  SG_CUDA(cudaGetLastError());
-  count_launch(KID_MISC);
-  return 0;
-}
-
-int launch_fire_step(const RelaxParams* P, RelaxState* st, double* R, double* V, const double* F, int64_t n_rep,
-                     int dimi, int advance, cudaStream_t s) {
-  k_fire_step<<<(unsigned)n_rep, MD_THREADS, 0, s>>>(P, st, R, V, F, dimi, advance);
-  SG_CUDA(cudaGetLastError());
-  count_launch(KID_MISC);
-  return 0;
-}
-
-int launch_lbfgs_step(const RelaxParams* P, RelaxState* st, double* R, double* D, const double* F, const double* E,
-                      int64_t n_rep, int dimi, int advance, cudaStream_t s) {
-  k_lbfgs_step<<<(unsigned)n_rep, MD_THREADS, 0, s>>>(P, st, R, D, F, E, dimi, advance);
-  SG_CUDA(cudaGetLastError());
-  count_launch(KID_MISC);
-  return 0;
-}
-
-int launch_relax_count(const RelaxState* st, int64_t n_rep, int* n_active, cudaStream_t s) {
-  k_relax_count<<<1, MD_THREADS, 0, s>>>(st, n_rep, n_active);
-  SG_CUDA(cudaGetLastError());
-  count_launch(KID_MISC);
-  return 0;
-}
-
-int launch_relax_report(const RelaxState* st, int64_t n_rep, int64_t* n_steps, int* conv, double* fmax,
-                        cudaStream_t s) {
-  k_relax_report<<<(unsigned)((n_rep + 255) / 256), 256, 0, s>>>(st, n_rep, n_steps, conv, fmax);
-  SG_CUDA(cudaGetLastError());
-  count_launch(KID_MISC);
-  return 0;
-}
-
 }  // namespace sgdml
+
+// ============================================================== driver (sgdml_b200_md_*, _pimd_*, _relax_*)
+// The state of n_rep replicas stays in device memory between steps and between runs.  One step is the integrator
+// kernel, then the forces and energies of the new positions (force_eval_run, predict.cuh) written back into the
+// state.  That sequence is captured once into a CUDA graph and replayed n_steps times on the caller's stream;
+// everything a run changes (dt, gamma, kT, seed, frame buffers) lives in device memory, and the step counter is
+// advanced by the integrator, so the graph bakes in no run.
+using namespace sgdml;
+
+struct sgdml_b200_md {
+  int64_t n_rep = 0;
+  int dimi = 0;
+  int nb = 1;  // beads per ring polymer: replica p nb + j is bead j of polymer p (1 for sgdml_b200_md_create)
+  ForceEval* fe = nullptr;  // the handle's own predictor workspace: predict calls never touch it, MD never theirs
+  double *R = nullptr, *V = nullptr, *F = nullptr, *E = nullptr;  // state: (n_rep, 3N) x 3, (n_rep)
+  double *Fs = nullptr, *Es = nullptr;  // outputs of the force evaluation that precedes a capture
+  uint64_t* step = nullptr;             // (n_rep) step counters, all equal
+  uint64_t step_host = 0;               // their value once the queued runs have finished
+  bool has_state = false;
+  double *s = nullptr, *sigma = nullptr;  // (3N) inverse mass, (nb, 3N) noise scale per mode and coordinate
+  std::vector<double> s_host;             // s on the host
+  MdParams* dP = nullptr;
+  MdParams* hP = nullptr;     // pinned staging of dP and sigma, reused once the previous run's upload is done
+  double* hSigma = nullptr;
+  PimdParams* dQ = nullptr;  // the ring-polymer run's parameter block
+  PimdParams* hQ = nullptr;
+  double *tab = nullptr, *hTab = nullptr;  // C (nb x nb) and the four mode tables (nb each)
+  cudaEvent_t uploaded = nullptr;
+  cudaStream_t gs = nullptr;  // capture stream
+  cudaEvent_t ge = nullptr;
+  cudaGraphExec_t exec = nullptr;
+  int graph_kind = -1;        // the MdKind of the captured step
+  int n_kernels = 0;
+  // geometry optimisation (sgdml_b200_relax_*), allocated by the first relaxation
+  RelaxState* rst = nullptr;  // (n_rep) per-replica optimiser state
+  RelaxParams* dR = nullptr;
+  RelaxParams* hR = nullptr;  // pinned staging of dR
+  int* hActive = nullptr;     // mapped pinned: unconverged replicas, written by k_relax_count
+  int* dActive = nullptr;     // its device address
+  cudaEvent_t counted = nullptr;
+  double *S = nullptr, *Y = nullptr, *rho = nullptr;        // L-BFGS ring, m_cap pairs per replica
+  double *r_prev = nullptr, *g_prev = nullptr;              // (n_rep, 3N)
+  int m_cap = 0;
+};
+
+namespace {
+
+void md_free(sgdml_b200_md* md) {
+  cudaDeviceSynchronize();  // blocks go back to the cache: nothing may still use them
+  if (md->exec) cudaGraphExecDestroy(md->exec);
+  if (md->gs) cudaStreamDestroy(md->gs);
+  if (md->ge) cudaEventDestroy(md->ge);
+  if (md->uploaded) cudaEventDestroy(md->uploaded);
+  if (md->counted) cudaEventDestroy(md->counted);
+  force_eval_destroy(md->fe);
+  for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s, md->sigma}) cached_free(p);
+  cached_free(md->step);
+  cached_free(md->dP);
+  cached_free(md->dQ);
+  cached_free(md->tab);
+  for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev}) cached_free(p);
+  cached_free(md->rst);
+  cached_free(md->dR);
+  cudaFreeHost(md->hR);
+  cudaFreeHost(md->hActive);
+  cudaFreeHost(md->hP);
+  cudaFreeHost(md->hQ);
+  cudaFreeHost(md->hTab);
+  cudaFreeHost(md->hSigma);
+  delete md;
+}
+
+// The outputs of one call, each a (caller's pointer, bytes) pair; a null pointer or 0 bytes is no output.  The kernels
+// write a caller's device array in place and a host array into one device staging block, which finish() copies back.
+// The stream is synchronised before that block goes back to the cache on every path: after an error return, launches
+// already queued may still write into it.
+class Outputs {
+ public:
+  struct Out {
+    void* user;
+    size_t bytes;
+  };
+  explicit Outputs(cudaStream_t s) : s_(s) {}
+  Outputs(const Outputs&) = delete;
+  Outputs& operator=(const Outputs&) = delete;
+  ~Outputs() {
+    if (block_ == nullptr) return;
+    if (!synced_) cudaStreamSynchronize(s_);
+    cached_free(block_);
+  }
+  int init(std::initializer_list<Out> outs) {  // at most MAX_OUTS
+    size_t off[MAX_OUTS], total = 0;
+    for (const Out& o : outs) {
+      const int i = n_++;
+      out_[i] = o;
+      dev_[i] = o.bytes > 0 ? o.user : nullptr;
+      staged_[i] = dev_[i] != nullptr && !is_device_ptr(o.user);
+      off[i] = total;
+      if (staged_[i]) total += (o.bytes + 255) & ~(size_t)255;
+    }
+    if (total == 0) return 0;
+    SG_CUDA(cached_malloc(&block_, total));
+    for (int i = 0; i < n_; ++i)
+      if (staged_[i]) dev_[i] = block_ + off[i];
+    return 0;
+  }
+  // where the kernels write output i (null: none)
+  template <class T = double>
+  T* dev(int i) const {
+    return static_cast<T*>(dev_[i]);
+  }
+  size_t bytes(int i) const { return out_[i].bytes; }
+  // queues the copies to the host arrays and, if there are any, waits for them
+  int finish() {
+    for (int i = 0; i < n_; ++i)
+      if (staged_[i]) SG_CUDA(cudaMemcpyAsync(out_[i].user, dev_[i], out_[i].bytes, cudaMemcpyDeviceToHost, s_));
+    if (block_ != nullptr) {
+      SG_CUDA(cudaStreamSynchronize(s_));
+      synced_ = true;
+    }
+    return 0;
+  }
+
+ private:
+  static constexpr int MAX_OUTS = 6;
+  cudaStream_t s_;
+  int n_ = 0;
+  Out out_[MAX_OUTS];
+  void* dev_[MAX_OUTS];
+  bool staged_[MAX_OUTS];
+  char* block_ = nullptr;
+  bool synced_ = false;
+};
+
+// what one step of the handle's graph integrates
+enum MdKind { MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3 };
+
+// the integrator of sgdml_b200_md_run, sgdml_b200_pimd_run or sgdml_b200_relax_*; advance == 0 completes a run's last
+// step (MD) or only tests convergence (relaxation).  L-BFGS keeps its direction in V, which relax_impl zeroes after.
+int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
+  switch (kind) {
+    case MD_RING_POLYMER:
+      k_pimd_step<<<(unsigned)(md->n_rep / md->nb), MD_THREADS, 0, s>>>(md->dQ, md->tab, md->s, md->sigma, md->R, md->V,
+                                                                      md->F, md->E, md->step, md->dimi, md->nb,
+                                                                      advance);
+      break;
+    case MD_FIRE:
+      k_fire_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(md->dR, md->rst, md->R, md->V, md->F, md->dimi, advance);
+      break;
+    case MD_LBFGS:
+      k_lbfgs_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(md->dR, md->rst, md->R, md->V, md->F, md->E, md->dimi,
+                                                              advance);
+      break;
+    default:
+      k_md_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E,
+                                                           md->step, md->dimi, advance);
+  }
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_MISC);
+  return 0;
+}
+
+int md_step(sgdml_b200_md* md, int kind, cudaStream_t s) {
+  SG_TRY(md_integrate(md, kind, 1, s));
+  return force_eval_run(md->fe, md->R, md->F, md->E, s);
+}
+
+// the step graph, captured again whenever the force evaluation it bakes in is stale or the integrator (MdKind) changes
+int md_graph(sgdml_b200_md* md, int kind, cudaStream_t s) {
+  if (md->exec != nullptr && md->graph_kind == kind && !force_eval_stale(md->fe)) return 0;
+  if (md->exec != nullptr) {
+    cudaGraphExecDestroy(md->exec);
+    md->exec = nullptr;
+  }
+  if (md->gs == nullptr) {
+    SG_CUDA(cudaStreamCreateWithFlags(&md->gs, cudaStreamNonBlocking));
+    SG_CUDA(cudaEventCreateWithFlags(&md->ge, cudaEventDisableTiming));
+  }
+  // captured on a private stream (the caller's may be the legacy stream); after the caller's queued work
+  SG_CUDA(cudaEventRecord(md->ge, s));
+  SG_CUDA(cudaStreamWaitEvent(md->gs, md->ge, 0));
+  // the force evaluation once un-captured, into scratch outputs: sets the kernels' shared-memory attributes
+  SG_TRY(force_eval_run(md->fe, md->R, md->Fs, md->Es, md->gs));
+  SG_CUDA(cudaStreamSynchronize(md->gs));
+  SG_TRY(capture_graph(md->gs, [&] { return md_step(md, kind, md->gs); }, &md->exec, &md->n_kernels));
+  force_eval_mark(md->fe);
+  md->graph_kind = kind;
+  return 0;
+}
+
+// n_steps steps of the handle's integrator: graph replays, or plain launches with SGDML_B200_GRAPH=0 or profiling
+int md_replay(sgdml_b200_md* md, int kind, int64_t n_steps, cudaStream_t s) {
+  if (g_graph_enabled() && !profiling_enabled()) {
+    SG_TRY(md_graph(md, kind, s));
+    for (int64_t k = 0; k < n_steps; ++k) {
+      SG_CUDA(cudaGraphLaunch(md->exec, s));
+      count_launch(KID_PREDICT_AUX, md->n_kernels);  // the kernels of a replay are launches too
+    }
+  } else {
+    for (int64_t k = 0; k < n_steps; ++k) SG_TRY(md_step(md, kind, s));
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------ MD and PIMD runs
+// The run's constants, once on the host in double precision.  First the fields MdParams and PimdParams share.
+template <class P>
+void run_params(P& p, const sgdml_b200_md* md, double dt, uint64_t seed, int64_t n_frames, int64_t stride,
+                const Outputs& out) {
+  p.h = 0.5 * dt;
+  p.key[0] = (uint32_t)seed;
+  p.key[1] = (uint32_t)(seed >> 32);
+  p.stride = n_frames > 0 ? (int)stride : 0;
+  p.run_start = md->step_host;
+  p.R_f = out.dev(0);
+  p.V_f = out.dev(1);
+  p.Ep_f = out.dev(2);
+  p.Ek_f = out.dev(3);
+}
+
+// MD: c1 and the (3N) sigma table
+int md_params(sgdml_b200_md* md, double dt, double gamma, double kT, cudaStream_t s) {
+  MdParams& p = *md->hP;
+  p.c1 = std::exp(-gamma * dt);
+  p.use_O = gamma > 0.0 ? 1 : 0;
+  for (int i = 0; i < md->dimi; ++i) md->hSigma[i] = std::sqrt((1.0 - p.c1 * p.c1) * kT * md->s_host[(size_t)i]);
+  SG_CUDA(cudaMemcpyAsync(md->dP, md->hP, sizeof(MdParams), cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * md->dimi, cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+// PIMD: the estimator constants, C, the mode tables and the (P, 3N) sigma table (tests/pimd_oracle.py restates them)
+int pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, double kT, double hbar, double gamma, double lambda,
+                cudaStream_t s) {
+  const int nb = md->nb, dimi = md->dimi;
+  PimdParams& p = *md->hQ;
+  const double h = 0.5 * dt;
+  const double kTP = nb * kT;
+  const double wP = kTP / hbar;
+  p.use_O = gamma > 0.0 || (lambda > 0.0 && nb > 1) ? 1 : 0;
+  p.kprim0 = 0.5 * (double)(dimi * nb) * kT;
+  p.kspring = 0.5 * wP * wP / nb;
+  p.kcv0 = 0.5 * dimi * kT;
+  p.kvir = 0.5 / nb;
+  p.Kp_f = out.dev(4);
+  p.Kcv_f = out.dev(5);
+  double* C = md->hTab;
+  double *m_cos = C + nb * nb, *m_sow = m_cos + nb, *m_msin = m_sow + nb, *m_c1 = m_msin + nb;
+  for (int j = 0; j < nb; ++j)
+    for (int k = 0; k < nb; ++k) {
+      double c;
+      if (k == 0)
+        c = std::sqrt(1.0 / nb);
+      else if (2 * k < nb)
+        c = std::sqrt(2.0 / nb) * std::cos(2.0 * M_PI * j * k / nb);
+      else if (2 * k == nb)
+        c = std::sqrt(1.0 / nb) * (j % 2 ? -1.0 : 1.0);
+      else
+        c = std::sqrt(2.0 / nb) * std::sin(2.0 * M_PI * j * k / nb);
+      C[j * nb + k] = c;
+    }
+  for (int k = 0; k < nb; ++k) {
+    double g = gamma;
+    m_cos[k] = 1.0;
+    m_sow[k] = h;
+    m_msin[k] = 0.0;
+    if (k > 0) {
+      const double wk = 2.0 * wP * std::sin(M_PI * k / nb);
+      m_cos[k] = std::cos(wk * h);
+      m_sow[k] = std::sin(wk * h) / wk;
+      m_msin[k] = -wk * std::sin(wk * h);
+      g = 2.0 * lambda * wk;
+    }
+    m_c1[k] = std::exp(-g * dt);
+    for (int i = 0; i < dimi; ++i)
+      md->hSigma[(size_t)k * dimi + i] = std::sqrt((1.0 - m_c1[k] * m_c1[k]) * kTP * md->s_host[(size_t)i]);
+  }
+  SG_CUDA(cudaMemcpyAsync(md->dQ, md->hQ, sizeof(PimdParams), cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaMemcpyAsync(md->tab, md->hTab, sizeof(double) * (nb * nb + 4 * nb), cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * nb * dimi, cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+// sgdml_b200_md_run (MD_CLASSICAL) and sgdml_b200_pimd_run (MD_RING_POLYMER; hbar and lambda are only its own).
+// frames: R, V, E_pot, E_kin, then the ring polymer's K_prim and K_cv.  n_steps steps, then the completing launch.
+int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, double hbar, double gamma, double lambda,
+           uint64_t seed, int64_t stride, double* const frames[6], cudaStream_t s) {
+  const bool ring = kind == MD_RING_POLYMER;
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
+  if (!ring && md->nb > 1)
+    return fail_arg("sgdml_b200_md_run: a ring-polymer handle (n_beads > 1) runs with sgdml_b200_pimd_run");
+  SG_ARG(std::isfinite(dt) && dt > 0.0);
+  if (!ring) SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
+  SG_ARG(std::isfinite(kT) && kT >= 0.0);
+  if (ring) {
+    SG_ARG(std::isfinite(hbar) && hbar > 0.0);
+    SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
+    SG_ARG(std::isfinite(lambda) && lambda >= 0.0);
+    if (md->nb > 1 && kT == 0.0) return fail_arg("a ring polymer (n_beads > 1) needs kT > 0");
+  }
+  if (md->nb == 1 && kT > 0.0 && gamma == 0.0)
+    return fail_arg("kT > 0 needs a friction gamma > 0 (a thermostat without coupling)");
+  if (stride > 0 && n_steps % stride != 0) return fail_arg("n_steps must be a multiple of stride");
+  if (!md->has_state)
+    return fail_arg(ring ? "sgdml_b200_pimd_run: no state yet (call sgdml_b200_md_set_state)"
+                         : "sgdml_b200_md_run: no state yet (call sgdml_b200_md_set_state)");
+  if (n_steps == 0) return 0;
+
+  const int64_t n_frames = stride > 0 ? n_steps / stride : 0;
+  const size_t fr = sizeof(double) * (size_t)(n_frames * md->n_rep);
+  const size_t fp = sizeof(double) * (size_t)(n_frames * (md->n_rep / md->nb));
+  Outputs out(s);
+  SG_TRY(out.init({{frames[0], fr * md->dimi}, {frames[1], fr * md->dimi}, {frames[2], fr}, {frames[3], fr},
+                   {frames[4], fp}, {frames[5], fp}}));
+  SG_TRY(force_eval_prepare(md->fe));
+  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous run has read the staging
+  if (ring) {
+    run_params(*md->hQ, md, dt, seed, n_frames, stride, out);
+    SG_TRY(pimd_params(md, out, dt, kT, hbar, gamma, lambda, s));
+  } else {
+    run_params(*md->hP, md, dt, seed, n_frames, stride, out);
+    SG_TRY(md_params(md, dt, gamma, kT, s));
+  }
+  SG_CUDA(cudaEventRecord(md->uploaded, s));
+  SG_TRY(md_replay(md, kind, n_steps, s));
+  md->step_host += (uint64_t)n_steps;
+  SG_TRY(md_integrate(md, kind, 0, s));  // the second half-kick of the last step (and its frame)
+  return out.finish();
+}
+
+// ------------------------------------------------------------------ geometry optimisation (sgdml_b200_relax_*)
+constexpr int64_t RELAX_BLOCK = 16;  // replays between convergence read-backs
+int64_t g_relax_block = 0;           // sgdml_b200_set_relax_block (test hook): 0 = RELAX_BLOCK
+
+// the optimiser state, made at the first relaxation; the L-BFGS ring grows to `memory` pairs per replica
+int relax_alloc(sgdml_b200_md* md, int memory) {
+  if (md->rst == nullptr) SG_CUDA(cached_malloc(&md->rst, sizeof(RelaxState) * (size_t)md->n_rep));
+  if (md->dR == nullptr) SG_CUDA(cached_malloc(&md->dR, sizeof(RelaxParams)));
+  if (md->hR == nullptr) SG_CUDA(cudaMallocHost(&md->hR, sizeof(RelaxParams)));
+  if (md->hActive == nullptr) {
+    SG_CUDA(cudaHostAlloc(&md->hActive, sizeof(int), cudaHostAllocMapped));
+    SG_CUDA(cudaHostGetDevicePointer((void**)&md->dActive, md->hActive, 0));
+  }
+  if (md->counted == nullptr) SG_CUDA(cudaEventCreateWithFlags(&md->counted, cudaEventDisableTiming));
+  if (memory > md->m_cap) {
+    const size_t vec = sizeof(double) * (size_t)(md->n_rep * md->dimi);
+    SG_CUDA(cudaDeviceSynchronize());  // the old ring goes back to the cache: nothing may still use it
+    for (double** p : {&md->S, &md->Y, &md->rho}) {
+      cached_free(*p);
+      *p = nullptr;
+    }
+    md->m_cap = 0;
+    SG_CUDA(cached_malloc(&md->S, vec * memory));
+    SG_CUDA(cached_malloc(&md->Y, vec * memory));
+    SG_CUDA(cached_malloc(&md->rho, sizeof(double) * (size_t)md->n_rep * memory));
+    if (md->r_prev == nullptr) {
+      SG_CUDA(cached_malloc(&md->r_prev, vec));
+      SG_CUDA(cached_malloc(&md->g_prev, vec));
+    }
+    md->m_cap = memory;
+  }
+  return 0;
+}
+
+// Relaxes every replica from the handle's state: blocks of step-graph replays, each followed by the convergence test
+// and a count of unconverged replicas read back through mapped pinned memory; stops when none is left or after
+// max_steps.  Frozen replicas make the block length a matter of cost only.  V is zero before and after.
+int relax_impl(sgdml_b200_md* md, int kind, int64_t max_steps, const RelaxParams& prm, int64_t* n_steps_out,
+               int* conv_out, double* fmax_out, cudaStream_t s) {
+  const int64_t n_rep = md->n_rep;
+  SG_TRY(force_eval_prepare(md->fe));
+  SG_TRY(relax_alloc(md, kind == MD_LBFGS ? prm.memory : 0));
+  Outputs out(s);
+  SG_TRY(out.init({{n_steps_out, sizeof(int64_t) * (size_t)n_rep}, {conv_out, sizeof(int) * (size_t)n_rep},
+                   {fmax_out, sizeof(double) * (size_t)n_rep}}));
+  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the staging
+  RelaxParams& p = *md->hR;
+  p = prm;
+  p.m_cap = md->m_cap;
+  p.S = md->S;
+  p.Y = md->Y;
+  p.rho = md->rho;
+  p.r_prev = md->r_prev;
+  p.g_prev = md->g_prev;
+  SG_CUDA(cudaMemcpyAsync(md->dR, md->hR, sizeof(RelaxParams), cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaEventRecord(md->uploaded, s));
+  const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
+  SG_CUDA(cudaMemsetAsync(md->rst, 0, sizeof(RelaxState) * (size_t)n_rep, s));
+  SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
+  const int64_t block = g_relax_block > 0 ? g_relax_block : RELAX_BLOCK;
+  for (int64_t done = 0;;) {
+    SG_TRY(md_integrate(md, kind, 0, s));  // the test on the current forces
+    k_relax_count<<<1, MD_THREADS, 0, s>>>(md->rst, n_rep, md->dActive);
+    SG_CUDA(cudaGetLastError());
+    count_launch(KID_MISC);
+    SG_CUDA(cudaEventRecord(md->counted, s));
+    SG_CUDA(cudaEventSynchronize(md->counted));
+    if (*(volatile int*)md->hActive == 0 || done >= max_steps) break;
+    const int64_t n = std::min(block, max_steps - done);
+    SG_TRY(md_replay(md, kind, n, s));
+    done += n;
+  }
+  SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));  // a following MD run starts at rest
+  k_relax_report<<<(unsigned)((n_rep + 255) / 256), 256, 0, s>>>(md->rst, n_rep, out.dev<int64_t>(0), out.dev<int>(1),
+                                                                out.dev<double>(2));
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_MISC);
+  return out.finish();
+}
+
+// the checks both optimisers share; a rejected call queues nothing
+int relax_check(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, const char* what) {
+  SG_ARG(md != nullptr && max_steps >= 0);
+  SG_ARG(std::isfinite(fmax) && fmax >= 0.0);
+  SG_ARG(std::isfinite(maxstep) && maxstep > 0.0);
+  if (!md->has_state) return fail_arg(what);
+  return 0;
+}
+
+// a handle of n_rep = n_poly nb replicas; the caller has checked the counts
+int md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, int nb, const double* inv_mass) {
+  SG_ARG(!is_device_ptr(inv_mass));
+  int64_t n_atoms = 0;
+  SG_TRY(sgdml_b200_model_dims(m, &n_atoms, nullptr, nullptr));
+  for (int i = 0; i < n_atoms; ++i)
+    if (!(std::isfinite(inv_mass[i]) && inv_mass[i] > 0.0)) return fail_arg("inv_mass must be finite and > 0");
+  sgdml_b200_md* md = new sgdml_b200_md();
+  md->n_rep = n_rep;
+  md->nb = nb;
+  md->dimi = 3 * (int)n_atoms;
+  auto body = [&]() -> int {
+    SG_TRY(force_eval_create(m, n_rep, &md->fe));
+    const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
+    for (double** p : {&md->R, &md->V, &md->F, &md->Fs}) SG_CUDA(cached_malloc(p, st));
+    SG_CUDA(cached_malloc(&md->E, sizeof(double) * n_rep));
+    SG_CUDA(cached_malloc(&md->Es, sizeof(double) * n_rep));
+    SG_CUDA(cached_malloc(&md->step, sizeof(uint64_t) * n_rep));
+    SG_CUDA(cached_malloc(&md->s, sizeof(double) * md->dimi));
+    SG_CUDA(cached_malloc(&md->sigma, sizeof(double) * nb * md->dimi));
+    SG_CUDA(cached_malloc(&md->dP, sizeof(MdParams)));
+    SG_CUDA(cached_malloc(&md->dQ, sizeof(PimdParams)));
+    SG_CUDA(cached_malloc(&md->tab, sizeof(double) * (nb * nb + 4 * nb)));
+    SG_CUDA(cudaMallocHost(&md->hP, sizeof(MdParams)));
+    SG_CUDA(cudaMallocHost(&md->hQ, sizeof(PimdParams)));
+    SG_CUDA(cudaMallocHost(&md->hTab, sizeof(double) * (nb * nb + 4 * nb)));
+    SG_CUDA(cudaMallocHost(&md->hSigma, sizeof(double) * nb * md->dimi));
+    SG_CUDA(cudaEventCreateWithFlags(&md->uploaded, cudaEventDisableTiming));
+    md->s_host.resize((size_t)md->dimi);
+    for (int i = 0; i < md->dimi; ++i) md->s_host[(size_t)i] = inv_mass[i / 3];
+    SG_CUDA(cudaMemcpy(md->s, md->s_host.data(), sizeof(double) * md->dimi, cudaMemcpyHostToDevice));
+    return force_eval_prepare(md->fe);
+  };
+  const int rc = body();
+  if (rc != 0) {
+    md_free(md);
+    return rc;
+  }
+  *out = md;
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, const double* inv_mass) {
+  SG_TRY(require_device());
+  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
+  SG_ARG(n_rep >= 1 && n_rep <= INT32_MAX);
+  return md_create(out, m, n_rep, 1, inv_mass);
+}
+
+int sgdml_b200_pimd_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_poly, int64_t n_beads,
+                           const double* inv_mass) {
+  SG_TRY(require_device());
+  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
+  SG_ARG(n_beads >= 1 && n_beads <= PIMD_MAX_BEADS);
+  SG_ARG(n_poly >= 1 && n_poly <= INT32_MAX / n_beads);
+  return md_create(out, m, n_poly * n_beads, (int)n_beads, inv_mass);
+}
+
+int sgdml_b200_md_destroy(sgdml_b200_md* md) {
+  if (md != nullptr) md_free(md);
+  return 0;
+}
+
+int sgdml_b200_md_set_state(sgdml_b200_md* md, const double* R, const double* V, uint64_t step, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr && R != nullptr);
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
+  SG_TRY(force_eval_prepare(md->fe));
+  SG_CUDA(cudaMemcpyAsync(md->R, R, st, cudaMemcpyDefault, s));
+  if (V != nullptr)
+    SG_CUDA(cudaMemcpyAsync(md->V, V, st, cudaMemcpyDefault, s));
+  else
+    SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
+  const std::vector<uint64_t> steps((size_t)md->n_rep, step);
+  SG_CUDA(cudaMemcpyAsync(md->step, steps.data(), sizeof(uint64_t) * md->n_rep, cudaMemcpyHostToDevice, s));
+  SG_TRY(force_eval_run(md->fe, md->R, md->F, md->E, s));
+  SG_CUDA(cudaStreamSynchronize(s));  // (the counters' host vector goes out of scope)
+  md->step_host = step;
+  md->has_state = true;
+  return 0;
+}
+
+int sgdml_b200_md_get_state(sgdml_b200_md* md, double* R, double* V, double* F, double* E_pot, uint64_t* step,
+                            void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr);
+  if (!md->has_state) return fail_arg("sgdml_b200_md_get_state: no state yet (call sgdml_b200_md_set_state)");
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
+  Outputs out(s);
+  SG_TRY(out.init({{R, st}, {V, st}, {F, st}, {E_pot, sizeof(double) * md->n_rep}, {step, sizeof(uint64_t)}}));
+  const void* src[5] = {md->R, md->V, md->F, md->E, md->step};
+  for (int i = 0; i < 5; ++i)
+    if (out.dev<void>(i) != nullptr)
+      SG_CUDA(cudaMemcpyAsync(out.dev<void>(i), src[i], out.bytes(i), cudaMemcpyDeviceToDevice, s));
+  return out.finish();
+}
+
+int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, uint64_t seed,
+                      int64_t stride, double* R_frames, double* V_frames, double* E_pot_frames, double* E_kin_frames,
+                      void* stream) {
+  double* const frames[6] = {R_frames, V_frames, E_pot_frames, E_kin_frames, nullptr, nullptr};
+  return md_run(md, MD_CLASSICAL, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, frames, (cudaStream_t)stream);
+}
+
+int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma,
+                        double lambda, uint64_t seed, int64_t stride, double* R_frames, double* V_frames,
+                        double* E_pot_frames, double* E_kin_frames, double* K_prim_frames, double* K_cv_frames,
+                        void* stream) {
+  double* const frames[6] = {R_frames, V_frames, E_pot_frames, E_kin_frames, K_prim_frames, K_cv_frames};
+  return md_run(md, MD_RING_POLYMER, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, frames, (cudaStream_t)stream);
+}
+
+int sgdml_b200_relax_fire(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, double dt, double dtmax,
+                          int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(relax_check(md, max_steps, fmax, maxstep,
+                     "sgdml_b200_relax_fire: no state yet (call sgdml_b200_md_set_state)"));
+  SG_ARG(std::isfinite(dt) && dt > 0.0);
+  SG_ARG(std::isfinite(dtmax) && dtmax > 0.0);
+  RelaxParams p = {};
+  p.fmax2 = fmax * fmax;
+  p.maxstep = maxstep;
+  p.dt0 = dt;
+  p.dtmax = dtmax;
+  return relax_impl(md, MD_FIRE, max_steps, p, n_steps_out, converged_out, fmax_out, (cudaStream_t)stream);
+}
+
+int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, int memory, double h0,
+                           int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(relax_check(md, max_steps, fmax, maxstep,
+                     "sgdml_b200_relax_lbfgs: no state yet (call sgdml_b200_md_set_state)"));
+  SG_ARG(memory >= 1 && memory <= LBFGS_MAX_MEMORY);
+  SG_ARG(std::isfinite(h0) && h0 > 0.0);
+  RelaxParams p = {};
+  p.fmax2 = fmax * fmax;
+  p.maxstep = maxstep;
+  p.h0 = h0;
+  p.memory = memory;
+  return relax_impl(md, MD_LBFGS, max_steps, p, n_steps_out, converged_out, fmax_out, (cudaStream_t)stream);
+}
+
+int sgdml_b200_set_relax_block(int64_t n_steps) {
+  SG_ARG(n_steps >= 0);
+  g_relax_block = n_steps;
+  return 0;
+}
+
+}  // extern "C"

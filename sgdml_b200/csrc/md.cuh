@@ -1,5 +1,6 @@
-// Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_pimd_*): the BAOAB integrator step, its ring-polymer
-// form, and their counter-based noise.
+// Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_pimd_*, sgdml_b200_relax_*): the contract of the
+// kernels in md.cu -- the BAOAB integrator step, its ring-polymer form, their counter-based noise, and the FIRE and
+// L-BFGS steps.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -18,15 +19,13 @@ struct MdParams {
   double *R_f, *V_f, *Ep_f, *Ek_f;  // frames (n_frames, n_rep, 3N) / (n_frames, n_rep)
 };
 
-// One step for every replica (grid: one CTA of MD_THREADS per replica).  With the handle's step counter at n:
+// k_md_step: one step for every replica (grid: one CTA of MD_THREADS per replica).  With the handle's step counter at n:
 //   if n != run_start:  v += h (F s)        second half-kick of step n - 1 (F is F(r) of the positions in R)
 //                       frame (n - run_start) / stride - 1 when that is whole: R, full-step V, E_pot, E_kin
 //   if advance:         B, A, O (noise of step n), A; R and V hold the new positions and half-step velocities,
 //                       and the counter becomes n + 1
 // advance == 0 only completes the last step of a run.  s, sigma: (3N) inverse mass and noise scale per coordinate.
 constexpr int MD_THREADS = 128;
-int launch_md_step(const MdParams* P, const double* s, const double* sigma, double* R, double* V, const double* F,
-                   const double* E, uint64_t* step, int64_t n_rep, int dimi, int advance, cudaStream_t st);
 
 // Path-integral MD (sgdml_b200_pimd_run): replica p P + j is bead j of ring polymer p.
 constexpr int PIMD_MAX_BEADS = 64;  // C (P x P) sits in shared memory: 32 KB at the cap
@@ -46,14 +45,11 @@ struct PimdParams {
   double *Kp_f, *Kcv_f;             // frames (n_frames, n_poly)
 };
 
-// One PILE-L step for every ring polymer (grid: one CTA of MD_THREADS per polymer), the counterpart of
-// launch_md_step: the pending second half-kick and the frame (per bead R, full-step V, E_pot, E_kin; per polymer
+// k_pimd_step: one PILE-L step for every ring polymer (grid: one CTA of MD_THREADS per polymer), the counterpart of
+// k_md_step: the pending second half-kick and the frame (per bead R, full-step V, E_pot, E_kin; per polymer
 // K_prim, K_cv), then, if advance, B, the transform to normal modes, A, O, A, the transform back.  tab: C (nb x nb,
 // C[j nb + k]) followed by the mode tables cos(w_k h), sin(w_k h) / w_k, -w_k sin(w_k h), c1_k (nb each);
 // sigma (nb, 3N) per mode and coordinate; s (3N) inverse masses.
-int launch_pimd_step(const PimdParams* P, const double* tab, const double* s, const double* sigma, double* R, double* V,
-                     const double* F, const double* E, uint64_t* step, int64_t n_poly, int dimi, int nb, int advance,
-                     cudaStream_t st);
 
 // Geometry optimisation (sgdml_b200_relax_fire, sgdml_b200_relax_lbfgs): one CTA of MD_THREADS per replica.
 //
@@ -93,7 +89,7 @@ struct RelaxParams {
   double *r_prev, *g_prev;  // L-BFGS: (n_rep, 3N) positions and -F of the previous step
 };
 
-// FIRE (Bitzek et al., PRL 97, 170201 (2006); ASE's mass-free form, Nmin 5, finc 1.1, fdec 0.5, alpha_start 0.1,
+// k_fire_step: FIRE (Bitzek et al., PRL 97, 170201 (2006); ASE's mass-free form, Nmin 5, finc 1.1, fdec 0.5, alpha_start 0.1,
 // f_alpha 0.99) with velocities V (n_rep, 3N).  After the test, on every step but the first:
 //   P = F.v;  P > 0:  vv = v.v, ff = F.F, c = alpha (sqrt(vv) / sqrt(ff)), v = (1 - alpha) v + c F,
 //                     if n_pos > 5: dt = min(dt 1.1, dtmax), alpha = alpha 0.99;  n_pos += 1
@@ -101,7 +97,7 @@ struct RelaxParams {
 // then on every step (the first starts from dt = dt0, alpha = 0.1, n_pos = 0 and the V the driver zeroed):
 //   v = v + dt F,  dr = dt v,  |dr| = sqrt(dr.dr),  if |dr| > maxstep: dr = (maxstep dr) / |dr|,  r = r + dr.
 //
-// L-BFGS (Nocedal & Wright, Alg. 7.4) with g = -F, direction scratch D (n_rep, 3N).  On every step but the first:
+// k_lbfgs_step: L-BFGS (Nocedal & Wright, Alg. 7.4) with g = -F, direction scratch D (n_rep, 3N).  On every step but the first:
 //   s = r - r_prev, y = g - g_prev into the slot after the newest;  sy = s.y, yy = y.y;
 //   sy > 0: push (rho = 1 / sy, gamma = sy / yy), the ring holding the newest min(n + 1, m);  else clear the history;
 //   E > E_prev: clear the history.
@@ -111,14 +107,8 @@ struct RelaxParams {
 // E_prev = E, r = r + d.
 //
 // advance == 0 runs only the test (it sets conv and fmax2 for every replica).
-int launch_fire_step(const RelaxParams* P, RelaxState* st, double* R, double* V, const double* F, int64_t n_rep,
-                     int dimi, int advance, cudaStream_t s);
-int launch_lbfgs_step(const RelaxParams* P, RelaxState* st, double* R, double* D, const double* F, const double* E,
-                      int64_t n_rep, int dimi, int advance, cudaStream_t s);
-// the number of replicas not yet converged, written by the device into *n_active (host-mapped pinned memory)
-int launch_relax_count(const RelaxState* st, int64_t n_rep, int* n_active, cudaStream_t s);
-// n_steps (int64), conv (int32) and sqrt(fmax2) per replica, into device arrays; each may be null
-int launch_relax_report(const RelaxState* st, int64_t n_rep, int64_t* n_steps, int* conv, double* fmax,
-                        cudaStream_t s);
+//
+// k_relax_count writes the number of replicas not yet converged into *n_active (host-mapped pinned memory);
+// k_relax_report writes n_steps (int64), conv (int32) and sqrt(fmax2) per replica into device arrays, each may be null.
 
 }  // namespace sgdml

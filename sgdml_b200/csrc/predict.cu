@@ -29,7 +29,7 @@
 
 #include "common.cuh"
 #include "desc.cuh"
-#include "md.cuh"
+#include "predict.cuh"
 #include "solve.cuh"
 
 namespace sgdml {
@@ -1546,36 +1546,6 @@ int opt_in_smem(size_t dyn) {
   return 0;
 }
 
-// Captures the work enqueue() queues on gs (not the legacy stream) into *exec; *n_kernels: the kernel launches counted
-// while it was queued, which a replay of the graph counts again
-template <class Enqueue>
-int capture_graph(cudaStream_t gs, Enqueue&& enqueue, cudaGraphExec_t* exec, int* n_kernels) {
-  auto launches = [] {
-    int64_t n = 0;
-    for (int k = 0; k < KID_COUNT; ++k) {
-      int64_t ln = 0;
-      sgdml_b200_profile_get(k, nullptr, nullptr, &ln);
-      n += ln;
-    }
-    return n;
-  };
-  const int64_t before = launches();
-  cudaGraph_t graph = nullptr;
-  SG_CUDA(cudaStreamBeginCapture(gs, cudaStreamCaptureModeThreadLocal));
-  const int rc = enqueue();
-  cudaError_t e = cudaStreamEndCapture(gs, &graph);
-  if (rc != 0) {
-    if (graph) cudaGraphDestroy(graph);
-    return rc;
-  }
-  SG_CUDA(e);
-  e = cudaGraphInstantiate(exec, graph, 0);
-  cudaGraphDestroy(graph);
-  SG_CUDA(e);
-  *n_kernels = (int)(launches() - before);
-  return 0;
-}
-
 // The two FP64 contractions of the GEMM-composed path (D > 256, and every Hessian-vector product) over `rows` rows of A:
 //   S1 = A Xc^T, S2 = A JA^T        (rows x Mpad, contraction over the padded descriptor)
 int contract_desc(const sgdml_b200_model* m, const double* A, int64_t rows, double* S1, double* S2, cudaStream_t s) {
@@ -1620,7 +1590,7 @@ int contract_points(const sgdml_b200_model* m, const double* C1, const double* C
 constexpr int64_t GRAPH_MAX_GEO = 16;  // batches up to this size with host buffers replay a captured graph
 // xq == nullptr: the query rows (w.Qg, w.qq) are already in place (k_desc_query_rows)
 // W_dev != nullptr: the finishing kernels' virial variants also write W (n_geo x 9); E and F are unchanged by it
-// w: one of the model's workspace slots, or the workspace of an MD handle
+// w: one of the model's workspace slots, or a ForceEval's (predict.cuh)
 int run_queries(sgdml_b200_model* m, sgdml_b200_model::WS& w, const double* xq, const double* gq, int64_t n_geo,
                 double std, double c, double* E_dev, double* F_dev, cudaStream_t s, double* W_dev = nullptr) {
   const int64_t n_rows = n_geo * m->S;
@@ -1883,12 +1853,6 @@ int sgdml_b200_model_create(sgdml_b200_model** out, int64_t n_atoms, int64_t n_t
 
 namespace {
 
-// SGDML_B200_GRAPH=0 switches the CUDA-graph replay of small host-buffer batches off (the replay saves launch
-// overhead on the B = 1 NumPy in/out path of MD stepping)
-bool g_graph_enabled() {
-  const char* e = getenv("SGDML_B200_GRAPH");
-  return e != nullptr ? (e[0] == '1') : true;
-}
 bool g_graph_zero_copy() {
   const char* e = getenv("SGDML_B200_GRAPH_ZEROCOPY");
   return e != nullptr ? (e[0] == '1') : true;
@@ -2441,625 +2405,77 @@ int sgdml_b200_model_get_R_d_desc_alpha(sgdml_b200_model* m, double* out) {
 
 }  // extern "C"
 
-// ============================================================== molecular dynamics (sgdml_b200_md_*)
-// The state of n_rep replicas stays in device memory between steps and between runs.  One step is the integrator
-// kernel (csrc/md.cu), then the descriptors of the new positions in the model's cell and the predictor on them, chunk by
-// chunk, writing F and E_pot back into the state.  That sequence is captured once into a CUDA graph and replayed
-// n_steps times on the caller's stream; everything a run changes (dt, gamma, kT, seed, frame buffers) lives in device
-// memory, and the step counter is advanced by the integrator, so the graph bakes in no run.
-struct sgdml_b200_md {
+// ============================================================== force evaluation of the dynamics driver (predict.cuh)
+bool sgdml::g_graph_enabled() {
+  const char* e = getenv("SGDML_B200_GRAPH");
+  return e != nullptr ? (e[0] == '1') : true;
+}
+
+struct sgdml::ForceEval {
   sgdml_b200_model* m = nullptr;
-  int64_t n_rep = 0, chunk = 0;
-  int dimi = 0;
-  int nb = 1;  // beads per ring polymer: replica p nb + j is bead j of polymer p (1 for sgdml_b200_md_create)
-  sgdml_b200_model::WS ws;  // the handle's own predictor workspace: predict calls never touch it, MD never theirs
-  int ws_oz = 0;            // the int8 slice count its buffers were sized for
-  double *R = nullptr, *V = nullptr, *F = nullptr, *E = nullptr;  // state: (n_rep, 3N) x 3, (n_rep)
-  double *Fs = nullptr, *Es = nullptr;  // outputs of the force evaluation that precedes a capture
-  uint64_t* step = nullptr;             // (n_rep) step counters, all equal
-  uint64_t step_host = 0;               // their value once the queued runs have finished
-  bool has_state = false;
-  double *s = nullptr, *sigma = nullptr;  // (3N) inverse mass, (nb, 3N) noise scale per mode and coordinate
-  std::vector<double> s_host;             // s on the host
-  MdParams* dP = nullptr;
-  MdParams* hP = nullptr;     // pinned staging of dP and sigma, reused once the previous run's upload is done
-  double* hSigma = nullptr;
-  PimdParams* dQ = nullptr;  // the ring-polymer run's parameter block
-  PimdParams* hQ = nullptr;
-  double *tab = nullptr, *hTab = nullptr;  // C (nb x nb) and the four mode tables (nb each)
-  cudaEvent_t uploaded = nullptr;
-  cudaStream_t gs = nullptr;  // capture stream
-  cudaEvent_t ge = nullptr;
-  cudaGraphExec_t exec = nullptr;
-  int graph_kind = -1;        // the MdKind of the captured step
-  uint64_t generation = 0;    // the model's generation at capture
-  Lattice lat = {0, {0}, {0}};  // the model's cell at capture (passed to the descriptor kernel by value)
-  int n_kernels = 0;
-  // geometry optimisation (sgdml_b200_relax_*), allocated by the first relaxation
-  RelaxState* rst = nullptr;  // (n_rep) per-replica optimiser state
-  RelaxParams* dR = nullptr;
-  RelaxParams* hR = nullptr;  // pinned staging of dR
-  int* hActive = nullptr;     // mapped pinned: unconverged replicas, written by k_relax_count
-  int* dActive = nullptr;     // its device address
-  cudaEvent_t counted = nullptr;
-  double *S = nullptr, *Y = nullptr, *rho = nullptr;        // L-BFGS ring, m_cap pairs per replica
-  double *r_prev = nullptr, *g_prev = nullptr;              // (n_rep, 3N)
-  int m_cap = 0;
+  int64_t n_geo = 0, chunk = 0;
+  sgdml_b200_model::WS ws;
+  int ws_oz = 0;             // the int8 slice count ws was sized for
+  bool moved = false;        // ws was reallocated since the last force_eval_mark
+  uint64_t generation = 0;   // the model's generation and cell at the last force_eval_mark
+  Lattice lat = {0, {0}, {0}};
 };
 
 namespace {
-
-void md_free(sgdml_b200_md* md) {
-  cudaDeviceSynchronize();  // blocks go back to the cache: nothing may still use them
-  if (md->exec) cudaGraphExecDestroy(md->exec);
-  if (md->gs) cudaStreamDestroy(md->gs);
-  if (md->ge) cudaEventDestroy(md->ge);
-  if (md->uploaded) cudaEventDestroy(md->uploaded);
-  if (md->counted) cudaEventDestroy(md->counted);
-  free_ws_slot(md->ws);
-  for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s, md->sigma}) cached_free(p);
-  cached_free(md->step);
-  cached_free(md->dP);
-  cached_free(md->dQ);
-  cached_free(md->tab);
-  for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev}) cached_free(p);
-  cached_free(md->rst);
-  cached_free(md->dR);
-  cudaFreeHost(md->hR);
-  cudaFreeHost(md->hActive);
-  cudaFreeHost(md->hP);
-  cudaFreeHost(md->hQ);
-  cudaFreeHost(md->hTab);
-  cudaFreeHost(md->hSigma);
-  delete md;
-}
-
-// the workspace for the current model settings; a reallocation drops the captured step
-int md_ready(sgdml_b200_md* md) {
-  sgdml_b200_model* m = md->m;
-  if (md->ws_oz != m->oz_s) {  // slice buffers sized for another contraction setting
-    SG_CUDA(cudaDeviceSynchronize());
-    free_ws_slot(md->ws);
-    md->ws_oz = m->oz_s;
-  }
-  const int rc = grow_ws(m, md->ws, md->chunk);
-  if (rc != 0 && md->exec != nullptr) {
-    cudaGraphExecDestroy(md->exec);
-    md->exec = nullptr;
-  }
-  return rc < 0 ? rc : 0;
-}
-
-// F(R), E(R) of every replica, chunk by chunk, exactly as sgdml_b200_predict evaluates device-resident geometries
-int md_forces(sgdml_b200_md* md, double* F, double* E, cudaStream_t s) {
-  sgdml_b200_model* m = md->m;
-  sgdml_b200_model::WS& w = md->ws;
-  for (int64_t g0 = 0; g0 < md->n_rep; g0 += md->chunk) {
-    const int64_t ng = std::min<int64_t>(md->chunk, md->n_rep - g0);
-    SG_TRY(launch_desc_from_R(md->R + g0 * md->dimi, ng, m->N, w.xq, w.gq, s, m->lat, nullptr));
-    SG_TRY(run_queries(m, w, w.xq, w.gq, ng, m->std, m->c, E + g0, F + g0 * md->dimi, s));
-  }
-  return 0;
-}
-
-// what one step of the handle's graph integrates
-enum MdKind { MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3 };
-
-// the integrator of sgdml_b200_md_run, sgdml_b200_pimd_run or sgdml_b200_relax_*; advance == 0 completes a run's last
-// step (MD) or only tests convergence (relaxation).  L-BFGS keeps its direction in V, which relax_impl zeroes after.
-int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
-  switch (kind) {
-    case MD_RING_POLYMER:
-      return launch_pimd_step(md->dQ, md->tab, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step,
-                              md->n_rep / md->nb, md->dimi, md->nb, advance, s);
-    case MD_FIRE:
-      return launch_fire_step(md->dR, md->rst, md->R, md->V, md->F, md->n_rep, md->dimi, advance, s);
-    case MD_LBFGS:
-      return launch_lbfgs_step(md->dR, md->rst, md->R, md->V, md->F, md->E, md->n_rep, md->dimi, advance, s);
-    default:
-      return launch_md_step(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E, md->step, md->n_rep, md->dimi,
-                            advance, s);
-  }
-}
-
-int md_step(sgdml_b200_md* md, int kind, cudaStream_t s) {
-  SG_TRY(md_integrate(md, kind, 1, s));
-  return md_forces(md, md->F, md->E, s);
-}
 
 bool same_cell(const Lattice& a, const Lattice& b) {
   if (a.on != b.on) return false;
   return !a.on || (std::equal(a.vec, a.vec + 9, b.vec) && std::equal(a.inv, a.inv + 9, b.inv));
 }
 
-// the step graph, captured again whenever something it bakes in has changed: the workspace (md_ready), the model's
-// generation (use_ae, contraction slices), the model's cell, or the integrator (MdKind)
-int md_graph(sgdml_b200_md* md, int kind, cudaStream_t s) {
-  sgdml_b200_model* m = md->m;
-  if (md->exec != nullptr && md->generation == m->generation && same_cell(md->lat, m->lat) && md->graph_kind == kind)
-    return 0;
-  if (md->exec != nullptr) {
-    cudaGraphExecDestroy(md->exec);
-    md->exec = nullptr;
-  }
-  if (md->gs == nullptr) {
-    SG_CUDA(cudaStreamCreateWithFlags(&md->gs, cudaStreamNonBlocking));
-    SG_CUDA(cudaEventCreateWithFlags(&md->ge, cudaEventDisableTiming));
-  }
-  // captured on a private stream (the caller's may be the legacy stream); after the caller's queued work
-  SG_CUDA(cudaEventRecord(md->ge, s));
-  SG_CUDA(cudaStreamWaitEvent(md->gs, md->ge, 0));
-  // the force evaluation once un-captured, into scratch outputs: sets the kernels' shared-memory attributes
-  SG_TRY(md_forces(md, md->Fs, md->Es, md->gs));
-  SG_CUDA(cudaStreamSynchronize(md->gs));
-  SG_TRY(capture_graph(md->gs, [&] { return md_step(md, kind, md->gs); }, &md->exec, &md->n_kernels));
-  md->generation = m->generation;
-  md->lat = m->lat;
-  md->graph_kind = kind;
-  return 0;
-}
-
-// a frame output: the caller's device buffer, or device staging for a host buffer (copied back at the end)
-struct FrameOut {
-  double* user = nullptr;
-  double* dev = nullptr;
-  size_t bytes = 0;
-  bool staged = false;
-  int init(double* p, size_t b) {
-    user = p;
-    bytes = b;
-    if (p == nullptr) return 0;
-    if (is_device_ptr(p)) {
-      dev = p;
-      return 0;
-    }
-    staged = true;
-    SG_CUDA(cached_malloc(&dev, b));
-    return 0;
-  }
-  ~FrameOut() {
-    if (staged) cached_free(dev);
-  }
-};
-
-// n_steps steps after the run's parameters are queued: graph replays or plain launches, then the completing launch
-// and the copy of host-staged frames
-// n_steps steps of the handle's integrator: graph replays, or plain launches with SGDML_B200_GRAPH=0 or profiling
-int md_replay(sgdml_b200_md* md, int kind, int64_t n_steps, cudaStream_t s) {
-  if (g_graph_enabled() && !profiling_enabled()) {
-    SG_TRY(md_graph(md, kind, s));
-    for (int64_t k = 0; k < n_steps; ++k) {
-      SG_CUDA(cudaGraphLaunch(md->exec, s));
-      count_launch(KID_PREDICT_AUX, md->n_kernels);  // the kernels of a replay are launches too
-    }
-  } else {
-    for (int64_t k = 0; k < n_steps; ++k) SG_TRY(md_step(md, kind, s));
-  }
-  return 0;
-}
-
-int md_steps(sgdml_b200_md* md, int kind, int64_t n_steps, FrameOut* out, int n_out, cudaStream_t s) {
-  SG_TRY(md_replay(md, kind, n_steps, s));
-  md->step_host += (uint64_t)n_steps;
-  // the second half-kick of the last step (and its frame)
-  SG_TRY(md_integrate(md, kind, 0, s));
-  bool sync = false;
-  for (int i = 0; i < n_out; ++i)
-    if (out[i].staged) {
-      SG_CUDA(cudaMemcpyAsync(out[i].user, out[i].dev, out[i].bytes, cudaMemcpyDeviceToHost, s));
-      sync = true;
-    }
-  if (sync) SG_CUDA(cudaStreamSynchronize(s));
-  return 0;
-}
-
-int md_run_impl(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, uint64_t seed, int64_t stride,
-                double* R_f, double* V_f, double* Ep_f, double* Ek_f, cudaStream_t s) {
-  const int64_t n_frames = stride > 0 ? n_steps / stride : 0;
-  const size_t fr = sizeof(double) * (size_t)(n_frames * md->n_rep);
-  FrameOut out[4];
-  if (n_frames > 0) {
-    SG_TRY(out[0].init(R_f, fr * md->dimi));
-    SG_TRY(out[1].init(V_f, fr * md->dimi));
-    SG_TRY(out[2].init(Ep_f, fr));
-    SG_TRY(out[3].init(Ek_f, fr));
-  }
-  SG_TRY(md_ready(md));
-  // the run's constants, once on the host in double precision
-  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous run has read the staging
-  MdParams& p = *md->hP;
-  p.h = 0.5 * dt;
-  p.c1 = std::exp(-gamma * dt);
-  p.key[0] = (uint32_t)seed;
-  p.key[1] = (uint32_t)(seed >> 32);
-  p.use_O = gamma > 0.0 ? 1 : 0;
-  p.stride = n_frames > 0 ? (int)stride : 0;
-  p.run_start = md->step_host;
-  p.R_f = out[0].dev;
-  p.V_f = out[1].dev;
-  p.Ep_f = out[2].dev;
-  p.Ek_f = out[3].dev;
-  for (int i = 0; i < md->dimi; ++i) md->hSigma[i] = std::sqrt((1.0 - p.c1 * p.c1) * kT * md->s_host[(size_t)i]);
-  SG_CUDA(cudaMemcpyAsync(md->dP, md->hP, sizeof(MdParams), cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * md->dimi, cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaEventRecord(md->uploaded, s));
-  return md_steps(md, MD_CLASSICAL, n_steps, out, 4, s);
-}
-
-int pimd_run_impl(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma, double lambda,
-                  uint64_t seed, int64_t stride, double* R_f, double* V_f, double* Ep_f, double* Ek_f, double* Kp_f,
-                  double* Kcv_f, cudaStream_t s) {
-  const int nb = md->nb, dimi = md->dimi;
-  const int64_t n_poly = md->n_rep / nb;
-  const int64_t n_frames = stride > 0 ? n_steps / stride : 0;
-  const size_t fr = sizeof(double) * (size_t)(n_frames * md->n_rep);
-  const size_t fp = sizeof(double) * (size_t)(n_frames * n_poly);
-  FrameOut out[6];
-  if (n_frames > 0) {
-    SG_TRY(out[0].init(R_f, fr * dimi));
-    SG_TRY(out[1].init(V_f, fr * dimi));
-    SG_TRY(out[2].init(Ep_f, fr));
-    SG_TRY(out[3].init(Ek_f, fr));
-    SG_TRY(out[4].init(Kp_f, fp));
-    SG_TRY(out[5].init(Kcv_f, fp));
-  }
-  SG_TRY(md_ready(md));
-  // the run's constants, once on the host in double precision (tests/pimd_oracle.py restates them)
-  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous run has read the staging
-  PimdParams& p = *md->hQ;
-  const double h = 0.5 * dt;
-  const double kTP = nb * kT;
-  const double wP = kTP / hbar;
-  p.h = h;
-  p.key[0] = (uint32_t)seed;
-  p.key[1] = (uint32_t)(seed >> 32);
-  p.use_O = gamma > 0.0 || (lambda > 0.0 && nb > 1) ? 1 : 0;
-  p.stride = n_frames > 0 ? (int)stride : 0;
-  p.run_start = md->step_host;
-  p.kprim0 = 0.5 * (double)(dimi * nb) * kT;
-  p.kspring = 0.5 * wP * wP / nb;
-  p.kcv0 = 0.5 * dimi * kT;
-  p.kvir = 0.5 / nb;
-  p.R_f = out[0].dev;
-  p.V_f = out[1].dev;
-  p.Ep_f = out[2].dev;
-  p.Ek_f = out[3].dev;
-  p.Kp_f = out[4].dev;
-  p.Kcv_f = out[5].dev;
-  double* C = md->hTab;
-  double *m_cos = C + nb * nb, *m_sow = m_cos + nb, *m_msin = m_sow + nb, *m_c1 = m_msin + nb;
-  for (int j = 0; j < nb; ++j)
-    for (int k = 0; k < nb; ++k) {
-      double c;
-      if (k == 0)
-        c = std::sqrt(1.0 / nb);
-      else if (2 * k < nb)
-        c = std::sqrt(2.0 / nb) * std::cos(2.0 * M_PI * j * k / nb);
-      else if (2 * k == nb)
-        c = std::sqrt(1.0 / nb) * (j % 2 ? -1.0 : 1.0);
-      else
-        c = std::sqrt(2.0 / nb) * std::sin(2.0 * M_PI * j * k / nb);
-      C[j * nb + k] = c;
-    }
-  for (int k = 0; k < nb; ++k) {
-    double g = gamma;
-    m_cos[k] = 1.0;
-    m_sow[k] = h;
-    m_msin[k] = 0.0;
-    if (k > 0) {
-      const double wk = 2.0 * wP * std::sin(M_PI * k / nb);
-      m_cos[k] = std::cos(wk * h);
-      m_sow[k] = std::sin(wk * h) / wk;
-      m_msin[k] = -wk * std::sin(wk * h);
-      g = 2.0 * lambda * wk;
-    }
-    m_c1[k] = std::exp(-g * dt);
-    for (int i = 0; i < dimi; ++i)
-      md->hSigma[(size_t)k * dimi + i] = std::sqrt((1.0 - m_c1[k] * m_c1[k]) * kTP * md->s_host[(size_t)i]);
-  }
-  SG_CUDA(cudaMemcpyAsync(md->dQ, md->hQ, sizeof(PimdParams), cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaMemcpyAsync(md->tab, md->hTab, sizeof(double) * (nb * nb + 4 * nb), cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * nb * dimi, cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaEventRecord(md->uploaded, s));
-  return md_steps(md, MD_RING_POLYMER, n_steps, out, 6, s);
-}
-
-// ------------------------------------------------------------------ geometry optimisation (sgdml_b200_relax_*)
-constexpr int64_t RELAX_BLOCK = 16;  // replays between convergence read-backs
-int64_t g_relax_block = 0;           // sgdml_b200_set_relax_block (test hook): 0 = RELAX_BLOCK
-
-// the optimiser state, made at the first relaxation; the L-BFGS ring grows to `memory` pairs per replica
-int relax_alloc(sgdml_b200_md* md, int memory) {
-  if (md->rst == nullptr) SG_CUDA(cached_malloc(&md->rst, sizeof(RelaxState) * (size_t)md->n_rep));
-  if (md->dR == nullptr) SG_CUDA(cached_malloc(&md->dR, sizeof(RelaxParams)));
-  if (md->hR == nullptr) SG_CUDA(cudaMallocHost(&md->hR, sizeof(RelaxParams)));
-  if (md->hActive == nullptr) {
-    SG_CUDA(cudaHostAlloc(&md->hActive, sizeof(int), cudaHostAllocMapped));
-    SG_CUDA(cudaHostGetDevicePointer((void**)&md->dActive, md->hActive, 0));
-  }
-  if (md->counted == nullptr) SG_CUDA(cudaEventCreateWithFlags(&md->counted, cudaEventDisableTiming));
-  if (memory > md->m_cap) {
-    const size_t vec = sizeof(double) * (size_t)(md->n_rep * md->dimi);
-    SG_CUDA(cudaDeviceSynchronize());  // the old ring goes back to the cache: nothing may still use it
-    for (double** p : {&md->S, &md->Y, &md->rho}) {
-      cached_free(*p);
-      *p = nullptr;
-    }
-    md->m_cap = 0;
-    SG_CUDA(cached_malloc(&md->S, vec * memory));
-    SG_CUDA(cached_malloc(&md->Y, vec * memory));
-    SG_CUDA(cached_malloc(&md->rho, sizeof(double) * (size_t)md->n_rep * memory));
-    if (md->r_prev == nullptr) {
-      SG_CUDA(cached_malloc(&md->r_prev, vec));
-      SG_CUDA(cached_malloc(&md->g_prev, vec));
-    }
-    md->m_cap = memory;
-  }
-  return 0;
-}
-
-// Relaxes every replica from the handle's state: blocks of step-graph replays, each followed by the convergence test
-// and a count of unconverged replicas read back through mapped pinned memory; stops when none is left or after
-// max_steps.  Frozen replicas make the block length a matter of cost only.  V is zero before and after.
-int relax_impl(sgdml_b200_md* md, int kind, int64_t max_steps, const RelaxParams& prm, int64_t* n_steps_out,
-               int* conv_out, double* fmax_out, cudaStream_t s) {
-  const int64_t n_rep = md->n_rep;
-  SG_TRY(md_ready(md));
-  SG_TRY(relax_alloc(md, kind == MD_LBFGS ? prm.memory : 0));
-  // outputs: the caller's device arrays, or one device staging block for the host ones
-  void* user[3] = {n_steps_out, conv_out, fmax_out};
-  const size_t bytes[3] = {sizeof(int64_t) * (size_t)n_rep, sizeof(int) * (size_t)n_rep,
-                           sizeof(double) * (size_t)n_rep};
-  void* dev[3] = {nullptr, nullptr, nullptr};
-  char* stage = nullptr;
-  size_t staged = 0;
-  for (int i = 0; i < 3; ++i)
-    if (user[i] != nullptr && !is_device_ptr(user[i])) staged += (bytes[i] + 255) & ~(size_t)255;
-  if (staged > 0) SG_CUDA(cached_malloc(&stage, staged));
-  auto body = [&]() -> int {
-    size_t off = 0;
-    for (int i = 0; i < 3; ++i) {
-      if (user[i] == nullptr) continue;
-      if (is_device_ptr(user[i])) {
-        dev[i] = user[i];
-      } else {
-        dev[i] = stage + off;
-        off += (bytes[i] + 255) & ~(size_t)255;
-      }
-    }
-    SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the staging
-    RelaxParams& p = *md->hR;
-    p = prm;
-    p.m_cap = md->m_cap;
-    p.S = md->S;
-    p.Y = md->Y;
-    p.rho = md->rho;
-    p.r_prev = md->r_prev;
-    p.g_prev = md->g_prev;
-    SG_CUDA(cudaMemcpyAsync(md->dR, md->hR, sizeof(RelaxParams), cudaMemcpyHostToDevice, s));
-    SG_CUDA(cudaEventRecord(md->uploaded, s));
-    const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
-    SG_CUDA(cudaMemsetAsync(md->rst, 0, sizeof(RelaxState) * (size_t)n_rep, s));
-    SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
-    const int64_t block = g_relax_block > 0 ? g_relax_block : RELAX_BLOCK;
-    for (int64_t done = 0;;) {
-      SG_TRY(md_integrate(md, kind, 0, s));  // the test on the current forces
-      SG_TRY(launch_relax_count(md->rst, n_rep, md->dActive, s));
-      SG_CUDA(cudaEventRecord(md->counted, s));
-      SG_CUDA(cudaEventSynchronize(md->counted));
-      if (*(volatile int*)md->hActive == 0 || done >= max_steps) break;
-      const int64_t n = std::min(block, max_steps - done);
-      SG_TRY(md_replay(md, kind, n, s));
-      done += n;
-    }
-    SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));  // a following MD run starts at rest
-    SG_TRY(launch_relax_report(md->rst, n_rep, (int64_t*)dev[0], (int*)dev[1], (double*)dev[2], s));
-    for (int i = 0; i < 3; ++i)
-      if (dev[i] != nullptr && dev[i] != user[i])
-        SG_CUDA(cudaMemcpyAsync(user[i], dev[i], bytes[i], cudaMemcpyDeviceToHost, s));
-    if (staged > 0) SG_CUDA(cudaStreamSynchronize(s));
-    return 0;
-  };
-  const int rc = body();
-  if (stage != nullptr) {
-    if (rc != 0) cudaStreamSynchronize(s);
-    cached_free(stage);
-  }
-  return rc;
-}
-
-// the checks both optimisers share; a rejected call queues nothing
-int relax_check(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, const char* what) {
-  SG_ARG(md != nullptr && max_steps >= 0);
-  SG_ARG(std::isfinite(fmax) && fmax >= 0.0);
-  SG_ARG(std::isfinite(maxstep) && maxstep > 0.0);
-  if (!md->has_state) return fail_arg(what);
-  return 0;
-}
-
-// a handle of n_rep = n_poly nb replicas; the caller has checked the counts
-int md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, int nb, const double* inv_mass) {
-  SG_ARG(!is_device_ptr(inv_mass));
-  for (int i = 0; i < m->N; ++i)
-    if (!(std::isfinite(inv_mass[i]) && inv_mass[i] > 0.0)) return fail_arg("inv_mass must be finite and > 0");
-  sgdml_b200_md* md = new sgdml_b200_md();
-  md->m = m;
-  md->n_rep = n_rep;
-  md->nb = nb;
-  md->dimi = 3 * m->N;
-  md->chunk = std::min<int64_t>(chunk_geos(m), n_rep);
-  md->ws_oz = m->oz_s;
-  auto body = [&]() -> int {
-    const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
-    for (double** p : {&md->R, &md->V, &md->F, &md->Fs}) SG_CUDA(cached_malloc(p, st));
-    SG_CUDA(cached_malloc(&md->E, sizeof(double) * n_rep));
-    SG_CUDA(cached_malloc(&md->Es, sizeof(double) * n_rep));
-    SG_CUDA(cached_malloc(&md->step, sizeof(uint64_t) * n_rep));
-    SG_CUDA(cached_malloc(&md->s, sizeof(double) * md->dimi));
-    SG_CUDA(cached_malloc(&md->sigma, sizeof(double) * nb * md->dimi));
-    SG_CUDA(cached_malloc(&md->dP, sizeof(MdParams)));
-    SG_CUDA(cached_malloc(&md->dQ, sizeof(PimdParams)));
-    SG_CUDA(cached_malloc(&md->tab, sizeof(double) * (nb * nb + 4 * nb)));
-    SG_CUDA(cudaMallocHost(&md->hP, sizeof(MdParams)));
-    SG_CUDA(cudaMallocHost(&md->hQ, sizeof(PimdParams)));
-    SG_CUDA(cudaMallocHost(&md->hTab, sizeof(double) * (nb * nb + 4 * nb)));
-    SG_CUDA(cudaMallocHost(&md->hSigma, sizeof(double) * nb * md->dimi));
-    SG_CUDA(cudaEventCreateWithFlags(&md->uploaded, cudaEventDisableTiming));
-    md->s_host.resize((size_t)md->dimi);
-    for (int i = 0; i < md->dimi; ++i) md->s_host[(size_t)i] = inv_mass[i / 3];
-    SG_CUDA(cudaMemcpy(md->s, md->s_host.data(), sizeof(double) * md->dimi, cudaMemcpyHostToDevice));
-    SG_TRY(md_ready(md));
-    return 0;
-  };
-  const int rc = body();
-  if (rc != 0) {
-    md_free(md);
-    return rc;
-  }
-  *out = md;
-  return 0;
-}
-
 }  // namespace
 
-extern "C" {
-
-int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, const double* inv_mass) {
-  SG_TRY(require_device());
-  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
-  SG_ARG(n_rep >= 1 && n_rep <= INT32_MAX);
-  return md_create(out, m, n_rep, 1, inv_mass);
-}
-
-int sgdml_b200_pimd_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_poly, int64_t n_beads,
-                           const double* inv_mass) {
-  SG_TRY(require_device());
-  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
-  SG_ARG(n_beads >= 1 && n_beads <= PIMD_MAX_BEADS);
-  SG_ARG(n_poly >= 1 && n_poly <= INT32_MAX / n_beads);
-  return md_create(out, m, n_poly * n_beads, (int)n_beads, inv_mass);
-}
-
-int sgdml_b200_md_destroy(sgdml_b200_md* md) {
-  if (md != nullptr) md_free(md);
+int sgdml::force_eval_create(sgdml_b200_model* m, int64_t n_geo, ForceEval** out) {
+  ForceEval* fe = new ForceEval();
+  fe->m = m;
+  fe->n_geo = n_geo;
+  fe->chunk = std::min<int64_t>(chunk_geos(m), n_geo);
+  fe->ws_oz = m->oz_s;
+  *out = fe;
   return 0;
 }
 
-int sgdml_b200_md_set_state(sgdml_b200_md* md, const double* R, const double* V, uint64_t step, void* stream) {
-  SG_TRY(require_device());
-  SG_ARG(md != nullptr && R != nullptr);
-  cudaStream_t s = (cudaStream_t)stream;
-  const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
-  SG_TRY(md_ready(md));
-  SG_CUDA(cudaMemcpyAsync(md->R, R, st, cudaMemcpyDefault, s));
-  if (V != nullptr)
-    SG_CUDA(cudaMemcpyAsync(md->V, V, st, cudaMemcpyDefault, s));
-  else
-    SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
-  const std::vector<uint64_t> steps((size_t)md->n_rep, step);
-  SG_CUDA(cudaMemcpyAsync(md->step, steps.data(), sizeof(uint64_t) * md->n_rep, cudaMemcpyHostToDevice, s));
-  SG_TRY(md_forces(md, md->F, md->E, s));
-  SG_CUDA(cudaStreamSynchronize(s));  // (the counters' host vector goes out of scope)
-  md->step_host = step;
-  md->has_state = true;
+void sgdml::force_eval_destroy(ForceEval* fe) {
+  if (fe == nullptr) return;
+  free_ws_slot(fe->ws);
+  delete fe;
+}
+
+int sgdml::force_eval_prepare(ForceEval* fe) {
+  sgdml_b200_model* m = fe->m;
+  if (fe->ws_oz != m->oz_s) {  // slice buffers sized for another contraction setting
+    SG_CUDA(cudaDeviceSynchronize());
+    free_ws_slot(fe->ws);
+    fe->ws_oz = m->oz_s;
+  }
+  const int rc = grow_ws(m, fe->ws, fe->chunk);
+  if (rc != 0) fe->moved = true;
+  return rc < 0 ? rc : 0;
+}
+
+bool sgdml::force_eval_stale(const ForceEval* fe) {
+  return fe->moved || fe->generation != fe->m->generation || !same_cell(fe->lat, fe->m->lat);
+}
+
+void sgdml::force_eval_mark(ForceEval* fe) {
+  fe->moved = false;
+  fe->generation = fe->m->generation;
+  fe->lat = fe->m->lat;
+}
+
+int sgdml::force_eval_run(ForceEval* fe, const double* R, double* F, double* E, cudaStream_t s) {
+  sgdml_b200_model* m = fe->m;
+  sgdml_b200_model::WS& w = fe->ws;
+  const int dimi = 3 * m->N;
+  for (int64_t g0 = 0; g0 < fe->n_geo; g0 += fe->chunk) {
+    const int64_t ng = std::min<int64_t>(fe->chunk, fe->n_geo - g0);
+    SG_TRY(launch_desc_from_R(R + g0 * dimi, ng, m->N, w.xq, w.gq, s, m->lat, nullptr));
+    SG_TRY(run_queries(m, w, w.xq, w.gq, ng, m->std, m->c, E + g0, F + g0 * dimi, s));
+  }
   return 0;
 }
-
-int sgdml_b200_md_get_state(sgdml_b200_md* md, double* R, double* V, double* F, double* E_pot, uint64_t* step,
-                            void* stream) {
-  SG_TRY(require_device());
-  SG_ARG(md != nullptr);
-  if (!md->has_state) return fail_arg("sgdml_b200_md_get_state: no state yet (call sgdml_b200_md_set_state)");
-  cudaStream_t s = (cudaStream_t)stream;
-  const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
-  bool host = false;
-  auto get = [&](void* dst, const void* src, size_t bytes) -> int {
-    if (dst == nullptr) return 0;
-    host = host || !is_device_ptr(dst);
-    SG_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, s));
-    return 0;
-  };
-  SG_TRY(get(R, md->R, st));
-  SG_TRY(get(V, md->V, st));
-  SG_TRY(get(F, md->F, st));
-  SG_TRY(get(E_pot, md->E, sizeof(double) * md->n_rep));
-  SG_TRY(get(step, md->step, sizeof(uint64_t)));
-  if (host) SG_CUDA(cudaStreamSynchronize(s));
-  return 0;
-}
-
-int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, uint64_t seed,
-                      int64_t stride, double* R_frames, double* V_frames, double* E_pot_frames, double* E_kin_frames,
-                      void* stream) {
-  SG_TRY(require_device());
-  SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
-  if (md->nb > 1) return fail_arg("sgdml_b200_md_run: a ring-polymer handle (n_beads > 1) runs with sgdml_b200_pimd_run");
-  SG_ARG(std::isfinite(dt) && dt > 0.0);
-  SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
-  SG_ARG(std::isfinite(kT) && kT >= 0.0);
-  if (kT > 0.0 && gamma == 0.0) return fail_arg("kT > 0 needs a friction gamma > 0 (a thermostat without coupling)");
-  if (stride > 0 && n_steps % stride != 0) return fail_arg("n_steps must be a multiple of stride");
-  if (!md->has_state) return fail_arg("sgdml_b200_md_run: no state yet (call sgdml_b200_md_set_state)");
-  if (n_steps == 0) return 0;
-  return md_run_impl(md, n_steps, dt, gamma, kT, seed, stride, R_frames, V_frames, E_pot_frames, E_kin_frames,
-                     (cudaStream_t)stream);
-}
-
-int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma,
-                        double lambda, uint64_t seed, int64_t stride, double* R_frames, double* V_frames,
-                        double* E_pot_frames, double* E_kin_frames, double* K_prim_frames, double* K_cv_frames,
-                        void* stream) {
-  SG_TRY(require_device());
-  SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
-  SG_ARG(std::isfinite(dt) && dt > 0.0);
-  SG_ARG(std::isfinite(kT) && kT >= 0.0);
-  SG_ARG(std::isfinite(hbar) && hbar > 0.0);
-  SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
-  SG_ARG(std::isfinite(lambda) && lambda >= 0.0);
-  if (md->nb > 1 && kT == 0.0) return fail_arg("a ring polymer (n_beads > 1) needs kT > 0");
-  if (md->nb == 1 && kT > 0.0 && gamma == 0.0)
-    return fail_arg("kT > 0 needs a friction gamma > 0 (a thermostat without coupling)");
-  if (stride > 0 && n_steps % stride != 0) return fail_arg("n_steps must be a multiple of stride");
-  if (!md->has_state) return fail_arg("sgdml_b200_pimd_run: no state yet (call sgdml_b200_md_set_state)");
-  if (n_steps == 0) return 0;
-  return pimd_run_impl(md, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, R_frames, V_frames, E_pot_frames,
-                       E_kin_frames, K_prim_frames, K_cv_frames, (cudaStream_t)stream);
-}
-
-int sgdml_b200_relax_fire(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, double dt, double dtmax,
-                          int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream) {
-  SG_TRY(require_device());
-  SG_TRY(relax_check(md, max_steps, fmax, maxstep,
-                     "sgdml_b200_relax_fire: no state yet (call sgdml_b200_md_set_state)"));
-  SG_ARG(std::isfinite(dt) && dt > 0.0);
-  SG_ARG(std::isfinite(dtmax) && dtmax > 0.0);
-  RelaxParams p = {};
-  p.fmax2 = fmax * fmax;
-  p.maxstep = maxstep;
-  p.dt0 = dt;
-  p.dtmax = dtmax;
-  return relax_impl(md, MD_FIRE, max_steps, p, n_steps_out, converged_out, fmax_out, (cudaStream_t)stream);
-}
-
-int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, int memory, double h0,
-                           int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream) {
-  SG_TRY(require_device());
-  SG_TRY(relax_check(md, max_steps, fmax, maxstep,
-                     "sgdml_b200_relax_lbfgs: no state yet (call sgdml_b200_md_set_state)"));
-  SG_ARG(memory >= 1 && memory <= LBFGS_MAX_MEMORY);
-  SG_ARG(std::isfinite(h0) && h0 > 0.0);
-  RelaxParams p = {};
-  p.fmax2 = fmax * fmax;
-  p.maxstep = maxstep;
-  p.h0 = h0;
-  p.memory = memory;
-  return relax_impl(md, MD_LBFGS, max_steps, p, n_steps_out, converged_out, fmax_out, (cudaStream_t)stream);
-}
-
-int sgdml_b200_set_relax_block(int64_t n_steps) {
-  SG_ARG(n_steps >= 0);
-  g_relax_block = n_steps;
-  return 0;
-}
-
-}  // extern "C"

@@ -132,12 +132,17 @@ class GDMLDynamics(object):
         )
         return {'R': R, 'V': V, 'F': F, 'E_pot': E, 'step': int(step[0])}
 
+    def _frames(self, n_steps, stride, frames, n_poly=0):
+        """Empty frame arrays for the names in `frames`: (n_frames, n_replicas, 3N) for R and V, (n_frames, n_poly) for
+        K_prim and K_cv, else (n_frames, n_replicas); {} when the run writes no frames."""
+        n_frames = n_steps // stride if stride > 0 and n_steps % stride == 0 else 0
+        dims = {'R': (self.n_replicas, 3 * self.n_atoms), 'V': (self.n_replicas, 3 * self.n_atoms), 'K_prim': (n_poly,),
+                'K_cv': (n_poly,)}
+        return {k: self._empty((n_frames,) + dims.get(k, (self.n_replicas,))) for k in frames} if n_frames > 0 else {}
+
     def _run_raw(self, n_steps, dt, gamma=0.0, kT=0.0, seed=0, stride=0, frames=('R', 'V', 'E_pot', 'E_kin')):
         n_steps, stride = int(n_steps), int(stride)
-        n_frames = n_steps // stride if stride > 0 and n_steps % stride == 0 else 0
-        shape = {'R': (n_frames, self.n_replicas, 3 * self.n_atoms), 'V': (n_frames, self.n_replicas, 3 * self.n_atoms),
-                 'E_pot': (n_frames, self.n_replicas), 'E_kin': (n_frames, self.n_replicas)}
-        out = {k: self._empty(shape[k]) for k in frames} if n_frames > 0 else {}
+        out = self._frames(n_steps, stride, frames)
         _lib.check(
             _lib.lib().sgdml_b200_md_run(self._handle, n_steps, float(dt), float(gamma), float(kT), int(seed), stride,
                                          *(_lib.ptr(out.get(k)) for k in ('R', 'V', 'E_pot', 'E_kin')),
@@ -221,11 +226,7 @@ class GDMLPathIntegralDynamics(GDMLDynamics):
     def _run_raw(self, n_steps, dt, kT, hbar, gamma=0.0, lam=0.0, seed=0, stride=0,
                  frames=('R', 'V', 'E_pot', 'E_kin', 'K_prim', 'K_cv')):
         n_steps, stride = int(n_steps), int(stride)
-        n_frames = n_steps // stride if stride > 0 and n_steps % stride == 0 else 0
-        B, dimi = self.n_replicas, 3 * self.n_atoms
-        shape = {'R': (n_frames, B, dimi), 'V': (n_frames, B, dimi), 'E_pot': (n_frames, B), 'E_kin': (n_frames, B),
-                 'K_prim': (n_frames, self.n_polymers), 'K_cv': (n_frames, self.n_polymers)}
-        out = {k: self._empty(shape[k]) for k in frames} if n_frames > 0 else {}
+        out = self._frames(n_steps, stride, frames, self.n_polymers)
         _lib.check(
             _lib.lib().sgdml_b200_pimd_run(self._handle, n_steps, float(dt), float(kT), float(hbar), float(gamma),
                                            float(lam), int(seed), stride,

@@ -15,9 +15,7 @@ import pytest
 
 import md_oracle
 from conftest import rel_err
-
-FIXTURES_MD = ['n5_m10_s1', 'n9_m16_s6', 'n12_m8_s12', 'n21_m6_s6', 'ecstr_n6_m8', 'pbc_n6_m8', 'big_n100_m2_s12',
-               'big_n240_m2_s3']
+from md_common import FIXTURES_MD, _K_SPRING, _N_SPRING, _cuda_forces, md_fs_masses, spring_task  # noqa: F401
 
 
 # ---------------------------------------------------------------------------------------------------- CPU
@@ -117,24 +115,6 @@ def _setup(name, n_rep=3, chunk=0, slices=0):
     dt = float(np.sqrt(2e-3 / np.max(np.abs(F0 * s))))
     V0 = np.random.default_rng(2).standard_normal(R0.shape) * 1e-3 / dt
     return gp, dyn, R0, V0, dt
-
-
-def md_fs_masses(m):
-    """Masses (amu) for which GDMLDynamics with E_to_eV = F_to_eV_Ang = 1 has the inverse masses 1 / m (model units,
-    femtoseconds)."""
-    from sgdml_b200 import md
-
-    return md.FS**2 * np.asarray(m, dtype=np.float64)
-
-
-def _cuda_forces(gp):
-    import torch
-
-    def forces(R):
-        E, F = gp.predict(torch.from_numpy(np.ascontiguousarray(R)).cuda())
-        return E.cpu().numpy(), F.cpu().numpy()
-
-    return forces
 
 
 def _same(a, b):
@@ -293,34 +273,6 @@ def test_equipartition():
     want = 1.5 * gp.n_atoms * kT
     print('<E_kin> = %.6g, (3N/2) kT = %.6g, standard error %.3g' % (series.mean(), want, se))
     assert abs(series.mean() - want) < 5.0 * se
-
-
-# harmonic pair springs about the base geometry: a bound PES for the conservation test
-_N_SPRING, _K_SPRING = 5, 2.0
-
-
-def _spring_pes(R):
-    from sgdml_b200 import synth
-
-    r0 = synth.base_geometry(_N_SPRING)
-    d0 = np.sqrt(((r0[:, None] - r0[None]) ** 2).sum(-1))
-    R = np.asarray(R, dtype=np.float64).reshape(-1, _N_SPRING, 3)
-    diff = R[:, :, None, :] - R[:, None, :, :]
-    d = np.sqrt((diff * diff).sum(-1)) + np.eye(_N_SPRING)
-    ext = (d - d0 - np.eye(_N_SPRING)) * (1 - np.eye(_N_SPRING))
-    E = 0.25 * _K_SPRING * (ext * ext).sum((1, 2))
-    F = -_K_SPRING * (ext[..., None] * diff / d[..., None]).sum(2)
-    return E, F
-
-
-@pytest.fixture(scope='module')
-def spring_task():
-    from sgdml_b200 import synth
-
-    task = synth.make_task(_N_SPRING, 60, np.arange(_N_SPRING)[None], 4, seed=3)
-    task['E_train'], task['F_train'] = _spring_pes(task['R_train'])
-    task['dataset_theory'] = 'harmonic_springs'
-    return task
 
 
 # max |E_tot(t) - E_tot(0)| / E_kin(0) over 2000 velocity-Verlet steps (dt = 0.02 / omega of the stiffest spring) of

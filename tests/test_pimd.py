@@ -10,17 +10,9 @@ import pytest
 
 import pimd_oracle
 from conftest import rel_err
+from md_common import FIXTURES_MD, _N_SPRING, _cuda_forces, make_spring_task, md_fs_masses
 
-FIXTURES_MD = ['n5_m10_s1', 'n9_m16_s6', 'n12_m8_s12', 'n21_m6_s6', 'ecstr_n6_m8', 'pbc_n6_m8', 'big_n100_m2_s12',
-               'big_n240_m2_s3']
 CASES = [(name, P) for name in FIXTURES_MD for P in (2, 3, 8)] + [('n9_m16_s6', 32), ('big_n240_m2_s3', 32)]
-
-
-def md_fs_masses(m):
-    """Masses (amu) for which the engine's inverse masses are 1 / m in model units and femtoseconds."""
-    from sgdml_b200 import md
-
-    return md.FS**2 * np.asarray(m, dtype=np.float64)
 
 
 def _setup(name, P, n_poly=2, chunk=0):
@@ -47,16 +39,6 @@ def _setup(name, P, n_poly=2, chunk=0):
     kT = float(np.mean(V0 * V0 / s))
     hbar = P * kT * dt / 0.4  # omega_P dt = 0.4
     return gp, dyn, R0.reshape(n_poly, P, -1), V0.reshape(n_poly, P, -1), s, dt, kT, hbar
-
-
-def _cuda_forces(gp):
-    import torch
-
-    def forces(R):
-        E, F = gp.predict(torch.from_numpy(np.ascontiguousarray(R)).cuda())
-        return E.cpu().numpy(), F.cpu().numpy()
-
-    return forces
 
 
 def _flat(x):
@@ -180,33 +162,6 @@ def test_thermostat_per_mode():
     assert abs(diff.mean()) < 5.0 * se
 
 
-# harmonic pair springs about the base geometry (as in test_md.py): a bound PES with a clear minimum
-_N_SPRING, _K_SPRING = 5, 2.0
-
-
-def _spring_pes(R):
-    from sgdml_b200 import synth
-
-    r0 = synth.base_geometry(_N_SPRING)
-    d0 = np.sqrt(((r0[:, None] - r0[None]) ** 2).sum(-1))
-    R = np.asarray(R, dtype=np.float64).reshape(-1, _N_SPRING, 3)
-    diff = R[:, :, None, :] - R[:, None, :, :]
-    d = np.sqrt((diff * diff).sum(-1)) + np.eye(_N_SPRING)
-    ext = (d - d0 - np.eye(_N_SPRING)) * (1 - np.eye(_N_SPRING))
-    E = 0.25 * _K_SPRING * (ext * ext).sum((1, 2))
-    F = -_K_SPRING * (ext[..., None] * diff / d[..., None]).sum(2)
-    return E, F
-
-
-def spring_task():
-    from sgdml_b200 import synth
-
-    task = synth.make_task(_N_SPRING, 60, np.arange(_N_SPRING)[None], 4, seed=3)
-    task['E_train'], task['F_train'] = _spring_pes(task['R_train'])
-    task['dataset_theory'] = 'harmonic_springs'
-    return task
-
-
 # The quantum-limit run (model units, masses 10, hbar 0.05, kT = hbar omega_max / 4, P = 8, 32 polymers): PILE-L at
 # lambda = 1 with centroid friction 0.5 omega_max, dt = 0.1 / omega_max, 1000 steps to equilibrate and 4000 sampled
 # every 10.  The harmonic value is the finite-P value (pimd_oracle.harmonic_value) of each vibrational mode of the
@@ -245,7 +200,7 @@ def test_quantum_kinetic_energy_of_a_trained_model():
     import sgdml_b200
 
     c = _SPRING
-    gp = sgdml_b200.GDMLPredict(sgdml_b200.GDMLTrain().train(spring_task()))
+    gp = sgdml_b200.GDMLPredict(sgdml_b200.GDMLTrain().train(make_spring_task()))
 
     def hvp(R, V):
         return gp.predict_hvp(torch.from_numpy(np.ascontiguousarray(R)).cuda(),

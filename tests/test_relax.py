@@ -9,7 +9,7 @@ import pytest
 
 import relax_oracle
 from conftest import rel_err
-from test_md import FIXTURES_MD, _N_SPRING, _cuda_forces, _spring_pes, md_fs_masses, spring_task  # noqa: F401
+from md_common import FIXTURES_MD, _N_SPRING, _cuda_forces, _spring_pes, md_fs_masses, spring_task  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 

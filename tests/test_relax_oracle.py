@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 import relax_oracle
-from test_md import _N_SPRING, _spring_pes
+from md_common import _N_SPRING, _spring_pes
 
 _EPS = np.finfo(np.float64).eps
 

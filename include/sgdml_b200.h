@@ -258,8 +258,33 @@ int sgdml_b200_relax_fire(sgdml_b200_md* md, int64_t max_steps, double fmax, dou
  * every atom (ASE's rule: the whole step is scaled so that its longest atom step is maxstep). */
 int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, int memory, double h0,
                            int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream);
-/* Test hook: graph replays between convergence read-backs of sgdml_b200_relax_*; 0 = the default (16).  Negative
- * values are rejected. */
+/* ---------------------------------------------------------------- nudged elastic band on the device
+ * Extension: minimum-energy paths and saddle points with the nudged elastic band (NEB) and its climbing-image form
+ * (CI-NEB), optimised by FIRE on each whole band, many bands and many steps per call.  The handle (sgdml_b200_md_create;
+ * a ring-polymer handle is rejected) holds n_rep = n_bands n_images replicas: replica b n_images + j is image j of band
+ * b.  Images 0 and n_images - 1 are fixed endpoints: they never move, but their forces and energies are evaluated with
+ * the rest of the batch every step.  Image differences are plain coordinate differences, with no minimum image, also
+ * for periodic models.  Tangents are Henkelman & Jonsson's improved tangent (J. Chem. Phys. 113, 9978 (2000)), the
+ * spring force k (|R[i+1] - R[i]| - |R[i] - R[i-1]|) acts along it; with climb != 0 the interior image of highest
+ * energy (the lowest index on ties, chosen again at every step) feels the model force with its tangent component
+ * reversed and no spring (Henkelman, Uberuaga & Jonsson, J. Chem. Phys. 113, 9901 (2000)).  The interior images of a
+ * band are one FIRE vector of (n_images - 2) 3N coordinates, as for ASE's optimisers on an NEB object: the FIRE rules,
+ * constants and arguments are sgdml_b200_relax_fire's, maxstep caps |dr| of the whole band, and a band has converged
+ * when max over the atoms of all its interior images of |F_neb,a| < fmax; it is frozen from then on.  L-BFGS is not
+ * offered: its energy-rise reset has no meaning for NEB forces, which are not a gradient.  The step graph is the NEB
+ * force kernel and the band FIRE kernel (k_neb_force, k_neb_fire_step) followed by the forces of every image; the
+ * driver, the block read-backs, the final state (R, F, E_pot at the final positions, V zero, step counter unchanged)
+ * and the launch families are those of sgdml_b200_relax_* above.  Exact sums and roundings are in csrc/md.cuh.
+ * Arguments: n_images >= 3 dividing n_rep; k >= 0 (force unit / L); fmax, maxstep, dt, dtmax as for
+ * sgdml_b200_relax_fire.  Outputs, each host, device or NULL, per band (n_rep / n_images): n_steps_out int64,
+ * converged_out int32, fmax_out double (max_a |F_neb,a| at the final positions) and climbing_out int32, the index of
+ * the band's highest interior image at the final positions.  Argument errors are reported before anything is queued,
+ * and a rejected call changes nothing. */
+int sgdml_b200_neb_fire(sgdml_b200_md* md, int64_t n_images, int64_t max_steps, double fmax, double k, int climb,
+                        double maxstep, double dt, double dtmax, int64_t* n_steps_out, int* converged_out,
+                        double* fmax_out, int* climbing_out, void* stream);
+/* Test hook: graph replays between convergence read-backs of sgdml_b200_relax_* and sgdml_b200_neb_fire; 0 = the
+ * default (16).  Negative values are rejected. */
 int sgdml_b200_set_relax_block(int64_t n_steps);
 
 /* Periodic model (predict.py:332-334: lat_and_inv from model['lattice']): query descriptors of

@@ -372,6 +372,58 @@ __device__ __forceinline__ void relax_store(RelaxState* st, const RelaxState& z)
   if (threadIdx.x == 0) *st = z;
 }
 
+// One FIRE step (md.cuh) of the n coordinates r, v, f after the convergence test: the arithmetic of k_fire_step (n the
+// replica's 3N) and of k_neb_fire_step (n a band's (P - 2) 3N).
+__device__ __forceinline__ void fire_update(RelaxState& z, double dt0, double dtmax, double maxstep, double* r,
+                                            double* v, const double* f, int n, double* red) {
+  if (z.n_steps == 0) {  // ASE's first step: no mixing, dt kept
+    z.dt = dt0;
+    z.alpha = FIRE_ALPHA0;
+    z.n_pos = 0;
+  } else {
+    double fv = 0.0;
+    for (int i = threadIdx.x; i < n; i += MD_THREADS) fv = __dadd_rn(fv, __dmul_rn(f[i], v[i]));
+    fv = block_sum(fv, red);
+    if (fv > 0.0) {
+      double vv = 0.0, ff = 0.0;
+      for (int i = threadIdx.x; i < n; i += MD_THREADS) {
+        vv = __dadd_rn(vv, __dmul_rn(v[i], v[i]));
+        ff = __dadd_rn(ff, __dmul_rn(f[i], f[i]));
+      }
+      vv = block_sum(vv, red);
+      ff = block_sum(ff, red);
+      const double c = __dmul_rn(z.alpha, __ddiv_rn(sqrt(vv), sqrt(ff)));
+      const double om = __dsub_rn(1.0, z.alpha);
+      for (int i = threadIdx.x; i < n; i += MD_THREADS) v[i] = __dadd_rn(__dmul_rn(om, v[i]), __dmul_rn(c, f[i]));
+      if (z.n_pos > FIRE_NMIN) {
+        z.dt = fmin(__dmul_rn(z.dt, FIRE_FINC), dtmax);
+        z.alpha = __dmul_rn(z.alpha, FIRE_FALPHA);
+      }
+      ++z.n_pos;
+    } else {
+      for (int i = threadIdx.x; i < n; i += MD_THREADS) v[i] = 0.0;
+      z.alpha = FIRE_ALPHA0;
+      z.dt = __dmul_rn(z.dt, FIRE_FDEC);
+      z.n_pos = 0;
+    }
+  }
+  double nn = 0.0;
+  for (int i = threadIdx.x; i < n; i += MD_THREADS) {
+    const double vi = __dadd_rn(v[i], __dmul_rn(z.dt, f[i]));
+    v[i] = vi;
+    const double dr = __dmul_rn(z.dt, vi);
+    nn = __dadd_rn(nn, __dmul_rn(dr, dr));
+  }
+  const double nrm = sqrt(block_sum(nn, red));
+  const bool cap = nrm > maxstep;
+  for (int i = threadIdx.x; i < n; i += MD_THREADS) {
+    double dr = __dmul_rn(z.dt, v[i]);
+    if (cap) dr = __ddiv_rn(__dmul_rn(maxstep, dr), nrm);
+    r[i] = __dadd_rn(r[i], dr);
+  }
+  ++z.n_steps;
+}
+
 __global__ void __launch_bounds__(MD_THREADS) k_fire_step(const RelaxParams* __restrict__ P, RelaxState* st,
                                                          double* __restrict__ R, double* __restrict__ V,
                                                          const double* __restrict__ F, int dimi, int advance) {
@@ -383,53 +435,7 @@ __global__ void __launch_bounds__(MD_THREADS) k_fire_step(const RelaxParams* __r
   double* v = V + rep * dimi;
   const double* f = F + rep * dimi;
   if (relax_test(z, f, dimi, p.fmax2, red) || !advance) return relax_store(st + rep, z);
-
-  if (z.n_steps == 0) {  // ASE's first step: no mixing, dt kept
-    z.dt = p.dt0;
-    z.alpha = FIRE_ALPHA0;
-    z.n_pos = 0;
-  } else {
-    double fv = 0.0;
-    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) fv = __dadd_rn(fv, __dmul_rn(f[i], v[i]));
-    fv = block_sum(fv, red);
-    if (fv > 0.0) {
-      double vv = 0.0, ff = 0.0;
-      for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
-        vv = __dadd_rn(vv, __dmul_rn(v[i], v[i]));
-        ff = __dadd_rn(ff, __dmul_rn(f[i], f[i]));
-      }
-      vv = block_sum(vv, red);
-      ff = block_sum(ff, red);
-      const double c = __dmul_rn(z.alpha, __ddiv_rn(sqrt(vv), sqrt(ff)));
-      const double om = __dsub_rn(1.0, z.alpha);
-      for (int i = threadIdx.x; i < dimi; i += MD_THREADS) v[i] = __dadd_rn(__dmul_rn(om, v[i]), __dmul_rn(c, f[i]));
-      if (z.n_pos > FIRE_NMIN) {
-        z.dt = fmin(__dmul_rn(z.dt, FIRE_FINC), p.dtmax);
-        z.alpha = __dmul_rn(z.alpha, FIRE_FALPHA);
-      }
-      ++z.n_pos;
-    } else {
-      for (int i = threadIdx.x; i < dimi; i += MD_THREADS) v[i] = 0.0;
-      z.alpha = FIRE_ALPHA0;
-      z.dt = __dmul_rn(z.dt, FIRE_FDEC);
-      z.n_pos = 0;
-    }
-  }
-  double nn = 0.0;
-  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
-    const double vi = __dadd_rn(v[i], __dmul_rn(z.dt, f[i]));
-    v[i] = vi;
-    const double dr = __dmul_rn(z.dt, vi);
-    nn = __dadd_rn(nn, __dmul_rn(dr, dr));
-  }
-  const double nrm = sqrt(block_sum(nn, red));
-  const bool cap = nrm > p.maxstep;
-  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
-    double dr = __dmul_rn(z.dt, v[i]);
-    if (cap) dr = __ddiv_rn(__dmul_rn(p.maxstep, dr), nrm);
-    r[i] = __dadd_rn(r[i], dr);
-  }
-  ++z.n_steps;
+  fire_update(z, p.dt0, p.dtmax, p.maxstep, r, v, f, dimi, red);
   relax_store(st + rep, z);
 }
 
@@ -535,6 +541,81 @@ __global__ void __launch_bounds__(MD_THREADS) k_lbfgs_step(const RelaxParams* __
   relax_store(st + rep, z);
 }
 
+// The NEB force of one interior image (md.cuh).  Each thread keeps its coordinates of tau, then of th, in its own
+// entries of Fn before overwriting them with F_neb, so no barrier beyond block_sum's is needed.
+__global__ void __launch_bounds__(MD_THREADS) k_neb_force(const NebParams* __restrict__ Q, const double* __restrict__ R,
+                                                         const double* __restrict__ F, const double* __restrict__ E,
+                                                         double* __restrict__ Fn, int* __restrict__ climb_idx,
+                                                         int dimi) {
+  __shared__ double red[MD_THREADS];
+  const NebParams p = *Q;
+  const int ni = p.P - 2;
+  const int64_t band = blockIdx.x / ni;
+  const int i = (int)(blockIdx.x % ni) + 1;
+  const double* eb = E + band * p.P;
+  int top = 1;  // the highest interior image, the lowest index on ties
+  for (int j = 2; j <= ni; ++j)
+    if (eb[j] > eb[top]) top = j;
+  if (i == 1 && threadIdx.x == 0) climb_idx[band] = top;
+
+  const int64_t rep = band * p.P + i;
+  const double* r = R + rep * dimi;
+  const double* f = F + rep * dimi;
+  double* fn = Fn + rep * dimi;
+  const double e = eb[i], ep = eb[i + 1], em = eb[i - 1];
+  const int mode = ep > e && e > em ? 1 : (ep < e && e < em ? 2 : 0);  // 1: tau = t+, 2: tau = t-, 0: the mixture
+  const double dp = fabs(__dsub_rn(ep, e)), dm = fabs(__dsub_rn(em, e));
+  const double dmax = dp > dm ? dp : dm, dmin = dp > dm ? dm : dp;
+  const double wp = ep > em ? dmax : dmin, wm = ep > em ? dmin : dmax;
+  double tt = 0.0, pp = 0.0, mm = 0.0;
+  for (int c = threadIdx.x; c < dimi; c += MD_THREADS) {
+    const double x = r[c];
+    const double tp = __dsub_rn(r[c + dimi], x), tm = __dsub_rn(x, r[c - dimi]);
+    const double t = mode == 1 ? tp : (mode == 2 ? tm : __dadd_rn(__dmul_rn(tp, wp), __dmul_rn(tm, wm)));
+    fn[c] = t;
+    tt = __dadd_rn(tt, __dmul_rn(t, t));
+    pp = __dadd_rn(pp, __dmul_rn(tp, tp));
+    mm = __dadd_rn(mm, __dmul_rn(tm, tm));
+  }
+  const double nt = sqrt(block_sum(tt, red));
+  const double np = sqrt(block_sum(pp, red));
+  const double nm = sqrt(block_sum(mm, red));
+  double fd = 0.0;
+  for (int c = threadIdx.x; c < dimi; c += MD_THREADS) {
+    const double th = nt == 0.0 ? 0.0 : __ddiv_rn(fn[c], nt);
+    fn[c] = th;
+    fd = __dadd_rn(fd, __dmul_rn(f[c], th));
+  }
+  fd = block_sum(fd, red);
+  const bool climbing = p.climb && i == top;
+  const double spring = __dmul_rn(p.k, __dsub_rn(np, nm));
+  const double fd2 = __dmul_rn(2.0, fd);
+  for (int c = threadIdx.x; c < dimi; c += MD_THREADS) {
+    const double th = fn[c];
+    fn[c] = climbing ? __dsub_rn(f[c], __dmul_rn(fd2, th))
+                     : __dadd_rn(__dsub_rn(f[c], __dmul_rn(fd, th)), __dmul_rn(spring, th));
+  }
+}
+
+// FIRE on one band's interior images with the NEB forces Fn (one RelaxState per band)
+__global__ void __launch_bounds__(MD_THREADS) k_neb_fire_step(const NebParams* __restrict__ Q, RelaxState* st,
+                                                             double* __restrict__ R, double* __restrict__ V,
+                                                             const double* __restrict__ Fn, int dimi, int advance) {
+  __shared__ double red[MD_THREADS];
+  const int64_t band = blockIdx.x;
+  const NebParams p = *Q;
+  RelaxState z = st[band];
+  // The L-BFGS fields are zero already (the driver zeroes the state and FIRE never writes them).  Storing the constant
+  // lets the compiler drop the two loaded values instead of carrying them through the step to relax_store, which
+  // otherwise costs 16 bytes of spills.
+  z.gamma = z.E_prev = 0.0;
+  const int64_t o = (band * p.P + 1) * dimi;  // image 1 of the band: the interior images are contiguous
+  const int n = (p.P - 2) * dimi;
+  if (relax_test(z, Fn + o, n, p.fmax2, red) || !advance) return relax_store(st + band, z);
+  fire_update(z, p.dt0, p.dtmax, p.maxstep, R + o, V + o, Fn + o, n, red);
+  relax_store(st + band, z);
+}
+
 __global__ void __launch_bounds__(MD_THREADS) k_relax_count(const RelaxState* __restrict__ st, int64_t n_rep,
                                                            int* n_active) {
   __shared__ int red[MD_THREADS];
@@ -604,6 +685,13 @@ struct sgdml_b200_md {
   double *S = nullptr, *Y = nullptr, *rho = nullptr;        // L-BFGS ring, m_cap pairs per replica
   double *r_prev = nullptr, *g_prev = nullptr;              // (n_rep, 3N)
   int m_cap = 0;
+  // nudged elastic band (sgdml_b200_neb_fire), allocated by the first NEB call
+  NebParams* dN = nullptr;
+  NebParams* hN = nullptr;    // pinned staging of dN
+  double* Fn = nullptr;       // (n_rep, 3N) NEB forces of the interior images
+  int* climb_idx = nullptr;   // (n_rep) the highest interior image of each band (the first n_rep / P entries)
+  int neb_P = 0;              // images per band of the current NEB call
+  int graph_P = 0;            // ... and of the captured NEB step
 };
 
 namespace {
@@ -621,10 +709,13 @@ void md_free(sgdml_b200_md* md) {
   cached_free(md->dP);
   cached_free(md->dQ);
   cached_free(md->tab);
-  for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev}) cached_free(p);
+  for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev, md->Fn}) cached_free(p);
   cached_free(md->rst);
   cached_free(md->dR);
+  cached_free(md->dN);
+  cached_free(md->climb_idx);
   cudaFreeHost(md->hR);
+  cudaFreeHost(md->hN);
   cudaFreeHost(md->hActive);
   cudaFreeHost(md->hP);
   cudaFreeHost(md->hQ);
@@ -696,10 +787,11 @@ class Outputs {
 };
 
 // what one step of the handle's graph integrates
-enum MdKind { MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3 };
+enum MdKind { MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, MD_NEB_FIRE = 4 };
 
-// the integrator of sgdml_b200_md_run, sgdml_b200_pimd_run or sgdml_b200_relax_*; advance == 0 completes a run's last
-// step (MD) or only tests convergence (relaxation).  L-BFGS keeps its direction in V, which relax_impl zeroes after.
+// the integrator of sgdml_b200_md_run, sgdml_b200_pimd_run, sgdml_b200_relax_* or sgdml_b200_neb_fire; advance == 0
+// completes a run's last step (MD) or only tests convergence (relaxation, NEB: after the force projection).  L-BFGS
+// keeps its direction in V, which relax_impl zeroes after.
 int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
   switch (kind) {
     case MD_RING_POLYMER:
@@ -714,6 +806,16 @@ int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
       k_lbfgs_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(md->dR, md->rst, md->R, md->V, md->F, md->E, md->dimi,
                                                               advance);
       break;
+    case MD_NEB_FIRE: {
+      const int64_t n_bands = md->n_rep / md->neb_P;
+      k_neb_force<<<(unsigned)(n_bands * (md->neb_P - 2)), MD_THREADS, 0, s>>>(md->dN, md->R, md->F, md->E, md->Fn,
+                                                                              md->climb_idx, md->dimi);
+      SG_CUDA(cudaGetLastError());
+      count_launch(KID_MISC);
+      k_neb_fire_step<<<(unsigned)n_bands, MD_THREADS, 0, s>>>(md->dN, md->rst, md->R, md->V, md->Fn, md->dimi,
+                                                               advance);
+      break;
+    }
     default:
       k_md_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E,
                                                            md->step, md->dimi, advance);
@@ -728,9 +830,12 @@ int md_step(sgdml_b200_md* md, int kind, cudaStream_t s) {
   return force_eval_run(md->fe, md->R, md->F, md->E, s);
 }
 
-// the step graph, captured again whenever the force evaluation it bakes in is stale or the integrator (MdKind) changes
+// the step graph, captured again whenever the force evaluation it bakes in is stale, the integrator (MdKind) changes
+// or, for NEB, the images per band (its grids) change
 int md_graph(sgdml_b200_md* md, int kind, cudaStream_t s) {
-  if (md->exec != nullptr && md->graph_kind == kind && !force_eval_stale(md->fe)) return 0;
+  if (md->exec != nullptr && md->graph_kind == kind && (kind != MD_NEB_FIRE || md->graph_P == md->neb_P) &&
+      !force_eval_stale(md->fe))
+    return 0;
   if (md->exec != nullptr) {
     cudaGraphExecDestroy(md->exec);
     md->exec = nullptr;
@@ -748,6 +853,7 @@ int md_graph(sgdml_b200_md* md, int kind, cudaStream_t s) {
   SG_TRY(capture_graph(md->gs, [&] { return md_step(md, kind, md->gs); }, &md->exec, &md->n_kernels));
   force_eval_mark(md->fe);
   md->graph_kind = kind;
+  md->graph_P = md->neb_P;
   return 0;
 }
 
@@ -896,8 +1002,9 @@ int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, d
 constexpr int64_t RELAX_BLOCK = 16;  // replays between convergence read-backs
 int64_t g_relax_block = 0;           // sgdml_b200_set_relax_block (test hook): 0 = RELAX_BLOCK
 
-// the optimiser state, made at the first relaxation; the L-BFGS ring grows to `memory` pairs per replica
-int relax_alloc(sgdml_b200_md* md, int memory) {
+// the optimiser state, made at the first relaxation; the L-BFGS ring grows to `memory` pairs per replica, and the NEB
+// buffers are made at the first NEB call
+int relax_alloc(sgdml_b200_md* md, int memory, bool neb) {
   if (md->rst == nullptr) SG_CUDA(cached_malloc(&md->rst, sizeof(RelaxState) * (size_t)md->n_rep));
   if (md->dR == nullptr) SG_CUDA(cached_malloc(&md->dR, sizeof(RelaxParams)));
   if (md->hR == nullptr) SG_CUDA(cudaMallocHost(&md->hR, sizeof(RelaxParams)));
@@ -906,6 +1013,12 @@ int relax_alloc(sgdml_b200_md* md, int memory) {
     SG_CUDA(cudaHostGetDevicePointer((void**)&md->dActive, md->hActive, 0));
   }
   if (md->counted == nullptr) SG_CUDA(cudaEventCreateWithFlags(&md->counted, cudaEventDisableTiming));
+  if (neb) {
+    if (md->dN == nullptr) SG_CUDA(cached_malloc(&md->dN, sizeof(NebParams)));
+    if (md->hN == nullptr) SG_CUDA(cudaMallocHost(&md->hN, sizeof(NebParams)));
+    if (md->climb_idx == nullptr) SG_CUDA(cached_malloc(&md->climb_idx, sizeof(int) * (size_t)md->n_rep));
+    if (md->Fn == nullptr) SG_CUDA(cached_malloc(&md->Fn, sizeof(double) * (size_t)(md->n_rep * md->dimi)));
+  }
   if (memory > md->m_cap) {
     const size_t vec = sizeof(double) * (size_t)(md->n_rep * md->dimi);
     SG_CUDA(cudaDeviceSynchronize());  // the old ring goes back to the cache: nothing may still use it
@@ -926,18 +1039,9 @@ int relax_alloc(sgdml_b200_md* md, int memory) {
   return 0;
 }
 
-// Relaxes every replica from the handle's state: blocks of step-graph replays, each followed by the convergence test
-// and a count of unconverged replicas read back through mapped pinned memory; stops when none is left or after
-// max_steps.  Frozen replicas make the block length a matter of cost only.  V is zero before and after.
-int relax_impl(sgdml_b200_md* md, int kind, int64_t max_steps, const RelaxParams& prm, int64_t* n_steps_out,
-               int* conv_out, double* fmax_out, cudaStream_t s) {
-  const int64_t n_rep = md->n_rep;
-  SG_TRY(force_eval_prepare(md->fe));
-  SG_TRY(relax_alloc(md, kind == MD_LBFGS ? prm.memory : 0));
-  Outputs out(s);
-  SG_TRY(out.init({{n_steps_out, sizeof(int64_t) * (size_t)n_rep}, {conv_out, sizeof(int) * (size_t)n_rep},
-                   {fmax_out, sizeof(double) * (size_t)n_rep}}));
-  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the staging
+// The parameters of one call into the pinned staging and their upload on s, once the previous call has read it:
+// an optimiser's RelaxParams (with the handle's L-BFGS ring) or an NEB call's NebParams (and its images per band).
+int stage_relax(sgdml_b200_md* md, const RelaxParams& prm, cudaStream_t s) {
   RelaxParams& p = *md->hR;
   p = prm;
   p.m_cap = md->m_cap;
@@ -947,14 +1051,42 @@ int relax_impl(sgdml_b200_md* md, int kind, int64_t max_steps, const RelaxParams
   p.r_prev = md->r_prev;
   p.g_prev = md->g_prev;
   SG_CUDA(cudaMemcpyAsync(md->dR, md->hR, sizeof(RelaxParams), cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+int stage_neb(sgdml_b200_md* md, const NebParams& q, cudaStream_t s) {
+  *md->hN = q;
+  md->neb_P = q.P;
+  SG_CUDA(cudaMemcpyAsync(md->dN, md->hN, sizeof(NebParams), cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+// Relaxes every replica (or NEB band) from the handle's state: blocks of step-graph replays, each followed by the
+// convergence test and a count of unconverged units read back through mapped pinned memory; stops when none is left or
+// after max_steps.  The unit of convergence is a group of g consecutive replicas: g = 1 for relaxation, g = P for NEB
+// (whose climbing_out gets each band's highest interior image).  memory: L-BFGS pairs per replica to allocate (0:
+// none).  stage() stages and uploads the call's parameters (stage_relax, stage_neb).  Frozen units make the block
+// length a matter of cost only.  V is zero before and after.
+template <class Stage>
+int relax_impl(sgdml_b200_md* md, int kind, int64_t g, int memory, int64_t max_steps, int64_t* n_steps_out,
+               int* conv_out, double* fmax_out, int* climbing_out, cudaStream_t s, Stage stage) {
+  const int64_t n_rep = md->n_rep;
+  const int64_t n_units = n_rep / g;
+  SG_TRY(force_eval_prepare(md->fe));
+  SG_TRY(relax_alloc(md, memory, kind == MD_NEB_FIRE));
+  Outputs out(s);
+  SG_TRY(out.init({{n_steps_out, sizeof(int64_t) * (size_t)n_units}, {conv_out, sizeof(int) * (size_t)n_units},
+                   {fmax_out, sizeof(double) * (size_t)n_units}, {climbing_out, sizeof(int) * (size_t)n_units}}));
+  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the staging
+  SG_TRY(stage());
   SG_CUDA(cudaEventRecord(md->uploaded, s));
   const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
-  SG_CUDA(cudaMemsetAsync(md->rst, 0, sizeof(RelaxState) * (size_t)n_rep, s));
+  SG_CUDA(cudaMemsetAsync(md->rst, 0, sizeof(RelaxState) * (size_t)n_units, s));
   SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
   const int64_t block = g_relax_block > 0 ? g_relax_block : RELAX_BLOCK;
   for (int64_t done = 0;;) {
     SG_TRY(md_integrate(md, kind, 0, s));  // the test on the current forces
-    k_relax_count<<<1, MD_THREADS, 0, s>>>(md->rst, n_rep, md->dActive);
+    k_relax_count<<<1, MD_THREADS, 0, s>>>(md->rst, n_units, md->dActive);
     SG_CUDA(cudaGetLastError());
     count_launch(KID_MISC);
     SG_CUDA(cudaEventRecord(md->counted, s));
@@ -965,10 +1097,12 @@ int relax_impl(sgdml_b200_md* md, int kind, int64_t max_steps, const RelaxParams
     done += n;
   }
   SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));  // a following MD run starts at rest
-  k_relax_report<<<(unsigned)((n_rep + 255) / 256), 256, 0, s>>>(md->rst, n_rep, out.dev<int64_t>(0), out.dev<int>(1),
-                                                                out.dev<double>(2));
+  k_relax_report<<<(unsigned)((n_units + 255) / 256), 256, 0, s>>>(md->rst, n_units, out.dev<int64_t>(0),
+                                                                  out.dev<int>(1), out.dev<double>(2));
   SG_CUDA(cudaGetLastError());
   count_launch(KID_MISC);
+  if (out.dev<int>(3) != nullptr)  // the last test ran k_neb_force at the final positions
+    SG_CUDA(cudaMemcpyAsync(out.dev<int>(3), md->climb_idx, out.bytes(3), cudaMemcpyDeviceToDevice, s));
   return out.finish();
 }
 
@@ -1111,7 +1245,9 @@ int sgdml_b200_relax_fire(sgdml_b200_md* md, int64_t max_steps, double fmax, dou
   p.maxstep = maxstep;
   p.dt0 = dt;
   p.dtmax = dtmax;
-  return relax_impl(md, MD_FIRE, max_steps, p, n_steps_out, converged_out, fmax_out, (cudaStream_t)stream);
+  cudaStream_t s = (cudaStream_t)stream;
+  return relax_impl(md, MD_FIRE, 1, 0, max_steps, n_steps_out, converged_out, fmax_out, nullptr, s,
+                    [&] { return stage_relax(md, p, s); });
 }
 
 int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, int memory, double h0,
@@ -1126,7 +1262,33 @@ int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, do
   p.maxstep = maxstep;
   p.h0 = h0;
   p.memory = memory;
-  return relax_impl(md, MD_LBFGS, max_steps, p, n_steps_out, converged_out, fmax_out, (cudaStream_t)stream);
+  cudaStream_t s = (cudaStream_t)stream;
+  return relax_impl(md, MD_LBFGS, 1, memory, max_steps, n_steps_out, converged_out, fmax_out, nullptr, s,
+                    [&] { return stage_relax(md, p, s); });
+}
+
+int sgdml_b200_neb_fire(sgdml_b200_md* md, int64_t n_images, int64_t max_steps, double fmax, double k, int climb,
+                        double maxstep, double dt, double dtmax, int64_t* n_steps_out, int* converged_out,
+                        double* fmax_out, int* climbing_out, void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(relax_check(md, max_steps, fmax, maxstep, "sgdml_b200_neb_fire: no state yet (call sgdml_b200_md_set_state)"));
+  if (md->nb > 1) return fail_arg("sgdml_b200_neb_fire: a ring-polymer handle (n_beads > 1) holds no bands");
+  SG_ARG(n_images >= 3 && md->n_rep % n_images == 0);
+  SG_ARG((n_images - 2) * md->dimi <= INT32_MAX);
+  SG_ARG(std::isfinite(k) && k >= 0.0);
+  SG_ARG(std::isfinite(dt) && dt > 0.0);
+  SG_ARG(std::isfinite(dtmax) && dtmax > 0.0);
+  NebParams q = {};
+  q.fmax2 = fmax * fmax;
+  q.maxstep = maxstep;
+  q.dt0 = dt;
+  q.dtmax = dtmax;
+  q.k = k;
+  q.climb = climb != 0 ? 1 : 0;
+  q.P = (int)n_images;
+  cudaStream_t s = (cudaStream_t)stream;
+  return relax_impl(md, MD_NEB_FIRE, n_images, 0, max_steps, n_steps_out, converged_out, fmax_out, climbing_out, s,
+                    [&] { return stage_neb(md, q, s); });
 }
 
 int sgdml_b200_set_relax_block(int64_t n_steps) {

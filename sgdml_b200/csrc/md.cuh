@@ -1,6 +1,6 @@
-// Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_pimd_*, sgdml_b200_relax_*): the contract of the
-// kernels in md.cu -- the BAOAB integrator step, its ring-polymer form, their counter-based noise, and the FIRE and
-// L-BFGS steps.
+// Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_pimd_*, sgdml_b200_relax_*, sgdml_b200_neb_fire): the
+// contract of the kernels in md.cu -- the BAOAB integrator step, its ring-polymer form, their counter-based noise, the
+// FIRE and L-BFGS steps, and the nudged elastic band.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -110,5 +110,36 @@ struct RelaxParams {
 //
 // k_relax_count writes the number of replicas not yet converged into *n_active (host-mapped pinned memory);
 // k_relax_report writes n_steps (int64), conv (int32) and sqrt(fmax2) per replica into device arrays, each may be null.
+// Both run over the driver's units of convergence: one replica for relaxation, one band for NEB (below).
+
+// Nudged elastic band (sgdml_b200_neb_fire).  The handle's n_rep = n_bands P replicas hold n_bands bands of P >= 3
+// images; replica b P + j is image j of band b.  Images 0 and P - 1 are fixed endpoints: they never move, but their
+// forces and energies are evaluated every step with the rest of the batch, and their energies enter the tangents of
+// their neighbours.  Image differences are plain coordinate differences, with no minimum image, also for periodic
+// models.
+//
+// k_neb_force: one CTA of MD_THREADS per interior image (grid n_bands (P - 2)).  With E the model energy and F = -dE/dR
+// of the image i and its neighbours, t+ = R[i+1] - R[i] and t- = R[i] - R[i-1] (each difference rounded), the tangent
+// of Henkelman & Jonsson, J. Chem. Phys. 113, 9978 (2000), eqs. 8-11:
+//   E[i+1] > E[i] > E[i-1]:  tau = t+;   E[i+1] < E[i] < E[i-1]:  tau = t-;
+//   otherwise, dmax / dmin the larger / smaller of |E[i+1] - E[i]|, |E[i-1] - E[i]|:
+//     E[i+1] > E[i-1]:  tau = t+ dmax + t- dmin;   else:  tau = t+ dmin + t- dmax
+// nt = sqrt(tau.tau), np = sqrt(t+.t+), nm = sqrt(t-.t-), th = tau / nt (th = 0 when nt == 0: coincident images give
+// no NaN), fd = F.th, all per image with block_sum's order.  Then
+//   ordinary image:  F_neb = (F - fd th) + (k (np - nm)) th                  (eq. 12)
+//   climbing image:  F_neb = F - (2 fd) th                                   (Henkelman, Uberuaga & Jonsson, JCP 113, 9901)
+// The climbing image is the interior image of highest E, the lowest index on ties, chosen again at every evaluation,
+// and climbs only when climb is set.  The CTA of image 1 writes that index per band to climb_idx.
+//
+// k_neb_fire_step: one CTA per band.  k_fire_step's test and update (fire_update in md.cu, one copy of the FIRE
+// arithmetic) on the band's interior images as one vector of (P - 2) 3N coordinates, with F_neb for F: F.v, v.v, F.F,
+// |dr| and the convergence test max_a |F_neb,a|^2 < fmax2 run over every atom of every interior image, and one
+// RelaxState per band.  FIRE only: L-BFGS's energy-rise reset has no meaning for NEB forces, which are no gradient.
+struct NebParams {
+  double fmax2, maxstep, dt0, dtmax;  // the band FIRE, as in RelaxParams
+  double k;                           // spring constant (force unit / L)
+  int climb;                          // 1: the highest interior image climbs
+  int P;                              // images per band (>= 3)
+};
 
 }  // namespace sgdml

@@ -333,3 +333,113 @@ class GDMLRelaxation(GDMLDynamics):
         st = self.get_state()
         return {'positions': st['positions'], 'forces': st['forces'], 'potential_energy': st['potential_energy'],
                 'fmax': fm * self.F_to_eV_Ang, 'converged': conv != 0, 'n_steps': n_steps}
+
+
+class GDMLNEB(GDMLRelaxation):
+    """Minimum-energy paths and saddle points of one model with the nudged elastic band (NEB) and its climbing-image
+    form (CI-NEB), optimised on the device (``sgdml_b200_neb_fire``): `n_bands` bands of `n_images` images (>= 3),
+    many bands and many steps per call.  Image j of band b is replica b n_images + j of a ``GDMLRelaxation`` handle;
+    images 0 and n_images - 1 are the fixed endpoints.  Image differences are plain coordinate differences, with no
+    minimum image, also for periodic models.
+
+    ``neb(images=None, fmax=0.05, max_steps=1000, k=0.1, climb=False, maxstep=0.2, dt=0.1, dtmax=1.0)`` runs FIRE on
+    every band (its interior images as one vector, as ASE's optimisers on an ``NEB`` object) until max over the atoms of
+    all interior images of |F_neb| < fmax, or max_steps steps.  Units are ASE's: images (n_bands, n_images, N, 3) [or
+    (n_images, N, 3) for one band] in Angstrom (None: continue from the current state, so that the usual two-stage run
+    is a call without `climb` and a second call with it); fmax in eV/Angstrom; the spring constant k in eV/Angstrom^2;
+    maxstep (Angstrom) caps the step of a whole band; dt and dtmax as in ``GDMLRelaxation.relax``.  Returns
+    {'positions', 'forces' (the model's forces): (n_bands, n_images, N, 3), 'energies': (n_bands, n_images), 'barrier':
+    the highest interior energy minus that of image 0, 'climbing_image' (the highest interior image), 'fmax' (of the NEB
+    forces), 'converged', 'n_steps': (n_bands,)} in Angstrom, eV/Angstrom and eV.  NumPy arrays or float64 CUDA tensors
+    in, the same kind out.  ``interpolate`` builds a linear band between two endpoints."""
+
+    def __init__(self, model, n_images, n_bands=1, E_to_eV=_KCAL_PER_MOL_IN_EV, F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        self.n_images = int(n_images)
+        self.n_bands = int(n_bands)
+        if self.n_images < 3 or self.n_bands < 1:
+            raise ValueError('a band needs n_images >= 3 (two endpoints and an interior image), and n_bands >= 1')
+        super().__init__(model, self.n_bands * self.n_images, E_to_eV, F_to_eV_Ang)
+
+    def interpolate(self, initial, final, n_images=None, align=True):
+        """Linear band from `initial` to `final` (host arrays (..., N, 3), Angstrom): (..., n_images, N, 3), image 0
+        exactly `initial` and the last image exactly the (aligned) `final`.  align: first move `final` onto `initial`
+        by the rigid rotation and translation of least squares (Kabsch), which a periodic model refuses."""
+        if align and self.gdml_predict.lat_and_inv is not None:
+            raise ValueError('align=True moves the atoms rigidly, which a periodic model does not allow: pass align=False')
+        n_images = self.n_images if n_images is None else int(n_images)
+        if n_images < 2:
+            raise ValueError('n_images must be >= 2')
+        a = np.asarray(initial, dtype=np.float64)
+        b = np.asarray(final, dtype=np.float64)
+        if a.shape != b.shape or a.ndim < 2 or a.shape[-1] != 3:
+            raise ValueError('initial and final must have the same shape (..., N, 3): %s, %s' % (a.shape, b.shape))
+        if align:
+            b = kabsch_align(b, a)
+        t = (np.arange(n_images, dtype=np.float64) / (n_images - 1)).reshape(n_images, 1, 1)
+        out = a[..., None, :, :] + t * (b - a)[..., None, :, :]
+        out[..., 0, :, :] = a
+        out[..., -1, :, :] = b
+        return out
+
+    def _bands(self, x):
+        """(n_bands, n_images, N, 3) or (n_images, N, 3) for one band."""
+        shape = tuple(x.shape)
+        want = (self.n_bands, self.n_images, self.n_atoms, 3)
+        if shape != want and not (self.n_bands == 1 and shape == want[1:]):
+            raise ValueError('images must be (n_bands, n_images, N, 3) = %s, or (n_images, N, 3) for one band: %s'
+                             % (want, shape))
+        return x
+
+    # ------------------------------------------------------------------ model units
+    def _neb_raw(self, max_steps, fmax, k, climb, maxstep, dt, dtmax):
+        """-> (n_steps, converged, fmax, climbing_image), each (n_bands,), in model units."""
+        n = self.n_bands
+        if self._torch_device is None:
+            out = (np.empty(n, dtype=np.int64), np.empty(n, dtype=np.int32), np.empty(n), np.empty(n, dtype=np.int32))
+        else:
+            import torch
+
+            out = tuple(torch.empty(n, dtype=t, device=self._torch_device)
+                        for t in (torch.int64, torch.int32, torch.float64, torch.int32))
+        _lib.check(
+            _lib.lib().sgdml_b200_neb_fire(self._handle, self.n_images, int(max_steps), float(fmax), float(k),
+                                           1 if climb else 0, float(maxstep), float(dt), float(dtmax),
+                                           *(_lib.ptr(x) for x in out), _lib.current_stream()),
+            'neb_fire',
+        )
+        return out
+
+    # ------------------------------------------------------------------ ASE units
+    def neb(self, images=None, fmax=0.05, max_steps=1000, k=0.1, climb=False, maxstep=0.2, dt=0.1, dtmax=1.0):
+        if images is not None:
+            self.set_state(self._bands(images))
+        c = self.Ang_to_R * self.F_to_eV_Ang  # eV / Angstrom^2 -> model force / model length, and dt^2
+        n_steps, conv, fm, top = self._neb_raw(max_steps, float(fmax) / self.F_to_eV_Ang, float(k) / c, climb,
+                                               float(maxstep) * self.Ang_to_R, float(dt) * np.sqrt(c),
+                                               float(dtmax) * np.sqrt(c))
+        st = self.get_state()
+        shape = (self.n_bands, self.n_images)
+        E = st['potential_energy'].reshape(shape)
+        inner = E[:, 1:-1]
+        top_E = inner.amax(1) if hasattr(inner, 'data_ptr') else inner.max(1)
+        return {'positions': st['positions'].reshape(shape + (self.n_atoms, 3)),
+                'forces': st['forces'].reshape(shape + (self.n_atoms, 3)), 'energies': E, 'barrier': top_E - E[:, 0],
+                'climbing_image': top, 'fmax': fm * self.F_to_eV_Ang, 'converged': conv != 0, 'n_steps': n_steps}
+
+
+def kabsch_align(x, ref):
+    """x (..., N, 3) moved by the proper rotation and translation that minimise its squared distance to ref (Kabsch,
+    Acta Cryst. A32, 922 (1976))."""
+    x = np.asarray(x, dtype=np.float64)
+    ref = np.asarray(ref, dtype=np.float64)
+    cx = x.mean(-2, keepdims=True)
+    cr = ref.mean(-2, keepdims=True)
+    H = np.swapaxes(x - cx, -1, -2) @ (ref - cr)  # (..., 3, 3)
+    U, _, Vt = np.linalg.svd(H)
+    d = np.sign(np.linalg.det(np.swapaxes(Vt, -1, -2) @ np.swapaxes(U, -1, -2)))
+    D = np.zeros(H.shape)
+    D[..., 0, 0] = 1.0
+    D[..., 1, 1] = 1.0
+    D[..., 2, 2] = np.where(d == 0.0, 1.0, d)
+    rot = U @ D @ Vt  # row vectors: x_aligned = (x - cx) rot + cr
+    return (x - cx) @ rot + cr

@@ -180,6 +180,45 @@ int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamm
                       int64_t stride, double* R_frames, double* V_frames, double* E_pot_frames,
                       double* E_kin_frames, void* stream);
 
+/* ---------------------------------------------------------------- replica-exchange molecular dynamics on the device
+ * Extension: temperature replica exchange (parallel tempering; Sugita & Okamoto, Chem. Phys. Lett. 314, 141 (1999)) of
+ * Langevin replicas, with the exchanges inside the step graph (no host round trip per exchange).  The handle
+ * (sgdml_b200_md_create; a ring-polymer handle is rejected) holds n_rep = n_ladders n_temps replicas: slot
+ * l n_temps + k sits at temperature kT[k] of ladder l for the whole run, and exchanges move configurations between
+ * neighbouring slots, never temperatures, so frames and the state are sorted by temperature.  Between exchanges every
+ * slot runs sgdml_b200_md_run's BAOAB step with its own sigma_i = sqrt((1 - c1^2) kT[k] s_i); units, streams, the
+ * Philox noise, frames (stride as there), E_kin, SGDML_B200_GRAPH=0, the workspace and the step counters are those of
+ * sgdml_b200_md_run.  The step graph is the exchange kernel (k_remd_exchange, one CTA per ladder), then k_md_step, then
+ * the forces of every replica.
+ * Schedule: let c be the handle's step index of the state R holds.  With exchange_every = E >= 1 an exchange is
+ * attempted on the state at c when c > run_start (the index when this run began) and c % E == 0; with e = c / E the
+ * pairs (k, k + 1) with k % 2 == e % 2 and k + 1 < n_temps are attempted, each independently.  The last state of a run
+ * is exchanged before the run returns and the first is not, so a run continued over several calls is one long run.
+ * E = 0: no exchanges, every slot runs Langevin at its own temperature.
+ * Acceptance: D = (beta_k - beta_k+1) (E_k - E_k+1), rounded as written, beta = 1 / kT computed on the host and E_pot
+ * as sgdml_b200_predict returns it (std and c applied; c cancels).  The swap is accepted iff D >= 0 or u < exp(D), with
+ * u = ((w0 2^32 + w1) >> 11 + 0.5) 2^-53 from the words w0, w1 of Philox4x32-10 under the run's key with counter
+ * (0x80000000 | k, l, c mod 2^32, c >> 32): the high bit keeps this stream apart from the O noise, whose first counter
+ * word is a coordinate-pair index below 2^31.
+ * Velocities: an accepted swap moves the R, V, F and E_pot rows together and swaps the two walker labels.  The
+ * full-step velocity w of a configuration moving from kT_a to kT_b is scaled by lam = sqrt(kT_b / kT_a), computed on
+ * the host: the handle holds v = w - h (F s) (before the step's pending half-kick), w = v + h (F s) and
+ * v' = lam w - h (F s), rounded as written with the configuration's own F.  Frame c shows the state after its exchange.
+ * Walker labels: one int32 per slot follows each configuration; it is the slot the configuration held at
+ * sgdml_b200_md_set_state, which resets the labels to the identity (the first replica-exchange call on a handle sets
+ * them to the identity too).
+ * Arguments: n_temps >= 2 dividing n_rep; kT (n_temps) HOST doubles, each finite and > 0; gamma > 0; exchange_every
+ * >= 0; n_steps, dt, seed, stride as sgdml_b200_md_run.  Outputs, each host, device or NULL: R_frames, V_frames
+ * (n_frames, n_rep, 3N), E_pot_frames, E_kin_frames (n_frames, n_rep) doubles and walker_frames (n_frames, n_rep)
+ * int32 as the frames of sgdml_b200_md_run; walkers_out (n_rep) int32, the labels after the run; n_accepted and
+ * n_attempted (n_ladders, n_temps - 1) int64, this run's accepted and attempted swaps of each neighbour pair.  Needs a
+ * state.  Launches count under family 8 (exchange, integrator) and 1 (graph replays).  Argument errors are reported
+ * before anything is queued, and a rejected call changes nothing. */
+int sgdml_b200_remd_run(sgdml_b200_md* md, int64_t n_temps, const double* kT, int64_t n_steps, double dt, double gamma,
+                        uint64_t seed, int64_t exchange_every, int64_t stride, double* R_frames, double* V_frames,
+                        double* E_pot_frames, double* E_kin_frames, int* walker_frames, int* walkers_out,
+                        int64_t* n_accepted, int64_t* n_attempted, void* stream);
+
 /* ---------------------------------------------------------------- path-integral molecular dynamics on the device
  * Extension: ring polymers of P beads (1 <= P <= 64), thermostatted mode by mode with PILE-L (Ceriotti, Parrinello,
  * Markland & Manolopoulos, J. Chem. Phys. 133, 124104 (2010)) in the BAOAB order of Liu, Li & Liu (J. Chem. Phys. 145,

@@ -1,6 +1,7 @@
-// Molecular dynamics, path-integral MD and geometry optimisation on the device: the integrator and optimiser kernels
-// (contract in md.cuh), then the driver of sgdml_b200_md_*, sgdml_b200_pimd_* and sgdml_b200_relax_*, which evaluates
-// forces through the predictor interface of predict.cuh.
+// Molecular dynamics, replica exchange, path-integral MD and geometry optimisation on the device: the integrator,
+// exchange and optimiser kernels (contract in md.cuh), then the driver of sgdml_b200_md_*, sgdml_b200_remd_run,
+// sgdml_b200_pimd_*, sgdml_b200_relax_* and sgdml_b200_neb_fire, which evaluates forces through the predictor interface
+// of predict.cuh.
 //
 // The BAOAB Langevin integrator step of sgdml_b200_md_run.
 //
@@ -67,6 +68,7 @@ __global__ void __launch_bounds__(MD_THREADS) k_md_step(const MdParams* __restri
   double* r = R + rep * dimi;
   double* v = V + rep * dimi;
   const double* f = F + rep * dimi;
+  const double* sg = sigma + (rep % p.n_temps) * dimi;
   const int64_t fo = (frame * n_rep + rep) * dimi;
   double ke = 0.0;
   const int n_pairs = (dimi + 1) / 2;
@@ -99,7 +101,7 @@ __global__ void __launch_bounds__(MD_THREADS) k_md_step(const MdParams* __restri
       if (advance) {
         vi = __dadd_rn(vi, kick);
         ri = __dadd_rn(ri, __dmul_rn(p.h, vi));
-        if (p.use_O) vi = __dadd_rn(__dmul_rn(p.c1, vi), __dmul_rn(sigma[i], xi[q]));
+        if (p.use_O) vi = __dadd_rn(__dmul_rn(p.c1, vi), __dmul_rn(sg[i], xi[q]));
         ri = __dadd_rn(ri, __dmul_rn(p.h, vi));
         r[i] = ri;
       }
@@ -120,6 +122,89 @@ __global__ void __launch_bounds__(MD_THREADS) k_md_step(const MdParams* __restri
   }
   __syncthreads();  // every thread has read the counter
   if (advance && threadIdx.x == 0) step[rep] = n + 1;
+}
+
+// The replica exchange of sgdml_b200_remd_run (contract in md.cuh).  Thread t decides the pairs t, t + MD_THREADS, ...
+// of its ladder and swaps their energies, walker labels and counts; then every thread swaps its coordinates of the
+// accepted pairs' R, V and F rows.  The pairs are disjoint, so no two threads touch the same entry.
+__global__ void __launch_bounds__(MD_THREADS) k_remd_exchange(const RemdParams* __restrict__ X,
+                                                             const MdParams* __restrict__ P,
+                                                             const double* __restrict__ s, double* __restrict__ R,
+                                                             double* __restrict__ V, double* __restrict__ F,
+                                                             double* __restrict__ E, int* __restrict__ walker,
+                                                             const uint64_t* __restrict__ step, int dimi) {
+  __shared__ int acc[MD_THREADS];
+  const RemdParams x = *X;
+  const int nt = x.n_temps;
+  const int64_t lad = blockIdx.x, n_rep = (int64_t)gridDim.x * nt, base = lad * nt;
+  const uint64_t c = step[base];
+  const uint64_t done = c - x.run_start;
+  const bool sample = done != 0 && x.stride > 0 && done % (uint64_t)x.stride == 0 && x.W_f != nullptr;
+  const bool exchange = x.every > 0 && done != 0 && c % (uint64_t)x.every == 0;
+  if (!exchange && !sample) return;
+  if (exchange) {
+    const double h = P->h;
+    const int par = (int)((c / (uint64_t)x.every) & 1);
+    const int n_pairs = (nt - par) / 2;  // k = 2 j + par for j < n_pairs
+    for (int j0 = 0; j0 < n_pairs; j0 += MD_THREADS) {
+      const int j = j0 + (int)threadIdx.x;
+      if (j < n_pairs) {
+        const int k = 2 * j + par;
+        const int64_t a = base + k, b = a + 1;
+        const double ea = E[a], eb = E[b];
+        const double d = __dmul_rn(__dsub_rn(x.beta[k], x.beta[k + 1]), __dsub_rn(ea, eb));
+        bool ok = d >= 0.0;
+        if (!ok) {
+          uint32_t ct[4] = {0x80000000u | (uint32_t)k, (uint32_t)lad, (uint32_t)c, (uint32_t)(c >> 32)};
+          philox4x32_10(ct, x.key[0], x.key[1]);
+          ok = uniform53(ct[0], ct[1]) < exp(d);
+        }
+        acc[threadIdx.x] = ok ? 1 : 0;
+        const int64_t q = lad * (nt - 1) + k;
+        x.n_att[q] += 1;
+        if (ok) {
+          x.n_acc[q] += 1;
+          E[a] = eb;
+          E[b] = ea;
+          const int w = walker[a];
+          walker[a] = walker[b];
+          walker[b] = w;
+        }
+      }
+      __syncthreads();  // the decisions are in acc
+      const int nj = min(MD_THREADS, n_pairs - j0);
+      for (int t = 0; t < nj; ++t) {
+        if (!acc[t]) continue;
+        const int k = 2 * (j0 + t) + par;
+        const int64_t o = (base + k) * dimi;
+        double *ra = R + o, *va = V + o, *fa = F + o;
+        double *rb = ra + dimi, *vb = va + dimi, *fb = fa + dimi;
+        const double lu = x.lam_up[k], ld = x.lam_dn[k];
+        for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+          const double ka = __dmul_rn(h, __dmul_rn(fa[i], s[i])), kb = __dmul_rn(h, __dmul_rn(fb[i], s[i]));
+          const double wa = __dadd_rn(va[i], ka), wb = __dadd_rn(vb[i], kb);
+          va[i] = __dsub_rn(__dmul_rn(ld, wb), kb);  // configuration b moves down to slot k
+          vb[i] = __dsub_rn(__dmul_rn(lu, wa), ka);  // configuration a moves up to slot k + 1
+          const double r = ra[i], f = fa[i];
+          ra[i] = rb[i];
+          rb[i] = r;
+          fa[i] = fb[i];
+          fb[i] = f;
+        }
+      }
+      __syncthreads();  // acc is free again, and the walker labels are swapped
+    }
+  }
+  if (sample) {
+    const int64_t frame = (int64_t)(done / (uint64_t)x.stride) - 1;
+    for (int k = threadIdx.x; k < nt; k += MD_THREADS) x.W_f[frame * n_rep + base + k] = walker[base + k];
+  }
+}
+
+// sets the walker labels of the n_rep slots to the identity
+__global__ void k_remd_identity(int* walker, int64_t n_rep) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < n_rep) walker[r] = (int)r;
 }
 
 // k_md_step's fixed-order tree over the CTA; every thread gets the sum
@@ -643,7 +728,7 @@ __global__ void k_relax_report(const RelaxState* __restrict__ st, int64_t n_rep,
 
 }  // namespace sgdml
 
-// ============================================================== driver (sgdml_b200_md_*, _pimd_*, _relax_*)
+// ============================================================== driver (sgdml_b200_md_*, _remd_run, _pimd_*, _relax_*)
 // The state of n_rep replicas stays in device memory between steps and between runs.  One step is the integrator
 // kernel, then the forces and energies of the new positions (force_eval_run, predict.cuh) written back into the
 // state.  That sequence is captured once into a CUDA graph and replayed n_steps times on the caller's stream;
@@ -661,7 +746,8 @@ struct sgdml_b200_md {
   uint64_t* step = nullptr;             // (n_rep) step counters, all equal
   uint64_t step_host = 0;               // their value once the queued runs have finished
   bool has_state = false;
-  double *s = nullptr, *sigma = nullptr;  // (3N) inverse mass, (nb, 3N) noise scale per mode and coordinate
+  double *s = nullptr, *sigma = nullptr;  // (3N) inverse mass, (sigma_rows, 3N) noise scale per mode or temperature
+  int sigma_rows = 0;                     // rows sigma and hSigma hold: nb at creation, more for a replica exchange
   std::vector<double> s_host;             // s on the host
   MdParams* dP = nullptr;
   MdParams* hP = nullptr;     // pinned staging of dP and sigma, reused once the previous run's upload is done
@@ -690,8 +776,15 @@ struct sgdml_b200_md {
   NebParams* hN = nullptr;    // pinned staging of dN
   double* Fn = nullptr;       // (n_rep, 3N) NEB forces of the interior images
   int* climb_idx = nullptr;   // (n_rep) the highest interior image of each band (the first n_rep / P entries)
-  int neb_P = 0;              // images per band of the current NEB call
-  int graph_P = 0;            // ... and of the captured NEB step
+  // replica exchange (sgdml_b200_remd_run), allocated by the first replica-exchange call
+  RemdParams* dX = nullptr;
+  RemdParams* hX = nullptr;   // pinned staging of dX
+  double *xtab = nullptr, *hXtab = nullptr;  // beta, lam_up, lam_dn (n_rep each) and their pinned staging
+  int* walker = nullptr;      // (n_rep) walker label per slot
+  int64_t* xcount = nullptr;  // (2, n_rep) accepted and attempted swaps of the current run
+  // replicas per group of the current call: images per band (NEB), temperatures per ladder (replica exchange)
+  int group = 0;
+  int graph_group = 0;        // ... and of the captured step
 };
 
 namespace {
@@ -714,6 +807,12 @@ void md_free(sgdml_b200_md* md) {
   cached_free(md->dR);
   cached_free(md->dN);
   cached_free(md->climb_idx);
+  cached_free(md->dX);
+  cached_free(md->xtab);
+  cached_free(md->walker);
+  cached_free(md->xcount);
+  cudaFreeHost(md->hX);
+  cudaFreeHost(md->hXtab);
   cudaFreeHost(md->hR);
   cudaFreeHost(md->hN);
   cudaFreeHost(md->hActive);
@@ -776,7 +875,7 @@ class Outputs {
   }
 
  private:
-  static constexpr int MAX_OUTS = 6;
+  static constexpr int MAX_OUTS = 8;
   cudaStream_t s_;
   int n_ = 0;
   Out out_[MAX_OUTS];
@@ -787,11 +886,12 @@ class Outputs {
 };
 
 // what one step of the handle's graph integrates
-enum MdKind { MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, MD_NEB_FIRE = 4 };
+enum MdKind { MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, MD_NEB_FIRE = 4, MD_REMD = 5 };
 
-// the integrator of sgdml_b200_md_run, sgdml_b200_pimd_run, sgdml_b200_relax_* or sgdml_b200_neb_fire; advance == 0
-// completes a run's last step (MD) or only tests convergence (relaxation, NEB: after the force projection).  L-BFGS
-// keeps its direction in V, which relax_impl zeroes after.
+// the integrator of sgdml_b200_md_run, sgdml_b200_remd_run, sgdml_b200_pimd_run, sgdml_b200_relax_* or
+// sgdml_b200_neb_fire; advance == 0 completes a run's last step (MD; a replica exchange first exchanges that last
+// state) or only tests convergence (relaxation, NEB: after the force projection).  L-BFGS keeps its direction in V,
+// which relax_impl zeroes after.
 int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
   switch (kind) {
     case MD_RING_POLYMER:
@@ -807,8 +907,8 @@ int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
                                                               advance);
       break;
     case MD_NEB_FIRE: {
-      const int64_t n_bands = md->n_rep / md->neb_P;
-      k_neb_force<<<(unsigned)(n_bands * (md->neb_P - 2)), MD_THREADS, 0, s>>>(md->dN, md->R, md->F, md->E, md->Fn,
+      const int64_t n_bands = md->n_rep / md->group;
+      k_neb_force<<<(unsigned)(n_bands * (md->group - 2)), MD_THREADS, 0, s>>>(md->dN, md->R, md->F, md->E, md->Fn,
                                                                               md->climb_idx, md->dimi);
       SG_CUDA(cudaGetLastError());
       count_launch(KID_MISC);
@@ -816,6 +916,13 @@ int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
                                                                advance);
       break;
     }
+    case MD_REMD:
+      k_remd_exchange<<<(unsigned)(md->n_rep / md->group), MD_THREADS, 0, s>>>(md->dX, md->dP, md->s, md->R, md->V,
+                                                                              md->F, md->E, md->walker, md->step,
+                                                                              md->dimi);
+      SG_CUDA(cudaGetLastError());
+      count_launch(KID_MISC);
+      [[fallthrough]];
     default:
       k_md_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E,
                                                            md->step, md->dimi, advance);
@@ -831,9 +938,10 @@ int md_step(sgdml_b200_md* md, int kind, cudaStream_t s) {
 }
 
 // the step graph, captured again whenever the force evaluation it bakes in is stale, the integrator (MdKind) changes
-// or, for NEB, the images per band (its grids) change
+// or, for NEB and replica exchange, the replicas per group (their grids) change
 int md_graph(sgdml_b200_md* md, int kind, cudaStream_t s) {
-  if (md->exec != nullptr && md->graph_kind == kind && (kind != MD_NEB_FIRE || md->graph_P == md->neb_P) &&
+  const bool grouped = kind == MD_NEB_FIRE || kind == MD_REMD;
+  if (md->exec != nullptr && md->graph_kind == kind && (!grouped || md->graph_group == md->group) &&
       !force_eval_stale(md->fe))
     return 0;
   if (md->exec != nullptr) {
@@ -853,7 +961,7 @@ int md_graph(sgdml_b200_md* md, int kind, cudaStream_t s) {
   SG_TRY(capture_graph(md->gs, [&] { return md_step(md, kind, md->gs); }, &md->exec, &md->n_kernels));
   force_eval_mark(md->fe);
   md->graph_kind = kind;
-  md->graph_P = md->neb_P;
+  md->graph_group = md->group;
   return 0;
 }
 
@@ -887,14 +995,96 @@ void run_params(P& p, const sgdml_b200_md* md, double dt, uint64_t seed, int64_t
   p.Ek_f = out.dev(3);
 }
 
-// MD: c1 and the (3N) sigma table
-int md_params(sgdml_b200_md* md, double dt, double gamma, double kT, cudaStream_t s) {
+// MD: c1 and the (n_temps, 3N) sigma table, one row per temperature kT[k] (n_temps = 1 for sgdml_b200_md_run)
+int md_params(sgdml_b200_md* md, double dt, double gamma, const double* kT, int n_temps, cudaStream_t s) {
   MdParams& p = *md->hP;
+  const int dimi = md->dimi;
   p.c1 = std::exp(-gamma * dt);
   p.use_O = gamma > 0.0 ? 1 : 0;
-  for (int i = 0; i < md->dimi; ++i) md->hSigma[i] = std::sqrt((1.0 - p.c1 * p.c1) * kT * md->s_host[(size_t)i]);
+  p.n_temps = n_temps;
+  for (int k = 0; k < n_temps; ++k)
+    for (int i = 0; i < dimi; ++i)
+      md->hSigma[(size_t)k * dimi + i] = std::sqrt((1.0 - p.c1 * p.c1) * kT[k] * md->s_host[(size_t)i]);
   SG_CUDA(cudaMemcpyAsync(md->dP, md->hP, sizeof(MdParams), cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * md->dimi, cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * n_temps * dimi, cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+// The sigma table and its staging grow to `rows` rows (one per temperature of a replica exchange).  The captured step
+// reads the old table, so it is captured again.
+int sigma_reserve(sgdml_b200_md* md, int rows) {
+  if (rows <= md->sigma_rows) return 0;
+  SG_CUDA(cudaDeviceSynchronize());  // the old table and its staging go back: nothing may still use them
+  if (md->exec != nullptr) {
+    cudaGraphExecDestroy(md->exec);
+    md->exec = nullptr;
+  }
+  cached_free(md->sigma);
+  cudaFreeHost(md->hSigma);
+  md->sigma = nullptr;
+  md->hSigma = nullptr;
+  md->sigma_rows = 0;
+  SG_CUDA(cached_malloc(&md->sigma, sizeof(double) * rows * md->dimi));
+  SG_CUDA(cudaMallocHost(&md->hSigma, sizeof(double) * rows * md->dimi));
+  md->sigma_rows = rows;
+  return 0;
+}
+
+// What a replica-exchange run (sgdml_b200_remd_run) adds to an MD run: its ladder (kT on the host, checked), its
+// schedule and its outputs beyond the frames.
+struct RemdRun {
+  int n_temps;
+  const double* kT;
+  int64_t every;
+  int *W_f, *walkers;
+  int64_t *n_acc, *n_att;
+};
+
+// the replica-exchange state, made at the first replica-exchange call, which sets the walker labels to the identity
+int remd_alloc(sgdml_b200_md* md, cudaStream_t s) {
+  const size_t n = (size_t)md->n_rep;
+  if (md->dX == nullptr) SG_CUDA(cached_malloc(&md->dX, sizeof(RemdParams)));
+  if (md->hX == nullptr) SG_CUDA(cudaMallocHost(&md->hX, sizeof(RemdParams)));
+  if (md->xtab == nullptr) SG_CUDA(cached_malloc(&md->xtab, 3 * sizeof(double) * n));
+  if (md->hXtab == nullptr) SG_CUDA(cudaMallocHost(&md->hXtab, 3 * sizeof(double) * n));
+  if (md->xcount == nullptr) SG_CUDA(cached_malloc(&md->xcount, 2 * sizeof(int64_t) * n));
+  if (md->walker == nullptr) {
+    SG_CUDA(cached_malloc(&md->walker, sizeof(int) * n));
+    k_remd_identity<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(md->walker, md->n_rep);
+    SG_CUDA(cudaGetLastError());
+    count_launch(KID_MISC);
+  }
+  return 0;
+}
+
+// the exchange's parameters into the pinned staging and their upload on s (after run_params and md_params), and the
+// run's counts zeroed.  beta and lam are computed here, on the host in double precision.
+int remd_params(sgdml_b200_md* md, const RemdRun& x, const Outputs& out, cudaStream_t s) {
+  const int nt = x.n_temps;
+  const MdParams& p = *md->hP;
+  RemdParams& q = *md->hX;
+  q.key[0] = p.key[0];
+  q.key[1] = p.key[1];
+  q.run_start = p.run_start;
+  q.stride = p.stride;
+  q.every = x.every;
+  q.n_temps = nt;
+  double *beta = md->hXtab, *up = beta + nt, *dn = up + nt;
+  for (int k = 0; k < nt; ++k) beta[k] = 1.0 / x.kT[k];
+  for (int k = 0; k + 1 < nt; ++k) {
+    up[k] = std::sqrt(x.kT[k + 1] / x.kT[k]);
+    dn[k] = std::sqrt(x.kT[k] / x.kT[k + 1]);
+  }
+  q.beta = md->xtab;
+  q.lam_up = md->xtab + nt;
+  q.lam_dn = md->xtab + 2 * nt;
+  q.n_acc = md->xcount;
+  q.n_att = md->xcount + md->n_rep;
+  q.W_f = out.dev<int>(4);
+  md->group = nt;
+  SG_CUDA(cudaMemcpyAsync(md->dX, md->hX, sizeof(RemdParams), cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaMemcpyAsync(md->xtab, md->hXtab, 3 * sizeof(double) * nt, cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaMemsetAsync(md->xcount, 0, 2 * sizeof(int64_t) * (size_t)md->n_rep, s));
   return 0;
 }
 
@@ -950,10 +1140,11 @@ int pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, double kT, dou
   return 0;
 }
 
-// sgdml_b200_md_run (MD_CLASSICAL) and sgdml_b200_pimd_run (MD_RING_POLYMER; hbar and lambda are only its own).
+// sgdml_b200_md_run (MD_CLASSICAL), sgdml_b200_pimd_run (MD_RING_POLYMER; hbar and lambda are only its own) and
+// sgdml_b200_remd_run (MD_REMD, with x: its ladder, checked by the caller, and kT = its first temperature).
 // frames: R, V, E_pot, E_kin, then the ring polymer's K_prim and K_cv.  n_steps steps, then the completing launch.
 int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, double hbar, double gamma, double lambda,
-           uint64_t seed, int64_t stride, double* const frames[6], cudaStream_t s) {
+           uint64_t seed, int64_t stride, double* const frames[6], const RemdRun* x, cudaStream_t s) {
   const bool ring = kind == MD_RING_POLYMER;
   SG_TRY(require_device());
   SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
@@ -972,29 +1163,50 @@ int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, d
     return fail_arg("kT > 0 needs a friction gamma > 0 (a thermostat without coupling)");
   if (stride > 0 && n_steps % stride != 0) return fail_arg("n_steps must be a multiple of stride");
   if (!md->has_state)
-    return fail_arg(ring ? "sgdml_b200_pimd_run: no state yet (call sgdml_b200_md_set_state)"
-                         : "sgdml_b200_md_run: no state yet (call sgdml_b200_md_set_state)");
-  if (n_steps == 0) return 0;
+    return fail_arg(ring        ? "sgdml_b200_pimd_run: no state yet (call sgdml_b200_md_set_state)"
+                    : x != nullptr ? "sgdml_b200_remd_run: no state yet (call sgdml_b200_md_set_state)"
+                                   : "sgdml_b200_md_run: no state yet (call sgdml_b200_md_set_state)");
+  if (n_steps == 0 && x == nullptr) return 0;  // (a replica exchange still reports its labels and zero counts)
 
   const int64_t n_frames = stride > 0 ? n_steps / stride : 0;
   const size_t fr = sizeof(double) * (size_t)(n_frames * md->n_rep);
   const size_t fp = sizeof(double) * (size_t)(n_frames * (md->n_rep / md->nb));
   Outputs out(s);
-  SG_TRY(out.init({{frames[0], fr * md->dimi}, {frames[1], fr * md->dimi}, {frames[2], fr}, {frames[3], fr},
-                   {frames[4], fp}, {frames[5], fp}}));
+  if (x == nullptr) {
+    SG_TRY(out.init({{frames[0], fr * md->dimi}, {frames[1], fr * md->dimi}, {frames[2], fr}, {frames[3], fr},
+                     {frames[4], fp}, {frames[5], fp}}));
+  } else {  // frames, walker frames, final walker labels, then the counts (n_ladders, n_temps - 1)
+    const size_t wf = sizeof(int) * (size_t)(n_frames * md->n_rep);
+    const size_t nc = sizeof(int64_t) * (size_t)(md->n_rep / x->n_temps * (x->n_temps - 1));
+    SG_TRY(out.init({{frames[0], fr * md->dimi}, {frames[1], fr * md->dimi}, {frames[2], fr}, {frames[3], fr},
+                     {x->W_f, wf}, {x->walkers, sizeof(int) * (size_t)md->n_rep}, {x->n_acc, nc}, {x->n_att, nc}}));
+  }
   SG_TRY(force_eval_prepare(md->fe));
+  if (x != nullptr) {
+    SG_TRY(sigma_reserve(md, x->n_temps));
+    SG_TRY(remd_alloc(md, s));
+  }
   SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous run has read the staging
   if (ring) {
     run_params(*md->hQ, md, dt, seed, n_frames, stride, out);
     SG_TRY(pimd_params(md, out, dt, kT, hbar, gamma, lambda, s));
   } else {
     run_params(*md->hP, md, dt, seed, n_frames, stride, out);
-    SG_TRY(md_params(md, dt, gamma, kT, s));
+    SG_TRY(md_params(md, dt, gamma, x != nullptr ? x->kT : &kT, x != nullptr ? x->n_temps : 1, s));
+    if (x != nullptr) SG_TRY(remd_params(md, *x, out, s));
   }
   SG_CUDA(cudaEventRecord(md->uploaded, s));
-  SG_TRY(md_replay(md, kind, n_steps, s));
-  md->step_host += (uint64_t)n_steps;
-  SG_TRY(md_integrate(md, kind, 0, s));  // the second half-kick of the last step (and its frame)
+  if (n_steps > 0) {
+    SG_TRY(md_replay(md, kind, n_steps, s));
+    md->step_host += (uint64_t)n_steps;
+    SG_TRY(md_integrate(md, kind, 0, s));  // the second half-kick of the last step (and its frame)
+  }
+  if (x != nullptr) {
+    const void* src[3] = {md->walker, md->xcount, md->xcount + md->n_rep};
+    for (int i = 0; i < 3; ++i)
+      if (out.dev<void>(5 + i) != nullptr)
+        SG_CUDA(cudaMemcpyAsync(out.dev<void>(5 + i), src[i], out.bytes(5 + i), cudaMemcpyDeviceToDevice, s));
+  }
   return out.finish();
 }
 
@@ -1056,7 +1268,7 @@ int stage_relax(sgdml_b200_md* md, const RelaxParams& prm, cudaStream_t s) {
 
 int stage_neb(sgdml_b200_md* md, const NebParams& q, cudaStream_t s) {
   *md->hN = q;
-  md->neb_P = q.P;
+  md->group = q.P;
   SG_CUDA(cudaMemcpyAsync(md->dN, md->hN, sizeof(NebParams), cudaMemcpyHostToDevice, s));
   return 0;
 }
@@ -1142,6 +1354,7 @@ int md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, int nb, c
     SG_CUDA(cudaMallocHost(&md->hQ, sizeof(PimdParams)));
     SG_CUDA(cudaMallocHost(&md->hTab, sizeof(double) * (nb * nb + 4 * nb)));
     SG_CUDA(cudaMallocHost(&md->hSigma, sizeof(double) * nb * md->dimi));
+    md->sigma_rows = nb;
     SG_CUDA(cudaEventCreateWithFlags(&md->uploaded, cudaEventDisableTiming));
     md->s_host.resize((size_t)md->dimi);
     for (int i = 0; i < md->dimi; ++i) md->s_host[(size_t)i] = inv_mass[i / 3];
@@ -1196,6 +1409,11 @@ int sgdml_b200_md_set_state(sgdml_b200_md* md, const double* R, const double* V,
   const std::vector<uint64_t> steps((size_t)md->n_rep, step);
   SG_CUDA(cudaMemcpyAsync(md->step, steps.data(), sizeof(uint64_t) * md->n_rep, cudaMemcpyHostToDevice, s));
   SG_TRY(force_eval_run(md->fe, md->R, md->F, md->E, s));
+  if (md->walker != nullptr) {  // a replica exchange's walkers start again from their slots
+    k_remd_identity<<<(unsigned)((md->n_rep + 255) / 256), 256, 0, s>>>(md->walker, md->n_rep);
+    SG_CUDA(cudaGetLastError());
+    count_launch(KID_MISC);
+  }
   SG_CUDA(cudaStreamSynchronize(s));  // (the counters' host vector goes out of scope)
   md->step_host = step;
   md->has_state = true;
@@ -1222,7 +1440,26 @@ int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamm
                       int64_t stride, double* R_frames, double* V_frames, double* E_pot_frames, double* E_kin_frames,
                       void* stream) {
   double* const frames[6] = {R_frames, V_frames, E_pot_frames, E_kin_frames, nullptr, nullptr};
-  return md_run(md, MD_CLASSICAL, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, frames, (cudaStream_t)stream);
+  return md_run(md, MD_CLASSICAL, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, frames, nullptr,
+                (cudaStream_t)stream);
+}
+
+int sgdml_b200_remd_run(sgdml_b200_md* md, int64_t n_temps, const double* kT, int64_t n_steps, double dt, double gamma,
+                        uint64_t seed, int64_t exchange_every, int64_t stride, double* R_frames, double* V_frames,
+                        double* E_pot_frames, double* E_kin_frames, int* walker_frames, int* walkers_out,
+                        int64_t* n_accepted, int64_t* n_attempted, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr && kT != nullptr);
+  if (md->nb > 1) return fail_arg("sgdml_b200_remd_run: a ring-polymer handle (n_beads > 1) holds no ladders");
+  SG_ARG(n_temps >= 2 && md->n_rep % n_temps == 0);
+  SG_ARG(!is_device_ptr(kT));
+  for (int64_t k = 0; k < n_temps; ++k)
+    if (!(std::isfinite(kT[k]) && kT[k] > 0.0)) return fail_arg("sgdml_b200_remd_run: every kT must be finite and > 0");
+  SG_ARG(std::isfinite(gamma) && gamma > 0.0);
+  SG_ARG(exchange_every >= 0);
+  const RemdRun x = {(int)n_temps, kT, exchange_every, walker_frames, walkers_out, n_accepted, n_attempted};
+  double* const frames[6] = {R_frames, V_frames, E_pot_frames, E_kin_frames, nullptr, nullptr};
+  return md_run(md, MD_REMD, n_steps, dt, kT[0], 0.0, gamma, 0.0, seed, stride, frames, &x, (cudaStream_t)stream);
 }
 
 int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma,
@@ -1230,7 +1467,8 @@ int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT
                         double* E_pot_frames, double* E_kin_frames, double* K_prim_frames, double* K_cv_frames,
                         void* stream) {
   double* const frames[6] = {R_frames, V_frames, E_pot_frames, E_kin_frames, K_prim_frames, K_cv_frames};
-  return md_run(md, MD_RING_POLYMER, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, frames, (cudaStream_t)stream);
+  return md_run(md, MD_RING_POLYMER, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, frames, nullptr,
+                (cudaStream_t)stream);
 }
 
 int sgdml_b200_relax_fire(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, double dt, double dtmax,

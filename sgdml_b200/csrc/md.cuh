@@ -1,6 +1,6 @@
-// Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_pimd_*, sgdml_b200_relax_*, sgdml_b200_neb_fire): the
-// contract of the kernels in md.cu -- the BAOAB integrator step, its ring-polymer form, their counter-based noise, the
-// FIRE and L-BFGS steps, and the nudged elastic band.
+// Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_pimd_*, sgdml_b200_relax_*,
+// sgdml_b200_neb_fire): the contract of the kernels in md.cu -- the BAOAB integrator step, the replica exchange, the
+// ring-polymer step, their counter-based noise, the FIRE and L-BFGS steps, and the nudged elastic band.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -17,6 +17,7 @@ struct MdParams {
   int stride;         // 0: no frames
   uint64_t run_start; // the handle's step index when the run began
   double *R_f, *V_f, *Ep_f, *Ek_f;  // frames (n_frames, n_rep, 3N) / (n_frames, n_rep)
+  int n_temps;        // rows of the sigma table: replica rep uses row rep % n_temps (1: one temperature)
 };
 
 // k_md_step: one step for every replica (grid: one CTA of MD_THREADS per replica).  With the handle's step counter at n:
@@ -24,8 +25,36 @@ struct MdParams {
 //                       frame (n - run_start) / stride - 1 when that is whole: R, full-step V, E_pot, E_kin
 //   if advance:         B, A, O (noise of step n), A; R and V hold the new positions and half-step velocities,
 //                       and the counter becomes n + 1
-// advance == 0 only completes the last step of a run.  s, sigma: (3N) inverse mass and noise scale per coordinate.
+// advance == 0 only completes the last step of a run.  s: (3N) inverse mass per coordinate; sigma: (n_temps, 3N)
+// noise scale per temperature and coordinate, row rep % n_temps for replica rep.
 constexpr int MD_THREADS = 128;
+
+// Replica exchange (sgdml_b200_remd_run): a plain MD handle of n_rep = n_ladders n_temps replicas; slot l n_temps + k
+// is temperature k of ladder l for the whole run, and exchanges move configurations between slots.
+struct RemdParams {
+  uint32_t key[2];      // the run's Philox key, as MdParams
+  uint64_t run_start;   // as MdParams
+  int64_t every;        // E: an exchange on the state at c when E >= 1, c > run_start and c % E == 0 (0: never)
+  int n_temps;          // slots per ladder (>= 2)
+  int stride;           // as MdParams (0: no walker frames)
+  const double* beta;   // (n_temps) 1 / kT_k
+  const double* lam_up; // (n_temps - 1) sqrt(kT_k+1 / kT_k): the configuration moving from slot k to k + 1
+  const double* lam_dn; // (n_temps - 1) sqrt(kT_k / kT_k+1): the configuration moving from slot k + 1 to k
+  int64_t *n_acc, *n_att;  // (n_ladders, n_temps - 1) accepted and attempted swaps of pair (k, k + 1) in this run
+  int* W_f;             // walker frames (n_frames, n_rep), or null
+};
+
+// k_remd_exchange: one CTA of MD_THREADS per ladder, launched before k_md_step on the same counter c (the state R
+// holds).  V holds the velocity before k_md_step's pending half-kick.  On an exchange step, with e = c / E, the pairs
+// (k, k + 1) with k % 2 == e % 2 and k + 1 < n_temps are attempted, each independently:
+//   D = (beta_k - beta_k+1) (E_k - E_k+1)   (rounded as written)
+//   accepted iff D >= 0 or u < exp(D), u = uniform53 of words 0, 1 of Philox4x32-10 under the run's key with counter
+//   (0x80000000 | k, l, c mod 2^32, c >> 32)  (the O noise's first counter word is a pair index below 2^31)
+// An accepted swap exchanges the R, F and E rows and the walker labels of the two slots, and the velocity of each
+// configuration, moving from slot a to slot b with lam = sqrt(kT_b / kT_a), becomes
+//   w = v + h (F s)  (k_md_step's rounding),  v' = lam w - h (F s)
+// with the configuration's own F.  n_att and n_acc of the pair count the attempt and the acceptance.  On a frame step
+// of k_md_step (the same rule) the CTA writes the ladder's walker labels after the swaps into W_f.
 
 // Path-integral MD (sgdml_b200_pimd_run): replica p P + j is bead j of ring polymer p.
 constexpr int PIMD_MAX_BEADS = 64;  // C (P x P) sits in shared memory: 32 KB at the cap

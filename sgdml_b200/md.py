@@ -4,6 +4,10 @@ positions, velocities and forces kept in GPU memory between steps.  ``GDMLPathIn
 of ring polymers on the same engine (``sgdml_b200_pimd_*``): PILE-L thermostatted (or NVE) ring-polymer trajectories
 with the primitive and centroid-virial quantum kinetic-energy estimators.
 
+``GDMLReplicaExchange`` -- temperature replica exchange (parallel tempering) on the same engine
+(``sgdml_b200_remd_run``): ladders of Langevin replicas at fixed temperatures whose neighbours swap configurations by a
+Metropolis test inside the step graph.
+
 ``GDMLRelaxation`` -- geometry optimisation of many replicas on the same engine (``sgdml_b200_relax_*``): FIRE and
 L-BFGS, each replica frozen once it has converged.
 
@@ -102,12 +106,12 @@ class GDMLDynamics(object):
             raise ValueError('%s must hold n_replicas x 3N = %d x %d values' % (name, self.n_replicas, dimi))
         return x.reshape(self.n_replicas, dimi).contiguous() if hasattr(x, 'data_ptr') else x.reshape(self.n_replicas, dimi)
 
-    def _empty(self, shape):
+    def _empty(self, shape, dtype=np.float64):
         if self._torch_device is None:
-            return np.empty(shape)
+            return np.empty(shape, dtype=dtype)
         import torch
 
-        return torch.empty(shape, dtype=torch.float64, device=self._torch_device)
+        return torch.empty(shape, dtype=getattr(torch, np.dtype(dtype).name), device=self._torch_device)
 
     # ------------------------------------------------------------------ model units (L, model energy, fs)
     def _set_state_raw(self, R, V=None, step=0):
@@ -134,11 +138,12 @@ class GDMLDynamics(object):
 
     def _frames(self, n_steps, stride, frames, n_poly=0):
         """Empty frame arrays for the names in `frames`: (n_frames, n_replicas, 3N) for R and V, (n_frames, n_poly) for
-        K_prim and K_cv, else (n_frames, n_replicas); {} when the run writes no frames."""
+        K_prim and K_cv, else (n_frames, n_replicas), int32 for the walker labels; {} when the run writes no frames."""
         n_frames = n_steps // stride if stride > 0 and n_steps % stride == 0 else 0
         dims = {'R': (self.n_replicas, 3 * self.n_atoms), 'V': (self.n_replicas, 3 * self.n_atoms), 'K_prim': (n_poly,),
                 'K_cv': (n_poly,)}
-        return {k: self._empty((n_frames,) + dims.get(k, (self.n_replicas,))) for k in frames} if n_frames > 0 else {}
+        return {k: self._empty((n_frames,) + dims.get(k, (self.n_replicas,)), np.int32 if k == 'walker' else np.float64)
+                for k in frames} if n_frames > 0 else {}
 
     def _run_raw(self, n_steps, dt, gamma=0.0, kT=0.0, seed=0, stride=0, frames=('R', 'V', 'E_pot', 'E_kin')):
         n_steps, stride = int(n_steps), int(stride)
@@ -210,17 +215,7 @@ class GDMLPathIntegralDynamics(GDMLDynamics):
 
     def _beads(self, x, name):
         """(n_polymers, n_beads, N, 3), (n_polymers, N, 3) or (N, 3) -> (n_polymers n_beads, 3N)."""
-        N, n_p, P = self.n_atoms, self.n_polymers, self.n_beads
-        shape = tuple(x.shape)
-        if shape == (n_p, P, N, 3):
-            return x
-        if shape == (n_p, N, 3) or shape == (N, 3):
-            x = x.reshape(-1, 1, N, 3)
-            if hasattr(x, 'data_ptr'):
-                return x.expand(n_p, P, N, 3).contiguous()
-            return np.ascontiguousarray(np.broadcast_to(np.asarray(x, dtype=np.float64), (n_p, P, N, 3)))
-        raise ValueError('%s must be (n_polymers, n_beads, N, 3), (n_polymers, N, 3) or (N, 3) = (%d, %d, %d, 3): %s'
-                         % (name, n_p, P, N, shape))
+        return _groups(x, name, self.n_polymers, self.n_beads, self.n_atoms, ('n_polymers', 'n_beads'))
 
     # ------------------------------------------------------------------ model units (L, model energy, fs)
     def _run_raw(self, n_steps, dt, kT, hbar, gamma=0.0, lam=0.0, seed=0, stride=0,
@@ -266,6 +261,113 @@ class GDMLPathIntegralDynamics(GDMLDynamics):
                 'potential_energy': (f['E_pot'] * self.E_to_eV).reshape(nf, n_p, P),
                 'kinetic_energy_primitive': f['K_prim'] * self.E_to_eV,
                 'kinetic_energy_virial': f['K_cv'] * self.E_to_eV}
+
+
+def _groups(x, name, n_g, per, N, axes):
+    """(n_g, per, N, 3), (n_g, N, 3) or (N, 3), the last two copied to every member (and group), as (n_g, per, N, 3);
+    axes names n_g and per in the error message."""
+    shape = tuple(x.shape)
+    if shape == (n_g, per, N, 3):
+        return x
+    if shape == (n_g, N, 3) or shape == (N, 3):
+        x = x.reshape(-1, 1, N, 3)
+        if hasattr(x, 'data_ptr'):
+            return x.expand(n_g, per, N, 3).contiguous()
+        return np.ascontiguousarray(np.broadcast_to(np.asarray(x, dtype=np.float64), (n_g, per, N, 3)))
+    raise ValueError('%s must be (%s, %s, N, 3), (%s, N, 3) or (N, 3) = (%d, %d, %d, 3): %s'
+                     % ((name,) + axes + axes[:1] + (n_g, per, N, shape)))
+
+
+class GDMLReplicaExchange(GDMLDynamics):
+    """Temperature replica exchange (parallel tempering; Sugita & Okamoto, Chem. Phys. Lett. 314, 141 (1999)) of
+    `n_ladders` ladders of Langevin replicas, in the units of ``GDMLDynamics``.  Slot k of ladder l (replica
+    l n_temps + k of the engine's handle) stays at temperatures_K[k] for the whole run; neighbours in `temperatures_K`
+    swap configurations by the Metropolis test, with the velocities rescaled to the new temperature, so every output is
+    sorted by temperature.  A geometric ladder, ``np.geomspace(T_low, T_high, n_temps)``, gives neighbours about equal
+    acceptance when the heat capacity varies little.  The exchanges run inside the step graph on the energies already in
+    device memory: no host round trip per exchange.  A walker label follows each configuration: the slot it held at
+    ``set_state``.
+
+    ``set_state(positions, velocities=None, step=0)``: positions (n_ladders, n_temps, N, 3), or (n_ladders, N, 3) /
+    (N, 3) copied to every slot (and ladder); velocities likewise (None: at rest).  ``set_state`` resets the walker
+    labels to the slots.  ``get_state()`` as ``GDMLDynamics``'s, shaped (n_ladders, n_temps, ...).
+    ``run(n_steps, dt_fs, friction_per_fs, exchange_every, seed=0, stride=0)`` integrates every slot with BAOAB
+    Langevin at its temperature (friction > 0) and attempts exchanges on every `exchange_every`-th state, alternating
+    the even and odd neighbour pairs (0: no exchanges).  It returns {'positions', 'velocities': (n_frames, n_ladders,
+    n_temps, N, 3), 'potential_energy', 'kinetic_energy', 'walker': (n_frames, n_ladders, n_temps)} after every
+    `stride`-th step (none for stride 0), and always 'walkers' (n_ladders, n_temps), the labels after the run, and
+    'n_accepted', 'n_attempted' (int64) and 'acceptance' (their ratio, NaN without attempts), (n_ladders, n_temps - 1),
+    this run's swaps of each neighbour pair (k, k + 1).  Angstrom, Angstrom/fs and eV; NumPy arrays or float64 CUDA
+    tensors in, the same kind out.  A run continued over several calls is one long run."""
+
+    def __init__(self, model, masses, temperatures_K, n_ladders=1, E_to_eV=_KCAL_PER_MOL_IN_EV,
+                 F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        self.temperatures_K = np.array(temperatures_K, dtype=np.float64).ravel()
+        self.n_temps = len(self.temperatures_K)
+        self.n_ladders = int(n_ladders)
+        if self.n_temps < 2 or self.n_ladders < 1:
+            raise ValueError('a ladder needs at least two temperatures, and n_ladders >= 1')
+        super().__init__(model, masses, self.n_ladders * self.n_temps, E_to_eV, F_to_eV_Ang)
+
+    # ------------------------------------------------------------------ model units (L, model energy, fs)
+    def _run_raw(self, n_steps, dt, gamma, kT, exchange_every, seed=0, stride=0,
+                 frames=('R', 'V', 'E_pot', 'E_kin', 'walker')):
+        """kT (n_temps,) in the model's energy unit.  -> frames and 'walkers' (n_replicas,), 'n_accepted',
+        'n_attempted' (n_ladders, n_temps - 1)."""
+        n_steps, stride = int(n_steps), int(stride)
+        out = self._frames(n_steps, stride, frames)
+        kT = np.ascontiguousarray(kT, dtype=np.float64)
+        if kT.shape != (self.n_temps,):
+            raise ValueError('kT must hold one value per temperature: %d' % self.n_temps)
+        walkers = self._empty((self.n_replicas,), np.int32)
+        acc, att = (self._empty((self.n_ladders, self.n_temps - 1), np.int64) for _ in range(2))
+        _lib.check(
+            _lib.lib().sgdml_b200_remd_run(self._handle, self.n_temps, _lib.ptr(kT), n_steps, float(dt), float(gamma),
+                                           int(seed), int(exchange_every), stride,
+                                           *(_lib.ptr(out.get(k)) for k in ('R', 'V', 'E_pot', 'E_kin', 'walker')),
+                                           _lib.ptr(walkers), _lib.ptr(acc), _lib.ptr(att), _lib.current_stream()),
+            'remd_run',
+        )
+        out.update(walkers=walkers, n_accepted=acc, n_attempted=att)
+        return out
+
+    # ------------------------------------------------------------------ ASE units
+    def set_state(self, positions, velocities=None, step=0):
+        axes = ('n_ladders', 'n_temps')
+        positions = _groups(positions, 'positions', self.n_ladders, self.n_temps, self.n_atoms, axes)
+        if velocities is not None:
+            velocities = _groups(velocities, 'velocities', self.n_ladders, self.n_temps, self.n_atoms, axes)
+        super().set_state(positions, velocities, step)
+
+    def get_state(self):
+        """{'positions', 'velocities', 'forces' (n_ladders, n_temps, N, 3), 'potential_energy' (n_ladders, n_temps),
+        'step'}: Angstrom, Angstrom/fs, eV/Angstrom, eV."""
+        st = super().get_state()
+        shape = (self.n_ladders, self.n_temps)
+        for k in ('positions', 'velocities', 'forces'):
+            st[k] = st[k].reshape(shape + (self.n_atoms, 3))
+        st['potential_energy'] = st['potential_energy'].reshape(shape)
+        return st
+
+    def run(self, n_steps, dt_fs, friction_per_fs, exchange_every, seed=0, stride=0):
+        kT = KB_EV * self.temperatures_K / self.E_to_eV
+        f = self._run_raw(n_steps, dt_fs, friction_per_fs, kT, exchange_every, seed, stride)
+        shape = (self.n_ladders, self.n_temps)
+        acc, att = f['n_accepted'], f['n_attempted']
+        if hasattr(att, 'data_ptr'):
+            ratio = acc.double() / att.clip(1).double()
+        else:
+            ratio = acc / att.clip(1)
+        ratio[att == 0] = np.nan
+        out = {'walkers': f['walkers'].reshape(shape), 'n_accepted': acc, 'n_attempted': att, 'acceptance': ratio}
+        if 'R' in f:
+            N, nf = self.n_atoms, f['R'].shape[0]
+            out.update(positions=(f['R'] / self.Ang_to_R).reshape((nf,) + shape + (N, 3)),
+                       velocities=(f['V'] / self.Ang_to_R).reshape((nf,) + shape + (N, 3)),
+                       potential_energy=(f['E_pot'] * self.E_to_eV).reshape((nf,) + shape),
+                       kinetic_energy=(f['E_kin'] * self.E_to_eV).reshape((nf,) + shape),
+                       walker=f['walker'].reshape((nf,) + shape))
+        return out
 
 
 class GDMLRelaxation(GDMLDynamics):

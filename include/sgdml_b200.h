@@ -361,8 +361,9 @@ int sgdml_b200_predict_train_virial(sgdml_b200_model* model, int64_t m_begin, in
 
 /* Large-descriptor models (D > 256: the predictor is four GEMMs around two element-wise kernels): run those GEMMs on
  * the int8 tensor cores (wgmma) through `slices` exact int8 slices per operand (2..7; csrc/ozaki.cu) or in FP64 DMMA (0, the
- * default unless SGDML_B200_OZAKI_PREDICT_SLICES is set when the model is created).  Forces against the FP64 form:
- * 8.8e-9 / 6.5e-11 / 5.4e-13 relative for 4 / 5 / 6 slices.  The iterative solver sets 5 for its K.v products
+ * default unless SGDML_B200_OZAKI_PREDICT_SLICES is set when the model is created).  Forces against the FP64 oracle,
+ * measured on an H100 (N = 24, M = 29; tests/test_ozaki_predict_classes.py): 1.2e-8 / 1.3e-10 / 1.1e-12 / 9.3e-15
+ * relative for 4 / 5 / 6 / 7 slices; tests/ozaki_predict_model.py bounds them componentwise.  The iterative solver sets 5 for its K.v products
  * (iterative.py:183-204: tolerance 1e-4).  No effect for D <= 256. */
 int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* model, int slices, void* stream);
 
@@ -372,6 +373,40 @@ int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* model, int slices,
  * the sweep over the training points.  Workspaces never shrink: it applies fully to models created after the call.
  * Tests lower it to cover the multi-chunk, pipelined and tail-chunk paths at small batch sizes. */
 int sgdml_b200_set_predict_chunk(int64_t max_geos);
+
+/* Test hook (large-descriptor models): the stages of one chunk of the GEMM-composed predictor, copied out of the
+ * production sequence before the next stage overwrites them in place.  Every pointer is a device pointer or NULL (that
+ * stage is not copied).  rows = n_geo * n_perms virtual query rows, row b * n_perms + p being query b under
+ * permutation p; DS = DP + 4, DP = D rounded up to 8, Mpad = M rounded up to 8 (written back by the call). */
+typedef struct sgdml_b200_predict_taps {
+  double* Qg;    /* rows x DS: x[pinv_p] - mu, zero beyond D */
+  double* qq;    /* rows: |Qg row|^2 */
+  double* S1;    /* rows x Mpad: Qg Xc^T as the first GEMM pair left it */
+  double* S2;    /* rows x Mpad: Qg JA^T */
+  double* C1;    /* rows x Mpad: the Matern factors after the transform (zero for m >= M) */
+  double* C2;    /* rows x Mpad */
+  double* csum;  /* rows: sum_m C1 */
+  double* Erow;  /* rows: the energy terms of each row */
+  double* acc;   /* rows x DP: C1 XcT^T + C2 JAT^T, before the combine */
+  double* G;     /* rows x DP: csum Qg - acc */
+  double* Xc;    /* Mpad x DS: the centred training descriptors */
+  double* JA;    /* Mpad x DS: R_d_desc_alpha */
+  double* XcT;   /* DP x Mpad */
+  double* JAT;   /* DP x Mpad */
+  double* mm;    /* Mpad: |Xc row|^2 */
+  double* xja;   /* Mpad: Xc row . JA row */
+  double* mu;    /* DS: the training mean */
+  double* ae;    /* Mpad: alphas_E, or zeros when the model has none */
+  int oz_s;      /* written: the slice count the four GEMMs ran with, 0 for FP64 */
+  int use_ae;    /* written: 1 when the energy-constraint terms were on */
+  int64_t DS, DP, Mpad;  /* written */
+} sgdml_b200_predict_taps;
+/* R != NULL: n_geo device geometries in the model's cell; R == NULL: the training points m_begin .. m_begin + n_geo - 1,
+ * raw or scaled as sgdml_b200_predict_train.  E (may be NULL) and F are device outputs and bit-identical to those of the
+ * untapped call.  n_geo must fit one chunk; models with D <= 256 are rejected (they run the fused kernel).  The call
+ * synchronises the stream. */
+int sgdml_b200_predict_stages(sgdml_b200_model* model, const double* R, int64_t n_geo, int64_t m_begin, int scaled,
+                              sgdml_b200_predict_taps* taps, double* E, double* F, void* stream);
 
 /* Shape of a model: n_atoms, n_train, n_perms (any pointer may be NULL). */
 int sgdml_b200_model_dims(const sgdml_b200_model* model, int64_t* n_atoms, int64_t* n_train, int64_t* n_perms);

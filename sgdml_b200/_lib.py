@@ -134,6 +134,8 @@ SIGNATURES = {
     'sgdml_b200_model_set_alphas_E': (C.c_int, [c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_model_set_contraction_slices': (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     'sgdml_b200_set_predict_chunk': (C.c_int, [i64]),
+    'sgdml_b200_predict_stages': (
+        C.c_int, [c_void_p, c_void_p, i64, i64, C.c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_model_dims': (C.c_int, [c_void_p, c_int64_p, c_int64_p, c_int64_p]),
     'sgdml_b200_pcg_workspace_doubles': (C.c_int64, [i64, i64, i64, i64]),
     'sgdml_b200_pcg': (

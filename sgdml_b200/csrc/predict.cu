@@ -1586,13 +1586,21 @@ int contract_points(const sgdml_b200_model* m, const double* C1, const double* C
   return launch_gemm(g, s);
 }
 
+// n doubles from src to dst (device) on s, unless dst is nullptr
+int tap(double* dst, const double* src, int64_t n, cudaStream_t s) {
+  if (dst != nullptr) SG_CUDA(cudaMemcpyAsync(dst, src, sizeof(double) * n, cudaMemcpyDeviceToDevice, s));
+  return 0;
+}
+
 // Runs the predictor on n_geo queries whose descriptors (xq, gq) are on the device.
 constexpr int64_t GRAPH_MAX_GEO = 16;  // batches up to this size with host buffers replay a captured graph
 // xq == nullptr: the query rows (w.Qg, w.qq) are already in place (k_desc_query_rows)
 // W_dev != nullptr: the finishing kernels' virial variants also write W (n_geo x 9); E and F are unchanged by it
 // w: one of the model's workspace slots, or a ForceEval's (predict.cuh)
+// taps != nullptr (sgdml_b200_predict_stages, large descriptors): each stage is also copied where taps points
 int run_queries(sgdml_b200_model* m, sgdml_b200_model::WS& w, const double* xq, const double* gq, int64_t n_geo,
-                double std, double c, double* E_dev, double* F_dev, cudaStream_t s, double* W_dev = nullptr) {
+                double std, double c, double* E_dev, double* F_dev, cudaStream_t s, double* W_dev = nullptr,
+                const sgdml_b200_predict_taps* taps = nullptr) {
   const int64_t n_rows = n_geo * m->S;
   const int64_t n_rows_pad = (n_rows + m->BQ - 1) / m->BQ * m->BQ;
   int n_splits = 1;
@@ -1607,31 +1615,48 @@ int run_queries(sgdml_b200_model* m, sgdml_b200_model::WS& w, const double* xq, 
     ProfScope ps(KID_PREDICT_MAIN, s);
     const MaternK mk = MaternK::from_sig(m->sig);
     const double* ae = m->use_ae ? m->ae : nullptr;
+    const int64_t nq = n_rows * m->DS, ns = n_rows * m->Mpad, ng = n_rows * m->DP;
+    if (taps != nullptr) {
+      SG_TRY(tap(taps->Qg, w.Qg, nq, s));
+      SG_TRY(tap(taps->qq, w.qq, n_rows, s));
+    }
     // The four contractions on the int8 tensor cores (wgmma) through exact int8 slice products (csrc/ozaki.cu): the
     // slices of the model matrices are kept with the model, those of Q, C1, C2 are cut per batch; everything is
     // stream-ordered (this path runs once per CG iteration inside sgdml_b200_pcg).  Slice count: m->oz_s
-    // (tools/ozaki_study.py predict: forces 8.8e-9 / 6.5e-11 / 5.4e-13 vs FP64 for 4 / 5 / 6 slices).
-    if (m->oz_s >= 2) {
-      const int S = m->oz_s;
+    // (forces against FP64 on an H100: see DESIGN.md, "FP64 through the int8 tensor cores").
+    const int S = m->oz_s;
+    if (S >= 2) {
       SG_TRY(ozaki_split(w.Qg, n_rows, m->DS, m->DS, S, w.ozQ.units, w.ozQ.exps, &w.ozQ, s));
       SG_TRY(ozaki_gemm(w.ozQ, m->ozXc, n_rows, m->Mpad, 1.0, 1, w.S1, m->Mpad, S, s));
       SG_TRY(ozaki_gemm(w.ozQ, m->ozJA, n_rows, m->Mpad, 1.0, 1, w.S2, m->Mpad, S, s));
-      k_transform_rows<<<(unsigned)((n_rows + 7) / 8), 256, 0, s>>>(w.S1, w.S2, m->Mpad, w.qq, m->mm, m->xja, ae, m->M,
-                                                                     m->Mpad, n_rows, mk, w.csum, w.Erow);
-      SG_CUDA(cudaGetLastError());
+    } else {
+      SG_TRY(contract_desc(m, w.Qg, n_rows, w.S1, w.S2, s));
+    }
+    if (taps != nullptr) {
+      SG_TRY(tap(taps->S1, w.S1, ns, s));
+      SG_TRY(tap(taps->S2, w.S2, ns, s));
+    }
+    k_transform_rows<<<(unsigned)((n_rows + 7) / 8), 256, 0, s>>>(w.S1, w.S2, m->Mpad, w.qq, m->mm, m->xja, ae, m->M,
+                                                                   m->Mpad, n_rows, mk, w.csum, w.Erow);
+    SG_CUDA(cudaGetLastError());
+    if (taps != nullptr) {
+      SG_TRY(tap(taps->C1, w.S1, ns, s));
+      SG_TRY(tap(taps->C2, w.S2, ns, s));
+      SG_TRY(tap(taps->csum, w.csum, n_rows, s));
+      SG_TRY(tap(taps->Erow, w.Erow, n_rows, s));
+    }
+    if (S >= 2) {
       SG_TRY(ozaki_split(w.S1, n_rows, m->Mpad, m->Mpad, S, w.ozC1.units, w.ozC1.exps, &w.ozC1, s));
       SG_TRY(ozaki_split(w.S2, n_rows, m->Mpad, m->Mpad, S, w.ozC2.units, w.ozC2.exps, &w.ozC2, s));
       SG_TRY(ozaki_gemm(w.ozC1, m->ozXcT, n_rows, m->DP, 1.0, 1, w.G, m->DP, S, s));
       SG_TRY(ozaki_gemm(w.ozC2, m->ozJAT, n_rows, m->DP, 1.0, 0, w.G, m->DP, S, s));
     } else {
-      SG_TRY(contract_desc(m, w.Qg, n_rows, w.S1, w.S2, s));
-      k_transform_rows<<<(unsigned)((n_rows + 7) / 8), 256, 0, s>>>(w.S1, w.S2, m->Mpad, w.qq, m->mm, m->xja, ae, m->M,
-                                                                     m->Mpad, n_rows, mk, w.csum, w.Erow);
-      SG_CUDA(cudaGetLastError());
       SG_TRY(contract_points(m, w.S1, w.S2, n_rows, w.G, s));
     }
+    if (taps != nullptr) SG_TRY(tap(taps->acc, w.G, ng, s));
     k_combine_rows<<<(unsigned)((n_rows * m->DP + 255) / 256), 256, 0, s>>>(w.Qg, m->DS, w.csum, w.G, m->DP, n_rows);
     SG_CUDA(cudaGetLastError());
+    if (taps != nullptr) SG_TRY(tap(taps->G, w.G, ng, s));
     count_launch(KID_PREDICT_MAIN, 2);
   } else {
     PredictArgs a;
@@ -2378,6 +2403,51 @@ int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* m, int slices, voi
 int sgdml_b200_set_predict_chunk(int64_t max_geos) {
   SG_ARG(max_geos >= 0);
   g_chunk_cap = max_geos;
+  return 0;
+}
+
+int sgdml_b200_predict_stages(sgdml_b200_model* m, const double* R, int64_t n_geo, int64_t m_begin, int scaled,
+                              sgdml_b200_predict_taps* taps, double* E, double* F, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(m != nullptr && taps != nullptr && F != nullptr && n_geo >= 1);
+  if (!m->large) return fail_arg("sgdml_b200_predict_stages: D <= 256 runs the fused kernel, which has no stages");
+  SG_ARG(n_geo <= chunk_geos(m));
+  SG_ARG(is_device_ptr(F) && (E == nullptr || is_device_ptr(E)));
+  if (R != nullptr) {
+    SG_ARG(is_device_ptr(R));
+  } else {
+    SG_ARG(m->R_d_desc != nullptr && m_begin >= 0 && m_begin + n_geo <= m->M);
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  SG_TRY(ensure_ws(m, 0, n_geo));
+  sgdml_b200_model::WS& w = m->ws[0];
+  taps->oz_s = m->oz_s;
+  taps->use_ae = m->use_ae;
+  taps->DS = m->DS;
+  taps->DP = m->DP;
+  taps->Mpad = m->Mpad;
+  const int64_t nm = (int64_t)m->Mpad * m->DS;
+  SG_TRY(tap(taps->Xc, m->Xc, nm, s));
+  SG_TRY(tap(taps->JA, m->JA, nm, s));
+  SG_TRY(tap(taps->XcT, m->XcT, (int64_t)m->DP * m->Mpad, s));
+  SG_TRY(tap(taps->JAT, m->JAT, (int64_t)m->DP * m->Mpad, s));
+  SG_TRY(tap(taps->mm, m->mm, m->Mpad, s));
+  SG_TRY(tap(taps->xja, m->xja, m->Mpad, s));
+  SG_TRY(tap(taps->mu, m->mu, m->DS, s));
+  SG_TRY(tap(taps->ae, m->ae, m->Mpad, s));
+  const double *xq = nullptr, *gq = nullptr;
+  double std = m->std, c = m->c;
+  if (R != nullptr) {
+    SG_TRY(launch_desc_from_R(R, n_geo, m->N, w.xq, w.gq, s, m->lat, nullptr));
+    xq = w.xq;
+    gq = w.gq;
+  } else {
+    xq = m->X + m_begin * m->D;
+    gq = m->R_d_desc + m_begin * m->D * 3;
+    if (!scaled) std = 1.0, c = 0.0;
+  }
+  SG_TRY(run_queries(m, w, xq, gq, n_geo, std, c, E, F, s, nullptr, taps));
+  SG_CUDA(cudaStreamSynchronize(s));
   return 0;
 }
 

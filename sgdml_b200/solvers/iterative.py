@@ -277,7 +277,7 @@ class Iterative(object):
         v_E = np.zeros(n_train) if ecstr else None
         model = self.gdml_train.create_model(task, 'cg', R_desc, R_d_desc, tril_perms_lin, 1.0, v_F, alphas_E=v_E)
         self.gdml_predict = GDMLPredict(model, max_memory=self._max_memory, max_processes=self._max_processes)
-        # K.v on the int8 tensor cores (wgmma) for large descriptors (5 exact int8 slices: forces within 6.5e-11 of the FP64
+        # K.v on the int8 tensor cores (wgmma) for large descriptors (5 exact int8 slices: forces within 1.3e-10 of the FP64
         # contractions, CG tolerance 1e-4; 1.43x the FP64 contractions' throughput at BASELINE config 3 on an H100 at 400 W);
         # SGDML_B200_OZAKI_PREDICT_SLICES (0 = FP64) overrides
         import os

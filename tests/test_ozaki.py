@@ -100,22 +100,28 @@ def test_potrf_with_int8_trailing_updates(monkeypatch, S, tol_llt, tol_l):
     assert rel_err(LS, L0) < tol_l
 
 
-@pytest.mark.parametrize('S,tol', [(4, 1e-6), (5, 1e-8), (7, 1e-11)], ids=['4', '5', '7'])
-def test_large_descriptor_predictor_on_int8_path(monkeypatch, S, tol):
-    """GEMM-composed predictor (D > 256) with its four contractions on the int8 path, 4, 5 and 7
-    slices: forces against the oracle (tools/ozaki_study.py predict: 8.8e-9 / 6.5e-11 for 4 / 5)."""
+@pytest.mark.parametrize('S', [4, 5, 7], ids=['4', '5', '7'])
+def test_large_descriptor_predictor_on_int8_path(monkeypatch, S):
+    """GEMM-composed predictor (D > 256) with its four contractions on the int8 path, 4, 5 and 7 slices (set through
+    SGDML_B200_OZAKI_PREDICT_SLICES at creation): E and F within the composed bound of the FP64 oracle
+    (tests/ozaki_predict_model.py e2e_bound), on the query rows the engine formed."""
     import sgdml_b200
-    from oracle import predict as opredict
+    import ozaki_predict_model as opm
     from sgdml_b200 import synth
+    from test_ozaki_predict_classes import tapped
 
     N, M = 30, 40
     perms = synth.rotor_swap_group(N, 1, 1)
     model = synth.random_model(N, M, perms, 30, seed=2)
     Rq = synth.geometries(N, 9, 1).reshape(9, -1)
-    E_ref, F_ref = opredict.Predictor(model).predict(Rq)
+    E_ref, F_ref, x, gq, scale, k = opm.oracle_case(model, R=Rq)
     monkeypatch.setenv('SGDML_B200_OZAKI_PREDICT_SLICES', str(S))
-    E, F = sgdml_b200.GDMLPredict(model).predict(Rq)
-    assert rel_err(F, F_ref) < tol and rel_err(E, E_ref) < tol
+    p = sgdml_b200.GDMLPredict(model)
+    E, F = p.predict(Rq)
+    t, arr, Et, Ft = tapped(p, model, R=Rq)
+    assert t['oz_s'] == S
+    assert np.array_equal(Et, E) and np.array_equal(Ft, F)
+    opm.check_e2e(E, F, E_ref, F_ref, opm.e2e_bound(arr, t['Qg'], t['qq'], gq, S, scale, k), 'S=%d' % S)
 
 
 @pytest.mark.parametrize('S', [5, 6])

@@ -18,6 +18,7 @@
 // and a run continued over several calls draws exactly the noise of one long run.
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <initializer_list>
 #include <vector>
 
@@ -52,6 +53,34 @@ __device__ __forceinline__ double uniform53(uint32_t hi, uint32_t lo) {
   return ((double)(u >> 11) + 0.5) * 0x1p-53;
 }
 
+// the normals of coordinate pair j of replica rep at step n: Philox4x32-10 under key (k0, k1), then Box-Muller
+__device__ __forceinline__ void normal_pair(double xi[2], uint32_t j, uint32_t rep, uint64_t n, uint32_t k0,
+                                            uint32_t k1) {
+  uint32_t c[4] = {j, rep, (uint32_t)n, (uint32_t)(n >> 32)};
+  philox4x32_10(c, k0, k1);
+  const double ua = uniform53(c[0], c[1]), ub = uniform53(c[2], c[3]);
+  const double rad = sqrt(-2.0 * log(ua));
+  double sn, cs;
+  sincos(2.0 * M_PI * ub, &sn, &cs);
+  xi[0] = rad * cs;
+  xi[1] = rad * sn;
+}
+
+// The fixed-order tree over the CTA (the same result on every run): red[t] = op(red[t], red[t + w]) for
+// w = MD_THREADS / 2, ..., 1, each level after a barrier; returns red[0]
+template <class T, class Op>
+__device__ __forceinline__ T block_tree(T x, T* red, Op op) {
+  red[threadIdx.x] = x;
+  __syncthreads();
+  for (int w = MD_THREADS / 2; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) red[threadIdx.x] = op(red[threadIdx.x], red[threadIdx.x + w]);
+    __syncthreads();
+  }
+  return red[0];
+}
+
+__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
+
 __global__ void __launch_bounds__(MD_THREADS) k_md_step(const MdParams* __restrict__ P, const double* __restrict__ s,
                                                        const double* __restrict__ sigma, double* __restrict__ R,
                                                        double* __restrict__ V, const double* __restrict__ F,
@@ -74,16 +103,7 @@ __global__ void __launch_bounds__(MD_THREADS) k_md_step(const MdParams* __restri
   const int n_pairs = (dimi + 1) / 2;
   for (int j = threadIdx.x; j < n_pairs; j += MD_THREADS) {
     double xi[2] = {0.0, 0.0};
-    if (advance && p.use_O) {
-      uint32_t c[4] = {(uint32_t)j, (uint32_t)rep, (uint32_t)n, (uint32_t)(n >> 32)};
-      philox4x32_10(c, p.key[0], p.key[1]);
-      const double ua = uniform53(c[0], c[1]), ub = uniform53(c[2], c[3]);
-      const double rad = sqrt(-2.0 * log(ua));
-      double sn, cs;
-      sincos(2.0 * M_PI * ub, &sn, &cs);
-      xi[0] = rad * cs;
-      xi[1] = rad * sn;
-    }
+    if (advance && p.use_O) normal_pair(xi, (uint32_t)j, (uint32_t)rep, n, p.key[0], p.key[1]);
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
       const int i = 2 * j + q;
@@ -108,15 +128,10 @@ __global__ void __launch_bounds__(MD_THREADS) k_md_step(const MdParams* __restri
       v[i] = vi;
     }
   }
-  if (sample) {  // fixed-order tree: the same sum on every run
-    red[threadIdx.x] = ke;
-    __syncthreads();
-    for (int w = MD_THREADS / 2; w > 0; w >>= 1) {
-      if ((int)threadIdx.x < w) red[threadIdx.x] = __dadd_rn(red[threadIdx.x], red[threadIdx.x + w]);
-      __syncthreads();
-    }
+  if (sample) {
+    ke = block_tree(ke, red, dadd);
     if (threadIdx.x == 0) {
-      if (p.Ek_f) p.Ek_f[frame * n_rep + rep] = 0.5 * red[0];
+      if (p.Ek_f) p.Ek_f[frame * n_rep + rep] = 0.5 * ke;
       if (p.Ep_f) p.Ep_f[frame * n_rep + rep] = E[rep];
     }
   }
@@ -207,15 +222,9 @@ __global__ void k_remd_identity(int* walker, int64_t n_rep) {
   if (r < n_rep) walker[r] = (int)r;
 }
 
-// k_md_step's fixed-order tree over the CTA; every thread gets the sum
+// k_md_step's sum over the CTA; every thread gets it
 __device__ __forceinline__ double block_sum(double x, double* red) {
-  red[threadIdx.x] = x;
-  __syncthreads();
-  for (int w = MD_THREADS / 2; w > 0; w >>= 1) {
-    if ((int)threadIdx.x < w) red[threadIdx.x] = __dadd_rn(red[threadIdx.x], red[threadIdx.x + w]);
-    __syncthreads();
-  }
-  const double r = red[0];
+  const double r = block_tree(x, red, dadd);
   __syncthreads();  // red is free again
   return r;
 }
@@ -362,17 +371,7 @@ __global__ void __launch_bounds__(MD_THREADS) k_pimd_step(const PimdParams* __re
       const int k = t / tp, c = 2 * (t % tp);
       if (c >= w) continue;
       double xi[2] = {0.0, 0.0};
-      if (p.use_O) {
-        const int64_t rep = rep0 + k;
-        uint32_t ct[4] = {(uint32_t)((i0 + c) / 2), (uint32_t)rep, (uint32_t)n, (uint32_t)(n >> 32)};
-        philox4x32_10(ct, p.key[0], p.key[1]);
-        const double ua = uniform53(ct[0], ct[1]), ub = uniform53(ct[2], ct[3]);
-        const double rad = sqrt(-2.0 * log(ua));
-        double sn, cs;
-        sincos(2.0 * M_PI * ub, &sn, &cs);
-        xi[0] = rad * cs;
-        xi[1] = rad * sn;
-      }
+      if (p.use_O) normal_pair(xi, (uint32_t)((i0 + c) / 2), (uint32_t)(rep0 + k), n, p.key[0], p.key[1]);
       const double cs = m_cos[k], so = m_sow[k], ms = m_msin[k], c1 = m_c1[k];
 #pragma unroll
       for (int qq = 0; qq < 2; ++qq) {
@@ -423,13 +422,7 @@ constexpr int FIRE_NMIN = 5;
 __device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
 
 __device__ __forceinline__ double block_max(double x, double* red) {
-  red[threadIdx.x] = x;
-  __syncthreads();
-  for (int w = MD_THREADS / 2; w > 0; w >>= 1) {
-    if ((int)threadIdx.x < w) red[threadIdx.x] = nan_max(red[threadIdx.x], red[threadIdx.x + w]);
-    __syncthreads();
-  }
-  const double r = red[0];
+  const double r = block_tree(x, red, nan_max);
   __syncthreads();
   return r;
 }
@@ -706,13 +699,8 @@ __global__ void __launch_bounds__(MD_THREADS) k_relax_count(const RelaxState* __
   __shared__ int red[MD_THREADS];
   int c = 0;
   for (int64_t r = threadIdx.x; r < n_rep; r += MD_THREADS) c += st[r].conv == 0;
-  red[threadIdx.x] = c;
-  __syncthreads();
-  for (int w = MD_THREADS / 2; w > 0; w >>= 1) {
-    if ((int)threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *n_active = red[0];
+  c = block_tree(c, red, [](int a, int b) { return a + b; });
+  if (threadIdx.x == 0) *n_active = c;
 }
 
 __global__ void k_relax_report(const RelaxState* __restrict__ st, int64_t n_rep, int64_t* n_steps, int* conv,
@@ -736,6 +724,28 @@ __global__ void k_relax_report(const RelaxState* __restrict__ st, int64_t n_rep,
 // advanced by the integrator, so the graph bakes in no run.
 using namespace sgdml;
 
+namespace {
+
+// The parameters of every integrator, at the head of the handle's upload block.  A call fills only its own.
+struct StepParams {
+  MdParams md;
+  PimdParams pimd;
+  RelaxParams relax;
+  NebParams neb;
+  RemdParams remd;
+};
+constexpr size_t STEP_PARAMS_BYTES = (sizeof(StepParams) + 255) & ~(size_t)255;  // where the tables start
+
+// What a captured step bakes in besides the force evaluation: the integrator (MdKind), the replicas per group (the
+// grids of the NEB and exchange kernels) and the upload block (the tab and sigma kernel arguments point into it).
+struct StepKey {
+  int kind, group;
+  const char* blk;
+  bool operator==(const StepKey& o) const { return kind == o.kind && group == o.group && blk == o.blk; }
+};
+
+}  // namespace
+
 struct sgdml_b200_md {
   int64_t n_rep = 0;
   int dimi = 0;
@@ -746,25 +756,24 @@ struct sgdml_b200_md {
   uint64_t* step = nullptr;             // (n_rep) step counters, all equal
   uint64_t step_host = 0;               // their value once the queued runs have finished
   bool has_state = false;
-  double *s = nullptr, *sigma = nullptr;  // (3N) inverse mass, (sigma_rows, 3N) noise scale per mode or temperature
-  int sigma_rows = 0;                     // rows sigma and hSigma hold: nb at creation, more for a replica exchange
-  std::vector<double> s_host;             // s on the host
-  MdParams* dP = nullptr;
-  MdParams* hP = nullptr;     // pinned staging of dP and sigma, reused once the previous run's upload is done
-  double* hSigma = nullptr;
-  PimdParams* dQ = nullptr;  // the ring-polymer run's parameter block
-  PimdParams* hQ = nullptr;
-  double *tab = nullptr, *hTab = nullptr;  // C (nb x nb) and the four mode tables (nb each)
+  double* s = nullptr;                  // (3N) inverse mass
+  std::vector<double> s_host;           // s on the host
+  // The upload block on the device (blk) and its pinned mirror (hblk): StepParams, then the tables -- the PIMD table
+  // C (nb x nb) and the four mode tables (nb each), sigma (rows, 3N), the noise scale per mode or temperature, and the
+  // ladder beta, lam_up, lam_dn (rows each).  A call fills its part of the mirror once the previous call's upload has
+  // read it (uploaded), then uploads the prefix it uses in one copy.
+  char *blk = nullptr, *hblk = nullptr;
+  int rows = 0;  // max(nb, the largest n_temps so far)
   cudaEvent_t uploaded = nullptr;
   cudaStream_t gs = nullptr;  // capture stream
   cudaEvent_t ge = nullptr;
   cudaGraphExec_t exec = nullptr;
-  int graph_kind = -1;        // the MdKind of the captured step
+  StepKey graph_key = {};     // the key of the captured step
   int n_kernels = 0;
+  // replicas per group of the current call: images per band (NEB), temperatures per ladder (replica exchange), else 1
+  int group = 1;
   // geometry optimisation (sgdml_b200_relax_*), allocated by the first relaxation
   RelaxState* rst = nullptr;  // (n_rep) per-replica optimiser state
-  RelaxParams* dR = nullptr;
-  RelaxParams* hR = nullptr;  // pinned staging of dR
   int* hActive = nullptr;     // mapped pinned: unconverged replicas, written by k_relax_count
   int* dActive = nullptr;     // its device address
   cudaEvent_t counted = nullptr;
@@ -772,19 +781,17 @@ struct sgdml_b200_md {
   double *r_prev = nullptr, *g_prev = nullptr;              // (n_rep, 3N)
   int m_cap = 0;
   // nudged elastic band (sgdml_b200_neb_fire), allocated by the first NEB call
-  NebParams* dN = nullptr;
-  NebParams* hN = nullptr;    // pinned staging of dN
   double* Fn = nullptr;       // (n_rep, 3N) NEB forces of the interior images
   int* climb_idx = nullptr;   // (n_rep) the highest interior image of each band (the first n_rep / P entries)
   // replica exchange (sgdml_b200_remd_run), allocated by the first replica-exchange call
-  RemdParams* dX = nullptr;
-  RemdParams* hX = nullptr;   // pinned staging of dX
-  double *xtab = nullptr, *hXtab = nullptr;  // beta, lam_up, lam_dn (n_rep each) and their pinned staging
   int* walker = nullptr;      // (n_rep) walker label per slot
   int64_t* xcount = nullptr;  // (2, n_rep) accepted and attempted swaps of the current run
-  // replicas per group of the current call: images per band (NEB), temperatures per ladder (replica exchange)
-  int group = 0;
-  int graph_group = 0;        // ... and of the captured step
+
+  // the block's parts in blk or hblk
+  StepParams* params(char* b) const { return reinterpret_cast<StepParams*>(b); }
+  double* tab(char* b) const { return reinterpret_cast<double*>(b + STEP_PARAMS_BYTES); }
+  double* sigma(char* b) const { return tab(b) + nb * nb + 4 * nb; }
+  double* ladder(char* b) const { return sigma(b) + (size_t)rows * dimi; }
 };
 
 namespace {
@@ -797,30 +804,43 @@ void md_free(sgdml_b200_md* md) {
   if (md->uploaded) cudaEventDestroy(md->uploaded);
   if (md->counted) cudaEventDestroy(md->counted);
   force_eval_destroy(md->fe);
-  for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s, md->sigma}) cached_free(p);
-  cached_free(md->step);
-  cached_free(md->dP);
-  cached_free(md->dQ);
-  cached_free(md->tab);
+  for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s}) cached_free(p);
   for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev, md->Fn}) cached_free(p);
+  cached_free(md->step);
+  cached_free(md->blk);
   cached_free(md->rst);
-  cached_free(md->dR);
-  cached_free(md->dN);
   cached_free(md->climb_idx);
-  cached_free(md->dX);
-  cached_free(md->xtab);
   cached_free(md->walker);
   cached_free(md->xcount);
-  cudaFreeHost(md->hX);
-  cudaFreeHost(md->hXtab);
-  cudaFreeHost(md->hR);
-  cudaFreeHost(md->hN);
+  cudaFreeHost(md->hblk);
   cudaFreeHost(md->hActive);
-  cudaFreeHost(md->hP);
-  cudaFreeHost(md->hQ);
-  cudaFreeHost(md->hTab);
-  cudaFreeHost(md->hSigma);
   delete md;
+}
+
+// The block holds `rows` sigma and ladder rows: nb at creation, more when a replica exchange needs them.  A grown
+// block moves, which changes the step key.  The mirror starts as zeros.
+int reserve(sgdml_b200_md* md, int rows) {
+  if (rows <= md->rows) return 0;
+  if (md->blk != nullptr) SG_CUDA(cudaDeviceSynchronize());  // the old block goes back: nothing may still use it
+  cached_free(md->blk);
+  cudaFreeHost(md->hblk);
+  md->blk = md->hblk = nullptr;
+  md->rows = 0;
+  const size_t bytes =
+      STEP_PARAMS_BYTES + sizeof(double) * ((size_t)md->nb * md->nb + 4 * md->nb + (size_t)rows * (md->dimi + 3));
+  SG_CUDA(cached_malloc(&md->blk, bytes));
+  SG_CUDA(cudaMallocHost(&md->hblk, bytes));
+  std::memset(md->hblk, 0, bytes);
+  md->rows = rows;
+  return 0;
+}
+
+// uploads the block's first bytes up to `end` (in hblk) on s, and marks when the mirror is free again
+int upload(sgdml_b200_md* md, const void* end, cudaStream_t s) {
+  const size_t bytes = (size_t)(static_cast<const char*>(end) - md->hblk);
+  SG_CUDA(cudaMemcpyAsync(md->blk, md->hblk, bytes, cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaEventRecord(md->uploaded, s));
+  return 0;
 }
 
 // The outputs of one call, each a (caller's pointer, bytes) pair; a null pointer or 0 bytes is no output.  The kernels
@@ -862,7 +882,15 @@ class Outputs {
   T* dev(int i) const {
     return static_cast<T*>(dev_[i]);
   }
-  size_t bytes(int i) const { return out_[i].bytes; }
+  // queues the copies of device arrays src[0], src[1], ... into outputs first, first + 1, ... (those that are outputs)
+  int copy_from(int first, std::initializer_list<const void*> src) {
+    int i = first;
+    for (const void* p : src) {
+      if (dev_[i] != nullptr) SG_CUDA(cudaMemcpyAsync(dev_[i], p, out_[i].bytes, cudaMemcpyDeviceToDevice, s_));
+      ++i;
+    }
+    return 0;
+  }
   // queues the copies to the host arrays and, if there are any, waits for them
   int finish() {
     for (int i = 0; i < n_; ++i)
@@ -875,7 +903,7 @@ class Outputs {
   }
 
  private:
-  static constexpr int MAX_OUTS = 8;
+  static constexpr int MAX_OUTS = 10;
   cudaStream_t s_;
   int n_ = 0;
   Out out_[MAX_OUTS];
@@ -893,39 +921,41 @@ enum MdKind { MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, 
 // state) or only tests convergence (relaxation, NEB: after the force projection).  L-BFGS keeps its direction in V,
 // which relax_impl zeroes after.
 int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
+  StepParams* p = md->params(md->blk);
   switch (kind) {
     case MD_RING_POLYMER:
-      k_pimd_step<<<(unsigned)(md->n_rep / md->nb), MD_THREADS, 0, s>>>(md->dQ, md->tab, md->s, md->sigma, md->R, md->V,
-                                                                      md->F, md->E, md->step, md->dimi, md->nb,
-                                                                      advance);
+      k_pimd_step<<<(unsigned)(md->n_rep / md->nb), MD_THREADS, 0, s>>>(&p->pimd, md->tab(md->blk), md->s,
+                                                                      md->sigma(md->blk), md->R, md->V, md->F, md->E,
+                                                                      md->step, md->dimi, md->nb, advance);
       break;
     case MD_FIRE:
-      k_fire_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(md->dR, md->rst, md->R, md->V, md->F, md->dimi, advance);
+      k_fire_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&p->relax, md->rst, md->R, md->V, md->F, md->dimi,
+                                                             advance);
       break;
     case MD_LBFGS:
-      k_lbfgs_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(md->dR, md->rst, md->R, md->V, md->F, md->E, md->dimi,
-                                                              advance);
+      k_lbfgs_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&p->relax, md->rst, md->R, md->V, md->F, md->E,
+                                                              md->dimi, advance);
       break;
     case MD_NEB_FIRE: {
       const int64_t n_bands = md->n_rep / md->group;
-      k_neb_force<<<(unsigned)(n_bands * (md->group - 2)), MD_THREADS, 0, s>>>(md->dN, md->R, md->F, md->E, md->Fn,
+      k_neb_force<<<(unsigned)(n_bands * (md->group - 2)), MD_THREADS, 0, s>>>(&p->neb, md->R, md->F, md->E, md->Fn,
                                                                               md->climb_idx, md->dimi);
       SG_CUDA(cudaGetLastError());
       count_launch(KID_MISC);
-      k_neb_fire_step<<<(unsigned)n_bands, MD_THREADS, 0, s>>>(md->dN, md->rst, md->R, md->V, md->Fn, md->dimi,
+      k_neb_fire_step<<<(unsigned)n_bands, MD_THREADS, 0, s>>>(&p->neb, md->rst, md->R, md->V, md->Fn, md->dimi,
                                                                advance);
       break;
     }
     case MD_REMD:
-      k_remd_exchange<<<(unsigned)(md->n_rep / md->group), MD_THREADS, 0, s>>>(md->dX, md->dP, md->s, md->R, md->V,
+      k_remd_exchange<<<(unsigned)(md->n_rep / md->group), MD_THREADS, 0, s>>>(&p->remd, &p->md, md->s, md->R, md->V,
                                                                               md->F, md->E, md->walker, md->step,
                                                                               md->dimi);
       SG_CUDA(cudaGetLastError());
       count_launch(KID_MISC);
       [[fallthrough]];
     default:
-      k_md_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(md->dP, md->s, md->sigma, md->R, md->V, md->F, md->E,
-                                                           md->step, md->dimi, advance);
+      k_md_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&p->md, md->s, md->sigma(md->blk), md->R, md->V, md->F,
+                                                           md->E, md->step, md->dimi, advance);
   }
   SG_CUDA(cudaGetLastError());
   count_launch(KID_MISC);
@@ -937,13 +967,10 @@ int md_step(sgdml_b200_md* md, int kind, cudaStream_t s) {
   return force_eval_run(md->fe, md->R, md->F, md->E, s);
 }
 
-// the step graph, captured again whenever the force evaluation it bakes in is stale, the integrator (MdKind) changes
-// or, for NEB and replica exchange, the replicas per group (their grids) change
+// the step graph, captured again whenever the force evaluation it bakes in is stale or its key changes
 int md_graph(sgdml_b200_md* md, int kind, cudaStream_t s) {
-  const bool grouped = kind == MD_NEB_FIRE || kind == MD_REMD;
-  if (md->exec != nullptr && md->graph_kind == kind && (!grouped || md->graph_group == md->group) &&
-      !force_eval_stale(md->fe))
-    return 0;
+  const StepKey key = {kind, md->group, md->blk};
+  if (md->exec != nullptr && md->graph_key == key && !force_eval_stale(md->fe)) return 0;
   if (md->exec != nullptr) {
     cudaGraphExecDestroy(md->exec);
     md->exec = nullptr;
@@ -960,8 +987,7 @@ int md_graph(sgdml_b200_md* md, int kind, cudaStream_t s) {
   SG_CUDA(cudaStreamSynchronize(md->gs));
   SG_TRY(capture_graph(md->gs, [&] { return md_step(md, kind, md->gs); }, &md->exec, &md->n_kernels));
   force_eval_mark(md->fe);
-  md->graph_kind = kind;
-  md->graph_group = md->group;
+  md->graph_key = key;
   return 0;
 }
 
@@ -979,7 +1005,13 @@ int md_replay(sgdml_b200_md* md, int kind, int64_t n_steps, cudaStream_t s) {
   return 0;
 }
 
-// ------------------------------------------------------------------ MD and PIMD runs
+// ------------------------------------------------------------------ MD, replica-exchange and PIMD runs
+// What a run writes, by Outputs slot: the frames, a ring polymer's estimator frames, then a replica exchange's walker
+// frames, final walker labels and counts.
+enum RunOut {
+  OUT_R, OUT_V, OUT_EPOT, OUT_EKIN, OUT_KPRIM, OUT_KCV, OUT_WALKER_F, OUT_WALKERS, OUT_NACC, OUT_NATT, N_RUN_OUTS
+};
+
 // The run's constants, once on the host in double precision.  First the fields MdParams and PimdParams share.
 template <class P>
 void run_params(P& p, const sgdml_b200_md* md, double dt, uint64_t seed, int64_t n_frames, int64_t stride,
@@ -989,64 +1021,38 @@ void run_params(P& p, const sgdml_b200_md* md, double dt, uint64_t seed, int64_t
   p.key[1] = (uint32_t)(seed >> 32);
   p.stride = n_frames > 0 ? (int)stride : 0;
   p.run_start = md->step_host;
-  p.R_f = out.dev(0);
-  p.V_f = out.dev(1);
-  p.Ep_f = out.dev(2);
-  p.Ek_f = out.dev(3);
+  p.R_f = out.dev(OUT_R);
+  p.V_f = out.dev(OUT_V);
+  p.Ep_f = out.dev(OUT_EPOT);
+  p.Ek_f = out.dev(OUT_EKIN);
 }
 
-// MD: c1 and the (n_temps, 3N) sigma table, one row per temperature kT[k] (n_temps = 1 for sgdml_b200_md_run)
-int md_params(sgdml_b200_md* md, double dt, double gamma, const double* kT, int n_temps, cudaStream_t s) {
-  MdParams& p = *md->hP;
+// MD: c1 and the (n_temps, 3N) sigma table, one row per temperature kT[k] (n_temps = 1 for sgdml_b200_md_run); returns
+// the end of what it filled
+const double* md_params(sgdml_b200_md* md, double dt, double gamma, const double* kT, int n_temps) {
+  MdParams& p = md->params(md->hblk)->md;
+  double* sigma = md->sigma(md->hblk);
   const int dimi = md->dimi;
   p.c1 = std::exp(-gamma * dt);
   p.use_O = gamma > 0.0 ? 1 : 0;
   p.n_temps = n_temps;
   for (int k = 0; k < n_temps; ++k)
     for (int i = 0; i < dimi; ++i)
-      md->hSigma[(size_t)k * dimi + i] = std::sqrt((1.0 - p.c1 * p.c1) * kT[k] * md->s_host[(size_t)i]);
-  SG_CUDA(cudaMemcpyAsync(md->dP, md->hP, sizeof(MdParams), cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * n_temps * dimi, cudaMemcpyHostToDevice, s));
-  return 0;
+      sigma[(size_t)k * dimi + i] = std::sqrt((1.0 - p.c1 * p.c1) * kT[k] * md->s_host[(size_t)i]);
+  return sigma + (size_t)n_temps * dimi;
 }
 
-// The sigma table and its staging grow to `rows` rows (one per temperature of a replica exchange).  The captured step
-// reads the old table, so it is captured again.
-int sigma_reserve(sgdml_b200_md* md, int rows) {
-  if (rows <= md->sigma_rows) return 0;
-  SG_CUDA(cudaDeviceSynchronize());  // the old table and its staging go back: nothing may still use them
-  if (md->exec != nullptr) {
-    cudaGraphExecDestroy(md->exec);
-    md->exec = nullptr;
-  }
-  cached_free(md->sigma);
-  cudaFreeHost(md->hSigma);
-  md->sigma = nullptr;
-  md->hSigma = nullptr;
-  md->sigma_rows = 0;
-  SG_CUDA(cached_malloc(&md->sigma, sizeof(double) * rows * md->dimi));
-  SG_CUDA(cudaMallocHost(&md->hSigma, sizeof(double) * rows * md->dimi));
-  md->sigma_rows = rows;
-  return 0;
-}
-
-// What a replica-exchange run (sgdml_b200_remd_run) adds to an MD run: its ladder (kT on the host, checked), its
-// schedule and its outputs beyond the frames.
+// What a replica-exchange run (sgdml_b200_remd_run) adds to an MD run: its ladder (kT on the host, checked) and its
+// schedule.
 struct RemdRun {
   int n_temps;
   const double* kT;
   int64_t every;
-  int *W_f, *walkers;
-  int64_t *n_acc, *n_att;
 };
 
 // the replica-exchange state, made at the first replica-exchange call, which sets the walker labels to the identity
 int remd_alloc(sgdml_b200_md* md, cudaStream_t s) {
   const size_t n = (size_t)md->n_rep;
-  if (md->dX == nullptr) SG_CUDA(cached_malloc(&md->dX, sizeof(RemdParams)));
-  if (md->hX == nullptr) SG_CUDA(cudaMallocHost(&md->hX, sizeof(RemdParams)));
-  if (md->xtab == nullptr) SG_CUDA(cached_malloc(&md->xtab, 3 * sizeof(double) * n));
-  if (md->hXtab == nullptr) SG_CUDA(cudaMallocHost(&md->hXtab, 3 * sizeof(double) * n));
   if (md->xcount == nullptr) SG_CUDA(cached_malloc(&md->xcount, 2 * sizeof(int64_t) * n));
   if (md->walker == nullptr) {
     SG_CUDA(cached_malloc(&md->walker, sizeof(int) * n));
@@ -1057,42 +1063,41 @@ int remd_alloc(sgdml_b200_md* md, cudaStream_t s) {
   return 0;
 }
 
-// the exchange's parameters into the pinned staging and their upload on s (after run_params and md_params), and the
-// run's counts zeroed.  beta and lam are computed here, on the host in double precision.
-int remd_params(sgdml_b200_md* md, const RemdRun& x, const Outputs& out, cudaStream_t s) {
+// the exchange's parameters and ladder (after run_params and md_params); beta and lam are computed here, on the host
+// in double precision.  Returns the end of what it filled.
+const double* remd_params(sgdml_b200_md* md, const RemdRun& x, const Outputs& out) {
   const int nt = x.n_temps;
-  const MdParams& p = *md->hP;
-  RemdParams& q = *md->hX;
+  StepParams& hp = *md->params(md->hblk);
+  const MdParams& p = hp.md;
+  RemdParams& q = hp.remd;
   q.key[0] = p.key[0];
   q.key[1] = p.key[1];
   q.run_start = p.run_start;
   q.stride = p.stride;
   q.every = x.every;
   q.n_temps = nt;
-  double *beta = md->hXtab, *up = beta + nt, *dn = up + nt;
+  double *beta = md->ladder(md->hblk), *up = beta + md->rows, *dn = up + md->rows;
   for (int k = 0; k < nt; ++k) beta[k] = 1.0 / x.kT[k];
   for (int k = 0; k + 1 < nt; ++k) {
     up[k] = std::sqrt(x.kT[k + 1] / x.kT[k]);
     dn[k] = std::sqrt(x.kT[k] / x.kT[k + 1]);
   }
-  q.beta = md->xtab;
-  q.lam_up = md->xtab + nt;
-  q.lam_dn = md->xtab + 2 * nt;
+  q.beta = md->ladder(md->blk);
+  q.lam_up = q.beta + md->rows;
+  q.lam_dn = q.lam_up + md->rows;
   q.n_acc = md->xcount;
   q.n_att = md->xcount + md->n_rep;
-  q.W_f = out.dev<int>(4);
-  md->group = nt;
-  SG_CUDA(cudaMemcpyAsync(md->dX, md->hX, sizeof(RemdParams), cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaMemcpyAsync(md->xtab, md->hXtab, 3 * sizeof(double) * nt, cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaMemsetAsync(md->xcount, 0, 2 * sizeof(int64_t) * (size_t)md->n_rep, s));
-  return 0;
+  q.W_f = out.dev<int>(OUT_WALKER_F);
+  return dn + (nt - 1);
 }
 
-// PIMD: the estimator constants, C, the mode tables and the (P, 3N) sigma table (tests/pimd_oracle.py restates them)
-int pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, double kT, double hbar, double gamma, double lambda,
-                cudaStream_t s) {
+// PIMD: the estimator constants, C, the mode tables and the (P, 3N) sigma table (tests/pimd_oracle.py restates them);
+// returns the end of what it filled
+const double* pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, double kT, double hbar, double gamma,
+                          double lambda) {
   const int nb = md->nb, dimi = md->dimi;
-  PimdParams& p = *md->hQ;
+  PimdParams& p = md->params(md->hblk)->pimd;
+  double* sigma = md->sigma(md->hblk);
   const double h = 0.5 * dt;
   const double kTP = nb * kT;
   const double wP = kTP / hbar;
@@ -1101,9 +1106,9 @@ int pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, double kT, dou
   p.kspring = 0.5 * wP * wP / nb;
   p.kcv0 = 0.5 * dimi * kT;
   p.kvir = 0.5 / nb;
-  p.Kp_f = out.dev(4);
-  p.Kcv_f = out.dev(5);
-  double* C = md->hTab;
+  p.Kp_f = out.dev(OUT_KPRIM);
+  p.Kcv_f = out.dev(OUT_KCV);
+  double* C = md->tab(md->hblk);
   double *m_cos = C + nb * nb, *m_sow = m_cos + nb, *m_msin = m_sow + nb, *m_c1 = m_msin + nb;
   for (int j = 0; j < nb; ++j)
     for (int k = 0; k < nb; ++k) {
@@ -1132,81 +1137,64 @@ int pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, double kT, dou
     }
     m_c1[k] = std::exp(-g * dt);
     for (int i = 0; i < dimi; ++i)
-      md->hSigma[(size_t)k * dimi + i] = std::sqrt((1.0 - m_c1[k] * m_c1[k]) * kTP * md->s_host[(size_t)i]);
+      sigma[(size_t)k * dimi + i] = std::sqrt((1.0 - m_c1[k] * m_c1[k]) * kTP * md->s_host[(size_t)i]);
   }
-  SG_CUDA(cudaMemcpyAsync(md->dQ, md->hQ, sizeof(PimdParams), cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaMemcpyAsync(md->tab, md->hTab, sizeof(double) * (nb * nb + 4 * nb), cudaMemcpyHostToDevice, s));
-  SG_CUDA(cudaMemcpyAsync(md->sigma, md->hSigma, sizeof(double) * nb * dimi, cudaMemcpyHostToDevice, s));
+  return sigma + (size_t)nb * dimi;
+}
+
+// the checks every run shares; a rejected call queues nothing
+int run_check(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double gamma, int64_t stride,
+              const char* no_state) {
+  SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
+  SG_ARG(std::isfinite(dt) && dt > 0.0);
+  SG_ARG(std::isfinite(kT) && kT >= 0.0);
+  if (md->nb == 1 && kT > 0.0 && gamma == 0.0)
+    return fail_arg("kT > 0 needs a friction gamma > 0 (a thermostat without coupling)");
+  if (stride > 0 && n_steps % stride != 0) return fail_arg("n_steps must be a multiple of stride");
+  if (!md->has_state) return fail_arg(no_state);
   return 0;
 }
 
 // sgdml_b200_md_run (MD_CLASSICAL), sgdml_b200_pimd_run (MD_RING_POLYMER; hbar and lambda are only its own) and
-// sgdml_b200_remd_run (MD_REMD, with x: its ladder, checked by the caller, and kT = its first temperature).
-// frames: R, V, E_pot, E_kin, then the ring polymer's K_prim and K_cv.  n_steps steps, then the completing launch.
+// sgdml_b200_remd_run (MD_REMD, with x: its ladder, and kT = its first temperature), after their checks.  n_steps
+// steps, then the completing launch.
 int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, double hbar, double gamma, double lambda,
-           uint64_t seed, int64_t stride, double* const frames[6], const RemdRun* x, cudaStream_t s) {
-  const bool ring = kind == MD_RING_POLYMER;
-  SG_TRY(require_device());
-  SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
-  if (!ring && md->nb > 1)
-    return fail_arg("sgdml_b200_md_run: a ring-polymer handle (n_beads > 1) runs with sgdml_b200_pimd_run");
-  SG_ARG(std::isfinite(dt) && dt > 0.0);
-  if (!ring) SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
-  SG_ARG(std::isfinite(kT) && kT >= 0.0);
-  if (ring) {
-    SG_ARG(std::isfinite(hbar) && hbar > 0.0);
-    SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
-    SG_ARG(std::isfinite(lambda) && lambda >= 0.0);
-    if (md->nb > 1 && kT == 0.0) return fail_arg("a ring polymer (n_beads > 1) needs kT > 0");
-  }
-  if (md->nb == 1 && kT > 0.0 && gamma == 0.0)
-    return fail_arg("kT > 0 needs a friction gamma > 0 (a thermostat without coupling)");
-  if (stride > 0 && n_steps % stride != 0) return fail_arg("n_steps must be a multiple of stride");
-  if (!md->has_state)
-    return fail_arg(ring        ? "sgdml_b200_pimd_run: no state yet (call sgdml_b200_md_set_state)"
-                    : x != nullptr ? "sgdml_b200_remd_run: no state yet (call sgdml_b200_md_set_state)"
-                                   : "sgdml_b200_md_run: no state yet (call sgdml_b200_md_set_state)");
+           uint64_t seed, int64_t stride, void* const outs[N_RUN_OUTS], const RemdRun* x, cudaStream_t s) {
   if (n_steps == 0 && x == nullptr) return 0;  // (a replica exchange still reports its labels and zero counts)
-
-  const int64_t n_frames = stride > 0 ? n_steps / stride : 0;
-  const size_t fr = sizeof(double) * (size_t)(n_frames * md->n_rep);
-  const size_t fp = sizeof(double) * (size_t)(n_frames * (md->n_rep / md->nb));
+  md->group = x != nullptr ? x->n_temps : 1;
+  const int64_t n_rep = md->n_rep, n_frames = stride > 0 ? n_steps / stride : 0;
+  const size_t fr = sizeof(double) * (size_t)(n_frames * n_rep);
+  const size_t fp = sizeof(double) * (size_t)(n_frames * (n_rep / md->nb));
+  const size_t nc = sizeof(int64_t) * (size_t)(n_rep / md->group * (md->group - 1));  // (n_ladders, n_temps - 1)
   Outputs out(s);
-  if (x == nullptr) {
-    SG_TRY(out.init({{frames[0], fr * md->dimi}, {frames[1], fr * md->dimi}, {frames[2], fr}, {frames[3], fr},
-                     {frames[4], fp}, {frames[5], fp}}));
-  } else {  // frames, walker frames, final walker labels, then the counts (n_ladders, n_temps - 1)
-    const size_t wf = sizeof(int) * (size_t)(n_frames * md->n_rep);
-    const size_t nc = sizeof(int64_t) * (size_t)(md->n_rep / x->n_temps * (x->n_temps - 1));
-    SG_TRY(out.init({{frames[0], fr * md->dimi}, {frames[1], fr * md->dimi}, {frames[2], fr}, {frames[3], fr},
-                     {x->W_f, wf}, {x->walkers, sizeof(int) * (size_t)md->n_rep}, {x->n_acc, nc}, {x->n_att, nc}}));
-  }
+  SG_TRY(out.init({{outs[OUT_R], fr * md->dimi}, {outs[OUT_V], fr * md->dimi}, {outs[OUT_EPOT], fr},
+                   {outs[OUT_EKIN], fr}, {outs[OUT_KPRIM], fp}, {outs[OUT_KCV], fp},
+                   {outs[OUT_WALKER_F], sizeof(int) * (size_t)(n_frames * n_rep)},
+                   {outs[OUT_WALKERS], sizeof(int) * (size_t)n_rep}, {outs[OUT_NACC], nc}, {outs[OUT_NATT], nc}}));
   SG_TRY(force_eval_prepare(md->fe));
   if (x != nullptr) {
-    SG_TRY(sigma_reserve(md, x->n_temps));
+    SG_TRY(reserve(md, x->n_temps));
     SG_TRY(remd_alloc(md, s));
+    SG_CUDA(cudaMemsetAsync(md->xcount, 0, 2 * sizeof(int64_t) * (size_t)n_rep, s));  // the run's counts
   }
-  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous run has read the staging
-  if (ring) {
-    run_params(*md->hQ, md, dt, seed, n_frames, stride, out);
-    SG_TRY(pimd_params(md, out, dt, kT, hbar, gamma, lambda, s));
+  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the mirror
+  StepParams& p = *md->params(md->hblk);
+  const double* end;
+  if (kind == MD_RING_POLYMER) {
+    run_params(p.pimd, md, dt, seed, n_frames, stride, out);
+    end = pimd_params(md, out, dt, kT, hbar, gamma, lambda);
   } else {
-    run_params(*md->hP, md, dt, seed, n_frames, stride, out);
-    SG_TRY(md_params(md, dt, gamma, x != nullptr ? x->kT : &kT, x != nullptr ? x->n_temps : 1, s));
-    if (x != nullptr) SG_TRY(remd_params(md, *x, out, s));
+    run_params(p.md, md, dt, seed, n_frames, stride, out);
+    end = md_params(md, dt, gamma, x != nullptr ? x->kT : &kT, md->group);
+    if (x != nullptr) end = remd_params(md, *x, out);
   }
-  SG_CUDA(cudaEventRecord(md->uploaded, s));
+  SG_TRY(upload(md, end, s));
   if (n_steps > 0) {
     SG_TRY(md_replay(md, kind, n_steps, s));
     md->step_host += (uint64_t)n_steps;
     SG_TRY(md_integrate(md, kind, 0, s));  // the second half-kick of the last step (and its frame)
   }
-  if (x != nullptr) {
-    const void* src[3] = {md->walker, md->xcount, md->xcount + md->n_rep};
-    for (int i = 0; i < 3; ++i)
-      if (out.dev<void>(5 + i) != nullptr)
-        SG_CUDA(cudaMemcpyAsync(out.dev<void>(5 + i), src[i], out.bytes(5 + i), cudaMemcpyDeviceToDevice, s));
-  }
+  if (x != nullptr) SG_TRY(out.copy_from(OUT_WALKERS, {md->walker, md->xcount, md->xcount + n_rep}));
   return out.finish();
 }
 
@@ -1218,16 +1206,12 @@ int64_t g_relax_block = 0;           // sgdml_b200_set_relax_block (test hook): 
 // buffers are made at the first NEB call
 int relax_alloc(sgdml_b200_md* md, int memory, bool neb) {
   if (md->rst == nullptr) SG_CUDA(cached_malloc(&md->rst, sizeof(RelaxState) * (size_t)md->n_rep));
-  if (md->dR == nullptr) SG_CUDA(cached_malloc(&md->dR, sizeof(RelaxParams)));
-  if (md->hR == nullptr) SG_CUDA(cudaMallocHost(&md->hR, sizeof(RelaxParams)));
   if (md->hActive == nullptr) {
     SG_CUDA(cudaHostAlloc(&md->hActive, sizeof(int), cudaHostAllocMapped));
     SG_CUDA(cudaHostGetDevicePointer((void**)&md->dActive, md->hActive, 0));
   }
   if (md->counted == nullptr) SG_CUDA(cudaEventCreateWithFlags(&md->counted, cudaEventDisableTiming));
   if (neb) {
-    if (md->dN == nullptr) SG_CUDA(cached_malloc(&md->dN, sizeof(NebParams)));
-    if (md->hN == nullptr) SG_CUDA(cudaMallocHost(&md->hN, sizeof(NebParams)));
     if (md->climb_idx == nullptr) SG_CUDA(cached_malloc(&md->climb_idx, sizeof(int) * (size_t)md->n_rep));
     if (md->Fn == nullptr) SG_CUDA(cached_malloc(&md->Fn, sizeof(double) * (size_t)(md->n_rep * md->dimi)));
   }
@@ -1251,37 +1235,15 @@ int relax_alloc(sgdml_b200_md* md, int memory, bool neb) {
   return 0;
 }
 
-// The parameters of one call into the pinned staging and their upload on s, once the previous call has read it:
-// an optimiser's RelaxParams (with the handle's L-BFGS ring) or an NEB call's NebParams (and its images per band).
-int stage_relax(sgdml_b200_md* md, const RelaxParams& prm, cudaStream_t s) {
-  RelaxParams& p = *md->hR;
-  p = prm;
-  p.m_cap = md->m_cap;
-  p.S = md->S;
-  p.Y = md->Y;
-  p.rho = md->rho;
-  p.r_prev = md->r_prev;
-  p.g_prev = md->g_prev;
-  SG_CUDA(cudaMemcpyAsync(md->dR, md->hR, sizeof(RelaxParams), cudaMemcpyHostToDevice, s));
-  return 0;
-}
-
-int stage_neb(sgdml_b200_md* md, const NebParams& q, cudaStream_t s) {
-  *md->hN = q;
-  md->group = q.P;
-  SG_CUDA(cudaMemcpyAsync(md->dN, md->hN, sizeof(NebParams), cudaMemcpyHostToDevice, s));
-  return 0;
-}
-
 // Relaxes every replica (or NEB band) from the handle's state: blocks of step-graph replays, each followed by the
 // convergence test and a count of unconverged units read back through mapped pinned memory; stops when none is left or
 // after max_steps.  The unit of convergence is a group of g consecutive replicas: g = 1 for relaxation, g = P for NEB
-// (whose climbing_out gets each band's highest interior image).  memory: L-BFGS pairs per replica to allocate (0:
-// none).  stage() stages and uploads the call's parameters (stage_relax, stage_neb).  Frozen units make the block
-// length a matter of cost only.  V is zero before and after.
-template <class Stage>
-int relax_impl(sgdml_b200_md* md, int kind, int64_t g, int memory, int64_t max_steps, int64_t* n_steps_out,
-               int* conv_out, double* fmax_out, int* climbing_out, cudaStream_t s, Stage stage) {
+// (whose climbing_out gets each band's highest interior image).  call: the entry point's RelaxParams (FIRE, L-BFGS;
+// the handle's L-BFGS ring is added here) or NebParams (NEB).  memory: L-BFGS pairs per replica to allocate (0: none).
+// Frozen units make the block length a matter of cost only.  V is zero before and after.
+int relax_impl(sgdml_b200_md* md, int kind, int g, int memory, const StepParams& call, int64_t max_steps,
+               int64_t* n_steps_out, int* conv_out, double* fmax_out, int* climbing_out, cudaStream_t s) {
+  md->group = g;
   const int64_t n_rep = md->n_rep;
   const int64_t n_units = n_rep / g;
   SG_TRY(force_eval_prepare(md->fe));
@@ -1289,9 +1251,20 @@ int relax_impl(sgdml_b200_md* md, int kind, int64_t g, int memory, int64_t max_s
   Outputs out(s);
   SG_TRY(out.init({{n_steps_out, sizeof(int64_t) * (size_t)n_units}, {conv_out, sizeof(int) * (size_t)n_units},
                    {fmax_out, sizeof(double) * (size_t)n_units}, {climbing_out, sizeof(int) * (size_t)n_units}}));
-  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the staging
-  SG_TRY(stage());
-  SG_CUDA(cudaEventRecord(md->uploaded, s));
+  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the mirror
+  StepParams& p = *md->params(md->hblk);
+  if (kind == MD_NEB_FIRE) {
+    p.neb = call.neb;
+  } else {
+    p.relax = call.relax;
+    p.relax.m_cap = md->m_cap;
+    p.relax.S = md->S;
+    p.relax.Y = md->Y;
+    p.relax.rho = md->rho;
+    p.relax.r_prev = md->r_prev;
+    p.relax.g_prev = md->g_prev;
+  }
+  SG_TRY(upload(md, &p + 1, s));
   const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
   SG_CUDA(cudaMemsetAsync(md->rst, 0, sizeof(RelaxState) * (size_t)n_units, s));
   SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
@@ -1313,8 +1286,7 @@ int relax_impl(sgdml_b200_md* md, int kind, int64_t g, int memory, int64_t max_s
                                                                   out.dev<int>(1), out.dev<double>(2));
   SG_CUDA(cudaGetLastError());
   count_launch(KID_MISC);
-  if (out.dev<int>(3) != nullptr)  // the last test ran k_neb_force at the final positions
-    SG_CUDA(cudaMemcpyAsync(out.dev<int>(3), md->climb_idx, out.bytes(3), cudaMemcpyDeviceToDevice, s));
+  SG_TRY(out.copy_from(3, {md->climb_idx}));  // the last test ran k_neb_force at the final positions
   return out.finish();
 }
 
@@ -1346,15 +1318,7 @@ int md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, int nb, c
     SG_CUDA(cached_malloc(&md->Es, sizeof(double) * n_rep));
     SG_CUDA(cached_malloc(&md->step, sizeof(uint64_t) * n_rep));
     SG_CUDA(cached_malloc(&md->s, sizeof(double) * md->dimi));
-    SG_CUDA(cached_malloc(&md->sigma, sizeof(double) * nb * md->dimi));
-    SG_CUDA(cached_malloc(&md->dP, sizeof(MdParams)));
-    SG_CUDA(cached_malloc(&md->dQ, sizeof(PimdParams)));
-    SG_CUDA(cached_malloc(&md->tab, sizeof(double) * (nb * nb + 4 * nb)));
-    SG_CUDA(cudaMallocHost(&md->hP, sizeof(MdParams)));
-    SG_CUDA(cudaMallocHost(&md->hQ, sizeof(PimdParams)));
-    SG_CUDA(cudaMallocHost(&md->hTab, sizeof(double) * (nb * nb + 4 * nb)));
-    SG_CUDA(cudaMallocHost(&md->hSigma, sizeof(double) * nb * md->dimi));
-    md->sigma_rows = nb;
+    SG_TRY(reserve(md, nb));
     SG_CUDA(cudaEventCreateWithFlags(&md->uploaded, cudaEventDisableTiming));
     md->s_host.resize((size_t)md->dimi);
     for (int i = 0; i < md->dimi; ++i) md->s_host[(size_t)i] = inv_mass[i / 3];
@@ -1429,19 +1393,20 @@ int sgdml_b200_md_get_state(sgdml_b200_md* md, double* R, double* V, double* F, 
   const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
   Outputs out(s);
   SG_TRY(out.init({{R, st}, {V, st}, {F, st}, {E_pot, sizeof(double) * md->n_rep}, {step, sizeof(uint64_t)}}));
-  const void* src[5] = {md->R, md->V, md->F, md->E, md->step};
-  for (int i = 0; i < 5; ++i)
-    if (out.dev<void>(i) != nullptr)
-      SG_CUDA(cudaMemcpyAsync(out.dev<void>(i), src[i], out.bytes(i), cudaMemcpyDeviceToDevice, s));
+  SG_TRY(out.copy_from(0, {md->R, md->V, md->F, md->E, md->step}));
   return out.finish();
 }
 
 int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, uint64_t seed,
                       int64_t stride, double* R_frames, double* V_frames, double* E_pot_frames, double* E_kin_frames,
                       void* stream) {
-  double* const frames[6] = {R_frames, V_frames, E_pot_frames, E_kin_frames, nullptr, nullptr};
-  return md_run(md, MD_CLASSICAL, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, frames, nullptr,
-                (cudaStream_t)stream);
+  SG_TRY(require_device());
+  SG_TRY(run_check(md, n_steps, dt, kT, gamma, stride, "sgdml_b200_md_run: no state yet (call sgdml_b200_md_set_state)"));
+  if (md->nb > 1)
+    return fail_arg("sgdml_b200_md_run: a ring-polymer handle (n_beads > 1) runs with sgdml_b200_pimd_run");
+  SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
+  void* const outs[N_RUN_OUTS] = {R_frames, V_frames, E_pot_frames, E_kin_frames};
+  return md_run(md, MD_CLASSICAL, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, outs, nullptr, (cudaStream_t)stream);
 }
 
 int sgdml_b200_remd_run(sgdml_b200_md* md, int64_t n_temps, const double* kT, int64_t n_steps, double dt, double gamma,
@@ -1457,17 +1422,27 @@ int sgdml_b200_remd_run(sgdml_b200_md* md, int64_t n_temps, const double* kT, in
     if (!(std::isfinite(kT[k]) && kT[k] > 0.0)) return fail_arg("sgdml_b200_remd_run: every kT must be finite and > 0");
   SG_ARG(std::isfinite(gamma) && gamma > 0.0);
   SG_ARG(exchange_every >= 0);
-  const RemdRun x = {(int)n_temps, kT, exchange_every, walker_frames, walkers_out, n_accepted, n_attempted};
-  double* const frames[6] = {R_frames, V_frames, E_pot_frames, E_kin_frames, nullptr, nullptr};
-  return md_run(md, MD_REMD, n_steps, dt, kT[0], 0.0, gamma, 0.0, seed, stride, frames, &x, (cudaStream_t)stream);
+  SG_TRY(run_check(md, n_steps, dt, kT[0], gamma, stride,
+                   "sgdml_b200_remd_run: no state yet (call sgdml_b200_md_set_state)"));
+  const RemdRun x = {(int)n_temps, kT, exchange_every};
+  void* const outs[N_RUN_OUTS] = {R_frames,      V_frames,    E_pot_frames, E_kin_frames, nullptr,
+                                  nullptr,       walker_frames, walkers_out, n_accepted,   n_attempted};
+  return md_run(md, MD_REMD, n_steps, dt, kT[0], 0.0, gamma, 0.0, seed, stride, outs, &x, (cudaStream_t)stream);
 }
 
 int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma,
                         double lambda, uint64_t seed, int64_t stride, double* R_frames, double* V_frames,
                         double* E_pot_frames, double* E_kin_frames, double* K_prim_frames, double* K_cv_frames,
                         void* stream) {
-  double* const frames[6] = {R_frames, V_frames, E_pot_frames, E_kin_frames, K_prim_frames, K_cv_frames};
-  return md_run(md, MD_RING_POLYMER, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, frames, nullptr,
+  SG_TRY(require_device());
+  SG_TRY(run_check(md, n_steps, dt, kT, gamma, stride,
+                   "sgdml_b200_pimd_run: no state yet (call sgdml_b200_md_set_state)"));
+  SG_ARG(std::isfinite(hbar) && hbar > 0.0);
+  SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
+  SG_ARG(std::isfinite(lambda) && lambda >= 0.0);
+  if (md->nb > 1 && kT == 0.0) return fail_arg("a ring polymer (n_beads > 1) needs kT > 0");
+  void* const outs[N_RUN_OUTS] = {R_frames, V_frames, E_pot_frames, E_kin_frames, K_prim_frames, K_cv_frames};
+  return md_run(md, MD_RING_POLYMER, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, outs, nullptr,
                 (cudaStream_t)stream);
 }
 
@@ -1478,14 +1453,13 @@ int sgdml_b200_relax_fire(sgdml_b200_md* md, int64_t max_steps, double fmax, dou
                      "sgdml_b200_relax_fire: no state yet (call sgdml_b200_md_set_state)"));
   SG_ARG(std::isfinite(dt) && dt > 0.0);
   SG_ARG(std::isfinite(dtmax) && dtmax > 0.0);
-  RelaxParams p = {};
-  p.fmax2 = fmax * fmax;
-  p.maxstep = maxstep;
-  p.dt0 = dt;
-  p.dtmax = dtmax;
-  cudaStream_t s = (cudaStream_t)stream;
-  return relax_impl(md, MD_FIRE, 1, 0, max_steps, n_steps_out, converged_out, fmax_out, nullptr, s,
-                    [&] { return stage_relax(md, p, s); });
+  StepParams c = {};
+  c.relax.fmax2 = fmax * fmax;
+  c.relax.maxstep = maxstep;
+  c.relax.dt0 = dt;
+  c.relax.dtmax = dtmax;
+  return relax_impl(md, MD_FIRE, 1, 0, c, max_steps, n_steps_out, converged_out, fmax_out, nullptr,
+                    (cudaStream_t)stream);
 }
 
 int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, int memory, double h0,
@@ -1495,14 +1469,13 @@ int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, do
                      "sgdml_b200_relax_lbfgs: no state yet (call sgdml_b200_md_set_state)"));
   SG_ARG(memory >= 1 && memory <= LBFGS_MAX_MEMORY);
   SG_ARG(std::isfinite(h0) && h0 > 0.0);
-  RelaxParams p = {};
-  p.fmax2 = fmax * fmax;
-  p.maxstep = maxstep;
-  p.h0 = h0;
-  p.memory = memory;
-  cudaStream_t s = (cudaStream_t)stream;
-  return relax_impl(md, MD_LBFGS, 1, memory, max_steps, n_steps_out, converged_out, fmax_out, nullptr, s,
-                    [&] { return stage_relax(md, p, s); });
+  StepParams c = {};
+  c.relax.fmax2 = fmax * fmax;
+  c.relax.maxstep = maxstep;
+  c.relax.h0 = h0;
+  c.relax.memory = memory;
+  return relax_impl(md, MD_LBFGS, 1, memory, c, max_steps, n_steps_out, converged_out, fmax_out, nullptr,
+                    (cudaStream_t)stream);
 }
 
 int sgdml_b200_neb_fire(sgdml_b200_md* md, int64_t n_images, int64_t max_steps, double fmax, double k, int climb,
@@ -1516,17 +1489,16 @@ int sgdml_b200_neb_fire(sgdml_b200_md* md, int64_t n_images, int64_t max_steps, 
   SG_ARG(std::isfinite(k) && k >= 0.0);
   SG_ARG(std::isfinite(dt) && dt > 0.0);
   SG_ARG(std::isfinite(dtmax) && dtmax > 0.0);
-  NebParams q = {};
-  q.fmax2 = fmax * fmax;
-  q.maxstep = maxstep;
-  q.dt0 = dt;
-  q.dtmax = dtmax;
-  q.k = k;
-  q.climb = climb != 0 ? 1 : 0;
-  q.P = (int)n_images;
-  cudaStream_t s = (cudaStream_t)stream;
-  return relax_impl(md, MD_NEB_FIRE, n_images, 0, max_steps, n_steps_out, converged_out, fmax_out, climbing_out, s,
-                    [&] { return stage_neb(md, q, s); });
+  StepParams c = {};
+  c.neb.fmax2 = fmax * fmax;
+  c.neb.maxstep = maxstep;
+  c.neb.dt0 = dt;
+  c.neb.dtmax = dtmax;
+  c.neb.k = k;
+  c.neb.climb = climb != 0 ? 1 : 0;
+  c.neb.P = (int)n_images;
+  return relax_impl(md, MD_NEB_FIRE, (int)n_images, 0, c, max_steps, n_steps_out, converged_out, fmax_out,
+                    climbing_out, (cudaStream_t)stream);
 }
 
 int sgdml_b200_set_relax_block(int64_t n_steps) {

@@ -106,6 +106,11 @@ class GDMLDynamics(object):
             raise ValueError('%s must hold n_replicas x 3N = %d x %d values' % (name, self.n_replicas, dimi))
         return x.reshape(self.n_replicas, dimi).contiguous() if hasattr(x, 'data_ptr') else x.reshape(self.n_replicas, dimi)
 
+    @property
+    def _shape(self):
+        """The shape ``get_state`` and ``run`` give the replica axis."""
+        return (self.n_replicas,)
+
     def _empty(self, shape, dtype=np.float64):
         if self._torch_device is None:
             return np.empty(shape, dtype=dtype)
@@ -164,23 +169,29 @@ class GDMLDynamics(object):
 
     def get_state(self):
         """{'positions', 'velocities', 'forces' (n_replicas, N, 3), 'potential_energy' (n_replicas,), 'step'}: Angstrom,
-        Angstrom/fs, eV/Angstrom, eV."""
+        Angstrom/fs, eV/Angstrom, eV.  Path-integral and replica-exchange handles shape the replica axis (n_polymers,
+        n_beads) and (n_ladders, n_temps)."""
         s = self._get_state_raw()
-        N = self.n_atoms
-        return {'positions': (s['R'] / self.Ang_to_R).reshape(-1, N, 3),
-                'velocities': (s['V'] / self.Ang_to_R).reshape(-1, N, 3),
-                'forces': (s['F'] * self.F_to_eV_Ang).reshape(-1, N, 3),
-                'potential_energy': s['E_pot'] * self.E_to_eV, 'step': s['step']}
+        g, a = self._shape, (self.n_atoms, 3)
+        return {'positions': (s['R'] / self.Ang_to_R).reshape(g + a),
+                'velocities': (s['V'] / self.Ang_to_R).reshape(g + a),
+                'forces': (s['F'] * self.F_to_eV_Ang).reshape(g + a),
+                'potential_energy': (s['E_pot'] * self.E_to_eV).reshape(g), 'step': s['step']}
+
+    def _ase_frames(self, f):
+        """The frames R, V, E_pot, E_kin among f (model units) in ASE units, shaped (n_frames,) + _shape [+ (N, 3)]."""
+        out = {}
+        for k, name in (('R', 'positions'), ('V', 'velocities')):
+            if k in f:
+                out[name] = (f[k] / self.Ang_to_R).reshape((f[k].shape[0],) + self._shape + (self.n_atoms, 3))
+        for k, name in (('E_pot', 'potential_energy'), ('E_kin', 'kinetic_energy')):
+            if k in f:
+                out[name] = (f[k] * self.E_to_eV).reshape((f[k].shape[0],) + self._shape)
+        return out
 
     def run(self, n_steps, dt_fs, temperature_K=0.0, friction_per_fs=0.0, seed=0, stride=0):
         kT = KB_EV * float(temperature_K) / self.E_to_eV
-        f = self._run_raw(n_steps, dt_fs, friction_per_fs, kT, seed, stride)
-        if not f:
-            return {}
-        N, nf = self.n_atoms, f['R'].shape[0]
-        return {'positions': (f['R'] / self.Ang_to_R).reshape(nf, -1, N, 3),
-                'velocities': (f['V'] / self.Ang_to_R).reshape(nf, -1, N, 3),
-                'potential_energy': f['E_pot'] * self.E_to_eV, 'kinetic_energy': f['E_kin'] * self.E_to_eV}
+        return self._ase_frames(self._run_raw(n_steps, dt_fs, friction_per_fs, kT, seed, stride))
 
 
 class GDMLPathIntegralDynamics(GDMLDynamics):
@@ -213,6 +224,10 @@ class GDMLPathIntegralDynamics(GDMLDynamics):
         )
         return handle
 
+    @property
+    def _shape(self):
+        return (self.n_polymers, self.n_beads)
+
     def _beads(self, x, name):
         """(n_polymers, n_beads, N, 3), (n_polymers, N, 3) or (N, 3) -> (n_polymers n_beads, 3N)."""
         return _groups(x, name, self.n_polymers, self.n_beads, self.n_atoms, ('n_polymers', 'n_beads'))
@@ -238,16 +253,6 @@ class GDMLPathIntegralDynamics(GDMLDynamics):
         velocities = None if velocities is None else self._beads(velocities, 'velocities')
         super().set_state(positions, velocities, step)
 
-    def get_state(self):
-        """{'positions', 'velocities', 'forces' (n_polymers, n_beads, N, 3), 'potential_energy' (n_polymers, n_beads),
-        'step'}: Angstrom, Angstrom/fs, eV/Angstrom, eV."""
-        st = super().get_state()
-        shape = (self.n_polymers, self.n_beads)
-        for k in ('positions', 'velocities', 'forces'):
-            st[k] = st[k].reshape(shape + (self.n_atoms, 3))
-        st['potential_energy'] = st['potential_energy'].reshape(shape)
-        return st
-
     def run(self, n_steps, dt_fs, temperature_K, centroid_friction_per_fs=0.0, pile_lambda=1.0, seed=0, stride=0):
         kT = KB_EV * float(temperature_K) / self.E_to_eV
         hbar = HBAR_EV_FS / self.E_to_eV
@@ -255,12 +260,9 @@ class GDMLPathIntegralDynamics(GDMLDynamics):
                           frames=('R', 'V', 'E_pot', 'K_prim', 'K_cv'))
         if not f:
             return {}
-        N, nf, n_p, P = self.n_atoms, f['R'].shape[0], self.n_polymers, self.n_beads
-        return {'positions': (f['R'] / self.Ang_to_R).reshape(nf, n_p, P, N, 3),
-                'velocities': (f['V'] / self.Ang_to_R).reshape(nf, n_p, P, N, 3),
-                'potential_energy': (f['E_pot'] * self.E_to_eV).reshape(nf, n_p, P),
-                'kinetic_energy_primitive': f['K_prim'] * self.E_to_eV,
-                'kinetic_energy_virial': f['K_cv'] * self.E_to_eV}
+        out = self._ase_frames(f)
+        out.update(kinetic_energy_primitive=f['K_prim'] * self.E_to_eV, kinetic_energy_virial=f['K_cv'] * self.E_to_eV)
+        return out
 
 
 def _groups(x, name, n_g, per, N, axes):
@@ -309,6 +311,10 @@ class GDMLReplicaExchange(GDMLDynamics):
             raise ValueError('a ladder needs at least two temperatures, and n_ladders >= 1')
         super().__init__(model, masses, self.n_ladders * self.n_temps, E_to_eV, F_to_eV_Ang)
 
+    @property
+    def _shape(self):
+        return (self.n_ladders, self.n_temps)
+
     # ------------------------------------------------------------------ model units (L, model energy, fs)
     def _run_raw(self, n_steps, dt, gamma, kT, exchange_every, seed=0, stride=0,
                  frames=('R', 'V', 'E_pot', 'E_kin', 'walker')):
@@ -339,34 +345,19 @@ class GDMLReplicaExchange(GDMLDynamics):
             velocities = _groups(velocities, 'velocities', self.n_ladders, self.n_temps, self.n_atoms, axes)
         super().set_state(positions, velocities, step)
 
-    def get_state(self):
-        """{'positions', 'velocities', 'forces' (n_ladders, n_temps, N, 3), 'potential_energy' (n_ladders, n_temps),
-        'step'}: Angstrom, Angstrom/fs, eV/Angstrom, eV."""
-        st = super().get_state()
-        shape = (self.n_ladders, self.n_temps)
-        for k in ('positions', 'velocities', 'forces'):
-            st[k] = st[k].reshape(shape + (self.n_atoms, 3))
-        st['potential_energy'] = st['potential_energy'].reshape(shape)
-        return st
-
     def run(self, n_steps, dt_fs, friction_per_fs, exchange_every, seed=0, stride=0):
         kT = KB_EV * self.temperatures_K / self.E_to_eV
         f = self._run_raw(n_steps, dt_fs, friction_per_fs, kT, exchange_every, seed, stride)
-        shape = (self.n_ladders, self.n_temps)
         acc, att = f['n_accepted'], f['n_attempted']
         if hasattr(att, 'data_ptr'):
             ratio = acc.double() / att.clip(1).double()
         else:
             ratio = acc / att.clip(1)
         ratio[att == 0] = np.nan
-        out = {'walkers': f['walkers'].reshape(shape), 'n_accepted': acc, 'n_attempted': att, 'acceptance': ratio}
-        if 'R' in f:
-            N, nf = self.n_atoms, f['R'].shape[0]
-            out.update(positions=(f['R'] / self.Ang_to_R).reshape((nf,) + shape + (N, 3)),
-                       velocities=(f['V'] / self.Ang_to_R).reshape((nf,) + shape + (N, 3)),
-                       potential_energy=(f['E_pot'] * self.E_to_eV).reshape((nf,) + shape),
-                       kinetic_energy=(f['E_kin'] * self.E_to_eV).reshape((nf,) + shape),
-                       walker=f['walker'].reshape((nf,) + shape))
+        out = {'walkers': f['walkers'].reshape(self._shape), 'n_accepted': acc, 'n_attempted': att, 'acceptance': ratio}
+        out.update(self._ase_frames(f))
+        if 'walker' in f:
+            out['walker'] = f['walker'].reshape((f['walker'].shape[0],) + self._shape)
         return out
 
 
@@ -399,13 +390,7 @@ class GDMLRelaxation(GDMLDynamics):
     def _relax_raw(self, optimizer, max_steps, fmax, maxstep, *args):
         """FIRE: args = (dt, dtmax); L-BFGS: args = (memory, h0), all in model units.  -> (n_steps, converged, fmax)."""
         n = self.n_replicas
-        if self._torch_device is None:
-            out = (np.empty(n, dtype=np.int64), np.empty(n, dtype=np.int32), np.empty(n))
-        else:
-            import torch
-
-            out = tuple(torch.empty(n, dtype=t, device=self._torch_device)
-                        for t in (torch.int64, torch.int32, torch.float64))
+        out = (self._empty(n, np.int64), self._empty(n, np.int32), self._empty(n))
         L = _lib.lib()
         if optimizer == 'fire':
             rc = L.sgdml_b200_relax_fire(self._handle, int(max_steps), float(fmax), float(maxstep), float(args[0]),
@@ -496,13 +481,7 @@ class GDMLNEB(GDMLRelaxation):
     def _neb_raw(self, max_steps, fmax, k, climb, maxstep, dt, dtmax):
         """-> (n_steps, converged, fmax, climbing_image), each (n_bands,), in model units."""
         n = self.n_bands
-        if self._torch_device is None:
-            out = (np.empty(n, dtype=np.int64), np.empty(n, dtype=np.int32), np.empty(n), np.empty(n, dtype=np.int32))
-        else:
-            import torch
-
-            out = tuple(torch.empty(n, dtype=t, device=self._torch_device)
-                        for t in (torch.int64, torch.int32, torch.float64, torch.int32))
+        out = (self._empty(n, np.int64), self._empty(n, np.int32), self._empty(n), self._empty(n, np.int32))
         _lib.check(
             _lib.lib().sgdml_b200_neb_fire(self._handle, self.n_images, int(max_steps), float(fmax), float(k),
                                            1 if climb else 0, float(maxstep), float(dt), float(dtmax),

@@ -219,6 +219,48 @@ int sgdml_b200_remd_run(sgdml_b200_md* md, int64_t n_temps, const double* kT, in
                         double* E_pot_frames, double* E_kin_frames, int* walker_frames, int* walkers_out,
                         int64_t* n_accepted, int64_t* n_attempted, void* stream);
 
+/* ---------------------------------------------------------------- constant-pressure molecular dynamics on the device
+ * Extension: NPT trajectories of periodic models: BAOAB Langevin replicas (sgdml_b200_md_run's step) with the isotropic
+ * stochastic cell rescaling barostat of Bernetti & Bussi (J. Chem. Phys. 153, 114107 (2020)), each replica in a cell of
+ * its own that the barostat scales.  Units are the model's: P0 in energy / L^3, beta_T (isothermal compressibility) in
+ * L^3 / energy, tau_p in T.  An NPT handle is an sgdml_b200_md handle with one cell per replica:
+ * sgdml_b200_md_set_state evaluates F, E_pot and the virial W = -dE/d(strain) of each replica in its own cell;
+ * sgdml_b200_md_get_state and sgdml_b200_md_destroy are unchanged; sgdml_b200_md_run, _remd_run, _pimd_run, _relax_*
+ * and _neb_fire on it are argument errors, as is sgdml_b200_npt_run on any other handle.
+ * Barostat state per replica: eps, the log of its volume ratio V / V0 since the cell was set, its base cell L0 with
+ * the caller's inverse, and V0 = |det L0| (host).  The replica is evaluated in L = a L0 with inverse L0^-1 / a,
+ * a = exp(eps / 3).  One step, with the replica's step index at n and its W of the current state:
+ *   pending B and frame as sgdml_b200_md_run;  K = 1/2 sum_i v_i^2 / s_i in E_kin's order;  V = V0 exp(eps);
+ *   P_int = (2 K + ((W_0 + W_4) + W_8)) / (3 V);
+ *   de = -c_a (P0 - P_int) + sqrt(c_b / V) eta,  c_a = (beta_T / tau_p) dt, c_b = 2 kT (beta_T / tau_p) dt (host);
+ *   B, A, O, A as sgdml_b200_md_run;  mu = exp(de / 3),  r = r mu,  v = v / mu,  eps = eps + de;
+ *   F, E_pot and W at the new positions in the new cell.
+ * Every update is rounded as written.  eta = sqrt(-2 ln U_a) cos(2 pi U_b), U_a, U_b from the words of Philox4x32-10
+ * under the run's key with counter (0xFFFFFFFF, replica, n mod 2^32, n >> 32), apart from the O noise and the exchange
+ * draws; c_b == 0 draws nothing.  With beta_T = 0 every replica keeps its cell and its trajectory is
+ * sgdml_b200_md_run's bit for bit in that cell.  Positions are never wrapped into the cell.  Streams, host/device
+ * outputs, SGDML_B200_GRAPH=0, the workspace and the launch families (8 and 1) are those of sgdml_b200_md_run;
+ * argument errors are reported before anything is queued, and a rejected call changes nothing. */
+/* lattices, lattice_invs: (n_rep, 9) HOST doubles, row-major, lattice vectors as columns (the
+ * sgdml_b200_predict_virial_cells convention), each cell finite and not singular; inv_mass and n_rep as
+ * sgdml_b200_md_create. */
+int sgdml_b200_npt_create(sgdml_b200_md** out, sgdml_b200_model* model, int64_t n_rep, const double* inv_mass,
+                          const double* lattices, const double* lattice_invs);
+/* Replaces every replica's base cell (eps = 0), checked as at creation, and re-evaluates F, E_pot and W when the
+ * handle has a state.  Positions do not move. */
+int sgdml_b200_npt_set_cells(sgdml_b200_md* md, const double* lattices, const double* lattice_invs, void* stream);
+/* lattices, lattice_invs, W: (n_rep, 9) each, the current cells a L0, their inverses and the virial of the state;
+ * any output may be NULL. */
+int sgdml_b200_npt_get_cells(sgdml_b200_md* md, double* lattices, double* lattice_invs, double* W, void* stream);
+/* n_steps, dt, gamma, kT, seed and stride as sgdml_b200_md_run; P0 finite; beta_T finite and >= 0; tau_p finite and
+ * > 0.  Frames: R_frames, V_frames, E_pot_frames, E_kin_frames as sgdml_b200_md_run; cell_frames (n_frames, n_rep, 9)
+ * the cells a L0; P_frames (n_frames, n_rep) the instantaneous pressure P_int of the frame's state.  Each may be NULL.
+ * Needs a state. */
+int sgdml_b200_npt_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, double P0,
+                       double beta_T, double tau_p, uint64_t seed, int64_t stride, double* R_frames,
+                       double* V_frames, double* E_pot_frames, double* E_kin_frames, double* cell_frames,
+                       double* P_frames, void* stream);
+
 /* ---------------------------------------------------------------- path-integral molecular dynamics on the device
  * Extension: ring polymers of P beads (1 <= P <= 64), thermostatted mode by mode with PILE-L (Ceriotti, Parrinello,
  * Markland & Manolopoulos, J. Chem. Phys. 133, 124104 (2010)) in the BAOAB order of Liu, Li & Liu (J. Chem. Phys. 145,

@@ -9,7 +9,8 @@ CPU fallback.
 
 __version__ = '0.1.0'
 
-from .md import GDMLNEB, GDMLDynamics, GDMLPathIntegralDynamics, GDMLRelaxation, GDMLReplicaExchange  # noqa: F401
+from .md import (GDMLNEB, GDMLDynamics, GDMLNPTDynamics, GDMLPathIntegralDynamics, GDMLRelaxation,  # noqa: F401
+                 GDMLReplicaExchange)
 from .perm import find_perms  # noqa: F401
 from .predict import GDMLPredict  # noqa: F401
 from .train import GDMLTrain  # noqa: F401

@@ -55,6 +55,14 @@ SIGNATURES = {
         [c_void_p, i64, c_void_p, i64, C.c_double, C.c_double, C.c_uint64, i64, i64, c_void_p, c_void_p, c_void_p,
          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     ),
+    'sgdml_b200_npt_create': (C.c_int, [C.POINTER(c_void_p), c_void_p, i64, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_npt_set_cells': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_npt_get_cells': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_npt_run': (
+        C.c_int,
+        [c_void_p, i64, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_uint64, i64,
+         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
     'sgdml_b200_pimd_create': (C.c_int, [C.POINTER(c_void_p), c_void_p, i64, i64, c_void_p]),
     'sgdml_b200_pimd_run': (
         C.c_int,

@@ -18,6 +18,7 @@
 // and a run continued over several calls draws exactly the noise of one long run.
 #include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstring>
 #include <initializer_list>
 #include <vector>
@@ -81,6 +82,16 @@ __device__ __forceinline__ T block_tree(T x, T* red, Op op) {
 
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
 
+// B, A, O, A of coordinate i from (ri, vi), vi after the pending half-kick: the one copy of the update of k_md_step and
+// k_npt_step (kick = h (F s), sg the replica's sigma row, xi the coordinate's normal)
+__device__ __forceinline__ void baoab(const MdParams& p, double kick, const double* __restrict__ sg, int i, double xi,
+                                      double& ri, double& vi) {
+  vi = __dadd_rn(vi, kick);
+  ri = __dadd_rn(ri, __dmul_rn(p.h, vi));
+  if (p.use_O) vi = __dadd_rn(__dmul_rn(p.c1, vi), __dmul_rn(sg[i], xi));
+  ri = __dadd_rn(ri, __dmul_rn(p.h, vi));
+}
+
 __global__ void __launch_bounds__(MD_THREADS) k_md_step(const MdParams* __restrict__ P, const double* __restrict__ s,
                                                        const double* __restrict__ sigma, double* __restrict__ R,
                                                        double* __restrict__ V, const double* __restrict__ F,
@@ -119,10 +130,7 @@ __global__ void __launch_bounds__(MD_THREADS) k_md_step(const MdParams* __restri
         }
       }
       if (advance) {
-        vi = __dadd_rn(vi, kick);
-        ri = __dadd_rn(ri, __dmul_rn(p.h, vi));
-        if (p.use_O) vi = __dadd_rn(__dmul_rn(p.c1, vi), __dmul_rn(sg[i], xi[q]));
-        ri = __dadd_rn(ri, __dmul_rn(p.h, vi));
+        baoab(p, kick, sg, i, xi[q], ri, vi);
         r[i] = ri;
       }
       v[i] = vi;
@@ -137,6 +145,97 @@ __global__ void __launch_bounds__(MD_THREADS) k_md_step(const MdParams* __restri
   }
   __syncthreads();  // every thread has read the counter
   if (advance && threadIdx.x == 0) step[rep] = n + 1;
+}
+
+// The NPT step of sgdml_b200_npt_run (contract in md.cuh): k_md_step's pending half-kick and frame, the instantaneous
+// pressure, the barostat's volume move, then k_md_step's B, A, O, A followed by the isotropic rescaling.  The first
+// pass leaves the full-step velocities in V; each thread reads back only its own coordinates in the second.
+__global__ void __launch_bounds__(MD_THREADS) k_npt_step(const MdParams* __restrict__ P, const NptParams* __restrict__ Q,
+                                                        const double* __restrict__ s, const double* __restrict__ sigma,
+                                                        double* __restrict__ R, double* __restrict__ V,
+                                                        const double* __restrict__ F, const double* __restrict__ E,
+                                                        const double* __restrict__ W, NptCell* __restrict__ cell,
+                                                        Lattice* __restrict__ lat, uint64_t* __restrict__ step,
+                                                        int dimi, int advance) {
+  __shared__ double red[MD_THREADS];
+  const int64_t rep = blockIdx.x, n_rep = gridDim.x;
+  const MdParams p = *P;
+  const NptParams q = *Q;
+  const uint64_t n = step[rep];
+  const uint64_t done = n - p.run_start;
+  const bool pending = done != 0;
+  const bool sample = pending && p.stride > 0 && done % (uint64_t)p.stride == 0;
+  const int64_t frame = sample ? (int64_t)(done / (uint64_t)p.stride) - 1 : 0;
+  double* r = R + rep * dimi;
+  double* v = V + rep * dimi;
+  const double* f = F + rep * dimi;
+  const int64_t fo = (frame * n_rep + rep) * dimi;
+  const int n_pairs = (dimi + 1) / 2;
+  double ke = 0.0;
+  for (int j = threadIdx.x; j < n_pairs; j += MD_THREADS) {
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const int i = 2 * j + c;
+      if (i >= dimi) break;
+      double vi = v[i];
+      if (pending) vi = __dadd_rn(vi, __dmul_rn(p.h, __dmul_rn(f[i], s[i])));
+      if (sample) {
+        if (p.R_f) p.R_f[fo + i] = r[i];
+        if (p.V_f) p.V_f[fo + i] = vi;
+      }
+      ke = __dadd_rn(ke, __ddiv_rn(__dmul_rn(vi, vi), s[i]));
+      v[i] = vi;
+    }
+  }
+  const double K = 0.5 * block_tree(ke, red, dadd);
+  NptCell* cl = cell + rep;
+  const double eps0 = cl->eps;
+  const double* w = W + rep * 9;
+  const double vol = __dmul_rn(cl->V0, exp(eps0));
+  const double pint = __ddiv_rn(__dadd_rn(__dmul_rn(2.0, K), __dadd_rn(__dadd_rn(w[0], w[4]), w[8])),
+                                __dmul_rn(3.0, vol));
+  if (sample) {
+    const int64_t fr = frame * n_rep + rep;
+    if (threadIdx.x == 0) {
+      if (p.Ek_f) p.Ek_f[fr] = K;
+      if (p.Ep_f) p.Ep_f[fr] = E[rep];
+      if (q.P_f) q.P_f[fr] = pint;
+    }
+    if (q.cell_f && threadIdx.x < 9) q.cell_f[fr * 9 + threadIdx.x] = lat[rep].vec[threadIdx.x];
+  }
+  if (advance) {
+    double de = __dmul_rn(-q.c_a, __dsub_rn(q.P0, pint));
+    if (q.c_b != 0.0) {
+      double eta[2];
+      normal_pair(eta, 0xFFFFFFFFu, (uint32_t)rep, n, p.key[0], p.key[1]);
+      de = __dadd_rn(de, __dmul_rn(sqrt(__ddiv_rn(q.c_b, vol)), eta[0]));
+    }
+    const double mu = exp(__ddiv_rn(de, 3.0));
+    for (int j = threadIdx.x; j < n_pairs; j += MD_THREADS) {
+      double xi[2] = {0.0, 0.0};
+      if (p.use_O) normal_pair(xi, (uint32_t)j, (uint32_t)rep, n, p.key[0], p.key[1]);
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int i = 2 * j + c;
+        if (i >= dimi) break;
+        double vi = v[i], ri = r[i];
+        baoab(p, __dmul_rn(p.h, __dmul_rn(f[i], s[i])), sigma, i, xi[c], ri, vi);
+        r[i] = __dmul_rn(ri, mu);
+        v[i] = __ddiv_rn(vi, mu);
+      }
+    }
+    const double eps = __dadd_rn(eps0, de);
+    const double a = exp(__ddiv_rn(eps, 3.0));
+    if (threadIdx.x < 9) {
+      lat[rep].vec[threadIdx.x] = __dmul_rn(a, cl->L0[threadIdx.x]);
+      lat[rep].inv[threadIdx.x] = __ddiv_rn(cl->L0inv[threadIdx.x], a);
+    }
+    __syncthreads();  // every thread has read the counter and the cell
+    if (threadIdx.x == 0) {
+      cl->eps = eps;
+      step[rep] = n + 1;
+    }
+  }
 }
 
 // The replica exchange of sgdml_b200_remd_run (contract in md.cuh).  Thread t decides the pairs t, t + MD_THREADS, ...
@@ -733,6 +832,7 @@ struct StepParams {
   RelaxParams relax;
   NebParams neb;
   RemdParams remd;
+  NptParams npt;
 };
 constexpr size_t STEP_PARAMS_BYTES = (sizeof(StepParams) + 255) & ~(size_t)255;  // where the tables start
 
@@ -786,6 +886,10 @@ struct sgdml_b200_md {
   // replica exchange (sgdml_b200_remd_run), allocated by the first replica-exchange call
   int* walker = nullptr;      // (n_rep) walker label per slot
   int64_t* xcount = nullptr;  // (2, n_rep) accepted and attempted swaps of the current run
+  // NPT (sgdml_b200_npt_create): one cell per replica, made with the handle; null on every other handle
+  NptCell* cell = nullptr;    // (n_rep) barostat state
+  Lattice* lat = nullptr;     // (n_rep) the cells the descriptor kernel reads: a L0 and L0^-1 / a, a = exp(eps / 3)
+  double *W = nullptr, *Ws = nullptr;  // (n_rep, 9) virial of the state, and of the evaluation that precedes a capture
 
   // the block's parts in blk or hblk
   StepParams* params(char* b) const { return reinterpret_cast<StepParams*>(b); }
@@ -805,13 +909,15 @@ void md_free(sgdml_b200_md* md) {
   if (md->counted) cudaEventDestroy(md->counted);
   force_eval_destroy(md->fe);
   for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s}) cached_free(p);
-  for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev, md->Fn}) cached_free(p);
+  for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev, md->Fn, md->W, md->Ws}) cached_free(p);
   cached_free(md->step);
   cached_free(md->blk);
   cached_free(md->rst);
   cached_free(md->climb_idx);
   cached_free(md->walker);
   cached_free(md->xcount);
+  cached_free(md->cell);
+  cached_free(md->lat);
   cudaFreeHost(md->hblk);
   cudaFreeHost(md->hActive);
   delete md;
@@ -903,7 +1009,7 @@ class Outputs {
   }
 
  private:
-  static constexpr int MAX_OUTS = 10;
+  static constexpr int MAX_OUTS = 12;
   cudaStream_t s_;
   int n_ = 0;
   Out out_[MAX_OUTS];
@@ -914,10 +1020,12 @@ class Outputs {
 };
 
 // what one step of the handle's graph integrates
-enum MdKind { MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, MD_NEB_FIRE = 4, MD_REMD = 5 };
+enum MdKind {
+  MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, MD_NEB_FIRE = 4, MD_REMD = 5, MD_NPT = 6
+};
 
-// the integrator of sgdml_b200_md_run, sgdml_b200_remd_run, sgdml_b200_pimd_run, sgdml_b200_relax_* or
-// sgdml_b200_neb_fire; advance == 0 completes a run's last step (MD; a replica exchange first exchanges that last
+// the integrator of sgdml_b200_md_run, sgdml_b200_remd_run, sgdml_b200_npt_run, sgdml_b200_pimd_run,
+// sgdml_b200_relax_* or sgdml_b200_neb_fire; advance == 0 completes a run's last step (MD; a replica exchange first exchanges that last
 // state) or only tests convergence (relaxation, NEB: after the force projection).  L-BFGS keeps its direction in V,
 // which relax_impl zeroes after.
 int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
@@ -946,6 +1054,11 @@ int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
                                                                advance);
       break;
     }
+    case MD_NPT:
+      k_npt_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&p->md, &p->npt, md->s, md->sigma(md->blk), md->R, md->V,
+                                                            md->F, md->E, md->W, md->cell, md->lat, md->step, md->dimi,
+                                                            advance);
+      break;
     case MD_REMD:
       k_remd_exchange<<<(unsigned)(md->n_rep / md->group), MD_THREADS, 0, s>>>(&p->remd, &p->md, md->s, md->R, md->V,
                                                                               md->F, md->E, md->walker, md->step,
@@ -962,9 +1075,15 @@ int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
   return 0;
 }
 
+// F and E (and on an NPT handle W, each replica in its own cell) of the positions in R
+int md_forces(sgdml_b200_md* md, double* F, double* E, double* W, cudaStream_t s) {
+  if (md->cell == nullptr) return force_eval_run(md->fe, md->R, F, E, s);
+  return force_eval_run_cells(md->fe, md->R, md->lat, F, E, W, s);
+}
+
 int md_step(sgdml_b200_md* md, int kind, cudaStream_t s) {
   SG_TRY(md_integrate(md, kind, 1, s));
-  return force_eval_run(md->fe, md->R, md->F, md->E, s);
+  return md_forces(md, md->F, md->E, md->W, s);
 }
 
 // the step graph, captured again whenever the force evaluation it bakes in is stale or its key changes
@@ -983,7 +1102,7 @@ int md_graph(sgdml_b200_md* md, int kind, cudaStream_t s) {
   SG_CUDA(cudaEventRecord(md->ge, s));
   SG_CUDA(cudaStreamWaitEvent(md->gs, md->ge, 0));
   // the force evaluation once un-captured, into scratch outputs: sets the kernels' shared-memory attributes
-  SG_TRY(force_eval_run(md->fe, md->R, md->Fs, md->Es, md->gs));
+  SG_TRY(md_forces(md, md->Fs, md->Es, md->Ws, md->gs));
   SG_CUDA(cudaStreamSynchronize(md->gs));
   SG_TRY(capture_graph(md->gs, [&] { return md_step(md, kind, md->gs); }, &md->exec, &md->n_kernels));
   force_eval_mark(md->fe);
@@ -1006,10 +1125,11 @@ int md_replay(sgdml_b200_md* md, int kind, int64_t n_steps, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------ MD, replica-exchange and PIMD runs
-// What a run writes, by Outputs slot: the frames, a ring polymer's estimator frames, then a replica exchange's walker
-// frames, final walker labels and counts.
+// What a run writes, by Outputs slot: the frames, a ring polymer's estimator frames, a replica exchange's walker
+// frames, final walker labels and counts, then an NPT run's cell and pressure frames.
 enum RunOut {
-  OUT_R, OUT_V, OUT_EPOT, OUT_EKIN, OUT_KPRIM, OUT_KCV, OUT_WALKER_F, OUT_WALKERS, OUT_NACC, OUT_NATT, N_RUN_OUTS
+  OUT_R, OUT_V, OUT_EPOT, OUT_EKIN, OUT_KPRIM, OUT_KCV, OUT_WALKER_F, OUT_WALKERS, OUT_NACC, OUT_NATT, OUT_CELL,
+  OUT_PRESS, N_RUN_OUTS
 };
 
 // The run's constants, once on the host in double precision.  First the fields MdParams and PimdParams share.
@@ -1091,6 +1211,23 @@ const double* remd_params(sgdml_b200_md* md, const RemdRun& x, const Outputs& ou
   return dn + (nt - 1);
 }
 
+// What an NPT run (sgdml_b200_npt_run) adds to an MD run: the barostat's target pressure, compressibility and time
+// constant, checked.
+struct NptRun {
+  double P0, beta_T, tau_p;
+};
+
+// the barostat's constants, on the host in double precision (after run_params)
+void npt_params(sgdml_b200_md* md, const NptRun& b, double dt, double kT, const Outputs& out) {
+  NptParams& q = md->params(md->hblk)->npt;
+  const double rate = b.beta_T / b.tau_p;
+  q.P0 = b.P0;
+  q.c_a = rate * dt;
+  q.c_b = 2.0 * kT * rate * dt;
+  q.cell_f = out.dev(OUT_CELL);
+  q.P_f = out.dev(OUT_PRESS);
+}
+
 // PIMD: the estimator constants, C, the mode tables and the (P, 3N) sigma table (tests/pimd_oracle.py restates them);
 // returns the end of what it filled
 const double* pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, double kT, double hbar, double gamma,
@@ -1142,10 +1279,14 @@ const double* pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, doub
   return sigma + (size_t)nb * dimi;
 }
 
-// the checks every run shares; a rejected call queues nothing
+constexpr const char* NPT_ONLY = "an NPT handle (sgdml_b200_npt_create) runs only sgdml_b200_npt_run";
+
+// the checks every run shares (npt: the run is sgdml_b200_npt_run); a rejected call queues nothing
 int run_check(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double gamma, int64_t stride,
-              const char* no_state) {
+              const char* no_state, bool npt = false) {
   SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
+  if (npt && md->cell == nullptr) return fail_arg("sgdml_b200_npt_run needs an NPT handle (sgdml_b200_npt_create)");
+  if (!npt && md->cell != nullptr) return fail_arg(NPT_ONLY);
   SG_ARG(std::isfinite(dt) && dt > 0.0);
   SG_ARG(std::isfinite(kT) && kT >= 0.0);
   if (md->nb == 1 && kT > 0.0 && gamma == 0.0)
@@ -1155,11 +1296,12 @@ int run_check(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double g
   return 0;
 }
 
-// sgdml_b200_md_run (MD_CLASSICAL), sgdml_b200_pimd_run (MD_RING_POLYMER; hbar and lambda are only its own) and
-// sgdml_b200_remd_run (MD_REMD, with x: its ladder, and kT = its first temperature), after their checks.  n_steps
-// steps, then the completing launch.
+// sgdml_b200_md_run (MD_CLASSICAL), sgdml_b200_pimd_run (MD_RING_POLYMER; hbar and lambda are only its own),
+// sgdml_b200_remd_run (MD_REMD, with x: its ladder, and kT = its first temperature) and sgdml_b200_npt_run (MD_NPT,
+// with b: its barostat), after their checks.  n_steps steps, then the completing launch.
 int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, double hbar, double gamma, double lambda,
-           uint64_t seed, int64_t stride, void* const outs[N_RUN_OUTS], const RemdRun* x, cudaStream_t s) {
+           uint64_t seed, int64_t stride, void* const outs[N_RUN_OUTS], const RemdRun* x, const NptRun* b,
+           cudaStream_t s) {
   if (n_steps == 0 && x == nullptr) return 0;  // (a replica exchange still reports its labels and zero counts)
   md->group = x != nullptr ? x->n_temps : 1;
   const int64_t n_rep = md->n_rep, n_frames = stride > 0 ? n_steps / stride : 0;
@@ -1170,7 +1312,8 @@ int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, d
   SG_TRY(out.init({{outs[OUT_R], fr * md->dimi}, {outs[OUT_V], fr * md->dimi}, {outs[OUT_EPOT], fr},
                    {outs[OUT_EKIN], fr}, {outs[OUT_KPRIM], fp}, {outs[OUT_KCV], fp},
                    {outs[OUT_WALKER_F], sizeof(int) * (size_t)(n_frames * n_rep)},
-                   {outs[OUT_WALKERS], sizeof(int) * (size_t)n_rep}, {outs[OUT_NACC], nc}, {outs[OUT_NATT], nc}}));
+                   {outs[OUT_WALKERS], sizeof(int) * (size_t)n_rep}, {outs[OUT_NACC], nc}, {outs[OUT_NATT], nc},
+                   {outs[OUT_CELL], 9 * fr}, {outs[OUT_PRESS], fr}}));
   SG_TRY(force_eval_prepare(md->fe));
   if (x != nullptr) {
     SG_TRY(reserve(md, x->n_temps));
@@ -1187,6 +1330,7 @@ int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, d
     run_params(p.md, md, dt, seed, n_frames, stride, out);
     end = md_params(md, dt, gamma, x != nullptr ? x->kT : &kT, md->group);
     if (x != nullptr) end = remd_params(md, *x, out);
+    if (b != nullptr) npt_params(md, *b, dt, kT, out);
   }
   SG_TRY(upload(md, end, s));
   if (n_steps > 0) {
@@ -1295,6 +1439,7 @@ int relax_check(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxste
   SG_ARG(md != nullptr && max_steps >= 0);
   SG_ARG(std::isfinite(fmax) && fmax >= 0.0);
   SG_ARG(std::isfinite(maxstep) && maxstep > 0.0);
+  if (md->cell != nullptr) return fail_arg(NPT_ONLY);
   if (!md->has_state) return fail_arg(what);
   return 0;
 }
@@ -1334,6 +1479,44 @@ int md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, int nb, c
   return 0;
 }
 
+// The cells of an NPT handle from (n_rep, 9) HOST lattices and inverses, each checked as sgdml_b200_predict_virial_cells
+// checks them: the barostat state (eps = 0, V0 = |det L0|) and the cells the descriptor kernel reads.  Nothing is queued.
+int npt_parse(const double* lattices, const double* lattice_invs, int64_t n_rep, std::vector<NptCell>* cells,
+              std::vector<Lattice>* lats) {
+  SG_ARG(lattices != nullptr && lattice_invs != nullptr);
+  SG_ARG(!is_device_ptr(lattices) && !is_device_ptr(lattice_invs));
+  cells->assign((size_t)n_rep, NptCell());
+  lats->assign((size_t)n_rep, Lattice());
+  for (int64_t g = 0; g < n_rep; ++g) {
+    Lattice& l = (*lats)[(size_t)g];
+    NptCell& c = (*cells)[(size_t)g];
+    l.on = 1;
+    std::copy(lattices + 9 * g, lattices + 9 * g + 9, l.vec);
+    std::copy(lattice_invs + 9 * g, lattice_invs + 9 * g + 9, l.inv);
+    SG_TRY(check_cell(l));
+    const double* a = l.vec;
+    c.eps = 0.0;
+    c.V0 = std::fabs(a[0] * (a[4] * a[8] - a[5] * a[7]) - a[1] * (a[3] * a[8] - a[5] * a[6]) +
+                     a[2] * (a[3] * a[7] - a[4] * a[6]));
+    std::copy(l.vec, l.vec + 9, c.L0);
+    std::copy(l.inv, l.inv + 9, c.L0inv);
+  }
+  return 0;
+}
+
+// installs parsed cells on an NPT handle, and with a state evaluates F, E and W in them
+int npt_install(sgdml_b200_md* md, const std::vector<NptCell>& cells, const std::vector<Lattice>& lats,
+                cudaStream_t s) {
+  SG_CUDA(cudaMemcpyAsync(md->cell, cells.data(), sizeof(NptCell) * cells.size(), cudaMemcpyHostToDevice, s));
+  SG_CUDA(cudaMemcpyAsync(md->lat, lats.data(), sizeof(Lattice) * lats.size(), cudaMemcpyHostToDevice, s));
+  if (md->has_state) {
+    SG_TRY(force_eval_prepare(md->fe));
+    SG_TRY(md_forces(md, md->F, md->E, md->W, s));
+  }
+  SG_CUDA(cudaStreamSynchronize(s));  // (the host vectors go out of scope)
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1354,6 +1537,60 @@ int sgdml_b200_pimd_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_p
   return md_create(out, m, n_poly * n_beads, (int)n_beads, inv_mass);
 }
 
+int sgdml_b200_npt_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, const double* inv_mass,
+                          const double* lattices, const double* lattice_invs) {
+  SG_TRY(require_device());
+  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
+  SG_ARG(n_rep >= 1 && n_rep <= INT32_MAX);
+  std::vector<NptCell> cells;
+  std::vector<Lattice> lats;
+  SG_TRY(npt_parse(lattices, lattice_invs, n_rep, &cells, &lats));
+  sgdml_b200_md* md = nullptr;
+  SG_TRY(md_create(&md, m, n_rep, 1, inv_mass));
+  auto body = [&]() -> int {
+    SG_CUDA(cached_malloc(&md->cell, sizeof(NptCell) * (size_t)n_rep));
+    SG_CUDA(cached_malloc(&md->lat, sizeof(Lattice) * (size_t)n_rep));
+    SG_CUDA(cached_malloc(&md->W, sizeof(double) * 9 * (size_t)n_rep));
+    SG_CUDA(cached_malloc(&md->Ws, sizeof(double) * 9 * (size_t)n_rep));
+    SG_CUDA(cudaMemset(md->W, 0, sizeof(double) * 9 * (size_t)n_rep));
+    return npt_install(md, cells, lats, 0);
+  };
+  const int rc = body();
+  if (rc != 0) {
+    md_free(md);
+    return rc;
+  }
+  *out = md;
+  return 0;
+}
+
+int sgdml_b200_npt_set_cells(sgdml_b200_md* md, const double* lattices, const double* lattice_invs, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr);
+  if (md->cell == nullptr) return fail_arg("sgdml_b200_npt_set_cells needs an NPT handle (sgdml_b200_npt_create)");
+  std::vector<NptCell> cells;
+  std::vector<Lattice> lats;
+  SG_TRY(npt_parse(lattices, lattice_invs, md->n_rep, &cells, &lats));
+  return npt_install(md, cells, lats, (cudaStream_t)stream);
+}
+
+int sgdml_b200_npt_get_cells(sgdml_b200_md* md, double* lattices, double* lattice_invs, double* W, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr);
+  if (md->cell == nullptr) return fail_arg("sgdml_b200_npt_get_cells needs an NPT handle (sgdml_b200_npt_create)");
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t row = 9 * sizeof(double), n = (size_t)md->n_rep;
+  Outputs out(s);
+  SG_TRY(out.init({{lattices, row * n}, {lattice_invs, row * n}, {W, row * n}}));
+  const char* base = reinterpret_cast<const char*>(md->lat);
+  const size_t off[2] = {offsetof(Lattice, vec), offsetof(Lattice, inv)};
+  for (int k = 0; k < 2; ++k)
+    if (out.dev(k) != nullptr)
+      SG_CUDA(cudaMemcpy2DAsync(out.dev(k), row, base + off[k], sizeof(Lattice), row, n, cudaMemcpyDeviceToDevice, s));
+  SG_TRY(out.copy_from(2, {md->W}));
+  return out.finish();
+}
+
 int sgdml_b200_md_destroy(sgdml_b200_md* md) {
   if (md != nullptr) md_free(md);
   return 0;
@@ -1372,7 +1609,7 @@ int sgdml_b200_md_set_state(sgdml_b200_md* md, const double* R, const double* V,
     SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
   const std::vector<uint64_t> steps((size_t)md->n_rep, step);
   SG_CUDA(cudaMemcpyAsync(md->step, steps.data(), sizeof(uint64_t) * md->n_rep, cudaMemcpyHostToDevice, s));
-  SG_TRY(force_eval_run(md->fe, md->R, md->F, md->E, s));
+  SG_TRY(md_forces(md, md->F, md->E, md->W, s));
   if (md->walker != nullptr) {  // a replica exchange's walkers start again from their slots
     k_remd_identity<<<(unsigned)((md->n_rep + 255) / 256), 256, 0, s>>>(md->walker, md->n_rep);
     SG_CUDA(cudaGetLastError());
@@ -1406,7 +1643,26 @@ int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamm
     return fail_arg("sgdml_b200_md_run: a ring-polymer handle (n_beads > 1) runs with sgdml_b200_pimd_run");
   SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
   void* const outs[N_RUN_OUTS] = {R_frames, V_frames, E_pot_frames, E_kin_frames};
-  return md_run(md, MD_CLASSICAL, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, outs, nullptr, (cudaStream_t)stream);
+  return md_run(md, MD_CLASSICAL, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, outs, nullptr, nullptr,
+                (cudaStream_t)stream);
+}
+
+int sgdml_b200_npt_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, double P0,
+                       double beta_T, double tau_p, uint64_t seed, int64_t stride, double* R_frames,
+                       double* V_frames, double* E_pot_frames, double* E_kin_frames, double* cell_frames,
+                       double* P_frames, void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(run_check(md, n_steps, dt, kT, gamma, stride, "sgdml_b200_npt_run: no state yet (call sgdml_b200_md_set_state)",
+                   true));
+  SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
+  SG_ARG(std::isfinite(P0));
+  SG_ARG(std::isfinite(beta_T) && beta_T >= 0.0);
+  SG_ARG(std::isfinite(tau_p) && tau_p > 0.0);
+  const NptRun b = {P0, beta_T, tau_p};
+  void* outs[N_RUN_OUTS] = {R_frames, V_frames, E_pot_frames, E_kin_frames};
+  outs[OUT_CELL] = cell_frames;
+  outs[OUT_PRESS] = P_frames;
+  return md_run(md, MD_NPT, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, outs, nullptr, &b, (cudaStream_t)stream);
 }
 
 int sgdml_b200_remd_run(sgdml_b200_md* md, int64_t n_temps, const double* kT, int64_t n_steps, double dt, double gamma,
@@ -1427,7 +1683,8 @@ int sgdml_b200_remd_run(sgdml_b200_md* md, int64_t n_temps, const double* kT, in
   const RemdRun x = {(int)n_temps, kT, exchange_every};
   void* const outs[N_RUN_OUTS] = {R_frames,      V_frames,    E_pot_frames, E_kin_frames, nullptr,
                                   nullptr,       walker_frames, walkers_out, n_accepted,   n_attempted};
-  return md_run(md, MD_REMD, n_steps, dt, kT[0], 0.0, gamma, 0.0, seed, stride, outs, &x, (cudaStream_t)stream);
+  return md_run(md, MD_REMD, n_steps, dt, kT[0], 0.0, gamma, 0.0, seed, stride, outs, &x, nullptr,
+                (cudaStream_t)stream);
 }
 
 int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma,
@@ -1442,7 +1699,7 @@ int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT
   SG_ARG(std::isfinite(lambda) && lambda >= 0.0);
   if (md->nb > 1 && kT == 0.0) return fail_arg("a ring polymer (n_beads > 1) needs kT > 0");
   void* const outs[N_RUN_OUTS] = {R_frames, V_frames, E_pot_frames, E_kin_frames, K_prim_frames, K_cv_frames};
-  return md_run(md, MD_RING_POLYMER, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, outs, nullptr,
+  return md_run(md, MD_RING_POLYMER, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, outs, nullptr, nullptr,
                 (cudaStream_t)stream);
 }
 

@@ -1,6 +1,7 @@
-// Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_pimd_*, sgdml_b200_relax_*,
-// sgdml_b200_neb_fire): the contract of the kernels in md.cu -- the BAOAB integrator step, the replica exchange, the
-// ring-polymer step, their counter-based noise, the FIRE and L-BFGS steps, and the nudged elastic band.
+// Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_pimd_*,
+// sgdml_b200_relax_*, sgdml_b200_neb_fire): the contract of the kernels in md.cu -- the BAOAB integrator step, the
+// replica exchange, the NPT step, the ring-polymer step, their counter-based noise, the FIRE and L-BFGS steps, and the
+// nudged elastic band.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -55,6 +56,41 @@ struct RemdParams {
 //   w = v + h (F s)  (k_md_step's rounding),  v' = lam w - h (F s)
 // with the configuration's own F.  n_att and n_acc of the pair count the attempt and the acceptance.  On a frame step
 // of k_md_step (the same rule) the CTA writes the ladder's walker labels after the swaps into W_f.
+
+// Constant-pressure MD (sgdml_b200_npt_run): an NPT handle (sgdml_b200_npt_create) is an MD handle whose replica rep
+// lives in a cell of its own, isotropically scaled by the stochastic cell rescaling barostat (Bernetti & Bussi,
+// J. Chem. Phys. 153, 114107 (2020)).  Per replica, in device memory:
+struct NptCell {
+  double eps;              // log of the volume ratio V / V0 since the cell was set
+  double V0;               // |det L0|, computed on the host
+  double L0[9], L0inv[9];  // the base cell (lattice vectors as columns, row-major) and the inverse the caller gave
+};
+// The cell the descriptor kernel reads is the Lattice L = a L0, L^-1 = L0^-1 / a with a = exp(eps / 3) (each entry one
+// product or quotient), so it never drifts from its inverse.  W (n_rep, 9) holds the virial of the current state,
+// written with F and E by force_eval_run_cells (predict.cuh).
+struct NptParams {
+  double P0;              // target pressure (energy / L^3)
+  double c_a;             // (beta_T / tau_p) dt, on the host
+  double c_b;             // 2 kT (beta_T / tau_p) dt, on the host (0: no draws)
+  double *cell_f, *P_f;   // frames (n_frames, n_rep, 9) / (n_frames, n_rep), or null
+};
+
+// k_npt_step: one CTA of MD_THREADS per replica, k_md_step's counter, run_start and stride rules (MdParams; sigma row
+// 0).  With the replica's counter at n:
+//   1. if n != run_start:  v += h (F s), as k_md_step; on a frame step R, full-step V, E_pot, E_kin as k_md_step, the
+//      cell a L0 (the Lattice's vectors) and P_int of step 2
+//   2. K = 1/2 sum_i v_i^2 / s_i in k_md_step's E_kin order (on every step);  V = V0 exp(eps);
+//      P_int = (2 K + ((W_0 + W_4) + W_8)) / (3 V), rounded as written
+//   3. if advance:  de = -c_a (P0 - P_int) + sqrt(c_b / V) eta, rounded as written (c_b == 0: the first term only,
+//      no draw); eta = sqrt(-2 ln U_a) cos(2 pi U_b) from Philox4x32-10 under the run's key with counter
+//      (0xFFFFFFFF, rep, n mod 2^32, n >> 32), U_a and U_b as k_md_step's.  That first counter word is above every O
+//      pair index (< 2^31) and every exchange word (0x80000000 | k, k <= 2^31 - 3).
+//   4. if advance:  B, A, O, A exactly as k_md_step (one copy of the update, its noise), then mu = exp(de / 3),
+//      r = r mu, v = v / mu, eps = eps + de, the new Lattice, and the counter becomes n + 1
+// The driver then evaluates F, E and W at the new positions in the new cells; the next launch's first action is the
+// pending half-kick with those forces.
+// Drift: velocities scaled by 1 / mu keep dr dp, and with the instantaneous K in P_int the Ito drift that leaves
+// exp(-beta (H + P0 V)) dr dp dV stationary carries no kT / V term (DESIGN.md 4.1.7 has the derivation).
 
 // Path-integral MD (sgdml_b200_pimd_run): replica p P + j is bead j of ring polymer p.
 constexpr int PIMD_MAX_BEADS = 64;  // C (P x P) sits in shared memory: 32 KB at the cap

@@ -1776,6 +1776,17 @@ int refresh_row_dots(sgdml_b200_model* m, bool with_mm, cudaStream_t s) {
 
 }  // namespace
 
+// A cell given to sgdml_b200_predict_virial: host arrays (lattice_from_host), finite, and not singular
+int sgdml::check_cell(const Lattice& l) {
+  for (int i = 0; i < 9; ++i)
+    if (!std::isfinite(l.vec[i]) || !std::isfinite(l.inv[i])) return fail_arg("the cell must be finite");
+  const double* a = l.vec;
+  const double det = a[0] * (a[4] * a[8] - a[5] * a[7]) - a[1] * (a[3] * a[8] - a[5] * a[6]) +
+                     a[2] * (a[3] * a[7] - a[4] * a[6]);
+  if (!(det != 0.0)) return fail_arg("the cell is singular");
+  return 0;
+}
+
 extern "C" {
 
 int sgdml_b200_model_create(sgdml_b200_model** out, int64_t n_atoms, int64_t n_train, int64_t n_perms,
@@ -2061,16 +2072,6 @@ int predict_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, const Latt
   return 0;
 }
 
-// A cell given to sgdml_b200_predict_virial: host arrays (lattice_from_host), finite, and not singular
-int check_cell(const Lattice& l) {
-  for (int i = 0; i < 9; ++i)
-    if (!std::isfinite(l.vec[i]) || !std::isfinite(l.inv[i])) return fail_arg("the cell must be finite");
-  const double* a = l.vec;
-  const double det = a[0] * (a[4] * a[8] - a[5] * a[7]) - a[1] * (a[3] * a[8] - a[5] * a[6]) +
-                     a[2] * (a[3] * a[7] - a[4] * a[6]);
-  if (!(det != 0.0)) return fail_arg("the cell is singular");
-  return 0;
-}
 int lattice_for_call(const double* lattice, const double* lattice_inv, Lattice* l) {
   SG_TRY(lattice_from_host(lattice, lattice_inv, l));
   if (!l->on) return 0;
@@ -2546,6 +2547,20 @@ int sgdml::force_eval_run(ForceEval* fe, const double* R, double* F, double* E, 
     const int64_t ng = std::min<int64_t>(fe->chunk, fe->n_geo - g0);
     SG_TRY(launch_desc_from_R(R + g0 * dimi, ng, m->N, w.xq, w.gq, s, m->lat, nullptr));
     SG_TRY(run_queries(m, w, w.xq, w.gq, ng, m->std, m->c, E + g0, F + g0 * dimi, s));
+  }
+  return 0;
+}
+
+// predict_impl's chunk for device-resident R with one cell per geometry, on the evaluator's workspace
+int sgdml::force_eval_run_cells(ForceEval* fe, const double* R, const Lattice* cells, double* F, double* E, double* W,
+                                cudaStream_t s) {
+  sgdml_b200_model* m = fe->m;
+  sgdml_b200_model::WS& w = fe->ws;
+  const int dimi = 3 * m->N;
+  for (int64_t g0 = 0; g0 < fe->n_geo; g0 += fe->chunk) {
+    const int64_t ng = std::min<int64_t>(fe->chunk, fe->n_geo - g0);
+    SG_TRY(launch_desc_from_R(R + g0 * dimi, ng, m->N, w.xq, w.gq, s, m->lat, cells + g0));
+    SG_TRY(run_queries(m, w, w.xq, w.gq, ng, m->std, m->c, E + g0, F + g0 * dimi, s, W + 9 * g0));
   }
   return 0;
 }

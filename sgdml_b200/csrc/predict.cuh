@@ -3,6 +3,7 @@
 // sgdml_b200_model stays private to predict.cu.
 #pragma once
 #include "common.cuh"
+#include "desc.cuh"
 
 namespace sgdml {
 
@@ -56,5 +57,13 @@ bool force_eval_stale(const ForceEval* fe);
 void force_eval_mark(ForceEval* fe);
 // R (n_geo, 3N) -> F (n_geo, 3N), E (n_geo), all device arrays; chunk by chunk when n_geo exceeds the predictor's chunk
 int force_eval_run(ForceEval* fe, const double* R, double* F, double* E, cudaStream_t s);
+// As force_eval_run, with geometry g in its own cell cells[g] (n_geo cells in DEVICE memory), also writing the virial
+// W (n_geo, 9): bit for bit what sgdml_b200_predict_virial_cells returns for device-resident R in the same cells
+int force_eval_run_cells(ForceEval* fe, const double* R, const Lattice* cells, double* F, double* E, double* W,
+                         cudaStream_t s);
+
+// The rule for a caller's periodic cell (sgdml_b200_predict_virial*): every entry of the cell and of its inverse finite,
+// and the cell not singular.  0, or an argument error with the last-error message set.
+int check_cell(const Lattice& l);
 
 }  // namespace sgdml

@@ -8,6 +8,9 @@ with the primitive and centroid-virial quantum kinetic-energy estimators.
 (``sgdml_b200_remd_run``): ladders of Langevin replicas at fixed temperatures whose neighbours swap configurations by a
 Metropolis test inside the step graph.
 
+``GDMLNPTDynamics`` -- constant-pressure MD of periodic models on the same engine (``sgdml_b200_npt_*``): Langevin
+replicas, each in a cell of its own that an isotropic stochastic cell rescaling barostat scales.
+
 ``GDMLRelaxation`` -- geometry optimisation of many replicas on the same engine (``sgdml_b200_relax_*``): FIRE and
 L-BFGS, each replica frozen once it has converged.
 
@@ -142,11 +145,12 @@ class GDMLDynamics(object):
         return {'R': R, 'V': V, 'F': F, 'E_pot': E, 'step': int(step[0])}
 
     def _frames(self, n_steps, stride, frames, n_poly=0):
-        """Empty frame arrays for the names in `frames`: (n_frames, n_replicas, 3N) for R and V, (n_frames, n_poly) for
-        K_prim and K_cv, else (n_frames, n_replicas), int32 for the walker labels; {} when the run writes no frames."""
+        """Empty frame arrays for the names in `frames`: (n_frames, n_replicas, 3N) for R and V, (n_frames, n_replicas, 9)
+        for the NPT cells, (n_frames, n_poly) for K_prim and K_cv, else (n_frames, n_replicas), int32 for the walker
+        labels; {} when the run writes no frames."""
         n_frames = n_steps // stride if stride > 0 and n_steps % stride == 0 else 0
         dims = {'R': (self.n_replicas, 3 * self.n_atoms), 'V': (self.n_replicas, 3 * self.n_atoms), 'K_prim': (n_poly,),
-                'K_cv': (n_poly,)}
+                'K_cv': (n_poly,), 'cell': (self.n_replicas, 9)}
         return {k: self._empty((n_frames,) + dims.get(k, (self.n_replicas,)), np.int32 if k == 'walker' else np.float64)
                 for k in frames} if n_frames > 0 else {}
 
@@ -359,6 +363,128 @@ class GDMLReplicaExchange(GDMLDynamics):
         if 'walker' in f:
             out['walker'] = f['walker'].reshape((f['walker'].shape[0],) + self._shape)
         return out
+
+
+class GDMLNPTDynamics(GDMLDynamics):
+    """Constant-pressure (NPT) molecular dynamics of `n_replicas` replicas of a periodic model, in the units of
+    ``GDMLDynamics``: BAOAB Langevin with the isotropic stochastic cell rescaling barostat of Bernetti & Bussi
+    (J. Chem. Phys. 153, 114107 (2020)).  Every replica lives in a cell of its own, which the barostat scales with the
+    positions; the step, the forces and the virial run on the device, with no host round trip per step.
+
+    cells: (n_replicas, 3, 3) or (3, 3) in Angstrom with the lattice vectors as ROWS (ASE's ``atoms.cell``); None: the
+    model's own cell for every replica (a free-molecule model has none and raises).  NumPy arrays or torch tensors.
+    ``set_state(positions, velocities=None, step=0)`` as ``GDMLDynamics``'s; forces, energies and stresses are
+    evaluated in each replica's cell.  ``set_cells(cells)`` replaces the cells (positions do not move).
+    ``get_state()`` adds 'cells' (n_replicas, 3, 3) and 'stress' (n_replicas, 6), -W / V in eV/Angstrom^3 in Voigt
+    order (xx, yy, zz, yz, xz, xy), the calculator's 'stress'.
+    ``run(n_steps, dt_fs, temperature_K, friction_per_fs, pressure_au, compressibility_au, taup_fs, seed=0, stride=0)``
+    integrates at the target pressure (eV/Angstrom^3) with the isothermal compressibility (Angstrom^3/eV) and barostat
+    time constant taup_fs, the names and units of ASE's barostats; zero compressibility keeps every cell fixed.  It
+    returns ``GDMLDynamics.run``'s frames plus 'cells' (n_frames, n_replicas, 3, 3), 'volume' (Angstrom^3) and
+    'pressure' (eV/Angstrom^3, the instantaneous (2 E_kin + tr W) / 3V), (n_frames, n_replicas).  NumPy arrays or
+    float64 CUDA tensors in, the same kind out.  Positions are never wrapped into the cell."""
+
+    def __init__(self, model, masses, cells=None, n_replicas=1, E_to_eV=_KCAL_PER_MOL_IN_EV,
+                 F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        self._cells_arg = cells
+        super().__init__(model, masses, n_replicas, E_to_eV, F_to_eV_Ang)
+
+    def _raw_cells(self, cells):
+        """cells in Angstrom (rows), or None -> (lattices, inverses) (n_replicas, 9) in model units (columns)."""
+        n = self.n_replicas
+        if cells is None:
+            if self.gdml_predict.lat_and_inv is None:
+                raise ValueError('a free-molecule model has no cell: pass cells (Angstrom, vectors as rows)')
+            lat, inv = self.gdml_predict.lat_and_inv
+            return (np.ascontiguousarray(np.broadcast_to(np.asarray(lat, dtype=np.float64).reshape(1, 9), (n, 9))),
+                    np.ascontiguousarray(np.broadcast_to(np.asarray(inv, dtype=np.float64).reshape(1, 9), (n, 9))))
+        c = cells.detach().cpu().numpy() if hasattr(cells, 'data_ptr') else cells
+        c = np.asarray(c, dtype=np.float64)
+        if c.shape == (3, 3):
+            c = np.broadcast_to(c, (n, 3, 3))
+        if c.shape != (n, 3, 3):
+            raise ValueError('cells must be (n_replicas, 3, 3) or (3, 3) = (%d, 3, 3): %s' % (n, c.shape))
+        lat = np.ascontiguousarray(c.swapaxes(-1, -2) * self.Ang_to_R)
+        return lat.reshape(n, 9), np.ascontiguousarray(np.linalg.inv(lat)).reshape(n, 9)
+
+    def _create_handle(self):
+        lat, inv = self._raw_cells(self._cells_arg)
+        handle = ctypes.c_void_p()
+        _lib.check(
+            _lib.lib().sgdml_b200_npt_create(ctypes.byref(handle), self.gdml_predict._handle, self.n_replicas,
+                                             _lib.ptr(self.inv_mass), _lib.ptr(lat), _lib.ptr(inv)),
+            'npt_create',
+        )
+        return handle
+
+    # ------------------------------------------------------------------ model units (L, model energy, fs)
+    def _set_cells_raw(self, lattices, lattice_invs):
+        """(n_replicas, 9) HOST arrays each, model units, vectors as columns."""
+        lat = np.ascontiguousarray(lattices, dtype=np.float64)
+        inv = np.ascontiguousarray(lattice_invs, dtype=np.float64)
+        if lat.size != 9 * self.n_replicas or inv.size != 9 * self.n_replicas:
+            raise ValueError('lattices and lattice_invs must hold n_replicas x 9 values each: %d' % self.n_replicas)
+        _lib.check(_lib.lib().sgdml_b200_npt_set_cells(self._handle, _lib.ptr(lat), _lib.ptr(inv),
+                                                       _lib.current_stream()), 'npt_set_cells')
+
+    def _get_cells_raw(self):
+        """{'lattice', 'lattice_inv', 'W'}: (n_replicas, 9) each, model units."""
+        out = {k: self._empty((self.n_replicas, 9)) for k in ('lattice', 'lattice_inv', 'W')}
+        _lib.check(
+            _lib.lib().sgdml_b200_npt_get_cells(self._handle, *(_lib.ptr(out[k]) for k in ('lattice', 'lattice_inv', 'W')),
+                                                _lib.current_stream()),
+            'npt_get_cells',
+        )
+        return out
+
+    def _run_raw(self, n_steps, dt, gamma, kT, P0, beta_T, tau_p, seed=0, stride=0,
+                 frames=('R', 'V', 'E_pot', 'E_kin', 'cell', 'P')):
+        n_steps, stride = int(n_steps), int(stride)
+        out = self._frames(n_steps, stride, frames)
+        _lib.check(
+            _lib.lib().sgdml_b200_npt_run(self._handle, n_steps, float(dt), float(gamma), float(kT), float(P0),
+                                          float(beta_T), float(tau_p), int(seed), stride,
+                                          *(_lib.ptr(out.get(k)) for k in ('R', 'V', 'E_pot', 'E_kin', 'cell', 'P')),
+                                          _lib.current_stream()),
+            'npt_run',
+        )
+        return out
+
+    # ------------------------------------------------------------------ ASE units
+    def _ase_cells(self, lat):
+        """(..., 9) model-unit lattices (columns) -> (..., 3, 3) Angstrom cells (rows) and their volumes (...)."""
+        c = lat.reshape(lat.shape[:-1] + (3, 3)).swapaxes(-1, -2) / self.Ang_to_R
+        return c, abs(_det3(c))
+
+    def set_cells(self, cells):
+        self._set_cells_raw(*self._raw_cells(cells))
+
+    def get_state(self):
+        out = super().get_state()
+        c = self._get_cells_raw()
+        cells, vol = self._ase_cells(c['lattice'])
+        s = -c['W'].reshape(-1, 3, 3) * self.E_to_eV / vol.reshape(-1, 1, 1)
+        out.update(cells=cells, stress=s[:, [0, 1, 2, 1, 0, 0], [0, 1, 2, 2, 2, 1]])
+        return out
+
+    def run(self, n_steps, dt_fs, temperature_K, friction_per_fs, pressure_au, compressibility_au, taup_fs, seed=0,
+            stride=0):
+        kT = KB_EV * float(temperature_K) / self.E_to_eV
+        vol_unit = self.Ang_to_R**3  # Angstrom^3 -> L^3
+        f = self._run_raw(n_steps, dt_fs, friction_per_fs, kT, float(pressure_au) / (self.E_to_eV * vol_unit),
+                          float(compressibility_au) * self.E_to_eV * vol_unit, taup_fs, seed, stride)
+        out = self._ase_frames(f)
+        if 'cell' in f:
+            out['cells'], out['volume'] = self._ase_cells(f['cell'])
+            out['pressure'] = f['P'] * (self.E_to_eV * vol_unit)
+        return out
+
+
+def _det3(a):
+    """det of (..., 3, 3) NumPy arrays or torch tensors, by cofactors of the first row."""
+    return (a[..., 0, 0] * (a[..., 1, 1] * a[..., 2, 2] - a[..., 1, 2] * a[..., 2, 1])
+            - a[..., 0, 1] * (a[..., 1, 0] * a[..., 2, 2] - a[..., 1, 2] * a[..., 2, 0])
+            + a[..., 0, 2] * (a[..., 1, 0] * a[..., 2, 1] - a[..., 1, 1] * a[..., 2, 0]))
 
 
 class GDMLRelaxation(GDMLDynamics):

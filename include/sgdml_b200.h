@@ -261,6 +261,51 @@ int sgdml_b200_npt_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gam
                        double* V_frames, double* E_pot_frames, double* E_kin_frames, double* cell_frames,
                        double* P_frames, void* stream);
 
+/* ---------------------------------------------------------------- metadynamics on the device
+ * Extension: well-tempered multiple-walker metadynamics (Raiteri et al., J. Phys. Chem. B 110, 3533 (2006); Barducci,
+ * Bussi & Parrinello, PRL 100, 020603 (2008)) on 1 to 4 collective variables (CVs).  A metadynamics handle is an
+ * sgdml_b200_md handle of n_rep = n_groups n_walkers replicas, replica g n_walkers + w walker w of group g, each
+ * integrated by sgdml_b200_md_run's BAOAB step with the force F = F_model + F_bias.  The walkers of a group deposit
+ * Gaussian hills into one store and are biased by its sum V(s) = sum_k h_k exp(-sum_j (s_j - c_kj)^2 / (2 w_kj^2));
+ * groups never see each other's hills.  CVs (cv_type[j], atoms cv_atoms[4 j ...]): 0 distance |r_j - r_i| (atoms
+ * i, j), 1 angle atan2(|a x b|, a.b) with a = r_i - r_j, b = r_k - r_j, in [0, pi] (atoms i, j, k), 2 dihedral
+ * atan2(|b2| b1.(b2 x b3), (b1 x b2).(b2 x b3)), b1 = r_j - r_i, b2 = r_k - r_j, b3 = r_l - r_k, in (-pi, pi]
+ * (atoms i, j, k, l), on plain coordinate differences (no minimum image; positions are never wrapped).  A dihedral's
+ * hill difference is wrapped into [-pi, pi).  The formulas, their roundings and gradients are in csrc/md.cuh.
+ * Deposition: inside a run, walker w deposits on every state c > the run's first with c % pace == 0 a hill centred on
+ * its CVs, with the run's widths and height w0 exp(-V(s) / dkT) (w0 with dkT = +INFINITY: plain metadynamics).  Every
+ * walker of a group is biased by the same hills, those committed before state c: a hill becomes visible to the
+ * evaluation of the next state, never to its own.  sgdml_b200_md_set_state evaluates the model and then the bias
+ * without a deposit, so a run continued over several calls is one long run.  sgdml_b200_md_get_state's F and E_pot
+ * stay the model's.  sgdml_b200_md_run, _remd_run, _pimd_run, _npt_run, _relax_* and _neb_fire on a metadynamics
+ * handle are argument errors, as are the sgdml_b200_metad_* calls on any other handle.  Streams, host/device outputs,
+ * SGDML_B200_GRAPH=0 and the workspace are those of sgdml_b200_md_run; argument errors are reported before anything
+ * is queued, and a rejected call changes nothing. */
+/* n_groups, n_walkers >= 1, n_groups n_walkers <= INT32_MAX; 1 <= n_cv <= 4; cv_type (n_cv) and cv_atoms (n_cv, 4)
+ * HOST arrays, the atoms of each CV distinct and in [0, N) (unused entries ignored); inv_mass as sgdml_b200_md_create. */
+int sgdml_b200_metad_create(sgdml_b200_md** out, sgdml_b200_model* model, int64_t n_groups, int64_t n_walkers,
+                            const double* inv_mass, int64_t n_cv, const int* cv_type, const int64_t* cv_atoms);
+/* n_steps, dt, gamma, kT, seed and stride as sgdml_b200_md_run; w0 finite and >= 0 (energy); widths (n_cv) HOST, each
+ * finite and > 0 (L or radians); pace >= 1; dkT > 0, finite or +INFINITY (energy).  Frames: R, V, E_pot (the model's),
+ * E_kin as sgdml_b200_md_run; cv_frames (n_frames, n_rep, n_cv) and bias_frames (n_frames, n_rep) the CVs and bias
+ * energy of the frame's state (before its deposit).  Each may be NULL.  Needs a state.  The hill store grows before
+ * anything is queued to hold the run's n_walkers #{c in (start, start + n_steps] : c % pace == 0} new hills per group. */
+int sgdml_b200_metad_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, double w0,
+                         const double* widths, int64_t pace, double dkT, uint64_t seed, int64_t stride,
+                         double* R_frames, double* V_frames, double* E_pot_frames, double* E_kin_frames,
+                         double* cv_frames, double* bias_frames, void* stream);
+/* n_hills (n_groups) HOST int64: the hills of each group; centers, widths (H, n_cv) and heights (H), H = sum n_hills,
+ * group after group in deposition order; each may be NULL. */
+int sgdml_b200_metad_get_hills(sgdml_b200_md* md, int64_t* n_hills, double* centers, double* widths, double* heights,
+                               void* stream);
+/* Replaces every group's hills, laid out as sgdml_b200_metad_get_hills gives them (HOST arrays; every centre and height
+ * finite, every width finite and > 0), and re-evaluates the bias of the state when the handle has one. */
+int sgdml_b200_metad_set_hills(sgdml_b200_md* md, const int64_t* n_hills, const double* centers, const double* widths,
+                               const double* heights, void* stream);
+/* cv (n_rep, n_cv), V_bias (n_rep) and F_bias (n_rep, 3N): the CVs, bias energy and bias force of the state; any may be
+ * NULL.  Needs a state. */
+int sgdml_b200_metad_get_bias(sgdml_b200_md* md, double* cv, double* V_bias, double* F_bias, void* stream);
+
 /* ---------------------------------------------------------------- path-integral molecular dynamics on the device
  * Extension: ring polymers of P beads (1 <= P <= 64), thermostatted mode by mode with PILE-L (Ceriotti, Parrinello,
  * Markland & Manolopoulos, J. Chem. Phys. 133, 124104 (2010)) in the BAOAB order of Liu, Li & Liu (J. Chem. Phys. 145,

@@ -63,6 +63,15 @@ SIGNATURES = {
         [c_void_p, i64, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_uint64, i64,
          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     ),
+    'sgdml_b200_metad_create': (C.c_int, [C.POINTER(c_void_p), c_void_p, i64, i64, c_void_p, i64, c_void_p, c_void_p]),
+    'sgdml_b200_metad_run': (
+        C.c_int,
+        [c_void_p, i64, C.c_double, C.c_double, C.c_double, C.c_double, c_void_p, i64, C.c_double, C.c_uint64, i64,
+         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
+    'sgdml_b200_metad_get_hills': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_metad_set_hills': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_metad_get_bias': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_pimd_create': (C.c_int, [C.POINTER(c_void_p), c_void_p, i64, i64, c_void_p]),
     'sgdml_b200_pimd_run': (
         C.c_int,

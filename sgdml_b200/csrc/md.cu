@@ -1,7 +1,7 @@
-// Molecular dynamics, replica exchange, path-integral MD and geometry optimisation on the device: the integrator,
-// exchange and optimiser kernels (contract in md.cuh), then the driver of sgdml_b200_md_*, sgdml_b200_remd_run,
-// sgdml_b200_pimd_*, sgdml_b200_relax_* and sgdml_b200_neb_fire, which evaluates forces through the predictor interface
-// of predict.cuh.
+// Molecular dynamics, replica exchange, metadynamics, path-integral MD and geometry optimisation on the device: the
+// integrator, exchange, bias and optimiser kernels (contract in md.cuh), then the driver of sgdml_b200_md_*,
+// sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_metad_*, sgdml_b200_pimd_*, sgdml_b200_relax_* and
+// sgdml_b200_neb_fire, which evaluates forces through the predictor interface of predict.cuh.
 //
 // The BAOAB Langevin integrator step of sgdml_b200_md_run.
 //
@@ -811,6 +811,185 @@ __global__ void k_relax_report(const RelaxState* __restrict__ st, int64_t n_rep,
   if (fmax) fmax[r] = sqrt(st[r].fmax2);
 }
 
+// ---------------------------------------------------------------------------------- metadynamics
+// The CVs, the hill sum and the deposit of sgdml_b200_metad_run (contract in md.cuh).  Every operation rounds as
+// written there.
+
+__device__ __forceinline__ void sub3(double o[3], const double* a, const double* b) {
+  for (int x = 0; x < 3; ++x) o[x] = __dsub_rn(a[x], b[x]);
+}
+__device__ __forceinline__ double dot3(const double* a, const double* b) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(a[0], b[0]), __dmul_rn(a[1], b[1])), __dmul_rn(a[2], b[2]));
+}
+__device__ __forceinline__ void cross3(double o[3], const double* a, const double* b) {
+  o[0] = __dsub_rn(__dmul_rn(a[1], b[2]), __dmul_rn(a[2], b[1]));
+  o[1] = __dsub_rn(__dmul_rn(a[2], b[0]), __dmul_rn(a[0], b[2]));
+  o[2] = __dsub_rn(__dmul_rn(a[0], b[1]), __dmul_rn(a[1], b[0]));
+}
+
+// CV of `type` on atoms at of the replica's positions r: its value, and g (4 x 3) its gradient per atom slot
+__device__ void cv_eval(int type, const int* at, const double* r, double* sv, double g[4][3]) {
+  for (int p = 0; p < 4; ++p)
+    for (int x = 0; x < 3; ++x) g[p][x] = 0.0;
+  const double *ri = r + 3 * at[0], *rj = r + 3 * at[1], *rk = r + 3 * at[2], *rl = r + 3 * at[3];
+  if (type == CV_DISTANCE) {
+    double d[3];
+    sub3(d, rj, ri);
+    const double s = sqrt(dot3(d, d));
+    *sv = s;
+    if (s != 0.0)
+      for (int x = 0; x < 3; ++x) {
+        g[1][x] = __ddiv_rn(d[x], s);
+        g[0][x] = -g[1][x];
+      }
+  } else if (type == CV_ANGLE) {
+    double a[3], b[3], c[3];
+    sub3(a, ri, rj);
+    sub3(b, rk, rj);
+    cross3(c, a, b);
+    const double cn = sqrt(dot3(c, c));
+    *sv = atan2(cn, dot3(a, b));
+    if (cn != 0.0) {
+      double ac[3], cb[3];
+      cross3(ac, a, c);
+      cross3(cb, c, b);
+      const double da = __dmul_rn(dot3(a, a), cn), db = __dmul_rn(dot3(b, b), cn);
+      for (int x = 0; x < 3; ++x) {
+        g[0][x] = __ddiv_rn(ac[x], da);
+        g[2][x] = __ddiv_rn(cb[x], db);
+        g[1][x] = -__dadd_rn(g[0][x], g[2][x]);
+      }
+    }
+  } else {
+    double b1[3], b2[3], b3[3], m[3], n[3];
+    sub3(b1, rj, ri);
+    sub3(b2, rk, rj);
+    sub3(b3, rl, rk);
+    cross3(m, b1, b2);
+    cross3(n, b2, b3);
+    const double nb = sqrt(dot3(b2, b2));
+    *sv = atan2(__dmul_rn(nb, dot3(b1, n)), dot3(m, n));
+    const double mm = dot3(m, m), nn = dot3(n, n), bb = dot3(b2, b2);
+    if (mm != 0.0 && nn != 0.0) {
+      const double fi = __ddiv_rn(nb, mm), fl = __ddiv_rn(nb, nn);
+      const double p = __ddiv_rn(dot3(b1, b2), bb), q = __ddiv_rn(dot3(b3, b2), bb);
+      for (int x = 0; x < 3; ++x) {
+        const double gi = -__dmul_rn(fi, m[x]), gl = __dmul_rn(fl, n[x]);
+        const double t = __dsub_rn(__dmul_rn(p, gi), __dmul_rn(q, gl));
+        g[0][x] = gi;
+        g[1][x] = -__dadd_rn(gi, t);
+        g[2][x] = __dsub_rn(t, gl);
+        g[3][x] = gl;
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(MD_THREADS) k_metad_bias(const MetadParams* __restrict__ Q,
+                                                          const MdParams* __restrict__ P,
+                                                          const double* __restrict__ R, const double* __restrict__ Fm,
+                                                          double* __restrict__ F, const uint64_t* __restrict__ step,
+                                                          int dimi, int deposit) {
+  __shared__ double red[MD_THREADS];
+  __shared__ double s_cv[MD_MAX_CV], s_dv[MD_MAX_CV];
+  __shared__ double s_g[MD_MAX_CV][4][3];
+  const MetadParams& q = *Q;
+  const int n_cv = q.n_cv, nw = q.n_walkers;
+  const int64_t rep = blockIdx.x, n_rep = gridDim.x, grp = rep / nw, w = rep % nw;
+  const uint64_t c = step[rep];
+  const uint64_t run_start = P->run_start;
+  const double* r = R + rep * dimi;
+  const int tid = threadIdx.x;
+  if (tid < n_cv) cv_eval(q.type[tid], q.atoms[tid], r, &s_cv[tid], s_g[tid]);
+  __syncthreads();
+  const uint64_t pace = (uint64_t)q.pace;
+  const int64_t n_g = q.count[grp] + (deposit ? (int64_t)nw * (int64_t)((c - 1) / pace - run_start / pace) : 0);
+  const double* C = q.centers + grp * q.cap * n_cv;
+  const double* W = q.widths + grp * q.cap * n_cv;
+  const double* H = q.heights + grp * q.cap;
+  double v = 0.0, dv[MD_MAX_CV] = {0.0, 0.0, 0.0, 0.0};
+  for (int64_t k = tid; k < n_g; k += MD_THREADS) {
+    double u[MD_MAX_CV], wk[MD_MAX_CV], a = 0.0;
+#pragma unroll
+    for (int j = 0; j < MD_MAX_CV; ++j) {
+      if (j >= n_cv) break;
+      double e = __dsub_rn(s_cv[j], C[k * n_cv + j]);
+      if (q.type[j] == CV_DIHEDRAL) {
+        if (e >= M_PI)
+          e = __dsub_rn(e, 2.0 * M_PI);
+        else if (e < -M_PI)
+          e = __dadd_rn(e, 2.0 * M_PI);
+      }
+      wk[j] = W[k * n_cv + j];
+      u[j] = __ddiv_rn(e, wk[j]);
+      a = __dadd_rn(a, __dmul_rn(u[j], u[j]));
+    }
+    const double x = __dmul_rn(H[k], exp(__dmul_rn(-0.5, a)));
+    v = __dadd_rn(v, x);
+#pragma unroll
+    for (int j = 0; j < MD_MAX_CV; ++j) {
+      if (j >= n_cv) break;
+      dv[j] = __dsub_rn(dv[j], __dmul_rn(x, __ddiv_rn(u[j], wk[j])));
+    }
+  }
+  const double V = block_sum(v, red);
+#pragma unroll
+  for (int j = 0; j < MD_MAX_CV; ++j) {
+    if (j >= n_cv) break;
+    const double d = block_sum(dv[j], red);
+    if (tid == 0) s_dv[j] = d;
+  }
+  // F = Fm everywhere, then the touched atoms: thread j 4 + p owns atom slot p of CV j if it is that atom's first
+  // appearance in (j, p) order
+  const double* fm = Fm + rep * dimi;
+  double* f = F + rep * dimi;
+  for (int i = tid; i < dimi; i += MD_THREADS) f[i] = fm[i];
+  __syncthreads();  // s_dv is complete, and every plain F is written
+  if (tid < 4 * n_cv) {  // CV type t holds t + 2 atoms
+    const int j0 = tid / 4, p0 = tid % 4;
+    const int at = q.atoms[j0][p0];
+    bool first = p0 < q.type[j0] + 2;
+    for (int j = 0; j <= j0 && first; ++j)
+      for (int p = 0; p < (j == j0 ? p0 : q.type[j] + 2); ++p)
+        if (q.atoms[j][p] == at) first = false;
+    if (first) {
+      double fb[3] = {0.0, 0.0, 0.0};
+      for (int j = j0; j < n_cv; ++j)
+        for (int p = 0; p < q.type[j] + 2; ++p)
+          if (q.atoms[j][p] == at)
+            for (int x = 0; x < 3; ++x) fb[x] = __dsub_rn(fb[x], __dmul_rn(s_dv[j], s_g[j][p][x]));
+      for (int x = 0; x < 3; ++x) {
+        f[3 * at + x] = __dadd_rn(fm[3 * at + x], fb[x]);
+        q.Fb[rep * dimi + 3 * at + x] = fb[x];
+      }
+    }
+  }
+  if (tid < n_cv) q.cv[rep * n_cv + tid] = s_cv[tid];
+  if (tid == 0) q.Vb[rep] = V;
+  if (!deposit) return;
+  const MdParams& p = *P;
+  const uint64_t done = c - run_start;
+  if (p.stride > 0 && done % (uint64_t)p.stride == 0) {
+    const int64_t fr = (int64_t)(done / (uint64_t)p.stride) - 1;
+    if (q.cv_f != nullptr && tid < n_cv) q.cv_f[(fr * n_rep + rep) * n_cv + tid] = s_cv[tid];
+    if (q.bias_f != nullptr && tid == 0) q.bias_f[fr * n_rep + rep] = V;
+  }
+  if (c % pace == 0) {
+    const int64_t slot = grp * q.cap + n_g + w;
+    if (tid < n_cv) {
+      q.centers[slot * n_cv + tid] = s_cv[tid];
+      q.widths[slot * n_cv + tid] = q.width[tid];
+    }
+    if (tid == 0) q.heights[slot] = __dmul_rn(q.w0, exp(__ddiv_rn(-V, q.dkT)));
+  }
+}
+
+// the commit after a run: count[g] += add for every group
+__global__ void k_metad_commit(int64_t* count, int64_t n_groups, int64_t add) {
+  const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < n_groups) count[g] += add;
+}
+
 }  // namespace
 
 }  // namespace sgdml
@@ -833,6 +1012,7 @@ struct StepParams {
   NebParams neb;
   RemdParams remd;
   NptParams npt;
+  MetadParams metad;
 };
 constexpr size_t STEP_PARAMS_BYTES = (sizeof(StepParams) + 255) & ~(size_t)255;  // where the tables start
 
@@ -890,6 +1070,14 @@ struct sgdml_b200_md {
   NptCell* cell = nullptr;    // (n_rep) barostat state
   Lattice* lat = nullptr;     // (n_rep) the cells the descriptor kernel reads: a L0 and L0^-1 / a, a = exp(eps / 3)
   double *W = nullptr, *Ws = nullptr;  // (n_rep, 9) virial of the state, and of the evaluation that precedes a capture
+  // metadynamics (sgdml_b200_metad_create): null on every other handle.  The model's forces go to Fm, and k_metad_bias
+  // completes F; the hill store's pointers, its capacity and the CVs live in the mirror's MetadParams.
+  double* Fm = nullptr;        // (n_rep, 3N) the model's forces of the state
+  double *cv = nullptr, *Vb = nullptr, *Fb = nullptr;  // the state's CVs, bias energy and bias force
+  double *hc = nullptr, *hw = nullptr, *hh = nullptr;  // the hill store: centres, widths, heights
+  int64_t* hcount = nullptr;   // (n_groups) committed hills per group
+  std::vector<int64_t> hcount_host;  // the same, once the queued runs have finished
+  int64_t n_groups = 0;
 
   // the block's parts in blk or hblk
   StepParams* params(char* b) const { return reinterpret_cast<StepParams*>(b); }
@@ -910,6 +1098,8 @@ void md_free(sgdml_b200_md* md) {
   force_eval_destroy(md->fe);
   for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s}) cached_free(p);
   for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev, md->Fn, md->W, md->Ws}) cached_free(p);
+  for (double* p : {md->Fm, md->cv, md->Vb, md->Fb, md->hc, md->hw, md->hh}) cached_free(p);
+  cached_free(md->hcount);
   cached_free(md->step);
   cached_free(md->blk);
   cached_free(md->rst);
@@ -1009,7 +1199,7 @@ class Outputs {
   }
 
  private:
-  static constexpr int MAX_OUTS = 12;
+  static constexpr int MAX_OUTS = 14;
   cudaStream_t s_;
   int n_ = 0;
   Out out_[MAX_OUTS];
@@ -1021,7 +1211,8 @@ class Outputs {
 
 // what one step of the handle's graph integrates
 enum MdKind {
-  MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, MD_NEB_FIRE = 4, MD_REMD = 5, MD_NPT = 6
+  MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, MD_NEB_FIRE = 4, MD_REMD = 5, MD_NPT = 6,
+  MD_METAD = 7
 };
 
 // the integrator of sgdml_b200_md_run, sgdml_b200_remd_run, sgdml_b200_npt_run, sgdml_b200_pimd_run,
@@ -1081,9 +1272,22 @@ int md_forces(sgdml_b200_md* md, double* F, double* E, double* W, cudaStream_t s
   return force_eval_run_cells(md->fe, md->R, md->lat, F, E, W, s);
 }
 
+// The state's forces and energies: on a metadynamics handle the model's F into Fm, then k_metad_bias (deposit: inside
+// a run) completes F; on every other handle md_forces
+int md_state_forces(sgdml_b200_md* md, int deposit, cudaStream_t s) {
+  if (md->Fm == nullptr) return md_forces(md, md->F, md->E, md->W, s);
+  SG_TRY(md_forces(md, md->Fm, md->E, nullptr, s));
+  StepParams* p = md->params(md->blk);
+  k_metad_bias<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&p->metad, &p->md, md->R, md->Fm, md->F, md->step, md->dimi,
+                                                          deposit);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_MISC);
+  return 0;
+}
+
 int md_step(sgdml_b200_md* md, int kind, cudaStream_t s) {
   SG_TRY(md_integrate(md, kind, 1, s));
-  return md_forces(md, md->F, md->E, md->W, s);
+  return md_state_forces(md, 1, s);
 }
 
 // the step graph, captured again whenever the force evaluation it bakes in is stale or its key changes
@@ -1126,10 +1330,11 @@ int md_replay(sgdml_b200_md* md, int kind, int64_t n_steps, cudaStream_t s) {
 
 // ------------------------------------------------------------------ MD, replica-exchange and PIMD runs
 // What a run writes, by Outputs slot: the frames, a ring polymer's estimator frames, a replica exchange's walker
-// frames, final walker labels and counts, then an NPT run's cell and pressure frames.
+// frames, final walker labels and counts, an NPT run's cell and pressure frames, then a metadynamics run's CV and
+// bias-energy frames.
 enum RunOut {
   OUT_R, OUT_V, OUT_EPOT, OUT_EKIN, OUT_KPRIM, OUT_KCV, OUT_WALKER_F, OUT_WALKERS, OUT_NACC, OUT_NATT, OUT_CELL,
-  OUT_PRESS, N_RUN_OUTS
+  OUT_PRESS, OUT_CV, OUT_BIAS, N_RUN_OUTS
 };
 
 // The run's constants, once on the host in double precision.  First the fields MdParams and PimdParams share.
@@ -1228,6 +1433,53 @@ void npt_params(sgdml_b200_md* md, const NptRun& b, double dt, double kT, const 
   q.P_f = out.dev(OUT_PRESS);
 }
 
+// What a metadynamics run (sgdml_b200_metad_run) adds to an MD run: the deposition, checked, and the hills it deposits
+// per walker.
+struct MetadRun {
+  double w0, dkT;
+  const double* widths;
+  int64_t pace, n_dep;
+};
+
+// the deposit's constants and the frame outputs (the CVs and the store's pointers are the handle's, already there)
+void metad_params(sgdml_b200_md* md, const MetadRun& m, const Outputs& out) {
+  MetadParams& q = md->params(md->hblk)->metad;
+  q.w0 = m.w0;
+  q.dkT = m.dkT;
+  q.pace = m.pace;
+  for (int j = 0; j < q.n_cv; ++j) q.width[j] = m.widths[j];
+  q.cv_f = out.dev(OUT_CV);
+  q.bias_f = out.dev(OUT_BIAS);
+}
+
+// Grows every group's hill store to at least `need` slots, keeping its hills, before anything of the call is queued.
+// The store's pointers and capacity are in the mirror's MetadParams, which the caller uploads.
+int metad_reserve(sgdml_b200_md* md, int64_t need) {
+  MetadParams& q = md->params(md->hblk)->metad;
+  if (need <= q.cap) return 0;
+  const int64_t cap = std::max(need, 2 * q.cap);
+  const size_t nc = (size_t)q.n_cv, G = (size_t)md->n_groups;
+  double *c = nullptr, *w = nullptr, *h = nullptr;
+  SG_CUDA(cudaDeviceSynchronize());  // queued work may still use the old store
+  SG_CUDA(cached_malloc(&c, sizeof(double) * G * cap * nc));
+  SG_CUDA(cached_malloc(&w, sizeof(double) * G * cap * nc));
+  SG_CUDA(cached_malloc(&h, sizeof(double) * G * cap));
+  if (q.cap > 0) {
+    const size_t rc = sizeof(double) * q.cap * nc, rh = sizeof(double) * q.cap;
+    SG_CUDA(cudaMemcpy2D(c, sizeof(double) * cap * nc, md->hc, rc, rc, G, cudaMemcpyDeviceToDevice));
+    SG_CUDA(cudaMemcpy2D(w, sizeof(double) * cap * nc, md->hw, rc, rc, G, cudaMemcpyDeviceToDevice));
+    SG_CUDA(cudaMemcpy2D(h, sizeof(double) * cap, md->hh, rh, rh, G, cudaMemcpyDeviceToDevice));
+  }
+  cached_free(md->hc);
+  cached_free(md->hw);
+  cached_free(md->hh);
+  md->hc = q.centers = c;
+  md->hw = q.widths = w;
+  md->hh = q.heights = h;
+  q.cap = cap;
+  return 0;
+}
+
 // PIMD: the estimator constants, C, the mode tables and the (P, 3N) sigma table (tests/pimd_oracle.py restates them);
 // returns the end of what it filled
 const double* pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, double kT, double hbar, double gamma,
@@ -1280,13 +1532,18 @@ const double* pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, doub
 }
 
 constexpr const char* NPT_ONLY = "an NPT handle (sgdml_b200_npt_create) runs only sgdml_b200_npt_run";
+constexpr const char* METAD_ONLY = "a metadynamics handle (sgdml_b200_metad_create) runs only sgdml_b200_metad_run";
 
-// the checks every run shares (npt: the run is sgdml_b200_npt_run); a rejected call queues nothing
+// the checks every run shares (npt, metad: the run is sgdml_b200_npt_run, sgdml_b200_metad_run); a rejected call
+// queues nothing
 int run_check(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double gamma, int64_t stride,
-              const char* no_state, bool npt = false) {
+              const char* no_state, bool npt = false, bool metad = false) {
   SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
   if (npt && md->cell == nullptr) return fail_arg("sgdml_b200_npt_run needs an NPT handle (sgdml_b200_npt_create)");
   if (!npt && md->cell != nullptr) return fail_arg(NPT_ONLY);
+  if (metad && md->Fm == nullptr)
+    return fail_arg("sgdml_b200_metad_run needs a metadynamics handle (sgdml_b200_metad_create)");
+  if (!metad && md->Fm != nullptr) return fail_arg(METAD_ONLY);
   SG_ARG(std::isfinite(dt) && dt > 0.0);
   SG_ARG(std::isfinite(kT) && kT >= 0.0);
   if (md->nb == 1 && kT > 0.0 && gamma == 0.0)
@@ -1297,11 +1554,12 @@ int run_check(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double g
 }
 
 // sgdml_b200_md_run (MD_CLASSICAL), sgdml_b200_pimd_run (MD_RING_POLYMER; hbar and lambda are only its own),
-// sgdml_b200_remd_run (MD_REMD, with x: its ladder, and kT = its first temperature) and sgdml_b200_npt_run (MD_NPT,
-// with b: its barostat), after their checks.  n_steps steps, then the completing launch.
+// sgdml_b200_remd_run (MD_REMD, with x: its ladder, and kT = its first temperature), sgdml_b200_npt_run (MD_NPT,
+// with b: its barostat) and sgdml_b200_metad_run (MD_METAD, with mt: its deposition), after their checks.  n_steps
+// steps, then the completing launch.
 int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, double hbar, double gamma, double lambda,
            uint64_t seed, int64_t stride, void* const outs[N_RUN_OUTS], const RemdRun* x, const NptRun* b,
-           cudaStream_t s) {
+           cudaStream_t s, const MetadRun* mt = nullptr) {
   if (n_steps == 0 && x == nullptr) return 0;  // (a replica exchange still reports its labels and zero counts)
   md->group = x != nullptr ? x->n_temps : 1;
   const int64_t n_rep = md->n_rep, n_frames = stride > 0 ? n_steps / stride : 0;
@@ -1313,7 +1571,8 @@ int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, d
                    {outs[OUT_EKIN], fr}, {outs[OUT_KPRIM], fp}, {outs[OUT_KCV], fp},
                    {outs[OUT_WALKER_F], sizeof(int) * (size_t)(n_frames * n_rep)},
                    {outs[OUT_WALKERS], sizeof(int) * (size_t)n_rep}, {outs[OUT_NACC], nc}, {outs[OUT_NATT], nc},
-                   {outs[OUT_CELL], 9 * fr}, {outs[OUT_PRESS], fr}}));
+                   {outs[OUT_CELL], 9 * fr}, {outs[OUT_PRESS], fr},
+                   {outs[OUT_CV], fr * (mt != nullptr ? md->params(md->hblk)->metad.n_cv : 0)}, {outs[OUT_BIAS], fr}}));
   SG_TRY(force_eval_prepare(md->fe));
   if (x != nullptr) {
     SG_TRY(reserve(md, x->n_temps));
@@ -1321,6 +1580,11 @@ int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, d
     SG_CUDA(cudaMemsetAsync(md->xcount, 0, 2 * sizeof(int64_t) * (size_t)n_rep, s));  // the run's counts
   }
   SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the mirror
+  if (mt != nullptr) {
+    int64_t need = 0;
+    for (int64_t c : md->hcount_host) need = std::max(need, c);
+    SG_TRY(metad_reserve(md, need + (int64_t)md->params(md->hblk)->metad.n_walkers * mt->n_dep));
+  }
   StepParams& p = *md->params(md->hblk);
   const double* end;
   if (kind == MD_RING_POLYMER) {
@@ -1331,12 +1595,20 @@ int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, d
     end = md_params(md, dt, gamma, x != nullptr ? x->kT : &kT, md->group);
     if (x != nullptr) end = remd_params(md, *x, out);
     if (b != nullptr) npt_params(md, *b, dt, kT, out);
+    if (mt != nullptr) metad_params(md, *mt, out);
   }
   SG_TRY(upload(md, end, s));
   if (n_steps > 0) {
     SG_TRY(md_replay(md, kind, n_steps, s));
     md->step_host += (uint64_t)n_steps;
     SG_TRY(md_integrate(md, kind, 0, s));  // the second half-kick of the last step (and its frame)
+    if (mt != nullptr && mt->n_dep > 0) {  // the run's hills become committed
+      const int64_t add = (int64_t)md->params(md->hblk)->metad.n_walkers * mt->n_dep;
+      k_metad_commit<<<(unsigned)((md->n_groups + 255) / 256), 256, 0, s>>>(md->hcount, md->n_groups, add);
+      SG_CUDA(cudaGetLastError());
+      count_launch(KID_MISC);
+      for (int64_t& c : md->hcount_host) c += add;
+    }
   }
   if (x != nullptr) SG_TRY(out.copy_from(OUT_WALKERS, {md->walker, md->xcount, md->xcount + n_rep}));
   return out.finish();
@@ -1440,6 +1712,7 @@ int relax_check(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxste
   SG_ARG(std::isfinite(fmax) && fmax >= 0.0);
   SG_ARG(std::isfinite(maxstep) && maxstep > 0.0);
   if (md->cell != nullptr) return fail_arg(NPT_ONLY);
+  if (md->Fm != nullptr) return fail_arg(METAD_ONLY);
   if (!md->has_state) return fail_arg(what);
   return 0;
 }
@@ -1591,6 +1864,184 @@ int sgdml_b200_npt_get_cells(sgdml_b200_md* md, double* lattices, double* lattic
   return out.finish();
 }
 
+int sgdml_b200_metad_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_groups, int64_t n_walkers,
+                            const double* inv_mass, int64_t n_cv, const int* cv_type, const int64_t* cv_atoms) {
+  SG_TRY(require_device());
+  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr && cv_type != nullptr && cv_atoms != nullptr);
+  SG_ARG(n_groups >= 1 && n_walkers >= 1 && n_groups <= INT32_MAX / n_walkers);
+  SG_ARG(n_cv >= 1 && n_cv <= MD_MAX_CV);
+  SG_ARG(!is_device_ptr(cv_type) && !is_device_ptr(cv_atoms));
+  int64_t n_atoms = 0;
+  SG_TRY(sgdml_b200_model_dims(m, &n_atoms, nullptr, nullptr));
+  MetadParams q = {};
+  q.n_cv = (int)n_cv;
+  q.n_walkers = (int)n_walkers;
+  for (int j = 0; j < n_cv; ++j) {
+    if (cv_type[j] != CV_DISTANCE && cv_type[j] != CV_ANGLE && cv_type[j] != CV_DIHEDRAL)
+      return fail_arg("cv_type must be 0 (distance), 1 (angle) or 2 (dihedral)");
+    q.type[j] = cv_type[j];
+    const int na = cv_type[j] + 2;
+    for (int p = 0; p < na; ++p) {
+      const int64_t a = cv_atoms[4 * j + p];
+      if (a < 0 || a >= n_atoms) return fail_arg("cv_atoms must lie in [0, N)");
+      for (int o = 0; o < p; ++o)
+        if (cv_atoms[4 * j + o] == a) return fail_arg("the atoms of a CV must be distinct");
+      q.atoms[j][p] = (int)a;
+    }
+  }
+  const int64_t n_rep = n_groups * n_walkers;
+  sgdml_b200_md* md = nullptr;
+  SG_TRY(md_create(&md, m, n_rep, 1, inv_mass));
+  auto body = [&]() -> int {
+    const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
+    SG_CUDA(cached_malloc(&md->Fm, st));
+    SG_CUDA(cached_malloc(&md->Fb, st));
+    SG_CUDA(cached_malloc(&md->cv, sizeof(double) * (size_t)(n_rep * n_cv)));
+    SG_CUDA(cached_malloc(&md->Vb, sizeof(double) * (size_t)n_rep));
+    SG_CUDA(cached_malloc(&md->hcount, sizeof(int64_t) * (size_t)n_groups));
+    SG_CUDA(cudaMemset(md->Fb, 0, st));  // the coordinates no CV touches keep a zero bias force
+    SG_CUDA(cudaMemset(md->hcount, 0, sizeof(int64_t) * (size_t)n_groups));
+    md->n_groups = n_groups;
+    md->hcount_host.assign((size_t)n_groups, 0);
+    q.count = md->hcount;
+    q.cv = md->cv;
+    q.Vb = md->Vb;
+    q.Fb = md->Fb;
+    StepParams* p = md->params(md->hblk);
+    p->metad = q;
+    SG_TRY(upload(md, p + 1, 0));
+    SG_CUDA(cudaStreamSynchronize(0));
+    return 0;
+  };
+  const int rc = body();
+  if (rc != 0) {
+    md_free(md);
+    return rc;
+  }
+  *out = md;
+  return 0;
+}
+
+int sgdml_b200_metad_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, double w0,
+                         const double* widths, int64_t pace, double dkT, uint64_t seed, int64_t stride,
+                         double* R_frames, double* V_frames, double* E_pot_frames, double* E_kin_frames,
+                         double* cv_frames, double* bias_frames, void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(run_check(md, n_steps, dt, kT, gamma, stride,
+                   "sgdml_b200_metad_run: no state yet (call sgdml_b200_md_set_state)", false, true));
+  SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
+  SG_ARG(std::isfinite(w0) && w0 >= 0.0);
+  SG_ARG(pace >= 1);
+  SG_ARG(dkT > 0.0);  // finite or +inf (NaN fails)
+  SG_ARG(widths != nullptr && !is_device_ptr(widths));
+  const MetadParams& q = md->params(md->hblk)->metad;
+  for (int j = 0; j < q.n_cv; ++j)
+    if (!(std::isfinite(widths[j]) && widths[j] > 0.0)) return fail_arg("every width must be finite and > 0");
+  const uint64_t a = md->step_host, e = md->step_host + (uint64_t)n_steps, pc = (uint64_t)pace;
+  const MetadRun mt = {w0, dkT, widths, pace, (int64_t)(e / pc - a / pc)};
+  void* outs[N_RUN_OUTS] = {R_frames, V_frames, E_pot_frames, E_kin_frames};
+  outs[OUT_CV] = cv_frames;
+  outs[OUT_BIAS] = bias_frames;
+  return md_run(md, MD_METAD, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, outs, nullptr, nullptr,
+                (cudaStream_t)stream, &mt);
+}
+
+int sgdml_b200_metad_get_hills(sgdml_b200_md* md, int64_t* n_hills, double* centers, double* widths,
+                               double* heights, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr && n_hills != nullptr && !is_device_ptr(n_hills));
+  if (md->Fm == nullptr)
+    return fail_arg("sgdml_b200_metad_get_hills needs a metadynamics handle (sgdml_b200_metad_create)");
+  cudaStream_t s = (cudaStream_t)stream;
+  const MetadParams& q = md->params(md->hblk)->metad;
+  const size_t nc = (size_t)q.n_cv;
+  int64_t total = 0;
+  for (int64_t c : md->hcount_host) total += c;
+  Outputs out(s);
+  SG_TRY(out.init({{centers, sizeof(double) * total * nc}, {widths, sizeof(double) * total * nc},
+                   {heights, sizeof(double) * total}}));
+  int64_t off = 0;
+  for (int64_t g = 0; g < md->n_groups; ++g) {
+    const int64_t c = md->hcount_host[(size_t)g];
+    n_hills[g] = c;
+    if (c == 0) continue;
+    const size_t row = sizeof(double) * c * nc, src = (size_t)(g * q.cap) * nc;
+    if (out.dev(0)) SG_CUDA(cudaMemcpyAsync(out.dev(0) + off * nc, md->hc + src, row, cudaMemcpyDeviceToDevice, s));
+    if (out.dev(1)) SG_CUDA(cudaMemcpyAsync(out.dev(1) + off * nc, md->hw + src, row, cudaMemcpyDeviceToDevice, s));
+    if (out.dev(2))
+      SG_CUDA(cudaMemcpyAsync(out.dev(2) + off, md->hh + g * q.cap, sizeof(double) * c, cudaMemcpyDeviceToDevice, s));
+    off += c;
+  }
+  return out.finish();
+}
+
+int sgdml_b200_metad_set_hills(sgdml_b200_md* md, const int64_t* n_hills, const double* centers,
+                               const double* widths, const double* heights, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr && n_hills != nullptr && !is_device_ptr(n_hills));
+  if (md->Fm == nullptr)
+    return fail_arg("sgdml_b200_metad_set_hills needs a metadynamics handle (sgdml_b200_metad_create)");
+  int64_t total = 0, need = 0;
+  for (int64_t g = 0; g < md->n_groups; ++g) {
+    SG_ARG(n_hills[g] >= 0);
+    total += n_hills[g];
+    need = std::max(need, n_hills[g]);
+  }
+  const int nc = md->params(md->hblk)->metad.n_cv;
+  if (total > 0) {
+    SG_ARG(centers != nullptr && widths != nullptr && heights != nullptr);
+    SG_ARG(!is_device_ptr(centers) && !is_device_ptr(widths) && !is_device_ptr(heights));
+    for (int64_t k = 0; k < total; ++k) {
+      if (!std::isfinite(heights[k])) return fail_arg("every height must be finite");
+      for (int j = 0; j < nc; ++j) {
+        if (!std::isfinite(centers[k * nc + j])) return fail_arg("every centre must be finite");
+        if (!(std::isfinite(widths[k * nc + j]) && widths[k * nc + j] > 0.0))
+          return fail_arg("every width must be finite and > 0");
+      }
+    }
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the mirror
+  SG_TRY(metad_reserve(md, need));
+  StepParams* p = md->params(md->hblk);
+  const MetadParams& q = p->metad;
+  int64_t off = 0;
+  for (int64_t g = 0; g < md->n_groups; ++g) {
+    const int64_t c = n_hills[g];
+    if (c == 0) continue;
+    const size_t row = sizeof(double) * c * nc, dst = (size_t)(g * q.cap) * nc;
+    SG_CUDA(cudaMemcpyAsync(md->hc + dst, centers + off * nc, row, cudaMemcpyHostToDevice, s));
+    SG_CUDA(cudaMemcpyAsync(md->hw + dst, widths + off * nc, row, cudaMemcpyHostToDevice, s));
+    SG_CUDA(cudaMemcpyAsync(md->hh + g * q.cap, heights + off, sizeof(double) * c, cudaMemcpyHostToDevice, s));
+    off += c;
+  }
+  md->hcount_host.assign(n_hills, n_hills + md->n_groups);
+  SG_CUDA(cudaMemcpyAsync(md->hcount, md->hcount_host.data(), sizeof(int64_t) * md->n_groups, cudaMemcpyHostToDevice,
+                          s));
+  SG_TRY(upload(md, p + 1, s));
+  if (md->has_state) {
+    SG_TRY(force_eval_prepare(md->fe));
+    SG_TRY(md_state_forces(md, 0, s));
+  }
+  SG_CUDA(cudaStreamSynchronize(s));  // (the caller's arrays and the counts' host vector)
+  return 0;
+}
+
+int sgdml_b200_metad_get_bias(sgdml_b200_md* md, double* cv, double* V_bias, double* F_bias, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(md != nullptr);
+  if (md->Fm == nullptr)
+    return fail_arg("sgdml_b200_metad_get_bias needs a metadynamics handle (sgdml_b200_metad_create)");
+  if (!md->has_state) return fail_arg("sgdml_b200_metad_get_bias: no state yet (call sgdml_b200_md_set_state)");
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t n = (size_t)md->n_rep;
+  Outputs out(s);
+  SG_TRY(out.init({{cv, sizeof(double) * n * md->params(md->hblk)->metad.n_cv}, {V_bias, sizeof(double) * n},
+                   {F_bias, sizeof(double) * n * md->dimi}}));
+  SG_TRY(out.copy_from(0, {md->cv, md->Vb, md->Fb}));
+  return out.finish();
+}
+
 int sgdml_b200_md_destroy(sgdml_b200_md* md) {
   if (md != nullptr) md_free(md);
   return 0;
@@ -1609,7 +2060,7 @@ int sgdml_b200_md_set_state(sgdml_b200_md* md, const double* R, const double* V,
     SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
   const std::vector<uint64_t> steps((size_t)md->n_rep, step);
   SG_CUDA(cudaMemcpyAsync(md->step, steps.data(), sizeof(uint64_t) * md->n_rep, cudaMemcpyHostToDevice, s));
-  SG_TRY(md_forces(md, md->F, md->E, md->W, s));
+  SG_TRY(md_state_forces(md, 0, s));
   if (md->walker != nullptr) {  // a replica exchange's walkers start again from their slots
     k_remd_identity<<<(unsigned)((md->n_rep + 255) / 256), 256, 0, s>>>(md->walker, md->n_rep);
     SG_CUDA(cudaGetLastError());
@@ -1630,7 +2081,7 @@ int sgdml_b200_md_get_state(sgdml_b200_md* md, double* R, double* V, double* F, 
   const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
   Outputs out(s);
   SG_TRY(out.init({{R, st}, {V, st}, {F, st}, {E_pot, sizeof(double) * md->n_rep}, {step, sizeof(uint64_t)}}));
-  SG_TRY(out.copy_from(0, {md->R, md->V, md->F, md->E, md->step}));
+  SG_TRY(out.copy_from(0, {md->R, md->V, md->Fm != nullptr ? md->Fm : md->F, md->E, md->step}));
   return out.finish();
 }
 

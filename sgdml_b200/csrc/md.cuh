@@ -1,7 +1,7 @@
-// Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_pimd_*,
-// sgdml_b200_relax_*, sgdml_b200_neb_fire): the contract of the kernels in md.cu -- the BAOAB integrator step, the
-// replica exchange, the NPT step, the ring-polymer step, their counter-based noise, the FIRE and L-BFGS steps, and the
-// nudged elastic band.
+// Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_metad_*,
+// sgdml_b200_pimd_*, sgdml_b200_relax_*, sgdml_b200_neb_fire): the contract of the kernels in md.cu -- the BAOAB
+// integrator step, the replica exchange, the NPT step, the metadynamics bias, the ring-polymer step, their counter-based
+// noise, the FIRE and L-BFGS steps, and the nudged elastic band.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -91,6 +91,63 @@ struct NptParams {
 // pending half-kick with those forces.
 // Drift: velocities scaled by 1 / mu keep dr dp, and with the instantaneous K in P_int the Ito drift that leaves
 // exp(-beta (H + P0 V)) dr dp dV stationary carries no kT / V term (DESIGN.md 4.1.7 has the derivation).
+
+// Multiple-walker metadynamics (sgdml_b200_metad_run): a metadynamics handle (sgdml_b200_metad_create) is an MD handle
+// of n_rep = n_groups n_walkers replicas, replica g n_walkers + w walker w of group g, integrated by k_md_step (sigma
+// row 0).  The walkers of a group deposit Gaussian hills into one store and are biased by it; groups never see each
+// other's hills.  Collective variables (CVs), at most MD_MAX_CV, each of a type and up to 4 distinct atoms i, j, k, l,
+// on plain coordinate differences (no minimum image, as NEB: positions are never wrapped).  Every product, sum,
+// difference and quotient below is rounded as written (no fused multiply-add); dot(a, b) = (a0 b0 + a1 b1) + a2 b2,
+// cross(a, b) = (a1 b2 - a2 b1, a2 b0 - a0 b2, a0 b1 - a1 b0), |a| = sqrt(dot(a, a)), and x / y of a vector by a scalar
+// divides each component.
+//   CV_DISTANCE  d = r_j - r_i;  s = |d|;  ds/dr_j = d / s, ds/dr_i = -(d / s)  (both 0 when s == 0)
+//   CV_ANGLE     a = r_i - r_j, b = r_k - r_j, c = cross(a, b), cn = |c|;  s = atan2(cn, dot(a, b)) in [0, pi];
+//                ds/dr_i = cross(a, c) / (dot(a, a) cn), ds/dr_k = cross(c, b) / (dot(b, b) cn),
+//                ds/dr_j = -(ds/dr_i + ds/dr_k)  (all 0 when cn == 0: the collinear case)
+//   CV_DIHEDRAL  b1 = r_j - r_i, b2 = r_k - r_j, b3 = r_l - r_k, m = cross(b1, b2), n = cross(b2, b3), nb = |b2|;
+//                s = atan2(nb dot(b1, n), dot(m, n)) in (-pi, pi] (Blondel & Karplus, J. Comput. Chem. 17, 1132 (1996));
+//                gi = -((nb / dot(m, m)) m), gl = (nb / dot(n, n)) n, p = dot(b1, b2) / dot(b2, b2),
+//                q = dot(b3, b2) / dot(b2, b2), t = p gi - q gl;  ds/dr_i = gi, ds/dr_l = gl, ds/dr_j = -(gi + t),
+//                ds/dr_k = t - gl  (all 0 when dot(m, m) == 0 or dot(n, n) == 0)
+// A hill k of the store has a centre c_k, widths w_k (per CV) and a height h_k.  Per hill, j over the CVs in order:
+//   e_j = s_j - c_kj, for a dihedral wrapped into [-pi, pi) by one step: e_j >= pi: e_j - 2 pi, e_j < -pi: e_j + 2 pi
+//   (pi and 2 pi the doubles nearest them);  u_j = e_j / w_kj;  a = sum_j u_j u_j from 0.0;  x = h_k exp(-0.5 a);
+//   V += x;  dV_j -= x (u_j / w_kj)
+// V = sum_k h_k exp(-sum_j e_kj^2 / (2 w_kj^2)) and dV_j = dV/ds_j in block_sum's order: thread t adds the terms of
+// hills t, t + MD_THREADS, ... from 0.0 in increasing k, then the tree.  The bias force on an atom a touched by a CV is
+// Fb_a = sum over the CVs j in order of -(dV_j ds_j/dr_a) from 0.0 (only the CVs that hold a add a term), and the
+// force k_md_step reads is F = Fm + Fb_a, rounded once; coordinates no CV touches get F = Fm.
+constexpr int MD_MAX_CV = 4;
+enum CvType { CV_DISTANCE = 0, CV_ANGLE = 1, CV_DIHEDRAL = 2 };
+
+struct MetadParams {
+  int n_cv, n_walkers;
+  int type[MD_MAX_CV];
+  int atoms[MD_MAX_CV][4];   // unused entries 0
+  int64_t pace;              // a deposit on every state c with c % pace == 0
+  int64_t cap;               // hill slots per group
+  double w0;                 // the initial height
+  double dkT;                // the well-tempered Delta kT, > 0 (+inf: plain metadynamics)
+  double width[MD_MAX_CV];   // the widths the run deposits
+  double *centers, *widths;  // (n_groups, cap, n_cv) the hill store
+  double* heights;           // (n_groups, cap)
+  const int64_t* count;      // (n_groups) hills committed before the run
+  double *cv, *Vb, *Fb;      // the state's CVs (n_rep, n_cv), bias energy (n_rep) and bias force (n_rep, 3N)
+  double *cv_f, *bias_f;     // frames (n_frames, n_rep, n_cv) / (n_frames, n_rep), or null
+};
+
+// k_metad_bias: one CTA of MD_THREADS per replica, launched after the force evaluation that wrote the model force Fm
+// and E of the state R holds, with the replica's counter at c.  It computes s and ds/dR, V and dV over the n_g hills
+// of group g committed so far, writes F = Fm + Fb, the state's s, V and Fb, and with deposit == 1 (inside a run, with
+// MdParams' run_start and stride):
+//   n_g = count[g] + n_walkers ((c - 1) / pace - run_start / pace)  (the deposits of this run before state c; 0 with
+//         deposit == 0), so every walker of a group reads the same hills, and a hill deposited on state c becomes
+//         visible to the evaluation of state c + 1, never to its own;
+//   frame (c - run_start) / stride - 1 when that is whole: s and V of state c (V before its deposit);
+//   if c % pace == 0 (and c > run_start, which always holds inside a run): walker w writes slot n_g + w of its group:
+//         centre s, widths MetadParams.width, height w0 exp(-V / dkT) (w0 with dkT = +inf).
+// The driver commits a run's hills after it: count[g] += n_walkers #{c in (run_start, run_start + n_steps] :
+// c % pace == 0}.  The store's address is read from MetadParams, not baked into the step graph.
 
 // Path-integral MD (sgdml_b200_pimd_run): replica p P + j is bead j of ring polymer p.
 constexpr int PIMD_MAX_BEADS = 64;  // C (P x P) sits in shared memory: 32 KB at the cap

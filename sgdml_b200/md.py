@@ -11,6 +11,10 @@ Metropolis test inside the step graph.
 ``GDMLNPTDynamics`` -- constant-pressure MD of periodic models on the same engine (``sgdml_b200_npt_*``): Langevin
 replicas, each in a cell of its own that an isotropic stochastic cell rescaling barostat scales.
 
+``GDMLMetadynamics`` -- well-tempered multiple-walker metadynamics on the same engine (``sgdml_b200_metad_*``):
+groups of Langevin walkers, each group sharing one store of Gaussian hills on distance, angle and dihedral collective
+variables, for free-energy surfaces along chosen coordinates.
+
 ``GDMLRelaxation`` -- geometry optimisation of many replicas on the same engine (``sgdml_b200_relax_*``): FIRE and
 L-BFGS, each replica frozen once it has converged.
 
@@ -478,6 +482,215 @@ class GDMLNPTDynamics(GDMLDynamics):
             out['cells'], out['volume'] = self._ase_cells(f['cell'])
             out['pressure'] = f['P'] * (self.E_to_eV * vol_unit)
         return out
+
+
+_CV_TYPES = {'distance': 0, 'angle': 1, 'dihedral': 2}
+
+
+class GDMLMetadynamics(GDMLDynamics):
+    """Well-tempered multiple-walker metadynamics (Raiteri et al., J. Phys. Chem. B 110, 3533 (2006); Barducci, Bussi &
+    Parrinello, PRL 100, 020603 (2008)) on the device (``sgdml_b200_metad_*``), in the units of ``GDMLDynamics``.
+    `n_groups` groups of `n_walkers` Langevin walkers each: the walkers of a group deposit Gaussian hills into one
+    store and are all biased by it; groups never see each other's hills, so independent groups give error bars.
+    Walker w of group g is replica g n_walkers + w of the engine's handle.
+
+    cvs: 1 to 4 collective variables, each ('distance', (i, j)), ('angle', (i, j, k)) or ('dihedral', (i, j, k, l)),
+    in Angstrom or radians: |r_j - r_i|, the angle at j in [0, pi], the dihedral i-j-k-l in (-pi, pi], on plain
+    coordinate differences (positions are never wrapped).  ``set_state(positions, velocities=None, step=0)``:
+    positions (n_groups, n_walkers, N, 3), or (n_groups, N, 3) / (N, 3) copied to every walker (and group).
+    ``run(n_steps, dt_fs, temperature_K, friction_per_fs, height_eV, widths, pace, bias_factor=inf, seed=0, stride=0)``
+    integrates with BAOAB Langevin under the bias and deposits on every `pace`-th state a hill of the given widths (one
+    per CV, Angstrom or radians) and height height_eV exp(-V / ((bias_factor - 1) kT)); bias_factor = inf is plain
+    metadynamics, and bias_factor <= 1 is refused.  It returns ``GDMLDynamics.run``'s frames shaped (n_frames, n_groups,
+    n_walkers, ...), with the model's potential energy, plus 'cv' (n_frames, n_groups, n_walkers, n_cv) and
+    'bias_energy' (n_frames, n_groups, n_walkers) in eV, of the frame's state.  A hill becomes visible to the next
+    state's evaluation; a run continued over several calls is one long run.  ``get_state()`` adds 'cv', 'bias_energy'
+    and 'bias_forces' (eV/Angstrom); its 'forces' and 'potential_energy' are the model's.  ``hills()`` gives per group
+    {'centers', 'widths' (n_hills, n_cv), 'heights' (n_hills,)} in Angstrom/radians and eV, and ``set_hills`` takes
+    the same list to restart.  ``free_energy(grid)``: -bias_factor / (bias_factor - 1) V(s) (-V(s) for plain
+    metadynamics) per group, shifted to a minimum of zero, in eV.  NumPy arrays or float64 CUDA tensors in, the same kind
+    out."""
+
+    def __init__(self, model, masses, cvs, n_walkers=1, n_groups=1, E_to_eV=_KCAL_PER_MOL_IN_EV,
+                 F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        self.n_walkers = int(n_walkers)
+        self.n_groups = int(n_groups)
+        if self.n_walkers < 1 or self.n_groups < 1:
+            raise ValueError('n_walkers and n_groups must be >= 1')
+        cvs = list(cvs)
+        if not 1 <= len(cvs) <= 4:
+            raise ValueError('metadynamics takes 1 to 4 collective variables: %d' % len(cvs))
+        self.cvs = []
+        for kind, atoms in cvs:
+            if kind not in _CV_TYPES:
+                raise ValueError("a CV is 'distance', 'angle' or 'dihedral': %r" % (kind,))
+            atoms = tuple(int(a) for a in atoms)
+            if len(atoms) != _CV_TYPES[kind] + 2:
+                raise ValueError('a %s takes %d atoms: %s' % (kind, _CV_TYPES[kind] + 2, atoms))
+            self.cvs.append((kind, atoms))
+        self.n_cv = len(self.cvs)
+        self.bias_factor = np.inf  # of the last run: free_energy's default
+        super().__init__(model, masses, self.n_groups * self.n_walkers, E_to_eV, F_to_eV_Ang)
+        # Angstrom or radian -> the engine's CV unit (model length or radian)
+        self._cv_unit = np.array([self.Ang_to_R if k == 'distance' else 1.0 for k, _ in self.cvs])
+        self._periodic = np.array([k == 'dihedral' for k, _ in self.cvs])
+
+    def _create_handle(self):
+        types = np.array([_CV_TYPES[k] for k, _ in self.cvs], dtype=np.int32)
+        atoms = np.zeros((self.n_cv, 4), dtype=np.int64)
+        for j, (_, a) in enumerate(self.cvs):
+            atoms[j, :len(a)] = a
+        handle = ctypes.c_void_p()
+        _lib.check(
+            _lib.lib().sgdml_b200_metad_create(ctypes.byref(handle), self.gdml_predict._handle, self.n_groups,
+                                               self.n_walkers, _lib.ptr(self.inv_mass), self.n_cv, _lib.ptr(types),
+                                               _lib.ptr(atoms)),
+            'metad_create',
+        )
+        return handle
+
+    @property
+    def _shape(self):
+        return (self.n_groups, self.n_walkers)
+
+    def _like(self, v, x):
+        """the NumPy array v as x's kind (a tensor on x's device for a torch x)"""
+        if hasattr(x, 'data_ptr'):
+            import torch
+
+            return torch.as_tensor(v, device=x.device)
+        return v
+
+    # ------------------------------------------------------------------ model units (L, model energy, fs)
+    def _run_raw(self, n_steps, dt, gamma, kT, w0, widths, pace, dkT=np.inf, seed=0, stride=0,
+                 frames=('R', 'V', 'E_pot', 'E_kin', 'cv', 'bias')):
+        n_steps, stride = int(n_steps), int(stride)
+        out = self._frames(n_steps, stride, frames)
+        if 'cv' in out:
+            out['cv'] = self._empty(tuple(out['cv'].shape) + (self.n_cv,))
+        widths = np.ascontiguousarray(widths, dtype=np.float64).ravel()
+        if widths.shape != (self.n_cv,):
+            raise ValueError('widths must hold one value per CV: %d' % self.n_cv)
+        _lib.check(
+            _lib.lib().sgdml_b200_metad_run(self._handle, n_steps, float(dt), float(gamma), float(kT), float(w0),
+                                            _lib.ptr(widths), int(pace), float(dkT), int(seed), stride,
+                                            *(_lib.ptr(out.get(k)) for k in ('R', 'V', 'E_pot', 'E_kin', 'cv', 'bias')),
+                                            _lib.current_stream()),
+            'metad_run',
+        )
+        return out
+
+    def _get_bias_raw(self):
+        """{'cv' (n_replicas, n_cv), 'V' (n_replicas,), 'F' (n_replicas, 3N)} in model units."""
+        n = self.n_replicas
+        out = {'cv': self._empty((n, self.n_cv)), 'V': self._empty((n,)), 'F': self._empty((n, 3 * self.n_atoms))}
+        _lib.check(_lib.lib().sgdml_b200_metad_get_bias(self._handle, _lib.ptr(out['cv']), _lib.ptr(out['V']),
+                                                        _lib.ptr(out['F']), _lib.current_stream()), 'metad_get_bias')
+        return out
+
+    def _get_hills_raw(self):
+        """(n_hills (n_groups,) int64, centers, widths (H, n_cv), heights (H,)), host arrays in model units."""
+        n = np.zeros(self.n_groups, dtype=np.int64)
+        L = _lib.lib()
+        _lib.check(L.sgdml_b200_metad_get_hills(self._handle, _lib.ptr(n), None, None, None, _lib.current_stream()),
+                   'metad_get_hills')
+        H = int(n.sum())
+        c, w, h = np.empty((H, self.n_cv)), np.empty((H, self.n_cv)), np.empty(H)
+        _lib.check(L.sgdml_b200_metad_get_hills(self._handle, _lib.ptr(n), _lib.ptr(c), _lib.ptr(w), _lib.ptr(h),
+                                                _lib.current_stream()), 'metad_get_hills')
+        return n, c, w, h
+
+    def _set_hills_raw(self, n_hills, centers, widths, heights):
+        n = np.ascontiguousarray(n_hills, dtype=np.int64).ravel()
+        H = int(n.sum()) if n.size else 0
+        c = np.ascontiguousarray(centers, dtype=np.float64).reshape(H, self.n_cv)
+        w = np.ascontiguousarray(widths, dtype=np.float64).reshape(H, self.n_cv)
+        h = np.ascontiguousarray(heights, dtype=np.float64).reshape(H)
+        if n.shape != (self.n_groups,):
+            raise ValueError('n_hills must hold one count per group: %d' % self.n_groups)
+        _lib.check(_lib.lib().sgdml_b200_metad_set_hills(self._handle, _lib.ptr(n), _lib.ptr(c), _lib.ptr(w),
+                                                         _lib.ptr(h), _lib.current_stream()), 'metad_set_hills')
+
+    # ------------------------------------------------------------------ ASE units
+    def set_state(self, positions, velocities=None, step=0):
+        axes = ('n_groups', 'n_walkers')
+        positions = _groups(positions, 'positions', self.n_groups, self.n_walkers, self.n_atoms, axes)
+        if velocities is not None:
+            velocities = _groups(velocities, 'velocities', self.n_groups, self.n_walkers, self.n_atoms, axes)
+        super().set_state(positions, velocities, step)
+
+    def get_state(self):
+        out = super().get_state()
+        b = self._get_bias_raw()
+        g = self._shape
+        out.update(cv=(b['cv'] / self._like(self._cv_unit, b['cv'])).reshape(g + (self.n_cv,)),
+                   bias_energy=(b['V'] * self.E_to_eV).reshape(g),
+                   bias_forces=(b['F'] * self.F_to_eV_Ang).reshape(g + (self.n_atoms, 3)))
+        return out
+
+    def run(self, n_steps, dt_fs, temperature_K, friction_per_fs, height_eV, widths, pace, bias_factor=np.inf, seed=0,
+            stride=0):
+        bias_factor = float(bias_factor)
+        if not bias_factor > 1.0:
+            raise ValueError('bias_factor must be > 1 (inf: plain metadynamics): %r' % bias_factor)
+        kT = KB_EV * float(temperature_K) / self.E_to_eV
+        dkT = np.inf if np.isinf(bias_factor) else (bias_factor - 1.0) * kT
+        w = np.asarray(widths, dtype=np.float64).ravel() * self._cv_unit
+        f = self._run_raw(n_steps, dt_fs, friction_per_fs, kT, float(height_eV) / self.E_to_eV, w, pace, dkT, seed,
+                          stride)
+        self.bias_factor = bias_factor
+        out = self._ase_frames(f)
+        if 'cv' in f:
+            nf = f['cv'].shape[0]
+            out['cv'] = (f['cv'] / self._like(self._cv_unit, f['cv'])).reshape((nf,) + self._shape + (self.n_cv,))
+            out['bias_energy'] = (f['bias'] * self.E_to_eV).reshape((nf,) + self._shape)
+        return out
+
+    def hills(self):
+        """[{'centers', 'widths': (n_hills, n_cv), 'heights': (n_hills,)}] per group, Angstrom/radians and eV (NumPy)."""
+        n, c, w, h = self._get_hills_raw()
+        edges = np.concatenate([[0], np.cumsum(n)])
+        return [{'centers': c[a:b] / self._cv_unit, 'widths': w[a:b] / self._cv_unit, 'heights': h[a:b] * self.E_to_eV}
+                for a, b in zip(edges[:-1], edges[1:])]
+
+    def set_hills(self, hills):
+        """Replaces every group's hills with `hills`, a list of one dict per group as ``hills()`` gives them."""
+        if len(hills) != self.n_groups:
+            raise ValueError('hills must hold one entry per group: %d' % self.n_groups)
+        parts = [(np.asarray(g['centers'], dtype=np.float64).reshape(-1, self.n_cv) * self._cv_unit,
+                  np.asarray(g['widths'], dtype=np.float64).reshape(-1, self.n_cv) * self._cv_unit,
+                  np.asarray(g['heights'], dtype=np.float64).ravel() / self.E_to_eV) for g in hills]
+        n = [len(p[2]) for p in parts]
+        cat = [np.concatenate([p[i] for p in parts]) if sum(n) else np.empty((0,) + parts[0][i].shape[1:])
+               for i in range(3)]
+        self._set_hills_raw(n, *cat)
+
+    def bias(self, grid):
+        """V(s) (eV) per group on the grid: (n_groups, n) for one CV and a grid of n points, (n_groups, n0, n1) for two
+        CVs and a grid (g0, g1) of n0 and n1 points (Angstrom or radians), summed from ``hills()`` in NumPy."""
+        if self.n_cv == 1:
+            pts = np.asarray(grid, dtype=np.float64).reshape(-1, 1)
+            shape = (pts.shape[0],)
+        elif self.n_cv == 2:
+            g0, g1 = (np.asarray(g, dtype=np.float64).ravel() for g in grid)
+            pts = np.stack(np.meshgrid(g0, g1, indexing='ij'), -1).reshape(-1, 2)
+            shape = (len(g0), len(g1))
+        else:
+            raise ValueError('free_energy and bias take a grid over 1 or 2 CVs, not %d' % self.n_cv)
+        out = []
+        for g in self.hills():
+            d = pts[:, None, :] - g['centers'][None]
+            d = np.where(self._periodic, (d + np.pi) % (2.0 * np.pi) - np.pi, d)
+            a = ((d / g['widths'][None]) ** 2).sum(-1)
+            out.append((g['heights'][None] * np.exp(-0.5 * a)).sum(-1).reshape(shape))
+        return np.array(out)
+
+    def free_energy(self, grid, bias_factor=None):
+        """-bias_factor / (bias_factor - 1) V(s) per group (eV; -V(s) for bias_factor = inf), shifted so that each
+        group's minimum is zero; grid and shape as ``bias``.  bias_factor: that of the last run by default."""
+        gamma = self.bias_factor if bias_factor is None else float(bias_factor)
+        f = -self.bias(grid) * (1.0 if np.isinf(gamma) else gamma / (gamma - 1.0))
+        return f - f.reshape(self.n_groups, -1).min(1).reshape((self.n_groups,) + (1,) * (f.ndim - 1))
 
 
 def _det3(a):

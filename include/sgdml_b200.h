@@ -409,8 +409,36 @@ int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, do
 int sgdml_b200_neb_fire(sgdml_b200_md* md, int64_t n_images, int64_t max_steps, double fmax, double k, int climb,
                         double maxstep, double dt, double dtmax, int64_t* n_steps_out, int* converged_out,
                         double* fmax_out, int* climbing_out, void* stream);
-/* Test hook: graph replays between convergence read-backs of sgdml_b200_relax_* and sgdml_b200_neb_fire; 0 = the
- * default (16).  Negative values are rejected. */
+/* ---------------------------------------------------------------- dimer saddle search on the device
+ * Extension: first-order saddle points next to a minimum, with no final state, by the dimer method (Henkelman &
+ * Jonsson, J. Chem. Phys. 111, 7010 (1999)), many dimers and many steps per call.  The handle (sgdml_b200_md_create;
+ * ring-polymer, NPT and metadynamics handles are rejected) holds n_rep = 2 n_dimers replicas: replica 2d is the
+ * centre R0 of dimer d and replica 2d + 1 its image R0 + separation N, N the dimer's unit mode; both are evaluated
+ * every step, the other image is the central difference 2 F0 - F1.  Each step first tests the dimer: it has converged
+ * when max_a |F0_a| < fmax and the curvature along N, measured at the current centre, is negative; it is frozen from
+ * then on.  Otherwise, when the rotational force exceeds rot_min, it rotates once (a trial image at angle phi_t with
+ * cos_trial, sin_trial, then the analytic minimum of the fitted curvature, Heyden, Bell & Keil, J. Chem. Phys. 123,
+ * 224101 (2005)), which costs one extra force evaluation; then it translates the centre by one FIRE step (the rules,
+ * constants and arguments of sgdml_b200_relax_fire, maxstep capping the centre's whole step) with the force whose
+ * component along N is reversed (negative curvature) or alone and reversed (positive curvature).  N is kept orthogonal
+ * to rigid translations and, for free molecules, infinitesimal rotations of the centre.  L-BFGS is not offered: the
+ * dimer force is no gradient.  Exact sums and roundings are in csrc/md.cuh; the driver, block read-backs, final state
+ * (V zero, step counter unchanged) and launch families are those of sgdml_b200_relax_*.
+ * Arguments: modes (n_rep / 2, 3N), host or device, the initial modes (any length; projected and normalised at each
+ * centre), or NULL to keep the handle's modes from its previous dimer call (an argument error on the first); a mode
+ * that is not finite or is (almost) a rigid motion is an argument error.  max_steps bounds the force evaluations of
+ * the pairs (a rotating step takes two); separation > 0 (L); cos_trial, sin_trial > 0 with c^2 + s^2 = 1 within 1e-12;
+ * rot_min >= 0 (force / L^2, as the curvature); fmax, maxstep, dt, dtmax as for sgdml_b200_relax_fire.  Outputs,
+ * each host, device or NULL, per dimer: n_steps_out int64 (translations), converged_out int32, fmax_out double
+ * (max_a |F0_a|), curvature_out double (along the final mode at the final centre), n_rot_out int64 (rotations) and
+ * modes_out (n_rep / 2, 3N) double.  Argument errors are reported before anything of the handle changes (the modes are
+ * checked on scratch), and a rejected call changes nothing. */
+int sgdml_b200_dimer_fire(sgdml_b200_md* md, const double* modes, int64_t max_steps, double fmax, double separation,
+                          double cos_trial, double sin_trial, double rot_min, double maxstep, double dt, double dtmax,
+                          int64_t* n_steps_out, int* converged_out, double* fmax_out, double* curvature_out,
+                          int64_t* n_rot_out, double* modes_out, void* stream);
+/* Test hook: graph replays between convergence read-backs of sgdml_b200_relax_*, sgdml_b200_neb_fire and
+ * sgdml_b200_dimer_fire; 0 = the default (16).  Negative values are rejected. */
 int sgdml_b200_set_relax_block(int64_t n_steps);
 
 /* Periodic model (predict.py:332-334: lat_and_inv from model['lattice']): query descriptors of

@@ -9,8 +9,8 @@ CPU fallback.
 
 __version__ = '0.1.0'
 
-from .md import (GDMLNEB, GDMLDynamics, GDMLMetadynamics, GDMLNPTDynamics, GDMLPathIntegralDynamics,  # noqa: F401
-                 GDMLRelaxation, GDMLReplicaExchange)
+from .md import (GDMLNEB, GDMLDimer, GDMLDynamics, GDMLMetadynamics, GDMLNPTDynamics,  # noqa: F401
+                 GDMLPathIntegralDynamics, GDMLRelaxation, GDMLReplicaExchange)
 from .perm import find_perms  # noqa: F401
 from .predict import GDMLPredict  # noqa: F401
 from .train import GDMLTrain  # noqa: F401

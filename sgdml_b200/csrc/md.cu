@@ -1,7 +1,7 @@
-// Molecular dynamics, replica exchange, metadynamics, path-integral MD and geometry optimisation on the device: the
-// integrator, exchange, bias and optimiser kernels (contract in md.cuh), then the driver of sgdml_b200_md_*,
-// sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_metad_*, sgdml_b200_pimd_*, sgdml_b200_relax_* and
-// sgdml_b200_neb_fire, which evaluates forces through the predictor interface of predict.cuh.
+// Molecular dynamics, replica exchange, metadynamics, path-integral MD, geometry optimisation and saddle searches on the
+// device: the integrator, exchange, bias, optimiser and dimer kernels (contract in md.cuh), then the driver of
+// sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_metad_*, sgdml_b200_pimd_*, sgdml_b200_relax_*,
+// sgdml_b200_neb_fire and sgdml_b200_dimer_fire, which evaluates forces through the predictor interface of predict.cuh.
 //
 // The BAOAB Langevin integrator step of sgdml_b200_md_run.
 //
@@ -990,6 +990,237 @@ __global__ void k_metad_commit(int64_t* count, int64_t n_groups, int64_t add) {
   if (g < n_groups) count[g] += add;
 }
 
+// ---------------------------------------------------------------------------------- dimer search
+// The dimer kernels of sgdml_b200_dimer_fire (contract in md.cuh).  As in the optimiser kernels, every thread holds the
+// dimer's state and every CTA-wide sum, and each thread writes only its own coordinates i = t, t + MD_THREADS, ...; the
+// rigid projection's atom sums read other threads' coordinates of N, after a barrier.
+
+constexpr int DIMER_SUMS = 9;  // the most values one reduction carries: L (3) and I (6)
+
+// K sums over the CTA at once, each by block_sum's tree (the same bits as K block_sum calls); every thread gets them
+template <int K>
+__device__ __forceinline__ void block_sums(double (&x)[K], double* red) {
+#pragma unroll
+  for (int k = 0; k < K; ++k) red[k * MD_THREADS + threadIdx.x] = x[k];
+  __syncthreads();
+  for (int w = MD_THREADS / 2; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w)
+#pragma unroll
+      for (int k = 0; k < K; ++k)
+        red[k * MD_THREADS + threadIdx.x] = __dadd_rn(red[k * MD_THREADS + threadIdx.x],
+                                                      red[k * MD_THREADS + threadIdx.x + w]);
+    __syncthreads();
+  }
+#pragma unroll
+  for (int k = 0; k < K; ++k) x[k] = red[k * MD_THREADS];
+  __syncthreads();  // red is free again
+}
+
+// x if coordinate i belongs to component c, else 0.0 (the masked terms of the component sums)
+__device__ __forceinline__ double comp(int i, int c, double x) { return i % 3 == c ? x : 0.0; }
+
+// The rigid projection and normalisation (md.cuh, 5) of the mode n at centre r (n_atoms = dimi / 3), in place; the
+// caller's writes of n are its own coordinates.  Returns n.n before the normalisation.
+__device__ __forceinline__ double dimer_project(double* n, const double* r, int dimi, int periodic, double* red) {
+  const double na = (double)(dimi / 3);
+  double s[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};  // component sums of n (0..2) and of r (3..5)
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+    const double ni = n[i], ri = r[i];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      s[c] = __dadd_rn(s[c], comp(i, c, ni));
+      s[3 + c] = __dadd_rn(s[3 + c], comp(i, c, ri));
+    }
+  }
+  block_sums(s, red);
+  double m[3], rb[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    m[c] = __ddiv_rn(s[c], na);
+    rb[c] = __ddiv_rn(s[3 + c], na);
+  }
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+    const int c = i % 3;
+    n[i] = __dsub_rn(n[i], c == 0 ? m[0] : (c == 1 ? m[1] : m[2]));
+  }
+  if (!periodic) {
+    __syncthreads();  // the atom sums read the other threads' coordinates of n
+    double q[DIMER_SUMS] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};  // L0..2, I00, I11, I22, P01, P02, P12
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+      if (i % 3 != 0) continue;  // the other coordinates add 0.0
+      double x[3], na3[3], l[3];
+      sub3(x, r + i, rb);
+      for (int c = 0; c < 3; ++c) na3[c] = n[i + c];
+      cross3(l, x, na3);
+      const double x00 = __dmul_rn(x[0], x[0]), x11 = __dmul_rn(x[1], x[1]), x22 = __dmul_rn(x[2], x[2]);
+      const double t[DIMER_SUMS] = {l[0], l[1], l[2], __dadd_rn(x11, x22), __dadd_rn(x00, x22), __dadd_rn(x00, x11),
+                                    __dmul_rn(x[0], x[1]), __dmul_rn(x[0], x[2]), __dmul_rn(x[1], x[2])};
+#pragma unroll
+      for (int k = 0; k < DIMER_SUMS; ++k) q[k] = __dadd_rn(q[k], t[k]);
+    }
+    block_sums(q, red);
+    const double I00 = q[3], I11 = q[4], I22 = q[5], I01 = -q[6], I02 = -q[7], I12 = -q[8];
+    const double A00 = __dsub_rn(__dmul_rn(I11, I22), __dmul_rn(I12, I12));
+    const double A01 = __dsub_rn(__dmul_rn(I02, I12), __dmul_rn(I01, I22));
+    const double A02 = __dsub_rn(__dmul_rn(I01, I12), __dmul_rn(I11, I02));
+    const double A11 = __dsub_rn(__dmul_rn(I00, I22), __dmul_rn(I02, I02));
+    const double A12 = __dsub_rn(__dmul_rn(I01, I02), __dmul_rn(I00, I12));
+    const double A22 = __dsub_rn(__dmul_rn(I00, I11), __dmul_rn(I01, I01));
+    const double det = __dadd_rn(__dadd_rn(__dmul_rn(I00, A00), __dmul_rn(I01, A01)), __dmul_rn(I02, A02));
+    const double tr = __ddiv_rn(__dadd_rn(__dadd_rn(I00, I11), I22), 3.0);
+    if (det > __dmul_rn(1e-10, __dmul_rn(__dmul_rn(tr, tr), tr))) {
+      const double L0 = q[0], L1 = q[1], L2 = q[2];
+      const double w[3] = {
+          __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(A00, L0), __dmul_rn(A01, L1)), __dmul_rn(A02, L2)), det),
+          __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(A01, L0), __dmul_rn(A11, L1)), __dmul_rn(A12, L2)), det),
+          __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(A02, L0), __dmul_rn(A12, L1)), __dmul_rn(A22, L2)), det)};
+      for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+        const int c = i % 3;
+        double x[3], wx[3];
+        sub3(x, r + (i - c), rb);
+        cross3(wx, w, x);
+        n[i] = __dsub_rn(n[i], c == 0 ? wx[0] : (c == 1 ? wx[1] : wx[2]));
+      }
+    }
+  }
+  double nn = 0.0;
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) nn = __dadd_rn(nn, __dmul_rn(n[i], n[i]));
+  nn = block_sum(nn, red);
+  const double nrm = sqrt(nn);
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) n[i] = __ddiv_rn(n[i], nrm);
+  return nn;
+}
+
+// The initial modes of a call: src (n_dimers, 3N) projected at each centre into the scratch modes nd, the images
+// R0 + D N into the scratch rows img (n_dimers, 3N), bad[d] as md.cuh says.  Nothing of the handle changes.
+__global__ void __launch_bounds__(MD_THREADS) k_dimer_init(const DimerParams* __restrict__ Q,
+                                                          const double* __restrict__ R, const double* __restrict__ src,
+                                                          double* __restrict__ nd, double* __restrict__ img,
+                                                          int* __restrict__ bad, int dimi) {
+  __shared__ double red[DIMER_SUMS * MD_THREADS];
+  const int64_t d = blockIdx.x;
+  const double* r0 = R + 2 * d * dimi;
+  const double* s = src + d * dimi;
+  double* n = nd + d * dimi;
+  double n0 = 0.0;
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+    const double x = s[i];
+    n[i] = x;
+    n0 = __dadd_rn(n0, __dmul_rn(x, x));
+  }
+  n0 = block_sum(n0, red);
+  const double n1 = dimer_project(n, r0, dimi, Q->periodic, red);
+  if (threadIdx.x == 0) bad[d] = !(isfinite(n0) && n1 > __dmul_rn(1e-12, n0));
+  const double D = Q->D;
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) img[d * dimi + i] = __dadd_rn(r0[i], __dmul_rn(D, n[i]));
+}
+
+__device__ __forceinline__ void dimer_store(RelaxState* st, DimerState* ds, const RelaxState& z, const DimerState& y) {
+  __syncthreads();  // every thread has read the state
+  if (threadIdx.x == 0) {
+    *st = z;
+    *ds = y;
+  }
+}
+
+// The test and one step of dimer d (md.cuh): R rows 2d (centre) and 2d + 1 (image), the mode and T rows d, and the
+// translation force Fd into Fn row 2d.
+__global__ void __launch_bounds__(MD_THREADS) k_dimer_step(const DimerParams* __restrict__ Q, RelaxState* st,
+                                                          DimerState* ds, double* __restrict__ R,
+                                                          double* __restrict__ V, const double* __restrict__ F,
+                                                          double* __restrict__ Fn, double* __restrict__ Nm,
+                                                          double* __restrict__ Th, int dimi, int advance) {
+  __shared__ double red[DIMER_SUMS * MD_THREADS];
+  const int64_t d = blockIdx.x;
+  const DimerParams p = *Q;
+  RelaxState z = st[d];
+  DimerState y = ds[d];
+  z.gamma = z.E_prev = 0.0;  // (L-BFGS fields: zero already, as in k_neb_fire_step)
+  double* r0 = R + 2 * d * dimi;
+  double* r1 = r0 + dimi;
+  const double* f0 = F + 2 * d * dimi;
+  const double* f1 = f0 + dimi;
+  double* n = Nm + d * dimi;
+  double* th = Th + d * dimi;
+  if (z.conv) return dimer_store(st + d, ds + d, z, y);
+  if (y.phase == DIMER_EVAL_N) {
+    double c = 0.0;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) c = __dadd_rn(c, __dmul_rn(__dsub_rn(f0[i], f1[i]), n[i]));
+    y.C_N = __ddiv_rn(block_sum(c, red), p.D);
+  }
+  z.fmax2 = atom_max2(f0, dimi, red);
+  z.conv = z.fmax2 < p.fmax2 && y.C_N < 0.0 ? 1 : 0;
+  if (z.conv || !advance) return dimer_store(st + d, ds + d, z, y);
+
+  double cu;  // C_use
+  if (y.phase == DIMER_EVAL_N) {
+    double g = 0.0;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS)
+      g = __dadd_rn(g, __dmul_rn(__ddiv_rn(__dsub_rn(f1[i], f0[i]), p.D), n[i]));
+    g = block_sum(g, red);
+    double pp = 0.0;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+      const double pi = __dsub_rn(__ddiv_rn(__dsub_rn(f1[i], f0[i]), p.D), __dmul_rn(g, n[i]));
+      th[i] = pi;
+      pp = __dadd_rn(pp, __dmul_rn(pi, pi));
+    }
+    const double f = sqrt(block_sum(pp, red));
+    if (!(f < p.rot_min) && f != 0.0) {  // rotate: place the image on the trial direction
+      for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+        const double t = __ddiv_rn(th[i], f);
+        th[i] = t;
+        r1[i] = __dadd_rn(r0[i], __dmul_rn(p.D, __dadd_rn(__dmul_rn(p.c_t, n[i]), __dmul_rn(p.s_t, t))));
+      }
+      y.C0 = y.C_N;
+      y.b1 = -f;
+      y.phase = DIMER_TRIAL;
+      return dimer_store(st + d, ds + d, z, y);
+    }
+    cu = y.C_N;
+  } else {
+    double c = 0.0;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+      const double nt = __dadd_rn(__dmul_rn(p.c_t, n[i]), __dmul_rn(p.s_t, th[i]));
+      c = __dadd_rn(c, __dmul_rn(__dsub_rn(f0[i], f1[i]), nt));
+    }
+    const double ct = __ddiv_rn(block_sum(c, red), p.D);
+    const double a1 = __ddiv_rn(__dadd_rn(__dsub_rn(y.C0, ct), __dmul_rn(y.b1, p.s2_t)), p.omc2_t);
+    const double rr = sqrt(__dadd_rn(__dmul_rn(a1, a1), __dmul_rn(y.b1, y.b1)));
+    const double c2 = __ddiv_rn(-a1, rr), s2 = __ddiv_rn(-y.b1, rr);
+    double cs, sn;
+    if (c2 >= 0.0) {
+      cs = sqrt(__ddiv_rn(__dadd_rn(1.0, c2), 2.0));
+      sn = __ddiv_rn(s2, __dmul_rn(2.0, cs));
+    } else {
+      sn = sqrt(__ddiv_rn(__dsub_rn(1.0, c2), 2.0));
+      cs = __ddiv_rn(s2, __dmul_rn(2.0, sn));
+    }
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) n[i] = __dadd_rn(__dmul_rn(cs, n[i]), __dmul_rn(sn, th[i]));
+    dimer_project(n, r0, dimi, p.periodic, red);
+    cu = __dsub_rn(__dsub_rn(y.C0, a1), rr);
+    ++y.n_rot;
+  }
+  double* fd = Fn + 2 * d * dimi;
+  double pf = 0.0;
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) pf = __dadd_rn(pf, __dmul_rn(f0[i], n[i]));
+  pf = block_sum(pf, red);
+  const double pf2 = __dmul_rn(2.0, pf);
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS)
+    fd[i] = cu < 0.0 ? __dsub_rn(f0[i], __dmul_rn(pf2, n[i])) : -__dmul_rn(pf, n[i]);
+  fire_update(z, p.dt0, p.dtmax, p.maxstep, r0, V + 2 * d * dimi, fd, dimi, red);
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) r1[i] = __dadd_rn(r0[i], __dmul_rn(p.D, n[i]));
+  y.phase = DIMER_EVAL_N;
+  dimer_store(st + d, ds + d, z, y);
+}
+
+// the curvature, rotation count and mode of every dimer into the call's outputs (each may be null)
+__global__ void k_dimer_report(const DimerState* __restrict__ ds, int64_t n_dimers, double* curv, int64_t* n_rot) {
+  const int64_t d = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (d >= n_dimers) return;
+  if (curv) curv[d] = ds[d].C_N;
+  if (n_rot) n_rot[d] = ds[d].n_rot;
+}
+
 }  // namespace
 
 }  // namespace sgdml
@@ -1013,8 +1244,10 @@ struct StepParams {
   RemdParams remd;
   NptParams npt;
   MetadParams metad;
+  DimerParams dimer;
 };
 constexpr size_t STEP_PARAMS_BYTES = (sizeof(StepParams) + 255) & ~(size_t)255;  // where the tables start
+static_assert(STEP_PARAMS_BYTES == 768, "the dimer's parameters fit in the padding: the tables do not move");
 
 // What a captured step bakes in besides the force evaluation: the integrator (MdKind), the replicas per group (the
 // grids of the NEB and exchange kernels) and the upload block (the tab and sigma kernel arguments point into it).
@@ -1063,6 +1296,11 @@ struct sgdml_b200_md {
   // nudged elastic band (sgdml_b200_neb_fire), allocated by the first NEB call
   double* Fn = nullptr;       // (n_rep, 3N) NEB forces of the interior images
   int* climb_idx = nullptr;   // (n_rep) the highest interior image of each band (the first n_rep / P entries)
+  // dimer search (sgdml_b200_dimer_fire), allocated by the first dimer call; F-dagger goes to Fn
+  double *dmode = nullptr, *dtheta = nullptr;  // (n_rep / 2, 3N) unit modes, and T (or a caller's modes in transit)
+  DimerState* dstate = nullptr;               // (n_rep / 2)
+  int* dbad = nullptr;                        // (n_rep / 2) k_dimer_init's verdict per mode
+  bool has_modes = false;                     // dmode holds the modes of an earlier call
   // replica exchange (sgdml_b200_remd_run), allocated by the first replica-exchange call
   int* walker = nullptr;      // (n_rep) walker label per slot
   int64_t* xcount = nullptr;  // (2, n_rep) accepted and attempted swaps of the current run
@@ -1098,7 +1336,9 @@ void md_free(sgdml_b200_md* md) {
   force_eval_destroy(md->fe);
   for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s}) cached_free(p);
   for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev, md->Fn, md->W, md->Ws}) cached_free(p);
-  for (double* p : {md->Fm, md->cv, md->Vb, md->Fb, md->hc, md->hw, md->hh}) cached_free(p);
+  for (double* p : {md->Fm, md->cv, md->Vb, md->Fb, md->hc, md->hw, md->hh, md->dmode, md->dtheta}) cached_free(p);
+  cached_free(md->dstate);
+  cached_free(md->dbad);
   cached_free(md->hcount);
   cached_free(md->step);
   cached_free(md->blk);
@@ -1212,13 +1452,13 @@ class Outputs {
 // what one step of the handle's graph integrates
 enum MdKind {
   MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, MD_NEB_FIRE = 4, MD_REMD = 5, MD_NPT = 6,
-  MD_METAD = 7
+  MD_METAD = 7, MD_DIMER = 8
 };
 
 // the integrator of sgdml_b200_md_run, sgdml_b200_remd_run, sgdml_b200_npt_run, sgdml_b200_pimd_run,
-// sgdml_b200_relax_* or sgdml_b200_neb_fire; advance == 0 completes a run's last step (MD; a replica exchange first exchanges that last
-// state) or only tests convergence (relaxation, NEB: after the force projection).  L-BFGS keeps its direction in V,
-// which relax_impl zeroes after.
+// sgdml_b200_relax_*, sgdml_b200_neb_fire or sgdml_b200_dimer_fire; advance == 0 completes a run's last step (MD; a
+// replica exchange first exchanges that last state) or only tests convergence (relaxation, NEB: after the force
+// projection, dimer: with the curvature).  L-BFGS keeps its direction in V, which relax_impl zeroes after.
 int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
   StepParams* p = md->params(md->blk);
   switch (kind) {
@@ -1245,6 +1485,10 @@ int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
                                                                advance);
       break;
     }
+    case MD_DIMER:
+      k_dimer_step<<<(unsigned)(md->n_rep / 2), MD_THREADS, 0, s>>>(&p->dimer, md->rst, md->dstate, md->R, md->V, md->F,
+                                                                   md->Fn, md->dmode, md->dtheta, md->dimi, advance);
+      break;
     case MD_NPT:
       k_npt_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&p->md, &p->npt, md->s, md->sigma(md->blk), md->R, md->V,
                                                             md->F, md->E, md->W, md->cell, md->lat, md->step, md->dimi,
@@ -1619,8 +1863,9 @@ constexpr int64_t RELAX_BLOCK = 16;  // replays between convergence read-backs
 int64_t g_relax_block = 0;           // sgdml_b200_set_relax_block (test hook): 0 = RELAX_BLOCK
 
 // the optimiser state, made at the first relaxation; the L-BFGS ring grows to `memory` pairs per replica, and the NEB
-// buffers are made at the first NEB call
-int relax_alloc(sgdml_b200_md* md, int memory, bool neb) {
+// and dimer buffers are made at the first call of that kind
+int relax_alloc(sgdml_b200_md* md, int memory, int kind) {
+  const bool neb = kind == MD_NEB_FIRE, dimer = kind == MD_DIMER;
   if (md->rst == nullptr) SG_CUDA(cached_malloc(&md->rst, sizeof(RelaxState) * (size_t)md->n_rep));
   if (md->hActive == nullptr) {
     SG_CUDA(cudaHostAlloc(&md->hActive, sizeof(int), cudaHostAllocMapped));
@@ -1629,7 +1874,15 @@ int relax_alloc(sgdml_b200_md* md, int memory, bool neb) {
   if (md->counted == nullptr) SG_CUDA(cudaEventCreateWithFlags(&md->counted, cudaEventDisableTiming));
   if (neb) {
     if (md->climb_idx == nullptr) SG_CUDA(cached_malloc(&md->climb_idx, sizeof(int) * (size_t)md->n_rep));
-    if (md->Fn == nullptr) SG_CUDA(cached_malloc(&md->Fn, sizeof(double) * (size_t)(md->n_rep * md->dimi)));
+  }
+  if ((neb || dimer) && md->Fn == nullptr)
+    SG_CUDA(cached_malloc(&md->Fn, sizeof(double) * (size_t)(md->n_rep * md->dimi)));
+  if (dimer && md->dstate == nullptr) {
+    const size_t nd = (size_t)(md->n_rep / 2);
+    SG_CUDA(cached_malloc(&md->dmode, sizeof(double) * nd * md->dimi));
+    SG_CUDA(cached_malloc(&md->dtheta, sizeof(double) * nd * md->dimi));
+    SG_CUDA(cached_malloc(&md->dbad, sizeof(int) * nd));
+    SG_CUDA(cached_malloc(&md->dstate, sizeof(DimerState) * nd));
   }
   if (memory > md->m_cap) {
     const size_t vec = sizeof(double) * (size_t)(md->n_rep * md->dimi);
@@ -1651,26 +1904,76 @@ int relax_alloc(sgdml_b200_md* md, int memory, bool neb) {
   return 0;
 }
 
-// Relaxes every replica (or NEB band) from the handle's state: blocks of step-graph replays, each followed by the
-// convergence test and a count of unconverged units read back through mapped pinned memory; stops when none is left or
-// after max_steps.  The unit of convergence is a group of g consecutive replicas: g = 1 for relaxation, g = P for NEB
-// (whose climbing_out gets each band's highest interior image).  call: the entry point's RelaxParams (FIRE, L-BFGS;
-// the handle's L-BFGS ring is added here) or NebParams (NEB).  memory: L-BFGS pairs per replica to allocate (0: none).
-// Frozen units make the block length a matter of cost only.  V is zero before and after.
+// What a dimer search (sgdml_b200_dimer_fire) adds to relax_impl: the caller's modes (null: the handle's) and its
+// outputs per dimer.
+struct DimerRun {
+  const double* modes;
+  double* curvature_out;
+  int64_t* n_rot_out;
+  double* modes_out;
+};
+
+// The start of a dimer search, after the upload: k_dimer_init on scratch (the modes into Fn's first n_dimers rows,
+// the images into the next), the verdict read back, and only then the commit -- modes, images, a zero DimerState --
+// and one un-captured force evaluation of every replica.  A bad mode is an argument error with the handle unchanged.
+// A rejected call has still overwritten dtheta (the caller's modes in transit), Fn (the scratch rows) and the dimer
+// part of the upload block: none of them carries anything from one call to the next -- every dimer call rewrites all
+// three before it reads them, and Fn's rows are rewritten by every NEB force evaluation -- so keep it that way when
+// using them across calls.
+int dimer_start(sgdml_b200_md* md, const double* modes, cudaStream_t s) {
+  const int64_t nd = md->n_rep / 2;
+  const size_t row = sizeof(double) * (size_t)md->dimi, rows = row * (size_t)nd;
+  const double* src = md->dmode;
+  if (modes != nullptr) {
+    SG_CUDA(cudaMemcpyAsync(md->dtheta, modes, rows, cudaMemcpyDefault, s));
+    src = md->dtheta;
+  }
+  double* nd_s = md->Fn;
+  double* img_s = md->Fn + nd * md->dimi;
+  k_dimer_init<<<(unsigned)nd, MD_THREADS, 0, s>>>(&md->params(md->blk)->dimer, md->R, src, nd_s, img_s, md->dbad,
+                                                    md->dimi);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_MISC);
+  std::vector<int> bad((size_t)nd);
+  SG_CUDA(cudaMemcpyAsync(bad.data(), md->dbad, sizeof(int) * (size_t)nd, cudaMemcpyDeviceToHost, s));
+  SG_CUDA(cudaStreamSynchronize(s));
+  for (int b : bad)
+    if (b) return fail_arg("sgdml_b200_dimer_fire: every mode must be finite and not (almost) a rigid motion");
+  SG_CUDA(cudaMemcpyAsync(md->dmode, nd_s, rows, cudaMemcpyDeviceToDevice, s));
+  SG_CUDA(cudaMemcpy2DAsync(md->R + md->dimi, 2 * row, img_s, row, row, (size_t)nd, cudaMemcpyDeviceToDevice, s));
+  SG_CUDA(cudaMemsetAsync(md->dstate, 0, sizeof(DimerState) * (size_t)nd, s));
+  md->has_modes = true;
+  return md_state_forces(md, 0, s);
+}
+
+// Relaxes every replica (or NEB band, or dimer) from the handle's state: blocks of step-graph replays, each followed
+// by the convergence test and a count of unconverged units read back through mapped pinned memory; stops when none is
+// left or after max_steps.  The unit of convergence is a group of g consecutive replicas: g = 1 for relaxation, g = P
+// for NEB (whose climbing_out gets each band's highest interior image), g = 2 for the dimer (dm: its modes and
+// outputs).  call: the entry point's RelaxParams (FIRE, L-BFGS; the handle's L-BFGS ring is added here), NebParams
+// (NEB) or DimerParams (dimer).  memory: L-BFGS pairs per replica to allocate (0: none).  Frozen units make the block
+// length a matter of cost only.  V is zero before and after.
 int relax_impl(sgdml_b200_md* md, int kind, int g, int memory, const StepParams& call, int64_t max_steps,
-               int64_t* n_steps_out, int* conv_out, double* fmax_out, int* climbing_out, cudaStream_t s) {
+               int64_t* n_steps_out, int* conv_out, double* fmax_out, int* climbing_out, cudaStream_t s,
+               const DimerRun* dm = nullptr) {
   md->group = g;
   const int64_t n_rep = md->n_rep;
   const int64_t n_units = n_rep / g;
   SG_TRY(force_eval_prepare(md->fe));
-  SG_TRY(relax_alloc(md, memory, kind == MD_NEB_FIRE));
+  SG_TRY(relax_alloc(md, memory, kind));
   Outputs out(s);
-  SG_TRY(out.init({{n_steps_out, sizeof(int64_t) * (size_t)n_units}, {conv_out, sizeof(int) * (size_t)n_units},
-                   {fmax_out, sizeof(double) * (size_t)n_units}, {climbing_out, sizeof(int) * (size_t)n_units}}));
+  const size_t un = (size_t)n_units;
+  SG_TRY(out.init({{n_steps_out, sizeof(int64_t) * un}, {conv_out, sizeof(int) * un},
+                   {fmax_out, sizeof(double) * un}, {climbing_out, sizeof(int) * un},
+                   {dm ? dm->curvature_out : nullptr, sizeof(double) * un},
+                   {dm ? dm->n_rot_out : nullptr, sizeof(int64_t) * un},
+                   {dm ? dm->modes_out : nullptr, sizeof(double) * un * md->dimi}}));
   SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the mirror
   StepParams& p = *md->params(md->hblk);
   if (kind == MD_NEB_FIRE) {
     p.neb = call.neb;
+  } else if (kind == MD_DIMER) {
+    p.dimer = call.dimer;
   } else {
     p.relax = call.relax;
     p.relax.m_cap = md->m_cap;
@@ -1681,6 +1984,7 @@ int relax_impl(sgdml_b200_md* md, int kind, int g, int memory, const StepParams&
     p.relax.g_prev = md->g_prev;
   }
   SG_TRY(upload(md, &p + 1, s));
+  if (kind == MD_DIMER) SG_TRY(dimer_start(md, dm->modes, s));
   const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
   SG_CUDA(cudaMemsetAsync(md->rst, 0, sizeof(RelaxState) * (size_t)n_units, s));
   SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
@@ -1703,6 +2007,13 @@ int relax_impl(sgdml_b200_md* md, int kind, int g, int memory, const StepParams&
   SG_CUDA(cudaGetLastError());
   count_launch(KID_MISC);
   SG_TRY(out.copy_from(3, {md->climb_idx}));  // the last test ran k_neb_force at the final positions
+  if (kind == MD_DIMER) {
+    k_dimer_report<<<(unsigned)((n_units + 255) / 256), 256, 0, s>>>(md->dstate, n_units, out.dev<double>(4),
+                                                                    out.dev<int64_t>(5));
+    SG_CUDA(cudaGetLastError());
+    count_launch(KID_MISC);
+    SG_TRY(out.copy_from(6, {md->dmode}));
+  }
   return out.finish();
 }
 
@@ -2207,6 +2518,41 @@ int sgdml_b200_neb_fire(sgdml_b200_md* md, int64_t n_images, int64_t max_steps, 
   c.neb.P = (int)n_images;
   return relax_impl(md, MD_NEB_FIRE, (int)n_images, 0, c, max_steps, n_steps_out, converged_out, fmax_out,
                     climbing_out, (cudaStream_t)stream);
+}
+
+int sgdml_b200_dimer_fire(sgdml_b200_md* md, const double* modes, int64_t max_steps, double fmax, double separation,
+                          double cos_trial, double sin_trial, double rot_min, double maxstep, double dt, double dtmax,
+                          int64_t* n_steps_out, int* converged_out, double* fmax_out, double* curvature_out,
+                          int64_t* n_rot_out, double* modes_out, void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(relax_check(md, max_steps, fmax, maxstep,
+                     "sgdml_b200_dimer_fire: no state yet (call sgdml_b200_md_set_state)"));
+  if (md->nb > 1) return fail_arg("sgdml_b200_dimer_fire: a ring-polymer handle (n_beads > 1) holds no dimers");
+  if (md->n_rep % 2 != 0) return fail_arg("sgdml_b200_dimer_fire: n_rep must be even (a centre and an image per dimer)");
+  if (modes == nullptr && !md->has_modes)
+    return fail_arg("sgdml_b200_dimer_fire: no modes yet (pass modes on the handle's first dimer call)");
+  SG_ARG(std::isfinite(separation) && separation > 0.0);
+  SG_ARG(std::isfinite(cos_trial) && cos_trial > 0.0 && std::isfinite(sin_trial) && sin_trial > 0.0);
+  SG_ARG(std::fabs(cos_trial * cos_trial + sin_trial * sin_trial - 1.0) < 1e-12);
+  SG_ARG(std::isfinite(rot_min) && rot_min >= 0.0);
+  SG_ARG(std::isfinite(dt) && dt > 0.0);
+  SG_ARG(std::isfinite(dtmax) && dtmax > 0.0);
+  StepParams c = {};
+  DimerParams& q = c.dimer;
+  q.D = separation;
+  q.c_t = cos_trial;
+  q.s_t = sin_trial;
+  q.s2_t = 2.0 * sin_trial * cos_trial;
+  q.omc2_t = 2.0 * sin_trial * sin_trial;
+  q.rot_min = rot_min;
+  q.fmax2 = fmax * fmax;
+  q.maxstep = maxstep;
+  q.dt0 = dt;
+  q.dtmax = dtmax;
+  q.periodic = force_eval_periodic(md->fe) ? 1 : 0;
+  const DimerRun dm = {modes, curvature_out, n_rot_out, modes_out};
+  return relax_impl(md, MD_DIMER, 2, 0, c, max_steps, n_steps_out, converged_out, fmax_out, nullptr,
+                    (cudaStream_t)stream, &dm);
 }
 
 int sgdml_b200_set_relax_block(int64_t n_steps) {

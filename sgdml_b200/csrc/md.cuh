@@ -1,7 +1,7 @@
 // Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_metad_*,
-// sgdml_b200_pimd_*, sgdml_b200_relax_*, sgdml_b200_neb_fire): the contract of the kernels in md.cu -- the BAOAB
-// integrator step, the replica exchange, the NPT step, the metadynamics bias, the ring-polymer step, their counter-based
-// noise, the FIRE and L-BFGS steps, and the nudged elastic band.
+// sgdml_b200_pimd_*, sgdml_b200_relax_*, sgdml_b200_neb_fire, sgdml_b200_dimer_fire): the contract of the kernels in
+// md.cu -- the BAOAB integrator step, the replica exchange, the NPT step, the metadynamics bias, the ring-polymer step,
+// their counter-based noise, the FIRE and L-BFGS steps, the nudged elastic band and the dimer search.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -262,6 +262,71 @@ struct NebParams {
   double k;                           // spring constant (force unit / L)
   int climb;                          // 1: the highest interior image climbs
   int P;                              // images per band (>= 3)
+};
+
+// Dimer saddle search (sgdml_b200_dimer_fire; Henkelman & Jonsson, J. Chem. Phys. 111, 7010 (1999)).  The handle's
+// n_rep = 2 n_dimers replicas: replica 2d is the centre R0 of dimer d, replica 2d + 1 its image R1 = R0 + D N, with N
+// the dimer's unit mode (n_dimers, 3N) and D the separation.  Every force evaluation covers both (F0, F1); the image 2
+// is the central difference F2 = 2 F0 - F1, never evaluated.  Per dimer, with block_sum's order for every sum below
+// (over the dimer's 3N coordinates, thread t adding its coordinates i = t, t + MD_THREADS, ... from 0.0, then the tree)
+// and every operation rounded as written (no fused multiply-add):
+//   C    = (sum_i (F0_i - F1_i) N_i) / D                        the curvature along N
+//   G_i  = (F1_i - F0_i) / D;  g = sum_i G_i N_i;  P_i = G_i - g N_i;  f = sqrt(sum_i P_i P_i)   the rotational force
+//
+// k_dimer_step: one CTA of MD_THREADS per dimer, the dimer's RelaxState and DimerState.  Each launch:
+//   1. Test (as k_fire_step: first, a converged dimer frozen for the rest of the call).  In phase EVAL_N, C_N = C of
+//      the current forces.  fmax2 = atom_max2(F0);  conv = fmax2 < fmax2_thr and C_N < 0.  advance == 0 stops here.
+//   2. EVAL_N (F1 belongs to R0 + D N).  If f < rot_min or f == 0: translate (4) with C_use = C_N.  Otherwise
+//      T_i = P_i / f, C0 = C_N, b1 = -f, the image R1_i = R0_i + D Nt_i with Nt_i = c_t N_i + s_t T_i, phase TRIAL;
+//      nothing else moves.
+//   3. TRIAL (F1 belongs to R0 + D Nt; F0 unchanged): the curvature fit C(phi) = a0 / 2 + a1 cos 2phi + b1 sin 2phi in
+//      the plane (N, T) (Heyden, Bell & Keil, JCP 123, 224101 (2005); Kastner & Sherwood, JCP 128, 014106 (2008)):
+//        Ct = (sum_i (F0_i - F1_i) Nt_i) / D;  a1 = ((C0 - Ct) + b1 s2_t) / omc2_t;  r = sqrt(a1 a1 + b1 b1);
+//        c2 = (-a1) / r;  s2 = (-b1) / r;
+//        c2 >= 0:  c = sqrt((1 + c2) / 2), s = s2 / (2 c);   else:  s = sqrt((1 - c2) / 2), c = s2 / (2 s);
+//        N_i = c N_i + s T_i, then the rigid projection and normalisation (5);  C_use = (C0 - a1) - r;  n_rot += 1
+//   4. Translate:  p = sum_i F0_i N_i;  C_use < 0:  Fd_i = F0_i - (2 p) N_i;  else  Fd_i = -(p N_i);  then
+//      fire_update (k_fire_step's FIRE, its constants and whole-vector maxstep cap) on R0 and the centre's V row with
+//      Fd (which it keeps in the handle's Fn, row 2d), which counts the step in n_steps;  R1_i = R0_i + D N_i;  phase
+//      EVAL_N.
+// c_t = cos phi_t, s_t = sin phi_t, s2_t = 2 s_t c_t and omc2_t = 2 s_t s_t (1 - cos 2phi_t) are computed once on the
+// host, so the kernels and tests/dimer_oracle.py use the same doubles.
+//
+// 5. Rigid projection of a mode N at centre R0 (n atoms), then N = N / sqrt(sum_i N_i N_i).  "Component sums" are
+// block_sums over the 3N coordinates of the vector holding x_i at the coordinates i = 3a + c of component c and 0.0
+// elsewhere; "atom sums" hold the atom's term at coordinate 3a and 0.0 at 3a + 1, 3a + 2 (a multi-value reduction with
+// block_sum's tree for each value gives the same bits).
+//   translations:  m_c = (component sum of N) / n,  N_i = N_i - m_c(i)
+//   rotations (free molecules only; periodic models remove the translations only):
+//     rb_c = (component sum of R0) / n;  x_a = R0_a - rb;  L = atom sums of cross(x_a, N_a);
+//     I_00 = atom sum of (x1 x1 + x2 x2), I_11 of (x0 x0 + x2 x2), I_22 of (x0 x0 + x1 x1), I_01 = -(atom sum of
+//     x0 x1), I_02 = -(x0 x2), I_12 = -(x1 x2);  cofactors A00 = I11 I22 - I12 I12, A01 = I02 I12 - I01 I22,
+//     A02 = I01 I12 - I11 I02, A11 = I00 I22 - I02 I02, A12 = I01 I02 - I00 I12, A22 = I00 I11 - I01 I01;
+//     det = (I00 A00 + I01 A01) + I02 A02;  t = ((I00 + I11) + I22) / 3;  if det > 1e-10 ((t t) t):
+//     w_0 = ((A00 L0 + A01 L1) + A02 L2) / det, w_1 = ((A01 L0 + A11 L1) + A12 L2) / det,
+//     w_2 = ((A02 L0 + A12 L1) + A22 L2) / det, and N_a = N_a - cross(w, x_a); otherwise (a linear or one-atom
+//     geometry) no rotational part.
+//   cross(a, b) = (a1 b2 - a2 b1, a2 b0 - a0 b2, a0 b1 - a1 b0), as the metadynamics CVs.
+//
+// k_dimer_init: one CTA of MD_THREADS per dimer, before the force evaluation of a call: the projection (5) of the
+// source mode at the dimer's centre into a scratch mode, the image R0 + D N into a scratch image, and bad[d] = 1 when
+// the source's N.N (before the projection) is not finite or the projected N.N is not above 1e-12 of it (a mode that is
+// (almost) a rigid motion).  The driver commits the scratch rows only when no dimer is bad.
+enum DimerPhase { DIMER_EVAL_N = 0, DIMER_TRIAL = 1 };
+
+struct DimerState {  // per dimer, zeroed at the start of every call (phase EVAL_N)
+  int phase;
+  int64_t n_rot;     // rotations in this call
+  double C_N;        // the curvature last measured along N at the current centre
+  double C0, b1;     // TRIAL: C_N and -f of the rotation being fitted
+};
+
+struct DimerParams {
+  double D;                    // separation (L)
+  double c_t, s_t, s2_t, omc2_t;  // the trial rotation
+  double rot_min;              // below this |rotational force| (force / L^2) the dimer translates without rotating
+  double fmax2, maxstep, dt0, dtmax;  // the centre's FIRE, as in RelaxParams
+  int periodic;                // 1: remove the translations only
 };
 
 }  // namespace sgdml

@@ -2533,6 +2533,8 @@ bool sgdml::force_eval_stale(const ForceEval* fe) {
   return fe->moved || fe->generation != fe->m->generation || !same_cell(fe->lat, fe->m->lat);
 }
 
+bool sgdml::force_eval_periodic(const ForceEval* fe) { return fe->m->lat.on != 0; }
+
 void sgdml::force_eval_mark(ForceEval* fe) {
   fe->moved = false;
   fe->generation = fe->m->generation;

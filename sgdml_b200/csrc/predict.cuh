@@ -55,6 +55,8 @@ int force_eval_prepare(ForceEval* fe);
 // reallocated since, or the model's generation (use_ae, contraction slices) or cell has changed
 bool force_eval_stale(const ForceEval* fe);
 void force_eval_mark(ForceEval* fe);
+// true when the model has a periodic cell
+bool force_eval_periodic(const ForceEval* fe);
 // R (n_geo, 3N) -> F (n_geo, 3N), E (n_geo), all device arrays; chunk by chunk when n_geo exceeds the predictor's chunk
 int force_eval_run(ForceEval* fe, const double* R, double* F, double* E, cudaStream_t s);
 // As force_eval_run, with geometry g in its own cell cells[g] (n_geo cells in DEVICE memory), also writing the virial

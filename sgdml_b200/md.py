@@ -16,7 +16,9 @@ groups of Langevin walkers, each group sharing one store of Gaussian hills on di
 variables, for free-energy surfaces along chosen coordinates.
 
 ``GDMLRelaxation`` -- geometry optimisation of many replicas on the same engine (``sgdml_b200_relax_*``): FIRE and
-L-BFGS, each replica frozen once it has converged.
+L-BFGS, each replica frozen once it has converged.  ``GDMLNEB`` and ``GDMLDimer`` find saddle points on it: between
+two minima with the nudged elastic band (``sgdml_b200_neb_fire``), or next to one minimum with the dimer method
+(``sgdml_b200_dimer_fire``).
 
 Units follow ASE and ``intf.ase_calc.SGDMLCalculator``: positions in Angstrom, velocities in Angstrom/fs, masses in
 amu, energies in eV, time in fs, temperature in K.  ``E_to_eV`` and ``F_to_eV_Ang`` convert the model's units as in
@@ -25,6 +27,7 @@ femtosecond as its time unit.
 """
 
 import ctypes
+import math
 
 import numpy as np
 
@@ -845,6 +848,109 @@ class GDMLNEB(GDMLRelaxation):
         return {'positions': st['positions'].reshape(shape + (self.n_atoms, 3)),
                 'forces': st['forces'].reshape(shape + (self.n_atoms, 3)), 'energies': E, 'barrier': top_E - E[:, 0],
                 'climbing_image': top, 'fmax': fm * self.F_to_eV_Ang, 'converged': conv != 0, 'n_steps': n_steps}
+
+
+class GDMLDimer(GDMLRelaxation):
+    """First-order saddle points next to a minimum, with no final state, by the dimer method (Henkelman & Jonsson,
+    J. Chem. Phys. 111, 7010 (1999)) on the device (``sgdml_b200_dimer_fire``): `n_dimers` independent searches, many
+    steps per call.  Dimer d is replicas 2d (its centre) and 2d + 1 (its image, the centre plus `separation` along the
+    dimer's unit mode) of a ``GDMLRelaxation`` handle; the mode follows the lowest-curvature direction (one rotation per
+    translation at most, by the curvature fit of Heyden, Bell & Keil, J. Chem. Phys. 123, 224101 (2005)) and the centre
+    moves by FIRE up that mode and down every other.  The mode is kept orthogonal to rigid translations and, for free
+    molecules, rotations.
+
+    ``search(positions=None, modes=None, fmax=0.05, max_steps=1000, separation=1e-4, trial_angle=pi/4, rot_min=0.1,
+    maxstep=0.1, dt=0.1, dtmax=1.0, seed=0)`` runs until every dimer has max_a |F_a| < fmax at its centre with a
+    negative curvature along its mode, or `max_steps` force evaluations of the pairs (a rotating step takes two).
+    Units are ASE's: positions (n_dimers, N, 3), or (N, 3) for every dimer, in Angstrom (None: continue from the
+    current centres); modes (n_dimers, N, 3) or (N, 3), any length (None: keep the modes of the previous call, or on
+    the first call Gaussian modes from ``numpy.random.default_rng(seed)``); fmax in eV/Angstrom; separation and maxstep
+    (the centre's whole step) in Angstrom; rot_min, the rotational force below which a dimer translates without
+    rotating, in eV/Angstrom^2; dt and dtmax as in ``GDMLRelaxation.relax``.  Returns, for the centres, {'positions',
+    'forces', 'mode' (unit, (n_dimers, N, 3)), 'potential_energy', 'curvature' (eV/Angstrom^2, along the final mode),
+    'fmax', 'converged', 'n_steps' (translations), 'n_rotations': (n_dimers,)}.  NumPy arrays or float64 CUDA tensors
+    in, the same kind out."""
+
+    def __init__(self, model, n_dimers=1, E_to_eV=_KCAL_PER_MOL_IN_EV, F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        self.n_dimers = int(n_dimers)
+        if self.n_dimers < 1:
+            raise ValueError('n_dimers must be >= 1')
+        self._has_modes = False
+        super().__init__(model, 2 * self.n_dimers, E_to_eV, F_to_eV_Ang)
+
+    def _per_dimer(self, x, name):
+        """(n_dimers, N, 3) or (N, 3) -> (n_dimers, 3N), the same kind; torch inputs must be float64 CUDA tensors."""
+        if hasattr(x, 'data_ptr'):
+            _check_cuda_f64(x, name)
+        shape = tuple(x.shape)
+        N = self.n_atoms
+        if shape == (N, 3):
+            x = x.reshape(1, N, 3)
+            x = x.expand(self.n_dimers, N, 3) if hasattr(x, 'data_ptr') else np.broadcast_to(x, (self.n_dimers, N, 3))
+        elif shape != (self.n_dimers, N, 3):
+            raise ValueError('%s must be (n_dimers, N, 3) = (%d, %d, 3) or (N, 3): %s'
+                             % (name, self.n_dimers, N, shape))
+        if hasattr(x, 'data_ptr'):
+            return x.reshape(self.n_dimers, 3 * N).contiguous()
+        return np.ascontiguousarray(x, dtype=np.float64).reshape(self.n_dimers, 3 * N)
+
+    # ------------------------------------------------------------------ model units
+    def _dimer_raw(self, modes, max_steps, fmax, separation, cos_trial, sin_trial, rot_min, maxstep, dt, dtmax):
+        """modes (n_dimers, 3N) or None (keep) -> (n_steps, converged, fmax, curvature, n_rot (n_dimers,), modes
+        (n_dimers, 3N)), in model units."""
+        n = self.n_dimers
+        if modes is not None:  # the entry point copies n_dimers 3N doubles from this pointer
+            if hasattr(modes, 'data_ptr'):
+                _check_cuda_f64(modes, 'modes')
+                modes = modes.contiguous()
+            else:
+                modes = np.ascontiguousarray(modes, dtype=np.float64)
+            if tuple(modes.shape) != (n, 3 * self.n_atoms):
+                raise ValueError('modes must be (n_dimers, 3N) = (%d, %d): %s' % (n, 3 * self.n_atoms,
+                                                                                  tuple(modes.shape)))
+        out = (self._empty(n, np.int64), self._empty(n, np.int32), self._empty(n), self._empty(n),
+               self._empty(n, np.int64), self._empty((n, 3 * self.n_atoms)))
+        _lib.check(
+            _lib.lib().sgdml_b200_dimer_fire(self._handle, _lib.ptr(modes), int(max_steps), float(fmax),
+                                             float(separation), float(cos_trial), float(sin_trial), float(rot_min),
+                                             float(maxstep), float(dt), float(dtmax), *(_lib.ptr(x) for x in out),
+                                             _lib.current_stream()),
+            'dimer_fire',
+        )
+        self._has_modes = True
+        return out
+
+    # ------------------------------------------------------------------ ASE units
+    def search(self, positions=None, modes=None, fmax=0.05, max_steps=1000, separation=1e-4, trial_angle=np.pi / 4,
+               rot_min=0.1, maxstep=0.1, dt=0.1, dtmax=1.0, seed=0):
+        # both are checked before the state changes
+        R = None if positions is None else self._per_dimer(positions, 'positions')
+        if modes is not None:
+            modes = self._per_dimer(modes, 'modes')
+        if R is not None:
+            R = R.repeat_interleave(2, 0) if hasattr(R, 'data_ptr') else np.repeat(R, 2, axis=0)
+            self.set_state(R.reshape(self.n_replicas, self.n_atoms, 3))
+        if modes is None and not self._has_modes:
+            modes = np.random.default_rng(seed).standard_normal((self.n_dimers, 3 * self.n_atoms))
+        c = self.Ang_to_R * self.F_to_eV_Ang  # eV / Angstrom^2 -> model force / model length, and dt^2
+        phi = float(trial_angle)
+        n_steps, conv, fm, curv, n_rot, mode = self._dimer_raw(
+            modes, max_steps, float(fmax) / self.F_to_eV_Ang, float(separation) * self.Ang_to_R, math.cos(phi),
+            math.sin(phi), float(rot_min) / c, float(maxstep) * self.Ang_to_R, float(dt) * np.sqrt(c),
+            float(dtmax) * np.sqrt(c))
+        st = self.get_state()
+        g = (self.n_dimers, self.n_atoms, 3)
+        return {'positions': st['positions'][0::2].reshape(g), 'forces': st['forces'][0::2].reshape(g),
+                'potential_energy': st['potential_energy'][0::2], 'mode': mode.reshape(g), 'curvature': curv * c,
+                'fmax': fm * self.F_to_eV_Ang, 'converged': conv != 0, 'n_steps': n_steps, 'n_rotations': n_rot}
+
+
+def _check_cuda_f64(x, name):
+    """A torch input handed to the engine as a pointer must be a float64 CUDA tensor."""
+    import torch
+
+    if x.dtype != torch.float64 or not x.is_cuda:
+        raise ValueError('%s: torch inputs must be float64 CUDA tensors' % name)
 
 
 def kabsch_align(x, ref):

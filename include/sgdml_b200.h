@@ -161,7 +161,17 @@ int sgdml_b200_predict_hvp(sgdml_b200_model* model, const double* R, const doubl
  * change.  Later runs do evaluate the changed model.  Batches above the predictor's chunk size (fixed when the handle is
  * created) run their chunks inside each step.  Launches count under family 8 (integrator) and 1 (graph replays).
  * Arrays are host or device pointers as elsewhere in this header; calls with host outputs synchronise `stream`.
- * Argument errors are reported before anything is queued, and a rejected call changes nothing. */
+ * Argument errors are reported before anything is queued, and a rejected call changes nothing.
+ * Handle kinds: the call that makes a handle fixes its kind.  sgdml_b200_md_create, and sgdml_b200_pimd_create with
+ * n_beads = 1, make plain handles; sgdml_b200_pimd_create with n_beads > 1 makes ring-polymer handles,
+ * sgdml_b200_npt_create NPT handles and sgdml_b200_metad_create metadynamics handles.  An entry point called with a
+ * handle of a kind it does not take (no x below) returns an argument error:
+ *   entry point                                                              plain  ring  NPT  metadynamics
+ *   sgdml_b200_md_set_state, _md_get_state, _md_destroy                        x     x     x        x
+ *   sgdml_b200_md_run, _remd_run, _neb_fire, _dimer_fire                       x
+ *   sgdml_b200_pimd_run, _relax_fire, _relax_lbfgs                             x     x
+ *   sgdml_b200_npt_run, _npt_set_cells, _npt_get_cells                                     x
+ *   sgdml_b200_metad_run, _metad_get_hills, _metad_set_hills, _metad_get_bias                       x */
 typedef struct sgdml_b200_md sgdml_b200_md;
 /* inv_mass (N,) HOST doubles, each finite and > 0; n_rep >= 1. */
 int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* model, int64_t n_rep, const double* inv_mass);
@@ -182,8 +192,8 @@ int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamm
 
 /* ---------------------------------------------------------------- replica-exchange molecular dynamics on the device
  * Extension: temperature replica exchange (parallel tempering; Sugita & Okamoto, Chem. Phys. Lett. 314, 141 (1999)) of
- * Langevin replicas, with the exchanges inside the step graph (no host round trip per exchange).  The handle
- * (sgdml_b200_md_create; a ring-polymer handle is rejected) holds n_rep = n_ladders n_temps replicas: slot
+ * Langevin replicas, with the exchanges inside the step graph (no host round trip per exchange).  The handle (plain:
+ * see the handle kinds at sgdml_b200_md_create) holds n_rep = n_ladders n_temps replicas: slot
  * l n_temps + k sits at temperature kT[k] of ladder l for the whole run, and exchanges move configurations between
  * neighbouring slots, never temperatures, so frames and the state are sorted by temperature.  Between exchanges every
  * slot runs sgdml_b200_md_run's BAOAB step with its own sigma_i = sqrt((1 - c1^2) kT[k] s_i); units, streams, the
@@ -225,8 +235,8 @@ int sgdml_b200_remd_run(sgdml_b200_md* md, int64_t n_temps, const double* kT, in
  * its own that the barostat scales.  Units are the model's: P0 in energy / L^3, beta_T (isothermal compressibility) in
  * L^3 / energy, tau_p in T.  An NPT handle is an sgdml_b200_md handle with one cell per replica:
  * sgdml_b200_md_set_state evaluates F, E_pot and the virial W = -dE/d(strain) of each replica in its own cell;
- * sgdml_b200_md_get_state and sgdml_b200_md_destroy are unchanged; sgdml_b200_md_run, _remd_run, _pimd_run, _relax_*
- * and _neb_fire on it are argument errors, as is sgdml_b200_npt_run on any other handle.
+ * sgdml_b200_md_get_state and sgdml_b200_md_destroy are unchanged.  Which other entry points take an NPT handle: the
+ * handle kinds at sgdml_b200_md_create.
  * Barostat state per replica: eps, the log of its volume ratio V / V0 since the cell was set, its base cell L0 with
  * the caller's inverse, and V0 = |det L0| (host).  The replica is evaluated in L = a L0 with inverse L0^-1 / a,
  * a = exp(eps / 3).  One step, with the replica's step index at n and its W of the current state:
@@ -277,10 +287,9 @@ int sgdml_b200_npt_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gam
  * walker of a group is biased by the same hills, those committed before state c: a hill becomes visible to the
  * evaluation of the next state, never to its own.  sgdml_b200_md_set_state evaluates the model and then the bias
  * without a deposit, so a run continued over several calls is one long run.  sgdml_b200_md_get_state's F and E_pot
- * stay the model's.  sgdml_b200_md_run, _remd_run, _pimd_run, _npt_run, _relax_* and _neb_fire on a metadynamics
- * handle are argument errors, as are the sgdml_b200_metad_* calls on any other handle.  Streams, host/device outputs,
- * SGDML_B200_GRAPH=0 and the workspace are those of sgdml_b200_md_run; argument errors are reported before anything
- * is queued, and a rejected call changes nothing. */
+ * stay the model's.  Which entry points take a metadynamics handle: the handle kinds at sgdml_b200_md_create.
+ * Streams, host/device outputs, SGDML_B200_GRAPH=0 and the workspace are those of sgdml_b200_md_run; argument errors
+ * are reported before anything is queued, and a rejected call changes nothing. */
 /* n_groups, n_walkers >= 1, n_groups n_walkers <= INT32_MAX; 1 <= n_cv <= 4; cv_type (n_cv) and cv_atoms (n_cv, 4)
  * HOST arrays, the atoms of each CV distinct and in [0, N) (unused entries ignored); inv_mass as sgdml_b200_md_create. */
 int sgdml_b200_metad_create(sgdml_b200_md** out, sgdml_b200_model* model, int64_t n_groups, int64_t n_walkers,
@@ -311,10 +320,10 @@ int sgdml_b200_metad_get_bias(sgdml_b200_md* md, double* cv, double* V_bias, dou
  * Markland & Manolopoulos, J. Chem. Phys. 133, 124104 (2010)) in the BAOAB order of Liu, Li & Liu (J. Chem. Phys. 145,
  * 024103 (2016)).  A handle from sgdml_b200_pimd_create holds n_poly polymers; replica r = p P + j is bead j of polymer
  * p, and every state array has the layout of sgdml_b200_md_*: (n_poly P, 3N).  sgdml_b200_md_destroy, _set_state and
- * _get_state work on it unchanged; sgdml_b200_md_run on a handle with P > 1 is an argument error, and a handle from
- * sgdml_b200_md_create runs sgdml_b200_pimd_run as P = 1.  Units, streams, the step graph (one k_pimd_step launch,
- * then the forces of every bead as ordinary replicas, chunk by chunk), SGDML_B200_GRAPH=0, the step counters, the
- * workspace and the launch families are those of sgdml_b200_md_run above.
+ * _get_state work on it unchanged (the other entry points that take it: the handle kinds at
+ * sgdml_b200_md_create), and a handle from sgdml_b200_md_create runs sgdml_b200_pimd_run as P = 1.  Units, streams,
+ * the step graph (one k_pimd_step launch, then the forces of every bead as ordinary replicas, chunk by chunk),
+ * SGDML_B200_GRAPH=0, the step counters, the workspace and the launch families are those of sgdml_b200_md_run above.
  * Per run, on the host in double precision: h = dt / 2, kT_P = P kT, omega_P = kT_P / hbar,
  * omega_k = 2 omega_P sin(k pi / P); per mode cos(omega_k h), sin(omega_k h) / omega_k and -omega_k sin(omega_k h)
  * (1, h and 0 for k = 0); frictions gamma_0 = gamma, gamma_k = 2 lambda omega_k (k >= 1); c1_k = exp(-gamma_k dt) and
@@ -386,8 +395,8 @@ int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, do
                            int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream);
 /* ---------------------------------------------------------------- nudged elastic band on the device
  * Extension: minimum-energy paths and saddle points with the nudged elastic band (NEB) and its climbing-image form
- * (CI-NEB), optimised by FIRE on each whole band, many bands and many steps per call.  The handle (sgdml_b200_md_create;
- * a ring-polymer handle is rejected) holds n_rep = n_bands n_images replicas: replica b n_images + j is image j of band
+ * (CI-NEB), optimised by FIRE on each whole band, many bands and many steps per call.  The handle (plain: see handle
+ * kinds at sgdml_b200_md_create) holds n_rep = n_bands n_images replicas: replica b n_images + j is image j of band
  * b.  Images 0 and n_images - 1 are fixed endpoints: they never move, but their forces and energies are evaluated with
  * the rest of the batch every step.  Image differences are plain coordinate differences, with no minimum image, also
  * for periodic models.  Tangents are Henkelman & Jonsson's improved tangent (J. Chem. Phys. 113, 9978 (2000)), the
@@ -411,8 +420,8 @@ int sgdml_b200_neb_fire(sgdml_b200_md* md, int64_t n_images, int64_t max_steps, 
                         double* fmax_out, int* climbing_out, void* stream);
 /* ---------------------------------------------------------------- dimer saddle search on the device
  * Extension: first-order saddle points next to a minimum, with no final state, by the dimer method (Henkelman &
- * Jonsson, J. Chem. Phys. 111, 7010 (1999)), many dimers and many steps per call.  The handle (sgdml_b200_md_create;
- * ring-polymer, NPT and metadynamics handles are rejected) holds n_rep = 2 n_dimers replicas: replica 2d is the
+ * Jonsson, J. Chem. Phys. 111, 7010 (1999)), many dimers and many steps per call.  The handle (plain: see the
+ * handle kinds at sgdml_b200_md_create) holds n_rep = 2 n_dimers replicas: replica 2d is the
  * centre R0 of dimer d and replica 2d + 1 its image R0 + separation N, N the dimer's unit mode; both are evaluated
  * every step, the other image is the central difference 2 F0 - F1.  Each step first tests the dimer: it has converged
  * when max_a |F0_a| < fmax and the curvature along N, measured at the current centre, is negative; it is frozen from

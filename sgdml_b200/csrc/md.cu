@@ -20,6 +20,7 @@
 #include <cmath>
 #include <cstddef>
 #include <cstring>
+#include <functional>
 #include <initializer_list>
 #include <vector>
 
@@ -1257,9 +1258,14 @@ struct StepKey {
   bool operator==(const StepKey& o) const { return kind == o.kind && group == o.group && blk == o.blk; }
 };
 
+// What a handle is, fixed at creation (sgdml_b200_pimd_create makes PLAIN handles with one bead, RING with more): it
+// decides which entry points take the handle (check_kind) and how its state's forces are evaluated.
+enum HandleKind { PLAIN, RING, NPT, METAD };
+
 }  // namespace
 
 struct sgdml_b200_md {
+  HandleKind kind = PLAIN;
   int64_t n_rep = 0;
   int dimi = 0;
   int nb = 1;  // beads per ring polymer: replica p nb + j is bead j of polymer p (1 for sgdml_b200_md_create)
@@ -1512,14 +1518,14 @@ int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
 
 // F and E (and on an NPT handle W, each replica in its own cell) of the positions in R
 int md_forces(sgdml_b200_md* md, double* F, double* E, double* W, cudaStream_t s) {
-  if (md->cell == nullptr) return force_eval_run(md->fe, md->R, F, E, s);
+  if (md->kind != NPT) return force_eval_run(md->fe, md->R, F, E, s);
   return force_eval_run_cells(md->fe, md->R, md->lat, F, E, W, s);
 }
 
 // The state's forces and energies: on a metadynamics handle the model's F into Fm, then k_metad_bias (deposit: inside
 // a run) completes F; on every other handle md_forces
 int md_state_forces(sgdml_b200_md* md, int deposit, cudaStream_t s) {
-  if (md->Fm == nullptr) return md_forces(md, md->F, md->E, md->W, s);
+  if (md->kind != METAD) return md_forces(md, md->F, md->E, md->W, s);
   SG_TRY(md_forces(md, md->Fm, md->E, nullptr, s));
   StepParams* p = md->params(md->blk);
   k_metad_bias<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&p->metad, &p->md, md->R, md->Fm, md->F, md->step, md->dimi,
@@ -1775,86 +1781,106 @@ const double* pimd_params(sgdml_b200_md* md, const Outputs& out, double dt, doub
   return sigma + (size_t)nb * dimi;
 }
 
-constexpr const char* NPT_ONLY = "an NPT handle (sgdml_b200_npt_create) runs only sgdml_b200_npt_run";
-constexpr const char* METAD_ONLY = "a metadynamics handle (sgdml_b200_metad_create) runs only sgdml_b200_metad_run";
+// Which kinds of handle an entry point accepts: the rows of the table next to sgdml_b200_md_create in
+// include/sgdml_b200.h, each with the creators of its kinds for the refusal.
+struct Accepts {
+  unsigned kinds;  // bit k: HandleKind k
+  const char* needs;
+};
+constexpr Accepts ANY_KIND = {1u << PLAIN | 1u << RING | 1u << NPT | 1u << METAD, "a handle"};
+constexpr Accepts PLAIN_KIND = {1u << PLAIN, "a handle of sgdml_b200_md_create (or sgdml_b200_pimd_create, one bead)"};
+constexpr Accepts PLAIN_OR_RING = {1u << PLAIN | 1u << RING, "a handle of sgdml_b200_md_create or _pimd_create"};
+constexpr Accepts NPT_KIND = {1u << NPT, "an NPT handle (sgdml_b200_npt_create)"};
+constexpr Accepts METAD_KIND = {1u << METAD, "a metadynamics handle (sgdml_b200_metad_create)"};
 
-// the checks every run shares (npt, metad: the run is sgdml_b200_npt_run, sgdml_b200_metad_run); a rejected call
-// queues nothing
-int run_check(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double gamma, int64_t stride,
-              const char* no_state, bool npt = false, bool metad = false) {
-  SG_ARG(md != nullptr && n_steps >= 0 && stride >= 0 && stride <= INT32_MAX);
-  if (npt && md->cell == nullptr) return fail_arg("sgdml_b200_npt_run needs an NPT handle (sgdml_b200_npt_create)");
-  if (!npt && md->cell != nullptr) return fail_arg(NPT_ONLY);
-  if (metad && md->Fm == nullptr)
-    return fail_arg("sgdml_b200_metad_run needs a metadynamics handle (sgdml_b200_metad_create)");
-  if (!metad && md->Fm != nullptr) return fail_arg(METAD_ONLY);
-  SG_ARG(std::isfinite(dt) && dt > 0.0);
-  SG_ARG(std::isfinite(kT) && kT >= 0.0);
-  if (md->nb == 1 && kT > 0.0 && gamma == 0.0)
-    return fail_arg("kT > 0 needs a friction gamma > 0 (a thermostat without coupling)");
-  if (stride > 0 && n_steps % stride != 0) return fail_arg("n_steps must be a multiple of stride");
-  if (!md->has_state) return fail_arg(no_state);
+// the first check of every entry point that takes a handle
+int check_kind(const sgdml_b200_md* md, const char* entry, const Accepts& a) {
+  SG_ARG(md != nullptr);
+  if ((a.kinds >> md->kind & 1u) == 0) return fail_arg((std::string(entry) + " needs " + a.needs).c_str());
   return 0;
 }
 
-// sgdml_b200_md_run (MD_CLASSICAL), sgdml_b200_pimd_run (MD_RING_POLYMER; hbar and lambda are only its own),
-// sgdml_b200_remd_run (MD_REMD, with x: its ladder, and kT = its first temperature), sgdml_b200_npt_run (MD_NPT,
-// with b: its barostat) and sgdml_b200_metad_run (MD_METAD, with mt: its deposition), after their checks.  n_steps
-// steps, then the completing launch.
-int md_run(sgdml_b200_md* md, int kind, int64_t n_steps, double dt, double kT, double hbar, double gamma, double lambda,
-           uint64_t seed, int64_t stride, void* const outs[N_RUN_OUTS], const RemdRun* x, const NptRun* b,
-           cudaStream_t s, const MetadRun* mt = nullptr) {
-  if (n_steps == 0 && x == nullptr) return 0;  // (a replica exchange still reports its labels and zero counts)
-  md->group = x != nullptr ? x->n_temps : 1;
-  const int64_t n_rep = md->n_rep, n_frames = stride > 0 ? n_steps / stride : 0;
+// One call of md_run: the arguments every run shares, then those only one integrator reads
+struct Run {
+  int64_t n_steps, stride;
+  double dt, kT, gamma;  // kT: a replica exchange's first temperature
+  uint64_t seed;
+  void* outs[N_RUN_OUTS];
+  double hbar, lambda;  // MD_RING_POLYMER
+  RemdRun remd;         // MD_REMD
+  NptRun npt;           // MD_NPT
+  MetadRun metad;       // MD_METAD
+};
+
+// the checks every run shares; a rejected call queues nothing
+int run_check(const sgdml_b200_md* md, const Run& r, const char* entry) {
+  SG_ARG(r.n_steps >= 0 && r.stride >= 0 && r.stride <= INT32_MAX);
+  SG_ARG(std::isfinite(r.dt) && r.dt > 0.0);
+  SG_ARG(std::isfinite(r.kT) && r.kT >= 0.0);
+  if (md->nb == 1 && r.kT > 0.0 && r.gamma == 0.0)
+    return fail_arg("kT > 0 needs a friction gamma > 0 (a thermostat without coupling)");
+  if (r.stride > 0 && r.n_steps % r.stride != 0) return fail_arg("n_steps must be a multiple of stride");
+  if (!md->has_state) return fail_arg((std::string(entry) + ": no state yet (call sgdml_b200_md_set_state)").c_str());
+  return 0;
+}
+
+// sgdml_b200_md_run (MD_CLASSICAL), _pimd_run (MD_RING_POLYMER), _remd_run (MD_REMD), _npt_run (MD_NPT) and
+// _metad_run (MD_METAD), after their checks: n_steps steps, then the completing launch.
+int md_run(sgdml_b200_md* md, int kind, const Run& r, cudaStream_t s) {
+  if (r.n_steps == 0 && kind != MD_REMD) return 0;  // (a replica exchange still reports its labels and zero counts)
+  md->group = kind == MD_REMD ? r.remd.n_temps : 1;
+  const int64_t n_rep = md->n_rep, n_frames = r.stride > 0 ? r.n_steps / r.stride : 0;
   const size_t fr = sizeof(double) * (size_t)(n_frames * n_rep);
   const size_t fp = sizeof(double) * (size_t)(n_frames * (n_rep / md->nb));
   const size_t nc = sizeof(int64_t) * (size_t)(n_rep / md->group * (md->group - 1));  // (n_ladders, n_temps - 1)
+  const int n_cv = kind == MD_METAD ? md->params(md->hblk)->metad.n_cv : 0;
+  void* const* outs = r.outs;
   Outputs out(s);
   SG_TRY(out.init({{outs[OUT_R], fr * md->dimi}, {outs[OUT_V], fr * md->dimi}, {outs[OUT_EPOT], fr},
                    {outs[OUT_EKIN], fr}, {outs[OUT_KPRIM], fp}, {outs[OUT_KCV], fp},
                    {outs[OUT_WALKER_F], sizeof(int) * (size_t)(n_frames * n_rep)},
                    {outs[OUT_WALKERS], sizeof(int) * (size_t)n_rep}, {outs[OUT_NACC], nc}, {outs[OUT_NATT], nc},
-                   {outs[OUT_CELL], 9 * fr}, {outs[OUT_PRESS], fr},
-                   {outs[OUT_CV], fr * (mt != nullptr ? md->params(md->hblk)->metad.n_cv : 0)}, {outs[OUT_BIAS], fr}}));
+                   {outs[OUT_CELL], 9 * fr}, {outs[OUT_PRESS], fr}, {outs[OUT_CV], fr * n_cv}, {outs[OUT_BIAS], fr}}));
   SG_TRY(force_eval_prepare(md->fe));
-  if (x != nullptr) {
-    SG_TRY(reserve(md, x->n_temps));
+  if (kind == MD_REMD) {
+    SG_TRY(reserve(md, r.remd.n_temps));
     SG_TRY(remd_alloc(md, s));
     SG_CUDA(cudaMemsetAsync(md->xcount, 0, 2 * sizeof(int64_t) * (size_t)n_rep, s));  // the run's counts
   }
   SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the mirror
-  if (mt != nullptr) {
+  if (kind == MD_METAD) {
     int64_t need = 0;
     for (int64_t c : md->hcount_host) need = std::max(need, c);
-    SG_TRY(metad_reserve(md, need + (int64_t)md->params(md->hblk)->metad.n_walkers * mt->n_dep));
+    SG_TRY(metad_reserve(md, need + (int64_t)md->params(md->hblk)->metad.n_walkers * r.metad.n_dep));
   }
   StepParams& p = *md->params(md->hblk);
   const double* end;
   if (kind == MD_RING_POLYMER) {
-    run_params(p.pimd, md, dt, seed, n_frames, stride, out);
-    end = pimd_params(md, out, dt, kT, hbar, gamma, lambda);
+    run_params(p.pimd, md, r.dt, r.seed, n_frames, r.stride, out);
+    end = pimd_params(md, out, r.dt, r.kT, r.hbar, r.gamma, r.lambda);
   } else {
-    run_params(p.md, md, dt, seed, n_frames, stride, out);
-    end = md_params(md, dt, gamma, x != nullptr ? x->kT : &kT, md->group);
-    if (x != nullptr) end = remd_params(md, *x, out);
-    if (b != nullptr) npt_params(md, *b, dt, kT, out);
-    if (mt != nullptr) metad_params(md, *mt, out);
+    run_params(p.md, md, r.dt, r.seed, n_frames, r.stride, out);
+    end = md_params(md, r.dt, r.gamma, kind == MD_REMD ? r.remd.kT : &r.kT, md->group);
+    switch (kind) {
+      case MD_REMD: end = remd_params(md, r.remd, out); break;
+      case MD_NPT: npt_params(md, r.npt, r.dt, r.kT, out); break;
+      case MD_METAD: metad_params(md, r.metad, out); break;
+    }
   }
   SG_TRY(upload(md, end, s));
-  if (n_steps > 0) {
-    SG_TRY(md_replay(md, kind, n_steps, s));
-    md->step_host += (uint64_t)n_steps;
+  if (r.n_steps > 0) {
+    SG_TRY(md_replay(md, kind, r.n_steps, s));
+    md->step_host += (uint64_t)r.n_steps;
     SG_TRY(md_integrate(md, kind, 0, s));  // the second half-kick of the last step (and its frame)
-    if (mt != nullptr && mt->n_dep > 0) {  // the run's hills become committed
-      const int64_t add = (int64_t)md->params(md->hblk)->metad.n_walkers * mt->n_dep;
+    if (kind == MD_METAD && r.metad.n_dep > 0) {  // the run's hills become committed
+      const int64_t add = (int64_t)md->params(md->hblk)->metad.n_walkers * r.metad.n_dep;
       k_metad_commit<<<(unsigned)((md->n_groups + 255) / 256), 256, 0, s>>>(md->hcount, md->n_groups, add);
       SG_CUDA(cudaGetLastError());
       count_launch(KID_MISC);
       for (int64_t& c : md->hcount_host) c += add;
     }
   }
-  if (x != nullptr) SG_TRY(out.copy_from(OUT_WALKERS, {md->walker, md->xcount, md->xcount + n_rep}));
+  if (kind == MD_REMD) SG_TRY(out.copy_from(OUT_WALKERS, {md->walker, md->xcount, md->xcount + n_rep}));
   return out.finish();
 }
 
@@ -2018,24 +2044,25 @@ int relax_impl(sgdml_b200_md* md, int kind, int g, int memory, const StepParams&
 }
 
 // the checks both optimisers share; a rejected call queues nothing
-int relax_check(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, const char* what) {
-  SG_ARG(md != nullptr && max_steps >= 0);
+int relax_check(const sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, const char* entry) {
+  SG_ARG(max_steps >= 0);
   SG_ARG(std::isfinite(fmax) && fmax >= 0.0);
   SG_ARG(std::isfinite(maxstep) && maxstep > 0.0);
-  if (md->cell != nullptr) return fail_arg(NPT_ONLY);
-  if (md->Fm != nullptr) return fail_arg(METAD_ONLY);
-  if (!md->has_state) return fail_arg(what);
+  if (!md->has_state) return fail_arg((std::string(entry) + ": no state yet (call sgdml_b200_md_set_state)").c_str());
   return 0;
 }
 
-// a handle of n_rep = n_poly nb replicas; the caller has checked the counts
-int md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, int nb, const double* inv_mass) {
+// A handle of the given kind, n_rep = n_poly nb replicas; the caller has checked the counts and parsed the arguments of
+// its kind.  init, if given, makes the kind's own part; a failure anywhere frees the whole handle.
+int md_create(sgdml_b200_md** out, sgdml_b200_model* m, HandleKind kind, int64_t n_rep, int nb, const double* inv_mass,
+              const std::function<int(sgdml_b200_md*)>& init = nullptr) {
   SG_ARG(!is_device_ptr(inv_mass));
   int64_t n_atoms = 0;
   SG_TRY(sgdml_b200_model_dims(m, &n_atoms, nullptr, nullptr));
   for (int i = 0; i < n_atoms; ++i)
     if (!(std::isfinite(inv_mass[i]) && inv_mass[i] > 0.0)) return fail_arg("inv_mass must be finite and > 0");
   sgdml_b200_md* md = new sgdml_b200_md();
+  md->kind = kind;
   md->n_rep = n_rep;
   md->nb = nb;
   md->dimi = 3 * (int)n_atoms;
@@ -2052,10 +2079,10 @@ int md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, int nb, c
     md->s_host.resize((size_t)md->dimi);
     for (int i = 0; i < md->dimi; ++i) md->s_host[(size_t)i] = inv_mass[i / 3];
     SG_CUDA(cudaMemcpy(md->s, md->s_host.data(), sizeof(double) * md->dimi, cudaMemcpyHostToDevice));
-    return force_eval_prepare(md->fe);
+    SG_TRY(force_eval_prepare(md->fe));
+    return init ? init(md) : 0;
   };
-  const int rc = body();
-  if (rc != 0) {
+  if (const int rc = body()) {
     md_free(md);
     return rc;
   }
@@ -2109,7 +2136,7 @@ int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep
   SG_TRY(require_device());
   SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
   SG_ARG(n_rep >= 1 && n_rep <= INT32_MAX);
-  return md_create(out, m, n_rep, 1, inv_mass);
+  return md_create(out, m, PLAIN, n_rep, 1, inv_mass);
 }
 
 int sgdml_b200_pimd_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_poly, int64_t n_beads,
@@ -2118,7 +2145,7 @@ int sgdml_b200_pimd_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_p
   SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr);
   SG_ARG(n_beads >= 1 && n_beads <= PIMD_MAX_BEADS);
   SG_ARG(n_poly >= 1 && n_poly <= INT32_MAX / n_beads);
-  return md_create(out, m, n_poly * n_beads, (int)n_beads, inv_mass);
+  return md_create(out, m, n_beads > 1 ? RING : PLAIN, n_poly * n_beads, (int)n_beads, inv_mass);
 }
 
 int sgdml_b200_npt_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_rep, const double* inv_mass,
@@ -2129,29 +2156,19 @@ int sgdml_b200_npt_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_re
   std::vector<NptCell> cells;
   std::vector<Lattice> lats;
   SG_TRY(npt_parse(lattices, lattice_invs, n_rep, &cells, &lats));
-  sgdml_b200_md* md = nullptr;
-  SG_TRY(md_create(&md, m, n_rep, 1, inv_mass));
-  auto body = [&]() -> int {
+  return md_create(out, m, NPT, n_rep, 1, inv_mass, [&](sgdml_b200_md* md) -> int {
     SG_CUDA(cached_malloc(&md->cell, sizeof(NptCell) * (size_t)n_rep));
     SG_CUDA(cached_malloc(&md->lat, sizeof(Lattice) * (size_t)n_rep));
     SG_CUDA(cached_malloc(&md->W, sizeof(double) * 9 * (size_t)n_rep));
     SG_CUDA(cached_malloc(&md->Ws, sizeof(double) * 9 * (size_t)n_rep));
     SG_CUDA(cudaMemset(md->W, 0, sizeof(double) * 9 * (size_t)n_rep));
     return npt_install(md, cells, lats, 0);
-  };
-  const int rc = body();
-  if (rc != 0) {
-    md_free(md);
-    return rc;
-  }
-  *out = md;
-  return 0;
+  });
 }
 
 int sgdml_b200_npt_set_cells(sgdml_b200_md* md, const double* lattices, const double* lattice_invs, void* stream) {
   SG_TRY(require_device());
-  SG_ARG(md != nullptr);
-  if (md->cell == nullptr) return fail_arg("sgdml_b200_npt_set_cells needs an NPT handle (sgdml_b200_npt_create)");
+  SG_TRY(check_kind(md, "sgdml_b200_npt_set_cells", NPT_KIND));
   std::vector<NptCell> cells;
   std::vector<Lattice> lats;
   SG_TRY(npt_parse(lattices, lattice_invs, md->n_rep, &cells, &lats));
@@ -2160,8 +2177,7 @@ int sgdml_b200_npt_set_cells(sgdml_b200_md* md, const double* lattices, const do
 
 int sgdml_b200_npt_get_cells(sgdml_b200_md* md, double* lattices, double* lattice_invs, double* W, void* stream) {
   SG_TRY(require_device());
-  SG_ARG(md != nullptr);
-  if (md->cell == nullptr) return fail_arg("sgdml_b200_npt_get_cells needs an NPT handle (sgdml_b200_npt_create)");
+  SG_TRY(check_kind(md, "sgdml_b200_npt_get_cells", NPT_KIND));
   cudaStream_t s = (cudaStream_t)stream;
   const size_t row = 9 * sizeof(double), n = (size_t)md->n_rep;
   Outputs out(s);
@@ -2201,9 +2217,7 @@ int sgdml_b200_metad_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_
     }
   }
   const int64_t n_rep = n_groups * n_walkers;
-  sgdml_b200_md* md = nullptr;
-  SG_TRY(md_create(&md, m, n_rep, 1, inv_mass));
-  auto body = [&]() -> int {
+  return md_create(out, m, METAD, n_rep, 1, inv_mass, [&](sgdml_b200_md* md) -> int {
     const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
     SG_CUDA(cached_malloc(&md->Fm, st));
     SG_CUDA(cached_malloc(&md->Fb, st));
@@ -2223,14 +2237,7 @@ int sgdml_b200_metad_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_
     SG_TRY(upload(md, p + 1, 0));
     SG_CUDA(cudaStreamSynchronize(0));
     return 0;
-  };
-  const int rc = body();
-  if (rc != 0) {
-    md_free(md);
-    return rc;
-  }
-  *out = md;
-  return 0;
+  });
 }
 
 int sgdml_b200_metad_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, double w0,
@@ -2238,8 +2245,11 @@ int sgdml_b200_metad_run(sgdml_b200_md* md, int64_t n_steps, double dt, double g
                          double* R_frames, double* V_frames, double* E_pot_frames, double* E_kin_frames,
                          double* cv_frames, double* bias_frames, void* stream) {
   SG_TRY(require_device());
-  SG_TRY(run_check(md, n_steps, dt, kT, gamma, stride,
-                   "sgdml_b200_metad_run: no state yet (call sgdml_b200_md_set_state)", false, true));
+  SG_TRY(check_kind(md, "sgdml_b200_metad_run", METAD_KIND));
+  Run r = {n_steps, stride, dt, kT, gamma, seed, {R_frames, V_frames, E_pot_frames, E_kin_frames}};
+  r.outs[OUT_CV] = cv_frames;
+  r.outs[OUT_BIAS] = bias_frames;
+  SG_TRY(run_check(md, r, "sgdml_b200_metad_run"));
   SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
   SG_ARG(std::isfinite(w0) && w0 >= 0.0);
   SG_ARG(pace >= 1);
@@ -2249,20 +2259,15 @@ int sgdml_b200_metad_run(sgdml_b200_md* md, int64_t n_steps, double dt, double g
   for (int j = 0; j < q.n_cv; ++j)
     if (!(std::isfinite(widths[j]) && widths[j] > 0.0)) return fail_arg("every width must be finite and > 0");
   const uint64_t a = md->step_host, e = md->step_host + (uint64_t)n_steps, pc = (uint64_t)pace;
-  const MetadRun mt = {w0, dkT, widths, pace, (int64_t)(e / pc - a / pc)};
-  void* outs[N_RUN_OUTS] = {R_frames, V_frames, E_pot_frames, E_kin_frames};
-  outs[OUT_CV] = cv_frames;
-  outs[OUT_BIAS] = bias_frames;
-  return md_run(md, MD_METAD, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, outs, nullptr, nullptr,
-                (cudaStream_t)stream, &mt);
+  r.metad = {w0, dkT, widths, pace, (int64_t)(e / pc - a / pc)};
+  return md_run(md, MD_METAD, r, (cudaStream_t)stream);
 }
 
 int sgdml_b200_metad_get_hills(sgdml_b200_md* md, int64_t* n_hills, double* centers, double* widths,
                                double* heights, void* stream) {
   SG_TRY(require_device());
-  SG_ARG(md != nullptr && n_hills != nullptr && !is_device_ptr(n_hills));
-  if (md->Fm == nullptr)
-    return fail_arg("sgdml_b200_metad_get_hills needs a metadynamics handle (sgdml_b200_metad_create)");
+  SG_TRY(check_kind(md, "sgdml_b200_metad_get_hills", METAD_KIND));
+  SG_ARG(n_hills != nullptr && !is_device_ptr(n_hills));
   cudaStream_t s = (cudaStream_t)stream;
   const MetadParams& q = md->params(md->hblk)->metad;
   const size_t nc = (size_t)q.n_cv;
@@ -2289,9 +2294,8 @@ int sgdml_b200_metad_get_hills(sgdml_b200_md* md, int64_t* n_hills, double* cent
 int sgdml_b200_metad_set_hills(sgdml_b200_md* md, const int64_t* n_hills, const double* centers,
                                const double* widths, const double* heights, void* stream) {
   SG_TRY(require_device());
-  SG_ARG(md != nullptr && n_hills != nullptr && !is_device_ptr(n_hills));
-  if (md->Fm == nullptr)
-    return fail_arg("sgdml_b200_metad_set_hills needs a metadynamics handle (sgdml_b200_metad_create)");
+  SG_TRY(check_kind(md, "sgdml_b200_metad_set_hills", METAD_KIND));
+  SG_ARG(n_hills != nullptr && !is_device_ptr(n_hills));
   int64_t total = 0, need = 0;
   for (int64_t g = 0; g < md->n_groups; ++g) {
     SG_ARG(n_hills[g] >= 0);
@@ -2340,9 +2344,7 @@ int sgdml_b200_metad_set_hills(sgdml_b200_md* md, const int64_t* n_hills, const 
 
 int sgdml_b200_metad_get_bias(sgdml_b200_md* md, double* cv, double* V_bias, double* F_bias, void* stream) {
   SG_TRY(require_device());
-  SG_ARG(md != nullptr);
-  if (md->Fm == nullptr)
-    return fail_arg("sgdml_b200_metad_get_bias needs a metadynamics handle (sgdml_b200_metad_create)");
+  SG_TRY(check_kind(md, "sgdml_b200_metad_get_bias", METAD_KIND));
   if (!md->has_state) return fail_arg("sgdml_b200_metad_get_bias: no state yet (call sgdml_b200_md_set_state)");
   cudaStream_t s = (cudaStream_t)stream;
   const size_t n = (size_t)md->n_rep;
@@ -2360,7 +2362,8 @@ int sgdml_b200_md_destroy(sgdml_b200_md* md) {
 
 int sgdml_b200_md_set_state(sgdml_b200_md* md, const double* R, const double* V, uint64_t step, void* stream) {
   SG_TRY(require_device());
-  SG_ARG(md != nullptr && R != nullptr);
+  SG_TRY(check_kind(md, "sgdml_b200_md_set_state", ANY_KIND));
+  SG_ARG(R != nullptr);
   cudaStream_t s = (cudaStream_t)stream;
   const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
   SG_TRY(force_eval_prepare(md->fe));
@@ -2386,13 +2389,13 @@ int sgdml_b200_md_set_state(sgdml_b200_md* md, const double* R, const double* V,
 int sgdml_b200_md_get_state(sgdml_b200_md* md, double* R, double* V, double* F, double* E_pot, uint64_t* step,
                             void* stream) {
   SG_TRY(require_device());
-  SG_ARG(md != nullptr);
+  SG_TRY(check_kind(md, "sgdml_b200_md_get_state", ANY_KIND));
   if (!md->has_state) return fail_arg("sgdml_b200_md_get_state: no state yet (call sgdml_b200_md_set_state)");
   cudaStream_t s = (cudaStream_t)stream;
   const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
   Outputs out(s);
   SG_TRY(out.init({{R, st}, {V, st}, {F, st}, {E_pot, sizeof(double) * md->n_rep}, {step, sizeof(uint64_t)}}));
-  SG_TRY(out.copy_from(0, {md->R, md->V, md->Fm != nullptr ? md->Fm : md->F, md->E, md->step}));
+  SG_TRY(out.copy_from(0, {md->R, md->V, md->kind == METAD ? md->Fm : md->F, md->E, md->step}));
   return out.finish();
 }
 
@@ -2400,13 +2403,11 @@ int sgdml_b200_md_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamm
                       int64_t stride, double* R_frames, double* V_frames, double* E_pot_frames, double* E_kin_frames,
                       void* stream) {
   SG_TRY(require_device());
-  SG_TRY(run_check(md, n_steps, dt, kT, gamma, stride, "sgdml_b200_md_run: no state yet (call sgdml_b200_md_set_state)"));
-  if (md->nb > 1)
-    return fail_arg("sgdml_b200_md_run: a ring-polymer handle (n_beads > 1) runs with sgdml_b200_pimd_run");
+  SG_TRY(check_kind(md, "sgdml_b200_md_run", PLAIN_KIND));
+  const Run r = {n_steps, stride, dt, kT, gamma, seed, {R_frames, V_frames, E_pot_frames, E_kin_frames}};
+  SG_TRY(run_check(md, r, "sgdml_b200_md_run"));
   SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
-  void* const outs[N_RUN_OUTS] = {R_frames, V_frames, E_pot_frames, E_kin_frames};
-  return md_run(md, MD_CLASSICAL, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, outs, nullptr, nullptr,
-                (cudaStream_t)stream);
+  return md_run(md, MD_CLASSICAL, r, (cudaStream_t)stream);
 }
 
 int sgdml_b200_npt_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, double P0,
@@ -2414,17 +2415,17 @@ int sgdml_b200_npt_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gam
                        double* V_frames, double* E_pot_frames, double* E_kin_frames, double* cell_frames,
                        double* P_frames, void* stream) {
   SG_TRY(require_device());
-  SG_TRY(run_check(md, n_steps, dt, kT, gamma, stride, "sgdml_b200_npt_run: no state yet (call sgdml_b200_md_set_state)",
-                   true));
+  SG_TRY(check_kind(md, "sgdml_b200_npt_run", NPT_KIND));
+  Run r = {n_steps, stride, dt, kT, gamma, seed, {R_frames, V_frames, E_pot_frames, E_kin_frames}};
+  r.outs[OUT_CELL] = cell_frames;
+  r.outs[OUT_PRESS] = P_frames;
+  SG_TRY(run_check(md, r, "sgdml_b200_npt_run"));
   SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
   SG_ARG(std::isfinite(P0));
   SG_ARG(std::isfinite(beta_T) && beta_T >= 0.0);
   SG_ARG(std::isfinite(tau_p) && tau_p > 0.0);
-  const NptRun b = {P0, beta_T, tau_p};
-  void* outs[N_RUN_OUTS] = {R_frames, V_frames, E_pot_frames, E_kin_frames};
-  outs[OUT_CELL] = cell_frames;
-  outs[OUT_PRESS] = P_frames;
-  return md_run(md, MD_NPT, n_steps, dt, kT, 0.0, gamma, 0.0, seed, stride, outs, nullptr, &b, (cudaStream_t)stream);
+  r.npt = {P0, beta_T, tau_p};
+  return md_run(md, MD_NPT, r, (cudaStream_t)stream);
 }
 
 int sgdml_b200_remd_run(sgdml_b200_md* md, int64_t n_temps, const double* kT, int64_t n_steps, double dt, double gamma,
@@ -2432,21 +2433,20 @@ int sgdml_b200_remd_run(sgdml_b200_md* md, int64_t n_temps, const double* kT, in
                         double* E_pot_frames, double* E_kin_frames, int* walker_frames, int* walkers_out,
                         int64_t* n_accepted, int64_t* n_attempted, void* stream) {
   SG_TRY(require_device());
-  SG_ARG(md != nullptr && kT != nullptr);
-  if (md->nb > 1) return fail_arg("sgdml_b200_remd_run: a ring-polymer handle (n_beads > 1) holds no ladders");
+  SG_TRY(check_kind(md, "sgdml_b200_remd_run", PLAIN_KIND));
+  SG_ARG(kT != nullptr);
   SG_ARG(n_temps >= 2 && md->n_rep % n_temps == 0);
   SG_ARG(!is_device_ptr(kT));
   for (int64_t k = 0; k < n_temps; ++k)
     if (!(std::isfinite(kT[k]) && kT[k] > 0.0)) return fail_arg("sgdml_b200_remd_run: every kT must be finite and > 0");
   SG_ARG(std::isfinite(gamma) && gamma > 0.0);
   SG_ARG(exchange_every >= 0);
-  SG_TRY(run_check(md, n_steps, dt, kT[0], gamma, stride,
-                   "sgdml_b200_remd_run: no state yet (call sgdml_b200_md_set_state)"));
-  const RemdRun x = {(int)n_temps, kT, exchange_every};
-  void* const outs[N_RUN_OUTS] = {R_frames,      V_frames,    E_pot_frames, E_kin_frames, nullptr,
-                                  nullptr,       walker_frames, walkers_out, n_accepted,   n_attempted};
-  return md_run(md, MD_REMD, n_steps, dt, kT[0], 0.0, gamma, 0.0, seed, stride, outs, &x, nullptr,
-                (cudaStream_t)stream);
+  Run r = {n_steps, stride, dt, kT[0], gamma, seed,
+           {R_frames, V_frames, E_pot_frames, E_kin_frames, nullptr, nullptr, walker_frames, walkers_out, n_accepted,
+            n_attempted}};
+  SG_TRY(run_check(md, r, "sgdml_b200_remd_run"));
+  r.remd = {(int)n_temps, kT, exchange_every};
+  return md_run(md, MD_REMD, r, (cudaStream_t)stream);
 }
 
 int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT, double hbar, double gamma,
@@ -2454,22 +2454,22 @@ int sgdml_b200_pimd_run(sgdml_b200_md* md, int64_t n_steps, double dt, double kT
                         double* E_pot_frames, double* E_kin_frames, double* K_prim_frames, double* K_cv_frames,
                         void* stream) {
   SG_TRY(require_device());
-  SG_TRY(run_check(md, n_steps, dt, kT, gamma, stride,
-                   "sgdml_b200_pimd_run: no state yet (call sgdml_b200_md_set_state)"));
+  SG_TRY(check_kind(md, "sgdml_b200_pimd_run", PLAIN_OR_RING));
+  const Run r = {n_steps, stride, dt, kT, gamma, seed,
+                 {R_frames, V_frames, E_pot_frames, E_kin_frames, K_prim_frames, K_cv_frames}, hbar, lambda};
+  SG_TRY(run_check(md, r, "sgdml_b200_pimd_run"));
   SG_ARG(std::isfinite(hbar) && hbar > 0.0);
   SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
   SG_ARG(std::isfinite(lambda) && lambda >= 0.0);
   if (md->nb > 1 && kT == 0.0) return fail_arg("a ring polymer (n_beads > 1) needs kT > 0");
-  void* const outs[N_RUN_OUTS] = {R_frames, V_frames, E_pot_frames, E_kin_frames, K_prim_frames, K_cv_frames};
-  return md_run(md, MD_RING_POLYMER, n_steps, dt, kT, hbar, gamma, lambda, seed, stride, outs, nullptr, nullptr,
-                (cudaStream_t)stream);
+  return md_run(md, MD_RING_POLYMER, r, (cudaStream_t)stream);
 }
 
 int sgdml_b200_relax_fire(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, double dt, double dtmax,
                           int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream) {
   SG_TRY(require_device());
-  SG_TRY(relax_check(md, max_steps, fmax, maxstep,
-                     "sgdml_b200_relax_fire: no state yet (call sgdml_b200_md_set_state)"));
+  SG_TRY(check_kind(md, "sgdml_b200_relax_fire", PLAIN_OR_RING));
+  SG_TRY(relax_check(md, max_steps, fmax, maxstep, "sgdml_b200_relax_fire"));
   SG_ARG(std::isfinite(dt) && dt > 0.0);
   SG_ARG(std::isfinite(dtmax) && dtmax > 0.0);
   StepParams c = {};
@@ -2484,8 +2484,8 @@ int sgdml_b200_relax_fire(sgdml_b200_md* md, int64_t max_steps, double fmax, dou
 int sgdml_b200_relax_lbfgs(sgdml_b200_md* md, int64_t max_steps, double fmax, double maxstep, int memory, double h0,
                            int64_t* n_steps_out, int* converged_out, double* fmax_out, void* stream) {
   SG_TRY(require_device());
-  SG_TRY(relax_check(md, max_steps, fmax, maxstep,
-                     "sgdml_b200_relax_lbfgs: no state yet (call sgdml_b200_md_set_state)"));
+  SG_TRY(check_kind(md, "sgdml_b200_relax_lbfgs", PLAIN_OR_RING));
+  SG_TRY(relax_check(md, max_steps, fmax, maxstep, "sgdml_b200_relax_lbfgs"));
   SG_ARG(memory >= 1 && memory <= LBFGS_MAX_MEMORY);
   SG_ARG(std::isfinite(h0) && h0 > 0.0);
   StepParams c = {};
@@ -2501,8 +2501,8 @@ int sgdml_b200_neb_fire(sgdml_b200_md* md, int64_t n_images, int64_t max_steps, 
                         double maxstep, double dt, double dtmax, int64_t* n_steps_out, int* converged_out,
                         double* fmax_out, int* climbing_out, void* stream) {
   SG_TRY(require_device());
-  SG_TRY(relax_check(md, max_steps, fmax, maxstep, "sgdml_b200_neb_fire: no state yet (call sgdml_b200_md_set_state)"));
-  if (md->nb > 1) return fail_arg("sgdml_b200_neb_fire: a ring-polymer handle (n_beads > 1) holds no bands");
+  SG_TRY(check_kind(md, "sgdml_b200_neb_fire", PLAIN_KIND));
+  SG_TRY(relax_check(md, max_steps, fmax, maxstep, "sgdml_b200_neb_fire"));
   SG_ARG(n_images >= 3 && md->n_rep % n_images == 0);
   SG_ARG((n_images - 2) * md->dimi <= INT32_MAX);
   SG_ARG(std::isfinite(k) && k >= 0.0);
@@ -2525,9 +2525,8 @@ int sgdml_b200_dimer_fire(sgdml_b200_md* md, const double* modes, int64_t max_st
                           int64_t* n_steps_out, int* converged_out, double* fmax_out, double* curvature_out,
                           int64_t* n_rot_out, double* modes_out, void* stream) {
   SG_TRY(require_device());
-  SG_TRY(relax_check(md, max_steps, fmax, maxstep,
-                     "sgdml_b200_dimer_fire: no state yet (call sgdml_b200_md_set_state)"));
-  if (md->nb > 1) return fail_arg("sgdml_b200_dimer_fire: a ring-polymer handle (n_beads > 1) holds no dimers");
+  SG_TRY(check_kind(md, "sgdml_b200_dimer_fire", PLAIN_KIND));
+  SG_TRY(relax_check(md, max_steps, fmax, maxstep, "sgdml_b200_dimer_fire"));
   if (md->n_rep % 2 != 0) return fail_arg("sgdml_b200_dimer_fire: n_rep must be even (a centre and an image per dimer)");
   if (modes == nullptr && !md->has_modes)
     return fail_arg("sgdml_b200_dimer_fire: no modes yet (pass modes on the handle's first dimer call)");

@@ -3,8 +3,9 @@ restatement of tests/metad_oracle.py, fed by the engine's predictor on device-re
 
 GPU: trajectories, CVs, bias energies and hills against the restatement on two MD fixtures, zero height against
 sgdml_b200_md_run, graph against plain launches and chunks, continuation and restarts from the hills, isolation from
-the predictor's calls and from other handles, the handle-kind rules and bad input, the public units, and the physics of
-a trained double well: barrier crossing at low temperature and the free-energy profile against unbiased sampling.
+the predictor's calls and from other handles, bad input, the public units, and the physics of a trained double well:
+barrier crossing at low temperature and the free-energy profile against unbiased sampling.  Which entry points take a
+metadynamics handle is tests/test_md_handle_kinds.py's.
 """
 
 import ctypes
@@ -239,25 +240,7 @@ def test_handle_kind_rules_and_bad_input():
     dyn._set_state_raw(R0, V0, step=7)
     dyn._run_raw(6, dt, *args, seed=1)
     H = dyn._handle
-    o = np.zeros(64)
-    assert L.sgdml_b200_md_run(H, 10, dt, 0.0, 0.0, 0, 0, None, None, None, None, st) <= -1000
-    assert L.sgdml_b200_pimd_run(H, 10, dt, 0.0, 1.0, 0.0, 0.0, 0, 0, None, None, None, None, None, None, st) <= -1000
-    kT2 = np.array([1e-3, 2e-3])
-    assert L.sgdml_b200_remd_run(H, 2, kT2.ctypes.data, 10, dt, 1.0, 0, 1, 0, *([None] * 8), st) <= -1000
-    assert L.sgdml_b200_npt_run(H, 10, dt, 0.0, 0.0, 0.0, 0.0, 1.0, 0, 0, *([None] * 6), st) <= -1000
-    assert L.sgdml_b200_relax_fire(H, 10, 0.01, 0.1, 0.1, 1.0, None, None, None, st) <= -1000
-    assert L.sgdml_b200_relax_lbfgs(H, 10, 0.01, 0.1, 10, 1.0, None, None, None, st) <= -1000
-    assert L.sgdml_b200_neb_fire(H, 3, 10, 0.01, 0.1, 0, 0.1, 0.1, 1.0, None, None, None, None, st) <= -1000
-    md = sgdml_b200.GDMLDynamics(gp, masses, n_replicas=NW * NG, E_to_eV=1.0, F_to_eV_Ang=1.0)
-    md._set_state_raw(R0, V0)
-    w = np.full(4, 0.1)
-    n = np.zeros(NG, dtype=np.int64)
-    assert L.sgdml_b200_metad_run(md._handle, 10, dt, 0.0, 0.0, 0.1, w.ctypes.data, 1, np.inf, 0, 0,
-                                  *([None] * 6), st) <= -1000
-    assert L.sgdml_b200_metad_get_hills(md._handle, n.ctypes.data, None, None, None, st) <= -1000
-    assert L.sgdml_b200_metad_set_hills(md._handle, n.ctypes.data, None, None, None, st) <= -1000
-    assert L.sgdml_b200_metad_get_bias(md._handle, o.ctypes.data, None, None, st) <= -1000
-    # bad runs and hills change nothing
+    # bad runs and hills change nothing (which handles metad_* take: tests/test_md_handle_kinds.py)
     before = dyn._get_state_raw(), dyn._get_bias_raw(), dyn._get_hills_raw()
     gamma, kT, w0, widths, pace, dkT = args
     good = dict(n_steps=6, dt=dt, gamma=gamma, kT=kT, w0=w0, widths=widths, pace=pace, dkT=dkT, stride=0)

@@ -4,8 +4,8 @@ cells and inverses.
 
 GPU: trajectories against the restatement (a small periodic fixture and a D > 256 periodic model), zero
 compressibility against sgdml_b200_md_run, graph against plain launches and chunks, reproducibility and continuation,
-isolation from the predictor's calls, the handle-kind rules and bad input, the public units and stress, and the
-isothermal-isobaric ensemble of an ideal gas and of a trained periodic model.
+isolation from the predictor's calls, bad input, the public units and stress, and the isothermal-isobaric ensemble of
+an ideal gas and of a trained periodic model.  Which entry points take an NPT handle is tests/test_md_handle_kinds.py's.
 """
 
 import ctypes
@@ -263,22 +263,8 @@ def test_handle_kind_rules_and_bad_input():
         dyn._run_raw(10, dt, 0.0, 0.0, 0.0, 0.0, 1.0)  # no state yet
     dyn._set_cells_raw(L0, L0inv)
     dyn._set_state_raw(R0, V0, step=7)
-    # the other integrators refuse an NPT handle, and npt_run refuses the other handles
+    # bad runs and cells change nothing (which handles npt_* take: tests/test_md_handle_kinds.py)
     H = dyn._handle
-    o = np.zeros(64)
-    assert L.sgdml_b200_md_run(H, 10, dt, 0.0, 0.0, 0, 0, None, None, None, None, st) <= -1000
-    assert L.sgdml_b200_pimd_run(H, 10, dt, 0.0, 1.0, 0.0, 0.0, 0, 0, None, None, None, None, None, None, st) <= -1000
-    kT3 = np.array([1e-3, 2e-3, 3e-3])
-    assert L.sgdml_b200_remd_run(H, 3, kT3.ctypes.data, 10, dt, 1.0, 0, 1, 0, *([None] * 8), st) <= -1000
-    assert L.sgdml_b200_relax_fire(H, 10, 0.01, 0.1, 0.1, 1.0, None, None, None, st) <= -1000
-    assert L.sgdml_b200_relax_lbfgs(H, 10, 0.01, 0.1, 10, 1.0, None, None, None, st) <= -1000
-    assert L.sgdml_b200_neb_fire(H, 3, 10, 0.01, 0.1, 0, 0.1, 0.1, 1.0, None, None, None, None, st) <= -1000
-    md = sgdml_b200.GDMLDynamics(gp, masses, n_replicas=3, E_to_eV=1.0, F_to_eV_Ang=1.0)
-    md._set_state_raw(R0, V0)
-    assert L.sgdml_b200_npt_run(md._handle, 10, dt, 0.0, 0.0, 0.0, 0.0, 1.0, 0, 0, *([None] * 6), st) <= -1000
-    assert L.sgdml_b200_npt_set_cells(md._handle, L0.ctypes.data, L0inv.ctypes.data, st) <= -1000
-    assert L.sgdml_b200_npt_get_cells(md._handle, o.ctypes.data, None, None, st) <= -1000
-    # bad runs and cells change nothing
     before = dyn._get_state_raw(), dyn._get_cells_raw()
     good = dict(n_steps=10, dt=dt, gamma=1.0, kT=1e-3, P0=0.1, beta_T=1e-3, tau_p=1.0, stride=0)
     for bad in (dict(P0=np.nan), dict(P0=np.inf), dict(beta_T=-1e-3), dict(beta_T=np.nan), dict(tau_p=0.0),

@@ -588,7 +588,8 @@ int sgdml_b200_assemble_ecstr_rows(const double* R_desc, const double* R_d_desc,
 /* Tuning / test hook: 0 = kernel chosen by molecule size (default), 1 = always the large-molecule
  * kernel (tables in global memory), which molecules above ~50 atoms need; 2 / 4 / 5 = small-molecule kernel with
  * per-permutation phases (k_assemble) / chunks of up to 16 permutations with byte permutation tables and per-kind
- * phases over the kept column atoms (k_assemble_v4) / the same on the compressed pair arrays (k_assemble_v5), where
+ * phases over the kept column atoms (v4: k_assemble_tile on expanded pair tables) / the same on the compressed pair
+ * arrays (v5: k_assemble_tile on them), where
  * the shared-memory budget allows it; any other value is rejected; 1000 + r = at most r row
  * points per launch of the small-molecule kernel (default 65535, the grid limit; tests lower it to
  * cover the multi-launch path that row ranges above 65535 training points take). */
@@ -598,8 +599,8 @@ int sgdml_b200_set_assemble_variant(int variant);
  * on a device with n_sm SMs: n_atoms atoms, n_perms permutations, n_colpts column points with at most nk kept column
  * atoms each (nk = n_atoms without a column list), n_rowpts row points; square = 1 for the full matrix (no column list,
  * every row point: nk = n_atoms, n_colpts = n_rowpts).  Writes 10 values to out:
- *   {kernel (0 k_assemble, 1 k_assemble_v4, 2 k_assemble_v5, 3 k_assemble_large), TJ, PG, n_chunks (grid.z), grid_x,
- *    dynamic shared memory bytes, sym, rows_per_launch, slab (doubles per CTA, large only), dl_in_smem}.
+ *   {kernel (0 k_assemble, 1 v4 = k_assemble_tile<ExpandedPairs>, 2 v5 = k_assemble_tile<CompressedPairs>,
+ *    3 k_assemble_large), TJ, PG, n_chunks (grid.z), grid_x, dynamic shared memory bytes, sym, rows_per_launch, slab (doubles per CTA, large only), dl_in_smem}.
  * Host only: needs no device. */
 int sgdml_b200_assemble_plan(int64_t n_atoms, int64_t n_perms, int64_t nk, int64_t n_colpts, int64_t n_rowpts,
                              int square, int n_sm, int64_t* out);

@@ -17,6 +17,14 @@
 // i.e. ~33 N^2 FMAs per permutation instead of the reference's ~2 D 3N (3S + 3N) per block.
 // One CTA owns row point i and a tile of TJ column points; the per-(j,p) vectors are staged in
 // shared memory; each thread then owns 3x3 atom-pair sub-blocks and writes them once.
+//
+// Kernels.  k_assemble_tile, the default up to ~64 atoms, keeps every table in shared memory and is one template over
+// two layouts of a point's pair tables: ExpandedPairs (the antisymmetric N x N tables, odd row strides; up to ~50
+// atoms) and CompressedPairs (x and g as stored, D = N(N-1)/2 entries looked up through d(a, g) and the sign of a - g;
+// half the footprint, so C60 fits on chip).  A layout holds only its table size, its table load, the three
+// phase-A row sums and the off-diagonal T lookup.  k_assemble (a test hook's reference) and k_assemble_large (larger
+// molecules, tables in global memory) stage the delta table instead and share its row sums.  All four share the
+// Matern factors, the sub-block update and the store.
 #include <algorithm>
 #include <numeric>
 
@@ -45,8 +53,8 @@ struct AsmArgs {
 };
 
 // expands compressed g (D,3) into the antisymmetric table G (N,N,3), zero diagonal, and the
-// descriptor x (D) into the symmetric table X (N,N)
-__device__ void load_pair_tables(const double* __restrict__ g, const double* __restrict__ x, int N,
+// descriptor x (D) into the symmetric table X (N,N); gs, xs: row strides of G and X in doubles
+__device__ void load_pair_tables(const double* __restrict__ g, const double* __restrict__ x, int N, int gs, int xs,
                                  double* __restrict__ G, double* __restrict__ X, int warp, int lane, int nw) {
   for (int a = warp; a < N; a += nw)
     for (int b = lane; b < N; b += 32) {
@@ -60,11 +68,10 @@ __device__ void load_pair_tables(const double* __restrict__ g, const double* __r
         v2 = sgn * g[d * 3 + 2];
         xv = x[d];
       }
-      const int idx = a * N + b;
-      G[idx * 3 + 0] = v0;
-      G[idx * 3 + 1] = v1;
-      G[idx * 3 + 2] = v2;
-      X[idx] = xv;
+      G[a * gs + b * 3 + 0] = v0;
+      G[a * gs + b * 3 + 1] = v1;
+      G[a * gs + b * 3 + 2] = v2;
+      X[a * xs + b] = xv;
     }
 }
 
@@ -75,6 +82,158 @@ __device__ __forceinline__ int fastdiv(int x, unsigned m) { return (int)__umulhi
 __device__ __forceinline__ int ceil_div_dev(int a, int b) { return (a + b - 1) / b; }
 
 constexpr int ASM_NI = 4;  // 3x3 atom-pair sub-blocks per thread (accumulators live in registers)
+
+// The Matern factors c[0] = c1, c[1] = c2 of one permutation from n2, the sum of its squared deltas with every pair
+// counted twice.  The constants of sig are recomputed per call: held in registers across k_assemble_tile, they made
+// its ExpandedPairs instantiation spill.
+__device__ __forceinline__ void matern_factors(double n2, double sig, double* c) {
+  const double sig2 = sig * sig;
+  const double inv_div = 1.0 / (3.0 * sig2 * sig2);     // 1/mat52_base_div (train.py:179)
+  const double nrm = sqrt(5.0) * sqrt(0.5 * n2);        // train.py:201
+  const double base = exp(-nrm / sig) * inv_div * 5.0;  // train.py:202
+  c[0] = base * 5.0;                                    // c1 (train.py:211)
+  c[1] = (sig2 + sig * nrm) * base;                     // c2 (train.py:219)
+}
+
+// Sub-block update acc[a][b] += c1 u[a] (x) v[b] - c2 T[a][b], off the diagonal b != P a: T = -gi (x) gj, so
+// -c2 T = +w gi (x) gj with w the signed c2 of the pair-table layout.
+__device__ __forceinline__ void acc_outer(double (&acc)[9], double c1, const double* ua, const double* vb, double w,
+                                          const double* gi, const double* gj) {
+  double t0[3], t1[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    t0[c] = w * gi[c];
+    t1[c] = gj[c];
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const double cu = c1 * ua[c];
+#pragma unroll
+    for (int c2i = 0; c2i < 3; ++c2i)
+      acc[c * 3 + c2i] = fma(t0[c], t1[c2i], fma(cu, vb[c2i], acc[c * 3 + c2i]));
+  }
+}
+
+// The same on the diagonal b == P a, where T[a][b] is the 3x3 sum dg.
+__device__ __forceinline__ void acc_diag(double (&acc)[9], double c1, double c2, const double* ua, const double* vb,
+                                         const double* dg) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const double cu = c1 * ua[c];
+#pragma unroll
+    for (int c2i = 0; c2i < 3; ++c2i)
+      acc[c * 3 + c2i] = fma(-c2, dg[c * 3 + c2i], fma(cu, vb[c2i], acc[c * 3 + c2i]));
+  }
+}
+
+// Stores the finished sub-block (row point i, row atom a; column point jc, column atom b) to its kept columns, and with
+// MIRROR in symmetric mode also to block (jc, i).
+template <bool MIRROR>
+__device__ __forceinline__ void store_subblock(const AsmArgs& p, const double (&acc)[9], int i, int jc, int a, int b) {
+  const int N3 = 3 * p.N;
+  const int64_t* dst = p.dest + (int64_t)jc * N3 + 3 * b;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    double* Krow = p.K + ((int64_t)(i - p.i0) * N3 + 3 * a + c) * p.ldk;
+#pragma unroll
+    for (int c2i = 0; c2i < 3; ++c2i) {
+      const int64_t col = dst[c2i];
+      if (col >= 0) Krow[col] = p.scale * acc[c * 3 + c2i];
+    }
+  }
+  if (MIRROR && p.sym && jc > i) {  // (sym implies i0 == 0 and jpts the identity)
+#pragma unroll
+    for (int c2i = 0; c2i < 3; ++c2i) {
+      double* Krow = p.K + ((int64_t)jc * N3 + 3 * b + c2i) * p.ldk + (int64_t)i * N3 + 3 * a;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) Krow[c] = p.scale * acc[c * 3 + c2i];
+    }
+  }
+}
+
+// This thread's output items (t, a, b) = column point of the tile, row atom, kept column atom (it_t = -1: none), out
+// of the tile's tj N NK (row atom, kept column atom) pairs; klist / nk: the kept column atoms of each column point.
+// Zeroes the accumulators.
+__device__ __forceinline__ void assign_items(const AsmArgs& p, int i, int jt0, int tj, const int* klist, const int* nk,
+                                             int (&it_t)[ASM_NI], int (&it_a)[ASM_NI], int (&it_b)[ASM_NI],
+                                             double (&acc)[ASM_NI][9]) {
+  const int N = p.N, NK = p.NK, nt = blockDim.x;
+#pragma unroll
+  for (int q = 0; q < ASM_NI; ++q) {
+    // grid.z splits the sub-blocks of large molecules
+    const int it = (int)blockIdx.z * ASM_NI * nt + threadIdx.x + q * nt;
+    bool ok = it < tj * N * NK;
+    const int t = ok ? fastdiv(it, p.mNNK) : 0;
+    if (p.sym && jt0 + t < i) ok = false;  // mirrored from block (j, i) instead
+    const int ak = ok ? it - t * N * NK : 0;
+    it_a[q] = fastdiv(ak, p.mNK);
+    const int k = ak - it_a[q] * NK;
+    if (k >= nk[t]) ok = false;
+    it_b[q] = ok ? klist[t * N + k] : 0;
+    it_t[q] = ok ? t : -1;
+#pragma unroll
+    for (int e = 0; e < 9; ++e) acc[q][e] = 0.0;
+  }
+}
+
+// Row r < 5N of one permutation's vectors over a staged delta table Dl[b][g] = delta_p[d(P^-1 b, P^-1 g)] (j frame),
+// pair tables G (N, N, 3) of the row point (Gi) and the column point (Gj):
+//   r < N:    u[a] = -sum_g G_i[a][g] Dl[Pa][Pg]
+//   r < 2N:   v[b] = -sum_g G_j[b][g] Dl[b][g]                    (b = r - N)
+//   else:     Dg[a][c][0..2] = sum_g G_i[a][g][c] G_j[Pa][Pg]     (3a + c = r - 2N)
+// KEPT_ONLY: v and Dg rows only for column atoms b, P a with a kept column (need[b] != 0).
+template <bool KEPT_ONLY>
+__device__ __forceinline__ void staged_row(int r, int N, const double* Gi, const double* Gj, const double* Dl,
+                                           const int* P, const int* need, double* u, double* v, double* Dg) {
+  const int N3 = 3 * N;
+  if (r < N) {
+    const int a = r, pa = P[a];
+    const double* gi = Gi + a * N3;
+    const double* dl = Dl + pa * N;
+    double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+    for (int g = 0; g < N; ++g) {
+      const double d = dl[P[g]];
+      s0 = fma(gi[g * 3 + 0], d, s0);
+      s1 = fma(gi[g * 3 + 1], d, s1);
+      s2 = fma(gi[g * 3 + 2], d, s2);
+    }
+    u[3 * a + 0] = -s0;
+    u[3 * a + 1] = -s1;
+    u[3 * a + 2] = -s2;
+  } else if (r < 2 * N) {
+    const int b = r - N;
+    if (KEPT_ONLY && !need[b]) return;
+    const double* gj = Gj + b * N3;
+    const double* dl = Dl + b * N;
+    double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+    for (int g = 0; g < N; ++g) {
+      const double d = dl[g];
+      s0 = fma(gj[g * 3 + 0], d, s0);
+      s1 = fma(gj[g * 3 + 1], d, s1);
+      s2 = fma(gj[g * 3 + 2], d, s2);
+    }
+    v[3 * b + 0] = -s0;
+    v[3 * b + 1] = -s1;
+    v[3 * b + 2] = -s2;
+  } else {
+    const int ac = r - 2 * N;
+    const int a = (int)__umulhi((unsigned)ac, 0x55555556u), c = ac - 3 * a;
+    if (KEPT_ONLY && !need[P[a]]) return;  // only read for the sub-block (a, b = P a)
+    const double* gi = Gi + a * N3 + c;
+    const double* gj = Gj + P[a] * N3;
+    double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+    for (int g = 0; g < N; ++g) {
+      const double x = gi[g * 3];
+      const double* y = gj + P[g] * 3;
+      s0 = fma(x, y[0], s0);
+      s1 = fma(x, y[1], s1);
+      s2 = fma(x, y[2], s2);
+    }
+    Dg[ac * 3 + 0] = s0;
+    Dg[ac * 3 + 1] = s1;
+    Dg[ac * 3 + 2] = s2;
+  }
+}
 
 // One CTA: row point i, a tile of TJ column points.  Permutations are the OUTER loop; for each
 // permutation the per-point vectors (delta table, u, v, diagonal sums) are rebuilt in shared
@@ -108,11 +267,11 @@ __global__ void __launch_bounds__(256, 2) k_assemble(const AsmArgs p) {
   int* klist = need + TJ * N;                           // TJ*N: the kept column atoms of point t, compact
   int* nk = klist + TJ * N;                             // TJ: how many
 
-  load_pair_tables(p.R_d_desc + (int64_t)i * p.D * 3, p.R_desc + (int64_t)i * p.D, N, Gi, Xi, warp, lane, nw);
+  load_pair_tables(p.R_d_desc + (int64_t)i * p.D * 3, p.R_desc + (int64_t)i * p.D, N, N3, N, Gi, Xi, warp, lane, nw);
   for (int t = 0; t < tj; ++t) {
     const int j = p.jpts[jt0 + t];
-    load_pair_tables(p.R_d_desc + (int64_t)j * p.D * 3, p.R_desc + (int64_t)j * p.D, N, Gj + t * NN3, Xj + t * NN, warp,
-                     lane, nw);
+    load_pair_tables(p.R_d_desc + (int64_t)j * p.D * 3, p.R_desc + (int64_t)j * p.D, N, N3, N, Gj + t * NN3,
+                     Xj + t * NN, warp, lane, nw);
   }
   for (int idx = tid; idx < S * N; idx += nt) {
     sP[idx] = p.aperm[idx];
@@ -136,28 +295,9 @@ __global__ void __launch_bounds__(256, 2) k_assemble(const AsmArgs p) {
   }
   __syncthreads();
 
-  // this thread's output items: (t, a, b) = column point, row atom, kept column atom
   int it_t[ASM_NI], it_a[ASM_NI], it_b[ASM_NI];
   double acc[ASM_NI][9];
-#pragma unroll
-  for (int q = 0; q < ASM_NI; ++q) {
-    const int it = (int)blockIdx.z * ASM_NI * nt + tid + q * nt;  // grid.z splits the sub-blocks of large molecules
-    bool ok = it < tj * N * p.NK;
-    const int t = ok ? fastdiv(it, p.mNNK) : 0;
-    if (p.sym && jt0 + t < i) ok = false;  // mirrored from block (j, i) instead
-    const int ak = ok ? it - t * N * p.NK : 0;
-    it_a[q] = fastdiv(ak, p.mNK);
-    const int k = ak - it_a[q] * p.NK;
-    if (k >= nk[t]) ok = false;
-    it_b[q] = ok ? klist[t * N + k] : 0;
-    it_t[q] = ok ? t : -1;
-#pragma unroll
-    for (int e = 0; e < 9; ++e) acc[q][e] = 0.0;
-  }
-
-  const double sig = p.sig;
-  const double sig2 = sig * sig;
-  const double inv_div = 1.0 / (3.0 * sig2 * sig2);  // 1/mat52_base_div (train.py:179)
+  assign_items(p, i, jt0, tj, klist, nk, it_t, it_a, it_b, acc);
 
   for (int pp = 0; pp < S; ++pp) {
     const int* P = sP + pp * N;
@@ -180,73 +320,19 @@ __global__ void __launch_bounds__(256, 2) k_assemble(const AsmArgs p) {
     }
     __syncthreads();
 
-    // ---- S2: u[a] = -sum_g G_i[a][g] Dl[Pa][Pg],  v[b] = -sum_g G_j[b][g] Dl[b][g],
-    //          Dg[a][c][c'] = sum_g G_i[a][g][c] G_j[Pa][Pg][c']      (units of 3 outputs each)
-    {
-      // Matern factors of this permutation (one thread per column point, from the tail of the CTA)
-      if (tid >= nt - tj) {
-        const int t = nt - 1 - tid;
-        double n2 = 0.0;
-        for (int w = 0; w < nw; ++w) n2 += n2p[t * 8 + w];
-        const double nrm = sqrt(5.0) * sqrt(0.5 * n2);  // every pair twice; train.py:201
-        const double base = exp(-nrm / sig) * inv_div * 5.0;          // train.py:202
-        cc[(pp * TJ + t) * 2 + 0] = base * 5.0;                       // c1 (train.py:211)
-        cc[(pp * TJ + t) * 2 + 1] = (sig2 + sig * nrm) * base;        // c2 (train.py:219)
-      }
-      const int per = 5 * N;  // N (u) + N (v) + 3N (Dg rows a,c)
-      for (int idx = tid; idx < tj * per; idx += nt) {
-        const int t = fastdiv(idx, p.mPer);
-        const int r = idx - t * per;
-        const double* Gjt = Gj + t * NN3;
-        const double* Dlt = Dl + t * NN;
-        if (r < N) {  // u[a][0..2]
-          const int a = r, pa = P[a];
-          const double* gi = Gi + a * N3;
-          const double* dl = Dlt + pa * N;
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double d = dl[P[g]];
-            s0 = fma(gi[g * 3 + 0], d, s0);
-            s1 = fma(gi[g * 3 + 1], d, s1);
-            s2 = fma(gi[g * 3 + 2], d, s2);
-          }
-          u[t * N3 + 3 * a + 0] = -s0;
-          u[t * N3 + 3 * a + 1] = -s1;
-          u[t * N3 + 3 * a + 2] = -s2;
-        } else if (r < 2 * N) {  // v[b][0..2]
-          const int b = r - N;
-          if (!need[t * N + b]) continue;
-          const double* gj = Gjt + b * N3;
-          const double* dl = Dlt + b * N;
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double d = dl[g];
-            s0 = fma(gj[g * 3 + 0], d, s0);
-            s1 = fma(gj[g * 3 + 1], d, s1);
-            s2 = fma(gj[g * 3 + 2], d, s2);
-          }
-          v[t * N3 + 3 * b + 0] = -s0;
-          v[t * N3 + 3 * b + 1] = -s1;
-          v[t * N3 + 3 * b + 2] = -s2;
-        } else {  // Dg[a][c][0..2]
-          const int ac = r - 2 * N;
-          const int a = (int)__umulhi((unsigned)ac, 0x55555556u), c = ac - 3 * a;
-          if (!need[t * N + P[a]]) continue;  // only read for the sub-block (a, b = P a)
-          const double* gi = Gi + a * N3 + c;
-          const double* gj = Gjt + P[a] * N3;
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double x = gi[g * 3];
-            const double* y = gj + P[g] * 3;
-            s0 = fma(x, y[0], s0);
-            s1 = fma(x, y[1], s1);
-            s2 = fma(x, y[2], s2);
-          }
-          Dg[t * 3 * N3 + ac * 3 + 0] = s0;
-          Dg[t * 3 * N3 + ac * 3 + 1] = s1;
-          Dg[t * 3 * N3 + ac * 3 + 2] = s2;
-        }
-      }
+    // ---- S2: u, v and Dg of every column point of the tile (units of 3 outputs each)
+    // Matern factors of this permutation (one thread per column point, from the tail of the CTA)
+    if (tid >= nt - tj) {
+      const int t = nt - 1 - tid;
+      double n2 = 0.0;
+      for (int w = 0; w < nw; ++w) n2 += n2p[t * 8 + w];
+      matern_factors(n2, p.sig, cc + (pp * TJ + t) * 2);
+    }
+    const int per = 5 * N;  // N (u) + N (v) + 3N (Dg rows a,c)
+    for (int idx = tid; idx < tj * per; idx += nt) {
+      const int t = fastdiv(idx, p.mPer);
+      staged_row<true>(idx - t * per, N, Gi, Gj + t * NN3, Dl + t * NN, P, need + t * N, u + t * N3, v + t * N3,
+                       Dg + t * 3 * N3);
     }
     __syncthreads();
 
@@ -260,66 +346,22 @@ __global__ void __launch_bounds__(256, 2) k_assemble(const AsmArgs p) {
       const double* ua = u + t * N3 + 3 * a;
       const double* vb = v + t * N3 + 3 * b;
       const int pa = P[a];
-      double t0[3], t1[3];  // T[a][b] = t0[c] * t1[c'] (outer product) unless b == P a
-      if (b != pa) {
-        const double* gi = Gi + (a * N + Pi[b]) * 3;
-        const double* gj = Gj + t * NN3 + (pa * N + b) * 3;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          t0[c] = c2 * gi[c];   // -c2 * (-gi (x) gj) = +c2 gi (x) gj
-          t1[c] = gj[c];
-        }
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const double cu = c1 * ua[c];
-#pragma unroll
-          for (int c2i = 0; c2i < 3; ++c2i)
-            acc[q][c * 3 + c2i] = fma(t0[c], t1[c2i], fma(cu, vb[c2i], acc[q][c * 3 + c2i]));
-        }
-      } else {
-        const double* dg = Dg + t * 3 * N3 + 9 * a;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const double cu = c1 * ua[c];
-#pragma unroll
-          for (int c2i = 0; c2i < 3; ++c2i)
-            acc[q][c * 3 + c2i] = fma(-c2, dg[c * 3 + c2i], fma(cu, vb[c2i], acc[q][c * 3 + c2i]));
-        }
-      }
+      if (b != pa)
+        acc_outer(acc[q], c1, ua, vb, c2, Gi + (a * N + Pi[b]) * 3, Gj + t * NN3 + (pa * N + b) * 3);
+      else
+        acc_diag(acc[q], c1, c2, ua, vb, Dg + t * 3 * N3 + 9 * a);
     }
     // (no barrier here: the next S1 only writes Dl / cc[pp+1]; u, v, Dg are rewritten after it)
   }
 
   // ---- single store of the finished 3x3 sub-blocks (+ the mirrored block in symmetric mode)
 #pragma unroll
-  for (int q = 0; q < ASM_NI; ++q) {
-    const int t = it_t[q];
-    if (t < 0) continue;
-    const int a = it_a[q], b = it_b[q];
-    const int64_t* dst = p.dest + (int64_t)(jt0 + t) * N3 + 3 * b;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      double* Krow = p.K + ((int64_t)(i - p.i0) * N3 + 3 * a + c) * p.ldk;
-#pragma unroll
-      for (int c2i = 0; c2i < 3; ++c2i) {
-        const int64_t col = dst[c2i];
-        if (col >= 0) Krow[col] = p.scale * acc[q][c * 3 + c2i];
-      }
-    }
-    if (p.sym && jt0 + t > i) {  // (sym implies i0 == 0)
-      const int j = jt0 + t;
-#pragma unroll
-      for (int c2i = 0; c2i < 3; ++c2i) {
-        double* Krow = p.K + ((int64_t)j * N3 + 3 * b + c2i) * p.ldk + (int64_t)i * N3 + 3 * a;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) Krow[c] = p.scale * acc[q][c * 3 + c2i];
-      }
-    }
-  }
+  for (int q = 0; q < ASM_NI; ++q)
+    if (it_t[q] >= 0) store_subblock<true>(p, acc[q], i, jt0 + it_t[q], it_a[q], it_b[q]);
 }
 
 // ---------------------------------------------------------------------------------------------
-// k_assemble_v4: the default small-molecule kernel, built for many permutations and column subsets as well (BASELINE
+// k_assemble_tile: the default small-molecule kernel, built for many permutations and column subsets as well (BASELINE
 // config 3: N = 42, S = 243, the Nystroem set-up keeps ~9 of a point's 126 columns).  Against k_assemble, what the
 // first kernel's profile showed (few warps active, a mostly idle FP64 pipe, barrier / short-scoreboard / wait stalls):
 //  * permutations are processed in CHUNKS of PG: phase A computes the per-(point, permutation) vectors u, v, Dg of the
@@ -330,45 +372,160 @@ __global__ void __launch_bounds__(256, 2) k_assemble(const AsmArgs p) {
 //    comes out of the u rows, which are always needed;
 //  * the atom-permutation tables are bytes (20 KB instead of 82 KB at S = 243, N = 42), which leaves room for chunks of
 //    up to 16 permutations next to the four pair tables of a 42-atom block;
-//  * the pair tables have ODD row strides (3N | 1, N | 1 doubles): threads of a warp work on different table rows, and
-//    with N = 42 even strides put every fourth row on the same banks;
 //  * a CTA walks over `tiles_per_cta` column tiles with the row point's tables resident.
 // Phase B (the 3x3 sub-block accumulation in registers) is that of k_assemble.
-__device__ void load_pair_tables_strided(const double* __restrict__ g, const double* __restrict__ x, int N, int gs, int xs,
-                                         double* __restrict__ G, double* __restrict__ X, int warp, int lane, int nw) {
-  for (int a = warp; a < N; a += nw)
-    for (int b = lane; b < N; b += 32) {
-      double v0 = 0.0, v1 = 0.0, v2 = 0.0, xv = 0.0;
-      if (a != b) {
-        const int hi = a > b ? a : b, lo = a > b ? b : a;
-        const int d = pair_index(hi, lo);
-        const double sgn = a > b ? 1.0 : -1.0;
-        v0 = sgn * g[d * 3 + 0];
-        v1 = sgn * g[d * 3 + 1];
-        v2 = sgn * g[d * 3 + 2];
-        xv = x[d];
-      }
-      G[a * gs + b * 3 + 0] = v0;
-      G[a * gs + b * 3 + 1] = v1;
-      G[a * gs + b * 3 + 2] = v2;
-      X[a * xs + b] = xv;
-    }
-}
+//
+// The pair tables of a point come in one of two layouts (Pairs).  Each holds the shared-memory doubles of one point's
+// tables (g_doubles, x_doubles; doubles() on the host), their load, the phase-A row sums over them (u_row with
+// |delta|^2, v_row, dg_row) and the off-diagonal T lookup (t_pair).  Gj / Xj there are the tables of one column point.
 
-__global__ void __launch_bounds__(256, 2) k_assemble_v4(const AsmArgs p, int PG, int tiles_per_cta) {
+// The antisymmetric N x N tables G (N x N x 3) and X (N x N), with ODD row strides (3N | 1, N | 1 doubles): threads of
+// a warp work on different table rows, and with N = 42 even strides put every fourth row on the same banks.
+struct ExpandedPairs {
+  int N, gs, xs;
+  __device__ ExpandedPairs(int N_, int) : N(N_), gs(3 * N_ | 1), xs(N_ | 1) {}
+  static size_t doubles(int N) { return (size_t)N * ((3 * (size_t)N | 1) + ((size_t)N | 1)); }
+  __device__ __forceinline__ int g_doubles() const { return N * gs; }
+  __device__ __forceinline__ int x_doubles() const { return N * xs; }
+
+  __device__ __forceinline__ void load(const double* g, const double* x, double* G, double* X) const {
+    load_pair_tables(g, x, N, gs, xs, G, X, threadIdx.x >> 5, threadIdx.x & 31, blockDim.x >> 5);
+  }
+  // u[a] = -(s0, s1, s2) = -sum_g G_i[a][g] delta[a][g], q2 = sum_g delta[a][g]^2,
+  // delta[a][g] = x_i[a][g] - x_j[Pa][Pg]
+  __device__ __forceinline__ void u_row(const double* Gi, const double* Xi, const double* Xj, const unsigned char* P,
+                                        int a, double& s0, double& s1, double& s2, double& q2) const {
+    const double* gi = Gi + a * gs;
+    const double* xi = Xi + a * xs;
+    const double* xj = Xj + P[a] * xs;
+    for (int g = 0; g < N; ++g) {
+      const double d = xi[g] - xj[P[g]];
+      q2 = fma(d, d, q2);
+      s0 = fma(gi[g * 3 + 0], d, s0);
+      s1 = fma(gi[g * 3 + 1], d, s1);
+      s2 = fma(gi[g * 3 + 2], d, s2);
+    }
+  }
+  // v[b] = -(s0, s1, s2) = -sum_g G_j[b][g] delta[P^-1 b][P^-1 g]
+  __device__ __forceinline__ void v_row(const double* Xi, const double* Gj, const double* Xj, const unsigned char* Pi,
+                                        int b, double& s0, double& s1, double& s2) const {
+    const double* gj = Gj + b * gs;
+    const double* xj = Xj + b * xs;
+    const double* xi = Xi + Pi[b] * xs;
+    for (int g = 0; g < N; ++g) {
+      const double d = xi[Pi[g]] - xj[g];
+      s0 = fma(gj[g * 3 + 0], d, s0);
+      s1 = fma(gj[g * 3 + 1], d, s1);
+      s2 = fma(gj[g * 3 + 2], d, s2);
+    }
+  }
+  // Dg[a][c][0..2] = (s0, s1, s2) = sum_g G_i[a][g][c] G_j[Pa][Pg][0..2], b = P a
+  __device__ __forceinline__ void dg_row(const double* Gi, const double* Gj, const unsigned char* P, int a, int b,
+                                         int c, double& s0, double& s1, double& s2) const {
+    const double* gi = Gi + a * gs + c;
+    const double* gj = Gj + b * gs;
+    for (int g = 0; g < N; ++g) {
+      const double x = gi[g * 3];
+      const double* y = gj + P[g] * 3;
+      s0 = fma(x, y[0], s0);
+      s1 = fma(x, y[1], s1);
+      s2 = fma(x, y[2], s2);
+    }
+  }
+  // T[a][b] = -G_i[a][P^-1 b] (x) G_j[Pa][b] = -gi (x) gj (b != P a); returns the w of acc_outer
+  __device__ __forceinline__ double t_pair(const double* Gi, const double* Gj, int a, int pa, int b, int pib,
+                                           double c2, const double*& gi, const double*& gj) const {
+    gi = Gi + a * gs + pib * 3;
+    gj = Gj + pa * gs + b * 3;
+    return c2;
+  }
+};
+
+// The compressed pair arrays as stored: g (D x 3) and x (D), 4 D doubles per point instead of the 4 N^2 of the
+// expanded tables, looked up through the pair index d(a, g) = max(max - 1)/2 + min with the sign of a - g.  That halves
+// the table footprint: molecules up to ~64 atoms (BASELINE config 5: C60, N = 60, S = 120) keep everything on chip
+// with chunks of 11 permutations, where k_assemble_large walks per-CTA slabs in global memory one permutation at a
+// time.
+__device__ __forceinline__ int pidx(int a, int g) { return a > g ? a * (a - 1) / 2 + g : g * (g - 1) / 2 + a; }
+
+struct CompressedPairs {
+  int N, D;
+  __device__ CompressedPairs(int N_, int D_) : N(N_), D(D_) {}
+  static size_t doubles(int N) { return 4 * ((size_t)N * (N - 1) / 2); }
+  __device__ __forceinline__ int g_doubles() const { return 3 * D; }
+  __device__ __forceinline__ int x_doubles() const { return D; }
+
+  __device__ __forceinline__ void load(const double* g, const double* x, double* G, double* X) const {
+    for (int e = threadIdx.x; e < 3 * D; e += blockDim.x) G[e] = g[e];
+    for (int e = threadIdx.x; e < D; e += blockDim.x) X[e] = x[e];
+  }
+  __device__ __forceinline__ void u_row(const double* Gi, const double* Xi, const double* Xj, const unsigned char* P,
+                                        int a, double& s0, double& s1, double& s2, double& q2) const {
+    const int pa = P[a];
+    for (int g = 0; g < N; ++g) {
+      if (g == a) continue;
+      const int di = pidx(a, g), dj = pidx(pa, P[g]);
+      const double d = Xi[di] - Xj[dj];
+      q2 = fma(d, d, q2);
+      const double w = a > g ? d : -d;  // G_i[a][g] = sgn(a - g) g_i[d(a,g)]
+      const double* gi = Gi + 3 * di;
+      s0 = fma(gi[0], w, s0);
+      s1 = fma(gi[1], w, s1);
+      s2 = fma(gi[2], w, s2);
+    }
+  }
+  __device__ __forceinline__ void v_row(const double* Xi, const double* Gj, const double* Xj, const unsigned char* Pi,
+                                        int b, double& s0, double& s1, double& s2) const {
+    const int pib = Pi[b];
+    for (int g = 0; g < N; ++g) {
+      if (g == b) continue;
+      const int dj = pidx(b, g), di = pidx(pib, Pi[g]);
+      const double d = Xi[di] - Xj[dj];
+      const double w = b > g ? d : -d;
+      const double* gj = Gj + 3 * dj;
+      s0 = fma(gj[0], w, s0);
+      s1 = fma(gj[1], w, s1);
+      s2 = fma(gj[2], w, s2);
+    }
+  }
+  __device__ __forceinline__ void dg_row(const double* Gi, const double* Gj, const unsigned char* P, int a, int b,
+                                         int c, double& s0, double& s1, double& s2) const {
+    for (int g = 0; g < N; ++g) {
+      if (g == a) continue;
+      const int pg = P[g];
+      const int di = pidx(a, g), dj = pidx(b, pg);  // b = P a
+      const double gic = Gi[3 * di + c];
+      const double x = ((a > g) == (b > pg)) ? gic : -gic;  // sgn(a - g) sgn(Pa - Pg)
+      const double* y = Gj + 3 * dj;
+      s0 = fma(x, y[0], s0);
+      s1 = fma(x, y[1], s1);
+      s2 = fma(x, y[2], s2);
+    }
+  }
+  __device__ __forceinline__ double t_pair(const double* Gi, const double* Gj, int a, int pa, int b, int pib,
+                                           double c2, const double*& gi, const double*& gj) const {
+    gi = Gi + 3 * pidx(a, pib);
+    gj = Gj + 3 * pidx(pa, b);
+    return ((a > pib) == (pa > b)) ? c2 : -c2;  // sgn(a - P^-1 b) sgn(Pa - b) c2
+  }
+};
+
+template <class Pairs>
+__global__ void __launch_bounds__(256, 2) k_assemble_tile(const AsmArgs p, int PG, int tiles_per_cta) {
   extern __shared__ __align__(16) double sm[];
   const int N = p.N, S = p.S, TJ = p.TJ, NK = p.NK;
   const int N3 = 3 * N;
-  const int GS = N3 | 1, XS = N | 1;  // odd row strides of the pair tables
   const int tid = threadIdx.x, nt = blockDim.x;
   const int warp = tid >> 5, lane = tid & 31, nw = nt >> 5;
   const int i = p.i0 + blockIdx.y;
+  const Pairs L(N, p.D);
+  const int GT = L.g_doubles(), XT = L.x_doubles();
 
-  double* Gi = sm;                        // N*GS
-  double* Xi = Gi + N * GS;               // N*XS
-  double* Gj = Xi + N * XS;               // TJ*N*GS
-  double* Xj = Gj + TJ * N * GS;          // TJ*N*XS
-  double* uS = Xj + TJ * N * XS;          // TJ*PG*N3
+  double* Gi = sm;                        // GT     pair tables of the row point
+  double* Xi = Gi + GT;                   // XT
+  double* Gj = Xi + XT;                   // TJ*GT  pair tables of the column points
+  double* Xj = Gj + TJ * GT;              // TJ*XT
+  double* uS = Xj + TJ * XT;              // TJ*PG*N3
   double* vS = uS + TJ * PG * N3;         // TJ*PG*N3   (rows of kept column atoms only)
   double* DgS = vS + TJ * PG * N3;        // TJ*PG*3*N3 (rows a = P^-1 b of kept column atoms b only)
   double* n2p = DgS + TJ * PG * 3 * N3;   // TJ*PG*N    per-u-row sums of squared deltas (each pair twice)
@@ -378,15 +535,11 @@ __global__ void __launch_bounds__(256, 2) k_assemble_v4(const AsmArgs p, int PG,
   unsigned char* sP = reinterpret_cast<unsigned char*>(nk + TJ);  // S*N
   unsigned char* sPi = sP + S * N;                                     // S*N
 
-  load_pair_tables_strided(p.R_d_desc + (int64_t)i * p.D * 3, p.R_desc + (int64_t)i * p.D, N, GS, XS, Gi, Xi, warp, lane,
-                           nw);
+  L.load(p.R_d_desc + (int64_t)i * p.D * 3, p.R_desc + (int64_t)i * p.D, Gi, Xi);
   for (int idx = tid; idx < S * N; idx += nt) {
     sP[idx] = (unsigned char)p.aperm[idx];
     sPi[idx] = (unsigned char)p.apinv[idx];
   }
-  const double sig = p.sig;
-  const double sig2 = sig * sig;
-  const double inv_div = 1.0 / (3.0 * sig2 * sig2);  // 1/mat52_base_div (train.py:179)
 
   const int tile_begin = blockIdx.x * tiles_per_cta;
   const int tile_end = min(tile_begin + tiles_per_cta, ceil_div_dev(p.nJ, TJ));
@@ -397,8 +550,7 @@ __global__ void __launch_bounds__(256, 2) k_assemble_v4(const AsmArgs p, int PG,
     __syncthreads();  // the previous tile's phase B has finished with Gj / the vectors
     for (int t = 0; t < tj; ++t) {
       const int j = p.jpts[jt0 + t];
-      load_pair_tables_strided(p.R_d_desc + (int64_t)j * p.D * 3, p.R_desc + (int64_t)j * p.D, N, GS, XS, Gj + t * N * GS,
-                               Xj + t * N * XS, warp, lane, nw);
+      L.load(p.R_d_desc + (int64_t)j * p.D * 3, p.R_desc + (int64_t)j * p.D, Gj + t * GT, Xj + t * XT);
     }
     for (int tw = warp; tw < tj; tw += nw) {  // compact list of the kept column atoms of point tw (ballot over atoms)
       int c = 0;
@@ -416,24 +568,9 @@ __global__ void __launch_bounds__(256, 2) k_assemble_v4(const AsmArgs p, int PG,
       if (lane == 0) nk[tw] = c;
     }
     __syncthreads();
-    // this thread's output items: (t, a, b) = column point, row atom, kept column atom
     int it_t[ASM_NI], it_a[ASM_NI], it_b[ASM_NI];
     double acc[ASM_NI][9];
-#pragma unroll
-    for (int q = 0; q < ASM_NI; ++q) {
-      const int it = (int)blockIdx.z * ASM_NI * nt + tid + q * nt;  // grid.z splits the sub-blocks of large molecules
-      bool ok = it < tj * N * NK;
-      const int t = ok ? fastdiv(it, p.mNNK) : 0;
-      if (p.sym && jt0 + t < i) ok = false;  // mirrored from block (j, i) instead
-      const int ak = ok ? it - t * N * NK : 0;
-      it_a[q] = fastdiv(ak, p.mNK);
-      const int k = ak - it_a[q] * NK;
-      if (k >= nk[t]) ok = false;
-      it_b[q] = ok ? klist[t * N + k] : 0;
-      it_t[q] = ok ? t : -1;
-#pragma unroll
-      for (int e = 0; e < 9; ++e) acc[q][e] = 0.0;
-    }
+    assign_items(p, i, jt0, tj, klist, nk, it_t, it_a, it_b, acc);
 
     for (int p0 = 0; p0 < S; p0 += PG) {
       const int pg = min(PG, S - p0);
@@ -441,54 +578,32 @@ __global__ void __launch_bounds__(256, 2) k_assemble_v4(const AsmArgs p, int PG,
       const int n_slots = tj * pg;
       const int nU = n_slots * N, nV = n_slots * NK, nD = 3 * nV;
       for (int idx = tid; idx < nU + nV + nD; idx += nt) {
-        if (idx < nU) {
-          // u[a] = -sum_g G_i[a][g] delta[a][g],  delta[a][g] = x_i[a][g] - x_j[Pa][Pg]  (i frame)
+        double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+        if (idx < nU) {  // u rows, with the squared deltas
           const int sl = fastdiv(idx, p.mN);
           const int a = idx - sl * N;
           const int t = sl / pg, pl = sl - t * pg;
-          const unsigned char* P = sP + (p0 + pl) * N;
-          const double* gi = Gi + a * GS;
-          const double* xi = Xi + a * XS;
-          const double* xj = Xj + t * N * XS + P[a] * XS;
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0, q2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double d = xi[g] - xj[P[g]];
-            q2 = fma(d, d, q2);
-            s0 = fma(gi[g * 3 + 0], d, s0);
-            s1 = fma(gi[g * 3 + 1], d, s1);
-            s2 = fma(gi[g * 3 + 2], d, s2);
-          }
+          double q2 = 0.0;
+          L.u_row(Gi, Xi, Xj + t * XT, sP + (p0 + pl) * N, a, s0, s1, s2, q2);
           const int slot = t * PG + pl;
           double* u = uS + slot * N3 + 3 * a;
           u[0] = -s0;
           u[1] = -s1;
           u[2] = -s2;
           n2p[slot * N + a] = q2;
-        } else if (idx < nU + nV) {
-          // v[b] = -sum_g G_j[b][g] delta[P^-1 b][P^-1 g]  for the kept column atoms b
+        } else if (idx < nU + nV) {  // v rows of the kept column atoms b
           const int e = idx - nU;
           const int sl = fastdiv(e, p.mNK);
           const int k = e - sl * NK;
           const int t = sl / pg, pl = sl - t * pg;
           if (k >= nk[t]) continue;
           const int b = klist[t * N + k];
-          const unsigned char* Pi = sPi + (p0 + pl) * N;
-          const double* gj = Gj + t * N * GS + b * GS;
-          const double* xj = Xj + t * N * XS + b * XS;
-          const double* xi = Xi + Pi[b] * XS;
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double d = xi[Pi[g]] - xj[g];
-            s0 = fma(gj[g * 3 + 0], d, s0);
-            s1 = fma(gj[g * 3 + 1], d, s1);
-            s2 = fma(gj[g * 3 + 2], d, s2);
-          }
+          L.v_row(Xi, Gj + t * GT, Xj + t * XT, sPi + (p0 + pl) * N, b, s0, s1, s2);
           double* v = vS + (t * PG + pl) * N3 + 3 * b;
           v[0] = -s0;
           v[1] = -s1;
           v[2] = -s2;
-        } else {
-          // Dg[a][c][0..2] = sum_g G_i[a][g][c] G_j[Pa][Pg][0..2]  for a = P^-1 b, b a kept column atom
+        } else {  // Dg rows a = P^-1 b of the kept column atoms b
           const int e = idx - nU - nV;
           const int e3 = (int)__umulhi((unsigned)e, 0x55555556u), c = e - 3 * e3;
           const int sl = fastdiv(e3, p.mNK);
@@ -496,18 +611,8 @@ __global__ void __launch_bounds__(256, 2) k_assemble_v4(const AsmArgs p, int PG,
           const int t = sl / pg, pl = sl - t * pg;
           if (k >= nk[t]) continue;
           const int b = klist[t * N + k];
-          const unsigned char* P = sP + (p0 + pl) * N;
           const int a = sPi[(p0 + pl) * N + b];
-          const double* gi = Gi + a * GS + c;
-          const double* gj = Gj + t * N * GS + b * GS;  // b = P a
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double x = gi[g * 3];
-            const double* y = gj + P[g] * 3;
-            s0 = fma(x, y[0], s0);
-            s1 = fma(x, y[1], s1);
-            s2 = fma(x, y[2], s2);
-          }
+          L.dg_row(Gi, Gj + t * GT, sP + (p0 + pl) * N, a, b, c, s0, s1, s2);
           double* dg = DgS + (t * PG + pl) * 3 * N3 + (a * 3 + c) * 3;
           dg[0] = s0;
           dg[1] = s1;
@@ -521,10 +626,7 @@ __global__ void __launch_bounds__(256, 2) k_assemble_v4(const AsmArgs p, int PG,
         const int slot = t * PG + pl;
         double n2 = 0.0;
         for (int a = 0; a < N; ++a) n2 += n2p[slot * N + a];
-        const double nrm = sqrt(5.0) * sqrt(0.5 * n2);  // every pair twice; train.py:201
-        const double base = exp(-nrm / sig) * inv_div * 5.0;          // train.py:202
-        cc[slot * 2 + 0] = base * 5.0;                                 // c1 (train.py:211)
-        cc[slot * 2 + 1] = (sig2 + sig * nrm) * base;                  // c2 (train.py:219)
+        matern_factors(n2, p.sig, cc + slot * 2);
       }
       __syncthreads();
       // ---- phase B: acc[a][b] += c1 u[a] (x) v[b] - c2 T[a][b] for the permutations of the chunk
@@ -542,30 +644,11 @@ __global__ void __launch_bounds__(256, 2) k_assemble_v4(const AsmArgs p, int PG,
           const double* vb = vS + slot * N3 + 3 * b;
           const int pa = P[a];
           if (b != pa) {
-            const double* gi = Gi + a * GS + Pi[b] * 3;
-            const double* gj = Gj + t * N * GS + pa * GS + b * 3;
-            double t0[3], t1[3];  // T[a][b] = -gi (x) gj  ->  -c2 T = +c2 gi (x) gj
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              t0[c] = c2 * gi[c];
-              t1[c] = gj[c];
-            }
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              const double cu = c1 * ua[c];
-#pragma unroll
-              for (int c2i = 0; c2i < 3; ++c2i)
-                acc[q][c * 3 + c2i] = fma(t0[c], t1[c2i], fma(cu, vb[c2i], acc[q][c * 3 + c2i]));
-            }
+            const double *gi, *gj;
+            const double w = L.t_pair(Gi, Gj + t * GT, a, pa, b, Pi[b], c2, gi, gj);
+            acc_outer(acc[q], c1, ua, vb, w, gi, gj);
           } else {
-            const double* dg = DgS + slot * 3 * N3 + 9 * a;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              const double cu = c1 * ua[c];
-#pragma unroll
-              for (int c2i = 0; c2i < 3; ++c2i)
-                acc[q][c * 3 + c2i] = fma(-c2, dg[c * 3 + c2i], fma(cu, vb[c2i], acc[q][c * 3 + c2i]));
-            }
+            acc_diag(acc[q], c1, c2, ua, vb, DgS + slot * 3 * N3 + 9 * a);
           }
         }
       }
@@ -574,293 +657,8 @@ __global__ void __launch_bounds__(256, 2) k_assemble_v4(const AsmArgs p, int PG,
 
     // ---- single store of the finished 3x3 sub-blocks (+ the mirrored block in symmetric mode)
 #pragma unroll
-    for (int q = 0; q < ASM_NI; ++q) {
-      const int t = it_t[q];
-      if (t < 0) continue;
-      const int a = it_a[q], b = it_b[q];
-      const int64_t* dst = p.dest + (int64_t)(jt0 + t) * N3 + 3 * b;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        double* Krow = p.K + ((int64_t)(i - p.i0) * N3 + 3 * a + c) * p.ldk;
-#pragma unroll
-        for (int c2i = 0; c2i < 3; ++c2i) {
-          const int64_t col = dst[c2i];
-          if (col >= 0) Krow[col] = p.scale * acc[q][c * 3 + c2i];
-        }
-      }
-      if (p.sym && jt0 + t > i) {  // (sym implies i0 == 0)
-        const int j = jt0 + t;
-#pragma unroll
-        for (int c2i = 0; c2i < 3; ++c2i) {
-          double* Krow = p.K + ((int64_t)j * N3 + 3 * b + c2i) * p.ldk + (int64_t)i * N3 + 3 * a;
-#pragma unroll
-          for (int c = 0; c < 3; ++c) Krow[c] = p.scale * acc[q][c * 3 + c2i];
-        }
-      }
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// k_assemble_v5: k_assemble_v4 on the COMPRESSED pair arrays -- x (D) and g (D x 3) of the row point and of the column
-// point(s) sit in shared memory exactly as stored (4 D doubles per point instead of the 4 N^2 of the expanded
-// antisymmetric tables), looked up through the pair index d(a, g) = max(max - 1)/2 + min with the sign of a - g.  That
-// halves the table footprint: molecules up to ~64 atoms (BASELINE config 5: C60, N = 60, S = 120) keep everything on chip
-// with chunks of 11 permutations, where k_assemble_large walks per-CTA slabs in global memory one permutation at a time.
-__device__ __forceinline__ int pidx(int a, int g) { return a > g ? a * (a - 1) / 2 + g : g * (g - 1) / 2 + a; }
-
-__global__ void __launch_bounds__(256, 2) k_assemble_v5(const AsmArgs p, int PG, int tiles_per_cta) {
-  extern __shared__ __align__(16) double sm[];
-  const int N = p.N, S = p.S, TJ = p.TJ, NK = p.NK;
-  const int N3 = 3 * N, D = p.D, D3 = 3 * p.D;
-  const int tid = threadIdx.x, nt = blockDim.x;
-  const int warp = tid >> 5, lane = tid & 31, nw = nt >> 5;
-  const int i = p.i0 + blockIdx.y;
-
-  double* gI = sm;                        // 3D   compressed pair vectors of the row point, as stored: g[d][0..2]
-  double* xI = gI + D3;                   // D    descriptor of the row point
-  double* gJ = xI + D;                    // TJ*3D
-  double* xJ = gJ + TJ * D3;              // TJ*D
-  double* uS = xJ + TJ * D;               // TJ*PG*N3
-  double* vS = uS + TJ * PG * N3;         // TJ*PG*N3   (rows of kept column atoms only)
-  double* DgS = vS + TJ * PG * N3;        // TJ*PG*3*N3 (rows a = P^-1 b of kept column atoms b only)
-  double* n2p = DgS + TJ * PG * 3 * N3;   // TJ*PG*N    per-u-row sums of squared deltas (each pair twice)
-  double* cc = n2p + TJ * PG * N;         // TJ*PG*2
-  int* klist = reinterpret_cast<int*>(cc + TJ * PG * 2);  // TJ*N: the kept column atoms of point t, compact
-  int* nk = klist + TJ * N;                                    // TJ: how many
-  unsigned char* sP = reinterpret_cast<unsigned char*>(nk + TJ);  // S*N
-  unsigned char* sPi = sP + S * N;                                     // S*N
-
-  for (int e = tid; e < D3; e += nt) gI[e] = p.R_d_desc[(int64_t)i * D3 + e];
-  for (int e = tid; e < D; e += nt) xI[e] = p.R_desc[(int64_t)i * D + e];
-  for (int idx = tid; idx < S * N; idx += nt) {
-    sP[idx] = (unsigned char)p.aperm[idx];
-    sPi[idx] = (unsigned char)p.apinv[idx];
-  }
-  const double sig = p.sig;
-  const double sig2 = sig * sig;
-  const double inv_div = 1.0 / (3.0 * sig2 * sig2);  // 1/mat52_base_div (train.py:179)
-
-  const int tile_begin = blockIdx.x * tiles_per_cta;
-  const int tile_end = min(tile_begin + tiles_per_cta, ceil_div_dev(p.nJ, TJ));
-  for (int tile = tile_begin; tile < tile_end; ++tile) {
-    const int jt0 = tile * TJ;
-    const int tj = min(TJ, p.nJ - jt0);
-    if (p.sym && jt0 + tj - 1 < i) continue;  // (sym: jpts is the identity) every column point of the tile is < i
-    __syncthreads();  // the previous tile's phase B has finished with Gj / the vectors
-    for (int t = 0; t < tj; ++t) {
-      const int j = p.jpts[jt0 + t];
-      for (int e = tid; e < D3; e += nt) gJ[t * D3 + e] = p.R_d_desc[(int64_t)j * D3 + e];
-      for (int e = tid; e < D; e += nt) xJ[t * D + e] = p.R_desc[(int64_t)j * D + e];
-    }
-    for (int tw = warp; tw < tj; tw += nw) {  // compact list of the kept column atoms of point tw (ballot over atoms)
-      int c = 0;
-      for (int b0 = 0; b0 < N; b0 += 32) {
-        const int b = b0 + lane;
-        bool kept = false;
-        if (b < N) {
-          const int64_t* dst = p.dest + (int64_t)(jt0 + tw) * N3 + 3 * b;
-          kept = dst[0] >= 0 || dst[1] >= 0 || dst[2] >= 0;
-        }
-        const unsigned m = __ballot_sync(0xffffffffu, kept);
-        if (kept) klist[tw * N + c + __popc(m & ((1u << lane) - 1u))] = b;
-        c += __popc(m);
-      }
-      if (lane == 0) nk[tw] = c;
-    }
-    __syncthreads();
-    // this thread's output items: (t, a, b) = column point, row atom, kept column atom
-    int it_t[ASM_NI], it_a[ASM_NI], it_b[ASM_NI];
-    double acc[ASM_NI][9];
-#pragma unroll
-    for (int q = 0; q < ASM_NI; ++q) {
-      const int it = (int)blockIdx.z * ASM_NI * nt + tid + q * nt;  // grid.z splits the sub-blocks of large molecules
-      bool ok = it < tj * N * NK;
-      const int t = ok ? fastdiv(it, p.mNNK) : 0;
-      if (p.sym && jt0 + t < i) ok = false;  // mirrored from block (j, i) instead
-      const int ak = ok ? it - t * N * NK : 0;
-      it_a[q] = fastdiv(ak, p.mNK);
-      const int k = ak - it_a[q] * NK;
-      if (k >= nk[t]) ok = false;
-      it_b[q] = ok ? klist[t * N + k] : 0;
-      it_t[q] = ok ? t : -1;
-#pragma unroll
-      for (int e = 0; e < 9; ++e) acc[q][e] = 0.0;
-    }
-
-    for (int p0 = 0; p0 < S; p0 += PG) {
-      const int pg = min(PG, S - p0);
-      // ---- phase A, type-major over the chunk's (column point, permutation) slots
-      const int n_slots = tj * pg;
-      const int nU = n_slots * N, nV = n_slots * NK, nD = 3 * nV;
-      for (int idx = tid; idx < nU + nV + nD; idx += nt) {
-        if (idx < nU) {
-          // u[a] = -sum_g G_i[a][g] delta[a][g],  delta[a][g] = x_i[a][g] - x_j[Pa][Pg]  (i frame)
-          const int sl = fastdiv(idx, p.mN);
-          const int a = idx - sl * N;
-          const int t = sl / pg, pl = sl - t * pg;
-          const unsigned char* P = sP + (p0 + pl) * N;
-          const double* xj = xJ + t * D;
-          const int pa = P[a];
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0, q2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            if (g == a) continue;
-            const int di = pidx(a, g), dj = pidx(pa, P[g]);
-            const double d = xI[di] - xj[dj];
-            q2 = fma(d, d, q2);
-            const double w = a > g ? d : -d;  // G_i[a][g] = sgn(a - g) g_i[d(a,g)]
-            const double* gi = gI + 3 * di;
-            s0 = fma(gi[0], w, s0);
-            s1 = fma(gi[1], w, s1);
-            s2 = fma(gi[2], w, s2);
-          }
-          const int slot = t * PG + pl;
-          double* u = uS + slot * N3 + 3 * a;
-          u[0] = -s0;
-          u[1] = -s1;
-          u[2] = -s2;
-          n2p[slot * N + a] = q2;
-        } else if (idx < nU + nV) {
-          // v[b] = -sum_g G_j[b][g] delta[P^-1 b][P^-1 g]  for the kept column atoms b
-          const int e = idx - nU;
-          const int sl = fastdiv(e, p.mNK);
-          const int k = e - sl * NK;
-          const int t = sl / pg, pl = sl - t * pg;
-          if (k >= nk[t]) continue;
-          const int b = klist[t * N + k];
-          const unsigned char* Pi = sPi + (p0 + pl) * N;
-          const double* xj = xJ + t * D;
-          const int pib = Pi[b];
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            if (g == b) continue;
-            const int dj = pidx(b, g), di = pidx(pib, Pi[g]);
-            const double d = xI[di] - xj[dj];
-            const double w = b > g ? d : -d;
-            const double* gj = gJ + t * D3 + 3 * dj;
-            s0 = fma(gj[0], w, s0);
-            s1 = fma(gj[1], w, s1);
-            s2 = fma(gj[2], w, s2);
-          }
-          double* v = vS + (t * PG + pl) * N3 + 3 * b;
-          v[0] = -s0;
-          v[1] = -s1;
-          v[2] = -s2;
-        } else {
-          // Dg[a][c][0..2] = sum_g G_i[a][g][c] G_j[Pa][Pg][0..2]  for a = P^-1 b, b a kept column atom
-          const int e = idx - nU - nV;
-          const int e3 = (int)__umulhi((unsigned)e, 0x55555556u), c = e - 3 * e3;
-          const int sl = fastdiv(e3, p.mNK);
-          const int k = e3 - sl * NK;
-          const int t = sl / pg, pl = sl - t * pg;
-          if (k >= nk[t]) continue;
-          const int b = klist[t * N + k];
-          const unsigned char* P = sP + (p0 + pl) * N;
-          const int a = sPi[(p0 + pl) * N + b];
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0;
-          for (int g = 0; g < N; ++g) {
-            if (g == a) continue;
-            const int pg = P[g];
-            const int di = pidx(a, g), dj = pidx(b, pg);  // b = P a
-            const double gic = gI[3 * di + c];
-            const double x = ((a > g) == (b > pg)) ? gic : -gic;  // sgn(a - g) sgn(Pa - Pg)
-            const double* y = gJ + t * D3 + 3 * dj;
-            s0 = fma(x, y[0], s0);
-            s1 = fma(x, y[1], s1);
-            s2 = fma(x, y[2], s2);
-          }
-          double* dg = DgS + (t * PG + pl) * 3 * N3 + (a * 3 + c) * 3;
-          dg[0] = s0;
-          dg[1] = s1;
-          dg[2] = s2;
-        }
-      }
-      __syncthreads();
-      // ---- Matern factors of the chunk (fixed-order sum of the row partials: bit-reproducible K)
-      if (tid < n_slots) {
-        const int t = tid / pg, pl = tid - t * pg;
-        const int slot = t * PG + pl;
-        double n2 = 0.0;
-        for (int a = 0; a < N; ++a) n2 += n2p[slot * N + a];
-        const double nrm = sqrt(5.0) * sqrt(0.5 * n2);  // every pair twice; train.py:201
-        const double base = exp(-nrm / sig) * inv_div * 5.0;          // train.py:202
-        cc[slot * 2 + 0] = base * 5.0;                                 // c1 (train.py:211)
-        cc[slot * 2 + 1] = (sig2 + sig * nrm) * base;                  // c2 (train.py:219)
-      }
-      __syncthreads();
-      // ---- phase B: acc[a][b] += c1 u[a] (x) v[b] - c2 T[a][b] for the permutations of the chunk
-      for (int pl = 0; pl < pg; ++pl) {
-        const unsigned char* P = sP + (p0 + pl) * N;
-        const unsigned char* Pi = sPi + (p0 + pl) * N;
-#pragma unroll
-        for (int q = 0; q < ASM_NI; ++q) {
-          const int t = it_t[q];
-          if (t < 0) continue;
-          const int slot = t * PG + pl;
-          const int a = it_a[q], b = it_b[q];
-          const double c1 = cc[slot * 2 + 0], c2 = cc[slot * 2 + 1];
-          const double* ua = uS + slot * N3 + 3 * a;
-          const double* vb = vS + slot * N3 + 3 * b;
-          const int pa = P[a];
-          if (b != pa) {
-            const int pib = Pi[b];
-            const double* gi = gI + 3 * pidx(a, pib);
-            const double* gj = gJ + t * D3 + 3 * pidx(pa, b);
-            const double sg = ((a > pib) == (pa > b)) ? c2 : -c2;  // sgn(a - P^-1 b) sgn(Pa - b) c2
-            double t0[3], t1[3];  // T[a][b] = -G_i[a][P^-1 b] (x) G_j[Pa][b]  ->  -c2 T = +c2 G_i (x) G_j
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              t0[c] = sg * gi[c];
-              t1[c] = gj[c];
-            }
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              const double cu = c1 * ua[c];
-#pragma unroll
-              for (int c2i = 0; c2i < 3; ++c2i)
-                acc[q][c * 3 + c2i] = fma(t0[c], t1[c2i], fma(cu, vb[c2i], acc[q][c * 3 + c2i]));
-            }
-          } else {
-            const double* dg = DgS + slot * 3 * N3 + 9 * a;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              const double cu = c1 * ua[c];
-#pragma unroll
-              for (int c2i = 0; c2i < 3; ++c2i)
-                acc[q][c * 3 + c2i] = fma(-c2, dg[c * 3 + c2i], fma(cu, vb[c2i], acc[q][c * 3 + c2i]));
-            }
-          }
-        }
-      }
-      if (p0 + PG < S) __syncthreads();  // the next chunk overwrites the vectors
-    }
-
-    // ---- single store of the finished 3x3 sub-blocks (+ the mirrored block in symmetric mode)
-#pragma unroll
-    for (int q = 0; q < ASM_NI; ++q) {
-      const int t = it_t[q];
-      if (t < 0) continue;
-      const int a = it_a[q], b = it_b[q];
-      const int64_t* dst = p.dest + (int64_t)(jt0 + t) * N3 + 3 * b;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        double* Krow = p.K + ((int64_t)(i - p.i0) * N3 + 3 * a + c) * p.ldk;
-#pragma unroll
-        for (int c2i = 0; c2i < 3; ++c2i) {
-          const int64_t col = dst[c2i];
-          if (col >= 0) Krow[col] = p.scale * acc[q][c * 3 + c2i];
-        }
-      }
-      if (p.sym && jt0 + t > i) {  // (sym implies i0 == 0)
-        const int j = jt0 + t;
-#pragma unroll
-        for (int c2i = 0; c2i < 3; ++c2i) {
-          double* Krow = p.K + ((int64_t)j * N3 + 3 * b + c2i) * p.ldk + (int64_t)i * N3 + 3 * a;
-#pragma unroll
-          for (int c = 0; c < 3; ++c) Krow[c] = p.scale * acc[q][c * 3 + c2i];
-        }
-      }
-    }
+    for (int q = 0; q < ASM_NI; ++q)
+      if (it_t[q] >= 0) store_subblock<true>(p, acc[q], i, jt0 + it_t[q], it_a[q], it_b[q]);
   }
 }
 
@@ -892,9 +690,6 @@ __global__ void __launch_bounds__(256, 2)
   double* cc = DgS + (int64_t)S * 3 * N3;    // S*2
   double* Dl = dl_in_smem ? sm : cc + 2 * S;  // NN
 
-  const double sig = p.sig;
-  const double sig2 = sig * sig;
-  const double inv_div = 1.0 / (3.0 * sig2 * sig2);
 
   const int64_t w0 = n_work * (int64_t)blockIdx.x / gridDim.x;
   const int64_t w1 = n_work * ((int64_t)blockIdx.x + 1) / gridDim.x;
@@ -905,10 +700,11 @@ __global__ void __launch_bounds__(256, 2)
     const int j = p.jpts[jt];
     __syncthreads();  // the previous block's accumulation passes have finished reading the slab
     if (i != cur_i) {
-      load_pair_tables(p.R_d_desc + (int64_t)i * p.D * 3, p.R_desc + (int64_t)i * p.D, N, Gi, Xi, warp, lane, nw);
+      load_pair_tables(p.R_d_desc + (int64_t)i * p.D * 3, p.R_desc + (int64_t)i * p.D, N, N3, N, Gi, Xi, warp, lane,
+                       nw);
       cur_i = i;
     }
-    load_pair_tables(p.R_d_desc + (int64_t)j * p.D * 3, p.R_desc + (int64_t)j * p.D, N, Gj, Xj, warp, lane, nw);
+    load_pair_tables(p.R_d_desc + (int64_t)j * p.D * 3, p.R_desc + (int64_t)j * p.D, N, N3, N, Gj, Xj, warp, lane, nw);
     __syncthreads();
 
     // ---- phase A: per-permutation vectors (S1 + S2 of k_assemble), kept for all permutations
@@ -930,61 +726,11 @@ __global__ void __launch_bounds__(256, 2)
       if (tid == nt - 1) {
         double n2 = 0.0;
         for (int w8 = 0; w8 < nw; ++w8) n2 += n2p[w8];
-        const double nrm = sqrt(5.0) * sqrt(0.5 * n2);
-        const double base = exp(-nrm / sig) * inv_div * 5.0;
-        cc[pp * 2 + 0] = base * 5.0;
-        cc[pp * 2 + 1] = (sig2 + sig * nrm) * base;
+        matern_factors(n2, p.sig, cc + pp * 2);
       }
-      double* u = uS + (int64_t)pp * N3;
-      double* v = vS + (int64_t)pp * N3;
-      double* Dg = DgS + (int64_t)pp * 3 * N3;
-      for (int r = tid; r < 5 * N; r += nt) {
-        if (r < N) {
-          const int a = r, pa = P[a];
-          const double* gi = Gi + a * N3;
-          const double* dl = Dl + pa * N;
-          double s0 = 0.0, s1 = 0.0, s2b = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double d = dl[P[g]];
-            s0 = fma(gi[g * 3 + 0], d, s0);
-            s1 = fma(gi[g * 3 + 1], d, s1);
-            s2b = fma(gi[g * 3 + 2], d, s2b);
-          }
-          u[3 * a + 0] = -s0;
-          u[3 * a + 1] = -s1;
-          u[3 * a + 2] = -s2b;
-        } else if (r < 2 * N) {
-          const int b = r - N;
-          const double* gj = Gj + b * N3;
-          const double* dl = Dl + b * N;
-          double s0 = 0.0, s1 = 0.0, s2b = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double d = dl[g];
-            s0 = fma(gj[g * 3 + 0], d, s0);
-            s1 = fma(gj[g * 3 + 1], d, s1);
-            s2b = fma(gj[g * 3 + 2], d, s2b);
-          }
-          v[3 * b + 0] = -s0;
-          v[3 * b + 1] = -s1;
-          v[3 * b + 2] = -s2b;
-        } else {
-          const int ac = r - 2 * N;
-          const int a = (int)__umulhi((unsigned)ac, 0x55555556u), c = ac - 3 * a;
-          const double* gi = Gi + a * N3 + c;
-          const double* gj = Gj + P[a] * N3;
-          double s0 = 0.0, s1 = 0.0, s2b = 0.0;
-          for (int g = 0; g < N; ++g) {
-            const double x = gi[g * 3];
-            const double* y = gj + P[g] * 3;
-            s0 = fma(x, y[0], s0);
-            s1 = fma(x, y[1], s1);
-            s2b = fma(x, y[2], s2b);
-          }
-          Dg[ac * 3 + 0] = s0;
-          Dg[ac * 3 + 1] = s1;
-          Dg[ac * 3 + 2] = s2b;
-        }
-      }
+      for (int r = tid; r < 5 * N; r += nt)
+        staged_row<false>(r, N, Gi, Gj, Dl, P, nullptr, uS + (int64_t)pp * N3, vS + (int64_t)pp * N3,
+                          DgS + (int64_t)pp * 3 * N3);
       __syncthreads();  // Dl and n2p are rewritten by the next permutation
     }
 
@@ -1018,52 +764,16 @@ __global__ void __launch_bounds__(256, 2)
         for (int q = 0; q < ASM_NI; ++q) {
           const int a = it_a[q], b = it_b[q];
           if (a < 0) continue;
-          const double* ua = u + 3 * a;
-          const double* vb = v + 3 * b;
           const int pa = P[a];
-          if (b != pa) {
-            const double* gi = Gi + (a * N + Pi[b]) * 3;
-            const double* gj = Gj + (pa * N + b) * 3;
-            double t0[3], t1[3];
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              t0[c] = c2 * gi[c];
-              t1[c] = gj[c];
-            }
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              const double cu = c1 * ua[c];
-#pragma unroll
-              for (int c2i = 0; c2i < 3; ++c2i)
-                acc[q][c * 3 + c2i] = fma(t0[c], t1[c2i], fma(cu, vb[c2i], acc[q][c * 3 + c2i]));
-            }
-          } else {
-            const double* dg = Dg + 9 * a;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              const double cu = c1 * ua[c];
-#pragma unroll
-              for (int c2i = 0; c2i < 3; ++c2i)
-                acc[q][c * 3 + c2i] = fma(-c2, dg[c * 3 + c2i], fma(cu, vb[c2i], acc[q][c * 3 + c2i]));
-            }
-          }
+          if (b != pa)
+            acc_outer(acc[q], c1, u + 3 * a, v + 3 * b, c2, Gi + (a * N + Pi[b]) * 3, Gj + (pa * N + b) * 3);
+          else
+            acc_diag(acc[q], c1, c2, u + 3 * a, v + 3 * b, Dg + 9 * a);
         }
       }
 #pragma unroll
-      for (int q = 0; q < ASM_NI; ++q) {
-        const int a = it_a[q], b = it_b[q];
-        if (a < 0) continue;
-        const int64_t* dst = p.dest + (int64_t)jt * N3 + 3 * b;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          double* Krow = p.K + ((int64_t)(i - p.i0) * N3 + 3 * a + c) * p.ldk;
-#pragma unroll
-          for (int c2i = 0; c2i < 3; ++c2i) {
-            const int64_t col = dst[c2i];
-            if (col >= 0) Krow[col] = p.scale * acc[q][c * 3 + c2i];
-          }
-        }
-      }
+      for (int q = 0; q < ASM_NI; ++q)
+        if (it_a[q] >= 0) store_subblock<false>(p, acc[q], i, jt, it_a[q], it_b[q]);
     }
   }
 }
@@ -1199,22 +909,18 @@ __global__ void __launch_bounds__(1024) k_assemble_ecstr_rows(const double* __re
 
 // bound on the slabs of k_assemble_large, one per persistent CTA (asm_plan)
 constexpr size_t ASM_SLAB_BYTES_MAX = (size_t)2 << 30;
-constexpr int ASM_TILES_PER_CTA = 4;  // column tiles walked by one CTA of k_assemble_v4 / k_assemble_v5
+constexpr int ASM_TILES_PER_CTA = 4;  // column tiles walked by one CTA of k_assemble_tile
 
 static size_t asm_large_slab_doubles(int N, int S) {
   const size_t N3 = 3 * (size_t)N, NN = (size_t)N * N;
   return 2 * (NN * 3 + NN) + (size_t)S * (2 * N3 + 3 * N3 + 2) + NN;
 }
 
-static size_t asm_v4_smem_bytes(int N, int S, int TJ, int PG) {
-  const size_t N3 = 3 * (size_t)N, GS = N3 | 1, XS = (size_t)N | 1;
-  const size_t dbl = (size_t)N * (GS + XS) * (1 + TJ) + (size_t)TJ * PG * (2 * N3 + 3 * N3 + N + 2);
-  return dbl * 8 + ((size_t)TJ * N + TJ) * 4 + 2 * (size_t)S * N + 16;
-}
-
-static size_t asm_v5_smem_bytes(int N, int S, int TJ, int PG) {
-  const size_t N3 = 3 * (size_t)N, D = (size_t)N * (N - 1) / 2;
-  const size_t dbl = 4 * D * (1 + TJ) + (size_t)TJ * PG * (2 * N3 + 3 * N3 + N + 2);
+// k_assemble_tile: the pair tables of the row point and TJ column points (`tables` doubles each: Pairs::doubles), the
+// vectors of a chunk, the kept-atom lists and the byte permutation tables
+static size_t asm_tile_smem_bytes(size_t tables, int N, int S, int TJ, int PG) {
+  const size_t N3 = 3 * (size_t)N;
+  const size_t dbl = tables * (1 + TJ) + (size_t)TJ * PG * (2 * N3 + 3 * N3 + N + 2);
   return dbl * 8 + ((size_t)TJ * N + TJ) * 4 + 2 * (size_t)S * N + 16;
 }
 
@@ -1227,10 +933,11 @@ static size_t asm_smem_bytes(int N, int S, int TJ) {
 // Test and tuning hooks of the force-force assembly (sgdml_b200_set_assemble_variant).
 struct AsmHooks {
   bool force_large = false;  // variant 1: k_assemble_large for every size
-  int kernel = 0;            // 0: by size; 2, 4, 5: k_assemble, k_assemble_v4, k_assemble_v5 where it fits
+  int kernel = 0;            // 0: by size; 2, 4, 5: k_assemble, v4, v5 (see AsmKernel) where it fits
   int max_rowpts = 65535;    // row points per launch of the grid.y kernels: the grid.y limit (1000 + r lowers it)
 };
 
+// v4, v5: k_assemble_tile on ExpandedPairs, on CompressedPairs
 enum AsmKernel { ASM_K = 0, ASM_V4 = 1, ASM_V5 = 2, ASM_LARGE = 3 };
 
 struct AsmPlan {
@@ -1251,8 +958,8 @@ struct AsmPlan {
 // keeps two CTAs on an SM, 220 KB one.
 //
 //   k_assemble_large  hooks.force_large; else when k_assemble's tables exceed 220 KB at TJ = 1 and v5 does not run
-//   k_assemble_v5     hooks.kernel 5, or 0 where k_assemble_large would run; N <= 255, 220 KB at PG >= 4 or PG = S
-//   k_assemble_v4     hooks.kernel 0 or 4; N <= 255, 220 KB
+//   v5                hooks.kernel 5, or 0 where k_assemble_large would run; N <= 255, 220 KB at PG >= 4 or PG = S
+//   v4                hooks.kernel 0 or 4; N <= 255, 220 KB
 //   k_assemble        otherwise (hooks.kernel 2; 4 or 5 where theirs do not fit)
 //
 // TJ is 1 for k_assemble_large and v5 (grid.z splits v5's N NK sub-blocks, 1024 per CTA); v4 and k_assemble take the
@@ -1273,14 +980,15 @@ static AsmPlan asm_plan(int N, int S, int NK, int nJ, int n_rowpts, bool square,
         break;
       }
     const bool small_fits = TJ > 0 || asm_smem_bytes(N, S, 1) <= 220 * KB;
+    const size_t tab4 = ExpandedPairs::doubles(N), tab5 = CompressedPairs::doubles(N);
     int PG5 = std::min(S, 16);
-    while (PG5 > 1 && asm_v5_smem_bytes(N, S, 1, PG5) > 220 * KB) --PG5;
-    const bool fits5 = N <= 255 && asm_v5_smem_bytes(N, S, 1, PG5) <= 220 * KB && (PG5 >= 4 || PG5 == S);
+    while (PG5 > 1 && asm_tile_smem_bytes(tab5, N, S, 1, PG5) > 220 * KB) --PG5;
+    const bool fits5 = N <= 255 && asm_tile_smem_bytes(tab5, N, S, 1, PG5) <= 220 * KB && (PG5 >= 4 || PG5 == S);
     if (fits5 && (hooks.kernel == 5 || (hooks.kernel == 0 && !small_fits))) {
       p.kernel = ASM_V5;
       p.PG = PG5;
       p.n_chunks = z_chunks;
-      p.smem = asm_v5_smem_bytes(N, S, 1, PG5);
+      p.smem = asm_tile_smem_bytes(tab5, N, S, 1, PG5);
       p.grid_x = ceil_div(nJ, ASM_TILES_PER_CTA);
       return p;
     }
@@ -1291,13 +999,13 @@ static AsmPlan asm_plan(int N, int S, int NK, int nJ, int n_rowpts, bool square,
       }
       p.TJ = TJ = std::min(TJ, nJ);
       int PG4 = std::min(S, 16);
-      while (PG4 > 1 && (asm_v4_smem_bytes(N, S, TJ, PG4) > 220 * KB || TJ * PG4 > 256)) --PG4;
-      if (PG4 == S && asm_v4_smem_bytes(N, S, TJ, PG4) > 110 * KB) {  // chunks of >= 8 for two CTAs per SM
+      while (PG4 > 1 && (asm_tile_smem_bytes(tab4, N, S, TJ, PG4) > 220 * KB || TJ * PG4 > 256)) --PG4;
+      if (PG4 == S && asm_tile_smem_bytes(tab4, N, S, TJ, PG4) > 110 * KB) {  // chunks of >= 8 for two CTAs per SM
         int q = PG4;
-        while (q > 8 && asm_v4_smem_bytes(N, S, TJ, q) > 110 * KB) --q;
-        if (asm_v4_smem_bytes(N, S, TJ, q) <= 110 * KB) PG4 = q;
+        while (q > 8 && asm_tile_smem_bytes(tab4, N, S, TJ, q) > 110 * KB) --q;
+        if (asm_tile_smem_bytes(tab4, N, S, TJ, q) <= 110 * KB) PG4 = q;
       }
-      const size_t smem4 = asm_v4_smem_bytes(N, S, TJ, PG4);
+      const size_t smem4 = asm_tile_smem_bytes(tab4, N, S, TJ, PG4);
       // chosen by timing the variants (tools/asm_variants.py) at BASELINE config 2 (full matrix) and on the Ac-Ala3
       // shape (S = 243, random column subsets): v4 was the fastest on both
       if (N <= 255 && smem4 <= 220 * KB && TJ * PG4 <= 256 && (hooks.kernel == 0 || hooks.kernel == 4)) {
@@ -1546,7 +1254,8 @@ extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_
 
   // ---- launch: rows on grid.y, which is limited to 65535, so longer row ranges (the iterative solver assembles K_nm
   //      over ALL training points of a rank) run as several launches, each with its own first row point and K row offset
-  const void* const kernel_fn[] = {(const void*)k_assemble, (const void*)k_assemble_v4, (const void*)k_assemble_v5,
+  const void* const kernel_fn[] = {(const void*)k_assemble, (const void*)k_assemble_tile<ExpandedPairs>,
+                                   (const void*)k_assemble_tile<CompressedPairs>,
                                    (const void*)k_assemble_large};  // indexed by AsmKernel
   if (plan.smem > 0)
     SG_CUDA(cudaFuncSetAttribute(kernel_fn[plan.kernel], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
@@ -1560,8 +1269,12 @@ extern "C" int sgdml_b200_assemble_rows(const double* R_desc, const double* R_d_
       const dim3 grid((unsigned)plan.grid_x, (unsigned)nr, (unsigned)plan.n_chunks);
       switch (plan.kernel) {
         case ASM_K: k_assemble<<<grid, 256, plan.smem, s>>>(ac); break;
-        case ASM_V4: k_assemble_v4<<<grid, 256, plan.smem, s>>>(ac, plan.PG, ASM_TILES_PER_CTA); break;
-        case ASM_V5: k_assemble_v5<<<grid, 256, plan.smem, s>>>(ac, plan.PG, ASM_TILES_PER_CTA); break;
+        case ASM_V4:
+          k_assemble_tile<ExpandedPairs><<<grid, 256, plan.smem, s>>>(ac, plan.PG, ASM_TILES_PER_CTA);
+          break;
+        case ASM_V5:
+          k_assemble_tile<CompressedPairs><<<grid, 256, plan.smem, s>>>(ac, plan.PG, ASM_TILES_PER_CTA);
+          break;
         case ASM_LARGE:
           k_assemble_large<<<plan.grid_x, 256, plan.smem, s>>>(ac, d_slabs, (int64_t)plan.slab, (int64_t)nr * nJ,
                                                                 plan.dl_in_smem);

@@ -164,14 +164,16 @@ int sgdml_b200_predict_hvp(sgdml_b200_model* model, const double* R, const doubl
  * Argument errors are reported before anything is queued, and a rejected call changes nothing.
  * Handle kinds: the call that makes a handle fixes its kind.  sgdml_b200_md_create, and sgdml_b200_pimd_create with
  * n_beads = 1, make plain handles; sgdml_b200_pimd_create with n_beads > 1 makes ring-polymer handles,
- * sgdml_b200_npt_create NPT handles and sgdml_b200_metad_create metadynamics handles.  An entry point called with a
- * handle of a kind it does not take (no x below) returns an argument error:
- *   entry point                                                              plain  ring  NPT  metadynamics
- *   sgdml_b200_md_set_state, _md_get_state, _md_destroy                        x     x     x        x
+ * sgdml_b200_npt_create NPT handles, sgdml_b200_metad_create metadynamics handles and sgdml_b200_umbrella_create
+ * umbrella handles.  An entry point called with a handle of a kind it does not take (no x below) returns an argument
+ * error:
+ *   entry point                                                              plain  ring  NPT  metadynamics  umbrella
+ *   sgdml_b200_md_set_state, _md_get_state, _md_destroy                        x     x     x        x            x
  *   sgdml_b200_md_run, _remd_run, _neb_fire, _dimer_fire                       x
  *   sgdml_b200_pimd_run, _relax_fire, _relax_lbfgs                             x     x
  *   sgdml_b200_npt_run, _npt_set_cells, _npt_get_cells                                     x
- *   sgdml_b200_metad_run, _metad_get_hills, _metad_set_hills, _metad_get_bias                       x */
+ *   sgdml_b200_metad_run, _metad_get_hills, _metad_set_hills, _metad_get_bias                       x
+ *   sgdml_b200_umbrella_run, _umbrella_set_windows, _umbrella_get_bias                                           x */
 typedef struct sgdml_b200_md sgdml_b200_md;
 /* inv_mass (N,) HOST doubles, each finite and > 0; n_rep >= 1. */
 int sgdml_b200_md_create(sgdml_b200_md** out, sgdml_b200_model* model, int64_t n_rep, const double* inv_mass);
@@ -314,6 +316,56 @@ int sgdml_b200_metad_set_hills(sgdml_b200_md* md, const int64_t* n_hills, const 
 /* cv (n_rep, n_cv), V_bias (n_rep) and F_bias (n_rep, 3N): the CVs, bias energy and bias force of the state; any may be
  * NULL.  Needs a state. */
 int sgdml_b200_metad_get_bias(sgdml_b200_md* md, double* cv, double* V_bias, double* F_bias, void* stream);
+
+/* ---------------------------------------------------------------- umbrella sampling on the device
+ * Extension: umbrella sampling with Hamiltonian replica exchange between neighbouring windows (REUS; Sugita, Kitao &
+ * Okamoto, J. Chem. Phys. 113, 6042 (2000)) on 1 to 4 CVs, and its reweighting by MBAR (Shirts & Chodera, J. Chem.
+ * Phys. 129, 124105 (2008)).  An umbrella handle is an sgdml_b200_md handle of n_rep = n_ladders n_windows replicas:
+ * slot l n_windows + k sits in window k of ladder l for the whole run, each integrated by sgdml_b200_md_run's BAOAB
+ * step at one temperature with F = F_model + F_bias.  The CVs are those of sgdml_b200_metad_create.  Window k restrains
+ * CV j harmonically: b_k(s) = sum_j (0.5 kappa_kj e_j) e_j with e_j = s_j - c_kj (a dihedral's e_j wrapped into
+ * [-pi, pi)), summed in increasing j from 0.0 and rounded as written (csrc/md.cuh).
+ * Exchanges: the schedule, pairing, Philox draw and walker labels of sgdml_b200_remd_run.  With configuration a in slot
+ * k and b in slot k + 1, d = -(beta ((b_k(s_b) + b_k+1(s_a)) - (b_k(s_a) + b_k+1(s_b)))), beta = 1 / kT; accepted iff
+ * d >= 0 or u < exp(d).  An accepted swap moves R, the model's F and E_pot, the CVs and the labels, re-evaluates the
+ * bias of both slots in their new windows, and keeps each configuration's full-step velocity w: the handle holds
+ * v = w - h (F s), and stores v' = w - h (F_new s) against the new total force.  The last state of a run is exchanged
+ * before the run returns and the first is not.  sgdml_b200_md_set_state evaluates the model and the restraints and
+ * resets the labels to the identity; sgdml_b200_md_get_state's F and E_pot stay the model's.  Which entry points take
+ * an umbrella handle: the handle kinds at sgdml_b200_md_create.  Streams, host/device outputs, SGDML_B200_GRAPH=0 and
+ * the workspace are those of sgdml_b200_md_run; argument errors are reported before anything is queued, and a rejected
+ * call changes nothing. */
+/* n_ladders, n_windows >= 1, n_ladders n_windows <= INT32_MAX; n_cv, cv_type, cv_atoms as sgdml_b200_metad_create;
+ * centers, kappas (n_windows, n_cv) HOST doubles: finite, kappa >= 0 (energy / L^2 or energy / rad^2), a dihedral's
+ * centre in (-pi, pi]; inv_mass as sgdml_b200_md_create. */
+int sgdml_b200_umbrella_create(sgdml_b200_md** out, sgdml_b200_model* model, int64_t n_ladders, int64_t n_windows,
+                               const double* inv_mass, int64_t n_cv, const int* cv_type, const int64_t* cv_atoms,
+                               const double* centers, const double* kappas);
+/* Replaces every window (checked as at creation) and re-evaluates the restraints of the state when there is one. */
+int sgdml_b200_umbrella_set_windows(sgdml_b200_md* md, const double* centers, const double* kappas, void* stream);
+/* n_steps, dt, gamma, kT, seed and stride as sgdml_b200_md_run; exchange_every >= 0 (0: no exchanges; > 0 needs
+ * kT > 0 and n_windows >= 2).  Outputs, each host, device or NULL: R, V, E_pot (the model's), E_kin frames as
+ * sgdml_b200_md_run; cv_frames (n_frames, n_rep, n_cv), bias_frames (n_frames, n_rep) and walker_frames (n_frames,
+ * n_rep) int32 of the frame's state after its exchange; walkers_out (n_rep) int32; n_accepted, n_attempted
+ * (n_ladders, n_windows - 1) int64, this run's swaps of each neighbour pair.  Needs a state. */
+int sgdml_b200_umbrella_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, uint64_t seed,
+                            int64_t exchange_every, int64_t stride, double* R_frames, double* V_frames,
+                            double* E_pot_frames, double* E_kin_frames, double* cv_frames, double* bias_frames,
+                            int* walker_frames, int* walkers_out, int64_t* n_accepted, int64_t* n_attempted,
+                            void* stream);
+/* cv (n_rep, n_cv), V_bias (n_rep) and F_bias (n_rep, 3N) of the state under its windows; any may be NULL. */
+int sgdml_b200_umbrella_get_bias(sgdml_b200_md* md, double* cv, double* V_bias, double* F_bias, void* stream);
+/* MBAR over n_samples >= 1 samples (n_samples, n_cv) of CVs (host or device), pooled window after window with
+ * n_per_window (n_windows) HOST int64 >= 0 of them, summing to n_samples; the windows (centers, kappas) and CVs as
+ * sgdml_b200_umbrella_create, beta = 1 / kT > 0; every sample finite.  Iterates the self-consistent equations from
+ * f = 0 until max_k |df_k| < tol (>= 0) or max_iter (>= 1) iterations, f_0 held at 0 (csrc/md.cuh has the reduction
+ * order: the result is the same bits on every call).  Outputs, host or device: f (n_windows) the reduced free energies
+ * (f_k = beta F_k), log_w (n_samples) the log unbiased weights, normalised so that sum_n exp(log_w_n) = 1; n_iter (1)
+ * int64 the iterations run and resid (1) the last max_k |df_k| (HOST or NULL). */
+int sgdml_b200_umbrella_mbar(int64_t n_windows, int64_t n_cv, const int* cv_type, const double* centers,
+                             const double* kappas, double beta, int64_t n_samples, const double* samples,
+                             const int64_t* n_per_window, double tol, int64_t max_iter, double* f, double* log_w,
+                             int64_t* n_iter, double* resid, void* stream);
 
 /* ---------------------------------------------------------------- path-integral molecular dynamics on the device
  * Extension: ring polymers of P beads (1 <= P <= 64), thermostatted mode by mode with PILE-L (Ceriotti, Parrinello,

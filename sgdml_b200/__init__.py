@@ -10,7 +10,7 @@ CPU fallback.
 __version__ = '0.1.0'
 
 from .md import (GDMLNEB, GDMLDimer, GDMLDynamics, GDMLMetadynamics, GDMLNPTDynamics,  # noqa: F401
-                 GDMLPathIntegralDynamics, GDMLRelaxation, GDMLReplicaExchange)
+                 GDMLPathIntegralDynamics, GDMLRelaxation, GDMLReplicaExchange, GDMLUmbrellaSampling)
 from .perm import find_perms  # noqa: F401
 from .predict import GDMLPredict  # noqa: F401
 from .train import GDMLTrain  # noqa: F401

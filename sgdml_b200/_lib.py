@@ -72,6 +72,20 @@ SIGNATURES = {
     'sgdml_b200_metad_get_hills': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_metad_set_hills': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_metad_get_bias': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_umbrella_create': (
+        C.c_int, [C.POINTER(c_void_p), c_void_p, i64, i64, c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_umbrella_set_windows': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_umbrella_run': (
+        C.c_int,
+        [c_void_p, i64, C.c_double, C.c_double, C.c_double, C.c_uint64, i64, i64, c_void_p, c_void_p, c_void_p,
+         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
+    'sgdml_b200_umbrella_get_bias': (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_umbrella_mbar': (
+        C.c_int,
+        [i64, i64, c_void_p, c_void_p, c_void_p, C.c_double, i64, c_void_p, c_void_p, C.c_double, i64, c_void_p,
+         c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
     'sgdml_b200_pimd_create': (C.c_int, [C.POINTER(c_void_p), c_void_p, i64, i64, c_void_p]),
     'sgdml_b200_pimd_run': (
         C.c_int,

@@ -1,7 +1,8 @@
-// Molecular dynamics, replica exchange, metadynamics, path-integral MD, geometry optimisation and saddle searches on the
-// device: the integrator, exchange, bias, optimiser and dimer kernels (contract in md.cuh), then the driver of
-// sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_metad_*, sgdml_b200_pimd_*, sgdml_b200_relax_*,
-// sgdml_b200_neb_fire and sgdml_b200_dimer_fire, which evaluates forces through the predictor interface of predict.cuh.
+// Molecular dynamics, replica exchange, metadynamics, umbrella sampling, path-integral MD, geometry optimisation and
+// saddle searches on the device: the integrator, exchange, bias, optimiser and dimer kernels (contract in md.cuh), then
+// the driver of sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_metad_*, sgdml_b200_umbrella_*
+// (but _mbar, in mbar.cu), sgdml_b200_pimd_*, sgdml_b200_relax_*, sgdml_b200_neb_fire and sgdml_b200_dimer_fire, which
+// evaluates forces through the predictor interface of predict.cuh.
 //
 // The BAOAB Langevin integrator step of sgdml_b200_md_run.
 //
@@ -886,6 +887,46 @@ __device__ void cv_eval(int type, const int* at, const double* r, double* sv, do
   }
 }
 
+// The CTA stages the CVs of the replica's positions r and their gradients in shared memory: thread j < n_cv
+// evaluates CV j, then a barrier
+__device__ __forceinline__ void stage_cvs(int n_cv, const int* type, const int (*atoms)[4], const double* r,
+                                          double* s_cv, double (*s_g)[4][3]) {
+  const int tid = threadIdx.x;
+  if (tid < n_cv) cv_eval(type[tid], atoms[tid], r, &s_cv[tid], s_g[tid]);
+  __syncthreads();
+}
+
+// The CTA's bias force of one replica from dV/ds (s_dv, written before the call by any thread) and the staged
+// gradients s_g: f = fm, then on the touched atoms f = fm + fb and fb_out = fb (md.cuh).  Starts with a barrier.
+__device__ __forceinline__ void bias_force(int n_cv, const int* type, const int (*atoms)[4], const double* s_dv,
+                                           const double (*s_g)[4][3], const double* fm, double* f, double* fb_out,
+                                           int dimi) {
+  const int tid = threadIdx.x;
+  // F = Fm everywhere, then the touched atoms: thread j 4 + p owns atom slot p of CV j if it is that atom's first
+  // appearance in (j, p) order
+  for (int i = tid; i < dimi; i += MD_THREADS) f[i] = fm[i];
+  __syncthreads();  // s_dv is complete, and every plain F is written
+  if (tid < 4 * n_cv) {  // CV type t holds t + 2 atoms
+    const int j0 = tid / 4, p0 = tid % 4;
+    const int at = atoms[j0][p0];
+    bool first = p0 < type[j0] + 2;
+    for (int j = 0; j <= j0 && first; ++j)
+      for (int p = 0; p < (j == j0 ? p0 : type[j] + 2); ++p)
+        if (atoms[j][p] == at) first = false;
+    if (first) {
+      double fb[3] = {0.0, 0.0, 0.0};
+      for (int j = j0; j < n_cv; ++j)
+        for (int p = 0; p < type[j] + 2; ++p)
+          if (atoms[j][p] == at)
+            for (int x = 0; x < 3; ++x) fb[x] = __dsub_rn(fb[x], __dmul_rn(s_dv[j], s_g[j][p][x]));
+      for (int x = 0; x < 3; ++x) {
+        f[3 * at + x] = __dadd_rn(fm[3 * at + x], fb[x]);
+        fb_out[3 * at + x] = fb[x];
+      }
+    }
+  }
+}
+
 __global__ void __launch_bounds__(MD_THREADS) k_metad_bias(const MetadParams* __restrict__ Q,
                                                           const MdParams* __restrict__ P,
                                                           const double* __restrict__ R, const double* __restrict__ Fm,
@@ -899,10 +940,8 @@ __global__ void __launch_bounds__(MD_THREADS) k_metad_bias(const MetadParams* __
   const int64_t rep = blockIdx.x, n_rep = gridDim.x, grp = rep / nw, w = rep % nw;
   const uint64_t c = step[rep];
   const uint64_t run_start = P->run_start;
-  const double* r = R + rep * dimi;
   const int tid = threadIdx.x;
-  if (tid < n_cv) cv_eval(q.type[tid], q.atoms[tid], r, &s_cv[tid], s_g[tid]);
-  __syncthreads();
+  stage_cvs(n_cv, q.type, q.atoms, R + rep * dimi, s_cv, s_g);
   const uint64_t pace = (uint64_t)q.pace;
   const int64_t n_g = q.count[grp] + (deposit ? (int64_t)nw * (int64_t)((c - 1) / pace - run_start / pace) : 0);
   const double* C = q.centers + grp * q.cap * n_cv;
@@ -940,31 +979,7 @@ __global__ void __launch_bounds__(MD_THREADS) k_metad_bias(const MetadParams* __
     const double d = block_sum(dv[j], red);
     if (tid == 0) s_dv[j] = d;
   }
-  // F = Fm everywhere, then the touched atoms: thread j 4 + p owns atom slot p of CV j if it is that atom's first
-  // appearance in (j, p) order
-  const double* fm = Fm + rep * dimi;
-  double* f = F + rep * dimi;
-  for (int i = tid; i < dimi; i += MD_THREADS) f[i] = fm[i];
-  __syncthreads();  // s_dv is complete, and every plain F is written
-  if (tid < 4 * n_cv) {  // CV type t holds t + 2 atoms
-    const int j0 = tid / 4, p0 = tid % 4;
-    const int at = q.atoms[j0][p0];
-    bool first = p0 < q.type[j0] + 2;
-    for (int j = 0; j <= j0 && first; ++j)
-      for (int p = 0; p < (j == j0 ? p0 : q.type[j] + 2); ++p)
-        if (q.atoms[j][p] == at) first = false;
-    if (first) {
-      double fb[3] = {0.0, 0.0, 0.0};
-      for (int j = j0; j < n_cv; ++j)
-        for (int p = 0; p < q.type[j] + 2; ++p)
-          if (q.atoms[j][p] == at)
-            for (int x = 0; x < 3; ++x) fb[x] = __dsub_rn(fb[x], __dmul_rn(s_dv[j], s_g[j][p][x]));
-      for (int x = 0; x < 3; ++x) {
-        f[3 * at + x] = __dadd_rn(fm[3 * at + x], fb[x]);
-        q.Fb[rep * dimi + 3 * at + x] = fb[x];
-      }
-    }
-  }
+  bias_force(n_cv, q.type, q.atoms, s_dv, s_g, Fm + rep * dimi, F + rep * dimi, q.Fb + rep * dimi, dimi);
   if (tid < n_cv) q.cv[rep * n_cv + tid] = s_cv[tid];
   if (tid == 0) q.Vb[rep] = V;
   if (!deposit) return;
@@ -989,6 +1004,142 @@ __global__ void __launch_bounds__(MD_THREADS) k_metad_bias(const MetadParams* __
 __global__ void k_metad_commit(int64_t* count, int64_t n_groups, int64_t add) {
   const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (g < n_groups) count[g] += add;
+}
+
+// ---------------------------------------------------------------------------------- umbrella sampling
+// The restraint, its bias force and the Hamiltonian exchange of sgdml_b200_umbrella_run (contract in md.cuh).
+
+struct UmbrellaSmem {
+  double cv[MD_MAX_CV], dv[MD_MAX_CV];
+  double g[MD_MAX_CV][4][3];
+};
+
+// The CTA evaluates the configuration in slot rep under window k: its CVs and gradients, b and u, F = Fm + Fb, and the
+// state's s, b and Fb.  Shared memory is free again only after a barrier.
+__device__ __forceinline__ void umbrella_slot(const UmbrellaParams& q, int64_t rep, int k, const double* R,
+                                              const double* Fm, double* F, int dimi, UmbrellaSmem& sm) {
+  const int n_cv = q.n_cv;
+  stage_cvs(n_cv, q.type, q.atoms, R + rep * dimi, sm.cv, sm.g);
+  if (threadIdx.x == 0)
+    q.Vb[rep] = umbrella_restraint(n_cv, q.type, sm.cv, q.win + k * n_cv, q.win + (q.n_windows + k) * n_cv, sm.dv);
+  bias_force(n_cv, q.type, q.atoms, sm.dv, sm.g, Fm + rep * dimi, F + rep * dimi, q.Fb + rep * dimi, dimi);
+  if ((int)threadIdx.x < n_cv) q.cv[rep * n_cv + threadIdx.x] = sm.cv[threadIdx.x];
+}
+
+__global__ void __launch_bounds__(MD_THREADS) k_umbrella_bias(const UmbrellaParams* __restrict__ Q,
+                                                             const double* __restrict__ R,
+                                                             const double* __restrict__ Fm, double* __restrict__ F,
+                                                             int dimi) {
+  __shared__ UmbrellaSmem sm;
+  const UmbrellaParams& q = *Q;
+  umbrella_slot(q, blockIdx.x, (int)(blockIdx.x % (unsigned)q.n_windows), R, Fm, F, dimi, sm);
+}
+
+// Thread t decides the pairs t, t + MD_THREADS, ... of its ladder and swaps their energies, CVs, walker labels and
+// counts; then, pair by pair, every thread carries its coordinates of the two configurations' full-step velocities,
+// swaps R and Fm, the CTA re-evaluates both slots, and the velocities are stored against the new forces.
+__global__ void __launch_bounds__(MD_THREADS) k_umbrella_exchange(const RemdParams* __restrict__ X,
+                                                                 const UmbrellaParams* __restrict__ Q,
+                                                                 const MdParams* __restrict__ P,
+                                                                 const double* __restrict__ s, double* __restrict__ R,
+                                                                 double* __restrict__ V, double* __restrict__ F,
+                                                                 double* __restrict__ Fm, double* __restrict__ E,
+                                                                 int* __restrict__ walker,
+                                                                 const uint64_t* __restrict__ step, int dimi) {
+  __shared__ int acc[MD_THREADS];
+  __shared__ UmbrellaSmem sm;
+  const RemdParams& x = *X;
+  const UmbrellaParams& q = *Q;
+  const int nw = x.n_temps, n_cv = q.n_cv;
+  const int64_t lad = blockIdx.x, n_rep = (int64_t)gridDim.x * nw, base = lad * nw;
+  const uint64_t c = step[base];
+  const uint64_t done = c - x.run_start;
+  const bool sample = done != 0 && x.stride > 0 && done % (uint64_t)x.stride == 0;
+  const bool exchange = x.every > 0 && done != 0 && c % (uint64_t)x.every == 0;
+  if (!exchange && !sample) return;
+  if (exchange) {
+    const double h = P->h;
+    const int par = (int)((c / (uint64_t)x.every) & 1);
+    const int n_pairs = (nw - par) / 2;  // k = 2 j + par for j < n_pairs
+    for (int j0 = 0; j0 < n_pairs; j0 += MD_THREADS) {
+      const int j = j0 + (int)threadIdx.x;
+      if (j < n_pairs) {
+        const int k = 2 * j + par;
+        const int64_t a = base + k, b = a + 1;
+        double* ca = q.cv + a * n_cv;
+        double* cb = q.cv + b * n_cv;
+        const double *c0 = q.win + k * n_cv, *c1 = c0 + n_cv;
+        const double *k0 = q.win + (nw + k) * n_cv, *k1 = k0 + n_cv;
+        const double od = __dadd_rn(umbrella_restraint(n_cv, q.type, ca, c0, k0, nullptr),
+                                    umbrella_restraint(n_cv, q.type, cb, c1, k1, nullptr));
+        const double nd = __dadd_rn(umbrella_restraint(n_cv, q.type, cb, c0, k0, nullptr),
+                                    umbrella_restraint(n_cv, q.type, ca, c1, k1, nullptr));
+        const double d = -__dmul_rn(q.beta, __dsub_rn(nd, od));
+        bool ok = d >= 0.0;
+        if (!ok) {
+          uint32_t ct[4] = {0x80000000u | (uint32_t)k, (uint32_t)lad, (uint32_t)c, (uint32_t)(c >> 32)};
+          philox4x32_10(ct, x.key[0], x.key[1]);
+          ok = uniform53(ct[0], ct[1]) < exp(d);
+        }
+        acc[threadIdx.x] = ok ? 1 : 0;
+        const int64_t pq = lad * (nw - 1) + k;
+        x.n_att[pq] += 1;
+        if (ok) {
+          x.n_acc[pq] += 1;
+          const double e = E[a];
+          E[a] = E[b];
+          E[b] = e;
+          const int w = walker[a];
+          walker[a] = walker[b];
+          walker[b] = w;
+          for (int i = 0; i < n_cv; ++i) {
+            const double t = ca[i];
+            ca[i] = cb[i];
+            cb[i] = t;
+          }
+        }
+      }
+      __syncthreads();  // the decisions are in acc
+      const int nj = min(MD_THREADS, n_pairs - j0);
+      for (int t = 0; t < nj; ++t) {
+        if (!acc[t]) continue;
+        const int k = 2 * (j0 + t) + par;
+        const int64_t a = base + k, o = a * dimi;
+        for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {  // V holds w until the new forces are known
+          const int64_t ia = o + i, ib = ia + dimi;
+          const double wa = __dadd_rn(V[ia], __dmul_rn(h, __dmul_rn(F[ia], s[i])));
+          const double wb = __dadd_rn(V[ib], __dmul_rn(h, __dmul_rn(F[ib], s[i])));
+          V[ia] = wb;
+          V[ib] = wa;
+          const double r = R[ia], m = Fm[ia];
+          R[ia] = R[ib];
+          R[ib] = r;
+          Fm[ia] = Fm[ib];
+          Fm[ib] = m;
+        }
+        __syncthreads();  // the swapped rows are complete
+        umbrella_slot(q, a, k, R, Fm, F, dimi, sm);
+        __syncthreads();  // sm is free again
+        umbrella_slot(q, a + 1, k + 1, R, Fm, F, dimi, sm);
+        __syncthreads();  // both slots' F are complete
+        for (int i = threadIdx.x; i < 2 * dimi; i += MD_THREADS) {
+          const int64_t ia = o + i;
+          V[ia] = __dsub_rn(V[ia], __dmul_rn(h, __dmul_rn(F[ia], s[i % dimi])));
+        }
+      }
+      __syncthreads();  // acc is free again, and the labels, CVs and biases are final
+    }
+  }
+  if (sample) {
+    const int64_t fr = (int64_t)(done / (uint64_t)x.stride) - 1;
+    for (int k = threadIdx.x; k < nw; k += MD_THREADS) {
+      const int64_t r = base + k, o = fr * n_rep + r;
+      if (x.W_f) x.W_f[o] = walker[r];
+      if (q.bias_f) q.bias_f[o] = q.Vb[r];
+      if (q.cv_f)
+        for (int j = 0; j < n_cv; ++j) q.cv_f[o * n_cv + j] = q.cv[r * n_cv + j];
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------------- dimer search
@@ -1226,6 +1377,21 @@ __global__ void k_dimer_report(const DimerState* __restrict__ ds, int64_t n_dime
 
 }  // namespace sgdml
 
+// md.cuh: the checks of a window table, shared with mbar.cu
+int sgdml::umbrella_windows_check(int64_t n_windows, int n_cv, const int* type, const double* centers,
+                                  const double* kappas) {
+  SG_ARG(centers != nullptr && kappas != nullptr);
+  SG_ARG(!is_device_ptr(centers) && !is_device_ptr(kappas));
+  for (int64_t i = 0; i < n_windows * n_cv; ++i) {
+    const double c = centers[i], k = kappas[i];
+    if (!std::isfinite(c)) return fail_arg("every window centre must be finite");
+    if (!(std::isfinite(k) && k >= 0.0)) return fail_arg("every force constant must be finite and >= 0");
+    if (type[i % n_cv] == CV_DIHEDRAL && !(c > -M_PI && c <= M_PI))
+      return fail_arg("a dihedral's window centre must lie in (-pi, pi]");
+  }
+  return 0;
+}
+
 // ============================================================== driver (sgdml_b200_md_*, _remd_run, _pimd_*, _relax_*)
 // The state of n_rep replicas stays in device memory between steps and between runs.  One step is the integrator
 // kernel, then the forces and energies of the new positions (force_eval_run, predict.cuh) written back into the
@@ -1246,9 +1412,12 @@ struct StepParams {
   NptParams npt;
   MetadParams metad;
   DimerParams dimer;
+  UmbrellaParams umbrella;
 };
 constexpr size_t STEP_PARAMS_BYTES = (sizeof(StepParams) + 255) & ~(size_t)255;  // where the tables start
-static_assert(STEP_PARAMS_BYTES == 768, "the dimer's parameters fit in the padding: the tables do not move");
+// The umbrella parameters took the block past 768 bytes, so the tables start at 1024.  Every kernel that reads a table
+// gets its address as an argument, and a captured graph is keyed on the block, so the move changes no step.
+static_assert(STEP_PARAMS_BYTES == 1024, "the tables start at 1024 bytes");
 
 // What a captured step bakes in besides the force evaluation: the integrator (MdKind), the replicas per group (the
 // grids of the NEB and exchange kernels) and the upload block (the tab and sigma kernel arguments point into it).
@@ -1260,7 +1429,7 @@ struct StepKey {
 
 // What a handle is, fixed at creation (sgdml_b200_pimd_create makes PLAIN handles with one bead, RING with more): it
 // decides which entry points take the handle (check_kind) and how its state's forces are evaluated.
-enum HandleKind { PLAIN, RING, NPT, METAD };
+enum HandleKind { PLAIN, RING, NPT, METAD, UMBRELLA };
 
 }  // namespace
 
@@ -1322,6 +1491,9 @@ struct sgdml_b200_md {
   int64_t* hcount = nullptr;   // (n_groups) committed hills per group
   std::vector<int64_t> hcount_host;  // the same, once the queued runs have finished
   int64_t n_groups = 0;
+  // umbrella sampling (sgdml_b200_umbrella_create): Fm, cv, Vb and Fb as on a metadynamics handle, the walker labels
+  // and swap counts as on a replica exchange, and the window table, whose address is in the mirror's UmbrellaParams
+  double* win = nullptr;       // (2, n_windows, n_cv) centres, then force constants
 
   // the block's parts in blk or hblk
   StepParams* params(char* b) const { return reinterpret_cast<StepParams*>(b); }
@@ -1346,6 +1518,7 @@ void md_free(sgdml_b200_md* md) {
   cached_free(md->dstate);
   cached_free(md->dbad);
   cached_free(md->hcount);
+  cached_free(md->win);
   cached_free(md->step);
   cached_free(md->blk);
   cached_free(md->rst);
@@ -1458,13 +1631,14 @@ class Outputs {
 // what one step of the handle's graph integrates
 enum MdKind {
   MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, MD_NEB_FIRE = 4, MD_REMD = 5, MD_NPT = 6,
-  MD_METAD = 7, MD_DIMER = 8
+  MD_METAD = 7, MD_DIMER = 8, MD_UMBRELLA = 9
 };
 
-// the integrator of sgdml_b200_md_run, sgdml_b200_remd_run, sgdml_b200_npt_run, sgdml_b200_pimd_run,
-// sgdml_b200_relax_*, sgdml_b200_neb_fire or sgdml_b200_dimer_fire; advance == 0 completes a run's last step (MD; a
-// replica exchange first exchanges that last state) or only tests convergence (relaxation, NEB: after the force
-// projection, dimer: with the curvature).  L-BFGS keeps its direction in V, which relax_impl zeroes after.
+// the integrator of sgdml_b200_md_run, sgdml_b200_remd_run, sgdml_b200_npt_run, sgdml_b200_umbrella_run,
+// sgdml_b200_pimd_run, sgdml_b200_relax_*, sgdml_b200_neb_fire or sgdml_b200_dimer_fire; advance == 0 completes a
+// run's last step (MD; a replica exchange or umbrella run first exchanges that last state) or only tests convergence
+// (relaxation, NEB: after the force projection, dimer: with the curvature).  L-BFGS keeps its direction in V, which
+// relax_impl zeroes after.
 int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
   StepParams* p = md->params(md->blk);
   switch (kind) {
@@ -1501,9 +1675,14 @@ int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
                                                             advance);
       break;
     case MD_REMD:
-      k_remd_exchange<<<(unsigned)(md->n_rep / md->group), MD_THREADS, 0, s>>>(&p->remd, &p->md, md->s, md->R, md->V,
-                                                                              md->F, md->E, md->walker, md->step,
-                                                                              md->dimi);
+    case MD_UMBRELLA:
+      if (kind == MD_REMD)
+        k_remd_exchange<<<(unsigned)(md->n_rep / md->group), MD_THREADS, 0, s>>>(&p->remd, &p->md, md->s, md->R, md->V,
+                                                                                md->F, md->E, md->walker, md->step,
+                                                                                md->dimi);
+      else
+        k_umbrella_exchange<<<(unsigned)(md->n_rep / md->group), MD_THREADS, 0, s>>>(
+            &p->remd, &p->umbrella, &p->md, md->s, md->R, md->V, md->F, md->Fm, md->E, md->walker, md->step, md->dimi);
       SG_CUDA(cudaGetLastError());
       count_launch(KID_MISC);
       [[fallthrough]];
@@ -1522,11 +1701,21 @@ int md_forces(sgdml_b200_md* md, double* F, double* E, double* W, cudaStream_t s
   return force_eval_run_cells(md->fe, md->R, md->lat, F, E, W, s);
 }
 
-// The state's forces and energies: on a metadynamics handle the model's F into Fm, then k_metad_bias (deposit: inside
-// a run) completes F; on every other handle md_forces
+// The umbrella restraints of the state in R on top of the model's forces in Fm
+int umbrella_bias(sgdml_b200_md* md, cudaStream_t s) {
+  k_umbrella_bias<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&md->params(md->blk)->umbrella, md->R, md->Fm, md->F,
+                                                             md->dimi);
+  SG_CUDA(cudaGetLastError());
+  count_launch(KID_MISC);
+  return 0;
+}
+
+// The state's forces and energies: on a metadynamics or umbrella handle the model's F into Fm, then k_metad_bias
+// (deposit: inside a run) or k_umbrella_bias completes F; on every other handle md_forces
 int md_state_forces(sgdml_b200_md* md, int deposit, cudaStream_t s) {
-  if (md->kind != METAD) return md_forces(md, md->F, md->E, md->W, s);
+  if (md->kind != METAD && md->kind != UMBRELLA) return md_forces(md, md->F, md->E, md->W, s);
   SG_TRY(md_forces(md, md->Fm, md->E, nullptr, s));
+  if (md->kind == UMBRELLA) return umbrella_bias(md, s);
   StepParams* p = md->params(md->blk);
   k_metad_bias<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&p->metad, &p->md, md->R, md->Fm, md->F, md->step, md->dimi,
                                                           deposit);
@@ -1702,6 +1891,28 @@ void metad_params(sgdml_b200_md* md, const MetadRun& m, const Outputs& out) {
   q.bias_f = out.dev(OUT_BIAS);
 }
 
+// An umbrella run (sgdml_b200_umbrella_run): RemdParams' schedule, counters and walker frames, one temperature's beta,
+// and the CV and restraint frames (after run_params; the CVs and the window table are the handle's, already there)
+void umbrella_params(sgdml_b200_md* md, int64_t every, double kT, const Outputs& out) {
+  StepParams& hp = *md->params(md->hblk);
+  const MdParams& p = hp.md;
+  RemdParams& x = hp.remd;
+  UmbrellaParams& q = hp.umbrella;
+  x.key[0] = p.key[0];
+  x.key[1] = p.key[1];
+  x.run_start = p.run_start;
+  x.stride = p.stride;
+  x.every = every;
+  x.n_temps = q.n_windows;
+  x.beta = x.lam_up = x.lam_dn = nullptr;
+  x.n_acc = md->xcount;
+  x.n_att = md->xcount + md->n_rep;
+  x.W_f = out.dev<int>(OUT_WALKER_F);
+  q.beta = kT > 0.0 ? 1.0 / kT : 0.0;
+  q.cv_f = out.dev(OUT_CV);
+  q.bias_f = out.dev(OUT_BIAS);
+}
+
 // Grows every group's hill store to at least `need` slots, keeping its hills, before anything of the call is queued.
 // The store's pointers and capacity are in the mirror's MetadParams, which the caller uploads.
 int metad_reserve(sgdml_b200_md* md, int64_t need) {
@@ -1787,11 +1998,12 @@ struct Accepts {
   unsigned kinds;  // bit k: HandleKind k
   const char* needs;
 };
-constexpr Accepts ANY_KIND = {1u << PLAIN | 1u << RING | 1u << NPT | 1u << METAD, "a handle"};
+constexpr Accepts ANY_KIND = {1u << PLAIN | 1u << RING | 1u << NPT | 1u << METAD | 1u << UMBRELLA, "a handle"};
 constexpr Accepts PLAIN_KIND = {1u << PLAIN, "a handle of sgdml_b200_md_create (or sgdml_b200_pimd_create, one bead)"};
 constexpr Accepts PLAIN_OR_RING = {1u << PLAIN | 1u << RING, "a handle of sgdml_b200_md_create or _pimd_create"};
 constexpr Accepts NPT_KIND = {1u << NPT, "an NPT handle (sgdml_b200_npt_create)"};
 constexpr Accepts METAD_KIND = {1u << METAD, "a metadynamics handle (sgdml_b200_metad_create)"};
+constexpr Accepts UMBRELLA_KIND = {1u << UMBRELLA, "an umbrella handle (sgdml_b200_umbrella_create)"};
 
 // the first check of every entry point that takes a handle
 int check_kind(const sgdml_b200_md* md, const char* entry, const Accepts& a) {
@@ -1807,7 +2019,7 @@ struct Run {
   uint64_t seed;
   void* outs[N_RUN_OUTS];
   double hbar, lambda;  // MD_RING_POLYMER
-  RemdRun remd;         // MD_REMD
+  RemdRun remd;         // MD_REMD; MD_UMBRELLA: n_temps = n_windows and every (kT unused)
   NptRun npt;           // MD_NPT
   MetadRun metad;       // MD_METAD
 };
@@ -1824,16 +2036,19 @@ int run_check(const sgdml_b200_md* md, const Run& r, const char* entry) {
   return 0;
 }
 
-// sgdml_b200_md_run (MD_CLASSICAL), _pimd_run (MD_RING_POLYMER), _remd_run (MD_REMD), _npt_run (MD_NPT) and
-// _metad_run (MD_METAD), after their checks: n_steps steps, then the completing launch.
+// sgdml_b200_md_run (MD_CLASSICAL), _pimd_run (MD_RING_POLYMER), _remd_run (MD_REMD), _npt_run (MD_NPT),
+// _metad_run (MD_METAD) and _umbrella_run (MD_UMBRELLA), after their checks: n_steps steps, then the completing launch.
 int md_run(sgdml_b200_md* md, int kind, const Run& r, cudaStream_t s) {
-  if (r.n_steps == 0 && kind != MD_REMD) return 0;  // (a replica exchange still reports its labels and zero counts)
-  md->group = kind == MD_REMD ? r.remd.n_temps : 1;
+  const bool exch = kind == MD_REMD || kind == MD_UMBRELLA;
+  if (r.n_steps == 0 && !exch) return 0;  // (an exchange run still reports its labels and zero counts)
+  md->group = exch ? r.remd.n_temps : 1;
   const int64_t n_rep = md->n_rep, n_frames = r.stride > 0 ? r.n_steps / r.stride : 0;
   const size_t fr = sizeof(double) * (size_t)(n_frames * n_rep);
   const size_t fp = sizeof(double) * (size_t)(n_frames * (n_rep / md->nb));
   const size_t nc = sizeof(int64_t) * (size_t)(n_rep / md->group * (md->group - 1));  // (n_ladders, n_temps - 1)
-  const int n_cv = kind == MD_METAD ? md->params(md->hblk)->metad.n_cv : 0;
+  const int n_cv = kind == MD_METAD     ? md->params(md->hblk)->metad.n_cv
+                   : kind == MD_UMBRELLA ? md->params(md->hblk)->umbrella.n_cv
+                                         : 0;
   void* const* outs = r.outs;
   Outputs out(s);
   SG_TRY(out.init({{outs[OUT_R], fr * md->dimi}, {outs[OUT_V], fr * md->dimi}, {outs[OUT_EPOT], fr},
@@ -1845,8 +2060,8 @@ int md_run(sgdml_b200_md* md, int kind, const Run& r, cudaStream_t s) {
   if (kind == MD_REMD) {
     SG_TRY(reserve(md, r.remd.n_temps));
     SG_TRY(remd_alloc(md, s));
-    SG_CUDA(cudaMemsetAsync(md->xcount, 0, 2 * sizeof(int64_t) * (size_t)n_rep, s));  // the run's counts
   }
+  if (exch) SG_CUDA(cudaMemsetAsync(md->xcount, 0, 2 * sizeof(int64_t) * (size_t)n_rep, s));  // the run's counts
   SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the mirror
   if (kind == MD_METAD) {
     int64_t need = 0;
@@ -1860,11 +2075,13 @@ int md_run(sgdml_b200_md* md, int kind, const Run& r, cudaStream_t s) {
     end = pimd_params(md, out, r.dt, r.kT, r.hbar, r.gamma, r.lambda);
   } else {
     run_params(p.md, md, r.dt, r.seed, n_frames, r.stride, out);
-    end = md_params(md, r.dt, r.gamma, kind == MD_REMD ? r.remd.kT : &r.kT, md->group);
+    end = kind == MD_REMD ? md_params(md, r.dt, r.gamma, r.remd.kT, r.remd.n_temps)
+                          : md_params(md, r.dt, r.gamma, &r.kT, 1);
     switch (kind) {
       case MD_REMD: end = remd_params(md, r.remd, out); break;
       case MD_NPT: npt_params(md, r.npt, r.dt, r.kT, out); break;
       case MD_METAD: metad_params(md, r.metad, out); break;
+      case MD_UMBRELLA: umbrella_params(md, r.remd.every, r.kT, out); break;
     }
   }
   SG_TRY(upload(md, end, s));
@@ -1880,7 +2097,7 @@ int md_run(sgdml_b200_md* md, int kind, const Run& r, cudaStream_t s) {
       for (int64_t& c : md->hcount_host) c += add;
     }
   }
-  if (kind == MD_REMD) SG_TRY(out.copy_from(OUT_WALKERS, {md->walker, md->xcount, md->xcount + n_rep}));
+  if (exch) SG_TRY(out.copy_from(OUT_WALKERS, {md->walker, md->xcount, md->xcount + n_rep}));
   return out.finish();
 }
 
@@ -2128,6 +2345,61 @@ int npt_install(sgdml_b200_md* md, const std::vector<NptCell>& cells, const std:
   return 0;
 }
 
+// The CVs of sgdml_b200_metad_create and _umbrella_create from HOST arrays, checked: the types, and the atoms of
+// each CV distinct and in [0, n_atoms).  Nothing is queued.
+int cv_parse(int64_t n_cv, const int* cv_type, const int64_t* cv_atoms, int64_t n_atoms, int* type, int (*atoms)[4]) {
+  SG_ARG(n_cv >= 1 && n_cv <= MD_MAX_CV);
+  SG_ARG(!is_device_ptr(cv_type) && !is_device_ptr(cv_atoms));
+  for (int j = 0; j < n_cv; ++j) {
+    if (cv_type[j] != CV_DISTANCE && cv_type[j] != CV_ANGLE && cv_type[j] != CV_DIHEDRAL)
+      return fail_arg("cv_type must be 0 (distance), 1 (angle) or 2 (dihedral)");
+    type[j] = cv_type[j];
+    const int na = cv_type[j] + 2;
+    for (int p = 0; p < na; ++p) {
+      const int64_t a = cv_atoms[4 * j + p];
+      if (a < 0 || a >= n_atoms) return fail_arg("cv_atoms must lie in [0, N)");
+      for (int o = 0; o < p; ++o)
+        if (cv_atoms[4 * j + o] == a) return fail_arg("the atoms of a CV must be distinct");
+      atoms[j][p] = (int)a;
+    }
+  }
+  return 0;
+}
+
+// The buffers of a biased handle (metadynamics, umbrella): the model's forces Fm, the state's CVs, bias energy and
+// bias force, the last zero where no CV reaches
+int bias_alloc(sgdml_b200_md* md, int n_cv) {
+  const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
+  SG_CUDA(cached_malloc(&md->Fm, st));
+  SG_CUDA(cached_malloc(&md->Fb, st));
+  SG_CUDA(cached_malloc(&md->cv, sizeof(double) * (size_t)(md->n_rep * n_cv)));
+  SG_CUDA(cached_malloc(&md->Vb, sizeof(double) * (size_t)md->n_rep));
+  SG_CUDA(cudaMemset(md->Fb, 0, st));  // the coordinates no CV touches keep a zero bias force
+  return 0;
+}
+
+// The window table (centres, then force constants) of an umbrella handle from (n_windows, n_cv) HOST arrays, checked.
+// Nothing is queued.
+int windows_parse(int64_t n_windows, int n_cv, const int* type, const double* centers, const double* kappas,
+                  std::vector<double>* win) {
+  SG_TRY(umbrella_windows_check(n_windows, n_cv, type, centers, kappas));
+  const size_t n = (size_t)(n_windows * n_cv);
+  win->assign(centers, centers + n);
+  win->insert(win->end(), kappas, kappas + n);
+  return 0;
+}
+
+// The CV, bias-energy and bias-force rows of a biased handle's state
+int bias_get(sgdml_b200_md* md, int n_cv, double* cv, double* V_bias, double* F_bias, const char* entry,
+             cudaStream_t s) {
+  if (!md->has_state) return fail_arg((std::string(entry) + ": no state yet (call sgdml_b200_md_set_state)").c_str());
+  const size_t n = (size_t)md->n_rep;
+  Outputs out(s);
+  SG_TRY(out.init({{cv, sizeof(double) * n * n_cv}, {V_bias, sizeof(double) * n}, {F_bias, sizeof(double) * n * md->dimi}}));
+  SG_TRY(out.copy_from(0, {md->cv, md->Vb, md->Fb}));
+  return out.finish();
+}
+
 }  // namespace
 
 extern "C" {
@@ -2196,35 +2468,16 @@ int sgdml_b200_metad_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_
   SG_TRY(require_device());
   SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr && cv_type != nullptr && cv_atoms != nullptr);
   SG_ARG(n_groups >= 1 && n_walkers >= 1 && n_groups <= INT32_MAX / n_walkers);
-  SG_ARG(n_cv >= 1 && n_cv <= MD_MAX_CV);
-  SG_ARG(!is_device_ptr(cv_type) && !is_device_ptr(cv_atoms));
   int64_t n_atoms = 0;
   SG_TRY(sgdml_b200_model_dims(m, &n_atoms, nullptr, nullptr));
   MetadParams q = {};
+  SG_TRY(cv_parse(n_cv, cv_type, cv_atoms, n_atoms, q.type, q.atoms));
   q.n_cv = (int)n_cv;
   q.n_walkers = (int)n_walkers;
-  for (int j = 0; j < n_cv; ++j) {
-    if (cv_type[j] != CV_DISTANCE && cv_type[j] != CV_ANGLE && cv_type[j] != CV_DIHEDRAL)
-      return fail_arg("cv_type must be 0 (distance), 1 (angle) or 2 (dihedral)");
-    q.type[j] = cv_type[j];
-    const int na = cv_type[j] + 2;
-    for (int p = 0; p < na; ++p) {
-      const int64_t a = cv_atoms[4 * j + p];
-      if (a < 0 || a >= n_atoms) return fail_arg("cv_atoms must lie in [0, N)");
-      for (int o = 0; o < p; ++o)
-        if (cv_atoms[4 * j + o] == a) return fail_arg("the atoms of a CV must be distinct");
-      q.atoms[j][p] = (int)a;
-    }
-  }
   const int64_t n_rep = n_groups * n_walkers;
   return md_create(out, m, METAD, n_rep, 1, inv_mass, [&](sgdml_b200_md* md) -> int {
-    const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
-    SG_CUDA(cached_malloc(&md->Fm, st));
-    SG_CUDA(cached_malloc(&md->Fb, st));
-    SG_CUDA(cached_malloc(&md->cv, sizeof(double) * (size_t)(n_rep * n_cv)));
-    SG_CUDA(cached_malloc(&md->Vb, sizeof(double) * (size_t)n_rep));
+    SG_TRY(bias_alloc(md, (int)n_cv));
     SG_CUDA(cached_malloc(&md->hcount, sizeof(int64_t) * (size_t)n_groups));
-    SG_CUDA(cudaMemset(md->Fb, 0, st));  // the coordinates no CV touches keep a zero bias force
     SG_CUDA(cudaMemset(md->hcount, 0, sizeof(int64_t) * (size_t)n_groups));
     md->n_groups = n_groups;
     md->hcount_host.assign((size_t)n_groups, 0);
@@ -2345,14 +2598,81 @@ int sgdml_b200_metad_set_hills(sgdml_b200_md* md, const int64_t* n_hills, const 
 int sgdml_b200_metad_get_bias(sgdml_b200_md* md, double* cv, double* V_bias, double* F_bias, void* stream) {
   SG_TRY(require_device());
   SG_TRY(check_kind(md, "sgdml_b200_metad_get_bias", METAD_KIND));
-  if (!md->has_state) return fail_arg("sgdml_b200_metad_get_bias: no state yet (call sgdml_b200_md_set_state)");
+  return bias_get(md, md->params(md->hblk)->metad.n_cv, cv, V_bias, F_bias, "sgdml_b200_metad_get_bias",
+                  (cudaStream_t)stream);
+}
+
+int sgdml_b200_umbrella_create(sgdml_b200_md** out, sgdml_b200_model* m, int64_t n_ladders, int64_t n_windows,
+                               const double* inv_mass, int64_t n_cv, const int* cv_type, const int64_t* cv_atoms,
+                               const double* centers, const double* kappas) {
+  SG_TRY(require_device());
+  SG_ARG(out != nullptr && m != nullptr && inv_mass != nullptr && cv_type != nullptr && cv_atoms != nullptr);
+  SG_ARG(n_ladders >= 1 && n_windows >= 1 && n_ladders <= INT32_MAX / n_windows);
+  int64_t n_atoms = 0;
+  SG_TRY(sgdml_b200_model_dims(m, &n_atoms, nullptr, nullptr));
+  UmbrellaParams q = {};
+  SG_TRY(cv_parse(n_cv, cv_type, cv_atoms, n_atoms, q.type, q.atoms));
+  q.n_cv = (int)n_cv;
+  q.n_windows = (int)n_windows;
+  std::vector<double> win;
+  SG_TRY(windows_parse(n_windows, q.n_cv, q.type, centers, kappas, &win));
+  return md_create(out, m, UMBRELLA, n_ladders * n_windows, 1, inv_mass, [&](sgdml_b200_md* md) -> int {
+    SG_TRY(bias_alloc(md, q.n_cv));
+    SG_CUDA(cached_malloc(&md->win, sizeof(double) * win.size()));
+    SG_CUDA(cudaMemcpy(md->win, win.data(), sizeof(double) * win.size(), cudaMemcpyHostToDevice));
+    SG_TRY(remd_alloc(md, 0));
+    q.win = md->win;
+    q.cv = md->cv;
+    q.Vb = md->Vb;
+    q.Fb = md->Fb;
+    StepParams* p = md->params(md->hblk);
+    p->umbrella = q;
+    SG_TRY(upload(md, p + 1, 0));
+    SG_CUDA(cudaStreamSynchronize(0));
+    return 0;
+  });
+}
+
+int sgdml_b200_umbrella_set_windows(sgdml_b200_md* md, const double* centers, const double* kappas, void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(check_kind(md, "sgdml_b200_umbrella_set_windows", UMBRELLA_KIND));
+  const UmbrellaParams& q = md->params(md->hblk)->umbrella;
+  std::vector<double> win;
+  SG_TRY(windows_parse(q.n_windows, q.n_cv, q.type, centers, kappas, &win));
   cudaStream_t s = (cudaStream_t)stream;
-  const size_t n = (size_t)md->n_rep;
-  Outputs out(s);
-  SG_TRY(out.init({{cv, sizeof(double) * n * md->params(md->hblk)->metad.n_cv}, {V_bias, sizeof(double) * n},
-                   {F_bias, sizeof(double) * n * md->dimi}}));
-  SG_TRY(out.copy_from(0, {md->cv, md->Vb, md->Fb}));
-  return out.finish();
+  SG_CUDA(cudaMemcpyAsync(md->win, win.data(), sizeof(double) * win.size(), cudaMemcpyHostToDevice, s));
+  if (md->has_state) SG_TRY(umbrella_bias(md, s));  // Fm is the state's: only the restraints change
+  SG_CUDA(cudaStreamSynchronize(s));  // (the table's host vector goes out of scope)
+  return 0;
+}
+
+int sgdml_b200_umbrella_run(sgdml_b200_md* md, int64_t n_steps, double dt, double gamma, double kT, uint64_t seed,
+                            int64_t exchange_every, int64_t stride, double* R_frames, double* V_frames,
+                            double* E_pot_frames, double* E_kin_frames, double* cv_frames, double* bias_frames,
+                            int* walker_frames, int* walkers_out, int64_t* n_accepted, int64_t* n_attempted,
+                            void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(check_kind(md, "sgdml_b200_umbrella_run", UMBRELLA_KIND));
+  Run r = {n_steps, stride, dt, kT, gamma, seed,
+           {R_frames, V_frames, E_pot_frames, E_kin_frames, nullptr, nullptr, walker_frames, walkers_out, n_accepted,
+            n_attempted}};
+  r.outs[OUT_CV] = cv_frames;
+  r.outs[OUT_BIAS] = bias_frames;
+  SG_TRY(run_check(md, r, "sgdml_b200_umbrella_run"));
+  SG_ARG(std::isfinite(gamma) && gamma >= 0.0);
+  SG_ARG(exchange_every >= 0);
+  const int nw = md->params(md->hblk)->umbrella.n_windows;
+  if (exchange_every > 0 && !(kT > 0.0 && nw >= 2))
+    return fail_arg("sgdml_b200_umbrella_run: exchanges need kT > 0 and n_windows >= 2");
+  r.remd = {nw, nullptr, exchange_every};
+  return md_run(md, MD_UMBRELLA, r, (cudaStream_t)stream);
+}
+
+int sgdml_b200_umbrella_get_bias(sgdml_b200_md* md, double* cv, double* V_bias, double* F_bias, void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(check_kind(md, "sgdml_b200_umbrella_get_bias", UMBRELLA_KIND));
+  return bias_get(md, md->params(md->hblk)->umbrella.n_cv, cv, V_bias, F_bias, "sgdml_b200_umbrella_get_bias",
+                  (cudaStream_t)stream);
 }
 
 int sgdml_b200_md_destroy(sgdml_b200_md* md) {
@@ -2395,7 +2715,7 @@ int sgdml_b200_md_get_state(sgdml_b200_md* md, double* R, double* V, double* F, 
   const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
   Outputs out(s);
   SG_TRY(out.init({{R, st}, {V, st}, {F, st}, {E_pot, sizeof(double) * md->n_rep}, {step, sizeof(uint64_t)}}));
-  SG_TRY(out.copy_from(0, {md->R, md->V, md->kind == METAD ? md->Fm : md->F, md->E, md->step}));
+  SG_TRY(out.copy_from(0, {md->R, md->V, md->kind == METAD || md->kind == UMBRELLA ? md->Fm : md->F, md->E, md->step}));
   return out.finish();
 }
 

@@ -1,7 +1,8 @@
 // Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_metad_*,
-// sgdml_b200_pimd_*, sgdml_b200_relax_*, sgdml_b200_neb_fire, sgdml_b200_dimer_fire): the contract of the kernels in
-// md.cu -- the BAOAB integrator step, the replica exchange, the NPT step, the metadynamics bias, the ring-polymer step,
-// their counter-based noise, the FIRE and L-BFGS steps, the nudged elastic band and the dimer search.
+// sgdml_b200_umbrella_*, sgdml_b200_pimd_*, sgdml_b200_relax_*, sgdml_b200_neb_fire, sgdml_b200_dimer_fire): the
+// contract of the kernels in md.cu -- the BAOAB integrator step, the replica exchange, the NPT step, the metadynamics
+// bias, the umbrella restraints and their exchange, the ring-polymer step, their counter-based noise, the FIRE and
+// L-BFGS steps, the nudged elastic band and the dimer search -- and of MBAR in mbar.cu.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -148,6 +149,84 @@ struct MetadParams {
 //         centre s, widths MetadParams.width, height w0 exp(-V / dkT) (w0 with dkT = +inf).
 // The driver commits a run's hills after it: count[g] += n_walkers #{c in (run_start, run_start + n_steps] :
 // c % pace == 0}.  The store's address is read from MetadParams, not baked into the step graph.
+
+// Umbrella sampling with Hamiltonian replica exchange (sgdml_b200_umbrella_run; REUS: Sugita, Kitao & Okamoto, JCP 113,
+// 6042 (2000)): an umbrella handle (sgdml_b200_umbrella_create) is an MD handle of n_rep = n_ladders n_windows replicas,
+// slot l n_windows + k window k of ladder l, integrated by k_md_step (sigma row 0: one temperature).  Its CVs are the
+// metadynamics CVs above (types, atoms, formulas, no minimum image).  Window k restrains CV j about the centre c_kj with
+// the force constant kappa_kj >= 0; per CV j in increasing order, from b = 0.0, every operation rounded as written:
+//   e_j = s_j - c_kj (a dihedral's wrapped into [-pi, pi) by one step, as a hill difference);  u_j = kappa_kj e_j;
+//   b = b + (0.5 u_j) e_j;  db/ds_j = u_j
+// umbrella_restraint below is the one copy of it: the step graph, the exchange and MBAR all call it.  The bias force
+// is the metadynamics one with dV_j = u_j: Fb_a = sum over the CVs j holding atom a of -(u_j ds_j/dr_a) from 0.0, and
+// F = Fm + Fb_a rounded once on the touched atoms, F = Fm elsewhere.
+struct UmbrellaParams {
+  int n_cv, n_windows;
+  int type[MD_MAX_CV];
+  int atoms[MD_MAX_CV][4];   // unused entries 0
+  double beta;               // 1 / kT of the run (read by the exchange only)
+  const double* win;         // the window table: centres (n_windows, n_cv), then force constants (n_windows, n_cv)
+  double *cv, *Vb, *Fb;      // the state's CVs (n_rep, n_cv), restraint energy (n_rep) and bias force (n_rep, 3N)
+  double *cv_f, *bias_f;     // frames (n_frames, n_rep, n_cv) / (n_frames, n_rep), or null
+};
+
+#ifdef __CUDACC__
+// b of CVs s (n_cv) under one window (centres c, force constants kappa, n_cv each); u (null: not wanted) gets db/ds
+__device__ __forceinline__ double umbrella_restraint(int n_cv, const int* type, const double* s, const double* c,
+                                                     const double* kappa, double* u) {
+  double b = 0.0;
+  for (int j = 0; j < n_cv; ++j) {
+    double e = __dsub_rn(s[j], c[j]);
+    if (type[j] == CV_DIHEDRAL) {
+      if (e >= M_PI)
+        e = __dsub_rn(e, 2.0 * M_PI);
+      else if (e < -M_PI)
+        e = __dadd_rn(e, 2.0 * M_PI);
+    }
+    const double uj = __dmul_rn(kappa[j], e);
+    if (u != nullptr) u[j] = uj;
+    b = __dadd_rn(b, __dmul_rn(__dmul_rn(0.5, uj), e));
+  }
+  return b;
+}
+#endif
+
+// k_umbrella_bias: one CTA of MD_THREADS per replica, launched after the force evaluation that wrote the model force Fm
+// and E of the state R holds.  Replica rep under window rep % n_windows: s and ds/dR (cv_eval), b and u, F = Fm + Fb,
+// and the state's s, b and Fb.  It writes no frames.
+//
+// k_umbrella_exchange: one CTA of MD_THREADS per ladder, launched before k_md_step on the same counter c, with
+// RemdParams' key, run_start, every, n_temps (= n_windows), stride, n_acc, n_att and W_f.  On an exchange (k_remd_exchange's
+// schedule, pairing and Philox draw), with configuration a in slot k and b in slot k + 1 and b_k(s) the restraint of
+// window k at the stored CVs s (umbrella_restraint):
+//   d = -(beta ((b_k(s_b) + b_k+1(s_a)) - (b_k(s_a) + b_k+1(s_b))))  (rounded as written);  accepted iff d >= 0 or
+//   u < exp(d)
+// An accepted swap exchanges the R, Fm, E and CV rows and the walker labels of the two slots, recomputes Fb, b and
+// F = Fm + Fb of both slots in their new windows (k_umbrella_bias's arithmetic), and each configuration keeps its
+// full-step velocity: w = v + h (F_old s), v' = w - h (F_new s) (k_md_step's rounding of the kick).  On a frame step of
+// k_md_step (the same rule; also with every == 0) it then writes the ladder's walker labels, CVs and b into W_f, cv_f,
+// bias_f; k_md_step writes R, V, E_pot and E_kin of the same state.
+//
+// MBAR (sgdml_b200_umbrella_mbar; Shirts & Chodera, JCP 129, 124105 (2008), eq. 11), in mbar.cu.  K windows, samples
+// s_n (n, n_cv) pooled with N_k of them from window k, u_kn = beta b_k(s_n) by umbrella_restraint (never stored).  From
+// f = 0, each iteration:
+//   L_n = m_n + log(sum_k exp(a_kn - m_n)), a_kn = (ln N_k + f_k) - u_kn, m_n = max_k a_kn, the sum in increasing k
+//         from 0.0 (one thread per sample; ln N_k = -inf for an empty window)
+//   f_k' = -logsumexp_n(-u_kn - L_n): thread t of CTA c folds its samples n = c MBAR_CHUNK + t, ... + MBAR_THREADS,
+//         ... in increasing n into a running (max, sum) pair, then block_tree's fixed tree over the CTA merges the
+//         pairs; one CTA per window then folds the per-CTA pairs, thread t those of CTA t, t + MBAR_THREADS, ... in
+//         increasing c, and the same tree merges them (no atomics: the same bits on every call)
+//   f' = f' - f'_0;  resid = max_k |f'_k - f_k|;  stop when resid < tol or after max_iter iterations
+// The pair fold: (m, S) + x = x > m ? (x, S exp(m - x) + 1) : (m, S + exp(x - m)); a merge (m, S) + (m2, S2) with
+// S2 > 0 is (m2, S exp(m - m2) + S2) when m2 > m, else (m, S + S2 exp(m2 - m)), and an empty pair (S = 0) adds nothing;
+// logsumexp = m + log(S).  Every operation rounds as written.  After the last iteration L_n is evaluated once more with the final f, and log w_n = f_u - L_n with
+// f_u = -logsumexp_n(-L_n) (the unbiased state), so that sum_n w_n = 1.
+constexpr int MBAR_THREADS = 256;
+constexpr int MBAR_CHUNK = 16 * MBAR_THREADS;  // samples per CTA of the f reduction
+
+// The checks of a window table, shared by sgdml_b200_umbrella_create, _set_windows and _mbar: centers and kappas
+// (n_windows, n_cv) HOST arrays, finite, kappa >= 0, a dihedral's centre in (-pi, pi].  Returns 0 or an argument error.
+int umbrella_windows_check(int64_t n_windows, int n_cv, const int* type, const double* centers, const double* kappas);
 
 // Path-integral MD (sgdml_b200_pimd_run): replica p P + j is bead j of ring polymer p.
 constexpr int PIMD_MAX_BEADS = 64;  // C (P x P) sits in shared memory: 32 KB at the cap

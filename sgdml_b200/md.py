@@ -13,7 +13,8 @@ replicas, each in a cell of its own that an isotropic stochastic cell rescaling 
 
 ``GDMLMetadynamics`` -- well-tempered multiple-walker metadynamics on the same engine (``sgdml_b200_metad_*``):
 groups of Langevin walkers, each group sharing one store of Gaussian hills on distance, angle and dihedral collective
-variables, for free-energy surfaces along chosen coordinates.
+variables, for free-energy surfaces along chosen coordinates.  ``GDMLUmbrellaSampling`` -- umbrella sampling on the
+same CVs with replica exchange between neighbouring windows (``sgdml_b200_umbrella_*``), unbiased by MBAR on the device.
 
 ``GDMLRelaxation`` -- geometry optimisation of many replicas on the same engine (``sgdml_b200_relax_*``): FIRE and
 L-BFGS, each replica frozen once it has converged.  ``GDMLNEB`` and ``GDMLDimer`` find saddle points on it: between
@@ -490,6 +491,31 @@ class GDMLNPTDynamics(GDMLDynamics):
 _CV_TYPES = {'distance': 0, 'angle': 1, 'dihedral': 2}
 
 
+def _cv_list(cvs, what):
+    """[(kind, atoms)] checked: 1 to 4 CVs of a known kind, each with its number of atoms"""
+    cvs = list(cvs)
+    if not 1 <= len(cvs) <= 4:
+        raise ValueError('%s takes 1 to 4 collective variables: %d' % (what, len(cvs)))
+    out = []
+    for kind, atoms in cvs:
+        if kind not in _CV_TYPES:
+            raise ValueError("a CV is 'distance', 'angle' or 'dihedral': %r" % (kind,))
+        atoms = tuple(int(a) for a in atoms)
+        if len(atoms) != _CV_TYPES[kind] + 2:
+            raise ValueError('a %s takes %d atoms: %s' % (kind, _CV_TYPES[kind] + 2, atoms))
+        out.append((kind, atoms))
+    return out
+
+
+def _cv_arrays(cvs):
+    """the C ABI's cv_type (n_cv,) int32 and cv_atoms (n_cv, 4) int64 of a _cv_list"""
+    types = np.array([_CV_TYPES[k] for k, _ in cvs], dtype=np.int32)
+    atoms = np.zeros((len(cvs), 4), dtype=np.int64)
+    for j, (_, a) in enumerate(cvs):
+        atoms[j, :len(a)] = a
+    return types, atoms
+
+
 class GDMLMetadynamics(GDMLDynamics):
     """Well-tempered multiple-walker metadynamics (Raiteri et al., J. Phys. Chem. B 110, 3533 (2006); Barducci, Bussi &
     Parrinello, PRL 100, 020603 (2008)) on the device (``sgdml_b200_metad_*``), in the units of ``GDMLDynamics``.
@@ -520,17 +546,7 @@ class GDMLMetadynamics(GDMLDynamics):
         self.n_groups = int(n_groups)
         if self.n_walkers < 1 or self.n_groups < 1:
             raise ValueError('n_walkers and n_groups must be >= 1')
-        cvs = list(cvs)
-        if not 1 <= len(cvs) <= 4:
-            raise ValueError('metadynamics takes 1 to 4 collective variables: %d' % len(cvs))
-        self.cvs = []
-        for kind, atoms in cvs:
-            if kind not in _CV_TYPES:
-                raise ValueError("a CV is 'distance', 'angle' or 'dihedral': %r" % (kind,))
-            atoms = tuple(int(a) for a in atoms)
-            if len(atoms) != _CV_TYPES[kind] + 2:
-                raise ValueError('a %s takes %d atoms: %s' % (kind, _CV_TYPES[kind] + 2, atoms))
-            self.cvs.append((kind, atoms))
+        self.cvs = _cv_list(cvs, 'metadynamics')
         self.n_cv = len(self.cvs)
         self.bias_factor = np.inf  # of the last run: free_energy's default
         super().__init__(model, masses, self.n_groups * self.n_walkers, E_to_eV, F_to_eV_Ang)
@@ -539,10 +555,7 @@ class GDMLMetadynamics(GDMLDynamics):
         self._periodic = np.array([k == 'dihedral' for k, _ in self.cvs])
 
     def _create_handle(self):
-        types = np.array([_CV_TYPES[k] for k, _ in self.cvs], dtype=np.int32)
-        atoms = np.zeros((self.n_cv, 4), dtype=np.int64)
-        for j, (_, a) in enumerate(self.cvs):
-            atoms[j, :len(a)] = a
+        types, atoms = _cv_arrays(self.cvs)
         handle = ctypes.c_void_p()
         _lib.check(
             _lib.lib().sgdml_b200_metad_create(ctypes.byref(handle), self.gdml_predict._handle, self.n_groups,
@@ -694,6 +707,235 @@ class GDMLMetadynamics(GDMLDynamics):
         gamma = self.bias_factor if bias_factor is None else float(bias_factor)
         f = -self.bias(grid) * (1.0 if np.isinf(gamma) else gamma / (gamma - 1.0))
         return f - f.reshape(self.n_groups, -1).min(1).reshape((self.n_groups,) + (1,) * (f.ndim - 1))
+
+
+class GDMLUmbrellaSampling(GDMLDynamics):
+    """Umbrella sampling with Hamiltonian replica exchange between neighbouring windows (REUS; Sugita, Kitao & Okamoto,
+    J. Chem. Phys. 113, 6042 (2000)) on the device (``sgdml_b200_umbrella_*``), reweighted by MBAR (Shirts & Chodera,
+    J. Chem. Phys. 129, 124105 (2008)), in the units of ``GDMLDynamics``.  `n_ladders` independent ladders of
+    n_windows Langevin replicas: slot k of ladder l (replica l n_windows + k of the engine's handle) is restrained by
+    window k for the whole run, and neighbouring windows swap configurations by the Metropolis test on the restraint
+    energies, inside the step graph.  Independent ladders give error bars.
+
+    cvs: 1 to 4 CVs as ``GDMLMetadynamics`` takes them (Angstrom or radians).  centers, force_constants:
+    (n_windows, n_cv) (or (n_windows,) for one CV): window k adds sum_j 0.5 kappa_kj (s_j - c_kj)^2, kappa in eV/Angstrom^2
+    or eV/rad^2, a dihedral's difference wrapped into [-pi, pi) and its centre in (-pi, pi].
+    ``set_state(positions, velocities=None, step=0)``: positions (n_ladders, n_windows, N, 3), or (n_ladders, N, 3) /
+    (N, 3) copied to every window (and ladder); it resets the walker labels to the slots.  ``get_state()`` adds 'cv',
+    'bias_energy' and 'bias_forces'; its 'forces' and 'potential_energy' are the model's.  ``set_windows(centers,
+    force_constants)`` replaces the windows.
+    ``run(n_steps, dt_fs, temperature_K, friction_per_fs, exchange_every=0, seed=0, stride=0)`` returns
+    ``GDMLReplicaExchange.run``'s keys shaped (..., n_ladders, n_windows, ...), plus 'cv' (n_frames, n_ladders,
+    n_windows, n_cv) and 'bias_energy' (eV) of every frame's state after its exchange.  A run continued over several
+    calls is one long run.
+    ``mbar(cv_frames, temperature_K, windows=None, tol=1e-10, max_iter=10000)`` reweights `cv_frames` (run's 'cv', slot k
+    of every frame a sample of window k) per ladder on the device: [{'f' (n_windows,) the window free energies in eV
+    with f[0] = 0, 'log_w' (n_frames, n_windows) the log unbiased weight of each sample (they sum to 1), 'n_iter',
+    'resid' (the last max |df| in units of kT)}].  windows: (centers, force_constants) of the frames, default the
+    handle's.  ``free_energy(cv_frames, bins, temperature_K, windows=None)``: the profile -kT ln sum_{n in bin} w_n
+    (eV) per ladder, shifted to a minimum of zero, NaN for empty bins: bins are the edges along CV 0, or a pair of edge
+    arrays along CVs 0 and 1; the other CVs are marginalised.  NumPy arrays or float64 CUDA tensors in, the same kind
+    out."""
+
+    def __init__(self, model, masses, cvs, centers, force_constants, n_ladders=1, E_to_eV=_KCAL_PER_MOL_IN_EV,
+                 F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        self.cvs = _cv_list(cvs, 'umbrella sampling')
+        self.n_cv = len(self.cvs)
+        self._windows_arg = (centers, force_constants)
+        self.n_windows = len(self._window_arrays(centers, force_constants)[0])
+        self.n_ladders = int(n_ladders)
+        if self.n_ladders < 1 or self.n_windows < 1:
+            raise ValueError('n_ladders and the number of windows must be >= 1')
+        self._periodic = np.array([k == 'dihedral' for k, _ in self.cvs])
+        super().__init__(model, masses, self.n_ladders * self.n_windows, E_to_eV, F_to_eV_Ang)
+
+    @property
+    def _cv_unit(self):
+        """Angstrom or radian -> the engine's CV unit (model length or radian)"""
+        return np.array([self.Ang_to_R if k == 'distance' else 1.0 for k, _ in self.cvs])
+
+    def _window_arrays(self, centers, force_constants):
+        """(centers, force constants) as (n_windows, n_cv) float64 arrays in the caller's units"""
+        c = np.asarray(_host(centers), dtype=np.float64)
+        k = np.asarray(_host(force_constants), dtype=np.float64)
+        c = c.reshape(-1, 1) if c.ndim == 1 and self.n_cv == 1 else c
+        k = k.reshape(-1, 1) if k.ndim == 1 and self.n_cv == 1 else k
+        if c.ndim != 2 or c.shape[1] != self.n_cv or k.shape != c.shape:
+            raise ValueError('centers and force_constants must be (n_windows, n_cv) with n_cv = %d: %s, %s'
+                             % (self.n_cv, c.shape, k.shape))
+        return c, k
+
+    def _raw_windows(self, centers, force_constants):
+        """the window table in model units: centres in L or rad, force constants in model energy / L^2 or / rad^2"""
+        c, k = self._window_arrays(centers, force_constants)
+        if c.shape[0] != getattr(self, 'n_windows', c.shape[0]):
+            raise ValueError('the windows must number %d: %d' % (self.n_windows, c.shape[0]))
+        u = self._cv_unit
+        return np.ascontiguousarray(c * u), np.ascontiguousarray(k / self.E_to_eV / (u * u))
+
+    def _create_handle(self):
+        types, atoms = _cv_arrays(self.cvs)
+        c, k = self._raw_windows(*self._windows_arg)
+        self.windows = self._window_arrays(*self._windows_arg)
+        handle = ctypes.c_void_p()
+        _lib.check(
+            _lib.lib().sgdml_b200_umbrella_create(ctypes.byref(handle), self.gdml_predict._handle, self.n_ladders,
+                                                  self.n_windows, _lib.ptr(self.inv_mass), self.n_cv, _lib.ptr(types),
+                                                  _lib.ptr(atoms), _lib.ptr(c), _lib.ptr(k)),
+            'umbrella_create',
+        )
+        return handle
+
+    @property
+    def _shape(self):
+        return (self.n_ladders, self.n_windows)
+
+    def _like(self, v, x):
+        return GDMLMetadynamics._like(self, v, x)
+
+    # ------------------------------------------------------------------ model units (L, model energy, fs)
+    def _set_windows_raw(self, centers, kappas):
+        c = np.ascontiguousarray(centers, dtype=np.float64)
+        k = np.ascontiguousarray(kappas, dtype=np.float64)
+        if c.size != self.n_windows * self.n_cv or k.size != c.size:
+            raise ValueError('centers and kappas must hold n_windows x n_cv = %d x %d values each'
+                             % (self.n_windows, self.n_cv))
+        _lib.check(_lib.lib().sgdml_b200_umbrella_set_windows(self._handle, _lib.ptr(c), _lib.ptr(k),
+                                                              _lib.current_stream()), 'umbrella_set_windows')
+
+    def _run_raw(self, n_steps, dt, gamma, kT, exchange_every=0, seed=0, stride=0,
+                 frames=('R', 'V', 'E_pot', 'E_kin', 'cv', 'bias', 'walker')):
+        """-> frames, 'walkers' (n_replicas,), 'n_accepted', 'n_attempted' (n_ladders, n_windows - 1)."""
+        n_steps, stride = int(n_steps), int(stride)
+        out = self._frames(n_steps, stride, frames)
+        if 'cv' in out:
+            out['cv'] = self._empty(tuple(out['cv'].shape) + (self.n_cv,))
+        walkers = self._empty((self.n_replicas,), np.int32)
+        acc, att = (self._empty((self.n_ladders, self.n_windows - 1), np.int64) for _ in range(2))
+        _lib.check(
+            _lib.lib().sgdml_b200_umbrella_run(self._handle, n_steps, float(dt), float(gamma), float(kT), int(seed),
+                                               int(exchange_every), stride,
+                                               *(_lib.ptr(out.get(k)) for k in ('R', 'V', 'E_pot', 'E_kin', 'cv', 'bias',
+                                                                               'walker')),
+                                               _lib.ptr(walkers), _lib.ptr(acc), _lib.ptr(att), _lib.current_stream()),
+            'umbrella_run',
+        )
+        out.update(walkers=walkers, n_accepted=acc, n_attempted=att)
+        return out
+
+    def _get_bias_raw(self):
+        """{'cv' (n_replicas, n_cv), 'V' (n_replicas,), 'F' (n_replicas, 3N)} in model units."""
+        n = self.n_replicas
+        out = {'cv': self._empty((n, self.n_cv)), 'V': self._empty((n,)), 'F': self._empty((n, 3 * self.n_atoms))}
+        _lib.check(_lib.lib().sgdml_b200_umbrella_get_bias(self._handle, _lib.ptr(out['cv']), _lib.ptr(out['V']),
+                                                           _lib.ptr(out['F']), _lib.current_stream()),
+                   'umbrella_get_bias')
+        return out
+
+    def _mbar_raw(self, samples, n_per_window, beta, centers, kappas, tol=1e-10, max_iter=10000):
+        """MBAR over samples (n, n_cv) in model units (NumPy or a float64 CUDA tensor), pooled window after window.
+        -> (f (K,), log_w (n,) of the samples' kind, n_iter, resid)."""
+        n = int(samples.shape[0])
+        counts = np.ascontiguousarray(n_per_window, dtype=np.int64)
+        c = np.ascontiguousarray(centers, dtype=np.float64)
+        k = np.ascontiguousarray(kappas, dtype=np.float64)
+        types, _ = _cv_arrays(self.cvs)
+        if hasattr(samples, 'data_ptr'):
+            _check_cuda_f64(samples, 'samples')
+            import torch
+
+            samples = samples.contiguous()
+            f = torch.empty(len(counts), dtype=torch.float64, device=samples.device)
+            log_w = torch.empty(n, dtype=torch.float64, device=samples.device)
+        else:
+            samples = np.ascontiguousarray(samples, dtype=np.float64)
+            f, log_w = np.empty(len(counts)), np.empty(n)
+        n_iter, resid = np.zeros(1, dtype=np.int64), np.zeros(1)
+        _lib.check(
+            _lib.lib().sgdml_b200_umbrella_mbar(len(counts), self.n_cv, _lib.ptr(types), _lib.ptr(c), _lib.ptr(k),
+                                                float(beta), n, _lib.ptr(samples), _lib.ptr(counts), float(tol),
+                                                int(max_iter), _lib.ptr(f), _lib.ptr(log_w), _lib.ptr(n_iter),
+                                                _lib.ptr(resid), _lib.current_stream()),
+            'umbrella_mbar',
+        )
+        return f, log_w, int(n_iter[0]), float(resid[0])
+
+    # ------------------------------------------------------------------ ASE units
+    def set_state(self, positions, velocities=None, step=0):
+        axes = ('n_ladders', 'n_windows')
+        positions = _groups(positions, 'positions', self.n_ladders, self.n_windows, self.n_atoms, axes)
+        if velocities is not None:
+            velocities = _groups(velocities, 'velocities', self.n_ladders, self.n_windows, self.n_atoms, axes)
+        super().set_state(positions, velocities, step)
+
+    def get_state(self):
+        out = super().get_state()
+        b = self._get_bias_raw()
+        g = self._shape
+        out.update(cv=(b['cv'] / self._like(self._cv_unit, b['cv'])).reshape(g + (self.n_cv,)),
+                   bias_energy=(b['V'] * self.E_to_eV).reshape(g),
+                   bias_forces=(b['F'] * self.F_to_eV_Ang).reshape(g + (self.n_atoms, 3)))
+        return out
+
+    def set_windows(self, centers, force_constants):
+        self._set_windows_raw(*self._raw_windows(centers, force_constants))
+        self.windows = self._window_arrays(centers, force_constants)
+
+    def run(self, n_steps, dt_fs, temperature_K, friction_per_fs, exchange_every=0, seed=0, stride=0):
+        kT = KB_EV * float(temperature_K) / self.E_to_eV
+        f = self._run_raw(n_steps, dt_fs, friction_per_fs, kT, exchange_every, seed, stride)
+        acc, att = f['n_accepted'], f['n_attempted']
+        ratio = acc.double() / att.clip(1).double() if hasattr(att, 'data_ptr') else acc / att.clip(1)
+        ratio[att == 0] = np.nan
+        out = {'walkers': f['walkers'].reshape(self._shape), 'n_accepted': acc, 'n_attempted': att, 'acceptance': ratio}
+        out.update(self._ase_frames(f))
+        if 'walker' in f:
+            nf = f['walker'].shape[0]
+            out['walker'] = f['walker'].reshape((nf,) + self._shape)
+            out['cv'] = (f['cv'] / self._like(self._cv_unit, f['cv'])).reshape((nf,) + self._shape + (self.n_cv,))
+            out['bias_energy'] = (f['bias'] * self.E_to_eV).reshape((nf,) + self._shape)
+        return out
+
+    def mbar(self, cv_frames, temperature_K, windows=None, tol=1e-10, max_iter=10000):
+        kT_eV = KB_EV * float(temperature_K)
+        c, k = self._raw_windows(*(windows if windows is not None else self.windows))
+        x = cv_frames
+        if tuple(x.shape[1:]) != self._shape + (self.n_cv,):
+            raise ValueError('cv_frames must be (n_frames, n_ladders, n_windows, n_cv) = (n, %d, %d, %d): %s'
+                             % (self._shape + (self.n_cv, tuple(x.shape))))
+        nf = int(x.shape[0])
+        x = x * self._like(self._cv_unit, x)
+        out = []
+        for l in range(self.n_ladders):
+            s = x[:, l].transpose(1, 0, 2) if not hasattr(x, 'data_ptr') else x[:, l].permute(1, 0, 2)
+            s = s.reshape(self.n_windows * nf, self.n_cv)
+            f, log_w, n_iter, resid = self._mbar_raw(s, [nf] * self.n_windows, self.E_to_eV / kT_eV, c, k, tol,
+                                                      max_iter)
+            out.append({'f': f * kT_eV, 'log_w': log_w.reshape(self.n_windows, nf).T, 'n_iter': n_iter,
+                        'resid': resid})
+        return out
+
+    def free_energy(self, cv_frames, bins, temperature_K, windows=None):
+        kT_eV = KB_EV * float(temperature_K)
+        edges = [np.asarray(_host(b), dtype=np.float64).ravel() for b in
+                 (bins if isinstance(bins, (tuple, list)) and np.ndim(bins[0]) == 1 else [bins])]
+        if not 1 <= len(edges) <= min(2, self.n_cv):
+            raise ValueError('free_energy takes bin edges along 1 or 2 CVs (at most n_cv = %d)' % self.n_cv)
+        x = np.asarray(_host(cv_frames), dtype=np.float64)
+        out = []
+        for r in self.mbar(cv_frames, temperature_K, windows):
+            w = np.exp(np.asarray(_host(r['log_w'])))  # (n_frames, n_windows)
+            h, _ = np.histogramdd(x[:, len(out)].reshape(-1, self.n_cv)[:, :len(edges)], bins=edges,
+                                  weights=w.reshape(-1))
+            with np.errstate(divide='ignore'):
+                F = np.where(h > 0, -kT_eV * np.log(np.where(h > 0, h, 1.0)), np.nan)
+            out.append(F - np.nanmin(F))
+        return self._like(np.array(out), cv_frames)
+
+
+def _host(x):
+    """a NumPy view of x (a CUDA tensor is copied to the host)"""
+    return x.detach().cpu().numpy() if hasattr(x, 'data_ptr') else x
 
 
 def _det3(a):

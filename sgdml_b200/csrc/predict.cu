@@ -111,8 +111,12 @@ struct PredictArgs {
   int use_ae;
   int D, M, S, Mpad;
   double sig;
-  // queries: virtual rows (b, p) prepared by k_query_rows
-  const double* Qg;     // (rows padded to BQ, DS)  q_{b,p}[e] = x_b[pinv_p[e]] - mu[e], zero padded
+  // queries: virtual rows (b, p), q_{b,p}[e] = x_b[pinv_p[e]] - mu[e], zero padded.  With xq, the kernel builds each
+  // Q tile itself (query_rows); without, the rows are in Qg / qqg already (k_desc_query_rows, the graph path)
+  const double* xq;     // (n_rows / S, D) query descriptors, or nullptr
+  const int* pinv;      // (S, D)
+  const double* mu;     // (D)
+  const double* Qg;     // (rows padded to BQ, DS)
   const double* qqg;    // (rows padded to BQ)      |q_{b,p}|^2
   int64_t n_rows;       // B*S virtual rows
   int64_t n_rows_pad;   // rows rounded up to BQ (stride between the per-split output planes)
@@ -217,6 +221,48 @@ __device__ __forceinline__ void bar_sync_named(int id, int n_threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n_threads) : "memory");
 }
 
+// ============================================================== query rows of the main kernel
+// query_row (below) for NR rows of one warp at once, with DS a compile-time constant (the main kernel's Q tile in shared
+// memory): all permutation indices are loaded first, then all descriptor entries, so that the gathers of the NR rows
+// overlap instead of waiting on one another.  Each row's entries and sum are those of query_row, bit for bit.
+template <int DS, int NR>
+__device__ __forceinline__ void query_rows(const double* const (&x)[NR], const int* const (&pi)[NR],
+                                           const double* __restrict__ mu, int D, const int (&row)[NR],
+                                           double* __restrict__ Qs, double* __restrict__ qq) {
+  constexpr int NI = (DS + 31) / 32;
+  const int lane = threadIdx.x & 31;
+  int idx[NR][NI];
+#pragma unroll
+  for (int r = 0; r < NR; ++r)
+#pragma unroll
+    for (int i = 0; i < NI; ++i) {
+      const int e = lane + 32 * i;
+      idx[r][i] = x[r] != nullptr && e < D ? pi[r][e] : -1;
+    }
+  double v[NR][NI];
+#pragma unroll
+  for (int r = 0; r < NR; ++r)
+#pragma unroll
+    for (int i = 0; i < NI; ++i) v[r][i] = idx[r][i] >= 0 ? x[r][idx[r][i]] - mu[lane + 32 * i] : 0.0;
+#pragma unroll
+  for (int r = 0; r < NR; ++r) {
+    double s = 0.0;
+#pragma unroll
+    for (int i = 0; i < NI; ++i) {
+      const int e = lane + 32 * i;
+      if (e < DS) {
+        Qs[row[r] * DS + e] = v[r][i];
+        s = fma(v[r][i], v[r][i], s);
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) qq[row[r]] = s;
+  }
+}
+
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+
 // ============================================================== main kernel
 template <class C>
 __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs p) {
@@ -236,9 +282,15 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
   const int lr = lane >> 2, lc = lane & 3;  // fragment row / k (or col pair) index
-  const int64_t r0 = (int64_t)blockIdx.x * C::BQ;
+  // Persistent CTAs: this one sweeps training tiles [t_begin, t_end) for query tiles blockIdx.x, blockIdx.x +
+  // gridDim.x, ...  The model tiles stream through the two stages without a break between sweeps: g counts every tile
+  // this CTA has consumed and alone sets each tile's stage and mbarrier phase.
+  const int64_t q_tiles = p.n_rows_pad / C::BQ;
   const int t_begin = (int)blockIdx.y * p.tiles_per_split;
-  const int n_tiles = min(p.Mpad / C::BM, t_begin + p.tiles_per_split);  // exclusive end of this CTA's range
+  const int t_end = min(p.Mpad / C::BM, t_begin + p.tiles_per_split);
+  const int n_sweep = t_end - t_begin;
+  const int n_qt = blockIdx.x < q_tiles ? (int)((q_tiles - 1 - blockIdx.x) / gridDim.x + 1) : 0;
+  const int g_end = n_qt * n_sweep;
   constexpr uint32_t STAGE_BYTES = (uint32_t)((2 * C::BM * C::DS + 3 * C::BM) * 8);
 
   if (tid == 0) {
@@ -249,9 +301,9 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
   }
   __syncthreads();
 
-  auto issue_tile = [&](int t) {
-    const int s = (t - t_begin) & 1;
-    const int64_t m0 = (int64_t)t * C::BM;
+  auto issue_tile = [&](int g) {
+    const int s = g & 1;
+    const int64_t m0 = (int64_t)(t_begin + g % n_sweep) * C::BM;
     mbar_arrive_expect_tx(&bars[s], STAGE_BYTES);
     bulk_g2s(Xs + s * C::BM * C::DS, p.Xc + m0 * C::DS, C::BM * C::DS * 8, &bars[s]);
     bulk_g2s(JAs + s * C::BM * C::DS, p.JA + m0 * C::DS, C::BM * C::DS * 8, &bars[s]);
@@ -259,20 +311,10 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
     bulk_g2s(xjas + s * C::BM, p.xja + m0, C::BM * 8, &bars[s]);
     bulk_g2s(aes + s * C::BM, p.ae + m0, C::BM * 8, &bars[s]);
   };
-  if (tid == 0) {
-    // the Q tile (BQ prepared virtual rows, contiguous) and its row norms: two bulk copies
-    mbar_arrive_expect_tx(&bars[2], (uint32_t)((C::BQ * C::DS + C::BQ) * 8));
-    bulk_g2s(Qs, p.Qg + r0 * C::DS, C::BQ * C::DS * 8, &bars[2]);
-    bulk_g2s(qq, p.qqg + r0, C::BQ * 8, &bars[2]);
-    issue_tile(t_begin);
-    if (!C::OB && t_begin + 1 < n_tiles) issue_tile(t_begin + 1);
+  if (tid == 0 && g_end > 0) {
+    issue_tile(0);
+    if (!C::OB && g_end > 1) issue_tile(1);
   }
-  if (tid < C::BQ) {
-    csum_s[tid] = 0.0;
-    E_s[tid] = 0.0;
-  }
-  __syncthreads();
-  mbar_wait(&bars[2], 0);
 
   // GEMM1 warp coordinates
   const int w1k = warp % C::W1K;
@@ -289,311 +331,353 @@ __global__ void __launch_bounds__(256, C::MINB) k_predict_main(const PredictArgs
   const int row2 = w2q * (C::TR2 * 16);
   const int dcol2 = w2d * (C::TD2 * 8);
 
-  double accG[C::TR2][C::TD2][4];
-#pragma unroll
-  for (int i = 0; i < C::TR2; ++i)
-#pragma unroll
-    for (int j = 0; j < C::TD2; ++j) accG[i][j][0] = accG[i][j][1] = accG[i][j][2] = accG[i][j][3] = 0.0;
-
-  // running row sums: split-k path -> per epilogue element; fused path -> per fragment row (g and g + 8 of each
-  // 16-row fragment; XK: the one half this warp transforms)
-  constexpr int NPART = !C::FUSED ? C::EPT : C::XK ? 1 : 2 * C::TR1;
-  double csum_part[NPART], E_part[NPART];
-#pragma unroll
-  for (int j = 0; j < NPART; ++j) csum_part[j] = E_part[j] = 0.0;
-
   MaternK mk;
   mk.sig = p.sig;
   mk.sig_inv = 1.0 / p.sig;
   mk.k_base = 5.0 / (3.0 * p.sig * p.sig * p.sig);  // predict.py:195 mat52_base_fact
   mk.k_c1 = mk.k_base * 5.0 / p.sig;                // ... times predict.py:196 diag_scale_fact
 
-  double* C1s = Ps;
-  double* C2s = Ps + C::BQ * C::CS;
-
-  for (int t = t_begin; t < n_tiles; ++t) {
-    const int s = (t - t_begin) & 1;
-    if constexpr (C::OB) {
-      C1s = Ps + s * 2 * C::BQ * C::CS;
-      C2s = C1s + C::BQ * C::CS;
+  int g = 0;
+  for (int qi = 0; qi < n_qt; ++qi) {
+    const int64_t r0 = (blockIdx.x + (int64_t)qi * gridDim.x) * C::BQ;
+    // Q tile: the previous sweep's epilogue has read Qs / qq, csum_s and E_s (barrier at the end of the sweep)
+    if (p.xq != nullptr) {
+      // one warp per row, the arithmetic of k_query_rows; then the descriptors of this CTA's next query tile go to L2,
+      // so that its build a sweep later does not wait on HBM
+      constexpr int NR = C::BQ / (C::NT / 32);
+      const double* xs[NR];
+      const int* ps[NR];
+      int rs[NR];
+#pragma unroll
+      for (int i = 0; i < NR; ++i) {
+        rs[i] = warp + i * (C::NT / 32);
+        const int64_t row = r0 + rs[i];
+        const int64_t b = row / p.S;
+        xs[i] = row < p.n_rows ? p.xq + b * p.D : nullptr;
+        ps[i] = p.pinv + (row - b * p.S) * p.D;
+      }
+      query_rows<C::DS, NR>(xs, ps, p.mu, p.D, rs, Qs, qq);
+      const int64_t n0 = r0 + (int64_t)gridDim.x * C::BQ;
+      if (qi + 1 < n_qt && n0 < p.n_rows) {
+        const char* lo = reinterpret_cast<const char*>(p.xq + n0 / p.S * p.D);
+        const char* hi = reinterpret_cast<const char*>(p.xq + (min(n0 + C::BQ, p.n_rows) - 1) / p.S * p.D + p.D);
+        for (const char* line = lo - (reinterpret_cast<uintptr_t>(lo) & 127) + tid * 128; line < hi; line += C::NT * 128)
+          prefetch_l2(line);
+      }
+    } else if (tid == 0) {
+      // the prepared rows (contiguous) and their norms: two bulk copies
+      mbar_arrive_expect_tx(&bars[2], (uint32_t)((C::BQ * C::DS + C::BQ) * 8));
+      bulk_g2s(Qs, p.Qg + r0 * C::DS, C::BQ * C::DS * 8, &bars[2]);
+      bulk_g2s(qq, p.qqg + r0, C::BQ * 8, &bars[2]);
     }
-    const double* Xt = Xs + s * C::BM * C::DS;
-    const double* JAt = JAs + s * C::BM * C::DS;
-    const double* mmt = mms + s * C::BM;
-    const double* xjat = xjas + s * C::BM;
-    const double* aet = aes + s * C::BM;
-    mbar_wait(&bars[s], (uint32_t)(((t - t_begin) >> 1) & 1));
-    // real training points in this tile.  GEMM1 skips the 8-point fragments of the zero-padded tail: their S1 / S2
-    // are exactly zero, as are the model rows, so the transform below turns them into c1 = 0 and a finite c2 that
-    // GEMM2 multiplies by zero rows.  GEMM2's k16 steps read every C1 / C2 column, and every one is written each tile.
-    const int mvalid = min(C::BM, p.M - t * C::BM);
+    if (tid < C::BQ) {
+      csum_s[tid] = 0.0;
+      E_s[tid] = 0.0;
+    }
+    __syncthreads();
+    if (p.xq == nullptr) mbar_wait(&bars[2], (uint32_t)(qi & 1));
 
-    // ---------------- GEMM1: S1 = Q Xc^T, S2 = Q JA^T (over this warp's k-range)
-    {
-      double a1[C::KI][C::TR1][C::TC1][4], a2[C::KI][C::TR1][C::TC1][4];
+    double accG[C::TR2][C::TD2][4];
 #pragma unroll
-      for (int c = 0; c < C::KI; ++c)
+    for (int i = 0; i < C::TR2; ++i)
 #pragma unroll
-        for (int i = 0; i < C::TR1; ++i)
-#pragma unroll
-          for (int j = 0; j < C::TC1; ++j)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) a1[c][i][j][e] = a2[c][i][j][e] = 0.0;
-      const double* qa = Qs + (row1 + lr) * C::DS + k1 + lc;
-      const double* xb = Xt + (col1 + lr) * C::DS + k1 + lc;
-      const double* jb = JAt + (col1 + lr) * C::DS + k1 + lc;
-      // one k-step of width KW at k0, into accumulation chain c: each Q fragment feeds 2 * TC1 MMAs
-      auto kstep = [&](auto kw, int k0, int c) {
-        constexpr int KW = decltype(kw)::value;
-        double fa[C::TR1][KW / 2], fx[C::TC1][KW / 4], fj[C::TC1][KW / 4];
-#pragma unroll
-        for (int i = 0; i < C::TR1; ++i) frag_a<KW>(fa[i], qa + i * 16 * C::DS + k0, C::DS);
-#pragma unroll
-        for (int j = 0; j < C::TC1; ++j) {
-          frag_b_rows<KW>(fx[j], xb + j * 8 * C::DS + k0);
-          frag_b_rows<KW>(fj[j], jb + j * 8 * C::DS + k0);
-        }
-#pragma unroll
-        for (int j = 0; j < C::TC1; ++j) {
-          if (j == 0 || col1 + j * 8 < mvalid) {  // warp-uniform
-#pragma unroll
-            for (int i = 0; i < C::TR1; ++i) {
-              mma_f64<KW>(a1[c][i][j], fa[i], fx[j]);
-              mma_f64<KW>(a2[c][i][j], fa[i], fj[j]);
-            }
-          }
-        }
-      };
-      if (col1 < mvalid) {  // warp-uniform
-#pragma unroll
-        for (int ks = 0; ks < C::KN1; ++ks) kstep(std::integral_constant<int, C::KW1>(), ks * C::KW1, ks % C::KI);
-        if constexpr (C::K8 == 1) kstep(std::integral_constant<int, 8>(), C::KN1 * C::KW1, C::KN1 % C::KI);
-      }
-      if constexpr (C::KI == 2) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          a1[0][0][0][e] += a1[1][0][0][e];
-          a2[0][0][0][e] += a2[1][0][0][e];
-        }
-      }
+      for (int j = 0; j < C::TD2; ++j) accG[i][j][0] = accG[i][j][1] = accG[i][j][2] = accG[i][j][3] = 0.0;
 
-      // Matern transform of the elements (r, mc), (r, mc + 1) (predict.py:199-217) into C1 / C2; part: row-sum slot
-      auto xform = [&](int r, int mc, double s1a, double s1b, double s2a, double s2b, int part) {
-        const double q5 = 5.0 * qq[r];
-        const double aa = s2a - xjat[mc], ab = s2b - xjat[mc + 1];
-        const double x5a = fma(-10.0, s1a, q5 + 5.0 * mmt[mc]), x5b = fma(-10.0, s1b, q5 + 5.0 * mmt[mc + 1]);
-        double c1a_, c2a_, c1b_, c2b_;
-        if (p.use_ae) {  // warp-uniform: models with energy constraints in the kernel
-          E_part[part] += matern52_ecstr(x5a, aa, aet[mc], mk, c1a_, c2a_);
-          E_part[part] += matern52_ecstr(x5b, ab, aet[mc + 1], mk, c1b_, c2b_);
-        } else {
-          matern52(x5a, aa, mk, c1a_, c2a_);
-          matern52(x5b, ab, mk, c1b_, c2b_);
-          E_part[part] = fma(aa, c2a_, fma(ab, c2b_, E_part[part]));
-        }
-        csum_part[part] += c1a_ + c1b_;
-        const int off = r * C::CS + mc;
-        *reinterpret_cast<double2*>(C1s + off) = make_double2(c1a_, c1b_);
-        *reinterpret_cast<double2*>(C2s + off) = make_double2(c2a_, c2b_);
-      };
-      if constexpr (C::W1K == 1) {
-        // fused: the transform straight on the accumulator fragments
+    // running row sums: split-k path -> per epilogue element; fused path -> per fragment row (g and g + 8 of each
+    // 16-row fragment; XK: the one half this warp transforms)
+    constexpr int NPART = !C::FUSED ? C::EPT : C::XK ? 1 : 2 * C::TR1;
+    double csum_part[NPART], E_part[NPART];
 #pragma unroll
-        for (int j = 0; j < C::TC1; ++j)
+    for (int j = 0; j < NPART; ++j) csum_part[j] = E_part[j] = 0.0;
+
+    double* C1s = Ps;
+    double* C2s = Ps + C::BQ * C::CS;
+
+    for (int t = t_begin; t < t_end; ++t, ++g) {
+      const int s = g & 1;
+      if constexpr (C::OB) {
+        C1s = Ps + s * 2 * C::BQ * C::CS;
+        C2s = C1s + C::BQ * C::CS;
+      }
+      const double* Xt = Xs + s * C::BM * C::DS;
+      const double* JAt = JAs + s * C::BM * C::DS;
+      const double* mmt = mms + s * C::BM;
+      const double* xjat = xjas + s * C::BM;
+      const double* aet = aes + s * C::BM;
+      mbar_wait(&bars[s], (uint32_t)((g >> 1) & 1));
+      // real training points in this tile.  GEMM1 skips the 8-point fragments of the zero-padded tail: their S1 / S2
+      // are exactly zero, as are the model rows, so the transform below turns them into c1 = 0 and a finite c2 that
+      // GEMM2 multiplies by zero rows.  GEMM2's k16 steps read every C1 / C2 column, and every one is written each tile.
+      const int mvalid = min(C::BM, p.M - t * C::BM);
+
+      // ---------------- GEMM1: S1 = Q Xc^T, S2 = Q JA^T (over this warp's k-range)
+      {
+        double a1[C::KI][C::TR1][C::TC1][4], a2[C::KI][C::TR1][C::TC1][4];
+#pragma unroll
+        for (int c = 0; c < C::KI; ++c)
 #pragma unroll
           for (int i = 0; i < C::TR1; ++i)
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
-              xform(row1 + i * 16 + h * 8 + lr, col1 + j * 8 + 2 * lc, a1[0][i][j][2 * h], a1[0][i][j][2 * h + 1],
-                    a2[0][i][j][2 * h], a2[0][i][j][2 * h + 1], 2 * i + h);
-      } else if constexpr (C::XK) {
-        // warp w1k = 0 finishes rows g (c0, c1), w1k = 1 rows g + 8 (c2, c3); each hands its partner the other half.
-        // One exchange area suffices: the partner reads it before the CTA-wide barrier of this tile, and it is next
-        // written after that barrier.
-        const double* f1 = a1[0][0][0];
-        const double* f2 = a2[0][0][0];
-        double* xs = smem + C::OFF_XCH + (warp >> 1) * 256;
-        double2* out = reinterpret_cast<double2*>(xs + w1k * 128);
-        const double2* in = reinterpret_cast<const double2*>(xs + (w1k ^ 1) * 128);
-        out[lane] = w1k ? make_double2(f1[0], f1[1]) : make_double2(f1[2], f1[3]);
-        out[32 + lane] = w1k ? make_double2(f2[0], f2[1]) : make_double2(f2[2], f2[3]);
-        bar_sync_named(1 + (warp >> 1), 64);
-        const double2 o1 = in[lane], o2 = in[32 + lane];
-        xform(row1 + 8 * w1k + lr, col1 + 2 * lc, (w1k ? f1[2] : f1[0]) + o1.x, (w1k ? f1[3] : f1[1]) + o1.y,
-              (w1k ? f2[2] : f2[0]) + o2.x, (w1k ? f2[3] : f2[1]) + o2.y, 0);
-      } else {
-        double* P1 = Ps + (w1k * 2 + 0) * C::BQ * C::CS;
-        double* P2 = Ps + (w1k * 2 + 1) * C::BQ * C::CS;
+            for (int j = 0; j < C::TC1; ++j)
 #pragma unroll
-        for (int i = 0; i < C::TR1; ++i)
+              for (int e = 0; e < 4; ++e) a1[c][i][j][e] = a2[c][i][j][e] = 0.0;
+        const double* qa = Qs + (row1 + lr) * C::DS + k1 + lc;
+        const double* xb = Xt + (col1 + lr) * C::DS + k1 + lc;
+        const double* jb = JAt + (col1 + lr) * C::DS + k1 + lc;
+        // one k-step of width KW at k0, into accumulation chain c: each Q fragment feeds 2 * TC1 MMAs
+        auto kstep = [&](auto kw, int k0, int c) {
+          constexpr int KW = decltype(kw)::value;
+          double fa[C::TR1][KW / 2], fx[C::TC1][KW / 4], fj[C::TC1][KW / 4];
+#pragma unroll
+          for (int i = 0; i < C::TR1; ++i) frag_a<KW>(fa[i], qa + i * 16 * C::DS + k0, C::DS);
+#pragma unroll
+          for (int j = 0; j < C::TC1; ++j) {
+            frag_b_rows<KW>(fx[j], xb + j * 8 * C::DS + k0);
+            frag_b_rows<KW>(fj[j], jb + j * 8 * C::DS + k0);
+          }
+#pragma unroll
+          for (int j = 0; j < C::TC1; ++j) {
+            if (j == 0 || col1 + j * 8 < mvalid) {  // warp-uniform
+#pragma unroll
+              for (int i = 0; i < C::TR1; ++i) {
+                mma_f64<KW>(a1[c][i][j], fa[i], fx[j]);
+                mma_f64<KW>(a2[c][i][j], fa[i], fj[j]);
+              }
+            }
+          }
+        };
+        if (col1 < mvalid) {  // warp-uniform
+#pragma unroll
+          for (int ks = 0; ks < C::KN1; ++ks) kstep(std::integral_constant<int, C::KW1>(), ks * C::KW1, ks % C::KI);
+          if constexpr (C::K8 == 1) kstep(std::integral_constant<int, 8>(), C::KN1 * C::KW1, C::KN1 % C::KI);
+        }
+        if constexpr (C::KI == 2) {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            a1[0][0][0][e] += a1[1][0][0][e];
+            a2[0][0][0][e] += a2[1][0][0][e];
+          }
+        }
+
+        // Matern transform of the elements (r, mc), (r, mc + 1) (predict.py:199-217) into C1 / C2; part: row-sum slot
+        auto xform = [&](int r, int mc, double s1a, double s1b, double s2a, double s2b, int part) {
+          const double q5 = 5.0 * qq[r];
+          const double aa = s2a - xjat[mc], ab = s2b - xjat[mc + 1];
+          const double x5a = fma(-10.0, s1a, q5 + 5.0 * mmt[mc]), x5b = fma(-10.0, s1b, q5 + 5.0 * mmt[mc + 1]);
+          double c1a_, c2a_, c1b_, c2b_;
+          if (p.use_ae) {  // warp-uniform: models with energy constraints in the kernel
+            E_part[part] += matern52_ecstr(x5a, aa, aet[mc], mk, c1a_, c2a_);
+            E_part[part] += matern52_ecstr(x5b, ab, aet[mc + 1], mk, c1b_, c2b_);
+          } else {
+            matern52(x5a, aa, mk, c1a_, c2a_);
+            matern52(x5b, ab, mk, c1b_, c2b_);
+            E_part[part] = fma(aa, c2a_, fma(ab, c2b_, E_part[part]));
+          }
+          csum_part[part] += c1a_ + c1b_;
+          const int off = r * C::CS + mc;
+          *reinterpret_cast<double2*>(C1s + off) = make_double2(c1a_, c1b_);
+          *reinterpret_cast<double2*>(C2s + off) = make_double2(c2a_, c2b_);
+        };
+        if constexpr (C::W1K == 1) {
+          // fused: the transform straight on the accumulator fragments
 #pragma unroll
           for (int j = 0; j < C::TC1; ++j)
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int off = (row1 + i * 16 + h * 8 + lr) * C::CS + col1 + j * 8 + 2 * lc;
-              *reinterpret_cast<double2*>(P1 + off) = make_double2(a1[0][i][j][2 * h], a1[0][i][j][2 * h + 1]);
-              *reinterpret_cast<double2*>(P2 + off) = make_double2(a2[0][i][j][2 * h], a2[0][i][j][2 * h + 1]);
+            for (int i = 0; i < C::TR1; ++i)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                xform(row1 + i * 16 + h * 8 + lr, col1 + j * 8 + 2 * lc, a1[0][i][j][2 * h], a1[0][i][j][2 * h + 1],
+                      a2[0][i][j][2 * h], a2[0][i][j][2 * h + 1], 2 * i + h);
+        } else if constexpr (C::XK) {
+          // warp w1k = 0 finishes rows g (c0, c1), w1k = 1 rows g + 8 (c2, c3); each hands its partner the other half.
+          // One exchange area suffices: the partner reads it before the CTA-wide barrier of this tile, and it is next
+          // written after that barrier.
+          const double* f1 = a1[0][0][0];
+          const double* f2 = a2[0][0][0];
+          double* xs = smem + C::OFF_XCH + (warp >> 1) * 256;
+          double2* out = reinterpret_cast<double2*>(xs + w1k * 128);
+          const double2* in = reinterpret_cast<const double2*>(xs + (w1k ^ 1) * 128);
+          out[lane] = w1k ? make_double2(f1[0], f1[1]) : make_double2(f1[2], f1[3]);
+          out[32 + lane] = w1k ? make_double2(f2[0], f2[1]) : make_double2(f2[2], f2[3]);
+          bar_sync_named(1 + (warp >> 1), 64);
+          const double2 o1 = in[lane], o2 = in[32 + lane];
+          xform(row1 + 8 * w1k + lr, col1 + 2 * lc, (w1k ? f1[2] : f1[0]) + o1.x, (w1k ? f1[3] : f1[1]) + o1.y,
+                (w1k ? f2[2] : f2[0]) + o2.x, (w1k ? f2[3] : f2[1]) + o2.y, 0);
+        } else {
+          double* P1 = Ps + (w1k * 2 + 0) * C::BQ * C::CS;
+          double* P2 = Ps + (w1k * 2 + 1) * C::BQ * C::CS;
+#pragma unroll
+          for (int i = 0; i < C::TR1; ++i)
+#pragma unroll
+            for (int j = 0; j < C::TC1; ++j)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int off = (row1 + i * 16 + h * 8 + lr) * C::CS + col1 + j * 8 + 2 * lc;
+                *reinterpret_cast<double2*>(P1 + off) = make_double2(a1[0][i][j][2 * h], a1[0][i][j][2 * h + 1]);
+                *reinterpret_cast<double2*>(P2 + off) = make_double2(a2[0][i][j][2 * h], a2[0][i][j][2 * h + 1]);
+              }
+        }
+      }
+      __syncthreads();
+      if constexpr (C::OB) {
+        if (tid == 0 && g + 1 < g_end) issue_tile(g + 1);
+      }
+
+      if constexpr (!C::FUSED) {
+        // ---------------- split-k: sum the partials, Matern transform in place
+#pragma unroll
+        for (int j = 0; j < C::EPT; ++j) {
+          const int e = tid + j * C::NT;
+          const int r = e / C::BM, mc = e % C::BM;
+          const int off = r * C::CS + mc;
+          double s1 = Ps[off], s2 = Ps[C::BQ * C::CS + off];
+#pragma unroll
+          for (int wk = 1; wk < C::W1K; ++wk) {
+            s1 += Ps[(wk * 2 + 0) * C::BQ * C::CS + off];
+            s2 += Ps[(wk * 2 + 1) * C::BQ * C::CS + off];
+          }
+          const double a = s2 - xjat[mc];
+          double c1, c2;
+          if (p.use_ae) {
+            E_part[j] += matern52_ecstr(fma(-10.0, s1, 5.0 * (qq[r] + mmt[mc])), a, aet[mc], mk, c1, c2);
+          } else {
+            matern52(fma(-10.0, s1, 5.0 * (qq[r] + mmt[mc])), a, mk, c1, c2);
+            E_part[j] = fma(a, c2, E_part[j]);
+          }
+          csum_part[j] += c1;
+          C1s[off] = c1;
+          C2s[off] = c2;
+        }
+        __syncthreads();
+      }
+
+      // ---------------- GEMM2: accG += C1 Xc + C2 JA (contraction over the BM points)
+      {
+        constexpr int KW = C::KW2;
+        const double* c1a = C1s + (row2 + lr) * C::CS + lc;
+        const double* c2a = C2s + (row2 + lr) * C::CS + lc;
+        const double* xb = Xt + lc * C::DS + dcol2 + lr;
+        const double* jb = JAt + lc * C::DS + dcol2 + lr;
+        if constexpr (C::W2S == 1) {
+#pragma unroll
+          for (int k0 = 0; k0 < C::BM; k0 += KW) {
+            double f1[C::TR2][KW / 2], f2[C::TR2][KW / 2];
+#pragma unroll
+            for (int i = 0; i < C::TR2; ++i) {
+              frag_a<KW>(f1[i], c1a + i * 16 * C::CS + k0, C::CS);
+              frag_a<KW>(f2[i], c2a + i * 16 * C::CS + k0, C::CS);
             }
+#pragma unroll
+            for (int j = 0; j < C::TD2; ++j) {
+              double fx[KW / 4], fj[KW / 4];
+              frag_b_cols<KW>(fx, xb + k0 * C::DS + j * 8, C::DS);
+              frag_b_cols<KW>(fj, jb + k0 * C::DS + j * 8, C::DS);
+#pragma unroll
+              for (int i = 0; i < C::TR2; ++i) {
+                mma_f64<KW>(accG[i][j], f1[i], fx);
+                mma_f64<KW>(accG[i][j], f2[i], fj);
+              }
+            }
+          }
+        } else {
+          const double* ca = w2s ? c2a : c1a;
+          const double* ob = w2s ? jb : xb;
+#pragma unroll
+          for (int k0 = 0; k0 < C::BM; k0 += KW) {
+            double f[C::TR2][KW / 2];
+#pragma unroll
+            for (int i = 0; i < C::TR2; ++i) frag_a<KW>(f[i], ca + i * 16 * C::CS + k0, C::CS);
+#pragma unroll
+            for (int j = 0; j < C::TD2; ++j) {
+              double fo[KW / 4];
+              frag_b_cols<KW>(fo, ob + k0 * C::DS + j * 8, C::DS);
+#pragma unroll
+              for (int i = 0; i < C::TR2; ++i) mma_f64<KW>(accG[i][j], f[i], fo);
+            }
+          }
+        }
+      }
+      if constexpr (!C::OB) {
+        __syncthreads();
+        if (tid == 0 && g + 2 < g_end) issue_tile(g + 2);
+      }
+    }
+
+    // ---- row sums csum[r] = sum_m c1, E[r] = sum_m a c2
+    if constexpr (!C::FUSED) {
+#pragma unroll
+      for (int j = 0; j < C::EPT; ++j) {
+        double cs = csum_part[j], es = E_part[j];
+#pragma unroll
+        for (int o = C::BM / 2; o > 0; o >>= 1) {
+          cs += __shfl_xor_sync(0xffffffffu, cs, o);
+          es += __shfl_xor_sync(0xffffffffu, es, o);
+        }
+        const int e = tid + j * C::NT;
+        if (e % C::BM == 0) {
+          csum_s[e / C::BM] = cs;
+          E_s[e / C::BM] = es;
+        }
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < NPART; ++i) {
+        double cs = csum_part[i], es = E_part[i];
+        cs += __shfl_xor_sync(0xffffffffu, cs, 1);
+        es += __shfl_xor_sync(0xffffffffu, es, 1);
+        cs += __shfl_xor_sync(0xffffffffu, cs, 2);
+        es += __shfl_xor_sync(0xffffffffu, es, 2);
+        const int r = C::XK ? row1 + 8 * w1k + lr : row1 + (i >> 1) * 16 + (i & 1) * 8 + lr;
+        if (lc == 0) {  // W1M warps share a row: csum_s / E_s were zeroed before the sweep
+          atomicAdd(&csum_s[r], cs);
+          atomicAdd(&E_s[r], es);
+        }
+      }
+    }
+    if constexpr (C::W2S == 2) {
+      if constexpr (C::OB) __syncthreads();  // GEMM2 of the last tile still reads C1 / C2
+      // the JA group parks its partial sums in the (now free) S/C region
+      if (w2s == 1) {
+#pragma unroll
+        for (int i = 0; i < C::TR2; ++i)
+#pragma unroll
+          for (int j = 0; j < C::TD2; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              *reinterpret_cast<double2*>(Ps + (row2 + i * 16 + h * 8 + lr) * C::DP + dcol2 + j * 8 + 2 * lc) =
+                  make_double2(accG[i][j][2 * h], accG[i][j][2 * h + 1]);
       }
     }
     __syncthreads();
-    if constexpr (C::OB) {
-      if (tid == 0 && t + 1 < n_tiles) issue_tile(t + 1);
-    }
 
-    if constexpr (!C::FUSED) {
-      // ---------------- split-k: sum the partials, Matern transform in place
+    // ---- G = (sum_m c1) Q - (C1 Xc + C2 JA)
+    if (C::W2S == 1 || w2s == 0) {
 #pragma unroll
-      for (int j = 0; j < C::EPT; ++j) {
-        const int e = tid + j * C::NT;
-        const int r = e / C::BM, mc = e % C::BM;
-        const int off = r * C::CS + mc;
-        double s1 = Ps[off], s2 = Ps[C::BQ * C::CS + off];
-#pragma unroll
-        for (int wk = 1; wk < C::W1K; ++wk) {
-          s1 += Ps[(wk * 2 + 0) * C::BQ * C::CS + off];
-          s2 += Ps[(wk * 2 + 1) * C::BQ * C::CS + off];
-        }
-        const double a = s2 - xjat[mc];
-        double c1, c2;
-        if (p.use_ae) {
-          E_part[j] += matern52_ecstr(fma(-10.0, s1, 5.0 * (qq[r] + mmt[mc])), a, aet[mc], mk, c1, c2);
-        } else {
-          matern52(fma(-10.0, s1, 5.0 * (qq[r] + mmt[mc])), a, mk, c1, c2);
-          E_part[j] = fma(a, c2, E_part[j]);
-        }
-        csum_part[j] += c1;
-        C1s[off] = c1;
-        C2s[off] = c2;
-      }
-      __syncthreads();
-    }
-
-    // ---------------- GEMM2: accG += C1 Xc + C2 JA (contraction over the BM points)
-    {
-      constexpr int KW = C::KW2;
-      const double* c1a = C1s + (row2 + lr) * C::CS + lc;
-      const double* c2a = C2s + (row2 + lr) * C::CS + lc;
-      const double* xb = Xt + lc * C::DS + dcol2 + lr;
-      const double* jb = JAt + lc * C::DS + dcol2 + lr;
-      if constexpr (C::W2S == 1) {
-#pragma unroll
-        for (int k0 = 0; k0 < C::BM; k0 += KW) {
-          double f1[C::TR2][KW / 2], f2[C::TR2][KW / 2];
-#pragma unroll
-          for (int i = 0; i < C::TR2; ++i) {
-            frag_a<KW>(f1[i], c1a + i * 16 * C::CS + k0, C::CS);
-            frag_a<KW>(f2[i], c2a + i * 16 * C::CS + k0, C::CS);
-          }
+      for (int ih = 0; ih < 2 * C::TR2; ++ih) {
+        const int i = ih >> 1, h = ih & 1;
+        const int r = row2 + i * 16 + h * 8 + lr;
+        const int64_t row = r0 + r;
+        if (row < p.n_rows) {
+          const double cs = csum_s[r];
 #pragma unroll
           for (int j = 0; j < C::TD2; ++j) {
-            double fx[KW / 4], fj[KW / 4];
-            frag_b_cols<KW>(fx, xb + k0 * C::DS + j * 8, C::DS);
-            frag_b_cols<KW>(fj, jb + k0 * C::DS + j * 8, C::DS);
-#pragma unroll
-            for (int i = 0; i < C::TR2; ++i) {
-              mma_f64<KW>(accG[i][j], f1[i], fx);
-              mma_f64<KW>(accG[i][j], f2[i], fj);
+            const int col = dcol2 + j * 8 + 2 * lc;
+            double g0 = cs * Qs[r * C::DS + col] - accG[i][j][2 * h];
+            double g1 = cs * Qs[r * C::DS + col + 1] - accG[i][j][2 * h + 1];
+            if constexpr (C::W2S == 2) {
+              const double2 o = *reinterpret_cast<const double2*>(Ps + r * C::DP + col);
+              g0 -= o.x;
+              g1 -= o.y;
             }
-          }
-        }
-      } else {
-        const double* ca = w2s ? c2a : c1a;
-        const double* ob = w2s ? jb : xb;
-#pragma unroll
-        for (int k0 = 0; k0 < C::BM; k0 += KW) {
-          double f[C::TR2][KW / 2];
-#pragma unroll
-          for (int i = 0; i < C::TR2; ++i) frag_a<KW>(f[i], ca + i * 16 * C::CS + k0, C::CS);
-#pragma unroll
-          for (int j = 0; j < C::TD2; ++j) {
-            double fo[KW / 4];
-            frag_b_cols<KW>(fo, ob + k0 * C::DS + j * 8, C::DS);
-#pragma unroll
-            for (int i = 0; i < C::TR2; ++i) mma_f64<KW>(accG[i][j], f[i], fo);
+            *reinterpret_cast<double2*>(p.G + ((int64_t)blockIdx.y * p.n_rows_pad + row) * C::DP + col) =
+                make_double2(g0, g1);
           }
         }
       }
     }
-    if constexpr (!C::OB) {
-      __syncthreads();
-      if (tid == 0 && t + 2 < n_tiles) issue_tile(t + 2);
-    }
+    if (tid < C::BQ && r0 + tid < p.n_rows) p.Erow[(int64_t)blockIdx.y * p.n_rows_pad + r0 + tid] = E_s[tid];
+    __syncthreads();  // the next sweep rewrites Qs, qq, csum_s, E_s and the S/C region
   }
-
-  // ---- row sums csum[r] = sum_m c1, E[r] = sum_m a c2
-  if constexpr (!C::FUSED) {
-#pragma unroll
-    for (int j = 0; j < C::EPT; ++j) {
-      double cs = csum_part[j], es = E_part[j];
-#pragma unroll
-      for (int o = C::BM / 2; o > 0; o >>= 1) {
-        cs += __shfl_xor_sync(0xffffffffu, cs, o);
-        es += __shfl_xor_sync(0xffffffffu, es, o);
-      }
-      const int e = tid + j * C::NT;
-      if (e % C::BM == 0) {
-        csum_s[e / C::BM] = cs;
-        E_s[e / C::BM] = es;
-      }
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < NPART; ++i) {
-      double cs = csum_part[i], es = E_part[i];
-      cs += __shfl_xor_sync(0xffffffffu, cs, 1);
-      es += __shfl_xor_sync(0xffffffffu, es, 1);
-      cs += __shfl_xor_sync(0xffffffffu, cs, 2);
-      es += __shfl_xor_sync(0xffffffffu, es, 2);
-      const int r = C::XK ? row1 + 8 * w1k + lr : row1 + (i >> 1) * 16 + (i & 1) * 8 + lr;
-      if (lc == 0) {  // W1M warps share a row: csum_s / E_s were zeroed before the sweep
-        atomicAdd(&csum_s[r], cs);
-        atomicAdd(&E_s[r], es);
-      }
-    }
-  }
-  if constexpr (C::W2S == 2) {
-    if constexpr (C::OB) __syncthreads();  // GEMM2 of the last tile still reads C1 / C2
-    // the JA group parks its partial sums in the (now free) S/C region
-    if (w2s == 1) {
-#pragma unroll
-      for (int i = 0; i < C::TR2; ++i)
-#pragma unroll
-        for (int j = 0; j < C::TD2; ++j)
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            *reinterpret_cast<double2*>(Ps + (row2 + i * 16 + h * 8 + lr) * C::DP + dcol2 + j * 8 + 2 * lc) =
-                make_double2(accG[i][j][2 * h], accG[i][j][2 * h + 1]);
-    }
-  }
-  __syncthreads();
-
-  // ---- G = (sum_m c1) Q - (C1 Xc + C2 JA)
-  if (C::W2S == 1 || w2s == 0) {
-#pragma unroll
-    for (int ih = 0; ih < 2 * C::TR2; ++ih) {
-      const int i = ih >> 1, h = ih & 1;
-      const int r = row2 + i * 16 + h * 8 + lr;
-      const int64_t row = r0 + r;
-      if (row < p.n_rows) {
-        const double cs = csum_s[r];
-#pragma unroll
-        for (int j = 0; j < C::TD2; ++j) {
-          const int col = dcol2 + j * 8 + 2 * lc;
-          double g0 = cs * Qs[r * C::DS + col] - accG[i][j][2 * h];
-          double g1 = cs * Qs[r * C::DS + col + 1] - accG[i][j][2 * h + 1];
-          if constexpr (C::W2S == 2) {
-            const double2 o = *reinterpret_cast<const double2*>(Ps + r * C::DP + col);
-            g0 -= o.x;
-            g1 -= o.y;
-          }
-          *reinterpret_cast<double2*>(p.G + ((int64_t)blockIdx.y * p.n_rows_pad + row) * C::DP + col) =
-              make_double2(g0, g1);
-        }
-      }
-    }
-  }
-  if (tid < C::BQ && r0 + tid < p.n_rows) p.Erow[(int64_t)blockIdx.y * p.n_rows_pad + r0 + tid] = E_s[tid];
 }
 
 // ============================================================== query rows
@@ -1374,16 +1458,26 @@ struct CfgInfo {
 const CfgInfo kCfgs[] = {{40, 64, 32}, {72, 64, 32}, {112, 64, 16}, {160, 32, 16}, {224, 32, 16}, {256, 32, 8}};
 const int kNumCfgs = 6;
 
+// As many CTAs as fit on the GPU at once, each sweeping query tiles blockIdx.x, blockIdx.x + gridDim.x, ...: a CTA's
+// pipeline fill and start-up are paid once per launch rather than once per query tile, and the model tiles of the
+// next sweep are in flight while the last one ends.  The schedule is static, so no row depends on which CTA ran it.
+// One CTA per query tile instead when the sweep over the training points is split (grid.y > 1, small batches), and
+// for the two-CTA class (D <= 40), where the other CTA on the SM already covers a CTA's fill and the persistent grid
+// measured slower.
 template <class C>
 int launch_main_t(const PredictArgs& a, int n_splits, cudaStream_t s) {
-  static bool configured[64] = {false};
+  static int resident[64] = {0};  // CTAs per SM
   int dev = 0;
   SG_CUDA(cudaGetDevice(&dev));
-  if (dev >= 0 && dev < 64 && !configured[dev]) {
+  int per_sm = dev >= 0 && dev < 64 ? resident[dev] : 0;
+  if (per_sm == 0) {
     SG_CUDA(cudaFuncSetAttribute(k_predict_main<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
-    configured[dev] = true;
+    SG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_predict_main<C>, C::NT, C::SMEM_BYTES));
+    if (per_sm < 1) return fail_arg("the predictor's main kernel does not fit on this device");
+    if (dev >= 0 && dev < 64) resident[dev] = per_sm;
   }
-  const int64_t grid = (a.n_rows + C::BQ - 1) / C::BQ;
+  const int64_t q_tiles = a.n_rows_pad / C::BQ;
+  const int64_t grid = n_splits > 1 || C::MINB > 1 ? q_tiles : std::min<int64_t>(q_tiles, (int64_t)num_sms() * per_sm);
   k_predict_main<C><<<dim3((unsigned)grid, (unsigned)n_splits), C::NT, C::SMEM_BYTES, s>>>(a);
   SG_CUDA(cudaGetLastError());
   return 0;
@@ -1594,7 +1688,8 @@ int tap(double* dst, const double* src, int64_t n, cudaStream_t s) {
 
 // Runs the predictor on n_geo queries whose descriptors (xq, gq) are on the device.
 constexpr int64_t GRAPH_MAX_GEO = 16;  // batches up to this size with host buffers replay a captured graph
-// xq == nullptr: the query rows (w.Qg, w.qq) are already in place (k_desc_query_rows)
+// xq == nullptr: the query rows (w.Qg, w.qq) are already in place (k_desc_query_rows); otherwise the fused kernel
+// builds them from xq itself, and only the GEMM-composed path (large descriptors) has k_query_rows write them
 // W_dev != nullptr: the finishing kernels' virial variants also write W (n_geo x 9); E and F are unchanged by it
 // w: one of the model's workspace slots, or a ForceEval's (predict.cuh)
 // taps != nullptr (sgdml_b200_predict_stages, large descriptors): each stage is also copied where taps points
@@ -1604,7 +1699,7 @@ int run_queries(sgdml_b200_model* m, sgdml_b200_model::WS& w, const double* xq, 
   const int64_t n_rows = n_geo * m->S;
   const int64_t n_rows_pad = (n_rows + m->BQ - 1) / m->BQ * m->BQ;
   int n_splits = 1;
-  if (xq != nullptr) {
+  if (xq != nullptr && m->large) {
     ProfScope ps(KID_PREDICT_AUX, s);
     k_query_rows<<<(unsigned)((n_rows_pad + 7) / 8), 256, 0, s>>>(xq, m->pinv, m->mu, m->D, m->DS, m->S, n_rows,
                                                                  n_rows_pad, w.Qg, w.qq);
@@ -1671,6 +1766,9 @@ int run_queries(sgdml_b200_model* m, sgdml_b200_model::WS& w, const double* xq, 
     a.S = m->S;
     a.Mpad = m->Mpad;
     a.sig = m->sig;
+    a.xq = xq;
+    a.pinv = m->pinv;
+    a.mu = m->mu;
     a.Qg = w.Qg;
     a.qqg = w.qq;
     a.n_rows = n_rows;

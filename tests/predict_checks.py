@@ -4,19 +4,32 @@ Plain functions on NumPy arrays, shared by the GPU tests (tests/test_predict_bul
 every check can fail (tests/test_predict_checks.py).  Each check raises AssertionError with a short diagnosis.
 
 `chunk_plan` restates how `sgdml_b200_predict` / `sgdml_b200_predict_train` cut a batch into chunks, so that the tests
-know which rows sit on chunk edges and how many main-kernel launches the engine must count.  `predict_abs_scale` and
-`check_predict` give a componentwise error bound for E and F.
+know which rows sit on chunk edges and how many main-kernel launches the engine must count.  `main_schedule` restates
+how one launch of the fused main kernel spreads its query tiles over persistent CTAs, so that the tests know which
+rows each CTA computes in which sweep.  `predict_abs_scale` and `check_predict` give a componentwise error bound for E
+and F.
 """
 
 import collections
+import math
 
 import numpy as np
 
 U = 2.0 ** -53
 
 # ------------------------------------------------------------------------------------------------ chunk plan
-# predictor tile configurations of csrc/predict.cu (kCfgs): (DP, BQ, BM); D > 256 runs the GEMM-composed path
-_CFGS = ((40, 64, 32), (72, 64, 32), (112, 64, 16), (160, 32, 16), (224, 32, 16), (256, 32, 8))
+# template arguments of the fused predictor's tile classes (csrc/predict.cu, the PCfg of each Cfg*), by padded
+# descriptor length DP: (BQ, BM, W1Q, W1M, W1K, W2Q, W2D, MINB, W2S, OB)
+PCFG = {
+    40: (64, 32, 4, 2, 1, 4, 1, 2, 2, 0),
+    72: (64, 32, 4, 2, 1, 4, 1, 1, 2, 1),
+    112: (64, 16, 4, 2, 1, 4, 2, 1, 1, 1),
+    160: (32, 16, 2, 2, 2, 2, 4, 1, 1, 1),
+    224: (32, 16, 2, 2, 2, 2, 4, 1, 1, 1),
+    256: (32, 8, 2, 1, 4, 2, 4, 1, 1, 0),
+}
+# (DP, BQ, BM) in kCfgs order; D > 256 runs the GEMM-composed path
+_CFGS = tuple((DP, c[0], c[1]) for DP, c in sorted(PCFG.items()))
 GRAPH_MAX_GEO = 16  # host-buffer batches up to this size replay a captured CUDA graph
 PIPELINE_MIN_GEO = 4096  # host-buffer batches from this size run on two side streams
 
@@ -75,6 +88,106 @@ def chunk_plan(D, DP, Mpad, S, large, B, host_io, cap=0, train=False):
 def edge_rows(plan):
     """First and last query of every chunk."""
     return sorted({r for lo, hi in plan.chunks for r in (lo, hi - 1)})
+
+
+# ------------------------------------------------------------------------------------------------ main-kernel schedule
+SM_SMEM = 228 * 1024  # shared memory per SM (H100)
+CTA_SMEM_RESERVED = 1024  # reserved by the system per resident CTA
+SM_THREADS = 2048
+NT = 256  # threads per CTA of k_predict_main
+
+Schedule = collections.namedtuple('Schedule', 'B S BQ q_tiles n_tiles n_splits tiles_per_split grid per_sm cta_tiles')
+
+
+def smem_bytes(DP):
+    """Dynamic shared memory of k_predict_main for the tile class of DP: PCfg's carve-up (SMEM_BYTES), in doubles
+    Q [BQ DS], Xc and JA [2][BM DS] each, mm / xja / ae [2][BM] each, the S / C tiles [OB ? 2 : 1][PK][2][BQ CS],
+    qq / csum / E [BQ] each, the XK exchange area and three mbarriers (4 doubles)."""
+    BQ, BM, W1Q, W1M, W1K, W2Q, W2D, MINB, W2S, OB = PCFG[DP]
+    DS, CS = DP + 4, BM + 4
+    XK = bool(OB) and W1K == 2
+    PK = 1 if XK else W1K
+    n = BQ * DS + 2 * (2 * BM * DS) + 3 * (2 * BM) + (2 if OB else 1) * PK * 2 * BQ * CS + 3 * BQ
+    n += (4 * 2 * 2 * 32 * 2 if XK else 0) + 4
+    return 8 * n
+
+
+def ctas_per_sm(DP):
+    """Resident CTAs of the class on one SM as its shared memory allows (256 threads each; no class is held to fewer
+    by its registers than by its shared memory)."""
+    return min(SM_SMEM // (smem_bytes(DP) + CTA_SMEM_RESERVED), SM_THREADS // NT)
+
+
+def main_schedule(N, M, S, B, n_sms, ws_geo=None):
+    """How one launch of k_predict_main runs B geometries (B S virtual rows (b, p)) on a GPU of n_sms SMs
+    (run_queries and launch_main_t in csrc/predict.cu):
+      q_tiles = ceil(B S / BQ) query tiles, n_tiles = Mpad / BM training tiles;
+      sp = ceil(2 n_sms / q_tiles), capped at the workspace rows over the batch's (ws_geo: the geometries the
+           workspace slot holds; None leaves this cap out -- it cannot matter when sp is 1 anyway), at
+           2 ceil(sqrt(2 n_tiles)) and at n_tiles, at least 1; the sweep is cut into n_splits = ceil(n_tiles / tps)
+           pieces of tps = ceil(n_tiles / sp) tiles;
+      grid = q_tiles with a split sweep or for the two-CTA class, otherwise min(q_tiles, n_sms per_sm) persistent CTAs;
+      CTA x runs query tiles x, x + grid, ... (cta_tiles[x]), one sweep over its training tiles each.
+    sp = 1 whatever the workspace when q_tiles >= 2 n_sms or n_tiles == 1."""
+    ly = layout(N, M)
+    assert not ly.large, 'the GEMM-composed path has no persistent main kernel'
+    BQ, BM = ly.BQ, ly.BM
+    MINB = PCFG[ly.DP][7]
+    q_tiles = -(-B * S // BQ)
+    n_rows_pad = q_tiles * BQ
+    n_tiles = ly.Mpad // BM
+    sp = -(-2 * n_sms // q_tiles)
+    if ws_geo is not None:
+        sp = min(sp, -(-ws_geo * S // BQ) * BQ // n_rows_pad)
+    sp = min(sp, 2 * math.ceil(math.sqrt(2.0 * n_tiles)))
+    sp = max(1, min(sp, n_tiles))
+    tps = -(-n_tiles // sp)
+    n_splits = -(-n_tiles // tps)
+    per_sm = ctas_per_sm(ly.DP)
+    grid = q_tiles if n_splits > 1 or MINB > 1 else min(q_tiles, n_sms * per_sm)
+    cta_tiles = [range(x, q_tiles, grid) for x in range(grid)]
+    return Schedule(B, S, BQ, q_tiles, n_tiles, n_splits, tps, grid, per_sm, cta_tiles)
+
+
+def batch_for_tiles(N, M, S, T):
+    """The smallest batch B with ceil(B S / BQ) == T query tiles whose last tile is partly padded (B S % BQ != 0)."""
+    BQ = layout(N, M).BQ
+    B = (T - 1) * BQ // S + 1
+    while -(-B * S // BQ) == T:
+        if B * S % BQ:
+            return B
+        B += 1
+    raise ValueError('no batch of %d tiles with a padded last tile (S = %d, BQ = %d)' % (T, S, BQ))
+
+
+def tile_geos(sched, t):
+    """The geometries with at least one of their S rows in query tile t."""
+    return range(t * sched.BQ // sched.S, min(sched.B, ((t + 1) * sched.BQ - 1) // sched.S + 1))
+
+
+def schedule_rows(sched, ctas):
+    """The geometries whose rows lie in the first or the last query tile of each CTA in `ctas`."""
+    out = set()
+    for x in ctas:
+        tiles = sched.cta_tiles[x]
+        if len(tiles):
+            for t in (tiles[0], tiles[-1]):
+                out.update(tile_geos(sched, t))
+    return sorted(out)
+
+
+def ragged_round_rows(sched):
+    """The geometries of the last round of query tiles when only some CTAs have a tile in it (else none)."""
+    if sched.q_tiles % sched.grid == 0:
+        return []
+    t0 = sched.q_tiles // sched.grid * sched.grid
+    return list(range(tile_geos(sched, t0)[0], sched.B))
+
+
+def straddling_geos(sched):
+    """The geometries whose S rows lie in two query tiles."""
+    b = np.arange(sched.B)
+    return b[b * sched.S // sched.BQ != ((b + 1) * sched.S - 1) // sched.BQ]
 
 
 def n_terms(M, S, D):

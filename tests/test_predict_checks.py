@@ -1,7 +1,9 @@
 """The acceptance checks of tests/predict_checks.py on CPU: the chunk plan against hand-computed plans, and the
 componentwise force / energy bound against the oracle -- on a plain, an energy-constrained and a periodic model it
 passes an independent FP64 evaluation and fails each injected defect of the kind a multi-chunk prediction could have,
-plus defects specific to energy constraints and to cells.  No GPU needed."""
+plus defects specific to energy constraints and to cells.  The persistent main kernel's schedule (main_schedule) against
+hand-computed schedules at 132 and 114 SMs, its tile classes against the kernel source, and the bound against the
+outputs of four schedule faults in one query tile.  No GPU needed."""
 
 import numpy as np
 import pytest
@@ -384,3 +386,188 @@ def test_desc_pbc_bound(pbc_case):
     assert np.all(np.abs(x - xl) <= bx / 10) and np.all(np.abs(g - gl) <= bg[..., None] / 10)
     x2, g2 = odesc.from_R(R, (lat * (1 + 1e-12), lat_inv))
     assert not np.all(np.abs(g2 - g) <= bg[..., None])
+
+
+# ------------------------------------------------------------------------------------------------ main-kernel schedule
+# dynamic shared memory of k_predict_main per tile class (PCfg::SMEM_BYTES): pinned, so that a change to a class's
+# carve-up shows here before the GPU tests' schedules move
+SMEM_BYTES = {40: 107552, 72: 193568, 112: 162080, 160: 156192, 224: 205344, 256: 158880}
+CLASS_N = {'c1': 12, 'c2': 15, 'c3': 18, 'c4': 21, 'c5': 23}  # one molecule size per persistent tile class
+
+
+def test_tile_classes_match_the_kernel_source():
+    """PCFG is what csrc/predict.cu instantiates (template defaults MINB = 1, W2S = 1, OB = 0), and kCfgs agrees."""
+    import os
+    import re
+
+    src = open(os.path.join(os.path.dirname(__file__), '..', 'sgdml_b200', 'csrc', 'predict.cu')).read()
+    found = {}
+    for args in re.findall(r'using Cfg\w+ = PCfg<([\d,\s]+)>;', src):
+        a = [int(v) for v in args.split(',')]
+        a += [1, 1, 0][len(a) - 8 :]
+        found[a[0]] = tuple(a[1:])
+    assert found == pc.PCFG
+    k = re.search(r'const CfgInfo kCfgs\[\] = \{(.*?)\};', src).group(1)
+    assert [tuple(int(v) for v in t) for t in re.findall(r'\{(\d+), (\d+), (\d+)\}', k)] == list(pc._CFGS)
+
+
+def test_shared_memory_and_residency():
+    assert {DP: pc.smem_bytes(DP) for DP in pc.PCFG} == SMEM_BYTES
+    assert all(b <= 232448 for b in SMEM_BYTES.values())
+    # 152 - 201 KiB: one CTA per SM for every persistent class, two for the D <= 40 class it is compiled for
+    assert {DP: pc.ctas_per_sm(DP) for DP in pc.PCFG} == {40: 2, 72: 1, 112: 1, 160: 1, 224: 1, 256: 1}
+
+
+def test_main_schedule_by_hand():
+    # aspirin's first device chunk on 132 SMs: 24 966 x 6 rows in 4 682 tiles of 32; 4 682 = 35 x 132 + 62
+    s = pc.main_schedule(21, 1000, 6, 24966, 132)
+    assert (s.q_tiles, s.n_tiles, s.n_splits, s.grid, s.per_sm) == (4682, 63, 1, 132, 1)
+    assert [len(s.cta_tiles[x]) for x in (0, 61, 62, 131)] == [36, 36, 35, 35]
+    assert list(s.cta_tiles[5][:3]) == [5, 137, 269]
+    # 37 geometries: ceil(264 / 7) = 38 splits wanted, 2 ceil(sqrt(126)) = 24 allowed, 3 tiles each: 21 pieces; a
+    # workspace of just 37 geometries holds one plane of partial sums, so the sweep stays whole
+    s = pc.main_schedule(21, 1000, 6, 37, 132)
+    assert (s.q_tiles, s.n_splits, s.tiles_per_split, s.grid) == (7, 21, 3, 7)
+    s = pc.main_schedule(21, 1000, 6, 37, 132, ws_geo=37)
+    assert (s.n_splits, s.grid) == (1, 7)
+    # the two-CTA class runs one CTA per query tile
+    s = pc.main_schedule(9, 200, 6, 65536, 132)
+    assert (s.q_tiles, s.n_splits, s.grid, s.per_sm) == (6144, 1, 6144, 2)
+    # class 3, 1 409 geometries: rows 0..31 are geometries 0..5 (5 straddles tiles 0 and 1); tile 264 holds the
+    # padded last row block (geometry 1 408, rows 8 448..8 453)
+    s = pc.main_schedule(18, 43, 6, 1409, 132)
+    assert (s.q_tiles, s.n_tiles, s.grid) == (265, 3, 132)
+    assert list(pc.tile_geos(s, 0)) == [0, 1, 2, 3, 4, 5] and list(pc.tile_geos(s, 1)) == list(range(5, 11))
+    assert pc.schedule_rows(s, [0]) == [0, 1, 2, 3, 4, 5, 1408]
+    assert pc.ragged_round_rows(s) == [1408]
+    assert list(pc.straddling_geos(s)[:4]) == [5, 10, 21, 26]
+
+
+@pytest.mark.parametrize('n_sms', [132, 114])
+@pytest.mark.parametrize('cls', sorted(CLASS_N))
+def test_multi_sweep_schedules(cls, n_sms):
+    """The schedules the persistent-kernel GPU tests run: S = 6, sweeps of 1, 3 and about 8 training tiles (M never a
+    multiple of BM), T = 2 grid, 2 grid + 1 and 3 grid - 1 query tiles with the last one padded."""
+    N, S = CLASS_N[cls], 6
+    BM = pc.layout(N, 100).BM
+    for n_tiles, M in ((1, BM - 3), (3, 3 * BM - 5), (8, 8 * BM - 5)):
+        grid = pc.main_schedule(N, M, S, 10 ** 6, n_sms).grid
+        assert grid == n_sms
+        for T, first, last in ((2 * grid, 2, 2), (2 * grid + 1, 3, 2), (3 * grid - 1, 3, 2)):
+            B = pc.batch_for_tiles(N, M, S, T)
+            s = pc.main_schedule(N, M, S, B, n_sms)
+            assert (s.q_tiles, s.n_tiles, s.n_splits, s.grid) == (T, n_tiles, 1, n_sms)
+            assert B * S % s.BQ != 0 and -(-(B - 1) * S // s.BQ) < T  # the smallest such batch
+            assert len(s.cta_tiles[0]) == first and len(s.cta_tiles[-1]) == last
+            assert min(len(t) for t in s.cta_tiles) >= 2
+            assert sorted(t for ts in s.cta_tiles for t in ts) == list(range(T))
+            # any workspace at least as large as the batch leaves the sweep whole
+            assert pc.main_schedule(N, M, S, B, n_sms, ws_geo=B).n_splits == 1
+            assert pc.main_schedule(N, M, S, B, n_sms, ws_geo=65536).n_splits == 1
+            rr = pc.ragged_round_rows(s)
+            n_ragged = T % grid
+            assert (len(rr) > 0) == (n_ragged > 0) and (not rr or rr[-1] == B - 1)
+            assert not rr or rr[0] == (T - n_ragged) * s.BQ // S
+    # one training tile: the sweep is whole even when a few query tiles leave most SMs idle
+    s = pc.main_schedule(N, BM - 3, S, 16, n_sms, ws_geo=16)
+    assert s.n_splits == 1 and s.grid == s.q_tiles
+
+
+def test_batch_for_tiles_edges():
+    # class 3 (BQ 32), S = 16: 2 geometries fill one tile exactly, so T = 1 needs B = 1 and T = 2 has only B = 3
+    assert pc.batch_for_tiles(18, 43, 16, 1) == 1
+    assert pc.batch_for_tiles(18, 43, 16, 2) == 3
+    # S = 32: every batch fills its tiles exactly
+    with pytest.raises(ValueError):
+        pc.batch_for_tiles(18, 43, 32, 5)
+
+
+# ------------------------------------------------------------------------------------------------ schedule faults
+# A class 3 shape (D = 153, BQ 32, BM 16) with a sweep of three training tiles (M = 43, the last tile 11 points) and
+# T = 2 grid + 1 query tiles at 132 SMs; query tile t = grid + 7 is the second sweep of CTA 7, and its geometries that
+# lie wholly inside it get the outputs a schedule fault would give all their rows.  The virtual row (b, p) of the
+# kernel pairs with the oracle's permuted cache rows m S + p (m = 0..M-1).
+FN, FM, FS, F_SMS = 18, 43, 6, 132
+
+
+@pytest.fixture(scope='module')
+def fault_case():
+    from test_predict_ecstr_pbc import _make, _queries
+
+    model, _, _ = _make(FN, FM, seed=FN, ecstr=True)
+    B = pc.batch_for_tiles(FN, FM, FS, 2 * F_SMS + 1)
+    s = pc.main_schedule(FN, FM, FS, B, F_SMS)
+    assert (s.n_tiles, s.n_splits, s.grid, s.BQ) == (3, 1, F_SMS, 32) and s.grid * s.BQ % FS == 0
+    t = s.grid + 7
+    geos = [b for b in pc.tile_geos(s, t) if b * FS // s.BQ == t == ((b + 1) * FS - 1) // s.BQ]
+    assert len(geos) >= 4
+    R = _queries(FN, B, 77)
+    op = opredict.Predictor(model)
+    E, F = op.predict(R[geos])
+    k = pc.n_terms(FM, FS, FN * (FN - 1) // 2)
+    scale = pc.predict_abs_scale(model, R[geos], oracle=op)
+    fc = dict(model=model, op=op, R=R, geos=geos, sched=s, E=E, F=F, k=k, scale=scale)
+    E0, F0 = _fault_predict(fc)  # no fault: the construction itself passes
+    pc.check_predict(E0, F0, E, F, scale, k)
+    return fc
+
+
+def _fault_predict(fc, keep=None, extra=None, ae=None, src=None):
+    """Oracle outputs of the fault case's geometries with the cache rows `keep` (then the rows `extra` once more),
+    alphas_E per cache row `ae`, or the query descriptors of geometries `src` under each geometry's own Jacobian."""
+    op = fc['op']
+    sub = opredict.Predictor(fc['model'])
+    idx = np.arange(op.R_desc_perms.shape[0]) if keep is None else keep
+    if extra is not None:
+        idx = np.concatenate([idx, extra])
+    sub.R_desc_perms = op.R_desc_perms[idx]
+    sub.R_d_desc_alpha_perms = op.R_d_desc_alpha_perms[idx]
+    sub.alphas_E_lin = (op.alphas_E_lin if ae is None else ae)[idx]
+    geos = fc['geos']
+    x, g = odesc.from_R(fc['R'][geos])
+    if src is not None:
+        x, _ = odesc.from_R(fc['R'][src])
+    E = np.array([sub._raw(xi, gi) for xi, gi in zip(x, g)])
+    return E[:, 0] * op.std + op.c, E[:, 1:] * op.std
+
+
+def _tile_cache_rows(j):
+    """The oracle's cache rows m S + p of training tile j (all S permutations)."""
+    BM = pc.layout(FN, FM).BM
+    m = np.arange(j * BM, min((j + 1) * BM, FM))
+    return (m[:, None] * FS + np.arange(FS)[None]).ravel()
+
+
+def _rejects(fc, E, F):
+    assert not np.array_equal(F, fc['F'])
+    with pytest.raises(AssertionError, match='force entries'):
+        pc.check_predict(E, F, fc['E'], fc['F'], fc['scale'], fc['k'])
+    with pytest.raises(AssertionError, match='energies'):
+        pc.check_predict(E, fc['F'], fc['E'], fc['F'], fc['scale'], fc['k'])
+
+
+def test_schedule_fault_dropped_training_tile_fails(fault_case):
+    n = FM * FS
+    for j in range(3):
+        _rejects(fault_case, *_fault_predict(fault_case, keep=np.setdiff1d(np.arange(n), _tile_cache_rows(j))))
+
+
+def test_schedule_fault_training_tile_twice_fails(fault_case):
+    for j in range(3):
+        _rejects(fault_case, *_fault_predict(fault_case, extra=_tile_cache_rows(j)))
+
+
+def test_schedule_fault_previous_sweeps_query_tile_fails(fault_case):
+    """Tile t - grid's Q rows in place of tile t's: grid BQ rows back is grid BQ / S whole geometries back, with the
+    same permutation in each row."""
+    s = fault_case['sched']
+    shift = s.grid * s.BQ // FS
+    _rejects(fault_case, *_fault_predict(fault_case, src=[b - shift for b in fault_case['geos']]))
+
+
+def test_schedule_fault_neighbouring_alphas_E_fails(fault_case):
+    """Training tile 0 paired with the alphas_E of tile 1 (the aes stage of the other pipeline stage)."""
+    op = fault_case['op']
+    ae = op.alphas_E_lin.copy()
+    ae[_tile_cache_rows(0)] = op.alphas_E_lin[_tile_cache_rows(1)]
+    _rejects(fault_case, *_fault_predict(fault_case, ae=ae))

@@ -137,6 +137,43 @@ int sgdml_b200_predict_virial_cells(sgdml_b200_model* model, const double* R, in
 int sgdml_b200_predict_hvp(sgdml_b200_model* model, const double* R, const double* V, int64_t n_geo,
                            double* HV, void* stream);
 
+/* Extension: the energy Hessian H = d^2E/dR^2 = -dF/dR of every geometry, in the model's units and cell, FP64 always.
+ *   R (B, 3N) -> H (B, 3N, 3N) row-major; host or device as in sgdml_b200_predict.
+ * Column i of H[b] equals -sgdml_b200_predict_hvp(R[b], e_i) bit for bit (e_i the i-th unit vector): it is that
+ * product's arithmetic with the S query rows of a geometry built once and shared by its 3N tangent rows J e_i.  H is
+ * returned as computed, not symmetrised.  Energy-constrained models (alphas_E) and every descriptor size are covered.
+ * Workspace: separate from sgdml_b200_predict's and sgdml_b200_predict_hvp's, within ~2 GB.  A chunk holds whole
+ * geometries when (1 + 3N) S stacked rows fit; otherwise one geometry whose 3N columns run in blocks of consecutive
+ * directions.  sgdml_b200_set_predict_chunk(c), c > 0, caps a chunk at 2 c S rows: floor(2 c / (3N + 1)) geometries,
+ * or, when that is 0, one geometry in blocks of 2 c - 1 directions (c = 1: one column per block).  A rejected call
+ * writes nothing. */
+int sgdml_b200_predict_hessian(sgdml_b200_model* model, const double* R, int64_t n_geo, double* H, void* stream);
+
+/* ---------------------------------------------------------------- normal modes (csrc/vib.cu)
+ * Extension: the mass-weighted Hessian of n_geo geometries with the rigid modes moved to the top of its spectrum.
+ *   H (B, n, n), n = 3 n_atoms, in any consistent units; R (B, n); inv_sqrt_mass (n_atoms,) = m^-1/2 per atom
+ *   -> Hp (B, n, n), n_rigid (B,) int64.  DEVICE pointers only; Hp must not alias H.
+ * Hm = M^-1/2 (H + H^T) / 2 M^-1/2.  The rigid basis B holds, in mass-weighted coordinates, the 3 translations and,
+ * unless periodic != 0, the 3 rotations about the centre of mass, orthonormalised by two Gram-Schmidt passes in the
+ * order tx, ty, tz, rx, ry, rz; a vector that keeps less than 1e-6 of its norm is dropped (a linear geometry keeps 2
+ * rotations, a single atom none).  n_rigid is the number kept.  Then
+ *   Hp = P Hm P + c B B^T,  P = I - B B^T,  c = 2 |Hm|_inf + 1,
+ * exactly symmetric.  Every eigenvalue of P Hm P is below c, so the n_rigid largest eigenpairs of Hp are the rigid
+ * modes (eigenvalue c) and the others are the vibrations, orthogonal to every rigid mode.  Synchronises the stream. */
+int sgdml_b200_vib_project(const double* H, const double* R, const double* inv_sqrt_mass, int64_t n_geo,
+                           int64_t n_atoms, int periodic, double* Hp, int64_t* n_rigid, void* stream);
+
+/* Extension: eigenvalues (ascending) and orthonormal eigenvectors of n_geo symmetric n x n matrices, n <= the cap
+ * SGDML_B200_SYMEIG_MAX_N (sgdml_b200_symeig_max_n).
+ *   A (B, n, n) -> w (B, n), V (B, n, n) row-major with the eigenvectors as columns.  DEVICE pointers only; V must not
+ *   alias A, which is read only.
+ * Parallel cyclic Jacobi, one CTA per matrix, A in shared memory: sweeps of round-robin rotations until a sweep rotates
+ * no pair, where a pair is rotated when |a_pq| > eps |A|_F / n (at most 60 sweeps).  Ties in w keep index order.  No
+ * atomics and fixed reduction orders: the same bits on every call.  Stream-ordered, no synchronisation. */
+#define SGDML_B200_SYMEIG_MAX_N 160
+int sgdml_b200_symeig_batched(const double* A, int64_t n, int64_t n_geo, double* w, double* V, void* stream);
+int sgdml_b200_symeig_max_n(void);
+
 /* ---------------------------------------------------------------- molecular dynamics on the device
  * Extension: BAOAB Langevin (velocity Verlet at gamma = 0) trajectories of n_rep replicas of one model, many steps per
  * call.  Positions, velocities and forces stay in device memory between steps and between calls; one step is the
@@ -544,7 +581,8 @@ int sgdml_b200_predict_train_virial(sgdml_b200_model* model, int64_t m_begin, in
 int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* model, int slices, void* stream);
 
 /* Test hook: at most max_geos queries (or training points) per chunk of sgdml_b200_predict,
- * sgdml_b200_predict_train and sgdml_b200_predict_hvp, for every model; 0 = no cap (the default: chunks bounded by workspace size only).  Negative
+ * sgdml_b200_predict_train and sgdml_b200_predict_hvp, for every model, and 2 max_geos S rows per chunk of
+ * sgdml_b200_predict_hessian (see there); 0 = no cap (the default: chunks bounded by workspace size only).  Negative
  * values are rejected.  The cap also bounds the minimum per-batch workspace, which limits how far small batches split
  * the sweep over the training points.  Workspaces never shrink: it applies fully to models created after the call.
  * Tests lower it to cover the multi-chunk, pipelined and tail-chunk paths at small batch sizes. */

@@ -14,3 +14,4 @@ from .md import (GDMLNEB, GDMLDimer, GDMLDynamics, GDMLMetadynamics, GDMLNPTDyna
 from .perm import find_perms  # noqa: F401
 from .predict import GDMLPredict  # noqa: F401
 from .train import GDMLTrain  # noqa: F401
+from .vib import GDMLVibrations, harmonic_rate, thermo  # noqa: F401

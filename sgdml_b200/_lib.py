@@ -41,6 +41,10 @@ SIGNATURES = {
     'sgdml_b200_predict_virial_cells': (
         C.c_int, [c_void_p, c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_predict_hvp': (C.c_int, [c_void_p, c_void_p, c_void_p, i64, c_void_p, c_void_p]),
+    'sgdml_b200_predict_hessian': (C.c_int, [c_void_p, c_void_p, i64, c_void_p, c_void_p]),
+    'sgdml_b200_vib_project': (C.c_int, [c_void_p, c_void_p, c_void_p, i64, i64, C.c_int, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_symeig_batched': (C.c_int, [c_void_p, i64, i64, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_symeig_max_n': (C.c_int, []),
     'sgdml_b200_md_create': (C.c_int, [C.POINTER(c_void_p), c_void_p, i64, c_void_p]),
     'sgdml_b200_md_destroy': (C.c_int, [c_void_p]),
     'sgdml_b200_md_set_state': (C.c_int, [c_void_p, c_void_p, c_void_p, C.c_uint64, c_void_p]),

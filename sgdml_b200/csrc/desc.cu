@@ -58,11 +58,7 @@ __global__ void k_d_desc_dot_vec(const double* __restrict__ R_d_desc, const doub
   int a, b;
   pair_from_d(d, a, b);
   const double* v = vecs + g * 3 * n_atoms;
-  const double* gd = R_d_desc + idx * 3;
-  double s = gd[0] * (v[3 * b + 0] - v[3 * a + 0]);
-  s += gd[1] * (v[3 * b + 1] - v[3 * a + 1]);
-  s += gd[2] * (v[3 * b + 2] - v[3 * a + 2]);
-  out[g * out_stride + d] = s;
+  out[g * out_stride + d] = d_desc_dot(R_d_desc + idx * 3, a, b, [v](int i) { return v[i]; });
 }
 
 // ---------------------------------------------------------------- a-D4: J^T w

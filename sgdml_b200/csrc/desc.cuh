@@ -46,6 +46,16 @@ __device__ __forceinline__ void minimum_image(const Lattice& lat, double& dx, do
   dz -= dot3(lat.vec[6], lat.vec[7], lat.vec[8], c0, c1, c2);
 }
 
+// (J v)_d = g_d . (v_b - v_a) for pair d = (a, b), v read through v(i): k_d_desc_dot_vec's arithmetic, also the tangent
+// rows of sgdml_b200_predict_hessian (v = e_i, where every product is exact)
+template <class VecAt>
+__device__ __forceinline__ double d_desc_dot(const double* gd, int a, int b, VecAt v) {
+  double s = gd[0] * (v(3 * b + 0) - v(3 * a + 0));
+  s += gd[1] * (v(3 * b + 1) - v(3 * a + 1));
+  s += gd[2] * (v(3 * b + 2) - v(3 * a + 2));
+  return s;
+}
+
 // host-side launchers defined in desc.cu (device pointers only), reused by predict.cu
 // lats_dev == nullptr: every geometry in the cell `lat` (passed by value); otherwise geometry g in lats_dev[g], n_geo
 // cells in DEVICE memory

@@ -1250,28 +1250,46 @@ __global__ void k_unpad_rows(const double* __restrict__ src, int M, int D, int D
 // evaluated as is.  The forward c1, c2 need no floor: they multiply, never divide by n.
 constexpr double HVP_X5_FLOOR = 5.0 * 64.0 * 2.220446049250313e-16;
 
-// One warp per virtual row r < n_rows: S1 -> C1, S2 -> C2 in rows r, S3 -> dC1, S4 -> dC2 in rows n_rows + r (in place);
-// csum[r] = sum_m c1, csum[n_rows + r] = sum_m dc1.  Qg holds the query rows, then the tangent rows.
+// Which rows k_transform_tangent_rows and k_combine_tangent_rows serve.  Query rows come first (n_rows of them), then the
+// tangent rows.  The tangent rows of one geometry are laid out [direction][permutation], so tangent row t belongs to
+// query row (t / dir_rows) S + t % S with dir_rows = directions x S (the HVP has one direction: t serves query row t).
+//   TAN_PAIRED: the HVP: warp w takes query row w and tangent row w together, C1 / C2 overwrite S1 / S2 in place
+//   TAN_ONLY:   tangent rows only; they read their query row's S1 / S2, which stay in place for the other tangent rows
+//   TAN_QUERY:  query rows only (after TAN_ONLY, when one query row serves many tangent rows)
+enum TanMode { TAN_PAIRED = 0, TAN_ONLY = 1, TAN_QUERY = 2 };
+
+__device__ __forceinline__ int64_t tangent_query_row(int64_t t, int64_t dir_rows, int S) {
+  return (t / dir_rows) * S + t % S;
+}
+
+// One warp per work row w < n_work: S1 -> C1, S2 -> C2 in query row r, S3 -> dC1, S4 -> dC2 in tangent row n_rows + t
+// (in place); csum[r] = sum_m c1, csum[n_rows + t] = sum_m dc1.  Qg holds the query rows, then the tangent rows.
+template <int MODE>
 __global__ void __launch_bounds__(256) k_transform_tangent_rows(double* __restrict__ SX, double* __restrict__ SJ,
                                                                 int64_t ldS, const double* __restrict__ Qg, int DS,
                                                                 const double* __restrict__ qq,
                                                                 const double* __restrict__ mm,
                                                                 const double* __restrict__ xja,
                                                                 const double* __restrict__ ae, int M, int Mpad,
-                                                                int64_t n_rows, MaternK mk, double* __restrict__ csum) {
+                                                                int64_t n_rows, int64_t n_work, int64_t dir_rows, int S,
+                                                                MaternK mk, double* __restrict__ csum) {
   const int lane = threadIdx.x & 31;
-  const int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (r >= n_rows) return;
+  const int64_t w = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (w >= n_work) return;
+  const int64_t r = MODE == TAN_ONLY ? tangent_query_row(w, dir_rows, S) : w;
+  const int64_t tr = n_rows + w;  // the tangent row (not read by TAN_QUERY)
   const double* q = Qg + r * DS;
-  const double* t = Qg + (n_rows + r) * DS;
+  const double* t = Qg + tr * DS;
   double qt = 0.0;
-  for (int e = lane; e < DS; e += 32) qt = fma(q[e], t[e], qt);
+  if constexpr (MODE != TAN_QUERY) {
+    for (int e = lane; e < DS; e += 32) qt = fma(q[e], t[e], qt);
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) qt += __shfl_xor_sync(0xffffffffu, qt, o);
+    for (int o = 16; o > 0; o >>= 1) qt += __shfl_xor_sync(0xffffffffu, qt, o);
+  }
   double* s1 = SX + r * ldS;
   double* s2 = SJ + r * ldS;
-  double* s3 = SX + (n_rows + r) * ldS;
-  double* s4 = SJ + (n_rows + r) * ldS;
+  double* s3 = SX + tr * ldS;
+  double* s4 = SJ + tr * ldS;
   const double qqr = qq[r];
   const double q5 = 5.0 * qqr;
   const double k_dc2 = -5.0 * mk.k_base * mk.sig_inv;
@@ -1287,10 +1305,12 @@ __global__ void __launch_bounds__(256) k_transform_tangent_rows(double* __restri
       const double e = exp_neg(nrm * mk.sig_inv);
       c2 = (e * mk.k_base) * (nrm + mk.sig);
       c1 = a * (e * mk.k_c1);
-      const double ds = qt - s3[m];
-      const double inv_nf = rsqrt(fmax(x5, fmax(HVP_X5_FLOOR * (qqr + mm[m]), 1e-300)));
-      dc2 = k_dc2 * e * ds;
-      dc1 = (e * mk.k_c1) * (s4[m] - k_ads * a * ds * inv_nf);
+      if constexpr (MODE != TAN_QUERY) {
+        const double ds = qt - s3[m];
+        const double inv_nf = rsqrt(fmax(x5, fmax(HVP_X5_FLOOR * (qqr + mm[m]), 1e-300)));
+        dc2 = k_dc2 * e * ds;
+        dc1 = (e * mk.k_c1) * (s4[m] - k_ads * a * ds * inv_nf);
+      }
       if (ae != nullptr) {
         c1 = fma(ae[m], c2, c1);
         dc1 = fma(ae[m], dc2, dc1);
@@ -1298,10 +1318,14 @@ __global__ void __launch_bounds__(256) k_transform_tangent_rows(double* __restri
       cs += c1;
       dcs += dc1;
     }
-    s1[m] = c1;
-    s2[m] = c2;
-    s3[m] = dc1;
-    s4[m] = dc2;
+    if constexpr (MODE != TAN_ONLY) {
+      s1[m] = c1;
+      s2[m] = c2;
+    }
+    if constexpr (MODE != TAN_QUERY) {
+      s3[m] = dc1;
+      s4[m] = dc2;
+    }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -1309,51 +1333,50 @@ __global__ void __launch_bounds__(256) k_transform_tangent_rows(double* __restri
     dcs += __shfl_xor_sync(0xffffffffu, dcs, o);
   }
   if (lane == 0) {
-    csum[r] = cs;
-    csum[n_rows + r] = dcs;
+    if constexpr (MODE != TAN_ONLY) csum[r] = cs;
+    if constexpr (MODE != TAN_QUERY) csum[tr] = dcs;
   }
 }
 
-// acc (2 n_rows x DP) = [C1; dC1] XcT^T + [C2; dC2] JAT^T  ->  G = (sum c1) q - acc, dG = (sum dc1) q + (sum c1) T - acc
+// acc = [C1; dC1] XcT^T + [C2; dC2] JAT^T  ->  G = (sum c1) q - acc in query rows, dG = (sum dc1) q + (sum c1) T - acc
+// in tangent rows; one thread per entry of the n_work rows (rows as in k_transform_tangent_rows<MODE>)
+template <int MODE>
 __global__ void k_combine_tangent_rows(const double* __restrict__ Qg, int64_t ldq, const double* __restrict__ csum,
-                                       double* __restrict__ G, int DP, int64_t n_rows) {
+                                       double* __restrict__ G, int DP, int64_t n_rows, int64_t n_work,
+                                       int64_t dir_rows, int S) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n_rows * DP) return;
-  const int64_t r = idx / DP;
-  const int d = (int)(idx - r * DP);
-  const double q = Qg[r * ldq + d], t = Qg[(n_rows + r) * ldq + d];
+  if (idx >= n_work * DP) return;
+  const int64_t w = idx / DP;
+  const int d = (int)(idx - w * DP);
+  const int64_t r = MODE == TAN_ONLY ? tangent_query_row(w, dir_rows, S) : w;
+  const double q = Qg[r * ldq + d];
   const double cs = csum[r];
-  G[idx] = cs * q - G[idx];
-  double* dG = G + n_rows * DP;
-  dG[idx] = fma(csum[n_rows + r], q, cs * t) - dG[idx];
+  if constexpr (MODE != TAN_ONLY) G[r * DP + d] = cs * q - G[r * DP + d];
+  if constexpr (MODE != TAN_QUERY) {
+    const int64_t tr = n_rows + w;
+    const double t = Qg[tr * ldq + d];
+    G[tr * DP + d] = fma(csum[tr], q, cs * t) - G[tr * DP + d];
+  }
 }
 
-// One thread per (geometry, atom k):  HV[k] = std sum_d s_kd (g_d dF_desc[d] + dg_d F_desc[d]), s_kd = +1 for atom b
-// and -1 for atom a of pair d = (a, b), a > b (the signs of k_vec_dot_d_desc), where
+// Row k of HV for one geometry (k_hvp_project), V read through v(i):  HV[k] = sum_d s_kd (g_d dF_desc[d] + dg_d
+// F_desc[d]), s_kd = +1 for atom b and -1 for atom a of pair d = (a, b), a > b (the signs of k_vec_dot_d_desc), where
 //   dg_d = d(delta / |delta|^3) = dd / |delta|^3 - 3 delta (delta . dd) / |delta|^5,   dd = v_a - v_b,
 // with the minimum-image pair vector delta rebuilt from g_d as the virial kernels do (|g| = |delta|^-2):
 //   dg_d = |g|^3/2 dd - 3 (g . dd) g / |g|^1/2.
-__global__ void __launch_bounds__(256) k_hvp_project(const double* __restrict__ Fd, const double* __restrict__ dFd,
-                                                     const double* __restrict__ gq, const double* __restrict__ V,
-                                                     int n_atoms, int D, double std, int64_t n_geo,
-                                                     double* __restrict__ HV) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n_geo * n_atoms) return;
-  const int64_t b = idx / n_atoms;
-  const int k = (int)(idx - b * n_atoms);
-  const double* v = V + b * 3 * n_atoms;
-  const double* f = Fd + b * D;
-  const double* df = dFd + b * D;
-  const double* g = gq + b * (int64_t)D * 3;
-  double h0 = 0.0, h1 = 0.0, h2 = 0.0;
+template <class VecAt>
+__device__ __forceinline__ void hvp_atom(const double* __restrict__ f, const double* __restrict__ df,
+                                         const double* __restrict__ g, VecAt v, int n_atoms, int k, double& h0,
+                                         double& h1, double& h2) {
+  h0 = 0.0, h1 = 0.0, h2 = 0.0;
   for (int o = 0; o < n_atoms; ++o) {
     if (o == k) continue;
     const int pa = max(o, k), pb = min(o, k);
     const int d = pair_index(pa, pb);
     const double gx = g[d * 3 + 0], gy = g[d * 3 + 1], gz = g[d * 3 + 2];
-    const double ddx = v[3 * pa + 0] - v[3 * pb + 0];
-    const double ddy = v[3 * pa + 1] - v[3 * pb + 1];
-    const double ddz = v[3 * pa + 2] - v[3 * pb + 2];
+    const double ddx = v(3 * pa + 0) - v(3 * pb + 0);
+    const double ddy = v(3 * pa + 1) - v(3 * pb + 1);
+    const double ddz = v(3 * pa + 2) - v(3 * pb + 2);
     const double gn = sqrt(gx * gx + gy * gy + gz * gz);
     const double sgn = sqrt(gn);
     const double fv = f[d], dfv = df[d];
@@ -1364,9 +1387,79 @@ __global__ void __launch_bounds__(256) k_hvp_project(const double* __restrict__ 
     h1 += s * fma(cg, gy, cd * ddy);
     h2 += s * fma(cg, gz, cd * ddz);
   }
+}
+
+// One thread per (geometry, atom k)
+__global__ void __launch_bounds__(256) k_hvp_project(const double* __restrict__ Fd, const double* __restrict__ dFd,
+                                                     const double* __restrict__ gq, const double* __restrict__ V,
+                                                     int n_atoms, int D, double std, int64_t n_geo,
+                                                     double* __restrict__ HV) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_geo * n_atoms) return;
+  const int64_t b = idx / n_atoms;
+  const int k = (int)(idx - b * n_atoms);
+  const double* v = V + b * 3 * n_atoms;
+  double h0, h1, h2;
+  hvp_atom(Fd + b * D, dFd + b * D, gq + b * (int64_t)D * 3, [v](int i) { return v[i]; }, n_atoms, k, h0, h1, h2);
   HV[idx * 3 + 0] = h0 * std;
   HV[idx * 3 + 1] = h1 * std;
   HV[idx * 3 + 2] = h2 * std;
+}
+
+// ============================================================== Hessians (sgdml_b200_predict_hessian)
+// Column i of H is -HV at V = e_i: the HVP's arithmetic with the S query rows of a geometry built once and shared by its
+// 3N tangent rows per permutation, t_i = J e_i.  A direction block holds n_dir consecutive columns i0 .. i0 + n_dir - 1;
+// its tangent rows are laid out [geometry][direction][permutation], so that k_fdesc_gather folds each direction like a
+// geometry of its own.
+
+// One warp per tangent row (geometry b, direction i0 + j, permutation p): t = J e_i permuted like the query row, built
+// from the pair gradients gq with k_d_desc_dot_vec's arithmetic (every product exact: the bits of J e_i)
+__global__ void __launch_bounds__(256) k_hessian_tangent_rows(const double* __restrict__ gq,
+                                                              const int* __restrict__ pinv, int n_atoms, int D, int DS,
+                                                              int S, int i0, int n_dir, int64_t n_rows,
+                                                              double* __restrict__ T) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= n_rows) return;
+  const int64_t bj = row / S;
+  const int p = (int)(row - bj * S);
+  const int64_t b = bj / n_dir;
+  const int col = i0 + (int)(bj - b * n_dir);
+  const double* g = gq + b * (int64_t)D * 3;
+  const int* pi = pinv + (int64_t)p * D;
+  const auto unit = [col](int i) { return i == col ? 1.0 : 0.0; };
+  for (int e = lane; e < DS; e += 32) {
+    double v = 0.0;
+    if (e < D) {
+      const int d = pi[e];
+      int a, bb;
+      pair_from_d(d, a, bb);
+      v = d_desc_dot(g + (int64_t)d * 3, a, bb, unit);
+    }
+    T[row * DS + e] = v;
+  }
+}
+
+// One thread per (geometry b, atom k, direction j): rows 3k .. 3k + 2 of column i0 + j of H[b] (n x n, n = 3N), as
+// k_hvp_project writes HV at V = e_i, negated
+__global__ void __launch_bounds__(256) k_hessian_project(const double* __restrict__ Fd, const double* __restrict__ dFd,
+                                                         const double* __restrict__ gq, int n_atoms, int D, double std,
+                                                         int64_t n_geo, int i0, int n_dir, double* __restrict__ H) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_geo * n_atoms * n_dir) return;
+  const int64_t bk = idx / n_dir;
+  const int j = (int)(idx - bk * n_dir);
+  const int64_t b = bk / n_atoms;
+  const int k = (int)(bk - b * n_atoms);
+  const int col = i0 + j;
+  const int64_t n = 3 * (int64_t)n_atoms;
+  double h0, h1, h2;
+  hvp_atom(Fd + b * D, dFd + (b * n_dir + j) * D, gq + b * (int64_t)D * 3,
+           [col](int i) { return i == col ? 1.0 : 0.0; }, n_atoms, k, h0, h1, h2);
+  double* out = H + b * n * n + (3 * k) * n + col;
+  out[0] = -(h0 * std);
+  out[n] = -(h1 * std);
+  out[2 * n] = -(h2 * std);
 }
 
 }  // namespace sgdml
@@ -1411,6 +1504,13 @@ struct sgdml_b200_model {
            *qq = nullptr, *SX = nullptr, *SJ = nullptr, *G = nullptr, *csum = nullptr, *Fd = nullptr, *dFd = nullptr,
            *mu0 = nullptr;  // mu0: DS zeros, the "mean" of the tangent rows
   } hvp;
+  // sgdml_b200_predict_hessian: a workspace of its own as well (hessian_plan): `geo` geometries of query rows and
+  // geo x dirs x S tangent rows stacked below them in Qg, qq, SX, SJ, G, csum; H stages host outputs
+  struct HessWS {
+    int64_t geo = 0, dirs = 0;
+    double *R = nullptr, *xq = nullptr, *gq = nullptr, *Qg = nullptr, *qq = nullptr, *SX = nullptr, *SJ = nullptr,
+           *G = nullptr, *csum = nullptr, *Fd = nullptr, *dFd = nullptr, *H = nullptr;
+  } hess;
   cudaStream_t pipe_stream[2] = {nullptr, nullptr};
   cudaEvent_t pipe_event[3] = {nullptr, nullptr, nullptr};
   // MD latency path: the launch sequence of a small host-buffer batch, captured once per batch size into a CUDA graph
@@ -2292,13 +2392,13 @@ int hvp_impl(sgdml_b200_model* m, const double* R, const double* V, int64_t n_ge
       ProfScope ps(KID_PREDICT_MAIN, s);
       // [S1; S3] = [Q; T] Xc^T, [S2; S4] = [Q; T] JA^T, then acc = [C1; dC1] XcT^T + [C2; dC2] JAT^T
       SG_TRY(contract_desc(m, w.Qg, 2 * rows, w.SX, w.SJ, s));
-      k_transform_tangent_rows<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(
-          w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, m->use_ae ? m->ae : nullptr, m->M, m->Mpad, rows, mk,
-          w.csum);
+      k_transform_tangent_rows<TAN_PAIRED><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(
+          w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, m->use_ae ? m->ae : nullptr, m->M, m->Mpad, rows, rows,
+          m->S, m->S, mk, w.csum);
       SG_CUDA(cudaGetLastError());
       SG_TRY(contract_points(m, w.SX, w.SJ, 2 * rows, w.G, s));
-      k_combine_tangent_rows<<<(unsigned)((rows * m->DP + 255) / 256), 256, 0, s>>>(w.Qg, m->DS, w.csum, w.G, m->DP,
-                                                                                     rows);
+      k_combine_tangent_rows<TAN_PAIRED><<<(unsigned)((rows * m->DP + 255) / 256), 256, 0, s>>>(
+          w.Qg, m->DS, w.csum, w.G, m->DP, rows, rows, m->S, m->S);
       SG_CUDA(cudaGetLastError());
       count_launch(KID_PREDICT_MAIN, 2);
     }
@@ -2318,6 +2418,138 @@ int hvp_impl(sgdml_b200_model* m, const double* R, const double* V, int64_t n_ge
     SG_TRY(oHV.copy_back(g0, ng, w.HV, s));
   }
   if (!R_dev || !V_dev || oHV.staged()) SG_CUDA(cudaStreamSynchronize(s));
+  return 0;
+}
+
+// ---------------------------------------------------------------- Hessians
+void free_hess_ws(sgdml_b200_model::HessWS& w) {
+  for (double* p : {w.R, w.xq, w.gq, w.Qg, w.qq, w.SX, w.SJ, w.G, w.csum, w.Fd, w.dFd, w.H}) cached_free(p);
+  w = sgdml_b200_model::HessWS();
+}
+
+// How sgdml_b200_predict_hessian cuts its work: geometries per chunk and directions (columns) per block.  A chunk holds at
+// most `rows` stacked rows (Qg, SX, SJ and G: DS + 2 Mpad + DP doubles each) within ~2 GB, and at most 2 c S rows when
+// sgdml_b200_set_predict_chunk set a cap c (the rows of c HVP geometries).  A geometry needs (1 + 3N) S rows: whole
+// geometries when at least one fits, else one geometry per chunk in blocks of rows / S - 1 directions.
+struct HessPlan {
+  int64_t geo, dirs;
+};
+HessPlan hessian_plan(const sgdml_b200_model* m) {
+  const int64_t row_bytes = 8 * ((int64_t)m->DS + 2 * (int64_t)m->Mpad + m->DP + 2);
+  int64_t rows = (int64_t)(2048ll << 20) / row_bytes;
+  if (g_chunk_cap > 0) rows = std::min<int64_t>(rows, 2 * g_chunk_cap * m->S);
+  rows = std::max<int64_t>(rows, 2 * (int64_t)m->S);
+  const int64_t n = 3 * (int64_t)m->N, geo_rows = (1 + n) * m->S;
+  if (rows >= geo_rows) return {std::min<int64_t>(rows / geo_rows, 65536), n};
+  return {1, rows / m->S - 1};
+}
+
+int ensure_hess_ws(sgdml_b200_model* m, const HessPlan& p, int64_t n_geo, bool stage_H, cudaStream_t s) {
+  if (m->XcT == nullptr) {
+    SG_CUDA(cached_malloc(&m->XcT, sizeof(double) * (size_t)m->DP * m->Mpad));
+    SG_CUDA(cached_malloc(&m->JAT, sizeof(double) * (size_t)m->DP * m->Mpad));
+    SG_TRY(refresh_transposes(m, true, s));
+  }
+  sgdml_b200_model::HessWS& w = m->hess;
+  const bool H_ok = !stage_H || w.H != nullptr;
+  if (n_geo <= w.geo && p.dirs == w.dirs && H_ok) return 0;
+  n_geo = std::max(n_geo, w.geo);
+  if (w.geo > 0) SG_CUDA(cudaDeviceSynchronize());  // earlier calls may still run on the old workspace
+  const bool had_H = w.H != nullptr;
+  free_hess_ws(w);
+  const int64_t n = 3 * (int64_t)m->N;
+  const int64_t rows = n_geo * m->S * (1 + p.dirs);
+  SG_CUDA(cached_malloc(&w.R, sizeof(double) * n_geo * n));
+  SG_CUDA(cached_malloc(&w.xq, sizeof(double) * n_geo * m->D));
+  SG_CUDA(cached_malloc(&w.gq, sizeof(double) * n_geo * m->D * 3));
+  SG_CUDA(cached_malloc(&w.Qg, sizeof(double) * rows * m->DS));
+  SG_CUDA(cached_malloc(&w.qq, sizeof(double) * rows));
+  SG_CUDA(cached_malloc(&w.SX, sizeof(double) * rows * m->Mpad));
+  SG_CUDA(cached_malloc(&w.SJ, sizeof(double) * rows * m->Mpad));
+  SG_CUDA(cached_malloc(&w.G, sizeof(double) * rows * m->DP));
+  SG_CUDA(cached_malloc(&w.csum, sizeof(double) * rows));
+  SG_CUDA(cached_malloc(&w.Fd, sizeof(double) * n_geo * m->D));
+  SG_CUDA(cached_malloc(&w.dFd, sizeof(double) * n_geo * p.dirs * m->D));
+  if (stage_H || had_H) SG_CUDA(cached_malloc(&w.H, sizeof(double) * n_geo * n * n));
+  w.geo = n_geo;
+  w.dirs = p.dirs;
+  return 0;
+}
+
+// sgdml_b200_predict_hessian: the GEMM-composed HVP form in FP64, in the model's cell, chunk by chunk on the caller's
+// stream; per direction block the query rows, their tangent rows, both contractions, the folds and the projection
+int hessian_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, double* H, cudaStream_t s) {
+  const bool R_dev = is_device_ptr(R);
+  const int dimi = 3 * m->N;
+  const ChunkOut oH(H, (int64_t)dimi * dimi);
+  const HessPlan p = hessian_plan(m);
+  const int64_t chunk = std::min<int64_t>(p.geo, n_geo);
+  SG_TRY(ensure_hess_ws(m, p, chunk, oH.staged(), s));
+  sgdml_b200_model::HessWS& w = m->hess;
+  const MaternK mk = MaternK::from_sig(m->sig);
+  const double* ae = m->use_ae ? m->ae : nullptr;
+  for (int64_t g0 = 0; g0 < n_geo; g0 += chunk) {
+    const int64_t ng = std::min<int64_t>(chunk, n_geo - g0);
+    const int64_t rows = ng * m->S;
+    const double* Rd = R + g0 * dimi;
+    if (!R_dev) {
+      SG_CUDA(cudaMemcpyAsync(w.R, Rd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, s));
+      Rd = w.R;
+    }
+    double* Hc = oH.at(g0, w.H);
+    SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, s, m->lat, nullptr));
+    for (int i0 = 0; i0 < dimi; i0 += (int)p.dirs) {
+      const int nd = (int)std::min<int64_t>(p.dirs, dimi - i0);
+      const int64_t trows = rows * nd, dir_rows = (int64_t)nd * m->S;
+      {
+        ProfScope ps(KID_PREDICT_AUX, s);
+        k_query_rows<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(w.xq, m->pinv, m->mu, m->D, m->DS, m->S, rows, rows,
+                                                                  w.Qg, w.qq);
+        SG_CUDA(cudaGetLastError());
+        k_hessian_tangent_rows<<<(unsigned)((trows + 7) / 8), 256, 0, s>>>(w.gq, m->pinv, m->N, m->D, m->DS, m->S, i0,
+                                                                            nd, trows, w.Qg + rows * m->DS);
+        SG_CUDA(cudaGetLastError());
+        count_launch(KID_PREDICT_AUX, 2);
+      }
+      {
+        ProfScope ps(KID_PREDICT_MAIN, s);
+        SG_TRY(contract_desc(m, w.Qg, rows + trows, w.SX, w.SJ, s));
+        // every tangent row reads its query row's S1 / S2 before the query pass overwrites them with C1 / C2
+        k_transform_tangent_rows<TAN_ONLY><<<(unsigned)((trows + 7) / 8), 256, 0, s>>>(
+            w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, ae, m->M, m->Mpad, rows, trows, dir_rows, m->S, mk,
+            w.csum);
+        SG_CUDA(cudaGetLastError());
+        k_transform_tangent_rows<TAN_QUERY><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(
+            w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, ae, m->M, m->Mpad, rows, rows, m->S, m->S, mk,
+            w.csum);
+        SG_CUDA(cudaGetLastError());
+        SG_TRY(contract_points(m, w.SX, w.SJ, rows + trows, w.G, s));
+        k_combine_tangent_rows<TAN_ONLY><<<(unsigned)ceil_div(trows * m->DP, 256), 256, 0, s>>>(
+            w.Qg, m->DS, w.csum, w.G, m->DP, rows, trows, dir_rows, m->S);
+        SG_CUDA(cudaGetLastError());
+        k_combine_tangent_rows<TAN_QUERY><<<(unsigned)ceil_div(rows * m->DP, 256), 256, 0, s>>>(
+            w.Qg, m->DS, w.csum, w.G, m->DP, rows, rows, m->S, m->S);
+        SG_CUDA(cudaGetLastError());
+        count_launch(KID_PREDICT_MAIN, 4);
+      }
+      {
+        ProfScope ps(KID_PREDICT_FINISH, s);
+        const unsigned gx = (unsigned)ceil_div(m->D, 256);
+        k_fdesc_gather<false><<<dim3(gx, (unsigned)std::min<int64_t>(ng, 65535)), 256, 0, s>>>(
+            w.G, m->perm, m->D, m->DP, m->S, 1, rows, ng, w.Fd, nullptr, nullptr);
+        SG_CUDA(cudaGetLastError());
+        k_fdesc_gather<false><<<dim3(gx, (unsigned)std::min<int64_t>(ng * nd, 65535)), 256, 0, s>>>(
+            w.G + rows * m->DP, m->perm, m->D, m->DP, m->S, 1, trows, ng * nd, w.dFd, nullptr, nullptr);
+        SG_CUDA(cudaGetLastError());
+        k_hessian_project<<<(unsigned)ceil_div(ng * m->N * nd, 256), 256, 0, s>>>(w.Fd, w.dFd, w.gq, m->N, m->D,
+                                                                                  m->std, ng, i0, nd, Hc);
+        SG_CUDA(cudaGetLastError());
+        count_launch(KID_PREDICT_FINISH, 3);
+      }
+    }
+    SG_TRY(oH.copy_back(g0, ng, w.H, s));
+  }
+  if (!R_dev || oH.staged()) SG_CUDA(cudaStreamSynchronize(s));
   return 0;
 }
 
@@ -2347,6 +2579,7 @@ int sgdml_b200_model_destroy(sgdml_b200_model* m) {
   free_oz(m->ozJAT);
   free_ws(m);
   free_hvp_ws(m->hvp);
+  free_hess_ws(m->hess);
   for (int i = 0; i < 2; ++i)
     if (m->pipe_stream[i]) cudaStreamDestroy(m->pipe_stream[i]);
   for (int i = 0; i < 3; ++i)
@@ -2399,6 +2632,13 @@ int sgdml_b200_predict_hvp(sgdml_b200_model* m, const double* R, const double* V
   SG_ARG(m != nullptr && R != nullptr && V != nullptr && HV != nullptr && n_geo >= 0);
   if (n_geo == 0) return 0;
   return hvp_impl(m, R, V, n_geo, HV, (cudaStream_t)stream);
+}
+
+int sgdml_b200_predict_hessian(sgdml_b200_model* m, const double* R, int64_t n_geo, double* H, void* stream) {
+  SG_TRY(require_device());
+  SG_ARG(m != nullptr && R != nullptr && H != nullptr && n_geo >= 0);
+  if (n_geo == 0) return 0;
+  return hessian_impl(m, R, n_geo, H, (cudaStream_t)stream);
 }
 
 int sgdml_b200_model_set_lattice(sgdml_b200_model* m, const double* lattice, const double* lattice_inv) {

@@ -342,6 +342,41 @@ class GDMLPredict(object):
         )
         return HV
 
+    def predict_hessian(self, R, out=None):
+        """Extension: the energy Hessian H = d^2E/dR^2 of every geometry, R (B, 3N) [or (3N,)] -> H (B, 3N, 3N), in the
+        model's units and cell, always in FP64.  Column i of H[b] equals -predict_hvp(R[b], e_i) bit for bit; H is not
+        symmetrised.  `out`: a preallocated (B, 3N, 3N) buffer.  NumPy / torch conventions as `predict_hvp`."""
+        dim_i = 3 * self.n_atoms
+        size = R.size if isinstance(R, np.ndarray) else R.numel()
+        if size % dim_i != 0 or (R.ndim == 2 and R.shape[1] != dim_i):
+            raise ValueError('R must have 3*n_atoms columns')
+        if isinstance(R, np.ndarray):
+            R = np.ascontiguousarray(R, dtype=np.float64).reshape(-1, dim_i)
+            shape = (R.shape[0], dim_i, dim_i)
+            H = np.empty(shape) if out is None else out
+        else:
+            import torch
+
+            if R.dtype != torch.float64:
+                raise ValueError('torch inputs must be float64')
+            R = R.contiguous().reshape(-1, dim_i)
+            shape = (R.shape[0], dim_i, dim_i)
+            pin = (not R.is_cuda) and R.is_pinned()
+            H = torch.empty(shape, dtype=torch.float64, device=R.device, pin_memory=pin) if out is None else out
+        n = R.shape[0]
+        if out is not None:
+            if tuple(H.shape) != shape:
+                raise ValueError('out has the wrong shape %s (expected %s)' % (tuple(H.shape), shape))
+            if not (H.flags['C_CONTIGUOUS'] if isinstance(H, np.ndarray) else H.is_contiguous()):
+                raise ValueError('out must be contiguous')
+            # the dtype, layout and device checks of `predict`'s F, on the buffer seen as (B, 3N * 3N)
+            self._check_out(R, None, H.reshape(n, dim_i * dim_i), None, n, dim_i * dim_i)
+        _lib.check(
+            _lib.lib().sgdml_b200_predict_hessian(self._handle, _lib.ptr(R), n, _lib.ptr(H), _lib.current_stream()),
+            'predict_hessian',
+        )
+        return H
+
     @staticmethod
     def _results(E, F, W, return_E, with_W):
         res = (F, W) if with_W else (F,)

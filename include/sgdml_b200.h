@@ -206,7 +206,7 @@ int sgdml_b200_symeig_max_n(void);
  * error:
  *   entry point                                                              plain  ring  NPT  metadynamics  umbrella
  *   sgdml_b200_md_set_state, _md_get_state, _md_destroy                        x     x     x        x            x
- *   sgdml_b200_md_run, _remd_run, _neb_fire, _dimer_fire                       x
+ *   sgdml_b200_md_run, _remd_run, _neb_fire, _dimer_fire, _irc_rk4             x
  *   sgdml_b200_pimd_run, _relax_fire, _relax_lbfgs                             x     x
  *   sgdml_b200_npt_run, _npt_set_cells, _npt_get_cells                                     x
  *   sgdml_b200_metad_run, _metad_get_hills, _metad_set_hills, _metad_get_bias                       x
@@ -535,8 +535,35 @@ int sgdml_b200_dimer_fire(sgdml_b200_md* md, const double* modes, int64_t max_st
                           double cos_trial, double sin_trial, double rot_min, double maxstep, double dt, double dtmax,
                           int64_t* n_steps_out, int* converged_out, double* fmax_out, double* curvature_out,
                           int64_t* n_rot_out, double* modes_out, void* stream);
-/* Test hook: graph replays between convergence read-backs of sgdml_b200_relax_*, sgdml_b200_neb_fire and
- * sgdml_b200_dimer_fire; 0 = the default (16).  Negative values are rejected. */
+/* ---------------------------------------------------------------- intrinsic reaction coordinate on the device
+ * Extension: which two minima a first-order saddle connects, by the intrinsic reaction coordinate (IRC): the
+ * steepest-descent path in mass-weighted coordinates x_i = R_i / sqrt(s_i), s the handle's inverse masses, followed
+ * downhill from each saddle in both directions along its imaginary mode by classical RK4 (Schmidt, Gordon & Dupuis,
+ * JACS 107, 2585 (1985)) of dx/ds = r F / |r F|, r_i = sqrt(s_i), with a fixed step; many saddles and many points per
+ * call.  The handle (plain: see the handle kinds at sgdml_b200_md_create) holds n_rep = 2 n_saddles replicas (n_rep
+ * even): replica 2k's state is saddle k at the start of the call (as set_state stored it: R, F, E_pot), and replica
+ * 2k + 1's is overwritten with it; replica 2k follows +mode (forward), 2k + 1 -mode (backward).  Point 0 of a branch
+ * is the saddle, point 1 the saddle plus step along the mass-weighted unit mode, every later point one RK4 step (four
+ * force evaluations) from the one before.  A new point whose energy is not below the previous one's is rejected and
+ * the branch ends at the previous point (end 2); otherwise it is recorded, and the branch ends there when
+ * max_a |F_a| < fmax (end 1, ASE's criterion) or when it holds max_points points (end 3).  An ended branch is frozen
+ * for the rest of the call (its forces are still evaluated with the batch).  No rigid-mode projection: the model's
+ * energy is invariant under rigid motions.  Exact sums and roundings are in csrc/md.cuh; the driver, block read-backs
+ * and launch families are those of sgdml_b200_relax_*.
+ * Arguments: modes (n_rep / 2, 3N), host or device, the Cartesian displacement of each saddle's imaginary mode (any
+ * length; GDMLVibrations' modes or a dimer's mode); a mode that is not finite or whose mass-weighted norm is 0 is an
+ * argument error, checked before anything of the handle changes.  max_points >= 2; step > 0 in the handle's
+ * mass-weighted unit (L / sqrt(inverse-mass unit)); fmax >= 0 (force unit; 0: never ends by force).  Outputs, each
+ * host, device or NULL: R_path (n_rep, max_points, 3N) and E_path (n_rep, max_points), every entry written, NaN past
+ * the branch's n_points; n_points_out (n_rep) int64, the points recorded, the saddle included; end_out (n_rep) int32,
+ * 1, 2 or 3 as above; fmax_out (n_rep) double, max_a |F_a| at the branch end.  After the call R, F and E_pot of each
+ * replica are its branch end and the forces there, V is zero and the step counter is unchanged.  Argument errors are
+ * reported before anything is queued, and a rejected call changes nothing. */
+int sgdml_b200_irc_rk4(sgdml_b200_md* md, const double* modes, int64_t max_points, double step, double fmax,
+                       double* R_path, double* E_path, int64_t* n_points_out, int* end_out, double* fmax_out,
+                       void* stream);
+/* Test hook: graph replays between convergence read-backs of sgdml_b200_relax_*, sgdml_b200_neb_fire,
+ * sgdml_b200_dimer_fire and sgdml_b200_irc_rk4; 0 = the default (16).  Negative values are rejected. */
 int sgdml_b200_set_relax_block(int64_t n_steps);
 
 /* Periodic model (predict.py:332-334: lat_and_inv from model['lattice']): query descriptors of

@@ -9,7 +9,7 @@ CPU fallback.
 
 __version__ = '0.1.0'
 
-from .md import (GDMLNEB, GDMLDimer, GDMLDynamics, GDMLMetadynamics, GDMLNPTDynamics,  # noqa: F401
+from .md import (GDMLIRC, GDMLNEB, GDMLDimer, GDMLDynamics, GDMLMetadynamics, GDMLNPTDynamics,  # noqa: F401
                  GDMLPathIntegralDynamics, GDMLRelaxation, GDMLReplicaExchange, GDMLUmbrellaSampling)
 from .perm import find_perms  # noqa: F401
 from .predict import GDMLPredict  # noqa: F401

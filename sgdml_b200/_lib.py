@@ -108,6 +108,9 @@ SIGNATURES = {
         C.c_int,
         [c_void_p, c_void_p, i64, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
          C.c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sgdml_b200_irc_rk4': (
+        C.c_int,
+        [c_void_p, c_void_p, i64, C.c_double, C.c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_set_relax_block': (C.c_int, [i64]),
     'sgdml_b200_model_set_R_d_desc': (C.c_int, [c_void_p, c_void_p]),
     'sgdml_b200_model_set_alphas': (C.c_int, [c_void_p, c_void_p, c_void_p]),

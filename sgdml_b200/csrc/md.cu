@@ -1373,6 +1373,147 @@ __global__ void k_dimer_report(const DimerState* __restrict__ ds, int64_t n_dime
   if (n_rot) n_rot[d] = ds[d].n_rot;
 }
 
+// ---------------------------------------------------------------------------------- reaction path
+// The IRC kernels of sgdml_b200_irc_rk4 (contract in md.cuh).  As in the optimiser kernels, every thread holds the
+// branch's state and every CTA-wide sum, and each thread writes only its own coordinates i = t, t + MD_THREADS, ...
+
+// The check (commit == 0) or the commit (commit == 1) of pair k's start, V (n_pairs, 3N) the caller's modes in transit.
+__global__ void __launch_bounds__(MD_THREADS) k_irc_init(const IrcParams* __restrict__ Q, const double* __restrict__ s,
+                                                        double* __restrict__ R, const double* __restrict__ F,
+                                                        const double* __restrict__ E, double* __restrict__ V,
+                                                        int* __restrict__ bad, double* __restrict__ Rn,
+                                                        double* __restrict__ Fn, IrcState* __restrict__ is, int dimi,
+                                                        int commit) {
+  __shared__ double red[MD_THREADS];
+  const int64_t k = blockIdx.x;
+  double* v = V + k * dimi;
+  if (!commit) {
+    double q = 0.0;
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+      const double x = __ddiv_rn(v[i], sqrt(s[i]));
+      v[i] = x;
+      q = __dadd_rn(q, __dmul_rn(x, x));
+    }
+    q = block_sum(q, red);
+    const double nrm = sqrt(q);
+    for (int i = threadIdx.x; i < dimi; i += MD_THREADS) v[i] = __ddiv_rn(v[i], nrm);
+    if (threadIdx.x == 0) bad[k] = !(isfinite(q) && q > 0.0);
+    return;
+  }
+  const IrcParams p = *Q;
+  const int64_t mp = p.max_points;
+  const double e0 = E[2 * k];
+  const double nan = __longlong_as_double(0x7ff8000000000000LL);
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+    const double r0 = R[2 * k * dimi + i], f0 = F[2 * k * dimi + i], ri = sqrt(s[i]);
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int64_t b = 2 * k + j;
+      Rn[b * dimi + i] = r0;
+      Fn[b * dimi + i] = f0;
+      R[b * dimi + i] = __dadd_rn(r0, __dmul_rn(ri, __dmul_rn(j ? -p.h : p.h, v[i])));
+      if (p.R_path) p.R_path[b * mp * dimi + i] = r0;
+    }
+  }
+  for (int j = 0; j < 2; ++j) {
+    const int64_t b = 2 * k + j;
+    if (p.R_path)
+      for (int64_t o = dimi + threadIdx.x; o < mp * dimi; o += MD_THREADS) p.R_path[b * mp * dimi + o] = nan;
+    if (p.E_path)
+      for (int64_t o = threadIdx.x; o < mp; o += MD_THREADS) p.E_path[b * mp + o] = o == 0 ? e0 : nan;
+    if (threadIdx.x == 0) {
+      is[b].phase = IRC_POINT;
+      is[b].end = 0;
+      is[b].n_points = 1;
+      is[b].E_n = e0;
+    }
+  }
+}
+
+// The test and one stage of branch b (md.cuh): R, F, E rows b, the point buffers Rn, Fn and the running sum K rows b.
+__global__ void __launch_bounds__(MD_THREADS) k_irc_step(const IrcParams* __restrict__ Q, RelaxState* st,
+                                                        IrcState* is, const double* __restrict__ s,
+                                                        double* __restrict__ R, double* __restrict__ F,
+                                                        double* __restrict__ E, double* __restrict__ Rn,
+                                                        double* __restrict__ Fn, double* __restrict__ K, int dimi,
+                                                        int advance) {
+  __shared__ double red[MD_THREADS];
+  const int64_t b = blockIdx.x;
+  const IrcParams p = *Q;
+  RelaxState z = st[b];
+  IrcState y = is[b];
+  double* r = R + b * dimi;
+  double* f = F + b * dimi;
+  double* rn = Rn + b * dimi;
+  double* fn = Fn + b * dimi;
+  double* k = K + b * dimi;
+  if (y.end) return relax_store(st + b, z);
+  if (y.phase == IRC_POINT) {
+    const double e = E[b];
+    if (!(e < y.E_n)) {
+      for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+        r[i] = rn[i];
+        f[i] = fn[i];
+      }
+      z.fmax2 = atom_max2(fn, dimi, red);  // (its barriers: every thread has read E[b])
+      if (threadIdx.x == 0) E[b] = y.E_n;
+      y.end = 2;
+    } else {
+      const int64_t n = y.n_points;
+      for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+        const double ri = r[i];
+        rn[i] = ri;
+        fn[i] = f[i];
+        if (p.R_path) p.R_path[(b * p.max_points + n) * dimi + i] = ri;
+      }
+      if (p.E_path && threadIdx.x == 0) p.E_path[b * p.max_points + n] = e;
+      y.n_points = n + 1;
+      y.E_n = e;
+      z.fmax2 = atom_max2(f, dimi, red);
+      y.end = z.fmax2 < p.fmax2 ? 1 : (y.n_points == p.max_points ? 3 : 0);
+    }
+    y.phase = IRC_K1;
+    z.n_steps = y.n_points;
+    z.conv = y.end;
+  }
+  if (y.end || !advance) {
+    __syncthreads();  // every thread has read the state
+    if (threadIdx.x == 0) {
+      st[b] = z;
+      is[b] = y;
+    }
+    return;
+  }
+  double q = 0.0;
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+    const double g = __dmul_rn(sqrt(s[i]), f[i]);
+    q = __dadd_rn(q, __dmul_rn(g, g));
+  }
+  q = block_sum(q, red);
+  const double nrm = sqrt(q);
+  const int ph = y.phase;
+  const double c = ph == IRC_K3 ? p.h : (ph == IRC_K4 ? p.h6 : p.hh);
+  for (int i = threadIdx.x; i < dimi; i += MD_THREADS) {
+    const double ri = sqrt(s[i]);
+    const double d = q == 0.0 ? 0.0 : __ddiv_rn(__dmul_rn(ri, f[i]), nrm);
+    double x = d;  // what the stage moves along: d, or K after k4
+    if (ph == IRC_K1) {
+      k[i] = d;
+    } else if (ph == IRC_K4) {
+      x = __dadd_rn(k[i], d);
+    } else {
+      k[i] = __dadd_rn(k[i], __dmul_rn(2.0, d));
+    }
+    r[i] = __dadd_rn(rn[i], __dmul_rn(ri, __dmul_rn(c, x)));
+  }
+  y.phase = ph == IRC_K4 ? IRC_POINT : ph + 1;
+  __syncthreads();  // every thread has read the state
+  if (threadIdx.x == 0) {
+    st[b] = z;
+    is[b] = y;
+  }
+}
+
 }  // namespace
 
 }  // namespace sgdml
@@ -1413,6 +1554,7 @@ struct StepParams {
   MetadParams metad;
   DimerParams dimer;
   UmbrellaParams umbrella;
+  IrcParams irc;
 };
 constexpr size_t STEP_PARAMS_BYTES = (sizeof(StepParams) + 255) & ~(size_t)255;  // where the tables start
 // The umbrella parameters took the block past 768 bytes, so the tables start at 1024.  Every kernel that reads a table
@@ -1476,6 +1618,11 @@ struct sgdml_b200_md {
   DimerState* dstate = nullptr;               // (n_rep / 2)
   int* dbad = nullptr;                        // (n_rep / 2) k_dimer_init's verdict per mode
   bool has_modes = false;                     // dmode holds the modes of an earlier call
+  // reaction path (sgdml_b200_irc_rk4), allocated by the first IRC call
+  double *irc_rn = nullptr, *irc_fn = nullptr, *irc_k = nullptr;  // (n_rep, 3N) the newest point's R and F, RK4 sum
+  double* irc_v = nullptr;                    // (n_rep / 2, 3N) the caller's modes in transit, normalised in place
+  IrcState* istate = nullptr;                 // (n_rep)
+  int* ibad = nullptr;                        // (n_rep / 2) k_irc_init's verdict per mode
   // replica exchange (sgdml_b200_remd_run), allocated by the first replica-exchange call
   int* walker = nullptr;      // (n_rep) walker label per slot
   int64_t* xcount = nullptr;  // (2, n_rep) accepted and attempted swaps of the current run
@@ -1515,6 +1662,9 @@ void md_free(sgdml_b200_md* md) {
   for (double* p : {md->R, md->V, md->F, md->E, md->Fs, md->Es, md->s}) cached_free(p);
   for (double* p : {md->S, md->Y, md->rho, md->r_prev, md->g_prev, md->Fn, md->W, md->Ws}) cached_free(p);
   for (double* p : {md->Fm, md->cv, md->Vb, md->Fb, md->hc, md->hw, md->hh, md->dmode, md->dtheta}) cached_free(p);
+  for (double* p : {md->irc_rn, md->irc_fn, md->irc_k, md->irc_v}) cached_free(p);
+  cached_free(md->istate);
+  cached_free(md->ibad);
   cached_free(md->dstate);
   cached_free(md->dbad);
   cached_free(md->hcount);
@@ -1631,14 +1781,14 @@ class Outputs {
 // what one step of the handle's graph integrates
 enum MdKind {
   MD_CLASSICAL = 0, MD_RING_POLYMER = 1, MD_FIRE = 2, MD_LBFGS = 3, MD_NEB_FIRE = 4, MD_REMD = 5, MD_NPT = 6,
-  MD_METAD = 7, MD_DIMER = 8, MD_UMBRELLA = 9
+  MD_METAD = 7, MD_DIMER = 8, MD_UMBRELLA = 9, MD_IRC = 10
 };
 
 // the integrator of sgdml_b200_md_run, sgdml_b200_remd_run, sgdml_b200_npt_run, sgdml_b200_umbrella_run,
-// sgdml_b200_pimd_run, sgdml_b200_relax_*, sgdml_b200_neb_fire or sgdml_b200_dimer_fire; advance == 0 completes a
-// run's last step (MD; a replica exchange or umbrella run first exchanges that last state) or only tests convergence
-// (relaxation, NEB: after the force projection, dimer: with the curvature).  L-BFGS keeps its direction in V, which
-// relax_impl zeroes after.
+// sgdml_b200_pimd_run, sgdml_b200_relax_*, sgdml_b200_neb_fire, sgdml_b200_dimer_fire or sgdml_b200_irc_rk4;
+// advance == 0 completes a run's last step (MD; a replica exchange or umbrella run first exchanges that last state) or
+// only tests convergence (relaxation, NEB: after the force projection, dimer: with the curvature, IRC: a new point).
+// L-BFGS keeps its direction in V, which relax_impl zeroes after.
 int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
   StepParams* p = md->params(md->blk);
   switch (kind) {
@@ -1668,6 +1818,10 @@ int md_integrate(sgdml_b200_md* md, int kind, int advance, cudaStream_t s) {
     case MD_DIMER:
       k_dimer_step<<<(unsigned)(md->n_rep / 2), MD_THREADS, 0, s>>>(&p->dimer, md->rst, md->dstate, md->R, md->V, md->F,
                                                                    md->Fn, md->dmode, md->dtheta, md->dimi, advance);
+      break;
+    case MD_IRC:
+      k_irc_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&p->irc, md->rst, md->istate, md->s, md->R, md->F, md->E,
+                                                            md->irc_rn, md->irc_fn, md->irc_k, md->dimi, advance);
       break;
     case MD_NPT:
       k_npt_step<<<(unsigned)md->n_rep, MD_THREADS, 0, s>>>(&p->md, &p->npt, md->s, md->sigma(md->blk), md->R, md->V,
@@ -2105,10 +2259,17 @@ int md_run(sgdml_b200_md* md, int kind, const Run& r, cudaStream_t s) {
 constexpr int64_t RELAX_BLOCK = 16;  // replays between convergence read-backs
 int64_t g_relax_block = 0;           // sgdml_b200_set_relax_block (test hook): 0 = RELAX_BLOCK
 
-// the optimiser state, made at the first relaxation; the L-BFGS ring grows to `memory` pairs per replica, and the NEB
-// and dimer buffers are made at the first call of that kind
+// the optimiser state, made at the first relaxation; the L-BFGS ring grows to `memory` pairs per replica, and the NEB,
+// dimer and IRC buffers are made at the first call of that kind
 int relax_alloc(sgdml_b200_md* md, int memory, int kind) {
   const bool neb = kind == MD_NEB_FIRE, dimer = kind == MD_DIMER;
+  if (kind == MD_IRC && md->istate == nullptr) {
+    const size_t st = sizeof(double) * (size_t)(md->n_rep * md->dimi);
+    for (double** p : {&md->irc_rn, &md->irc_fn, &md->irc_k}) SG_CUDA(cached_malloc(p, st));
+    SG_CUDA(cached_malloc(&md->irc_v, st / 2));
+    SG_CUDA(cached_malloc(&md->ibad, sizeof(int) * (size_t)(md->n_rep / 2)));
+    SG_CUDA(cached_malloc(&md->istate, sizeof(IrcState) * (size_t)md->n_rep));
+  }
   if (md->rst == nullptr) SG_CUDA(cached_malloc(&md->rst, sizeof(RelaxState) * (size_t)md->n_rep));
   if (md->hActive == nullptr) {
     SG_CUDA(cudaHostAlloc(&md->hActive, sizeof(int), cudaHostAllocMapped));
@@ -2189,16 +2350,46 @@ int dimer_start(sgdml_b200_md* md, const double* modes, cudaStream_t s) {
   return md_state_forces(md, 0, s);
 }
 
+// What an IRC call (sgdml_b200_irc_rk4) adds to relax_impl: the caller's modes and its outputs per branch.
+struct IrcRun {
+  const double* modes;
+  double *R_path, *E_path;
+};
+
+// The start of an IRC call, after the upload: the modes into irc_v, k_irc_init's check on them, the verdict read back,
+// and only then its commit and one un-captured force evaluation of every replica (point 1).  A bad mode is an argument
+// error with the handle unchanged; a rejected call has overwritten only irc_v, ibad and the IRC part of the upload
+// block, which every IRC call rewrites before reading them.
+int irc_start(sgdml_b200_md* md, const double* modes, cudaStream_t s) {
+  const int64_t np = md->n_rep / 2;
+  SG_CUDA(cudaMemcpyAsync(md->irc_v, modes, sizeof(double) * (size_t)(np * md->dimi), cudaMemcpyDefault, s));
+  const IrcParams* q = &md->params(md->blk)->irc;
+  for (int commit = 0; commit < 2; ++commit) {
+    k_irc_init<<<(unsigned)np, MD_THREADS, 0, s>>>(q, md->s, md->R, md->F, md->E, md->irc_v, md->ibad, md->irc_rn,
+                                                   md->irc_fn, md->istate, md->dimi, commit);
+    SG_CUDA(cudaGetLastError());
+    count_launch(KID_MISC);
+    if (commit) break;
+    std::vector<int> bad((size_t)np);
+    SG_CUDA(cudaMemcpyAsync(bad.data(), md->ibad, sizeof(int) * (size_t)np, cudaMemcpyDeviceToHost, s));
+    SG_CUDA(cudaStreamSynchronize(s));
+    for (int b : bad)
+      if (b) return fail_arg("sgdml_b200_irc_rk4: every mode must be finite with a nonzero mass-weighted norm");
+  }
+  return md_state_forces(md, 0, s);
+}
+
 // Relaxes every replica (or NEB band, or dimer) from the handle's state: blocks of step-graph replays, each followed
 // by the convergence test and a count of unconverged units read back through mapped pinned memory; stops when none is
 // left or after max_steps.  The unit of convergence is a group of g consecutive replicas: g = 1 for relaxation, g = P
 // for NEB (whose climbing_out gets each band's highest interior image), g = 2 for the dimer (dm: its modes and
-// outputs).  call: the entry point's RelaxParams (FIRE, L-BFGS; the handle's L-BFGS ring is added here), NebParams
-// (NEB) or DimerParams (dimer).  memory: L-BFGS pairs per replica to allocate (0: none).  Frozen units make the block
-// length a matter of cost only.  V is zero before and after.
+// outputs), g = 1 for the IRC (ir: its modes and outputs; n_steps_out and conv_out get n_points and end).  call: the
+// entry point's RelaxParams (FIRE, L-BFGS; the handle's L-BFGS ring is added here), NebParams (NEB), DimerParams
+// (dimer) or IrcParams (IRC; the path outputs are added here).  memory: L-BFGS pairs per replica to allocate (0: none).
+// Frozen units make the block length a matter of cost only.  V is zero before and after.
 int relax_impl(sgdml_b200_md* md, int kind, int g, int memory, const StepParams& call, int64_t max_steps,
                int64_t* n_steps_out, int* conv_out, double* fmax_out, int* climbing_out, cudaStream_t s,
-               const DimerRun* dm = nullptr) {
+               const DimerRun* dm = nullptr, const IrcRun* ir = nullptr) {
   md->group = g;
   const int64_t n_rep = md->n_rep;
   const int64_t n_units = n_rep / g;
@@ -2210,13 +2401,19 @@ int relax_impl(sgdml_b200_md* md, int kind, int g, int memory, const StepParams&
                    {fmax_out, sizeof(double) * un}, {climbing_out, sizeof(int) * un},
                    {dm ? dm->curvature_out : nullptr, sizeof(double) * un},
                    {dm ? dm->n_rot_out : nullptr, sizeof(int64_t) * un},
-                   {dm ? dm->modes_out : nullptr, sizeof(double) * un * md->dimi}}));
+                   {dm ? dm->modes_out : nullptr, sizeof(double) * un * md->dimi},
+                   {ir ? ir->R_path : nullptr, sizeof(double) * un * (size_t)(call.irc.max_points * md->dimi)},
+                   {ir ? ir->E_path : nullptr, sizeof(double) * un * (size_t)call.irc.max_points}}));
   SG_CUDA(cudaEventSynchronize(md->uploaded));  // the previous call has read the mirror
   StepParams& p = *md->params(md->hblk);
   if (kind == MD_NEB_FIRE) {
     p.neb = call.neb;
   } else if (kind == MD_DIMER) {
     p.dimer = call.dimer;
+  } else if (kind == MD_IRC) {
+    p.irc = call.irc;
+    p.irc.R_path = out.dev(7);
+    p.irc.E_path = out.dev(8);
   } else {
     p.relax = call.relax;
     p.relax.m_cap = md->m_cap;
@@ -2228,6 +2425,7 @@ int relax_impl(sgdml_b200_md* md, int kind, int g, int memory, const StepParams&
   }
   SG_TRY(upload(md, &p + 1, s));
   if (kind == MD_DIMER) SG_TRY(dimer_start(md, dm->modes, s));
+  if (kind == MD_IRC) SG_TRY(irc_start(md, ir->modes, s));
   const size_t st = sizeof(double) * (size_t)(n_rep * md->dimi);
   SG_CUDA(cudaMemsetAsync(md->rst, 0, sizeof(RelaxState) * (size_t)n_units, s));
   SG_CUDA(cudaMemsetAsync(md->V, 0, st, s));
@@ -2872,6 +3070,29 @@ int sgdml_b200_dimer_fire(sgdml_b200_md* md, const double* modes, int64_t max_st
   const DimerRun dm = {modes, curvature_out, n_rot_out, modes_out};
   return relax_impl(md, MD_DIMER, 2, 0, c, max_steps, n_steps_out, converged_out, fmax_out, nullptr,
                     (cudaStream_t)stream, &dm);
+}
+
+int sgdml_b200_irc_rk4(sgdml_b200_md* md, const double* modes, int64_t max_points, double step, double fmax,
+                       double* R_path, double* E_path, int64_t* n_points_out, int* end_out, double* fmax_out,
+                       void* stream) {
+  SG_TRY(require_device());
+  SG_TRY(check_kind(md, "sgdml_b200_irc_rk4", PLAIN_KIND));
+  if (md->n_rep % 2 != 0) return fail_arg("sgdml_b200_irc_rk4: n_rep must be even (two branches per saddle)");
+  if (!md->has_state) return fail_arg("sgdml_b200_irc_rk4: no state yet (call sgdml_b200_md_set_state)");
+  SG_ARG(modes != nullptr);
+  SG_ARG(max_points >= 2 && max_points <= INT64_MAX / 4 / md->n_rep / md->dimi);
+  SG_ARG(std::isfinite(step) && step > 0.0);
+  SG_ARG(std::isfinite(fmax) && fmax >= 0.0);
+  StepParams c = {};
+  IrcParams& q = c.irc;
+  q.h = step;
+  q.hh = step / 2.0;
+  q.h6 = step / 6.0;
+  q.fmax2 = fmax * fmax;
+  q.max_points = max_points;
+  const IrcRun ir = {modes, R_path, E_path};
+  return relax_impl(md, MD_IRC, 1, 0, c, 4 * (max_points - 1), n_points_out, end_out, fmax_out, nullptr,
+                    (cudaStream_t)stream, nullptr, &ir);
 }
 
 int sgdml_b200_set_relax_block(int64_t n_steps) {

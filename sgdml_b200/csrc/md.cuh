@@ -1,8 +1,9 @@
 // Molecular dynamics on the device (sgdml_b200_md_*, sgdml_b200_remd_run, sgdml_b200_npt_*, sgdml_b200_metad_*,
-// sgdml_b200_umbrella_*, sgdml_b200_pimd_*, sgdml_b200_relax_*, sgdml_b200_neb_fire, sgdml_b200_dimer_fire): the
-// contract of the kernels in md.cu -- the BAOAB integrator step, the replica exchange, the NPT step, the metadynamics
-// bias, the umbrella restraints and their exchange, the ring-polymer step, their counter-based noise, the FIRE and
-// L-BFGS steps, the nudged elastic band and the dimer search -- and of MBAR in mbar.cu.
+// sgdml_b200_umbrella_*, sgdml_b200_pimd_*, sgdml_b200_relax_*, sgdml_b200_neb_fire, sgdml_b200_dimer_fire,
+// sgdml_b200_irc_rk4): the contract of the kernels in md.cu -- the BAOAB integrator step, the replica exchange, the NPT
+// step, the metadynamics bias, the umbrella restraints and their exchange, the ring-polymer step, their counter-based
+// noise, the FIRE and L-BFGS steps, the nudged elastic band, the dimer search and the reaction path -- and of MBAR in
+// mbar.cu.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -406,6 +407,56 @@ struct DimerParams {
   double rot_min;              // below this |rotational force| (force / L^2) the dimer translates without rotating
   double fmax2, maxstep, dt0, dtmax;  // the centre's FIRE, as in RelaxParams
   int periodic;                // 1: remove the translations only
+};
+
+// Intrinsic reaction coordinate (sgdml_b200_irc_rk4): the steepest-descent path from a first-order saddle in
+// mass-weighted coordinates x_i = R_i / r_i, r_i = sqrt(s_i) with s the handle's inverse masses (the path's geometry
+// depends on mass ratios only, so no other mass unit enters), followed downhill in both directions along the saddle's
+// imaginary mode by classical RK4 on dx/ds = d(F(x)) (Schmidt, Gordon & Dupuis, JACS 107, 2585 (1985)).  The handle's
+// n_rep = 2 n_pairs replicas: pair k is replicas 2k (forward, sigma = +1) and 2k + 1 (backward, sigma = -1), one branch
+// each.  No rigid-mode projection: sGDML energies are exactly invariant under rotations and translations, so the
+// mass-weighted gradient has no rigid part beyond rounding.  Every sum is block_sum's over the branch's 3N coordinates
+// and every operation rounds as written (no fused multiply-add):
+//   r_i = sqrt(s_i);  g_i = r_i F_i;  q = sum_i g_i g_i;  d_i = g_i / sqrt(q)  (d = 0 when q == 0: no division)
+//
+// k_irc_init: one CTA of MD_THREADS per pair, launched twice before the force evaluation of a call.
+//   check (commit == 0): the caller's mode m (n_pairs, 3N), a Cartesian displacement, in the scratch rows V:
+//     v_i = m_i / r_i;  q = sum_i v_i v_i;  v_i = v_i / sqrt(q);  bad[k] = !(q finite and q > 0)
+//     Nothing of the handle changes; the driver reads every verdict back and commits only when no mode is bad.
+//   commit (commit == 1), with R0, F0, E0 replica 2k's state (the saddle, as set_state stored it), for both branches b:
+//     Rn_b = R0, Fn_b = F0 (point 0: the saddle);  R_b,i = R0_i + r_i ((sigma h) v_i)  (point 1);
+//     IrcState {phase IRC_POINT, n_points 1, E_n E0};  path row 0 = (R0, E0), every other path entry NaN.
+//   The driver then evaluates F and E of every replica (point 1).
+//
+// k_irc_step: one CTA of MD_THREADS per branch, its RelaxState z and IrcState y; R, F, E are the replica's state and
+// F, E always belong to the positions in R.  Each launch, for a branch that has not ended (an ended one is frozen):
+//   1. IRC_POINT (R is a new point n + 1):  if !(E < E_n) (a rise, or NaN): R, F, E = Rn, Fn, E_n (point n again),
+//      fmax2 = atom_max2(Fn), end = 2.  Otherwise the point is recorded: Rn = R, Fn = F, path row n_points = (R, E),
+//      n_points += 1, E_n = E, fmax2 = atom_max2(F), and end = 1 if fmax2 < fmax2_thr (ASE's criterion, as relax),
+//      else 3 if n_points == max_points.  phase = IRC_K1.  z.n_steps = n_points and z.conv = end (k_relax_count and
+//      k_relax_report read them).  advance == 0 stops here, and an ended branch stops here.
+//   2. Stages (advance == 1 only), d the direction of the current F, K the branch's running sum (3N):
+//      IRC_K1:  K_i = d_i;            R_i = Rn_i + r_i (hh d_i);    phase IRC_K2
+//      IRC_K2:  K_i = K_i + 2 d_i;    R_i = Rn_i + r_i (hh d_i);    phase IRC_K3
+//      IRC_K3:  K_i = K_i + 2 d_i;    R_i = Rn_i + r_i (h d_i);     phase IRC_K4
+//      IRC_K4:  K_i = K_i + d_i;      R_i = Rn_i + r_i (h6 K_i);    phase IRC_POINT
+//      so that R_n+1 = R_n + (h / 6) r (((k1 + 2 k2) + 2 k3) + k4), summed in that order.
+// hh = h / 2 and h6 = h / 6 are computed once on the host, so the kernels and tests/irc_oracle.py use the same doubles.
+// One point costs four force evaluations (one step-graph replay each); point 1 costs the one after the commit.
+enum IrcPhase { IRC_POINT = 0, IRC_K1 = 1, IRC_K2 = 2, IRC_K3 = 3, IRC_K4 = 4 };
+
+struct IrcState {    // per branch, written by k_irc_init's commit at the start of every call
+  int phase;
+  int end;           // 0: running;  1: max_a |F_a| < fmax;  2: energy rise;  3: max_points points
+  int64_t n_points;  // points recorded, the saddle included
+  double E_n;        // the energy of the newest point
+};
+
+struct IrcParams {
+  double h, hh, h6;            // the step (mass-weighted unit), h / 2, h / 6
+  double fmax2;                // fmax^2 (0: never ends by force)
+  int64_t max_points;          // >= 2
+  double *R_path, *E_path;     // (n_rep, max_points, 3N) / (n_rep, max_points), device pointers or null
 };
 
 }  // namespace sgdml

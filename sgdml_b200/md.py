@@ -19,7 +19,8 @@ same CVs with replica exchange between neighbouring windows (``sgdml_b200_umbrel
 ``GDMLRelaxation`` -- geometry optimisation of many replicas on the same engine (``sgdml_b200_relax_*``): FIRE and
 L-BFGS, each replica frozen once it has converged.  ``GDMLNEB`` and ``GDMLDimer`` find saddle points on it: between
 two minima with the nudged elastic band (``sgdml_b200_neb_fire``), or next to one minimum with the dimer method
-(``sgdml_b200_dimer_fire``).
+(``sgdml_b200_dimer_fire``).  ``GDMLIRC`` follows the intrinsic reaction coordinate down from a saddle to the two minima
+it connects (``sgdml_b200_irc_rk4``).
 
 Units follow ASE and ``intf.ase_calc.SGDMLCalculator``: positions in Angstrom, velocities in Angstrom/fs, masses in
 amu, energies in eV, time in fs, temperature in K.  ``E_to_eV`` and ``F_to_eV_Ang`` convert the model's units as in
@@ -1122,19 +1123,7 @@ class GDMLDimer(GDMLRelaxation):
 
     def _per_dimer(self, x, name):
         """(n_dimers, N, 3) or (N, 3) -> (n_dimers, 3N), the same kind; torch inputs must be float64 CUDA tensors."""
-        if hasattr(x, 'data_ptr'):
-            _check_cuda_f64(x, name)
-        shape = tuple(x.shape)
-        N = self.n_atoms
-        if shape == (N, 3):
-            x = x.reshape(1, N, 3)
-            x = x.expand(self.n_dimers, N, 3) if hasattr(x, 'data_ptr') else np.broadcast_to(x, (self.n_dimers, N, 3))
-        elif shape != (self.n_dimers, N, 3):
-            raise ValueError('%s must be (n_dimers, N, 3) = (%d, %d, 3) or (N, 3): %s'
-                             % (name, self.n_dimers, N, shape))
-        if hasattr(x, 'data_ptr'):
-            return x.reshape(self.n_dimers, 3 * N).contiguous()
-        return np.ascontiguousarray(x, dtype=np.float64).reshape(self.n_dimers, 3 * N)
+        return _per_unit(x, name, self.n_dimers, self.n_atoms, 'n_dimers')
 
     # ------------------------------------------------------------------ model units
     def _dimer_raw(self, modes, max_steps, fmax, separation, cos_trial, sin_trial, rot_min, maxstep, dt, dtmax):
@@ -1185,6 +1174,105 @@ class GDMLDimer(GDMLRelaxation):
         return {'positions': st['positions'][0::2].reshape(g), 'forces': st['forces'][0::2].reshape(g),
                 'potential_energy': st['potential_energy'][0::2], 'mode': mode.reshape(g), 'curvature': curv * c,
                 'fmax': fm * self.F_to_eV_Ang, 'converged': conv != 0, 'n_steps': n_steps, 'n_rotations': n_rot}
+
+
+class GDMLIRC(GDMLRelaxation):
+    """Which two minima a first-order saddle connects: the intrinsic reaction coordinate (IRC), the steepest-descent
+    path in mass-weighted coordinates, followed downhill from each saddle in both directions along its imaginary mode
+    on the device (``sgdml_b200_irc_rk4``), by classical RK4 with a fixed step (Schmidt, Gordon & Dupuis, JACS 107,
+    2585 (1985)); `n_saddles` saddles, two branches each, many points per call.  Branch j of saddle k is replica 2k + j
+    of a ``GDMLRelaxation`` handle that carries the real inverse masses (masses (N,) in amu), so the inherited ``relax``
+    works on the branch ends.
+
+    ``run(saddles, modes, step=0.05, max_points=500, fmax=0.05, relax_ends=True, relax_steps=1000)``: saddles
+    (n_saddles, N, 3) or (N, 3) in Angstrom; modes of the same shape, the Cartesian displacement of each saddle's
+    imaginary mode in any length (``GDMLVibrations.analyse(saddle)['modes'][:, 0]``, or a dimer's mode); step in
+    amu^1/2 Angstrom (the default is close to the common 0.1 amu^1/2 bohr); fmax in eV/Angstrom.  Branch 0 follows
+    +mode, branch 1 -mode.  A branch ends when a new point's energy is not below the last one's (end 2, at the last
+    point), when max_a |F_a| < fmax (end 1) or at max_points points (end 3).  Returns {'positions' (n_saddles, 2,
+    max_points, N, 3), 'energies' (n_saddles, 2, max_points), 's' (n_saddles, 2, max_points): the signed mass-weighted
+    arc length in amu^1/2 Angstrom (+ forward, - backward), n step at point n, which RK4 integrates as the arc length;
+    all NaN past the branch's point count; 'n_points', 'end', 'fmax' (n_saddles, 2)} in Angstrom and eV.  With relax_ends, L-BFGS (``relax`` at the same fmax, relax_steps steps) then
+    takes the branch ends to their minima: 'minima' {'positions' (n_saddles, 2, N, 3), 'potential_energy', 'converged',
+    'fmax' (n_saddles, 2)} and 'barriers' (n_saddles, 2), the saddle's energy minus each minimum's.  NumPy arrays or
+    float64 CUDA tensors in, the same kind out."""
+
+    def __init__(self, model, masses, n_saddles=1, E_to_eV=_KCAL_PER_MOL_IN_EV, F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
+        self.n_saddles = int(n_saddles)
+        if self.n_saddles < 1:
+            raise ValueError('n_saddles must be >= 1')
+        GDMLDynamics.__init__(self, model, masses, 2 * self.n_saddles, E_to_eV, F_to_eV_Ang)
+
+    # ------------------------------------------------------------------ model units
+    def _irc_raw(self, modes, max_points, step, fmax):
+        """modes (n_saddles, 3N) -> (R_path (n_rep, max_points, 3N), E_path (n_rep, max_points), n_points, end, fmax
+        (n_rep,)), in model units; step in the handle's mass-weighted unit."""
+        if hasattr(modes, 'data_ptr'):  # the entry point copies n_saddles 3N doubles from this pointer
+            _check_cuda_f64(modes, 'modes')
+            modes = modes.contiguous()
+        else:
+            modes = np.ascontiguousarray(modes, dtype=np.float64)
+        if tuple(modes.shape) != (self.n_saddles, 3 * self.n_atoms):
+            raise ValueError('modes must be (n_saddles, 3N) = (%d, %d): %s' % (self.n_saddles, 3 * self.n_atoms,
+                                                                                tuple(modes.shape)))
+        n, mp = self.n_replicas, int(max_points)
+        out = (self._empty((n, max(mp, 0), 3 * self.n_atoms)), self._empty((n, max(mp, 0))), self._empty(n, np.int64),
+               self._empty(n, np.int32), self._empty(n))
+        _lib.check(
+            _lib.lib().sgdml_b200_irc_rk4(self._handle, _lib.ptr(modes), mp, float(step), float(fmax),
+                                          *(_lib.ptr(x) for x in out), _lib.current_stream()),
+            'irc_rk4',
+        )
+        return out
+
+    # ------------------------------------------------------------------ ASE units
+    def run(self, saddles, modes, step=0.05, max_points=500, fmax=0.05, relax_ends=True, relax_steps=1000):
+        # both are checked before the state changes
+        R = _per_unit(saddles, 'saddles', self.n_saddles, self.n_atoms, 'n_saddles')
+        modes = _per_unit(modes, 'modes', self.n_saddles, self.n_atoms, 'n_saddles')
+        if not (math.isfinite(float(step)) and float(step) > 0.0):
+            raise ValueError('step must be finite and > 0')
+        R = R.repeat_interleave(2, 0) if hasattr(R, 'data_ptr') else np.repeat(R, 2, axis=0)
+        self.set_state(R.reshape(self.n_replicas, self.n_atoms, 3))
+        # x = R / sqrt(inv_mass): amu^1/2 Angstrom -> the handle's unit (model length over sqrt of its inverse mass)
+        c = self.F_to_eV_Ang * self.Ang_to_R * FS**2
+        Rp, Ep, n_points, end, fm = self._irc_raw(modes, max_points, float(step) * self.Ang_to_R / math.sqrt(c),
+                                                  float(fmax) / self.F_to_eV_Ang)
+        g, mp = (self.n_saddles, 2), int(max_points)
+        k = np.arange(mp, dtype=np.float64)[None, None, :]
+        npt = _host(n_points).reshape(g + (1,))
+        s = np.where(k < npt, np.array([1.0, -1.0])[None, :, None] * k * float(step), np.nan)
+        if hasattr(Ep, 'data_ptr'):
+            import torch
+
+            s = torch.from_numpy(s).to(Ep.device)
+        out = {'positions': (Rp / self.Ang_to_R).reshape(g + (mp, self.n_atoms, 3)),
+               'energies': (Ep * self.E_to_eV).reshape(g + (mp,)), 's': s, 'n_points': n_points.reshape(g),
+               'end': end.reshape(g), 'fmax': (fm * self.F_to_eV_Ang).reshape(g)}
+        if relax_ends:
+            m = self.relax(fmax=fmax, max_steps=relax_steps)
+            E_min = m['potential_energy'].reshape(g)
+            out['minima'] = {'positions': m['positions'].reshape(g + (self.n_atoms, 3)), 'potential_energy': E_min,
+                             'converged': m['converged'].reshape(g), 'fmax': m['fmax'].reshape(g)}
+            out['barriers'] = out['energies'][:, :, 0] - E_min
+        return out
+
+
+def _per_unit(x, name, n, N, what):
+    """(n, N, 3) or (N, 3) -> (n, 3N), the same kind; torch inputs must be float64 CUDA tensors.  what: n's name."""
+    if hasattr(x, 'data_ptr'):
+        _check_cuda_f64(x, name)
+    else:
+        x = np.asarray(x)
+    shape = tuple(x.shape)
+    if shape == (N, 3):
+        x = x.reshape(1, N, 3)
+        x = x.expand(n, N, 3) if hasattr(x, 'data_ptr') else np.broadcast_to(x, (n, N, 3))
+    elif shape != (n, N, 3):
+        raise ValueError('%s must be (%s, N, 3) = (%d, %d, 3) or (N, 3): %s' % (name, what, n, N, shape))
+    if hasattr(x, 'data_ptr'):
+        return x.reshape(n, 3 * N).contiguous()
+    return np.ascontiguousarray(x, dtype=np.float64).reshape(n, 3 * N)
 
 
 def _check_cuda_f64(x, name):

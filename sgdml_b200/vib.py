@@ -48,7 +48,11 @@ class GDMLVibrations(object):
     """Normal modes of a model at many geometries.
 
     model: a model dict or .npz path, or a ``GDMLPredict``.  masses: (N,) in amu.  A model with a cell is periodic: its
-    rigid modes are the 3 translations only."""
+    rigid modes are the 3 translations only.
+
+    The transition-state workflow: a saddle (``GDMLNEB``, ``GDMLDimer``) -> ``analyse(saddle)`` (exactly one imaginary
+    mode) -> ``GDMLIRC(model, masses).run(saddle, modes[:, 0])`` -> the two minima it connects -> ``harmonic_rate`` from
+    each of them over the saddle."""
 
     def __init__(self, model, masses, E_to_eV=_KCAL_PER_MOL_IN_EV, F_to_eV_Ang=_KCAL_PER_MOL_IN_EV):
         import torch
@@ -161,7 +165,9 @@ def harmonic_rate(minimum, saddle, temperature_K):
       k = (prod_i nu_i^min / prod_j nu_j^saddle) exp(-(E_saddle - E_min) / kT),
     nu = hbar omega / h over the vibrations (the saddle's real ones), evaluated in log space.  Returns {'rate'} in s^-1,
     {'prefactor'} in s^-1, {'barrier'} in eV and {'log_rate'}.  Raises ValueError unless every minimum has no imaginary
-    mode, every saddle exactly one, and both have the same number of rigid modes."""
+    mode, every saddle exactly one, and both have the same number of rigid modes.  Which minimum a saddle leads to is
+    the caller's claim; ``GDMLIRC.run(saddle, analyse(saddle)['modes'][:, 0])`` finds the two minima it connects, one
+    rate per direction."""
     T = float(temperature_K)
     if not T > 0.0 or not math.isfinite(T):
         raise ValueError('temperature_K must be finite and > 0')

@@ -132,17 +132,22 @@ int sgdml_b200_predict_virial_cells(sgdml_b200_model* model, const double* R, in
  * (sgdml_b200/torchtools.py); it costs about one more prediction.  It runs the four contractions as FP64 GEMMs on query
  * rows stacked with their tangent rows, for every descriptor size and whatever sgdml_b200_model_set_contraction_slices
  * chose.  The first call on a model with D <= 256 keeps transposed copies of its training matrices, which
- * sgdml_b200_model_set_alphas refreshes from then on.  Its workspace is separate from sgdml_b200_predict's, whose results
- * and captured graphs it does not change.  A rejected call writes nothing. */
+ * sgdml_b200_model_set_alphas refreshes from then on.
+ * Workspace: shared with sgdml_b200_predict_hessian and separate from sgdml_b200_predict's, whose results and captured
+ * graphs it does not change.  It grows to the largest request seen and never shrinks, so calls of either entry point at
+ * sizes already seen neither allocate nor synchronise the device.  One chunk rule serves both: a stacked row (query or
+ * tangent) takes DS + 2 Mpad + DP + 2 doubles, a chunk at most ~2 GB of them and at most 65 536 geometries; a geometry
+ * needs (1 + n_dir) S rows, n_dir = 1 here, and sgdml_b200_set_predict_chunk(c), c > 0, caps a chunk at 2 c S rows, that
+ * is c geometries.  A rejected call writes nothing. */
 int sgdml_b200_predict_hvp(sgdml_b200_model* model, const double* R, const double* V, int64_t n_geo,
                            double* HV, void* stream);
 
 /* Extension: the energy Hessian H = d^2E/dR^2 = -dF/dR of every geometry, in the model's units and cell, FP64 always.
  *   R (B, 3N) -> H (B, 3N, 3N) row-major; host or device as in sgdml_b200_predict.
  * Column i of H[b] equals -sgdml_b200_predict_hvp(R[b], e_i) bit for bit (e_i the i-th unit vector): it is that
- * product's arithmetic with the S query rows of a geometry built once and shared by its 3N tangent rows J e_i.  H is
- * returned as computed, not symmetrised.  Energy-constrained models (alphas_E) and every descriptor size are covered.
- * Workspace: separate from sgdml_b200_predict's and sgdml_b200_predict_hvp's, within ~2 GB.  A chunk holds whole
+ * product's pipeline with n_dir = 3N directions, the S query rows of a geometry built once and shared by its 3N tangent
+ * rows J e_i.  H is returned as computed, not symmetrised.  Energy-constrained models (alphas_E) and every descriptor
+ * size are covered.  Workspace and chunk rule: those of sgdml_b200_predict_hvp, with n_dir = 3N.  A chunk holds whole
  * geometries when (1 + 3N) S stacked rows fit; otherwise one geometry whose 3N columns run in blocks of consecutive
  * directions.  sgdml_b200_set_predict_chunk(c), c > 0, caps a chunk at 2 c S rows: floor(2 c / (3N + 1)) geometries,
  * or, when that is 0, one geometry in blocks of 2 c - 1 directions (c = 1: one column per block).  A rejected call
@@ -607,12 +612,13 @@ int sgdml_b200_predict_train_virial(sgdml_b200_model* model, int64_t m_begin, in
  * (iterative.py:183-204: tolerance 1e-4).  No effect for D <= 256. */
 int sgdml_b200_model_set_contraction_slices(sgdml_b200_model* model, int slices, void* stream);
 
-/* Test hook: at most max_geos queries (or training points) per chunk of sgdml_b200_predict,
- * sgdml_b200_predict_train and sgdml_b200_predict_hvp, for every model, and 2 max_geos S rows per chunk of
- * sgdml_b200_predict_hessian (see there); 0 = no cap (the default: chunks bounded by workspace size only).  Negative
- * values are rejected.  The cap also bounds the minimum per-batch workspace, which limits how far small batches split
- * the sweep over the training points.  Workspaces never shrink: it applies fully to models created after the call.
- * Tests lower it to cover the multi-chunk, pipelined and tail-chunk paths at small batch sizes. */
+/* Test hook: at most max_geos queries (or training points) per chunk of sgdml_b200_predict and
+ * sgdml_b200_predict_train, for every model, and 2 max_geos S stacked rows per chunk of sgdml_b200_predict_hvp and
+ * sgdml_b200_predict_hessian (their one chunk rule, see sgdml_b200_predict_hvp: max_geos geometries for the HVP);
+ * 0 = no cap (the default: chunks bounded by workspace size only).  Negative values are rejected.  The cap also bounds
+ * the minimum per-batch workspace, which limits how far small batches split the sweep over the training points.
+ * Workspaces never shrink: it applies fully to models created after the call.  Tests lower it to cover the
+ * multi-chunk, pipelined and tail-chunk paths at small batch sizes. */
 int sgdml_b200_set_predict_chunk(int64_t max_geos);
 
 /* Test hook (large-descriptor models): the stages of one chunk of the GEMM-composed predictor, copied out of the

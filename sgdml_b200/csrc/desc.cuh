@@ -47,7 +47,7 @@ __device__ __forceinline__ void minimum_image(const Lattice& lat, double& dx, do
 }
 
 // (J v)_d = g_d . (v_b - v_a) for pair d = (a, b), v read through v(i): k_d_desc_dot_vec's arithmetic, also the tangent
-// rows of sgdml_b200_predict_hessian (v = e_i, where every product is exact)
+// rows of sgdml_b200_predict_hvp (v a row of V) and sgdml_b200_predict_hessian (v = e_i, where every product is exact)
 template <class VecAt>
 __device__ __forceinline__ double d_desc_dot(const double* gd, int a, int b, VecAt v) {
   double s = gd[0] * (v(3 * b + 0) - v(3 * a + 0));

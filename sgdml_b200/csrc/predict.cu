@@ -1229,11 +1229,14 @@ __global__ void k_unpad_rows(const double* __restrict__ src, int M, int D, int D
   dst[idx] = src[(int64_t)m * DS + d];
 }
 
-// ============================================================== Hessian-vector product (sgdml_b200_predict_hvp)
-// HV = (dF/dR) V = -H V per geometry: the derivative of the GEMM-composed prediction along V.  The descriptor moves along
-// t = J V (k_d_desc_dot_vec); each virtual row q gets a companion tangent row T (t permuted like q, not centred), stacked
-// below the query rows, so that every GEMM of the large-descriptor path runs once on 2 x rows.  With S3 = T Xc^T,
-// S4 = T JA^T, delta = q - Xc_m, n = sqrt5 |delta|, e = exp(-n/sig), a = delta . JA_m:
+// ============================================================== tangent derivatives of the forces
+// (sgdml_b200_predict_hvp, sgdml_b200_predict_hessian)
+// HV = (dF/dR) V = -H V per geometry and direction V: the derivative of the GEMM-composed prediction along V.  The HVP
+// has one direction per geometry, a row of the caller's V; the Hessian has the 3N unit vectors, column i of H being -HV
+// at V = e_i, run in blocks of consecutive directions.  The descriptor moves along t = J V; each virtual row q gets a
+// companion tangent row T per direction (t permuted like q, not centred: k_tangent_rows), stacked below the query rows,
+// so that every GEMM of the large-descriptor path runs once on all of them.  With S3 = T Xc^T, S4 = T JA^T,
+// delta = q - Xc_m, n = sqrt5 |delta|, e = exp(-n/sig), a = delta . JA_m:
 //   ds = delta . T = q.t - S3,  da = S4,
 //   dc2 = -5 k_base e ds / sig                       (n cancels: no singularity)
 //   dc1 = k_c1 e (da - 5 a ds / (n sig))  [+ ae dc2]
@@ -1252,8 +1255,8 @@ constexpr double HVP_X5_FLOOR = 5.0 * 64.0 * 2.220446049250313e-16;
 
 // Which rows k_transform_tangent_rows and k_combine_tangent_rows serve.  Query rows come first (n_rows of them), then the
 // tangent rows.  The tangent rows of one geometry are laid out [direction][permutation], so tangent row t belongs to
-// query row (t / dir_rows) S + t % S with dir_rows = directions x S (the HVP has one direction: t serves query row t).
-//   TAN_PAIRED: the HVP: warp w takes query row w and tangent row w together, C1 / C2 overwrite S1 / S2 in place
+// query row (t / dir_rows) S + t % S with dir_rows = directions x S (one direction: t serves query row t).
+//   TAN_PAIRED: one direction: warp w takes query row w and tangent row w together, C1 / C2 overwrite S1 / S2 in place
 //   TAN_ONLY:   tangent rows only; they read their query row's S1 / S2, which stay in place for the other tangent rows
 //   TAN_QUERY:  query rows only (after TAN_ONLY, when one query row serves many tangent rows)
 enum TanMode { TAN_PAIRED = 0, TAN_ONLY = 1, TAN_QUERY = 2 };
@@ -1359,7 +1362,7 @@ __global__ void k_combine_tangent_rows(const double* __restrict__ Qg, int64_t ld
   }
 }
 
-// Row k of HV for one geometry (k_hvp_project), V read through v(i):  HV[k] = sum_d s_kd (g_d dF_desc[d] + dg_d
+// Row k of HV for one geometry and direction, V read through v(i):  HV[k] = sum_d s_kd (g_d dF_desc[d] + dg_d
 // F_desc[d]), s_kd = +1 for atom b and -1 for atom a of pair d = (a, b), a > b (the signs of k_vec_dot_d_desc), where
 //   dg_d = d(delta / |delta|^3) = dd / |delta|^3 - 3 delta (delta . dd) / |delta|^5,   dd = v_a - v_b,
 // with the minimum-image pair vector delta rebuilt from g_d as the virial kernels do (|g| = |delta|^-2):
@@ -1389,77 +1392,80 @@ __device__ __forceinline__ void hvp_atom(const double* __restrict__ f, const dou
   }
 }
 
-// One thread per (geometry, atom k)
-__global__ void __launch_bounds__(256) k_hvp_project(const double* __restrict__ Fd, const double* __restrict__ dFd,
-                                                     const double* __restrict__ gq, const double* __restrict__ V,
-                                                     int n_atoms, int D, double std, int64_t n_geo,
-                                                     double* __restrict__ HV) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n_geo * n_atoms) return;
-  const int64_t b = idx / n_atoms;
-  const int k = (int)(idx - b * n_atoms);
-  const double* v = V + b * 3 * n_atoms;
-  double h0, h1, h2;
-  hvp_atom(Fd + b * D, dFd + b * D, gq + b * (int64_t)D * 3, [v](int i) { return v[i]; }, n_atoms, k, h0, h1, h2);
-  HV[idx * 3 + 0] = h0 * std;
-  HV[idx * 3 + 1] = h1 * std;
-  HV[idx * 3 + 2] = h2 * std;
+// Where the directions of a block come from: DIR_V, row b of the caller's V (the HVP: one direction per geometry), or
+// DIR_UNIT, the unit vectors e_i0 .. e_(i0 + n_dir - 1) (the Hessian).  A template parameter, so that each source keeps
+// its own instruction sequence.
+enum DirSource { DIR_V = 0, DIR_UNIT = 1 };
+
+// Direction `col` of geometry b, read through v(i)
+template <int DIRS>
+__device__ __forceinline__ auto direction(const double* __restrict__ V, int n_atoms, int64_t b, int col) {
+  if constexpr (DIRS == DIR_UNIT) {
+    return [col](int i) { return i == col ? 1.0 : 0.0; };
+  } else {
+    const double* v = V + b * 3 * n_atoms;
+    return [v](int i) { return v[i]; };
+  }
 }
 
-// ============================================================== Hessians (sgdml_b200_predict_hessian)
-// Column i of H is -HV at V = e_i: the HVP's arithmetic with the S query rows of a geometry built once and shared by its
-// 3N tangent rows per permutation, t_i = J e_i.  A direction block holds n_dir consecutive columns i0 .. i0 + n_dir - 1;
-// its tangent rows are laid out [geometry][direction][permutation], so that k_fdesc_gather folds each direction like a
-// geometry of its own.
-
-// One warp per tangent row (geometry b, direction i0 + j, permutation p): t = J e_i permuted like the query row, built
-// from the pair gradients gq with k_d_desc_dot_vec's arithmetic (every product exact: the bits of J e_i)
-__global__ void __launch_bounds__(256) k_hessian_tangent_rows(const double* __restrict__ gq,
-                                                              const int* __restrict__ pinv, int n_atoms, int D, int DS,
-                                                              int S, int i0, int n_dir, int64_t n_rows,
-                                                              double* __restrict__ T) {
+// One warp per tangent row (geometry b, direction i0 + j, permutation p), laid out [geometry][direction][permutation] so
+// that k_fdesc_gather folds each direction like a geometry of its own: t = J v permuted like the query row, built from
+// the pair gradients gq with k_d_desc_dot_vec's arithmetic (for e_i every product is exact: the bits of J e_i)
+template <int DIRS>
+__global__ void __launch_bounds__(256) k_tangent_rows(const double* __restrict__ gq, const double* __restrict__ V,
+                                                      const int* __restrict__ pinv, int n_atoms, int D, int DS, int S,
+                                                      int i0, int n_dir, int64_t n_rows, double* __restrict__ T) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= n_rows) return;
+  const int nd = DIRS == DIR_UNIT ? n_dir : 1;
   const int64_t bj = row / S;
   const int p = (int)(row - bj * S);
-  const int64_t b = bj / n_dir;
-  const int col = i0 + (int)(bj - b * n_dir);
+  const int64_t b = bj / nd;
+  const auto dir = direction<DIRS>(V, n_atoms, b, i0 + (int)(bj - b * nd));
   const double* g = gq + b * (int64_t)D * 3;
   const int* pi = pinv + (int64_t)p * D;
-  const auto unit = [col](int i) { return i == col ? 1.0 : 0.0; };
   for (int e = lane; e < DS; e += 32) {
     double v = 0.0;
     if (e < D) {
       const int d = pi[e];
       int a, bb;
       pair_from_d(d, a, bb);
-      v = d_desc_dot(g + (int64_t)d * 3, a, bb, unit);
+      v = d_desc_dot(g + (int64_t)d * 3, a, bb, dir);
     }
     T[row * DS + e] = v;
   }
 }
 
-// One thread per (geometry b, atom k, direction j): rows 3k .. 3k + 2 of column i0 + j of H[b] (n x n, n = 3N), as
-// k_hvp_project writes HV at V = e_i, negated
-__global__ void __launch_bounds__(256) k_hessian_project(const double* __restrict__ Fd, const double* __restrict__ dFd,
-                                                         const double* __restrict__ gq, int n_atoms, int D, double std,
-                                                         int64_t n_geo, int i0, int n_dir, double* __restrict__ H) {
+// One thread per (geometry b, atom k, direction j): rows 3k .. 3k + 2 of column i0 + j of out[b] (3N x n_cols): HV with
+// n_cols = 1 (DIR_V), or H = -HV at e_i with n_cols = 3N (DIR_UNIT)
+template <int DIRS>
+__global__ void __launch_bounds__(256) k_tangent_project(const double* __restrict__ Fd, const double* __restrict__ dFd,
+                                                         const double* __restrict__ gq, const double* __restrict__ V,
+                                                         int n_atoms, int D, double std, int64_t n_geo, int i0,
+                                                         int n_dir, double* __restrict__ out) {
+  const int nd = DIRS == DIR_UNIT ? n_dir : 1;
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n_geo * n_atoms * n_dir) return;
-  const int64_t bk = idx / n_dir;
-  const int j = (int)(idx - bk * n_dir);
+  if (idx >= n_geo * n_atoms * nd) return;
+  const int64_t bk = idx / nd;
+  const int j = (int)(idx - bk * nd);
   const int64_t b = bk / n_atoms;
   const int k = (int)(bk - b * n_atoms);
   const int col = i0 + j;
-  const int64_t n = 3 * (int64_t)n_atoms;
+  const int64_t n = 3 * (int64_t)n_atoms, n_cols = DIRS == DIR_UNIT ? n : 1;
   double h0, h1, h2;
-  hvp_atom(Fd + b * D, dFd + (b * n_dir + j) * D, gq + b * (int64_t)D * 3,
-           [col](int i) { return i == col ? 1.0 : 0.0; }, n_atoms, k, h0, h1, h2);
-  double* out = H + b * n * n + (3 * k) * n + col;
-  out[0] = -(h0 * std);
-  out[n] = -(h1 * std);
-  out[2 * n] = -(h2 * std);
+  hvp_atom(Fd + b * D, dFd + (b * nd + j) * D, gq + b * (int64_t)D * 3, direction<DIRS>(V, n_atoms, b, col), n_atoms,
+           k, h0, h1, h2);
+  double* o = out + (b * n + 3 * k) * n_cols + col;
+  if constexpr (DIRS == DIR_UNIT) {
+    o[0] = -(h0 * std);
+    o[n_cols] = -(h1 * std);
+    o[2 * n_cols] = -(h2 * std);
+  } else {
+    o[0] = h0 * std;
+    o[n_cols] = h1 * std;
+    o[2 * n_cols] = h2 * std;
+  }
 }
 
 }  // namespace sgdml
@@ -1496,21 +1502,15 @@ struct sgdml_b200_model {
     Lattice* lat = nullptr;     // (geo) the chunk's cells of a call with one cell per geometry
     OzOperand ozQ, ozC1, ozC2;  // slices of the per-batch operands (int8 path of large descriptors)
   } ws[2];
-  // sgdml_b200_predict_hvp: a workspace of its own, grown on first use (predict's slots, graphs and generation are never
-  // touched).  Query and tangent rows are stacked: Qg, qq, SX (S1; S3), SJ (S2; S4), G (G; dG), csum hold 2 x rows.
-  struct HvpWS {
-    int64_t geo = 0;
-    double *R = nullptr, *V = nullptr, *HV = nullptr, *xq = nullptr, *gq = nullptr, *t = nullptr, *Qg = nullptr,
-           *qq = nullptr, *SX = nullptr, *SJ = nullptr, *G = nullptr, *csum = nullptr, *Fd = nullptr, *dFd = nullptr,
-           *mu0 = nullptr;  // mu0: DS zeros, the "mean" of the tangent rows
-  } hvp;
-  // sgdml_b200_predict_hessian: a workspace of its own as well (hessian_plan): `geo` geometries of query rows and
-  // geo x dirs x S tangent rows stacked below them in Qg, qq, SX, SJ, G, csum; H stages host outputs
-  struct HessWS {
-    int64_t geo = 0, dirs = 0;
-    double *R = nullptr, *xq = nullptr, *gq = nullptr, *Qg = nullptr, *qq = nullptr, *SX = nullptr, *SJ = nullptr,
-           *G = nullptr, *csum = nullptr, *Fd = nullptr, *dFd = nullptr, *H = nullptr;
-  } hess;
+  // sgdml_b200_predict_hvp and sgdml_b200_predict_hessian: one workspace, shared by both and separate from predict's
+  // (whose slots, graphs and generation they never touch).  R, V and Out stage host arrays; the query rows of the chunk
+  // come first and the tangent rows of every direction are stacked below them in Qg, qq, SX (S1; S3), SJ (S2; S4),
+  // G (G; dG) and csum.  Each group of buffers grows to the largest request seen and never shrinks (tangent_plan).
+  struct TangentWS {
+    int64_t geo = 0, rows = 0, geo_dirs = 0, out = 0;  // capacities: geometries, stacked rows, dFd rows, Out doubles
+    double *R = nullptr, *V = nullptr, *Out = nullptr, *xq = nullptr, *gq = nullptr, *Qg = nullptr, *qq = nullptr,
+           *SX = nullptr, *SJ = nullptr, *G = nullptr, *csum = nullptr, *Fd = nullptr, *dFd = nullptr;
+  } tangent;
   cudaStream_t pipe_stream[2] = {nullptr, nullptr};
   cudaEvent_t pipe_event[3] = {nullptr, nullptr, nullptr};
   // MD latency path: the launch sequence of a small host-buffer batch, captured once per batch size into a CUDA graph
@@ -2303,71 +2303,99 @@ int predict_train_impl(sgdml_b200_model* m, int64_t m_begin, int64_t m_end, int 
   return 0;
 }
 
-// ---------------------------------------------------------------- Hessian-vector products
-void free_hvp_ws(sgdml_b200_model::HvpWS& w) {
-  for (double* p : {w.R, w.V, w.HV, w.xq, w.gq, w.t, w.Qg, w.qq, w.SX, w.SJ, w.G, w.csum, w.Fd, w.dFd, w.mu0})
-    cached_free(p);
-  w = sgdml_b200_model::HvpWS();
+// ---------------------------------------------------------------- tangent derivatives (HVP and Hessian)
+void free_tangent_ws(sgdml_b200_model::TangentWS& w) {
+  for (double* p : {w.R, w.V, w.Out, w.xq, w.gq, w.Qg, w.qq, w.SX, w.SJ, w.G, w.csum, w.Fd, w.dFd}) cached_free(p);
+  w = sgdml_b200_model::TangentWS();
 }
 
-// geometries per HVP chunk: S1-S4 (4 x Mpad) and G, dG (2 x DP) per virtual row within ~2 GB
-int64_t hvp_chunk_geos(const sgdml_b200_model* m) {
-  const int64_t row_bytes = 8 * (4 * (int64_t)m->Mpad + 2 * (int64_t)m->DP);
-  int64_t g = (int64_t)(2048ll << 20) / (row_bytes * m->S);
-  g = std::max<int64_t>(1, std::min<int64_t>(g, 65536));
-  if (g_chunk_cap > 0 && g > g_chunk_cap) g = g_chunk_cap;
-  return g;
+// How the tangent pipeline cuts a batch with n_dir directions per geometry (1 for the HVP, 3N for the Hessian):
+// geometries per chunk and directions per block.  A chunk holds at most `rows` stacked rows (Qg, SX, SJ, G, qq and csum:
+// DS + 2 Mpad + DP + 2 doubles each) within ~2 GB, and at most 2 c S rows when sgdml_b200_set_predict_chunk set a cap c
+// (c geometries of one direction).  A geometry needs (1 + n_dir) S rows: whole geometries when at least one fits, at
+// most 65 536 of them, else one geometry per chunk in blocks of rows / S - 1 directions.
+struct TangentPlan {
+  int64_t geo, dirs;
+};
+TangentPlan tangent_plan(const sgdml_b200_model* m, int64_t n_dir) {
+  const int64_t row_bytes = 8 * ((int64_t)m->DS + 2 * (int64_t)m->Mpad + m->DP + 2);
+  int64_t rows = (int64_t)(2048ll << 20) / row_bytes;
+  if (g_chunk_cap > 0) rows = std::min<int64_t>(rows, 2 * g_chunk_cap * m->S);
+  rows = std::max<int64_t>(rows, 2 * (int64_t)m->S);
+  const int64_t geo_rows = (1 + n_dir) * m->S;
+  if (rows >= geo_rows) return {std::min<int64_t>(rows / geo_rows, 65536), n_dir};
+  return {1, rows / m->S - 1};
 }
 
-// The transposed model matrices of the second contraction: kept by large-descriptor models anyway, made on the first HVP
-// of a fused-kernel model (and from then on refreshed by set_alphas); then the workspace for n_geo geometries.
-int ensure_hvp_ws(sgdml_b200_model* m, int64_t n_geo, cudaStream_t s) {
+// Allocates every buffer of w at the capacities it holds
+int alloc_tangent_ws(const sgdml_b200_model* m, sgdml_b200_model::TangentWS& w) {
+  const int64_t dimi = 3 * (int64_t)m->N;
+  SG_CUDA(cached_malloc(&w.R, sizeof(double) * w.geo * dimi));
+  SG_CUDA(cached_malloc(&w.V, sizeof(double) * w.geo * dimi));
+  SG_CUDA(cached_malloc(&w.Out, sizeof(double) * w.out));
+  SG_CUDA(cached_malloc(&w.xq, sizeof(double) * w.geo * m->D));
+  SG_CUDA(cached_malloc(&w.gq, sizeof(double) * w.geo * m->D * 3));
+  SG_CUDA(cached_malloc(&w.Qg, sizeof(double) * w.rows * m->DS));
+  SG_CUDA(cached_malloc(&w.qq, sizeof(double) * w.rows));
+  SG_CUDA(cached_malloc(&w.SX, sizeof(double) * w.rows * m->Mpad));
+  SG_CUDA(cached_malloc(&w.SJ, sizeof(double) * w.rows * m->Mpad));
+  SG_CUDA(cached_malloc(&w.G, sizeof(double) * w.rows * m->DP));
+  SG_CUDA(cached_malloc(&w.csum, sizeof(double) * w.rows));
+  SG_CUDA(cached_malloc(&w.Fd, sizeof(double) * w.geo * m->D));
+  SG_CUDA(cached_malloc(&w.dFd, sizeof(double) * w.geo_dirs * m->D));
+  return 0;
+}
+
+// The transposed model matrices of the second contraction: kept by large-descriptor models anyway, made on the first
+// HVP or Hessian of a fused-kernel model (and from then on refreshed by set_alphas); then the workspace for chunks of
+// `geo` geometries in blocks of `dirs` directions with `out` doubles of staged output, grown to the largest request seen.
+// The old buffers go first; the grown workspace takes their place only once every buffer is allocated, so a failed
+// allocation leaves an empty workspace (no capacity) and the next call allocates again.
+int ensure_tangent_ws(sgdml_b200_model* m, int64_t geo, int64_t dirs, int64_t out, cudaStream_t s) {
   if (m->XcT == nullptr) {
     SG_CUDA(cached_malloc(&m->XcT, sizeof(double) * (size_t)m->DP * m->Mpad));
     SG_CUDA(cached_malloc(&m->JAT, sizeof(double) * (size_t)m->DP * m->Mpad));
     SG_TRY(refresh_transposes(m, true, s));
   }
-  sgdml_b200_model::HvpWS& w = m->hvp;
-  if (n_geo <= w.geo) return 0;
+  sgdml_b200_model::TangentWS& w = m->tangent;
+  const int64_t rows = geo * m->S * (1 + dirs);
+  if (geo <= w.geo && rows <= w.rows && geo * dirs <= w.geo_dirs && out <= w.out) return 0;
   if (w.geo > 0) SG_CUDA(cudaDeviceSynchronize());  // earlier calls may still run on the old workspace
-  free_hvp_ws(w);
-  const int64_t rows2 = 2 * n_geo * m->S;
-  const int64_t dimi = 3 * (int64_t)m->N;
-  SG_CUDA(cached_malloc(&w.R, sizeof(double) * n_geo * dimi));
-  SG_CUDA(cached_malloc(&w.V, sizeof(double) * n_geo * dimi));
-  SG_CUDA(cached_malloc(&w.HV, sizeof(double) * n_geo * dimi));
-  SG_CUDA(cached_malloc(&w.xq, sizeof(double) * n_geo * m->D));
-  SG_CUDA(cached_malloc(&w.gq, sizeof(double) * n_geo * m->D * 3));
-  SG_CUDA(cached_malloc(&w.t, sizeof(double) * n_geo * m->D));
-  SG_CUDA(cached_malloc(&w.Qg, sizeof(double) * rows2 * m->DS));
-  SG_CUDA(cached_malloc(&w.qq, sizeof(double) * rows2));
-  SG_CUDA(cached_malloc(&w.SX, sizeof(double) * rows2 * m->Mpad));
-  SG_CUDA(cached_malloc(&w.SJ, sizeof(double) * rows2 * m->Mpad));
-  SG_CUDA(cached_malloc(&w.G, sizeof(double) * rows2 * m->DP));
-  SG_CUDA(cached_malloc(&w.csum, sizeof(double) * rows2));
-  SG_CUDA(cached_malloc(&w.Fd, sizeof(double) * n_geo * m->D));
-  SG_CUDA(cached_malloc(&w.dFd, sizeof(double) * n_geo * m->D));
-  SG_CUDA(cached_malloc(&w.mu0, sizeof(double) * m->DS));
-  SG_CUDA(cudaMemsetAsync(w.mu0, 0, sizeof(double) * m->DS, s));
-  w.geo = n_geo;
+  sgdml_b200_model::TangentWS n;
+  n.geo = std::max(geo, w.geo);
+  n.rows = std::max(rows, w.rows);
+  n.geo_dirs = std::max(geo * dirs, w.geo_dirs);
+  n.out = std::max(out, w.out);
+  free_tangent_ws(w);
+  const int rc = alloc_tangent_ws(m, n);
+  if (rc != 0) {
+    free_tangent_ws(n);
+    return rc;
+  }
+  w = n;
   return 0;
 }
 
-// sgdml_b200_predict_hvp: always the GEMM-composed form in FP64 (the int8-slice setting of large descriptors does not
-// apply), in the model's cell, chunk by chunk on the caller's stream
-int hvp_impl(sgdml_b200_model* m, const double* R, const double* V, int64_t n_geo, double* HV, cudaStream_t s) {
-  const bool R_dev = is_device_ptr(R), V_dev = is_device_ptr(V);
+// sgdml_b200_predict_hvp (V: one direction per geometry, out (B, 3N)) and sgdml_b200_predict_hessian (V == nullptr: the
+// 3N unit directions, out (B, 3N, 3N)): always the GEMM-composed form in FP64 (the int8-slice setting of large
+// descriptors does not apply), in the model's cell, chunk by chunk on the caller's stream; per direction block the query
+// rows, their tangent rows, both contractions, the folds and the projection
+int tangent_impl(sgdml_b200_model* m, const double* R, const double* V, int64_t n_geo, double* out, cudaStream_t s) {
+  const bool R_dev = is_device_ptr(R), V_dev = V == nullptr || is_device_ptr(V);
   const int dimi = 3 * m->N;
-  const ChunkOut oHV(HV, dimi);
-  const int64_t chunk = std::min<int64_t>(hvp_chunk_geos(m), n_geo);
-  SG_TRY(ensure_hvp_ws(m, chunk, s));
-  sgdml_b200_model::HvpWS& w = m->hvp;
+  const int n_dir = V != nullptr ? 1 : dimi;
+  const ChunkOut o(out, (int64_t)dimi * (V != nullptr ? 1 : dimi));
+  const TangentPlan p = tangent_plan(m, n_dir);
+  const int64_t chunk = std::min<int64_t>(p.geo, n_geo);
+  SG_TRY(ensure_tangent_ws(m, chunk, p.dirs, o.staged() ? chunk * o.k : 0, s));
+  sgdml_b200_model::TangentWS& w = m->tangent;
   const MaternK mk = MaternK::from_sig(m->sig);
+  const double* ae = m->use_ae ? m->ae : nullptr;
   for (int64_t g0 = 0; g0 < n_geo; g0 += chunk) {
     const int64_t ng = std::min<int64_t>(chunk, n_geo - g0);
     const int64_t rows = ng * m->S;
     const double* Rd = R + g0 * dimi;
-    const double* Vd = V + g0 * dimi;
+    const double* Vd = V != nullptr ? V + g0 * dimi : nullptr;
     if (!R_dev) {
       SG_CUDA(cudaMemcpyAsync(w.R, Rd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, s));
       Rd = w.R;
@@ -2376,161 +2404,59 @@ int hvp_impl(sgdml_b200_model* m, const double* R, const double* V, int64_t n_ge
       SG_CUDA(cudaMemcpyAsync(w.V, Vd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, s));
       Vd = w.V;
     }
+    double* oc = o.at(g0, w.Out);
     SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, s, m->lat, nullptr));
-    SG_TRY(launch_d_desc_dot_vec(w.gq, Vd, ng, m->N, w.t, m->D, s));
-    {
-      ProfScope ps(KID_PREDICT_AUX, s);
-      k_query_rows<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(w.xq, m->pinv, m->mu, m->D, m->DS, m->S, rows, rows,
-                                                                w.Qg, w.qq);
-      SG_CUDA(cudaGetLastError());
-      k_query_rows<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(w.t, m->pinv, w.mu0, m->D, m->DS, m->S, rows, rows,
-                                                                w.Qg + rows * m->DS, w.qq + rows);
-      SG_CUDA(cudaGetLastError());
-      count_launch(KID_PREDICT_AUX, 2);
-    }
-    {
-      ProfScope ps(KID_PREDICT_MAIN, s);
-      // [S1; S3] = [Q; T] Xc^T, [S2; S4] = [Q; T] JA^T, then acc = [C1; dC1] XcT^T + [C2; dC2] JAT^T
-      SG_TRY(contract_desc(m, w.Qg, 2 * rows, w.SX, w.SJ, s));
-      k_transform_tangent_rows<TAN_PAIRED><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(
-          w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, m->use_ae ? m->ae : nullptr, m->M, m->Mpad, rows, rows,
-          m->S, m->S, mk, w.csum);
-      SG_CUDA(cudaGetLastError());
-      SG_TRY(contract_points(m, w.SX, w.SJ, 2 * rows, w.G, s));
-      k_combine_tangent_rows<TAN_PAIRED><<<(unsigned)((rows * m->DP + 255) / 256), 256, 0, s>>>(
-          w.Qg, m->DS, w.csum, w.G, m->DP, rows, rows, m->S, m->S);
-      SG_CUDA(cudaGetLastError());
-      count_launch(KID_PREDICT_MAIN, 2);
-    }
-    {
-      ProfScope ps(KID_PREDICT_FINISH, s);
-      const dim3 grid((unsigned)ceil_div(m->D, 256), (unsigned)std::min<int64_t>(ng, 65535));
-      k_fdesc_gather<false><<<grid, 256, 0, s>>>(w.G, m->perm, m->D, m->DP, m->S, 1, rows, ng, w.Fd, nullptr, nullptr);
-      SG_CUDA(cudaGetLastError());
-      k_fdesc_gather<false><<<grid, 256, 0, s>>>(w.G + rows * m->DP, m->perm, m->D, m->DP, m->S, 1, rows, ng, w.dFd,
-                                                 nullptr, nullptr);
-      SG_CUDA(cudaGetLastError());
-      k_hvp_project<<<(unsigned)ceil_div(ng * m->N, 256), 256, 0, s>>>(w.Fd, w.dFd, w.gq, Vd, m->N, m->D, m->std, ng,
-                                                                       oHV.at(g0, w.HV));
-      SG_CUDA(cudaGetLastError());
-      count_launch(KID_PREDICT_FINISH, 3);
-    }
-    SG_TRY(oHV.copy_back(g0, ng, w.HV, s));
-  }
-  if (!R_dev || !V_dev || oHV.staged()) SG_CUDA(cudaStreamSynchronize(s));
-  return 0;
-}
-
-// ---------------------------------------------------------------- Hessians
-void free_hess_ws(sgdml_b200_model::HessWS& w) {
-  for (double* p : {w.R, w.xq, w.gq, w.Qg, w.qq, w.SX, w.SJ, w.G, w.csum, w.Fd, w.dFd, w.H}) cached_free(p);
-  w = sgdml_b200_model::HessWS();
-}
-
-// How sgdml_b200_predict_hessian cuts its work: geometries per chunk and directions (columns) per block.  A chunk holds at
-// most `rows` stacked rows (Qg, SX, SJ and G: DS + 2 Mpad + DP doubles each) within ~2 GB, and at most 2 c S rows when
-// sgdml_b200_set_predict_chunk set a cap c (the rows of c HVP geometries).  A geometry needs (1 + 3N) S rows: whole
-// geometries when at least one fits, else one geometry per chunk in blocks of rows / S - 1 directions.
-struct HessPlan {
-  int64_t geo, dirs;
-};
-HessPlan hessian_plan(const sgdml_b200_model* m) {
-  const int64_t row_bytes = 8 * ((int64_t)m->DS + 2 * (int64_t)m->Mpad + m->DP + 2);
-  int64_t rows = (int64_t)(2048ll << 20) / row_bytes;
-  if (g_chunk_cap > 0) rows = std::min<int64_t>(rows, 2 * g_chunk_cap * m->S);
-  rows = std::max<int64_t>(rows, 2 * (int64_t)m->S);
-  const int64_t n = 3 * (int64_t)m->N, geo_rows = (1 + n) * m->S;
-  if (rows >= geo_rows) return {std::min<int64_t>(rows / geo_rows, 65536), n};
-  return {1, rows / m->S - 1};
-}
-
-int ensure_hess_ws(sgdml_b200_model* m, const HessPlan& p, int64_t n_geo, bool stage_H, cudaStream_t s) {
-  if (m->XcT == nullptr) {
-    SG_CUDA(cached_malloc(&m->XcT, sizeof(double) * (size_t)m->DP * m->Mpad));
-    SG_CUDA(cached_malloc(&m->JAT, sizeof(double) * (size_t)m->DP * m->Mpad));
-    SG_TRY(refresh_transposes(m, true, s));
-  }
-  sgdml_b200_model::HessWS& w = m->hess;
-  const bool H_ok = !stage_H || w.H != nullptr;
-  if (n_geo <= w.geo && p.dirs == w.dirs && H_ok) return 0;
-  n_geo = std::max(n_geo, w.geo);
-  if (w.geo > 0) SG_CUDA(cudaDeviceSynchronize());  // earlier calls may still run on the old workspace
-  const bool had_H = w.H != nullptr;
-  free_hess_ws(w);
-  const int64_t n = 3 * (int64_t)m->N;
-  const int64_t rows = n_geo * m->S * (1 + p.dirs);
-  SG_CUDA(cached_malloc(&w.R, sizeof(double) * n_geo * n));
-  SG_CUDA(cached_malloc(&w.xq, sizeof(double) * n_geo * m->D));
-  SG_CUDA(cached_malloc(&w.gq, sizeof(double) * n_geo * m->D * 3));
-  SG_CUDA(cached_malloc(&w.Qg, sizeof(double) * rows * m->DS));
-  SG_CUDA(cached_malloc(&w.qq, sizeof(double) * rows));
-  SG_CUDA(cached_malloc(&w.SX, sizeof(double) * rows * m->Mpad));
-  SG_CUDA(cached_malloc(&w.SJ, sizeof(double) * rows * m->Mpad));
-  SG_CUDA(cached_malloc(&w.G, sizeof(double) * rows * m->DP));
-  SG_CUDA(cached_malloc(&w.csum, sizeof(double) * rows));
-  SG_CUDA(cached_malloc(&w.Fd, sizeof(double) * n_geo * m->D));
-  SG_CUDA(cached_malloc(&w.dFd, sizeof(double) * n_geo * p.dirs * m->D));
-  if (stage_H || had_H) SG_CUDA(cached_malloc(&w.H, sizeof(double) * n_geo * n * n));
-  w.geo = n_geo;
-  w.dirs = p.dirs;
-  return 0;
-}
-
-// sgdml_b200_predict_hessian: the GEMM-composed HVP form in FP64, in the model's cell, chunk by chunk on the caller's
-// stream; per direction block the query rows, their tangent rows, both contractions, the folds and the projection
-int hessian_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, double* H, cudaStream_t s) {
-  const bool R_dev = is_device_ptr(R);
-  const int dimi = 3 * m->N;
-  const ChunkOut oH(H, (int64_t)dimi * dimi);
-  const HessPlan p = hessian_plan(m);
-  const int64_t chunk = std::min<int64_t>(p.geo, n_geo);
-  SG_TRY(ensure_hess_ws(m, p, chunk, oH.staged(), s));
-  sgdml_b200_model::HessWS& w = m->hess;
-  const MaternK mk = MaternK::from_sig(m->sig);
-  const double* ae = m->use_ae ? m->ae : nullptr;
-  for (int64_t g0 = 0; g0 < n_geo; g0 += chunk) {
-    const int64_t ng = std::min<int64_t>(chunk, n_geo - g0);
-    const int64_t rows = ng * m->S;
-    const double* Rd = R + g0 * dimi;
-    if (!R_dev) {
-      SG_CUDA(cudaMemcpyAsync(w.R, Rd, sizeof(double) * ng * dimi, cudaMemcpyHostToDevice, s));
-      Rd = w.R;
-    }
-    double* Hc = oH.at(g0, w.H);
-    SG_TRY(launch_desc_from_R(Rd, ng, m->N, w.xq, w.gq, s, m->lat, nullptr));
-    for (int i0 = 0; i0 < dimi; i0 += (int)p.dirs) {
-      const int nd = (int)std::min<int64_t>(p.dirs, dimi - i0);
+    for (int i0 = 0; i0 < n_dir; i0 += (int)p.dirs) {
+      const int nd = (int)std::min<int64_t>(p.dirs, n_dir - i0);
       const int64_t trows = rows * nd, dir_rows = (int64_t)nd * m->S;
+      double* T = w.Qg + rows * m->DS;
       {
         ProfScope ps(KID_PREDICT_AUX, s);
         k_query_rows<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(w.xq, m->pinv, m->mu, m->D, m->DS, m->S, rows, rows,
                                                                   w.Qg, w.qq);
         SG_CUDA(cudaGetLastError());
-        k_hessian_tangent_rows<<<(unsigned)((trows + 7) / 8), 256, 0, s>>>(w.gq, m->pinv, m->N, m->D, m->DS, m->S, i0,
-                                                                            nd, trows, w.Qg + rows * m->DS);
+        if (V != nullptr)
+          k_tangent_rows<DIR_V><<<(unsigned)((trows + 7) / 8), 256, 0, s>>>(w.gq, Vd, m->pinv, m->N, m->D, m->DS, m->S,
+                                                                             i0, nd, trows, T);
+        else
+          k_tangent_rows<DIR_UNIT><<<(unsigned)((trows + 7) / 8), 256, 0, s>>>(w.gq, nullptr, m->pinv, m->N, m->D,
+                                                                                m->DS, m->S, i0, nd, trows, T);
         SG_CUDA(cudaGetLastError());
         count_launch(KID_PREDICT_AUX, 2);
       }
       {
         ProfScope ps(KID_PREDICT_MAIN, s);
+        // [S1; S3] = [Q; T] Xc^T, [S2; S4] = [Q; T] JA^T, then acc = [C1; dC1] XcT^T + [C2; dC2] JAT^T.  One direction:
+        // one pass per step.  More: every tangent row reads its query row's S1 / S2 before the query pass overwrites
+        // them with C1 / C2.  Both give the same bits per element (the same expressions in the same order).
         SG_TRY(contract_desc(m, w.Qg, rows + trows, w.SX, w.SJ, s));
-        // every tangent row reads its query row's S1 / S2 before the query pass overwrites them with C1 / C2
-        k_transform_tangent_rows<TAN_ONLY><<<(unsigned)((trows + 7) / 8), 256, 0, s>>>(
-            w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, ae, m->M, m->Mpad, rows, trows, dir_rows, m->S, mk,
-            w.csum);
-        SG_CUDA(cudaGetLastError());
-        k_transform_tangent_rows<TAN_QUERY><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(
-            w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, ae, m->M, m->Mpad, rows, rows, m->S, m->S, mk,
-            w.csum);
+        if (nd == 1) {
+          k_transform_tangent_rows<TAN_PAIRED><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(
+              w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, ae, m->M, m->Mpad, rows, rows, m->S, m->S, mk,
+              w.csum);
+        } else {
+          k_transform_tangent_rows<TAN_ONLY><<<(unsigned)((trows + 7) / 8), 256, 0, s>>>(
+              w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, ae, m->M, m->Mpad, rows, trows, dir_rows, m->S, mk,
+              w.csum);
+          SG_CUDA(cudaGetLastError());
+          k_transform_tangent_rows<TAN_QUERY><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(
+              w.SX, w.SJ, m->Mpad, w.Qg, m->DS, w.qq, m->mm, m->xja, ae, m->M, m->Mpad, rows, rows, m->S, m->S, mk,
+              w.csum);
+        }
         SG_CUDA(cudaGetLastError());
         SG_TRY(contract_points(m, w.SX, w.SJ, rows + trows, w.G, s));
-        k_combine_tangent_rows<TAN_ONLY><<<(unsigned)ceil_div(trows * m->DP, 256), 256, 0, s>>>(
-            w.Qg, m->DS, w.csum, w.G, m->DP, rows, trows, dir_rows, m->S);
+        if (nd == 1) {
+          k_combine_tangent_rows<TAN_PAIRED><<<(unsigned)ceil_div(rows * m->DP, 256), 256, 0, s>>>(
+              w.Qg, m->DS, w.csum, w.G, m->DP, rows, rows, m->S, m->S);
+        } else {
+          k_combine_tangent_rows<TAN_ONLY><<<(unsigned)ceil_div(trows * m->DP, 256), 256, 0, s>>>(
+              w.Qg, m->DS, w.csum, w.G, m->DP, rows, trows, dir_rows, m->S);
+          SG_CUDA(cudaGetLastError());
+          k_combine_tangent_rows<TAN_QUERY><<<(unsigned)ceil_div(rows * m->DP, 256), 256, 0, s>>>(
+              w.Qg, m->DS, w.csum, w.G, m->DP, rows, rows, m->S, m->S);
+        }
         SG_CUDA(cudaGetLastError());
-        k_combine_tangent_rows<TAN_QUERY><<<(unsigned)ceil_div(rows * m->DP, 256), 256, 0, s>>>(
-            w.Qg, m->DS, w.csum, w.G, m->DP, rows, rows, m->S, m->S);
-        SG_CUDA(cudaGetLastError());
-        count_launch(KID_PREDICT_MAIN, 4);
+        count_launch(KID_PREDICT_MAIN, nd == 1 ? 2 : 4);
       }
       {
         ProfScope ps(KID_PREDICT_FINISH, s);
@@ -2541,15 +2467,19 @@ int hessian_impl(sgdml_b200_model* m, const double* R, int64_t n_geo, double* H,
         k_fdesc_gather<false><<<dim3(gx, (unsigned)std::min<int64_t>(ng * nd, 65535)), 256, 0, s>>>(
             w.G + rows * m->DP, m->perm, m->D, m->DP, m->S, 1, trows, ng * nd, w.dFd, nullptr, nullptr);
         SG_CUDA(cudaGetLastError());
-        k_hessian_project<<<(unsigned)ceil_div(ng * m->N * nd, 256), 256, 0, s>>>(w.Fd, w.dFd, w.gq, m->N, m->D,
-                                                                                  m->std, ng, i0, nd, Hc);
+        const unsigned grid = (unsigned)ceil_div(ng * m->N * nd, 256);
+        if (V != nullptr)
+          k_tangent_project<DIR_V><<<grid, 256, 0, s>>>(w.Fd, w.dFd, w.gq, Vd, m->N, m->D, m->std, ng, i0, nd, oc);
+        else
+          k_tangent_project<DIR_UNIT><<<grid, 256, 0, s>>>(w.Fd, w.dFd, w.gq, nullptr, m->N, m->D, m->std, ng, i0, nd,
+                                                            oc);
         SG_CUDA(cudaGetLastError());
         count_launch(KID_PREDICT_FINISH, 3);
       }
     }
-    SG_TRY(oH.copy_back(g0, ng, w.H, s));
+    SG_TRY(o.copy_back(g0, ng, w.Out, s));
   }
-  if (!R_dev || oH.staged()) SG_CUDA(cudaStreamSynchronize(s));
+  if (!R_dev || !V_dev || o.staged()) SG_CUDA(cudaStreamSynchronize(s));
   return 0;
 }
 
@@ -2578,8 +2508,7 @@ int sgdml_b200_model_destroy(sgdml_b200_model* m) {
   free_oz(m->ozXcT);
   free_oz(m->ozJAT);
   free_ws(m);
-  free_hvp_ws(m->hvp);
-  free_hess_ws(m->hess);
+  free_tangent_ws(m->tangent);
   for (int i = 0; i < 2; ++i)
     if (m->pipe_stream[i]) cudaStreamDestroy(m->pipe_stream[i]);
   for (int i = 0; i < 3; ++i)
@@ -2631,14 +2560,14 @@ int sgdml_b200_predict_hvp(sgdml_b200_model* m, const double* R, const double* V
   SG_TRY(require_device());
   SG_ARG(m != nullptr && R != nullptr && V != nullptr && HV != nullptr && n_geo >= 0);
   if (n_geo == 0) return 0;
-  return hvp_impl(m, R, V, n_geo, HV, (cudaStream_t)stream);
+  return tangent_impl(m, R, V, n_geo, HV, (cudaStream_t)stream);
 }
 
 int sgdml_b200_predict_hessian(sgdml_b200_model* m, const double* R, int64_t n_geo, double* H, void* stream) {
   SG_TRY(require_device());
   SG_ARG(m != nullptr && R != nullptr && H != nullptr && n_geo >= 0);
   if (n_geo == 0) return 0;
-  return hessian_impl(m, R, n_geo, H, (cudaStream_t)stream);
+  return tangent_impl(m, R, nullptr, n_geo, H, (cudaStream_t)stream);
 }
 
 int sgdml_b200_model_set_lattice(sgdml_b200_model* m, const double* lattice, const double* lattice_inv) {

@@ -316,28 +316,14 @@ class GDMLPredict(object):
             raise ValueError('V must match R in type, shape and dtype')
         if not isinstance(R, np.ndarray) and V.device != R.device:
             raise ValueError('V lives on %s but R on %s' % (V.device, R.device))
-        dim_i = 3 * self.n_atoms
-        size = R.size if isinstance(R, np.ndarray) else R.numel()
-        if size % dim_i != 0 or (R.ndim == 2 and R.shape[1] != dim_i):
-            raise ValueError('R must have 3*n_atoms columns')
+        R, HV = self._tangent_io(R, out, None)
         if isinstance(R, np.ndarray):
-            R = np.ascontiguousarray(R, dtype=np.float64).reshape(-1, dim_i)
-            V = np.ascontiguousarray(V, dtype=np.float64).reshape(-1, dim_i)
-            HV = np.empty_like(R) if out is None else out
+            V = np.ascontiguousarray(V, dtype=np.float64).reshape(R.shape)
         else:
-            import torch
-
-            if R.dtype != torch.float64:
-                raise ValueError('torch inputs must be float64')
-            R = R.contiguous().reshape(-1, dim_i)
-            V = V.contiguous().reshape(-1, dim_i)
-            pin = (not R.is_cuda) and R.is_pinned()
-            HV = torch.empty(R.shape, dtype=torch.float64, device=R.device, pin_memory=pin) if out is None else out
-        n = R.shape[0]
-        if out is not None:
-            self._check_out(R, None, HV, None, n, dim_i)
+            V = V.contiguous().reshape(R.shape)
         _lib.check(
-            _lib.lib().sgdml_b200_predict_hvp(self._handle, _lib.ptr(R), _lib.ptr(V), n, _lib.ptr(HV), _lib.current_stream()),
+            _lib.lib().sgdml_b200_predict_hvp(self._handle, _lib.ptr(R), _lib.ptr(V), R.shape[0], _lib.ptr(HV),
+                                              _lib.current_stream()),
             'predict_hvp',
         )
         return HV
@@ -346,36 +332,50 @@ class GDMLPredict(object):
         """Extension: the energy Hessian H = d^2E/dR^2 of every geometry, R (B, 3N) [or (3N,)] -> H (B, 3N, 3N), in the
         model's units and cell, always in FP64.  Column i of H[b] equals -predict_hvp(R[b], e_i) bit for bit; H is not
         symmetrised.  `out`: a preallocated (B, 3N, 3N) buffer.  NumPy / torch conventions as `predict_hvp`."""
+        R, H = self._tangent_io(R, out, 3 * self.n_atoms)
+        _lib.check(
+            _lib.lib().sgdml_b200_predict_hessian(self._handle, _lib.ptr(R), R.shape[0], _lib.ptr(H),
+                                                  _lib.current_stream()),
+            'predict_hessian',
+        )
+        return H
+
+    def _tangent_io(self, R, out, n_cols):
+        """`predict_hvp`'s and `predict_hessian`'s R in either form, as a contiguous (B, 3N) float64 array or tensor, and
+        their output: (B, 3N) for n_cols None, else (B, 3N, n_cols), allocated like R or taken from `out` and checked
+        as `predict`'s F."""
         dim_i = 3 * self.n_atoms
         size = R.size if isinstance(R, np.ndarray) else R.numel()
         if size % dim_i != 0 or (R.ndim == 2 and R.shape[1] != dim_i):
             raise ValueError('R must have 3*n_atoms columns')
         if isinstance(R, np.ndarray):
             R = np.ascontiguousarray(R, dtype=np.float64).reshape(-1, dim_i)
-            shape = (R.shape[0], dim_i, dim_i)
-            H = np.empty(shape) if out is None else out
+            empty = np.empty
         else:
             import torch
 
             if R.dtype != torch.float64:
                 raise ValueError('torch inputs must be float64')
             R = R.contiguous().reshape(-1, dim_i)
-            shape = (R.shape[0], dim_i, dim_i)
-            pin = (not R.is_cuda) and R.is_pinned()
-            H = torch.empty(shape, dtype=torch.float64, device=R.device, pin_memory=pin) if out is None else out
+            pin = (not R.is_cuda) and R.is_pinned()  # pinned host tensor in -> pinned host tensor out
+
+            def empty(shape):
+                return torch.empty(shape, dtype=torch.float64, device=R.device, pin_memory=pin)
+
         n = R.shape[0]
-        if out is not None:
-            if tuple(H.shape) != shape:
-                raise ValueError('out has the wrong shape %s (expected %s)' % (tuple(H.shape), shape))
-            if not (H.flags['C_CONTIGUOUS'] if isinstance(H, np.ndarray) else H.is_contiguous()):
-                raise ValueError('out must be contiguous')
-            # the dtype, layout and device checks of `predict`'s F, on the buffer seen as (B, 3N * 3N)
-            self._check_out(R, None, H.reshape(n, dim_i * dim_i), None, n, dim_i * dim_i)
-        _lib.check(
-            _lib.lib().sgdml_b200_predict_hessian(self._handle, _lib.ptr(R), n, _lib.ptr(H), _lib.current_stream()),
-            'predict_hessian',
-        )
-        return H
+        shape = (n, dim_i) if n_cols is None else (n, dim_i, n_cols)
+        if out is None:
+            return R, empty(shape)
+        if n_cols is None:
+            self._check_out(R, None, out, None, n, dim_i)
+            return R, out
+        if tuple(out.shape) != shape:
+            raise ValueError('out has the wrong shape %s (expected %s)' % (tuple(out.shape), shape))
+        if not (out.flags['C_CONTIGUOUS'] if isinstance(out, np.ndarray) else out.is_contiguous()):
+            raise ValueError('out must be contiguous')
+        # the dtype, layout and device checks of `predict`'s F, on the buffer seen as (B, 3N * n_cols)
+        self._check_out(R, None, out.reshape(n, dim_i * n_cols), None, n, dim_i * n_cols)
+        return R, out
 
     @staticmethod
     def _results(E, F, W, return_E, with_W):

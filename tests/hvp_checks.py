@@ -8,7 +8,7 @@ reference is right and every check can fail (tests/test_hvp_checks.py).
   tangent formulas, valid on and near training points (the term (delta.JA)(delta.t)/|delta| has its exact limit 0).
 - `hvp_abs_scale` and `check_hvp` give the componentwise bound |HV - HV_ref| <= tau(k) scale, in the style of
   predict_checks.predict_abs_scale / check_predict.
-- `hvp_chunk_plan` restates how `sgdml_b200_predict_hvp` cuts a batch into chunks (hvp_chunk_geos).
+- `hvp_chunk_plan` restates how `sgdml_b200_predict_hvp` cuts a batch into chunks (tangent_plan with one direction).
 """
 
 import collections
@@ -149,7 +149,7 @@ def hvp_reference(model, R, V=None, lat_and_inv='model'):
 # ------------------------------------------------------------------------------------------------ magnitude
 def hvp_abs_scale(model, R, V, lat_and_inv='model'):
     """Per-output magnitudes scale (B, 3N) for `check_hvp`: the engine's HVP (csrc/predict.cu,
-    k_transform_tangent_rows, k_combine_tangent_rows, k_hvp_project) with every term replaced by its absolute value, so
+    k_transform_tangent_rows, k_combine_tangent_rows, k_tangent_project) with every term replaced by its absolute value, so
     that tau(k) scale bounds the rounding of each term.  Notation per cache row k: q = x - mu and X_k - mu the centred
     query and training descriptors as the engine stores them, A = |q| + |X_k - mu| (componentwise), rho = |q|^2 +
     |X_k - mu|^2, ta_d = sum_c |g_dc| (|v_ac| + |v_bc|) (a bound on |t_d| and on its rounding), |.|_2 Euclidean norms.
@@ -252,7 +252,7 @@ def check_hvp(HV, HV_ref, scale, k, what='hvp'):
         k_c1 e |JA_m|_2 |t|_2 n_floor / sig times (D / 2 + 10) / 8 -- and tau |JA|_2 |t|_2 rho / (sqrt5 d_eff) with
         d_eff = 8 sqrt(u rho) is k sqrt(u rho) |JA|_2 |t|_2 / sqrt5: enough when 8 k >= 4 D + 76.
       * GEMM2 sums 2 M + 1 terms per virtual row (padded training columns are zero: exact), k_combine_tangent_rows
-        two roundings, the fold over S permutations S, k_hvp_project N - 1 pairs of <= 4 roundings each.  It rebuilds
+        two roundings, the fold over S permutations S, k_tangent_project N - 1 pairs of <= 4 roundings each.  It rebuilds
         the pair vector from g (|g|_2 = |d|^-2, 3 + 2 roundings), so dg carries <= 10 u of the dg of the scale; the
         difference dF_desc - 3 (g.dd) F_desc / |g|^1/2 is bounded by the sum of absolute values.  std: one rounding.
     The engine's error is therefore within gamma_{3 D + 2 M + S + 4 N + 40} of the scale, and the reference's (long
@@ -388,12 +388,15 @@ HvpPlan = collections.namedtuple('HvpPlan', 'chunk chunks edges')
 
 
 def hvp_chunk_geos(layout, S, cap=0):
-    """Geometries per HVP chunk (csrc/predict.cu hvp_chunk_geos): S1-S4 (4 Mpad) and G, dG (2 DP) doubles per virtual
-    row, S virtual rows per geometry, within 2 GiB; at least 1, at most 65 536, at most `cap` when the test hook sets
-    one."""
-    g = (2048 << 20) // (8 * (4 * layout.Mpad + 2 * layout.DP) * S)
-    g = max(1, min(g, 65536))
-    return min(g, cap) if cap > 0 else g
+    """Geometries per HVP chunk (csrc/predict.cu tangent_plan with one direction per geometry): a stacked row holds
+    DS + 2 Mpad + DP + 2 doubles (Qg, SX, SJ, G, qq, csum), a geometry 2 S rows (S query rows, S tangent rows), within
+    2 GiB; at least 1, at most 65 536, at most `cap` (a cap of 2 cap S rows) when the test hook sets one."""
+    DS = layout.DP + 4  # the model's row stride (m->DS in csrc/predict.cu); pc.Layout does not carry it
+    rows = (2048 << 20) // (8 * (DS + 2 * layout.Mpad + layout.DP + 2))
+    if cap > 0:
+        rows = min(rows, 2 * cap * S)
+    rows = max(rows, 2 * S)
+    return min(rows // (2 * S), 65536)
 
 
 def hvp_chunk_plan(layout, S, B, cap=0):

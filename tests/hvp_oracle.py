@@ -4,7 +4,7 @@
   energy constraints), differentiable end to end.  Its HV = (dF/dR) V comes from forward-mode autograd on F, so it
   is independent of the engine's hand-derived tangent formulas.
 - `gemm_form_hvp`: a NumPy model of the engine's GEMM-composed HVP (csrc/predict.cu: stacked query and tangent rows,
-  k_transform_tangent_rows with its floor under n, the permutation fold and k_hvp_project), run on the same GEMM-form
+  k_transform_tangent_rows with its floor under n, the permutation fold and k_tangent_project), run on the same GEMM-form
   quantities (S1 = Q Xc^T, ..., x5 = 5 (qq + mm) - 10 S1) that the device computes.
 """
 
@@ -131,7 +131,7 @@ DEFECTS = ('dJ', 'csT', 'ae_dc2', 'pinv_fold')
 def gemm_form_hvp(model, R, V, lat_and_inv='model', guard=True, defect=None, floor_scale=1.0):
     """The engine's HVP in NumPy, R, V (B, 3N) -> HV (B, 3N).  guard=False drops the floor under n in a ds / n and
     clamps x5 at 1e-300 as the forward does.  defect (for showing that a check fails; one of DEFECTS): 'dJ' drops the
-    (dJ)^T F_desc term of k_hvp_project, 'csT' the (sum c1) T term of dG, 'ae_dc2' leaves ae dc2 out of dc1,
+    (dJ)^T F_desc term of k_tangent_project, 'csT' the (sum c1) T term of dG, 'ae_dc2' leaves ae dc2 out of dc1,
     'pinv_fold' folds the permutations with pinv instead of perm; floor_scale multiplies the floor."""
     assert defect is None or defect in DEFECTS, defect
     R = np.asarray(R, dtype=np.float64).reshape(-1, np.asarray(model['z']).shape[0] * 3)

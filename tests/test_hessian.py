@@ -1,7 +1,8 @@
 """Batched energy Hessians (sgdml_b200_predict_hessian, GDMLPredict.predict_hessian): every column equals
 -predict_hvp(R, e_i) bit for bit on golden fixtures and on models of both descriptor classes (plain, alphas_E, periodic),
 sampled columns pass the HVP's componentwise bound against the long-double reference, direction blocks and chunks do
-not change a bit, host / device / pinned buffers, B = 0, rejected calls, and one 370-atom geometry."""
+not change a bit, host / device / pinned buffers, B = 0, rejected calls, one 370-atom geometry, and HVP and Hessian
+calls interleaved on one workspace."""
 
 import numpy as np
 import pytest
@@ -128,3 +129,31 @@ def test_370_atoms():
     assert H.shape == (1, 1110, 1110) and np.all(np.isfinite(H))
     cols = [0, 1, 554, 1108, 1109]
     assert np.array_equal(H[:, :, cols], _columns_by_hvp(gp, R, cols))
+
+
+def test_hvp_and_hessian_share_one_workspace():
+    """predict_hvp and predict_hessian share one workspace that grows to the largest request and never shrinks: calls
+    interleaved on one model, with growing and shrinking batches, host and device buffers and a chunk cap set and cleared
+    in between, each bit-identical to the same call on a fresh model."""
+    import torch
+
+    model, _ = hc.class_model('n24', 'ecstr')
+    R, V = hc.queries(model, 40, seed=9)
+
+    def call(gp, kind, B, dev):
+        Rb, Vb = R[:B], V[:B]
+        if dev:
+            Rb, Vb = torch.from_numpy(Rb).cuda(), torch.from_numpy(Vb).cuda()
+        out = gp.predict_hessian(Rb) if kind == 'hessian' else gp.predict_hvp(Rb, Vb)
+        return out.cpu().numpy() if dev else out
+
+    gp = _gp(model)
+    calls = [('hessian', 3, False, 0), ('hvp', 40, False, 0), ('hessian', 7, True, 0), ('hvp', 2, True, 0),
+             ('hessian', 2, False, 4), ('hvp', 40, True, 4), ('hessian', 1, True, 1), ('hvp', 9, False, 0),
+             ('hessian', 7, False, 0), ('hvp', 1, False, 1), ('hessian', 5, True, 0), ('hvp', 40, False, 0)]
+    try:
+        for kind, B, dev, cap in calls:
+            _chunk(cap)
+            assert np.array_equal(call(gp, kind, B, dev), call(_gp(model), kind, B, dev)), (kind, B, dev, cap)
+    finally:
+        _chunk(0)

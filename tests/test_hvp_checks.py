@@ -176,17 +176,18 @@ def test_one_entry_moved_fails(name):
 
 # ------------------------------------------------------------------------------------------------ chunk plans
 def test_chunk_plan_aspirin():
-    # 2^31 / (8 (4 * 1008 + 2 * 224) 6) = 9 986 geometries per chunk
+    # a stacked row is 228 + 2 * 1008 + 224 + 2 = 2 470 doubles: 2^31 / (8 * 2 470) = 108 678 rows, 2 * 6 per geometry:
+    # 9 056 geometries per chunk
     ly = pc.layout(21, 1000)
-    assert hc.hvp_chunk_geos(ly, 6) == 9986
-    p = hc.hvp_chunk_plan(ly, 6, 2 * 9986 + 3)
-    assert p.chunk == 9986 and p.chunks == [(0, 9986), (9986, 19972), (19972, 19975)]
-    assert p.edges == [0, 9985, 9986, 19971, 19972, 19974]
+    assert hc.hvp_chunk_geos(ly, 6) == 9056
+    p = hc.hvp_chunk_plan(ly, 6, 2 * 9056 + 3)
+    assert p.chunk == 9056 and p.chunks == [(0, 9056), (9056, 18112), (18112, 18115)]
+    assert p.edges == [0, 9055, 9056, 18111, 18112, 18114]
     assert hc.hvp_chunk_plan(ly, 6, 19975, cap=1000).chunks[-1] == (19000, 19975)
 
 
 def test_chunk_plan_small_models_hit_the_cap():
-    # N = 6, S = 2, M = 33: 2^31 / (8 (4 * 64 + 2 * 40) 2) = 399 457 -> 65 536
+    # N = 6, S = 2, M = 33: 2^31 / (8 (44 + 2 * 64 + 40 + 2)) = 1 254 371 rows, 313 592 geometries -> 65 536
     ly = pc.layout(6, 33)
     assert (ly.DP, ly.Mpad) == (40, 64)
     p = hc.hvp_chunk_plan(ly, 2, 65536 + 3)
@@ -196,11 +197,11 @@ def test_chunk_plan_small_models_hit_the_cap():
 
 
 def test_chunk_plan_large_descriptors():
-    # big_n240_m2_s3: DP = 28 680, Mpad = 8: 2^31 / (8 (32 + 57 360) 3) = 1 559
+    # big_n240_m2_s3: DP = 28 680, Mpad = 8: 2^31 / (8 (28 684 + 16 + 28 680 + 2)) = 4 678 rows / (2 * 3) = 779
     ly = pc.layout(240, 2)
     assert (ly.DP, ly.Mpad, ly.large) == (28680, 8, True)
-    assert hc.hvp_chunk_geos(ly, 3) == 1559
-    # ac-ala3-nhme: DP 864, Mpad 2000, S 243: 2^31 / (8 (8000 + 1728) 243) = 113
-    assert hc.hvp_chunk_geos(pc.layout(42, 2000), 243) == 113
+    assert hc.hvp_chunk_geos(ly, 3) == 779
+    # ac-ala3-nhme: DP 864, Mpad 2000, S 243: 2^31 / (8 (868 + 4000 + 864 + 2)) = 46 814 rows / (2 * 243) = 96
+    assert hc.hvp_chunk_geos(pc.layout(42, 2000), 243) == 96
     assert hc.hvp_chunk_plan(pc.layout(42, 2000), 243, 10, cap=4).chunks == [(0, 4), (4, 8), (8, 10)]
     assert hc.hvp_chunk_geos(pc.layout(42, 2000), 243 * 1000) == 1  # at least one geometry

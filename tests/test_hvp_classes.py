@@ -102,7 +102,7 @@ def _edge_rows(plan, width=64):
 
 
 def test_hvp_full_capped_chunk_and_tail(eng):
-    """N = 6, S = 2, M = 33 (Mpad 64): the chunk rule gives 399 457 geometries, capped at 65 536, so B = 65 539 runs one
+    """N = 6, S = 2, M = 33 (Mpad 64): the chunk rule gives 313 592 geometries, capped at 65 536, so B = 65 539 runs one
     full chunk -- k_fdesc_gather's grid stops at y = 65 535 and its grid-stride loop must reach geometry 65 535 -- and a
     tail of 3.  Every row of the first and last 64 geometries of each chunk is checked, and the whole output is
     bit-identical to chunks of 1 000."""
@@ -126,7 +126,7 @@ def test_hvp_full_capped_chunk_and_tail(eng):
 
 
 def test_hvp_aspirin_default_chunks(eng):
-    """The benchmarked aspirin shape (N 21, M 1000, S 6, random coefficients): 9 986 geometries per default (~2 GB)
+    """The benchmarked aspirin shape (N 21, M 1000, S 6, random coefficients): 9 056 geometries per default (~2 GB)
     chunk, B = 2 chunks + 3, from CUDA tensors.  Chunk-edge rows and a seeded sample of 64 rows against the reference;
     the whole output bit-identical to chunks of 1 000."""
     import torch
@@ -137,8 +137,8 @@ def test_hvp_aspirin_default_chunks(eng):
     N, M = cfg['n_atoms'], cfg['n_train']
     perms, _ = synth.config_perms_and_r0('aspirin')
     model = synth.random_model(N, M, perms, cfg['sig'])
-    plan = hc.hvp_chunk_plan(_layout(model), perms.shape[0], 2 * 9986 + 3)
-    assert plan.chunk == 9986 and len(plan.chunks) == 3
+    plan = hc.hvp_chunk_plan(_layout(model), perms.shape[0], 2 * 9056 + 3)
+    assert plan.chunk == 9056 and len(plan.chunks) == 3
     B = plan.chunks[-1][1]
     R = synth.geometries(N, B, 41).reshape(B, -1)
     V = np.random.default_rng(42).standard_normal(R.shape)

@@ -798,6 +798,19 @@ int sgdml_b200_trsm_right_lt(const double* L, int64_t m, int64_t ldl, double* X,
  * 128 x 128 diagonal tiles may be written too (with the same products); padding columns (ldc > m) are not. */
 int sgdml_b200_gram_tn(const double* X, int64_t n_rows, int64_t m, int64_t ldx, double lam, double* C,
                        int64_t ldc, void* stream);
+/* Posterior covariance blocks of an analytic-solver model (sgdml_b200/posterior.py, DESIGN.md section 4.1.13).
+ * V (DEVICE, (3N + 1) n_query rows of n columns, row stride ldv >= n) holds the solved cross rows C(z, X) L^-T of
+ * n_query queries in the row layout of sgdml_b200_assemble_ecstr_rows: the 3N force rows of query q at q 3N + r, then
+ * the energy row of q at 3N n_query + q.  prior (n_query, d, d), d = 3N + 1, holds P_q = C(z_q, z_q) in the order
+ * [F (3N); E] with the energy row and column standing for -E, as assembled.  Writes, for every query,
+ *   out[q][i][j] = scale * sgn(i, j) * (P_q[i][j] - sum_k V[row(q, i)][k] V[row(q, j)][k]),
+ * sgn = -1 where exactly one of i, j is the energy component (the blocks are for +E), +1 elsewhere.  Only the lower
+ * triangle of P_q is read; each entry i >= j is computed once and stored at [i][j] and [j][i], so out is exactly
+ * symmetric.  The sum over k runs in fixed 4096-column slices, each in increasing k, then over the slices in order,
+ * without atomics: out[q] is bit-identical whatever n_query and whichever position q has.  prior and out may be host
+ * or device pointers.  1 <= n_query <= 65535, 1 <= N <= 1023.  Returns after the kernels have finished. */
+int sgdml_b200_posterior_blocks(const double* V, int64_t ldv, int64_t n, int64_t n_query, int64_t n_atoms,
+                                const double* prior, double scale, double* out, void* stream);
 /* out[r] = |X[r, :]|^2 -- the leverage scores (iterative.py:107-109). */
 int sgdml_b200_row_sqnorms(const double* X, int64_t n_rows, int64_t m, int64_t ldx, double* out,
                            void* stream);

@@ -12,6 +12,7 @@ __version__ = '0.1.0'
 from .md import (GDMLIRC, GDMLNEB, GDMLDimer, GDMLDynamics, GDMLMetadynamics, GDMLNPTDynamics,  # noqa: F401
                  GDMLPathIntegralDynamics, GDMLRelaxation, GDMLReplicaExchange, GDMLUmbrellaSampling)
 from .perm import find_perms  # noqa: F401
+from .posterior import GDMLPosterior  # noqa: F401
 from .predict import GDMLPredict  # noqa: F401
 from .train import GDMLTrain  # noqa: F401
 from .vib import GDMLVibrations, harmonic_rate, thermo  # noqa: F401

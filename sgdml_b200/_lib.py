@@ -164,6 +164,8 @@ SIGNATURES = {
     'sgdml_b200_add_diag': (C.c_int, [c_void_p, i64, i64, C.c_double, c_void_p]),
     'sgdml_b200_trsm_right_lt': (C.c_int, [c_void_p, i64, i64, c_void_p, i64, i64, c_void_p]),
     'sgdml_b200_gram_tn': (C.c_int, [c_void_p, i64, i64, i64, C.c_double, c_void_p, i64, c_void_p]),
+    'sgdml_b200_posterior_blocks': (
+        C.c_int, [c_void_p, i64, i64, i64, i64, c_void_p, C.c_double, c_void_p, c_void_p]),
     'sgdml_b200_row_sqnorms': (C.c_int, [c_void_p, i64, i64, i64, c_void_p, c_void_p]),
     'sgdml_b200_nystroem_apply': (C.c_int, [c_void_p, i64, i64, i64, C.c_double, c_void_p, c_void_p, c_void_p]),
     'sgdml_b200_nystroem_project': (C.c_int, [c_void_p, i64, i64, i64, c_void_p, c_void_p, c_void_p]),

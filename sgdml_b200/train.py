@@ -31,6 +31,20 @@ def _torch():
     return torch
 
 
+def labels(task, use_E_cstr):
+    """The normalised label vector train() solves for (train.py:939-947): y = F_train.ravel() / std, with energy
+    constraints [F_train.ravel(); -E_train + mean(E_train)] / std.  Returns (y, std, mean(E_train) or None)."""
+    y = np.asarray(task['F_train'], dtype=np.float64).ravel().copy()
+    E_train_mean = None
+    if use_E_cstr:
+        E_train = np.asarray(task['E_train'], dtype=np.float64).ravel().copy()
+        E_train_mean = np.mean(E_train)
+        y = np.hstack((y, -E_train + E_train_mean))
+    y_std = np.std(y)
+    y /= y_std
+    return y, y_std, E_train_mean
+
+
 class GDMLTrain(object):
     def __init__(self, max_memory=None, max_processes=None, use_torch=False):
         """train.py:306-361.  `max_memory` [GB] caps the device memory the analytic solver
@@ -162,14 +176,7 @@ class GDMLTrain(object):
         R_desc, R_d_desc, R_desc_dev, R_d_desc_dev = self._descriptors(desc, R, lat_and_inv)
         self._dev_views = {id(R_desc): R_desc_dev, id(R_d_desc): R_d_desc_dev}  # device twins of the host arrays
 
-        y = np.asarray(task['F_train'], dtype=np.float64).ravel().copy()  # train.py:939-947
-        E_train_mean = None
-        if use_E_cstr:
-            E_train = np.asarray(task['E_train'], dtype=np.float64).ravel().copy()
-            E_train_mean = np.mean(E_train)
-            y = np.hstack((y, -E_train + E_train_mean))
-        y_std = np.std(y)
-        y /= y_std
+        y, y_std, E_train_mean = labels(task, use_E_cstr)
 
         t_desc = timeit.default_timer() - t_all
         # solver choice by memory, like train.py:949-975 -- but against DEVICE memory
